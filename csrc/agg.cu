@@ -345,49 +345,13 @@ __global__ void k_partial_merge(GroupTable gt, AggPlan ap, const uint64_t* src, 
     }
 }
 
-// Result extraction: one output row per occupied slot.  Output columns (canonical 64-bit images +
-// one null byte each), in this order: group expressions, then per aggregate its final value and,
-// for AVG, the intermediate {sum, count} pair (AggFnCall::finalize, agg_fn_call.cpp:927-990).
+// Result extraction: one output row per occupied slot (extract_group, agg_kernels.cuh), rows of stride out_cap.
 __global__ void k_extract(GroupTable gt, AggPlan ap, uint64_t* outv, uint8_t* outn, uint32_t out_cap, uint32_t* cursor, int emit_default) {
-    const uint32_t cap = gt.cap_mask + 1;
     BK_FOR_EACH_GROUP(gt, ap, i) {
-        const uint64_t nrows = gt.lanes[i];
-        if (ap.n_keyw == 0 && nrows == 0 && !emit_default) continue;
+        if (ap.n_keyw == 0 && gt.lanes[i] == 0 && !emit_default) continue;
         const uint32_t pos = atomicAdd(cursor, 1u);
         if (pos >= out_cap) continue;
-        int c = 0;
-        for (int g = 0; g < ap.n_group; g++, c++) {
-            const bool isnull = ap.key_null_word[g] != 0xFF &&
-                                ((gt.keys[(size_t)ap.key_null_word[g] * cap + i] >> ap.key_null_shift[g]) & 1ull);
-            uint64_t v = gt.keys[(size_t)ap.key_word[g] * cap + i] >> ap.key_shift[g];
-            if (ap.key_bits[g] < 64) v &= (1ull << ap.key_bits[g]) - 1ull;
-            // sign-extend narrow signed keys back to their canonical image
-            if (ap.key_bits[g] == 32 && prim_class(ap.key_prim[g]) == VC_I64) v = (uint64_t)(int64_t)(int32_t)v;
-            outv[(size_t)c * out_cap + pos] = isnull ? 0 : v;
-            outn[(size_t)c * out_cap + pos] = isnull ? 1 : 0;
-        }
-        for (int k = 0; k < ap.n_agg; k++) {
-            const AggSpec a = ap.agg[k];
-            if (a.hidden) continue;
-            const uint64_t cnt = a.cnt_lane ? gt.lanes[(size_t)a.cnt_lane * cap + i] : nrows;
-            const uint64_t acc = gt.lanes[(size_t)a.acc_lane * cap + i];
-            uint64_t v = 0; uint8_t isnull = 0;
-            switch (a.kind) {
-                case AG_COUNT_STAR: v = nrows; break;
-                case AG_COUNT: v = cnt; break;
-                case AG_COUNT_MERGE: v = acc; break;
-                case AG_AVG:
-                    if (cnt == 0) isnull = 1; else v = f64_bits(__ddiv_rn(bits_f64(acc), (double)(int64_t)cnt));
-                    break;
-                default: if (cnt == 0) isnull = 1; else v = acc; break;  // SUM / MIN / MAX: NULL without input
-            }
-            outv[(size_t)c * out_cap + pos] = v; outn[(size_t)c * out_cap + pos] = isnull; c++;
-            if (a.kind == AG_AVG) {  // intermediate blob {double sum; int64 count}
-                // the blank row of an empty scalar aggregate initialises only its counts (agg_node.cpp:489-503): blob stays NULL
-                outv[(size_t)c * out_cap + pos] = acc; outn[(size_t)c * out_cap + pos] = (ap.n_keyw == 0 && nrows == 0) ? 1 : 0; c++;
-                outv[(size_t)c * out_cap + pos] = cnt; outn[(size_t)c * out_cap + pos] = 0; c++;
-            }
-        }
+        extract_group(gt, ap, i, pos, outv, outn, out_cap);
     }
 }
 
@@ -445,21 +409,22 @@ static int occupancy_grid(K kernel, size_t smem, int sm_count) {
     return per_sm * sm_count;  // persistent grid: a whole number of CTAs per SM (132 SMs on H100 SXM)
 }
 
-cudaError_t launch_agg(const AggArgs& a, bool direct, int sm_count, cudaStream_t s, const char** kernel_name) {
+cudaError_t launch_agg(const AggArgs& a, bool direct, int sm_count, cudaStream_t s, cudaEvent_t start, const char** kernel_name) {
     const bool grouped = a.plan.n_keyw > 0;
     const size_t smem = grouped ? agg_smem_bytes(a.smem_keyw, a.n_smem_lanes, a.smem_cap_log2) : 0;
     if (a.nrows <= 0) return cudaSuccess;
     if (direct && !grouped && a.scalar_tma) {
         cudaError_t e = cudaSuccess;
+        if (start) cudaEventRecord(start, s);
         if (launch_count_where_tma(a, sm_count, s, &e)) { *kernel_name = "k_count_where_tma"; return e; }
     }
     if (direct) {
         const size_t dsmem = grouped ? direct_smem_bytes(a.smem_keyw, a.n_smem_lanes, a.smem_cap_log2, a.direct.n_vals) + (a.lean_fx ? fx_ext_bytes(a.direct.n_vals, a.smem_cap_log2) : 0) : 0;
         *kernel_name = grouped ? "k_agg_group_direct" : "k_agg_scalar_direct";
         switch (a.direct.n_terms) {
-            case 0: return launch_direct_np0(a, a.direct.n_vals, sm_count, dsmem, s, grouped);
-            case 1: return launch_direct_np1(a, a.direct.n_vals, sm_count, dsmem, s, grouped);
-            default: return launch_direct_np2(a, a.direct.n_vals, sm_count, dsmem, s, grouped);
+            case 0: return launch_direct_np0(a, a.direct.n_vals, sm_count, dsmem, s, grouped, start);
+            case 1: return launch_direct_np1(a, a.direct.n_vals, sm_count, dsmem, s, grouped, start);
+            default: return launch_direct_np2(a, a.direct.n_vals, sm_count, dsmem, s, grouped, start);
         }
     }
     *kernel_name = "k_agg_interp";
@@ -470,6 +435,7 @@ cudaError_t launch_agg(const AggArgs& a, bool direct, int sm_count, cudaStream_t
     int grid = occupancy_grid(k_agg_interp, smem, sm_count);
     int64_t want = (a.nrows + 255) / 256;
     if (want < grid) grid = (int)want;
+    if (start) cudaEventRecord(start, s);
     k_agg_interp<<<grid, 256, smem, s>>>(a);
     return cudaGetLastError();
 }

@@ -70,6 +70,10 @@ struct AggArgs {
     int32_t wp_warps;        // warps per CTA (one accumulator table each): 8, 12 or 16
     int32_t wp_dense;        // 1 = no key table: id = key - wp_dense_sub (keys known to lie in a range of wp_gcap values)
     uint32_t wp_dense_sub;
+    // lean kernel: the last CTA to finish extracts the table's rows into this mapped host buffer (fused_extract, agg_kernels.cuh):
+    // [32-byte counter block][values n_img x n][null bytes n_img x n], n = the groups in the table.  nullptr = no fused extraction
+    uint8_t* fused_out;
+    uint32_t fused_cap;      // rows the buffer holds: a table with more groups leaves only the counter block there (the host runs k_extract)
 };
 
 // shared memory of k_agg_group_wp: key table + id counter + one accumulator set {sums 8 B x na, cnt 4 B} x gcap per warp
@@ -82,10 +86,11 @@ cudaError_t launch_images_to_columns(const uint64_t* outv, const uint8_t* outn, 
 size_t agg_smem_bytes(int smem_keyw, int n_smem_lanes, int cap_log2);
 // scalar_tma.cu: TMA-staged COUNT(*) WHERE int32 <cmp> c (experiment, option "scalar_tma"); false = not this kernel's shape
 bool launch_count_where_tma(const AggArgs& a, int sm_count, cudaStream_t s, cudaError_t* err);
-cudaError_t launch_agg(const AggArgs& a, bool direct, int sm_count, cudaStream_t s, const char** kernel_name);
-cudaError_t launch_direct_np0(const AggArgs& a, int na, int sm_count, size_t smem, cudaStream_t s, bool grouped);
-cudaError_t launch_direct_np1(const AggArgs& a, int na, int sm_count, size_t smem, cudaStream_t s, bool grouped);
-cudaError_t launch_direct_np2(const AggArgs& a, int na, int sm_count, size_t smem, cudaStream_t s, bool grouped);
+// `start` (optional) is recorded on `s` right before the kernel launch, after the launch setup
+cudaError_t launch_agg(const AggArgs& a, bool direct, int sm_count, cudaStream_t s, cudaEvent_t start, const char** kernel_name);
+cudaError_t launch_direct_np0(const AggArgs& a, int na, int sm_count, size_t smem, cudaStream_t s, bool grouped, cudaEvent_t start);
+cudaError_t launch_direct_np1(const AggArgs& a, int na, int sm_count, size_t smem, cudaStream_t s, bool grouped, cudaEvent_t start);
+cudaError_t launch_direct_np2(const AggArgs& a, int na, int sm_count, size_t smem, cudaStream_t s, bool grouped, cudaEvent_t start);
 size_t direct_smem_bytes(int smem_keyw, int n_smem_lanes, int cap_log2, int na);
 size_t fx_ext_bytes(int na, int cap_log2);
 cudaError_t launch_join_build(const DevCol& key, int from_prim, int cast_prim, int64_t nrows, uint64_t* keys, uint32_t* rows, uint32_t cap_mask, cudaStream_t s);

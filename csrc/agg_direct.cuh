@@ -17,6 +17,9 @@
 // resolved into registers before the loop; uncommon shapes (min/max, float/bool/narrow columns,
 // NULL keys wider than 32 bits ...) take out-of-line routines so the hot loop stays lean.
 #pragma once
+#include <map>
+#include <mutex>
+#include <tuple>
 #include "agg_kernels.cuh"
 #include "fx.h"
 
@@ -894,6 +897,7 @@ if (NA == 2 && fx_pair) fx_add2(a, acc_addr[0] + slot * 16u, acc_addr[NA > 1 ? 1
 #pragma unroll
         for (int d = 16; d > 0; d >>= 1) passed += __shfl_xor_sync(0xFFFFFFFFu, passed, d);
         if (lane == 0 && passed) atomicAdd((unsigned long long*)a.rows_passed, (unsigned long long)passed);
+        if (a.fused_out) fused_extract(a);
         return;
     }
     }
@@ -1140,6 +1144,7 @@ if (NA == 2 && fx_pair) fx_add2(a, acc_addr[0] + slot * 16u, acc_addr[NA > 1 ? 1
 #pragma unroll
     for (int d = 16; d > 0; d >>= 1) passed += __shfl_xor_sync(0xFFFFFFFFu, passed, d);
     if (lane == 0 && passed) atomicAdd((unsigned long long*)a.rows_passed, (unsigned long long)passed);
+    if (a.fused_out) fused_extract(a);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1256,78 +1261,78 @@ __global__ void __launch_bounds__(DIRECT_THREADS, NA == 0 ? 2 : 1) k_agg_scalar_
 }
 
 // ------------------------------------------------------------------------------------------
+// Launch setup paid once per kernel: its dynamic shared-memory limit is raised only when a launch needs more than was set before, and
+// its resident CTAs per SM are asked once per (device, threads, shared bytes) — the answers never change, and asking costs
+// microseconds of host time on every request.
+struct LaunchSetupCache {
+    std::mutex mu;
+    std::map<std::pair<int, const void*>, size_t> smem_set;
+    std::map<std::tuple<int, const void*, int, size_t>, int> per_sm;
+};
+inline LaunchSetupCache& launch_setup_cache() { static LaunchSetupCache c; return c; }
+
+// persistent grid: whole CTAs per SM x the device's SMs (132 on H100 SXM), fewer for a small batch.  `start` (optional) is recorded
+// right before the launch, after the setup, so that it times the kernel alone.
 template <class K>
-static inline int direct_grid(K kernel, size_t smem, int sm_count, int64_t nrows, int threads = DIRECT_THREADS) {
-    int per_sm = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-    const int64_t want = ((nrows + 3) / 4 + threads - 1) / threads;
-    const int64_t full = (int64_t)per_sm * sm_count;  // persistent grid: whole CTAs per SM x the device's SMs (132 on H100 SXM)
-    return (int)(want < full ? want : full);
+static inline cudaError_t launch_persistent(K kernel, const AggArgs& a, size_t smem, int sm_count, int threads, cudaStream_t s, cudaEvent_t start) {
+    int dev = 0, per_sm = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    {
+        LaunchSetupCache& c = launch_setup_cache();
+        std::lock_guard<std::mutex> g(c.mu);
+        if (smem > 48 * 1024) {
+            size_t& have = c.smem_set[{dev, (const void*)kernel}];
+            if (smem > have) {
+                if ((e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
+                have = smem;
+            }
+        }
+        const auto key = std::make_tuple(dev, (const void*)kernel, threads, smem);
+        const auto it = c.per_sm.find(key);
+        if (it != c.per_sm.end()) per_sm = it->second;
+        else {
+            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+            c.per_sm[key] = per_sm;
+        }
+    }
+    const int64_t want = ((a.nrows + 3) / 4 + threads - 1) / threads;
+    const int64_t full = (int64_t)per_sm * sm_count;
+    if (start) cudaEventRecord(start, s);
+    kernel<<<(int)(want < full ? want : full), threads, smem, s>>>(a);
+    return cudaGetLastError();
 }
 
 template <int NP, int NA>
 static inline cudaError_t launch_wp(const AggArgs& a, int sm_count, cudaStream_t s);   // agg_wp.cuh
 
 template <int NP, int NA>
-static inline cudaError_t launch_direct(const AggArgs& a, int sm_count, size_t smem, cudaStream_t s, bool grouped) {
-    if (grouped && a.wp) return launch_wp<NP, NA>(a, sm_count, s);
-    if (grouped) {
-        if (smem > 48 * 1024) {
-            cudaError_t e = cudaFuncSetAttribute(k_agg_group_direct<NP, NA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            if (e != cudaSuccess) return e;
-        }
-        if (a.lean) {
-            if (smem > 48 * 1024) {
-                cudaError_t e = cudaFuncSetAttribute(k_agg_group_lean<NP, NA, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                if (e == cudaSuccess) e = cudaFuncSetAttribute(k_agg_group_lean<NP, NA, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                if (e != cudaSuccess) return e;
-            }
-            int grid = a.jp.mode ? direct_grid(k_agg_group_lean<NP, NA, true>, smem, sm_count, a.nrows, LEAN_THREADS)
-                                 : direct_grid(k_agg_group_lean<NP, NA, false>, smem, sm_count, a.nrows, LEAN_THREADS);
-            if (a.lean_mm) {
-                cudaError_t e = cudaFuncSetAttribute(k_agg_group_lean<NP, NA, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                if (e != cudaSuccess) return e;
-                // (one instantiation serves batches with and without NULLs: without bitmaps the NULL masks are simply zero)
-                k_agg_group_lean<NP, NA, false, true, true><<<direct_grid(k_agg_group_lean<NP, NA, false, true, true>, smem, sm_count, a.nrows, LEAN_THREADS), LEAN_THREADS, smem, s>>>(a);
-            }
-            else if (a.lean_nulls) {
-                cudaError_t e = cudaFuncSetAttribute(k_agg_group_lean<NP, NA, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                if (e != cudaSuccess) return e;
-                k_agg_group_lean<NP, NA, false, true><<<direct_grid(k_agg_group_lean<NP, NA, false, true>, smem, sm_count, a.nrows, LEAN_THREADS), LEAN_THREADS, smem, s>>>(a);
-            }
-            else if (NA >= 1 && a.lean_fx) {   // double sums as fixed-point limbs (native 32-bit shared atomics)
-                if constexpr (NA >= 1) {
-                    cudaError_t e = cudaFuncSetAttribute(k_agg_group_lean<NP, NA, false, false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_agg_group_lean<NP, NA, true, false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                    if (e != cudaSuccess) return e;
-                    if (a.jp.mode) k_agg_group_lean<NP, NA, true, false, false, false, true><<<direct_grid(k_agg_group_lean<NP, NA, true, false, false, false, true>, smem, sm_count, a.nrows, LEAN_THREADS), LEAN_THREADS, smem, s>>>(a);
-                    else k_agg_group_lean<NP, NA, false, false, false, false, true><<<direct_grid(k_agg_group_lean<NP, NA, false, false, false, false, true>, smem, sm_count, a.nrows, LEAN_THREADS), LEAN_THREADS, smem, s>>>(a);
-                }
-            }
-            else if (a.jp.mode) k_agg_group_lean<NP, NA, true><<<grid, LEAN_THREADS, smem, s>>>(a);
-            else if (NA <= 2 && a.lean_bank) {
-                if constexpr (NA <= 2) {
-                    cudaError_t e = cudaFuncSetAttribute(k_agg_group_lean<NP, NA, false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                    if (e != cudaSuccess) return e;
-                    k_agg_group_lean<NP, NA, false, false, false, true><<<direct_grid(k_agg_group_lean<NP, NA, false, false, false, true>, smem, sm_count, a.nrows, LEAN_THREADS), LEAN_THREADS, smem, s>>>(a);
-                }
-            }
-            else k_agg_group_lean<NP, NA, false><<<grid, LEAN_THREADS, smem, s>>>(a);
-        } else
-        k_agg_group_direct<NP, NA><<<direct_grid(k_agg_group_direct<NP, NA>, smem, sm_count, a.nrows), DIRECT_THREADS, smem, s>>>(a);
-    } else {
-        k_agg_scalar_direct<NP, NA><<<direct_grid(k_agg_scalar_direct<NP, NA>, 0, sm_count, a.nrows), DIRECT_THREADS, 0, s>>>(a);
+static inline cudaError_t launch_direct(const AggArgs& a, int sm_count, size_t smem, cudaStream_t s, bool grouped, cudaEvent_t start) {
+    if (grouped && a.wp) { if (start) cudaEventRecord(start, s); return launch_wp<NP, NA>(a, sm_count, s); }
+    if (!grouped) return launch_persistent(k_agg_scalar_direct<NP, NA>, a, 0, sm_count, DIRECT_THREADS, s, start);
+    if (!a.lean) return launch_persistent(k_agg_group_direct<NP, NA>, a, smem, sm_count, DIRECT_THREADS, s, start);
+    constexpr int T = LEAN_THREADS;
+    // (one MM / NULLS instantiation serves batches with and without NULLs: without bitmaps the NULL masks are simply zero)
+    if (a.lean_mm) return launch_persistent(k_agg_group_lean<NP, NA, false, true, true>, a, smem, sm_count, T, s, start);
+    if (a.lean_nulls) return launch_persistent(k_agg_group_lean<NP, NA, false, true>, a, smem, sm_count, T, s, start);
+    if constexpr (NA >= 1) {   // double sums as fixed-point limbs (native 32-bit shared atomics)
+        if (a.lean_fx) return a.jp.mode ? launch_persistent(k_agg_group_lean<NP, NA, true, false, false, false, true>, a, smem, sm_count, T, s, start)
+                                        : launch_persistent(k_agg_group_lean<NP, NA, false, false, false, false, true>, a, smem, sm_count, T, s, start);
     }
-    return cudaGetLastError();
+    if (a.jp.mode) return launch_persistent(k_agg_group_lean<NP, NA, true>, a, smem, sm_count, T, s, start);
+    if constexpr (NA <= 2) {
+        if (a.lean_bank) return launch_persistent(k_agg_group_lean<NP, NA, false, false, false, true>, a, smem, sm_count, T, s, start);
+    }
+    return launch_persistent(k_agg_group_lean<NP, NA, false>, a, smem, sm_count, T, s, start);
 }
 template <int NP>
-static inline cudaError_t launch_direct_np(const AggArgs& a, int na, int sm_count, size_t smem, cudaStream_t s, bool grouped) {
+static inline cudaError_t launch_direct_np(const AggArgs& a, int na, int sm_count, size_t smem, cudaStream_t s, bool grouped, cudaEvent_t start) {
     switch (na) {
-        case 0: return launch_direct<NP, 0>(a, sm_count, smem, s, grouped);
-        case 1: return launch_direct<NP, 1>(a, sm_count, smem, s, grouped);
-        case 2: return launch_direct<NP, 2>(a, sm_count, smem, s, grouped);
-        case 3: return launch_direct<NP, 3>(a, sm_count, smem, s, grouped);
-        default: return launch_direct<NP, 4>(a, sm_count, smem, s, grouped);
+        case 0: return launch_direct<NP, 0>(a, sm_count, smem, s, grouped, start);
+        case 1: return launch_direct<NP, 1>(a, sm_count, smem, s, grouped, start);
+        case 2: return launch_direct<NP, 2>(a, sm_count, smem, s, grouped, start);
+        case 3: return launch_direct<NP, 3>(a, sm_count, smem, s, grouped, start);
+        default: return launch_direct<NP, 4>(a, sm_count, smem, s, grouped, start);
     }
 }
 

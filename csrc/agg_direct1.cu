@@ -3,7 +3,7 @@
 #include "agg_wp.cuh"
 
 namespace bk {
-cudaError_t launch_direct_np1(const AggArgs& a, int na, int sm_count, size_t smem, cudaStream_t s, bool grouped) {
-    return launch_direct_np<1>(a, na, sm_count, smem, s, grouped);
+cudaError_t launch_direct_np1(const AggArgs& a, int na, int sm_count, size_t smem, cudaStream_t s, bool grouped, cudaEvent_t start) {
+    return launch_direct_np<1>(a, na, sm_count, smem, s, grouped, start);
 }
 }  // namespace bk

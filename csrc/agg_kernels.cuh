@@ -109,5 +109,81 @@ __device__ __forceinline__ void smem_table_flush(const SmemTable& t, const AggAr
     }
 }
 
+// ------------------------------------------------------------------------------------------
+// result extraction: one output row per group.  Output columns (canonical 64-bit images + one null
+// byte each, column-major with stride `stride`), in this order: group expressions, then per aggregate
+// its final value and, for AVG, the intermediate {sum, count} pair (AggFnCall::finalize,
+// agg_fn_call.cpp:927-990).  Reads go to L2 (ld.cg): the fused caller runs in the launch that updated the table.  Every key word
+// and lane of the slot is loaded before the first store, so a group costs one round trip to L2, not one per output column.
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ void extract_group(const GroupTable& gt, const AggPlan& ap, uint32_t i, uint32_t pos, uint64_t* outv, uint8_t* outn, uint32_t stride) {
+    const uint32_t cap = gt.cap_mask + 1;
+    uint64_t kw[MAX_KEYW], lw[MAX_LANES];
+#pragma unroll 4
+    for (int w = 0; w < ap.n_keyw; w++) kw[w] = __ldcg((const unsigned long long*)gt.keys + (size_t)w * cap + i);
+#pragma unroll 4
+    for (int l = 0; l < ap.n_lanes; l++) lw[l] = __ldcg((const unsigned long long*)gt.lanes + (size_t)l * cap + i);
+    const uint64_t nrows = lw[0];
+    int c = 0;
+    for (int g = 0; g < ap.n_group; g++, c++) {
+        const bool isnull = ap.key_null_word[g] != 0xFF && ((kw[ap.key_null_word[g]] >> ap.key_null_shift[g]) & 1ull);
+        uint64_t v = kw[ap.key_word[g]] >> ap.key_shift[g];
+        if (ap.key_bits[g] < 64) v &= (1ull << ap.key_bits[g]) - 1ull;
+        // sign-extend narrow signed keys back to their canonical image
+        if (ap.key_bits[g] == 32 && prim_class(ap.key_prim[g]) == VC_I64) v = (uint64_t)(int64_t)(int32_t)v;
+        outv[(size_t)c * stride + pos] = isnull ? 0 : v;
+        outn[(size_t)c * stride + pos] = isnull ? 1 : 0;
+    }
+    for (int k = 0; k < ap.n_agg; k++) {
+        const AggSpec a = ap.agg[k];
+        if (a.hidden) continue;
+        const uint64_t cnt = a.cnt_lane < ap.n_lanes ? lw[a.cnt_lane] : 0;   // (lane 0 = the group's row count)
+        const uint64_t acc = a.acc_lane < ap.n_lanes ? lw[a.acc_lane] : 0;
+        uint64_t v = 0; uint8_t isnull = 0;
+        switch (a.kind) {
+            case AG_COUNT_STAR: v = nrows; break;
+            case AG_COUNT: v = cnt; break;
+            case AG_COUNT_MERGE: v = acc; break;
+            case AG_AVG:
+                if (cnt == 0) isnull = 1; else v = f64_bits(__ddiv_rn(bits_f64(acc), (double)(int64_t)cnt));
+                break;
+            default: if (cnt == 0) isnull = 1; else v = acc; break;  // SUM / MIN / MAX: NULL without input
+        }
+        outv[(size_t)c * stride + pos] = v; outn[(size_t)c * stride + pos] = isnull; c++;
+        if (a.kind == AG_AVG) {  // intermediate blob {double sum; int64 count}
+            // the blank row of an empty scalar aggregate initialises only its counts (agg_node.cpp:489-503): blob stays NULL
+            outv[(size_t)c * stride + pos] = acc; outn[(size_t)c * stride + pos] = (ap.n_keyw == 0 && nrows == 0) ? 1 : 0; c++;
+            outv[(size_t)c * stride + pos] = cnt; outn[(size_t)c * stride + pos] = 0; c++;
+        }
+    }
+}
+
+// The end of a grouped launch that extracts its own result (AggArgs::fused_out): every CTA takes a ticket once its table updates are
+// done; the CTA that draws the last one sees the whole table and writes the counter block and every group's row straight into the
+// mapped host buffer, so the request needs no extraction kernel and no copies after it.  Each launch of a multi-batch request
+// overwrites the previous launch's rows; the host reads them only after the last.  The table itself is left as it is (it stays the
+// request's partial state until bkgpu_reset clears it).
+__device__ __forceinline__ void fused_extract(const AggArgs& a) {
+    __shared__ uint32_t is_last;
+    __threadfence();   // this thread's table updates, before the CTA's ticket
+    __syncthreads();
+    if (threadIdx.x == 0) is_last = atomicAdd(a.gt.n_groups + GT_TICKET, 1u) == gridDim.x - 1;
+    __syncthreads();
+    if (!is_last) return;
+    __threadfence();
+    const GroupTable& gt = a.gt;
+    const AggPlan& ap = a.plan;
+    const uint32_t n = __ldcg(gt.n_groups);
+    uint32_t* ctr = (uint32_t*)a.fused_out;
+    if (threadIdx.x < GT_OCC_OFF) ctr[threadIdx.x] = threadIdx.x == GT_TICKET ? 0u : __ldcg(gt.n_groups + threadIdx.x);
+    if (threadIdx.x == 0) gt.n_groups[GT_TICKET] = 0u;   // (every CTA has drawn: the next launch of the request starts from 0)
+    if (n > a.fused_cap) return;
+    int n_img = ap.n_group;
+    for (int k = 0; k < ap.n_agg; k++) if (!ap.agg[k].hidden) n_img += ap.agg[k].kind == AG_AVG ? 3 : 1;
+    uint64_t* outv = (uint64_t*)(a.fused_out + 32);
+    uint8_t* outn = (uint8_t*)(outv + (size_t)n_img * n);
+    for (uint32_t j = threadIdx.x; j < n; j += blockDim.x) extract_group(gt, ap, __ldcg(gt.n_groups + GT_OCC_OFF + j), j, outv, outn, n);
+}
+
 
 }  // namespace bk

@@ -99,7 +99,10 @@ struct bkgpu_plan {
     std::vector<cudaEvent_t> event_pool;
     uint64_t* h_outv = nullptr; uint8_t* h_outn = nullptr; size_t h_out_cap = 0;   // pinned landing area of the extracted rows
     uint32_t known_groups = 0;
-    uint32_t* h_pinned = nullptr;   // [0] groups seen (async copy after every aggregate launch), pinned
+    uint32_t* h_pinned = nullptr;   // [0] groups seen (async copy after every aggregate launch that does not extract its result), pinned
+    // mapped host buffer the lean kernel's last CTA extracts the result into (AggArgs::fused_out), and whether the request's last
+    // aggregate launch did so: then bkgpu_finish only waits and reads it
+    uint8_t* h_fused = nullptr; uint8_t* d_fused = nullptr; size_t fused_bytes = 0; uint32_t fused_cap = 0; bool fused_last = false;
     // hash join (K4): retained build side + multimap
     std::vector<uint8_t*> jb_vals, jb_nullbytes, jb_bitmap;   // per plan column (side 1 only)
     std::vector<bool> jb_has_null;
@@ -208,6 +211,31 @@ struct DevCache {
     }
 };
 DevCache& dev_cache() { static DevCache c; return c; }
+// the mapped host buffers of the fused extraction (bkgpu_plan::h_fused) are kept the same way: pinning and unpinning one costs a
+// plan's open and close about a tenth of a millisecond
+struct MappedCache {
+    std::mutex mu;
+    std::multimap<size_t, uint8_t*> free_;
+    uint8_t* take(size_t bytes) {
+        std::lock_guard<std::mutex> g(mu);
+        auto it = free_.find(bytes);
+        if (it == free_.end()) return nullptr;
+        uint8_t* q = it->second; free_.erase(it);
+        return q;
+    }
+    bool put(size_t bytes, uint8_t* q) {
+        std::lock_guard<std::mutex> g(mu);
+        if (dev_cache().off || free_.size() >= 64) return false;
+        free_.insert({bytes, q});
+        return true;
+    }
+    void release_all() {
+        std::lock_guard<std::mutex> g(mu);
+        for (auto& kv : free_) cudaFreeHost(kv.second);
+        free_.clear();
+    }
+};
+MappedCache& mapped_cache() { static MappedCache c; return c; }
 size_t size_class(size_t b) {   // eight classes per power of two: at most 12.5 % slack
     if (b < 256) return 256;
     size_t p2 = 1; while (p2 < b) p2 <<= 1;
@@ -215,7 +243,7 @@ size_t size_class(size_t b) {   // eight classes per power of two: at most 12.5 
     return (b + step - 1) / step * step;
 }
 }  // namespace
-extern "C" void bkgpu_release_cache(void) { dev_cache().release_all(); }
+extern "C" void bkgpu_release_cache(void) { dev_cache().release_all(); mapped_cache().release_all(); }
 
 static int dev_alloc(bkgpu_plan* p, void** out, size_t bytes) {
     const size_t sc = size_class(bytes ? bytes : 8);
@@ -249,14 +277,15 @@ static int ensure_buf(bkgpu_plan* p, void** ptr, size_t* cap, size_t bytes) {
     if (rc == BKGPU_OK) *cap = bytes;
     return rc;
 }
-static EventPair* timer_begin(bkgpu_plan* p, std::vector<EventPair>& v, int64_t bytes) {
+// record = false: the caller records ep->a itself (right before its launch)
+static EventPair* timer_begin(bkgpu_plan* p, std::vector<EventPair>& v, int64_t bytes, bool record = true) {
     EventPair ep{};
     for (cudaEvent_t* e : {&ep.a, &ep.b}) {   // events are recycled: a re-armed plan launches the same kernels again and again
         if (!p->event_pool.empty()) { *e = p->event_pool.back(); p->event_pool.pop_back(); }
         else if (cudaEventCreate(e) != cudaSuccess) return nullptr;
     }
     ep.bytes = bytes;
-    cudaEventRecord(ep.a, p->stream);
+    if (record) cudaEventRecord(ep.a, p->stream);
     v.push_back(ep);
     return &v.back();
 }
@@ -367,6 +396,13 @@ extern "C" int bkgpu_open(bkgpu_plan* p) {
     return BKGPU_OK;
 }
 
+// the group count an earlier launch left in pinned memory: the 4-byte copy after a launch, or the counter block of a fused extraction
+// (read without a synchronisation: a stale value only costs speed)
+static void learn_groups(bkgpu_plan* p) {
+    if (p->h_pinned && p->h_pinned[0] > p->known_groups) p->known_groups = p->h_pinned[0];
+    if (p->h_fused) { const uint32_t g = *(const volatile uint32_t*)p->h_fused; if (g > p->known_groups) p->known_groups = g; }
+}
+
 // choose the shared-table capacity for this batch: >= 2x the groups seen so far, 2048 slots when
 // nothing is known yet, 0 (straight to the global table) when the groups cannot fit one CTA's 227 KB
 static int pick_smem_log2(bkgpu_plan* p, int n_smem_lanes, bool direct, int na) {
@@ -374,13 +410,41 @@ static int pick_smem_log2(bkgpu_plan* p, int n_smem_lanes, bool direct, int na) 
     const size_t budget = 220 * 1024;
     auto bytes = [&](int log2) { return direct ? direct_smem_bytes(p->c.ap.n_keyw, n_smem_lanes, log2, na) : agg_smem_bytes(p->c.ap.n_keyw, n_smem_lanes, log2); };
     if (p->smem_cap_log2 >= 0) { int l = p->smem_cap_log2; while (l > 0 && bytes(l) > budget) l--; return l; }
-    if (p->h_pinned && p->h_pinned[0] > p->known_groups) p->known_groups = p->h_pinned[0];
+    learn_groups(p);
     uint32_t g = p->known_groups;
     int log2 = 11;
     while (((uint32_t)1 << log2) < 2 * g && log2 < 14) log2++;
     while (log2 > 0 && bytes(log2) > budget) log2--;
     if (((uint32_t)1 << log2) < g) return 0;  // would mostly miss: skip the shared table
     return log2;
+}
+
+// device images of an extracted row: one per group expression, per aggregate its final value (+2 for an AVG blob)
+static int agg_n_img(const AggPlan& ap) {
+    int n = ap.n_group;
+    for (int k = 0; k < ap.n_agg; k++) if (!ap.agg[k].hidden) n += ap.agg[k].kind == AG_AVG ? 3 : 1;
+    return n;
+}
+
+// the mapped host buffer of the fused extraction, sized for the groups seen so far (at least 2048 rows); false = too many groups
+// to extract this way (the table is then read back by k_extract)
+static bool ensure_fused(bkgpu_plan* p) {
+    uint32_t want = 2048;
+    while (want < p->known_groups && want < (1u << 16)) want *= 2;
+    if (want < p->known_groups) return false;
+    if (p->h_fused && p->fused_cap >= want) return true;
+    if (p->h_fused) {   // (a launch still running may write into it)
+        cudaStreamSynchronize(p->stream);
+        if (!mapped_cache().put(p->fused_bytes, p->h_fused)) cudaFreeHost(p->h_fused);
+        p->h_fused = p->d_fused = nullptr; p->fused_cap = 0;
+    }
+    const size_t bytes = 32 + (size_t)want * (size_t)agg_n_img(p->c.ap) * 9;
+    uint8_t* h = mapped_cache().take(bytes);
+    if (!h && cudaHostAlloc((void**)&h, bytes, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) { cudaGetLastError(); return false; }
+    if (cudaHostGetDevicePointer((void**)&p->d_fused, h, 0) != cudaSuccess) { cudaGetLastError(); cudaFreeHost(h); return false; }
+    memset(h, 0, 32);
+    p->h_fused = h; p->fused_bytes = bytes; p->fused_cap = want;
+    return true;
 }
 
 // `jp`: fused FK -> PK probe (lean kernel only); returns +1 without launching when this batch does not fit the lean kernel
@@ -510,7 +574,7 @@ static int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols
         const DevCol& kc = a.cols[np];
         bool ok = kc.stype == ST_I32 || kc.stype == ST_U32;
         for (int v = 0; v < na && ok; v++) ok = a.vops[v].n_ops == 1 && (a.vops[v].op[0] == LN_ADD_F64 || a.vops[v].op[0] == LN_ADD_I64);
-        if (p->h_pinned && p->h_pinned[0] > p->known_groups) p->known_groups = p->h_pinned[0];
+        learn_groups(p);
         if (ok) {
             const size_t budget = 226 * 1024;
             const uint32_t g = p->known_groups;
@@ -531,6 +595,10 @@ static int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols
             if (fits(gcap, kl)) { a.wp = 1; a.wp_gcap = (int)gcap; a.wp_kt_log2 = kl; a.wp_warps = warps; a.wp_dense = 0; a.wp_dense_sub = 0; }
         }
     }
+    // a lean launch on one rank whose rows go straight to the host extracts its own result: any of them may be the request's last
+    if (direct && a.lean && !a.wp && a.plan.n_keyw > 0 && !(p->nccl_comm && p->nranks > 1) && !p->c.post && ensure_fused(p)) {
+        a.fused_out = p->d_fused; a.fused_cap = p->fused_cap;
+    }
     const int64_t kMax = (int64_t)1 << 30;  // rows per launch (32-bit counters inside a CTA)
     int64_t algo_bytes_per_row = 0;
     for (int i = 0; i < a.n_cols; i++) algo_bytes_per_row += storage_bytes(a.cols[i].stype);
@@ -542,9 +610,10 @@ static int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols
             if (a.cols[i].validity) b.cols[i].validity = a.cols[i].validity + off / 8;
         }
         const char* name = "";
-        EventPair* ep = timer_begin(p, p->timed, b.nrows * algo_bytes_per_row);
-        cudaError_t e = launch_agg(b, direct, p->sm_count, p->stream, &name);
+        EventPair* ep = timer_begin(p, p->timed, b.nrows * algo_bytes_per_row, false);
+        cudaError_t e = launch_agg(b, direct, p->sm_count, p->stream, ep ? ep->a : nullptr, &name);
         timer_end(p, ep);
+        p->fused_last = b.fused_out != nullptr;
         if (e != cudaSuccess) return p->cuda_fail(e, "launch_agg");
         snprintf(p->stats.main_kernel_name, sizeof p->stats.main_kernel_name, "%s", b.wp && direct ? "k_agg_group_wp" : (b.lean && direct ? (b.lean_fx ? "k_agg_group_lean_fx" : "k_agg_group_lean") : name));
         p->stats.kernel_launches++;
@@ -1183,8 +1252,10 @@ static int bkgpu_push_impl(bkgpu_plan* p, const bkgpu_column* cols, int ncols, i
         case PK_AGG: {
             int rc = feed(p, p->c.cols, cols, ncols, nrows, on_device, agg_batch);
             if (rc) return rc;
-            if (p->c.ap.n_keyw > 0 && p->smem_cap_log2 < 0 && p->h_pinned)   // learn the cardinality for later batches' table size;
-                CK(p, cudaMemcpyAsync(p->h_pinned, p->gt.n_groups, 4, cudaMemcpyDeviceToHost, p->stream));  // no sync: a stale value only costs speed
+            // learn the cardinality for later batches' table size (no sync: a stale value only costs speed); a launch that extracted its
+            // result has already left the count in h_fused
+            if (p->c.ap.n_keyw > 0 && p->smem_cap_log2 < 0 && p->h_pinned && !p->fused_last)
+                CK(p, cudaMemcpyAsync(p->h_pinned, p->gt.n_groups, 4, cudaMemcpyDeviceToHost, p->stream));
             return BKGPU_OK;
         }
         case PK_JOIN_AGG: case PK_JOIN: return join_push(p, cols, ncols, nrows, on_device);
@@ -1193,18 +1264,6 @@ static int bkgpu_push_impl(bkgpu_plan* p, const bkgpu_column* cols, int ncols, i
     }
 }
 
-// ---- result materialisation: device images -> typed host columns ----
-static void put_value(HostCol& hc, int64_t row, uint64_t bits, bool isnull, int prim) {
-    uint8_t* dst = hc.values.data() + (size_t)row * (size_t)hc.elem;
-    if (isnull) { hc.validity[(size_t)row >> 3] &= (uint8_t)~(1u << (row & 7)); return; }
-    switch (prim_storage(prim)) {
-        case ST_I32: { int32_t v = (int32_t)(int64_t)bits; memcpy(dst, &v, 4); } break;
-        case ST_U32: { uint32_t v = (uint32_t)bits; memcpy(dst, &v, 4); } break;
-        case ST_F32: { double d; memcpy(&d, &bits, 8); float f = (float)d; memcpy(dst, &f, 4); } break;
-        case ST_U8: dst[0] = bits ? 1 : 0; break;
-        default: memcpy(dst, &bits, 8); break;
-    }
-}
 
 // One-time setup of the peer-memory merge: allocate this rank's buffer, trade CUDA IPC handles through the communicator, map the peers'.
 static int peer_setup(bkgpu_plan* p, size_t seg_words) {
@@ -1365,6 +1424,74 @@ static int agg_post(bkgpu_plan* p, uint32_t n_out, uint32_t out_cap) {
     return BKGPU_OK;
 }
 
+// the one wait of a request.  With several ranks on a host whose CPU budget is small (8 ranks under a 16-CPU cgroup quota: two CPUs per
+// rank for the python thread, NCCL's proxy thread and this wait) a spinning wait burns the quota the other ranks' launches need:
+// there the thread sleeps on a blocking-sync event instead (option blocking_sync: -1 auto, 0 spin, 1 sleep)
+static int agg_wait(bkgpu_plan* p) {
+    const double t0 = HostClock::now();
+    if (p->blocking_wait) {
+        if (!p->wait_event) CK(p, cudaEventCreateWithFlags(&p->wait_event, cudaEventBlockingSync | cudaEventDisableTiming));
+        CK(p, cudaEventRecord(p->wait_event, p->stream));
+        CK(p, cudaEventSynchronize(p->wait_event));
+    } else CK(p, cudaStreamSynchronize(p->stream));
+    p->hclk.extract_wait += HostClock::now() - t0;
+    return BKGPU_OK;
+}
+
+// what the counter block of a finished request tells the plan: rows that passed, FX's exact-path count, the groups it holds
+static int agg_take_counters(bkgpu_plan* p, const uint32_t* ctr) {
+    memcpy(&p->rows_passed_host, ctr + 4, 8);
+    // FX: values beyond the sampled scale are added exactly, one global atomic each; a plan whose double columns keep producing many of them
+    // (a column spanning dozens of binades, outliers dominating the sample) goes back to the CAS kernel for its later launches
+    if (ctr[GT_FX_EXACT] > 4096 && (uint64_t)ctr[GT_FX_EXACT] * 64 > (uint64_t)std::max<int64_t>(p->rows_passed_host, 1)) p->fx_off = 1;
+    if (ctr[1]) return p->fail(BKGPU_ETOOBIG, "group table overflow (capacity 2^%d slots / partial_capacity %lld): raise group_capacity_log2",
+                               (int)p->gt.cap_log2, (long long)p->partial_cap);
+    if (ctr[0] > p->known_groups) p->known_groups = ctr[0];
+    p->finish_groups = ctr[0];
+    return BKGPU_OK;
+}
+
+// typed host columns from `n_out` extracted rows (images + null bytes, column-major with stride `stride`), after OFFSET / LIMIT
+static void agg_result(bkgpu_plan* p, const uint64_t* hv, const uint8_t* hn, size_t stride, uint32_t n_out) {
+    const int64_t rows = n_out;
+    const int64_t skip = p->c.offset > 0 ? std::min<int64_t>(p->c.offset, rows) : 0;
+    int64_t lim = p->c.agg_limit;   // AggNode::get_next stops at its limit (agg_node.cpp:555)
+    if (p->c.limit >= 0 && (lim < 0 || p->c.limit < lim)) lim = p->c.limit;
+    int64_t keep = rows - skip;
+    if (lim >= 0 && keep > lim) keep = lim;
+    p->result.clear();
+    int img = 0;
+    for (const OutCol& oc : p->c.out_cols) {
+        HostCol hc; hc.desc = oc;
+        hc.elem = oc.kind == 1 ? 16 : storage_bytes(prim_storage(oc.prim));
+        hc.values.assign((size_t)std::max<int64_t>(keep, 1) * (size_t)hc.elem, 0);
+        const uint64_t* v = hv + (size_t)img * stride + skip;
+        const uint8_t* nb = hn + (size_t)img * stride + skip;
+        // (a NULL's image is 0, which is also what a NULL row's value bytes hold)
+        uint8_t* d = hc.values.data();
+        if (oc.kind == 1) {
+            const uint64_t* v2 = hv + (size_t)(img + 1) * stride + skip;
+            for (int64_t r = 0; r < keep; r++) { memcpy(d + (size_t)r * 16, v + r, 8); memcpy(d + (size_t)r * 16 + 8, v2 + r, 8); }
+        } else switch (prim_storage(oc.prim)) {
+            case ST_I32: for (int64_t r = 0; r < keep; r++) { const int32_t x = (int32_t)(int64_t)v[r]; memcpy(d + (size_t)r * 4, &x, 4); } break;
+            case ST_U32: for (int64_t r = 0; r < keep; r++) { const uint32_t x = (uint32_t)v[r]; memcpy(d + (size_t)r * 4, &x, 4); } break;
+            case ST_F32: for (int64_t r = 0; r < keep; r++) { double x; memcpy(&x, v + r, 8); const float f = (float)x; memcpy(d + (size_t)r * 4, &f, 4); } break;
+            case ST_U8: for (int64_t r = 0; r < keep; r++) d[r] = v[r] ? 1 : 0; break;
+            default:
+                if (hc.elem == 8) { if (keep > 0) memcpy(d, v, (size_t)keep * 8); }
+                else for (int64_t r = 0; r < keep; r++) memcpy(d + (size_t)r * hc.elem, v + r, 8);
+                break;
+        }
+        if (keep > 0 && memchr(nb, 1, (size_t)keep)) {
+            hc.validity.assign((size_t)(keep + 7) / 8 + 1, 0xFF);
+            for (int64_t r = 0; r < keep; r++) if (nb[r]) { hc.validity[(size_t)r >> 3] &= (uint8_t)~(1u << (r & 7)); if (oc.kind != 1) memset(d + (size_t)r * hc.elem, 0, (size_t)hc.elem); }
+        }
+        img += oc.kind == 1 ? 2 : 1;
+        p->result.push_back(std::move(hc));
+    }
+    p->result_rows = keep; p->result_pos = 0;
+}
+
 static int agg_finish(bkgpu_plan* p) {
     const AggPlan& ap = p->c.ap;
     GroupTable& gt = p->gt;
@@ -1372,10 +1499,22 @@ static int agg_finish(bkgpu_plan* p) {
     uint64_t* finish_hv = nullptr; uint8_t* finish_hn = nullptr; uint32_t finish_n_out = 0, finish_out_cap = 0;
     const bool multi = p->nccl_comm && p->nranks > 1;
     bool rows_mode = false;
-    // device images: one per group expr, per aggregate its final (+2 for an AVG blob)
-    int n_img = ap.n_group;
-    for (int k = 0; k < ap.n_agg; k++) if (!ap.agg[k].hidden) n_img += ap.agg[k].kind == AG_AVG ? 3 : 1;
+    const int n_img = agg_n_img(ap);
     int rc;
+    // the request ended with a launch that extracted its own result into mapped host memory: one wait, nothing else on the device
+    if (p->fused_last && !multi && !p->c.post) {
+        if ((rc = agg_wait(p))) return rc;
+        const uint32_t* ctr = (const uint32_t*)p->h_fused;
+        if ((rc = agg_take_counters(p, ctr))) return rc;
+        const uint32_t n = ctr[0];
+        if (n <= p->fused_cap) {
+            p->stats.d2h_bytes += (int64_t)(32 + (size_t)n * (size_t)n_img * 9);
+            const uint64_t* hv = (const uint64_t*)(p->h_fused + 32);
+            agg_result(p, hv, (const uint8_t*)(hv + (size_t)n * (size_t)n_img), n, n);
+            return BKGPU_OK;
+        }
+        // more groups than the buffer holds: the table is read back below (the next launch's buffer is sized for them)
+    }
   for (int mtry = 0; mtry < 3; mtry++) {   // (a second trip only when some rank held more groups than the exchange was sized for)
     { const double t0 = HostClock::now(); if (multi && (rc = agg_collective(p, &rows_mode))) return rc; p->hclk.collective += HostClock::now() - t0; }
     uint32_t n_out = 0, out_cap = 0, merge_max = 0;
@@ -1414,22 +1553,8 @@ static int agg_finish(bkgpu_plan* p) {
             CK(p, cudaMemcpyAsync(hv, p->d_outv, n_words * 8, cudaMemcpyDeviceToHost, p->stream));
             CK(p, cudaMemcpyAsync(hn, p->d_outn, n_words, cudaMemcpyDeviceToHost, p->stream));
         }
-        {   // the one wait of the request.  With several ranks on a host whose CPU budget is small (8 ranks under a 16-CPU cgroup quota: two CPUs per
-            // rank for the python thread, NCCL's proxy thread and this wait) a spinning wait burns the quota the other ranks' launches need:
-            // there the thread sleeps on a blocking-sync event instead (option blocking_sync: -1 auto, 0 spin, 1 sleep)
-            const double t0 = HostClock::now();
-            if (p->blocking_wait) {
-                if (!p->wait_event) CK(p, cudaEventCreateWithFlags(&p->wait_event, cudaEventBlockingSync | cudaEventDisableTiming));
-                CK(p, cudaEventRecord(p->wait_event, p->stream));
-                CK(p, cudaEventSynchronize(p->wait_event));
-            } else CK(p, cudaStreamSynchronize(p->stream));
-            p->hclk.extract_wait += HostClock::now() - t0;
-        }
+        if ((rc = agg_wait(p))) return rc;
         host_counts[0] = hc3[0]; host_counts[1] = hc3[1]; n_out = hc3[2]; merge_max = hc3[3];
-        memcpy(&p->rows_passed_host, hc3 + 4, 8);
-        // FX: values beyond the sampled scale are added exactly, one global atomic each; a plan whose double columns keep producing many of them
-        // (a column spanning dozens of binades, outliers dominating the sample) goes back to the CAS kernel for its later launches
-        if (hc3[GT_FX_EXACT] > 4096 && (uint64_t)hc3[GT_FX_EXACT] * 64 > (uint64_t)std::max<int64_t>(p->rows_passed_host, 1)) p->fx_off = 1;
         if (p->peer_ready && p->h_pinned && p->h_pinned[6]) return p->fail(BKGPU_ENCCL, "peer merge: a rank did not publish its partial state within the time limit");
         if (rows_mode) {
             const uint32_t mx = merge_max;
@@ -1443,49 +1568,16 @@ static int agg_finish(bkgpu_plan* p) {
             if (learned > p->merge_bound) p->merge_bound = learned;
         }
         p->stats.d2h_bytes += (int64_t)(n_words * 9 + 12);
-        if (host_counts[1]) return p->fail(BKGPU_ETOOBIG, "group table overflow (capacity 2^%d slots / partial_capacity %lld): raise group_capacity_log2",
-                                           (int)gt.cap_log2, (long long)p->partial_cap);
-        if (host_counts[0] > p->known_groups) p->known_groups = host_counts[0];
-        p->finish_groups = host_counts[0];
+        if ((rc = agg_take_counters(p, hc3))) return rc;
         if (n_out <= out_cap) break;   // everything fitted
     }
     if (!redo_merge) { finish_hv = hv; finish_hn = hn; finish_n_out = n_out; finish_out_cap = out_cap; break; }
     if (mtry == 2) return p->fail(BKGPU_ENCCL, "partial-state exchange did not converge");
   }
-    uint64_t* hv = finish_hv; uint8_t* hn = finish_hn; uint32_t n_out = finish_n_out, out_cap = finish_out_cap;
+    uint32_t n_out = finish_n_out, out_cap = finish_out_cap;
     if (n_out > out_cap) n_out = out_cap;
     if (p->c.post) return agg_post(p, n_out, out_cap);
-    int64_t rows = n_out;
-    int64_t skip = p->c.offset > 0 ? std::min<int64_t>(p->c.offset, rows) : 0;
-    int64_t lim = p->c.agg_limit;   // AggNode::get_next stops at its limit (agg_node.cpp:555)
-    if (p->c.limit >= 0 && (lim < 0 || p->c.limit < lim)) lim = p->c.limit;
-    int64_t keep = rows - skip;
-    if (lim >= 0 && keep > lim) keep = lim;
-    p->result.clear();
-    int img = 0;
-    for (const OutCol& oc : p->c.out_cols) {
-        HostCol hc; hc.desc = oc;
-        hc.elem = oc.kind == 1 ? 16 : storage_bytes(prim_storage(oc.prim));
-        hc.values.assign((size_t)std::max<int64_t>(keep, 1) * (size_t)hc.elem, 0);
-        hc.validity.assign((size_t)(keep + 7) / 8 + 1, 0xFF);
-        bool any_null = false;
-        for (int64_t r = 0; r < keep; r++) {
-            const size_t src = (size_t)(r + skip);
-            if (oc.kind == 1) {
-                if (hn[(size_t)img * out_cap + src]) { any_null = true; hc.validity[(size_t)r >> 3] &= (uint8_t)~(1u << (r & 7)); }
-                memcpy(hc.values.data() + (size_t)r * 16, &hv[(size_t)img * out_cap + src], 8);
-                memcpy(hc.values.data() + (size_t)r * 16 + 8, &hv[(size_t)(img + 1) * out_cap + src], 8);
-            } else {
-                bool isnull = hn[(size_t)img * out_cap + src] != 0;
-                any_null |= isnull;
-                put_value(hc, r, hv[(size_t)img * out_cap + src], isnull, oc.prim);
-            }
-        }
-        if (!any_null) hc.validity.clear();
-        img += oc.kind == 1 ? 2 : 1;
-        p->result.push_back(std::move(hc));
-    }
-    p->result_rows = keep; p->result_pos = 0;
+    agg_result(p, finish_hv, finish_hn, out_cap, n_out);
     return BKGPU_OK;
 }
 
@@ -1540,7 +1632,8 @@ static int bkgpu_finish_impl(bkgpu_plan* p) {
         } break;
         default: rc = p->fail(BKGPU_EUNSUPPORTED, "plan kind %d cannot finish", p->c.kind);
     }
-    cudaStreamSynchronize(p->stream);
+    // (a finished aggregate without a post fragment has already waited for everything it queued: agg_wait)
+    if (rc || !((p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG) && !p->c.post)) cudaStreamSynchronize(p->stream);
     resolve_timers(p);
     if (rc) return rc;
     p->stats.rows_returned = p->result_rows;
@@ -1596,6 +1689,7 @@ static int bkgpu_reset_impl(bkgpu_plan* p) {
         if (p->state == S_FINISHED && p->finish_groups >= 0 && p->c.ap.n_keyw > 0) CK(p, launch_table_clear(p->gt, p->c.ap, (uint32_t)p->finish_groups, p->stream));
         else CK(p, launch_table_init(p->gt, p->c.ap, p->stream));
         p->finish_groups = -1;
+        p->fused_last = false;
         p->stats.kernel_launches++;
     }
     p->jb_rows = 0; p->jt_built = false; p->jt_generic = false; std::fill(p->jb_has_null.begin(), p->jb_has_null.end(), false);
@@ -1631,6 +1725,7 @@ extern "C" void bkgpu_close(bkgpu_plan* p) {
     if (p->wait_event) cudaEventDestroy(p->wait_event);
     if (p->h_pinned) cudaFreeHost(p->h_pinned);
     if (p->h_outv) cudaFreeHost(p->h_outv);
+    if (p->h_fused && !mapped_cache().put(p->fused_bytes, p->h_fused)) cudaFreeHost(p->h_fused);   // (the stream was drained above)
     if (p->copy_stream) cudaStreamDestroy(p->copy_stream);
     if (p->own_stream && p->stream) cudaStreamDestroy(p->stream);
     delete p;
@@ -1759,6 +1854,7 @@ extern "C" int bkgpu_partial_merge(bkgpu_plan* p, const void* dev_src, size_t by
     }
     CK(p, launch_table_init(p->gt, p->c.ap, p->stream, 1));
     CK(p, launch_partial_merge_rows(p->gt, p->c.ap, (const uint64_t*)dev_src, need / 8, eff_pcap(p), nranks, -1 /* fold every segment */, p->d_cursor + 1, p->stream));
+    p->fused_last = false;   // (the merged table is read back by k_extract)
     p->stats.kernel_launches += 2;
     void* comm = p->nccl_comm; int nr = p->nranks; p->nccl_comm = nullptr; p->nranks = 1;  // already merged: finalize locally
     rc = agg_finish(p);

@@ -163,8 +163,9 @@ struct GroupTable {
                          // re-initialisation, export and result extraction walk the groups that exist, not the table's capacity)
     uint32_t* overflow;  // = n_groups + 1: set when an insert could not find a free slot
 };
+constexpr int GT_TICKET = 6;    // word 6 of the counter block: CTAs of the running lean launch that have finished (fused_extract, agg_kernels.cuh); 0 between launches
 constexpr int GT_FX_EXACT = 7;  // word 7 of the counter block: double values the lean kernel's FX variant could not put on its fixed-point grid (agg_direct.cuh)
-constexpr int GT_OCC_OFF = 8;   // words 0-7 of the counter block: groups, overflow, result cursor, merge info, rows passed (u64), spare:
+constexpr int GT_OCC_OFF = 8;   // words 0-7 of the counter block: groups, overflow, result cursor, merge info, rows passed (u64), ticket, FX exact:
                                 // one 32-byte device-to-host copy brings every counter of a finished request back
 
 }  // namespace bk

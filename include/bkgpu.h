@@ -152,8 +152,9 @@ void  bkgpu_cancel(bkgpu_plan*);
 void  bkgpu_close(bkgpu_plan*);
 int   bkgpu_get_stats(bkgpu_plan*, bkgpu_stats* out);
 
-/* Device buffers of closed plans are kept in a process-wide cache and handed to the next plan (a store opens one plan per request;
- * cudaMalloc / cudaFree of the group table would cost milliseconds each).  This returns the cached memory to the driver.
+/* Device buffers (and the mapped host buffers GROUP BY results land in) of closed plans are kept in a process-wide cache and handed
+ * to the next plan (a store opens one plan per request; cudaMalloc / cudaFree of the group table would cost milliseconds each).  This
+ * returns the cached memory to the driver.
  * Environment BKGPU_NO_ALLOC_CACHE=1 disables the cache. */
 void  bkgpu_release_cache(void);
 
