@@ -133,6 +133,28 @@ def c3_dim(row0: int, n: int, n_dim: int, seed: int = 3, n_groups: int = 1000) -
             make_column(1, 2, T.INT32, gen_values(T.INT32, DIST_UNIFORM_INT, seed, 12, row0, n, 0, n_groups))]
 
 
+PART_KEY_STRIDE, PART_KEY_BASE = 7, 3   # part keys are sparse (stride 7): the join index is the packed table, not the dense array
+
+
+def c6_tables(n_fact: int, n_date: int = 2_556, n_part: int = 1_000_000, n_supp: int = 100_000, seed: int = 6):
+    """The star tables of config C6 (queries.STAR_TUPLES): date and supplier keys are a permutation of [0, n) (dense index), part keys
+    PART_KEY_BASE + PART_KEY_STRIDE * a permutation of [0, n) (sparse); the fact's foreign keys are drawn uniformly from those key sets.
+    Returns (fact, date, part, supplier) column lists."""
+    g = lambda pt, dist, cid, n, lo=0, hi=0: gen_values(pt, dist, seed, cid, 0, n, lo, hi)
+    dkey = g(T.INT32, DIST_PERMUTATION, 11, n_date, 0, n_date)
+    date = [make_column(1, 1, T.INT32, dkey), make_column(1, 2, T.INT32, (1992 + dkey // 365).astype(np.int32))]
+    pkey = (PART_KEY_BASE + PART_KEY_STRIDE * g(T.INT64, DIST_PERMUTATION, 21, n_part, 0, n_part)).astype(np.int32)
+    part = [make_column(2, 1, T.INT32, pkey), make_column(2, 2, T.INT32, g(T.INT32, DIST_UNIFORM_INT, 22, n_part, 0, 1000)),
+            make_column(2, 3, T.INT32, g(T.INT32, DIST_UNIFORM_INT, 23, n_part, 0, 25))]
+    supp = [make_column(3, 1, T.INT32, g(T.INT32, DIST_PERMUTATION, 31, n_supp, 0, n_supp)),
+            make_column(3, 2, T.INT32, g(T.INT32, DIST_UNIFORM_INT, 32, n_supp, 0, 5))]
+    fact = [make_column(0, 1, T.INT32, g(T.INT32, DIST_UNIFORM_INT, 1, n_fact, 0, n_date)),
+            make_column(0, 2, T.INT32, (PART_KEY_BASE + PART_KEY_STRIDE * g(T.INT64, DIST_UNIFORM_INT, 2, n_fact, 0, n_part)).astype(np.int32)),
+            make_column(0, 3, T.INT32, g(T.INT32, DIST_UNIFORM_INT, 3, n_fact, 0, n_supp)),
+            make_column(0, 4, T.DOUBLE, g(T.DOUBLE, DIST_UNIFORM_01, 4, n_fact))]
+    return fact, date, part, supp
+
+
 def c5_table(row0: int, n: int, seed: int = 5) -> List[Column]:
     return [make_column(0, 1, T.INT64, gen_values(T.INT64, DIST_INT64_FULL, seed, 1, row0, n)),
             make_column(0, 2, T.INT32, gen_values(T.INT32, DIST_UNIFORM_INT, seed, 2, row0, n, 0, 1 << 30))]

@@ -41,6 +41,28 @@ def c3_join_groupby() -> P.Plan:
                          2: P.agg_tuple_slots(aggs, [T.INT64, T.DOUBLE])})
 
 
+STAR_TUPLES = {0: [(1, T.INT32), (2, T.INT32), (3, T.INT32), (4, T.DOUBLE)],   # lineorder: lo_orderdate, lo_partkey, lo_suppkey, lo_revenue
+               1: [(1, T.INT32), (2, T.INT32)],                                # date: d_datekey, d_year
+               2: [(1, T.INT32), (2, T.INT32), (3, T.INT32)],                  # part: p_partkey, p_brand, p_category
+               3: [(1, T.INT32), (2, T.INT32)]}                                # supplier: s_suppkey, s_region
+
+
+def c6_star_groupby(category: int = 12, region: int = 1) -> P.Plan:
+    """SELECT d_year, p_brand, SUM(lo_revenue), COUNT(*) FROM lineorder JOIN date ON lo_orderdate = d_datekey
+    JOIN part ON lo_partkey = p_partkey JOIN supplier ON lo_suppkey = s_suppkey WHERE p_category = 12 AND s_region = 1
+    GROUP BY d_year, p_brand   (config C6, SSB Q2.1-like).  A chain of INNER joins whose outer (build) children are the
+    dimensions (the reference's hash join builds on the outer child, src/exec/join_node.cpp:920-1022), with the dimension
+    filters pushed down to their scans."""
+    aggs = [P.agg_expr("sum", 4, 1, None, P.slot_ref(0, 4, T.DOUBLE)), P.agg_expr("count_star", 4, 2)]
+    part = P.where(P.scan(2), P.eq(P.slot_ref(2, 3, T.INT32), P.int_lit(category)))
+    supp = P.where(P.scan(3), P.eq(P.slot_ref(3, 2, T.INT32), P.int_lit(region)))
+    j = P.join(P.scan(1), P.scan(0), [P.eq(P.slot_ref(1, 1, T.INT32), P.slot_ref(0, 1, T.INT32))])
+    j = P.join(part, j, [P.eq(P.slot_ref(2, 1, T.INT32), P.slot_ref(0, 2, T.INT32))])
+    j = P.join(supp, j, [P.eq(P.slot_ref(3, 1, T.INT32), P.slot_ref(0, 3, T.INT32))])
+    root = P.agg(j, 4, [P.slot_ref(1, 2, T.INT32), P.slot_ref(2, 2, T.INT32)], aggs)
+    return P.Plan(root, {**STAR_TUPLES, 4: P.agg_tuple_slots(aggs, [T.DOUBLE, T.INT64])})
+
+
 def c5_topk(k: int = 1000, asc: bool = True) -> P.Plan:
     """SELECT `0_1`, `0_2` FROM t ORDER BY `0_1` ASC LIMIT k          (config C5)"""
     root = P.sort(P.scan(0), [P.slot_ref(0, 1, T.INT64)], [asc], limit=k, tuple_id=0)

@@ -2,7 +2,8 @@
 """bench_configs.py — the OTHER BASELINE.json configs on one H100 (C1 count-where, C3 join+aggregate, C5 top-k):
 device-resident synthetic columns (SURVEY.md §8d), CUDA events around reset+push+finish+get_next, one JSON line per
 config with rows/s and achieved GB/s on the config's algorithmic bytes.  The headline line is bench.py's;
-this script measures the side configs on their own.   usage: python bench_configs.py [c1] [c3] [c5] [--scale 0.1] [--steps 10]"""
+this script measures the side configs on their own (C6, the star join, also its kernels, a parity flag and the Acero time).
+usage: python bench_configs.py [c1] [c3] [c5] [c6] [--scale 0.1] [--steps 10]"""
 import argparse
 import ctypes
 import json
@@ -12,11 +13,13 @@ import sys
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
+import numpy as np
 import torch
 
 from baikaldb_b200 import _lib, datagen, queries
 from baikaldb_b200._lib import BkgpuColumn, BkgpuStats
-from baikaldb_b200.plan import PrimitiveType as T
+from baikaldb_b200.column import make_column
+from baikaldb_b200.plan import PrimitiveType as T, storage_dtype
 
 L = _lib.lib()
 PEAK = 3350.0   # H100 SXM data sheet, GB/s; MEASURED_PEAKS.json (a measured copy peak) replaces it when present
@@ -43,7 +46,8 @@ def cols_array(specs, tensors):
     return arr
 
 
-def run(name, plan, pushes, rows, algo_bytes, steps, warmup, options=()):
+def run(name, plan, pushes, rows, algo_bytes, steps, warmup, options=(), collect=False, emit=True):
+    """emit = False: return the JSON line instead of printing it; collect: also return the last step's result columns by name"""
     pb = plan.serialize()
     h = ctypes.c_void_p()
     _lib.check(L.bkgpu_init(ctypes.byref(h), pb, len(pb), 0, None))
@@ -56,6 +60,7 @@ def run(name, plan, pushes, rows, algo_bytes, steps, warmup, options=()):
         _lib.check(L.bkgpu_set_option(h, k.encode(), int(v)), h)
     _lib.check(L.bkgpu_open(h), h)
     out = (BkgpuColumn * 16)()
+    got = {}
 
     def step():
         _lib.check(L.bkgpu_reset(h), h)
@@ -67,8 +72,16 @@ def run(name, plan, pushes, rows, algo_bytes, steps, warmup, options=()):
             ncols, nrows = ctypes.c_int(16), ctypes.c_int64(0)
             _lib.check(L.bkgpu_get_next(h, out, ctypes.byref(ncols), ctypes.byref(nrows), ctypes.byref(eos)), h)
             total += nrows.value
+            if collect:
+                for i in range(ncols.value):
+                    dt = np.dtype(storage_dtype(out[i].prim_type))
+                    vals = np.frombuffer((ctypes.c_uint8 * max(1, nrows.value * dt.itemsize)).from_address(out[i].values), dtype=dt, count=nrows.value)
+                    got.setdefault(f"{out[i].tuple_id}_{out[i].slot_id}", []).extend(vals.tolist())
         return total
     for _ in range(warmup):
+        n_out = step()
+    if collect:
+        got.clear()
         n_out = step()
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -85,8 +98,91 @@ def run(name, plan, pushes, rows, algo_bytes, steps, warmup, options=()):
             "gbs_whole_step": algo_bytes / (ms / 1e3) / 1e9, "frac_of_measured_hbm_whole_step": algo_bytes / (ms / 1e3) / 1e9 / PEAK,
             "main_kernel": st.main_kernel_name.decode(), "main_kernel_ms_per_step": kms / steps, "result_rows": n_out,
             "gpu_launches_per_step": None}
-    print(json.dumps(line), flush=True)
     L.bkgpu_close(h)
+    if not emit:
+        return (line, got) if collect else line
+    print(json.dumps(line), flush=True)
+
+
+def c6(a):
+    """C6, a star join: lineorder (100M rows) JOIN date (2,556) JOIN part (1M, sparse keys) JOIN supplier (100k), two dimensions filtered,
+    GROUP BY d_year, p_brand.  Device-resident, dimensions pushed first.  Besides the step: the time of k_star_probe and of the aggregate
+    kernel (torch.profiler, a run of its own), a parity flag against a torch computation over all rows, and the same query as an Acero plan
+    (hashjoin chain + aggregate) over the same tables on all host threads."""
+    import time
+    import pyarrow.acero as ac
+    import pyarrow.compute as pc
+    from oracle.acero_oracle import to_table
+    nf = int(100_000_000 * a.scale)
+    nd = {"date": 2_556, "part": max(1000, int(1_000_000 * a.scale)), "supplier": max(1000, int(100_000 * a.scale))}
+    seed = 6
+    # the columns of datagen.c6_tables, generated on the device
+    date_k = gen(nd["date"], (1, 1, T.INT32, 4, 11, 0, nd["date"], 1.0), seed)
+    part_k = gen(nd["part"], (2, 1, T.INT32, 4, 21, 0, nd["part"], 1.0), seed) * datagen.PART_KEY_STRIDE + datagen.PART_KEY_BASE
+    dims = {"date": ([(1, 1, T.INT32), (1, 2, T.INT32)], [date_k, (1992 + date_k // 365).to(torch.int32)]),
+            "part": ([(2, 1, T.INT32), (2, 2, T.INT32), (2, 3, T.INT32)],
+                     [part_k.to(torch.int32), gen(nd["part"], (2, 2, T.INT32, 0, 22, 0, 1000, 1.0), seed), gen(nd["part"], (2, 3, T.INT32, 0, 23, 0, 25, 1.0), seed)]),
+            "supplier": ([(3, 1, T.INT32), (3, 2, T.INT32)],
+                         [gen(nd["supplier"], (3, 1, T.INT32, 4, 31, 0, nd["supplier"], 1.0), seed), gen(nd["supplier"], (3, 2, T.INT32, 0, 32, 0, 5, 1.0), seed)])}
+    fs = [(0, 1, T.INT32, 0, 1, 0, nd["date"], 1.0), (0, 2, T.INT64, 0, 2, 0, nd["part"], 1.0), (0, 3, T.INT32, 0, 3, 0, nd["supplier"], 1.0), (0, 4, T.DOUBLE, 1, 4, 0, 0, 1.0)]
+    ft = [gen(nf, s, seed) for s in fs]
+    ft[1] = (ft[1] * datagen.PART_KEY_STRIDE + datagen.PART_KEY_BASE).to(torch.int32)
+    fspec = [(0, 1, T.INT32), (0, 2, T.INT32), (0, 3, T.INT32), (0, 4, T.DOUBLE)]
+    pushes = [(cols_array(s, t), len(s), t[0].numel()) for s, t in dims.values()] + [(cols_array(fspec, ft), 4, nf)]
+    plan = queries.c6_star_groupby()
+    algo = (3 * 4 + 8) * nf + 8 * nd["date"] + 12 * nd["part"] + 8 * nd["supplier"]   # fact keys + revenue, every dimension column read once
+    line, got = run("C6 star join: lineorder JOIN date, part, supplier; 2 dimension filters; GROUP BY d_year, p_brand", plan, pushes, nf, algo,
+                    a.steps, a.warmup, collect=True, emit=False)
+    # parity: the same aggregate in torch over all rows (dense lookups by key; part keys are stride-7)
+    dk, dy = dims["date"][1]
+    year = torch.empty(nd["date"], dtype=torch.int64, device="cuda"); year[dk.long()] = dy.long()
+    pk, pb, pcat = dims["part"][1]
+    pidx = (pk.long() - datagen.PART_KEY_BASE) // datagen.PART_KEY_STRIDE
+    brand = torch.empty(nd["part"], dtype=torch.int64, device="cuda"); brand[pidx] = pb.long()
+    cat = torch.empty(nd["part"], dtype=torch.int64, device="cuda"); cat[pidx] = pcat.long()
+    sk, sr = dims["supplier"][1]
+    region = torch.empty(nd["supplier"], dtype=torch.int64, device="cuda"); region[sk.long()] = sr.long()
+    fidx = (ft[1].long() - datagen.PART_KEY_BASE) // datagen.PART_KEY_STRIDE
+    keep = (cat[fidx] == 12) & (region[ft[2].long()] == 1)
+    g = (year[ft[0].long()] * 1000 + brand[fidx])[keep]
+    rev = ft[3][keep]
+    uk, inv = torch.unique(g, return_inverse=True)
+    want_sum = torch.zeros(len(uk), dtype=torch.float64, device="cuda").index_add_(0, inv, rev)
+    want_cnt = torch.bincount(inv, minlength=len(uk))
+    want = {int(k): (float(s), int(c)) for k, s, c in zip(uk.tolist(), want_sum.tolist(), want_cnt.tolist())}
+    have = {int(y) * 1000 + int(b): (s, c) for y, b, s, c in zip(got["1_2"], got["2_2"], got["4_1"], got["4_2"])}
+    line["parity"] = set(have) == set(want) and all(have[k][1] == want[k][1] and abs(have[k][0] - want[k][0]) <= 1e-9 * max(1.0, abs(want[k][0])) for k in want)
+    line["result_rows"] = len(have)
+    # kernel times: a profiled run of its own
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        run("profile", plan, pushes, nf, algo, a.steps, 1, emit=False)
+        torch.cuda.synchronize()
+    kt = {}
+    for e in prof.key_averages():
+        name = e.key.split("(")[0].replace("bk::", "")
+        if name.startswith(("k_star_", "k_agg", "k_join_", "k_pack_validity")):
+            kt[name] = getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) / 1e3 / a.steps
+    line["kernel_ms_per_step"] = kt
+    # Acero: the same query over the same tables on the host (copied outside the timed region)
+    host = lambda spec, ts: to_table([make_column(s[0], s[1], s[2], t.cpu().numpy()) for s, t in zip(spec, ts)])
+    tabs = {k: host(s, t) for k, (s, t) in dims.items()}
+    fact = host(fspec, ft)
+    src = lambda t: ac.Declaration("table_source", ac.TableSourceNodeOptions(t))
+    j = ac.Declaration("hashjoin", ac.HashJoinNodeOptions("inner", ["0_1"], ["1_1"]), inputs=[src(fact), src(tabs["date"])])
+    j = ac.Declaration("hashjoin", ac.HashJoinNodeOptions("inner", ["0_2"], ["2_1"]),
+                       inputs=[j, ac.Declaration("filter", ac.FilterNodeOptions(pc.field("2_3") == 12), inputs=[src(tabs["part"])])])
+    j = ac.Declaration("hashjoin", ac.HashJoinNodeOptions("inner", ["0_3"], ["3_1"]),
+                       inputs=[j, ac.Declaration("filter", ac.FilterNodeOptions(pc.field("3_2") == 1), inputs=[src(tabs["supplier"])])])
+    agg = ac.Declaration("aggregate", ac.AggregateNodeOptions([("0_4", "hash_sum", None, "4_1"), ([], "hash_count_all", None, "4_2")], keys=["1_2", "2_2"]), inputs=[j])
+    times = []
+    for _ in range(3):
+        t0 = time.perf_counter(); out = agg.to_table(use_threads=True); times.append((time.perf_counter() - t0) * 1e3)
+    line["acero_ms"] = min(times)
+    line["acero_rows"] = out.num_rows
+    line["host_cpus"] = os.cpu_count()
+    print(json.dumps(line), flush=True)
+    del ft, dims
 
 
 def main():
@@ -140,6 +236,8 @@ def main():
             "the step also gathers the payload and copies 1.5 GB of sorted rows to the host", plan, [(cols_array(specs, ts), 2, n)], n,
             (8 + 8 * 24) * n, max(1, a.steps // 5), 1)
         del ts
+    if "c6" in a.configs:
+        c6(a)
     if "c3" in a.configs:
         nf, nd = int(100_000_000 * a.scale), int(10_000_000 * a.scale)
         fs = [(0, 1, T.INT32, 0, 1, 0, nd, 1.0), (0, 2, T.DOUBLE, 1, 2, 0, 0, 1.0)]

@@ -136,12 +136,14 @@ __global__ void __launch_bounds__(256) k_join_pairs(const __grid_constant__ AggA
         }
     }
 }
-// one output column of the joined rows: element `which` of each pair addresses `src`; JOIN_NO_ROW (the NULL-extended side) gives NULL
-__global__ void k_join_rows_gather(DevCol src, const uint32_t* pairs, int which, uint32_t n, int eb, uint8_t* dst, uint8_t* dst_null) {
+// one output column of the joined rows: element `which` of each row-id tuple (`width` row ids: (probe, build) pairs of a two-table join,
+// [fact, dim x D] of a star join) addresses `src`; JOIN_NO_ROW (the NULL-extended side) gives NULL.  dst_null may be nullptr when no
+// element can be NULL
+__global__ void k_join_rows_gather(DevCol src, const uint32_t* tuples, int width, int which, uint32_t n, int eb, uint8_t* dst, uint8_t* dst_null) {
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const uint32_t r = pairs[2 * (size_t)i + which];
+        const uint32_t r = tuples[(size_t)width * i + which];
         const bool isnull = r == JOIN_NO_ROW || elem_is_null(src, r);
-        dst_null[i] = isnull ? 1 : 0;
+        if (dst_null) dst_null[i] = isnull ? 1 : 0;
         const uint8_t* s = (const uint8_t*)src.values + (size_t)r * eb;
         uint8_t* d = dst + (size_t)i * eb;
         if (isnull) { for (int b = 0; b < eb; b++) d[b] = 0; continue; }
@@ -546,6 +548,136 @@ __global__ void k_join_compose(JoinFast jf, const uint32_t* attr_by_row, uint32_
         }
     }
 }
+
+// ---- K4 star join (PK_STAR_AGG): one fact table INNER-joined to up to four dimensions ----
+// Build time: the conjuncts over one dimension alone, once per dimension row.  A row's build key is valid when the key is not NULL and the
+// conjunction is TRUE: this bitmap (beside the column's own) is the key's validity for k_join_build_fast / k_join_build, which skip NULL keys.
+__global__ void __launch_bounds__(256) k_star_dim_filter(const __grid_constant__ StarFilter a, uint32_t* keybits) {
+    const int lane = threadIdx.x & 31;
+    const int64_t T = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t w0 = (int64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31); w0 < a.nrows; w0 += T) {   // (warp-uniform: one bitmap word per warp and pass)
+        const int64_t r = w0 + lane;
+        bool ok = r < a.nrows && !elem_is_null(a.cols[a.key_col], r);
+        if (ok && a.prog.n_instr > 0) {
+            uint64_t out[1]; uint32_t out_null;
+            run_program(a.prog, a.cols, r, out, out_null);
+            ok = !(out_null & 1u) && out[0] != 0;
+        }
+        const uint32_t m = __ballot_sync(0xFFFFFFFFu, ok);
+        if (lane == 0) keybits[w0 >> 5] = m;
+    }
+}
+// four consecutive foreign keys [r0, r0 + 4) as canonical images: one 128-bit load (4-byte keys) or two (8-byte keys) when the chunk is 32-byte
+// aligned and the four rows exist
+__device__ __forceinline__ void load_quad(const DevCol& c, int64_t r0, int64_t nrows, bool vec, uint64_t (&v)[4]) {
+    if (vec && r0 + 4 <= nrows && (c.stype == ST_I32 || c.stype == ST_U32)) {
+        const uint4 q = __ldg((const uint4*)((const uint32_t*)c.values + r0));
+        const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+        for (int u = 0; u < 4; u++) v[u] = narrow_prim(c.stype == ST_I32 ? (uint64_t)(int64_t)(int32_t)w[u] : (uint64_t)w[u], c.prim);
+        return;
+    }
+    if (vec && r0 + 4 <= nrows && (c.stype == ST_I64 || c.stype == ST_U64)) {
+        const ulonglong2 a = __ldg((const ulonglong2*)((const unsigned long long*)c.values + r0));
+        const ulonglong2 b = __ldg((const ulonglong2*)((const unsigned long long*)c.values + r0 + 2));
+        v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
+        return;
+    }
+#pragma unroll
+    for (int u = 0; u < 4; u++) v[u] = r0 + u < nrows ? load_elem(c, r0 + u) : 0;
+}
+// Probe: one pass over a chunk's fact rows.  A row survives when every dimension with unique keys has a partner (a NULL foreign key has none:
+// one L2-resident index read per dimension).  Survivors leave as row-id tuples [fact row, dim row x D] in any order, compacted with warp
+// ballots and one cursor atomic per warp; the slots of dimensions with duplicate keys are filled by k_star_expand.
+__global__ void __launch_bounds__(256) k_star_probe(const __grid_constant__ StarProbe a, uint32_t* out, uint32_t* cursor) {
+    const int lane = threadIdx.x & 31;
+    const int64_t T = (int64_t)gridDim.x * blockDim.x;
+    const int64_t nq = (a.nrows + 3) / 4;
+    for (int64_t q0 = (int64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31); q0 < nq; q0 += T) {   // (warp-uniform trip count: the ballots below)
+        const int64_t r0 = (q0 + lane) * 4;
+        uint32_t br[4][4];
+        // every lookup is issued before any result is tested: up to 16 independent index reads in flight per thread
+#pragma unroll
+        for (int d = 0; d < 4; d++) {
+            if (d >= a.n) break;
+            const StarLookup& L = a.d[d];
+            uint64_t v[4];
+            load_quad(L.fk, r0, a.nrows, a.vec != 0, v);
+#pragma unroll
+            for (int u = 0; u < 4; u++)
+                br[u][d] = r0 + u < a.nrows && !elem_is_null(L.fk, r0 + u) ? join_lookup(L.jf, cast_prim(v[u], L.from_prim, L.cast_prim)) : JOIN_NO_ROW;
+        }
+        uint32_t live = 0;
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+            bool ok = r0 + u < a.nrows;
+#pragma unroll
+            for (int d = 0; d < 4; d++) if (d < a.n) ok = ok && br[u][d] != JOIN_NO_ROW;
+            if (ok) live |= 1u << u;
+        }
+        uint32_t b[4]; uint32_t total = 0;
+#pragma unroll
+        for (int u = 0; u < 4; u++) { b[u] = __ballot_sync(0xFFFFFFFFu, (live >> u) & 1u); total += (uint32_t)__popc(b[u]); }
+        if (total == 0) continue;
+        uint32_t base = 0;
+        if (lane == 0) base = atomicAdd(cursor, total);
+        base = __shfl_sync(0xFFFFFFFFu, base, 0);
+        const uint32_t lt = (1u << lane) - 1u;
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+            if ((live >> u) & 1u) {
+                uint32_t* t = out + (size_t)a.width * (base + (uint32_t)__popc(b[u] & lt));
+                t[0] = (uint32_t)(r0 + u);
+#pragma unroll
+                for (int d = 0; d < 4; d++) if (d < a.n) t[a.d[d].slot] = br[u][d];
+            }
+            base += (uint32_t)__popc(b[u]);
+        }
+    }
+}
+// A dimension with duplicate keys: every tuple becomes one tuple per matching row of the dimension's multimap (k_join_build), or none.
+// Past `cap` only the count goes on: the host grows the buffer to the count and runs the pass again.
+__global__ void __launch_bounds__(256) k_star_expand(DevCol fk, int from_prim, int cast_to, const uint64_t* keys, const uint32_t* rows, uint32_t cap_mask,
+                                                     const uint32_t* in, uint32_t n_in, int width, int slot, uint32_t* out, uint32_t cap, uint32_t* cursor) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_in; i += gridDim.x * blockDim.x) {
+        const uint32_t* t = in + (size_t)width * i;
+        const uint32_t f = t[0];
+        if (elem_is_null(fk, f)) continue;
+        const uint64_t img = cast_prim(load_elem(fk, f), from_prim, cast_to);
+        for (uint32_t h = hash_key1(img) & cap_mask;; h = (h + 1) & cap_mask) {
+            const uint32_t br = rows[h];
+            if (br == 0xFFFFFFFFu) break;
+            if (keys[h] != img) continue;
+            const uint32_t pos = atomicAdd(cursor, 1u);
+            if (pos >= cap) continue;
+            uint32_t* o = out + (size_t)width * pos;
+            for (int k = 0; k < width; k++) o[k] = t[k];
+            o[slot] = br;
+        }
+    }
+}
+cudaError_t launch_star_dim_filter(const StarFilter& f, uint32_t* keybits, cudaStream_t s) {
+    if (f.nrows == 0) return cudaSuccess;
+    int grid = (int)((f.nrows + 255) / 256); if (grid > 132 * 16) grid = 132 * 16;
+    k_star_dim_filter<<<grid, 256, 0, s>>>(f, keybits);
+    return cudaGetLastError();
+}
+cudaError_t launch_star_probe(const StarProbe& sp, uint32_t* out, uint32_t* cursor, int sm_count, cudaStream_t s) {
+    cudaError_t e = cudaMemsetAsync(cursor, 0, 4, s);
+    if (e != cudaSuccess || sp.nrows == 0) return e;
+    int64_t g = (sp.nrows + 1023) / 1024; if (g > (int64_t)sm_count * 8) g = (int64_t)sm_count * 8;
+    k_star_probe<<<(int)(g < 1 ? 1 : g), 256, 0, s>>>(sp, out, cursor);
+    return cudaGetLastError();
+}
+cudaError_t launch_star_expand(const DevCol& fk, int from_prim, int cast_prim_, const uint64_t* keys, const uint32_t* rows, uint32_t cap_mask, const uint32_t* in, uint32_t n_in,
+                               int width, int slot, uint32_t* out, uint32_t cap, uint32_t* cursor, cudaStream_t s) {
+    cudaError_t e = cudaMemsetAsync(cursor, 0, 4, s);
+    if (e != cudaSuccess || n_in == 0) return e;
+    int grid = (int)((n_in + 255) / 256); if (grid > 132 * 16) grid = 132 * 16;
+    k_star_expand<<<grid, 256, 0, s>>>(fk, from_prim, cast_prim_, keys, rows, cap_mask, in, n_in, width, slot, out, cap, cursor);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_join_compose(const JoinFast& jf, const uint32_t* attr_by_row, uint32_t* attr_of_key, uint64_t* packed_attr, uint32_t* bad_flag, cudaStream_t s) {
     cudaError_t e = cudaMemsetAsync(bad_flag, 0, 4, s);
     if (e != cudaSuccess) return e;
@@ -610,10 +742,10 @@ cudaError_t launch_join_pairs(const AggArgs& a, uint32_t* pairs, uint32_t cap, u
     k_join_pairs<<<grid, 256, 0, s>>>(a, pairs, cap, cursor);
     return cudaGetLastError();
 }
-cudaError_t launch_join_rows_gather(const DevCol& src, const uint32_t* pairs, int which, uint32_t n, int eb, uint8_t* dst, uint8_t* dst_null, cudaStream_t s) {
+cudaError_t launch_join_rows_gather(const DevCol& src, const uint32_t* tuples, int width, int which, uint32_t n, int eb, uint8_t* dst, uint8_t* dst_null, cudaStream_t s) {
     if (n == 0) return cudaSuccess;
     int grid = (int)((n + 255) / 256); if (grid > 132 * 16) grid = 132 * 16;
-    k_join_rows_gather<<<grid, 256, 0, s>>>(src, pairs, which, n, eb, dst, dst_null);
+    k_join_rows_gather<<<grid, 256, 0, s>>>(src, tuples, width, which, n, eb, dst, dst_null);
     return cudaGetLastError();
 }
 cudaError_t launch_join_build(const DevCol& key, int from_prim, int cast_prim_, int64_t nrows, uint64_t* keys, uint32_t* rows, uint32_t cap_mask, cudaStream_t s) {

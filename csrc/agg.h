@@ -110,7 +110,17 @@ cudaError_t launch_unpack_validity(const uint8_t* bitmap, int64_t n, uint8_t* nu
 cudaError_t launch_pack_validity(const uint8_t* null_bytes, int64_t n, uint8_t* bitmap, cudaStream_t s);
 // a JOIN that returns rows: (probe row, build row) pairs of the joined rows that pass the conditions, then one gather per output column
 cudaError_t launch_join_pairs(const AggArgs& a, uint32_t* pairs, uint32_t cap, uint32_t* cursor, int sm_count, cudaStream_t s);
-cudaError_t launch_join_rows_gather(const DevCol& src, const uint32_t* pairs, int which, uint32_t n, int elem_bytes, uint8_t* dst, uint8_t* dst_null, cudaStream_t s);
+// element `which` of each `width`-word row-id tuple addresses `src` (pairs: width 2); dst_null may be nullptr when no element can be NULL
+cudaError_t launch_join_rows_gather(const DevCol& src, const uint32_t* tuples, int width, int which, uint32_t n, int elem_bytes, uint8_t* dst, uint8_t* dst_null, cudaStream_t s);
+// star join (PK_STAR_AGG): per dimension with unique keys, the fact foreign key, its slot in the row-id tuple and the dimension's key index
+struct StarLookup { DevCol fk; int32_t from_prim, cast_prim, slot; JoinFast jf; };
+struct StarProbe { StarLookup d[4]; int32_t n; int32_t width; int64_t nrows; int32_t vec; };
+// the build-time filter of one dimension: program over the plan's columns (this dimension's retained rows), validity of its join key
+struct StarFilter { DevCol cols[MAX_COLS]; Program prog; int32_t key_col; int64_t nrows; };
+cudaError_t launch_star_dim_filter(const StarFilter& f, uint32_t* keybits, cudaStream_t s);
+cudaError_t launch_star_probe(const StarProbe& sp, uint32_t* out, uint32_t* cursor, int sm_count, cudaStream_t s);
+cudaError_t launch_star_expand(const DevCol& fk, int from_prim, int cast_prim, const uint64_t* keys, const uint32_t* rows, uint32_t cap_mask, const uint32_t* in, uint32_t n_in,
+                               int width, int slot, uint32_t* out, uint32_t cap, uint32_t* cursor, cudaStream_t s);
 cudaError_t launch_table_init(const GroupTable& gt, const AggPlan& ap, cudaStream_t s, int keep_overflow = 0);
 cudaError_t launch_table_clear(const GroupTable& gt, const AggPlan& ap, uint32_t n_occupied, cudaStream_t s);
 cudaError_t launch_partial_export_rows(const GroupTable& gt, const AggPlan& ap, uint64_t* dst, uint32_t bound, cudaStream_t s);

@@ -42,6 +42,17 @@ struct HostCol {  // one materialised result column (host memory owned by the pl
 
 struct EventPair { cudaEvent_t a, b; int64_t bytes; };
 
+// one retained build side of a hash join (K4) and its key indexes
+struct JoinSide {
+    std::vector<uint8_t*> vals, nullbytes, bitmap;   // per plan column (this side's columns only)
+    std::vector<bool> has_null;
+    int64_t rows = 0, cap = 0;
+    uint8_t* keybits = nullptr; size_t keybits_cap = 0;   // star join: validity of the build key AND the dimension's build-time filter
+    uint64_t* jt_keys = nullptr; uint32_t* jt_rows = nullptr; uint32_t jt_mask = 0; bool jt_generic = false;   // multimap (duplicate keys)
+    JoinFast jf{}; uint32_t* jf_dense = nullptr; uint64_t* jf_packed = nullptr; size_t jf_dense_cap = 0, jf_packed_cap = 0;   // unique-key index
+    bool learned = false; uint64_t learn_min = 0, learn_max = 0;   // key range of the side's previous build (skips the min/max pass + round trip)
+};
+
 // BKGPU_TRACE=1: wall-clock time the HOST spends in each phase of a request (summed per plan, printed by bkgpu_close)
 struct HostClock {
     double reset = 0, push = 0, collective = 0, extract_wait = 0, finish = 0; int64_t n = 0;
@@ -103,21 +114,20 @@ struct bkgpu_plan {
     // mapped host buffer the lean kernel's last CTA extracts the result into (AggArgs::fused_out), and whether the request's last
     // aggregate launch did so: then bkgpu_finish only waits and reads it
     uint8_t* h_fused = nullptr; uint8_t* d_fused = nullptr; size_t fused_bytes = 0; uint32_t fused_cap = 0; bool fused_last = false;
-    // hash join (K4): retained build side + multimap
-    std::vector<uint8_t*> jb_vals, jb_nullbytes, jb_bitmap;   // per plan column (side 1 only)
-    std::vector<bool> jb_has_null;
-    int64_t jb_rows = 0, jb_cap = 0;
-    uint64_t* jt_keys = nullptr; uint32_t* jt_rows = nullptr; uint32_t jt_mask = 0; bool jt_built = false, jt_generic = false;
-    JoinFast jf{}; uint32_t* jf_dense = nullptr; uint64_t* jf_packed = nullptr;   // FK -> PK fast path (unique build keys)
-    int join_pipeline = 0;        // opt-in: the fused probe issues its lookups one drain ahead (no gain while the kernel is bound by its shared-memory atomics)
+    // hash join (K4): the retained build side(s) and their indexes; the two-table join uses js[0], a star join one per dimension
+    JoinSide js[4];
+    bool jt_built = false;        // the build side is complete and indexed: probe batches have started
+    int star_expand_cap = 0;      // test option "star_expand_capacity": first capacity (tuples) of a star join's expansion pass (0 = twice its input)
+    uint32_t* st_tuples[2] = {nullptr, nullptr}; size_t st_tuples_cap[2] = {0, 0};   // star join: row-id tuples of one chunk (probe / expansion ping-pong)
+    std::vector<uint8_t*> st_vals, st_nullb, st_bits; std::vector<size_t> st_vals_cap, st_nullb_cap, st_bits_cap;   // ... and its gathered columns
+    int join_pipeline = 0;       // opt-in: the fused probe issues its lookups one drain ahead (no gain while the kernel is bound by its shared-memory atomics)
     int join_learn_range = 1;     // a re-run plan builds with the key range it saw before (checked by the build kernel): -0.05 ms per C3 request
     int fx_off = 0;               // set when a finished request saw more than 1/64 of its surviving rows take FX's exact path (see agg_finish)
     int lean_bank = 0;            // opt-in: bank-aware dealing of the lean kernel's drain (agg_direct.cuh, BANK)
     int lean_fx = [] { const char* e = getenv("BKGPU_LEAN_FX"); return e ? atoi(e) != 0 : BK_LEAN_FX_DEFAULT; }();   // double sums as fixed-point limbs with native shared atomics (agg_direct.cuh, FX); option lean_fx
     int blocking_sync = -1; bool blocking_wait = false; cudaEvent_t wait_event = nullptr;   // see agg_finish
-    bool jf_learned = false; uint64_t jf_learn_min = 0, jf_learn_max = 0;   // key range of the plan's previous build (skips the min/max pass + round trip)
     JoinProbe jp{}; uint32_t* jp_attr = nullptr; uint64_t* jp_packed = nullptr; int jp_key_pos = 0;   // ... fused into the lean aggregate
-    size_t jf_dense_cap = 0, jf_packed_cap = 0, jp_attr_cap = 0, jp_packed_cap = 0, j_scratch_cap = 0;
+    size_t jp_attr_cap = 0, jp_packed_cap = 0, j_scratch_cap = 0;
     uint64_t* j_scratch = nullptr;   // [0..1] key min / max, then u32 flags: [4] duplicate build key, [5] fused probe unusable
     int no_fused_probe = 0, no_lean_nulls = 0, no_lean_mm = 0;
     int use_wp = 0;               // 1 = launch the warp-private aggregate kernel where the batch fits it (opt-in: k_agg_group_lean is the default)
@@ -336,6 +346,7 @@ extern "C" int bkgpu_set_option(bkgpu_plan* p, const char* key, int64_t v) {
     else if (k == "lean_fx") p->lean_fx = v != 0;
     else if (k == "blocking_sync") p->blocking_sync = (int)v;
     else if (k == "join_learn_range") p->join_learn_range = v != 0;
+    else if (k == "star_expand_capacity") { if (v < 0 || v > 0x7FFFFFFF) return p->fail(BKGPU_EINVAL, "star_expand_capacity out of range"); p->star_expand_cap = (int)v; }
     else if (k == "no_lean") p->no_lean = v != 0;
     else if (k == "no_fused_probe") p->no_fused_probe = v != 0;
     else if (k == "repartition") p->repartition = v != 0;
@@ -388,7 +399,7 @@ extern "C" int bkgpu_open(bkgpu_plan* p) {
     }
     p->blocking_wait = p->blocking_sync >= 0 ? p->blocking_sync != 0 : (p->nranks > 1 && cpu_budget() < 4 * p->nranks);
     int rc = BKGPU_OK;
-    if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG) rc = alloc_group_table(p);
+    if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) rc = alloc_group_table(p);
     if (!rc && (p->c.kind == PK_SORT || p->c.kind == PK_FILTER)) rc = sort_open(p->c, p->device, p->stream, p->region_base, &p->sort, p->last_error);
     if (!rc && p->c.post) rc = sort_open(*p->c.post, p->device, p->stream, 0, &p->post_sort, p->last_error);
     if (rc) { g_thread_error = p->last_error; return rc; }
@@ -452,9 +463,9 @@ static int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols
     AggArgs a; memset(&a, 0, sizeof a);
     a.plan = c.ap; a.prog = c.prog; a.direct = c.direct; a.gt = p->gt; a.rows_passed = p->d_rows_passed;
     if (c.kind == PK_JOIN_AGG) {
-        a.join.enabled = 1; a.join.keys = p->jt_keys; a.join.rows = p->jt_rows; a.join.cap_mask = p->jt_mask;
+        a.join.enabled = 1; a.join.keys = p->js[0].jt_keys; a.join.rows = p->js[0].jt_rows; a.join.cap_mask = p->js[0].jt_mask;
         a.join.probe_col = c.probe_key_col; a.join.probe_prim = c.cols[(size_t)c.probe_key_col].prim; a.join.cast_prim = c.join_key_prim;
-        a.join.join_type = c.join_type; a.join.matched = c.join_type == BK_INNER_JOIN ? nullptr : p->jb_matched; a.join.n_build = p->jb_rows;
+        a.join.join_type = c.join_type; a.join.matched = c.join_type == BK_INNER_JOIN ? nullptr : p->jb_matched; a.join.n_build = p->js[0].rows;
         a.join.tail = p->join_tail_launch ? 1 : 0;
     }
     const bool direct = c.has_direct && vec_ok && !p->force_generic && c.kind == PK_AGG;   // (the join's fast-path plan is lowered as PK_AGG)
@@ -851,39 +862,50 @@ static int sort_batch(bkgpu_plan* p, const DevCol* cols, int64_t nrows, int64_t,
 }
 
 // ---- K4: retain the build (outer / driver) table, build the multimap at the first probe batch ----
-static int join_retain_build(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device) {
+static void side_init(bkgpu_plan* p, JoinSide& s) {
+    const size_t nc = p->c.cols.size();
+    if (s.vals.empty()) { s.vals.assign(nc, nullptr); s.nullbytes.assign(nc, nullptr); s.bitmap.assign(nc, nullptr); s.has_null.assign(nc, false); }
+}
+// plan column i as retained by side s
+static DevCol side_col(const Compiled& c, const JoinSide& s, size_t i) {
+    DevCol d{};
+    d.values = s.vals[i]; d.validity = s.bitmap[i]; d.stype = prim_storage(c.cols[i].prim); d.prim = c.cols[i].prim;
+    return d;
+}
+// `side`: the Compiled::col_side value of this table's columns (1 for the two-table join, 1 + d for dimension d of a star join)
+static int join_retain_build(bkgpu_plan* p, JoinSide& s, int side, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device) {
     const Compiled& c = p->c;
     if (p->jt_built) return p->fail(BKGPU_ESTATE, "build-side rows arrived after probing started (the reference fetches the whole driver table first, join_node.cpp:920-1022)");
     const size_t nc = c.cols.size();
-    if (p->jb_vals.empty()) { p->jb_vals.assign(nc, nullptr); p->jb_nullbytes.assign(nc, nullptr); p->jb_bitmap.assign(nc, nullptr); p->jb_has_null.assign(nc, false); }
+    side_init(p, s);
     std::vector<ColRef> want; std::vector<int> idx;
-    for (size_t i = 0; i < nc; i++) if (c.col_side[i] == 1) { want.push_back(c.cols[i]); idx.push_back((int)i); }
+    for (size_t i = 0; i < nc; i++) if (c.col_side[i] == side) { want.push_back(c.cols[i]); idx.push_back((int)i); }
     std::vector<const bkgpu_column*> bound;
     int rc = bind_columns(p, want, cols, ncols, nrows, bound);
     if (rc) return rc;
-    if (p->jb_rows + nrows > 0xFFFFFFF0ll) return p->fail(BKGPU_EUNSUPPORTED, "build side larger than 2^32 rows");
-    if (p->jb_rows + nrows > p->jb_cap) {
-        const int64_t cap = std::max<int64_t>(p->jb_rows + nrows, std::max<int64_t>(p->jb_cap * 2, 1 << 16));
+    if (s.rows + nrows > 0xFFFFFFF0ll) return p->fail(BKGPU_EUNSUPPORTED, "build side larger than 2^32 rows");
+    if (s.rows + nrows > s.cap) {
+        const int64_t cap = std::max<int64_t>(s.rows + nrows, std::max<int64_t>(s.cap * 2, 1 << 16));
         for (int i : idx) {
             const size_t eb = (size_t)storage_bytes(prim_storage(c.cols[(size_t)i].prim));
             uint8_t *nv = nullptr, *nn = nullptr;
             if ((rc = dev_alloc(p, (void**)&nv, (size_t)cap * eb))) return rc;
             if ((rc = dev_alloc(p, (void**)&nn, (size_t)cap))) return rc;
-            if (p->jb_rows) {
-                CK(p, cudaMemcpyAsync(nv, p->jb_vals[(size_t)i], (size_t)p->jb_rows * eb, cudaMemcpyDeviceToDevice, p->stream));
-                CK(p, cudaMemcpyAsync(nn, p->jb_nullbytes[(size_t)i], (size_t)p->jb_rows, cudaMemcpyDeviceToDevice, p->stream));
+            if (s.rows) {
+                CK(p, cudaMemcpyAsync(nv, s.vals[(size_t)i], (size_t)s.rows * eb, cudaMemcpyDeviceToDevice, p->stream));
+                CK(p, cudaMemcpyAsync(nn, s.nullbytes[(size_t)i], (size_t)s.rows, cudaMemcpyDeviceToDevice, p->stream));
                 CK(p, cudaStreamSynchronize(p->stream));
             }
-            dev_free(p, p->jb_vals[(size_t)i]); dev_free(p, p->jb_nullbytes[(size_t)i]);
-            p->jb_vals[(size_t)i] = nv; p->jb_nullbytes[(size_t)i] = nn;
+            dev_free(p, s.vals[(size_t)i]); dev_free(p, s.nullbytes[(size_t)i]);
+            s.vals[(size_t)i] = nv; s.nullbytes[(size_t)i] = nn;
         }
-        p->jb_cap = cap;
+        s.cap = cap;
     }
     for (size_t w = 0; w < want.size(); w++) {
         const int i = idx[w];
         const size_t eb = (size_t)storage_bytes(prim_storage(c.cols[(size_t)i].prim));
-        uint8_t* dv = p->jb_vals[(size_t)i] + (size_t)p->jb_rows * eb;
-        uint8_t* dn = p->jb_nullbytes[(size_t)i] + p->jb_rows;
+        uint8_t* dv = s.vals[(size_t)i] + (size_t)s.rows * eb;
+        uint8_t* dn = s.nullbytes[(size_t)i] + s.rows;
         if (on_device) {
             CK(p, cudaMemcpyAsync(dv, bound[w]->values, (size_t)nrows * eb, cudaMemcpyDeviceToDevice, p->stream));
             CK(p, launch_unpack_validity(bound[w]->validity, nrows, dn, p->stream));
@@ -896,9 +918,9 @@ static int join_retain_build(bkgpu_plan* p, const bkgpu_column* cols, int ncols,
             CK(p, cudaStreamSynchronize(p->stream));
             p->stats.h2d_bytes += (int64_t)((size_t)nrows * (eb + 1));
         }
-        if (bound[w]->validity) p->jb_has_null[(size_t)i] = true;
+        if (bound[w]->validity) s.has_null[(size_t)i] = true;
     }
-    p->jb_rows += nrows;
+    s.rows += nrows;
     return BKGPU_OK;
 }
 
@@ -906,6 +928,7 @@ static int join_retain_build(bkgpu_plan* p, const bkgpu_column* cols, int ncols,
 // key and the probe key is a 32-bit integer column whose cast to the comparison type keeps the canonical image.
 static int join_compose_probe(bkgpu_plan* p, uint32_t* flag) {
     const Compiled& c = p->c;
+    const JoinSide& s = p->js[0];
     p->jp = JoinProbe{};
     if (!c.jfast || !c.jfast->has_direct || c.jfast->direct.n_keys != 1) return BKGPU_OK;
     const Compiled& f = *c.jfast;
@@ -925,114 +948,134 @@ static int join_compose_probe(bkgpu_plan* p, uint32_t* flag) {
     if (!ident) return BKGPU_OK;
     int rc;
     JoinProbe jp{};
-    jp.mode = p->jf.mode; jp.key_signed = pp == BK_INT32 ? 1 : 0;
-    jp.dense_min = p->jf.dense_min; jp.dense_size = p->jf.dense_size; jp.bias = p->jf.bias; jp.packed_mask = p->jf.packed_mask;
+    jp.mode = s.jf.mode; jp.key_signed = pp == BK_INT32 ? 1 : 0;
+    jp.dense_min = s.jf.dense_min; jp.dense_size = s.jf.dense_size; jp.bias = s.jf.bias; jp.packed_mask = s.jf.packed_mask;
     if (jp.mode == 1) {
         if ((rc = ensure_buf(p, (void**)&p->jp_attr, &p->jp_attr_cap, (size_t)jp.dense_size * 4))) return rc;
         jp.attr = p->jp_attr;
-        jp.present = (uint64_t)p->jb_rows == jp.dense_size ? nullptr : p->jf.dense;   // unique, NULL-free keys filling the range: every key exists
+        jp.present = (uint64_t)s.rows == jp.dense_size ? nullptr : s.jf.dense;   // unique, NULL-free keys filling the range: every key exists
     } else {
         if ((rc = ensure_buf(p, (void**)&p->jp_packed, &p->jp_packed_cap, ((size_t)jp.packed_mask + 1) * 8))) return rc;
         jp.packed = p->jp_packed;
     }
-    CK(p, launch_join_compose(p->jf, (const uint32_t*)p->jb_vals[(size_t)attr_main], p->jp_attr, p->jp_packed, flag, p->stream));
+    CK(p, launch_join_compose(s.jf, (const uint32_t*)s.vals[(size_t)attr_main], p->jp_attr, p->jp_packed, flag, p->stream));
     p->stats.kernel_launches++;
     p->jp = jp; p->jp_key_pos = (int)kpos;   // (the caller drops it again when `flag` comes back set)
     return BKGPU_OK;
 }
 
-static int join_build_table(bkgpu_plan* p) {
+// validity bitmaps of the side's retained columns that hold NULLs
+static int join_pack_validity(bkgpu_plan* p, JoinSide& s, int side) {
     const Compiled& c = p->c;
-    const size_t nc = c.cols.size();
-    if (p->jb_vals.empty()) { p->jb_vals.assign(nc, nullptr); p->jb_nullbytes.assign(nc, nullptr); p->jb_bitmap.assign(nc, nullptr); p->jb_has_null.assign(nc, false); }
+    side_init(p, s);
     int rc;
-    for (size_t i = 0; i < nc; i++) {
-        if (c.col_side[i] != 1) continue;
+    for (size_t i = 0; i < c.cols.size(); i++) {
+        if (c.col_side[i] != side) continue;
         // (a bitmap kept from an earlier run of the plan must not mask this run's rows: a column without NULLs has none)
-        dev_free(p, p->jb_bitmap[i]); p->jb_bitmap[i] = nullptr;
-        if (!p->jb_has_null[i]) continue;
-        if ((rc = dev_alloc(p, (void**)&p->jb_bitmap[i], (size_t)(p->jb_rows + 7) / 8 + 8))) return rc;
-        CK(p, launch_pack_validity(p->jb_nullbytes[i], p->jb_rows, p->jb_bitmap[i], p->stream));
+        dev_free(p, s.bitmap[i]); s.bitmap[i] = nullptr;
+        if (!s.has_null[i]) continue;
+        if ((rc = dev_alloc(p, (void**)&s.bitmap[i], (size_t)(s.rows + 7) / 8 + 8))) return rc;
+        CK(p, launch_pack_validity(s.nullbytes[i], s.rows, s.bitmap[i], p->stream));
         p->stats.kernel_launches++;
     }
-    DevCol key{};
-    const size_t ki = (size_t)c.build_key_col;
-    key.values = p->jb_vals[ki]; key.validity = p->jb_bitmap[ki]; key.stype = prim_storage(c.cols[ki].prim); key.prim = c.cols[ki].prim;
-    p->jt_built = true; p->jt_generic = false;   // the multimap of the general probe is built on first use (join_generic_table)
-    // ---- FK -> PK fast path: are the build keys unique, and is their range dense or their type <= 32 bits? ----
-    p->jf = JoinFast{}; p->jp = JoinProbe{};
-    if (p->jg_buf.empty()) p->jg_buf.assign(nc, nullptr);
-    bool build_nulls = false;
-    for (size_t i = 0; i < nc; i++) if (c.col_side[i] == 1 && p->jb_has_null[i]) build_nulls = true;   // gathered columns must be NULL-free
+    return BKGPU_OK;
+}
+
+// The unique-key index of side `s` (FK -> PK fast path): a dense array when the key range is small, else a packed table for keys of at most
+// 32 bits.  s.jf.mode stays 0 when neither fits or a key repeats.  `compose`: the two-table join's fused probe is composed behind the build,
+// so that its flag comes back in the same round trip.
+static int join_build_index(bkgpu_plan* p, JoinSide& s, const DevCol& key, int cast_prim, bool compose) {
+    int rc;
+    s.jf = JoinFast{};
+    if (s.rows <= 0) return BKGPU_OK;
     bool retry_measured = false;
 again:
-    if (c.jfast && !build_nulls && p->jb_rows > 0) {
-        const int cls = host_prim_class(c.join_key_prim);
-        const uint64_t bias = cls == VC_I64 ? 0x8000000000000000ull : 0ull;
-        if ((rc = ensure_buf(p, (void**)&p->j_scratch, &p->j_scratch_cap, 64))) return rc;
-        uint64_t* mm = p->j_scratch; uint32_t* dup = (uint32_t*)(p->j_scratch + 2);
-        // the key range: measured (one pass over the keys + a round trip), or — when this plan has built before — the range it saw then,
-        // checked by the build kernel itself (a key outside it raises a flag and the build is redone with a measured range)
-        uint64_t h_mm[2];
-        bool guessed = p->jf_learned && !retry_measured && p->join_learn_range;
-        if (guessed) { h_mm[0] = p->jf_learn_min; h_mm[1] = p->jf_learn_max; }
-        else {
-            CK(p, launch_join_minmax(key, c.cols[ki].prim, c.join_key_prim, p->jb_rows, bias, mm, p->stream));
-            CK(p, cudaMemcpyAsync(h_mm, mm, 16, cudaMemcpyDeviceToHost, p->stream));
-            CK(p, cudaStreamSynchronize(p->stream));
-            p->stats.kernel_launches++;
-        }
-        JoinFast jf{}; jf.bias = bias;
-        const uint64_t range = h_mm[1] >= h_mm[0] ? h_mm[1] - h_mm[0] + 1 : 0;
-        const int kb = storage_bytes(prim_storage(c.join_key_prim));
-        if (range > 0 && range <= (uint64_t)4 * (uint64_t)p->jb_rows + 1024 && range <= (1ull << 30)) {
-            jf.mode = 1; jf.dense_min = h_mm[0]; jf.dense_size = range;
-            if ((rc = ensure_buf(p, (void**)&p->jf_dense, &p->jf_dense_cap, (size_t)range * 4))) return rc;
-            jf.dense = p->jf_dense;
-        } else if (kb <= 4) {
-            uint32_t pc = 1024; while ((int64_t)pc < 2 * p->jb_rows) pc <<= 1;
-            jf.mode = 2; jf.packed_mask = pc - 1;
-            if ((rc = ensure_buf(p, (void**)&p->jf_packed, &p->jf_packed_cap, (size_t)pc * 8))) return rc;
-            jf.packed = p->jf_packed;
-        }
-        if (jf.mode) {
-            CK(p, launch_join_build_fast(key, c.cols[ki].prim, c.join_key_prim, p->jb_rows, jf, p->jf_dense, p->jf_packed, dup, p->stream));
-            p->stats.kernel_launches += 1;
-            p->jf = jf;
-            if ((rc = join_compose_probe(p, dup + 1))) return rc;   // enqueued behind the build: all flags come back in one round trip
-            uint32_t h_flags[3] = {0, 0, 0};
-            CK(p, cudaMemcpyAsync(h_flags, dup, 12, cudaMemcpyDeviceToHost, p->stream));
-            CK(p, cudaStreamSynchronize(p->stream));
-            if (h_flags[2] && guessed) { retry_measured = true; goto again; }   // this run's keys left the learned range
-            if (h_flags[0]) { p->jf = JoinFast{}; p->jp = JoinProbe{}; }   // duplicate build keys: not a PK, the general probe runs
-            else if (h_flags[1]) p->jp = JoinProbe{};
-            p->jf_learned = true; p->jf_learn_min = h_mm[0]; p->jf_learn_max = h_mm[1];
-        } else if (guessed) { retry_measured = true; goto again; }   // (the learned range no longer fits this row count)
+    const int cls = host_prim_class(cast_prim);
+    const uint64_t bias = cls == VC_I64 ? 0x8000000000000000ull : 0ull;
+    if ((rc = ensure_buf(p, (void**)&p->j_scratch, &p->j_scratch_cap, 64))) return rc;
+    uint64_t* mm = p->j_scratch; uint32_t* dup = (uint32_t*)(p->j_scratch + 2);
+    // the key range: measured (one pass over the keys + a round trip), or — when this plan has built before — the range it saw then,
+    // checked by the build kernel itself (a key outside it raises a flag and the build is redone with a measured range)
+    uint64_t h_mm[2];
+    bool guessed = s.learned && !retry_measured && p->join_learn_range;
+    if (guessed) { h_mm[0] = s.learn_min; h_mm[1] = s.learn_max; }
+    else {
+        CK(p, launch_join_minmax(key, key.prim, cast_prim, s.rows, bias, mm, p->stream));
+        CK(p, cudaMemcpyAsync(h_mm, mm, 16, cudaMemcpyDeviceToHost, p->stream));
+        CK(p, cudaStreamSynchronize(p->stream));
+        p->stats.kernel_launches++;
     }
+    JoinFast jf{}; jf.bias = bias;
+    const uint64_t range = h_mm[1] >= h_mm[0] ? h_mm[1] - h_mm[0] + 1 : 0;
+    const int kb = storage_bytes(prim_storage(cast_prim));
+    if (range > 0 && range <= (uint64_t)4 * (uint64_t)s.rows + 1024 && range <= (1ull << 30)) {
+        jf.mode = 1; jf.dense_min = h_mm[0]; jf.dense_size = range;
+        if ((rc = ensure_buf(p, (void**)&s.jf_dense, &s.jf_dense_cap, (size_t)range * 4))) return rc;
+        jf.dense = s.jf_dense;
+    } else if (kb <= 4) {
+        uint32_t pc = 1024; while ((int64_t)pc < 2 * s.rows) pc <<= 1;
+        jf.mode = 2; jf.packed_mask = pc - 1;
+        if ((rc = ensure_buf(p, (void**)&s.jf_packed, &s.jf_packed_cap, (size_t)pc * 8))) return rc;
+        jf.packed = s.jf_packed;
+    }
+    if (jf.mode) {
+        CK(p, launch_join_build_fast(key, key.prim, cast_prim, s.rows, jf, s.jf_dense, s.jf_packed, dup, p->stream));
+        p->stats.kernel_launches += 1;
+        s.jf = jf;
+        if (compose && (rc = join_compose_probe(p, dup + 1))) return rc;   // enqueued behind the build: all flags come back in one round trip
+        uint32_t h_flags[3] = {0, 0, 0};
+        CK(p, cudaMemcpyAsync(h_flags, dup, 12, cudaMemcpyDeviceToHost, p->stream));
+        CK(p, cudaStreamSynchronize(p->stream));
+        if (h_flags[2] && guessed) { retry_measured = true; goto again; }   // this run's keys left the learned range
+        if (h_flags[0]) { s.jf = JoinFast{}; p->jp = JoinProbe{}; }   // duplicate build keys: not a PK, the general probe runs
+        else if (h_flags[1]) p->jp = JoinProbe{};
+        s.learned = true; s.learn_min = h_mm[0]; s.learn_max = h_mm[1];
+    } else if (guessed) { retry_measured = true; goto again; }   // (the learned range no longer fits this row count)
+    return BKGPU_OK;
+}
+
+static int join_build_table(bkgpu_plan* p) {
+    const Compiled& c = p->c;
+    JoinSide& s = p->js[0];
+    const size_t nc = c.cols.size();
+    int rc;
+    if ((rc = join_pack_validity(p, s, 1))) return rc;
+    p->jt_built = true; s.jt_generic = false;   // the multimap of the general probe is built on first use (join_generic_table)
+    // ---- FK -> PK fast path: are the build keys unique, and is their range dense or their type <= 32 bits? ----
+    s.jf = JoinFast{}; p->jp = JoinProbe{};
+    if (p->jg_buf.empty()) p->jg_buf.assign(nc, nullptr);
+    bool build_nulls = false;
+    for (size_t i = 0; i < nc; i++) if (c.col_side[i] == 1 && s.has_null[i]) build_nulls = true;   // gathered columns must be NULL-free
+    if (!c.jfast || build_nulls) return BKGPU_OK;
+    return join_build_index(p, s, side_col(c, s, (size_t)c.build_key_col), c.join_key_prim, true);
+}
+
+// the multimap of side `s` (duplicate build keys, the general probe): open addressing from the cast key image to the build row
+static int join_build_multimap(bkgpu_plan* p, JoinSide& s, const DevCol& key, int cast_prim) {
+    int rc;
+    uint32_t cap = 1024;
+    while ((int64_t)cap < 2 * s.rows) cap <<= 1;
+    dev_free(p, s.jt_keys); dev_free(p, s.jt_rows); s.jt_keys = nullptr; s.jt_rows = nullptr;
+    if ((rc = dev_alloc(p, (void**)&s.jt_keys, (size_t)cap * 8))) return rc;
+    if ((rc = dev_alloc(p, (void**)&s.jt_rows, (size_t)cap * 4))) return rc;
+    s.jt_mask = cap - 1;
+    CK(p, launch_join_build(key, key.prim, cast_prim, s.rows, s.jt_keys, s.jt_rows, s.jt_mask, p->stream));
+    p->stats.kernel_launches++;
+    s.jt_generic = true;
     return BKGPU_OK;
 }
 
 // the general probe's multimap (duplicate build keys, unmatched probe rows): built only when a batch needs it
 static int join_generic_table(bkgpu_plan* p) {
-    if (p->jt_generic) return BKGPU_OK;
     const Compiled& c = p->c;
+    JoinSide& s = p->js[0];
+    if (s.jt_generic) return BKGPU_OK;
     int rc;
-    uint32_t cap = 1024;
-    while ((int64_t)cap < 2 * p->jb_rows) cap <<= 1;
-    dev_free(p, p->jt_keys); dev_free(p, p->jt_rows);
-    if ((rc = dev_alloc(p, (void**)&p->jt_keys, (size_t)cap * 8))) return rc;
-    if ((rc = dev_alloc(p, (void**)&p->jt_rows, (size_t)cap * 4))) return rc;
-    p->jt_mask = cap - 1;
-    DevCol key{};
-    const size_t ki = (size_t)c.build_key_col;
-    key.values = p->jb_vals[ki]; key.validity = p->jb_bitmap[ki]; key.stype = prim_storage(c.cols[ki].prim); key.prim = c.cols[ki].prim;
-    CK(p, launch_join_build(key, c.cols[ki].prim, c.join_key_prim, p->jb_rows, p->jt_keys, p->jt_rows, p->jt_mask, p->stream));
-    p->stats.kernel_launches++;
+    if ((rc = join_build_multimap(p, s, side_col(c, s, (size_t)c.build_key_col), c.join_key_prim))) return rc;
     if (c.join_type != BK_INNER_JOIN) {   // one "found a partner" byte per build row
-        if ((rc = ensure_buf(p, (void**)&p->jb_matched, &p->jb_matched_cap, (size_t)std::max<int64_t>(p->jb_rows, 1)))) return rc;
-        CK(p, cudaMemsetAsync(p->jb_matched, 0, (size_t)std::max<int64_t>(p->jb_rows, 1), p->stream));
+        if ((rc = ensure_buf(p, (void**)&p->jb_matched, &p->jb_matched_cap, (size_t)std::max<int64_t>(s.rows, 1)))) return rc;
+        CK(p, cudaMemsetAsync(p->jb_matched, 0, (size_t)std::max<int64_t>(s.rows, 1), p->stream));
     }
-    p->jt_generic = true;
     return BKGPU_OK;
 }
 
@@ -1040,11 +1083,11 @@ static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nro
     const Compiled& c = p->c;
     std::vector<DevCol> all(c.cols.size());
     for (size_t i = 0; i < c.cols.size(); i++) {
-        if (c.col_side[i] == 1) { all[i].values = p->jb_vals[i]; all[i].validity = p->jb_bitmap[i]; all[i].stype = prim_storage(c.cols[i].prim); all[i].prim = c.cols[i].prim; }
+        if (c.col_side[i] == 1) { all[i].values = p->js[0].vals[i]; all[i].validity = p->js[0].bitmap[i]; all[i].stype = prim_storage(c.cols[i].prim); all[i].prim = c.cols[i].prim; }
     }
     for (size_t w = 0; w < p->probe_map.size(); w++) all[(size_t)p->probe_map[w]] = probe_cols[w];
     // ---- FK -> PK fast path: gather the build columns next to the probe rows, then the ordinary (lean) aggregate ----
-    if (p->jf.mode != 0 && p->jp.mode != 0 && c.jfast && !p->force_generic && !p->no_fused_probe) {
+    if (p->js[0].jf.mode != 0 && p->jp.mode != 0 && c.jfast && !p->force_generic && !p->no_fused_probe) {
         // ---- fused probe: the lean aggregate reads the foreign key and looks the group key up itself ----
         const Compiled& f = *c.jfast;
         std::vector<DevCol> fc(f.cols.size());
@@ -1057,7 +1100,7 @@ static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nro
         const int rc = launch_agg_batch(p, f, fc.data(), nrows, vec_ok, &p->jp);
         if (rc <= 0) return rc;   // launched (0) or failed (< 0); +1: this batch does not fit the lean kernel
     }
-    if (p->jf.mode != 0 && c.jfast && !p->force_generic) {
+    if (p->js[0].jf.mode != 0 && c.jfast && !p->force_generic) {
         const Compiled& f = *c.jfast;
         const int64_t chunk = 16 << 20;   // the gathered chunk is re-read immediately: keep it L2-sized
         for (int64_t off = 0; off < nrows; off += chunk) {
@@ -1072,7 +1115,7 @@ static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nro
                         dev_free(p, p->jg_buf[m]); p->jg_buf[m] = nullptr;
                         if ((rc = dev_alloc(p, (void**)&p->jg_buf[m], (size_t)chunk * eb))) return rc;
                     }
-                    gc.src[gc.n] = p->jb_vals[m]; gc.dst[gc.n] = p->jg_buf[m]; gc.elem[gc.n] = (int32_t)eb; gc.n++;
+                    gc.src[gc.n] = p->js[0].vals[m]; gc.dst[gc.n] = p->jg_buf[m]; gc.elem[gc.n] = (int32_t)eb; gc.n++;
                     fc[i].values = p->jg_buf[m]; fc[i].validity = nullptr; fc[i].stype = prim_storage(c.cols[m].prim); fc[i].prim = c.cols[m].prim;
                 } else {
                     fc[i] = all[m];
@@ -1085,7 +1128,7 @@ static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nro
             pk.values = (const uint8_t*)pk.values + (size_t)off * (size_t)storage_bytes(pk.stype);
             if (pk.validity) pk.validity += off / 8;
             CK(p, cudaMemsetAsync(p->d_cursor + 1, 0, 4, p->stream));
-            CK(p, launch_join_gather(pk, c.cols[(size_t)c.probe_key_col].prim, c.join_key_prim, n, p->jf, gc, p->d_cursor + 1, p->stream));
+            CK(p, launch_join_gather(pk, c.cols[(size_t)c.probe_key_col].prim, c.join_key_prim, n, p->js[0].jf, gc, p->d_cursor + 1, p->stream));
             p->stats.kernel_launches++;
             uint32_t miss = 0;
             CK(p, cudaMemcpyAsync(&miss, p->d_cursor + 1, 4, cudaMemcpyDeviceToHost, p->stream));
@@ -1114,17 +1157,17 @@ static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nro
 // aggregate — unmatched rows NULL-extended (LEFT), matched rows (SEMI), unmatched rows (ANTI_SEMI); join_node.cpp:1200-1276
 static int join_tail(bkgpu_plan* p) {
     const Compiled& c = p->c;
-    if (p->jb_rows == 0) return BKGPU_OK;
+    if (p->js[0].rows == 0) return BKGPU_OK;
     int rc;
     if (!p->jt_built && (rc = join_build_table(p))) return rc;
     if ((rc = join_generic_table(p))) return rc;
     std::vector<DevCol> all(c.cols.size());
     for (size_t i = 0; i < c.cols.size(); i++) {
         all[i].stype = prim_storage(c.cols[i].prim); all[i].prim = c.cols[i].prim;
-        if (c.col_side[i] == 1) { all[i].values = p->jb_vals[i]; all[i].validity = p->jb_bitmap[i]; }   // (probe-side columns are never read: row = -1 is NULL)
+        if (c.col_side[i] == 1) { all[i].values = p->js[0].vals[i]; all[i].validity = p->js[0].bitmap[i]; }   // (probe-side columns are never read: row = -1 is NULL)
     }
     p->join_tail_launch = true;
-    rc = launch_agg_batch(p, c, all.data(), p->jb_rows, false);
+    rc = launch_agg_batch(p, c, all.data(), p->js[0].rows, false);
     p->join_tail_launch = false;
     return rc;
 }
@@ -1138,12 +1181,12 @@ static int join_rows_emit(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t
     const int ncols = (int)c.cols.size();
     for (int i = 0; i < ncols; i++) a.cols[i] = all[(size_t)i];
     a.n_cols = ncols;
-    a.join.enabled = 1; a.join.keys = p->jt_keys; a.join.rows = p->jt_rows; a.join.cap_mask = p->jt_mask;
+    a.join.enabled = 1; a.join.keys = p->js[0].jt_keys; a.join.rows = p->js[0].jt_rows; a.join.cap_mask = p->js[0].jt_mask;
     a.join.probe_col = c.probe_key_col; a.join.probe_prim = c.cols[(size_t)c.probe_key_col].prim; a.join.cast_prim = c.join_key_prim;
-    a.join.join_type = c.join_type; a.join.matched = c.join_type == BK_INNER_JOIN ? nullptr : p->jb_matched; a.join.n_build = p->jb_rows;
+    a.join.join_type = c.join_type; a.join.matched = c.join_type == BK_INNER_JOIN ? nullptr : p->jb_matched; a.join.n_build = p->js[0].rows;
     a.join.tail = tail ? 1 : 0;
     if ((rc = ensure_buf(p, (void**)&p->jr_cursor, &p->jr_cursor_cap, 64))) return rc;
-    size_t want = (size_t)std::max<int64_t>(tail ? p->jb_rows : n_probe, 1 << 12);
+    size_t want = (size_t)std::max<int64_t>(tail ? p->js[0].rows : n_probe, 1 << 12);
     uint32_t found = 0;
     for (int attempt = 0; attempt < 2; attempt++) {   // a batch with more pairs than the buffer holds is counted, the buffer grown, the batch rerun
         if (want > 0x7FFFFFF0ull) return p->fail(BKGPU_ETOOBIG, "a probe batch joins to more than 2^31 rows: push smaller batches");
@@ -1173,7 +1216,7 @@ static int join_rows_emit(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t
     std::vector<DevCol> dc(std::max<size_t>(nc, 1));
     for (size_t k = 0; k < nc; k++) {   // sink column k = output column k = device column k of the join (plan.cpp::lower_join_rows)
         const int st = prim_storage(pc.cols[k].prim);
-        CK(p, launch_join_rows_gather(all[k], p->jr_pairs, c.col_side[k] == 1 ? 1 : 0, found, storage_bytes(st), p->post_vals[k], p->post_nullb[k], p->stream));
+        CK(p, launch_join_rows_gather(all[k], p->jr_pairs, 2, c.col_side[k] == 1 ? 1 : 0, found, storage_bytes(st), p->post_vals[k], p->post_nullb[k], p->stream));
         CK(p, launch_pack_validity(p->post_nullb[k], found, p->post_bitmap[k], p->stream));
         dc[k].values = p->post_vals[k]; dc[k].validity = p->post_bitmap[k]; dc[k].stype = st; dc[k].prim = pc.cols[k].prim;
     }
@@ -1188,7 +1231,7 @@ static void join_all_cols(bkgpu_plan* p, const DevCol* probe_cols, std::vector<D
     all.assign(c.cols.size(), DevCol{});
     for (size_t i = 0; i < c.cols.size(); i++) {
         all[i].stype = prim_storage(c.cols[i].prim); all[i].prim = c.cols[i].prim;
-        if (c.col_side[i] == 1) { all[i].values = p->jb_vals[i]; all[i].validity = p->jb_bitmap[i]; }
+        if (c.col_side[i] == 1) { all[i].values = p->js[0].vals[i]; all[i].validity = p->js[0].bitmap[i]; }
     }
     if (probe_cols) for (size_t w = 0; w < p->probe_map.size(); w++) all[(size_t)p->probe_map[w]] = probe_cols[w];
 }
@@ -1202,7 +1245,7 @@ static int join_rows_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nrow
 static int join_rows_finish(bkgpu_plan* p) {
     const Compiled& c = p->c;
     int rc;
-    if (c.join_type != BK_INNER_JOIN && p->jb_rows > 0) {   // LEFT: the preserved rows that found no partner, NULL-extended
+    if (c.join_type != BK_INNER_JOIN && p->js[0].rows > 0) {   // LEFT: the preserved rows that found no partner, NULL-extended
         if (!p->jt_built && (rc = join_build_table(p))) return rc;
         if ((rc = join_generic_table(p))) return rc;
         std::vector<DevCol> all;
@@ -1227,10 +1270,137 @@ static int join_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t
     const Compiled& c = p->c;
     bool is_build = false;
     for (int k = 0; k < ncols; k++) if (cols[k].tuple_id == c.build_tuple) is_build = true;
-    if (is_build) return join_retain_build(p, cols, ncols, nrows, on_device);
+    if (is_build) return join_retain_build(p, p->js[0], 1, cols, ncols, nrows, on_device);
     if (!p->jt_built) { int rc = join_build_table(p); if (rc) return rc; }
     if (p->probe_want.empty()) for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] == 0) { p->probe_want.push_back(c.cols[i]); p->probe_map.push_back((int)i); }
     return feed(p, p->probe_want, cols, ncols, nrows, on_device, c.kind == PK_JOIN ? join_rows_batch : join_probe_batch);
+}
+
+// ---- star join (PK_STAR_AGG): every dimension is retained and indexed before the first fact batch ----
+static int star_build(bkgpu_plan* p) {
+    const Compiled& c = p->c;
+    p->jt_built = true;
+    int rc;
+    for (size_t d = 0; d < c.dims.size(); d++) {
+        JoinSide& s = p->js[d];
+        const StarDim& sd = c.dims[d];
+        if ((rc = join_pack_validity(p, s, 1 + (int)d))) return rc;
+        s.jt_generic = false; s.jf = JoinFast{};
+        if (s.rows == 0) continue;
+        DevCol key = side_col(c, s, (size_t)sd.key_col);
+        if (sd.n_filter > 0) {   // the build key's validity: the key is not NULL and the dimension's own conjuncts are TRUE
+            if ((rc = ensure_buf(p, (void**)&s.keybits, &s.keybits_cap, ((size_t)s.rows + 31) / 32 * 4))) return rc;
+            StarFilter f; memset(&f, 0, sizeof f);
+            for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] == 1 + (int)d) f.cols[i] = side_col(c, s, i);
+            f.prog = sd.filter; f.key_col = sd.key_col; f.nrows = s.rows;
+            CK(p, launch_star_dim_filter(f, (uint32_t*)s.keybits, p->stream));
+            p->stats.kernel_launches++;
+            key.validity = s.keybits;
+        }
+        // unique keys: the dense or packed index; duplicate keys (or 64-bit keys over a wide range): the multimap
+        if ((rc = join_build_index(p, s, key, sd.cast_prim, false))) return rc;
+        if (s.jf.mode == 0 && (rc = join_build_multimap(p, s, key, sd.cast_prim))) return rc;
+    }
+    return BKGPU_OK;
+}
+
+// the tuple buffer `k` with room for `n` tuples of `w` row ids
+static int star_tuples(bkgpu_plan* p, int k, uint64_t n, int w) {
+    if (n * (uint64_t)w > 0xFFFFFFF0ull) return p->fail(BKGPU_ETOOBIG, "a star join chunk joins to more than 2^32 row ids: push smaller batches");
+    return ensure_buf(p, (void**)&p->st_tuples[k], &p->st_tuples_cap[k], (size_t)std::max<uint64_t>(n, 1) * (size_t)w * 4);
+}
+
+// A fact batch, chunk by chunk: k_star_probe keeps the rows with a partner in every dimension of unique keys, each dimension with duplicate
+// keys expands the survivors (k_star_expand), the referenced columns are gathered side by side, and the aggregate runs over them as the
+// virtual joined tuple (Compiled::jfast: the lean kernel when the shape fits).
+static int star_probe_batch(bkgpu_plan* p, const DevCol* fact_cols, int64_t nrows, int64_t, bool vec_ok) {
+    const Compiled& c = p->c;
+    const Compiled& f = *c.jfast;
+    const int D = (int)c.dims.size(), W = 1 + D;
+    for (int d = 0; d < D; d++) if (p->js[d].rows == 0) return BKGPU_OK;   // an empty dimension: no row joins
+    std::vector<DevCol> all(c.cols.size());
+    for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] > 0) all[i] = side_col(c, p->js[c.col_side[i] - 1], i);
+    for (size_t w = 0; w < p->probe_map.size(); w++) all[(size_t)p->probe_map[w]] = fact_cols[w];
+    if (p->st_vals.empty()) for (auto* v : {&p->st_vals, &p->st_nullb, &p->st_bits}) v->assign(c.cols.size(), nullptr);
+    if (p->st_vals_cap.empty()) for (auto* v : {&p->st_vals_cap, &p->st_nullb_cap, &p->st_bits_cap}) v->assign(c.cols.size(), 0);
+    int rc;
+    const int64_t chunk = 16 << 20;
+    for (int64_t off = 0; off < nrows; off += chunk) {
+        const int64_t n = std::min(chunk, nrows - off);
+        auto fact_col = [&](size_t i) {   // (the chunk of a fact column)
+            DevCol x = all[i];
+            x.values = (const uint8_t*)x.values + (size_t)off * (size_t)storage_bytes(x.stype);
+            if (x.validity) x.validity += off / 8;
+            return x;
+        };
+        StarProbe sp; memset(&sp, 0, sizeof sp);
+        sp.width = W; sp.nrows = n; sp.vec = vec_ok ? 1 : 0;
+        for (int d = 0; d < D; d++) {
+            if (p->js[d].jf.mode == 0) continue;
+            const StarDim& sd = c.dims[(size_t)d];
+            StarLookup& L = sp.d[sp.n++];
+            L.fk = fact_col((size_t)sd.fk_col); L.from_prim = c.cols[(size_t)sd.fk_col].prim; L.cast_prim = sd.cast_prim; L.slot = 1 + d; L.jf = p->js[d].jf;
+        }
+        if ((rc = star_tuples(p, 0, (uint64_t)n, W))) return rc;
+        CK(p, launch_star_probe(sp, p->st_tuples[0], p->d_cursor + 1, p->sm_count, p->stream));
+        p->stats.kernel_launches++;
+        uint32_t found = 0;
+        CK(p, cudaMemcpyAsync(&found, p->d_cursor + 1, 4, cudaMemcpyDeviceToHost, p->stream));
+        CK(p, cudaStreamSynchronize(p->stream));
+        int cur = 0;
+        for (int d = 0; d < D && found; d++) {   // dimensions with duplicate keys: one expansion pass each
+            const JoinSide& s = p->js[d];
+            if (s.jf.mode != 0) continue;
+            const StarDim& sd = c.dims[(size_t)d];
+            uint64_t cap = p->star_expand_cap > 0 ? (uint64_t)p->star_expand_cap : std::max<uint64_t>(2 * (uint64_t)found, 4096);
+            uint32_t got = 0;
+            for (int attempt = 0; attempt < 2; attempt++) {   // more tuples than the buffer holds: counted, the buffer grown to the count, the pass rerun
+                if ((rc = star_tuples(p, 1 - cur, cap, W))) return rc;
+                CK(p, launch_star_expand(fact_col((size_t)sd.fk_col), c.cols[(size_t)sd.fk_col].prim, sd.cast_prim, s.jt_keys, s.jt_rows, s.jt_mask, p->st_tuples[cur], found,
+                                         W, 1 + d, p->st_tuples[1 - cur], (uint32_t)cap, p->d_cursor + 1, p->stream));
+                p->stats.kernel_launches++;
+                CK(p, cudaMemcpyAsync(&got, p->d_cursor + 1, 4, cudaMemcpyDeviceToHost, p->stream));
+                CK(p, cudaStreamSynchronize(p->stream));
+                if (got <= cap) break;
+                cap = got;
+            }
+            found = got; cur = 1 - cur;
+        }
+        if (!found) continue;
+        // the joined chunk: every column the aggregate reads, gathered from its tuple's row
+        std::vector<DevCol> fc(f.cols.size());
+        for (size_t i = 0; i < f.cols.size(); i++) {
+            const size_t m = (size_t)c.jfast_of_main[i];
+            const int side = c.col_side[m];
+            const DevCol src = side == 0 ? fact_col(m) : all[m];
+            const int eb = storage_bytes(src.stype);
+            if ((rc = ensure_buf(p, (void**)&p->st_vals[m], &p->st_vals_cap[m], (size_t)found * (size_t)eb))) return rc;
+            fc[i] = src; fc[i].values = p->st_vals[m]; fc[i].validity = nullptr;
+            if (src.validity) {   // NULLs travel along: null bytes, then a bitmap
+                if ((rc = ensure_buf(p, (void**)&p->st_nullb[m], &p->st_nullb_cap[m], (size_t)found))) return rc;
+                if ((rc = ensure_buf(p, (void**)&p->st_bits[m], &p->st_bits_cap[m], (size_t)found / 8 + 8))) return rc;
+            }
+            CK(p, launch_join_rows_gather(src, p->st_tuples[cur], W, side, found, eb, p->st_vals[m], src.validity ? p->st_nullb[m] : nullptr, p->stream));
+            p->stats.kernel_launches++;
+            if (src.validity) {
+                CK(p, launch_pack_validity(p->st_nullb[m], found, p->st_bits[m], p->stream));
+                p->stats.kernel_launches++;
+                fc[i].validity = p->st_bits[m];
+            }
+        }
+        if ((rc = launch_agg_batch(p, f, fc.data(), found, true))) return rc;
+    }
+    return BKGPU_OK;
+}
+
+static int star_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device) {
+    const Compiled& c = p->c;
+    for (size_t d = 0; d < c.dims.size(); d++)
+        for (int k = 0; k < ncols; k++)
+            if (cols[k].tuple_id == c.dims[d].tuple_id) return join_retain_build(p, p->js[d], 1 + (int)d, cols, ncols, nrows, on_device);
+    if (!p->jt_built) { int rc = star_build(p); if (rc) return rc; }
+    if (p->probe_want.empty()) for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] == 0) { p->probe_want.push_back(c.cols[i]); p->probe_map.push_back((int)i); }
+    return feed(p, p->probe_want, cols, ncols, nrows, on_device, star_probe_batch);
 }
 
 static int bkgpu_push_impl(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device);
@@ -1259,6 +1429,7 @@ static int bkgpu_push_impl(bkgpu_plan* p, const bkgpu_column* cols, int ncols, i
             return BKGPU_OK;
         }
         case PK_JOIN_AGG: case PK_JOIN: return join_push(p, cols, ncols, nrows, on_device);
+        case PK_STAR_AGG: return star_push(p, cols, ncols, nrows, on_device);
         case PK_SORT: case PK_FILTER: return feed(p, p->c.cols, cols, ncols, nrows, on_device, sort_batch);
         default: return p->fail(BKGPU_EUNSUPPORTED, "plan kind %d has no push path yet", p->c.kind);
     }
@@ -1610,7 +1781,7 @@ static int bkgpu_finish_impl(bkgpu_plan* p) {
     CK(p, cudaSetDevice(p->device));
     int rc = BKGPU_OK;
     switch (p->c.kind) {
-        case PK_AGG: case PK_JOIN_AGG: {
+        case PK_AGG: case PK_JOIN_AGG: case PK_STAR_AGG: {
             if (p->c.kind == PK_JOIN_AGG && p->c.join_type != BK_INNER_JOIN && (rc = join_tail(p))) break;
             rc = agg_finish(p);
             if (!rc) {
@@ -1633,7 +1804,7 @@ static int bkgpu_finish_impl(bkgpu_plan* p) {
         default: rc = p->fail(BKGPU_EUNSUPPORTED, "plan kind %d cannot finish", p->c.kind);
     }
     // (a finished aggregate without a post fragment has already waited for everything it queued: agg_wait)
-    if (rc || !((p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG) && !p->c.post)) cudaStreamSynchronize(p->stream);
+    if (rc || !((p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) && !p->c.post)) cudaStreamSynchronize(p->stream);
     resolve_timers(p);
     if (rc) return rc;
     p->stats.rows_returned = p->result_rows;
@@ -1683,7 +1854,7 @@ static int bkgpu_reset_impl(bkgpu_plan* p) {
     if (p->state != S_OPEN && p->state != S_FINISHED) return p->fail(BKGPU_ESTATE, "bkgpu_reset needs an opened plan");
     CK(p, cudaSetDevice(p->device));
     p->cancelled.store(0);
-    if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG) {
+    if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) {
         // a finished run knows how many groups its table holds (the count came back with the result): clear those slots through the
         // occupied list instead of re-initialising the whole capacity (2^20 slots = 44 MB by default)
         if (p->state == S_FINISHED && p->finish_groups >= 0 && p->c.ap.n_keyw > 0) CK(p, launch_table_clear(p->gt, p->c.ap, (uint32_t)p->finish_groups, p->stream));
@@ -1692,8 +1863,11 @@ static int bkgpu_reset_impl(bkgpu_plan* p) {
         p->fused_last = false;
         p->stats.kernel_launches++;
     }
-    p->jb_rows = 0; p->jt_built = false; p->jt_generic = false; std::fill(p->jb_has_null.begin(), p->jb_has_null.end(), false);
-    for (size_t i = 0; i < p->jb_bitmap.size(); i++) { dev_free(p, p->jb_bitmap[i]); p->jb_bitmap[i] = nullptr; }   // build-side validity of the previous run
+    p->jt_built = false;
+    for (JoinSide& s : p->js) {
+        s.rows = 0; s.jt_generic = false; std::fill(s.has_null.begin(), s.has_null.end(), false);
+        for (size_t i = 0; i < s.bitmap.size(); i++) { dev_free(p, s.bitmap[i]); s.bitmap[i] = nullptr; }   // build-side validity of the previous run
+    }
     if (p->sort) { int rc = sort_reset(p->sort, p->stream, p->last_error); if (rc) { g_thread_error = p->last_error; return rc; } }
     if (p->c.kind == PK_JOIN && p->post_sort) { int rc = sort_reset(p->post_sort, p->stream, p->last_error); if (rc) { g_thread_error = p->last_error; return rc; } }
     p->result.clear(); p->result_rows = 0; p->result_pos = 0;
@@ -1813,7 +1987,7 @@ extern "C" int bkgpu_push_region(bkgpu_plan* p, int64_t region_id) {
 // ------------------------------------------------------------------ partial state
 extern "C" int bkgpu_partial_capacity(bkgpu_plan* p, size_t* bytes) {
     if (!p || !bytes) return thread_fail(BKGPU_EINVAL, "bkgpu_partial_capacity: NULL argument");
-    if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG) { *bytes = 8 * (1 + (size_t)(p->c.ap.n_keyw + p->c.ap.n_lanes) * (size_t)eff_pcap(p)); return BKGPU_OK; }
+    if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) { *bytes = 8 * (1 + (size_t)(p->c.ap.n_keyw + p->c.ap.n_lanes) * (size_t)eff_pcap(p)); return BKGPU_OK; }
     if (p->c.kind == PK_SORT && p->sort) { *bytes = sort_partial_bytes(p->sort); return BKGPU_OK; }
     return p->fail(BKGPU_EUNSUPPORTED, "plan kind %d has no partial state", p->c.kind);
 }

@@ -13,6 +13,7 @@
 #include <stdarg.h>
 #include <stdio.h>
 #include <string.h>
+#include <algorithm>
 #include <map>
 #include "../include/bkgpu.h"
 #include "datetime.h"
@@ -931,7 +932,14 @@ static void explain(Compiled& c) {
     std::string& s = c.explain;
     snprintf(buf, sizeof buf, "kind=%d scan_tuple=%d cols=%zu\n", c.kind, c.scan_tuple, c.cols.size()); s += buf;
     for (size_t i = 0; i < c.cols.size(); i++) { snprintf(buf, sizeof buf, "  col[%zu] = %d_%d prim=%d\n", i, c.cols[i].tuple_id, c.cols[i].slot_id, c.cols[i].prim); s += buf; }
-    if (c.kind == PK_AGG || c.kind == PK_JOIN_AGG) {
+    for (size_t k = 0; k < c.dims.size(); k++) {
+        const StarDim& d = c.dims[k];
+        if (k == 0) { snprintf(buf, sizeof buf, "star: fact tuple=%d dims=%zu\n", c.scan_tuple, c.dims.size()); s += buf; }
+        const ColRef &dk = c.cols[(size_t)d.key_col], &fk = c.cols[(size_t)d.fk_col];
+        snprintf(buf, sizeof buf, "  dim[%zu] tuple=%d key=%d_%d fk=%d_%d cast=%d build_conjuncts=%d\n", k, d.tuple_id, dk.tuple_id, dk.slot_id, fk.tuple_id, fk.slot_id,
+                 d.cast_prim, d.n_filter); s += buf;
+    }
+    if (c.kind == PK_AGG || c.kind == PK_JOIN_AGG || c.kind == PK_STAR_AGG) {
         const AggPlan& ap = c.ap;
         snprintf(buf, sizeof buf, "agg: n_group=%d n_keyw=%d n_agg=%d n_lanes=%d pred_out=%d direct=%d emit_default=%d\n", ap.n_group, ap.n_keyw,
                  ap.n_agg, ap.n_lanes, ap.pred_out, (int)c.has_direct, (int)c.emit_default); s += buf;
@@ -968,6 +976,8 @@ bool lower_filter(Infer& in, Compiled& out, const HNode* limit_node, const HNode
 bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& join, bool under_packet, const HNode* above);
 bool lower_post(Infer& in, Compiled& out, const HNode* sort, const HNode* having, const HNode* limit_node);
 bool lower_join_rows(Infer& in, Compiled& out, const HNode& join, const HNode* above, const HNode* sort, const HNode* limit_node);
+bool lower_star_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& join, bool under_packet, const HNode* above);
+static int join_leaves(const HNode* n);
 
 static bool infer_node(Infer& in, HNode& n) {
     for (auto& e : n.conjuncts) if (!infer_expr(in, e)) return false;
@@ -1035,7 +1045,7 @@ int compile_plan(const uint8_t* desc, size_t len, Compiled& out, std::string& er
             if (ok && limit_node && !post_sort && !post_having) { out.limit = limit_node->limit; out.offset = limit_node->offset; }
         } else if (c && c->node_type == BK_JOIN_NODE) {   // AGG -> [FILTER ->] JOIN: the store-side chain of a filtered join (separate.cpp:241-260)
             if (filter && filter->limit != -1) { err = "LIMIT on a filter below an aggregate is order dependent: outside the GPU path"; return BKGPU_EUNSUPPORTED; }
-            ok = lower_join_agg(in, out, *top, *c, under_packet, filter);
+            ok = join_leaves(c) > 2 ? lower_star_agg(in, out, *top, *c, under_packet, filter) : lower_join_agg(in, out, *top, *c, under_packet, filter);
             if (ok && limit_node && !post_sort && !post_having) { out.limit = limit_node->limit; out.offset = limit_node->offset; }   // LimitNode over the joined aggregate
         } else { err = "AGG child must be [FILTER ->] SCAN or JOIN"; return BKGPU_EUNSUPPORTED; }
         if (ok && (post_sort || post_having)) ok = lower_post(in, out, post_sort, post_having, limit_node);
@@ -1043,6 +1053,7 @@ int compile_plan(const uint8_t* desc, size_t len, Compiled& out, std::string& er
         const HNode* t = top; const HNode *js = nullptr, *jf = nullptr;
         if (t->node_type == BK_SORT_NODE) { js = t; t = skip_passthrough(&t->ch[0], nullptr); }
         if (is_filter(t)) jf = t;
+        if (join_leaves(jn) > 2) { err = "a join of more than two tables that returns rows is outside the GPU path (an aggregate over a star join is lowered)"; return BKGPU_EUNSUPPORTED; }
         ok = lower_join_rows(in, out, *jn, jf, js, limit_node);
     } else if (top->node_type == BK_SORT_NODE) {
         const HNode* c = top->ch.empty() ? nullptr : skip_passthrough(&top->ch[0], nullptr);
@@ -1278,6 +1289,133 @@ bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
             if (ok) out.jfast = jf; else out.jfast_of_main.clear();
         }
     }
+    return true;
+}
+
+// ---- star joins: AGG over a tree of INNER joins with 3 to 5 [FILTER ->] SCAN leaves ----
+// The reference runs these as nested JoinNodes (a left-deep chain from JoinReorder, src/physical_plan/join_reorder.cpp:116-134).  For INNER
+// joins the joined rows do not depend on the tree's shape, so left-deep, right-deep and bushy trees lower alike: the fact tuple is the leaf
+// that has an equality with every other leaf, every other leaf is a dimension keyed by its first equality with the fact tuple.
+static int join_leaves(const HNode* n) {
+    n = skip_passthrough(n, nullptr);
+    if (is_filter(n)) n = n->ch.empty() ? nullptr : skip_passthrough(&n->ch[0], nullptr);
+    if (!n || n->node_type != BK_JOIN_NODE) return 1;
+    int k = 0;
+    for (auto& c : n->ch) k += join_leaves(&c);
+    return k;
+}
+static bool star_walk(Infer& in, const HNode* n, std::vector<int>& leaves, std::vector<const HExpr*>& conds) {
+    n = skip_passthrough(n, nullptr);
+    if (is_filter(n)) {
+        if (n->limit != -1) return in.fail(BKGPU_EUNSUPPORTED, "LIMIT on a filter inside a join is order dependent: outside the GPU path");
+        for (auto& e : n->conjuncts) conds.push_back(&e);
+        n = n->ch.empty() ? nullptr : skip_passthrough(&n->ch[0], nullptr);
+    }
+    if (n && n->node_type == BK_JOIN_NODE) {
+        if (n->join_type != BK_INNER_JOIN) return in.fail(BKGPU_EUNSUPPORTED, "join type %d in a join of more than two tables: only INNER joins are lowered", n->join_type);
+        if (n->ch.size() != 2) return in.fail(BKGPU_EINVAL, "JOIN node needs two children");
+        for (auto& e : n->conjuncts) conds.push_back(&e);
+        return star_walk(in, &n->ch[0], leaves, conds) && star_walk(in, &n->ch[1], leaves, conds);
+    }
+    if (!n || n->node_type != BK_SCAN_NODE) return in.fail(BKGPU_EUNSUPPORTED, "JOIN children must be [FILTER ->] SCAN or JOIN");
+    leaves.push_back(n->tuple_id);
+    return true;
+}
+static void expr_tuples(const HExpr& e, std::vector<int>& t) {
+    if (e.node_type == BK_SLOT_REF && std::find(t.begin(), t.end(), e.tuple_id) == t.end()) t.push_back(e.tuple_id);
+    for (auto& c : e.ch) expr_tuples(c, t);
+}
+static bool slot_eq(const HExpr& e) {
+    return e.node_type == BK_FUNCTION_CALL && e.fn_op == BK_FT_EQ && e.ch.size() == 2 && e.ch[0].node_type == BK_SLOT_REF && e.ch[1].node_type == BK_SLOT_REF &&
+           e.ch[0].tuple_id != e.ch[1].tuple_id;
+}
+
+bool lower_star_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& join, bool under_packet, const HNode* above) {
+    std::vector<int> leaves; std::vector<const HExpr*> conds;
+    if (!star_walk(in, &join, leaves, conds)) return false;
+    if (leaves.size() > 5) return in.fail(BKGPU_EUNSUPPORTED, "a star join of %zu tables has more than 4 dimensions", leaves.size());
+    if (above) for (auto& e : above->conjuncts) conds.push_back(&e);
+    auto linked = [&](int a, int b) {
+        for (auto* e : conds)
+            if (slot_eq(*e) && ((e->ch[0].tuple_id == a && e->ch[1].tuple_id == b) || (e->ch[0].tuple_id == b && e->ch[1].tuple_id == a))) return true;
+        return false;
+    };
+    int fact = -1;
+    for (int t : leaves) {
+        bool all = true;
+        for (int u : leaves) if (u != t && !linked(t, u)) all = false;
+        if (all) { fact = t; break; }
+    }
+    if (fact < 0) return in.fail(BKGPU_EUNSUPPORTED, "join of %zu tables without a star centre (a dimension keyed only to another dimension): outside the GPU path", leaves.size());
+    std::vector<const HExpr*> taken;
+    auto is_signed_t = [](int t) { return t >= BK_INT8 && t <= BK_INT64; };
+    for (int t : leaves) {
+        if (t == fact) continue;
+        StarDim d; d.tuple_id = t;
+        const HExpr *dk = nullptr, *fk = nullptr;
+        for (auto* e : conds) {
+            if (!slot_eq(*e)) continue;
+            const HExpr *a = &e->ch[0], *b = &e->ch[1];
+            if (a->tuple_id == fact && b->tuple_id == t) std::swap(a, b);
+            if (a->tuple_id == t && b->tuple_id == fact) { dk = a; fk = b; taken.push_back(e); break; }
+        }
+        const int dt = dk->col_type, ft = fk->col_type;
+        if (dt == ft) d.cast_prim = dt;
+        else if (is_signed_t(dt) && is_signed_t(ft)) d.cast_prim = BK_INT64;
+        else if (is_uint_t(dt) && is_uint_t(ft)) d.cast_prim = BK_UINT64;
+        else return in.fail(BKGPU_EUNSUPPORTED, "join keys of types %d and %d are compared as STRING in the reference: outside the GPU path", dt, ft);
+        if (d.cast_prim == BK_STRING || is_double_t(d.cast_prim)) return in.fail(BKGPU_EUNSUPPORTED, "join key type %d is outside the GPU path", d.cast_prim);
+        d.key_col = dk->slot_id; d.fk_col = fk->slot_id;   // (slot ids until the columns are interned below)
+        out.dims.push_back(d);
+    }
+    // conjuncts over one dimension alone run once over its rows at build time; everything else is the aggregate's predicate
+    std::vector<const HExpr*> conj;
+    std::vector<std::vector<const HExpr*>> dim_conj(out.dims.size());
+    for (auto* e : conds) {
+        if (std::find(taken.begin(), taken.end(), e) != taken.end()) continue;
+        std::vector<int> ts; expr_tuples(*e, ts);
+        int di = -1;
+        if (ts.size() == 1) for (size_t i = 0; i < out.dims.size(); i++) if (out.dims[i].tuple_id == ts[0]) di = (int)i;
+        if (di >= 0) dim_conj[(size_t)di].push_back(e); else conj.push_back(e);
+    }
+    if (!lower_agg(in, out, agg, conj, fact, under_packet, false)) return false;
+    out.kind = PK_STAR_AGG;
+    Program dummy; memset(&dummy, 0, sizeof dummy);
+    Lower lw{&out, &in, &dummy, {}};
+    for (size_t i = 0; i < out.dims.size(); i++) {
+        StarDim& d = out.dims[i];
+        d.key_col = lw.intern_col(d.tuple_id, d.key_col, in.slot_type(d.tuple_id, d.key_col));
+        d.fk_col = lw.intern_col(fact, d.fk_col, in.slot_type(fact, d.fk_col));
+        memset(&d.filter, 0, sizeof d.filter);
+        if (dim_conj[i].empty()) continue;
+        if (dim_conj[i].size() > 8) return in.fail(BKGPU_EUNSUPPORTED, "more than 8 conjuncts on dimension %d", d.tuple_id);
+        const int n_const = out.n_const;   // (constants are numbered per program)
+        out.n_const = 0;
+        Lower fl{&out, &in, &d.filter, {}};
+        for (auto* c : dim_conj[i]) { int depth = 0; if (!fl.expr(*c, depth) || !fl.to_bool(*c)) return false; }
+        if (dim_conj[i].size() > 1 && !fl.emit(OP_AND, (uint8_t)dim_conj[i].size())) return false;
+        if (!fl.out_reg(0)) return false;
+        d.filter.n_out = 1; d.n_filter = (int)dim_conj[i].size();
+        out.n_const = n_const;
+    }
+    if ((int)out.cols.size() > MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d columns referenced", MAX_COLS);
+    for (size_t i = 0; i < out.cols.size(); i++) {
+        out.col_side[i] = 0;
+        for (size_t k = 0; k < out.dims.size(); k++) if (out.cols[i].tuple_id == out.dims[k].tuple_id) out.col_side[i] = 1 + (int)k;
+    }
+    // the aggregate over the gathered chunk: every column as a column of ONE (virtual, joined) tuple
+    auto jf = std::make_shared<Compiled>();
+    jf->tuples = out.tuples; jf->build_tuple = -1;
+    Infer in2{}; in2.tuples = &jf->tuples;
+    if (!lower_agg(in2, *jf, agg, conj, fact, under_packet, true) || memcmp(&jf->ap.n_keyw, &out.ap.n_keyw, sizeof(int32_t) * 4) != 0 || jf->ap.n_lanes != out.ap.n_lanes)
+        return in.fail(BKGPU_EUNSUPPORTED, "the aggregate over the joined row could not be lowered: %s", in2.err.c_str());
+    for (auto& c : jf->cols) {
+        int m = -1;
+        for (size_t i = 0; i < out.cols.size(); i++) if (out.cols[i].tuple_id == c.tuple_id && out.cols[i].slot_id == c.slot_id) m = (int)i;
+        if (m < 0) return in.fail(BKGPU_EINVAL, "column %d_%d of the joined row is not a plan column", c.tuple_id, c.slot_id);
+        out.jfast_of_main.push_back(m);
+    }
+    out.jfast = jf;
     return true;
 }
 

@@ -51,9 +51,18 @@ struct OutCol {
     int kind;       // 0 = plain value column, 1 = AVG intermediate blob (two device images: sum, count)
 };
 
-enum PlanKind { PK_AGG = 1, PK_FILTER = 2, PK_SORT = 3, PK_JOIN_AGG = 4, PK_JOIN = 5 };
+enum PlanKind { PK_AGG = 1, PK_FILTER = 2, PK_SORT = 3, PK_JOIN_AGG = 4, PK_JOIN = 5, PK_STAR_AGG = 6 };
 
 struct SortKey { int out_reg; int prim; bool asc, null_first; };
+
+// one dimension of a star join (PK_STAR_AGG): a table INNER-joined to the fact tuple on one key
+struct StarDim {
+    int tuple_id = -1;
+    int key_col = -1, fk_col = -1;     // indices into Compiled::cols: the dimension's key, the fact tuple's foreign key
+    int cast_prim = 0;                 // type both keys are compared in (strip_out_equal_slots' cast, joiner.cpp:166-217)
+    int n_filter = 0;                  // conjuncts that read this dimension alone: evaluated once over its rows at build time
+    Program filter;                    // output 0 = their conjunction (column indices into Compiled::cols)
+};
 
 struct Compiled {
     int kind = 0;
@@ -61,7 +70,7 @@ struct Compiled {
     // main (probe-side / only) scan
     int scan_tuple = -1;
     std::vector<ColRef> cols;          // columns the device program references (index = DevCol index)
-    std::vector<int> col_side;         // per column: 0 = probe / only scan tuple, 1 = build side of a join
+    std::vector<int> col_side;         // per column: 0 = probe / only scan tuple, 1 = build side of a join; star join: 0 = fact, 1 + d = dims[d]
     Program prog;                      // outputs: [predicate][keys...][agg args...] / sort keys
     int n_const = 0;
     // aggregate
@@ -87,6 +96,8 @@ struct Compiled {
     // to probe-row alignment first); usable while every probe row has exactly one match
     std::shared_ptr<Compiled> jfast;
     std::vector<int> jfast_of_main;    // for every column of jfast->cols: index of the same column in this->cols
+    // star join (PK_STAR_AGG): scan_tuple is the fact tuple; the aggregate runs as `jfast` over fact and dimension columns gathered side by side
+    std::vector<StarDim> dims;
     // operators ABOVE the aggregate ([LIMIT ->] [SORT ->] [HAVING ->] AGG, exec_node.cpp:347-394): a second, small fragment of kind
     // PK_SORT / PK_FILTER whose "scan tuple" is the aggregate's output row (its columns = this->out_cols, in order)
     std::shared_ptr<Compiled> post;

@@ -118,6 +118,8 @@ int   bkgpu_init(bkgpu_plan** out, const uint8_t* plan_desc, size_t len,
  *   "no_stream_copy"       the bounce copy uses memcpy instead of non-temporal stores (A/B)
  *   "join_learn_range"     (default 1) a re-run plan builds its join index with the key range it saw before, checked by the build kernel
  *   "join_pipeline"        (default 0) the fused FK->PK probe issues its lookups one drain ahead (opt-in)
+ *   "star_expand_capacity" (tests) first capacity, in row-id tuples, of a star join's expansion pass over a dimension with duplicate keys
+ *                          (0 = twice the pass's input); a pass that outgrows it is counted, grown to the exact count and run again
  *   "blocking_sync"        the wait for a request's result: 0 spins (cudaStreamSynchronize), 1 sleeps on a blocking-sync event, -1 (default) sleeps only
  *                          when several ranks share a small CPU budget (ranks > 1 and budget < 4 CPUs per rank)
  *   "lean_bank"            (default 0) the lean kernel deals each drained pass to lanes by shared-memory bank group (opt-in)
@@ -133,7 +135,11 @@ int   bkgpu_open(bkgpu_plan*);
  * read them when bkgpu_push returns (pinned or pageable alike).  on_device != 0 means `values`/`validity` are
  * device pointers on the plan's device; the kernels read them asynchronously on the plan's stream, so DEVICE
  * buffers must stay valid and unmodified until bkgpu_finish has returned (or until work the caller orders after
- * the plan's stream has run). */
+ * the plan's stream has run).
+ * Joins: a batch belongs to the table whose tuple its columns name.  Every batch of the build side (a two-table join's
+ * outer child; every dimension of a star join) is retained and must come before the first batch of the probe side (the
+ * inner child; the star join's fact table): a build-side batch after that returns BKGPU_ESTATE.  A caller that pulls
+ * its children in order puts the fact scan last. */
 int   bkgpu_push(bkgpu_plan*, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device);
 /* End of input: drain, run the cross-GPU merge when a communicator was given,
  * finalize aggregates (AggFnCall::finalize, src/expr/agg_fn_call.cpp:927-990). */
