@@ -1,166 +1,20 @@
 // api.cu — the C ABI of include/bkgpu.h: plan lifecycle (ExecNode::init/open/get_next/close
-// inverted into init/open/push/finish/get_next/close), batch staging, result materialisation.
-#include <cuda_runtime.h>
+// inverted into init/open/push/finish/get_next/close), batch staging, the aggregate's launch, exchange and result materialisation.
+// The hash join's host path is join.cu; the plan object (bkgpu_plan) is api_state.h.
 #include <dlfcn.h>
 #include <sched.h>
-#include <stdarg.h>
-#include <stdio.h>
-#include <stdlib.h>
-#include <time.h>
 #include <string.h>
 #include <algorithm>
-#include <atomic>
 #include <condition_variable>
 #include <functional>
 #include <map>
 #include <mutex>
-#include <string>
 #include <thread>
-#include <vector>
-#include "../include/bkgpu.h"
-#include "agg.h"
-#include "plan.h"
-#include "sort.h"
+#include "api_state.h"
 #include "nccl_dl.h"
 #include "build_id.h"
 
-using namespace bk;
-
-namespace {
-
 thread_local std::string g_thread_error;
-
-enum State { S_INIT = 0, S_OPEN = 1, S_FINISHED = 2, S_CLOSED = 3 };
-
-struct HostCol {  // one materialised result column (host memory owned by the plan)
-    OutCol desc;
-    int elem = 0;
-    std::vector<uint8_t> values;
-    std::vector<uint8_t> validity;  // LSB bitmap; empty = all valid
-    void* dev_values = nullptr;     // output_on_device
-};
-
-struct EventPair { cudaEvent_t a, b; int64_t bytes; };
-
-// one retained build side of a hash join (K4) and its key indexes
-struct JoinSide {
-    std::vector<uint8_t*> vals, nullbytes, bitmap;   // per plan column (this side's columns only)
-    std::vector<bool> has_null;
-    int64_t rows = 0, cap = 0;
-    uint8_t* keybits = nullptr; size_t keybits_cap = 0;   // star join: validity of the build key AND the dimension's build-time filter
-    uint64_t* jt_keys = nullptr; uint32_t* jt_rows = nullptr; uint32_t jt_mask = 0; bool jt_generic = false;   // multimap (duplicate keys)
-    JoinFast jf{}; uint32_t* jf_dense = nullptr; uint64_t* jf_packed = nullptr; size_t jf_dense_cap = 0, jf_packed_cap = 0;   // unique-key index
-    bool learned = false; uint64_t learn_min = 0, learn_max = 0;   // key range of the side's previous build (skips the min/max pass + round trip)
-};
-
-// BKGPU_TRACE=1: wall-clock time the HOST spends in each phase of a request (summed per plan, printed by bkgpu_close)
-struct HostClock {
-    double reset = 0, push = 0, collective = 0, extract_wait = 0, finish = 0; int64_t n = 0;
-    static double now() { timespec ts; clock_gettime(CLOCK_MONOTONIC, &ts); return ts.tv_sec * 1e3 + ts.tv_nsec / 1e6; }
-};
-
-}  // namespace
-
-struct bkgpu_plan {
-    Compiled c;
-    int device = 0;
-    int sm_count = 132;
-    State state = S_INIT;
-    std::string last_error;
-    std::atomic<int> cancelled{0};
-    void* nccl_comm = nullptr;
-    int nranks = 1;
-    // options
-    cudaStream_t stream = nullptr; bool own_stream = false;
-    cudaStream_t copy_stream = nullptr;
-    int group_cap_log2 = 20;
-    int smem_cap_log2 = -1;       // -1 = choose per batch
-    int64_t batch_capacity = 1 << 20;
-    int64_t chunk_rows = 8 << 20;
-    int64_t partial_cap = 1 << 16;
-    int force_generic = 0;
-    int no_lean = 0;
-    int output_on_device = 0;
-    int64_t region_base = 0;      // arrival index of this plan's first row (ties across GPUs break by (region, row))
-    // aggregate state
-    GroupTable gt{};
-    uint64_t* d_rows_passed = nullptr;
-    uint32_t* d_cursor = nullptr;
-    uint64_t* d_partial = nullptr;  // export buffer (this rank)
-    uint64_t* d_gather = nullptr;   // nranks export buffers
-    size_t d_partial_words = 0, d_gather_words = 0;
-    HostClock hclk; bool trace = getenv("BKGPU_TRACE") != nullptr;
-    std::vector<uint8_t*> bounce[2]; size_t bounce_rows = 0; cudaEvent_t bounce_done[2] = {nullptr, nullptr}; bool bounce_busy[2] = {false, false};
-    int scalar_tma = 1;           // COUNT(*) WHERE int32 <cmp> c runs the TMA-staged kernel (scalar_tma.cu); 0 = the LDG kernel
-    int no_bounce = 0;            // 1 = pageable host input goes straight to cudaMemcpyAsync (A/B of the bounce path)
-    int no_stream_copy = 0;       // 1 = the bounce copy uses memcpy instead of non-temporal stores (A/B, hostcopy.cpp)
-    uint32_t* jr_pairs = nullptr; size_t jr_pairs_cap = 0; uint32_t* jr_cursor = nullptr; size_t jr_cursor_cap = 0;   // PK_JOIN: (probe row, build row) pairs of one batch
-    uint8_t* jb_matched = nullptr; size_t jb_matched_cap = 0; bool join_tail_launch = false;   // LEFT / SEMI / ANTI: build rows that found a partner
-    SortState* post_sort = nullptr;                         // the post fragment above the aggregate (Compiled::post)
-    std::vector<uint8_t*> post_vals, post_nullb, post_bitmap; size_t post_cap = 0;
-    uint64_t rows_passed_host = 0;
-    int64_t finish_groups = -1;   // groups in the table when the last finish read the result back (-1 = unknown: full re-initialisation)
-    uint32_t merge_bound = 0, merge_bound_used = 0;   // groups per rank the all-gather is sized for (learned from earlier runs)
-    uint32_t* d_part_cursors = nullptr; int repartition = 0;   // hash repartition of the groups across ranks (option "repartition")
-    // merge over NVLink peer memory (option "peer_merge"): this rank's buffer, the peers' mappings of theirs, step counter
-    int peer_merge = 0, peer_rank = -1; bool peer_ready = false;
-    uint64_t* peer_local = nullptr; std::vector<uint64_t*> peer_ptr; uint64_t** d_peer_ptrs = nullptr; uint64_t peer_seq = 0; size_t peer_seg_words = 0;
-    uint32_t* d_peer_timeout = nullptr;
-    uint64_t* d_outv = nullptr; uint8_t* d_outn = nullptr; size_t out_cap_alloc = 0;  // extraction buffers (kept across resets)
-    std::vector<cudaEvent_t> event_pool;
-    uint64_t* h_outv = nullptr; uint8_t* h_outn = nullptr; size_t h_out_cap = 0;   // pinned landing area of the extracted rows
-    uint32_t known_groups = 0;
-    uint32_t* h_pinned = nullptr;   // [0] groups seen (async copy after every aggregate launch that does not extract its result), pinned
-    // mapped host buffer the lean kernel's last CTA extracts the result into (AggArgs::fused_out), and whether the request's last
-    // aggregate launch did so: then bkgpu_finish only waits and reads it
-    uint8_t* h_fused = nullptr; uint8_t* d_fused = nullptr; size_t fused_bytes = 0; uint32_t fused_cap = 0; bool fused_last = false;
-    // hash join (K4): the retained build side(s) and their indexes; the two-table join uses js[0], a star join one per dimension
-    JoinSide js[4];
-    bool jt_built = false;        // the build side is complete and indexed: probe batches have started
-    int star_expand_cap = 0;      // test option "star_expand_capacity": first capacity (tuples) of a star join's expansion pass (0 = twice its input)
-    uint32_t* st_tuples[2] = {nullptr, nullptr}; size_t st_tuples_cap[2] = {0, 0};   // star join: row-id tuples of one chunk (probe / expansion ping-pong)
-    std::vector<uint8_t*> st_vals, st_nullb, st_bits; std::vector<size_t> st_vals_cap, st_nullb_cap, st_bits_cap;   // ... and its gathered columns
-    int join_pipeline = 0;       // opt-in: the fused probe issues its lookups one drain ahead (no gain while the kernel is bound by its shared-memory atomics)
-    int join_learn_range = 1;     // a re-run plan builds with the key range it saw before (checked by the build kernel): -0.05 ms per C3 request
-    int fx_off = 0;               // set when a finished request saw more than 1/64 of its surviving rows take FX's exact path (see agg_finish)
-    int lean_bank = 0;            // opt-in: bank-aware dealing of the lean kernel's drain (agg_direct.cuh, BANK)
-    int lean_fx = [] { const char* e = getenv("BKGPU_LEAN_FX"); return e ? atoi(e) != 0 : BK_LEAN_FX_DEFAULT; }();   // double sums as fixed-point limbs with native shared atomics (agg_direct.cuh, FX); option lean_fx
-    int blocking_sync = -1; bool blocking_wait = false; cudaEvent_t wait_event = nullptr;   // see agg_finish
-    JoinProbe jp{}; uint32_t* jp_attr = nullptr; uint64_t* jp_packed = nullptr; int jp_key_pos = 0;   // ... fused into the lean aggregate
-    size_t jp_attr_cap = 0, jp_packed_cap = 0, j_scratch_cap = 0;
-    uint64_t* j_scratch = nullptr;   // [0..1] key min / max, then u32 flags: [4] duplicate build key, [5] fused probe unusable
-    int no_fused_probe = 0, no_lean_nulls = 0, no_lean_mm = 0;
-    int use_wp = 0;               // 1 = launch the warp-private aggregate kernel where the batch fits it (opt-in: k_agg_group_lean is the default)
-    int wp_kt_log2 = 0;           // log2 words of the warp-private kernel's key table (0 = sized from the cardinality)
-    int wp_warps = 0;             // warps per CTA of the warp-private kernel (0 = chosen from the table size; 8, 12 or 16)
-    std::vector<uint8_t*> jg_buf; int64_t jg_rows = 0;                            // gathered build columns, one chunk
-    std::vector<ColRef> probe_want; std::vector<int> probe_map;   // probe-side columns and their index in c.cols
-    // sort / filter state
-    SortState* sort = nullptr;
-    // host staging for pageable / pinned pushes
-    std::vector<void*> stage[2];
-    std::vector<void*> stage_valid[2];
-    size_t stage_rows = 0;
-    cudaEvent_t stage_free[2] = {nullptr, nullptr}, stage_ready[2] = {nullptr, nullptr};
-    // results
-    std::vector<HostCol> result;
-    int64_t result_rows = 0, result_pos = 0;
-    // stats
-    bkgpu_stats stats{};
-    std::vector<EventPair> timed;
-    std::vector<EventPair> timed_coll;
-    std::vector<std::pair<void*, size_t>> dev_allocs;   // (buffer, size class) — returned to the process-wide cache on free / close
-
-    int fail(int code, const char* fmt, ...) {
-        char buf[512]; va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof buf, fmt, ap); va_end(ap);
-        last_error = buf; g_thread_error = buf; return code;
-    }
-    int cuda_fail(cudaError_t e, const char* what) {
-        return fail(e == cudaErrorMemoryAllocation ? BKGPU_ENOMEM : BKGPU_ENODEV, "%s: %s", what, cudaGetErrorString(e));
-    }
-};
-
-#define CK(plan, call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return (plan)->cuda_fail(e__, #call); } while (0)
 
 static int thread_fail(int code, const char* fmt, ...) {
     char buf[512];
@@ -255,7 +109,7 @@ size_t size_class(size_t b) {   // eight classes per power of two: at most 12.5 
 }  // namespace
 extern "C" void bkgpu_release_cache(void) { dev_cache().release_all(); mapped_cache().release_all(); }
 
-static int dev_alloc(bkgpu_plan* p, void** out, size_t bytes) {
+int dev_alloc(bkgpu_plan* p, void** out, size_t bytes) {
     const size_t sc = size_class(bytes ? bytes : 8);
     void* q = dev_cache().take(p->device, sc);
     if (!q) {
@@ -267,7 +121,7 @@ static int dev_alloc(bkgpu_plan* p, void** out, size_t bytes) {
     p->dev_allocs.push_back({q, sc});
     return BKGPU_OK;
 }
-static void dev_free(bkgpu_plan* p, void* ptr) {
+void dev_free(bkgpu_plan* p, void* ptr) {
     if (!ptr) return;
     size_t sc = 0;
     for (auto it = p->dev_allocs.begin(); it != p->dev_allocs.end(); ++it) if (it->first == ptr) { sc = it->second; p->dev_allocs.erase(it); break; }
@@ -280,7 +134,7 @@ static void dev_free(bkgpu_plan* p, void* ptr) {
 }
 // grow-only device buffer: plans are re-armed with bkgpu_reset and run again; cudaMalloc / cudaFree per run would
 // serialise the device every time
-static int ensure_buf(bkgpu_plan* p, void** ptr, size_t* cap, size_t bytes) {
+int ensure_buf(bkgpu_plan* p, void** ptr, size_t* cap, size_t bytes) {
     if (*ptr && *cap >= bytes) return BKGPU_OK;
     dev_free(p, *ptr); *ptr = nullptr; *cap = 0;
     const int rc = dev_alloc(p, ptr, bytes);
@@ -341,14 +195,13 @@ extern "C" int bkgpu_set_option(bkgpu_plan* p, const char* key, int64_t v) {
     else if (k == "partial_capacity") { if (v < 1) return p->fail(BKGPU_EINVAL, "partial_capacity must be positive"); p->partial_cap = v; }
     else if (k == "force_generic") p->force_generic = v != 0;
     else if (k == "no_stream_copy") p->no_stream_copy = v != 0;
-    else if (k == "join_pipeline") p->join_pipeline = v != 0;
+    else if (k == "join_pipeline") p->join.pipeline = v != 0;
     else if (k == "lean_bank") p->lean_bank = v != 0;
     else if (k == "lean_fx") p->lean_fx = v != 0;
     else if (k == "blocking_sync") p->blocking_sync = (int)v;
-    else if (k == "join_learn_range") p->join_learn_range = v != 0;
-    else if (k == "star_expand_capacity") { if (v < 0 || v > 0x7FFFFFFF) return p->fail(BKGPU_EINVAL, "star_expand_capacity out of range"); p->star_expand_cap = (int)v; }
+    else if (k == "star_expand_capacity") { if (v < 0 || v > 0x7FFFFFFF) return p->fail(BKGPU_EINVAL, "star_expand_capacity out of range"); p->join.star_expand_cap = (int)v; }
     else if (k == "no_lean") p->no_lean = v != 0;
-    else if (k == "no_fused_probe") p->no_fused_probe = v != 0;
+    else if (k == "no_fused_probe") p->join.no_fused_probe = v != 0;
     else if (k == "repartition") p->repartition = v != 0;
     else if (k == "peer_merge") p->peer_merge = v != 0;
     else if (k == "no_lean_nulls") p->no_lean_nulls = v != 0;
@@ -400,9 +253,9 @@ extern "C" int bkgpu_open(bkgpu_plan* p) {
     p->blocking_wait = p->blocking_sync >= 0 ? p->blocking_sync != 0 : (p->nranks > 1 && cpu_budget() < 4 * p->nranks);
     int rc = BKGPU_OK;
     if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) rc = alloc_group_table(p);
-    if (!rc && (p->c.kind == PK_SORT || p->c.kind == PK_FILTER)) rc = sort_open(p->c, p->device, p->stream, p->region_base, &p->sort, p->last_error);
-    if (!rc && p->c.post) rc = sort_open(*p->c.post, p->device, p->stream, 0, &p->post_sort, p->last_error);
-    if (rc) { g_thread_error = p->last_error; return rc; }
+    if (!rc && (p->c.kind == PK_SORT || p->c.kind == PK_FILTER)) rc = sort_check(p, sort_open(p->c, p->device, p->stream, p->region_base, &p->sort, p->last_error));
+    if (!rc && p->c.post) rc = sort_check(p, sort_open(*p->c.post, p->device, p->stream, 0, &p->post_sort, p->last_error));
+    if (rc) return rc;
     p->state = S_OPEN;
     return BKGPU_OK;
 }
@@ -458,16 +311,10 @@ static bool ensure_fused(bkgpu_plan* p) {
     return true;
 }
 
-// `jp`: fused FK -> PK probe (lean kernel only); returns +1 without launching when this batch does not fit the lean kernel
-static int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp = nullptr) {
+int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp) {
     AggArgs a; memset(&a, 0, sizeof a);
     a.plan = c.ap; a.prog = c.prog; a.direct = c.direct; a.gt = p->gt; a.rows_passed = p->d_rows_passed;
-    if (c.kind == PK_JOIN_AGG) {
-        a.join.enabled = 1; a.join.keys = p->js[0].jt_keys; a.join.rows = p->js[0].jt_rows; a.join.cap_mask = p->js[0].jt_mask;
-        a.join.probe_col = c.probe_key_col; a.join.probe_prim = c.cols[(size_t)c.probe_key_col].prim; a.join.cast_prim = c.join_key_prim;
-        a.join.join_type = c.join_type; a.join.matched = c.join_type == BK_INNER_JOIN ? nullptr : p->jb_matched; a.join.n_build = p->js[0].rows;
-        a.join.tail = p->join_tail_launch ? 1 : 0;
-    }
+    if (c.kind == PK_JOIN_AGG) a.join = join_args(p, p->join.tail_launch);
     const bool direct = c.has_direct && vec_ok && !p->force_generic && c.kind == PK_AGG;   // (the join's fast-path plan is lowered as PK_AGG)
     const int ncols = (int)c.cols.size();
     if (direct) { for (size_t i = 0; i < c.direct_cols.size(); i++) a.cols[i] = cols[c.direct_cols[i]]; a.n_cols = (int)c.direct_cols.size(); }
@@ -478,7 +325,7 @@ static int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols
     for (int k = 0; k < a.plan.n_agg; k++) {
         AggSpec& s = a.plan.agg[k];
         if (s.kind == AG_COUNT_STAR) continue;
-        bool nullable = c.arg_can_null[(size_t)k] || p->join_tail_launch;   // (the tail's probe-side columns are NULL on every row)
+        bool nullable = c.arg_can_null[(size_t)k] || p->join.tail_launch;   // (the tail's probe-side columns are NULL on every row)
         for (int i = 0; i < ncols; i++) if ((c.arg_cols_mask[(size_t)k] >> i) & 1) nullable = nullable || cols[i].validity != nullptr;
         s.nullable = nullable ? 1 : 0;
         if (s.cnt_lane && s.cnt_owner) {
@@ -575,7 +422,7 @@ static int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols
 
         }
     }
-    if (jp) { if (!a.lean) return 1; a.jp = *jp; a.jp_pipeline = p->join_pipeline; }
+    if (jp) { if (!a.lean) return 1; a.jp = *jp; a.jp_pipeline = p->join.pipeline; }
     // warp-private tables (agg_wp.cuh): the plainest lean batches whose groups fit one table per warp.  The capacity follows the
     // cardinality learned from earlier batches / runs of this plan; an unknown cardinality starts with the largest table.
     a.scalar_tma = p->scalar_tma; a.lean_bank = p->lean_bank;
@@ -616,10 +463,7 @@ static int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols
     for (int64_t off = 0; off < nrows; off += kMax) {
         AggArgs b = a;
         b.nrows = std::min(kMax, nrows - off);
-        for (int i = 0; i < b.n_cols; i++) {
-            b.cols[i].values = (const uint8_t*)a.cols[i].values + (size_t)off * storage_bytes(a.cols[i].stype);
-            if (a.cols[i].validity) b.cols[i].validity = a.cols[i].validity + off / 8;
-        }
+        for (int i = 0; i < b.n_cols; i++) b.cols[i] = col_at(a.cols[i], off);
         const char* name = "";
         EventPair* ep = timer_begin(p, p->timed, b.nrows * algo_bytes_per_row, false);
         cudaError_t e = launch_agg(b, direct, p->sm_count, p->stream, ep ? ep->a : nullptr, &name);
@@ -632,9 +476,8 @@ static int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols
     return BKGPU_OK;
 }
 
-// resolve the plan's columns against one pushed batch
-static int bind_columns(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* cols, int ncols, int64_t nrows,
-                        std::vector<const bkgpu_column*>& bound) {
+int bind_columns(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* cols, int ncols, int64_t nrows,
+                 std::vector<const bkgpu_column*>& bound) {
     bound.assign(want.size(), nullptr);
     for (size_t i = 0; i < want.size(); i++) {
         for (int k = 0; k < ncols; k++) if (cols[k].tuple_id == want[i].tuple_id && cols[k].slot_id == want[i].slot_id) { bound[i] = &cols[k]; break; }
@@ -681,8 +524,6 @@ static int ensure_bounce(bkgpu_plan* p, const std::vector<ColRef>& want, size_t 
     p->bounce_rows = rows;
     return BKGPU_OK;
 }
-
-typedef int (*BatchFn)(bkgpu_plan*, const DevCol*, int64_t nrows, int64_t row_base, bool vec_ok);
 
 // ---- host-side copy workers: pageable input (what an Arrow RecordBatch of RocksdbVectorizedReader hands over) is copied into
 // pinned bounce buffers by several threads — cudaMemcpyAsync from pageable memory goes through the driver's single staging buffer
@@ -784,7 +625,7 @@ bool is_pageable(const void* p) {
 
 // feed a batch: device-resident columns go straight to the kernels; host columns stream through
 // two sets of device staging buffers (H2D of chunk i+1 overlaps the kernel on chunk i)
-static int feed(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device, BatchFn fn) {
+int feed(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device, BatchFn fn) {
     std::vector<const bkgpu_column*> bound;
     int rc = bind_columns(p, want, cols, ncols, nrows, bound);
     if (rc) return rc;
@@ -856,551 +697,23 @@ static int feed(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_colu
 
 static int agg_batch(bkgpu_plan* p, const DevCol* cols, int64_t nrows, int64_t, bool vec_ok) { return launch_agg_batch(p, p->c, cols, nrows, vec_ok); }
 static int sort_batch(bkgpu_plan* p, const DevCol* cols, int64_t nrows, int64_t, bool) {
-    int rc = sort_push(p->sort, cols, nrows, p->stream, &p->stats, p->last_error);
+    return sort_check(p, sort_push(p->sort, cols, nrows, p->stream, &p->stats, p->last_error));
+}
+
+int sort_check(bkgpu_plan* p, int rc) {
     if (rc) g_thread_error = p->last_error;
     return rc;
 }
 
-// ---- K4: retain the build (outer / driver) table, build the multimap at the first probe batch ----
-static void side_init(bkgpu_plan* p, JoinSide& s) {
-    const size_t nc = p->c.cols.size();
-    if (s.vals.empty()) { s.vals.assign(nc, nullptr); s.nullbytes.assign(nc, nullptr); s.bitmap.assign(nc, nullptr); s.has_null.assign(nc, false); }
-}
-// plan column i as retained by side s
-static DevCol side_col(const Compiled& c, const JoinSide& s, size_t i) {
-    DevCol d{};
-    d.values = s.vals[i]; d.validity = s.bitmap[i]; d.stype = prim_storage(c.cols[i].prim); d.prim = c.cols[i].prim;
-    return d;
-}
-// `side`: the Compiled::col_side value of this table's columns (1 for the two-table join, 1 + d for dimension d of a star join)
-static int join_retain_build(bkgpu_plan* p, JoinSide& s, int side, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device) {
-    const Compiled& c = p->c;
-    if (p->jt_built) return p->fail(BKGPU_ESTATE, "build-side rows arrived after probing started (the reference fetches the whole driver table first, join_node.cpp:920-1022)");
-    const size_t nc = c.cols.size();
-    side_init(p, s);
-    std::vector<ColRef> want; std::vector<int> idx;
-    for (size_t i = 0; i < nc; i++) if (c.col_side[i] == side) { want.push_back(c.cols[i]); idx.push_back((int)i); }
-    std::vector<const bkgpu_column*> bound;
-    int rc = bind_columns(p, want, cols, ncols, nrows, bound);
-    if (rc) return rc;
-    if (s.rows + nrows > 0xFFFFFFF0ll) return p->fail(BKGPU_EUNSUPPORTED, "build side larger than 2^32 rows");
-    if (s.rows + nrows > s.cap) {
-        const int64_t cap = std::max<int64_t>(s.rows + nrows, std::max<int64_t>(s.cap * 2, 1 << 16));
-        for (int i : idx) {
-            const size_t eb = (size_t)storage_bytes(prim_storage(c.cols[(size_t)i].prim));
-            uint8_t *nv = nullptr, *nn = nullptr;
-            if ((rc = dev_alloc(p, (void**)&nv, (size_t)cap * eb))) return rc;
-            if ((rc = dev_alloc(p, (void**)&nn, (size_t)cap))) return rc;
-            if (s.rows) {
-                CK(p, cudaMemcpyAsync(nv, s.vals[(size_t)i], (size_t)s.rows * eb, cudaMemcpyDeviceToDevice, p->stream));
-                CK(p, cudaMemcpyAsync(nn, s.nullbytes[(size_t)i], (size_t)s.rows, cudaMemcpyDeviceToDevice, p->stream));
-                CK(p, cudaStreamSynchronize(p->stream));
-            }
-            dev_free(p, s.vals[(size_t)i]); dev_free(p, s.nullbytes[(size_t)i]);
-            s.vals[(size_t)i] = nv; s.nullbytes[(size_t)i] = nn;
-        }
-        s.cap = cap;
-    }
-    for (size_t w = 0; w < want.size(); w++) {
-        const int i = idx[w];
-        const size_t eb = (size_t)storage_bytes(prim_storage(c.cols[(size_t)i].prim));
-        uint8_t* dv = s.vals[(size_t)i] + (size_t)s.rows * eb;
-        uint8_t* dn = s.nullbytes[(size_t)i] + s.rows;
-        if (on_device) {
-            CK(p, cudaMemcpyAsync(dv, bound[w]->values, (size_t)nrows * eb, cudaMemcpyDeviceToDevice, p->stream));
-            CK(p, launch_unpack_validity(bound[w]->validity, nrows, dn, p->stream));
-            p->stats.kernel_launches++;
-        } else {
-            CK(p, cudaMemcpyAsync(dv, bound[w]->values, (size_t)nrows * eb, cudaMemcpyHostToDevice, p->stream));
-            std::vector<uint8_t> nb((size_t)nrows, 0);
-            if (bound[w]->validity) for (int64_t r = 0; r < nrows; r++) nb[(size_t)r] = ((bound[w]->validity[r >> 3] >> (r & 7)) & 1) ? 0 : 1;
-            CK(p, cudaMemcpyAsync(dn, nb.data(), (size_t)nrows, cudaMemcpyHostToDevice, p->stream));
-            CK(p, cudaStreamSynchronize(p->stream));
-            p->stats.h2d_bytes += (int64_t)((size_t)nrows * (eb + 1));
-        }
-        if (bound[w]->validity) s.has_null[(size_t)i] = true;
-    }
-    s.rows += nrows;
-    return BKGPU_OK;
-}
-
-// Fused probe (JoinProbe in agg.h): usable when the only build-side column the aggregate reads is its 4-byte GROUP BY
-// key and the probe key is a 32-bit integer column whose cast to the comparison type keeps the canonical image.
-static int join_compose_probe(bkgpu_plan* p, uint32_t* flag) {
-    const Compiled& c = p->c;
-    const JoinSide& s = p->js[0];
-    p->jp = JoinProbe{};
-    if (!c.jfast || !c.jfast->has_direct || c.jfast->direct.n_keys != 1) return BKGPU_OK;
-    const Compiled& f = *c.jfast;
-    const size_t kpos = (size_t)f.direct.n_terms;
-    int attr_main = -1;
-    for (size_t i = 0; i < f.direct_cols.size(); i++) {
-        const int m = c.jfast_of_main[(size_t)f.direct_cols[i]];
-        if (c.col_side[(size_t)m] != 1) continue;
-        if (i != kpos) return BKGPU_OK;   // a predicate or an aggregate argument comes from the build side: gather path
-        attr_main = m;
-    }
-    if (attr_main < 0) return BKGPU_OK;
-    const int ast = prim_storage(c.cols[(size_t)attr_main].prim);
-    if ((ast != ST_I32 && ast != ST_U32) || (c.cols[(size_t)attr_main].prim != BK_INT32 && c.cols[(size_t)attr_main].prim != BK_UINT32)) return BKGPU_OK;
-    const int pp = c.cols[(size_t)c.probe_key_col].prim, ct = c.join_key_prim;
-    const bool ident = (pp == BK_INT32 && (ct == BK_INT32 || ct == BK_INT64)) || (pp == BK_UINT32 && (ct == BK_UINT32 || ct == BK_UINT64 || ct == BK_INT64));
-    if (!ident) return BKGPU_OK;
-    int rc;
-    JoinProbe jp{};
-    jp.mode = s.jf.mode; jp.key_signed = pp == BK_INT32 ? 1 : 0;
-    jp.dense_min = s.jf.dense_min; jp.dense_size = s.jf.dense_size; jp.bias = s.jf.bias; jp.packed_mask = s.jf.packed_mask;
-    if (jp.mode == 1) {
-        if ((rc = ensure_buf(p, (void**)&p->jp_attr, &p->jp_attr_cap, (size_t)jp.dense_size * 4))) return rc;
-        jp.attr = p->jp_attr;
-        jp.present = (uint64_t)s.rows == jp.dense_size ? nullptr : s.jf.dense;   // unique, NULL-free keys filling the range: every key exists
-    } else {
-        if ((rc = ensure_buf(p, (void**)&p->jp_packed, &p->jp_packed_cap, ((size_t)jp.packed_mask + 1) * 8))) return rc;
-        jp.packed = p->jp_packed;
-    }
-    CK(p, launch_join_compose(s.jf, (const uint32_t*)s.vals[(size_t)attr_main], p->jp_attr, p->jp_packed, flag, p->stream));
-    p->stats.kernel_launches++;
-    p->jp = jp; p->jp_key_pos = (int)kpos;   // (the caller drops it again when `flag` comes back set)
-    return BKGPU_OK;
-}
-
-// validity bitmaps of the side's retained columns that hold NULLs
-static int join_pack_validity(bkgpu_plan* p, JoinSide& s, int side) {
-    const Compiled& c = p->c;
-    side_init(p, s);
-    int rc;
-    for (size_t i = 0; i < c.cols.size(); i++) {
-        if (c.col_side[i] != side) continue;
-        // (a bitmap kept from an earlier run of the plan must not mask this run's rows: a column without NULLs has none)
-        dev_free(p, s.bitmap[i]); s.bitmap[i] = nullptr;
-        if (!s.has_null[i]) continue;
-        if ((rc = dev_alloc(p, (void**)&s.bitmap[i], (size_t)(s.rows + 7) / 8 + 8))) return rc;
-        CK(p, launch_pack_validity(s.nullbytes[i], s.rows, s.bitmap[i], p->stream));
-        p->stats.kernel_launches++;
-    }
-    return BKGPU_OK;
-}
-
-// The unique-key index of side `s` (FK -> PK fast path): a dense array when the key range is small, else a packed table for keys of at most
-// 32 bits.  s.jf.mode stays 0 when neither fits or a key repeats.  `compose`: the two-table join's fused probe is composed behind the build,
-// so that its flag comes back in the same round trip.
-static int join_build_index(bkgpu_plan* p, JoinSide& s, const DevCol& key, int cast_prim, bool compose) {
-    int rc;
-    s.jf = JoinFast{};
-    if (s.rows <= 0) return BKGPU_OK;
-    bool retry_measured = false;
-again:
-    const int cls = host_prim_class(cast_prim);
-    const uint64_t bias = cls == VC_I64 ? 0x8000000000000000ull : 0ull;
-    if ((rc = ensure_buf(p, (void**)&p->j_scratch, &p->j_scratch_cap, 64))) return rc;
-    uint64_t* mm = p->j_scratch; uint32_t* dup = (uint32_t*)(p->j_scratch + 2);
-    // the key range: measured (one pass over the keys + a round trip), or — when this plan has built before — the range it saw then,
-    // checked by the build kernel itself (a key outside it raises a flag and the build is redone with a measured range)
-    uint64_t h_mm[2];
-    bool guessed = s.learned && !retry_measured && p->join_learn_range;
-    if (guessed) { h_mm[0] = s.learn_min; h_mm[1] = s.learn_max; }
-    else {
-        CK(p, launch_join_minmax(key, key.prim, cast_prim, s.rows, bias, mm, p->stream));
-        CK(p, cudaMemcpyAsync(h_mm, mm, 16, cudaMemcpyDeviceToHost, p->stream));
-        CK(p, cudaStreamSynchronize(p->stream));
-        p->stats.kernel_launches++;
-    }
-    JoinFast jf{}; jf.bias = bias;
-    const uint64_t range = h_mm[1] >= h_mm[0] ? h_mm[1] - h_mm[0] + 1 : 0;
-    const int kb = storage_bytes(prim_storage(cast_prim));
-    if (range > 0 && range <= (uint64_t)4 * (uint64_t)s.rows + 1024 && range <= (1ull << 30)) {
-        jf.mode = 1; jf.dense_min = h_mm[0]; jf.dense_size = range;
-        if ((rc = ensure_buf(p, (void**)&s.jf_dense, &s.jf_dense_cap, (size_t)range * 4))) return rc;
-        jf.dense = s.jf_dense;
-    } else if (kb <= 4) {
-        uint32_t pc = 1024; while ((int64_t)pc < 2 * s.rows) pc <<= 1;
-        jf.mode = 2; jf.packed_mask = pc - 1;
-        if ((rc = ensure_buf(p, (void**)&s.jf_packed, &s.jf_packed_cap, (size_t)pc * 8))) return rc;
-        jf.packed = s.jf_packed;
-    }
-    if (jf.mode) {
-        CK(p, launch_join_build_fast(key, key.prim, cast_prim, s.rows, jf, s.jf_dense, s.jf_packed, dup, p->stream));
-        p->stats.kernel_launches += 1;
-        s.jf = jf;
-        if (compose && (rc = join_compose_probe(p, dup + 1))) return rc;   // enqueued behind the build: all flags come back in one round trip
-        uint32_t h_flags[3] = {0, 0, 0};
-        CK(p, cudaMemcpyAsync(h_flags, dup, 12, cudaMemcpyDeviceToHost, p->stream));
-        CK(p, cudaStreamSynchronize(p->stream));
-        if (h_flags[2] && guessed) { retry_measured = true; goto again; }   // this run's keys left the learned range
-        if (h_flags[0]) { s.jf = JoinFast{}; p->jp = JoinProbe{}; }   // duplicate build keys: not a PK, the general probe runs
-        else if (h_flags[1]) p->jp = JoinProbe{};
-        s.learned = true; s.learn_min = h_mm[0]; s.learn_max = h_mm[1];
-    } else if (guessed) { retry_measured = true; goto again; }   // (the learned range no longer fits this row count)
-    return BKGPU_OK;
-}
-
-static int join_build_table(bkgpu_plan* p) {
-    const Compiled& c = p->c;
-    JoinSide& s = p->js[0];
-    const size_t nc = c.cols.size();
-    int rc;
-    if ((rc = join_pack_validity(p, s, 1))) return rc;
-    p->jt_built = true; s.jt_generic = false;   // the multimap of the general probe is built on first use (join_generic_table)
-    // ---- FK -> PK fast path: are the build keys unique, and is their range dense or their type <= 32 bits? ----
-    s.jf = JoinFast{}; p->jp = JoinProbe{};
-    if (p->jg_buf.empty()) p->jg_buf.assign(nc, nullptr);
-    bool build_nulls = false;
-    for (size_t i = 0; i < nc; i++) if (c.col_side[i] == 1 && s.has_null[i]) build_nulls = true;   // gathered columns must be NULL-free
-    if (!c.jfast || build_nulls) return BKGPU_OK;
-    return join_build_index(p, s, side_col(c, s, (size_t)c.build_key_col), c.join_key_prim, true);
-}
-
-// the multimap of side `s` (duplicate build keys, the general probe): open addressing from the cast key image to the build row
-static int join_build_multimap(bkgpu_plan* p, JoinSide& s, const DevCol& key, int cast_prim) {
-    int rc;
-    uint32_t cap = 1024;
-    while ((int64_t)cap < 2 * s.rows) cap <<= 1;
-    dev_free(p, s.jt_keys); dev_free(p, s.jt_rows); s.jt_keys = nullptr; s.jt_rows = nullptr;
-    if ((rc = dev_alloc(p, (void**)&s.jt_keys, (size_t)cap * 8))) return rc;
-    if ((rc = dev_alloc(p, (void**)&s.jt_rows, (size_t)cap * 4))) return rc;
-    s.jt_mask = cap - 1;
-    CK(p, launch_join_build(key, key.prim, cast_prim, s.rows, s.jt_keys, s.jt_rows, s.jt_mask, p->stream));
-    p->stats.kernel_launches++;
-    s.jt_generic = true;
-    return BKGPU_OK;
-}
-
-// the general probe's multimap (duplicate build keys, unmatched probe rows): built only when a batch needs it
-static int join_generic_table(bkgpu_plan* p) {
-    const Compiled& c = p->c;
-    JoinSide& s = p->js[0];
-    if (s.jt_generic) return BKGPU_OK;
-    int rc;
-    if ((rc = join_build_multimap(p, s, side_col(c, s, (size_t)c.build_key_col), c.join_key_prim))) return rc;
-    if (c.join_type != BK_INNER_JOIN) {   // one "found a partner" byte per build row
-        if ((rc = ensure_buf(p, (void**)&p->jb_matched, &p->jb_matched_cap, (size_t)std::max<int64_t>(s.rows, 1)))) return rc;
-        CK(p, cudaMemsetAsync(p->jb_matched, 0, (size_t)std::max<int64_t>(s.rows, 1), p->stream));
-    }
-    return BKGPU_OK;
-}
-
-static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nrows, int64_t, bool) {
-    const Compiled& c = p->c;
-    std::vector<DevCol> all(c.cols.size());
-    for (size_t i = 0; i < c.cols.size(); i++) {
-        if (c.col_side[i] == 1) { all[i].values = p->js[0].vals[i]; all[i].validity = p->js[0].bitmap[i]; all[i].stype = prim_storage(c.cols[i].prim); all[i].prim = c.cols[i].prim; }
-    }
-    for (size_t w = 0; w < p->probe_map.size(); w++) all[(size_t)p->probe_map[w]] = probe_cols[w];
-    // ---- FK -> PK fast path: gather the build columns next to the probe rows, then the ordinary (lean) aggregate ----
-    if (p->js[0].jf.mode != 0 && p->jp.mode != 0 && c.jfast && !p->force_generic && !p->no_fused_probe) {
-        // ---- fused probe: the lean aggregate reads the foreign key and looks the group key up itself ----
-        const Compiled& f = *c.jfast;
-        std::vector<DevCol> fc(f.cols.size());
-        const int key_fcol = f.direct_cols[(size_t)p->jp_key_pos];
-        bool vec_ok = true;
-        for (size_t i = 0; i < f.cols.size(); i++) {
-            fc[i] = (int)i == key_fcol ? all[(size_t)c.probe_key_col] : all[(size_t)c.jfast_of_main[i]];
-            if (((uintptr_t)fc[i].values & 31) != 0) vec_ok = false;
-        }
-        const int rc = launch_agg_batch(p, f, fc.data(), nrows, vec_ok, &p->jp);
-        if (rc <= 0) return rc;   // launched (0) or failed (< 0); +1: this batch does not fit the lean kernel
-    }
-    if (p->js[0].jf.mode != 0 && c.jfast && !p->force_generic) {
-        const Compiled& f = *c.jfast;
-        const int64_t chunk = 16 << 20;   // the gathered chunk is re-read immediately: keep it L2-sized
-        for (int64_t off = 0; off < nrows; off += chunk) {
-            const int64_t n = std::min(chunk, nrows - off);
-            GatherCols gc{}; std::vector<DevCol> fc(f.cols.size());
-            int rc;
-            for (size_t i = 0; i < f.cols.size(); i++) {
-                const size_t m = (size_t)c.jfast_of_main[i];
-                const size_t eb = (size_t)storage_bytes(prim_storage(c.cols[m].prim));
-                if (c.col_side[m] == 1) {
-                    if (!p->jg_buf[m] || p->jg_rows < n) {
-                        dev_free(p, p->jg_buf[m]); p->jg_buf[m] = nullptr;
-                        if ((rc = dev_alloc(p, (void**)&p->jg_buf[m], (size_t)chunk * eb))) return rc;
-                    }
-                    gc.src[gc.n] = p->js[0].vals[m]; gc.dst[gc.n] = p->jg_buf[m]; gc.elem[gc.n] = (int32_t)eb; gc.n++;
-                    fc[i].values = p->jg_buf[m]; fc[i].validity = nullptr; fc[i].stype = prim_storage(c.cols[m].prim); fc[i].prim = c.cols[m].prim;
-                } else {
-                    fc[i] = all[m];
-                    fc[i].values = (const uint8_t*)all[m].values + (size_t)off * eb;
-                    if (all[m].validity) fc[i].validity = all[m].validity + off / 8;
-                }
-            }
-            p->jg_rows = chunk;
-            DevCol pk = all[(size_t)c.probe_key_col];
-            pk.values = (const uint8_t*)pk.values + (size_t)off * (size_t)storage_bytes(pk.stype);
-            if (pk.validity) pk.validity += off / 8;
-            CK(p, cudaMemsetAsync(p->d_cursor + 1, 0, 4, p->stream));
-            CK(p, launch_join_gather(pk, c.cols[(size_t)c.probe_key_col].prim, c.join_key_prim, n, p->js[0].jf, gc, p->d_cursor + 1, p->stream));
-            p->stats.kernel_launches++;
-            uint32_t miss = 0;
-            CK(p, cudaMemcpyAsync(&miss, p->d_cursor + 1, 4, cudaMemcpyDeviceToHost, p->stream));
-            CK(p, cudaStreamSynchronize(p->stream));
-            if (miss) {   // some probe row has no partner (or a NULL key): this chunk takes the general probe
-                std::vector<DevCol> sl(all);
-                for (size_t i = 0; i < sl.size(); i++) if (c.col_side[i] == 0) {
-                    sl[i].values = (const uint8_t*)all[i].values + (size_t)off * (size_t)storage_bytes(all[i].stype);
-                    if (all[i].validity) sl[i].validity = all[i].validity + off / 8;
-                }
-                if ((rc = join_generic_table(p))) return rc;
-                if ((rc = launch_agg_batch(p, c, sl.data(), n, false))) return rc;
-            } else {
-                bool vec_ok = true;
-                for (auto& d : fc) if (((uintptr_t)d.values & 31) != 0) vec_ok = false;
-                if ((rc = launch_agg_batch(p, f, fc.data(), n, vec_ok))) return rc;
-            }
-        }
-        return BKGPU_OK;
-    }
-    { int rc = join_generic_table(p); if (rc) return rc; }
-    return launch_agg_batch(p, c, all.data(), nrows, false);
-}
-
-// LEFT / SEMI / ANTI_SEMI: once every probe batch has run, the preserved (build) side's rows the join type asks for go through the
-// aggregate — unmatched rows NULL-extended (LEFT), matched rows (SEMI), unmatched rows (ANTI_SEMI); join_node.cpp:1200-1276
-static int join_tail(bkgpu_plan* p) {
-    const Compiled& c = p->c;
-    if (p->js[0].rows == 0) return BKGPU_OK;
-    int rc;
-    if (!p->jt_built && (rc = join_build_table(p))) return rc;
-    if ((rc = join_generic_table(p))) return rc;
-    std::vector<DevCol> all(c.cols.size());
-    for (size_t i = 0; i < c.cols.size(); i++) {
-        all[i].stype = prim_storage(c.cols[i].prim); all[i].prim = c.cols[i].prim;
-        if (c.col_side[i] == 1) { all[i].values = p->js[0].vals[i]; all[i].validity = p->js[0].bitmap[i]; }   // (probe-side columns are never read: row = -1 is NULL)
-    }
-    p->join_tail_launch = true;
-    rc = launch_agg_batch(p, c, all.data(), p->js[0].rows, false);
-    p->join_tail_launch = false;
-    return rc;
-}
-
-// ---- a JOIN that returns rows (PK_JOIN): pairs -> gather -> the sink fragment (p->post_sort) ----
-static int join_rows_emit(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t n_probe, bool tail) {
-    const Compiled& c = p->c;
-    int rc;
-    AggArgs a; memset(&a, 0, sizeof a);
-    a.plan = c.ap; a.prog = c.prog; a.nrows = n_probe;
-    const int ncols = (int)c.cols.size();
-    for (int i = 0; i < ncols; i++) a.cols[i] = all[(size_t)i];
-    a.n_cols = ncols;
-    a.join.enabled = 1; a.join.keys = p->js[0].jt_keys; a.join.rows = p->js[0].jt_rows; a.join.cap_mask = p->js[0].jt_mask;
-    a.join.probe_col = c.probe_key_col; a.join.probe_prim = c.cols[(size_t)c.probe_key_col].prim; a.join.cast_prim = c.join_key_prim;
-    a.join.join_type = c.join_type; a.join.matched = c.join_type == BK_INNER_JOIN ? nullptr : p->jb_matched; a.join.n_build = p->js[0].rows;
-    a.join.tail = tail ? 1 : 0;
-    if ((rc = ensure_buf(p, (void**)&p->jr_cursor, &p->jr_cursor_cap, 64))) return rc;
-    size_t want = (size_t)std::max<int64_t>(tail ? p->js[0].rows : n_probe, 1 << 12);
-    uint32_t found = 0;
-    for (int attempt = 0; attempt < 2; attempt++) {   // a batch with more pairs than the buffer holds is counted, the buffer grown, the batch rerun
-        if (want > 0x7FFFFFF0ull) return p->fail(BKGPU_ETOOBIG, "a probe batch joins to more than 2^31 rows: push smaller batches");
-        if ((rc = ensure_buf(p, (void**)&p->jr_pairs, &p->jr_pairs_cap, want * 8))) return rc;
-        CK(p, cudaMemsetAsync(p->jr_cursor, 0, 4, p->stream));
-        // (a rerun of a LEFT batch sets the same matched[] flags again: they only ever go from 0 to 1)
-        CK(p, launch_join_pairs(a, p->jr_pairs, (uint32_t)want, p->jr_cursor, p->sm_count, p->stream));
-        CK(p, cudaMemcpyAsync(&found, p->jr_cursor, 4, cudaMemcpyDeviceToHost, p->stream));
-        CK(p, cudaStreamSynchronize(p->stream));
-        p->stats.kernel_launches++;
-        if ((size_t)found <= want) break;
-        want = found;
-    }
-    if (!found) return BKGPU_OK;
-    const Compiled& pc = *c.post;
-    const size_t nc = pc.cols.size();
-    if (p->post_cap < found || p->post_vals.size() != nc) {
-        for (auto& v : {&p->post_vals, &p->post_nullb, &p->post_bitmap}) { for (uint8_t* q : *v) dev_free(p, q); v->assign(nc, nullptr); }
-        const size_t cap = std::max<size_t>((size_t)found + found / 4, 1 << 16);
-        for (size_t k = 0; k < nc; k++) {
-            if ((rc = dev_alloc(p, (void**)&p->post_vals[k], cap * (size_t)storage_bytes(prim_storage(pc.cols[k].prim)) + 64))) return rc;
-            if ((rc = dev_alloc(p, (void**)&p->post_nullb[k], cap + 64))) return rc;
-            if ((rc = dev_alloc(p, (void**)&p->post_bitmap[k], cap / 8 + 64))) return rc;
-        }
-        p->post_cap = cap;
-    }
-    std::vector<DevCol> dc(std::max<size_t>(nc, 1));
-    for (size_t k = 0; k < nc; k++) {   // sink column k = output column k = device column k of the join (plan.cpp::lower_join_rows)
-        const int st = prim_storage(pc.cols[k].prim);
-        CK(p, launch_join_rows_gather(all[k], p->jr_pairs, 2, c.col_side[k] == 1 ? 1 : 0, found, storage_bytes(st), p->post_vals[k], p->post_nullb[k], p->stream));
-        CK(p, launch_pack_validity(p->post_nullb[k], found, p->post_bitmap[k], p->stream));
-        dc[k].values = p->post_vals[k]; dc[k].validity = p->post_bitmap[k]; dc[k].stype = st; dc[k].prim = pc.cols[k].prim;
-    }
-    p->stats.kernel_launches += 2 * (int64_t)nc;
-    p->rows_passed_host += found;
-    if ((rc = sort_push(p->post_sort, dc.data(), (int64_t)found, p->stream, &p->stats, p->last_error))) { g_thread_error = p->last_error; return rc; }
-    CK(p, cudaStreamSynchronize(p->stream));   // the gather buffers are reused by the next batch
-    return BKGPU_OK;
-}
-static void join_all_cols(bkgpu_plan* p, const DevCol* probe_cols, std::vector<DevCol>& all) {
-    const Compiled& c = p->c;
-    all.assign(c.cols.size(), DevCol{});
-    for (size_t i = 0; i < c.cols.size(); i++) {
-        all[i].stype = prim_storage(c.cols[i].prim); all[i].prim = c.cols[i].prim;
-        if (c.col_side[i] == 1) { all[i].values = p->js[0].vals[i]; all[i].validity = p->js[0].bitmap[i]; }
-    }
-    if (probe_cols) for (size_t w = 0; w < p->probe_map.size(); w++) all[(size_t)p->probe_map[w]] = probe_cols[w];
-}
-static int join_rows_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nrows, int64_t, bool) {
-    int rc;
-    if ((rc = join_generic_table(p))) return rc;
-    std::vector<DevCol> all;
-    join_all_cols(p, probe_cols, all);
-    return join_rows_emit(p, all, nrows, false);
-}
-static int join_rows_finish(bkgpu_plan* p) {
-    const Compiled& c = p->c;
-    int rc;
-    if (c.join_type != BK_INNER_JOIN && p->js[0].rows > 0) {   // LEFT: the preserved rows that found no partner, NULL-extended
-        if (!p->jt_built && (rc = join_build_table(p))) return rc;
-        if ((rc = join_generic_table(p))) return rc;
-        std::vector<DevCol> all;
-        join_all_cols(p, nullptr, all);
-        if ((rc = join_rows_emit(p, all, 0, true))) return rc;
-    }
-    std::vector<SortOutCol> cols; int64_t rows = 0;
-    if ((rc = sort_finish(p->post_sort, nullptr, 1, p->stream, &p->stats, cols, &rows, p->last_error))) { g_thread_error = p->last_error; return rc; }
+void set_result(bkgpu_plan* p, std::vector<SortOutCol>& cols, int64_t rows, const OutCol* desc) {
     p->result.clear();
     for (size_t k = 0; k < cols.size(); k++) {
         SortOutCol& sc = cols[k];
-        HostCol hc; hc.desc = c.out_cols[k]; hc.elem = sc.elem;
+        HostCol hc; hc.desc = desc ? desc[k] : OutCol{sc.tuple_id, sc.slot_id, sc.prim, 0}; hc.elem = sc.elem;
         hc.values = std::move(sc.values); hc.validity = std::move(sc.validity);
         p->result.push_back(std::move(hc));
     }
     p->result_rows = rows; p->result_pos = 0;
-    p->stats.rows_filtered = 0;
-    return BKGPU_OK;
-}
-
-static int join_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device) {
-    const Compiled& c = p->c;
-    bool is_build = false;
-    for (int k = 0; k < ncols; k++) if (cols[k].tuple_id == c.build_tuple) is_build = true;
-    if (is_build) return join_retain_build(p, p->js[0], 1, cols, ncols, nrows, on_device);
-    if (!p->jt_built) { int rc = join_build_table(p); if (rc) return rc; }
-    if (p->probe_want.empty()) for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] == 0) { p->probe_want.push_back(c.cols[i]); p->probe_map.push_back((int)i); }
-    return feed(p, p->probe_want, cols, ncols, nrows, on_device, c.kind == PK_JOIN ? join_rows_batch : join_probe_batch);
-}
-
-// ---- star join (PK_STAR_AGG): every dimension is retained and indexed before the first fact batch ----
-static int star_build(bkgpu_plan* p) {
-    const Compiled& c = p->c;
-    p->jt_built = true;
-    int rc;
-    for (size_t d = 0; d < c.dims.size(); d++) {
-        JoinSide& s = p->js[d];
-        const StarDim& sd = c.dims[d];
-        if ((rc = join_pack_validity(p, s, 1 + (int)d))) return rc;
-        s.jt_generic = false; s.jf = JoinFast{};
-        if (s.rows == 0) continue;
-        DevCol key = side_col(c, s, (size_t)sd.key_col);
-        if (sd.n_filter > 0) {   // the build key's validity: the key is not NULL and the dimension's own conjuncts are TRUE
-            if ((rc = ensure_buf(p, (void**)&s.keybits, &s.keybits_cap, ((size_t)s.rows + 31) / 32 * 4))) return rc;
-            StarFilter f; memset(&f, 0, sizeof f);
-            for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] == 1 + (int)d) f.cols[i] = side_col(c, s, i);
-            f.prog = sd.filter; f.key_col = sd.key_col; f.nrows = s.rows;
-            CK(p, launch_star_dim_filter(f, (uint32_t*)s.keybits, p->stream));
-            p->stats.kernel_launches++;
-            key.validity = s.keybits;
-        }
-        // unique keys: the dense or packed index; duplicate keys (or 64-bit keys over a wide range): the multimap
-        if ((rc = join_build_index(p, s, key, sd.cast_prim, false))) return rc;
-        if (s.jf.mode == 0 && (rc = join_build_multimap(p, s, key, sd.cast_prim))) return rc;
-    }
-    return BKGPU_OK;
-}
-
-// the tuple buffer `k` with room for `n` tuples of `w` row ids
-static int star_tuples(bkgpu_plan* p, int k, uint64_t n, int w) {
-    if (n * (uint64_t)w > 0xFFFFFFF0ull) return p->fail(BKGPU_ETOOBIG, "a star join chunk joins to more than 2^32 row ids: push smaller batches");
-    return ensure_buf(p, (void**)&p->st_tuples[k], &p->st_tuples_cap[k], (size_t)std::max<uint64_t>(n, 1) * (size_t)w * 4);
-}
-
-// A fact batch, chunk by chunk: k_star_probe keeps the rows with a partner in every dimension of unique keys, each dimension with duplicate
-// keys expands the survivors (k_star_expand), the referenced columns are gathered side by side, and the aggregate runs over them as the
-// virtual joined tuple (Compiled::jfast: the lean kernel when the shape fits).
-static int star_probe_batch(bkgpu_plan* p, const DevCol* fact_cols, int64_t nrows, int64_t, bool vec_ok) {
-    const Compiled& c = p->c;
-    const Compiled& f = *c.jfast;
-    const int D = (int)c.dims.size(), W = 1 + D;
-    for (int d = 0; d < D; d++) if (p->js[d].rows == 0) return BKGPU_OK;   // an empty dimension: no row joins
-    std::vector<DevCol> all(c.cols.size());
-    for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] > 0) all[i] = side_col(c, p->js[c.col_side[i] - 1], i);
-    for (size_t w = 0; w < p->probe_map.size(); w++) all[(size_t)p->probe_map[w]] = fact_cols[w];
-    if (p->st_vals.empty()) for (auto* v : {&p->st_vals, &p->st_nullb, &p->st_bits}) v->assign(c.cols.size(), nullptr);
-    if (p->st_vals_cap.empty()) for (auto* v : {&p->st_vals_cap, &p->st_nullb_cap, &p->st_bits_cap}) v->assign(c.cols.size(), 0);
-    int rc;
-    const int64_t chunk = 16 << 20;
-    for (int64_t off = 0; off < nrows; off += chunk) {
-        const int64_t n = std::min(chunk, nrows - off);
-        auto fact_col = [&](size_t i) {   // (the chunk of a fact column)
-            DevCol x = all[i];
-            x.values = (const uint8_t*)x.values + (size_t)off * (size_t)storage_bytes(x.stype);
-            if (x.validity) x.validity += off / 8;
-            return x;
-        };
-        StarProbe sp; memset(&sp, 0, sizeof sp);
-        sp.width = W; sp.nrows = n; sp.vec = vec_ok ? 1 : 0;
-        for (int d = 0; d < D; d++) {
-            if (p->js[d].jf.mode == 0) continue;
-            const StarDim& sd = c.dims[(size_t)d];
-            StarLookup& L = sp.d[sp.n++];
-            L.fk = fact_col((size_t)sd.fk_col); L.from_prim = c.cols[(size_t)sd.fk_col].prim; L.cast_prim = sd.cast_prim; L.slot = 1 + d; L.jf = p->js[d].jf;
-        }
-        if ((rc = star_tuples(p, 0, (uint64_t)n, W))) return rc;
-        CK(p, launch_star_probe(sp, p->st_tuples[0], p->d_cursor + 1, p->sm_count, p->stream));
-        p->stats.kernel_launches++;
-        uint32_t found = 0;
-        CK(p, cudaMemcpyAsync(&found, p->d_cursor + 1, 4, cudaMemcpyDeviceToHost, p->stream));
-        CK(p, cudaStreamSynchronize(p->stream));
-        int cur = 0;
-        for (int d = 0; d < D && found; d++) {   // dimensions with duplicate keys: one expansion pass each
-            const JoinSide& s = p->js[d];
-            if (s.jf.mode != 0) continue;
-            const StarDim& sd = c.dims[(size_t)d];
-            uint64_t cap = p->star_expand_cap > 0 ? (uint64_t)p->star_expand_cap : std::max<uint64_t>(2 * (uint64_t)found, 4096);
-            uint32_t got = 0;
-            for (int attempt = 0; attempt < 2; attempt++) {   // more tuples than the buffer holds: counted, the buffer grown to the count, the pass rerun
-                if ((rc = star_tuples(p, 1 - cur, cap, W))) return rc;
-                CK(p, launch_star_expand(fact_col((size_t)sd.fk_col), c.cols[(size_t)sd.fk_col].prim, sd.cast_prim, s.jt_keys, s.jt_rows, s.jt_mask, p->st_tuples[cur], found,
-                                         W, 1 + d, p->st_tuples[1 - cur], (uint32_t)cap, p->d_cursor + 1, p->stream));
-                p->stats.kernel_launches++;
-                CK(p, cudaMemcpyAsync(&got, p->d_cursor + 1, 4, cudaMemcpyDeviceToHost, p->stream));
-                CK(p, cudaStreamSynchronize(p->stream));
-                if (got <= cap) break;
-                cap = got;
-            }
-            found = got; cur = 1 - cur;
-        }
-        if (!found) continue;
-        // the joined chunk: every column the aggregate reads, gathered from its tuple's row
-        std::vector<DevCol> fc(f.cols.size());
-        for (size_t i = 0; i < f.cols.size(); i++) {
-            const size_t m = (size_t)c.jfast_of_main[i];
-            const int side = c.col_side[m];
-            const DevCol src = side == 0 ? fact_col(m) : all[m];
-            const int eb = storage_bytes(src.stype);
-            if ((rc = ensure_buf(p, (void**)&p->st_vals[m], &p->st_vals_cap[m], (size_t)found * (size_t)eb))) return rc;
-            fc[i] = src; fc[i].values = p->st_vals[m]; fc[i].validity = nullptr;
-            if (src.validity) {   // NULLs travel along: null bytes, then a bitmap
-                if ((rc = ensure_buf(p, (void**)&p->st_nullb[m], &p->st_nullb_cap[m], (size_t)found))) return rc;
-                if ((rc = ensure_buf(p, (void**)&p->st_bits[m], &p->st_bits_cap[m], (size_t)found / 8 + 8))) return rc;
-            }
-            CK(p, launch_join_rows_gather(src, p->st_tuples[cur], W, side, found, eb, p->st_vals[m], src.validity ? p->st_nullb[m] : nullptr, p->stream));
-            p->stats.kernel_launches++;
-            if (src.validity) {
-                CK(p, launch_pack_validity(p->st_nullb[m], found, p->st_bits[m], p->stream));
-                p->stats.kernel_launches++;
-                fc[i].validity = p->st_bits[m];
-            }
-        }
-        if ((rc = launch_agg_batch(p, f, fc.data(), found, true))) return rc;
-    }
-    return BKGPU_OK;
-}
-
-static int star_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device) {
-    const Compiled& c = p->c;
-    for (size_t d = 0; d < c.dims.size(); d++)
-        for (int k = 0; k < ncols; k++)
-            if (cols[k].tuple_id == c.dims[d].tuple_id) return join_retain_build(p, p->js[d], 1 + (int)d, cols, ncols, nrows, on_device);
-    if (!p->jt_built) { int rc = star_build(p); if (rc) return rc; }
-    if (p->probe_want.empty()) for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] == 0) { p->probe_want.push_back(c.cols[i]); p->probe_map.push_back((int)i); }
-    return feed(p, p->probe_want, cols, ncols, nrows, on_device, star_probe_batch);
 }
 
 static int bkgpu_push_impl(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device);
@@ -1428,8 +741,7 @@ static int bkgpu_push_impl(bkgpu_plan* p, const bkgpu_column* cols, int ncols, i
                 CK(p, cudaMemcpyAsync(p->h_pinned, p->gt.n_groups, 4, cudaMemcpyDeviceToHost, p->stream));
             return BKGPU_OK;
         }
-        case PK_JOIN_AGG: case PK_JOIN: return join_push(p, cols, ncols, nrows, on_device);
-        case PK_STAR_AGG: return star_push(p, cols, ncols, nrows, on_device);
+        case PK_JOIN_AGG: case PK_JOIN: case PK_STAR_AGG: return join_push(p, cols, ncols, nrows, on_device);
         case PK_SORT: case PK_FILTER: return feed(p, p->c.cols, cols, ncols, nrows, on_device, sort_batch);
         default: return p->fail(BKGPU_EUNSUPPORTED, "plan kind %d has no push path yet", p->c.kind);
     }
@@ -1548,22 +860,28 @@ static int agg_collective(bkgpu_plan* p, bool* rows_mode) {
     return BKGPU_OK;
 }
 
+int ensure_post(bkgpu_plan* p, size_t need, size_t cap) {
+    const Compiled& pc = *p->c.post;
+    const size_t nc = pc.cols.size();
+    if (p->post_cap >= need && p->post_vals.size() == nc) return BKGPU_OK;
+    for (auto& v : {&p->post_vals, &p->post_nullb, &p->post_bitmap}) { for (uint8_t* q : *v) dev_free(p, q); v->assign(nc, nullptr); }
+    int rc;
+    for (size_t k = 0; k < nc; k++) {
+        if ((rc = dev_alloc(p, (void**)&p->post_vals[k], cap * (size_t)storage_bytes(prim_storage(pc.cols[k].prim)) + 64))) return rc;
+        if ((rc = dev_alloc(p, (void**)&p->post_nullb[k], cap + 64))) return rc;
+        if ((rc = dev_alloc(p, (void**)&p->post_bitmap[k], cap / 8 + 64))) return rc;
+    }
+    p->post_cap = cap;
+    return BKGPU_OK;
+}
+
 // [LIMIT ->] [SORT ->] [HAVING ->] above the aggregate: the extracted rows (still on the device) become typed columns and run through
 // the post fragment's sort / filter kernels; only the final rows travel to the host
 static int agg_post(bkgpu_plan* p, uint32_t n_out, uint32_t out_cap) {
     const Compiled& pc = *p->c.post;
     const size_t nc = pc.cols.size();
     int rc;
-    if (p->post_cap < std::max<size_t>(n_out, 1) || p->post_vals.size() != nc) {
-        for (auto& v : {&p->post_vals, &p->post_nullb, &p->post_bitmap}) { for (uint8_t* q : *v) dev_free(p, q); v->assign(nc, nullptr); }
-        const size_t cap = std::max<size_t>(n_out, 2048);
-        for (size_t c = 0; c < nc; c++) {
-            if ((rc = dev_alloc(p, (void**)&p->post_vals[c], cap * (size_t)storage_bytes(prim_storage(pc.cols[c].prim)) + 64))) return rc;
-            if ((rc = dev_alloc(p, (void**)&p->post_nullb[c], cap + 64))) return rc;
-            if ((rc = dev_alloc(p, (void**)&p->post_bitmap[c], cap / 8 + 64))) return rc;
-        }
-        p->post_cap = cap;
-    }
+    if ((rc = ensure_post(p, std::max<size_t>(n_out, 1), std::max<size_t>(n_out, 2048)))) return rc;
     PostCols pcs; memset(&pcs, 0, sizeof pcs);
     pcs.n = (int)nc;
     int img = 0;
@@ -1578,20 +896,13 @@ static int agg_post(bkgpu_plan* p, uint32_t n_out, uint32_t out_cap) {
         dc[c].values = p->post_vals[c]; dc[c].validity = p->post_bitmap[c]; dc[c].stype = prim_storage(pc.cols[c].prim); dc[c].prim = pc.cols[c].prim;
     }
     p->stats.kernel_launches += 1 + (int64_t)nc;
-    if ((rc = sort_reset(p->post_sort, p->stream, p->last_error))) { g_thread_error = p->last_error; return rc; }
+    if ((rc = sort_check(p, sort_reset(p->post_sort, p->stream, p->last_error)))) return rc;
     bkgpu_stats scratch{};   // (the post fragment's kernels are not the request's "main kernel")
-    if (n_out && (rc = sort_push(p->post_sort, dc.data(), n_out, p->stream, &scratch, p->last_error))) { g_thread_error = p->last_error; return rc; }
+    if (n_out && (rc = sort_check(p, sort_push(p->post_sort, dc.data(), n_out, p->stream, &scratch, p->last_error)))) return rc;
     std::vector<SortOutCol> cols; int64_t rows = 0;
-    if ((rc = sort_finish(p->post_sort, nullptr, 1, p->stream, &scratch, cols, &rows, p->last_error))) { g_thread_error = p->last_error; return rc; }
+    if ((rc = sort_check(p, sort_finish(p->post_sort, nullptr, 1, p->stream, &scratch, cols, &rows, p->last_error)))) return rc;
     p->stats.kernel_launches += scratch.kernel_launches;
-    p->result.clear();
-    for (size_t c = 0; c < cols.size(); c++) {
-        SortOutCol& sc = cols[c];
-        HostCol hc; hc.desc = p->c.out_cols[c]; hc.elem = sc.elem;
-        hc.values = std::move(sc.values); hc.validity = std::move(sc.validity);
-        p->result.push_back(std::move(hc));
-    }
-    p->result_rows = rows; p->result_pos = 0;
+    set_result(p, cols, rows, p->c.out_cols.data());
     return BKGPU_OK;
 }
 
@@ -1782,24 +1093,22 @@ static int bkgpu_finish_impl(bkgpu_plan* p) {
     int rc = BKGPU_OK;
     switch (p->c.kind) {
         case PK_AGG: case PK_JOIN_AGG: case PK_STAR_AGG: {
-            if (p->c.kind == PK_JOIN_AGG && p->c.join_type != BK_INNER_JOIN && (rc = join_tail(p))) break;
+            if (p->c.kind == PK_JOIN_AGG && (rc = join_tail(p))) break;
             rc = agg_finish(p);
             if (!rc) {
                 p->stats.rows_filtered = p->stats.rows_scanned - (int64_t)p->rows_passed_host;   // (came back with the counter block)
             }
         } break;
-        case PK_JOIN: rc = join_rows_finish(p); break;
+        case PK_JOIN: {   // the outer join's preserved rows, then the sink fragment's result
+            std::vector<SortOutCol> cols; int64_t rows = 0;
+            if ((rc = join_tail(p)) || (rc = sort_check(p, sort_finish(p->post_sort, nullptr, 1, p->stream, &p->stats, cols, &rows, p->last_error)))) break;
+            set_result(p, cols, rows, p->c.out_cols.data());
+            p->stats.rows_filtered = 0;
+        } break;
         case PK_SORT: case PK_FILTER: {
             std::vector<SortOutCol> cols; int64_t rows = 0;
-            rc = sort_finish(p->sort, p->nccl_comm, p->nranks, p->stream, &p->stats, cols, &rows, p->last_error);
-            if (rc) { g_thread_error = p->last_error; break; }
-            p->result.clear();
-            for (auto& sc : cols) {
-                HostCol hc; hc.desc = {sc.tuple_id, sc.slot_id, sc.prim, 0}; hc.elem = sc.elem;
-                hc.values = std::move(sc.values); hc.validity = std::move(sc.validity);
-                p->result.push_back(std::move(hc));
-            }
-            p->result_rows = rows; p->result_pos = 0;
+            if ((rc = sort_check(p, sort_finish(p->sort, p->nccl_comm, p->nranks, p->stream, &p->stats, cols, &rows, p->last_error)))) break;
+            set_result(p, cols, rows, nullptr);
         } break;
         default: rc = p->fail(BKGPU_EUNSUPPORTED, "plan kind %d cannot finish", p->c.kind);
     }
@@ -1863,13 +1172,9 @@ static int bkgpu_reset_impl(bkgpu_plan* p) {
         p->fused_last = false;
         p->stats.kernel_launches++;
     }
-    p->jt_built = false;
-    for (JoinSide& s : p->js) {
-        s.rows = 0; s.jt_generic = false; std::fill(s.has_null.begin(), s.has_null.end(), false);
-        for (size_t i = 0; i < s.bitmap.size(); i++) { dev_free(p, s.bitmap[i]); s.bitmap[i] = nullptr; }   // build-side validity of the previous run
-    }
-    if (p->sort) { int rc = sort_reset(p->sort, p->stream, p->last_error); if (rc) { g_thread_error = p->last_error; return rc; } }
-    if (p->c.kind == PK_JOIN && p->post_sort) { int rc = sort_reset(p->post_sort, p->stream, p->last_error); if (rc) { g_thread_error = p->last_error; return rc; } }
+    join_reset(p);
+    if (p->sort) { int rc = sort_check(p, sort_reset(p->sort, p->stream, p->last_error)); if (rc) return rc; }
+    if (p->c.kind == PK_JOIN && p->post_sort) { int rc = sort_check(p, sort_reset(p->post_sort, p->stream, p->last_error)); if (rc) return rc; }
     p->result.clear(); p->result_rows = 0; p->result_pos = 0;
     bkgpu_stats z{}; z.kernel_launches = p->stats.kernel_launches; p->stats = z;
     p->state = S_OPEN;
@@ -1998,7 +1303,7 @@ extern "C" int bkgpu_partial_export(bkgpu_plan* p, void* dev_dst, size_t bytes) 
     if (rc) return rc;
     if (bytes < need) return p->fail(BKGPU_EINVAL, "partial buffer too small: %zu < %zu", bytes, need);
     CK(p, cudaSetDevice(p->device));
-    if (p->c.kind == PK_SORT) { rc = sort_partial_export(p->sort, dev_dst, p->stream, p->last_error); if (rc) g_thread_error = p->last_error; return rc; }
+    if (p->c.kind == PK_SORT) return sort_check(p, sort_partial_export(p->sort, dev_dst, p->stream, p->last_error));
     // compact rows (the layout the in-library all-gather ships): [u64 groups][groups x (key words + lane words)]
     CK(p, launch_partial_export_rows(p->gt, p->c.ap, (uint64_t*)dev_dst, eff_pcap(p), p->stream));
     p->stats.kernel_launches += 1;
@@ -2019,11 +1324,9 @@ extern "C" int bkgpu_partial_merge(bkgpu_plan* p, const void* dev_src, size_t by
     CK(p, cudaSetDevice(p->device));
     if (p->c.kind == PK_SORT) {
         std::vector<SortOutCol> cols; int64_t rows = 0;
-        rc = sort_partial_merge(p->sort, dev_src, nranks, p->stream, cols, &rows, p->last_error);
-        if (rc) { g_thread_error = p->last_error; return rc; }
-        p->result.clear();
-        for (auto& sc : cols) { HostCol hc; hc.desc = {sc.tuple_id, sc.slot_id, sc.prim, 0}; hc.elem = sc.elem; hc.values = std::move(sc.values); hc.validity = std::move(sc.validity); p->result.push_back(std::move(hc)); }
-        p->result_rows = rows; p->result_pos = 0; p->stats.rows_returned = rows; p->state = S_FINISHED;
+        if ((rc = sort_check(p, sort_partial_merge(p->sort, dev_src, nranks, p->stream, cols, &rows, p->last_error)))) return rc;
+        set_result(p, cols, rows, nullptr);
+        p->stats.rows_returned = rows; p->state = S_FINISHED;
         return BKGPU_OK;
     }
     CK(p, launch_table_init(p->gt, p->c.ap, p->stream, 1));

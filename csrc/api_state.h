@@ -1,0 +1,197 @@
+// api_state.h — the plan object behind the C ABI (bkgpu_plan) and the host helpers api.cu and join.cu share.
+#pragma once
+#include <cuda_runtime.h>
+#include <stdarg.h>
+#include <stdio.h>
+#include <stdlib.h>
+#include <time.h>
+#include <atomic>
+#include <string>
+#include <vector>
+#include "../include/bkgpu.h"
+#include "agg.h"
+#include "plan.h"
+#include "sort.h"
+
+using namespace bk;
+
+namespace bk {
+
+enum State { S_INIT = 0, S_OPEN = 1, S_FINISHED = 2, S_CLOSED = 3 };
+
+struct HostCol {  // one materialised result column (host memory owned by the plan)
+    OutCol desc;
+    int elem = 0;
+    std::vector<uint8_t> values;
+    std::vector<uint8_t> validity;  // LSB bitmap; empty = all valid
+    void* dev_values = nullptr;     // output_on_device
+};
+
+struct EventPair { cudaEvent_t a, b; int64_t bytes; };
+
+// one retained build side of a hash join (K4) and its key indexes
+struct JoinSide {
+    std::vector<uint8_t*> vals, nullbytes, bitmap;   // per plan column (this side's columns only)
+    std::vector<bool> has_null;
+    int64_t rows = 0, cap = 0;
+    uint8_t* keybits = nullptr; size_t keybits_cap = 0;   // star join: validity of the build key AND the dimension's build-time filter
+    uint64_t* jt_keys = nullptr; uint32_t* jt_rows = nullptr; uint32_t jt_mask = 0; bool jt_generic = false;   // multimap (duplicate keys)
+    JoinFast jf{}; uint32_t* jf_dense = nullptr; uint64_t* jf_packed = nullptr; size_t jf_dense_cap = 0, jf_packed_cap = 0;   // unique-key index
+    bool learned = false; uint64_t learn_min = 0, learn_max = 0;   // key range of the side's previous build (skips the min/max pass + round trip)
+};
+
+// one plan column of a join's gathered chunk: values, and for a star join's columns with NULLs their null bytes and bitmap
+struct ChunkCol {
+    uint8_t *vals = nullptr, *nullb = nullptr, *bits = nullptr;
+    size_t vals_cap = 0, nullb_cap = 0, bits_cap = 0;
+};
+
+// the hash join (K4) of a plan (join.cu): retained build sides, their indexes, the probe's buffers.  Buffers and indexes are kept
+// across bkgpu_reset; join_reset clears what belongs to one request.
+struct JoinState {
+    JoinSide side[4];            // the two-table join uses side[0], a star join one per dimension
+    bool built = false;          // the build side is complete and indexed: probe batches have started
+    bool tail_launch = false;    // the aggregate launch in progress is the outer-join tail (join_tail)
+    std::vector<ColRef> probe_want; std::vector<int> probe_map;   // probe-side columns and their index in c.cols
+    uint64_t* scratch = nullptr; size_t scratch_cap = 0;   // [0..1] key min / max, then u32 flags: [4] duplicate build key, [5] fused probe unusable, [6] key outside the learned range
+    JoinProbe jp{}; int jp_key_pos = 0;   // the FK -> PK probe fused into the lean aggregate
+    uint32_t* jp_attr = nullptr; uint64_t* jp_packed = nullptr; size_t jp_attr_cap = 0, jp_packed_cap = 0;
+    uint8_t* matched = nullptr; size_t matched_cap = 0;   // LEFT / SEMI / ANTI: build rows that found a partner
+    uint32_t* pairs = nullptr; size_t pairs_cap = 0; uint32_t* cursor = nullptr; size_t cursor_cap = 0;   // PK_JOIN: (probe row, build row) pairs of one batch
+    uint32_t* tuples[2] = {nullptr, nullptr}; size_t tuples_cap[2] = {0, 0};   // star join: row-id tuples of one chunk (probe / expansion ping-pong)
+    std::vector<ChunkCol> chunk;   // the gathered chunk (two-table gather path, star join), per plan column
+    // options
+    int pipeline = 0;            // "join_pipeline": the fused probe issues its lookups one drain ahead (no gain while the kernel is bound by its shared-memory atomics)
+    int no_fused_probe = 0;
+    int star_expand_cap = 0;     // test option "star_expand_capacity": first capacity (tuples) of a star join's expansion pass (0 = twice its input)
+};
+
+// BKGPU_TRACE=1: wall-clock time the HOST spends in each phase of a request (summed per plan, printed by bkgpu_close)
+struct HostClock {
+    double reset = 0, push = 0, collective = 0, extract_wait = 0, finish = 0; int64_t n = 0;
+    static double now() { timespec ts; clock_gettime(CLOCK_MONOTONIC, &ts); return ts.tv_sec * 1e3 + ts.tv_nsec / 1e6; }
+};
+
+}  // namespace bk
+
+extern thread_local std::string g_thread_error;
+
+struct bkgpu_plan {
+    Compiled c;
+    int device = 0;
+    int sm_count = 132;
+    State state = S_INIT;
+    std::string last_error;
+    std::atomic<int> cancelled{0};
+    void* nccl_comm = nullptr;
+    int nranks = 1;
+    // options
+    cudaStream_t stream = nullptr; bool own_stream = false;
+    cudaStream_t copy_stream = nullptr;
+    int group_cap_log2 = 20;
+    int smem_cap_log2 = -1;       // -1 = choose per batch
+    int64_t batch_capacity = 1 << 20;
+    int64_t chunk_rows = 8 << 20;
+    int64_t partial_cap = 1 << 16;
+    int force_generic = 0;
+    int no_lean = 0;
+    int output_on_device = 0;
+    int64_t region_base = 0;      // arrival index of this plan's first row (ties across GPUs break by (region, row))
+    // aggregate state
+    GroupTable gt{};
+    uint64_t* d_rows_passed = nullptr;
+    uint32_t* d_cursor = nullptr;
+    uint64_t* d_partial = nullptr;  // export buffer (this rank)
+    uint64_t* d_gather = nullptr;   // nranks export buffers
+    size_t d_partial_words = 0, d_gather_words = 0;
+    HostClock hclk; bool trace = getenv("BKGPU_TRACE") != nullptr;
+    std::vector<uint8_t*> bounce[2]; size_t bounce_rows = 0; cudaEvent_t bounce_done[2] = {nullptr, nullptr}; bool bounce_busy[2] = {false, false};
+    int scalar_tma = 1;           // COUNT(*) WHERE int32 <cmp> c runs the TMA-staged kernel (scalar_tma.cu); 0 = the LDG kernel
+    int no_bounce = 0;            // 1 = pageable host input goes straight to cudaMemcpyAsync (A/B of the bounce path)
+    int no_stream_copy = 0;       // 1 = the bounce copy uses memcpy instead of non-temporal stores (A/B, hostcopy.cpp)
+    SortState* post_sort = nullptr;                         // the post fragment above the aggregate (Compiled::post)
+    std::vector<uint8_t*> post_vals, post_nullb, post_bitmap; size_t post_cap = 0;
+    uint64_t rows_passed_host = 0;
+    int64_t finish_groups = -1;   // groups in the table when the last finish read the result back (-1 = unknown: full re-initialisation)
+    uint32_t merge_bound = 0, merge_bound_used = 0;   // groups per rank the all-gather is sized for (learned from earlier runs)
+    uint32_t* d_part_cursors = nullptr; int repartition = 0;   // hash repartition of the groups across ranks (option "repartition")
+    // merge over NVLink peer memory (option "peer_merge"): this rank's buffer, the peers' mappings of theirs, step counter
+    int peer_merge = 0, peer_rank = -1; bool peer_ready = false;
+    uint64_t* peer_local = nullptr; std::vector<uint64_t*> peer_ptr; uint64_t** d_peer_ptrs = nullptr; uint64_t peer_seq = 0; size_t peer_seg_words = 0;
+    uint32_t* d_peer_timeout = nullptr;
+    uint64_t* d_outv = nullptr; uint8_t* d_outn = nullptr; size_t out_cap_alloc = 0;  // extraction buffers (kept across resets)
+    std::vector<cudaEvent_t> event_pool;
+    uint64_t* h_outv = nullptr; uint8_t* h_outn = nullptr; size_t h_out_cap = 0;   // pinned landing area of the extracted rows
+    uint32_t known_groups = 0;
+    uint32_t* h_pinned = nullptr;   // [0] groups seen (async copy after every aggregate launch that does not extract its result), pinned
+    // mapped host buffer the lean kernel's last CTA extracts the result into (AggArgs::fused_out), and whether the request's last
+    // aggregate launch did so: then bkgpu_finish only waits and reads it
+    uint8_t* h_fused = nullptr; uint8_t* d_fused = nullptr; size_t fused_bytes = 0; uint32_t fused_cap = 0; bool fused_last = false;
+    JoinState join;               // hash join (K4): PK_JOIN_AGG, PK_JOIN, PK_STAR_AGG
+    int fx_off = 0;               // set when a finished request saw more than 1/64 of its surviving rows take FX's exact path (see agg_finish)
+    int lean_bank = 0;            // opt-in: bank-aware dealing of the lean kernel's drain (agg_direct.cuh, BANK)
+    int lean_fx = [] { const char* e = getenv("BKGPU_LEAN_FX"); return e ? atoi(e) != 0 : BK_LEAN_FX_DEFAULT; }();   // double sums as fixed-point limbs with native shared atomics (agg_direct.cuh, FX); option lean_fx
+    int blocking_sync = -1; bool blocking_wait = false; cudaEvent_t wait_event = nullptr;   // see agg_finish
+    int no_lean_nulls = 0, no_lean_mm = 0;
+    int use_wp = 0;               // 1 = launch the warp-private aggregate kernel where the batch fits it (opt-in: k_agg_group_lean is the default)
+    int wp_kt_log2 = 0;           // log2 words of the warp-private kernel's key table (0 = sized from the cardinality)
+    int wp_warps = 0;             // warps per CTA of the warp-private kernel (0 = chosen from the table size; 8, 12 or 16)
+    // sort / filter state
+    SortState* sort = nullptr;
+    // host staging for pageable / pinned pushes
+    std::vector<void*> stage[2];
+    std::vector<void*> stage_valid[2];
+    size_t stage_rows = 0;
+    cudaEvent_t stage_free[2] = {nullptr, nullptr}, stage_ready[2] = {nullptr, nullptr};
+    // results
+    std::vector<HostCol> result;
+    int64_t result_rows = 0, result_pos = 0;
+    // stats
+    bkgpu_stats stats{};
+    std::vector<EventPair> timed;
+    std::vector<EventPair> timed_coll;
+    std::vector<std::pair<void*, size_t>> dev_allocs;   // (buffer, size class) — returned to the process-wide cache on free / close
+
+    int fail(int code, const char* fmt, ...) {
+        char buf[512]; va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof buf, fmt, ap); va_end(ap);
+        last_error = buf; g_thread_error = buf; return code;
+    }
+    int cuda_fail(cudaError_t e, const char* what) {
+        return fail(e == cudaErrorMemoryAllocation ? BKGPU_ENOMEM : BKGPU_ENODEV, "%s: %s", what, cudaGetErrorString(e));
+    }
+};
+
+#define CK(plan, call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return (plan)->cuda_fail(e__, #call); } while (0)
+
+// ---- api.cu
+// device buffers from the process-wide cache; ensure_buf: grow-only (plans are re-armed with bkgpu_reset and run again)
+int dev_alloc(bkgpu_plan* p, void** out, size_t bytes);
+void dev_free(bkgpu_plan* p, void* ptr);
+int ensure_buf(bkgpu_plan* p, void** ptr, size_t* cap, size_t bytes);
+// the plan's columns `want` resolved against one pushed batch
+int bind_columns(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* cols, int ncols, int64_t nrows, std::vector<const bkgpu_column*>& bound);
+// a batch as device columns (host columns chunk by chunk through the staging buffers), handed to `fn`
+typedef int (*BatchFn)(bkgpu_plan*, const DevCol*, int64_t nrows, int64_t row_base, bool vec_ok);
+int feed(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device, BatchFn fn);
+// the aggregate of `c` over one batch; `jp`: fused FK -> PK probe (lean kernel only), +1 without launching when the batch does not fit it
+int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp = nullptr);
+// the post fragment's input columns, reallocated with room for `cap` rows when they hold fewer than `need`
+int ensure_post(bkgpu_plan* p, size_t need, size_t cap);
+// the result of a sort_* call: a failure's message becomes the thread's error too
+int sort_check(bkgpu_plan* p, int rc);
+// the plan's result from a sort fragment's columns; `desc`: their output column descriptions (nullptr = the sort's own)
+void set_result(bkgpu_plan* p, std::vector<SortOutCol>& cols, int64_t rows, const OutCol* desc);
+
+// rows [off, ...) of a device column
+inline DevCol col_at(const DevCol& c, int64_t off) {
+    DevCol x = c;
+    x.values = (const uint8_t*)c.values + (size_t)off * (size_t)storage_bytes(c.stype);
+    if (c.validity) x.validity = c.validity + off / 8;
+    return x;
+}
+
+// ---- join.cu
+int join_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device);   // PK_JOIN_AGG, PK_JOIN, PK_STAR_AGG
+int join_tail(bkgpu_plan* p);    // LEFT / SEMI / ANTI_SEMI, after the last probe batch: the preserved rows the join type asks for
+void join_reset(bkgpu_plan* p);  // bkgpu_reset: the next request retains its build sides afresh
+JoinArgs join_args(const bkgpu_plan* p, bool tail);   // the general probe of the two-table join, as the aggregate kernels read it

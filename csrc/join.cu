@@ -1,0 +1,526 @@
+// join.cu — host path of the hash join (K4): the retained build sides and their indexes, the two-table probe (fused into the lean
+// aggregate, gather, general), the outer-join tail, the join that returns rows, and the star join's build and probe.
+#include <string.h>
+#include <algorithm>
+#include <vector>
+#include "api_state.h"
+
+static void side_init(bkgpu_plan* p, JoinSide& s) {
+    const size_t nc = p->c.cols.size();
+    if (s.vals.empty()) { s.vals.assign(nc, nullptr); s.nullbytes.assign(nc, nullptr); s.bitmap.assign(nc, nullptr); s.has_null.assign(nc, false); }
+}
+// plan column i as retained by side s
+static DevCol side_col(const Compiled& c, const JoinSide& s, size_t i) {
+    DevCol d{};
+    d.values = s.vals[i]; d.validity = s.bitmap[i]; d.stype = prim_storage(c.cols[i].prim); d.prim = c.cols[i].prim;
+    return d;
+}
+// every plan column of the joined row: the build sides' retained columns and the probe batch's (nullptr: the outer-join tail, whose
+// probe-side columns are never read — row = -1 is NULL)
+static std::vector<DevCol> join_cols(const bkgpu_plan* p, const DevCol* probe_cols) {
+    const Compiled& c = p->c;
+    std::vector<DevCol> all(c.cols.size());
+    for (size_t i = 0; i < c.cols.size(); i++) {
+        all[i].stype = prim_storage(c.cols[i].prim); all[i].prim = c.cols[i].prim;
+        if (c.col_side[i] > 0) all[i] = side_col(c, p->join.side[c.col_side[i] - 1], i);
+    }
+    if (probe_cols) for (size_t w = 0; w < p->join.probe_map.size(); w++) all[(size_t)p->join.probe_map[w]] = probe_cols[w];
+    return all;
+}
+
+// a 4-byte device counter, read once the stream has reached it
+static int read_u32(bkgpu_plan* p, const uint32_t* dev, uint32_t* out) {
+    CK(p, cudaMemcpyAsync(out, dev, 4, cudaMemcpyDeviceToHost, p->stream));
+    CK(p, cudaStreamSynchronize(p->stream));
+    return BKGPU_OK;
+}
+// a pass whose output can outgrow its buffer: `run(cap)` sizes the buffer for `cap` items and launches the pass, which writes at most
+// `cap` of them and counts all of them in `cursor`; a pass that found more is rerun once, with the buffer grown to the count
+template <class Run>
+static int run_counted(bkgpu_plan* p, uint64_t cap, const uint32_t* cursor, uint32_t* found, Run run) {
+    for (int attempt = 0; attempt < 2; attempt++) {
+        int rc;
+        if ((rc = run(cap)) || (rc = read_u32(p, cursor, found))) return rc;
+        if (*found <= cap) break;
+        cap = *found;
+    }
+    return BKGPU_OK;
+}
+
+// the gathered chunk's buffers of plan column m for `rows` rows: values, and null bytes + bitmap when `nulls`
+static int chunk_col(bkgpu_plan* p, size_t m, size_t rows, bool nulls) {
+    std::vector<ChunkCol>& chunk = p->join.chunk;
+    if (chunk.empty()) chunk.assign(p->c.cols.size(), ChunkCol{});
+    ChunkCol& g = chunk[m];
+    int rc;
+    if ((rc = ensure_buf(p, (void**)&g.vals, &g.vals_cap, rows * (size_t)storage_bytes(prim_storage(p->c.cols[m].prim))))) return rc;
+    if (nulls && ((rc = ensure_buf(p, (void**)&g.nullb, &g.nullb_cap, rows)) || (rc = ensure_buf(p, (void**)&g.bits, &g.bits_cap, rows / 8 + 8)))) return rc;
+    return BKGPU_OK;
+}
+
+JoinArgs join_args(const bkgpu_plan* p, bool tail) {
+    const Compiled& c = p->c;
+    const JoinSide& s = p->join.side[0];
+    JoinArgs a; memset(&a, 0, sizeof a);
+    a.enabled = 1; a.keys = s.jt_keys; a.rows = s.jt_rows; a.cap_mask = s.jt_mask;
+    a.probe_col = c.probe_key_col; a.probe_prim = c.cols[(size_t)c.probe_key_col].prim; a.cast_prim = c.join_key_prim;
+    a.join_type = c.join_type; a.matched = c.join_type == BK_INNER_JOIN ? nullptr : p->join.matched; a.n_build = s.rows;
+    a.tail = tail ? 1 : 0;
+    return a;
+}
+
+// ---- retain the build (outer / driver) table, build its indexes at the first probe batch ----
+// `side`: the Compiled::col_side value of this table's columns (1 for the two-table join, 1 + d for dimension d of a star join)
+static int join_retain_build(bkgpu_plan* p, int side, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device) {
+    const Compiled& c = p->c;
+    JoinSide& s = p->join.side[side - 1];
+    if (p->join.built) return p->fail(BKGPU_ESTATE, "build-side rows arrived after probing started (the reference fetches the whole driver table first, join_node.cpp:920-1022)");
+    const size_t nc = c.cols.size();
+    side_init(p, s);
+    std::vector<ColRef> want; std::vector<int> idx;
+    for (size_t i = 0; i < nc; i++) if (c.col_side[i] == side) { want.push_back(c.cols[i]); idx.push_back((int)i); }
+    std::vector<const bkgpu_column*> bound;
+    int rc = bind_columns(p, want, cols, ncols, nrows, bound);
+    if (rc) return rc;
+    if (s.rows + nrows > 0xFFFFFFF0ll) return p->fail(BKGPU_EUNSUPPORTED, "build side larger than 2^32 rows");
+    if (s.rows + nrows > s.cap) {
+        const int64_t cap = std::max<int64_t>(s.rows + nrows, std::max<int64_t>(s.cap * 2, 1 << 16));
+        for (int i : idx) {
+            const size_t eb = (size_t)storage_bytes(prim_storage(c.cols[(size_t)i].prim));
+            uint8_t *nv = nullptr, *nn = nullptr;
+            if ((rc = dev_alloc(p, (void**)&nv, (size_t)cap * eb))) return rc;
+            if ((rc = dev_alloc(p, (void**)&nn, (size_t)cap))) return rc;
+            if (s.rows) {
+                CK(p, cudaMemcpyAsync(nv, s.vals[(size_t)i], (size_t)s.rows * eb, cudaMemcpyDeviceToDevice, p->stream));
+                CK(p, cudaMemcpyAsync(nn, s.nullbytes[(size_t)i], (size_t)s.rows, cudaMemcpyDeviceToDevice, p->stream));
+                CK(p, cudaStreamSynchronize(p->stream));
+            }
+            dev_free(p, s.vals[(size_t)i]); dev_free(p, s.nullbytes[(size_t)i]);
+            s.vals[(size_t)i] = nv; s.nullbytes[(size_t)i] = nn;
+        }
+        s.cap = cap;
+    }
+    for (size_t w = 0; w < want.size(); w++) {
+        const int i = idx[w];
+        const size_t eb = (size_t)storage_bytes(prim_storage(c.cols[(size_t)i].prim));
+        uint8_t* dv = s.vals[(size_t)i] + (size_t)s.rows * eb;
+        uint8_t* dn = s.nullbytes[(size_t)i] + s.rows;
+        if (on_device) {
+            CK(p, cudaMemcpyAsync(dv, bound[w]->values, (size_t)nrows * eb, cudaMemcpyDeviceToDevice, p->stream));
+            CK(p, launch_unpack_validity(bound[w]->validity, nrows, dn, p->stream));
+            p->stats.kernel_launches++;
+        } else {
+            CK(p, cudaMemcpyAsync(dv, bound[w]->values, (size_t)nrows * eb, cudaMemcpyHostToDevice, p->stream));
+            std::vector<uint8_t> nb((size_t)nrows, 0);
+            if (bound[w]->validity) for (int64_t r = 0; r < nrows; r++) nb[(size_t)r] = ((bound[w]->validity[r >> 3] >> (r & 7)) & 1) ? 0 : 1;
+            CK(p, cudaMemcpyAsync(dn, nb.data(), (size_t)nrows, cudaMemcpyHostToDevice, p->stream));
+            CK(p, cudaStreamSynchronize(p->stream));
+            p->stats.h2d_bytes += (int64_t)((size_t)nrows * (eb + 1));
+        }
+        if (bound[w]->validity) s.has_null[(size_t)i] = true;
+    }
+    s.rows += nrows;
+    return BKGPU_OK;
+}
+
+// Fused probe (JoinProbe in agg.h): usable when the only build-side column the aggregate reads is its 4-byte GROUP BY
+// key and the probe key is a 32-bit integer column whose cast to the comparison type keeps the canonical image.
+static int join_compose_probe(bkgpu_plan* p, uint32_t* flag) {
+    const Compiled& c = p->c;
+    JoinState& j = p->join;
+    const JoinSide& s = j.side[0];
+    j.jp = JoinProbe{};
+    if (!c.jfast || !c.jfast->has_direct || c.jfast->direct.n_keys != 1) return BKGPU_OK;
+    const Compiled& f = *c.jfast;
+    const size_t kpos = (size_t)f.direct.n_terms;
+    int attr_main = -1;
+    for (size_t i = 0; i < f.direct_cols.size(); i++) {
+        const int m = c.jfast_of_main[(size_t)f.direct_cols[i]];
+        if (c.col_side[(size_t)m] != 1) continue;
+        if (i != kpos) return BKGPU_OK;   // a predicate or an aggregate argument comes from the build side: gather path
+        attr_main = m;
+    }
+    if (attr_main < 0) return BKGPU_OK;
+    const int ast = prim_storage(c.cols[(size_t)attr_main].prim);
+    if ((ast != ST_I32 && ast != ST_U32) || (c.cols[(size_t)attr_main].prim != BK_INT32 && c.cols[(size_t)attr_main].prim != BK_UINT32)) return BKGPU_OK;
+    const int pp = c.cols[(size_t)c.probe_key_col].prim, ct = c.join_key_prim;
+    const bool ident = (pp == BK_INT32 && (ct == BK_INT32 || ct == BK_INT64)) || (pp == BK_UINT32 && (ct == BK_UINT32 || ct == BK_UINT64 || ct == BK_INT64));
+    if (!ident) return BKGPU_OK;
+    int rc;
+    JoinProbe jp{};
+    jp.mode = s.jf.mode; jp.key_signed = pp == BK_INT32 ? 1 : 0;
+    jp.dense_min = s.jf.dense_min; jp.dense_size = s.jf.dense_size; jp.bias = s.jf.bias; jp.packed_mask = s.jf.packed_mask;
+    if (jp.mode == 1) {
+        if ((rc = ensure_buf(p, (void**)&j.jp_attr, &j.jp_attr_cap, (size_t)jp.dense_size * 4))) return rc;
+        jp.attr = j.jp_attr;
+        jp.present = (uint64_t)s.rows == jp.dense_size ? nullptr : s.jf.dense;   // unique, NULL-free keys filling the range: every key exists
+    } else {
+        if ((rc = ensure_buf(p, (void**)&j.jp_packed, &j.jp_packed_cap, ((size_t)jp.packed_mask + 1) * 8))) return rc;
+        jp.packed = j.jp_packed;
+    }
+    CK(p, launch_join_compose(s.jf, (const uint32_t*)s.vals[(size_t)attr_main], j.jp_attr, j.jp_packed, flag, p->stream));
+    p->stats.kernel_launches++;
+    j.jp = jp; j.jp_key_pos = (int)kpos;   // (the caller drops it again when `flag` comes back set)
+    return BKGPU_OK;
+}
+
+// validity bitmaps of the side's retained columns that hold NULLs
+static int join_pack_validity(bkgpu_plan* p, JoinSide& s, int side) {
+    const Compiled& c = p->c;
+    side_init(p, s);
+    int rc;
+    for (size_t i = 0; i < c.cols.size(); i++) {
+        if (c.col_side[i] != side) continue;
+        // (a bitmap kept from an earlier run of the plan must not mask this run's rows: a column without NULLs has none)
+        dev_free(p, s.bitmap[i]); s.bitmap[i] = nullptr;
+        if (!s.has_null[i]) continue;
+        if ((rc = dev_alloc(p, (void**)&s.bitmap[i], (size_t)(s.rows + 7) / 8 + 8))) return rc;
+        CK(p, launch_pack_validity(s.nullbytes[i], s.rows, s.bitmap[i], p->stream));
+        p->stats.kernel_launches++;
+    }
+    return BKGPU_OK;
+}
+
+// The unique-key index of side `s` (FK -> PK fast path): a dense array when the key range is small, else a packed table for keys of at most
+// 32 bits.  s.jf.mode stays 0 when neither fits or a key repeats.  `compose`: the two-table join's fused probe is composed behind the build,
+// so that its flag comes back in the same round trip.
+static int join_build_index(bkgpu_plan* p, JoinSide& s, const DevCol& key, int cast_prim, bool compose) {
+    JoinState& j = p->join;
+    int rc;
+    s.jf = JoinFast{};
+    if (s.rows <= 0) return BKGPU_OK;
+    bool retry_measured = false;
+again:
+    const int cls = host_prim_class(cast_prim);
+    const uint64_t bias = cls == VC_I64 ? 0x8000000000000000ull : 0ull;
+    if ((rc = ensure_buf(p, (void**)&j.scratch, &j.scratch_cap, 64))) return rc;
+    uint64_t* mm = j.scratch; uint32_t* dup = (uint32_t*)(j.scratch + 2);
+    // the key range: measured (one pass over the keys + a round trip), or — when this plan has built before — the range it saw then,
+    // checked by the build kernel itself (a key outside it raises a flag and the build is redone with a measured range)
+    uint64_t h_mm[2];
+    bool guessed = s.learned && !retry_measured;
+    if (guessed) { h_mm[0] = s.learn_min; h_mm[1] = s.learn_max; }
+    else {
+        CK(p, launch_join_minmax(key, key.prim, cast_prim, s.rows, bias, mm, p->stream));
+        CK(p, cudaMemcpyAsync(h_mm, mm, 16, cudaMemcpyDeviceToHost, p->stream));
+        CK(p, cudaStreamSynchronize(p->stream));
+        p->stats.kernel_launches++;
+    }
+    JoinFast jf{}; jf.bias = bias;
+    const uint64_t range = h_mm[1] >= h_mm[0] ? h_mm[1] - h_mm[0] + 1 : 0;
+    const int kb = storage_bytes(prim_storage(cast_prim));
+    if (range > 0 && range <= (uint64_t)4 * (uint64_t)s.rows + 1024 && range <= (1ull << 30)) {
+        jf.mode = 1; jf.dense_min = h_mm[0]; jf.dense_size = range;
+        if ((rc = ensure_buf(p, (void**)&s.jf_dense, &s.jf_dense_cap, (size_t)range * 4))) return rc;
+        jf.dense = s.jf_dense;
+    } else if (kb <= 4) {
+        uint32_t pc = 1024; while ((int64_t)pc < 2 * s.rows) pc <<= 1;
+        jf.mode = 2; jf.packed_mask = pc - 1;
+        if ((rc = ensure_buf(p, (void**)&s.jf_packed, &s.jf_packed_cap, (size_t)pc * 8))) return rc;
+        jf.packed = s.jf_packed;
+    }
+    if (jf.mode) {
+        CK(p, launch_join_build_fast(key, key.prim, cast_prim, s.rows, jf, s.jf_dense, s.jf_packed, dup, p->stream));
+        p->stats.kernel_launches += 1;
+        s.jf = jf;
+        if (compose && (rc = join_compose_probe(p, dup + 1))) return rc;   // enqueued behind the build: all flags come back in one round trip
+        uint32_t h_flags[3] = {0, 0, 0};
+        CK(p, cudaMemcpyAsync(h_flags, dup, 12, cudaMemcpyDeviceToHost, p->stream));
+        CK(p, cudaStreamSynchronize(p->stream));
+        if (h_flags[2] && guessed) { retry_measured = true; goto again; }   // this run's keys left the learned range
+        if (h_flags[0]) { s.jf = JoinFast{}; j.jp = JoinProbe{}; }   // duplicate build keys: not a PK, the general probe runs
+        else if (h_flags[1]) j.jp = JoinProbe{};
+        s.learned = true; s.learn_min = h_mm[0]; s.learn_max = h_mm[1];
+    } else if (guessed) { retry_measured = true; goto again; }   // (the learned range no longer fits this row count)
+    return BKGPU_OK;
+}
+
+static int join_build_table(bkgpu_plan* p) {
+    const Compiled& c = p->c;
+    JoinState& j = p->join;
+    JoinSide& s = j.side[0];
+    int rc;
+    if ((rc = join_pack_validity(p, s, 1))) return rc;
+    j.built = true; s.jt_generic = false;   // the multimap of the general probe is built on first use (join_generic_table)
+    // ---- FK -> PK fast path: are the build keys unique, and is their range dense or their type <= 32 bits? ----
+    s.jf = JoinFast{}; j.jp = JoinProbe{};
+    bool build_nulls = false;
+    for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] == 1 && s.has_null[i]) build_nulls = true;   // gathered columns must be NULL-free
+    if (!c.jfast || build_nulls) return BKGPU_OK;
+    return join_build_index(p, s, side_col(c, s, (size_t)c.build_key_col), c.join_key_prim, true);
+}
+
+// the multimap of side `s` (duplicate build keys, the general probe): open addressing from the cast key image to the build row
+static int join_build_multimap(bkgpu_plan* p, JoinSide& s, const DevCol& key, int cast_prim) {
+    int rc;
+    uint32_t cap = 1024;
+    while ((int64_t)cap < 2 * s.rows) cap <<= 1;
+    dev_free(p, s.jt_keys); dev_free(p, s.jt_rows); s.jt_keys = nullptr; s.jt_rows = nullptr;
+    if ((rc = dev_alloc(p, (void**)&s.jt_keys, (size_t)cap * 8))) return rc;
+    if ((rc = dev_alloc(p, (void**)&s.jt_rows, (size_t)cap * 4))) return rc;
+    s.jt_mask = cap - 1;
+    CK(p, launch_join_build(key, key.prim, cast_prim, s.rows, s.jt_keys, s.jt_rows, s.jt_mask, p->stream));
+    p->stats.kernel_launches++;
+    s.jt_generic = true;
+    return BKGPU_OK;
+}
+
+// the general probe's multimap (duplicate build keys, unmatched probe rows): built only when a batch needs it
+static int join_generic_table(bkgpu_plan* p) {
+    const Compiled& c = p->c;
+    JoinState& j = p->join;
+    JoinSide& s = j.side[0];
+    if (s.jt_generic) return BKGPU_OK;
+    int rc;
+    if ((rc = join_build_multimap(p, s, side_col(c, s, (size_t)c.build_key_col), c.join_key_prim))) return rc;
+    if (c.join_type != BK_INNER_JOIN) {   // one "found a partner" byte per build row
+        if ((rc = ensure_buf(p, (void**)&j.matched, &j.matched_cap, (size_t)std::max<int64_t>(s.rows, 1)))) return rc;
+        CK(p, cudaMemsetAsync(j.matched, 0, (size_t)std::max<int64_t>(s.rows, 1), p->stream));
+    }
+    return BKGPU_OK;
+}
+
+static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nrows, int64_t, bool) {
+    const Compiled& c = p->c;
+    JoinState& j = p->join;
+    const JoinSide& s = j.side[0];
+    const std::vector<DevCol> all = join_cols(p, probe_cols);
+    // ---- FK -> PK fast path: gather the build columns next to the probe rows, then the ordinary (lean) aggregate ----
+    if (s.jf.mode != 0 && j.jp.mode != 0 && c.jfast && !p->force_generic && !j.no_fused_probe) {
+        // ---- fused probe: the lean aggregate reads the foreign key and looks the group key up itself ----
+        const Compiled& f = *c.jfast;
+        std::vector<DevCol> fc(f.cols.size());
+        const int key_fcol = f.direct_cols[(size_t)j.jp_key_pos];
+        bool vec_ok = true;
+        for (size_t i = 0; i < f.cols.size(); i++) {
+            fc[i] = (int)i == key_fcol ? all[(size_t)c.probe_key_col] : all[(size_t)c.jfast_of_main[i]];
+            if (((uintptr_t)fc[i].values & 31) != 0) vec_ok = false;
+        }
+        const int rc = launch_agg_batch(p, f, fc.data(), nrows, vec_ok, &j.jp);
+        if (rc <= 0) return rc;   // launched (0) or failed (< 0); +1: this batch does not fit the lean kernel
+    }
+    if (s.jf.mode != 0 && c.jfast && !p->force_generic) {
+        const Compiled& f = *c.jfast;
+        const int64_t chunk = 16 << 20;   // the gathered chunk is re-read immediately: keep it L2-sized
+        for (int64_t off = 0; off < nrows; off += chunk) {
+            const int64_t n = std::min(chunk, nrows - off);
+            GatherCols gc{}; std::vector<DevCol> fc(f.cols.size());
+            int rc;
+            for (size_t i = 0; i < f.cols.size(); i++) {
+                const size_t m = (size_t)c.jfast_of_main[i];
+                if (c.col_side[m] != 1) { fc[i] = col_at(all[m], off); continue; }
+                if ((rc = chunk_col(p, m, (size_t)chunk, false))) return rc;
+                uint8_t* dst = j.chunk[m].vals;
+                gc.src[gc.n] = s.vals[m]; gc.dst[gc.n] = dst; gc.elem[gc.n] = storage_bytes(all[m].stype); gc.n++;
+                fc[i] = all[m]; fc[i].values = dst; fc[i].validity = nullptr;
+            }
+            CK(p, cudaMemsetAsync(p->d_cursor + 1, 0, 4, p->stream));
+            CK(p, launch_join_gather(col_at(all[(size_t)c.probe_key_col], off), c.cols[(size_t)c.probe_key_col].prim, c.join_key_prim, n, s.jf, gc, p->d_cursor + 1, p->stream));
+            p->stats.kernel_launches++;
+            uint32_t miss = 0;
+            if ((rc = read_u32(p, p->d_cursor + 1, &miss))) return rc;
+            if (miss) {   // some probe row has no partner (or a NULL key): this chunk takes the general probe
+                std::vector<DevCol> sl(all);
+                for (size_t i = 0; i < sl.size(); i++) if (c.col_side[i] == 0) sl[i] = col_at(all[i], off);
+                if ((rc = join_generic_table(p))) return rc;
+                if ((rc = launch_agg_batch(p, c, sl.data(), n, false))) return rc;
+            } else {
+                bool vec_ok = true;
+                for (auto& d : fc) if (((uintptr_t)d.values & 31) != 0) vec_ok = false;
+                if ((rc = launch_agg_batch(p, f, fc.data(), n, vec_ok))) return rc;
+            }
+        }
+        return BKGPU_OK;
+    }
+    { int rc = join_generic_table(p); if (rc) return rc; }
+    return launch_agg_batch(p, c, all.data(), nrows, false);
+}
+
+// ---- a JOIN that returns rows (PK_JOIN): pairs -> gather -> the sink fragment (p->post_sort) ----
+static int join_rows_emit(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t n_probe, bool tail) {
+    const Compiled& c = p->c;
+    JoinState& j = p->join;
+    int rc;
+    AggArgs a; memset(&a, 0, sizeof a);
+    a.plan = c.ap; a.prog = c.prog; a.nrows = n_probe;
+    const int ncols = (int)c.cols.size();
+    for (int i = 0; i < ncols; i++) a.cols[i] = all[(size_t)i];
+    a.n_cols = ncols;
+    a.join = join_args(p, tail);
+    if ((rc = ensure_buf(p, (void**)&j.cursor, &j.cursor_cap, 64))) return rc;
+    uint32_t found = 0;
+    rc = run_counted(p, (uint64_t)std::max<int64_t>(tail ? j.side[0].rows : n_probe, 1 << 12), j.cursor, &found, [&](uint64_t want) -> int {
+        if (want > 0x7FFFFFF0ull) return p->fail(BKGPU_ETOOBIG, "a probe batch joins to more than 2^31 rows: push smaller batches");
+        int r;
+        if ((r = ensure_buf(p, (void**)&j.pairs, &j.pairs_cap, (size_t)want * 8))) return r;
+        CK(p, cudaMemsetAsync(j.cursor, 0, 4, p->stream));
+        // (a rerun of a LEFT batch sets the same matched[] flags again: they only ever go from 0 to 1)
+        CK(p, launch_join_pairs(a, j.pairs, (uint32_t)want, j.cursor, p->sm_count, p->stream));
+        p->stats.kernel_launches++;
+        return BKGPU_OK;
+    });
+    if (rc || !found) return rc;
+    const Compiled& pc = *c.post;
+    const size_t nc = pc.cols.size();
+    if ((rc = ensure_post(p, found, std::max<size_t>((size_t)found + found / 4, 1 << 16)))) return rc;
+    std::vector<DevCol> dc(std::max<size_t>(nc, 1));
+    for (size_t k = 0; k < nc; k++) {   // sink column k = output column k = device column k of the join (plan.cpp::lower_join_rows)
+        const int st = prim_storage(pc.cols[k].prim);
+        CK(p, launch_join_rows_gather(all[k], j.pairs, 2, c.col_side[k] == 1 ? 1 : 0, found, storage_bytes(st), p->post_vals[k], p->post_nullb[k], p->stream));
+        CK(p, launch_pack_validity(p->post_nullb[k], found, p->post_bitmap[k], p->stream));
+        dc[k].values = p->post_vals[k]; dc[k].validity = p->post_bitmap[k]; dc[k].stype = st; dc[k].prim = pc.cols[k].prim;
+    }
+    p->stats.kernel_launches += 2 * (int64_t)nc;
+    p->rows_passed_host += found;
+    if ((rc = sort_check(p, sort_push(p->post_sort, dc.data(), (int64_t)found, p->stream, &p->stats, p->last_error)))) return rc;
+    CK(p, cudaStreamSynchronize(p->stream));   // the gather buffers are reused by the next batch
+    return BKGPU_OK;
+}
+static int join_rows_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nrows, int64_t, bool) {
+    int rc;
+    if ((rc = join_generic_table(p))) return rc;
+    return join_rows_emit(p, join_cols(p, probe_cols), nrows, false);
+}
+
+// LEFT / SEMI / ANTI_SEMI: once every probe batch has run, the preserved (build) side's rows the join type asks for go through the
+// aggregate (PK_JOIN_AGG) or the sink (PK_JOIN) — unmatched rows NULL-extended (LEFT), matched rows (SEMI), unmatched rows (ANTI_SEMI);
+// join_node.cpp:1200-1276
+int join_tail(bkgpu_plan* p) {
+    const Compiled& c = p->c;
+    JoinState& j = p->join;
+    if (c.join_type == BK_INNER_JOIN || j.side[0].rows == 0) return BKGPU_OK;
+    int rc;
+    if (!j.built && (rc = join_build_table(p))) return rc;
+    if ((rc = join_generic_table(p))) return rc;
+    const std::vector<DevCol> all = join_cols(p, nullptr);
+    if (c.kind == PK_JOIN) return join_rows_emit(p, all, 0, true);
+    j.tail_launch = true;
+    rc = launch_agg_batch(p, c, all.data(), j.side[0].rows, false);
+    j.tail_launch = false;
+    return rc;
+}
+
+// ---- star join (PK_STAR_AGG): every dimension is retained and indexed before the first fact batch ----
+static int star_build(bkgpu_plan* p) {
+    const Compiled& c = p->c;
+    p->join.built = true;
+    int rc;
+    for (size_t d = 0; d < c.dims.size(); d++) {
+        JoinSide& s = p->join.side[d];
+        const StarDim& sd = c.dims[d];
+        if ((rc = join_pack_validity(p, s, 1 + (int)d))) return rc;
+        s.jt_generic = false; s.jf = JoinFast{};
+        if (s.rows == 0) continue;
+        DevCol key = side_col(c, s, (size_t)sd.key_col);
+        if (sd.n_filter > 0) {   // the build key's validity: the key is not NULL and the dimension's own conjuncts are TRUE
+            if ((rc = ensure_buf(p, (void**)&s.keybits, &s.keybits_cap, ((size_t)s.rows + 31) / 32 * 4))) return rc;
+            StarFilter f; memset(&f, 0, sizeof f);
+            for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] == 1 + (int)d) f.cols[i] = side_col(c, s, i);
+            f.prog = sd.filter; f.key_col = sd.key_col; f.nrows = s.rows;
+            CK(p, launch_star_dim_filter(f, (uint32_t*)s.keybits, p->stream));
+            p->stats.kernel_launches++;
+            key.validity = s.keybits;
+        }
+        // unique keys: the dense or packed index; duplicate keys (or 64-bit keys over a wide range): the multimap
+        if ((rc = join_build_index(p, s, key, sd.cast_prim, false))) return rc;
+        if (s.jf.mode == 0 && (rc = join_build_multimap(p, s, key, sd.cast_prim))) return rc;
+    }
+    return BKGPU_OK;
+}
+
+// the tuple buffer `k` with room for `n` tuples of `w` row ids
+static int star_tuples(bkgpu_plan* p, int k, uint64_t n, int w) {
+    if (n * (uint64_t)w > 0xFFFFFFF0ull) return p->fail(BKGPU_ETOOBIG, "a star join chunk joins to more than 2^32 row ids: push smaller batches");
+    return ensure_buf(p, (void**)&p->join.tuples[k], &p->join.tuples_cap[k], (size_t)std::max<uint64_t>(n, 1) * (size_t)w * 4);
+}
+
+// A fact batch, chunk by chunk: k_star_probe keeps the rows with a partner in every dimension of unique keys, each dimension with duplicate
+// keys expands the survivors (k_star_expand), the referenced columns are gathered side by side, and the aggregate runs over them as the
+// virtual joined tuple (Compiled::jfast: the lean kernel when the shape fits).
+static int star_probe_batch(bkgpu_plan* p, const DevCol* fact_cols, int64_t nrows, int64_t, bool vec_ok) {
+    const Compiled& c = p->c;
+    const Compiled& f = *c.jfast;
+    JoinState& j = p->join;
+    const int D = (int)c.dims.size(), W = 1 + D;
+    for (int d = 0; d < D; d++) if (j.side[d].rows == 0) return BKGPU_OK;   // an empty dimension: no row joins
+    const std::vector<DevCol> all = join_cols(p, fact_cols);
+    int rc;
+    const int64_t chunk = 16 << 20;
+    for (int64_t off = 0; off < nrows; off += chunk) {
+        const int64_t n = std::min(chunk, nrows - off);
+        StarProbe sp; memset(&sp, 0, sizeof sp);
+        sp.width = W; sp.nrows = n; sp.vec = vec_ok ? 1 : 0;
+        for (int d = 0; d < D; d++) {
+            if (j.side[d].jf.mode == 0) continue;
+            const StarDim& sd = c.dims[(size_t)d];
+            StarLookup& L = sp.d[sp.n++];
+            L.fk = col_at(all[(size_t)sd.fk_col], off); L.from_prim = c.cols[(size_t)sd.fk_col].prim; L.cast_prim = sd.cast_prim; L.slot = 1 + d; L.jf = j.side[d].jf;
+        }
+        if ((rc = star_tuples(p, 0, (uint64_t)n, W))) return rc;
+        CK(p, launch_star_probe(sp, j.tuples[0], p->d_cursor + 1, p->sm_count, p->stream));
+        p->stats.kernel_launches++;
+        uint32_t found = 0;
+        if ((rc = read_u32(p, p->d_cursor + 1, &found))) return rc;
+        int cur = 0;
+        for (int d = 0; d < D && found; d++) {   // dimensions with duplicate keys: one expansion pass each
+            const JoinSide& s = j.side[d];
+            if (s.jf.mode != 0) continue;
+            const StarDim& sd = c.dims[(size_t)d];
+            const DevCol fk = col_at(all[(size_t)sd.fk_col], off);
+            uint32_t got = 0;
+            rc = run_counted(p, j.star_expand_cap > 0 ? (uint64_t)j.star_expand_cap : std::max<uint64_t>(2 * (uint64_t)found, 4096), p->d_cursor + 1, &got,
+                             [&](uint64_t cap) -> int {
+                int r;
+                if ((r = star_tuples(p, 1 - cur, cap, W))) return r;
+                CK(p, launch_star_expand(fk, c.cols[(size_t)sd.fk_col].prim, sd.cast_prim, s.jt_keys, s.jt_rows, s.jt_mask, j.tuples[cur], found,
+                                         W, 1 + d, j.tuples[1 - cur], (uint32_t)cap, p->d_cursor + 1, p->stream));
+                p->stats.kernel_launches++;
+                return BKGPU_OK;
+            });
+            if (rc) return rc;
+            found = got; cur = 1 - cur;
+        }
+        if (!found) continue;
+        // the joined chunk: every column the aggregate reads, gathered from its tuple's row
+        std::vector<DevCol> fc(f.cols.size());
+        for (size_t i = 0; i < f.cols.size(); i++) {
+            const size_t m = (size_t)c.jfast_of_main[i];
+            const int side = c.col_side[m];
+            const DevCol src = side == 0 ? col_at(all[m], off) : all[m];
+            if ((rc = chunk_col(p, m, found, src.validity != nullptr))) return rc;   // NULLs travel along: null bytes, then a bitmap
+            const ChunkCol& g = j.chunk[m];
+            fc[i] = src; fc[i].values = g.vals; fc[i].validity = nullptr;
+            CK(p, launch_join_rows_gather(src, j.tuples[cur], W, side, found, storage_bytes(src.stype), g.vals, src.validity ? g.nullb : nullptr, p->stream));
+            p->stats.kernel_launches++;
+            if (src.validity) {
+                CK(p, launch_pack_validity(g.nullb, found, g.bits, p->stream));
+                p->stats.kernel_launches++;
+                fc[i].validity = g.bits;
+            }
+        }
+        if ((rc = launch_agg_batch(p, f, fc.data(), found, true))) return rc;
+    }
+    return BKGPU_OK;
+}
+
+// a batch of a build table — the two-table join's build side, a star join's dimensions — is retained; any other batch is probed
+int join_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device) {
+    const Compiled& c = p->c;
+    JoinState& j = p->join;
+    const bool star = c.kind == PK_STAR_AGG;
+    int side = 0;   // (the Compiled::col_side value of the build table's columns)
+    if (!star) { for (int k = 0; k < ncols; k++) if (cols[k].tuple_id == c.build_tuple) side = 1; }
+    else for (size_t d = 0; d < c.dims.size() && !side; d++) for (int k = 0; k < ncols; k++) if (cols[k].tuple_id == c.dims[d].tuple_id) side = 1 + (int)d;
+    if (side) return join_retain_build(p, side, cols, ncols, nrows, on_device);
+    if (!j.built) { int rc = star ? star_build(p) : join_build_table(p); if (rc) return rc; }
+    if (j.probe_want.empty()) for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] == 0) { j.probe_want.push_back(c.cols[i]); j.probe_map.push_back((int)i); }
+    return feed(p, j.probe_want, cols, ncols, nrows, on_device, star ? star_probe_batch : c.kind == PK_JOIN ? join_rows_batch : join_probe_batch);
+}
+
+void join_reset(bkgpu_plan* p) {
+    p->join.built = false;
+    for (JoinSide& s : p->join.side) {
+        s.rows = 0; s.jt_generic = false; std::fill(s.has_null.begin(), s.has_null.end(), false);
+        for (size_t i = 0; i < s.bitmap.size(); i++) { dev_free(p, s.bitmap[i]); s.bitmap[i] = nullptr; }   // build-side validity of the previous run
+    }
+}

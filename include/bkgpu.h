@@ -116,7 +116,6 @@ int   bkgpu_init(bkgpu_plan** out, const uint8_t* plan_desc, size_t len,
  *   "scalar_tma"           0 = COUNT(*) WHERE int32 <cmp> c takes the LDG kernel instead of the TMA-staged one (csrc/scalar_tma.cu; default 1)
  *   "no_bounce"            pageable host input goes straight to cudaMemcpyAsync instead of the threaded pinned bounce buffers (A/B)
  *   "no_stream_copy"       the bounce copy uses memcpy instead of non-temporal stores (A/B)
- *   "join_learn_range"     (default 1) a re-run plan builds its join index with the key range it saw before, checked by the build kernel
  *   "join_pipeline"        (default 0) the fused FK->PK probe issues its lookups one drain ahead (opt-in)
  *   "star_expand_capacity" (tests) first capacity, in row-id tuples, of a star join's expansion pass over a dimension with duplicate keys
  *                          (0 = twice the pass's input); a pass that outgrows it is counted, grown to the exact count and run again

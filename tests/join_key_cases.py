@@ -251,7 +251,7 @@ def fused_plan(dim: Dim) -> P.Plan:
     return P.Plan(a, {**tuples([dim]), AT: P.agg_tuple_slots(aggs, [T.INT64, T.DOUBLE])})
 
 
-# ---- what the build picks (join_build_index in csrc/api.cu) ----
+# ---- what the build picks (join_build_index in csrc/join.cu) ----
 def index_mode(dim: Dim, cast: Optional[int] = None) -> str:
     """"dense" when the biased key range is at most 4 * rows + 1024 (and 2^30), else "packed" for keys of at most 4 bytes, else (and
     whenever a key repeats) "multimap".  Signed keys are biased by 2^63, so that their order is the unsigned order of the image."""
