@@ -14,6 +14,7 @@
 // cardinality is handled; the global table is also the per-GPU partial state that NCCL ships.
 #include "agg_kernels.cuh"
 #include "interp.cuh"
+#include "agg_select.h"
 
 namespace bk {
 
@@ -386,24 +387,6 @@ cudaError_t launch_images_to_columns(const uint64_t* outv, const uint8_t* outn, 
 // ------------------------------------------------------------------------------------------
 // host-side launchers
 // ------------------------------------------------------------------------------------------
-size_t agg_smem_bytes(int smem_keyw, int n_smem_lanes, int cap_log2) {
-    if (cap_log2 <= 0 || smem_keyw == 0) return 0;
-    return ((size_t)(smem_keyw + n_smem_lanes) * 8 + 4) << cap_log2;
-}
-
-// shared memory of the direct GROUP BY kernel: the table plus one compaction queue per warp
-size_t direct_smem_bytes(int smem_keyw, int n_smem_lanes, int cap_log2, int na) {
-    const size_t table = (agg_smem_bytes(smem_keyw, n_smem_lanes, cap_log2) + 127) & ~(size_t)127;
-    const size_t q_direct = ((size_t)(2 + na) * 128 + 16) * 8;  // QCAP = 128 entries per warp, up to 2 key words
-    const size_t q_lean = ((((size_t)(1 + na) * 160 + 20) + 15) & ~(size_t)15) * 8 + 8;   // LEAN_QCAP = 160-entry ring, one key word, 128-byte aligned (+ slack for the base)
-    const size_t queue = q_direct > q_lean ? q_direct : q_lean;
-    const int warps = (DIRECT_THREADS > LEAN_THREADS ? DIRECT_THREADS : LEAN_THREADS) / 32;   // sized for the larger of the two CTA shapes
-    return table + queue * warps;
-}
-
-// FX (agg_direct.cuh): one low-extension limb (4 bytes) per value column and slot, behind the queues
-size_t fx_ext_bytes(int na, int cap_log2) { return ((size_t)4 * (size_t)na) << cap_log2; }
-
 template <class K>
 static int occupancy_grid(K kernel, size_t smem, int sm_count) {
     int per_sm = 0;
@@ -411,35 +394,29 @@ static int occupancy_grid(K kernel, size_t smem, int sm_count) {
     return per_sm * sm_count;  // persistent grid: a whole number of CTAs per SM (132 SMs on H100 SXM)
 }
 
-cudaError_t launch_agg(const AggArgs& a, bool direct, int sm_count, cudaStream_t s, cudaEvent_t start, const char** kernel_name) {
-    const bool grouped = a.plan.n_keyw > 0;
-    const size_t smem = grouped ? agg_smem_bytes(a.smem_keyw, a.n_smem_lanes, a.smem_cap_log2) : 0;
+cudaError_t launch_agg(const AggArgs& a, AggKernel k, size_t smem, int sm_count, cudaStream_t s, cudaEvent_t start) {
     if (a.nrows <= 0) return cudaSuccess;
-    if (direct && !grouped && a.scalar_tma) {
-        cudaError_t e = cudaSuccess;
-        if (start) cudaEventRecord(start, s);
-        if (launch_count_where_tma(a, sm_count, s, &e)) { *kernel_name = "k_count_where_tma"; return e; }
-    }
-    if (direct) {
-        const size_t dsmem = grouped ? direct_smem_bytes(a.smem_keyw, a.n_smem_lanes, a.smem_cap_log2, a.direct.n_vals) + (a.lean_fx ? fx_ext_bytes(a.direct.n_vals, a.smem_cap_log2) : 0) : 0;
-        *kernel_name = grouped ? "k_agg_group_direct" : "k_agg_scalar_direct";
-        switch (a.direct.n_terms) {
-            case 0: return launch_direct_np0(a, a.direct.n_vals, sm_count, dsmem, s, grouped, start);
-            case 1: return launch_direct_np1(a, a.direct.n_vals, sm_count, dsmem, s, grouped, start);
-            default: return launch_direct_np2(a, a.direct.n_vals, sm_count, dsmem, s, grouped, start);
+    switch (k) {
+        case INTERP: {
+            if (smem > 48 * 1024) {
+                cudaError_t e = cudaFuncSetAttribute(k_agg_interp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+                if (e != cudaSuccess) return e;
+            }
+            int grid = occupancy_grid(k_agg_interp, smem, sm_count);
+            int64_t want = (a.nrows + 255) / 256;
+            if (want < grid) grid = (int)want;
+            if (start) cudaEventRecord(start, s);
+            k_agg_interp<<<grid, 256, smem, s>>>(a);
+            return cudaGetLastError();
         }
+        case COUNT_WHERE_TMA: return launch_count_where_tma(a, sm_count, s, start);
+        default:
+            switch (a.direct.n_terms) {
+                case 0: return launch_direct_np0(a, k, sm_count, smem, s, start);
+                case 1: return launch_direct_np1(a, k, sm_count, smem, s, start);
+                default: return launch_direct_np2(a, k, sm_count, smem, s, start);
+            }
     }
-    *kernel_name = "k_agg_interp";
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(k_agg_interp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-    }
-    int grid = occupancy_grid(k_agg_interp, smem, sm_count);
-    int64_t want = (a.nrows + 255) / 256;
-    if (want < grid) grid = (int)want;
-    if (start) cudaEventRecord(start, s);
-    k_agg_interp<<<grid, 256, smem, s>>>(a);
-    return cudaGetLastError();
 }
 
 // ---- FK -> PK fast path (see JoinFast in agg.h) ----

@@ -83,16 +83,15 @@ inline size_t wp_smem_bytes(int na, uint32_t gcap, int kt_log2, int warps) { ret
 // typed columns built from the aggregate's extracted images (input of the post fragment)
 struct PostCols { int32_t n; int32_t img[MAX_COLS]; int32_t stype[MAX_COLS]; uint8_t* values[MAX_COLS]; uint8_t* null_bytes[MAX_COLS]; };
 cudaError_t launch_images_to_columns(const uint64_t* outv, const uint8_t* outn, uint32_t out_cap, uint32_t n, const PostCols& pc, cudaStream_t s);
-size_t agg_smem_bytes(int smem_keyw, int n_smem_lanes, int cap_log2);
-// scalar_tma.cu: TMA-staged COUNT(*) WHERE int32 <cmp> c (experiment, option "scalar_tma"); false = not this kernel's shape
-bool launch_count_where_tma(const AggArgs& a, int sm_count, cudaStream_t s, cudaError_t* err);
-// `start` (optional) is recorded on `s` right before the kernel launch, after the launch setup
-cudaError_t launch_agg(const AggArgs& a, bool direct, int sm_count, cudaStream_t s, cudaEvent_t start, const char** kernel_name);
-cudaError_t launch_direct_np0(const AggArgs& a, int na, int sm_count, size_t smem, cudaStream_t s, bool grouped, cudaEvent_t start);
-cudaError_t launch_direct_np1(const AggArgs& a, int na, int sm_count, size_t smem, cudaStream_t s, bool grouped, cudaEvent_t start);
-cudaError_t launch_direct_np2(const AggArgs& a, int na, int sm_count, size_t smem, cudaStream_t s, bool grouped, cudaEvent_t start);
-size_t direct_smem_bytes(int smem_keyw, int n_smem_lanes, int cap_log2, int na);
-size_t fx_ext_bytes(int na, int cap_log2);
+enum AggKernel : int;   // agg_select.h: the kernel select_agg_launch chose for a batch
+// scalar_tma.cu: TMA-staged COUNT(*) WHERE int32 <cmp> c (the batch has the kernel's shape)
+cudaError_t launch_count_where_tma(const AggArgs& a, int sm_count, cudaStream_t s, cudaEvent_t start);
+// the aggregate kernel `k` over one batch; `smem`: its dynamic shared memory (AggSelection::smem).  `start` (optional) is recorded on `s`
+// right before the kernel launch, after the launch setup
+cudaError_t launch_agg(const AggArgs& a, AggKernel k, size_t smem, int sm_count, cudaStream_t s, cudaEvent_t start);
+cudaError_t launch_direct_np0(const AggArgs& a, AggKernel k, int sm_count, size_t smem, cudaStream_t s, cudaEvent_t start);
+cudaError_t launch_direct_np1(const AggArgs& a, AggKernel k, int sm_count, size_t smem, cudaStream_t s, cudaEvent_t start);
+cudaError_t launch_direct_np2(const AggArgs& a, AggKernel k, int sm_count, size_t smem, cudaStream_t s, cudaEvent_t start);
 cudaError_t launch_join_build(const DevCol& key, int from_prim, int cast_prim, int64_t nrows, uint64_t* keys, uint32_t* rows, uint32_t cap_mask, cudaStream_t s);
 // FK -> PK join fast path: unique build keys, looked up through a dense array (small key range) or a packed
 // (key32 << 32 | row) table; build-side columns are gathered to probe-row alignment

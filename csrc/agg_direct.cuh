@@ -21,6 +21,7 @@
 #include <mutex>
 #include <tuple>
 #include "agg_kernels.cuh"
+#include "agg_select.h"
 #include "fx.h"
 
 namespace bk {
@@ -1304,35 +1305,42 @@ static inline cudaError_t launch_persistent(K kernel, const AggArgs& a, size_t s
 }
 
 template <int NP, int NA>
-static inline cudaError_t launch_wp(const AggArgs& a, int sm_count, cudaStream_t s);   // agg_wp.cuh
+static inline cudaError_t launch_wp(const AggArgs& a, int sm_count, cudaStream_t s, cudaEvent_t start);   // agg_wp.cuh
 
+// the kernel select_agg_launch (agg_select.cpp) chose; exactly these instantiations of k_agg_group_lean exist
 template <int NP, int NA>
-static inline cudaError_t launch_direct(const AggArgs& a, int sm_count, size_t smem, cudaStream_t s, bool grouped, cudaEvent_t start) {
-    if (grouped && a.wp) { if (start) cudaEventRecord(start, s); return launch_wp<NP, NA>(a, sm_count, s); }
-    if (!grouped) return launch_persistent(k_agg_scalar_direct<NP, NA>, a, 0, sm_count, DIRECT_THREADS, s, start);
-    if (!a.lean) return launch_persistent(k_agg_group_direct<NP, NA>, a, smem, sm_count, DIRECT_THREADS, s, start);
+static inline cudaError_t launch_direct(const AggArgs& a, AggKernel k, int sm_count, size_t smem, cudaStream_t s, cudaEvent_t start) {
     constexpr int T = LEAN_THREADS;
-    // (one MM / NULLS instantiation serves batches with and without NULLs: without bitmaps the NULL masks are simply zero)
-    if (a.lean_mm) return launch_persistent(k_agg_group_lean<NP, NA, false, true, true>, a, smem, sm_count, T, s, start);
-    if (a.lean_nulls) return launch_persistent(k_agg_group_lean<NP, NA, false, true>, a, smem, sm_count, T, s, start);
-    if constexpr (NA >= 1) {   // double sums as fixed-point limbs (native 32-bit shared atomics)
-        if (a.lean_fx) return a.jp.mode ? launch_persistent(k_agg_group_lean<NP, NA, true, false, false, false, true>, a, smem, sm_count, T, s, start)
-                                        : launch_persistent(k_agg_group_lean<NP, NA, false, false, false, false, true>, a, smem, sm_count, T, s, start);
+    switch (k) {
+        case SCALAR_DIRECT: return launch_persistent(k_agg_scalar_direct<NP, NA>, a, 0, sm_count, DIRECT_THREADS, s, start);
+        case GROUP_DIRECT: return launch_persistent(k_agg_group_direct<NP, NA>, a, smem, sm_count, DIRECT_THREADS, s, start);
+        case WP: return launch_wp<NP, NA>(a, sm_count, s, start);
+        case LEAN: return launch_persistent(k_agg_group_lean<NP, NA, false>, a, smem, sm_count, T, s, start);
+        // (one MM / NULLS instantiation serves batches with and without NULLs: without bitmaps the NULL masks are simply zero)
+        case LEAN_MM: return launch_persistent(k_agg_group_lean<NP, NA, false, true, true>, a, smem, sm_count, T, s, start);
+        case LEAN_NULLS: return launch_persistent(k_agg_group_lean<NP, NA, false, true>, a, smem, sm_count, T, s, start);
+        case LEAN_JOIN: return launch_persistent(k_agg_group_lean<NP, NA, true>, a, smem, sm_count, T, s, start);
+        case LEAN_FX:   // double sums as fixed-point limbs (native 32-bit shared atomics)
+            if constexpr (NA >= 1) return launch_persistent(k_agg_group_lean<NP, NA, false, false, false, false, true>, a, smem, sm_count, T, s, start);
+            break;
+        case LEAN_FX_JOIN:
+            if constexpr (NA >= 1) return launch_persistent(k_agg_group_lean<NP, NA, true, false, false, false, true>, a, smem, sm_count, T, s, start);
+            break;
+        case LEAN_BANK:
+            if constexpr (NA <= 2) return launch_persistent(k_agg_group_lean<NP, NA, false, false, false, true>, a, smem, sm_count, T, s, start);
+            break;
+        default: break;
     }
-    if (a.jp.mode) return launch_persistent(k_agg_group_lean<NP, NA, true>, a, smem, sm_count, T, s, start);
-    if constexpr (NA <= 2) {
-        if (a.lean_bank) return launch_persistent(k_agg_group_lean<NP, NA, false, false, false, true>, a, smem, sm_count, T, s, start);
-    }
-    return launch_persistent(k_agg_group_lean<NP, NA, false>, a, smem, sm_count, T, s, start);
+    return cudaErrorInvalidValue;
 }
 template <int NP>
-static inline cudaError_t launch_direct_np(const AggArgs& a, int na, int sm_count, size_t smem, cudaStream_t s, bool grouped, cudaEvent_t start) {
-    switch (na) {
-        case 0: return launch_direct<NP, 0>(a, sm_count, smem, s, grouped, start);
-        case 1: return launch_direct<NP, 1>(a, sm_count, smem, s, grouped, start);
-        case 2: return launch_direct<NP, 2>(a, sm_count, smem, s, grouped, start);
-        case 3: return launch_direct<NP, 3>(a, sm_count, smem, s, grouped, start);
-        default: return launch_direct<NP, 4>(a, sm_count, smem, s, grouped, start);
+static inline cudaError_t launch_direct_np(const AggArgs& a, AggKernel k, int sm_count, size_t smem, cudaStream_t s, cudaEvent_t start) {
+    switch (a.direct.n_vals) {
+        case 0: return launch_direct<NP, 0>(a, k, sm_count, smem, s, start);
+        case 1: return launch_direct<NP, 1>(a, k, sm_count, smem, s, start);
+        case 2: return launch_direct<NP, 2>(a, k, sm_count, smem, s, start);
+        case 3: return launch_direct<NP, 3>(a, k, sm_count, smem, s, start);
+        default: return launch_direct<NP, 4>(a, k, sm_count, smem, s, start);
     }
 }
 

@@ -3,7 +3,7 @@
 #include "agg_wp.cuh"
 
 namespace bk {
-cudaError_t launch_direct_np1(const AggArgs& a, int na, int sm_count, size_t smem, cudaStream_t s, bool grouped, cudaEvent_t start) {
-    return launch_direct_np<1>(a, na, sm_count, smem, s, grouped, start);
+cudaError_t launch_direct_np1(const AggArgs& a, AggKernel k, int sm_count, size_t smem, cudaStream_t s, cudaEvent_t start) {
+    return launch_direct_np<1>(a, k, sm_count, smem, s, start);
 }
 }  // namespace bk

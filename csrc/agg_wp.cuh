@@ -443,37 +443,38 @@ __global__ void __maxnreg__(wp_regs(WARPS)) k_agg_group_wp(const __grid_constant
 }
 
 template <int NP, int NA, bool JOIN, bool F64, bool DENSE, int WARPS>
-static inline cudaError_t launch_wp_k(const AggArgs& a, int sm_count, cudaStream_t s) {
+static inline cudaError_t launch_wp_k(const AggArgs& a, int sm_count, cudaStream_t s, cudaEvent_t start) {
     const size_t smem = wp_smem_bytes(NA, (uint32_t)a.wp_gcap, a.wp_dense ? -1 : a.wp_kt_log2, WARPS);
     const int64_t want = ((a.nrows + 3) / 4 + WARPS * 32 - 1) / (WARPS * 32);
     const int grid = (int)(want < sm_count ? want : sm_count);   // persistent: one CTA per SM
     cudaError_t e = cudaFuncSetAttribute(k_agg_group_wp<NP, NA, JOIN, F64, DENSE, WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
+    if (start) cudaEventRecord(start, s);
     k_agg_group_wp<NP, NA, JOIN, F64, DENSE, WARPS><<<grid, WARPS * 32, smem, s>>>(a);
     return cudaGetLastError();
 }
 template <int NP, int NA, bool JOIN, bool F64, bool DENSE>
-static inline cudaError_t launch_wp_w(const AggArgs& a, int sm_count, cudaStream_t s) {
+static inline cudaError_t launch_wp_w(const AggArgs& a, int sm_count, cudaStream_t s, cudaEvent_t start) {
     if constexpr (NA <= 1) {   // (two value columns: 20 bytes per group and warp — more than eight tables never fit a useful capacity)
-        if (a.wp_warps == 16) return launch_wp_k<NP, NA, JOIN, F64, DENSE, 16>(a, sm_count, s);
-        if (a.wp_warps == 12) return launch_wp_k<NP, NA, JOIN, F64, DENSE, 12>(a, sm_count, s);
+        if (a.wp_warps == 16) return launch_wp_k<NP, NA, JOIN, F64, DENSE, 16>(a, sm_count, s, start);
+        if (a.wp_warps == 12) return launch_wp_k<NP, NA, JOIN, F64, DENSE, 12>(a, sm_count, s, start);
     }
-    return launch_wp_k<NP, NA, JOIN, F64, DENSE, 8>(a, sm_count, s);
+    return launch_wp_k<NP, NA, JOIN, F64, DENSE, 8>(a, sm_count, s, start);
 }
 template <int NP, int NA, bool JOIN, bool F64>
-static inline cudaError_t launch_wp_d(const AggArgs& a, int sm_count, cudaStream_t s) {
-    return a.wp_dense ? launch_wp_w<NP, NA, JOIN, F64, true>(a, sm_count, s) : launch_wp_w<NP, NA, JOIN, F64, false>(a, sm_count, s);
+static inline cudaError_t launch_wp_d(const AggArgs& a, int sm_count, cudaStream_t s, cudaEvent_t start) {
+    return a.wp_dense ? launch_wp_w<NP, NA, JOIN, F64, true>(a, sm_count, s, start) : launch_wp_w<NP, NA, JOIN, F64, false>(a, sm_count, s, start);
 }
 
 template <int NP, int NA>
-static inline cudaError_t launch_wp(const AggArgs& a, int sm_count, cudaStream_t s) {
+static inline cudaError_t launch_wp(const AggArgs& a, int sm_count, cudaStream_t s, cudaEvent_t start) {
     if constexpr (NA <= 2) {
         bool all_f64 = true;   // every value column feeds a double sum: the adds are compiled in (no per-entry type select)
         for (int v = 0; v < NA; v++) all_f64 = all_f64 && a.vops[v].op[0] == LN_ADD_F64;
-        if (a.jp.mode) return all_f64 ? launch_wp_d<NP, NA, true, true>(a, sm_count, s) : launch_wp_d<NP, NA, true, false>(a, sm_count, s);
-        return all_f64 ? launch_wp_d<NP, NA, false, true>(a, sm_count, s) : launch_wp_d<NP, NA, false, false>(a, sm_count, s);
+        if (a.jp.mode) return all_f64 ? launch_wp_d<NP, NA, true, true>(a, sm_count, s, start) : launch_wp_d<NP, NA, true, false>(a, sm_count, s, start);
+        return all_f64 ? launch_wp_d<NP, NA, false, true>(a, sm_count, s, start) : launch_wp_d<NP, NA, false, false>(a, sm_count, s, start);
     } else {
-        (void)a; (void)sm_count; (void)s;
+        (void)a; (void)sm_count; (void)s; (void)start;
         return cudaErrorInvalidValue;
     }
 }

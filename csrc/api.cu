@@ -267,22 +267,6 @@ static void learn_groups(bkgpu_plan* p) {
     if (p->h_fused) { const uint32_t g = *(const volatile uint32_t*)p->h_fused; if (g > p->known_groups) p->known_groups = g; }
 }
 
-// choose the shared-table capacity for this batch: >= 2x the groups seen so far, 2048 slots when
-// nothing is known yet, 0 (straight to the global table) when the groups cannot fit one CTA's 227 KB
-static int pick_smem_log2(bkgpu_plan* p, int n_smem_lanes, bool direct, int na) {
-    if (p->c.ap.n_keyw == 0) return 0;
-    const size_t budget = 220 * 1024;
-    auto bytes = [&](int log2) { return direct ? direct_smem_bytes(p->c.ap.n_keyw, n_smem_lanes, log2, na) : agg_smem_bytes(p->c.ap.n_keyw, n_smem_lanes, log2); };
-    if (p->smem_cap_log2 >= 0) { int l = p->smem_cap_log2; while (l > 0 && bytes(l) > budget) l--; return l; }
-    learn_groups(p);
-    uint32_t g = p->known_groups;
-    int log2 = 11;
-    while (((uint32_t)1 << log2) < 2 * g && log2 < 14) log2++;
-    while (log2 > 0 && bytes(log2) > budget) log2--;
-    if (((uint32_t)1 << log2) < g) return 0;  // would mostly miss: skip the shared table
-    return log2;
-}
-
 // device images of an extracted row: one per group expression, per aggregate its final value (+2 for an AVG blob)
 static int agg_n_img(const AggPlan& ap) {
     int n = ap.n_group;
@@ -312,151 +296,22 @@ static bool ensure_fused(bkgpu_plan* p) {
 }
 
 int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp) {
-    AggArgs a; memset(&a, 0, sizeof a);
-    a.plan = c.ap; a.prog = c.prog; a.direct = c.direct; a.gt = p->gt; a.rows_passed = p->d_rows_passed;
+    AggEnv env;
+    env.force_generic = p->force_generic; env.no_lean = p->no_lean; env.no_lean_nulls = p->no_lean_nulls; env.no_lean_mm = p->no_lean_mm;
+    env.lean_fx = p->lean_fx; env.fx_off = p->fx_off; env.lean_bank = p->lean_bank;
+    env.use_wp = p->use_wp; env.wp_warps = p->wp_warps; env.wp_kt_log2 = p->wp_kt_log2;
+    env.scalar_tma = p->scalar_tma; env.smem_cap_log2 = p->smem_cap_log2; env.join_pipeline = p->join.pipeline;
+    env.tail_launch = p->join.tail_launch;
+    env.multi_rank = p->nccl_comm && p->nranks > 1; env.has_post = p->c.post != nullptr;
+    if (c.ap.n_keyw > 0 && (p->smem_cap_log2 < 0 || p->use_wp)) learn_groups(p);   // (the shared and warp-private tables are sized from it)
+    env.known_groups = p->known_groups;
+    AggArgs a; AggSelection sel;
+    const int rc = select_agg_launch(c, cols, nrows, vec_ok, jp, env, a, sel);
+    if (rc == BKGPU_ENOMEM) return p->fail(rc, "lean kernel: shared table does not fit");
+    if (rc) return rc;
+    a.gt = p->gt; a.rows_passed = p->d_rows_passed;
     if (c.kind == PK_JOIN_AGG) a.join = join_args(p, p->join.tail_launch);
-    const bool direct = c.has_direct && vec_ok && !p->force_generic && c.kind == PK_AGG;   // (the join's fast-path plan is lowered as PK_AGG)
-    const int ncols = (int)c.cols.size();
-    if (direct) { for (size_t i = 0; i < c.direct_cols.size(); i++) a.cols[i] = cols[c.direct_cols[i]]; a.n_cols = (int)c.direct_cols.size(); }
-    else { for (int i = 0; i < ncols; i++) a.cols[i] = cols[i]; a.n_cols = ncols; }
-    // per-batch nullability -> which lanes need per-row work in the shared table
-    memset(a.smem_lane, 0xFF, sizeof a.smem_lane);
-    a.smem_lane[0] = 0; a.n_smem_lanes = 1; a.alias_mask = 0;
-    for (int k = 0; k < a.plan.n_agg; k++) {
-        AggSpec& s = a.plan.agg[k];
-        if (s.kind == AG_COUNT_STAR) continue;
-        bool nullable = c.arg_can_null[(size_t)k] || p->join.tail_launch;   // (the tail's probe-side columns are NULL on every row)
-        for (int i = 0; i < ncols; i++) if ((c.arg_cols_mask[(size_t)k] >> i) & 1) nullable = nullable || cols[i].validity != nullptr;
-        s.nullable = nullable ? 1 : 0;
-        if (s.cnt_lane && s.cnt_owner) {
-            if (nullable) { if (a.smem_lane[s.cnt_lane] == 0xFF) a.smem_lane[s.cnt_lane] = (uint8_t)a.n_smem_lanes++; }
-            else a.alias_mask |= 1u << s.cnt_lane;
-        }
-        if (s.kind != AG_COUNT && a.smem_lane[s.acc_lane] == 0xFF) a.smem_lane[s.acc_lane] = (uint8_t)a.n_smem_lanes++;
-    }
-    for (int l = 1; l < a.plan.n_lanes; l++) if (a.smem_lane[l] != 0xFF) a.alias_mask &= ~(1u << l);
-    a.smem_cap_log2 = pick_smem_log2(p, a.n_smem_lanes, direct, c.direct.n_vals);
-    a.smem_sentinel = direct && a.plan.n_keyw == 1 ? 1 : 0;
-    a.smem_keyw = a.plan.n_keyw;
-
-    if (direct) {  // per value column: the lane operations it feeds
-        memset(a.vops, 0, sizeof a.vops);
-        for (int v = 0; v < c.direct.n_vals; v++) { a.vops[v].cnt_smem = 0xFF; }
-        for (int k = 0; k < a.plan.n_agg; k++) {
-            const AggSpec& s = a.plan.agg[k];
-            if (s.kind == AG_COUNT_STAR) continue;
-            ValOps& vo = a.vops[c.direct.agg_val[k]];
-            vo.arg_class = s.arg_vclass;
-            if (s.cnt_lane && s.cnt_owner) { vo.cnt_glob = s.cnt_lane; vo.cnt_smem = s.nullable ? a.smem_lane[s.cnt_lane] : 0xFF; }
-            if (s.kind != AG_COUNT && s.acc_owner) {
-                const int n = vo.n_ops++;
-                vo.op[n] = a.plan.lane_op[s.acc_lane]; vo.lane_class[n] = s.vclass; vo.glob_lane[n] = s.acc_lane; vo.smem_lane[n] = a.smem_lane[s.acc_lane];
-            }
-        }
-    }
-    a.lean = 0;
-    // lean shape: one key word, or a 64-bit key whose second word only carries the (here unused) NULL flag
-    const bool lean_keyw = a.plan.n_keyw == 1 || (a.plan.n_keyw == 2 && a.plan.n_group == 1 && a.plan.key_bits[0] == 64 && a.plan.key_null_word[0] == 1);
-    if (direct && lean_keyw && a.smem_cap_log2 > 0 && !p->no_lean) {  // does this batch fit the lean kernel?
-        bool ok = true;
-        const int np = c.direct.n_terms, na = c.direct.n_vals;
-        bool any_valid = false;
-        for (int i = 0; i < a.n_cols; i++) if (a.cols[i].validity) any_valid = true;
-        if (a.cols[np].validity || (any_valid && (jp || p->no_lean_nulls))) ok = false;   // NULL keys (and NULLs under the fused probe) take the general kernel
-        for (int t = 0; t < np && ok; t++) {
-            const DirectTerm& tm = c.direct.term[t];
-            const int64_t cv = (int64_t)tm.cbits;
-            ok = a.cols[t].stype == ST_I32 && a.cols[t].prim == BK_INT32 && tm.vclass == VC_I64 && cv >= INT32_MIN && cv <= INT32_MAX;
-        }
-        const DevCol& kc = a.cols[np];
-        ok = ok && ((kc.stype == ST_I32 && kc.prim == BK_INT32) || (kc.stype == ST_U32 && kc.prim == BK_UINT32) || kc.stype == ST_I64 || kc.stype == ST_U64);
-        bool mm = false;   // some column feeds MIN / MAX or several lanes: the MM instantiation of the lean kernel
-        for (int v = 0; v < na && ok; v++) {
-            const DevCol& vc = a.cols[np + 1 + v];
-            const ValOps& vo = a.vops[v];
-            ok = (vc.stype == ST_F64 || vc.stype == ST_I64 || vc.stype == ST_U64) && vo.n_ops <= 3 && (vo.cnt_smem == 0xFF || vo.cnt_glob != 0);
-            const int col_class = vc.stype == ST_F64 ? VC_F64 : (vc.stype == ST_U64 ? VC_U64 : VC_I64);
-            for (int k = 0; k < vo.n_ops && ok; k++) {
-                const int op = vo.op[k];
-                if (op == LN_ADD_F64) ok = vc.stype == ST_F64 && vo.lane_class[k] == VC_F64;
-                else if (op == LN_ADD_I64) ok = vc.stype != ST_F64;
-                else { ok = vo.lane_class[k] == col_class && vo.arg_class == col_class; mm = true; }   // MIN / MAX in the column's own class
-            }
-            if (vo.n_ops != 1) mm = true;
-        }
-        if (mm && (jp || p->no_lean_mm)) ok = false;
-        a.lean = ok ? 1 : 0;
-        if (a.lean) {
-            a.smem_sentinel = 1; a.smem_keyw = 1; a.smem_paired = 1;
-            // lane placement for 128-bit shared CAS: ONE double sum shares a 16-byte word with the row count
-            // ({rows, sum}: a single atomic per row); otherwise double sums sit in pairs {sumA, sumB}
-            memset(a.smem_lane, 0xFF, sizeof a.smem_lane);
-            a.smem_lane[0] = 0;
-            int nf64 = 0;   // columns that feed exactly one double sum (they sit in {sumA, sumB} pairs)
-            for (int v = 0; v < na; v++) if (a.vops[v].n_ops == 1 && a.vops[v].op[0] == LN_ADD_F64) nf64++;
-            int next_f = nf64 == 1 ? 1 : 2, next_i = nf64 == 1 ? 2 : 2 + ((nf64 + 1) & ~1);
-            for (int v = 0; v < na; v++) {
-                ValOps& vo = a.vops[v];
-                for (int k = 0; k < vo.n_ops; k++) {
-                    const int sl = (vo.n_ops == 1 && vo.op[0] == LN_ADD_F64) ? next_f++ : next_i++;
-                    vo.smem_lane[k] = (uint8_t)sl; a.smem_lane[vo.glob_lane[k]] = (uint8_t)sl;
-                }
-            }
-            a.lean_mm = mm ? 1 : 0;
-            int next = std::max(next_f, next_i);
-            for (int v = 0; v < na; v++) {   // non-NULL counters of the value columns that carry NULLs in this batch
-                ValOps& vo = a.vops[v];
-                if (vo.cnt_smem == 0xFF) continue;
-                vo.cnt_smem = (uint8_t)next; a.smem_lane[vo.cnt_glob] = (uint8_t)next; next++;
-            }
-            a.lean_nulls = any_valid ? 1 : 0;
-            a.n_smem_lanes = (next + 1) & ~1;
-            if (a.n_smem_lanes < 2) a.n_smem_lanes = 2;
-            a.smem_cap_log2 = pick_smem_log2(p, a.n_smem_lanes, true, na);
-            if (a.smem_cap_log2 <= 0) { a.lean = 0; a.smem_paired = 0; return p->fail(BKGPU_ENOMEM, "lean kernel: shared table does not fit"); }
-            // FX: plain batches (no NULLs, no MIN / MAX) with at least one double sum, when the extension limbs fit beside table and queues
-            if (p->lean_fx && !p->fx_off && !p->lean_bank && !mm && !any_valid && nf64 >= 1 && nrows < ((int64_t)1 << 31)) {
-                const size_t base = direct_smem_bytes(a.smem_keyw, a.n_smem_lanes, a.smem_cap_log2, na);
-                if (base + fx_ext_bytes(na, a.smem_cap_log2) <= (size_t)224 * 1024) { a.lean_fx = 1; a.fx_ext_off = (uint32_t)base; }   // (227 KB per CTA less the kernel's 1 KB of static shared memory)
-            }
-
-        }
-    }
-    if (jp) { if (!a.lean) return 1; a.jp = *jp; a.jp_pipeline = p->join.pipeline; }
-    // warp-private tables (agg_wp.cuh): the plainest lean batches whose groups fit one table per warp.  The capacity follows the
-    // cardinality learned from earlier batches / runs of this plan; an unknown cardinality starts with the largest table.
-    a.scalar_tma = p->scalar_tma; a.lean_bank = p->lean_bank;
-    a.wp = 0;
-    if (a.lean && !a.lean_nulls && !a.lean_mm && p->use_wp && c.direct.n_vals <= 2) {
-        const int np = c.direct.n_terms, na = c.direct.n_vals;
-        const DevCol& kc = a.cols[np];
-        bool ok = kc.stype == ST_I32 || kc.stype == ST_U32;
-        for (int v = 0; v < na && ok; v++) ok = a.vops[v].n_ops == 1 && (a.vops[v].op[0] == LN_ADD_F64 || a.vops[v].op[0] == LN_ADD_I64);
-        learn_groups(p);
-        if (ok) {
-            const size_t budget = 226 * 1024;
-            const uint32_t g = p->known_groups;
-            int warps = 8;
-            if (na <= 1 && g) {   // one value column: the tables are small enough for 12 or 16 warps (three / four per scheduler)
-                const uint32_t gc = (g + 31) & ~31u;
-                int kl4 = 8; while ((1u << kl4) < 4 * gc) kl4++;
-                if (wp_smem_bytes(na, gc, kl4, 16) <= budget) warps = 16;
-                else if (wp_smem_bytes(na, gc, kl4, 12) <= budget) warps = 12;
-            }
-            if (p->wp_warps && (na <= 1 || p->wp_warps == 8)) warps = p->wp_warps;
-            uint32_t gcap = g ? ((g + 31) & ~31u) : 0;
-            auto fits = [&](uint32_t gc, int kl) { return wp_smem_bytes(na, gc, kl, warps) <= budget; };
-            auto kt_for = [&](uint32_t gc, int factor) { int kl = 8; while ((1u << kl) < (uint32_t)factor * gc) kl++; return kl; };
-            if (gcap == 0) { gcap = 32; while (fits(gcap + 32, kt_for(gcap + 32, 2))) gcap += 32; }   // unknown: the largest table that fits
-            int kl = p->wp_kt_log2 > 0 ? p->wp_kt_log2 : kt_for(gcap, 4);          // key table at <= 25 % load when it fits ...
-            if (!fits(gcap, kl)) kl = kt_for(gcap, 2);                              // ... else <= 50 %
-            if (fits(gcap, kl)) { a.wp = 1; a.wp_gcap = (int)gcap; a.wp_kt_log2 = kl; a.wp_warps = warps; a.wp_dense = 0; a.wp_dense_sub = 0; }
-        }
-    }
-    // a lean launch on one rank whose rows go straight to the host extracts its own result: any of them may be the request's last
-    if (direct && a.lean && !a.wp && a.plan.n_keyw > 0 && !(p->nccl_comm && p->nranks > 1) && !p->c.post && ensure_fused(p)) {
-        a.fused_out = p->d_fused; a.fused_cap = p->fused_cap;
-    }
+    if (sel.fused_ok && ensure_fused(p)) { a.fused_out = p->d_fused; a.fused_cap = p->fused_cap; }
     const int64_t kMax = (int64_t)1 << 30;  // rows per launch (32-bit counters inside a CTA)
     int64_t algo_bytes_per_row = 0;
     for (int i = 0; i < a.n_cols; i++) algo_bytes_per_row += storage_bytes(a.cols[i].stype);
@@ -464,13 +319,12 @@ int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64
         AggArgs b = a;
         b.nrows = std::min(kMax, nrows - off);
         for (int i = 0; i < b.n_cols; i++) b.cols[i] = col_at(a.cols[i], off);
-        const char* name = "";
         EventPair* ep = timer_begin(p, p->timed, b.nrows * algo_bytes_per_row, false);
-        cudaError_t e = launch_agg(b, direct, p->sm_count, p->stream, ep ? ep->a : nullptr, &name);
+        cudaError_t e = launch_agg(b, sel.kernel, sel.smem, p->sm_count, p->stream, ep ? ep->a : nullptr);
         timer_end(p, ep);
         p->fused_last = b.fused_out != nullptr;
         if (e != cudaSuccess) return p->cuda_fail(e, "launch_agg");
-        snprintf(p->stats.main_kernel_name, sizeof p->stats.main_kernel_name, "%s", b.wp && direct ? "k_agg_group_wp" : (b.lean && direct ? (b.lean_fx ? "k_agg_group_lean_fx" : "k_agg_group_lean") : name));
+        snprintf(p->stats.main_kernel_name, sizeof p->stats.main_kernel_name, "%s", agg_kernel_name(sel.kernel));
         p->stats.kernel_launches++;
     }
     return BKGPU_OK;

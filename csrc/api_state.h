@@ -9,7 +9,7 @@
 #include <string>
 #include <vector>
 #include "../include/bkgpu.h"
-#include "agg.h"
+#include "agg_select.h"
 #include "plan.h"
 #include "sort.h"
 

@@ -86,17 +86,12 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) k_count_where_tma(const uint8_
 }
 }  // namespace
 
-// COUNT(*) WHERE int32 column <cmp> c over one batch; false when the shape is not this kernel's (the caller takes the LDG kernel)
-bool launch_count_where_tma(const AggArgs& a, int sm_count, cudaStream_t s, cudaError_t* err) {
-    *err = cudaSuccess;
-    if (a.plan.n_keyw != 0 || a.direct.n_terms != 1 || a.direct.n_vals != 0 || a.plan.n_agg < 1) return false;
-    for (int k = 0; k < a.plan.n_agg; k++) if (a.plan.agg[k].kind != AG_COUNT_STAR) return false;
+// COUNT(*) WHERE int32 column <cmp> c over one batch (select_agg_launch has checked the shape)
+cudaError_t launch_count_where_tma(const AggArgs& a, int sm_count, cudaStream_t s, cudaEvent_t start) {
     const DevCol& c = a.cols[0];
     const DirectTerm& tm = a.direct.term[0];
-    const int64_t cv = (int64_t)tm.cbits;
-    if (c.stype != ST_I32 || c.prim != BK_INT32 || c.validity || tm.vclass != VC_I64 || cv < INT32_MIN || cv > INT32_MAX || ((uintptr_t)c.values & 15)) return false;
+    const int32_t ci = (int32_t)(int64_t)tm.cbits;
     uint32_t m, t, flip;
-    const int32_t ci = (int32_t)cv;
     switch (tm.cmp) {   // ((x ^ m) <u t) != flip
         case BK_FT_EQ: m = (uint32_t)ci; t = 1; flip = 0; break;
         case BK_FT_NE: m = (uint32_t)ci; t = 1; flip = 1; break;
@@ -106,14 +101,14 @@ bool launch_count_where_tma(const AggArgs& a, int sm_count, cudaStream_t s, cuda
         default: m = 0x80000000u; t = ci == INT32_MAX ? 0u : ((uint32_t)(ci + 1) ^ 0x80000000u); flip = ci != INT32_MAX; break;
     }
     const size_t smem = (size_t)TMA_STAGES * TMA_TILE_BYTES + 2 * TMA_STAGES * 8;
-    *err = cudaFuncSetAttribute(k_count_where_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (*err != cudaSuccess) return true;
+    cudaError_t e = cudaFuncSetAttribute(k_count_where_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
     const int64_t ntiles = (a.nrows * 4) / TMA_TILE_BYTES;
     int grid = 2 * sm_count;
     if (ntiles < grid) grid = (int)(ntiles > 0 ? ntiles : 1);
+    if (start) cudaEventRecord(start, s);
     k_count_where_tma<<<grid, TMA_THREADS, smem, s>>>((const uint8_t*)c.values, a.nrows, m, t, flip, (unsigned long long*)a.gt.lanes, (unsigned long long*)a.rows_passed);
-    *err = cudaGetLastError();
-    return true;
+    return cudaGetLastError();
 }
 
 }  // namespace bk
