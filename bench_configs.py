@@ -3,7 +3,7 @@
 device-resident synthetic columns (SURVEY.md §8d), CUDA events around reset+push+finish+get_next, one JSON line per
 config with rows/s and achieved GB/s on the config's algorithmic bytes.  The headline line is bench.py's;
 this script measures the side configs on their own (C6, the star join, also its kernels, a parity flag and the Acero time).
-usage: python bench_configs.py [c1] [c3] [c5] [c6] [--scale 0.1] [--steps 10]"""
+usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [--scale 0.1] [--steps 10]"""
 import argparse
 import ctypes
 import json
@@ -185,6 +185,68 @@ def c6(a):
     del ft, dims
 
 
+def c7(a):
+    """C7, GROUP BY date parts: SELECT year(d), month(d), COUNT(*), SUM(x) WHERE datediff(d, '1995-01-01') >= 0 GROUP BY year(d), month(d)
+    over 100M rows: a DATE column generated on the device (days 1992-01-01 .. 1998-12-31) and C2's value column.  Besides the step: the time
+    of k_agg_interp (torch.profiler), a parity flag against torch's year and month of the DATE image, and the same query grouped by two plain
+    INT32 columns holding that year and month (the comparison point)."""
+    from baikaldb_b200 import plan as P
+    n = int(100_000_000 * a.scale)
+    day = gen(n, (0, 1, T.INT32, 0, 1, 0, 2557, 1.0), 7).long()
+    # day number -> DATE image ((year * 13 + month) << 5 | day) with a torch civil-from-days over 1992-01-01 + day
+    z = day + 8035 + 719468                                  # days since 0000-03-01 (8035 = 1992-01-01 - 1970-01-01)
+    era = z // 146097; doe = z - era * 146097
+    yoe = (doe - doe // 1460 + doe // 36524 - doe // 146096) // 365
+    doy = doe - (365 * yoe + yoe // 4 - yoe // 100); mp = (5 * doy + 2) // 153
+    dd = doy - (153 * mp + 2) // 5 + 1; mm = torch.where(mp < 10, mp + 3, mp - 9); yy = yoe + era * 400 + (mm <= 2).long()
+    img = (((yy * 13 + mm) << 5) | dd).to(torch.int32)      # (uint32 image; every value < 2^31)
+    del day, z, era, doe, yoe, doy, mp, dd
+    x = gen(n, (0, 2, T.DOUBLE, 1, 3, 0, 0, 1.0), 2)
+    d = P.slot_ref(0, 1, T.DATE)
+    aggs = [P.agg_expr("count_star", 1, 3), P.agg_expr("sum", 1, 4, None, P.slot_ref(0, 2, T.DOUBLE))]
+    keys = [P.common("year", d), P.common("month", d)]
+    root = P.agg(P.where(P.scan(0), P.ge(P.common("datediff", d, P.str_lit("1995-01-01")), P.int_lit(0))), 1, keys, aggs)
+    plan = P.Plan(root, {0: [(1, T.DATE), (2, T.DOUBLE)], 1: [(1, T.UINT32), (2, T.UINT32), (3, T.INT64), (4, T.DOUBLE)]})
+    arr = cols_array([(0, 1, T.DATE), (0, 2, T.DOUBLE)], [img, x])
+    line, got = run("C7 year(d), month(d), COUNT(*), SUM(x) WHERE datediff(d, '1995-01-01') >= 0 GROUP BY year(d), month(d)", plan, [(arr, 2, n)], n, 12 * n,
+                    a.steps, a.warmup, collect=True, emit=False)
+    # parity: year and month straight from the image, the filter as the image's order (DATE images order like dates)
+    yr, mo = (img >> 5) // 13, (img >> 5) % 13
+    keep = img >= ((1995 * 13 + 1) << 5 | 1)
+    g = (yr * 13 + mo)[keep].long()
+    uk, inv = torch.unique(g, return_inverse=True)
+    want_sum = torch.zeros(len(uk), dtype=torch.float64, device="cuda").index_add_(0, inv, x[keep])
+    want_cnt = torch.bincount(inv, minlength=len(uk))
+    want = {(int(k) // 13, int(k) % 13): (float(s), int(c)) for k, s, c in zip(uk.tolist(), want_sum.tolist(), want_cnt.tolist())}
+    have = {(int(y), int(m)): (s, c) for y, m, s, c in zip(got["-1_0"], got["-1_1"], got["1_4"], got["1_3"])}
+    line["parity"] = set(have) == set(want) and all(have[k][1] == want[k][1] and abs(have[k][0] - want[k][0]) <= 1e-9 * max(1.0, abs(want[k][0])) for k in want)
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        run("profile", plan, [(arr, 2, n)], n, 12 * n, a.steps, 1, emit=False)
+        torch.cuda.synchronize()
+    line["k_agg_interp_ms_per_step"] = sum(getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) for e in prof.key_averages()
+                                           if "k_agg_interp" in e.key) / 1e3 / a.steps
+    # the comparison point: the same query grouped by two INT32 columns holding year and month, filtered on a third
+    specs = [(0, 1, T.INT32), (0, 2, T.INT32), (0, 3, T.INT32), (0, 4, T.DOUBLE)]
+    plain = [yr.to(torch.int32), mo.to(torch.int32), keep.to(torch.int32), x]
+    aggs2 = [P.agg_expr("count_star", 1, 3), P.agg_expr("sum", 1, 4, None, P.slot_ref(0, 4, T.DOUBLE))]
+    root2 = P.agg(P.where(P.scan(0), P.eq(P.slot_ref(0, 3, T.INT32), P.int_lit(1))), 1, [P.slot_ref(0, 1, T.INT32), P.slot_ref(0, 2, T.INT32)], aggs2)
+    plan2 = P.Plan(root2, {0: [(1, T.INT32), (2, T.INT32), (3, T.INT32), (4, T.DOUBLE)], 1: [(3, T.INT64), (4, T.DOUBLE)]})
+    cmp = run("C7 comparison: GROUP BY two INT32 columns", plan2, [(cols_array(specs, plain), 4, n)], n, 20 * n, a.steps, a.warmup, emit=False)
+    line["int32_keys_ms_per_step"] = cmp["ms_per_step"]
+    line["int32_keys_main_kernel"] = cmp["main_kernel"]
+    props = torch.cuda.get_device_properties(0)
+    line["device"] = props.name
+    try:
+        import subprocess
+        line["power_limit_w"] = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", "0"],
+                                               capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception:
+        line["power_limit_w"] = None
+    print(json.dumps(line), flush=True)
+    del img, x, plain
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("configs", nargs="*", default=["c1", "c3", "c5"])
@@ -238,6 +300,8 @@ def main():
         del ts
     if "c6" in a.configs:
         c6(a)
+    if "c7" in a.configs:
+        c7(a)
     if "c3" in a.configs:
         nf, nd = int(100_000_000 * a.scale), int(10_000_000 * a.scale)
         fs = [(0, 1, T.INT32, 0, 1, 0, nd, 1.0), (0, 2, T.DOUBLE, 1, 2, 0, 0, 1.0)]

@@ -68,6 +68,7 @@ enum Op : uint8_t {
     OP_IFNULL,       // pops [a, b]: a NULL ? b : a                           ifnull (internal_functions.cpp:2390-2395)
     OP_MATH,         // a = MathFn on a DOUBLE image, b = constant index (round: 10^bits)   internal_functions.cpp:52-99
     OP_MATH2,        // a = Math2Fn: pops [x, y] DOUBLE images, NULL if either is or outside the domain   internal_functions.cpp:114-127,234-317
+    OP_DATEFN,       // a = DateFn, b = mode / unit (datetime.h), c = arguments popped (1, or 2 for datediff); NULL in -> NULL
 };
 enum MathFn : uint8_t { MF_ABS = 0, MF_FLOOR = 1, MF_CEIL = 2, MF_ROUND = 3,
                         // one DOUBLE argument, NULL outside the domain (internal_functions.cpp:101-232); SIGN and BIT_COUNT leave an INT64 image

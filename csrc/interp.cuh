@@ -9,6 +9,9 @@ namespace bk {
 // generic path: the lowered expression program is interpreted per row (any predicate, computed
 // keys and arguments, multi-column keys).  Postfix bytecode, warp-uniform dispatch.
 // ------------------------------------------------------------------------------------------
+// OP_DATEFN's calendar code (datetime.h), out of line: one call site keeps it out of run_program's registers
+static __device__ __noinline__ uint64_t date_fn(uint32_t fn, uint32_t arg, uint64_t x, uint64_t x2) { return dt_date_fn((int)fn, (int)arg, x, x2); }
+
 // `brow`: row of the join's build side; LOAD_COL instructions with c == 1 read there (the joined row of
 // Joiner::construct_result_batch, src/exec/joiner.cpp:633-685, without materialising it)
 static __device__ __noinline__ void run_program(const Program& p, const DevCol* cols, int64_t row, uint64_t* out, uint32_t& out_null, int64_t brow = -1) {
@@ -183,6 +186,16 @@ static __device__ __noinline__ void run_program(const Program& p, const DevCol* 
                     default: r = y < x ? y : x; break;
                 }
                 st[sp - 1] = f64_bits(r);
+                nul = n ? (nul | (1u << (sp - 1))) : (nul & ~(1u << (sp - 1)));
+            } break;
+            case OP_DATEFN: {
+                sp -= in.c - 1;   // datediff's two arguments are at sp - 1 and sp
+                bool n = (nul >> (sp - 1)) & 1u;
+                if (in.c == 2) n = n || ((nul >> sp) & 1u);
+                if (!n) {
+                    st[sp - 1] = date_fn(in.a, in.b, st[sp - 1], st[sp]);
+                    n = st[sp - 1] == DT_FN_NULL;
+                }
                 nul = n ? (nul | (1u << (sp - 1))) : (nul & ~(1u << (sp - 1)));
             } break;
             case OP_OUT:

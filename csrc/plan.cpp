@@ -223,6 +223,51 @@ static int math2_fn(const std::string& n) {
     return -1;
 }
 
+// date-part and day-number functions (OP_DATEFN, datetime.h): name -> how the reference reads the argument and what it returns
+// (internal_functions.cpp; return_type_map, fn_manager.cpp:184-243)
+struct DateFnDef {
+    const char* name;
+    uint8_t fn;         // DateFn
+    int arg_prim;       // the argument's cast_to before the computation (datediff: DATE, then TIMESTAMP)
+    int ret;            // registered return type
+    bool via_text;      // an INT64 argument is first written out as text (`if (in.type == pb::INT64) in.cast_to(pb::STRING)`)
+    int extra;          // 0 = none, 1 = an optional mode after the value (week, yearweek), 2 = a unit before it (extract), 3 = a second value (datediff)
+};
+static const DateFnDef* date_fn_def(const std::string& n) {
+    static const DateFnDef t[] = {
+        {"year", DF_YEAR, BK_DATETIME, BK_UINT32, true, 0},            {"month", DF_MONTH, BK_DATETIME, BK_UINT32, true, 0},
+        {"day", DF_DAY, BK_DATETIME, BK_UINT32, true, 0},              {"dayofmonth", DF_DAY, BK_DATETIME, BK_UINT32, true, 0},
+        {"quarter", DF_QUARTER, BK_DATE, BK_INT32, false, 0},          {"hour", DF_HOUR, BK_TIME, BK_UINT32, false, 0},
+        {"minute", DF_MINUTE, BK_TIME, BK_INT32, false, 0},            {"second", DF_SECOND, BK_TIME, BK_INT32, false, 0},
+        {"dayofweek", DF_DAYOFWEEK, BK_DATETIME, BK_UINT32, true, 0},  {"weekday", DF_WEEKDAY, BK_DATETIME, BK_UINT32, true, 0},
+        {"dayofyear", DF_DAYOFYEAR, BK_DATETIME, BK_UINT32, true, 0},  {"week", DF_WEEK, BK_DATETIME, BK_UINT32, false, 1},
+        {"yearweek", DF_YEARWEEK, BK_DATETIME, BK_UINT32, false, 1},   {"weekofyear", DF_WEEKOFYEAR, BK_DATETIME, BK_UINT32, false, 0},
+        {"to_days", DF_TO_DAYS, BK_TIMESTAMP, BK_INT64, false, 0},     {"to_seconds", DF_TO_SECONDS, BK_TIMESTAMP, BK_INT64, false, 0},
+        {"unix_timestamp", DF_UNIX_TIMESTAMP, BK_TIMESTAMP, BK_INT64, true, 0},
+        {"datediff", DF_DATEDIFF, BK_DATE, BK_INT32, true, 3},         {"extract", DF_EXTRACT, BK_TIMESTAMP, BK_UINT32, false, 2},
+        {"date", DF_DATE, BK_DATETIME, BK_DATE, true, 0}};
+    for (auto& d : t) if (n == d.name) return &d;
+    return nullptr;
+}
+// date/time functions that stay on the CPU, and why
+static const char* date_fn_refusal(const std::string& n) {
+    static const std::pair<const char*, const char*> t[] = {
+        {"date_add", "its registered return type differs from the type of the value it returns"}, {"date_sub", nullptr}, {"adddate", nullptr},
+        {"subdate", nullptr}, {"timestampadd", nullptr}, {"timestampdiff", nullptr}, {"timediff", nullptr},
+        {"now", "it reads the current time"}, {"sysdate", nullptr}, {"curdate", nullptr}, {"current_date", nullptr}, {"curtime", nullptr},
+        {"current_time", nullptr}, {"current_timestamp", nullptr}, {"utc_timestamp", nullptr}, {"utc_date", nullptr}, {"utc_time", nullptr},
+        {"date_format", "it returns STRING"}, {"dayname", nullptr}, {"monthname", nullptr}, {"time_format", nullptr},
+        {"microsecond", "it is computed through the value's text"},
+        {"time_to_sec", "its registered and run-time result types differ in sign"}, {"sec_to_time", nullptr},
+        {"from_unixtime", "it is outside the GPU path"}, {"str_to_date", nullptr}, {"convert_tz", nullptr}};
+    const char* why = nullptr;
+    for (auto& p : t) {
+        if (p.second) why = p.second;   // (an entry without a reason shares the one above it)
+        if (n == p.first) return why;
+    }
+    return nullptr;
+}
+
 // A literal's value as the image of type `to` — ExprValue::cast_to (include/common/expr_value.h:502-611) on the host.
 // `via_text`: Literal::cast_to_col_type (include/expr/literal.h:204-210) — a numeric literal that meets a date/time type is first
 // written out in decimal and then read as a date ("20240131" -> 2024-01-31); a plain cast_to reinterprets the number as the image.
@@ -243,6 +288,37 @@ static bool fold_literal(Infer& in, HExpr& c, int to, bool via_text) {
         c.lit_bits = parse_literal(c.lit_str.c_str(), c.lit_str.size(), to);
     } else c.lit_bits = host_cast_prim(c.lit_bits, c.lit_prim, to);
     c.lit_prim = to;
+    return true;
+}
+
+// A date function's arguments: date/time expressions are cast on the device, literals are folded here to the type the function
+// casts them to; a non-literal number or string is refused (the reference would parse its text on every row).  extract's unit and
+// week / yearweek's mode must be literals: they become the instruction's operand.
+static bool infer_date_fn(Infer& in, HExpr& e, const DateFnDef& d) {
+    const char* nm = e.name.c_str();
+    const size_t n = e.ch.size(), v0 = d.extra == 2 ? 1 : 0, nv = d.extra == 3 ? 2 : 1;
+    if (d.fn == DF_UNIX_TIMESTAMP && n == 0) return in.fail(BKGPU_EUNSUPPORTED, "unix_timestamp() without an argument reads the current time: outside the GPU path");
+    if (d.extra == 1 ? (n < 1 || n > 2) : n != v0 + nv) return in.fail(BKGPU_EUNSUPPORTED, "%s() with %zu arguments is outside the GPU path", nm, n);
+    for (size_t i = v0; i < v0 + nv; i++) {
+        HExpr& c = e.ch[i];
+        if (c.col_type == BK_TIME && d.arg_prim != BK_TIME)
+            return in.fail(BKGPU_EUNSUPPORTED, "a TIME value as DATE/DATETIME/TIMESTAMP depends on the current date: outside the GPU path");
+        if (is_literal_node(c.node_type)) {
+            if (c.lit_null) continue;
+            if (!fold_literal(in, c, d.arg_prim, d.via_text && c.lit_prim == BK_INT64)) return false;
+            c.col_type = d.arg_prim;
+        } else if (!dt_is_family(c.col_type))
+            return in.fail(BKGPU_EUNSUPPORTED, "%s() over a non-literal argument of type %d: the reference parses its text on every row, outside the GPU path", nm, c.col_type);
+    }
+    if (d.extra == 1 && n == 2) {
+        const HExpr& m = e.ch[1];
+        if (!is_literal_node(m.node_type) || m.lit_null || !(is_int_t(m.lit_prim) || m.lit_prim == BK_BOOL))
+            return in.fail(BKGPU_EUNSUPPORTED, "%s() takes a literal integer mode", nm);
+    }
+    if (d.extra == 2 && !is_literal_node(e.ch[0].node_type)) return in.fail(BKGPU_EUNSUPPORTED, "extract() takes a literal unit");
+    e.arg_types.clear();   // named builtins cast nothing on the way in (complete_common_fn)
+    e.return_type = d.ret;
+    if (!e.col_type) e.col_type = d.ret;
     return true;
 }
 
@@ -319,6 +395,10 @@ static bool infer_expr(Infer& in, HExpr& e) {
         default: break;
     }
     // FUNCTION_CALL
+    if (e.fn_op == BK_FT_COMMON) {
+        if (const DateFnDef* d = date_fn_def(e.name)) return infer_date_fn(in, e, *d);
+        if (const char* why = date_fn_refusal(e.name)) return in.fail(BKGPU_EUNSUPPORTED, "%s() is outside the GPU path: %s", e.name.c_str(), why);
+    }
     if (!e.arg_types.empty() && e.return_type != BK_INVALID_TYPE) {  // completed by the db already
         if (!e.col_type) e.col_type = e.return_type;
     } else {
@@ -564,7 +644,46 @@ struct Lower {
     }
     // named builtins (FT_COMMON): arguments are NOT cast (arg_types stay empty), the result is cast to the node's col_type
     bool branch(const HExpr& c, int to, int& depth) { return expr(c, depth) && cast(c.col_type, to); }
+    // a date function: the argument, its cast_to (OP_CAST), then OP_DATEFN; a call over literals alone is computed here instead
+    bool date_fn(const HExpr& e, const DateFnDef& d, int& depth) {
+        const int d0 = depth;
+        const size_t v0 = d.extra == 2 ? 1 : 0, nv = d.extra == 3 ? 2 : 1;
+        int arg = 0;
+        bool is_null = false;   // an unknown extract unit or a NULL literal argument: the call is NULL
+        if (d.extra == 1) arg = e.ch.size() == 2 ? (int)((uint32_t)e.ch[1].lit_bits % 8) : DT_NO_MODE;   // get_numberic<uint32_t>() % 8
+        if (d.extra == 2) {                                                                                  // input[0].str_val == "year" ...
+            static const char* const units[] = {"year", "month", "day", "hour", "minute", "second"};
+            const HExpr& u = e.ch[0];
+            arg = -1;
+            for (int i = 0; i < 6; i++) if (!u.lit_null && u.lit_prim == BK_STRING && u.lit_str == units[i]) arg = i;
+            is_null = arg < 0;
+        }
+        bool all_literal = true;
+        uint64_t img[2] = {0, 0};
+        for (size_t i = 0; i < nv; i++) {
+            const HExpr& c = e.ch[v0 + i];
+            if (!is_literal_node(c.node_type)) { all_literal = false; continue; }
+            if (c.lit_null) is_null = true;
+            else img[i] = d.fn == DF_DATEDIFF ? host_cast_prim(c.lit_bits, BK_DATE, BK_TIMESTAMP) : c.lit_bits;   // (already the argument's type)
+        }
+        const int ct = e.col_type ? e.col_type : d.ret;
+        if (all_literal || is_null) {
+            const uint64_t v = is_null ? DT_FN_NULL : dt_date_fn(d.fn, arg, img[0], img[1]);
+            const int k = v == DT_FN_NULL ? add_const(0, true) : add_const(host_cast_prim(v, d.ret, ct), false);
+            if (k < 0) return false;
+            depth++;
+            return emit(OP_CONST, (uint8_t)k);
+        }
+        for (size_t i = 0; i < nv; i++) {
+            const HExpr& c = e.ch[v0 + i];
+            if (!expr(c, depth) || !cast(c.col_type, d.arg_prim)) return false;
+            if (d.fn == DF_DATEDIFF && !cast(BK_DATE, BK_TIMESTAMP)) return false;
+        }
+        depth = d0 + 1;
+        return emit(OP_DATEFN, d.fn, (uint8_t)arg, (uint8_t)nv) && cast(d.ret, ct);
+    }
     bool common_fn(const HExpr& e, int& depth) {
+        if (const DateFnDef* d = date_fn_def(e.name)) return date_fn(e, *d, depth);
         const int d0 = depth;
         const int ct = e.col_type;
         if (e.name == "if") {
@@ -638,6 +757,8 @@ static std::string expr_key(const HExpr& e) {  // structural identity, for lane 
     char buf[96];
     snprintf(buf, sizeof buf, "(%d:%d:%d_%d:%d:%llx", e.node_type, e.col_type, e.tuple_id, e.slot_id, e.fn_op, (unsigned long long)e.lit_bits);
     std::string s = buf;
+    if (e.node_type == BK_FUNCTION_CALL && e.fn_op == BK_FT_COMMON) s += ":" + e.name;   // year(d) is not month(d)
+    if (e.lit_prim == BK_STRING) s += ":'" + e.lit_str + "'";                            // nor is extract('year', d) extract('month', d)
     for (auto& c : e.ch) s += expr_key(c);
     return s + ")";
 }
@@ -652,6 +773,10 @@ static bool expr_makes_null(const HExpr& e) {
     if (e.node_type == BK_IS_NULL_PREDICATE || e.node_type == BK_IS_TRUE_PREDICATE) return false;
     if (e.node_type == BK_FUNCTION_CALL && (e.fn_op == BK_FT_DIVIDES || e.fn_op == BK_FT_MOD)) return true;
     if (e.node_type == BK_FUNCTION_CALL && e.fn_op == BK_FT_COMMON && e.name == "case_when" && e.ch.size() % 2 == 0) return true;
+    if (e.node_type == BK_FUNCTION_CALL && e.fn_op == BK_FT_COMMON)
+        if (const DateFnDef* d = date_fn_def(e.name))   // NULL for a date boost rejects, and for an unknown extract unit
+            if (d->fn == DF_DAYOFWEEK || d->fn == DF_WEEKDAY || d->fn == DF_DAYOFYEAR || d->fn == DF_WEEK || d->fn == DF_YEARWEEK ||
+                d->fn == DF_WEEKOFYEAR || d->fn == DF_EXTRACT) return true;
     if (e.node_type == BK_IN_PREDICATE) for (size_t i = 1; i < e.ch.size(); i++) if (e.ch[i].lit_null) return true;
     for (auto& c : e.ch) if (expr_makes_null(c)) return true;
     return false;
@@ -924,8 +1049,8 @@ static bool lower_agg(Infer& in, Compiled& out, const HNode& agg, const std::vec
 // ---------------------------------------------------------------- explain
 static const char* op_name(int op) {
     static const char* n[] = {"END", "LOAD_COL", "CONST", "CAST", "CMP", "ARITH", "DIV_F64", "MOD", "BIT", "BIT_NOT", "NEG",
-                              "LOGIC_NOT", "AND", "OR", "XOR", "NOT3", "IS_NULL", "IS_TRUE", "IN", "OUT", "SELECT", "IFNULL", "MATH", "MATH2"};
-    return op >= 0 && op <= OP_MATH2 ? n[op] : "?";
+                              "LOGIC_NOT", "AND", "OR", "XOR", "NOT3", "IS_NULL", "IS_TRUE", "IN", "OUT", "SELECT", "IFNULL", "MATH", "MATH2", "DATEFN"};
+    return op >= 0 && op <= OP_DATEFN ? n[op] : "?";
 }
 static void explain(Compiled& c) {
     char buf[256];
