@@ -30,6 +30,7 @@ class PlanNodeType(IntEnum):  # proto/plan.proto:9-53
     HAVING_FILTER_NODE = 13
     PACKET_NODE = 14
     SELECT_MANAGER_NODE = 25
+    WINDOW_NODE = 42
 
 
 class ExprNodeType(IntEnum):  # proto/expr.proto:6-37
@@ -54,6 +55,7 @@ class ExprNodeType(IntEnum):  # proto/expr.proto:6-37
     TIME_LITERAL = 20
     IS_TRUE_PREDICATE = 19
     ROW_EXPR = 22
+    WINDOW_EXPR = 30
 
 
 class PrimitiveType(IntEnum):  # proto/common.proto:46-72
@@ -118,6 +120,17 @@ class JoinType(IntEnum):  # proto/plan.proto:218-226
     SEMI_JOIN = 4
     ANTI_SEMI_JOIN = 5
     FULL_JOIN = 6
+
+
+class FrameType(IntEnum):  # proto/plan.proto:427-430
+    ROWS = 0
+    RANGE = 1
+
+
+class BoundType(IntEnum):  # proto/plan.proto:432-436
+    PRECEDING = 0
+    FOLLOWING = 1
+    CURRENT_ROW = 2
 
 
 T = PrimitiveType
@@ -207,6 +220,10 @@ class Expr:
             out.w(self.tuple_id)
             out.w(self.final_slot_id)
             out.w(self.intermediate_slot_id)
+        elif nt == ExprNodeType.WINDOW_EXPR:
+            out.s(self.name)
+            out.w(self.tuple_id)
+            out.w(self.slot_id)
         else:
             out.w(self.fn_op)
             out.s(self.name)
@@ -338,6 +355,42 @@ def agg_expr(name: str, agg_tuple_id: int, final_slot_id: int, intermediate_slot
                 final_slot_id=final_slot_id, intermediate_slot_id=inter)
 
 
+def window_expr(name: str, tuple_id: int, slot_id: int, *children: Expr) -> Expr:
+    """WINDOW_EXPR node: fn.name in {count_star, count, sum, avg, min, max, row_number, rank, dense_rank, percent_rank, cume_dist,
+    ntile, lead, lag, first_value, last_value, nth_value} (src/expr/window_fn_call.cpp:20-38); the result lands in slot
+    ``tuple_id``_``slot_id`` (DeriveExprNode)."""
+    return Expr(ExprNodeType.WINDOW_EXPR, 0, list(children), name=name, tuple_id=tuple_id, slot_id=slot_id)
+
+
+@dataclass
+class FrameBound:  # pb::FrameBound
+    bound_type: int
+    is_unbounded: bool = False
+    expr: Optional[Expr] = None
+
+
+@dataclass
+class WindowFrame:  # pb::WindowFrame
+    frame_type: int
+    start: FrameBound
+    end: FrameBound
+
+
+def bound(kind: str, n: Optional[int] = None) -> FrameBound:
+    """``kind``: "unbounded preceding", "preceding", "current row", "following" or "unbounded following"; ``n``: the offset
+    of "preceding" / "following" (an INT_LITERAL)."""
+    k = kind.lower()
+    if k == "current row":
+        return FrameBound(BoundType.CURRENT_ROW)
+    unb = k.startswith("unbounded ")
+    bt = BoundType.PRECEDING if k.endswith("preceding") else BoundType.FOLLOWING
+    return FrameBound(bt, unb, None if unb or n is None else int_lit(n))
+
+
+def frame(frame_type: int, start: FrameBound, end: FrameBound) -> WindowFrame:
+    return WindowFrame(int(frame_type), start, end)
+
+
 @dataclass
 class PlanNode:
     node_type: int
@@ -354,6 +407,9 @@ class PlanNode:
     is_null_first: List[bool] = field(default_factory=list)
     join_type: int = JoinType.INNER_JOIN
     offset: int = 0
+    window_fns: List[Expr] = field(default_factory=list)
+    partition_exprs: List[Expr] = field(default_factory=list)
+    frame: Optional[WindowFrame] = None
 
     def count(self) -> int:
         return 1 + sum(c.count() for c in self.children)
@@ -394,6 +450,26 @@ class PlanNode:
             out.w64(self.offset)
         elif nt in (PlanNodeType.PACKET_NODE, PlanNodeType.SELECT_MANAGER_NODE):
             pass
+        elif nt == PlanNodeType.WINDOW_NODE:
+            out.w(len(self.window_fns))
+            for e in self.window_fns:
+                e.emit(out)
+            out.w(len(self.partition_exprs))
+            for e in self.partition_exprs:
+                e.emit(out)
+            out.w(len(self.order_exprs))
+            for e, a in zip(self.order_exprs, self.is_asc):
+                e.emit(out)
+                out.w(1 if a else 0)
+            out.w(1 if self.frame is not None else 0)
+            if self.frame is not None:
+                out.w(self.frame.frame_type)
+                for b in (self.frame.start, self.frame.end):
+                    out.w(b.bound_type)
+                    out.w(1 if b.is_unbounded else 0)
+                    out.w(1 if b.expr is not None else 0)
+                    if b.expr is not None:
+                        b.expr.emit(out)
         else:
             raise ValueError(f"plan node type {nt} is outside the GPU path")
         for c in self.children:
@@ -431,6 +507,25 @@ def join(outer: PlanNode, inner: PlanNode, conditions: Sequence[Expr],
 
 def limit(child: PlanNode, n: int, offset: int = 0) -> PlanNode:
     return PlanNode(PlanNodeType.LIMIT_NODE, [child], limit=n, offset=offset)
+
+
+def window(child: PlanNode, func_exprs: Sequence[Expr], partition_exprs: Sequence[Expr] = (), order_exprs: Sequence[Expr] = (),
+           is_asc: Sequence[bool] = (), window_frame: Optional[WindowFrame] = None, limit: int = -1) -> PlanNode:
+    """WINDOW_NODE: the order part of the spec only (the planner strips the partition expressions from it,
+    select_planner.cpp:727-737)."""
+    return PlanNode(PlanNodeType.WINDOW_NODE, [child], window_fns=list(func_exprs), partition_exprs=list(partition_exprs),
+                    order_exprs=list(order_exprs), is_asc=[bool(a) for a in is_asc], frame=window_frame, limit=limit)
+
+
+def window_stage(child: PlanNode, func_exprs: Sequence[Expr], partition_exprs: Sequence[Expr] = (), order_exprs: Sequence[Expr] = (),
+                 is_asc: Optional[Sequence[bool]] = None, window_frame: Optional[WindowFrame] = None, tuple_id: int = -1) -> PlanNode:
+    """WINDOW -> SORT as the planner emits them (select_planner.cpp:705-760): the SORT orders by the partition expressions
+    (ascending) followed by the order expressions, with is_null_first = is_asc."""
+    asc = [True] * len(order_exprs) if is_asc is None else [bool(a) for a in is_asc]
+    keys = list(partition_exprs) + list(order_exprs)
+    sort_asc = [True] * len(partition_exprs) + asc
+    s = sort(child, keys, sort_asc, tuple_id=tuple_id)
+    return window(s, func_exprs, partition_exprs, order_exprs, asc, window_frame)
 
 
 def packet(child: PlanNode) -> PlanNode:

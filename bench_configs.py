@@ -3,7 +3,7 @@
 device-resident synthetic columns (SURVEY.md §8d), CUDA events around reset+push+finish+get_next, one JSON line per
 config with rows/s and achieved GB/s on the config's algorithmic bytes.  The headline line is bench.py's;
 this script measures the side configs on their own (C6, the star join, also its kernels, a parity flag and the Acero time).
-usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [--scale 0.1] [--steps 10]"""
+usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [--scale 0.1] [--steps 10]"""
 import argparse
 import ctypes
 import json
@@ -247,6 +247,75 @@ def c7(a):
     del img, x, plain
 
 
+def c8(a):
+    """C8, window functions: SELECT k, v, ROW_NUMBER(), RANK(), SUM(x) (running), LAG(x) OVER (PARTITION BY k ORDER BY v) WHERE v < 2^30
+    over 100M device-resident rows in 1000 partitions.  Besides the step: the window stage's kernel time (CUDA events inside the library,
+    the sort excluded), the time of the same radix sort run as ORDER BY k, v, the window stage's bytes and share of HBM, a parity flag
+    against torch on a 1M-row slice, and the row oracle's time on a 20k-row slice scaled to the full table (labelled as such)."""
+    import time
+    from baikaldb_b200 import plan as P
+    from tests import window_oracle
+    n = int(100_000_000 * a.scale)
+    specs = [(0, 1, T.INT32, 0, 1, 0, 1000, 1.0), (0, 2, T.INT32, 0, 2, 0, 1 << 31, 1.0), (0, 3, T.DOUBLE, 1, 3, 0, 0, 1.0)]
+    ts = [gen(n, sp, 8) for sp in specs]
+    tup = {0: [(1, T.INT32), (2, T.INT32), (3, T.DOUBLE)], 1: [(1, T.INT64), (2, T.INT64), (3, T.DOUBLE), (4, T.DOUBLE)]}
+    k, v, x = (P.slot_ref(0, s, t) for s, t in tup[0])
+    filt = P.where(P.scan(0), P.lt(v, P.int_lit(1 << 30)))
+    ranked = P.window_stage(filt, [P.window_expr("row_number", 1, 1), P.window_expr("rank", 1, 2), P.window_expr("lag", 1, 4, x)], [k], [v])
+    running = P.frame(P.FrameType.RANGE, P.bound("unbounded preceding"), P.bound("current row"))
+    plan = P.Plan(P.window_stage(ranked, [P.window_expr("sum", 1, 3, x)], [k], [v], window_frame=running), tup)
+    kept = int((ts[1] < (1 << 30)).sum())
+    # window stage bytes (sort excluded): 3 expressions evaluated (4 B row id + 8 B image + 1 B null, and the column read), flags, four
+    # index scans (2 passes of 1 + 8 B), one value scan (2 passes of 9 B + 16 B out), four functions (4 x 8 B bounds + inputs + 9 B out)
+    wbytes = kept * (3 * (4 + 13 + 6) + 2 * 13 + 2 + 4 * 18 + 34 + 4 * (32 + 4 + 9 + 9) + 16)
+    line = run("C8 window: ROW_NUMBER, RANK, running SUM, LAG OVER (PARTITION BY k ORDER BY v), 1000 partitions", plan,
+               [(cols_array(specs, ts), 3, n)], n, wbytes, max(1, a.steps // 5), 1, emit=False)
+    sort_plan = P.Plan(P.sort(filt, [k, v], [True, True], tuple_id=0), {0: tup[0]})
+    sline = run("the same sort as ORDER BY k, v", sort_plan, [(cols_array(specs, ts), 3, n)], n, 0, max(1, a.steps // 5), 1, emit=False)
+    line["window_stage_kernel_ms"] = line.pop("main_kernel_ms_per_step")
+    line["window_stage_bytes"] = wbytes
+    line["window_stage_frac_of_hbm"] = wbytes / (line["window_stage_kernel_ms"] / 1e3) / 1e9 / PEAK if line["window_stage_kernel_ms"] > 0 else None
+    line["sort_ms_as_order_by_k_v"] = sline["main_kernel_ms_per_step"]
+    # parity on a 1M-row slice: row_number from the segment starts, rank from the peer starts, a per-segment cumsum, lag
+    m = min(n, 1_000_000)
+    sl = [t[:m].contiguous() for t in ts]
+    lline, got = run("parity slice", plan, [(cols_array(specs, sl), 3, m)], m, 0, 1, 0, collect=True, emit=False)
+    kk, vv, xx = (t.cpu().numpy() for t in sl)
+    keep = vv < (1 << 30)
+    kk, vv, xx = kk[keep], vv[keep], xx[keep]
+    o = np.lexsort((vv, kk))
+    kk, vv, xx = kk[o], vv[o], xx[o]
+    tk, tv, tx = (torch.from_numpy(q).cuda() for q in (kk.astype(np.int64), vv.astype(np.int64), xx))
+    idx = torch.arange(len(tk), device="cuda")
+    pstart = torch.ones_like(tk, dtype=torch.bool); pstart[1:] = tk[1:] != tk[:-1]
+    qstart = pstart.clone(); qstart[1:] |= tv[1:] != tv[:-1]
+    ps = torch.cummax(torch.where(pstart, idx, torch.zeros_like(idx)), 0).values
+    qs = torch.cummax(torch.where(qstart, idx, torch.zeros_like(idx)), 0).values
+    rn, rk = idx - ps + 1, qs - ps + 1
+    cs = torch.cumsum(tx, 0); base = torch.where(ps > 0, cs[(ps - 1).clamp(min=0)], torch.zeros_like(cs)); run_sum = cs - base
+    last = torch.ones_like(pstart); last[:-1] = qstart[1:]
+    qe = torch.flip(torch.cummin(torch.flip(torch.where(last, idx, torch.full_like(idx, len(idx))), [0]), 0).values, [0])
+    want_sum = run_sum[qe].cpu().numpy()
+    g = {name: np.array(vals[:len(kk)]) for name, vals in got.items()}   # (the collected step's rows; the timed step appends a copy)
+    ok = (len(got["1_1"]) >= len(kk) and np.array_equal(g["1_1"], rn.cpu().numpy()) and np.array_equal(g["1_2"], rk.cpu().numpy())
+          and np.allclose(g["1_3"], want_sum, rtol=1e-9, atol=1e-6) and np.array_equal(g["0_2"], vv))
+    line["parity_1M_slice_vs_torch"] = bool(ok)
+    # the row oracle on a 20k-row slice, scaled linearly to the full table (its frame loop is quadratic per partition: a lower bound)
+    q = 20_000
+    qc = [make_column(0, s, t, ts[i][:q].cpu().numpy()) for i, (s, t) in enumerate(tup[0])]
+    t0 = time.time(); window_oracle.execute(plan, qc); dt = time.time() - t0
+    line["row_oracle_20k_rows_s"] = dt
+    line["row_oracle_scaled_to_full_table_s (linear extrapolation, a lower bound)"] = dt * n / q
+    line["gpu"] = torch.cuda.get_device_name(0)
+    try:
+        import subprocess
+        line["power_limit"] = subprocess.check_output(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"], text=True).split("\n")[0].strip()
+    except Exception:
+        line["power_limit"] = None
+    print(json.dumps(line), flush=True)
+    del ts
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("configs", nargs="*", default=["c1", "c3", "c5"])
@@ -302,6 +371,8 @@ def main():
         c6(a)
     if "c7" in a.configs:
         c7(a)
+    if "c8" in a.configs:
+        c8(a)
     if "c3" in a.configs:
         nf, nd = int(100_000_000 * a.scale), int(10_000_000 * a.scale)
         fs = [(0, 1, T.INT32, 0, 1, 0, nd, 1.0), (0, 2, T.DOUBLE, 1, 2, 0, 0, 1.0)]

@@ -253,7 +253,8 @@ extern "C" int bkgpu_open(bkgpu_plan* p) {
     p->blocking_wait = p->blocking_sync >= 0 ? p->blocking_sync != 0 : (p->nranks > 1 && cpu_budget() < 4 * p->nranks);
     int rc = BKGPU_OK;
     if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) rc = alloc_group_table(p);
-    if (!rc && (p->c.kind == PK_SORT || p->c.kind == PK_FILTER)) rc = sort_check(p, sort_open(p->c, p->device, p->stream, p->region_base, &p->sort, p->last_error));
+    if (!rc && (p->c.kind == PK_SORT || p->c.kind == PK_FILTER || p->c.kind == PK_WINDOW))   // (a window retains its rows like a full sort)
+        rc = sort_check(p, sort_open(p->c, p->device, p->stream, p->region_base, &p->sort, p->last_error));
     if (!rc && p->c.post) rc = sort_check(p, sort_open(*p->c.post, p->device, p->stream, 0, &p->post_sort, p->last_error));
     if (rc) return rc;
     p->state = S_OPEN;
@@ -596,7 +597,7 @@ static int bkgpu_push_impl(bkgpu_plan* p, const bkgpu_column* cols, int ncols, i
             return BKGPU_OK;
         }
         case PK_JOIN_AGG: case PK_JOIN: case PK_STAR_AGG: return join_push(p, cols, ncols, nrows, on_device);
-        case PK_SORT: case PK_FILTER: return feed(p, p->c.cols, cols, ncols, nrows, on_device, sort_batch);
+        case PK_SORT: case PK_FILTER: case PK_WINDOW: return feed(p, p->c.cols, cols, ncols, nrows, on_device, sort_batch);
         default: return p->fail(BKGPU_EUNSUPPORTED, "plan kind %d has no push path yet", p->c.kind);
     }
 }
@@ -962,6 +963,12 @@ static int bkgpu_finish_impl(bkgpu_plan* p) {
         case PK_SORT: case PK_FILTER: {
             std::vector<SortOutCol> cols; int64_t rows = 0;
             if ((rc = sort_check(p, sort_finish(p->sort, p->nccl_comm, p->nranks, p->stream, &p->stats, cols, &rows, p->last_error)))) break;
+            set_result(p, cols, rows, nullptr);
+        } break;
+        case PK_WINDOW: {   // the retained rows through the window stages (window.cu), then the query's ORDER BY when there is one
+            if (p->nccl_comm && p->nranks > 1) { rc = p->fail(BKGPU_EUNSUPPORTED, "a window fragment runs on one GPU: multi-GPU merge is implemented for ORDER BY ... LIMIT (top-k) and aggregates"); break; }
+            std::vector<SortOutCol> cols; int64_t rows = 0;
+            if ((rc = sort_check(p, window_finish(p->c, p->sort, p->post_sort, p->stream, &p->stats, cols, &rows, p->last_error)))) break;
             set_result(p, cols, rows, nullptr);
         } break;
         default: rc = p->fail(BKGPU_EUNSUPPORTED, "plan kind %d cannot finish", p->c.kind);

@@ -12,6 +12,7 @@
 #include "agg_select.h"
 #include "plan.h"
 #include "sort.h"
+#include "window.h"
 
 using namespace bk;
 

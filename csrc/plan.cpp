@@ -131,6 +131,7 @@ static void parse_enode(Reader& r, HExpr& e, int& remaining, int depth) {
             // into the GROUP BY of the aggregate below (select_planner.cpp:640-667), so each distinct value arrives once
             if (e.name == "count_distinct" || e.name == "sum_distinct" || e.name == "avg_distinct") { e.distinct = true; e.name.resize(e.name.size() - 9); }
             break;
+        case BK_WINDOW_EXPR: e.name = r.rdstr(); e.tuple_id = r.rd(); e.slot_id = r.rd(); break;   // WindowFnCall::init (window_fn_call.cpp:19-63)
         case BK_FUNCTION_CALL: case BK_IS_NULL_PREDICATE: case BK_IN_PREDICATE: case BK_NOT_PREDICATE:
         case BK_AND_PREDICATE: case BK_OR_PREDICATE: case BK_XOR_PREDICATE: case BK_IS_TRUE_PREDICATE: {
             e.fn_op = r.rd(); e.name = r.rdstr();
@@ -153,7 +154,8 @@ static void parse_expr(Reader& r, HExpr& e) {
     if (!r.fail && n != 0) r.bad("expr node count mismatch");
 }
 static void parse_node(Reader& r, HNode& nd, int& remaining, int depth) {
-    if (remaining <= 0 || depth > 32) { r.bad("plan node list does not match its node count"); return; }
+    // (depth: a fragment has at most 64 nodes, so a chain of WINDOW -> SORT pairs — one per window function — nests that deep)
+    if (remaining <= 0 || depth > 64) { r.bad("plan node list does not match its node count"); return; }
     remaining--;
     nd.node_type = r.rd();
     int nch = r.rd();
@@ -181,6 +183,21 @@ static void parse_node(Reader& r, HNode& nd, int& remaining, int depth) {
         case BK_JOIN_NODE: nd.join_type = r.rd(); exprs(nd.conjuncts); break;
         case BK_LIMIT_NODE: nd.offset = r.rd64(); break;
         case BK_PACKET_NODE: case BK_SELECT_MANAGER_NODE: break;
+        case BK_WINDOW_NODE: {   // pb::WindowNode: func_exprs, window_spec {partition_exprs, order_exprs, is_asc, window_frame}
+            exprs(nd.agg_fns); exprs(nd.group_exprs);
+            int n = r.rd();
+            if (n < 0 || n > 64) { r.bad("bad order expr count"); return; }
+            nd.order_exprs.resize((size_t)n);
+            for (int i = 0; i < n && !r.fail; i++) { parse_expr(r, nd.order_exprs[(size_t)i]); nd.is_asc.push_back(r.rd()); }
+            nd.has_frame = r.rd() != 0;
+            if (nd.has_frame) {
+                nd.frame_type = r.rd();
+                for (HFrameBound* b : {&nd.frame_start, &nd.frame_end}) {
+                    b->type = r.rd(); b->unbounded = r.rd() != 0; b->has_expr = r.rd() != 0;
+                    if (b->has_expr && !r.fail) parse_expr(r, b->expr);
+                }
+            }
+        } break;
         default: r.bad("plan node type outside the GPU path"); return;
     }
     if (nch < 0 || nch > 2) { r.bad("bad plan num_children"); return; }
@@ -359,6 +376,20 @@ static bool infer_expr(Infer& in, HExpr& e) {
             } else return in.fail(BKGPU_EUNSUPPORTED, "aggregate '%s' is outside the GPU path", e.name.c_str());
             if (e.name != "count_star" && e.name != "count" && !e.ch.empty() && ct == BK_STRING)
                 return in.fail(BKGPU_EUNSUPPORTED, "%s over a STRING argument is outside the GPU path", e.name.c_str());
+            return true;
+        }
+        case BK_WINDOW_EXPR: {   // WindowFnCall::type_inferer (window_fn_call.cpp:206-285)
+            const int ct = e.ch.empty() ? BK_INVALID_TYPE : e.ch[0].col_type;
+            const std::string& n = e.name;
+            if (n == "count_star" || n == "count" || n == "row_number" || n == "rank" || n == "dense_rank" || n == "ntile") e.col_type = BK_INT64;
+            else if (n == "avg" || n == "percent_rank" || n == "cume_dist") e.col_type = BK_DOUBLE;
+            else if (n == "sum") {
+                if (e.ch.empty()) return in.fail(BKGPU_EINVAL, "window sum() without an argument");
+                e.col_type = is_double_t(ct) || ct == BK_STRING ? BK_DOUBLE : BK_INT64;
+            } else if (n == "min" || n == "max" || n == "lead" || n == "lag" || n == "first_value" || n == "last_value" || n == "nth_value") {
+                if (e.ch.empty()) return in.fail(BKGPU_EINVAL, "window %s() without an argument", n.c_str());
+                e.col_type = ct;
+            } else return in.fail(BKGPU_EUNSUPPORTED, "window function '%s' is outside the GPU path", n.c_str());
             return true;
         }
         case BK_AND_PREDICATE: case BK_OR_PREDICATE: case BK_XOR_PREDICATE: case BK_NOT_PREDICATE:
@@ -1084,6 +1115,33 @@ static void explain(Compiled& c) {
         snprintf(buf, sizeof buf, "rows: pred_out=%d limit=%lld offset=%lld direct=%d\n", c.ap.pred_out, (long long)c.limit, (long long)c.offset, (int)c.has_direct); s += buf;
         for (auto& k : c.sort_keys) { snprintf(buf, sizeof buf, "  order key: out=%d prim=%d asc=%d null_first=%d\n", k.out_reg, k.prim, (int)k.asc, (int)k.null_first); s += buf; }
     }
+    if (c.kind == PK_WINDOW) {
+        static const char* fn_names[] = {"count_star", "count", "sum", "avg", "min", "max", "row_number", "rank", "dense_rank", "percent_rank",
+                                         "cume_dist", "ntile", "lead", "lag", "first_value", "last_value", "nth_value"};
+        static const char* bound_names[] = {"PRECEDING", "FOLLOWING", "CURRENT ROW"};
+        snprintf(buf, sizeof buf, "rows: pred_out=%d limit=%lld offset=%lld stages=%zu\n", c.ap.pred_out, (long long)c.limit, (long long)c.offset, c.win.size()); s += buf;
+        for (size_t k = 0; k < c.win.size(); k++) {
+            const WinStage& w = c.win[k];
+            snprintf(buf, sizeof buf, "window stage[%zu]: sort=%s keys=%zu partition=%d exprs=%zu fns=%zu", k, w.new_sort ? "new" : (w.sort_keys.empty() ? "none" : "shared"),
+                     w.sort_keys.size(), w.n_part, w.exprs.size(), w.fns.size()); s += buf;
+            if (w.has_frame) {
+                auto bound = [&](const WinBound& b) {
+                    char t[48];
+                    if (b.unbounded) snprintf(t, sizeof t, "UNBOUNDED %s", bound_names[b.type]);
+                    else if (b.type == BK_BT_CURRENT_ROW) snprintf(t, sizeof t, "CURRENT ROW");
+                    else snprintf(t, sizeof t, "%lld %s", (long long)b.num, bound_names[b.type]);
+                    return std::string(t);
+                };
+                s += std::string(" frame=") + (w.frame_type == BK_FRAME_ROWS ? "ROWS " : "RANGE ") + bound(w.start) + " .. " + bound(w.end);
+            }
+            s += "\n";
+            for (auto& sk : w.sort_keys) { snprintf(buf, sizeof buf, "  %s key: expr=%d prim=%d asc=%d\n", (&sk - w.sort_keys.data()) < w.n_part ? "partition" : "order", sk.out_reg, sk.prim, (int)sk.asc); s += buf; }
+            for (auto& f : w.fns) { snprintf(buf, sizeof buf, "  fn %s -> %d_%d prim=%d arg=%d default=%d n=%lld method=%d\n", fn_names[f.kind], f.tuple_id, f.slot_id, f.out_prim, f.arg, f.def,
+                                             (long long)f.n, f.method); s += buf; }
+        }
+        if (c.post) { snprintf(buf, sizeof buf, "post fragment above the window: kind=%d keys=%zu limit=%lld offset=%lld\n", c.post->kind, c.post->sort_keys.size(),
+                               (long long)c.post->limit, (long long)c.post->offset); s += buf; }
+    } else
     if (c.post) { snprintf(buf, sizeof buf, "post fragment above the aggregate: kind=%d keys=%zu pred_out=%d limit=%lld offset=%lld\n", c.post->kind, c.post->sort_keys.size(),
                            c.post->ap.pred_out, (long long)c.post->limit, (long long)c.post->offset); s += buf; }
     snprintf(buf, sizeof buf, "program: %d instr, %d outputs\n", c.prog.n_instr, c.prog.n_out); s += buf;
@@ -1102,6 +1160,7 @@ bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
 bool lower_post(Infer& in, Compiled& out, const HNode* sort, const HNode* having, const HNode* limit_node);
 bool lower_join_rows(Infer& in, Compiled& out, const HNode& join, const HNode* above, const HNode* sort, const HNode* limit_node);
 bool lower_star_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& join, bool under_packet, const HNode* above);
+bool lower_window(Infer& in, Compiled& out, const HNode& wtop, const HNode* outer_sort, const HNode* limit_node);
 static int join_leaves(const HNode* n);
 
 static bool infer_node(Infer& in, HNode& n) {
@@ -1109,6 +1168,8 @@ static bool infer_node(Infer& in, HNode& n) {
     for (auto& e : n.group_exprs) if (!infer_expr(in, e)) return false;
     for (auto& e : n.agg_fns) if (!infer_expr(in, e)) return false;
     for (auto& e : n.order_exprs) if (!infer_expr(in, e)) return false;
+    if (n.frame_start.has_expr && !infer_expr(in, n.frame_start.expr)) return false;
+    if (n.frame_end.has_expr && !infer_expr(in, n.frame_end.expr)) return false;
     for (auto& c : n.ch) if (!infer_node(in, c)) return false;
     return true;
 }
@@ -1157,7 +1218,14 @@ int compile_plan(const uint8_t* desc, size_t len, Compiled& out, std::string& er
         if (t && (is_filter(t) || t->node_type == BK_HAVING_FILTER_NODE) && !t->ch.empty()) { ph = t; t = skip_passthrough(&t->ch[0], nullptr); }
         if (t && (ps || ph) && (t->node_type == BK_AGG_NODE || t->node_type == BK_MERGE_AGG_NODE)) { post_sort = ps; post_having = ph; top = t; }
     }
-    if (top->node_type == BK_AGG_NODE || top->node_type == BK_MERGE_AGG_NODE) {
+    const HNode* win_sort = nullptr;   // [SORT ->] WINDOW: the query's ORDER BY above the window stages
+    if (top->node_type == BK_SORT_NODE && !top->ch.empty()) {
+        const HNode* c = skip_passthrough(&top->ch[0], nullptr);
+        if (c && c->node_type == BK_WINDOW_NODE) win_sort = top;
+    }
+    if (win_sort || top->node_type == BK_WINDOW_NODE) {
+        ok = lower_window(in, out, win_sort ? *skip_passthrough(&win_sort->ch[0], nullptr) : *top, win_sort, limit_node);
+    } else if (top->node_type == BK_AGG_NODE || top->node_type == BK_MERGE_AGG_NODE) {
         if (top->ch.empty()) { err = "AGG node without a child"; return BKGPU_EINVAL; }
         const HNode* c = skip_passthrough(&top->ch[0], nullptr);
         const HNode* filter = nullptr;
@@ -1659,6 +1727,195 @@ bool lower_join_rows(Infer& in, Compiled& out, const HNode& join, const HNode* a
     pc.has_direct = false;
     out.post = post;
     out.limit = pc.limit; out.offset = pc.offset;
+    return true;
+}
+
+// ---------------------------------------------------------------- window
+// [LIMIT ->] [SORT ->] (WINDOW -> SORT){1..8} [FILTER ->] SCAN (select_planner.cpp:705-760): the planner gives every window spec its own
+// SORT by the partition expressions followed by the order expressions (is_null_first = is_asc) and a WINDOW that keeps the order part.
+// Each pair becomes one stage over the retained scan rows; the operators above the top WINDOW are the query's ORDER BY / LIMIT.
+namespace {
+struct WinName { const char* name; int kind; };
+const WinName k_win_names[] = {{"count_star", WF_COUNT_STAR}, {"count", WF_COUNT}, {"sum", WF_SUM}, {"avg", WF_AVG}, {"min", WF_MIN}, {"max", WF_MAX},
+                               {"row_number", WF_ROW_NUMBER}, {"rank", WF_RANK}, {"dense_rank", WF_DENSE_RANK}, {"percent_rank", WF_PERCENT_RANK},
+                               {"cume_dist", WF_CUME_DIST}, {"ntile", WF_NTILE}, {"lead", WF_LEAD}, {"lag", WF_LAG}, {"first_value", WF_FIRST_VALUE},
+                               {"last_value", WF_LAST_VALUE}, {"nth_value", WF_NTH_VALUE}};
+bool win_is_agg(int k) { return k <= WF_MAX; }
+bool win_no_frame(int k) { return k >= WF_ROW_NUMBER && k <= WF_LAG; }
+// the value of an INT_LITERAL argument; false when the node is not one
+bool int_literal(const HExpr& e, int64_t& v) {
+    if (e.node_type != BK_INT_LITERAL || e.lit_null) return false;
+    v = (int64_t)e.lit_bits;
+    return true;
+}
+std::string sort_key_text(const HNode& s) {
+    std::string k;
+    for (size_t i = 0; i < s.order_exprs.size(); i++) k += expr_key(s.order_exprs[i]) + (s.is_asc[i] ? "A" : "D") + (s.is_null_first[i] ? "F" : "L");
+    return k;
+}
+}  // namespace
+
+bool lower_window(Infer& in, Compiled& out, const HNode& wtop, const HNode* outer_sort, const HNode* limit_node) {
+    out.kind = PK_WINDOW;
+    std::vector<std::pair<const HNode*, const HNode*>> pairs;   // (WINDOW, SORT), top-down
+    const HNode* t = &wtop;
+    while (t && t->node_type == BK_WINDOW_NODE) {
+        const HNode* s = t->ch.empty() ? nullptr : skip_passthrough(&t->ch[0], nullptr);
+        if (!s || s->node_type != BK_SORT_NODE || s->ch.empty()) return in.fail(BKGPU_EUNSUPPORTED, "a WINDOW node's child must be its SORT node");
+        pairs.push_back({t, s});
+        t = skip_passthrough(&s->ch[0], nullptr);
+    }
+    const HNode* filter = nullptr;
+    if (is_filter(t)) { filter = t; t = t->ch.empty() ? nullptr : skip_passthrough(&t->ch[0], nullptr); }
+    if (!t || t->node_type != BK_SCAN_NODE)
+        return in.fail(BKGPU_EUNSUPPORTED, "window stages must sit on [FILTER ->] SCAN: a window over an aggregate or a join is outside the GPU path");
+    if (filter && filter->limit != -1) return in.fail(BKGPU_EUNSUPPORTED, "LIMIT on a filter below a window is order dependent");
+    out.scan_tuple = t->tuple_id;
+    Program& p = out.prog; memset(&p, 0, sizeof p);
+    memset(&out.ap, 0, sizeof out.ap);
+    Lower lw{&out, &in, &p, {}};
+    if (!intern_scan_tuple(in, out, lw, t->tuple_id)) return false;
+    const size_t n_scan_cols = out.cols.size();
+    int reg = 0;
+    if (!lower_predicate(in, lw, filter, out.ap, reg)) return false;
+    p.n_out = reg;
+    // one device program per distinct (expression, result type) of a stage
+    auto intern_expr = [&](WinStage& st, std::map<std::string, int>& seen, const HExpr& e, int to) -> int {
+        const std::string key = expr_key(e) + ":" + std::to_string(to);
+        auto it = seen.find(key);
+        if (it != seen.end()) return it->second;
+        Program q; memset(&q, 0, sizeof q);
+        const int save = out.n_const; out.n_const = 0;
+        Lower l2{&out, &in, &q, {}};
+        int depth = 0;
+        const bool ok = l2.expr(e, depth) && l2.cast(e.col_type, to) && l2.out_reg(0);
+        out.n_const = save;
+        if (!ok) return -1;
+        if (out.cols.size() != n_scan_cols) { in.fail(BKGPU_EUNSUPPORTED, "a window expression reads a column outside the scan tuple %d", out.scan_tuple); return -1; }
+        q.n_out = 1;
+        st.exprs.push_back(q); st.expr_prim.push_back(to);
+        return seen[key] = (int)st.exprs.size() - 1;
+    };
+    std::string prev_keys;
+    size_t n_fns = 0, n_sorts = 0;
+    std::vector<OutCol> win_cols;
+    for (size_t pi = pairs.size(); pi-- > 0;) {   // bottom-up: the order the rows pass through them
+        const HNode& W = *pairs[pi].first;
+        const HNode& S = *pairs[pi].second;
+        WinStage st;
+        std::map<std::string, int> seen;
+        if (W.limit != -1) return in.fail(BKGPU_EUNSUPPORTED, "a LIMIT on a WINDOW node (the subquery rewrite's) is outside the GPU path");
+        if (S.limit != -1) return in.fail(BKGPU_EUNSUPPORTED, "a LIMIT on a window's SORT node is outside the GPU path");
+        const size_t np = W.group_exprs.size(), no = W.order_exprs.size();
+        bool match = S.order_exprs.size() == np + no;
+        for (size_t k = 0; match && k < S.order_exprs.size(); k++) {
+            const HExpr& want = k < np ? W.group_exprs[k] : W.order_exprs[k - np];
+            match = expr_key(want) == expr_key(S.order_exprs[k]) && S.is_null_first[k] == S.is_asc[k] && (k < np || (S.is_asc[k] != 0) == (W.is_asc[k - np] != 0));
+        }
+        if (!match) return in.fail(BKGPU_EUNSUPPORTED, "the SORT below a WINDOW must order by its partition expressions, then its order expressions");
+        if (np + no > 4) return in.fail(BKGPU_EUNSUPPORTED, "more than 4 partition and order expressions in one window");
+        for (size_t k = 0; k < np; k++) {
+            const int ct = W.group_exprs[k].col_type;
+            if (ct == BK_STRING) return in.fail(BKGPU_EUNSUPPORTED, "PARTITION BY over a STRING key is outside the GPU path");
+            if (is_double_t(ct)) return in.fail(BKGPU_EUNSUPPORTED, "PARTITION BY over a FLOAT / DOUBLE key is outside the GPU path: its byte encoding separates values the sort treats as equal");
+        }
+        for (size_t k = 0; k < no; k++)
+            if (W.order_exprs[k].col_type == BK_STRING) return in.fail(BKGPU_EUNSUPPORTED, "window ORDER BY over a STRING key is outside the GPU path");
+        for (size_t k = 0; k < S.order_exprs.size(); k++) {
+            const HExpr& e = S.order_exprs[k];
+            const int x = intern_expr(st, seen, e, e.col_type);
+            if (x < 0) return false;
+            st.sort_keys.push_back({x, e.col_type, S.is_asc[k] != 0, S.is_null_first[k] != 0});
+        }
+        st.n_part = (int)np;
+        const std::string keys = sort_key_text(S);
+        st.new_sort = !S.order_exprs.empty() && keys != prev_keys;   // (no keys: OVER () keeps the current order; equal keys: a stable re-sort is the identity)
+        if (!S.order_exprs.empty()) prev_keys = keys;
+        if (st.new_sort && ++n_sorts > 8) return in.fail(BKGPU_EUNSUPPORTED, "more than 8 distinct window sorts in one fragment");
+        // frame (WindowProcessor::init, window_node.cpp:337-394; Row/RangeFrameWindowProcessor::get_start_row / get_end_row)
+        st.has_frame = W.has_frame;
+        st.frame_type = W.frame_type;
+        if (W.has_frame) {
+            if (W.frame_type != BK_FRAME_ROWS && W.frame_type != BK_FRAME_RANGE) return in.fail(BKGPU_EINVAL, "bad window frame type %d", W.frame_type);
+            const HFrameBound* hb[2] = {&W.frame_start, &W.frame_end};
+            WinBound* wb[2] = {&st.start, &st.end};
+            for (int b = 0; b < 2; b++) {
+                const HFrameBound& h = *hb[b];
+                if (h.type < BK_BT_PRECEDING || h.type > BK_BT_CURRENT_ROW) return in.fail(BKGPU_EINVAL, "bad window frame bound type %d", h.type);
+                if (h.unbounded && b == 0 && h.type != BK_BT_PRECEDING) return in.fail(BKGPU_EUNSUPPORTED, "an unbounded frame start must be UNBOUNDED PRECEDING");
+                if (h.unbounded && b == 1 && h.type != BK_BT_FOLLOWING) return in.fail(BKGPU_EUNSUPPORTED, "an unbounded frame end must be UNBOUNDED FOLLOWING");
+                wb[b]->type = h.type; wb[b]->unbounded = h.unbounded; wb[b]->num = 0;
+                if (!h.unbounded && h.type != BK_BT_CURRENT_ROW) {
+                    int64_t v = -1;
+                    if (!h.has_expr || !int_literal(h.expr, v) || v < 0 || v > INT32_MAX) return in.fail(BKGPU_EUNSUPPORTED, "a window frame offset must be an integer literal >= 0");
+                    if (W.frame_type == BK_FRAME_RANGE) return in.fail(BKGPU_EUNSUPPORTED, "a RANGE frame with an offset is outside the GPU path (the reference fails at run time)");
+                    wb[b]->num = v;
+                }
+            }
+            if (W.frame_type == BK_FRAME_ROWS && !st.start.unbounded && !st.end.unbounded) {
+                auto pos = [](const WinBound& x) { return x.type == BK_BT_PRECEDING ? -x.num : (x.type == BK_BT_FOLLOWING ? x.num : 0); };
+                if (pos(st.end) - pos(st.start) + 1 > 4096) return in.fail(BKGPU_EUNSUPPORTED, "a bounded ROWS frame wider than 4096 rows is outside the GPU path");
+            }
+        }
+        const bool whole = !st.has_frame || (st.start.unbounded && st.end.unbounded);
+        int method = WM_FWD;
+        if (!whole) {
+            if (st.start.unbounded) method = WM_FWD;
+            else if (st.end.unbounded) method = WM_BWD;
+            else if (st.frame_type == BK_FRAME_RANGE) method = WM_PEER;
+            else method = WM_DIRECT;
+        }
+        for (const HExpr& f : W.agg_fns) {
+            if (f.node_type != BK_WINDOW_EXPR) return in.fail(BKGPU_EINVAL, "a WINDOW node's function must be a WINDOW_EXPR");
+            WinFn wf;
+            wf.kind = -1;
+            for (const WinName& nm : k_win_names) if (f.name == nm.name) wf.kind = nm.kind;
+            if (wf.kind < 0) return in.fail(BKGPU_EUNSUPPORTED, "window function '%s' is outside the GPU path", f.name.c_str());
+            wf.tuple_id = f.tuple_id; wf.slot_id = f.slot_id; wf.out_prim = f.col_type;
+            if (st.has_frame && win_no_frame(wf.kind)) return in.fail(BKGPU_EUNSUPPORTED, "a frame on %s() is outside the GPU path (the planner never emits one)", f.name.c_str());
+            const bool takes_value = wf.kind != WF_COUNT_STAR && wf.kind != WF_ROW_NUMBER && wf.kind != WF_RANK && wf.kind != WF_DENSE_RANK &&
+                                     wf.kind != WF_PERCENT_RANK && wf.kind != WF_CUME_DIST && wf.kind != WF_NTILE;
+            if (takes_value) {
+                if (f.ch.empty()) return in.fail(BKGPU_EINVAL, "window %s() without an argument", f.name.c_str());
+                const HExpr& x = f.ch[0];
+                if (x.col_type == BK_STRING) return in.fail(BKGPU_EUNSUPPORTED, "window %s() over a STRING argument is outside the GPU path", f.name.c_str());
+                if ((wf.kind == WF_SUM || wf.kind == WF_AVG) && is_datetime_family(x.col_type))
+                    return in.fail(BKGPU_EUNSUPPORTED, "window %s() over a date/time argument is outside the GPU path", f.name.c_str());
+                // SUM / AVG read value.cast_to(_col_type); MIN / MAX / LEAD / LAG / FIRST / LAST / NTH keep the argument's type
+                wf.arg_prim = wf.kind == WF_COUNT ? x.col_type : wf.out_prim;
+                if ((wf.arg = intern_expr(st, seen, x, wf.arg_prim)) < 0) return false;
+            }
+            if (wf.kind == WF_NTILE && (f.ch.empty() || !int_literal(f.ch[0], wf.n) || wf.n <= 0)) return in.fail(BKGPU_EUNSUPPORTED, "NTILE needs an integer literal > 0");
+            if (wf.kind == WF_NTH_VALUE && (f.ch.size() < 2 || !int_literal(f.ch[1], wf.n) || wf.n <= 0)) return in.fail(BKGPU_EUNSUPPORTED, "NTH_VALUE needs an integer literal > 0");
+            if (wf.kind == WF_LEAD || wf.kind == WF_LAG) {
+                wf.n = 1;
+                if (f.ch.size() > 1 && (!int_literal(f.ch[1], wf.n) || wf.n < 0)) return in.fail(BKGPU_EUNSUPPORTED, "the LEAD / LAG offset must be an integer literal >= 0");
+                if (f.ch.size() > 2) {
+                    if (f.ch[2].col_type == BK_STRING) return in.fail(BKGPU_EUNSUPPORTED, "a STRING LEAD / LAG default is outside the GPU path");
+                    if ((wf.def = intern_expr(st, seen, f.ch[2], wf.out_prim)) < 0) return false;   // default_expr->get_value(current row).cast_to(_col_type)
+                }
+            }
+            wf.method = win_is_agg(wf.kind) ? method : WM_NONE;
+            st.fns.push_back(wf);
+            win_cols.push_back({wf.tuple_id, wf.slot_id, wf.out_prim, 0});
+            if (++n_fns > 32) return in.fail(BKGPU_EUNSUPPORTED, "more than 32 window functions in one fragment");
+        }
+        out.win.push_back(std::move(st));
+    }
+    for (const OutCol& oc : win_cols) {
+        for (const OutCol& x : out.out_cols)
+            if (x.tuple_id == oc.tuple_id && x.slot_id == oc.slot_id) return in.fail(BKGPU_EINVAL, "window output column %d_%d appears twice", oc.tuple_id, oc.slot_id);
+        out.out_cols.push_back(oc);
+    }
+    out.limit = -1; out.offset = 0;
+    if (outer_sort) {   // the query's ORDER BY over the window rows (window columns included) [+ LIMIT / OFFSET]
+        if (out.out_cols.size() > (size_t)MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d window output columns under an ORDER BY", MAX_COLS);
+        return lower_post(in, out, outer_sort, nullptr, limit_node);
+    }
+    if (limit_node) {   // LIMIT / OFFSET over the top stage's order
+        out.offset = limit_node->offset;
+        out.limit = limit_node->limit < 0 ? -1 : limit_node->limit + limit_node->offset;
+    }
     return true;
 }
 

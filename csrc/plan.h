@@ -7,6 +7,7 @@
 #include <string>
 #include <vector>
 #include "dev_types.h"
+#include "../include/bkgpu_plan.h"
 
 namespace bk {
 
@@ -28,6 +29,9 @@ struct HExpr {
     bool is_constant = false;
 };
 
+// WINDOW_NODE frame bound (pb::FrameBound): type BK_BT_*, unbounded flag, optional INT_LITERAL offset
+struct HFrameBound { int type = 0; bool unbounded = false; bool has_expr = false; HExpr expr; };
+
 struct HNode {
     int node_type = 0;
     int64_t limit = -1;
@@ -40,6 +44,10 @@ struct HNode {
     std::vector<int> is_asc, is_null_first;
     int join_type = 0;
     int64_t offset = 0;
+    // window (pb::WindowNode): func_exprs in agg_fns, partition exprs in group_exprs, order exprs + is_asc in order_exprs / is_asc
+    bool has_frame = false;
+    int frame_type = 0;
+    HFrameBound frame_start, frame_end;
 };
 
 struct HTuple { int tuple_id; std::vector<std::pair<int, int>> slots; /* (slot_id, prim) */ };
@@ -51,7 +59,7 @@ struct OutCol {
     int kind;       // 0 = plain value column, 1 = AVG intermediate blob (two device images: sum, count)
 };
 
-enum PlanKind { PK_AGG = 1, PK_FILTER = 2, PK_SORT = 3, PK_JOIN_AGG = 4, PK_JOIN = 5, PK_STAR_AGG = 6 };
+enum PlanKind { PK_AGG = 1, PK_FILTER = 2, PK_SORT = 3, PK_JOIN_AGG = 4, PK_JOIN = 5, PK_STAR_AGG = 6, PK_WINDOW = 7 };
 
 struct SortKey { int out_reg; int prim; bool asc, null_first; };
 
@@ -62,6 +70,37 @@ struct StarDim {
     int cast_prim = 0;                 // type both keys are compared in (strip_out_equal_slots' cast, joiner.cpp:166-217)
     int n_filter = 0;                  // conjuncts that read this dimension alone: evaluated once over its rows at build time
     Program filter;                    // output 0 = their conjunction (column indices into Compiled::cols)
+};
+
+// window functions (WindowFnCall::init's name table, window_fn_call.cpp:20-38)
+enum WinFnKind { WF_COUNT_STAR = 0, WF_COUNT, WF_SUM, WF_AVG, WF_MIN, WF_MAX, WF_ROW_NUMBER, WF_RANK, WF_DENSE_RANK, WF_PERCENT_RANK,
+                 WF_CUME_DIST, WF_NTILE, WF_LEAD, WF_LAG, WF_FIRST_VALUE, WF_LAST_VALUE, WF_NTH_VALUE };
+// how an aggregate / value function reads its frame [start, end) on the device
+enum WinMethod { WM_NONE = 0,   // ranking, LEAD / LAG: no frame
+                 WM_FWD,        // the frame starts at the partition start: a forward scan segmented by partition, read at end - 1
+                 WM_BWD,        // the frame ends at the partition end: a backward scan segmented by partition, read at start
+                 WM_PEER,       // RANGE CURRENT ROW .. CURRENT ROW: a forward scan segmented by peer group, read at the group's last row
+                 WM_DIRECT };   // bounded ROWS frame (<= 4096 rows): each row loops over its frame
+struct WinBound { int type = BK_BT_PRECEDING; bool unbounded = true; int64_t num = 0; };
+struct WinFn {
+    int kind = 0, tuple_id = 0, slot_id = 0;
+    int out_prim = 0;                  // result type (WindowFnCall::type_inferer)
+    int arg = -1, def = -1;            // indices into WinStage::exprs: the value argument, LEAD / LAG's default
+    int arg_prim = 0;                  // type of the argument's image as evaluated (after the cast to the result type)
+    int64_t n = 0;                     // NTILE buckets, LEAD / LAG offset, NTH_VALUE position
+    int method = WM_NONE;
+};
+// one WINDOW -> SORT pair.  Every expression is its own one-output device program over the scan columns.
+struct WinStage {
+    bool new_sort = true;              // false: the SORT's keys equal the previous stage's (a stable re-sort is the identity)
+    std::vector<Program> exprs;
+    std::vector<int> expr_prim;
+    std::vector<SortKey> sort_keys;    // out_reg = index into exprs; partition keys first
+    int n_part = 0;                    // the first n_part sort keys are the partition expressions, the rest the order expressions
+    bool has_frame = false;
+    int frame_type = 0;
+    WinBound start, end;
+    std::vector<WinFn> fns;
 };
 
 struct Compiled {
@@ -101,6 +140,9 @@ struct Compiled {
     // operators ABOVE the aggregate ([LIMIT ->] [SORT ->] [HAVING ->] AGG, exec_node.cpp:347-394): a second, small fragment of kind
     // PK_SORT / PK_FILTER whose "scan tuple" is the aggregate's output row (its columns = this->out_cols, in order)
     std::shared_ptr<Compiled> post;
+    // window (PK_WINDOW): the stages bottom-up; the output rows are the scan tuple's slots (out_cols) followed by one column per window
+    // function, in the topmost stage's sort order.  `post` (kind PK_SORT), when present, is the query's ORDER BY over those rows.
+    std::vector<WinStage> win;
     std::string explain;
 };
 

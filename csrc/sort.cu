@@ -843,12 +843,12 @@ int retain_batch(SortState* s, const RowArgs& ra, cudaStream_t st, bkgpu_stats* 
     return 0;
 }
 
-int copy_out(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, const uint32_t* perm_dev, int64_t n, int64_t skip, cudaStream_t st,
-             std::vector<SortOutCol>& out, std::string& err) {
+int copy_cols_out(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, const std::vector<ColRef>& desc, const uint32_t* perm_dev, int64_t n, int64_t skip,
+                  cudaStream_t st, std::vector<SortOutCol>& out, std::string& err) {
     // perm_dev == nullptr: rows [skip, skip+n) in place; else gather through a device permutation first
     out.clear();
-    for (int c = 0; c < s->ncols; c++) {
-        const ColRef& cr = s->c.cols[(size_t)c];
+    for (size_t c = 0; c < desc.size(); c++) {
+        const ColRef& cr = desc[c];
         SortOutCol oc; oc.tuple_id = cr.tuple_id; oc.slot_id = cr.slot_id; oc.prim = cr.prim; oc.elem = elem_bytes_of(cr.prim);
         oc.values.assign((size_t)std::max<int64_t>(n, 1) * oc.elem, 0);
         std::vector<uint8_t> nb((size_t)std::max<int64_t>(n, 1));
@@ -883,7 +883,107 @@ int copy_out(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, const ui
     }
     return 0;
 }
+int copy_out(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, const uint32_t* perm_dev, int64_t n, int64_t skip, cudaStream_t st,
+             std::vector<SortOutCol>& out, std::string& err) {
+    return copy_cols_out(s, vals, nulls, s->c.cols, perm_dev, n, skip, st, out, err);
+}
 
+// scratch of one radix sort of n (key image, row id) pairs
+struct RadixBufs {
+    uint64_t *img_row = nullptr, *img[2] = {nullptr, nullptr}; uint32_t *ids[2] = {nullptr, nullptr}, *hist = nullptr, *status = nullptr;
+    uint32_t n = 0, ntiles = 0; size_t rs_smem = 0;
+};
+int radix_alloc(SortState* s, int64_t n, RadixBufs& b, std::string& err) {
+    b.n = (uint32_t)n;
+    b.ntiles = (b.n + RS_TILE - 1) / RS_TILE;
+    int rc;
+    if ((rc = dalloc(s, &b.img_row, (size_t)n * 8, err))) return rc;
+    if ((rc = dalloc(s, &b.img[0], (size_t)n * 8, err))) return rc;
+    if ((rc = dalloc(s, &b.img[1], (size_t)n * 8, err))) return rc;
+    if ((rc = dalloc(s, &b.ids[0], (size_t)n * 4, err))) return rc;
+    if ((rc = dalloc(s, &b.ids[1], (size_t)n * 4, err))) return rc;
+    if ((rc = dalloc(s, &b.hist, (size_t)(8 * 256 * 2 + 8 + 8) * 4, err))) return rc;       // histograms, bases, active flags, tickets
+    if ((rc = dalloc(s, &b.status, (size_t)b.ntiles * 256 * 8 * 4, err))) return rc;       // one look-back array per pass
+    b.rs_smem = (size_t)RS_TILE * 12 + (8 * 256 + 256 + 256) * 4;
+    SCK(cudaFuncSetAttribute(k_rs_pass, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b.rs_smem));
+    return 0;
+}
+void radix_free(SortState* s, RadixBufs& b) {
+    dfree(s, b.img_row); dfree(s, b.img[0]); dfree(s, b.img[1]); dfree(s, b.ids[0]); dfree(s, b.ids[1]); dfree(s, b.hist); dfree(s, b.status);
+    b = RadixBufs();
+}
+
+// retained columns as DevCols of `ra` (values + validity bitmaps packed from the null bytes); h_null_flags[c]: column c holds a NULL
+int retained_bitmaps(SortState* s, cudaStream_t st, RowArgs& ra, std::vector<uint8_t*>& bitmaps, uint32_t* h_null_flags, std::string& err) {
+    const int64_t n = s->ret_rows;
+    int rc;
+    for (int c = 0; c < s->ncols; c++) { ra.cols[c].values = s->ret_vals[(size_t)c]; ra.cols[c].validity = nullptr; ra.cols[c].stype = prim_storage(s->c.cols[(size_t)c].prim); ra.cols[c].prim = s->c.cols[(size_t)c].prim; }
+    bitmaps.assign((size_t)s->ncols, nullptr);
+    uint32_t* null_flags = nullptr;
+    if ((rc = dalloc(s, &null_flags, sizeof(uint32_t) * MAX_COLS, err))) return rc;
+    SCK(cudaMemsetAsync(null_flags, 0, sizeof(uint32_t) * MAX_COLS, st));
+    for (int c = 0; c < s->ncols; c++) {
+        if ((rc = dalloc(s, &bitmaps[(size_t)c], (size_t)(n + 7) / 8 + 64, err))) return rc;
+        k_pack_null_bytes<<<grid_for((n + 7) / 8, 256, s->sm_count), 256, 0, st>>>(s->ret_null[(size_t)c], n, bitmaps[(size_t)c], null_flags + c);
+        ra.cols[c].validity = bitmaps[(size_t)c];
+    }
+    SCK(cudaMemcpyAsync(h_null_flags, null_flags, sizeof(uint32_t) * (size_t)s->ncols, cudaMemcpyDeviceToHost, st));
+    SCK(cudaStreamSynchronize(st));
+    dfree(s, null_flags);
+    ra.n_cols = s->ncols; ra.nrows = n;
+    return 0;
+}
+
+// stable LSD radix sort of the row ids b.ids[cur] by `keys` (least significant first).  Key k's image comes from program progs[k] (its
+// output register keys[k].out_reg), or straight from column `direct_col` when that is >= 0 (one key).  identity_start: b.ids[cur] holds
+// 0..n-1, so the first key's images need no gather into the current order.
+int radix_sort_keys(SortState* s, RowArgs& ra, const std::vector<SortKey>& keys, const std::vector<const Program*>& progs, int direct_col,
+                    bool direct_has_nulls, RadixBufs& b, int& cur, bool identity_start, cudaStream_t st, bkgpu_stats* stats, int64_t& pass_bytes, std::string& err) {
+    const int64_t n = b.n;
+    const uint32_t un = b.n, ntiles = b.ntiles;
+    uint32_t* hist = b.hist; uint32_t* bases = hist + 8 * 256; uint32_t* active = bases + 8 * 256; uint32_t* tickets = active + 8;
+    uint64_t** img = b.img; uint32_t** ids = b.ids; uint64_t* img_row = b.img_row; uint32_t* status = b.status;
+    bool first = identity_start;
+    // sorts the pairs (img[cur], ids[cur]) by the 64-bit image: one histogram pass, then one Onesweep pass per digit that varies
+    auto sort_pairs = [&]() -> int {
+        SCK(cudaMemsetAsync(hist, 0, (size_t)(8 * 256 * 2 + 8 + 8) * 4, st));
+        k_rs_hist<<<std::min(s->sm_count * 4, (int)((un + 1023) / 1024)), 256, 0, st>>>(img[cur], un, hist);
+        k_rs_bases<<<8, 256, 0, st>>>(hist, bases, active);
+        uint32_t h_active[8];
+        SCK(cudaMemcpyAsync(h_active, active, 32, cudaMemcpyDeviceToHost, st));
+        SCK(cudaStreamSynchronize(st));
+        int n_active = 0;
+        for (int d = 0; d < 8; d++) n_active += h_active[d] != 0;
+        if (n_active) SCK(cudaMemsetAsync(status, 0, (size_t)ntiles * 256 * 4 * (size_t)n_active, st));
+        stats->kernel_launches += 2; pass_bytes += (int64_t)n * 8;
+        int slot = 0;
+        for (int d = 0; d < 8; d++) {
+            if (!h_active[d]) continue;
+            k_rs_pass<<<ntiles, RS_THREADS, b.rs_smem, st>>>(img[cur], ids[cur], img[cur ^ 1], ids[cur ^ 1], un, 8 * d, bases + 256 * d,
+                                                          status + (size_t)slot * ntiles * 256, tickets + d);
+            cur ^= 1; slot++;
+            stats->kernel_launches++; pass_bytes += (int64_t)n * 24;
+        }
+        return 0;
+    };
+    int rc;
+    for (int ki = (int)keys.size() - 1; ki >= 0; ki--) {
+        const SortKey& sk = keys[(size_t)ki];
+        ra.prog = *progs[(size_t)ki];
+        for (int mode = 0; mode < 2; mode++) {   // the key's value image first, then its NULL rank (stable: NULLs end up strictly first / last)
+            if (mode == 1 && direct_col >= 0 && !direct_has_nulls) continue;
+            uint64_t* dst = first ? img[cur] : img_row;
+            if (mode == 0 && direct_col >= 0) k_sort_images_direct<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(ra.cols[direct_col], n, host_prim_class(sk.prim), sk.asc ? 0 : 1, dst);
+            else
+            k_sort_images<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(ra, sk.out_reg, host_prim_class(sk.prim), sk.asc ? 0 : 1, sk.null_first ? 1 : 0, mode, dst, nullptr);
+            if (!first) k_rs_gather_u64<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(img_row, ids[cur], img[cur], un);   // images in the current order
+            first = false;
+            stats->kernel_launches += 2;
+            if ((rc = sort_pairs())) return rc;
+        }
+    }
+    return 0;
+}
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1135,79 +1235,23 @@ int sort_finish(SortState* s, void* nccl_comm, int nranks, cudaStream_t st, bkgp
     const int64_t n = s->ret_rows;
     if (n >= (int64_t)RS_VAL_MASK) return fail(err, BKGPU_EUNSUPPORTED, "full sort is limited to 2^30 rows per GPU");
     if (n == 0) { *nrows = 0; return copy_out(s, s->ret_vals.data(), s->ret_null.data(), nullptr, 0, 0, st, out, err); }
-    const uint32_t un = (uint32_t)n;
-    const uint32_t ntiles = (un + RS_TILE - 1) / RS_TILE;
-    uint64_t *img_row = nullptr, *img[2] = {nullptr, nullptr}; uint32_t *ids[2] = {nullptr, nullptr}, *hist = nullptr, *status = nullptr; int rc;
-    if ((rc = dalloc(s, &img_row, (size_t)n * 8, err))) return rc;
-    if ((rc = dalloc(s, &img[0], (size_t)n * 8, err))) return rc;
-    if ((rc = dalloc(s, &img[1], (size_t)n * 8, err))) return rc;
-    if ((rc = dalloc(s, &ids[0], (size_t)n * 4, err))) return rc;
-    if ((rc = dalloc(s, &ids[1], (size_t)n * 4, err))) return rc;
-    if ((rc = dalloc(s, &hist, (size_t)(8 * 256 * 2 + 8 + 8) * 4, err))) return rc;       // histograms, bases, active flags, tickets
-    if ((rc = dalloc(s, &status, (size_t)ntiles * 256 * 8 * 4, err))) return rc;           // one look-back array per pass
-    uint32_t* bases = hist + 8 * 256; uint32_t* active = bases + 8 * 256; uint32_t* tickets = active + 8;
-    const size_t rs_smem = (size_t)RS_TILE * 12 + (8 * 256 + 256 + 256) * 4;
-    SCK(cudaFuncSetAttribute(k_rs_pass, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rs_smem));
+    RadixBufs b; int rc;
+    if ((rc = radix_alloc(s, n, b, err))) return rc;
     RowArgs ra; memset(&ra, 0, sizeof ra);
-    for (int c = 0; c < s->ncols; c++) { ra.cols[c].values = s->ret_vals[(size_t)c]; ra.cols[c].validity = nullptr; ra.cols[c].stype = prim_storage(s->c.cols[(size_t)c].prim); ra.cols[c].prim = s->c.cols[(size_t)c].prim; }
     // retained columns carry null BYTES: pack them into bitmaps on the device so the key program sees NULLs
-    std::vector<uint8_t*> bitmaps((size_t)s->ncols, nullptr);
-    uint32_t* null_flags = nullptr;
-    if ((rc = dalloc(s, &null_flags, sizeof(uint32_t) * MAX_COLS, err))) return rc;
-    SCK(cudaMemsetAsync(null_flags, 0, sizeof(uint32_t) * MAX_COLS, st));
-    for (int c = 0; c < s->ncols; c++) {
-        if ((rc = dalloc(s, &bitmaps[(size_t)c], (size_t)(n + 7) / 8 + 64, err))) return rc;
-        k_pack_null_bytes<<<grid_for((n + 7) / 8, 256, s->sm_count), 256, 0, st>>>(s->ret_null[(size_t)c], n, bitmaps[(size_t)c], null_flags + c);
-        ra.cols[c].validity = bitmaps[(size_t)c];
-    }
-    uint32_t h_null_flags[MAX_COLS] = {0};
-    SCK(cudaMemcpyAsync(h_null_flags, null_flags, sizeof(uint32_t) * (size_t)s->ncols, cudaMemcpyDeviceToHost, st));
-    SCK(cudaStreamSynchronize(st));
-    ra.n_cols = s->ncols; ra.nrows = n; ra.prog = s->c.prog; ra.key.pred_out = -1;
-    k_rs_iota<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(ids[0], un);
-    int cur = 0; bool first = true;
+    std::vector<uint8_t*> bitmaps; uint32_t h_null_flags[MAX_COLS] = {0};
+    if ((rc = retained_bitmaps(s, st, ra, bitmaps, h_null_flags, err))) return rc;
+    ra.prog = s->c.prog; ra.key.pred_out = -1;
+    k_rs_iota<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(b.ids[0], (uint32_t)n);
+    int cur = 0;
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
     cudaEventRecord(e0, st);
     int64_t pass_bytes = 0;
-    // sorts the pairs (img[cur], ids[cur]) by the 64-bit image: one histogram pass, then one Onesweep pass per digit that varies
-    auto sort_pairs = [&]() -> int {
-        SCK(cudaMemsetAsync(hist, 0, (size_t)(8 * 256 * 2 + 8 + 8) * 4, st));
-        k_rs_hist<<<std::min(s->sm_count * 4, (int)((un + 1023) / 1024)), 256, 0, st>>>(img[cur], un, hist);
-        k_rs_bases<<<8, 256, 0, st>>>(hist, bases, active);
-        uint32_t h_active[8];
-        SCK(cudaMemcpyAsync(h_active, active, 32, cudaMemcpyDeviceToHost, st));
-        SCK(cudaStreamSynchronize(st));
-        int n_active = 0;
-        for (int d = 0; d < 8; d++) n_active += h_active[d] != 0;
-        if (n_active) SCK(cudaMemsetAsync(status, 0, (size_t)ntiles * 256 * 4 * (size_t)n_active, st));
-        stats->kernel_launches += 2; pass_bytes += (int64_t)n * 8;
-        int slot = 0;
-        for (int d = 0; d < 8; d++) {
-            if (!h_active[d]) continue;
-            k_rs_pass<<<ntiles, RS_THREADS, rs_smem, st>>>(img[cur], ids[cur], img[cur ^ 1], ids[cur ^ 1], un, 8 * d, bases + 256 * d,
-                                                        status + (size_t)slot * ntiles * 256, tickets + d);
-            cur ^= 1; slot++;
-            stats->kernel_launches++; pass_bytes += (int64_t)n * 24;
-        }
-        return 0;
-    };
-    for (int ki = (int)s->c.sort_keys.size() - 1; ki >= 0; ki--) {
-        const SortKey& sk = s->c.sort_keys[(size_t)ki];
-        // a plain column key (config C5's shape): its image comes straight from the column, and without NULLs in it the NULL-rank pass is void
-        const bool direct_key = s->c.has_direct && s->c.sort_keys.size() == 1 && !s->c.direct_cols.empty();
-        const int dcol = direct_key ? s->c.direct_cols[0] : -1;
-        for (int mode = 0; mode < 2; mode++) {   // the key's value image first, then its NULL rank (stable: NULLs end up strictly first / last)
-            if (mode == 1 && direct_key && !h_null_flags[dcol]) continue;
-            uint64_t* dst = first ? img[cur] : img_row;
-            if (mode == 0 && direct_key) k_sort_images_direct<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(ra.cols[dcol], n, host_prim_class(sk.prim), sk.asc ? 0 : 1, dst);
-            else
-            k_sort_images<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(ra, sk.out_reg, host_prim_class(sk.prim), sk.asc ? 0 : 1, sk.null_first ? 1 : 0, mode, dst, nullptr);
-            if (!first) k_rs_gather_u64<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(img_row, ids[cur], img[cur], un);   // images in the current order
-            first = false;
-            stats->kernel_launches += 2;
-            if ((rc = sort_pairs())) return rc;
-        }
-    }
+    // a plain column key (config C5's shape): its image comes straight from the column, and without NULLs in it the NULL-rank pass is void
+    const bool direct_key = s->c.has_direct && s->c.sort_keys.size() == 1 && !s->c.direct_cols.empty();
+    const int dcol = direct_key ? s->c.direct_cols[0] : -1;
+    std::vector<const Program*> progs(s->c.sort_keys.size(), &s->c.prog);
+    if ((rc = radix_sort_keys(s, ra, s->c.sort_keys, progs, dcol, dcol >= 0 && h_null_flags[dcol], b, cur, true, st, stats, pass_bytes, err))) return rc;
     cudaEventRecord(e1, st);
     SCK(cudaStreamSynchronize(st));
     { float ms = 0; cudaEventElapsedTime(&ms, e0, e1); stats->main_kernel_ms += ms; stats->main_kernel_launches += 1; stats->main_kernel_bytes += pass_bytes; }
@@ -1216,11 +1260,63 @@ int sort_finish(SortState* s, void* nccl_comm, int nranks, cudaStream_t st, bkgp
     int64_t keep = n; if (s->k >= 0 && keep > s->k) keep = s->k;
     int64_t skip = std::min<int64_t>(s->c.offset, keep); keep -= skip;
     *nrows = keep;
-    rc = copy_out(s, s->ret_vals.data(), s->ret_null.data(), ids[cur], keep, skip, st, out, err);
-    dfree(s, img_row); dfree(s, img[0]); dfree(s, img[1]); dfree(s, ids[0]); dfree(s, ids[1]); dfree(s, hist); dfree(s, status);
-    for (auto b : bitmaps) dfree(s, b);
-    dfree(s, null_flags);
+    rc = copy_out(s, s->ret_vals.data(), s->ret_null.data(), b.ids[cur], keep, skip, st, out, err);
+    radix_free(s, b);
+    for (auto bm : bitmaps) dfree(s, bm);
     return rc;
+}
+
+// ---- the window stage's access to the retained rows and the radix sort (window.cu) ----
+int sort_retained_cols(SortState* s, cudaStream_t st, std::vector<DevCol>& cols, std::vector<void*>& scratch, int64_t* nrows, std::string& err) {
+    RowArgs ra; memset(&ra, 0, sizeof ra);
+    std::vector<uint8_t*> bitmaps; uint32_t h_null_flags[MAX_COLS] = {0};
+    int rc = retained_bitmaps(s, st, ra, bitmaps, h_null_flags, err);
+    if (rc) return rc;
+    cols.assign(ra.cols, ra.cols + s->ncols);
+    for (auto bm : bitmaps) scratch.push_back(bm);
+    *nrows = s->ret_rows;
+    return 0;
+}
+
+int sort_retained_raw(SortState* s, std::vector<uint8_t*>& vals, std::vector<uint8_t*>& nulls) {
+    vals = s->ret_vals; nulls = s->ret_null;
+    return 0;
+}
+
+void sort_free_scratch(SortState* s, std::vector<void*>& scratch) { for (void* p : scratch) dfree(s, p); scratch.clear(); }
+
+int sort_stable_ids(SortState* s, const DevCol* cols, int64_t n, const std::vector<SortKey>& keys, const std::vector<const Program*>& progs,
+                    uint32_t* ids, cudaStream_t st, bkgpu_stats* stats, std::string& err) {
+    if (n >= (int64_t)RS_VAL_MASK) return fail(err, BKGPU_EUNSUPPORTED, "a window sort is limited to 2^30 rows per GPU");
+    if (n == 0 || keys.empty()) return 0;
+    RadixBufs b; int rc;
+    if ((rc = radix_alloc(s, n, b, err))) return rc;
+    RowArgs ra; memset(&ra, 0, sizeof ra);
+    for (int c = 0; c < s->ncols; c++) ra.cols[c] = cols[c];
+    ra.n_cols = s->ncols; ra.nrows = n; ra.key.pred_out = -1;
+    SCK(cudaMemcpyAsync(b.ids[0], ids, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
+    int cur = 0; int64_t pass_bytes = 0;
+    if ((rc = radix_sort_keys(s, ra, keys, progs, -1, true, b, cur, false, st, stats, pass_bytes, err))) return rc;
+    SCK(cudaMemcpyAsync(ids, b.ids[cur], (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
+    SCK(cudaStreamSynchronize(st));
+    radix_free(s, b);
+    return 0;
+}
+
+int sort_copy_rows(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, const std::vector<ColRef>& desc, const uint32_t* perm_dev, int64_t n, int64_t skip,
+                   cudaStream_t st, std::vector<SortOutCol>& out, std::string& err) {
+    return copy_cols_out(s, vals, nulls, desc, perm_dev, n, skip, st, out, err);
+}
+
+int sort_gather_rows(SortState* s, const uint8_t* src_vals, const uint8_t* src_null, int prim, const uint32_t* perm_dev, int64_t n,
+                     uint8_t* dst_vals, uint8_t* dst_null, cudaStream_t st) {
+    if (n <= 0) return 0;
+    GatherArgs g; memset(&g, 0, sizeof g);
+    g.cols[0].values = src_vals; g.cols[0].validity = nullptr; g.cols[0].stype = prim_storage(prim); g.cols[0].prim = prim;
+    g.n_cols = 1; g.dst_vals[0] = dst_vals; g.dst_null[0] = dst_null;
+    k_gather_sel<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(g, perm_dev, (uint64_t)n, 0);
+    k_rs_gather_bytes<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(src_null, perm_dev, dst_null, (uint64_t)n);
+    return cudaGetLastError() == cudaSuccess ? 0 : BKGPU_ENODEV;
 }
 
 void sort_close(SortState* s) {

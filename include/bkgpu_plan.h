@@ -22,6 +22,9 @@
  *     SORT_NODE                      : tuple_id n_order (EXPR is_asc is_null_first)*  pb::SortNode
  *     JOIN_NODE                      : join_type n_conditions EXPR*  pb::JoinNode
  *     LIMIT_NODE                     : offset64                      pb::LimitNode
+ *     WINDOW_NODE                    : n_fn EXPR* n_part EXPR* n_order (EXPR is_asc)* has_frame [FRAME]   pb::WindowNode
+ *       FRAME := frame_type BOUND(start) BOUND(end)                  pb::WindowFrame (FT_ROWS 0, FT_RANGE 1)
+ *       BOUND := bound_type is_unbounded has_expr [EXPR]             pb::FrameBound (BT_PRECEDING 0, BT_FOLLOWING 1, BT_CURRENT_ROW 2)
  *     PACKET_NODE / SELECT_MANAGER_NODE : (nothing; accepted and skipped)
  *   EXPR  := n_nodes ENODE*                                          (ENODE* pre-order)
  *   ENODE := node_type col_type num_children PAYLOAD                 pb::ExprNode
@@ -39,6 +42,7 @@
  *                        ScalarFnCall::type_inferer + FunctionManager::complete_fn,
  *                        src/expr/scalar_fn_call.cpp:40-120, src/expr/fn_manager.cpp:316-409)
  *     AGG_EXPR        : STR(name) tuple_id final_slot_id intermediate_slot_id
+ *     WINDOW_EXPR     : STR(name) tuple_id slot_id                   pb::Function.name + DeriveExprNode (window_fn_call.cpp:19-63)
  */
 #ifndef BKGPU_PLAN_H_
 #define BKGPU_PLAN_H_
@@ -53,7 +57,7 @@ enum bkgpu_plan_node_type {
     BK_SCAN_NODE = 1, BK_SORT_NODE = 2, BK_AGG_NODE = 4, BK_MERGE_AGG_NODE = 5,
     BK_TABLE_FILTER_NODE = 6, BK_JOIN_NODE = 7, BK_LIMIT_NODE = 11,
     BK_WHERE_FILTER_NODE = 12, BK_HAVING_FILTER_NODE = 13, BK_PACKET_NODE = 14,
-    BK_SELECT_MANAGER_NODE = 25
+    BK_SELECT_MANAGER_NODE = 25, BK_WINDOW_NODE = 42
 };
 
 /* pb::ExprNodeType — proto/expr.proto:6-37 */
@@ -63,8 +67,12 @@ enum bkgpu_expr_node_type {
     BK_IS_NULL_PREDICATE = 9, BK_IN_PREDICATE = 10, BK_LIKE_PREDICATE = 11,
     BK_NOT_PREDICATE = 12, BK_AND_PREDICATE = 13, BK_OR_PREDICATE = 14,
     BK_XOR_PREDICATE = 15, BK_TIMESTAMP_LITERAL = 16, BK_DATETIME_LITERAL = 17, BK_DATE_LITERAL = 18,
-    BK_IS_TRUE_PREDICATE = 19, BK_TIME_LITERAL = 20, BK_ROW_EXPR = 22
+    BK_IS_TRUE_PREDICATE = 19, BK_TIME_LITERAL = 20, BK_ROW_EXPR = 22, BK_WINDOW_EXPR = 30
 };
+
+/* pb::FrameType / pb::BoundType — proto/plan.proto:427-436 */
+enum bkgpu_frame_type { BK_FRAME_ROWS = 0, BK_FRAME_RANGE = 1 };
+enum bkgpu_bound_type { BK_BT_PRECEDING = 0, BK_BT_FOLLOWING = 1, BK_BT_CURRENT_ROW = 2 };
 
 /* pb::PrimitiveType — proto/common.proto:46-72 */
 enum bkgpu_primitive_type {
