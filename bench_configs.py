@@ -3,7 +3,7 @@
 device-resident synthetic columns (SURVEY.md §8d), CUDA events around reset+push+finish+get_next, one JSON line per
 config with rows/s and achieved GB/s on the config's algorithmic bytes.  The headline line is bench.py's;
 this script measures the side configs on their own (C6, the star join, also its kernels, a parity flag and the Acero time).
-usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [--scale 0.1] [--steps 10]"""
+usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [c9] [--scale 0.1] [--steps 10]"""
 import argparse
 import ctypes
 import json
@@ -316,6 +316,54 @@ def c8(a):
     del ts
 
 
+def c9(a):
+    """C9, long IN lists: SELECT g, COUNT(*), SUM(x) WHERE f IN (S values) GROUP BY g over 100M device-resident rows, g INT32 in 1000
+    groups, f INT64 uniform over [0, 4S) (about a quarter of the rows pass at every S), the list S distinct seeded values.  S = 64 fits
+    the constant pool (OP_IN's linear scan); 65, 10,000 and 1,000,000 are probed as a hashed set (OP_IN_SET).  Per S: the step, the main
+    kernel, the rows passed, parity against torch.isin, and the host wall time of bkgpu_init (plan compilation, the set's build
+    included) and of bkgpu_open (the set's upload included)."""
+    import time
+    from baikaldb_b200 import plan as P
+    from tests.in_set_cases import BulkIn
+    n = int(100_000_000 * a.scale)
+    specs = [(0, 1, T.INT32, 0, 1, 0, 1000, 1.0), (0, 2, T.INT64, 0, 2, 0, 0, 1.0), (0, 3, T.DOUBLE, 1, 3, 0, 0, 1.0)]
+    g, x = gen(n, specs[0], 9), gen(n, specs[2], 9)
+    tup = {0: [(1, T.INT32), (2, T.INT64), (3, T.DOUBLE)]}
+    aggs = [P.agg_expr("count_star", 1, 1), P.agg_expr("sum", 1, 2, None, P.slot_ref(0, 3, T.DOUBLE))]
+    tup[1] = P.agg_tuple_slots(aggs, [T.INT64, T.DOUBLE])
+    info = {"gpu": torch.cuda.get_device_name(0)}
+    try:
+        import subprocess
+        info["power_limit"] = subprocess.check_output(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"], text=True).split("\n")[0].strip()
+    except Exception:
+        info["power_limit"] = None
+    for s in (64, 65, 10_000, 1_000_000):
+        f = torch.randint(0, 4 * s, (n,), device="cuda", dtype=torch.int64, generator=torch.Generator(device="cuda").manual_seed(s))
+        vals = np.random.default_rng(s).choice(4 * s, s, replace=False).astype(np.int64)
+        plan = P.Plan(P.agg(P.where(P.scan(0), BulkIn(P.slot_ref(0, 2, T.INT64), vals)), 1, [P.slot_ref(0, 1, T.INT32)], aggs), tup)
+        pb = plan.serialize()
+        h = ctypes.c_void_p()
+        t0 = time.perf_counter(); _lib.check(L.bkgpu_init(ctypes.byref(h), pb, len(pb), 0, None)); t1 = time.perf_counter()
+        _lib.check(L.bkgpu_open(h), h); t2 = time.perf_counter()
+        L.bkgpu_close(h)
+        lowered = "IN_SET" if "IN_SET" in _lib.explain(pb) else "IN"
+        line, got = run(f"C9 GROUP BY g WHERE f IN ({s} values)", plan, [(cols_array(specs, [g, f, x]), 3, n)], n, 20 * n, a.steps, a.warmup,
+                        options=[(b"group_capacity_log2", 14)], collect=True, emit=False)
+        keep = torch.isin(f, torch.from_numpy(vals).cuda())
+        cnt = torch.bincount(g[keep].long(), minlength=1000).cpu().numpy()
+        sm = torch.zeros(1000, dtype=torch.float64, device="cuda").index_add_(0, g[keep].long(), x[keep]).cpu().numpy()
+        r = line["result_rows"]
+        kk, gc, gs = (np.array(got[c][:r]) for c in ("0_1", "1_1", "1_2"))
+        line["lowered_to"] = "OP_" + lowered
+        line["rows_passed"] = int(gc.sum())
+        line["parity_vs_torch_isin"] = bool(int(gc.sum()) == int(keep.sum()) and np.array_equal(gc, cnt[kk]) and np.allclose(gs, sm[kk], rtol=1e-9, atol=0))
+        line["bkgpu_init_host_ms"] = (t1 - t0) * 1e3
+        line["bkgpu_open_host_ms"] = (t2 - t1) * 1e3
+        line.update(info)
+        print(json.dumps(line), flush=True)
+        del f, keep
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("configs", nargs="*", default=["c1", "c3", "c5"])
@@ -373,6 +421,8 @@ def main():
         c7(a)
     if "c8" in a.configs:
         c8(a)
+    if "c9" in a.configs:
+        c9(a)
     if "c3" in a.configs:
         nf, nd = int(100_000_000 * a.scale), int(10_000_000 * a.scale)
         fs = [(0, 1, T.INT32, 0, 1, 0, nd, 1.0), (0, 2, T.DOUBLE, 1, 2, 0, 0, 1.0)]

@@ -239,6 +239,27 @@ static int alloc_group_table(bkgpu_plan* p) {
 
 namespace { int cpu_budget(); }   // CPUs this process may use (affinity, cgroup quota): defined with the copy pool
 
+// the plan's IN sets (OP_IN_SET) in one device allocation, kept until bkgpu_close (bkgpu_reset keeps them), and their addresses
+// patched into every program that probes them.  Part of opening the plan, not of a request: not counted in h2d_bytes.
+static int upload_in_sets(bkgpu_plan* p) {
+    if (!p->c.in_sets || p->c.in_sets->sets.empty()) return BKGPU_OK;
+    const std::vector<InSet>& sets = p->c.in_sets->sets;
+    size_t words = 0;
+    for (const InSet& s : sets) words += s.image.size();
+    uint64_t* d = nullptr;
+    int rc = dev_alloc(p, (void**)&d, words * 8);
+    if (rc) return rc;
+    std::vector<uint64_t> addr;
+    for (const InSet& s : sets) {
+        addr.push_back((uint64_t)(uintptr_t)d);
+        CK(p, cudaMemcpyAsync(d, s.image.data(), s.image.size() * 8, cudaMemcpyHostToDevice, p->stream));
+        d += s.image.size();
+    }
+    CK(p, cudaStreamSynchronize(p->stream));
+    patch_in_sets(p->c, addr);
+    return BKGPU_OK;
+}
+
 extern "C" int bkgpu_open(bkgpu_plan* p) {
     if (!p) return thread_fail(BKGPU_EINVAL, "bkgpu_open: NULL plan");
     if (p->state != S_INIT) return p->fail(BKGPU_ESTATE, "bkgpu_open called twice");
@@ -251,7 +272,8 @@ extern "C" int bkgpu_open(bkgpu_plan* p) {
         CK(p, cudaEventCreateWithFlags(&p->stage_ready[i], cudaEventDisableTiming));
     }
     p->blocking_wait = p->blocking_sync >= 0 ? p->blocking_sync != 0 : (p->nranks > 1 && cpu_budget() < 4 * p->nranks);
-    int rc = BKGPU_OK;
+    int rc = upload_in_sets(p);   // (before sort_open: it copies the programs)
+    if (rc) return rc;
     if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) rc = alloc_group_table(p);
     if (!rc && (p->c.kind == PK_SORT || p->c.kind == PK_FILTER || p->c.kind == PK_WINDOW))   // (a window retains its rows like a full sort)
         rc = sort_check(p, sort_open(p->c, p->device, p->stream, p->region_base, &p->sort, p->last_error));

@@ -16,7 +16,7 @@ enum VClass : uint8_t { VC_I64 = 0, VC_U64 = 1, VC_F64 = 2 };
 
 constexpr int MAX_COLS = 16;      // distinct input columns one kernel can reference
 constexpr int MAX_INSTR = 96;     // bytecode length
-constexpr int MAX_CONST = 64;     // constant pool (literals + IN lists)
+constexpr int MAX_CONST = 64;     // constant pool (literals + IN lists + the address of each IN set)
 constexpr int MAX_KEYW = 8;       // 64-bit words of a packed GROUP BY key (incl. the null-flag word)
 constexpr int MAX_GROUP = 8;      // GROUP BY expressions: encode_exprs_key has 8 null-flag bits
 constexpr int MAX_AGG = 12;       // aggregate functions per AggNode
@@ -69,6 +69,7 @@ enum Op : uint8_t {
     OP_MATH,         // a = MathFn on a DOUBLE image, b = constant index (round: 10^bits)   internal_functions.cpp:52-99
     OP_MATH2,        // a = Math2Fn: pops [x, y] DOUBLE images, NULL if either is or outside the domain   internal_functions.cpp:114-127,234-317
     OP_DATEFN,       // a = DateFn, b = mode / unit (datetime.h), c = arguments popped (1, or 2 for datediff); NULL in -> NULL
+    OP_IN_SET,       // a = constant holding the set's device address, b = set index in the plan, c = as OP_IN   (in_set.h)
 };
 enum MathFn : uint8_t { MF_ABS = 0, MF_FLOOR = 1, MF_CEIL = 2, MF_ROUND = 3,
                         // one DOUBLE argument, NULL outside the domain (internal_functions.cpp:101-232); SIGN and BIT_COUNT leave an INT64 image

@@ -2,6 +2,7 @@
 // sort / filter kernels (sort.cu): postfix bytecode lowered by plan.cpp, warp-uniform dispatch.
 #pragma once
 #include "dev_common.cuh"
+#include "in_set.h"
 
 namespace bk {
 
@@ -11,6 +12,8 @@ namespace bk {
 // ------------------------------------------------------------------------------------------
 // OP_DATEFN's calendar code (datetime.h), out of line: one call site keeps it out of run_program's registers
 static __device__ __noinline__ uint64_t date_fn(uint32_t fn, uint32_t arg, uint64_t x, uint64_t x2) { return dt_date_fn((int)fn, (int)arg, x, x2); }
+// OP_IN_SET's probe of the hashed set at device address `set` (in_set.h), out of line for the same reason
+static __device__ __noinline__ bool in_set_probe(uint64_t set, uint64_t x, uint32_t vclass) { return in_set_contains((const uint64_t*)set, x, (int)vclass); }
 
 // `brow`: row of the join's build side; LOAD_COL instructions with c == 1 read there (the joined row of
 // Joiner::construct_result_batch, src/exec/joiner.cpp:633-685, without materialising it)
@@ -130,6 +133,13 @@ static __device__ __noinline__ void run_program(const Program& p, const DevCol* 
                     if (!found && (in.c >> 4)) nul |= 1u << (sp - 1);  // not found and the list holds a NULL
                 }
             } break;
+            case OP_IN_SET:
+                if (!((nul >> (sp - 1)) & 1u)) {
+                    const bool found = in_set_probe(p.cbits[in.a], st[sp - 1], in.c & 0xF);
+                    st[sp - 1] = found ? 1ull : 0ull;
+                    if (!found && (in.c >> 4)) nul |= 1u << (sp - 1);
+                }
+                break;
             case OP_SELECT: {   // get_numberic<bool>() of a NULL condition is false
                 sp -= 2;
                 const bool take_a = !((nul >> (sp - 1)) & 1u) && st[sp - 1] != 0;

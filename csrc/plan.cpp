@@ -17,8 +17,12 @@
 #include <map>
 #include "../include/bkgpu.h"
 #include "datetime.h"
+#include "in_set.h"
 
 namespace bk {
+
+constexpr int MAX_IN_LIST = 1 << 22;   // entries of one IN list (the planner writes an IN subquery's result rows into the plan as its list)
+constexpr int MAX_IN_SETS = 256;       // IN sets of one plan (OP_IN_SET's b)
 
 // ---------------------------------------------------------------- type helpers
 static bool is_int_t(int t) { return t >= BK_INT8 && t <= BK_UINT64; }
@@ -144,7 +148,14 @@ static void parse_enode(Reader& r, HExpr& e, int& remaining, int depth) {
             r.bad("LIKE / ROW expressions are outside the GPU path"); return;
         default: r.bad("unknown expr node type"); return;
     }
-    if (nch < 0 || nch > 1024) { r.bad("bad expr num_children"); return; }
+    if (e.node_type == BK_IN_PREDICATE && nch > MAX_IN_LIST + 1) {
+        char buf[128];
+        snprintf(buf, sizeof buf, "IN list of %d entries is longer than %d: outside the GPU path", nch - 1, MAX_IN_LIST);
+        r.bad(buf); return;
+    }
+    if (nch < 0 || (nch > 1024 && e.node_type != BK_IN_PREDICATE)) { r.bad("bad expr num_children"); return; }
+    // (a long list must be there before its children are allocated: each is a node of at least 3 words)
+    if (nch > 1024 && (nch > remaining || (size_t)nch * 3 > r.n - r.pos)) { r.bad("expr node list does not match its node count"); return; }
     e.ch.resize((size_t)nch);
     for (int i = 0; i < nch && !r.fail; i++) parse_enode(r, e.ch[(size_t)i], remaining, depth + 1);
 }
@@ -631,16 +642,15 @@ struct Lower {
                 int map_type = e.arg_types[0];
                 if (!expr(e.ch[0], depth) || !cast(e.ch[0].col_type, map_type)) return false;
                 int first = out->n_const, cnt = 0; bool has_null = false;
-                for (size_t i = 1; i < e.ch.size(); i++) {
-                    const HExpr& c = e.ch[i];
-                    if (c.lit_null) { has_null = true; continue; }
-                    uint64_t bits = c.col_type ? host_cast_prim(c.lit_bits, c.lit_prim, c.col_type) : c.lit_bits;  // Literal::get_value
-                    bits = host_cast_prim(bits, c.col_type ? c.col_type : c.lit_prim, map_type);                  // value.cast_to(_map_type)
-                    if (add_const(bits, false) < 0) return false;
-                    cnt++;
+                for (size_t i = 1; i < e.ch.size(); i++) { if (e.ch[i].lit_null) has_null = true; else cnt++; }
+                const uint8_t flags = (uint8_t)((has_null ? 16 : 0) | host_prim_class(map_type));
+                if (cnt > 255 || out->n_const + cnt > MAX_CONST) {   // a list the constant pool cannot hold is probed as a hashed set
+                    const int s = in_set(e, map_type, has_null), k = s < 0 ? -1 : add_const(0, false);
+                    return k >= 0 && emit(OP_IN_SET, (uint8_t)k, (uint8_t)s, flags);
                 }
-                if (cnt > 255) return in->fail(BKGPU_EUNSUPPORTED, "IN list longer than 255");
-                return emit(OP_IN, (uint8_t)first, (uint8_t)cnt, (uint8_t)((has_null ? 16 : 0) | host_prim_class(map_type)));
+                for (size_t i = 1; i < e.ch.size(); i++)
+                    if (!e.ch[i].lit_null && add_const(in_entry(e.ch[i], map_type), false) < 0) return false;
+                return emit(OP_IN, (uint8_t)first, (uint8_t)cnt, flags);
             }
             case BK_FUNCTION_CALL: {
                 if (e.fn_op == BK_FT_COMMON) return common_fn(e, depth);
@@ -672,6 +682,27 @@ struct Lower {
             }
             default: return in->fail(BKGPU_EUNSUPPORTED, "expr node type %d cannot be lowered", e.node_type);
         }
+    }
+    // an IN list entry as the image of the set's type
+    static uint64_t in_entry(const HExpr& c, int map_type) {
+        const uint64_t bits = c.col_type ? host_cast_prim(c.lit_bits, c.lit_prim, c.col_type) : c.lit_bits;   // Literal::get_value
+        return host_cast_prim(bits, c.col_type ? c.col_type : c.lit_prim, map_type);                          // value.cast_to(_map_type)
+    }
+    // the set of `e`'s entries: built at its first lowering, found again at the next (jfast lowers the same expressions)
+    int in_set(const HExpr& e, int map_type, bool has_null) {
+        InSets& reg = *out->in_sets;
+        for (auto& x : reg.of_expr) if (x.first == &e) return x.second;
+        if ((int)reg.sets.size() >= MAX_IN_SETS) { in->fail(BKGPU_EUNSUPPORTED, "more than %d long IN lists in one plan", MAX_IN_SETS); return -1; }
+        std::vector<uint64_t> v;
+        v.reserve(e.ch.size() - 1);
+        for (size_t i = 1; i < e.ch.size(); i++) if (!e.ch[i].lit_null) v.push_back(in_entry(e.ch[i], map_type));
+        InSet s;
+        s.vclass = host_prim_class(map_type);
+        s.has_null = has_null;
+        s.image = in_set_build(v.data(), v.size(), s.vclass, &s.n_distinct);
+        reg.sets.push_back(std::move(s));
+        reg.of_expr.push_back({&e, (int)reg.sets.size() - 1});
+        return (int)reg.sets.size() - 1;
     }
     // named builtins (FT_COMMON): arguments are NOT cast (arg_types stay empty), the result is cast to the node's col_type
     bool branch(const HExpr& c, int to, int& depth) { return expr(c, depth) && cast(c.col_type, to); }
@@ -1080,8 +1111,15 @@ static bool lower_agg(Infer& in, Compiled& out, const HNode& agg, const std::vec
 // ---------------------------------------------------------------- explain
 static const char* op_name(int op) {
     static const char* n[] = {"END", "LOAD_COL", "CONST", "CAST", "CMP", "ARITH", "DIV_F64", "MOD", "BIT", "BIT_NOT", "NEG",
-                              "LOGIC_NOT", "AND", "OR", "XOR", "NOT3", "IS_NULL", "IS_TRUE", "IN", "OUT", "SELECT", "IFNULL", "MATH", "MATH2", "DATEFN"};
-    return op >= 0 && op <= OP_DATEFN ? n[op] : "?";
+                              "LOGIC_NOT", "AND", "OR", "XOR", "NOT3", "IS_NULL", "IS_TRUE", "IN", "OUT", "SELECT", "IFNULL", "MATH", "MATH2", "DATEFN", "IN_SET"};
+    return op >= 0 && op <= OP_IN_SET ? n[op] : "?";
+}
+// an IN set's shape (never its entries)
+static std::string in_set_text(const InSet& s) {
+    char buf[160];
+    const size_t cap = s.image.size() - IN_SET_HEADER;
+    snprintf(buf, sizeof buf, "distinct=%u capacity=%zu class=%d null=%d bytes=%zu", s.n_distinct, cap, s.vclass, (int)s.has_null, s.image.size() * 8);
+    return buf;
 }
 static void explain(Compiled& c) {
     char buf[256];
@@ -1149,8 +1187,26 @@ static void explain(Compiled& c) {
         const Instr& in = c.prog.code[i];
         snprintf(buf, sizeof buf, "  %02d %-9s a=%d b=%d c=%d", i, op_name(in.op), in.a, in.b, in.c); s += buf;
         if (in.op == OP_CONST) { snprintf(buf, sizeof buf, "   ; 0x%llx%s", (unsigned long long)c.prog.cbits[in.a], ((c.prog.cnull >> in.a) & 1) ? " NULL" : ""); s += buf; }
+        if (in.op == OP_IN_SET) s += "   ; set " + std::to_string(in.b) + ": " + in_set_text(c.in_sets->sets[in.b]);
         s += "\n";
     }
+    if (c.in_sets && !c.in_sets->sets.empty()) {   // every set of the plan, whichever of its programs probes it
+        size_t bytes = 0;
+        for (auto& x : c.in_sets->sets) bytes += x.image.size() * 8;
+        snprintf(buf, sizeof buf, "in sets: %zu, %zu bytes\n", c.in_sets->sets.size(), bytes); s += buf;
+        for (size_t i = 0; i < c.in_sets->sets.size(); i++) s += "  set " + std::to_string(i) + ": " + in_set_text(c.in_sets->sets[i]) + "\n";
+    }
+}
+
+void patch_in_sets(Compiled& c, const std::vector<uint64_t>& addr) {
+    auto fix = [&](Program& q) {
+        for (int i = 0; i < q.n_instr; i++) if (q.code[i].op == OP_IN_SET) q.cbits[q.code[i].a] = addr[q.code[i].b];
+    };
+    fix(c.prog);
+    for (StarDim& d : c.dims) fix(d.filter);
+    for (WinStage& w : c.win) for (Program& q : w.exprs) fix(q);
+    if (c.post) patch_in_sets(*c.post, addr);
+    if (c.jfast) patch_in_sets(*c.jfast, addr);
 }
 
 // ---------------------------------------------------------------- entry
@@ -1201,6 +1257,7 @@ int compile_plan(const uint8_t* desc, size_t len, Compiled& out, std::string& er
     if (r.fail) { err = r.err; return r.err.find("outside the GPU path") != std::string::npos ? BKGPU_EUNSUPPORTED : BKGPU_EINVAL; }
     Infer in{}; in.tuples = &out.tuples;
     if (!infer_node(in, root)) { err = in.err; return in.code; }
+    out.in_sets = std::make_shared<InSets>();
 
     bool under_packet = false;
     const HNode* top = skip_passthrough(&root, &under_packet);
@@ -1363,6 +1420,7 @@ bool lower_post(Infer& in, Compiled& out, const HNode* sort, const HNode* having
     pc.kind = sort ? PK_SORT : PK_FILTER;
     pc.tuples = out.tuples;
     pc.scan_tuple = -1;
+    pc.in_sets = out.in_sets;
     Program& p = pc.prog; memset(&p, 0, sizeof p);
     memset(&pc.ap, 0, sizeof pc.ap);
     Lower lw{&pc, &in, &p, {}};
@@ -1468,7 +1526,7 @@ bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
     // fast path: lower the same aggregate again with every column treated as a column of ONE (virtual, joined) tuple
     if (jt == BK_INNER_JOIN) {
         auto jf = std::make_shared<Compiled>();
-        jf->tuples = out.tuples; jf->build_tuple = -1;
+        jf->tuples = out.tuples; jf->build_tuple = -1; jf->in_sets = out.in_sets;
         Infer in2{}; in2.tuples = &jf->tuples;
         if (lower_agg(in2, *jf, agg, conj, probe_tuple, under_packet, true) && memcmp(&jf->ap.n_keyw, &out.ap.n_keyw, sizeof(int32_t) * 4) == 0 &&
             jf->ap.n_lanes == out.ap.n_lanes) {
@@ -1598,7 +1656,7 @@ bool lower_star_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
     }
     // the aggregate over the gathered chunk: every column as a column of ONE (virtual, joined) tuple
     auto jf = std::make_shared<Compiled>();
-    jf->tuples = out.tuples; jf->build_tuple = -1;
+    jf->tuples = out.tuples; jf->build_tuple = -1; jf->in_sets = out.in_sets;
     Infer in2{}; in2.tuples = &jf->tuples;
     if (!lower_agg(in2, *jf, agg, conj, fact, under_packet, true) || memcmp(&jf->ap.n_keyw, &out.ap.n_keyw, sizeof(int32_t) * 4) != 0 || jf->ap.n_lanes != out.ap.n_lanes)
         return in.fail(BKGPU_EUNSUPPORTED, "the aggregate over the joined row could not be lowered: %s", in2.err.c_str());
@@ -1690,7 +1748,7 @@ bool lower_join_rows(Infer& in, Compiled& out, const HNode& join, const HNode* a
     auto post = std::make_shared<Compiled>();
     Compiled& pc = *post;
     pc.kind = sort ? PK_SORT : PK_FILTER;
-    pc.tuples = out.tuples; pc.scan_tuple = -1;
+    pc.tuples = out.tuples; pc.scan_tuple = -1; pc.in_sets = out.in_sets;
     Program& pp = pc.prog; memset(&pp, 0, sizeof pp);
     memset(&pc.ap, 0, sizeof pc.ap);
     pc.ap.pred_out = -1;

@@ -103,6 +103,19 @@ struct WinStage {
     std::vector<WinFn> fns;
 };
 
+// An IN list lowered to OP_IN_SET: the hashed set of its entries (in_set.h), built once per IN expression and shared by every
+// program lowered from it (a join's jfast lowers the same conjuncts again).  bkgpu_open uploads all of a plan's sets in one allocation.
+struct InSet {
+    int vclass = 0;
+    bool has_null = false;             // the list held a NULL literal: a miss is NULL
+    uint32_t n_distinct = 0;
+    std::vector<uint64_t> image;       // the device image: header + slots
+};
+struct InSets {
+    std::vector<InSet> sets;           // index = OP_IN_SET's b
+    std::vector<std::pair<const HExpr*, int>> of_expr;   // (IN expression, set index)
+};
+
 struct Compiled {
     int kind = 0;
     std::vector<HTuple> tuples;
@@ -143,11 +156,15 @@ struct Compiled {
     // window (PK_WINDOW): the stages bottom-up; the output rows are the scan tuple's slots (out_cols) followed by one column per window
     // function, in the topmost stage's sort order.  `post` (kind PK_SORT), when present, is the query's ORDER BY over those rows.
     std::vector<WinStage> win;
+    // the plan's IN sets, shared with its post and jfast fragments
+    std::shared_ptr<InSets> in_sets;
     std::string explain;
 };
 
 // returns 0 or a negative BKGPU_E* code; `err` receives the message
 int compile_plan(const uint8_t* desc, size_t len, Compiled& out, std::string& err);
+// every program of the plan (main, post, jfast, star dimensions' filters, window stages' expressions): OP_IN_SET's constant := addr[set]
+void patch_in_sets(Compiled& c, const std::vector<uint64_t>& addr);
 
 // host-side ExprValue::cast_to on canonical images (x86 semantics == the reference's build)
 uint64_t host_cast_prim(uint64_t v, int from, int to);
