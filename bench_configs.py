@@ -3,7 +3,7 @@
 device-resident synthetic columns (SURVEY.md §8d), CUDA events around reset+push+finish+get_next, one JSON line per
 config with rows/s and achieved GB/s on the config's algorithmic bytes.  The headline line is bench.py's;
 this script measures the side configs on their own (C6, the star join, also its kernels, a parity flag and the Acero time).
-usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [c9] [--scale 0.1] [--steps 10]"""
+usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [c9] [c10] [--scale 0.1] [--steps 10]"""
 import argparse
 import ctypes
 import json
@@ -364,6 +364,91 @@ def c9(a):
         del f, keep
 
 
+def c10(a):
+    """C10, a FULL OUTER join: 100M device-resident fact rows FULL-joined to 10M dimension rows on an INT32 key, GROUP BY a dimension attribute,
+    COUNT(*), SUM(x).  About 5 % of the fact keys and 10 % of the dimension keys have no partner, and one key in 32768 on either side is NULL.
+    Besides the step: the time of the pair kernel, of the gathers and of the aggregate kernel (torch.profiler, a run of its own), parity of
+    every group against torch, the same query as LEFT and as INNER through the general path (option force_generic), and Acero's full outer
+    hashjoin + aggregate over the same rows on the host CPUs."""
+    import time
+    from baikaldb_b200 import plan as P
+    nf, nd = int(100_000_000 * a.scale), int(10_000_000 * a.scale)
+    gen_ = torch.Generator(device="cuda").manual_seed(10)
+    key = torch.randperm(nd, device="cuda", generator=gen_).to(torch.int32)
+    attr = (key % 1000 + 1).to(torch.int32)                     # groups 1..1000 (the NULL group extracts as 0)
+    lo = nd // 10                                                # dimension keys below lo have no fact row
+    fk = torch.randint(lo, lo + int((nd - lo) / 0.95), (nf,), device="cuda", generator=gen_, dtype=torch.int32)   # ~5 % above nd - 1
+    x = torch.rand(nf, device="cuda", dtype=torch.float64, generator=gen_)
+    def bitmap(n):   # one NULL in 32768 rows
+        b = torch.full(((n + 7) // 8 + 64,), 0xFF, dtype=torch.uint8, device="cuda")
+        b[::4096] = 0xFE
+        return b
+    fbits, dbits = bitmap(nf), bitmap(nd)
+    fvalid = ((fbits[torch.arange(nf, device="cuda") >> 3] >> (torch.arange(nf, device="cuda") & 7)) & 1).bool()
+    dvalid = ((dbits[torch.arange(nd, device="cuda") >> 3] >> (torch.arange(nd, device="cuda") & 7)) & 1).bool()
+    tup = {0: [(1, T.INT32), (2, T.DOUBLE)], 1: [(1, T.INT32), (2, T.INT32)]}
+    aggs = [P.agg_expr("count_star", 2, 1), P.agg_expr("sum", 2, 2, None, P.slot_ref(0, 2, T.DOUBLE))]
+    tup[2] = P.agg_tuple_slots(aggs, [T.INT64, T.DOUBLE])
+    def plan(jt):
+        j = P.join(P.scan(1), P.scan(0), [P.eq(P.slot_ref(1, 1, T.INT32), P.slot_ref(0, 1, T.INT32))], join_type=jt)
+        return P.Plan(P.agg(j, 2, [P.slot_ref(1, 2, T.INT32)], aggs), tup)
+    darr, farr = cols_array([(1, 1, T.INT32), (1, 2, T.INT32)], [key, attr]), cols_array([(0, 1, T.INT32), (0, 2, T.DOUBLE)], [fk, x])
+    darr[0].validity, farr[0].validity = dbits.data_ptr(), fbits.data_ptr()
+    pushes = [(darr, 2, nd), (farr, 2, nf)]
+    steps = max(1, a.steps // 3)
+    line, got = run("C10 fact FULL JOIN dim ON int32 key, GROUP BY dim attr, COUNT(*), SUM(x) (100M x 10M)", plan(P.JoinType.FULL_JOIN), pushes, nf,
+                    12 * nf + 8 * nd, steps, 1, options=[(b"group_capacity_log2", 14)], collect=True, emit=False)
+    # parity: the partner of every fact row through the dimension's key -> row map, the unmatched rows of both sides NULL-extended
+    row_of = torch.full((nd,), -1, dtype=torch.int64, device="cuda")
+    row_of[key[dvalid].long()] = torch.arange(nd, device="cuda")[dvalid]
+    in_range = fvalid & (fk < nd)
+    partner = torch.full((nf,), -1, dtype=torch.int64, device="cuda")
+    partner[in_range] = row_of[fk[in_range].long()]
+    hit = partner >= 0
+    grp = torch.zeros(nf, dtype=torch.int64, device="cuda")      # 0 = the NULL group
+    grp[hit] = attr[partner[hit]].long()
+    matched = torch.zeros(nd, dtype=torch.bool, device="cuda"); matched[partner[hit]] = True
+    cnt = torch.bincount(grp, minlength=1001) + torch.bincount(attr[~matched].long(), minlength=1001)
+    sm = torch.zeros(1001, dtype=torch.float64, device="cuda").index_add_(0, grp, x)
+    cnt, sm = cnt.cpu().numpy(), sm.cpu().numpy()
+    r = line["result_rows"]
+    kk, gc, gs = (np.array(got[c][:r]) for c in ("1_2", "2_1", "2_2"))
+    want_groups = set(np.nonzero(cnt)[0].tolist())
+    line["parity_vs_torch_all_groups"] = bool(set(kk.tolist()) == want_groups and len(kk) == len(want_groups) and np.array_equal(gc, cnt[kk])
+                                              and np.allclose(gs, sm[kk], rtol=1e-9, atol=1e-9))
+    line["unmatched_fact_rows"] = int((~hit).sum()); line["unmatched_dim_rows"] = int((~matched).sum())
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        run("profile", plan(P.JoinType.FULL_JOIN), pushes, nf, 0, steps, 1, options=[(b"group_capacity_log2", 14)], emit=False)
+        torch.cuda.synchronize()
+    dev = lambda e: getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) / 1e3 / (steps + 1)   # (the profiled run: 1 warm-up + steps)
+    ka = prof.key_averages()
+    line["k_join_pairs_full_ms_per_step"] = sum(dev(e) for e in ka if "k_join_pairs_full" in e.key)
+    line["gather_ms_per_step (k_join_rows_gather + k_pack_validity)"] = sum(dev(e) for e in ka if "k_join_rows_gather" in e.key or "k_pack_validity" in e.key)
+    line["aggregate_kernel_ms_per_step"] = sum(dev(e) for e in ka if line["main_kernel"] in e.key)
+    for name, jt in (("left", P.JoinType.LEFT_JOIN), ("inner", P.JoinType.INNER_JOIN)):
+        o = run(f"the same query as {name.upper()}, general path", plan(jt), pushes, nf, 12 * nf + 8 * nd, steps, 1,
+                options=[(b"group_capacity_log2", 14), (b"force_generic", 1)], emit=False)
+        line[f"{name}_force_generic_ms_per_step"] = o["ms_per_step"]
+    # Acero's full outer hashjoin + aggregate over the same rows on the host CPUs (table construction not timed)
+    import pyarrow as pa, pyarrow.acero as ac
+    ft = pa.table({"0_1": pa.array(fk.cpu().numpy(), mask=~fvalid.cpu().numpy()), "0_2": pa.array(x.cpu().numpy())})
+    dt = pa.table({"1_1": pa.array(key.cpu().numpy(), mask=~dvalid.cpu().numpy()), "1_2": pa.array(attr.cpu().numpy())})
+    j = ac.Declaration("hashjoin", ac.HashJoinNodeOptions("full outer", ["1_1"], ["0_1"]),
+                       inputs=[ac.Declaration("table_source", ac.TableSourceNodeOptions(dt)), ac.Declaration("table_source", ac.TableSourceNodeOptions(ft))])
+    agg = ac.Declaration("aggregate", ac.AggregateNodeOptions([([], "hash_count_all", None, "2_1"), ("0_2", "hash_sum", None, "2_2")], keys=["1_2"]), inputs=[j])
+    t0 = time.perf_counter(); at = agg.to_table(use_threads=True); line["acero_full_outer_host_s"] = time.perf_counter() - t0
+    line["acero_groups"] = at.num_rows
+    line["acero_host_cpus"] = os.cpu_count()
+    line["gpu"] = torch.cuda.get_device_name(0)
+    try:
+        import subprocess
+        line["power_limit"] = subprocess.check_output(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"], text=True).split("\n")[0].strip()
+    except Exception:
+        line["power_limit"] = None
+    print(json.dumps(line), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("configs", nargs="*", default=["c1", "c3", "c5"])
@@ -423,6 +508,8 @@ def main():
         c8(a)
     if "c9" in a.configs:
         c9(a)
+    if "c10" in a.configs:
+        c10(a)
     if "c3" in a.configs:
         nf, nd = int(100_000_000 * a.scale), int(10_000_000 * a.scale)
         fs = [(0, 1, T.INT32, 0, 1, 0, nd, 1.0), (0, 2, T.DOUBLE, 1, 2, 0, 0, 1.0)]

@@ -137,6 +137,44 @@ __global__ void __launch_bounds__(256) k_join_pairs(const __grid_constant__ AggA
         }
     }
 }
+// FULL (Acero's FULL_OUTER hashjoin with the residual conditions as its filter, join_node.cpp:857-875): a probe row leaves one pair per partner
+// that satisfies the conditions (setting matched[]), or one (row, JOIN_NO_ROW) when none does — a NULL key included.  Every probe row emits,
+// so output slots are reserved per warp and round (ballot + one cursor atomic) rather than per pair.  Same capacity contract as k_join_pairs;
+// the tail (unmatched build rows) is k_join_pairs' tail branch.
+__global__ void __launch_bounds__(256) k_join_pairs_full(const __grid_constant__ AggArgs a, uint32_t* pairs, uint32_t cap, uint32_t* cursor) {
+    InterpCtx cx; cx.grouped = false; cx.use_smem = false; cx.gcap = 0; cx.st = SmemTable{};
+    const int lane = threadIdx.x & 31;
+    const uint32_t lt = (1u << lane) - 1u;
+    const DevCol& pc = a.cols[a.join.probe_col];
+    for (int64_t w0 = (int64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31); w0 < a.nrows; w0 += (int64_t)gridDim.x * blockDim.x) {   // (warp-uniform: the ballots)
+        const int64_t row = w0 + lane;
+        int state = 0;   // 0 = done, 1 = walking the multimap, 2 = no partner passed: the NULL-extended pair is due
+        bool found = false;
+        uint64_t img = 0; uint32_t slot = 0;
+        if (row < a.nrows) {
+            if (elem_is_null(pc, row)) state = 2;
+            else { img = cast_prim(load_elem(pc, row), a.join.probe_prim, a.join.cast_prim); slot = hash_key1(img) & a.join.cap_mask; state = 1; }
+        }
+        for (;;) {   // one round: every lane emits at most one pair
+            uint32_t br = JOIN_NO_ROW;
+            bool emit = false;
+            while (state == 1) {
+                const uint32_t s = slot, r = a.join.rows[s];
+                if (r == 0xFFFFFFFFu) { state = found ? 0 : 2; break; }
+                slot = (slot + 1) & a.join.cap_mask;
+                if (a.join.keys[s] == img && interp_row(a, cx, row, (int64_t)r, 1)) { a.join.matched[r] = 1; found = true; br = r; emit = true; break; }
+            }
+            if (state == 2) { emit = true; state = 0; }
+            const uint32_t b = __ballot_sync(0xFFFFFFFFu, emit);
+            if (!b) break;   // (a lane still walking always emits: no emitter means every lane is done)
+            uint32_t base = 0;
+            if (lane == 0) base = atomicAdd(cursor, (uint32_t)__popc(b));
+            base = __shfl_sync(0xFFFFFFFFu, base, 0);
+            const uint32_t pos = base + (uint32_t)__popc(b & lt);
+            if (emit && pos < cap) { pairs[2 * (size_t)pos] = (uint32_t)row; pairs[2 * (size_t)pos + 1] = br; }
+        }
+    }
+}
 // one output column of the joined rows: element `which` of each row-id tuple (`width` row ids: (probe, build) pairs of a two-table join,
 // [fact, dim x D] of a star join) addresses `src`; JOIN_NO_ROW (the NULL-extended side) gives NULL.  dst_null may be nullptr when no
 // element can be NULL
@@ -716,7 +754,8 @@ cudaError_t launch_join_pairs(const AggArgs& a, uint32_t* pairs, uint32_t cap, u
     if (n == 0) return cudaSuccess;
     int64_t g64 = (n + 255) / 256; if (g64 > (int64_t)sm_count * 8) g64 = (int64_t)sm_count * 8;
     const int grid = g64 < 1 ? 1 : (int)g64;
-    k_join_pairs<<<grid, 256, 0, s>>>(a, pairs, cap, cursor);
+    if (a.join.join_type == 6 /*FULL*/ && !a.join.tail) k_join_pairs_full<<<grid, 256, 0, s>>>(a, pairs, cap, cursor);
+    else k_join_pairs<<<grid, 256, 0, s>>>(a, pairs, cap, cursor);
     return cudaGetLastError();
 }
 cudaError_t launch_join_rows_gather(const DevCol& src, const uint32_t* tuples, int width, int which, uint32_t n, int eb, uint8_t* dst, uint8_t* dst_null, cudaStream_t s) {

@@ -16,7 +16,7 @@ struct JoinArgs {
     // LEFT / SEMI / ANTI_SEMI (the build side = the reference's outer / driver table is the preserved side, join_node.cpp:1200-1276,
     // joiner.cpp:633-685): `matched[build row]` is set by the probe; the TAIL launch (tail = 1) walks the n_build build rows and emits the
     // unmatched ones NULL-extended (LEFT), the matched ones (SEMI) or the unmatched ones (ANTI_SEMI)
-    int32_t join_type;       // pb::JoinType: 1 LEFT, 3 INNER, 4 SEMI, 5 ANTI_SEMI (RIGHT arrives as LEFT with the children swapped)
+    int32_t join_type;       // pb::JoinType: 1 LEFT, 3 INNER, 4 SEMI, 5 ANTI_SEMI, 6 FULL (RIGHT arrives as LEFT with the children swapped)
     int32_t tail;
     uint8_t* matched;
     int64_t n_build;
@@ -108,6 +108,7 @@ cudaError_t launch_join_compose(const JoinFast& jf, const uint32_t* attr_by_row,
 cudaError_t launch_unpack_validity(const uint8_t* bitmap, int64_t n, uint8_t* null_bytes, cudaStream_t s);
 cudaError_t launch_pack_validity(const uint8_t* null_bytes, int64_t n, uint8_t* bitmap, cudaStream_t s);
 // a JOIN that returns rows: (probe row, build row) pairs of the joined rows that pass the conditions, then one gather per output column
+// (FULL, not the tail: k_join_pairs_full, which also emits the probe rows without a partner)
 cudaError_t launch_join_pairs(const AggArgs& a, uint32_t* pairs, uint32_t cap, uint32_t* cursor, int sm_count, cudaStream_t s);
 // element `which` of each `width`-word row-id tuple addresses `src` (pairs: width 2); dst_null may be nullptr when no element can be NULL
 cudaError_t launch_join_rows_gather(const DevCol& src, const uint32_t* tuples, int width, int which, uint32_t n, int elem_bytes, uint8_t* dst, uint8_t* dst_null, cudaStream_t s);

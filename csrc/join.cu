@@ -246,7 +246,7 @@ static int join_build_table(bkgpu_plan* p) {
     s.jf = JoinFast{}; j.jp = JoinProbe{};
     bool build_nulls = false;
     for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] == 1 && s.has_null[i]) build_nulls = true;   // gathered columns must be NULL-free
-    if (!c.jfast || build_nulls) return BKGPU_OK;
+    if (!c.jfast || c.join_type == BK_FULL_JOIN || build_nulls) return BKGPU_OK;
     return join_build_index(p, s, side_col(c, s, (size_t)c.build_key_col), c.join_key_prim, true);
 }
 
@@ -336,8 +336,9 @@ static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nro
     return launch_agg_batch(p, c, all.data(), nrows, false);
 }
 
-// ---- a JOIN that returns rows (PK_JOIN): pairs -> gather -> the sink fragment (p->post_sort) ----
-static int join_rows_emit(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t n_probe, bool tail) {
+// the (probe row, build row) pairs of `n_probe` probe rows (`all`: every plan column, the probe side's at the rows' start), or of the
+// outer-join tail, into j.pairs; *found = their number
+static int join_pairs(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t n_probe, bool tail, uint32_t* found) {
     const Compiled& c = p->c;
     JoinState& j = p->join;
     int rc;
@@ -348,17 +349,26 @@ static int join_rows_emit(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t
     a.n_cols = ncols;
     a.join = join_args(p, tail);
     if ((rc = ensure_buf(p, (void**)&j.cursor, &j.cursor_cap, 64))) return rc;
-    uint32_t found = 0;
-    rc = run_counted(p, (uint64_t)std::max<int64_t>(tail ? j.side[0].rows : n_probe, 1 << 12), j.cursor, &found, [&](uint64_t want) -> int {
+    *found = 0;
+    return run_counted(p, (uint64_t)std::max<int64_t>(tail ? j.side[0].rows : n_probe, 1 << 12), j.cursor, found, [&](uint64_t want) -> int {
         if (want > 0x7FFFFFF0ull) return p->fail(BKGPU_ETOOBIG, "a probe batch joins to more than 2^31 rows: push smaller batches");
         int r;
         if ((r = ensure_buf(p, (void**)&j.pairs, &j.pairs_cap, (size_t)want * 8))) return r;
         CK(p, cudaMemsetAsync(j.cursor, 0, 4, p->stream));
-        // (a rerun of a LEFT batch sets the same matched[] flags again: they only ever go from 0 to 1)
+        // (a rerun of a LEFT / FULL batch sets the same matched[] flags again: they only ever go from 0 to 1)
         CK(p, launch_join_pairs(a, j.pairs, (uint32_t)want, j.cursor, p->sm_count, p->stream));
         p->stats.kernel_launches++;
         return BKGPU_OK;
     });
+}
+
+// ---- a JOIN that returns rows (PK_JOIN): pairs -> gather -> the sink fragment (p->post_sort) ----
+static int join_rows_emit(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t n_probe, bool tail) {
+    const Compiled& c = p->c;
+    JoinState& j = p->join;
+    int rc;
+    uint32_t found = 0;
+    rc = join_pairs(p, all, n_probe, tail, &found);
     if (rc || !found) return rc;
     const Compiled& pc = *c.post;
     const size_t nc = pc.cols.size();
@@ -382,8 +392,44 @@ static int join_rows_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nrow
     return join_rows_emit(p, join_cols(p, probe_cols), nrows, false);
 }
 
-// LEFT / SEMI / ANTI_SEMI: once every probe batch has run, the preserved (build) side's rows the join type asks for go through the
-// aggregate (PK_JOIN_AGG) or the sink (PK_JOIN) — unmatched rows NULL-extended (LEFT), matched rows (SEMI), unmatched rows (ANTI_SEMI);
+// ---- FULL join under an aggregate (PK_JOIN_AGG): pairs -> gather -> the aggregate over the joined row (Compiled::jfast, whose predicate is
+// the filter above the join).  Never the FK -> PK path: that assumes exactly one partner per probe row. ----
+// the pairs of `n_probe` probe rows (or of the tail), every column jfast reads gathered from its pair (NULL on the side a pair lacks), the aggregate
+static int full_join_agg(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t n_probe, bool tail) {
+    const Compiled& c = p->c;
+    const Compiled& f = *c.jfast;
+    JoinState& j = p->join;
+    uint32_t found = 0;
+    int rc = join_pairs(p, all, n_probe, tail, &found);
+    if (rc || !found) return rc;
+    std::vector<DevCol> fc(f.cols.size());
+    for (size_t i = 0; i < f.cols.size(); i++) {
+        const size_t m = (size_t)c.jfast_of_main[i];
+        if ((rc = chunk_col(p, m, found, true))) return rc;
+        const ChunkCol& g = j.chunk[m];
+        CK(p, launch_join_rows_gather(all[m], j.pairs, 2, c.col_side[m] == 1 ? 1 : 0, found, storage_bytes(all[m].stype), g.vals, g.nullb, p->stream));
+        CK(p, launch_pack_validity(g.nullb, found, g.bits, p->stream));
+        p->stats.kernel_launches += 2;
+        fc[i] = all[m]; fc[i].values = g.vals; fc[i].validity = g.bits;
+    }
+    return launch_agg_batch(p, f, fc.data(), found, true);
+}
+static int full_join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nrows, int64_t, bool) {
+    const Compiled& c = p->c;
+    int rc;
+    if ((rc = join_generic_table(p))) return rc;
+    const std::vector<DevCol> all = join_cols(p, probe_cols);
+    const int64_t chunk = 16 << 20;   // bounds the pairs and the gathered chunk
+    for (int64_t off = 0; off < nrows; off += chunk) {
+        std::vector<DevCol> sl(all);
+        for (size_t i = 0; i < sl.size(); i++) if (c.col_side[i] == 0) sl[i] = col_at(all[i], off);
+        if ((rc = full_join_agg(p, sl, std::min(chunk, nrows - off), false))) return rc;
+    }
+    return BKGPU_OK;
+}
+
+// LEFT / SEMI / ANTI_SEMI / FULL: once every probe batch has run, the preserved (build) side's rows the join type asks for go through the
+// aggregate (PK_JOIN_AGG) or the sink (PK_JOIN) — unmatched rows NULL-extended (LEFT, FULL), matched rows (SEMI), unmatched rows (ANTI_SEMI);
 // join_node.cpp:1200-1276
 int join_tail(bkgpu_plan* p) {
     const Compiled& c = p->c;
@@ -394,6 +440,7 @@ int join_tail(bkgpu_plan* p) {
     if ((rc = join_generic_table(p))) return rc;
     const std::vector<DevCol> all = join_cols(p, nullptr);
     if (c.kind == PK_JOIN) return join_rows_emit(p, all, 0, true);
+    if (c.join_type == BK_FULL_JOIN) return full_join_agg(p, all, 0, true);
     j.tail_launch = true;
     rc = launch_agg_batch(p, c, all.data(), j.side[0].rows, false);
     j.tail_launch = false;
@@ -514,7 +561,8 @@ int join_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows,
     if (side) return join_retain_build(p, side, cols, ncols, nrows, on_device);
     if (!j.built) { int rc = star ? star_build(p) : join_build_table(p); if (rc) return rc; }
     if (j.probe_want.empty()) for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] == 0) { j.probe_want.push_back(c.cols[i]); j.probe_map.push_back((int)i); }
-    return feed(p, j.probe_want, cols, ncols, nrows, on_device, star ? star_probe_batch : c.kind == PK_JOIN ? join_rows_batch : join_probe_batch);
+    return feed(p, j.probe_want, cols, ncols, nrows, on_device, star ? star_probe_batch : c.kind == PK_JOIN ? join_rows_batch :
+                                                                c.join_type == BK_FULL_JOIN ? full_join_probe_batch : join_probe_batch);
 }
 
 void join_reset(bkgpu_plan* p) {

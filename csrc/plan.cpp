@@ -1182,6 +1182,11 @@ static void explain(Compiled& c) {
     } else
     if (c.post) { snprintf(buf, sizeof buf, "post fragment above the aggregate: kind=%d keys=%zu pred_out=%d limit=%lld offset=%lld\n", c.post->kind, c.post->sort_keys.size(),
                            c.post->ap.pred_out, (long long)c.post->limit, (long long)c.post->offset); s += buf; }
+    if (c.join_type == BK_FULL_JOIN) {
+        const bool agg = c.kind == PK_JOIN_AGG;
+        snprintf(buf, sizeof buf, "full join: k_join_pairs_full (the program below: the join conditions) -> gather -> %s; the filter above the join is the %s predicate (pred_out=%d)\n",
+                 agg ? "aggregate over the joined row" : "sink", agg ? "aggregate's" : "sink's", agg ? c.jfast->ap.pred_out : c.post->ap.pred_out); s += buf;
+    }
     snprintf(buf, sizeof buf, "program: %d instr, %d outputs\n", c.prog.n_instr, c.prog.n_out); s += buf;
     for (int i = 0; i < c.prog.n_instr; i++) {
         const Instr& in = c.prog.code[i];
@@ -1472,10 +1477,20 @@ bool lower_post(Infer& in, Compiled& out, const HNode* sort, const HNode* having
 // src/exec/joiner.cpp:624-631); the key is the cast equal-slot value (strip_out_equal_slots, joiner.cpp:166-217).
 // Filters of both children and the residual join conditions become one predicate over the joined row — for an
 // INNER join that is the same set of rows.
+// FULL: the residual conditions decide the pairs (k_join_pairs_full); the filter above the join — the planner keeps a join FULL only under a
+// NULL-tolerant one (join_node.cpp:171-203) — judges every emitted row, NULL-extended ones included, as the predicate of `jfast`, the
+// aggregate over the pairs' gathered columns.
+static void intern_slots(Lower& lw, Infer& in, const HExpr& e) {   // every column `e` reads becomes a plan column
+    if (e.node_type == BK_SLOT_REF) {
+        const int st = in.slot_type(e.tuple_id, e.slot_id);
+        lw.intern_col(e.tuple_id, e.slot_id, st == BK_INVALID_TYPE ? e.col_type : st);
+    }
+    for (auto& c : e.ch) intern_slots(lw, in, c);
+}
 bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& join, bool under_packet, const HNode* above) {
     int jt = join.join_type;
-    if (jt != BK_INNER_JOIN && jt != BK_LEFT_JOIN && jt != BK_RIGHT_JOIN && jt != BK_SEMI_JOIN && jt != BK_ANTI_SEMI_JOIN)
-        return in.fail(BKGPU_EUNSUPPORTED, "join type %d (FULL / NULL) is outside the GPU path", jt);
+    if (jt != BK_INNER_JOIN && jt != BK_LEFT_JOIN && jt != BK_RIGHT_JOIN && jt != BK_SEMI_JOIN && jt != BK_ANTI_SEMI_JOIN && jt != BK_FULL_JOIN)
+        return in.fail(BKGPU_EUNSUPPORTED, "join type %d is outside the GPU path", jt);
     if (join.ch.size() != 2) return in.fail(BKGPU_EINVAL, "JOIN node needs two children");
     const HNode* side[2]; const HNode* filt[2] = {nullptr, nullptr};
     for (int i = 0; i < 2; i++) {
@@ -1490,7 +1505,9 @@ bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
     // the fused predicate (child filters + residual conditions over the joined row) equals filter-then-join only for INNER joins
     // a filter ABOVE the join sees the joined row: for an INNER join it simply joins the residual conditions; above an outer join it would also
     // have to judge the NULL-extended rows, after the match decision — a second predicate the probe does not carry
-    if (jt != BK_INNER_JOIN && above) return in.fail(BKGPU_EUNSUPPORTED, "a filter between the aggregate and a LEFT / SEMI / ANTI join is outside the GPU path");
+    const bool full = jt == BK_FULL_JOIN;
+    if (full && (filt[0] || filt[1])) return in.fail(BKGPU_EUNSUPPORTED, "FULL join over filtered children is outside the GPU path");
+    if (jt != BK_INNER_JOIN && !full && above) return in.fail(BKGPU_EUNSUPPORTED, "a filter between the aggregate and a LEFT / SEMI / ANTI join is outside the GPU path");
     if (jt != BK_INNER_JOIN && (filt[0] || filt[1])) return in.fail(BKGPU_EUNSUPPORTED, "LEFT / SEMI / ANTI join over filtered children is outside the GPU path");
     const int build_tuple = side[0]->tuple_id, probe_tuple = side[1]->tuple_id;
     out.build_tuple = build_tuple;
@@ -1507,7 +1524,8 @@ bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
     }
     if (!bk) return in.fail(BKGPU_EUNSUPPORTED, "join without an equality between the two tables (nested loop) is outside the GPU path");
     for (int i = 0; i < 2; i++) if (filt[i]) for (auto& e : filt[i]->conjuncts) conj.push_back(&e);
-    if (above) for (auto& e : above->conjuncts) conj.push_back(&e);
+    std::vector<const HExpr*> above_conj;
+    if (above) for (auto& e : above->conjuncts) (full ? above_conj : conj).push_back(&e);
     int ot = bk->col_type, it = pk->col_type, cast;
     auto is_signed_t = [](int t) { return t >= BK_INT8 && t <= BK_INT64; };
     if (ot == it) cast = ot;
@@ -1515,20 +1533,29 @@ bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
     else if (is_uint_t(ot) && is_uint_t(it)) cast = BK_UINT64;
     else return in.fail(BKGPU_EUNSUPPORTED, "join keys of types %d and %d are compared as STRING in the reference: outside the GPU path", ot, it);
     if (cast == BK_STRING || is_double_t(cast)) return in.fail(BKGPU_EUNSUPPORTED, "join key type %d is outside the GPU path", cast);
+    if (full && agg.node_type == BK_MERGE_AGG_NODE) return in.fail(BKGPU_EUNSUPPORTED, "MERGE_AGG over a FULL join is outside the GPU path");
     if (!lower_agg(in, out, agg, conj, probe_tuple, under_packet, false)) return false;
+    if (full) {   // the pairs kernel runs the main program for its predicate alone (the residual conditions): the aggregate is jfast's
+        Program& q = out.prog;
+        int n = 0;
+        if (out.ap.pred_out >= 0) { while (n < q.n_instr && !(q.code[n].op == OP_OUT && q.code[n].a == out.ap.pred_out)) n++; n++; }
+        q.n_instr = n; q.n_out = out.ap.pred_out >= 0 ? out.ap.pred_out + 1 : 0;
+    }
     out.kind = PK_JOIN_AGG;
     out.join_type = jt; out.join_key_prim = cast;
     Program dummy; memset(&dummy, 0, sizeof dummy);
     Lower lw{&out, &in, &dummy, {}};
     out.build_key_col = lw.intern_col(bk->tuple_id, bk->slot_id, in.slot_type(bk->tuple_id, bk->slot_id));
     out.probe_key_col = lw.intern_col(pk->tuple_id, pk->slot_id, in.slot_type(pk->tuple_id, pk->slot_id));
+    for (auto* e : above_conj) intern_slots(lw, in, *e);   // (FULL: read by jfast's predicate alone, gathered like the aggregate's columns)
     if ((int)out.cols.size() > MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d columns referenced", MAX_COLS);
-    // fast path: lower the same aggregate again with every column treated as a column of ONE (virtual, joined) tuple
-    if (jt == BK_INNER_JOIN) {
+    // fast path: lower the same aggregate again with every column treated as a column of ONE (virtual, joined) tuple.  FULL: the path
+    // itself, with the filter above the join as the predicate
+    if (jt == BK_INNER_JOIN || full) {
         auto jf = std::make_shared<Compiled>();
         jf->tuples = out.tuples; jf->build_tuple = -1; jf->in_sets = out.in_sets;
         Infer in2{}; in2.tuples = &jf->tuples;
-        if (lower_agg(in2, *jf, agg, conj, probe_tuple, under_packet, true) && memcmp(&jf->ap.n_keyw, &out.ap.n_keyw, sizeof(int32_t) * 4) == 0 &&
+        if (lower_agg(in2, *jf, agg, full ? above_conj : conj, probe_tuple, under_packet, true) && memcmp(&jf->ap.n_keyw, &out.ap.n_keyw, sizeof(int32_t) * 4) == 0 &&
             jf->ap.n_lanes == out.ap.n_lanes) {
             bool ok = true;
             for (auto& c : jf->cols) {
@@ -1539,6 +1566,7 @@ bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
             }
             if (ok) out.jfast = jf; else out.jfast_of_main.clear();
         }
+        if (full && !out.jfast) return in.fail(BKGPU_EUNSUPPORTED, "the aggregate over the FULL join's row could not be lowered: %s", in2.err.c_str());
     }
     return true;
 }
@@ -1674,11 +1702,12 @@ bool lower_star_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
 // pass the conditions are produced on the device batch by batch (pairs + one gather per column) and handed to a sink fragment
 // (Compiled::post, kind PK_FILTER without a predicate, or PK_SORT) whose "scan tuple" is the joined row: every slot of both tuples.
 // INNER: child filters, the residual conditions and a filter above the join are one predicate.  LEFT / RIGHT: the outer (build) side is
-// preserved, unmatched rows come out NULL-extended; filtered children or a filter above are refused (as in lower_join_agg).
+// preserved, unmatched rows come out NULL-extended; filtered children or a filter above are refused (as in lower_join_agg).  FULL: both sides
+// are preserved; a filter above the join is the sink's predicate, so it also judges the NULL-extended rows.
 bool lower_join_rows(Infer& in, Compiled& out, const HNode& join, const HNode* above, const HNode* sort, const HNode* limit_node) {
     int jt = join.join_type;
-    if (jt != BK_INNER_JOIN && jt != BK_LEFT_JOIN && jt != BK_RIGHT_JOIN)
-        return in.fail(BKGPU_EUNSUPPORTED, "a join of type %d that returns rows is outside the GPU path (INNER / LEFT / RIGHT are lowered)", jt);
+    if (jt != BK_INNER_JOIN && jt != BK_LEFT_JOIN && jt != BK_RIGHT_JOIN && jt != BK_FULL_JOIN)
+        return in.fail(BKGPU_EUNSUPPORTED, "a join of type %d that returns rows is outside the GPU path (INNER / LEFT / RIGHT / FULL are lowered)", jt);
     if (join.ch.size() != 2) return in.fail(BKGPU_EINVAL, "JOIN node needs two children");
     if (above && above->limit != -1) return in.fail(BKGPU_EUNSUPPORTED, "LIMIT on a filter above a join: use a LIMIT node");
     const HNode* side[2]; const HNode* filt[2] = {nullptr, nullptr};
@@ -1690,7 +1719,9 @@ bool lower_join_rows(Infer& in, Compiled& out, const HNode& join, const HNode* a
         side[i] = c;
     }
     if (jt == BK_RIGHT_JOIN) jt = BK_LEFT_JOIN;
-    if (jt != BK_INNER_JOIN && (filt[0] || filt[1] || above)) return in.fail(BKGPU_EUNSUPPORTED, "LEFT join with filtered children or a filter above it is outside the GPU path");
+    const bool full = jt == BK_FULL_JOIN;
+    if (full && (filt[0] || filt[1])) return in.fail(BKGPU_EUNSUPPORTED, "FULL join over filtered children is outside the GPU path");
+    if (jt != BK_INNER_JOIN && !full && (filt[0] || filt[1] || above)) return in.fail(BKGPU_EUNSUPPORTED, "LEFT join with filtered children or a filter above it is outside the GPU path");
     const int build_tuple = side[0]->tuple_id, probe_tuple = side[1]->tuple_id;
     out.kind = PK_JOIN; out.build_tuple = build_tuple; out.scan_tuple = probe_tuple; out.join_type = jt;
     std::vector<const HExpr*> conj;
@@ -1706,7 +1737,7 @@ bool lower_join_rows(Infer& in, Compiled& out, const HNode& join, const HNode* a
     }
     if (!bk) return in.fail(BKGPU_EUNSUPPORTED, "join without an equality between the two tables (nested loop) is outside the GPU path");
     for (int i = 0; i < 2; i++) if (filt[i]) for (auto& e : filt[i]->conjuncts) conj.push_back(&e);
-    if (above) for (auto& e : above->conjuncts) conj.push_back(&e);
+    if (above && !full) for (auto& e : above->conjuncts) conj.push_back(&e);   // (FULL: the sink's predicate, below)
     int ot = bk->col_type, it = pk->col_type, cast;
     auto is_signed_t = [](int t) { return t >= BK_INT8 && t <= BK_INT64; };
     if (ot == it) cast = ot;
@@ -1756,6 +1787,8 @@ bool lower_join_rows(Infer& in, Compiled& out, const HNode& join, const HNode* a
     Lower lw2{&pc, &in2, &pp, {}};
     for (const OutCol& oc : out.out_cols) { lw2.intern_col(oc.tuple_id, oc.slot_id, oc.prim); pc.out_cols.push_back(oc); }
     int preg = 0;
+    // FULL: the filter above the join judges every joined row, the NULL-extended ones included, after the match decision
+    if (full && !lower_predicate(in2, lw2, above, pc.ap, preg)) { in.code = in2.code; in.err = in2.err; return false; }
     if (sort) {
         pc.limit = sort->limit;
         if (sort->order_exprs.empty()) return in.fail(BKGPU_EINVAL, "SORT node without order expressions");
