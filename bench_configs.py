@@ -3,7 +3,7 @@
 device-resident synthetic columns (SURVEY.md §8d), CUDA events around reset+push+finish+get_next, one JSON line per
 config with rows/s and achieved GB/s on the config's algorithmic bytes.  The headline line is bench.py's;
 this script measures the side configs on their own (C6, the star join, also its kernels, a parity flag and the Acero time).
-usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [c9] [c10] [--scale 0.1] [--steps 10]"""
+usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [c9] [c10] [c11] [--scale 0.1] [--steps 10]"""
 import argparse
 import ctypes
 import json
@@ -449,6 +449,92 @@ def c10(a):
     print(json.dumps(line), flush=True)
 
 
+def c11(a):
+    """C11, SEMI / ANTI / LEFT joins over a filtered inner side (`… WHERE k IN (SELECT k FROM t WHERE a < b + 12)`, NOT EXISTS, and a LEFT join
+    whose ON condition reads the inner table alone): 10M device-resident outer (build) rows, one key in 32768 NULL, and 100M inner (probe)
+    rows whose filter, a column-vs-column compare, passes about 61 %.  GROUP BY an outer INT32 attribute, COUNT(*) (SEMI, ANTI) or
+    COUNT(inner col) (LEFT).  Per join type: the step, the kernel times of one profiled run (the probe child's filter, the multimap build,
+    the probe, the tail), parity of every group against torch on the same tensors, and Acero's filter -> hashjoin -> aggregate on the host CPUs."""
+    import time
+    from baikaldb_b200 import plan as P
+    from torch.profiler import ProfilerActivity, profile
+    nf, nd = int(100_000_000 * a.scale), int(10_000_000 * a.scale)
+    gen_ = torch.Generator(device="cuda").manual_seed(11)
+    key = torch.randperm(nd, device="cuda", generator=gen_).to(torch.int32)
+    attr = (key % 1000 + 1).to(torch.int32)
+    fk = torch.randint(0, nd + nd // 10, (nf,), device="cuda", generator=gen_, dtype=torch.int32)   # ~9 % of the inner keys have no partner
+    fa = torch.randint(0, 100, (nf,), device="cuda", generator=gen_, dtype=torch.int32)
+    fb = torch.randint(0, 100, (nf,), device="cuda", generator=gen_, dtype=torch.int32)
+    dbits = torch.full(((nd + 7) // 8 + 64,), 0xFF, dtype=torch.uint8, device="cuda")
+    dbits[::4096] = 0xFE                                         # one NULL key in 32768 rows
+    idx = torch.arange(nd, device="cuda")
+    dvalid = ((dbits[idx >> 3] >> (idx & 7)) & 1).bool()
+    tup = {0: [(1, T.INT32), (2, T.INT32), (3, T.INT32)], 1: [(1, T.INT32), (2, T.INT32)]}
+    darr, farr = cols_array([(1, 1, T.INT32), (1, 2, T.INT32)], [key, attr]), cols_array([(0, 1, T.INT32), (0, 2, T.INT32), (0, 3, T.INT32)], [fk, fa, fb])
+    darr[0].validity = dbits.data_ptr()
+    pushes = [(darr, 2, nd), (farr, 3, nf)]
+    # torch: the partner of every inner row that passes its filter, through the outer table's key -> row map
+    live = (fa < fb + 12) & (fk < nd)
+    row_of = torch.full((nd,), -1, dtype=torch.int64, device="cuda")
+    row_of[key[dvalid].long()] = idx[dvalid]
+    partner = row_of[fk[live].long()]
+    partner = partner[partner >= 0]
+    matched = torch.zeros(nd, dtype=torch.bool, device="cuda"); matched[partner] = True
+    want = {"SEMI_JOIN": torch.bincount(attr[matched].long(), minlength=1001), "ANTI_SEMI_JOIN": torch.bincount(attr[~matched].long(), minlength=1001),
+            "LEFT_JOIN": torch.bincount(attr[partner].long(), minlength=1001)}   # LEFT: COUNT(inner col) counts the joined rows alone
+    import pyarrow as pa, pyarrow.acero as ac, pyarrow.compute as pc
+    ft = pa.table({"0_1": pa.array(fk.cpu().numpy()), "0_2": pa.array(fa.cpu().numpy()), "0_3": pa.array(fb.cpu().numpy())})
+    dt = pa.table({"1_1": pa.array(key.cpu().numpy(), mask=~dvalid.cpu().numpy()), "1_2": pa.array(attr.cpu().numpy())})
+    steps = max(1, a.steps // 3)
+    gpu_name = torch.cuda.get_device_name(0)
+    try:
+        import subprocess
+        power = subprocess.check_output(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"], text=True).split("\n")[0].strip()
+    except Exception:
+        power = None
+    for jt, acero_jt in (("SEMI_JOIN", "right semi"), ("ANTI_SEMI_JOIN", "right anti"), ("LEFT_JOIN", "right outer")):
+        aggs = [P.agg_expr("count_star", 2, 1)] if jt != "LEFT_JOIN" else [P.agg_expr("count", 2, 1, None, P.slot_ref(0, 2, T.INT32))]
+        inner = P.where(P.scan(0), P.lt(P.slot_ref(0, 2, T.INT32), P.add(P.slot_ref(0, 3, T.INT32), P.int_lit(12))))
+        j = P.join(P.scan(1), inner, [P.eq(P.slot_ref(1, 1, T.INT32), P.slot_ref(0, 1, T.INT32))], join_type=getattr(P.JoinType, jt))
+        plan = P.Plan(P.agg(j, 2, [P.slot_ref(1, 2, T.INT32)], aggs), {**tup, 2: P.agg_tuple_slots(aggs, [T.INT64])})
+        opts = [(b"group_capacity_log2", 14)]
+        line, got = run(f"C11 outer {jt.replace('_JOIN', '')} JOIN filtered inner ON int32 key, GROUP BY outer attr, {'COUNT(inner col)' if jt == 'LEFT_JOIN' else 'COUNT(*)'} "
+                        "(10M outer x 100M inner)", plan, pushes, nf, 12 * nf + 8 * nd, steps, 1, options=opts, collect=True, emit=False)
+        r = line["result_rows"]
+        kk, gc = np.array(got["1_2"][:r]), np.array(got["2_1"][:r])
+        w = want[jt].cpu().numpy()
+        want_groups = set(np.nonzero(w)[0].tolist()) if jt != "LEFT_JOIN" else set(torch.unique(attr).cpu().numpy().tolist())
+        line["parity_vs_torch_all_groups"] = bool(set(kk.tolist()) == want_groups and len(kk) == len(want_groups) and np.array_equal(gc, w[kk]))
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            run("profile", plan, pushes, nf, 0, steps, 1, options=opts, emit=False)
+            torch.cuda.synchronize()
+        per = lambda us: us / 1e3 / (steps + 1)   # (the profiled run: 1 warm-up + steps)
+        ka = prof.key_averages()
+        dev = lambda e: getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0))
+        line["filter_ms_per_step (k_star_dim_filter over the inner rows)"] = per(sum(dev(e) for e in ka if "k_star_dim_filter" in e.key))
+        line["multimap_build_ms_per_step (k_join_build)"] = per(sum(dev(e) for e in ka if "k_join_build(" in e.key))
+        # the probe and the tail are both k_agg_interp launches: the tail is the last of each step's
+        interp = sorted((e for e in prof.events() if "k_agg_interp" in e.name and dev(e) > 0), key=lambda e: e.time_range.start)
+        k = len(interp) // (steps + 1)
+        tail = [e for i, e in enumerate(interp) if k and i % k == k - 1]
+        line["probe_ms_per_step (k_agg_interp over the inner rows)"] = per(sum(dev(e) for e in interp) - sum(dev(e) for e in tail))
+        line["tail_ms_per_step (k_agg_interp over the outer rows)"] = per(sum(dev(e) for e in tail))
+        line["inner_rows_passing_filter"] = int((fa < fb + 12).sum())
+        # Acero on the host CPUs: the inner table's filter, then the hashjoin (hash table on the outer table), then the aggregate
+        src = lambda t: ac.Declaration("table_source", ac.TableSourceNodeOptions(t))
+        filt = ac.Declaration("filter", ac.FilterNodeOptions(pc.field("0_2") < pc.field("0_3") + 12), inputs=[src(ft)])
+        hj = ac.Declaration("hashjoin", ac.HashJoinNodeOptions(acero_jt, ["0_1"], ["1_1"]), inputs=[filt, src(dt)])
+        spec = ([], "hash_count_all", None, "2_1") if jt != "LEFT_JOIN" else ("0_2", "hash_count", None, "2_1")
+        agg = ac.Declaration("aggregate", ac.AggregateNodeOptions([spec], keys=["1_2"]), inputs=[hj])
+        t0 = time.perf_counter(); at = agg.to_table(use_threads=True); line["acero_filter_hashjoin_aggregate_host_s"] = time.perf_counter() - t0
+        ad = at.to_pydict()
+        line["acero_matches_torch"] = bool(len(ad["1_2"]) == len(want_groups) and all(int(w[g]) == c for g, c in zip(ad["1_2"], ad["2_1"])))
+        line["acero_host_cpus"] = os.cpu_count()
+        line["gpu"] = gpu_name
+        line["power_limit"] = power
+        print(json.dumps(line), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("configs", nargs="*", default=["c1", "c3", "c5"])
@@ -510,6 +596,8 @@ def main():
         c9(a)
     if "c10" in a.configs:
         c10(a)
+    if "c11" in a.configs:
+        c11(a)
     if "c3" in a.configs:
         nf, nd = int(100_000_000 * a.scale), int(10_000_000 * a.scale)
         fs = [(0, 1, T.INT32, 0, 1, 0, nd, 1.0), (0, 2, T.DOUBLE, 1, 2, 0, 0, 1.0)]

@@ -78,8 +78,8 @@ __global__ void __launch_bounds__(256) k_agg_interp(const __grid_constant__ AggA
     if (a.join.enabled && a.join.tail) {   // after the last probe batch: the preserved (build) side's rows the join type asks for
         const int jt = a.join.join_type;
         for (int64_t br = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; br < a.join.n_build; br += (int64_t)gridDim.x * blockDim.x) {
-            const bool m = a.join.matched[br] != 0;
-            if (jt == 4 /*SEMI*/ ? m : !m) passed += interp_row(a, cx, -1, br, 2);
+            const uint8_t m = a.join.matched[br];   // (2: removed by the build side's own filter, never emitted)
+            if (jt == 4 /*SEMI*/ ? m == 1 : m == 0) passed += interp_row(a, cx, -1, br, 2);
         }
     } else
     for (int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; row < a.nrows; row += (int64_t)gridDim.x * blockDim.x) {
@@ -118,7 +118,7 @@ __global__ void __launch_bounds__(256) k_join_pairs(const __grid_constant__ AggA
     };
     if (a.join.tail) {
         for (int64_t br = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; br < a.join.n_build; br += (int64_t)gridDim.x * blockDim.x)
-            if (!a.join.matched[br]) emit(JOIN_NO_ROW, (uint32_t)br);
+            if (a.join.matched[br] == 0) emit(JOIN_NO_ROW, (uint32_t)br);
         return;
     }
     for (int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; row < a.nrows; row += (int64_t)gridDim.x * blockDim.x) {
@@ -567,16 +567,20 @@ __global__ void k_join_compose(JoinFast jf, const uint32_t* attr_by_row, uint32_
 // ---- K4 star join (PK_STAR_AGG): one fact table INNER-joined to up to four dimensions ----
 // Build time: the conjuncts over one dimension alone, once per dimension row.  A row's build key is valid when the key is not NULL and the
 // conjunction is TRUE: this bitmap (beside the column's own) is the key's validity for k_join_build_fast / k_join_build, which skip NULL keys.
-__global__ void __launch_bounds__(256) k_star_dim_filter(const __grid_constant__ StarFilter a, uint32_t* keybits) {
+// The two-table join runs it over a child's own filter: the build side's (with `dropped`: a row whose conjunction is not TRUE, whatever its
+// key, is marked 2 in matched[]) and each probe batch's.  The program reads the row both as the probe row and as the build row.
+__global__ void __launch_bounds__(256) k_star_dim_filter(const __grid_constant__ StarFilter a, uint32_t* keybits, uint8_t* dropped) {
     const int lane = threadIdx.x & 31;
     const int64_t T = (int64_t)gridDim.x * blockDim.x;
     for (int64_t w0 = (int64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31); w0 < a.nrows; w0 += T) {   // (warp-uniform: one bitmap word per warp and pass)
         const int64_t r = w0 + lane;
         bool ok = r < a.nrows && !elem_is_null(a.cols[a.key_col], r);
-        if (ok && a.prog.n_instr > 0) {
+        if ((ok || (dropped && r < a.nrows)) && a.prog.n_instr > 0) {
             uint64_t out[1]; uint32_t out_null;
-            run_program(a.prog, a.cols, r, out, out_null);
-            ok = !(out_null & 1u) && out[0] != 0;
+            run_program(a.prog, a.cols, r, out, out_null, r);
+            const bool pass = !(out_null & 1u) && out[0] != 0;
+            ok = ok && pass;
+            if (dropped && !pass) dropped[r] = 2;
         }
         const uint32_t m = __ballot_sync(0xFFFFFFFFu, ok);
         if (lane == 0) keybits[w0 >> 5] = m;
@@ -671,10 +675,10 @@ __global__ void __launch_bounds__(256) k_star_expand(DevCol fk, int from_prim, i
         }
     }
 }
-cudaError_t launch_star_dim_filter(const StarFilter& f, uint32_t* keybits, cudaStream_t s) {
+cudaError_t launch_star_dim_filter(const StarFilter& f, uint32_t* keybits, uint8_t* dropped, cudaStream_t s) {
     if (f.nrows == 0) return cudaSuccess;
     int grid = (int)((f.nrows + 255) / 256); if (grid > 132 * 16) grid = 132 * 16;
-    k_star_dim_filter<<<grid, 256, 0, s>>>(f, keybits);
+    k_star_dim_filter<<<grid, 256, 0, s>>>(f, keybits, dropped);
     return cudaGetLastError();
 }
 cudaError_t launch_star_probe(const StarProbe& sp, uint32_t* out, uint32_t* cursor, int sm_count, cudaStream_t s) {

@@ -14,8 +14,9 @@ struct JoinArgs {
     int32_t probe_col;       // index into cols of the probe key
     int32_t probe_prim, cast_prim;
     // LEFT / SEMI / ANTI_SEMI (the build side = the reference's outer / driver table is the preserved side, join_node.cpp:1200-1276,
-    // joiner.cpp:633-685): `matched[build row]` is set by the probe; the TAIL launch (tail = 1) walks the n_build build rows and emits the
-    // unmatched ones NULL-extended (LEFT), the matched ones (SEMI) or the unmatched ones (ANTI_SEMI)
+    // joiner.cpp:633-685): `matched[build row]` is set to 1 by the probe; the TAIL launch (tail = 1) walks the n_build build rows and emits the
+    // unmatched ones (0) NULL-extended (LEFT), the matched ones (1) (SEMI) or the unmatched ones (0) (ANTI_SEMI).  2 = removed by the build
+    // side's own filter: never in the multimap, never emitted
     int32_t join_type;       // pb::JoinType: 1 LEFT, 3 INNER, 4 SEMI, 5 ANTI_SEMI, 6 FULL (RIGHT arrives as LEFT with the children swapped)
     int32_t tail;
     uint8_t* matched;
@@ -115,9 +116,11 @@ cudaError_t launch_join_rows_gather(const DevCol& src, const uint32_t* tuples, i
 // star join (PK_STAR_AGG): per dimension with unique keys, the fact foreign key, its slot in the row-id tuple and the dimension's key index
 struct StarLookup { DevCol fk; int32_t from_prim, cast_prim, slot; JoinFast jf; };
 struct StarProbe { StarLookup d[4]; int32_t n; int32_t width; int64_t nrows; int32_t vec; };
-// the build-time filter of one dimension: program over the plan's columns (this dimension's retained rows), validity of its join key
+// the build-time filter of one dimension: program over the plan's columns (this dimension's retained rows), validity of its join key.
+// Also a two-table join child's own filter (its retained build rows, or one probe batch).
 struct StarFilter { DevCol cols[MAX_COLS]; Program prog; int32_t key_col; int64_t nrows; };
-cudaError_t launch_star_dim_filter(const StarFilter& f, uint32_t* keybits, cudaStream_t s);
+// `dropped` (optional): dropped[row] = 2 where the conjunction is not TRUE (the join's matched[] of a filtered build side)
+cudaError_t launch_star_dim_filter(const StarFilter& f, uint32_t* keybits, uint8_t* dropped, cudaStream_t s);
 cudaError_t launch_star_probe(const StarProbe& sp, uint32_t* out, uint32_t* cursor, int sm_count, cudaStream_t s);
 cudaError_t launch_star_expand(const DevCol& fk, int from_prim, int cast_prim, const uint64_t* keys, const uint32_t* rows, uint32_t cap_mask, const uint32_t* in, uint32_t n_in,
                                int width, int slot, uint32_t* out, uint32_t cap, uint32_t* cursor, cudaStream_t s);

@@ -35,7 +35,7 @@ struct JoinSide {
     std::vector<uint8_t*> vals, nullbytes, bitmap;   // per plan column (this side's columns only)
     std::vector<bool> has_null;
     int64_t rows = 0, cap = 0;
-    uint8_t* keybits = nullptr; size_t keybits_cap = 0;   // star join: validity of the build key AND the dimension's build-time filter
+    uint8_t* keybits = nullptr; size_t keybits_cap = 0;   // validity of the build key AND the dimension's (star) / build child's (two-table) own filter
     uint64_t* jt_keys = nullptr; uint32_t* jt_rows = nullptr; uint32_t jt_mask = 0; bool jt_generic = false;   // multimap (duplicate keys)
     JoinFast jf{}; uint32_t* jf_dense = nullptr; uint64_t* jf_packed = nullptr; size_t jf_dense_cap = 0, jf_packed_cap = 0;   // unique-key index
     bool learned = false; uint64_t learn_min = 0, learn_max = 0;   // key range of the side's previous build (skips the min/max pass + round trip)
@@ -57,7 +57,8 @@ struct JoinState {
     uint64_t* scratch = nullptr; size_t scratch_cap = 0;   // [0..1] key min / max, then u32 flags: [4] duplicate build key, [5] fused probe unusable, [6] key outside the learned range
     JoinProbe jp{}; int jp_key_pos = 0;   // the FK -> PK probe fused into the lean aggregate
     uint32_t* jp_attr = nullptr; uint64_t* jp_packed = nullptr; size_t jp_attr_cap = 0, jp_packed_cap = 0;
-    uint8_t* matched = nullptr; size_t matched_cap = 0;   // LEFT / SEMI / ANTI: build rows that found a partner
+    uint8_t* matched = nullptr; size_t matched_cap = 0;   // LEFT / SEMI / ANTI: build rows that found a partner (1), or that the build child's filter removed (2)
+    uint8_t* probe_bits = nullptr; size_t probe_bits_cap = 0;   // the probe key's validity AND the probe child's own filter, for one probe batch
     uint32_t* pairs = nullptr; size_t pairs_cap = 0; uint32_t* cursor = nullptr; size_t cursor_cap = 0;   // PK_JOIN: (probe row, build row) pairs of one batch
     uint32_t* tuples[2] = {nullptr, nullptr}; size_t tuples_cap[2] = {0, 0};   // star join: row-id tuples of one chunk (probe / expansion ping-pong)
     std::vector<ChunkCol> chunk;   // the gathered chunk (two-table gather path, star join), per plan column

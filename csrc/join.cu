@@ -265,6 +265,20 @@ static int join_build_multimap(bkgpu_plan* p, JoinSide& s, const DevCol& key, in
     return BKGPU_OK;
 }
 
+// a two-table join child's own filter (Compiled::build_filter / probe_filter) over `nrows` rows of `cols` (every plan column, this child's at
+// the rows' start) into *bits: "key not NULL and the conjunction TRUE".  `dropped`: matched[] of the build side, 2 where the conjunction is not TRUE
+static int join_child_filter(bkgpu_plan* p, const Program& prog, int key_col, const DevCol* cols, int64_t nrows, uint8_t** bits, size_t* bits_cap, uint8_t* dropped) {
+    const Compiled& c = p->c;
+    int rc;
+    if ((rc = ensure_buf(p, (void**)bits, bits_cap, ((size_t)nrows + 31) / 32 * 4 + 4))) return rc;
+    StarFilter f; memset(&f, 0, sizeof f);
+    for (size_t i = 0; i < c.cols.size(); i++) f.cols[i] = cols[i];
+    f.prog = prog; f.key_col = key_col; f.nrows = nrows;
+    CK(p, launch_star_dim_filter(f, (uint32_t*)*bits, dropped, p->stream));
+    p->stats.kernel_launches++;
+    return BKGPU_OK;
+}
+
 // the general probe's multimap (duplicate build keys, unmatched probe rows): built only when a batch needs it
 static int join_generic_table(bkgpu_plan* p) {
     const Compiled& c = p->c;
@@ -272,19 +286,36 @@ static int join_generic_table(bkgpu_plan* p) {
     JoinSide& s = j.side[0];
     if (s.jt_generic) return BKGPU_OK;
     int rc;
-    if ((rc = join_build_multimap(p, s, side_col(c, s, (size_t)c.build_key_col), c.join_key_prim))) return rc;
+    DevCol key = side_col(c, s, (size_t)c.build_key_col);
     if (c.join_type != BK_INNER_JOIN) {   // one "found a partner" byte per build row
         if ((rc = ensure_buf(p, (void**)&j.matched, &j.matched_cap, (size_t)std::max<int64_t>(s.rows, 1)))) return rc;
         CK(p, cudaMemsetAsync(j.matched, 0, (size_t)std::max<int64_t>(s.rows, 1), p->stream));
+        if (c.n_build_filter > 0) {   // (SEMI / ANTI) a row that fails its own filter is neither in the multimap nor in the tail
+            const std::vector<DevCol> all = join_cols(p, nullptr);
+            if ((rc = join_child_filter(p, c.build_filter, c.build_key_col, all.data(), s.rows, &s.keybits, &s.keybits_cap, j.matched))) return rc;
+            key.validity = s.keybits;
+        }
     }
-    return BKGPU_OK;
+    return join_build_multimap(p, s, key, c.join_key_prim);
+}
+
+// the probe child's own filter over one batch (`all`: every plan column): its bitmap becomes the probe key's validity for the batch, so a row that
+// fails it finds no partner, as a row with a NULL key.  Never for FULL, where such a row would still come out NULL-extended.  A row that passes
+// has a valid key: every row the aggregate or the sink sees reads the key column as before.
+static int join_probe_filter(bkgpu_plan* p, std::vector<DevCol>& all, int64_t nrows) {
+    const Compiled& c = p->c;
+    JoinState& j = p->join;
+    if (c.n_probe_filter == 0) return BKGPU_OK;
+    const int rc = join_child_filter(p, c.probe_filter, c.probe_key_col, all.data(), nrows, &j.probe_bits, &j.probe_bits_cap, nullptr);
+    all[(size_t)c.probe_key_col].validity = j.probe_bits;
+    return rc;
 }
 
 static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nrows, int64_t, bool) {
     const Compiled& c = p->c;
     JoinState& j = p->join;
     const JoinSide& s = j.side[0];
-    const std::vector<DevCol> all = join_cols(p, probe_cols);
+    std::vector<DevCol> all = join_cols(p, probe_cols);
     // ---- FK -> PK fast path: gather the build columns next to the probe rows, then the ordinary (lean) aggregate ----
     if (s.jf.mode != 0 && j.jp.mode != 0 && c.jfast && !p->force_generic && !j.no_fused_probe) {
         // ---- fused probe: the lean aggregate reads the foreign key and looks the group key up itself ----
@@ -332,7 +363,7 @@ static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nro
         }
         return BKGPU_OK;
     }
-    { int rc = join_generic_table(p); if (rc) return rc; }
+    { int rc; if ((rc = join_generic_table(p)) || (rc = join_probe_filter(p, all, nrows))) return rc; }
     return launch_agg_batch(p, c, all.data(), nrows, false);
 }
 
@@ -355,7 +386,7 @@ static int join_pairs(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t n_p
         int r;
         if ((r = ensure_buf(p, (void**)&j.pairs, &j.pairs_cap, (size_t)want * 8))) return r;
         CK(p, cudaMemsetAsync(j.cursor, 0, 4, p->stream));
-        // (a rerun of a LEFT / FULL batch sets the same matched[] flags again: they only ever go from 0 to 1)
+        // (a rerun of a LEFT / FULL batch sets the same matched[] flags again: they only ever go from 0 to 1; a 2 is never in the multimap)
         CK(p, launch_join_pairs(a, j.pairs, (uint32_t)want, j.cursor, p->sm_count, p->stream));
         p->stats.kernel_launches++;
         return BKGPU_OK;
@@ -388,8 +419,9 @@ static int join_rows_emit(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t
 }
 static int join_rows_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nrows, int64_t, bool) {
     int rc;
-    if ((rc = join_generic_table(p))) return rc;
-    return join_rows_emit(p, join_cols(p, probe_cols), nrows, false);
+    std::vector<DevCol> all = join_cols(p, probe_cols);
+    if ((rc = join_generic_table(p)) || (rc = join_probe_filter(p, all, nrows))) return rc;
+    return join_rows_emit(p, all, nrows, false);
 }
 
 // ---- FULL join under an aggregate (PK_JOIN_AGG): pairs -> gather -> the aggregate over the joined row (Compiled::jfast, whose predicate is
@@ -464,7 +496,7 @@ static int star_build(bkgpu_plan* p) {
             StarFilter f; memset(&f, 0, sizeof f);
             for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] == 1 + (int)d) f.cols[i] = side_col(c, s, i);
             f.prog = sd.filter; f.key_col = sd.key_col; f.nrows = s.rows;
-            CK(p, launch_star_dim_filter(f, (uint32_t*)s.keybits, p->stream));
+            CK(p, launch_star_dim_filter(f, (uint32_t*)s.keybits, nullptr, p->stream));
             p->stats.kernel_launches++;
             key.validity = s.keybits;
         }

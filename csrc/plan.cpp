@@ -1187,6 +1187,10 @@ static void explain(Compiled& c) {
         snprintf(buf, sizeof buf, "full join: k_join_pairs_full (the program below: the join conditions) -> gather -> %s; the filter above the join is the %s predicate (pred_out=%d)\n",
                  agg ? "aggregate over the joined row" : "sink", agg ? "aggregate's" : "sink's", agg ? c.jfast->ap.pred_out : c.post->ap.pred_out); s += buf;
     }
+    if (c.n_build_filter || c.n_probe_filter) {
+        snprintf(buf, sizeof buf, "child filters: build tuple=%d conjuncts=%d (once over the retained rows: multimap key validity, failing rows never in the tail); "
+                 "probe tuple=%d conjuncts=%d (per probe batch: probe key validity)\n", c.build_tuple, c.n_build_filter, c.scan_tuple, c.n_probe_filter); s += buf;
+    }
     snprintf(buf, sizeof buf, "program: %d instr, %d outputs\n", c.prog.n_instr, c.prog.n_out); s += buf;
     for (int i = 0; i < c.prog.n_instr; i++) {
         const Instr& in = c.prog.code[i];
@@ -1208,6 +1212,7 @@ void patch_in_sets(Compiled& c, const std::vector<uint64_t>& addr) {
         for (int i = 0; i < q.n_instr; i++) if (q.code[i].op == OP_IN_SET) q.cbits[q.code[i].a] = addr[q.code[i].b];
     };
     fix(c.prog);
+    fix(c.build_filter); fix(c.probe_filter);
     for (StarDim& d : c.dims) fix(d.filter);
     for (WinStage& w : c.win) for (Program& q : w.exprs) fix(q);
     if (c.post) patch_in_sets(*c.post, addr);
@@ -1476,7 +1481,9 @@ bool lower_post(Infer& in, Compiled& out, const HNode* sort, const HNode* having
 // with the inner child's rows (JoinNode::hash_join, src/exec/join_node.cpp:920-1022; Joiner::construct_hash_map,
 // src/exec/joiner.cpp:624-631); the key is the cast equal-slot value (strip_out_equal_slots, joiner.cpp:166-217).
 // Filters of both children and the residual join conditions become one predicate over the joined row — for an
-// INNER join that is the same set of rows.
+// INNER join that is the same set of rows.  LEFT / SEMI / ANTI: a child's filter must remove the child's rows before the join (a build row
+// that fails it would still come out of the ANTI tail, or NULL-extended), so each child's filter is a program of its own
+// (Compiled::build_filter / probe_filter) and the main program keeps the residual conditions alone.
 // FULL: the residual conditions decide the pairs (k_join_pairs_full); the filter above the join — the planner keeps a join FULL only under a
 // NULL-tolerant one (join_node.cpp:171-203) — judges every emitted row, NULL-extended ones included, as the predicate of `jfast`, the
 // aggregate over the pairs' gathered columns.
@@ -1486,6 +1493,27 @@ static void intern_slots(Lower& lw, Infer& in, const HExpr& e) {   // every colu
         lw.intern_col(e.tuple_id, e.slot_id, st == BK_INVALID_TYPE ? e.col_type : st);
     }
     for (auto& c : e.ch) intern_slots(lw, in, c);
+}
+static void expr_tuples(const HExpr& e, std::vector<int>& t);
+// LEFT / SEMI / ANTI_SEMI: the filter of the child scanning `tuple_id` (FilterNode under JoinNode) stays that child's: a program of its own
+// whose output 0 is the conjunction, constants numbered per program (as a star dimension's filter).  Its columns become plan columns.
+static bool lower_child_filter(Infer& in, Compiled& out, const HNode* filt, int tuple_id, Program& prog, int& n) {
+    memset(&prog, 0, sizeof prog); n = 0;
+    if (!filt || filt->conjuncts.empty()) return true;
+    if (filt->conjuncts.size() > 8) return in.fail(BKGPU_EUNSUPPORTED, "more than 8 conjuncts in the filter of join child %d", tuple_id);
+    for (auto& e : filt->conjuncts) {
+        std::vector<int> ts; expr_tuples(e, ts);
+        for (int t : ts) if (t != tuple_id) return in.fail(BKGPU_EINVAL, "the filter of join child %d reads tuple %d", tuple_id, t);
+    }
+    const int n_const = out.n_const;
+    out.n_const = 0;
+    Lower fl{&out, &in, &prog, {}};
+    for (auto& e : filt->conjuncts) { int depth = 0; if (!fl.expr(e, depth) || !fl.to_bool(e)) return false; }
+    if (filt->conjuncts.size() > 1 && !fl.emit(OP_AND, (uint8_t)filt->conjuncts.size())) return false;
+    if (!fl.out_reg(0)) return false;
+    prog.n_out = 1; n = (int)filt->conjuncts.size();
+    out.n_const = n_const;
+    return true;
 }
 bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& join, bool under_packet, const HNode* above) {
     int jt = join.join_type;
@@ -1508,7 +1536,8 @@ bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
     const bool full = jt == BK_FULL_JOIN;
     if (full && (filt[0] || filt[1])) return in.fail(BKGPU_EUNSUPPORTED, "FULL join over filtered children is outside the GPU path");
     if (jt != BK_INNER_JOIN && !full && above) return in.fail(BKGPU_EUNSUPPORTED, "a filter between the aggregate and a LEFT / SEMI / ANTI join is outside the GPU path");
-    if (jt != BK_INNER_JOIN && (filt[0] || filt[1])) return in.fail(BKGPU_EUNSUPPORTED, "LEFT / SEMI / ANTI join over filtered children is outside the GPU path");
+    // LEFT / SEMI / ANTI: a child's filter removes that child's rows before the join (lower_child_filter), except on the preserved side of LEFT
+    if (jt == BK_LEFT_JOIN && filt[0]) return in.fail(BKGPU_EUNSUPPORTED, "a filter on the preserved side of a LEFT / RIGHT join is outside the GPU path");
     const int build_tuple = side[0]->tuple_id, probe_tuple = side[1]->tuple_id;
     out.build_tuple = build_tuple;
     std::vector<const HExpr*> conj;
@@ -1523,7 +1552,7 @@ bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
         if (!taken) conj.push_back(&e);
     }
     if (!bk) return in.fail(BKGPU_EUNSUPPORTED, "join without an equality between the two tables (nested loop) is outside the GPU path");
-    for (int i = 0; i < 2; i++) if (filt[i]) for (auto& e : filt[i]->conjuncts) conj.push_back(&e);
+    if (jt == BK_INNER_JOIN) for (int i = 0; i < 2; i++) if (filt[i]) for (auto& e : filt[i]->conjuncts) conj.push_back(&e);
     std::vector<const HExpr*> above_conj;
     if (above) for (auto& e : above->conjuncts) (full ? above_conj : conj).push_back(&e);
     int ot = bk->col_type, it = pk->col_type, cast;
@@ -1548,6 +1577,8 @@ bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
     out.build_key_col = lw.intern_col(bk->tuple_id, bk->slot_id, in.slot_type(bk->tuple_id, bk->slot_id));
     out.probe_key_col = lw.intern_col(pk->tuple_id, pk->slot_id, in.slot_type(pk->tuple_id, pk->slot_id));
     for (auto* e : above_conj) intern_slots(lw, in, *e);   // (FULL: read by jfast's predicate alone, gathered like the aggregate's columns)
+    if (jt != BK_INNER_JOIN && (!lower_child_filter(in, out, filt[0], build_tuple, out.build_filter, out.n_build_filter) ||
+                                !lower_child_filter(in, out, filt[1], probe_tuple, out.probe_filter, out.n_probe_filter))) return false;
     if ((int)out.cols.size() > MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d columns referenced", MAX_COLS);
     // fast path: lower the same aggregate again with every column treated as a column of ONE (virtual, joined) tuple.  FULL: the path
     // itself, with the filter above the join as the predicate
@@ -1702,7 +1733,8 @@ bool lower_star_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
 // pass the conditions are produced on the device batch by batch (pairs + one gather per column) and handed to a sink fragment
 // (Compiled::post, kind PK_FILTER without a predicate, or PK_SORT) whose "scan tuple" is the joined row: every slot of both tuples.
 // INNER: child filters, the residual conditions and a filter above the join are one predicate.  LEFT / RIGHT: the outer (build) side is
-// preserved, unmatched rows come out NULL-extended; filtered children or a filter above are refused (as in lower_join_agg).  FULL: both sides
+// preserved, unmatched rows come out NULL-extended; the inner child's filter is its own program (as in lower_join_agg), a filter on the
+// preserved child or above the join is refused.  FULL: both sides
 // are preserved; a filter above the join is the sink's predicate, so it also judges the NULL-extended rows.
 bool lower_join_rows(Infer& in, Compiled& out, const HNode& join, const HNode* above, const HNode* sort, const HNode* limit_node) {
     int jt = join.join_type;
@@ -1721,7 +1753,8 @@ bool lower_join_rows(Infer& in, Compiled& out, const HNode& join, const HNode* a
     if (jt == BK_RIGHT_JOIN) jt = BK_LEFT_JOIN;
     const bool full = jt == BK_FULL_JOIN;
     if (full && (filt[0] || filt[1])) return in.fail(BKGPU_EUNSUPPORTED, "FULL join over filtered children is outside the GPU path");
-    if (jt != BK_INNER_JOIN && !full && (filt[0] || filt[1] || above)) return in.fail(BKGPU_EUNSUPPORTED, "LEFT join with filtered children or a filter above it is outside the GPU path");
+    if (jt == BK_LEFT_JOIN && above) return in.fail(BKGPU_EUNSUPPORTED, "LEFT join with a filter above it is outside the GPU path");
+    if (jt == BK_LEFT_JOIN && filt[0]) return in.fail(BKGPU_EUNSUPPORTED, "a filter on the preserved side of a LEFT / RIGHT join is outside the GPU path");
     const int build_tuple = side[0]->tuple_id, probe_tuple = side[1]->tuple_id;
     out.kind = PK_JOIN; out.build_tuple = build_tuple; out.scan_tuple = probe_tuple; out.join_type = jt;
     std::vector<const HExpr*> conj;
@@ -1736,7 +1769,7 @@ bool lower_join_rows(Infer& in, Compiled& out, const HNode& join, const HNode* a
         if (!taken) conj.push_back(&e);
     }
     if (!bk) return in.fail(BKGPU_EUNSUPPORTED, "join without an equality between the two tables (nested loop) is outside the GPU path");
-    for (int i = 0; i < 2; i++) if (filt[i]) for (auto& e : filt[i]->conjuncts) conj.push_back(&e);
+    if (jt == BK_INNER_JOIN) for (int i = 0; i < 2; i++) if (filt[i]) for (auto& e : filt[i]->conjuncts) conj.push_back(&e);
     if (above && !full) for (auto& e : above->conjuncts) conj.push_back(&e);   // (FULL: the sink's predicate, below)
     int ot = bk->col_type, it = pk->col_type, cast;
     auto is_signed_t = [](int t) { return t >= BK_INT8 && t <= BK_INT64; };
@@ -1774,6 +1807,7 @@ bool lower_join_rows(Infer& in, Compiled& out, const HNode& join, const HNode* a
         if (!lw.out_reg(reg++)) return false;
     }
     p.n_out = reg;
+    if (jt == BK_LEFT_JOIN && !lower_child_filter(in, out, filt[1], probe_tuple, out.probe_filter, out.n_probe_filter)) return false;
     if (out.cols.size() != n_payload) return in.fail(BKGPU_EINVAL, "join conditions reference a slot that is in neither tuple descriptor");
     // the sink over the joined rows
     auto post = std::make_shared<Compiled>();

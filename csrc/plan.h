@@ -144,6 +144,10 @@ struct Compiled {
     int probe_key_col = -1;            // index into cols
     int join_type = 0;
     int join_key_prim = 0;
+    // LEFT / SEMI / ANTI_SEMI over filtered children: each child's own filter, apart from the join conditions (a build row that fails it must
+    // not exist, not even in the tail).  Output 0 = the conjunction of that child's n_*_filter conjuncts (column indices into cols).
+    int n_build_filter = 0, n_probe_filter = 0;
+    Program build_filter{}, probe_filter{};
     // FK -> PK fast path: the same aggregate lowered over the virtual joined tuple (build-side columns are gathered
     // to probe-row alignment first); usable while every probe row has exactly one match
     std::shared_ptr<Compiled> jfast;
@@ -163,7 +167,7 @@ struct Compiled {
 
 // returns 0 or a negative BKGPU_E* code; `err` receives the message
 int compile_plan(const uint8_t* desc, size_t len, Compiled& out, std::string& err);
-// every program of the plan (main, post, jfast, star dimensions' filters, window stages' expressions): OP_IN_SET's constant := addr[set]
+// every program of the plan (main, post, jfast, join children's and star dimensions' filters, window stages' expressions): OP_IN_SET's constant := addr[set]
 void patch_in_sets(Compiled& c, const std::vector<uint64_t>& addr);
 
 // host-side ExprValue::cast_to on canonical images (x86 semantics == the reference's build)
