@@ -27,6 +27,7 @@ constexpr int MAX_IN_SETS = 256;       // IN sets of one plan (OP_IN_SET's b)
 // ---------------------------------------------------------------- type helpers
 static bool is_int_t(int t) { return t >= BK_INT8 && t <= BK_UINT64; }
 static bool is_uint_t(int t) { return t >= BK_UINT8 && t <= BK_UINT64; }
+static bool is_signed_t(int t) { return t >= BK_INT8 && t <= BK_INT64; }
 static bool is_double_t(int t) { return t == BK_FLOAT || t == BK_DOUBLE; }
 static bool is_datetime_family(int t) { return t == BK_DATETIME || t == BK_TIMESTAMP || t == BK_DATE || t == BK_TIME; }
 static bool is_numeric_path_type(int t) { return t == BK_BOOL || is_int_t(t) || is_double_t(t) || is_datetime_family(t); }
@@ -557,11 +558,17 @@ static bool is_filter(const HNode* n) {
     return n && (n->node_type == BK_WHERE_FILTER_NODE || n->node_type == BK_TABLE_FILTER_NODE);
 }
 
+// FilterNode passes a row when every conjunct is non-NULL true (filter_node.cpp:726-734); one OP_AND takes at most 8 of them
+static bool at_most_8_conjuncts(Infer& in, size_t n, const std::string& where) {
+    return n <= 8 || in.fail(BKGPU_EUNSUPPORTED, "more than 8 conjuncts%s", where.c_str());
+}
+
+// lowers expressions into one program; its constants are numbered from 0
 struct Lower {
     Compiled* out;
     Infer* in;
     Program* p;
-    std::map<int, int> build_cols;  // (unused unless joining)
+    int n_const = 0;
     int intern_col(int tuple_id, int slot_id, int prim) {
         auto& cols = out->cols;
         for (size_t i = 0; i < cols.size(); i++) if (cols[i].tuple_id == tuple_id && cols[i].slot_id == slot_id) return (int)i;
@@ -575,8 +582,8 @@ struct Lower {
         return true;
     }
     int add_const(uint64_t bits, bool isnull) {
-        if (out->n_const >= MAX_CONST) { in->fail(BKGPU_EUNSUPPORTED, "too many constants (%d)", MAX_CONST); return -1; }
-        int i = out->n_const++;
+        if (n_const >= MAX_CONST) { in->fail(BKGPU_EUNSUPPORTED, "too many constants (%d)", MAX_CONST); return -1; }
+        int i = n_const++;
         p->cbits[i] = bits;
         if (isnull) p->cnull |= 1ull << i;
         return i;
@@ -641,10 +648,10 @@ struct Lower {
             case BK_IN_PREDICATE: {
                 int map_type = e.arg_types[0];
                 if (!expr(e.ch[0], depth) || !cast(e.ch[0].col_type, map_type)) return false;
-                int first = out->n_const, cnt = 0; bool has_null = false;
+                int first = n_const, cnt = 0; bool has_null = false;
                 for (size_t i = 1; i < e.ch.size(); i++) { if (e.ch[i].lit_null) has_null = true; else cnt++; }
                 const uint8_t flags = (uint8_t)((has_null ? 16 : 0) | host_prim_class(map_type));
-                if (cnt > 255 || out->n_const + cnt > MAX_CONST) {   // a list the constant pool cannot hold is probed as a hashed set
+                if (cnt > 255 || n_const + cnt > MAX_CONST) {   // a list the constant pool cannot hold is probed as a hashed set
                     const int s = in_set(e, map_type, has_null), k = s < 0 ? -1 : add_const(0, false);
                     return k >= 0 && emit(OP_IN_SET, (uint8_t)k, (uint8_t)s, flags);
                 }
@@ -813,6 +820,13 @@ struct Lower {
     // children of logical predicates are read with get_numberic<bool>() (predicate.h:31)
     bool to_bool(const HExpr& c) { return c.col_type == BK_BOOL ? true : emit(OP_CAST, (uint8_t)c.col_type, (uint8_t)BK_BOOL); }
     bool out_reg(int r) { return emit(OP_OUT, (uint8_t)r); }
+    // the conjunction of `conj` as output `reg`; `where` names the conjuncts in the refusal of more than 8
+    bool predicate(const std::vector<const HExpr*>& conj, int reg, const std::string& where = "") {
+        if (!at_most_8_conjuncts(*in, conj.size(), where)) return false;
+        for (auto* c : conj) { int depth = 0; if (!expr(*c, depth) || !to_bool(*c)) return false; }
+        if (conj.size() > 1 && !emit(OP_AND, (uint8_t)conj.size())) return false;
+        return out_reg(reg);
+    }
 };
 
 static std::string expr_key(const HExpr& e) {  // structural identity, for lane sharing
@@ -869,7 +883,7 @@ static bool lower_agg(Infer& in, Compiled& out, const HNode& agg, const std::vec
     if (agg.agg_fns.size() > MAX_AGG) return in.fail(BKGPU_EUNSUPPORTED, "more than %d aggregate functions", MAX_AGG);
     Program& p = out.prog; memset(&p, 0, sizeof p);
     AggPlan& ap = out.ap; memset(&ap, 0, sizeof ap);
-    Lower lw{&out, &in, &p, {}};
+    Lower lw{&out, &in, &p};
     int reg = 0, depth = 0;
     // ---- predicate: all conjuncts non-NULL true (filter_node.cpp:726-734) ----
     ap.pred_out = -1;
@@ -896,11 +910,8 @@ static bool lower_agg(Infer& in, Compiled& out, const HNode& agg, const std::vec
         if (!lw.out_reg(reg++)) return false;
     }
     if (!conjuncts.empty()) {
-        if (conjuncts.size() > 8) return in.fail(BKGPU_EUNSUPPORTED, "more than 8 conjuncts");
-        for (auto* c : conjuncts) { depth = 0; if (!lw.expr(*c, depth) || !lw.to_bool(*c)) return false; }
-        if (conjuncts.size() > 1 && !lw.emit(OP_AND, (uint8_t)conjuncts.size())) return false;
         ap.pred_out = reg;
-        if (!lw.out_reg(reg++)) return false;
+        if (!lw.predicate(conjuncts, reg++)) return false;
     }
     // ---- group keys ----
     ap.n_group = (int)agg.group_exprs.size();
@@ -1219,16 +1230,7 @@ void patch_in_sets(Compiled& c, const std::vector<uint64_t>& addr) {
     if (c.jfast) patch_in_sets(*c.jfast, addr);
 }
 
-// ---------------------------------------------------------------- entry
-bool lower_sort(Infer& in, Compiled& out, const HNode& sort, const HNode* filter, const HNode& scan);
-bool lower_filter(Infer& in, Compiled& out, const HNode* limit_node, const HNode& filter_or_scan, const HNode& scan);
-bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& join, bool under_packet, const HNode* above);
-bool lower_post(Infer& in, Compiled& out, const HNode* sort, const HNode* having, const HNode* limit_node);
-bool lower_join_rows(Infer& in, Compiled& out, const HNode& join, const HNode* above, const HNode* sort, const HNode* limit_node);
-bool lower_star_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& join, bool under_packet, const HNode* above);
-bool lower_window(Infer& in, Compiled& out, const HNode& wtop, const HNode* outer_sort, const HNode* limit_node);
-static int join_leaves(const HNode* n);
-
+// ---------------------------------------------------------------- steps shared by the fragments
 static bool infer_node(Infer& in, HNode& n) {
     for (auto& e : n.conjuncts) if (!infer_expr(in, e)) return false;
     for (auto& e : n.group_exprs) if (!infer_expr(in, e)) return false;
@@ -1240,151 +1242,122 @@ static bool infer_node(Infer& in, HNode& n) {
     return true;
 }
 
-// [SORT ->] [FILTER ->] JOIN at the top of the fragment -> the JOIN node, else nullptr
-static const HNode* join_rows_shape(const HNode* t) {
-    if (t && t->node_type == BK_SORT_NODE && !t->ch.empty()) t = skip_passthrough(&t->ch[0], nullptr);
-    if (t && is_filter(t) && !t->ch.empty()) t = skip_passthrough(&t->ch[0], nullptr);
-    return t && t->node_type == BK_JOIN_NODE ? t : nullptr;
+static std::vector<const HExpr*> conjuncts_of(const HNode* n) {
+    std::vector<const HExpr*> v;
+    if (n) for (auto& e : n->conjuncts) v.push_back(&e);
+    return v;
 }
 
-int compile_plan(const uint8_t* desc, size_t len, Compiled& out, std::string& err) {
-    if (!desc || len < 16 || (len & 3)) { err = "plan descriptor is empty or not a multiple of 4 bytes"; return BKGPU_EINVAL; }
-    Reader r{}; r.w = (const int32_t*)desc; r.n = len / 4;
-    if ((uint32_t)r.rd() != BKGPU_PLAN_MAGIC) { err = "bad plan magic"; return BKGPU_EINVAL; }
-    if (r.rd() != BKGPU_PLAN_VERSION) { err = "unsupported plan version"; return BKGPU_EINVAL; }
-    int nt = r.rd(), nn = r.rd();
-    if (nt < 0 || nt > 16 || nn <= 0 || nn > 64) { err = "bad tuple / node count"; return BKGPU_EINVAL; }
-    for (int i = 0; i < nt && !r.fail; i++) {
-        HTuple t; t.tuple_id = r.rd(); int ns = r.rd();
-        if (ns < 0 || ns > 4096) { r.bad("bad slot count"); break; }
-        for (int k = 0; k < ns; k++) { int sid = r.rd(); int pt = r.rd(); t.slots.push_back({sid, pt}); }
-        out.tuples.push_back(t);
+// LIMIT n OFFSET m (LimitNode) over rows already capped at `limit` (-1 = none): the fragment keeps the first n + m rows and skips m of them
+static void merge_limit(const HNode* limit_node, int64_t& limit, int64_t& offset) {
+    if (!limit_node) return;
+    offset = limit_node->offset;
+    if (limit_node->limit >= 0) {   // (limit -1 = OFFSET only: every row is kept)
+        const int64_t lim = limit_node->limit + limit_node->offset;
+        if (limit < 0 || lim < limit) limit = lim;
     }
-    HNode root;
-    if (!r.fail) parse_node(r, root, nn, 0);
-    if (!r.fail && nn != 0) r.bad("plan node count mismatch");
-    if (!r.fail && r.pos != r.n) r.bad("trailing words after the plan");
-    if (r.fail) { err = r.err; return r.err.find("outside the GPU path") != std::string::npos ? BKGPU_EUNSUPPORTED : BKGPU_EINVAL; }
-    Infer in{}; in.tuples = &out.tuples;
-    if (!infer_node(in, root)) { err = in.err; return in.code; }
-    out.in_sets = std::make_shared<InSets>();
-
-    bool under_packet = false;
-    const HNode* top = skip_passthrough(&root, &under_packet);
-    if (!top) { err = "empty plan"; return BKGPU_EINVAL; }
-    bool ok = false;
-    const HNode* limit_node = nullptr;
-    if (top->node_type == BK_LIMIT_NODE && !top->ch.empty()) { limit_node = top; top = skip_passthrough(&top->ch[0], &under_packet); }
-    // the db-side chain above an aggregate: [LIMIT ->] [SORT ->] [HAVING_FILTER ->] (MERGE_)AGG (separate.cpp:241-260): the operators
-    // above the aggregate become a post fragment over the aggregate's output rows
-    const HNode *post_sort = nullptr, *post_having = nullptr;
-    {
-        const HNode* t = top;
-        const HNode *ps = nullptr, *ph = nullptr;
-        if (t->node_type == BK_SORT_NODE && !t->ch.empty()) { ps = t; t = skip_passthrough(&t->ch[0], nullptr); }
-        if (t && (is_filter(t) || t->node_type == BK_HAVING_FILTER_NODE) && !t->ch.empty()) { ph = t; t = skip_passthrough(&t->ch[0], nullptr); }
-        if (t && (ps || ph) && (t->node_type == BK_AGG_NODE || t->node_type == BK_MERGE_AGG_NODE)) { post_sort = ps; post_having = ph; top = t; }
-    }
-    const HNode* win_sort = nullptr;   // [SORT ->] WINDOW: the query's ORDER BY above the window stages
-    if (top->node_type == BK_SORT_NODE && !top->ch.empty()) {
-        const HNode* c = skip_passthrough(&top->ch[0], nullptr);
-        if (c && c->node_type == BK_WINDOW_NODE) win_sort = top;
-    }
-    if (win_sort || top->node_type == BK_WINDOW_NODE) {
-        ok = lower_window(in, out, win_sort ? *skip_passthrough(&win_sort->ch[0], nullptr) : *top, win_sort, limit_node);
-    } else if (top->node_type == BK_AGG_NODE || top->node_type == BK_MERGE_AGG_NODE) {
-        if (top->ch.empty()) { err = "AGG node without a child"; return BKGPU_EINVAL; }
-        const HNode* c = skip_passthrough(&top->ch[0], nullptr);
-        const HNode* filter = nullptr;
-        if (is_filter(c)) { filter = c; c = c->ch.empty() ? nullptr : skip_passthrough(&c->ch[0], nullptr); }
-        if (c && c->node_type == BK_SCAN_NODE) {
-            if (filter && filter->limit != -1) { err = "LIMIT on a filter below an aggregate is order dependent: outside the GPU path"; return BKGPU_EUNSUPPORTED; }
-            std::vector<const HExpr*> conj;
-            if (filter) for (auto& e : filter->conjuncts) conj.push_back(&e);
-            ok = lower_agg(in, out, *top, conj, c->tuple_id, under_packet, true);
-            if (ok && limit_node && !post_sort && !post_having) { out.limit = limit_node->limit; out.offset = limit_node->offset; }
-        } else if (c && c->node_type == BK_JOIN_NODE) {   // AGG -> [FILTER ->] JOIN: the store-side chain of a filtered join (separate.cpp:241-260)
-            if (filter && filter->limit != -1) { err = "LIMIT on a filter below an aggregate is order dependent: outside the GPU path"; return BKGPU_EUNSUPPORTED; }
-            ok = join_leaves(c) > 2 ? lower_star_agg(in, out, *top, *c, under_packet, filter) : lower_join_agg(in, out, *top, *c, under_packet, filter);
-            if (ok && limit_node && !post_sort && !post_having) { out.limit = limit_node->limit; out.offset = limit_node->offset; }   // LimitNode over the joined aggregate
-        } else { err = "AGG child must be [FILTER ->] SCAN or JOIN"; return BKGPU_EUNSUPPORTED; }
-        if (ok && (post_sort || post_having)) ok = lower_post(in, out, post_sort, post_having, limit_node);
-    } else if (const HNode* jn = join_rows_shape(top)) {   // [SORT ->] [FILTER ->] JOIN: a join that returns its rows
-        const HNode* t = top; const HNode *js = nullptr, *jf = nullptr;
-        if (t->node_type == BK_SORT_NODE) { js = t; t = skip_passthrough(&t->ch[0], nullptr); }
-        if (is_filter(t)) jf = t;
-        if (join_leaves(jn) > 2) { err = "a join of more than two tables that returns rows is outside the GPU path (an aggregate over a star join is lowered)"; return BKGPU_EUNSUPPORTED; }
-        ok = lower_join_rows(in, out, *jn, jf, js, limit_node);
-    } else if (top->node_type == BK_SORT_NODE) {
-        const HNode* c = top->ch.empty() ? nullptr : skip_passthrough(&top->ch[0], nullptr);
-        const HNode* filter = nullptr;
-        if (is_filter(c)) { filter = c; c = c->ch.empty() ? nullptr : skip_passthrough(&c->ch[0], nullptr); }
-        if (!c || c->node_type != BK_SCAN_NODE) { err = "SORT child must be [FILTER ->] SCAN"; return BKGPU_EUNSUPPORTED; }
-        ok = lower_sort(in, out, *top, filter, *c);
-        if (ok && limit_node) {
-            out.offset = limit_node->offset;
-            if (limit_node->limit >= 0) {   // (limit -1 = OFFSET only: the sort keeps every row)
-                const int64_t lim = limit_node->limit + limit_node->offset;
-                if (out.limit < 0 || lim < out.limit) out.limit = lim;
-            }
-        }
-    } else if (is_filter(top) || top->node_type == BK_SCAN_NODE) {
-        const HNode* c = top;
-        if (is_filter(c)) c = c->ch.empty() ? nullptr : skip_passthrough(&c->ch[0], nullptr);
-        if (!c || c->node_type != BK_SCAN_NODE) { err = "FILTER child must be SCAN"; return BKGPU_EUNSUPPORTED; }
-        ok = lower_filter(in, out, limit_node, *top, *c);
-    } else { err = "plan root is outside the GPU path"; return BKGPU_EUNSUPPORTED; }
-    if (!ok) { err = in.err.empty() ? "plan could not be lowered" : in.err; return in.code ? in.code : BKGPU_EUNSUPPORTED; }
-    explain(out);
-    return BKGPU_OK;
 }
 
-// ---------------------------------------------------------------- SORT / filter-only fragments
-// Rows of the scan tuple are returned (all slots of its tuple descriptor), ordered / filtered.
-static bool intern_scan_tuple(Infer& in, Compiled& out, Lower& lw, int tuple_id) {
+// the keys of a SORT node, one program output each from `reg` on
+static bool lower_order_by(Lower& lw, const HNode& sort, std::vector<SortKey>& keys, int& reg) {
+    if (sort.order_exprs.empty()) return lw.in->fail(BKGPU_EINVAL, "SORT node without order expressions");
+    if (sort.order_exprs.size() > 4) return lw.in->fail(BKGPU_EUNSUPPORTED, "more than 4 ORDER BY expressions");
+    for (size_t i = 0; i < sort.order_exprs.size(); i++) {
+        const HExpr& e = sort.order_exprs[i];
+        if (e.col_type == BK_STRING) return lw.in->fail(BKGPU_EUNSUPPORTED, "ORDER BY over a STRING key is outside the GPU path");
+        int depth = 0;
+        if (!lw.expr(e, depth)) return false;
+        keys.push_back({reg, e.col_type, sort.is_asc[i] != 0, sort.is_null_first[i] != 0});
+        if (!lw.out_reg(reg++)) return false;
+    }
+    return true;
+}
+
+// a filter node's conjunction as output `reg` (ap.pred_out; -1 without conjuncts)
+static bool lower_predicate(Lower& lw, const HNode* filter, AggPlan& ap, int& reg) {
+    ap.pred_out = -1;
+    if (!filter || filter->conjuncts.empty()) return true;
+    ap.pred_out = reg;
+    return lw.predicate(conjuncts_of(filter), reg++);
+}
+
+// a one-output program of its own (a join child's or a star dimension's filter, a window expression): constants numbered from 0, the
+// columns it reads become plan columns
+template <class F> static bool lower_own_program(Infer& in, Compiled& out, Program& prog, F&& body) {
+    memset(&prog, 0, sizeof prog);
+    Lower l{&out, &in, &prog};
+    if (!body(l)) return false;
+    prog.n_out = 1;
+    return true;
+}
+
+// every slot of `tuple_id` becomes a plan column and an output column, in the order of its descriptor
+static bool intern_tuple(Infer& in, Compiled& out, Lower& lw, int tuple_id, const char* tuple_name, const char* row_name) {
     const HTuple* t = nullptr;
     for (auto& x : out.tuples) if (x.tuple_id == tuple_id) t = &x;
-    if (!t || t->slots.empty()) return in.fail(BKGPU_EINVAL, "scan tuple %d has no descriptor", tuple_id);
+    if (!t || t->slots.empty()) return in.fail(BKGPU_EINVAL, "%s %d has no descriptor", tuple_name, tuple_id);
     for (auto& sl : t->slots) {
         if (prim_storage(sl.second) < 0 || sl.second == BK_STRING)
             return in.fail(BKGPU_EUNSUPPORTED, "column %d_%d has type %d: outside the GPU path", tuple_id, sl.first, sl.second);
-        int ci = lw.intern_col(tuple_id, sl.first, sl.second);
-        if (ci >= MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d columns in the scan tuple", MAX_COLS);
+        if (lw.intern_col(tuple_id, sl.first, sl.second) >= MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d columns in %s", MAX_COLS, row_name);
         out.out_cols.push_back({tuple_id, sl.first, sl.second, 0});
     }
     return true;
 }
-static bool lower_predicate(Infer& in, Lower& lw, const HNode* filter, AggPlan& ap, int& reg) {
-    ap.pred_out = -1;
-    if (!filter || filter->conjuncts.empty()) return true;
-    if (filter->conjuncts.size() > 8) return in.fail(BKGPU_EUNSUPPORTED, "more than 8 conjuncts");
-    for (auto& c : filter->conjuncts) { int depth = 0; if (!lw.expr(c, depth) || !lw.to_bool(c)) return false; }
-    if (filter->conjuncts.size() > 1 && !lw.emit(OP_AND, (uint8_t)filter->conjuncts.size())) return false;
-    ap.pred_out = reg;
-    return lw.out_reg(reg++);
+
+// A sink fragment (Compiled::post, kind PK_SORT / PK_FILTER) over another fragment's output rows: its "scan tuple" is `out.out_cols`, in
+// order.  Above an aggregate ([LIMIT ->] [SORT ->] [HAVING ->]: SortNode::open src/exec/sort_node.cpp:278-346, FilterNode::get_next
+// src/exec/filter_node.cpp:726-795 over the rows AggNode::get_next emits), the query's ORDER BY above window stages, and the joined rows
+// of a join that returns them.
+struct Sink {
+    const HNode* sort;       // ORDER BY keys: PK_SORT, else PK_FILTER
+    const HNode* pred;       // HAVING, or the filter above a FULL join (it judges the NULL-extended rows too)
+    int64_t own_limit;       // without a SORT: the rows' own limit
+    bool agg_rows;           // rows of an aggregate or a window: AVG blobs ride along as 16-byte payload columns, a column twice is refused
+    const char* too_wide;    // refused: more than MAX_COLS input columns
+    const char* outside;     // refused: a key or the predicate reads a column that is not an input column
+};
+static bool lower_sink(Infer& in, Compiled& out, const Sink& s, const HNode* limit_node) {
+    if (out.out_cols.size() > (size_t)MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d %s", MAX_COLS, s.too_wide);
+    auto post = std::make_shared<Compiled>();
+    Compiled& pc = *post;
+    pc.kind = s.sort ? PK_SORT : PK_FILTER;
+    pc.tuples = out.tuples; pc.scan_tuple = -1; pc.in_sets = out.in_sets;
+    Program& p = pc.prog; memset(&p, 0, sizeof p);
+    memset(&pc.ap, 0, sizeof pc.ap);
+    Lower lw{&pc, &in, &p};
+    for (const OutCol& oc : out.out_cols) {
+        const int prim = s.agg_rows && oc.kind == 1 ? BK_STRING : oc.prim;
+        const int ci = lw.intern_col(oc.tuple_id, oc.slot_id, prim);
+        if (s.agg_rows && ci != (int)pc.out_cols.size()) return in.fail(BKGPU_EUNSUPPORTED, "aggregate output columns %d_%d appear twice", oc.tuple_id, oc.slot_id);
+        pc.out_cols.push_back({oc.tuple_id, oc.slot_id, prim, oc.kind});
+    }
+    int reg = 0;
+    if (s.pred && s.pred->limit != -1 && s.sort) return in.fail(BKGPU_EUNSUPPORTED, "LIMIT on a HAVING filter below a sort is order dependent");
+    if (!lower_predicate(lw, s.pred, pc.ap, reg)) return false;
+    pc.limit = s.sort ? s.sort->limit : s.own_limit;
+    if (s.sort && !lower_order_by(lw, *s.sort, pc.sort_keys, reg)) return false;
+    merge_limit(limit_node, pc.limit, pc.offset);
+    p.n_out = reg;
+    if (pc.cols.size() != out.out_cols.size()) return in.fail(BKGPU_EUNSUPPORTED, "%s", s.outside);
+    pc.has_direct = false;
+    out.post = post;
+    return true;
 }
 
-bool lower_sort(Infer& in, Compiled& out, const HNode& sort, const HNode* filter, const HNode& scan) {
+// ---------------------------------------------------------------- SORT / filter-only fragments
+// Rows of the scan tuple are returned (all slots of its tuple descriptor), ordered / filtered.
+static bool lower_sort(Infer& in, Compiled& out, const HNode& sort, const HNode* filter, const HNode& scan) {
     out.kind = PK_SORT;
     out.scan_tuple = scan.tuple_id;
     out.limit = sort.limit;
     if (filter && filter->limit != -1) return in.fail(BKGPU_EUNSUPPORTED, "LIMIT on a filter below a sort is order dependent");
     Program& p = out.prog; memset(&p, 0, sizeof p);
     memset(&out.ap, 0, sizeof out.ap);
-    Lower lw{&out, &in, &p, {}};
-    if (!intern_scan_tuple(in, out, lw, scan.tuple_id)) return false;
+    Lower lw{&out, &in, &p};
+    if (!intern_tuple(in, out, lw, scan.tuple_id, "scan tuple", "the scan tuple")) return false;
     int reg = 0;
-    if (!lower_predicate(in, lw, filter, out.ap, reg)) return false;
-    if (sort.order_exprs.empty()) return in.fail(BKGPU_EINVAL, "SORT node without order expressions");
-    if (sort.order_exprs.size() > 4) return in.fail(BKGPU_EUNSUPPORTED, "more than 4 ORDER BY expressions");
-    for (size_t i = 0; i < sort.order_exprs.size(); i++) {
-        const HExpr& e = sort.order_exprs[i];
-        if (e.col_type == BK_STRING) return in.fail(BKGPU_EUNSUPPORTED, "ORDER BY over a STRING key is outside the GPU path");
-        int depth = 0;
-        if (!lw.expr(e, depth)) return false;
-        out.sort_keys.push_back({reg, e.col_type, sort.is_asc[i] != 0, sort.is_null_first[i] != 0});
-        if (!lw.out_reg(reg++)) return false;
-    }
+    if (!lower_predicate(lw, filter, out.ap, reg) || !lower_order_by(lw, sort, out.sort_keys, reg)) return false;
     p.n_out = reg;
     // direct shape: one plain column key, no filter (config C5)
     out.has_direct = false;
@@ -1400,93 +1373,27 @@ bool lower_sort(Infer& in, Compiled& out, const HNode& sort, const HNode* filter
     return true;
 }
 
-bool lower_filter(Infer& in, Compiled& out, const HNode* limit_node, const HNode& top, const HNode& scan) {
+static bool lower_filter(Infer& in, Compiled& out, const HNode* limit_node, const HNode& top, const HNode& scan) {
     out.kind = PK_FILTER;
     out.scan_tuple = scan.tuple_id;
     const HNode* filter = is_filter(&top) ? &top : nullptr;
     out.limit = filter ? filter->limit : scan.limit;   // FilterNode honours its own limit in input order (filter_node.cpp:786-791)
     out.offset = 0;
-    if (limit_node) {
-        out.offset = limit_node->offset;
-        int64_t lim = limit_node->limit < 0 ? -1 : limit_node->limit + limit_node->offset;
-        if (lim >= 0 && (out.limit < 0 || lim < out.limit)) out.limit = lim;
-    }
+    merge_limit(limit_node, out.limit, out.offset);
     Program& p = out.prog; memset(&p, 0, sizeof p);
     memset(&out.ap, 0, sizeof out.ap);
-    Lower lw{&out, &in, &p, {}};
-    if (!intern_scan_tuple(in, out, lw, scan.tuple_id)) return false;
+    Lower lw{&out, &in, &p};
+    if (!intern_tuple(in, out, lw, scan.tuple_id, "scan tuple", "the scan tuple")) return false;
     int reg = 0;
-    if (!lower_predicate(in, lw, filter, out.ap, reg)) return false;
+    if (!lower_predicate(lw, filter, out.ap, reg)) return false;
     p.n_out = reg;
     return true;
 }
 
-// [LIMIT ->] [SORT ->] [HAVING ->] over an aggregate: a fragment of kind PK_SORT / PK_FILTER whose input rows are the aggregate's
-// output columns (SortNode::open src/exec/sort_node.cpp:278-346, FilterNode::get_next src/exec/filter_node.cpp:726-795 over the
-// rows AggNode::get_next emits).  The AVG intermediate blobs ride along as 16-byte payload columns.
-bool lower_post(Infer& in, Compiled& out, const HNode* sort, const HNode* having, const HNode* limit_node) {
-    auto post = std::make_shared<Compiled>();
-    Compiled& pc = *post;
-    pc.kind = sort ? PK_SORT : PK_FILTER;
-    pc.tuples = out.tuples;
-    pc.scan_tuple = -1;
-    pc.in_sets = out.in_sets;
-    Program& p = pc.prog; memset(&p, 0, sizeof p);
-    memset(&pc.ap, 0, sizeof pc.ap);
-    Lower lw{&pc, &in, &p, {}};
-    if (out.out_cols.size() > (size_t)MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d aggregate output columns under a SORT / HAVING", MAX_COLS);
-    for (const OutCol& oc : out.out_cols) {
-        const int prim = oc.kind == 1 ? BK_STRING : oc.prim;
-        const int ci = lw.intern_col(oc.tuple_id, oc.slot_id, prim);
-        if (ci != (int)pc.out_cols.size()) return in.fail(BKGPU_EUNSUPPORTED, "aggregate output columns %d_%d appear twice", oc.tuple_id, oc.slot_id);
-        pc.out_cols.push_back({oc.tuple_id, oc.slot_id, prim, oc.kind});
-    }
-    const size_t n_payload = pc.cols.size();
-    int reg = 0;
-    if (having && having->limit != -1 && sort) return in.fail(BKGPU_EUNSUPPORTED, "LIMIT on a HAVING filter below a sort is order dependent");
-    if (!lower_predicate(in, lw, having, pc.ap, reg)) return false;
-    if (sort) {
-        pc.limit = sort->limit;
-        if (sort->order_exprs.empty()) return in.fail(BKGPU_EINVAL, "SORT node without order expressions");
-        if (sort->order_exprs.size() > 4) return in.fail(BKGPU_EUNSUPPORTED, "more than 4 ORDER BY expressions");
-        for (size_t i = 0; i < sort->order_exprs.size(); i++) {
-            const HExpr& e = sort->order_exprs[i];
-            if (e.col_type == BK_STRING) return in.fail(BKGPU_EUNSUPPORTED, "ORDER BY over a STRING key is outside the GPU path");
-            int depth = 0;
-            if (!lw.expr(e, depth)) return false;
-            pc.sort_keys.push_back({reg, e.col_type, sort->is_asc[i] != 0, sort->is_null_first[i] != 0});
-            if (!lw.out_reg(reg++)) return false;
-        }
-        if (limit_node) {
-            pc.offset = limit_node->offset;
-            if (limit_node->limit >= 0) { const int64_t lim = limit_node->limit + limit_node->offset; if (pc.limit < 0 || lim < pc.limit) pc.limit = lim; }
-        }
-    } else {
-        pc.limit = having ? having->limit : -1;
-        pc.offset = 0;
-        if (limit_node) {
-            pc.offset = limit_node->offset;
-            const int64_t lim = limit_node->limit < 0 ? -1 : limit_node->limit + limit_node->offset;
-            if (lim >= 0 && (pc.limit < 0 || lim < pc.limit)) pc.limit = lim;
-        }
-    }
-    p.n_out = reg;
-    if (pc.cols.size() != n_payload) return in.fail(BKGPU_EUNSUPPORTED, "SORT / HAVING above an aggregate references a column the aggregate does not output");
-    pc.has_direct = false;
-    out.post = post;
-    return true;
-}
-
-// AGG over an equi-join (config C3).  The reference builds its hash map on the OUTER (driver) child and probes
-// with the inner child's rows (JoinNode::hash_join, src/exec/join_node.cpp:920-1022; Joiner::construct_hash_map,
-// src/exec/joiner.cpp:624-631); the key is the cast equal-slot value (strip_out_equal_slots, joiner.cpp:166-217).
-// Filters of both children and the residual join conditions become one predicate over the joined row — for an
-// INNER join that is the same set of rows.  LEFT / SEMI / ANTI: a child's filter must remove the child's rows before the join (a build row
-// that fails it would still come out of the ANTI tail, or NULL-extended), so each child's filter is a program of its own
-// (Compiled::build_filter / probe_filter) and the main program keeps the residual conditions alone.
-// FULL: the residual conditions decide the pairs (k_join_pairs_full); the filter above the join — the planner keeps a join FULL only under a
-// NULL-tolerant one (join_node.cpp:171-203) — judges every emitted row, NULL-extended ones included, as the predicate of `jfast`, the
-// aggregate over the pairs' gathered columns.
+// ---------------------------------------------------------------- two-table joins
+// The reference builds its hash map on the OUTER (driver) child and probes with the inner child's rows (JoinNode::hash_join,
+// src/exec/join_node.cpp:920-1022; Joiner::construct_hash_map, src/exec/joiner.cpp:624-631); the key is the cast equal-slot value
+// (strip_out_equal_slots, joiner.cpp:166-217).
 static void intern_slots(Lower& lw, Infer& in, const HExpr& e) {   // every column `e` reads becomes a plan column
     if (e.node_type == BK_SLOT_REF) {
         const int st = in.slot_type(e.tuple_id, e.slot_id);
@@ -1494,42 +1401,100 @@ static void intern_slots(Lower& lw, Infer& in, const HExpr& e) {   // every colu
     }
     for (auto& c : e.ch) intern_slots(lw, in, c);
 }
-static void expr_tuples(const HExpr& e, std::vector<int>& t);
+static void expr_tuples(const HExpr& e, std::vector<int>& t) {
+    if (e.node_type == BK_SLOT_REF && std::find(t.begin(), t.end(), e.tuple_id) == t.end()) t.push_back(e.tuple_id);
+    for (auto& c : e.ch) expr_tuples(c, t);
+}
 // LEFT / SEMI / ANTI_SEMI: the filter of the child scanning `tuple_id` (FilterNode under JoinNode) stays that child's: a program of its own
-// whose output 0 is the conjunction, constants numbered per program (as a star dimension's filter).  Its columns become plan columns.
+// whose output 0 is the conjunction.  Its columns become plan columns.
 static bool lower_child_filter(Infer& in, Compiled& out, const HNode* filt, int tuple_id, Program& prog, int& n) {
     memset(&prog, 0, sizeof prog); n = 0;
     if (!filt || filt->conjuncts.empty()) return true;
-    if (filt->conjuncts.size() > 8) return in.fail(BKGPU_EUNSUPPORTED, "more than 8 conjuncts in the filter of join child %d", tuple_id);
+    const std::string where = " in the filter of join child " + std::to_string(tuple_id);
+    if (!at_most_8_conjuncts(in, filt->conjuncts.size(), where)) return false;   // (before the check of the tuples it reads)
     for (auto& e : filt->conjuncts) {
         std::vector<int> ts; expr_tuples(e, ts);
         for (int t : ts) if (t != tuple_id) return in.fail(BKGPU_EINVAL, "the filter of join child %d reads tuple %d", tuple_id, t);
     }
-    const int n_const = out.n_const;
-    out.n_const = 0;
-    Lower fl{&out, &in, &prog, {}};
-    for (auto& e : filt->conjuncts) { int depth = 0; if (!fl.expr(e, depth) || !fl.to_bool(e)) return false; }
-    if (filt->conjuncts.size() > 1 && !fl.emit(OP_AND, (uint8_t)filt->conjuncts.size())) return false;
-    if (!fl.out_reg(0)) return false;
-    prog.n_out = 1; n = (int)filt->conjuncts.size();
-    out.n_const = n_const;
-    return true;
+    n = (int)filt->conjuncts.size();
+    return lower_own_program(in, out, prog, [&](Lower& l) { return l.predicate(conjuncts_of(filt), 0, where); });
 }
-bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& join, bool under_packet, const HNode* above) {
-    int jt = join.join_type;
-    if (jt != BK_INNER_JOIN && jt != BK_LEFT_JOIN && jt != BK_RIGHT_JOIN && jt != BK_SEMI_JOIN && jt != BK_ANTI_SEMI_JOIN && jt != BK_FULL_JOIN)
-        return in.fail(BKGPU_EUNSUPPORTED, "join type %d is outside the GPU path", jt);
-    if (join.ch.size() != 2) return in.fail(BKGPU_EINVAL, "JOIN node needs two children");
-    const HNode* side[2]; const HNode* filt[2] = {nullptr, nullptr};
+// the children, build (outer) side first, each [FILTER ->] SCAN.  RIGHT JOIN: the reference swaps the roles — the right child becomes the
+// outer (preserved, driver) table (join_node.cpp:151-156) — and the join is lowered as LEFT.
+static bool join_children(Infer& in, const HNode& join, int& jt, const HNode* side[2], const HNode* filt[2]) {
     for (int i = 0; i < 2; i++) {
-        // RIGHT JOIN: the reference swaps the roles — the right child becomes the outer (preserved, driver) table (join_node.cpp:151-156)
         const HNode* c = skip_passthrough(&join.ch[(size_t)(jt == BK_RIGHT_JOIN ? 1 - i : i)], nullptr);
+        filt[i] = nullptr;
         if (is_filter(c)) { filt[i] = c; c = c->ch.empty() ? nullptr : skip_passthrough(&c->ch[0], nullptr); }
         if (!c || c->node_type != BK_SCAN_NODE) return in.fail(BKGPU_EUNSUPPORTED, "JOIN children must be [FILTER ->] SCAN");
         if (filt[i] && filt[i]->limit != -1) return in.fail(BKGPU_EUNSUPPORTED, "LIMIT below a join is order dependent");
         side[i] = c;
     }
     if (jt == BK_RIGHT_JOIN) jt = BK_LEFT_JOIN;
+    return true;
+}
+// the join key: the first build = probe slot equality among the join conditions; the others go to `rest` (residual conditions)
+static bool join_equality(Infer& in, const HNode& join, int build_tuple, int probe_tuple, const HExpr*& bk, const HExpr*& pk, std::vector<const HExpr*>& rest) {
+    bk = pk = nullptr;
+    for (auto& e : join.conjuncts) {
+        bool taken = false;
+        if (!bk && e.node_type == BK_FUNCTION_CALL && e.fn_op == BK_FT_EQ && e.ch.size() == 2 && e.ch[0].node_type == BK_SLOT_REF && e.ch[1].node_type == BK_SLOT_REF) {
+            const HExpr *a = &e.ch[0], *b = &e.ch[1];
+            if (a->tuple_id == build_tuple && b->tuple_id == probe_tuple) { bk = a; pk = b; taken = true; }
+            else if (b->tuple_id == build_tuple && a->tuple_id == probe_tuple) { bk = b; pk = a; taken = true; }
+        }
+        if (!taken) rest.push_back(&e);
+    }
+    return bk || in.fail(BKGPU_EUNSUPPORTED, "join without an equality between the two tables (nested loop) is outside the GPU path");
+}
+// the type the build / dimension key `a` and the probe / fact key `b` are compared in (strip_out_equal_slots' cast, joiner.cpp:166-217):
+// equal types as they are, two signed types as INT64, two unsigned ones as UINT64; the reference compares any other pair as STRING
+static bool join_key_cast(Infer& in, int a, int b, int& cast) {
+    if (a == b) cast = a;
+    else if (is_signed_t(a) && is_signed_t(b)) cast = BK_INT64;
+    else if (is_uint_t(a) && is_uint_t(b)) cast = BK_UINT64;
+    else return in.fail(BKGPU_EUNSUPPORTED, "join keys of types %d and %d are compared as STRING in the reference: outside the GPU path", a, b);
+    if (cast == BK_STRING || is_double_t(cast)) return in.fail(BKGPU_EUNSUPPORTED, "join key type %d is outside the GPU path", cast);
+    return true;
+}
+
+// The aggregate over the joined row (Compiled::jfast): the same aggregate lowered again with every column as a column of ONE (virtual,
+// joined) tuple, build-side / dimension columns gathered to probe-row alignment first.  Its key words and lanes must be the main plan's and
+// every column it reads one of the main plan's (jfast_of_main).  1 = lowered; 0 = it does not lower alike (`why`: its error); -1 = it
+// reads `missing`, which is no main plan column.
+static int lower_joined_row_agg(Compiled& out, const HNode& agg, const std::vector<const HExpr*>& conj, int scan_tuple, bool under_packet,
+                                std::string& why, ColRef& missing) {
+    auto jf = std::make_shared<Compiled>();
+    jf->tuples = out.tuples; jf->build_tuple = -1; jf->in_sets = out.in_sets;
+    Infer in2{}; in2.tuples = &jf->tuples;
+    if (!lower_agg(in2, *jf, agg, conj, scan_tuple, under_packet, true) || memcmp(&jf->ap.n_keyw, &out.ap.n_keyw, sizeof(int32_t) * 4) != 0 ||
+        jf->ap.n_lanes != out.ap.n_lanes) { why = in2.err; return 0; }
+    std::vector<int> of_main;
+    for (auto& c : jf->cols) {
+        int m = -1;
+        for (size_t i = 0; i < out.cols.size(); i++) if (out.cols[i].tuple_id == c.tuple_id && out.cols[i].slot_id == c.slot_id) m = (int)i;
+        if (m < 0) { missing = c; return -1; }
+        of_main.push_back(m);
+    }
+    out.jfast = jf;
+    out.jfast_of_main = of_main;
+    return 1;
+}
+
+// AGG over an equi-join (config C3).  Filters of both children and the residual join conditions become one predicate over the joined
+// row — for an INNER join that is the same set of rows.  LEFT / SEMI / ANTI: a child's filter must remove the child's rows before the join
+// (a build row that fails it would still come out of the ANTI tail, or NULL-extended), so each child's filter is a program of its own
+// (Compiled::build_filter / probe_filter) and the main program keeps the residual conditions alone.
+// FULL: the residual conditions decide the pairs (k_join_pairs_full); the filter above the join — the planner keeps a join FULL only under a
+// NULL-tolerant one (join_node.cpp:171-203) — judges every emitted row, NULL-extended ones included, as the predicate of `jfast`, the
+// aggregate over the pairs' gathered columns.
+static bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& join, bool under_packet, const HNode* above) {
+    int jt = join.join_type;
+    if (jt != BK_INNER_JOIN && jt != BK_LEFT_JOIN && jt != BK_RIGHT_JOIN && jt != BK_SEMI_JOIN && jt != BK_ANTI_SEMI_JOIN && jt != BK_FULL_JOIN)
+        return in.fail(BKGPU_EUNSUPPORTED, "join type %d is outside the GPU path", jt);
+    if (join.ch.size() != 2) return in.fail(BKGPU_EINVAL, "JOIN node needs two children");
+    const HNode *side[2], *filt[2];
+    if (!join_children(in, join, jt, side, filt)) return false;
     // the fused predicate (child filters + residual conditions over the joined row) equals filter-then-join only for INNER joins
     // a filter ABOVE the join sees the joined row: for an INNER join it simply joins the residual conditions; above an outer join it would also
     // have to judge the NULL-extended rows, after the match decision — a second predicate the probe does not carry
@@ -1541,27 +1506,13 @@ bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
     const int build_tuple = side[0]->tuple_id, probe_tuple = side[1]->tuple_id;
     out.build_tuple = build_tuple;
     std::vector<const HExpr*> conj;
-    const HExpr *bk = nullptr, *pk = nullptr;
-    for (auto& e : join.conjuncts) {
-        bool taken = false;
-        if (!bk && e.node_type == BK_FUNCTION_CALL && e.fn_op == BK_FT_EQ && e.ch.size() == 2 && e.ch[0].node_type == BK_SLOT_REF && e.ch[1].node_type == BK_SLOT_REF) {
-            const HExpr *a = &e.ch[0], *b = &e.ch[1];
-            if (a->tuple_id == build_tuple && b->tuple_id == probe_tuple) { bk = a; pk = b; taken = true; }
-            else if (b->tuple_id == build_tuple && a->tuple_id == probe_tuple) { bk = b; pk = a; taken = true; }
-        }
-        if (!taken) conj.push_back(&e);
-    }
-    if (!bk) return in.fail(BKGPU_EUNSUPPORTED, "join without an equality between the two tables (nested loop) is outside the GPU path");
+    const HExpr *bk, *pk;
+    if (!join_equality(in, join, build_tuple, probe_tuple, bk, pk, conj)) return false;
     if (jt == BK_INNER_JOIN) for (int i = 0; i < 2; i++) if (filt[i]) for (auto& e : filt[i]->conjuncts) conj.push_back(&e);
     std::vector<const HExpr*> above_conj;
     if (above) for (auto& e : above->conjuncts) (full ? above_conj : conj).push_back(&e);
-    int ot = bk->col_type, it = pk->col_type, cast;
-    auto is_signed_t = [](int t) { return t >= BK_INT8 && t <= BK_INT64; };
-    if (ot == it) cast = ot;
-    else if (is_signed_t(ot) && is_signed_t(it)) cast = BK_INT64;
-    else if (is_uint_t(ot) && is_uint_t(it)) cast = BK_UINT64;
-    else return in.fail(BKGPU_EUNSUPPORTED, "join keys of types %d and %d are compared as STRING in the reference: outside the GPU path", ot, it);
-    if (cast == BK_STRING || is_double_t(cast)) return in.fail(BKGPU_EUNSUPPORTED, "join key type %d is outside the GPU path", cast);
+    int cast;
+    if (!join_key_cast(in, bk->col_type, pk->col_type, cast)) return false;
     if (full && agg.node_type == BK_MERGE_AGG_NODE) return in.fail(BKGPU_EUNSUPPORTED, "MERGE_AGG over a FULL join is outside the GPU path");
     if (!lower_agg(in, out, agg, conj, probe_tuple, under_packet, false)) return false;
     if (full) {   // the pairs kernel runs the main program for its predicate alone (the residual conditions): the aggregate is jfast's
@@ -1573,31 +1524,19 @@ bool lower_join_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
     out.kind = PK_JOIN_AGG;
     out.join_type = jt; out.join_key_prim = cast;
     Program dummy; memset(&dummy, 0, sizeof dummy);
-    Lower lw{&out, &in, &dummy, {}};
+    Lower lw{&out, &in, &dummy};
     out.build_key_col = lw.intern_col(bk->tuple_id, bk->slot_id, in.slot_type(bk->tuple_id, bk->slot_id));
     out.probe_key_col = lw.intern_col(pk->tuple_id, pk->slot_id, in.slot_type(pk->tuple_id, pk->slot_id));
     for (auto* e : above_conj) intern_slots(lw, in, *e);   // (FULL: read by jfast's predicate alone, gathered like the aggregate's columns)
     if (jt != BK_INNER_JOIN && (!lower_child_filter(in, out, filt[0], build_tuple, out.build_filter, out.n_build_filter) ||
                                 !lower_child_filter(in, out, filt[1], probe_tuple, out.probe_filter, out.n_probe_filter))) return false;
     if ((int)out.cols.size() > MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d columns referenced", MAX_COLS);
-    // fast path: lower the same aggregate again with every column treated as a column of ONE (virtual, joined) tuple.  FULL: the path
-    // itself, with the filter above the join as the predicate
+    // INNER: the FK -> PK fast path, usable while every probe row has exactly one match.  FULL: the path itself, with the filter above the
+    // join as the predicate
     if (jt == BK_INNER_JOIN || full) {
-        auto jf = std::make_shared<Compiled>();
-        jf->tuples = out.tuples; jf->build_tuple = -1; jf->in_sets = out.in_sets;
-        Infer in2{}; in2.tuples = &jf->tuples;
-        if (lower_agg(in2, *jf, agg, full ? above_conj : conj, probe_tuple, under_packet, true) && memcmp(&jf->ap.n_keyw, &out.ap.n_keyw, sizeof(int32_t) * 4) == 0 &&
-            jf->ap.n_lanes == out.ap.n_lanes) {
-            bool ok = true;
-            for (auto& c : jf->cols) {
-                int m = -1;
-                for (size_t i = 0; i < out.cols.size(); i++) if (out.cols[i].tuple_id == c.tuple_id && out.cols[i].slot_id == c.slot_id) m = (int)i;
-                if (m < 0) ok = false;
-                out.jfast_of_main.push_back(m);
-            }
-            if (ok) out.jfast = jf; else out.jfast_of_main.clear();
-        }
-        if (full && !out.jfast) return in.fail(BKGPU_EUNSUPPORTED, "the aggregate over the FULL join's row could not be lowered: %s", in2.err.c_str());
+        std::string why; ColRef missing;
+        if (lower_joined_row_agg(out, agg, full ? above_conj : conj, probe_tuple, under_packet, why, missing) <= 0 && full)
+            return in.fail(BKGPU_EUNSUPPORTED, "the aggregate over the FULL join's row could not be lowered: %s", why.c_str());
     }
     return true;
 }
@@ -1631,16 +1570,12 @@ static bool star_walk(Infer& in, const HNode* n, std::vector<int>& leaves, std::
     leaves.push_back(n->tuple_id);
     return true;
 }
-static void expr_tuples(const HExpr& e, std::vector<int>& t) {
-    if (e.node_type == BK_SLOT_REF && std::find(t.begin(), t.end(), e.tuple_id) == t.end()) t.push_back(e.tuple_id);
-    for (auto& c : e.ch) expr_tuples(c, t);
-}
 static bool slot_eq(const HExpr& e) {
     return e.node_type == BK_FUNCTION_CALL && e.fn_op == BK_FT_EQ && e.ch.size() == 2 && e.ch[0].node_type == BK_SLOT_REF && e.ch[1].node_type == BK_SLOT_REF &&
            e.ch[0].tuple_id != e.ch[1].tuple_id;
 }
 
-bool lower_star_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& join, bool under_packet, const HNode* above) {
+static bool lower_star_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& join, bool under_packet, const HNode* above) {
     std::vector<int> leaves; std::vector<const HExpr*> conds;
     if (!star_walk(in, &join, leaves, conds)) return false;
     if (leaves.size() > 5) return in.fail(BKGPU_EUNSUPPORTED, "a star join of %zu tables has more than 4 dimensions", leaves.size());
@@ -1658,7 +1593,6 @@ bool lower_star_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
     }
     if (fact < 0) return in.fail(BKGPU_EUNSUPPORTED, "join of %zu tables without a star centre (a dimension keyed only to another dimension): outside the GPU path", leaves.size());
     std::vector<const HExpr*> taken;
-    auto is_signed_t = [](int t) { return t >= BK_INT8 && t <= BK_INT64; };
     for (int t : leaves) {
         if (t == fact) continue;
         StarDim d; d.tuple_id = t;
@@ -1669,12 +1603,7 @@ bool lower_star_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
             if (a->tuple_id == fact && b->tuple_id == t) std::swap(a, b);
             if (a->tuple_id == t && b->tuple_id == fact) { dk = a; fk = b; taken.push_back(e); break; }
         }
-        const int dt = dk->col_type, ft = fk->col_type;
-        if (dt == ft) d.cast_prim = dt;
-        else if (is_signed_t(dt) && is_signed_t(ft)) d.cast_prim = BK_INT64;
-        else if (is_uint_t(dt) && is_uint_t(ft)) d.cast_prim = BK_UINT64;
-        else return in.fail(BKGPU_EUNSUPPORTED, "join keys of types %d and %d are compared as STRING in the reference: outside the GPU path", dt, ft);
-        if (d.cast_prim == BK_STRING || is_double_t(d.cast_prim)) return in.fail(BKGPU_EUNSUPPORTED, "join key type %d is outside the GPU path", d.cast_prim);
+        if (!join_key_cast(in, dk->col_type, fk->col_type, d.cast_prim)) return false;
         d.key_col = dk->slot_id; d.fk_col = fk->slot_id;   // (slot ids until the columns are interned below)
         out.dims.push_back(d);
     }
@@ -1691,41 +1620,26 @@ bool lower_star_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
     if (!lower_agg(in, out, agg, conj, fact, under_packet, false)) return false;
     out.kind = PK_STAR_AGG;
     Program dummy; memset(&dummy, 0, sizeof dummy);
-    Lower lw{&out, &in, &dummy, {}};
+    Lower lw{&out, &in, &dummy};
     for (size_t i = 0; i < out.dims.size(); i++) {
         StarDim& d = out.dims[i];
         d.key_col = lw.intern_col(d.tuple_id, d.key_col, in.slot_type(d.tuple_id, d.key_col));
         d.fk_col = lw.intern_col(fact, d.fk_col, in.slot_type(fact, d.fk_col));
-        memset(&d.filter, 0, sizeof d.filter);
         if (dim_conj[i].empty()) continue;
-        if (dim_conj[i].size() > 8) return in.fail(BKGPU_EUNSUPPORTED, "more than 8 conjuncts on dimension %d", d.tuple_id);
-        const int n_const = out.n_const;   // (constants are numbered per program)
-        out.n_const = 0;
-        Lower fl{&out, &in, &d.filter, {}};
-        for (auto* c : dim_conj[i]) { int depth = 0; if (!fl.expr(*c, depth) || !fl.to_bool(*c)) return false; }
-        if (dim_conj[i].size() > 1 && !fl.emit(OP_AND, (uint8_t)dim_conj[i].size())) return false;
-        if (!fl.out_reg(0)) return false;
-        d.filter.n_out = 1; d.n_filter = (int)dim_conj[i].size();
-        out.n_const = n_const;
+        d.n_filter = (int)dim_conj[i].size();
+        if (!lower_own_program(in, out, d.filter, [&](Lower& l) { return l.predicate(dim_conj[i], 0, " on dimension " + std::to_string(d.tuple_id)); }))
+            return false;
     }
     if ((int)out.cols.size() > MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d columns referenced", MAX_COLS);
     for (size_t i = 0; i < out.cols.size(); i++) {
         out.col_side[i] = 0;
         for (size_t k = 0; k < out.dims.size(); k++) if (out.cols[i].tuple_id == out.dims[k].tuple_id) out.col_side[i] = 1 + (int)k;
     }
-    // the aggregate over the gathered chunk: every column as a column of ONE (virtual, joined) tuple
-    auto jf = std::make_shared<Compiled>();
-    jf->tuples = out.tuples; jf->build_tuple = -1; jf->in_sets = out.in_sets;
-    Infer in2{}; in2.tuples = &jf->tuples;
-    if (!lower_agg(in2, *jf, agg, conj, fact, under_packet, true) || memcmp(&jf->ap.n_keyw, &out.ap.n_keyw, sizeof(int32_t) * 4) != 0 || jf->ap.n_lanes != out.ap.n_lanes)
-        return in.fail(BKGPU_EUNSUPPORTED, "the aggregate over the joined row could not be lowered: %s", in2.err.c_str());
-    for (auto& c : jf->cols) {
-        int m = -1;
-        for (size_t i = 0; i < out.cols.size(); i++) if (out.cols[i].tuple_id == c.tuple_id && out.cols[i].slot_id == c.slot_id) m = (int)i;
-        if (m < 0) return in.fail(BKGPU_EINVAL, "column %d_%d of the joined row is not a plan column", c.tuple_id, c.slot_id);
-        out.jfast_of_main.push_back(m);
-    }
-    out.jfast = jf;
+    // the aggregate runs over the gathered chunk
+    std::string why; ColRef missing;
+    const int r = lower_joined_row_agg(out, agg, conj, fact, under_packet, why, missing);
+    if (r == 0) return in.fail(BKGPU_EUNSUPPORTED, "the aggregate over the joined row could not be lowered: %s", why.c_str());
+    if (r < 0) return in.fail(BKGPU_EINVAL, "column %d_%d of the joined row is not a plan column", missing.tuple_id, missing.slot_id);
     return true;
 }
 
@@ -1736,21 +1650,14 @@ bool lower_star_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& joi
 // preserved, unmatched rows come out NULL-extended; the inner child's filter is its own program (as in lower_join_agg), a filter on the
 // preserved child or above the join is refused.  FULL: both sides
 // are preserved; a filter above the join is the sink's predicate, so it also judges the NULL-extended rows.
-bool lower_join_rows(Infer& in, Compiled& out, const HNode& join, const HNode* above, const HNode* sort, const HNode* limit_node) {
+static bool lower_join_rows(Infer& in, Compiled& out, const HNode& join, const HNode* above, const HNode* sort, const HNode* limit_node) {
     int jt = join.join_type;
     if (jt != BK_INNER_JOIN && jt != BK_LEFT_JOIN && jt != BK_RIGHT_JOIN && jt != BK_FULL_JOIN)
         return in.fail(BKGPU_EUNSUPPORTED, "a join of type %d that returns rows is outside the GPU path (INNER / LEFT / RIGHT / FULL are lowered)", jt);
     if (join.ch.size() != 2) return in.fail(BKGPU_EINVAL, "JOIN node needs two children");
     if (above && above->limit != -1) return in.fail(BKGPU_EUNSUPPORTED, "LIMIT on a filter above a join: use a LIMIT node");
-    const HNode* side[2]; const HNode* filt[2] = {nullptr, nullptr};
-    for (int i = 0; i < 2; i++) {
-        const HNode* c = skip_passthrough(&join.ch[(size_t)(jt == BK_RIGHT_JOIN ? 1 - i : i)], nullptr);
-        if (is_filter(c)) { filt[i] = c; c = c->ch.empty() ? nullptr : skip_passthrough(&c->ch[0], nullptr); }
-        if (!c || c->node_type != BK_SCAN_NODE) return in.fail(BKGPU_EUNSUPPORTED, "JOIN children must be [FILTER ->] SCAN");
-        if (filt[i] && filt[i]->limit != -1) return in.fail(BKGPU_EUNSUPPORTED, "LIMIT below a join is order dependent");
-        side[i] = c;
-    }
-    if (jt == BK_RIGHT_JOIN) jt = BK_LEFT_JOIN;
+    const HNode *side[2], *filt[2];
+    if (!join_children(in, join, jt, side, filt)) return false;
     const bool full = jt == BK_FULL_JOIN;
     if (full && (filt[0] || filt[1])) return in.fail(BKGPU_EUNSUPPORTED, "FULL join over filtered children is outside the GPU path");
     if (jt == BK_LEFT_JOIN && above) return in.fail(BKGPU_EUNSUPPORTED, "LEFT join with a filter above it is outside the GPU path");
@@ -1758,100 +1665,33 @@ bool lower_join_rows(Infer& in, Compiled& out, const HNode& join, const HNode* a
     const int build_tuple = side[0]->tuple_id, probe_tuple = side[1]->tuple_id;
     out.kind = PK_JOIN; out.build_tuple = build_tuple; out.scan_tuple = probe_tuple; out.join_type = jt;
     std::vector<const HExpr*> conj;
-    const HExpr *bk = nullptr, *pk = nullptr;
-    for (auto& e : join.conjuncts) {
-        bool taken = false;
-        if (!bk && e.node_type == BK_FUNCTION_CALL && e.fn_op == BK_FT_EQ && e.ch.size() == 2 && e.ch[0].node_type == BK_SLOT_REF && e.ch[1].node_type == BK_SLOT_REF) {
-            const HExpr *a = &e.ch[0], *b = &e.ch[1];
-            if (a->tuple_id == build_tuple && b->tuple_id == probe_tuple) { bk = a; pk = b; taken = true; }
-            else if (b->tuple_id == build_tuple && a->tuple_id == probe_tuple) { bk = b; pk = a; taken = true; }
-        }
-        if (!taken) conj.push_back(&e);
-    }
-    if (!bk) return in.fail(BKGPU_EUNSUPPORTED, "join without an equality between the two tables (nested loop) is outside the GPU path");
+    const HExpr *bk, *pk;
+    if (!join_equality(in, join, build_tuple, probe_tuple, bk, pk, conj)) return false;
     if (jt == BK_INNER_JOIN) for (int i = 0; i < 2; i++) if (filt[i]) for (auto& e : filt[i]->conjuncts) conj.push_back(&e);
     if (above && !full) for (auto& e : above->conjuncts) conj.push_back(&e);   // (FULL: the sink's predicate, below)
-    int ot = bk->col_type, it = pk->col_type, cast;
-    auto is_signed_t = [](int t) { return t >= BK_INT8 && t <= BK_INT64; };
-    if (ot == it) cast = ot;
-    else if (is_signed_t(ot) && is_signed_t(it)) cast = BK_INT64;
-    else if (is_uint_t(ot) && is_uint_t(it)) cast = BK_UINT64;
-    else return in.fail(BKGPU_EUNSUPPORTED, "join keys of types %d and %d are compared as STRING in the reference: outside the GPU path", ot, it);
-    if (cast == BK_STRING || is_double_t(cast)) return in.fail(BKGPU_EUNSUPPORTED, "join key type %d is outside the GPU path", cast);
-    out.join_key_prim = cast;
+    if (!join_key_cast(in, bk->col_type, pk->col_type, out.join_key_prim)) return false;
     Program& p = out.prog; memset(&p, 0, sizeof p);
     memset(&out.ap, 0, sizeof out.ap);
-    Lower lw{&out, &in, &p, {}};
+    Lower lw{&out, &in, &p};
     // every slot of both tuples is an output column (and a device column): build tuple first, as the joined row lists them
-    for (int sd = 0; sd < 2; sd++) {
-        const int tid = sd == 0 ? build_tuple : probe_tuple;
-        const HTuple* t = nullptr;
-        for (auto& x : out.tuples) if (x.tuple_id == tid) t = &x;
-        if (!t || t->slots.empty()) return in.fail(BKGPU_EINVAL, "join tuple %d has no descriptor", tid);
-        for (auto& sl : t->slots) {
-            if (prim_storage(sl.second) < 0 || sl.second == BK_STRING) return in.fail(BKGPU_EUNSUPPORTED, "column %d_%d has type %d: outside the GPU path", tid, sl.first, sl.second);
-            if (lw.intern_col(tid, sl.first, sl.second) >= MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d columns in the joined row", MAX_COLS);
-            out.out_cols.push_back({tid, sl.first, sl.second, 0});
-        }
-    }
+    if (!intern_tuple(in, out, lw, build_tuple, "join tuple", "the joined row") || !intern_tuple(in, out, lw, probe_tuple, "join tuple", "the joined row")) return false;
     const size_t n_payload = out.cols.size();
     out.build_key_col = lw.intern_col(bk->tuple_id, bk->slot_id, in.slot_type(bk->tuple_id, bk->slot_id));
     out.probe_key_col = lw.intern_col(pk->tuple_id, pk->slot_id, in.slot_type(pk->tuple_id, pk->slot_id));
     int reg = 0;
     out.ap.pred_out = -1;
     if (!conj.empty()) {
-        if (conj.size() > 8) return in.fail(BKGPU_EUNSUPPORTED, "more than 8 conjuncts");
-        for (auto* c : conj) { int depth = 0; if (!lw.expr(*c, depth) || !lw.to_bool(*c)) return false; }
-        if (conj.size() > 1 && !lw.emit(OP_AND, (uint8_t)conj.size())) return false;
         out.ap.pred_out = reg;
-        if (!lw.out_reg(reg++)) return false;
+        if (!lw.predicate(conj, reg++)) return false;
     }
     p.n_out = reg;
     if (jt == BK_LEFT_JOIN && !lower_child_filter(in, out, filt[1], probe_tuple, out.probe_filter, out.n_probe_filter)) return false;
     if (out.cols.size() != n_payload) return in.fail(BKGPU_EINVAL, "join conditions reference a slot that is in neither tuple descriptor");
-    // the sink over the joined rows
-    auto post = std::make_shared<Compiled>();
-    Compiled& pc = *post;
-    pc.kind = sort ? PK_SORT : PK_FILTER;
-    pc.tuples = out.tuples; pc.scan_tuple = -1; pc.in_sets = out.in_sets;
-    Program& pp = pc.prog; memset(&pp, 0, sizeof pp);
-    memset(&pc.ap, 0, sizeof pc.ap);
-    pc.ap.pred_out = -1;
-    Infer in2{}; in2.tuples = &pc.tuples;
-    Lower lw2{&pc, &in2, &pp, {}};
-    for (const OutCol& oc : out.out_cols) { lw2.intern_col(oc.tuple_id, oc.slot_id, oc.prim); pc.out_cols.push_back(oc); }
-    int preg = 0;
-    // FULL: the filter above the join judges every joined row, the NULL-extended ones included, after the match decision
-    if (full && !lower_predicate(in2, lw2, above, pc.ap, preg)) { in.code = in2.code; in.err = in2.err; return false; }
-    if (sort) {
-        pc.limit = sort->limit;
-        if (sort->order_exprs.empty()) return in.fail(BKGPU_EINVAL, "SORT node without order expressions");
-        if (sort->order_exprs.size() > 4) return in.fail(BKGPU_EUNSUPPORTED, "more than 4 ORDER BY expressions");
-        for (size_t i = 0; i < sort->order_exprs.size(); i++) {
-            const HExpr& e = sort->order_exprs[i];
-            if (e.col_type == BK_STRING) return in.fail(BKGPU_EUNSUPPORTED, "ORDER BY over a STRING key is outside the GPU path");
-            int depth = 0;
-            if (!lw2.expr(e, depth)) { in.code = in2.code; in.err = in2.err; return false; }
-            pc.sort_keys.push_back({preg, e.col_type, sort->is_asc[i] != 0, sort->is_null_first[i] != 0});
-            if (!lw2.out_reg(preg++)) return false;
-        }
-        if (limit_node) {
-            pc.offset = limit_node->offset;
-            if (limit_node->limit >= 0) { const int64_t lim = limit_node->limit + limit_node->offset; if (pc.limit < 0 || lim < pc.limit) pc.limit = lim; }
-        }
-    } else {
-        pc.limit = join.limit; pc.offset = 0;
-        if (limit_node) {
-            pc.offset = limit_node->offset;
-            const int64_t lim = limit_node->limit < 0 ? -1 : limit_node->limit + limit_node->offset;
-            if (lim >= 0 && (pc.limit < 0 || lim < pc.limit)) pc.limit = lim;
-        }
-    }
-    pp.n_out = preg;
-    if (pc.cols.size() != out.out_cols.size()) return in.fail(BKGPU_EUNSUPPORTED, "ORDER BY above a join references a column outside the joined row");
-    pc.has_direct = false;
-    out.post = post;
-    out.limit = pc.limit; out.offset = pc.offset;
+    // the sink over the joined rows.  FULL: the filter above the join judges every joined row, the NULL-extended ones included, after the
+    // match decision
+    if (!lower_sink(in, out, {sort, full ? above : nullptr, join.limit, false, "columns in the joined row under a sink",
+                              "ORDER BY above a join references a column outside the joined row"}, limit_node)) return false;
+    out.limit = out.post->limit; out.offset = out.post->offset;
     return true;
 }
 
@@ -1880,7 +1720,7 @@ std::string sort_key_text(const HNode& s) {
 }
 }  // namespace
 
-bool lower_window(Infer& in, Compiled& out, const HNode& wtop, const HNode* outer_sort, const HNode* limit_node) {
+static bool lower_window(Infer& in, Compiled& out, const HNode& wtop, const HNode* outer_sort, const HNode* limit_node) {
     out.kind = PK_WINDOW;
     std::vector<std::pair<const HNode*, const HNode*>> pairs;   // (WINDOW, SORT), top-down
     const HNode* t = &wtop;
@@ -1898,26 +1738,20 @@ bool lower_window(Infer& in, Compiled& out, const HNode& wtop, const HNode* oute
     out.scan_tuple = t->tuple_id;
     Program& p = out.prog; memset(&p, 0, sizeof p);
     memset(&out.ap, 0, sizeof out.ap);
-    Lower lw{&out, &in, &p, {}};
-    if (!intern_scan_tuple(in, out, lw, t->tuple_id)) return false;
+    Lower lw{&out, &in, &p};
+    if (!intern_tuple(in, out, lw, t->tuple_id, "scan tuple", "the scan tuple")) return false;
     const size_t n_scan_cols = out.cols.size();
     int reg = 0;
-    if (!lower_predicate(in, lw, filter, out.ap, reg)) return false;
+    if (!lower_predicate(lw, filter, out.ap, reg)) return false;
     p.n_out = reg;
     // one device program per distinct (expression, result type) of a stage
     auto intern_expr = [&](WinStage& st, std::map<std::string, int>& seen, const HExpr& e, int to) -> int {
         const std::string key = expr_key(e) + ":" + std::to_string(to);
         auto it = seen.find(key);
         if (it != seen.end()) return it->second;
-        Program q; memset(&q, 0, sizeof q);
-        const int save = out.n_const; out.n_const = 0;
-        Lower l2{&out, &in, &q, {}};
-        int depth = 0;
-        const bool ok = l2.expr(e, depth) && l2.cast(e.col_type, to) && l2.out_reg(0);
-        out.n_const = save;
-        if (!ok) return -1;
+        Program q;
+        if (!lower_own_program(in, out, q, [&](Lower& l) { int depth = 0; return l.expr(e, depth) && l.cast(e.col_type, to) && l.out_reg(0); })) return -1;
         if (out.cols.size() != n_scan_cols) { in.fail(BKGPU_EUNSUPPORTED, "a window expression reads a column outside the scan tuple %d", out.scan_tuple); return -1; }
-        q.n_out = 1;
         st.exprs.push_back(q); st.expr_prim.push_back(to);
         return seen[key] = (int)st.exprs.size() - 1;
     };
@@ -2033,15 +1867,104 @@ bool lower_window(Infer& in, Compiled& out, const HNode& wtop, const HNode* oute
         out.out_cols.push_back(oc);
     }
     out.limit = -1; out.offset = 0;
-    if (outer_sort) {   // the query's ORDER BY over the window rows (window columns included) [+ LIMIT / OFFSET]
-        if (out.out_cols.size() > (size_t)MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d window output columns under an ORDER BY", MAX_COLS);
-        return lower_post(in, out, outer_sort, nullptr, limit_node);
-    }
-    if (limit_node) {   // LIMIT / OFFSET over the top stage's order
-        out.offset = limit_node->offset;
-        out.limit = limit_node->limit < 0 ? -1 : limit_node->limit + limit_node->offset;
-    }
+    if (outer_sort)   // the query's ORDER BY over the window rows (window columns included) [+ LIMIT / OFFSET]
+        return lower_sink(in, out, {outer_sort, nullptr, -1, true, "window output columns under an ORDER BY",
+                                    "SORT / HAVING above an aggregate references a column the aggregate does not output"}, limit_node);
+    merge_limit(limit_node, out.limit, out.offset);   // LIMIT / OFFSET over the top stage's order
     return true;
+}
+
+// ---------------------------------------------------------------- entry
+// [SORT ->] [FILTER ->] JOIN at the top of the fragment -> the JOIN node, else nullptr
+static const HNode* join_rows_shape(const HNode* t) {
+    if (t && t->node_type == BK_SORT_NODE && !t->ch.empty()) t = skip_passthrough(&t->ch[0], nullptr);
+    if (t && is_filter(t) && !t->ch.empty()) t = skip_passthrough(&t->ch[0], nullptr);
+    return t && t->node_type == BK_JOIN_NODE ? t : nullptr;
+}
+
+int compile_plan(const uint8_t* desc, size_t len, Compiled& out, std::string& err) {
+    if (!desc || len < 16 || (len & 3)) { err = "plan descriptor is empty or not a multiple of 4 bytes"; return BKGPU_EINVAL; }
+    Reader r{}; r.w = (const int32_t*)desc; r.n = len / 4;
+    if ((uint32_t)r.rd() != BKGPU_PLAN_MAGIC) { err = "bad plan magic"; return BKGPU_EINVAL; }
+    if (r.rd() != BKGPU_PLAN_VERSION) { err = "unsupported plan version"; return BKGPU_EINVAL; }
+    int nt = r.rd(), nn = r.rd();
+    if (nt < 0 || nt > 16 || nn <= 0 || nn > 64) { err = "bad tuple / node count"; return BKGPU_EINVAL; }
+    for (int i = 0; i < nt && !r.fail; i++) {
+        HTuple t; t.tuple_id = r.rd(); int ns = r.rd();
+        if (ns < 0 || ns > 4096) { r.bad("bad slot count"); break; }
+        for (int k = 0; k < ns; k++) { int sid = r.rd(); int pt = r.rd(); t.slots.push_back({sid, pt}); }
+        out.tuples.push_back(t);
+    }
+    HNode root;
+    if (!r.fail) parse_node(r, root, nn, 0);
+    if (!r.fail && nn != 0) r.bad("plan node count mismatch");
+    if (!r.fail && r.pos != r.n) r.bad("trailing words after the plan");
+    if (r.fail) { err = r.err; return r.err.find("outside the GPU path") != std::string::npos ? BKGPU_EUNSUPPORTED : BKGPU_EINVAL; }
+    Infer in{}; in.tuples = &out.tuples;
+    if (!infer_node(in, root)) { err = in.err; return in.code; }
+    out.in_sets = std::make_shared<InSets>();
+
+    bool under_packet = false;
+    const HNode* top = skip_passthrough(&root, &under_packet);
+    if (!top) { err = "empty plan"; return BKGPU_EINVAL; }
+    bool ok = false;
+    const HNode* limit_node = nullptr;
+    if (top->node_type == BK_LIMIT_NODE && !top->ch.empty()) { limit_node = top; top = skip_passthrough(&top->ch[0], &under_packet); }
+    // the db-side chain above an aggregate: [LIMIT ->] [SORT ->] [HAVING_FILTER ->] (MERGE_)AGG (separate.cpp:241-260): the operators
+    // above the aggregate become a post fragment over the aggregate's output rows
+    const HNode *post_sort = nullptr, *post_having = nullptr;
+    {
+        const HNode* t = top;
+        const HNode *ps = nullptr, *ph = nullptr;
+        if (t->node_type == BK_SORT_NODE && !t->ch.empty()) { ps = t; t = skip_passthrough(&t->ch[0], nullptr); }
+        if (t && (is_filter(t) || t->node_type == BK_HAVING_FILTER_NODE) && !t->ch.empty()) { ph = t; t = skip_passthrough(&t->ch[0], nullptr); }
+        if (t && (ps || ph) && (t->node_type == BK_AGG_NODE || t->node_type == BK_MERGE_AGG_NODE)) { post_sort = ps; post_having = ph; top = t; }
+    }
+    const HNode* win_sort = nullptr;   // [SORT ->] WINDOW: the query's ORDER BY above the window stages
+    if (top->node_type == BK_SORT_NODE && !top->ch.empty()) {
+        const HNode* c = skip_passthrough(&top->ch[0], nullptr);
+        if (c && c->node_type == BK_WINDOW_NODE) win_sort = top;
+    }
+    if (win_sort || top->node_type == BK_WINDOW_NODE) {
+        ok = lower_window(in, out, win_sort ? *skip_passthrough(&win_sort->ch[0], nullptr) : *top, win_sort, limit_node);
+    } else if (top->node_type == BK_AGG_NODE || top->node_type == BK_MERGE_AGG_NODE) {
+        if (top->ch.empty()) { err = "AGG node without a child"; return BKGPU_EINVAL; }
+        const HNode* c = skip_passthrough(&top->ch[0], nullptr);
+        const HNode* filter = nullptr;
+        if (is_filter(c)) { filter = c; c = c->ch.empty() ? nullptr : skip_passthrough(&c->ch[0], nullptr); }
+        if (!c || (c->node_type != BK_SCAN_NODE && c->node_type != BK_JOIN_NODE)) { err = "AGG child must be [FILTER ->] SCAN or JOIN"; return BKGPU_EUNSUPPORTED; }
+        if (filter && filter->limit != -1) { err = "LIMIT on a filter below an aggregate is order dependent: outside the GPU path"; return BKGPU_EUNSUPPORTED; }
+        if (c->node_type == BK_SCAN_NODE) ok = lower_agg(in, out, *top, conjuncts_of(filter), c->tuple_id, under_packet, true);
+        // AGG -> [FILTER ->] JOIN: the store-side chain of a filtered join (separate.cpp:241-260)
+        else ok = join_leaves(c) > 2 ? lower_star_agg(in, out, *top, *c, under_packet, filter) : lower_join_agg(in, out, *top, *c, under_packet, filter);
+        // LimitNode straight over the aggregate: the result extraction (agg_result) skips `offset` groups and then keeps `limit` of them,
+        // so the limit is stored as it is — not as the first limit + offset rows that a sort or a filter keeps before skipping
+        if (ok && limit_node && !post_sort && !post_having) { out.limit = limit_node->limit; out.offset = limit_node->offset; }
+        if (ok && (post_sort || post_having))
+            ok = lower_sink(in, out, {post_sort, post_having, post_having ? post_having->limit : -1, true, "aggregate output columns under a SORT / HAVING",
+                                      "SORT / HAVING above an aggregate references a column the aggregate does not output"}, limit_node);
+    } else if (const HNode* jn = join_rows_shape(top)) {   // [SORT ->] [FILTER ->] JOIN: a join that returns its rows
+        const HNode* t = top; const HNode *js = nullptr, *jf = nullptr;
+        if (t->node_type == BK_SORT_NODE) { js = t; t = skip_passthrough(&t->ch[0], nullptr); }
+        if (is_filter(t)) jf = t;
+        if (join_leaves(jn) > 2) { err = "a join of more than two tables that returns rows is outside the GPU path (an aggregate over a star join is lowered)"; return BKGPU_EUNSUPPORTED; }
+        ok = lower_join_rows(in, out, *jn, jf, js, limit_node);
+    } else if (top->node_type == BK_SORT_NODE) {
+        const HNode* c = top->ch.empty() ? nullptr : skip_passthrough(&top->ch[0], nullptr);
+        const HNode* filter = nullptr;
+        if (is_filter(c)) { filter = c; c = c->ch.empty() ? nullptr : skip_passthrough(&c->ch[0], nullptr); }
+        if (!c || c->node_type != BK_SCAN_NODE) { err = "SORT child must be [FILTER ->] SCAN"; return BKGPU_EUNSUPPORTED; }
+        ok = lower_sort(in, out, *top, filter, *c);
+        if (ok) merge_limit(limit_node, out.limit, out.offset);
+    } else if (is_filter(top) || top->node_type == BK_SCAN_NODE) {
+        const HNode* c = top;
+        if (is_filter(c)) c = c->ch.empty() ? nullptr : skip_passthrough(&c->ch[0], nullptr);
+        if (!c || c->node_type != BK_SCAN_NODE) { err = "FILTER child must be SCAN"; return BKGPU_EUNSUPPORTED; }
+        ok = lower_filter(in, out, limit_node, *top, *c);
+    } else { err = "plan root is outside the GPU path"; return BKGPU_EUNSUPPORTED; }
+    if (!ok) { err = in.err.empty() ? "plan could not be lowered" : in.err; return in.code ? in.code : BKGPU_EUNSUPPORTED; }
+    explain(out);
+    return BKGPU_OK;
 }
 
 }  // namespace bk

@@ -69,7 +69,7 @@ struct StarDim {
     int key_col = -1, fk_col = -1;     // indices into Compiled::cols: the dimension's key, the fact tuple's foreign key
     int cast_prim = 0;                 // type both keys are compared in (strip_out_equal_slots' cast, joiner.cpp:166-217)
     int n_filter = 0;                  // conjuncts that read this dimension alone: evaluated once over its rows at build time
-    Program filter;                    // output 0 = their conjunction (column indices into Compiled::cols)
+    Program filter{};                  // output 0 = their conjunction (column indices into Compiled::cols)
 };
 
 // window functions (WindowFnCall::init's name table, window_fn_call.cpp:20-38)
@@ -124,7 +124,6 @@ struct Compiled {
     std::vector<ColRef> cols;          // columns the device program references (index = DevCol index)
     std::vector<int> col_side;         // per column: 0 = probe / only scan tuple, 1 = build side of a join; star join: 0 = fact, 1 + d = dims[d]
     Program prog;                      // outputs: [predicate][keys...][agg args...] / sort keys
-    int n_const = 0;
     // aggregate
     AggPlan ap;
     bool is_merge = false, emit_default = false;
