@@ -30,6 +30,7 @@ class PlanNodeType(IntEnum):  # proto/plan.proto:9-53
     HAVING_FILTER_NODE = 13
     PACKET_NODE = 14
     SELECT_MANAGER_NODE = 25
+    APPLY_NODE = 37
     WINDOW_NODE = 42
 
 
@@ -120,6 +121,13 @@ class JoinType(IntEnum):  # proto/plan.proto:218-226
     SEMI_JOIN = 4
     ANTI_SEMI_JOIN = 5
     FULL_JOIN = 6
+
+
+class CompareType(IntEnum):  # proto/plan.proto:239-244 (ApplyNode.compare_type)
+    CMP_NULL = 0
+    CMP_ANY = 1
+    CMP_ALL = 2
+    CMP_SOME = 3
 
 
 class FrameType(IntEnum):  # proto/plan.proto:427-430
@@ -410,6 +418,9 @@ class PlanNode:
     window_fns: List[Expr] = field(default_factory=list)
     partition_exprs: List[Expr] = field(default_factory=list)
     frame: Optional[WindowFrame] = None
+    max_one_row: bool = False        # APPLY_NODE (its conditions are `conjuncts`)
+    compare_type: int = CompareType.CMP_NULL
+    is_select_field: bool = False
 
     def count(self) -> int:
         return 1 + sum(c.count() for c in self.children)
@@ -446,6 +457,14 @@ class PlanNode:
             out.w(len(self.conjuncts))
             for e in self.conjuncts:
                 e.emit(out)
+        elif nt == PlanNodeType.APPLY_NODE:
+            out.w(self.join_type)
+            out.w(len(self.conjuncts))
+            for e in self.conjuncts:
+                e.emit(out)
+            out.w(1 if self.max_one_row else 0)
+            out.w(self.compare_type)
+            out.w(1 if self.is_select_field else 0)
         elif nt == PlanNodeType.LIMIT_NODE:
             out.w64(self.offset)
         elif nt in (PlanNodeType.PACKET_NODE, PlanNodeType.SELECT_MANAGER_NODE):
@@ -503,6 +522,15 @@ def join(outer: PlanNode, inner: PlanNode, conditions: Sequence[Expr],
          join_type: int = JoinType.INNER_JOIN, limit: int = -1) -> PlanNode:
     return PlanNode(PlanNodeType.JOIN_NODE, [outer, inner], conjuncts=list(conditions), join_type=int(join_type),
                     limit=limit)
+
+
+def apply(outer: PlanNode, inner: PlanNode, conditions: Sequence[Expr], join_type: int, max_one_row: bool = False,
+          compare_type: int = CompareType.CMP_NULL, is_select_field: bool = False) -> PlanNode:
+    """APPLY_NODE (a subquery the planner did not turn into a join, logical_planner.cpp construct_apply_node): `outer` is the outer query's
+    child, `inner` the subquery's; `conditions` are the outer WHERE conjunct that holds the subquery (``x = <subquery column>`` for IN), while
+    the correlated conjuncts stay in the subquery's own filters.  EXISTS / IN: SEMI_JOIN; NOT EXISTS / NOT IN: ANTI_SEMI_JOIN."""
+    return PlanNode(PlanNodeType.APPLY_NODE, [outer, inner], conjuncts=list(conditions), join_type=int(join_type), max_one_row=bool(max_one_row),
+                    compare_type=int(compare_type), is_select_field=bool(is_select_field))
 
 
 def limit(child: PlanNode, n: int, offset: int = 0) -> PlanNode:

@@ -3,7 +3,7 @@
 device-resident synthetic columns (SURVEY.md §8d), CUDA events around reset+push+finish+get_next, one JSON line per
 config with rows/s and achieved GB/s on the config's algorithmic bytes.  The headline line is bench.py's;
 this script measures the side configs on their own (C6, the star join, also its kernels, a parity flag and the Acero time).
-usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [c9] [c10] [c11] [--scale 0.1] [--steps 10]"""
+usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [c9] [c10] [c11] [c12] [--scale 0.1] [--steps 10]"""
 import argparse
 import ctypes
 import json
@@ -535,6 +535,83 @@ def c11(a):
         print(json.dumps(line), flush=True)
 
 
+def c12(a):
+    """C12, TPC-H Q4's shape as a correlated subquery (APPLY): `SELECT o_orderpriority, COUNT(*) FROM orders WHERE o_orderdate in a 92-day range
+    AND EXISTS (SELECT * FROM lineitem WHERE l_orderkey = o_orderkey AND l_commitdate < l_receiptdate) GROUP BY o_orderpriority ORDER BY
+    o_orderpriority` over 15M device-resident orders (the outer, build side; about 3.8 % pass the date range) and 60M lineitem rows (the
+    subquery, probe side; about half pass commit < receipt), TPC-H SF10's row counts.  The APPLY runs as the decorrelated SEMI join.  Reported:
+    the step, the same step for the query written as that join, the kernel times of one profiled run (both children's filters, the multimap
+    build, the probe, the tail), parity of every group against torch on the same tensors, and Acero's filter -> semi hashjoin -> aggregate
+    on the host CPUs."""
+    import subprocess
+    import time
+    from baikaldb_b200 import plan as P
+    from torch.profiler import ProfilerActivity, profile
+    no, nl = int(15_000_000 * a.scale), int(60_000_000 * a.scale)
+    g = torch.Generator(device="cuda").manual_seed(12)
+    okey = torch.randperm(no, device="cuda", generator=g).to(torch.int32)
+    odate = torch.randint(0, 2_406, (no,), device="cuda", generator=g, dtype=torch.int32)   # days since 1992-01-01
+    prio = torch.randint(1, 6, (no,), device="cuda", generator=g, dtype=torch.int32)
+    lkey = torch.randint(0, no, (nl,), device="cuda", generator=g, dtype=torch.int32)       # about 4 lineitem rows per order
+    commit = torch.randint(0, 120, (nl,), device="cuda", generator=g, dtype=torch.int32)
+    receipt = torch.randint(0, 120, (nl,), device="cuda", generator=g, dtype=torch.int32)
+    tup = {1: [(1, T.INT32), (2, T.INT32), (3, T.INT32)], 0: [(1, T.INT32), (2, T.INT32), (3, T.INT32)]}
+    oarr, larr = cols_array([(1, 1, T.INT32), (1, 2, T.INT32), (1, 3, T.INT32)], [okey, odate, prio]), cols_array([(0, 1, T.INT32), (0, 2, T.INT32), (0, 3, T.INT32)], [lkey, commit, receipt])
+    pushes = [(oarr, 3, no), (larr, 3, nl)]
+    lo, hi = 1_300, 1_392
+    s = lambda t, k: P.slot_ref(t, k, T.INT32)
+    aggs = [P.agg_expr("count_star", 2, 1)]
+    orders = P.where(P.scan(1), P.ge(s(1, 2), P.int_lit(lo)), P.lt(s(1, 2), P.int_lit(hi)))
+
+    def q4(sub_root):
+        return P.Plan(P.sort(P.agg(sub_root, 2, [s(1, 3)], aggs), [s(1, 3)], [True], tuple_id=2), {**tup, 2: P.agg_tuple_slots(aggs, [T.INT64])})
+    apply_plan = q4(P.apply(orders, P.where(P.scan(0), P.eq(s(0, 1), s(1, 1)), P.lt(s(0, 2), s(0, 3))), [], P.JoinType.SEMI_JOIN))
+    join_plan = q4(P.join(orders, P.where(P.scan(0), P.lt(s(0, 2), s(0, 3))), [P.eq(s(1, 1), s(0, 1))], join_type=P.JoinType.SEMI_JOIN))
+    hit = torch.zeros(no, dtype=torch.bool, device="cuda")
+    hit[lkey[commit < receipt].long()] = True
+    emit = (odate >= lo) & (odate < hi) & hit[okey.long()]
+    want = torch.bincount(prio[emit].long(), minlength=6).cpu().numpy()
+    want_groups = [k for k in range(6) if want[k] > 0]
+    steps = max(1, a.steps // 3)
+    opts = [(b"group_capacity_log2", 14)]
+    line, got = run("C12 TPC-H Q4 shape: orders (date range) WHERE EXISTS (lineitem ON key AND commit < receipt) as APPLY, GROUP BY priority "
+                    "ORDER BY priority (15M orders x 60M lineitem)", apply_plan, pushes, nl, 12 * nl + 12 * no, steps, 1, options=opts, collect=True, emit=False)
+    r = line["result_rows"]
+    line["parity_vs_torch_all_groups"] = bool(got.get("1_3", [])[:r] == want_groups and got["2_1"][:r] == [int(want[k]) for k in want_groups])
+    line["decorrelated_join_ms_per_step"] = run("join", join_plan, pushes, nl, 0, steps, 1, options=opts, emit=False)["ms_per_step"]
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        run("profile", apply_plan, pushes, nl, 0, steps, 1, options=opts, emit=False)
+        torch.cuda.synchronize()
+    per = lambda us: us / 1e3 / (steps + 1)   # (the profiled run: 1 warm-up + steps)
+    ka = prof.key_averages()
+    dev = lambda e: getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0))
+    line["filters_ms_per_step (k_star_dim_filter over both children)"] = per(sum(dev(e) for e in ka if "k_star_dim_filter" in e.key))
+    line["multimap_build_ms_per_step (k_join_build)"] = per(sum(dev(e) for e in ka if "k_join_build(" in e.key))
+    interp = sorted((e for e in prof.events() if "k_agg_interp" in e.name and dev(e) > 0), key=lambda e: e.time_range.start)
+    k = len(interp) // (steps + 1)
+    tail = [e for i, e in enumerate(interp) if k and i % k == k - 1]
+    line["probe_ms_per_step (k_agg_interp over the lineitem rows)"] = per(sum(dev(e) for e in interp) - sum(dev(e) for e in tail))
+    line["tail_ms_per_step (k_agg_interp over the orders rows)"] = per(sum(dev(e) for e in tail))
+    import pyarrow as pa, pyarrow.acero as ac, pyarrow.compute as pc
+    ot = pa.table({"1_1": pa.array(okey.cpu().numpy()), "1_2": pa.array(odate.cpu().numpy()), "1_3": pa.array(prio.cpu().numpy())})
+    lt = pa.table({"0_1": pa.array(lkey.cpu().numpy()), "0_2": pa.array(commit.cpu().numpy()), "0_3": pa.array(receipt.cpu().numpy())})
+    src = lambda t: ac.Declaration("table_source", ac.TableSourceNodeOptions(t))
+    of = ac.Declaration("filter", ac.FilterNodeOptions((pc.field("1_2") >= lo) & (pc.field("1_2") < hi)), inputs=[src(ot)])
+    lf = ac.Declaration("filter", ac.FilterNodeOptions(pc.field("0_2") < pc.field("0_3")), inputs=[src(lt)])
+    hj = ac.Declaration("hashjoin", ac.HashJoinNodeOptions("left semi", ["1_1"], ["0_1"]), inputs=[of, lf])
+    agg = ac.Declaration("aggregate", ac.AggregateNodeOptions([([], "hash_count_all", None, "2_1")], keys=["1_3"]), inputs=[hj])
+    t0 = time.perf_counter(); at = agg.to_table(use_threads=True); line["acero_filter_semi_hashjoin_aggregate_host_s"] = time.perf_counter() - t0
+    ad = at.to_pydict()
+    line["acero_matches_torch"] = bool(sorted(zip(ad["1_3"], ad["2_1"])) == [(k, int(want[k])) for k in want_groups])
+    line["acero_host_cpus"] = os.cpu_count()
+    line["gpu"] = torch.cuda.get_device_name(0)
+    try:
+        line["power_limit"] = subprocess.check_output(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"], text=True).split("\n")[0].strip()
+    except Exception:
+        line["power_limit"] = None
+    print(json.dumps(line), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("configs", nargs="*", default=["c1", "c3", "c5"])
@@ -598,6 +675,8 @@ def main():
         c10(a)
     if "c11" in a.configs:
         c11(a)
+    if "c12" in a.configs:
+        c12(a)
     if "c3" in a.configs:
         nf, nd = int(100_000_000 * a.scale), int(10_000_000 * a.scale)
         fs = [(0, 1, T.INT32, 0, 1, 0, nd, 1.0), (0, 2, T.DOUBLE, 1, 2, 0, 0, 1.0)]

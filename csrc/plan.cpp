@@ -193,6 +193,10 @@ static void parse_node(Reader& r, HNode& nd, int& remaining, int depth) {
             }
         } break;
         case BK_JOIN_NODE: nd.join_type = r.rd(); exprs(nd.conjuncts); break;
+        case BK_APPLY_NODE:
+            nd.join_type = r.rd(); exprs(nd.conjuncts);
+            nd.max_one_row = r.rd() != 0; nd.compare_type = r.rd(); nd.is_select_field = r.rd() != 0;
+            break;
         case BK_LIMIT_NODE: nd.offset = r.rd64(); break;
         case BK_PACKET_NODE: case BK_SELECT_MANAGER_NODE: break;
         case BK_WINDOW_NODE: {   // pb::WindowNode: func_exprs, window_spec {partition_exprs, order_exprs, is_asc, window_frame}
@@ -1202,6 +1206,10 @@ static void explain(Compiled& c) {
         snprintf(buf, sizeof buf, "child filters: build tuple=%d conjuncts=%d (once over the retained rows: multimap key validity, failing rows never in the tail); "
                  "probe tuple=%d conjuncts=%d (per probe batch: probe key validity)\n", c.build_tuple, c.n_build_filter, c.scan_tuple, c.n_probe_filter); s += buf;
     }
+    if (c.apply_join_type) {
+        snprintf(buf, sizeof buf, "apply: %s decorrelated into the join above; conjuncts moved from the subquery into the join conditions=%d, "
+                 "folded from the filter above into the outer filter=%d\n", c.apply_join_type == BK_SEMI_JOIN ? "SEMI" : "ANTI_SEMI", c.apply_moved, c.apply_folded); s += buf;
+    }
     snprintf(buf, sizeof buf, "program: %d instr, %d outputs\n", c.prog.n_instr, c.prog.n_out); s += buf;
     for (int i = 0; i < c.prog.n_instr; i++) {
         const Instr& in = c.prog.code[i];
@@ -1643,6 +1651,88 @@ static bool lower_star_agg(Infer& in, Compiled& out, const HNode& agg, const HNo
     return true;
 }
 
+// ---- APPLY: a correlated EXISTS / NOT EXISTS / [NOT] IN subquery under an aggregate ----
+// [FILTER ->] APPLY(SEMI | ANTI_SEMI) with outer child [FILTER ->] SCAN and inner child (the subquery) [SORT ->] [FILTER ->]* SCAN.
+// The reference's ApplyNode (src/exec/apply_node.cpp) runs an APPLY whose conditions hold no outer = inner column equality as a nested loop:
+// for every outer row it puts the row's values in place of the outer columns inside the subquery and fetches the subquery's rows again
+// (nested_loop_apply, replace_slot_ref_to_literal, fetcher_inner_table_data).  SEMI emits the outer row once if some subquery row makes
+// every condition TRUE, ANTI_SEMI if none does (get_next_for_nested_loop_join); a NULL comparison is not TRUE.  Per outer row that is the
+// SEMI / ANTI_SEMI join of the outer child with the subquery's scan, ON the APPLY's conditions and every subquery conjunct that reads the
+// outer tuple (is_correlate_expr's classification), with the conjuncts that read the subquery alone as the inner child's own filter.  SEMI /
+// ANTI_SEMI emit outer rows unchanged, so the filter between the aggregate and the APPLY, which reads the outer tuple alone, is part of the
+// outer child's filter.  That JOIN is built here and lowered by lower_join_agg.
+// An APPLY whose own conditions hold an outer = inner column equality (a correlated IN) runs as hash_apply instead: the subquery is opened
+// once, with no outer row, so a correlated conjunct inside it reads the outer columns as NULL and no subquery row passes.  That is not the
+// per-row meaning, and such a plan is refused.
+static bool lower_apply_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& apply, bool under_packet, const HNode* above) {
+    const int jt = apply.join_type;
+    if (jt == BK_LEFT_JOIN) return in.fail(BKGPU_EUNSUPPORTED, "a LEFT apply (a scalar subquery) is outside the GPU path");
+    if (jt != BK_SEMI_JOIN && jt != BK_ANTI_SEMI_JOIN) return in.fail(BKGPU_EUNSUPPORTED, "an APPLY of join type %d is outside the GPU path (SEMI / ANTI_SEMI are lowered)", jt);
+    if (apply.max_one_row) return in.fail(BKGPU_EUNSUPPORTED, "an APPLY with max_one_row (a subquery that must return at most one row) is outside the GPU path");
+    if (apply.is_select_field) return in.fail(BKGPU_EUNSUPPORTED, "an APPLY of a subquery in the select list is outside the GPU path");
+    if (apply.compare_type != BK_CMP_NULL) return in.fail(BKGPU_EUNSUPPORTED, "an APPLY with an ANY / ALL / SOME comparison (compare_type %d) is outside the GPU path", apply.compare_type);
+    if (apply.ch.size() != 2) return in.fail(BKGPU_EINVAL, "APPLY node needs two children");
+    auto below = [](const HNode* n) { return n->ch.empty() ? nullptr : skip_passthrough(&n->ch[0], nullptr); };
+    const HNode* o = skip_passthrough(&apply.ch[0], nullptr);
+    const HNode* ofilt = nullptr;
+    if (is_filter(o)) { ofilt = o; o = below(o); }
+    if (o && o->node_type == BK_JOIN_NODE) return in.fail(BKGPU_EUNSUPPORTED, "an APPLY whose outer child is a join is outside the GPU path");
+    if (!o || o->node_type != BK_SCAN_NODE) return in.fail(BKGPU_EUNSUPPORTED, "the outer child of an APPLY must be [FILTER ->] SCAN");
+    if (ofilt && ofilt->limit != -1) return in.fail(BKGPU_EUNSUPPORTED, "LIMIT on a filter below an APPLY is order dependent: outside the GPU path");
+    const int ot = o->tuple_id;
+    // the subquery: a SORT does not change which rows exist; every filter's conjuncts are classified
+    std::vector<const HExpr*> own, moved;
+    const HNode* i = skip_passthrough(&apply.ch[1], nullptr);
+    if (i && i->node_type == BK_SORT_NODE && i->limit == -1) i = below(i);
+    for (; is_filter(i) && i->limit == -1; i = below(i))
+        for (auto& e : i->conjuncts) {
+            std::vector<int> ts; expr_tuples(e, ts);
+            (std::find(ts.begin(), ts.end(), ot) != ts.end() ? moved : own).push_back(&e);
+        }
+    if (i && (i->node_type == BK_AGG_NODE || i->node_type == BK_MERGE_AGG_NODE))
+        return in.fail(BKGPU_EUNSUPPORTED, "an aggregate inside the subquery of an APPLY is outside the GPU path");
+    if (i && (i->node_type == BK_LIMIT_NODE || i->limit != -1)) return in.fail(BKGPU_EUNSUPPORTED, "a LIMIT inside the subquery of an APPLY is outside the GPU path");
+    if (i && i->node_type == BK_JOIN_NODE) return in.fail(BKGPU_EUNSUPPORTED, "a join inside the subquery of an APPLY is outside the GPU path");
+    if (!i || i->node_type != BK_SCAN_NODE) return in.fail(BKGPU_EUNSUPPORTED, "the subquery of an APPLY must be [SORT ->] [FILTER ->]* SCAN");
+    const int it = i->tuple_id;
+    if (it == ot) return in.fail(BKGPU_EINVAL, "both children of an APPLY scan tuple %d", it);
+    auto key_eq = [&](const HExpr& e) {
+        return slot_eq(e) && ((e.ch[0].tuple_id == ot && e.ch[1].tuple_id == it) || (e.ch[0].tuple_id == it && e.ch[1].tuple_id == ot));
+    };
+    if (std::any_of(apply.conjuncts.begin(), apply.conjuncts.end(), key_eq) && !moved.empty())
+        return in.fail(BKGPU_EUNSUPPORTED, "a correlated IN subquery: the reference runs an APPLY whose conditions hold an outer = inner equality as hash_apply, "
+                       "which reads the outer columns of the subquery's %zu correlated conjuncts as NULL instead of per outer row: outside the GPU path", moved.size());
+    std::vector<const HExpr*> folded;
+    if (above)
+        for (auto& e : above->conjuncts) {
+            std::vector<int> ts; expr_tuples(e, ts);
+            for (int t : ts) if (t != ot) return in.fail(BKGPU_EINVAL, "the filter above an APPLY reads tuple %d: only the outer tuple %d reaches it", t, ot);
+            folded.push_back(&e);
+        }
+    std::vector<const HExpr*> conds = conjuncts_of(&apply);
+    conds.insert(conds.end(), moved.begin(), moved.end());
+    if (std::none_of(conds.begin(), conds.end(), [&](const HExpr* e) { return key_eq(*e); }))
+        return in.fail(BKGPU_EUNSUPPORTED, "an APPLY without an outer = inner column equality among its conditions and correlated conjuncts runs as the "
+                       "reference's nested loop: outside the GPU path");
+    // the decorrelated join: JOIN(outer [FILTER: own + folded] -> SCAN, inner [FILTER: own] -> SCAN) ON conditions + moved
+    auto child = [](const HNode& scan, std::vector<const HExpr*> conj) {
+        if (conj.empty()) return scan;
+        HNode f; f.node_type = BK_WHERE_FILTER_NODE;
+        for (auto* e : conj) f.conjuncts.push_back(*e);
+        f.ch.push_back(scan);
+        return f;
+    };
+    std::vector<const HExpr*> oconj = conjuncts_of(ofilt);
+    oconj.insert(oconj.end(), folded.begin(), folded.end());
+    HNode join; join.node_type = BK_JOIN_NODE; join.join_type = jt; join.limit = apply.limit;
+    for (auto* e : conds) join.conjuncts.push_back(*e);
+    join.ch.push_back(child(*o, oconj));
+    join.ch.push_back(child(*i, own));
+    if (!lower_join_agg(in, out, agg, join, under_packet, nullptr)) return false;
+    out.apply_join_type = jt; out.apply_moved = (int)moved.size(); out.apply_folded = (int)folded.size();
+    return true;
+}
+
 // A JOIN whose rows are the result ([LIMIT ->] [SORT ->] [FILTER ->] JOIN; JoinNode::get_next, join_node.cpp:1200-1326).  The joined rows that
 // pass the conditions are produced on the device batch by batch (pairs + one gather per column) and handed to a sink fragment
 // (Compiled::post, kind PK_FILTER without a predicate, or PK_SORT) whose "scan tuple" is the joined row: every slot of both tuples.
@@ -1875,11 +1965,11 @@ static bool lower_window(Infer& in, Compiled& out, const HNode& wtop, const HNod
 }
 
 // ---------------------------------------------------------------- entry
-// [SORT ->] [FILTER ->] JOIN at the top of the fragment -> the JOIN node, else nullptr
-static const HNode* join_rows_shape(const HNode* t) {
+// [SORT ->] [FILTER ->] JOIN / APPLY (`node_type`) at the top of the fragment -> that node, else nullptr
+static const HNode* rows_shape(const HNode* t, int node_type) {
     if (t && t->node_type == BK_SORT_NODE && !t->ch.empty()) t = skip_passthrough(&t->ch[0], nullptr);
     if (t && is_filter(t) && !t->ch.empty()) t = skip_passthrough(&t->ch[0], nullptr);
-    return t && t->node_type == BK_JOIN_NODE ? t : nullptr;
+    return t && t->node_type == node_type ? t : nullptr;
 }
 
 int compile_plan(const uint8_t* desc, size_t len, Compiled& out, std::string& err) {
@@ -1932,9 +2022,10 @@ int compile_plan(const uint8_t* desc, size_t len, Compiled& out, std::string& er
         const HNode* c = skip_passthrough(&top->ch[0], nullptr);
         const HNode* filter = nullptr;
         if (is_filter(c)) { filter = c; c = c->ch.empty() ? nullptr : skip_passthrough(&c->ch[0], nullptr); }
-        if (!c || (c->node_type != BK_SCAN_NODE && c->node_type != BK_JOIN_NODE)) { err = "AGG child must be [FILTER ->] SCAN or JOIN"; return BKGPU_EUNSUPPORTED; }
+        if (!c || (c->node_type != BK_SCAN_NODE && c->node_type != BK_JOIN_NODE && c->node_type != BK_APPLY_NODE)) { err = "AGG child must be [FILTER ->] SCAN or JOIN"; return BKGPU_EUNSUPPORTED; }
         if (filter && filter->limit != -1) { err = "LIMIT on a filter below an aggregate is order dependent: outside the GPU path"; return BKGPU_EUNSUPPORTED; }
         if (c->node_type == BK_SCAN_NODE) ok = lower_agg(in, out, *top, conjuncts_of(filter), c->tuple_id, under_packet, true);
+        else if (c->node_type == BK_APPLY_NODE) ok = lower_apply_agg(in, out, *top, *c, under_packet, filter);
         // AGG -> [FILTER ->] JOIN: the store-side chain of a filtered join (separate.cpp:241-260)
         else ok = join_leaves(c) > 2 ? lower_star_agg(in, out, *top, *c, under_packet, filter) : lower_join_agg(in, out, *top, *c, under_packet, filter);
         // LimitNode straight over the aggregate: the result extraction (agg_result) skips `offset` groups and then keeps `limit` of them,
@@ -1943,7 +2034,9 @@ int compile_plan(const uint8_t* desc, size_t len, Compiled& out, std::string& er
         if (ok && (post_sort || post_having))
             ok = lower_sink(in, out, {post_sort, post_having, post_having ? post_having->limit : -1, true, "aggregate output columns under a SORT / HAVING",
                                       "SORT / HAVING above an aggregate references a column the aggregate does not output"}, limit_node);
-    } else if (const HNode* jn = join_rows_shape(top)) {   // [SORT ->] [FILTER ->] JOIN: a join that returns its rows
+    } else if (rows_shape(top, BK_APPLY_NODE)) {
+        err = "an APPLY (correlated subquery) that returns rows is outside the GPU path (an aggregate over it is lowered)"; return BKGPU_EUNSUPPORTED;
+    } else if (const HNode* jn = rows_shape(top, BK_JOIN_NODE)) {   // [SORT ->] [FILTER ->] JOIN: a join that returns its rows
         const HNode* t = top; const HNode *js = nullptr, *jf = nullptr;
         if (t->node_type == BK_SORT_NODE) { js = t; t = skip_passthrough(&t->ch[0], nullptr); }
         if (is_filter(t)) jf = t;

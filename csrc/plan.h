@@ -44,6 +44,9 @@ struct HNode {
     std::vector<int> is_asc, is_null_first;
     int join_type = 0;
     int64_t offset = 0;
+    // apply (pb::ApplyNode): join_type and the conditions in conjuncts
+    bool max_one_row = false, is_select_field = false;
+    int compare_type = 0;
     // window (pb::WindowNode): func_exprs in agg_fns, partition exprs in group_exprs, order exprs + is_asc in order_exprs / is_asc
     bool has_frame = false;
     int frame_type = 0;
@@ -147,6 +150,9 @@ struct Compiled {
     // not exist, not even in the tail).  Output 0 = the conjunction of that child's n_*_filter conjuncts (column indices into cols).
     int n_build_filter = 0, n_probe_filter = 0;
     Program build_filter{}, probe_filter{};
+    // an APPLY (correlated subquery) lowered as the SEMI / ANTI_SEMI join above: its join type (0 = no APPLY), the conjuncts moved from the
+    // subquery's filters into the join conditions, the conjuncts of the filter above it folded into the outer child's filter (explain only)
+    int apply_join_type = 0, apply_moved = 0, apply_folded = 0;
     // FK -> PK fast path: the same aggregate lowered over the virtual joined tuple (build-side columns are gathered
     // to probe-row alignment first); usable while every probe row has exactly one match
     std::shared_ptr<Compiled> jfast;

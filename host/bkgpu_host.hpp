@@ -55,10 +55,11 @@ struct PlanNode {
     int64_t limit = -1;
     std::vector<PlanNode> children;
     int tuple_id = 0; int64_t table_id = 0;              // SCAN / SORT
-    std::vector<Expr> conjuncts;                         // FILTER / JOIN conditions
+    std::vector<Expr> conjuncts;                         // FILTER / JOIN / APPLY conditions
     int agg_tuple_id = -1; std::vector<Expr> group_exprs, agg_fn_calls;
     std::vector<Expr> order_exprs; std::vector<bool> is_asc, is_null_first;
     int join_type = BK_INNER_JOIN; int64_t offset = 0;
+    bool max_one_row = false, is_select_field = false; int compare_type = BK_CMP_NULL;   // APPLY (its conditions in conjuncts)
     int count() const { int n = 1; for (auto& c : children) n += c.count(); return n; }
 };
 
@@ -86,6 +87,9 @@ public:
                 for (size_t i = 0; i < n.order_exprs.size(); i++) { expr(n.order_exprs[i]); w(n.is_asc[i] ? 1 : 0); w(n.is_null_first[i] ? 1 : 0); }
                 break;
             case BK_JOIN_NODE: w(n.join_type); w((int32_t)n.conjuncts.size()); for (auto& e : n.conjuncts) expr(e); break;
+            case BK_APPLY_NODE:
+                w(n.join_type); w((int32_t)n.conjuncts.size()); for (auto& e : n.conjuncts) expr(e);
+                w(n.max_one_row ? 1 : 0); w(n.compare_type); w(n.is_select_field ? 1 : 0); break;
             case BK_LIMIT_NODE: w64(n.offset); break;
             default: break;   // PACKET / SELECT_MANAGER: no payload
         }

@@ -21,6 +21,9 @@
  *     AGG_NODE / MERGE_AGG_NODE      : agg_tuple_id n_group EXPR* n_agg EXPR*   pb::AggNode
  *     SORT_NODE                      : tuple_id n_order (EXPR is_asc is_null_first)*  pb::SortNode
  *     JOIN_NODE                      : join_type n_conditions EXPR*  pb::JoinNode
+ *     APPLY_NODE                     : join_type n_conditions EXPR* max_one_row compare_type is_select_field   pb::ApplyNode
+ *                                      (child 0 = outer query, child 1 = subquery; their scan tuples are the outer / inner tuples, so
+ *                                       left / right tuple id lists are not carried.  compare_type: CMP_NULL 0, ANY 1, ALL 2, SOME 3)
  *     LIMIT_NODE                     : offset64                      pb::LimitNode
  *     WINDOW_NODE                    : n_fn EXPR* n_part EXPR* n_order (EXPR is_asc)* has_frame [FRAME]   pb::WindowNode
  *       FRAME := frame_type BOUND(start) BOUND(end)                  pb::WindowFrame (FT_ROWS 0, FT_RANGE 1)
@@ -57,7 +60,7 @@ enum bkgpu_plan_node_type {
     BK_SCAN_NODE = 1, BK_SORT_NODE = 2, BK_AGG_NODE = 4, BK_MERGE_AGG_NODE = 5,
     BK_TABLE_FILTER_NODE = 6, BK_JOIN_NODE = 7, BK_LIMIT_NODE = 11,
     BK_WHERE_FILTER_NODE = 12, BK_HAVING_FILTER_NODE = 13, BK_PACKET_NODE = 14,
-    BK_SELECT_MANAGER_NODE = 25, BK_WINDOW_NODE = 42
+    BK_SELECT_MANAGER_NODE = 25, BK_APPLY_NODE = 37, BK_WINDOW_NODE = 42
 };
 
 /* pb::ExprNodeType — proto/expr.proto:6-37 */
@@ -97,5 +100,8 @@ enum bkgpu_join_type {
     BK_NULL_JOIN = 0, BK_LEFT_JOIN = 1, BK_RIGHT_JOIN = 2, BK_INNER_JOIN = 3,
     BK_SEMI_JOIN = 4, BK_ANTI_SEMI_JOIN = 5, BK_FULL_JOIN = 6
 };
+
+/* pb::CompareType — proto/plan.proto:239-244 (ApplyNode.compare_type) */
+enum bkgpu_compare_type { BK_CMP_NULL = 0, BK_CMP_ANY = 1, BK_CMP_ALL = 2, BK_CMP_SOME = 3 };
 
 #endif /* BKGPU_PLAN_H_ */
