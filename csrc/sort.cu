@@ -23,6 +23,7 @@
 #include "dev_common.cuh"
 #include "interp.cuh"
 #include "nccl_dl.h"
+#include "sort_key.h"   // key_image: the order-preserving 64-bit image (ascending); DESC complements it
 
 namespace bk {
 
@@ -46,15 +47,6 @@ struct RowArgs {
     Program prog;
     KeySpec key;
 };
-
-// order-preserving 64-bit image (ascending); DESC complements it
-__device__ __forceinline__ uint64_t key_image(uint64_t v, int vclass, int desc) {
-    uint64_t t;
-    if (vclass == VC_F64) t = (v >> 63) ? ~v : (v | 0x8000000000000000ull);
-    else if (vclass == VC_I64) t = v ^ 0x8000000000000000ull;
-    else t = v;
-    return desc ? ~t : t;
-}
 
 // cls: 0 = row filtered out, 1 = key present, 2 = key is NULL
 __device__ __forceinline__ int row_key(const RowArgs& a, int64_t row, uint64_t& image) {
@@ -711,11 +703,14 @@ int grid_for(int64_t n, int per_block, int sm) { int64_t g = (n + per_block - 1)
 int select_topk_class(SortState* s, const RowArgs& ra, int cls, cudaStream_t st, bkgpu_stats* stats, std::string& err) {
     Pool& P = s->pool[cls - 1];
     const uint32_t k = (uint32_t)s->k;
-    uint32_t* cnt = s->d_counts;     // [0] sample count  [1] level-1 candidates  [2] level-2  [3] rows of this class  [4] kept rows  [5] level-3
+    uint32_t* cnt = s->d_counts;     // [0] sample count  [1] level-1 candidates  [2] level-2  [3] rows of this class  [4] kept rows  [5] level-3  [6] two_step: best of the batch
     uint64_t* thr = s->d_rank;       // three {key, idx, n} triples: thresholds of the three levels
     const uint32_t old_n = std::min<uint32_t>(P.n, k);
-    const uint32_t room = SMALL_N - old_n;
-    const uint32_t trim = std::min<uint32_t>(room, std::max<uint32_t>(2 * k, 2048) - std::min<uint32_t>(old_n, 1024));
+    // The last level leaves about 1.5 k candidates.  Beside k kept rows they fit one CTA sort only while k is small (at k = 4096 the room
+    // would be exactly k: no sampled threshold hits that): a larger k sorts the candidates alone, keeps k, and merges those with the kept rows.
+    const bool two_step = old_n > 0 && old_n + 2 * k > SMALL_N;
+    const uint32_t room = two_step ? SMALL_N : SMALL_N - old_n;
+    const uint32_t trim = std::min<uint32_t>(room, std::max<uint32_t>(2 * k, 2048) - (two_step ? 0 : std::min<uint32_t>(old_n, 1024)));
     const int nxt = P.cur ^ 1;
     const uint64_t* pool_thr = nullptr;
     if (P.n >= k) {   // later rows must beat the k-th composite key kept so far
@@ -764,6 +759,13 @@ int select_topk_class(SortState* s, const RowArgs& ra, int cls, cudaStream_t st,
             stats->kernel_launches += 3;
         }
         // final: candidates + kept rows sorted by one CTA, keep k, fetch the payload of the survivors
+        if (two_step) {   // cand[0] (cnt[5]) -> its k best in cand[1] (cnt[6]) -> merged with the kept rows
+            k_sort_small<<<1, 1024, SMALL_N * 16, st>>>(s->cand_key[0], s->cand_idx[0], cnt + 5, room, nullptr, nullptr, 0,
+                                                        s->cand_key[1], s->cand_idx[1], k, cnt + 6, 0, nullptr, nullptr, 0, 0, 0, nullptr);
+            k_sort_small<<<1, 1024, SMALL_N * 16, st>>>(s->cand_key[1], s->cand_idx[1], cnt + 6, k, P.key[P.cur], P.idx[P.cur], old_n,
+                                                        P.key[nxt], P.idx[nxt], k, cnt + 4, 0, nullptr, nullptr, 0, 0, 0, nullptr);
+            stats->kernel_launches++;
+        } else
         k_sort_small<<<1, 1024, SMALL_N * 16, st>>>(s->cand_key[0], s->cand_idx[0], cnt + 5, room, P.key[P.cur], P.idx[P.cur], old_n,
                                                     P.key[nxt], P.idx[nxt], k, cnt + 4, 0, nullptr, nullptr, 0, 0, 0, nullptr);
         GatherArgs g; memset(&g, 0, sizeof g);

@@ -91,6 +91,20 @@ def test_no_partition_no_order_all_peers():
                        window_frame=None), same)                             # all rows peers of one partition
 
 
+@pytest.mark.parametrize("asc", [True, False])
+def test_signed_zero_order_keys_are_equal(asc):
+    """-0.0 and +0.0 are one sort key (MemRowCompare): such rows stay in arrival order, fall through to the next ORDER BY key, and are
+    peers.  ROW_NUMBER and LAG of the arrival index show the order the rows reached the window in, RANK / DENSE_RANK the peer groups."""
+    rng = np.random.default_rng(23)
+    n = 6000
+    cols = table(23, n, n_keys=5)
+    cols[2] = make_column(0, 3, T.DOUBLE, rng.choice(np.array([-0.0, 0.0, -0.0, 0.0, 1.5, -2.0]), n), rng.random(n) > 0.05)
+    fns = [P.window_expr("row_number", 1, 1), P.window_expr("rank", 1, 2), P.window_expr("dense_rank", 1, 3), P.window_expr("lag", 1, 4, Y),
+           P.window_expr("cume_dist", 1, 5)]
+    run(P.window_stage(P.scan(0), fns, [K], [X], [asc]), cols)                     # ties between the zeros: arrival order
+    run(P.window_stage(P.scan(0), fns, [K], [X, V], [asc, not asc]), cols)         # ... and then the next key
+
+
 def test_ragged_batches_filter_and_zero_rows():
     cols = table(13, 20000, n_keys=7)
     cuts = [0, 1, 777, 778, 9000, 20000]

@@ -7,7 +7,7 @@ It keeps the reference's structure on purpose: partitions are runs of equal part
 every function once over the whole partition, FrameWindowProcessor resets the frame and calls again for every row (O(rows *
 frame)), and RANK / DENSE_RANK / PERCENT_RANK / CUME_DIST / NTILE / LEAD / LAG step through their intermediate state the way
 get_result does.  The sort is stable (rows with equal keys keep their arrival order), with the device's total order: NULLs
-first / last per is_null_first, doubles in IEEE bit order (so -0.0 sorts before +0.0, and NaN by its bits).
+first / last per is_null_first, -0.0 and +0.0 equal keys (as in MemRowCompare), NaN by its IEEE bits.
 
 Expressions: slot references, INT / DOUBLE / NULL literals, + - *, comparisons and AND — enough for the tests' arguments,
 filters and keys.
@@ -36,10 +36,13 @@ def _dbits(d: float) -> int:
     return struct.unpack("<Q", struct.pack("<d", d))[0]
 
 
-def _image(v, prim: int, asc: bool) -> int:
-    """the device's order-preserving 64-bit key image (sort.cu key_image)"""
+def _image(v, prim: int, asc: bool, zeros_equal: bool = True) -> int:
+    """the device's order-preserving 64-bit key image (csrc/sort_key.h key_image): -0.0 and +0.0 share one image, as they compare equal
+    in MemRowCompare.  zeros_equal=False is the plain IEEE bit order window.cu's MIN / MAX compare (ord_image: -0.0 below +0.0)."""
     if prim in FLOATS:
         b = _dbits(float(v))
+        if zeros_equal and b == 1 << 63:
+            b = 0
         t = (~b & M64) if b >> 63 else (b | (1 << 63))
     elif prim in UINTS or prim == T.BOOL:
         t = int(v) & M64
@@ -204,7 +207,7 @@ class _Fn:
                 if self.min_max is None:
                     self.min_max = v
                 else:
-                    iv, im = _image(v, at, True), _image(self.min_max, at, True)
+                    iv, im = _image(v, at, True, zeros_equal=False), _image(self.min_max, at, True, zeros_equal=False)
                     if (nm == "min" and im > iv) or (nm == "max" and im < iv):
                         self.min_max = v
         elif nm in ("rank", "dense_rank", "percent_rank", "cume_dist", "lead", "lag"):
