@@ -59,27 +59,14 @@ struct AggArgs {
     JoinProbe jp;            // lean kernel only: the key column holds the probe-side foreign key (see JoinProbe)
     int32_t lean_nulls;      // lean kernel: some predicate / value column of this batch carries a validity bitmap
     int32_t lean_mm;         // lean kernel: some value column feeds MIN / MAX lanes or more than one lane
-    // warp-private kernel (agg_wp.cuh): chosen by the host for the plainest lean batches
     int32_t scalar_tma;      // 1 = try the TMA-staged scalar kernel (scalar_tma.cu)
-    int32_t jp_pipeline;     // 1 = the fused probe issues its dimension lookups one drain ahead (agg_direct.cuh)
-    int32_t lean_bank;       // 1 = the lean kernel's drain deals entries to lanes by the bank group of their home slot (option lean_bank)
     int32_t lean_fx;         // 1 = the lean kernel accumulates its double sums as fixed-point limbs with native 32-bit shared atomics (FX, agg_direct.cuh)
     uint32_t fx_ext_off;     // FX: byte offset (in the CTA's dynamic shared memory) of the low-extension limb arrays [value column][slot]
-    int32_t wp;              // 1 = launch k_agg_group_wp
-    int32_t wp_gcap;         // dense group ids per warp table (multiple of 32)
-    int32_t wp_kt_log2;      // log2 words of the CTA's key -> id table
-    int32_t wp_warps;        // warps per CTA (one accumulator table each): 8, 12 or 16
-    int32_t wp_dense;        // 1 = no key table: id = key - wp_dense_sub (keys known to lie in a range of wp_gcap values)
-    uint32_t wp_dense_sub;
     // lean kernel: the last CTA to finish extracts the table's rows into this mapped host buffer (fused_extract, agg_kernels.cuh):
     // [32-byte counter block][values n_img x n][null bytes n_img x n], n = the groups in the table.  nullptr = no fused extraction
     uint8_t* fused_out;
     uint32_t fused_cap;      // rows the buffer holds: a table with more groups leaves only the counter block there (the host runs k_extract)
 };
-
-// shared memory of k_agg_group_wp: key table + id counter + one accumulator set {sums 8 B x na, cnt 4 B} x gcap per warp
-inline size_t wp_warp_bytes(int na, uint32_t gcap) { return ((size_t)gcap * (8u * (uint32_t)na + 4u) + 15) & ~(size_t)15; }
-inline size_t wp_smem_bytes(int na, uint32_t gcap, int kt_log2, int warps) { return (kt_log2 < 0 ? 0 : ((size_t)8 << kt_log2)) + 16 + wp_warp_bytes(na, gcap) * (size_t)warps; }
 
 // typed columns built from the aggregate's extracted images (input of the post fragment)
 struct PostCols { int32_t n; int32_t img[MAX_COLS]; int32_t stype[MAX_COLS]; uint8_t* values[MAX_COLS]; uint8_t* null_bytes[MAX_COLS]; };

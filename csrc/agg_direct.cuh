@@ -544,15 +544,8 @@ __global__ void __launch_bounds__(DIRECT_THREADS, 1) k_agg_group_direct(const __
 // (AggFnCall::update's `add` is a sequential double add, agg_fn_call.cpp:496-555; any parallel order already differs from it in the
 // last bits.)
 // ------------------------------------------------------------------------------------------
-#ifndef BK_FX_EXACT_INLINE
-#define BK_FX_EXACT_INLINE 0   // 1 = the rare exact path inlined: no spills (the call costs 24 bytes of them) but the loop outgrows the instruction cache
-#endif
-#if BK_FX_EXACT_INLINE
-static __device__ __forceinline__ void global_add_f64(const AggArgs& a, uint64_t k0, int glob_lane, double x)
-#else
-static __device__ __noinline__ void global_add_f64(const AggArgs& a, uint64_t k0, int glob_lane, double x)
-#endif
-{
+// (out of line although the call costs 24 bytes of spills: inlined, this rare path makes the loop outgrow the instruction cache)
+static __device__ __noinline__ void global_add_f64(const AggArgs& a, uint64_t k0, int glob_lane, double x) {
     const AggPlan& ap = a.plan;
     const GroupTable& gt = a.gt;
     const uint32_t gcap = gt.cap_mask + 1;
@@ -565,12 +558,6 @@ static __device__ __noinline__ void global_add_f64(const AggArgs& a, uint64_t k0
     atomicAdd(gt.n_groups + GT_FX_EXACT, 1u);   // values that took this path: when they are many the host stops choosing FX for this plan (api.cu)
 }
 __device__ __forceinline__ void reds_add32(uint32_t a, uint32_t v) { asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
-#ifndef BK_FX_PAIR
-#define BK_FX_PAIR 0      // 1 = fx_add2's interleaved pair path (its registers push a loaded column into local memory)
-#endif
-#ifndef BK_FX_HI_ALWAYS
-#define BK_FX_HI_ALWAYS 0
-#endif
 // one value into the fixed-point limbs of `slot`: word = shared address of the slot's {mid, hi} pair, ext = of its low-extension limb
 __device__ __forceinline__ void fx_add(const AggArgs& a, uint32_t word, uint32_t ext, double scale, uint32_t fx_lo, uint64_t k0, int glob_lane, uint64_t vbits) {
     uint32_t lo; uint64_t up;
@@ -578,7 +565,7 @@ __device__ __forceinline__ void fx_add(const AggArgs& a, uint32_t word, uint32_t
     if (kind == FX_MAIN) {
         const uint32_t old = atoms_add32(word, lo);
         const uint32_t h = (uint32_t)up + ((old + lo) < old ? 1u : 0u);
-        if (BK_FX_HI_ALWAYS || h) reds_add32(word + 4u, h);
+        if (h) reds_add32(word + 4u, h);
     } else if (kind == FX_FINE) {
         const uint32_t old = atoms_add32(ext, lo);
         const uint64_t t = up + ((old + lo) < old ? 1u : 0u);   // sign-extended upper part + carry
@@ -587,26 +574,6 @@ __device__ __forceinline__ void fx_add(const AggArgs& a, uint32_t word, uint32_t
         const uint32_t h = (uint32_t)(t >> 32) + ((old2 + m) < old2 ? 1u : 0u);
         if (h) reds_add32(word + 4u, h);
     } else if (kind == FX_EXACT) global_add_f64(a, k0, glob_lane, bits_f64(vbits));
-}
-// two double sums of one row: when both values are main values (the common case by construction of the scale) their two chains
-// DMUL -> F2I -> ATOMS.ADD -> carry -> RED run interleaved in ONE branch region; anything else takes fx_add per value
-__device__ __forceinline__ void fx_add2(const AggArgs& a, uint32_t word0, uint32_t word1, uint32_t ext0, uint32_t ext1, double scale0, double scale1, uint32_t fx_lo,
-                                        uint64_t k0, int glob_lane0, int glob_lane1, uint64_t v0, uint64_t v1) {
-    if (BK_FX_PAIR) {
-        const double y0 = bits_f64(v0) * scale0, y1 = bits_f64(v1) * scale1;
-        const uint32_t d0 = ((fx_hi_word(y0) >> 20) & 0x7FFu) - fx_lo - (uint32_t)FX_FINE_BINADES;
-        const uint32_t d1 = ((fx_hi_word(y1) >> 20) & 0x7FFu) - fx_lo - (uint32_t)FX_FINE_BINADES;
-        if ((d0 < (uint32_t)FX_MAIN_BINADES) & (d1 < (uint32_t)FX_MAIN_BINADES)) {
-            const long long f0 = fx_round(y0), f1 = fx_round(y1);
-            const uint32_t l0 = (uint32_t)f0, l1 = (uint32_t)f1;
-            const uint32_t o0 = atoms_add32(word0, l0), o1 = atoms_add32(word1, l1);
-            reds_add32(word0 + 4u, (uint32_t)((uint64_t)f0 >> 32) + ((o0 + l0) < o0 ? 1u : 0u));
-            reds_add32(word1 + 4u, (uint32_t)((uint64_t)f1 >> 32) + ((o1 + l1) < o1 ? 1u : 0u));
-            return;
-        }
-    }
-    fx_add(a, word0, ext0, scale0, fx_lo, k0, glob_lane0, v0);
-    fx_add(a, word1, ext1, scale1, fx_lo, k0, glob_lane1, v1);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -621,10 +588,8 @@ __device__ __forceinline__ void fx_add2(const AggArgs& a, uint32_t word0, uint32
 // aggregate: its sum gets +0 and its non-NULL counter no increment); the key column stays NULL-free in this kernel.
 // MM: value columns may feed MIN / MAX lanes (LDS -> compare -> ATOMS.CAS.64 only when the row improves the extreme: after the
 // first rows of a group that is one LDS per row) and up to three lanes each (SUM + MIN + MAX over one column).
-// BANK (opt-in `lean_bank`, experimental): the drain re-deals the 32 entries of a pass so that lane L serves an entry whose home slot
-// is L mod 8 (mod the eight 16-byte bank groups): the 16-byte LDS / CAS of a quarter-warp then hit eight different bank groups.
 // FX: double sums as fixed-point limbs updated with native 32-bit shared atomics (see above).
-template <int NP, int NA, bool JOIN, bool NULLS = false, bool MM = false, bool BANK = false, bool FX = false>
+template <int NP, int NA, bool JOIN, bool NULLS = false, bool MM = false, bool FX = false>
 __global__ void __launch_bounds__(LEAN_THREADS, 1) k_agg_group_lean(const __grid_constant__ AggArgs a) {
     constexpr int NS = NP + 1 + NA;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -684,7 +649,6 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) k_agg_group_lean(const __grid
     const int64_t stride = (int64_t)gridDim.x * LEAN_THREADS;
     // ---- FX: per-CTA scale of every double sum, from a sample of 640 rows spread over the whole batch ----
     double fx_scale[NA > 0 ? NA : 1]; uint32_t fx_lo = 0, fx_ext = 0;
-    const bool fx_pair = BK_FX_PAIR && FX && NA == 2 && acc_f64[0] && acc_f64[NA > 1 ? 1 : 0];   // both value columns feed double sums: fx_add2
     __shared__ uint32_t fx_emax[4];
     __shared__ int32_t fx_F[4];
     if constexpr (FX) {
@@ -754,154 +718,6 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) k_agg_group_lean(const __grid
     };
     if (q0 + lane < nquads) issue_loads(q0 + lane);
     uint32_t qhead = 0, qcount = 0;   // warp-uniform: ring start (a multiple of 32) and entries waiting in it
-    if constexpr (JOIN && !NULLS && !MM) {
-    if (a.jp.mode == 1 && a.jp_pipeline) {
-        // ---- K4 fused, software-pipelined: the dimension lookups of a trip are ISSUED, then the rows the
-        //      previous trip queued are drained while they fly (the table work hides the L2 round trip), then they are consumed and the
-        //      trip's rows queued.  The next trip's foreign keys load into the key registers as soon as the lookups have left.
-        const JoinProbe& jp = a.jp;
-#pragma unroll 1
-        for (;;) {
-            const bool last = q0 >= nquads;
-            const int64_t q = q0 + lane;
-            uint32_t pass = 0, g[4] = {0, 0, 0, 0}, pr4[4] = {0, 0, 0, 0};
-            if (!last) {
-                if (q < nquads) {
-                    pass = 0xFu;
-#pragma unroll
-                    for (int t = 0; t < NP; t++) {
-                        uint32_t r8[8];
-#pragma unroll
-                        for (int j = 0; j < 4; j++) r8[j] = pr[t][j];
-                        pass &= term_mask_i32(tcmp[t], tconst[t], r8);
-                    }
-                }
-                uint32_t inr = 0;
-#pragma unroll
-                for (int j = 0; j < 4; j++) {
-                    const uint64_t img = jp.key_signed ? (uint64_t)(int64_t)(int32_t)kr[j] : (uint64_t)kr[j];
-                    const uint64_t off = (img ^ jp.bias) - jp.dense_min;
-                    if (((pass >> j) & 1u) && off < jp.dense_size) {
-                        inr |= 1u << j;
-                        g[j] = __ldg(jp.attr + off);
-                        if (jp.present) pr4[j] = __ldg(jp.present + off);
-                    }
-                }
-                pass &= inr;
-                if (q + stride < nquads) {   // the keys of the next trip (the lookups above no longer need these registers)
-                    const U32x4 r = ldg128_u32(kptr + (q + stride) * 16);
-#pragma unroll
-                    for (int j = 0; j < 4; j++) kr[j] = r.v[j];
-                }
-            }
-            // ---- drain what the previous trip queued ----
-            {
-                const uint32_t limit = (last || NP == 0) ? qcount : (qcount & ~31u);
-#pragma unroll 1
-                for (uint32_t e0 = 0; e0 < limit; e0 += 32) {
-                    if (e0 + lane >= limit) continue;
-                    uint32_t e = qhead + e0 + lane;
-                    if (NP > 0) e -= e >= LQ ? LQ : 0u;
-                    const uint64_t k0 = lds64(qkey + e * 8u);
-                    uint64_t v[NA > 0 ? NA : 1];
-#pragma unroll
-                    for (int s = 0; s < NA; s++) v[s] = lds64(qval + (s * LQ + e) * 8u);
-                    const uint32_t h = ((uint32_t)k0 ^ (uint32_t)(k0 >> 32)) * 0x9E3779B1u;
-                    int slot = -1;
-                    if (k0 != EMPTY_KEY) slot = smem32_upsert1(keys_addr, cap_mask, k0, h >> hash_shift);
-                    if (slot >= 0) {
-                      if constexpr (FX) {   // native 32-bit atomics only: row count, then two (rarely three) limbs per double sum
-                          reds_inc32(lanes_addr + slot * 16u);
-if (NA == 2 && fx_pair) fx_add2(a, acc_addr[0] + slot * 16u, acc_addr[NA > 1 ? 1 : 0] + slot * 16u, fx_ext + slot * 4u, fx_ext + (tcap + slot) * 4u,
-                                                          fx_scale[0], fx_scale[NA > 1 ? 1 : 0], fx_lo, k0, a.vops[0].glob_lane[0], a.vops[NA > 1 ? 1 : 0].glob_lane[0], v[0], v[NA > 1 ? 1 : 0]);
-                          else
-#pragma unroll
-                          for (int s = 0; s < NA; s++) {
-                              if (acc_f64[s]) fx_add(a, acc_addr[s] + slot * 16u, fx_ext + ((uint32_t)s * tcap + slot) * 4u, fx_scale[s], fx_lo, k0, a.vops[s].glob_lane[0], v[s]);
-                              else smem32_add_u64(acc_addr[s] + slot * 16u, v[s]);
-                          }
-                      } else {
-                        reds_inc32(lanes_addr + slot * 16u);
-                        int first = 0;
-                        if (pair2) {
-                            const uint32_t addr = acc_addr[0] + slot * 16u;
-                            uint64_t c0, c1;
-                            lds128(addr, c0, c1);
-                            for (;;) {
-                                uint64_t p0, p1;
-                                atoms_cas128(addr, c0, c1, f64_bits(bits_f64(c0) + bits_f64(v[0])), f64_bits(bits_f64(c1) + bits_f64(v[NA > 1 ? 1 : 0])), p0, p1);
-                                if (p0 == c0 && p1 == c1) break;
-                                c0 = p0; c1 = p1;
-                            }
-                            first = 2;
-                        }
-#pragma unroll
-                        for (int s = 0; s < NA; s++) {
-                            if (s < first) continue;
-                            if (acc_f64[s]) smem32_add_f64(acc_addr[s] + slot * 16u, bits_f64(v[s])); else smem32_add_u64(acc_addr[s] + slot * 16u, v[s]);
-                        }
-                      }
-                    } else {
-                        uint64_t key[2] = {k0, 0ull};
-                        uint64_t gv[NA > 0 ? NA : 1];
-#pragma unroll
-                        for (int s = 0; s < NA; s++) gv[s] = lds64(qval + (s * LQ + e) * 8u);
-                        global_update_row<NA>(a, key, gv, 0u);
-                    }
-                }
-                if (NP > 0) { qhead = (qhead + limit) % LQ; qcount -= limit; } else qcount = 0;
-            }
-            __syncwarp();
-            if (last) break;
-            // ---- consume the lookups: rows without a partner leave the mask (inner join); queue the survivors ----
-            if (jp.present) {
-#pragma unroll
-                for (int j = 0; j < 4; j++) if (pr4[j] == 0xFFFFFFFFu) pass &= ~(1u << j);
-            }
-            {
-                uint32_t bal[4];
-#pragma unroll
-                for (int j = 0; j < 4; j++) bal[j] = __ballot_sync(0xFFFFFFFFu, (pass >> j) & 1u);
-                uint32_t fresh = 0;
-                const uint32_t tail = qhead + qcount;
-#pragma unroll
-                for (int j = 0; j < 4; j++) {
-                    if ((pass >> j) & 1u) {
-                        uint32_t pos = tail + fresh + (uint32_t)__popc(bal[j] & lane_lt);
-                        if (NP > 0) pos -= pos >= LQ ? LQ : 0u;
-                        sts64(qkey + pos * 8u, (uint64_t)g[j] & kmask);
-#pragma unroll
-                        for (int s = 0; s < NA; s++) sts64(qval + (s * LQ + pos) * 8u, vr[s][j]);
-                    }
-                    fresh += __popc(bal[j]);
-                }
-                qcount += fresh;
-            }
-            passed += __popc(pass);
-            // ---- the other columns of the next trip (its keys are already on their way) ----
-            if (q + stride < nquads) {
-#pragma unroll
-                for (int t = 0; t < NP; t++) { const U32x4 r = ldg128_u32(tptr[t] + (q + stride) * 16);
-#pragma unroll
-                    for (int j = 0; j < 4; j++) pr[t][j] = r.v[j]; }
-#pragma unroll
-                for (int s = 0; s < NA; s++) { const U64x4 r = ldg256_u64(vptr[s] + (q + stride) * 32);
-#pragma unroll
-                    for (int j = 0; j < 4; j++) vr[s][j] = r.v[j]; }
-            }
-            __syncwarp();
-            q0 += stride;
-        }
-        fx_finish();
-        smem_table_flush(st, a);
-        if (blockIdx.x == 0 && threadIdx.x < (a.nrows & 3)) passed += direct_tail_row<NP, NA, JOIN>(a, (a.nrows & ~(int64_t)3) + threadIdx.x);
-#pragma unroll
-        for (int d = 16; d > 0; d >>= 1) passed += __shfl_xor_sync(0xFFFFFFFFu, passed, d);
-        if (lane == 0 && passed) atomicAdd((unsigned long long*)a.rows_passed, (unsigned long long)passed);
-        if (a.fused_out) fused_extract(a);
-        return;
-    }
-    }
 #pragma unroll 1
     for (;;) {
         const bool last = q0 >= nquads;   // (warp-uniform) one extra trip drains what is left in the ring
@@ -996,69 +812,6 @@ if (NA == 2 && fx_pair) fx_add2(a, acc_addr[0] + slot * 16u, acc_addr[NA > 1 ? 1
         const uint32_t limit = (last || NP == 0) ? total : (total & ~31u);
         // (one entry per lane: a two-entries-per-lane variant needs more registers and leaves more
         //  lanes idle in the last pass)
-        if constexpr (BANK && !NULLS && !MM && !JOIN) {
-            auto update = [&](bool active, uint64_t k0, uint32_t e) {
-                if (!active) return;
-                uint64_t v[NA > 0 ? NA : 1];
-#pragma unroll
-                for (int s = 0; s < NA; s++) v[s] = lds64(qval + (s * LQ + e) * 8u);
-                const uint32_t h = ((uint32_t)k0 ^ (uint32_t)(k0 >> 32)) * 0x9E3779B1u;
-                int slot = -1;
-                if (k0 != EMPTY_KEY) slot = smem32_upsert1(keys_addr, cap_mask, k0, h >> hash_shift);
-                if (slot >= 0) {
-                    reds_inc32(lanes_addr + slot * 16u);
-                    int first = 0;
-                    if (pair2) {
-                        const uint32_t addr = acc_addr[0] + slot * 16u;
-                        uint64_t c0, c1;
-                        lds128(addr, c0, c1);
-                        for (;;) {
-                            uint64_t p0, p1;
-                            atoms_cas128(addr, c0, c1, f64_bits(bits_f64(c0) + bits_f64(v[0])), f64_bits(bits_f64(c1) + bits_f64(v[NA > 1 ? 1 : 0])), p0, p1);
-                            if (p0 == c0 && p1 == c1) break;
-                            c0 = p0; c1 = p1;
-                        }
-                        first = 2;
-                    }
-#pragma unroll
-                    for (int s = 0; s < NA; s++) {
-                        if (s < first) continue;
-                        if (acc_f64[s]) smem32_add_f64(acc_addr[s] + slot * 16u, bits_f64(v[s])); else smem32_add_u64(acc_addr[s] + slot * 16u, v[s]);
-                    }
-                } else {   // rare: re-read the entry so that v[] never needs an address (no local-memory copy per pass)
-                    uint64_t key[2] = {k0, 0ull};
-                    uint64_t gv[NA > 0 ? NA : 1];
-#pragma unroll
-                    for (int s = 0; s < NA; s++) gv[s] = lds64(qval + (s * LQ + e) * 8u);
-                    global_update_row<NA>(a, key, gv, 0u);
-                }
-            };
-#pragma unroll 1
-            for (uint32_t e0 = 0; e0 < limit; e0 += 32) {
-                const bool have = e0 + lane < limit;
-                uint32_t e = qhead + e0 + lane;
-                if (NP > 0) e -= e >= LQ ? LQ : 0u;
-                const uint64_t k0 = have ? lds64(qkey + e * 8u) : EMPTY_KEY;
-                const uint32_t b = ((((uint32_t)k0 ^ (uint32_t)(k0 >> 32)) * 0x9E3779B1u) >> hash_shift) & 7u;   // bank group of the home slot
-                const uint32_t act = __ballot_sync(0xFFFFFFFFu, have && k0 != EMPTY_KEY);
-                const uint32_t m0 = __ballot_sync(0xFFFFFFFFu, b & 1u), m1 = __ballot_sync(0xFFFFFFFFu, b & 2u), m2 = __ballot_sync(0xFFFFFFFFu, b & 4u);
-                auto members = [&](uint32_t g) { return act & ((g & 1u) ? m0 : ~m0) & ((g & 2u) ? m1 : ~m1) & ((g & 4u) ? m2 : ~m2); };
-                const uint32_t rank = __popc(members(b) & lane_lt);
-                // lane L serves the (L / 8)-th entry of bank group L % 8
-                uint32_t dm = members((uint32_t)lane & 7u);
-                const int r = lane >> 3;
-                if (r > 0) dm &= dm - 1u;
-                if (r > 1) dm &= dm - 1u;
-                if (r > 2) dm &= dm - 1u;
-                const bool served = dm != 0u;
-                const int src = served ? __ffs(dm) - 1 : lane;
-                const uint64_t ks = __shfl_sync(0xFFFFFFFFu, k0, src);
-                uint32_t es = qhead + e0 + (uint32_t)src;
-                if (NP > 0) es -= es >= LQ ? LQ : 0u;
-                update(served, ks, es);
-                update(have && (k0 == EMPTY_KEY || rank >= 4u), k0, e);   // a fifth entry of a bank group, or the sentinel key: by its own lane
-            }
-        } else
 #pragma unroll 1
         for (uint32_t e0 = 0; e0 < limit; e0 += 32) {
             if (e0 + lane >= limit) continue;   // (only the final trip has a ragged pass)
@@ -1080,9 +833,6 @@ if (NA == 2 && fx_pair) fx_add2(a, acc_addr[0] + slot * 16u, acc_addr[NA > 1 ? 1
             if (slot >= 0) {
                 if constexpr (FX) {   // native 32-bit atomics only: row count, then two (rarely three) limbs per double sum
                     reds_inc32(lanes_addr + slot * 16u);
-if (NA == 2 && fx_pair) fx_add2(a, acc_addr[0] + slot * 16u, acc_addr[NA > 1 ? 1 : 0] + slot * 16u, fx_ext + slot * 4u, fx_ext + (tcap + slot) * 4u,
-                                                    fx_scale[0], fx_scale[NA > 1 ? 1 : 0], fx_lo, k0, a.vops[0].glob_lane[0], a.vops[NA > 1 ? 1 : 0].glob_lane[0], v[0], v[NA > 1 ? 1 : 0]);
-                    else
 #pragma unroll
                     for (int s = 0; s < NA; s++) {
                         if (acc_f64[s]) fx_add(a, acc_addr[s] + slot * 16u, fx_ext + ((uint32_t)s * tcap + slot) * 4u, fx_scale[s], fx_lo, k0, a.vops[s].glob_lane[0], v[s]);
@@ -1304,9 +1054,6 @@ static inline cudaError_t launch_persistent(K kernel, const AggArgs& a, size_t s
     return cudaGetLastError();
 }
 
-template <int NP, int NA>
-static inline cudaError_t launch_wp(const AggArgs& a, int sm_count, cudaStream_t s, cudaEvent_t start);   // agg_wp.cuh
-
 // the kernel select_agg_launch (agg_select.cpp) chose; exactly these instantiations of k_agg_group_lean exist
 template <int NP, int NA>
 static inline cudaError_t launch_direct(const AggArgs& a, AggKernel k, int sm_count, size_t smem, cudaStream_t s, cudaEvent_t start) {
@@ -1314,20 +1061,16 @@ static inline cudaError_t launch_direct(const AggArgs& a, AggKernel k, int sm_co
     switch (k) {
         case SCALAR_DIRECT: return launch_persistent(k_agg_scalar_direct<NP, NA>, a, 0, sm_count, DIRECT_THREADS, s, start);
         case GROUP_DIRECT: return launch_persistent(k_agg_group_direct<NP, NA>, a, smem, sm_count, DIRECT_THREADS, s, start);
-        case WP: return launch_wp<NP, NA>(a, sm_count, s, start);
         case LEAN: return launch_persistent(k_agg_group_lean<NP, NA, false>, a, smem, sm_count, T, s, start);
         // (one MM / NULLS instantiation serves batches with and without NULLs: without bitmaps the NULL masks are simply zero)
         case LEAN_MM: return launch_persistent(k_agg_group_lean<NP, NA, false, true, true>, a, smem, sm_count, T, s, start);
         case LEAN_NULLS: return launch_persistent(k_agg_group_lean<NP, NA, false, true>, a, smem, sm_count, T, s, start);
         case LEAN_JOIN: return launch_persistent(k_agg_group_lean<NP, NA, true>, a, smem, sm_count, T, s, start);
         case LEAN_FX:   // double sums as fixed-point limbs (native 32-bit shared atomics)
-            if constexpr (NA >= 1) return launch_persistent(k_agg_group_lean<NP, NA, false, false, false, false, true>, a, smem, sm_count, T, s, start);
+            if constexpr (NA >= 1) return launch_persistent(k_agg_group_lean<NP, NA, false, false, false, true>, a, smem, sm_count, T, s, start);
             break;
         case LEAN_FX_JOIN:
-            if constexpr (NA >= 1) return launch_persistent(k_agg_group_lean<NP, NA, true, false, false, false, true>, a, smem, sm_count, T, s, start);
-            break;
-        case LEAN_BANK:
-            if constexpr (NA <= 2) return launch_persistent(k_agg_group_lean<NP, NA, false, false, false, true>, a, smem, sm_count, T, s, start);
+            if constexpr (NA >= 1) return launch_persistent(k_agg_group_lean<NP, NA, true, false, false, true>, a, smem, sm_count, T, s, start);
             break;
         default: break;
     }

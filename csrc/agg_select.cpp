@@ -1,5 +1,5 @@
 // agg_select.cpp — the choice of the aggregate kernel for one batch (see agg_select.h).  Pure host code: the launchers in agg.cu,
-// scalar_tma.cu, agg_direct.cuh and agg_wp.cuh dispatch on its AggKernel and decide nothing themselves.
+// scalar_tma.cu and agg_direct.cuh dispatch on its AggKernel and decide nothing themselves.
 #include "agg_select.h"
 #include <stdint.h>
 #include <string.h>
@@ -16,7 +16,6 @@ const char* agg_kernel_name(AggKernel k) {
         case COUNT_WHERE_TMA: return "k_count_where_tma";
         case GROUP_DIRECT: return "k_agg_group_direct";
         case LEAN_FX: case LEAN_FX_JOIN: return "k_agg_group_lean_fx";
-        case WP: return "k_agg_group_wp";
         default: return "k_agg_group_lean";
     }
 }
@@ -92,33 +91,6 @@ static bool lean_fits(const Compiled& c, const AggArgs& a, bool nulls_ok, bool m
         if (vo.n_ops != 1) mm = true;
     }
     return ok && (!mm || mm_ok);
-}
-
-// warp-private tables (agg_wp.cuh) for the plainest lean batches whose groups fit one table per warp.  The capacity follows the cardinality
-// learned from earlier batches / runs of this plan; an unknown cardinality starts with the largest table.
-static void plan_wp(const Compiled& c, const AggEnv& env, AggArgs& a) {
-    const int np = c.direct.n_terms, na = c.direct.n_vals;
-    const DevCol& kc = a.cols[np];
-    bool ok = kc.stype == ST_I32 || kc.stype == ST_U32;
-    for (int v = 0; v < na && ok; v++) ok = a.vops[v].n_ops == 1 && (a.vops[v].op[0] == LN_ADD_F64 || a.vops[v].op[0] == LN_ADD_I64);
-    if (!ok) return;
-    const size_t budget = 226 * 1024;
-    const uint32_t g = env.known_groups;
-    int warps = 8;
-    if (na <= 1 && g) {   // one value column: the tables are small enough for 12 or 16 warps (three / four per scheduler)
-        const uint32_t gc = (g + 31) & ~31u;
-        int kl4 = 8; while ((1u << kl4) < 4 * gc) kl4++;
-        if (wp_smem_bytes(na, gc, kl4, 16) <= budget) warps = 16;
-        else if (wp_smem_bytes(na, gc, kl4, 12) <= budget) warps = 12;
-    }
-    if (env.wp_warps && (na <= 1 || env.wp_warps == 8)) warps = env.wp_warps;
-    uint32_t gcap = g ? ((g + 31) & ~31u) : 0;
-    auto fits = [&](uint32_t gc, int kl) { return wp_smem_bytes(na, gc, kl, warps) <= budget; };
-    auto kt_for = [&](uint32_t gc, int factor) { int kl = 8; while ((1u << kl) < (uint32_t)factor * gc) kl++; return kl; };
-    if (gcap == 0) { gcap = 32; while (fits(gcap + 32, kt_for(gcap + 32, 2))) gcap += 32; }   // unknown: the largest table that fits
-    int kl = env.wp_kt_log2 > 0 ? env.wp_kt_log2 : kt_for(gcap, 4);          // key table at <= 25 % load when it fits ...
-    if (!fits(gcap, kl)) kl = kt_for(gcap, 2);                                // ... else <= 50 %
-    if (fits(gcap, kl)) { a.wp = 1; a.wp_gcap = (int)gcap; a.wp_kt_log2 = kl; a.wp_warps = warps; a.wp_dense = 0; a.wp_dense_sub = 0; }
 }
 
 int select_agg_launch(const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp, const AggEnv& env, AggArgs& a,
@@ -202,33 +174,29 @@ int select_agg_launch(const Compiled& c, const DevCol* cols, int64_t nrows, bool
         a.smem_cap_log2 = pick_smem_log2(env, a.plan.n_keyw, a.n_smem_lanes, true, na);
         if (a.smem_cap_log2 <= 0) { a.lean = 0; a.smem_paired = 0; return BKGPU_ENOMEM; }
         // FX: plain batches (no NULLs, no MIN / MAX) with at least one double sum, when the extension limbs fit beside table and queues
-        if (env.lean_fx && !env.fx_off && !env.lean_bank && !mm && !any_valid && nf64 >= 1 && nrows < ((int64_t)1 << 31)) {
+        if (env.lean_fx && !env.fx_off && !mm && !any_valid && nf64 >= 1 && nrows < ((int64_t)1 << 31)) {
             const size_t base = direct_smem_bytes(a.smem_keyw, a.n_smem_lanes, a.smem_cap_log2, na);
             if (base + fx_ext_bytes(na, a.smem_cap_log2) <= (size_t)224 * 1024) { a.lean_fx = 1; a.fx_ext_off = (uint32_t)base; }   // (227 KB per CTA less the kernel's 1 KB of static shared memory)
         }
     }
-    if (jp) { if (!a.lean) return 1; a.jp = *jp; a.jp_pipeline = env.join_pipeline; }
-    a.scalar_tma = env.scalar_tma; a.lean_bank = env.lean_bank;
-    a.wp = 0;
-    if (a.lean && !a.lean_nulls && !a.lean_mm && env.use_wp && c.direct.n_vals <= 2) plan_wp(c, env, a);
+    if (jp) { if (!a.lean) return 1; a.jp = *jp; }
+    a.scalar_tma = env.scalar_tma;
 
     const bool grouped = a.plan.n_keyw > 0;
     const int na = c.direct.n_vals;
     if (!direct) out.kernel = INTERP;
     else if (!grouped) out.kernel = env.scalar_tma && count_where_tma_shape(a) ? COUNT_WHERE_TMA : SCALAR_DIRECT;
-    else if (a.wp) out.kernel = WP;
     else if (!a.lean) out.kernel = GROUP_DIRECT;
     else if (a.lean_mm) out.kernel = LEAN_MM;   // (one MM / NULLS instantiation serves batches with and without NULLs)
     else if (a.lean_nulls) out.kernel = LEAN_NULLS;
     else if (a.lean_fx) out.kernel = a.jp.mode ? LEAN_FX_JOIN : LEAN_FX;
     else if (a.jp.mode) out.kernel = LEAN_JOIN;
-    else if (a.lean_bank && na <= 2) out.kernel = LEAN_BANK;
     else out.kernel = LEAN;
-    if (!grouped || out.kernel == COUNT_WHERE_TMA || out.kernel == WP) out.smem = 0;
+    if (!grouped || out.kernel == COUNT_WHERE_TMA) out.smem = 0;
     else if (!direct) out.smem = agg_smem_bytes(a.smem_keyw, a.n_smem_lanes, a.smem_cap_log2);
     else out.smem = direct_smem_bytes(a.smem_keyw, a.n_smem_lanes, a.smem_cap_log2, na) + (a.lean_fx ? fx_ext_bytes(na, a.smem_cap_log2) : 0);
     // a lean launch on one rank whose rows go straight to the host extracts its own result: any of them may be the request's last
-    out.fused_ok = direct && a.lean && !a.wp && grouped && !env.multi_rank && !env.has_post;
+    out.fused_ok = direct && a.lean && grouped && !env.multi_rank && !env.has_post;
     return BKGPU_OK;
 }
 

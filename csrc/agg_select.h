@@ -18,8 +18,6 @@ enum AggKernel : int {
     LEAN_FX,           // ... double sums as fixed-point limbs
     LEAN_JOIN,         // ... with the fused FK -> PK probe
     LEAN_FX_JOIN,      // ... FX and the fused probe
-    LEAN_BANK,         // ... bank-aware drain (option lean_bank)
-    WP,                // k_agg_group_wp: warp-private tables (agg_wp.cuh)
 };
 
 // the name bkgpu_stats.main_kernel_name reports for a launch of `k`
@@ -28,11 +26,9 @@ const char* agg_kernel_name(AggKernel k);
 // what the choice reads from the plan object: its options and the state learned from earlier launches
 struct AggEnv {
     int force_generic = 0, no_lean = 0, no_lean_nulls = 0, no_lean_mm = 0;
-    int lean_fx = 0, fx_off = 0, lean_bank = 0;
-    int use_wp = 0, wp_warps = 0, wp_kt_log2 = 0;
+    int lean_fx = 0, fx_off = 0;
     int scalar_tma = 0;
     int smem_cap_log2 = -1;       // -1 = chosen per batch from known_groups
-    int join_pipeline = 0;
     bool tail_launch = false;     // the outer-join tail: its probe-side columns are NULL on every row
     uint32_t known_groups = 0;    // groups seen by earlier launches of the plan
     bool multi_rank = false;      // the result is merged across ranks
@@ -41,7 +37,7 @@ struct AggEnv {
 
 struct AggSelection {
     AggKernel kernel = INTERP;
-    size_t smem = 0;              // dynamic shared memory of the INTERP and direct kernels (TMA and WP size their own)
+    size_t smem = 0;              // dynamic shared memory of the INTERP and direct kernels (TMA sizes its own)
     bool fused_ok = false;        // the launch may extract its own result (fused_extract): the caller still has to get the buffer
 };
 

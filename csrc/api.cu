@@ -195,8 +195,6 @@ extern "C" int bkgpu_set_option(bkgpu_plan* p, const char* key, int64_t v) {
     else if (k == "partial_capacity") { if (v < 1) return p->fail(BKGPU_EINVAL, "partial_capacity must be positive"); p->partial_cap = v; }
     else if (k == "force_generic") p->force_generic = v != 0;
     else if (k == "no_stream_copy") p->no_stream_copy = v != 0;
-    else if (k == "join_pipeline") p->join.pipeline = v != 0;
-    else if (k == "lean_bank") p->lean_bank = v != 0;
     else if (k == "lean_fx") p->lean_fx = v != 0;
     else if (k == "blocking_sync") p->blocking_sync = (int)v;
     else if (k == "star_expand_capacity") { if (v < 0 || v > 0x7FFFFFFF) return p->fail(BKGPU_EINVAL, "star_expand_capacity out of range"); p->join.star_expand_cap = (int)v; }
@@ -206,11 +204,8 @@ extern "C" int bkgpu_set_option(bkgpu_plan* p, const char* key, int64_t v) {
     else if (k == "peer_merge") p->peer_merge = v != 0;
     else if (k == "no_lean_nulls") p->no_lean_nulls = v != 0;
     else if (k == "no_lean_mm") p->no_lean_mm = v != 0;
-    else if (k == "use_wp") p->use_wp = v != 0;
     else if (k == "no_bounce") p->no_bounce = v != 0;
     else if (k == "scalar_tma") p->scalar_tma = v != 0;
-    else if (k == "wp_warps") { if (v != 0 && v != 8 && v != 12 && v != 16) return p->fail(BKGPU_EINVAL, "wp_warps: 0, 8, 12 or 16"); p->wp_warps = (int)v; }
-    else if (k == "wp_kt_log2") { if (v < 0 || v > 14) return p->fail(BKGPU_EINVAL, "wp_kt_log2 out of range"); p->wp_kt_log2 = (int)v; }
     else if (k == "output_on_device") p->output_on_device = v != 0;
     else if (k == "region_base") p->region_base = v;
     else return p->fail(BKGPU_EINVAL, "unknown option '%s'", key);
@@ -321,12 +316,11 @@ static bool ensure_fused(bkgpu_plan* p) {
 int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp) {
     AggEnv env;
     env.force_generic = p->force_generic; env.no_lean = p->no_lean; env.no_lean_nulls = p->no_lean_nulls; env.no_lean_mm = p->no_lean_mm;
-    env.lean_fx = p->lean_fx; env.fx_off = p->fx_off; env.lean_bank = p->lean_bank;
-    env.use_wp = p->use_wp; env.wp_warps = p->wp_warps; env.wp_kt_log2 = p->wp_kt_log2;
-    env.scalar_tma = p->scalar_tma; env.smem_cap_log2 = p->smem_cap_log2; env.join_pipeline = p->join.pipeline;
+    env.lean_fx = p->lean_fx; env.fx_off = p->fx_off;
+    env.scalar_tma = p->scalar_tma; env.smem_cap_log2 = p->smem_cap_log2;
     env.tail_launch = p->join.tail_launch;
     env.multi_rank = p->nccl_comm && p->nranks > 1; env.has_post = p->c.post != nullptr;
-    if (c.ap.n_keyw > 0 && (p->smem_cap_log2 < 0 || p->use_wp)) learn_groups(p);   // (the shared and warp-private tables are sized from it)
+    if (c.ap.n_keyw > 0 && p->smem_cap_log2 < 0) learn_groups(p);   // (the shared table is sized from it)
     env.known_groups = p->known_groups;
     AggArgs a; AggSelection sel;
     const int rc = select_agg_launch(c, cols, nrows, vec_ok, jp, env, a, sel);

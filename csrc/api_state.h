@@ -63,7 +63,6 @@ struct JoinState {
     uint32_t* tuples[2] = {nullptr, nullptr}; size_t tuples_cap[2] = {0, 0};   // star join: row-id tuples of one chunk (probe / expansion ping-pong)
     std::vector<ChunkCol> chunk;   // the gathered chunk (two-table gather path, star join), per plan column
     // options
-    int pipeline = 0;            // "join_pipeline": the fused probe issues its lookups one drain ahead (no gain while the kernel is bound by its shared-memory atomics)
     int no_fused_probe = 0;
     int star_expand_cap = 0;     // test option "star_expand_capacity": first capacity (tuples) of a star join's expansion pass (0 = twice its input)
 };
@@ -131,13 +130,9 @@ struct bkgpu_plan {
     uint8_t* h_fused = nullptr; uint8_t* d_fused = nullptr; size_t fused_bytes = 0; uint32_t fused_cap = 0; bool fused_last = false;
     JoinState join;               // hash join (K4): PK_JOIN_AGG, PK_JOIN, PK_STAR_AGG
     int fx_off = 0;               // set when a finished request saw more than 1/64 of its surviving rows take FX's exact path (see agg_finish)
-    int lean_bank = 0;            // opt-in: bank-aware dealing of the lean kernel's drain (agg_direct.cuh, BANK)
     int lean_fx = [] { const char* e = getenv("BKGPU_LEAN_FX"); return e ? atoi(e) != 0 : BK_LEAN_FX_DEFAULT; }();   // double sums as fixed-point limbs with native shared atomics (agg_direct.cuh, FX); option lean_fx
     int blocking_sync = -1; bool blocking_wait = false; cudaEvent_t wait_event = nullptr;   // see agg_finish
     int no_lean_nulls = 0, no_lean_mm = 0;
-    int use_wp = 0;               // 1 = launch the warp-private aggregate kernel where the batch fits it (opt-in: k_agg_group_lean is the default)
-    int wp_kt_log2 = 0;           // log2 words of the warp-private kernel's key table (0 = sized from the cardinality)
-    int wp_warps = 0;             // warps per CTA of the warp-private kernel (0 = chosen from the table size; 8, 12 or 16)
     // sort / filter state
     SortState* sort = nullptr;
     // host staging for pageable / pinned pushes

@@ -7,7 +7,9 @@
 //              shared-memory ring; each stage has a FULL mbarrier (armed with expect_tx, completed by the copy engine) and an EMPTY
 //              mbarrier (one arrival per consumer thread)
 //   consumers: all 256 threads wait on FULL (mbarrier.try_wait.parity), read the tile with conflict-free LDS.128, evaluate the
-//              predicate ((x ^ m) <u t) != flip (agg_wp.cuh's folding of the six comparison operators), arrive on EMPTY
+//              predicate ((x ^ m) <u t) != flip, arrive on EMPTY.  All six comparison operators fold into that one unsigned compare:
+//              EQ / NE test (x ^ c) <u 1, LT / GE compare in the sign-biased domain (m = 2^31), LE / GT use c + 1 there
+//              (c = INT32_MAX: a constant result)
 // Replaces FilterNode::need_copy + AggFnCall::update(COUNT_STAR) for one batch (src/exec/filter_node.cpp:726-795,
 // src/expr/agg_fn_call.cpp:496-555), like k_agg_scalar_direct<1, 0>.
 #include "agg.h"

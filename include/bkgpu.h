@@ -112,16 +112,13 @@ int   bkgpu_init(bkgpu_plan** out, const uint8_t* plan_desc, size_t len,
  *   "repartition"          with a communicator: groups are hash-partitioned across the ranks by one all-to-all (ncclSend/ncclRecv)
  *                          instead of gathered everywhere; each rank then returns only the groups it owns (high-cardinality GROUP BY)
  *   "force_generic" / "no_lean" / "no_lean_nulls" / "no_lean_mm" / "no_fused_probe"   pin the kernel variant (tests, A/B measurements)
- *   "use_wp" / "wp_warps" / "wp_kt_log2"   opt into the warp-private (atomics-free) aggregate kernel and size it (csrc/agg_wp.cuh)
  *   "scalar_tma"           0 = COUNT(*) WHERE int32 <cmp> c takes the LDG kernel instead of the TMA-staged one (csrc/scalar_tma.cu; default 1)
  *   "no_bounce"            pageable host input goes straight to cudaMemcpyAsync instead of the threaded pinned bounce buffers (A/B)
  *   "no_stream_copy"       the bounce copy uses memcpy instead of non-temporal stores (A/B)
- *   "join_pipeline"        (default 0) the fused FK->PK probe issues its lookups one drain ahead (opt-in)
  *   "star_expand_capacity" (tests) first capacity, in row-id tuples, of a star join's expansion pass over a dimension with duplicate keys
  *                          (0 = twice the pass's input); a pass that outgrows it is counted, grown to the exact count and run again
  *   "blocking_sync"        the wait for a request's result: 0 spins (cudaStreamSynchronize), 1 sleeps on a blocking-sync event, -1 (default) sleeps only
  *                          when several ranks share a small CPU budget (ranks > 1 and budget < 4 CPUs per rank)
- *   "lean_bank"            (default 0) the lean kernel deals each drained pass to lanes by shared-memory bank group (opt-in)
  *   "lean_fx"              (default 1; environment BKGPU_LEAN_FX) SUM / AVG over DOUBLE columns in the lean kernel accumulate as fixed-point
  *                          limbs with native 32-bit shared-memory atomics (csrc/fx.h: every value keeps >= 27 significant bits, typically
  *                          1e-13 of sum|x|; 0 = IEEE adds through 64/128-bit compare-and-swap loops); bkgpu_stats.main_kernel_name says

@@ -196,16 +196,6 @@ def c2_cas():
 
 
 @case(["0_1"])
-def c2_bank():
-    return c2({"lean_bank": 1})
-
-
-@case(["0_1"])
-def c2_wp():
-    return c2({"use_wp": 1}, n_groups=50)
-
-
-@case(["0_1"])
 def c2_no_lean():
     return c2({"no_lean": 1})
 

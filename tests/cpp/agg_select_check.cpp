@@ -15,7 +15,7 @@
 using namespace bk;
 
 static const char* const kKernels[] = {"INTERP", "SCALAR_DIRECT", "COUNT_WHERE_TMA", "GROUP_DIRECT", "LEAN", "LEAN_NULLS", "LEAN_MM",
-                                       "LEAN_FX", "LEAN_JOIN", "LEAN_FX_JOIN", "LEAN_BANK", "WP"};
+                                       "LEAN_FX", "LEAN_JOIN", "LEAN_FX_JOIN"};
 
 static int col_index(const Compiled& c, const std::string& name) {
     for (size_t i = 0; i < c.cols.size(); i++)
@@ -60,8 +60,7 @@ int main(int argc, char** argv) {
     }
     struct { const char* name; int* field; } ints[] = {
         {"force_generic", &env.force_generic}, {"no_lean", &env.no_lean}, {"no_lean_nulls", &env.no_lean_nulls}, {"no_lean_mm", &env.no_lean_mm},
-        {"lean_fx", &env.lean_fx}, {"fx_off", &env.fx_off}, {"lean_bank", &env.lean_bank}, {"use_wp", &env.use_wp}, {"wp_warps", &env.wp_warps},
-        {"wp_kt_log2", &env.wp_kt_log2}, {"scalar_tma", &env.scalar_tma}, {"smem_cap_log2", &env.smem_cap_log2}, {"join_pipeline", &env.join_pipeline}};
+        {"lean_fx", &env.lean_fx}, {"fx_off", &env.fx_off}, {"scalar_tma", &env.scalar_tma}, {"smem_cap_log2", &env.smem_cap_log2}};
     for (int k = 2; k < argc; k++) {
         const std::string arg = argv[k];
         const size_t eq = arg.find('=');
@@ -107,6 +106,5 @@ int main(int argc, char** argv) {
     printf("smem_cap_log2=%d\nn_smem_lanes=%d\nsmem_lane=", a.smem_cap_log2, a.n_smem_lanes);
     for (int l = 0; l < a.plan.n_lanes; l++) printf(l ? ",%d" : "%d", a.smem_lane[l] == 0xFF ? -1 : (int)a.smem_lane[l]);
     printf("\nlean=%d\nlean_fx=%d\nfx_ext_off=%u\n", a.lean, a.lean_fx, a.fx_ext_off);
-    printf("wp=%d\nwp_gcap=%d\nwp_kt_log2=%d\nwp_warps=%d\n", a.wp, a.wp_gcap, a.wp_kt_log2, a.wp_warps);
     return 0;
 }

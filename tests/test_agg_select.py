@@ -56,20 +56,6 @@ def scalar_sum_plan():
     return P.Plan(P.packet(root), {0: [(1, T.INT32), (2, T.INT32), (3, T.DOUBLE), (4, T.DOUBLE)], 1: P.agg_tuple_slots(aggs, [T.DOUBLE])})
 
 
-def one_sum_plan():
-    """C2's key and filter with one SUM(double)"""
-    aggs = [P.agg_expr("count_star", 1, 1), P.agg_expr("sum", 1, 2, None, P.slot_ref(0, 3, T.DOUBLE))]
-    root = P.agg(P.where(P.scan(0), P.lt(P.slot_ref(0, 2, T.INT32), P.int_lit(1 << 19))), 1, [P.slot_ref(0, 1, T.INT32)], aggs)
-    return P.Plan(root, {0: [(1, T.INT32), (2, T.INT32), (3, T.DOUBLE)], 1: P.agg_tuple_slots(aggs, [T.INT64, T.DOUBLE])})
-
-
-def three_sums_plan():
-    aggs = [P.agg_expr("count_star", 1, 1)] + [P.agg_expr("sum", 1, 2 + i, None, P.slot_ref(0, 3 + i, T.DOUBLE)) for i in range(3)]
-    root = P.agg(P.where(P.scan(0), P.lt(P.slot_ref(0, 2, T.INT32), P.int_lit(1 << 19))), 1, [P.slot_ref(0, 1, T.INT32)], aggs)
-    return P.Plan(root, {0: [(1, T.INT32), (2, T.INT32), (3, T.DOUBLE), (4, T.DOUBLE), (5, T.DOUBLE)],
-                         1: P.agg_tuple_slots(aggs, [T.INT64, T.DOUBLE, T.DOUBLE, T.DOUBLE])})
-
-
 def c3_min_max_plan():
     aggs = [P.agg_expr("count_star", 2, 1), P.agg_expr("sum", 2, 2, None, P.slot_ref(0, 2, T.DOUBLE)), P.agg_expr("min", 2, 3, None, P.slot_ref(0, 2, T.DOUBLE))]
     j = P.join(P.scan(1), P.scan(0), [P.eq(P.slot_ref(1, 1, T.INT32), P.slot_ref(0, 1, T.INT32))])
@@ -108,7 +94,7 @@ def test_c2_default_is_fx_with_its_lane_layout(select):
     # {rows, -, sumA, -, sumB}: the two double sums share a 16-byte pair; the extension limbs sit behind table and queues
     assert (r["smem_cap_log2"], r["n_smem_lanes"], r["smem_lane"]) == ("11", "4", "0,-1,2,-1,3")
     assert (r["lean_fx"], r["fx_ext_off"], r["smem"]) == ("1", str(174592), str(174592 + 2 * 4 * 2048))
-    assert (r["wp"], r["fused_ok"]) == ("0", "1")
+    assert r["fused_ok"] == "1"
 
 
 @pytest.mark.parametrize("args,kernel", [
@@ -116,8 +102,8 @@ def test_c2_default_is_fx_with_its_lane_layout(select):
     ({"fx_off": 1}, "LEAN"),
     ({"nrows": 1 << 31}, "LEAN"),
     ({"nrows": (1 << 31) - 1}, "LEAN_FX"),
-    ({"lean_bank": 1}, "LEAN_BANK"),
-    ({"lean_bank": 1, "lean_fx": 0}, "LEAN_BANK"),
+    ({"fx_off": 1, "known_groups": 1000}, "LEAN"),
+    ({"lean_fx": 0, "known_groups": 1000}, "LEAN"),
     ({"no_lean": 1}, "GROUP_DIRECT"),
     ({"force_generic": 1}, "INTERP"),
     ({"vec_ok": 0}, "INTERP"),
@@ -185,40 +171,11 @@ def test_shared_table_size(select, args, log2, kernel):
     assert (r["smem_cap_log2"], r["kernel"]) == (log2, kernel)
 
 
-# ---- warp-private tables ----
-def test_wp_with_known_groups(select):
-    r = select(queries.c2_filter_groupby(), use_wp=1, known_groups=50)
-    assert (r["kernel"], r["name"], r["wp_gcap"], r["wp_kt_log2"], r["wp_warps"], r["fused_ok"]) == ("WP", "k_agg_group_wp", "64", "8", "8", "0")
-
-
-def test_wp_unknown_cardinality_takes_the_largest_table(select):
-    r = select(queries.c2_filter_groupby(), use_wp=1)
-    assert (r["kernel"], r["wp_gcap"], r["wp_kt_log2"], r["wp_warps"]) == ("WP", "1216", "12", "8")
-
-
-def test_wp_one_value_column(select):
-    r = select(one_sum_plan(), use_wp=1, known_groups=50)
-    assert (r["kernel"], r["wp_gcap"], r["wp_kt_log2"], r["wp_warps"]) == ("WP", "64", "8", "16")
-    r = select(one_sum_plan(), use_wp=1, known_groups=50, wp_warps=12, wp_kt_log2=10)
-    assert (r["kernel"], r["wp_gcap"], r["wp_kt_log2"], r["wp_warps"]) == ("WP", "64", "10", "12")
-
-
-def test_wp_options_on_two_value_columns(select):
-    r = select(queries.c2_filter_groupby(), use_wp=1, known_groups=50, wp_warps=12, wp_kt_log2=11)
-    assert (r["kernel"], r["wp_gcap"], r["wp_kt_log2"], r["wp_warps"]) == ("WP", "64", "11", "8")
-
-
-def test_wp_not_for_three_value_columns(select):
-    r = select(three_sums_plan(), use_wp=1, known_groups=50)
-    assert (r["kernel"], r["wp"], r["fused_ok"]) == ("LEAN_FX", "0", "1")
-
-
 # ---- C3: the FK -> PK probe fused into the lean kernel ----
 def test_c3_fused_probe(select):
     r = select(queries.c3_join_groupby(), fused=1)
     assert (r["rc"], r["kernel"], r["name"], r["fused_ok"]) == ("0", "LEAN_FX_JOIN", "k_agg_group_lean_fx", "1")
     assert select(queries.c3_join_groupby(), fused=1, lean_fx=0)["kernel"] == "LEAN_JOIN"
-    assert select(queries.c3_join_groupby(), fused=1, use_wp=1, known_groups=50)["kernel"] == "WP"
 
 
 @pytest.mark.parametrize("plan,args", [(queries.c3_join_groupby, {"valid": "0_2"}), (c3_min_max_plan, {}), (queries.c3_join_groupby, {"no_lean": 1})])
@@ -236,7 +193,7 @@ def test_c3_general_probe_is_the_interpreter(select):
     (queries.c2_filter_groupby, {"multi_rank": 1}, "0"),
     (lambda: c2_with("having"), {}, "0"),
     (lambda: c2_with("sort"), {}, "0"),
-    (queries.c2_filter_groupby, {"use_wp": 1, "known_groups": 50}, "0"),
+    (queries.c2_filter_groupby, {"force_generic": 1}, "0"),
     (queries.c2_filter_groupby, {"no_lean": 1}, "0"),
 ])
 def test_fused_extraction(select, plan, args, fused):

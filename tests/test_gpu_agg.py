@@ -4,8 +4,10 @@ import pytest
 
 from baikaldb_b200 import datagen, plan as P, queries
 from baikaldb_b200.column import make_column
+from baikaldb_b200.exec_node import ColumnSource, GpuExecNode, RowBatch, RuntimeState
 from baikaldb_b200.plan import PrimitiveType as T
-from tests.util import LEAN_KERNELS, run_both
+from tests.util import LEAN_KERNELS, assert_same_rows, run_both
+from oracle import oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -20,14 +22,16 @@ def test_c1_count_where():
     assert stats.main_kernel_name.decode() == "k_agg_scalar_direct" and stats.rows_filtered == want.rows_filtered
 
 
-@pytest.mark.parametrize("n", [1, 3, 4, 5, 127, 128, 129, 1000, 65537, 300_003])
-@pytest.mark.parametrize("variant", ["wp", "lean", "direct", "bank"])
+@pytest.mark.parametrize("n", [1, 2, 3, 4, 5, 127, 128, 129, 1000, 2048, 2560, 2561, 65537, 300_003])
+@pytest.mark.parametrize("variant", ["lean", "direct", "cas"])
 def test_c2_sizes(n, variant):
-    """ragged sizes around the 4-rows-per-lane / 128-rows-per-warp boundaries: warp-private, lean and general direct kernels"""
+    """ragged sizes around the 4-rows-per-lane / 128-rows-per-warp boundaries and one CTA's first trip (2048 rows for the general direct
+    kernel's 512 threads, 2560 for the lean kernel's 640): the lean kernel (FX by default, the CAS path with lean_fx=0) and the general
+    direct kernel"""
     cols = datagen.c2_table(0, n, n_groups=50)
-    opts = {"wp": {"use_wp": 1}, "lean": {}, "direct": {"no_lean": 1}, "bank": {"lean_bank": 1, "lean_fx": 0}}[variant]
+    opts = {"lean": {}, "direct": {"no_lean": 1}, "cas": {"lean_fx": 0}}[variant]
     _, stats, _ = run_both(queries.c2_filter_groupby(), cols, keys=["0_1"], options=opts)
-    assert stats.main_kernel_name.decode() in {"wp": ("k_agg_group_wp",), "lean": ("k_agg_group_lean", "k_agg_group_lean_fx"), "direct": ("k_agg_group_direct",), "bank": ("k_agg_group_lean",)}[variant]
+    assert stats.main_kernel_name.decode() in {"lean": LEAN_KERNELS, "direct": ("k_agg_group_direct",), "cas": ("k_agg_group_lean",)}[variant]
 
 
 def test_lean_int64_key_and_integer_sums():
@@ -273,10 +277,99 @@ def test_literal_wider_than_the_column_keeps_its_value(variant):
     assert sum({c.name: c for c in got}["1_1"].to_list()) == int(cols[0].valid.sum())
 
 
-@pytest.mark.parametrize("n_groups", [7, 1000, 5000])
-def test_lean_bank_dealing_gives_the_same_groups(n_groups):
-    """option lean_bank: the drain deals each pass's entries to lanes by the bank group of their home slot (and lets the fifth entry of a
-    bank group be served by its own lane): same rows as the oracle at low, C2 and table-overflowing cardinalities, 0 % .. 100 % selectivity"""
-    for k in (0, 1 << 19, 1 << 21):
-        cols = datagen.c2_table(3, 250_003, n_groups=n_groups)
-        run_both(queries.c2_filter_groupby(k), cols, keys=["0_1"], options={"lean_bank": 1})
+# ---- the lean kernel at its edges: key-table inserts and overflow, few and many groups, learned cardinality, value shapes, every
+# comparison operator of the filter ----
+@pytest.mark.parametrize("n_groups", [1, 2, 7, 33, 1000, 1100, 1500, 5000, 40_000])
+def test_lean_cardinalities(n_groups):
+    """1..40k groups: few groups = every lane of a warp updates the same slot; 5000+ = more groups than the shared table sized before any
+    cardinality is known holds (the rest take the global path); the result never depends on which path a row took"""
+    cols = datagen.c2_table(0, 300_000, n_groups=n_groups)
+    _, stats, _ = run_both(queries.c2_filter_groupby(), cols, keys=["0_1"])
+    assert stats.main_kernel_name.decode() in LEAN_KERNELS
+
+
+@pytest.mark.parametrize("n_groups", [50, 1000, 3000])
+def test_lean_second_run_uses_learned_cardinality(n_groups):
+    """prepared-statement reuse: the second run sizes the shared table from the first run's group count; same rows every time"""
+    cols = datagen.c2_table(0, 200_000, n_groups=n_groups)
+    pl = queries.c2_filter_groupby()
+    want = oracle.execute(pl.serialize(), cols)
+    node, st = GpuExecNode(), RuntimeState(device=0, options={})
+    node.init(pl)
+    node.add_child(ColumnSource([cols]))
+    try:
+        assert node.open(st) == 0, st.error_msg
+        for run in range(3):
+            if run:
+                node.reset()
+                node.push(cols)
+                node.finish()
+            got, eos, rb = [], False, RowBatch()
+            while not eos:
+                rc, eos = node.get_next(st, rb)
+                assert rc == 0
+                got = got or list(rb.columns)
+            assert_same_rows(got, want.columns, ["0_1"])
+            # (3000 groups do not fit the lean kernel's shared table: once the cardinality is known the general direct kernel takes over)
+            name = node.stats().main_kernel_name.decode()
+            assert name in LEAN_KERNELS if (n_groups <= 1000 or run == 0) else name in LEAN_KERNELS + ("k_agg_group_direct",)
+    finally:
+        node.close(st)
+
+
+def test_lean_sparse_and_negative_keys():
+    rng = np.random.default_rng(5)
+    n = 150_000
+    keys = rng.choice(np.array([-(1 << 31), -1, 0, 1, (1 << 31) - 1, 123456789, -987654321] + list(rng.integers(-(1 << 31), 1 << 31, 500))), n)
+    cols = [make_column(0, 1, T.INT32, keys), make_column(0, 2, T.INT32, rng.integers(0, 1 << 20, n)),
+            make_column(0, 3, T.DOUBLE, rng.random(n)), make_column(0, 4, T.DOUBLE, rng.normal(size=n) * 1e3)]
+    _, stats, _ = run_both(queries.c2_filter_groupby(), cols, keys=["0_1"])
+    assert stats.main_kernel_name.decode() in LEAN_KERNELS
+
+
+def test_lean_uint32_key_with_all_ones():
+    rng = np.random.default_rng(6)
+    n = 90_000
+    keys = rng.choice(np.array([0xFFFFFFFF, 0xFFFFFFFE, 0xFFFFFFF0, 0, 1, 0x80000000], dtype=np.uint32), n)
+    cols = [make_column(0, 1, T.UINT32, keys), make_column(0, 2, T.DOUBLE, rng.random(n))]
+    aggs = [P.agg_expr("count_star", 1, 1), P.agg_expr("sum", 1, 2, None, P.slot_ref(0, 2, T.DOUBLE))]
+    pl = P.Plan(P.agg(P.scan(0), 1, [P.slot_ref(0, 1, T.UINT32)], aggs), {0: [(1, T.UINT32), (2, T.DOUBLE)], 1: P.agg_tuple_slots(aggs, [T.INT64, T.DOUBLE])})
+    _, stats, _ = run_both(pl, cols, keys=["0_1"])
+    assert stats.main_kernel_name.decode() in LEAN_KERNELS
+
+
+@pytest.mark.parametrize("shape", ["count_only", "one_double", "one_int64", "int64_and_double", "two_int64"])
+def test_lean_value_shapes(shape):
+    rng = np.random.default_rng(len(shape))
+    n = 120_001
+    cols = [make_column(0, 1, T.INT32, rng.integers(0, 300, n)), make_column(0, 2, T.INT32, rng.integers(0, 100, n)),
+            make_column(0, 3, T.DOUBLE, rng.normal(size=n)), make_column(0, 4, T.INT64, rng.integers(-(1 << 61), 1 << 61, n)),
+            make_column(0, 5, T.INT64, rng.integers(-5, 5, n))]
+    d, i1, i2 = P.slot_ref(0, 3, T.DOUBLE), P.slot_ref(0, 4, T.INT64), P.slot_ref(0, 5, T.INT64)
+    aggs = {"count_only": [P.agg_expr("count_star", 1, 1)],
+            "one_double": [P.agg_expr("count_star", 1, 1), P.agg_expr("avg", 1, 2, 3, d)],
+            "one_int64": [P.agg_expr("sum", 1, 1, None, i1)],
+            "int64_and_double": [P.agg_expr("sum", 1, 1, None, i1), P.agg_expr("sum", 1, 2, None, d), P.agg_expr("count_star", 1, 3)],
+            "two_int64": [P.agg_expr("sum", 1, 1, None, i1), P.agg_expr("sum", 1, 2, None, i2)]}[shape]
+    types = {"count_only": [T.INT64], "one_double": [T.INT64, T.DOUBLE], "one_int64": [T.INT64], "int64_and_double": [T.INT64, T.DOUBLE, T.INT64],
+             "two_int64": [T.INT64, T.INT64]}[shape]
+    root = P.agg(P.where(P.scan(0), P.lt(P.slot_ref(0, 2, T.INT32), P.int_lit(60))), 1, [P.slot_ref(0, 1, T.INT32)], aggs)
+    pl = P.Plan(root, {0: [(1, T.INT32), (2, T.INT32), (3, T.DOUBLE), (4, T.INT64), (5, T.INT64)], 1: P.agg_tuple_slots(aggs, types)})
+    _, stats, _ = run_both(pl, cols, keys=["0_1"])
+    assert stats.main_kernel_name.decode() in LEAN_KERNELS
+
+
+@pytest.mark.parametrize("op", ["eq", "ne", "lt", "le", "gt", "ge"])
+@pytest.mark.parametrize("c", [-(1 << 31), -7, 0, 41, (1 << 31) - 1])
+def test_lean_filter_operators(op, c):
+    """every comparison of `int32 column <cmp> constant` at the int32 limits"""
+    rng = np.random.default_rng(abs(c) % 1000 + len(op))
+    n = 50_000
+    f = rng.choice(np.array([-(1 << 31), -(1 << 31) + 1, -8, -7, -6, -1, 0, 1, 40, 41, 42, (1 << 31) - 2, (1 << 31) - 1]), n)
+    cols = [make_column(0, 1, T.INT32, rng.integers(0, 64, n)), make_column(0, 2, T.INT32, f), make_column(0, 3, T.DOUBLE, rng.random(n))]
+    aggs = [P.agg_expr("count_star", 1, 1), P.agg_expr("sum", 1, 2, None, P.slot_ref(0, 3, T.DOUBLE))]
+    pred = getattr(P, op)(P.slot_ref(0, 2, T.INT32), P.int_lit(c))
+    root = P.agg(P.where(P.scan(0), pred, P.ge(P.slot_ref(0, 1, T.INT32), P.int_lit(3))), 1, [P.slot_ref(0, 1, T.INT32)], aggs)
+    pl = P.Plan(root, {0: [(1, T.INT32), (2, T.INT32), (3, T.DOUBLE)], 1: P.agg_tuple_slots(aggs, [T.INT64, T.DOUBLE])})
+    _, stats, _ = run_both(pl, cols, keys=["0_1"])
+    assert stats.main_kernel_name.decode() in LEAN_KERNELS

@@ -55,7 +55,6 @@ def test_join_fused_probe_dense_with_gaps_negative_keys_and_ragged_tail(nf):
     _, stats, _ = run_both(queries.c3_join_groupby(), fact + dim, keys=["1_2"], batches=[dim, fact])
     if nf > 4:
         assert stats.main_kernel_name.decode() in LEAN_KERNELS
-    run_both(queries.c3_join_groupby(), fact + dim, keys=["1_2"], batches=[dim, fact], options={"join_pipeline": 1})   # the pipelined probe (opt-in)
 
 
 def test_c3_streamed_in_several_batches_host_and_build_first_rule():
@@ -120,7 +119,6 @@ def test_fused_probe_with_a_fact_side_filter(nf):
     _, stats, _ = run_both(pl, fact + dim, keys=["1_2"], batches=[dim, fact])
     assert stats.main_kernel_name.decode() in LEAN_KERNELS
     run_both(pl, fact + dim, keys=["1_2"], batches=[dim, fact], options={"no_fused_probe": 1})
-    run_both(pl, fact + dim, keys=["1_2"], batches=[dim, fact], options={"join_pipeline": 1})
 
 
 def _outer_join_tables(seed, nd=2_500, nf=40_000):

@@ -8,8 +8,8 @@ from baikaldb_b200.column import Column, rows_as_set
 from baikaldb_b200.exec_node import execute
 from oracle import oracle
 
-# names bkgpu_stats.main_kernel_name reports for the lean GROUP BY path (_fx: double sums as fixed-point limbs; wp: opt-in warp-private tables)
-LEAN_KERNELS = ("k_agg_group_lean", "k_agg_group_lean_fx", "k_agg_group_wp")
+# names bkgpu_stats.main_kernel_name reports for the lean GROUP BY path (_fx: double sums as fixed-point limbs)
+LEAN_KERNELS = ("k_agg_group_lean", "k_agg_group_lean_fx")
 REL_TOL = 1e-6  # north_star: SUM/AVG(double) within 1e-6 relative; everything integer bit-exact
 
 
