@@ -51,6 +51,7 @@ SYMBOLS = [
     ("bkgpu_release_cache", None, []),
     ("bkgpu_parse_datetime", c_int, [c_char_p, c_size_t, c_int, POINTER(c_uint64)]),
     ("bkgpu_cast_image", c_int, [c_uint64, c_int, c_int, POINTER(c_uint64)]),
+    ("bkgpu_hll_estimate", c_int, [c_char_p, c_size_t, POINTER(c_uint64)]),
     ("bkgpu_push_region", c_int, [c_void_p, c_int64]),
     ("bkgpu_partial_capacity", c_int, [c_void_p, POINTER(c_size_t)]),
     ("bkgpu_partial_export", c_int, [c_void_p, c_void_p, c_size_t]),

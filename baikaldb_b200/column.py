@@ -16,7 +16,7 @@ class Column:
     tuple_id: int
     slot_id: int
     prim_type: int
-    values: np.ndarray                     # storage dtype (see plan.storage_dtype); (n,16) u1 for AVG blobs
+    values: np.ndarray                     # storage dtype (see plan.storage_dtype); (n,16) u1 for AVG blobs, (n,16400) u1 for HLL sketches
     valid: Optional[np.ndarray] = None     # bool[n]; None = no NULLs
 
     @property
@@ -34,7 +34,7 @@ class Column:
 
     def to_list(self) -> list:
         v = self.values
-        if self.prim_type == PrimitiveType.STRING:
+        if self.prim_type in (PrimitiveType.STRING, PrimitiveType.HLL):
             out = [bytes(x) for x in v]
         else:
             out = v.tolist()
@@ -46,6 +46,8 @@ class Column:
 def make_column(tuple_id: int, slot_id: int, prim_type: int, values, valid=None) -> Column:
     if prim_type == PrimitiveType.STRING:
         arr = np.ascontiguousarray(values, dtype=np.uint8).reshape(-1, 16)
+    elif prim_type == PrimitiveType.HLL:   # RAW sketches (hll_add_agg's MERGE_AGG input): 16400 bytes each
+        arr = np.ascontiguousarray(values, dtype=np.uint8).reshape(-1, 16400)
     else:
         arr = np.ascontiguousarray(values, dtype=np.dtype(storage_dtype(prim_type)))
     v = None if valid is None else np.ascontiguousarray(valid, dtype=bool)

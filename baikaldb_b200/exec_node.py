@@ -123,7 +123,7 @@ def _marshal(cols: Sequence[AnyColumn]):
             vals = np.ascontiguousarray(c.values)
             bitmap = c.validity_bitmap()
             keep += [vals, bitmap]
-            arr[i].elem_size = 16 if c.prim_type == PrimitiveType.STRING else vals.dtype.itemsize
+            arr[i].elem_size = vals.shape[1] if c.prim_type in (PrimitiveType.STRING, PrimitiveType.HLL) else vals.dtype.itemsize
             arr[i].values = vals.ctypes.data
             arr[i].validity = bitmap.ctypes.data if bitmap is not None else None
             arr[i].length = len(c)
@@ -217,9 +217,10 @@ class GpuExecNode:
         n = nrows.value
         for i in range(ncols.value):
             oc = out[i]
-            if oc.prim_type == PrimitiveType.STRING:
-                raw = (ctypes.c_uint8 * (max(n, 1) * 16)).from_address(oc.values)
-                vals = np.frombuffer(raw, dtype=np.uint8, count=n * 16).reshape(n, 16).copy()
+            if oc.prim_type in (PrimitiveType.STRING, PrimitiveType.HLL):   # byte blobs: AVG's {sum, count}, hll_add_agg's RAW sketch
+                w = oc.elem_size
+                raw = (ctypes.c_uint8 * (max(n, 1) * w)).from_address(oc.values)
+                vals = np.frombuffer(raw, dtype=np.uint8, count=n * w).reshape(n, w).copy()
             else:
                 dt = np.dtype(storage_dtype(oc.prim_type))
                 raw = (ctypes.c_uint8 * (max(n, 1) * dt.itemsize)).from_address(oc.values)

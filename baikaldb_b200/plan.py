@@ -587,7 +587,7 @@ class Plan:
 def agg_tuple_slots(agg_fns: Sequence[Expr], arg_types: Sequence[int]) -> List[Tuple[int, int]]:
     """Slot types of the aggregate tuple, as AggFnCall::type_inferer(tuple_desc) assigns them
     (src/expr/agg_fn_call.cpp:87-122,176-200): COUNT -> INT64, SUM -> INT64/UINT64/DOUBLE by argument,
-    AVG -> final DOUBLE + intermediate STRING blob, MIN/MAX -> argument type."""
+    AVG -> final DOUBLE + intermediate STRING blob, MIN/MAX -> argument type, hll_add_agg -> HLL."""
     slots: Dict[int, int] = {}
     for f, at in zip(agg_fns, arg_types):
         name = f.name
@@ -602,6 +602,8 @@ def agg_tuple_slots(agg_fns: Sequence[Expr], arg_types: Sequence[int]) -> List[T
                 ft = T.INT64
         elif name == "avg":
             ft = T.DOUBLE
+        elif name == "hll_add_agg":
+            ft = T.HLL
         else:
             ft = at
         slots[f.final_slot_id] = int(ft)

@@ -3,7 +3,7 @@
 device-resident synthetic columns (SURVEY.md §8d), CUDA events around reset+push+finish+get_next, one JSON line per
 config with rows/s and achieved GB/s on the config's algorithmic bytes.  The headline line is bench.py's;
 this script measures the side configs on their own (C6, the star join, also its kernels, a parity flag and the Acero time).
-usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [c9] [c10] [c11] [c12] [--scale 0.1] [--steps 10]"""
+usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [c9] [c10] [c11] [c12] [c13] [--scale 0.1] [--steps 10]"""
 import argparse
 import ctypes
 import json
@@ -612,6 +612,55 @@ def c12(a):
     print(json.dumps(line), flush=True)
 
 
+def c13(a):
+    """C13, approximate distinct counts: hll_add_agg(x) over 100M device-resident rows, scalar and GROUP BY g (1000 groups), x INT64 uniform
+    over [0, 10,000).  Each line carries parity (every sketch byte-identical to tests/hll_oracle.py's numpy restatement of the reference) and
+    the estimate of the scalar sketch (bkgpu_hll_estimate).  Beside them, the exact COUNT(DISTINCT x)'s store-side level on the same rows
+    (the planner's two-level layout: GROUP BY [g,] x below a MERGE_AGG), whose cost grows with the distinct values."""
+    from baikaldb_b200 import plan as P
+    from baikaldb_b200.exec_node import DeviceColumn, execute
+    from tests import hll_cases as HC, hll_oracle as H
+    import subprocess
+    n = int(100_000_000 * a.scale)
+    specs = [(0, 1, T.INT32, 0, 1, 0, 1000, 1.0), (0, 2, T.INT64, 0, 2, 0, 10_000, 1.0)]
+    g, x = gen(n, specs[0], 13), gen(n, specs[1], 13)
+    arr = cols_array(specs, [g, x])
+    info = {"gpu": torch.cuda.get_device_name(0)}
+    try:
+        info["power_limit"] = subprocess.check_output(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"], text=True).split("\n")[0].strip()
+    except Exception:
+        info["power_limit"] = None
+    dev = [DeviceColumn(0, 1, int(T.INT32), g.data_ptr(), n, keepalive=g), DeviceColumn(0, 2, int(T.INT64), x.data_ptr(), n, keepalive=x)]
+    regs = H.registers(x.cpu().numpy(), T.INT64, g.cpu().numpy(), 1000)
+    tup = {0: [(1, T.INT32), (2, T.INT64)]}
+    for grouped in (False, True):
+        plan = HC.scan_plan(T.INT64, grouped=grouped)
+        plan.tuples[0] = tup[0]
+        line = run(f"C13 hll_add_agg(x){' GROUP BY g (1000 groups)' if grouped else ' scalar'}", plan, [(arr, 2, n)], n, 12 * n, a.steps, a.warmup, emit=False)
+        got, _ = execute(plan, dev)
+        cols = {c.name: c.to_list() for c in got}
+        if grouped:
+            line["parity_vs_numpy_oracle"] = all(s == H.raw_sketch(regs[k], True) for k, s in zip(cols["0_1"], cols[f"{HC.AGG_TUPLE}_1"])) and len(cols["0_1"]) == 1000
+        else:
+            sk = cols[f"{HC.AGG_TUPLE}_1"][0]
+            line["parity_vs_numpy_oracle"] = sk == H.raw_sketch(regs.max(axis=0), True)
+            est = ctypes.c_uint64(0)
+            _lib.check(L.bkgpu_hll_estimate(sk, len(sk), ctypes.byref(est)))
+            line["estimate"] = est.value
+            line["exact_distinct"] = int(torch.unique(x).numel())
+        line.update(info)
+        print(json.dumps(line), flush=True)
+    for grouped in (False, True):   # the exact count's first level: one group per distinct (g, x)
+        keys = ([P.slot_ref(0, 1, T.INT32)] if grouped else []) + [P.slot_ref(0, 2, T.INT64)]
+        aggs = [P.agg_expr("count_star", 1, 1)]
+        plan = P.Plan(P.agg(P.scan(0), 1, keys, aggs), {0: tup[0], 1: P.agg_tuple_slots(aggs, [T.INT64])})
+        line = run(f"C13 exact COUNT(DISTINCT x){' GROUP BY g' if grouped else ''}, store-side level: GROUP BY {'g, ' if grouped else ''}x", plan,
+                   [(arr, 2, n)], n, 12 * n, a.steps, a.warmup, options=[(b"group_capacity_log2", 24 if grouped else 15)], emit=False)
+        line.update(info)
+        print(json.dumps(line), flush=True)
+    del g, x
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("configs", nargs="*", default=["c1", "c3", "c5"])
@@ -677,6 +726,8 @@ def main():
         c11(a)
     if "c12" in a.configs:
         c12(a)
+    if "c13" in a.configs:
+        c13(a)
     if "c3" in a.configs:
         nf, nd = int(100_000_000 * a.scale), int(10_000_000 * a.scale)
         fs = [(0, 1, T.INT32, 0, 1, 0, nd, 1.0), (0, 2, T.DOUBLE, 1, 2, 0, 0, 1.0)]

@@ -22,10 +22,22 @@ namespace bk {
 // generic path: the lowered expression program (interp.cuh) is interpreted per row (any predicate,
 // computed keys and arguments, multi-column keys).
 // ------------------------------------------------------------------------------------------
+// the AG_HLL aggregates of one row that reached group `slot` (out of line: the other plans' interpreter keeps its registers)
+static __device__ __noinline__ void hll_row(const AggArgs& a, const uint64_t* out, uint32_t out_null, int slot) {
+    const AggPlan& ap = a.plan;
+    for (int i = 0; i < ap.n_agg; i++) {
+        const AggSpec s = ap.agg[i];
+        if (s.kind != AG_HLL || ((out_null >> s.arg_out) & 1u)) continue;
+        if (s.arg_prim == BK_HLL) hll_merge_value(a.gt, s, a.cols[s.hll_col], (int64_t)out[s.arg_out], a.gt.lanes, a.gt.cap_mask + 1, slot);
+        else hll_add_value(a.gt, s, a.gt.lanes, a.gt.cap_mask + 1, slot, out[s.arg_out]);
+    }
+}
 // one (possibly joined) row through the program into the tables
 struct InterpCtx { SmemTable st; bool grouped, use_smem; uint32_t gcap; };
 // how: 0 = filter, then aggregate the row; 1 = filter only (SEMI / ANTI probe: does the joined row satisfy the conditions?);
 //      2 = aggregate without the filter (the NULL-extended / preserved rows of the join's tail)
+// HLL: the plan has AG_HLL aggregates (the instantiation without them keeps the interpreter's registers as they were)
+template <bool HLL = false>
 __device__ __forceinline__ uint32_t interp_row(const AggArgs& a, const InterpCtx& cx, int64_t row, int64_t brow, int how = 0) {
     const AggPlan& ap = a.plan;
     const GroupTable& gt = a.gt;
@@ -39,8 +51,11 @@ __device__ __forceinline__ uint32_t interp_row(const AggArgs& a, const InterpCtx
         if (r == 0xFF) { v = 0; isnull = true; return; }
         v = out[r]; isnull = (out_null >> r) & 1u;
     };
+    // hll_add_agg (a plan with AG_HLL never uses the shared table: a sketch lives in the global table's arena)
+    auto hll = [&](int slot) { if (HLL) hll_row(a, out, out_null, slot); };
     if (!cx.grouped) {  // single group: slot 0 of the global table
         accumulate_row<false>(a, gt.lanes, cx.gcap, 0, arg);
+        hll(0);
         return 1;
     }
     uint64_t key[MAX_KEYW];
@@ -60,11 +75,12 @@ __device__ __forceinline__ uint32_t interp_row(const AggArgs& a, const InterpCtx
     else {
         slot = table_upsert<false, 0>(gt.state, gt.keys, gt.cap_mask, key, ap.n_keyw, h, (int)cx.gcap, gt.n_groups);
         if (slot < 0) atomicExch(gt.overflow, 1u);
-        else accumulate_row<false>(a, gt.lanes, cx.gcap, slot, arg);
+        else { accumulate_row<false>(a, gt.lanes, cx.gcap, slot, arg); hll(slot); }
     }
     return 1;
 }
 
+template <bool HLL>
 __global__ void __launch_bounds__(256) k_agg_interp(const __grid_constant__ AggArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const AggPlan& ap = a.plan;
@@ -79,11 +95,11 @@ __global__ void __launch_bounds__(256) k_agg_interp(const __grid_constant__ AggA
         const int jt = a.join.join_type;
         for (int64_t br = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; br < a.join.n_build; br += (int64_t)gridDim.x * blockDim.x) {
             const uint8_t m = a.join.matched[br];   // (2: removed by the build side's own filter, never emitted)
-            if (jt == 4 /*SEMI*/ ? m == 1 : m == 0) passed += interp_row(a, cx, -1, br, 2);
+            if (jt == 4 /*SEMI*/ ? m == 1 : m == 0) passed += interp_row<HLL>(a, cx, -1, br, 2);
         }
     } else
     for (int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; row < a.nrows; row += (int64_t)gridDim.x * blockDim.x) {
-        if (!a.join.enabled) { passed += interp_row(a, cx, row, -1); continue; }
+        if (!a.join.enabled) { passed += interp_row<HLL>(a, cx, row, -1); continue; }
         // K4 probe: every build row whose cast key equals this row's (Joiner::encode_hash_key + FlatMap seek,
         // src/exec/joiner.cpp:608-622, join_node.cpp:1290-1292); a NULL key never matches (SQL / Acero hashjoin)
         const DevCol& pc = a.cols[a.join.probe_col];
@@ -94,8 +110,8 @@ __global__ void __launch_bounds__(256) k_agg_interp(const __grid_constant__ AggA
             const uint32_t br = a.join.rows[slot];
             if (br == 0xFFFFFFFFu) break;
             if (a.join.keys[slot] == img) {
-                if (a.join.join_type == 3 /*INNER*/ || !a.join.matched) passed += interp_row(a, cx, row, (int64_t)br);
-                else if (a.join.join_type == 1 /*LEFT*/) { if (interp_row(a, cx, row, (int64_t)br)) { passed++; a.join.matched[br] = 1; } }
+                if (a.join.join_type == 3 /*INNER*/ || !a.join.matched) passed += interp_row<HLL>(a, cx, row, (int64_t)br);
+                else if (a.join.join_type == 1 /*LEFT*/) { if (interp_row<HLL>(a, cx, row, (int64_t)br)) { passed++; a.join.matched[br] = 1; } }
                 else if (interp_row(a, cx, row, (int64_t)br, 1)) a.join.matched[br] = 1;   // SEMI / ANTI_SEMI: only whether a partner exists
             }
             slot = (slot + 1) & a.join.cap_mask;
@@ -221,6 +237,7 @@ __global__ void k_table_init(GroupTable gt, AggPlan ap, int keep_overflow) {
     //  while rows were pushed, or an export that met more groups than the exchange format holds, must still fail the plan)
     if (blockIdx.x == 0 && threadIdx.x < GT_OCC_OFF && !keep_overflow) gt.n_groups[threadIdx.x] = 0;   // fresh request: every counter of the block
     if (blockIdx.x == 0 && threadIdx.x == 0 && keep_overflow) *gt.n_groups = 0;                          // mid-request re-initialisation (multi-GPU merge): the group count only
+    if (blockIdx.x == 0 && threadIdx.x < 3 && gt.hll_ctr && !(threadIdx.x >= 1 && keep_overflow)) gt.hll_ctr[threadIdx.x] = 0;   // (the sketch lanes are 0 again)
 }
 
 // walk the groups a table holds: the occupied list of a GROUP BY table (slots in insertion order), slot 0 of a scalar aggregate
@@ -238,6 +255,7 @@ __global__ void k_table_clear(GroupTable gt, AggPlan ap, uint32_t n) {
     }
     // (the counters can go in the same launch: nobody here reads them — `n` came by value, the occupied list sits behind them)
     if (blockIdx.x == 0 && threadIdx.x < GT_OCC_OFF) gt.n_groups[threadIdx.x] = 0;
+    if (blockIdx.x == 0 && threadIdx.x < 3 && gt.hll_ctr) gt.hll_ctr[threadIdx.x] = 0;
 }
 
 // Partial state layout (fixed capacity `pcap` groups): [u64 n_groups][keys n_keyw x pcap][lanes n_lanes x pcap]
@@ -260,7 +278,7 @@ __global__ void k_partial_count(uint64_t* dst, const uint32_t* cursor, uint32_t 
 // Only `1 + bound * row words` cross NVLink; `bound` follows the group counts seen in earlier runs (api.cu).
 __global__ void k_partial_export_rows(GroupTable gt, AggPlan ap, uint64_t* dst, uint32_t bound) {
     const uint32_t cap = gt.cap_mask + 1;
-    const int rw = ap.n_keyw + ap.n_lanes;
+    const int rw = ap.n_keyw + ap.n_lanes + ap.n_hll * HLL_ROW_WORDS;
     BK_FOR_EACH_GROUP(gt, ap, i) {
         if (ap.n_keyw == 0 && gt.lanes[i] == 0) continue;  // no row reached the single group
         const uint32_t pos = atomicAdd((uint32_t*)dst, 1u);
@@ -268,6 +286,37 @@ __global__ void k_partial_export_rows(GroupTable gt, AggPlan ap, uint64_t* dst, 
         uint64_t* row = dst + 1 + (size_t)pos * rw;
         for (int w = 0; w < ap.n_keyw; w++) row[w] = gt.keys[(size_t)w * cap + i];
         for (int l = 0; l < ap.n_lanes; l++) row[ap.n_keyw + l] = gt.lanes[(size_t)l * cap + i];
+        // each sketch's registers after the lanes, in aggregate order (all zero for a group without a value); its lane keeps only
+        // whether the group has a sketch: 0 none, 1 a sketch, 2 one this table lost to a full arena (the merger fails too).  A block
+        // index means nothing to another table
+        uint64_t* regs_out = row + ap.n_keyw + ap.n_lanes;
+        for (int k = 0; k < ap.n_agg; k++) {
+            if (ap.agg[k].kind != AG_HLL) continue;
+            const uint64_t ref = gt.lanes[(size_t)ap.agg[k].acc_lane * cap + i];
+            row[ap.n_keyw + ap.agg[k].acc_lane] = ref == 0 ? 0 : ref >= HLL_LANE_FULL ? 2 : 1;
+            const uint64_t* src = ref == 0 || ref >= HLL_LANE_FULL ? nullptr : (const uint64_t*)(gt.hll_regs + (size_t)(ref - 1) * HLL_REGISTERS);
+            for (int w = 0; w < HLL_ROW_WORDS; w++) regs_out[w] = src ? __ldcg((const unsigned long long*)src + w) : 0ull;
+            regs_out += HLL_ROW_WORDS;
+        }
+    }
+}
+// the sketches of an imported group row (k_partial_export_rows' layout) folded into the group at `slot`: register-wise max
+__device__ __forceinline__ void hll_merge_row(const AggPlan& ap, const GroupTable& gt, int slot, const uint64_t* row) {
+    const uint32_t cap = gt.cap_mask + 1;
+    const uint64_t* regs_in = row + ap.n_keyw + ap.n_lanes;
+    for (int k = 0; k < ap.n_agg; k++) {
+        if (ap.agg[k].kind != AG_HLL) continue;
+        const uint64_t has = row[ap.n_keyw + ap.agg[k].acc_lane];
+        if (has == 2) atomicExch(gt.hll_ctr + 1, 1u);   // (the exporting table's arena overflowed: this sketch would be truncated)
+        else if (has) {
+            uint8_t* regs = hll_sketch(gt, gt.lanes + (size_t)ap.agg[k].acc_lane * cap + slot);
+            if (regs)
+                for (int w = 0; w < 2 * HLL_ROW_WORDS; w++) {
+                    const unsigned int x = ((const unsigned int*)regs_in)[w];
+                    if (x) hll_max_word((unsigned int*)regs + w, x, __ldcg((const unsigned int*)regs + w));
+                }
+        }
+        regs_in += HLL_ROW_WORDS;
     }
 }
 // K3 on the gathered rows: every rank folds the OTHER ranks' groups into its own table (its own groups are already there), so
@@ -282,12 +331,18 @@ __global__ void k_partial_merge_rows(GroupTable gt, AggPlan ap, const uint64_t* 
     if (r == self) return;
     const uint64_t* base = src + (size_t)r * words_per_rank;
     const uint32_t n = (uint32_t)base[0];
-    const int rw = ap.n_keyw + ap.n_lanes;
+    const int rw = ap.n_keyw + ap.n_lanes + ap.n_hll * HLL_ROW_WORDS;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const uint64_t* row = base + 1 + (size_t)i * rw;
         uint64_t key[MAX_KEYW];
         for (int w = 0; w < ap.n_keyw; w++) key[w] = row[w];
-        merge_group(ap, gt, key, [&](int l, uint64_t& v) { v = row[ap.n_keyw + l]; return true; });
+        merge_group(ap, gt, key, [&](int l, uint64_t& v) { v = row[ap.n_keyw + l]; return ap.lane_op[l] != LN_HLL; });
+        if (ap.n_hll) {   // the group's slot, which merge_group has just found or inserted
+            const int slot = ap.n_keyw == 0 ? 0 : table_upsert<false, 0>(gt.state, gt.keys, gt.cap_mask, key, ap.n_keyw,
+                                                                       ap.n_keyw == 1 ? hash_key1(key[0]) : hash_key(key, ap.n_keyw),
+                                                                       (int)(gt.cap_mask + 1), gt.n_groups);
+            if (slot >= 0) hll_merge_row(ap, gt, slot, row);
+        }
     }
 }
 
@@ -436,15 +491,16 @@ cudaError_t launch_agg(const AggArgs& a, AggKernel k, size_t smem, int sm_count,
     if (a.nrows <= 0) return cudaSuccess;
     switch (k) {
         case INTERP: {
+            auto kern = a.gt.hll_regs ? k_agg_interp<true> : k_agg_interp<false>;
             if (smem > 48 * 1024) {
-                cudaError_t e = cudaFuncSetAttribute(k_agg_interp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+                cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
                 if (e != cudaSuccess) return e;
             }
-            int grid = occupancy_grid(k_agg_interp, smem, sm_count);
+            int grid = occupancy_grid(kern, smem, sm_count);
             int64_t want = (a.nrows + 255) / 256;
             if (want < grid) grid = (int)want;
             if (start) cudaEventRecord(start, s);
-            k_agg_interp<<<grid, 256, smem, s>>>(a);
+            kern<<<grid, 256, smem, s>>>(a);
             return cudaGetLastError();
         }
         case COUNT_WHERE_TMA: return launch_count_where_tma(a, sm_count, s, start);

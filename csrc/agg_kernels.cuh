@@ -3,6 +3,7 @@
 #pragma once
 #include "agg.h"
 #include "dev_common.cuh"
+#include "hll.cuh"
 
 namespace bk {
 
@@ -39,6 +40,7 @@ __device__ __forceinline__ void accumulate_row(const AggArgs& args, uint64_t* la
 // merge the lane values of one group (a shared-table slot or an imported partial) into the global
 // table: AggFnCall::merge (src/expr/agg_fn_call.cpp:779-822) lane by lane.  lane_val(l, v) yields
 // the value for global lane l or returns false when the source has nothing for it.
+// (a sketch lane, LN_HLL, has nothing to add here: the caller's lane_val skips it, and the sketch's registers travel apart)
 template <class LaneVal>
 __device__ __forceinline__ void merge_group(const AggPlan& ap, const GroupTable& gt, const uint64_t* key, LaneVal lane_val) {
     int slot = 0;
@@ -57,6 +59,74 @@ __device__ __forceinline__ void merge_group(const AggPlan& ap, const GroupTable&
         if (v == lane_identity(op)) continue;
         lane_atomic<false>(op, gt.lanes + (size_t)l * cap + slot, v);
     }
+}
+
+// ------------------------------------------------------------------------------------------
+// hll_add_agg (AG_HLL): a group's sketch is a 16384-byte block of the register arena, referenced by its lane as block + 1
+// ------------------------------------------------------------------------------------------
+// the registers of the sketch behind `lane`, claimed on first use: the first thread to CAS the lane from 0 takes the next block, zeroes it
+// and publishes it; others wait for the publication.  nullptr when the arena is full (hll_ctr[1] is then set and the request fails).
+static __device__ __noinline__ uint8_t* hll_sketch(const GroupTable& gt, uint64_t* lane) {
+    unsigned long long v = __ldcg((const unsigned long long*)lane);
+    if (v == 0) {
+        v = atomicCAS((unsigned long long*)lane, 0ull, (unsigned long long)HLL_LANE_BUSY);
+        if (v == 0) {
+            const uint32_t b = atomicAdd(gt.hll_ctr, 1u);
+            if (b >= gt.hll_cap) { atomicExch(gt.hll_ctr + 1, 1u); atomicExch((unsigned long long*)lane, (unsigned long long)HLL_LANE_FULL); return nullptr; }
+            uint4* r = (uint4*)(gt.hll_regs + (size_t)b * HLL_REGISTERS);
+            for (int i = 0; i < HLL_REGISTERS / 16; i++) __stcg(r + i, make_uint4(0u, 0u, 0u, 0u));
+            __threadfence();   // (the zeroed block before its reference)
+            atomicExch((unsigned long long*)lane, (unsigned long long)b + 1ull);
+            return (uint8_t*)r;
+        }
+    }
+    while (v == HLL_LANE_BUSY) { __nanosleep(64); v = __ldcg((const unsigned long long*)lane); }
+    if (v == HLL_LANE_FULL) return nullptr;
+    __threadfence();
+    return gt.hll_regs + (size_t)(v - 1) * HLL_REGISTERS;
+}
+// register = max(register, count) on the 32-bit word holding it.  The register is read first: once a sketch has filled up, almost
+// every row finds its register already as large and writes nothing.  Registers live in L2 (atomics and ld.cg), never in L1.
+__device__ __forceinline__ void hll_max_word(unsigned int* w, unsigned int want, unsigned int cur) {
+    for (;;) {
+        const unsigned int nv = __vmaxu4(cur, want);
+        if (nv == cur) return;
+        const unsigned int prev = atomicCAS(w, cur, nv);
+        if (prev == cur) return;
+        cur = prev;
+    }
+}
+__device__ __forceinline__ void hll_max_register(uint8_t* regs, uint32_t reg, uint32_t count) {
+    unsigned int* w = (unsigned int*)(regs + (reg & ~3u));
+    const uint32_t shift = (reg & 3u) * 8u;
+    const unsigned int cur = __ldcg(w);
+    if (((cur >> shift) & 0xFFu) < count) hll_max_word(w, count << shift, cur);
+}
+// MERGE_AGG: the RAW sketch at row `row` of column `c` into the sketch of `slot` (hll_merge_agg, hll_common.cpp:630-703): register-wise
+// max.  The group's sketch is claimed even when no register grows, as hll_merge_agg invalidates the cached cardinality whatever it merges.
+// A value whose magic or encoding is not RAW's sets hll_ctr[2] and the request fails (DENSE and SPARSE sketches vary in length)
+__device__ __forceinline__ void hll_merge_value(const GroupTable& gt, const AggSpec& a, const DevCol& c, int64_t row, uint64_t* lanes, uint32_t cap, int slot) {
+    const uint8_t* v = (const uint8_t*)c.values + (size_t)row * HLL_RAW_BYTES;
+    const uint32_t magic = __ldg((const uint32_t*)v), enc = __ldg(v + 4);
+    if (magic != 0x4C4C5948u /* "HYLL" */ || enc != HLL_ENC_RAW) { atomicExch(gt.hll_ctr + 2, 1u); return; }
+    uint8_t* regs = hll_sketch(gt, lanes + (size_t)a.acc_lane * cap + slot);
+    if (!regs) return;
+    const uint32_t* src = (const uint32_t*)(v + HLL_HDR_BYTES);   // (16400 and 16 are multiples of 16: every value is word-aligned)
+    unsigned int* dst = (unsigned int*)regs;
+    for (int w = 0; w < HLL_REGISTERS / 4; w++) {
+        const unsigned int x = __ldg(src + w);
+        if (!x) continue;
+        const unsigned int cur = __ldcg(dst + w);
+        if (__vmaxu4(cur, x) != cur) hll_max_word(dst + w, x, cur);
+    }
+}
+// one non-NULL argument value of an AG_HLL aggregate into the sketch of `slot`
+__device__ __forceinline__ void hll_add_value(const GroupTable& gt, const AggSpec& a, uint64_t* lanes, uint32_t cap, int slot, uint64_t v) {
+    if (a.arg_prim == BK_FLOAT && a.arg_vclass == VC_F64) v = __float_as_uint((float)bits_f64(v));   // (a computed FLOAT value: its float bytes)
+    uint32_t reg;
+    const int count = hll_pat_len(hll_hash(v, hll_key_bytes(a.arg_prim)), &reg);
+    uint8_t* regs = hll_sketch(gt, lanes + (size_t)a.acc_lane * cap + slot);
+    if (regs) hll_max_register(regs, reg, (uint32_t)count);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -143,7 +213,7 @@ __device__ __forceinline__ void extract_group(const GroupTable& gt, const AggPla
         switch (a.kind) {
             case AG_COUNT_STAR: v = nrows; break;
             case AG_COUNT: v = cnt; break;
-            case AG_COUNT_MERGE: v = acc; break;
+            case AG_COUNT_MERGE: case AG_HLL: v = acc; break;   // (AG_HLL: the sketch reference; the host copies its registers)
             case AG_AVG:
                 if (cnt == 0) isnull = 1; else v = f64_bits(__ddiv_rn(bits_f64(acc), (double)(int64_t)cnt));
                 break;

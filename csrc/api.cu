@@ -11,6 +11,7 @@
 #include <mutex>
 #include <thread>
 #include "api_state.h"
+#include "hll.cuh"
 #include "nccl_dl.h"
 #include "build_id.h"
 
@@ -192,6 +193,7 @@ extern "C" int bkgpu_set_option(bkgpu_plan* p, const char* key, int64_t v) {
     else if (k == "smem_capacity_log2") { if (v < -1 || v > 13) return p->fail(BKGPU_EINVAL, "smem_capacity_log2 out of range"); p->smem_cap_log2 = (int)v; }
     else if (k == "batch_capacity") { if (v < 1) return p->fail(BKGPU_EINVAL, "batch_capacity must be positive"); p->batch_capacity = v; }
     else if (k == "chunk_rows") { if (v < 1024) return p->fail(BKGPU_EINVAL, "chunk_rows too small"); p->chunk_rows = (v + 7) & ~7ll; }
+    else if (k == "hll_group_capacity") { if (v < 1 || v > (1 << 20)) return p->fail(BKGPU_EINVAL, "hll_group_capacity out of range (1 .. 2^20)"); p->hll_cap = v; }
     else if (k == "partial_capacity") { if (v < 1) return p->fail(BKGPU_EINVAL, "partial_capacity must be positive"); p->partial_cap = v; }
     else if (k == "force_generic") p->force_generic = v != 0;
     else if (k == "no_stream_copy") p->no_stream_copy = v != 0;
@@ -224,6 +226,12 @@ static int alloc_group_table(bkgpu_plan* p) {
     if ((rc = dev_alloc(p, (void**)&gt.lanes, cap * 8 * (size_t)ap.n_lanes))) return rc;
     if ((rc = dev_alloc(p, (void**)&gt.n_groups, 4 * ((size_t)GT_OCC_OFF + cap)))) return rc;   // counter, overflow flag, occupied list
     gt.overflow = gt.n_groups + 1;
+    if (ap.n_hll) {   // hll_add_agg: the register arena, one block per (group, sketch) that receives a value
+        if ((rc = dev_alloc(p, (void**)&gt.hll_regs, (size_t)p->hll_cap * HLL_REGISTERS))) return rc;
+        if ((rc = dev_alloc(p, (void**)&gt.hll_ctr, 16))) return rc;
+        gt.hll_cap = (uint32_t)p->hll_cap;
+        CK(p, cudaMemsetAsync(gt.hll_ctr, 0, 16, p->stream));
+    }
     p->d_cursor = gt.n_groups + 2;                       // [2] result cursor [3] merge info
     p->d_rows_passed = (uint64_t*)(gt.n_groups + 4);     // [4..5] rows that passed the filter
     CK(p, cudaMemsetAsync(gt.n_groups, 0, 4 * GT_OCC_OFF, p->stream));
@@ -267,6 +275,9 @@ extern "C" int bkgpu_open(bkgpu_plan* p) {
         CK(p, cudaEventCreateWithFlags(&p->stage_ready[i], cudaEventDisableTiming));
     }
     p->blocking_wait = p->blocking_sync >= 0 ? p->blocking_sync != 0 : (p->nranks > 1 && cpu_budget() < 4 * p->nranks);
+    if (p->c.ap.n_hll && (p->repartition || p->peer_merge))
+        return p->fail(BKGPU_EUNSUPPORTED, "hll_add_agg with the %s merge is outside the GPU path: its sketches travel only with the all-gather of group rows",
+                       p->repartition ? "repartition" : "peer_merge");
     int rc = upload_in_sets(p);   // (before sort_open: it copies the programs)
     if (rc) return rc;
     if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) rc = alloc_group_table(p);
@@ -514,7 +525,9 @@ int feed(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* col
     for (size_t i = 0; i < want.size() && !p->no_bounce; i++) pageable = pageable || is_pageable(bound[i]->values);
     // (pageable input adds a CPU copy stage of about the link's speed in front of the H2D copy: smaller chunks keep the fill / drain
     //  of that three-stage pipeline at ~2 % of the batch instead of ~8 %)
-    const int64_t chunk_cap = pageable ? std::min<int64_t>(p->chunk_rows, (int64_t)2 << 20) : p->chunk_rows;
+    int64_t chunk_cap = pageable ? std::min<int64_t>(p->chunk_rows, (int64_t)2 << 20) : p->chunk_rows;
+    for (const ColRef& w : want)   // (a 16400-byte HLL sketch column: staging chunks of at most 256 MB per buffer, a multiple of 8 rows)
+        if (prim_storage(w.prim) == ST_HLL) chunk_cap = std::min<int64_t>(chunk_cap, ((int64_t)256 << 20) / HLL_RAW_BYTES & ~7ll);
     const int64_t chunk = std::min<int64_t>(chunk_cap, std::max<int64_t>((nrows + 7) & ~7ll, 8));
     if ((rc = ensure_stage(p, want, (size_t)chunk))) return rc;
     if (pageable && (rc = ensure_bounce(p, want, (size_t)chunk))) return rc;
@@ -587,6 +600,27 @@ void set_result(bkgpu_plan* p, std::vector<SortOutCol>& cols, int64_t rows, cons
     p->result_rows = rows; p->result_pos = 0;
 }
 
+// MERGE_AGG of hll_add_agg over host memory: every non-NULL input value must be a RAW sketch, or the push fails (device-resident input is
+// checked by the merge kernel itself, and the request then fails at bkgpu_finish)
+static int hll_check_host_sketches(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows) {
+    const AggPlan& ap = p->c.ap;
+    for (int k = 0; k < ap.n_agg; k++) {
+        if (ap.agg[k].kind != AG_HLL || ap.agg[k].arg_prim != BK_HLL) continue;
+        const ColRef& w = p->c.cols[ap.agg[k].hll_col];
+        for (int i = 0; i < ncols; i++) {
+            if (cols[i].tuple_id != w.tuple_id || cols[i].slot_id != w.slot_id || !cols[i].values || cols[i].length != nrows) continue;   // (bind_columns reports those)
+            for (int64_t r = 0; r < nrows; r++) {
+                if (cols[i].validity && !((cols[i].validity[r >> 3] >> (r & 7)) & 1)) continue;
+                const uint8_t* v = (const uint8_t*)cols[i].values + (size_t)r * HLL_RAW_BYTES;
+                if (memcmp(v, "HYLL", 4) != 0 || v[4] != HLL_ENC_RAW)
+                    return p->fail(BKGPU_EINVAL, "column %d_%d row %lld is not a RAW HLL sketch (\"HYLL\", encoding 255, 16400 bytes): MERGE_AGG of hll_add_agg "
+                                   "merges RAW sketches only", w.tuple_id, w.slot_id, (long long)r);
+            }
+        }
+    }
+    return BKGPU_OK;
+}
+
 static int bkgpu_push_impl(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device);
 extern "C" int bkgpu_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device) {
     const double t0 = HostClock::now();
@@ -604,7 +638,9 @@ static int bkgpu_push_impl(bkgpu_plan* p, const bkgpu_column* cols, int ncols, i
     if (nrows == 0) return BKGPU_OK;
     switch (p->c.kind) {
         case PK_AGG: {
-            int rc = feed(p, p->c.cols, cols, ncols, nrows, on_device, agg_batch);
+            int rc = on_device ? BKGPU_OK : hll_check_host_sketches(p, cols, ncols, nrows);
+            if (rc) return rc;
+            rc = feed(p, p->c.cols, cols, ncols, nrows, on_device, agg_batch);
             if (rc) return rc;
             // learn the cardinality for later batches' table size (no sync: a stale value only costs speed); a launch that extracted its
             // result has already left the count in h_fused
@@ -693,7 +729,7 @@ static int agg_collective(bkgpu_plan* p, bool* rows_mode) {
         uint32_t bound = p->merge_bound ? p->merge_bound : 2048u;
         if (ap.n_keyw == 0) bound = 1;
         bound = std::min<uint32_t>(bound, pcap);
-        const size_t rw = (size_t)(ap.n_keyw + ap.n_lanes);
+        const size_t rw = (size_t)(ap.n_keyw + ap.n_lanes + ap.n_hll * HLL_ROW_WORDS);
         const size_t words = 1 + rw * bound;
         if ((rc = ensure_words(p, &p->d_partial, &p->d_partial_words, words))) return rc;
         if ((rc = ensure_words(p, &p->d_gather, &p->d_gather_words, words * (size_t)p->nranks))) return rc;
@@ -816,7 +852,7 @@ static void agg_result(bkgpu_plan* p, const uint64_t* hv, const uint8_t* hn, siz
     int img = 0;
     for (const OutCol& oc : p->c.out_cols) {
         HostCol hc; hc.desc = oc;
-        hc.elem = oc.kind == 1 ? 16 : storage_bytes(prim_storage(oc.prim));
+        hc.elem = oc.kind == 1 ? 16 : oc.kind == 2 ? HLL_RAW_BYTES : storage_bytes(prim_storage(oc.prim));
         hc.values.assign((size_t)std::max<int64_t>(keep, 1) * (size_t)hc.elem, 0);
         const uint64_t* v = hv + (size_t)img * stride + skip;
         const uint8_t* nb = hn + (size_t)img * stride + skip;
@@ -825,6 +861,15 @@ static void agg_result(bkgpu_plan* p, const uint64_t* hv, const uint8_t* hn, siz
         if (oc.kind == 1) {
             const uint64_t* v2 = hv + (size_t)(img + 1) * stride + skip;
             for (int64_t r = 0; r < keep; r++) { memcpy(d + (size_t)r * 16, v + r, 8); memcpy(d + (size_t)r * 16 + 8, v2 + r, 8); }
+        } else if (oc.kind == 2) {
+            // hll_row_init's RAW sketch (hll_common.cpp:834-842): "HYLL", encoding HLL_RAW, then the registers.  hll_row_add invalidates the
+            // cached cardinality (bit 7 of header byte 15) whenever a register grows, which the first value always does: a group that
+            // received a value has the bit set, a group without one (every argument NULL) is the empty sketch with the byte 0
+            for (int64_t r = 0; r < keep; r++) {
+                uint8_t* o = d + (size_t)r * HLL_RAW_BYTES;
+                memcpy(o, "HYLL", 4); o[4] = HLL_ENC_RAW;
+                if (v[r]) { o[15] = 0x80; memcpy(o + HLL_HDR_BYTES, p->hll_host.data() + (size_t)(v[r] - 1) * HLL_REGISTERS, HLL_REGISTERS); }
+            }
         } else switch (prim_storage(oc.prim)) {
             case ST_I32: for (int64_t r = 0; r < keep; r++) { const int32_t x = (int32_t)(int64_t)v[r]; memcpy(d + (size_t)r * 4, &x, 4); } break;
             case ST_U32: for (int64_t r = 0; r < keep; r++) { const uint32_t x = (uint32_t)v[r]; memcpy(d + (size_t)r * 4, &x, 4); } break;
@@ -837,12 +882,29 @@ static void agg_result(bkgpu_plan* p, const uint64_t* hv, const uint8_t* hn, siz
         }
         if (keep > 0 && memchr(nb, 1, (size_t)keep)) {
             hc.validity.assign((size_t)(keep + 7) / 8 + 1, 0xFF);
-            for (int64_t r = 0; r < keep; r++) if (nb[r]) { hc.validity[(size_t)r >> 3] &= (uint8_t)~(1u << (r & 7)); if (oc.kind != 1) memset(d + (size_t)r * hc.elem, 0, (size_t)hc.elem); }
+            for (int64_t r = 0; r < keep; r++) if (nb[r]) { hc.validity[(size_t)r >> 3] &= (uint8_t)~(1u << (r & 7)); if (oc.kind == 0) memset(d + (size_t)r * hc.elem, 0, (size_t)hc.elem); }
         }
         img += oc.kind == 1 ? 2 : 1;
         p->result.push_back(std::move(hc));
     }
     p->result_rows = keep; p->result_pos = 0;
+}
+
+// hll_add_agg: the arena's claimed blocks to the host (the extracted rows reference them), after the request's last kernel.  A claim
+// that found the arena full fails the request: a sketch that lost values would be wrong, not approximate
+static int hll_fetch(bkgpu_plan* p) {
+    if (!p->c.ap.n_hll) return BKGPU_OK;
+    uint32_t ctr[3] = {0, 0, 0};
+    CK(p, cudaMemcpyAsync(ctr, p->gt.hll_ctr, 12, cudaMemcpyDeviceToHost, p->stream));
+    CK(p, cudaStreamSynchronize(p->stream));
+    if (ctr[2]) return p->fail(BKGPU_EINVAL, "MERGE_AGG of hll_add_agg: an input value is not a RAW HLL sketch (\"HYLL\", encoding 255, 16400 bytes)");
+    if (ctr[1] || ctr[0] > p->gt.hll_cap)
+        return p->fail(BKGPU_ETOOBIG, "hll_add_agg: more than %u sketches (groups x hll_add_agg aggregates with a value): raise hll_group_capacity",
+                       p->gt.hll_cap);
+    p->hll_host.resize((size_t)ctr[0] * HLL_REGISTERS);
+    if (ctr[0]) CK(p, cudaMemcpy(p->hll_host.data(), p->gt.hll_regs, (size_t)ctr[0] * HLL_REGISTERS, cudaMemcpyDeviceToHost));
+    p->stats.d2h_bytes += (int64_t)p->hll_host.size() + 8;
+    return BKGPU_OK;
 }
 
 static int agg_finish(bkgpu_plan* p) {
@@ -929,6 +991,7 @@ static int agg_finish(bkgpu_plan* p) {
   }
     uint32_t n_out = finish_n_out, out_cap = finish_out_cap;
     if (n_out > out_cap) n_out = out_cap;
+    if ((rc = hll_fetch(p))) return rc;
     if (p->c.post) return agg_post(p, n_out, out_cap);
     agg_result(p, finish_hv, finish_hn, out_cap, n_out);
     return BKGPU_OK;
@@ -1169,7 +1232,10 @@ extern "C" int bkgpu_push_region(bkgpu_plan* p, int64_t region_id) {
 // ------------------------------------------------------------------ partial state
 extern "C" int bkgpu_partial_capacity(bkgpu_plan* p, size_t* bytes) {
     if (!p || !bytes) return thread_fail(BKGPU_EINVAL, "bkgpu_partial_capacity: NULL argument");
-    if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) { *bytes = 8 * (1 + (size_t)(p->c.ap.n_keyw + p->c.ap.n_lanes) * (size_t)eff_pcap(p)); return BKGPU_OK; }
+    if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) {   // (a sketch's registers ride along: HLL_ROW_WORDS per hll_add_agg)
+        *bytes = 8 * (1 + (size_t)(p->c.ap.n_keyw + p->c.ap.n_lanes + p->c.ap.n_hll * HLL_ROW_WORDS) * (size_t)eff_pcap(p));
+        return BKGPU_OK;
+    }
     if (p->c.kind == PK_SORT && p->sort) { *bytes = sort_partial_bytes(p->sort); return BKGPU_OK; }
     return p->fail(BKGPU_EUNSUPPORTED, "plan kind %d has no partial state", p->c.kind);
 }
@@ -1184,10 +1250,13 @@ extern "C" int bkgpu_partial_export(bkgpu_plan* p, void* dev_dst, size_t bytes) 
     // compact rows (the layout the in-library all-gather ships): [u64 groups][groups x (key words + lane words)]
     CK(p, launch_partial_export_rows(p->gt, p->c.ap, (uint64_t*)dev_dst, eff_pcap(p), p->stream));
     p->stats.kernel_launches += 1;
-    uint64_t held = 0; uint32_t ov = 0;
+    uint64_t held = 0; uint32_t ov = 0, hll_ctr[3] = {0, 0, 0};
     CK(p, cudaMemcpyAsync(&held, dev_dst, 8, cudaMemcpyDeviceToHost, p->stream));
     CK(p, cudaMemcpyAsync(&ov, p->gt.overflow, 4, cudaMemcpyDeviceToHost, p->stream));
+    if (p->gt.hll_ctr) CK(p, cudaMemcpyAsync(hll_ctr, p->gt.hll_ctr, 12, cudaMemcpyDeviceToHost, p->stream));
     CK(p, cudaStreamSynchronize(p->stream));
+    if (hll_ctr[2]) return p->fail(BKGPU_EINVAL, "MERGE_AGG of hll_add_agg: an input value is not a RAW HLL sketch (\"HYLL\", encoding 255, 16400 bytes)");
+    if (hll_ctr[1]) return p->fail(BKGPU_ETOOBIG, "hll_add_agg: more than %u sketches: raise hll_group_capacity", p->gt.hll_cap);
     if (ov) return p->fail(BKGPU_ETOOBIG, "group table overflow (capacity 2^%d slots): raise group_capacity_log2", (int)p->gt.cap_log2);
     if (held > eff_pcap(p)) return p->fail(BKGPU_ETOOBIG, "this rank holds %llu groups, more than partial_capacity=%lld", (unsigned long long)held, (long long)p->partial_cap);
     return BKGPU_OK;

@@ -94,6 +94,8 @@ struct bkgpu_plan {
     int64_t batch_capacity = 1 << 20;
     int64_t chunk_rows = 8 << 20;
     int64_t partial_cap = 1 << 16;
+    int64_t hll_cap = 4096;       // option hll_group_capacity: sketches the register arena holds (16 KB each: 64 MB by default)
+    std::vector<uint8_t> hll_host;   // the arena's claimed blocks, copied back by a finished request (agg_result reads the sketches there)
     int force_generic = 0;
     int no_lean = 0;
     int output_on_device = 0;

@@ -262,7 +262,7 @@ __device__ __forceinline__ int table_upsert(uint32_t* state, uint64_t* keys, uin
 // accumulator lanes
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint64_t lane_identity(int op) {
-    switch (op) {
+    switch (op) {   // (LN_HLL: 0 = no sketch)
         case LN_MIN_I64: return 0x7FFFFFFFFFFFFFFFull;
         case LN_MAX_I64: return 0x8000000000000000ull;
         case LN_MIN_U64: return 0xFFFFFFFFFFFFFFFFull;

@@ -8,7 +8,8 @@
 namespace bk {
 
 // ---- column storage classes (Arrow layout; src/runtime/chunk.cpp:33-92 in the reference) ----
-enum SType : int32_t { ST_I32 = 0, ST_U32 = 1, ST_I64 = 2, ST_U64 = 3, ST_F32 = 4, ST_F64 = 5, ST_U8 = 6, ST_BLOB16 = 7 };
+enum SType : int32_t { ST_I32 = 0, ST_U32 = 1, ST_I64 = 2, ST_U64 = 3, ST_F32 = 4, ST_F64 = 5, ST_U8 = 6, ST_BLOB16 = 7,
+                       ST_HLL = 8 };   // a RAW HLL sketch of 16400 bytes (MERGE_AGG input of hll_add_agg)
 
 // ---- value classes a device value is held in (the reference evaluates every operator in
 //      INT64 / UINT64 / DOUBLE after FunctionManager::complete_fn, src/expr/fn_manager.cpp:316-409) ----
@@ -46,6 +47,8 @@ struct DevCol {
 enum Op : uint8_t {
     OP_END = 0,
     OP_LOAD_COL,     // a = column index, b = 0 | 1 | 2: whole value | {sum | count} half of a 16-byte AVG blob                      -> push value (class by storage), null from bitmap
+                     //   b = 3: a FLOAT column's own 4 bytes, zero-extended (hll_add_agg hashes them; the double image may not keep a NaN's bits)
+                     //   b = 4: the row index itself (a 16400-byte HLL sketch column: the reader addresses the bytes), null from the bitmap
     OP_CONST,        // a = constant index                    -> push constant
     OP_CAST,         // a = from prim, b = to prim            ExprValue::cast_to (expr_value.h:502-611)
     OP_CMP,          // a = FuncType (EQ..LE), b = VClass     operators.cpp:84-100
@@ -91,8 +94,10 @@ struct Program {
 // accumulates in and the lane that counts its non-NULL inputs (0 when the argument cannot be NULL,
 // so several aggregates share one counter).
 enum AggKind : uint8_t { AG_COUNT_STAR = 0, AG_COUNT = 1, AG_SUM = 2, AG_AVG = 3, AG_MIN = 4, AG_MAX = 5,
-                         AG_COUNT_MERGE = 6 };   // MERGE_AGG_NODE: counts shipped by the stores are summed (AggFnCall::merge, agg_fn_call.cpp:779-790)
-enum LaneOp : uint8_t { LN_ADD_I64 = 0, LN_ADD_F64 = 1, LN_MIN_I64, LN_MAX_I64, LN_MIN_U64, LN_MAX_U64, LN_MIN_F64, LN_MAX_F64 };
+                         AG_COUNT_MERGE = 6,     // MERGE_AGG_NODE: counts shipped by the stores are summed (AggFnCall::merge, agg_fn_call.cpp:779-790)
+                         AG_HLL = 7 };           // hll_add_agg: the value lane holds the group's sketch (index + 1 into GroupTable::hll_regs, 0 = none yet)
+enum LaneOp : uint8_t { LN_ADD_I64 = 0, LN_ADD_F64 = 1, LN_MIN_I64, LN_MAX_I64, LN_MIN_U64, LN_MAX_U64, LN_MIN_F64, LN_MAX_F64,
+                        LN_HLL };                // a sketch reference: never combined as a number (its registers are, by the export / merge kernels)
 
 struct AggSpec {
     uint8_t kind;        // AggKind
@@ -107,6 +112,10 @@ struct AggSpec {
     uint8_t cnt_owner;   // lanes can be shared by aggregates over the same argument (SUM(x), AVG(x), COUNT(x)):
     uint8_t acc_owner;   // only the owner updates the lane, everyone reads it at finalize
     uint8_t hidden;      // helper accumulator without an output column (the count half of a merged AVG blob)
+    uint8_t arg_prim;    // AG_HLL: the argument's type after inference, which sets the bytes hashed (hll_key_bytes); with arg_vclass VC_U64
+                         // a FLOAT argument arrives as the column's own 4 bytes (OP_LOAD_COL b = 3), else as its widened double.
+                         // BK_HLL: MERGE_AGG over RAW sketches: the argument is the row (OP_LOAD_COL b = 4) of column `hll_col`
+    uint8_t hll_col;
 };
 
 struct AggPlan {
@@ -126,6 +135,7 @@ struct AggPlan {
     uint8_t key_null_shift[MAX_GROUP];
     uint8_t key_prim[MAX_GROUP];  // pb::PrimitiveType of the group expression
     int32_t pred_out;             // output register of the filter predicate (-1 = no filter)
+    int32_t n_hll;                // AG_HLL aggregates: each adds HLL_ROW_WORDS register words to a group's exported row
 };
 
 // ---- specialised ("direct") row evaluation for the canonical shapes: the predicate is a
@@ -164,7 +174,16 @@ struct GroupTable {
     uint32_t* n_groups;  // number of occupied slots; n_groups[GT_OCC_OFF + i] = slot of the i-th inserted group (the "occupied list":
                          // re-initialisation, export and result extraction walk the groups that exist, not the table's capacity)
     uint32_t* overflow;  // = n_groups + 1: set when an insert could not find a free slot
+    // hll_add_agg: the register arena, one 16384-byte block per (group, AG_HLL aggregate), claimed on a group's first non-NULL value.
+    // hll_ctr[0] = blocks claimed, hll_ctr[1] = set when a claim found the arena full (option hll_group_capacity), hll_ctr[2] = set when a
+    // MERGE_AGG input value was not a RAW sketch.  nullptr without AG_HLL
+    uint8_t* hll_regs;
+    uint32_t* hll_ctr;
+    uint32_t hll_cap;    // blocks the arena holds
 };
+constexpr int HLL_ROW_WORDS = 2048;   // one sketch's 16384 registers as 64-bit words of an exported group row
+constexpr uint64_t HLL_LANE_BUSY = ~0ull;          // a sketch lane while its block is being claimed and zeroed
+constexpr uint64_t HLL_LANE_FULL = ~0ull - 1;      // a sketch lane whose claim found the arena full (the request fails with ETOOBIG)
 constexpr int GT_TICKET = 6;    // word 6 of the counter block: CTAs of the running lean launch that have finished (fused_extract, agg_kernels.cuh); 0 between launches
 constexpr int GT_FX_EXACT = 7;  // word 7 of the counter block: double values the lean kernel's FX variant could not put on its fixed-point grid (agg_direct.cuh)
 constexpr int GT_OCC_OFF = 8;   // words 0-7 of the counter block: groups, overflow, result cursor, merge info, rows passed (u64), ticket, FX exact:

@@ -30,7 +30,8 @@ static __device__ __noinline__ void run_program(const Program& p, const DevCol* 
                 const DevCol& c = cols[in.a];
                 const int64_t r = in.c ? brow : row;
                 if (r < 0) { st[sp] = 0; nul |= 1u << sp; sp++; break; }   // the NULL-extended side of an outer join's unmatched row (Joiner::construct_null_result_batch)
-                st[sp] = in.b ? __ldg((const unsigned long long*)c.values + 2 * r + (in.b - 1)) : load_elem(c, r);
+                st[sp] = in.b == 4 ? (uint64_t)r : in.b == 3 ? (uint64_t)__ldg((const uint32_t*)c.values + r)
+                       : in.b ? __ldg((const unsigned long long*)c.values + 2 * r + (in.b - 1)) : load_elem(c, r);
                 nul = elem_is_null(c, r) ? (nul | (1u << sp)) : (nul & ~(1u << sp));
                 sp++;
             } break;

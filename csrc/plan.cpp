@@ -9,6 +9,7 @@
 // and then lowers instead of interpreting: expressions become postfix bytecode whose operand
 // classes are fixed here (no run-time type tags on the device).
 #include "plan.h"
+#include "hll.cuh"
 #include <math.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -50,11 +51,12 @@ int prim_storage(int prim) {  // src/common/common.cpp:514-544
         case BK_DOUBLE: return ST_F64;
         case BK_BOOL: return ST_U8;
         case BK_STRING: return ST_BLOB16;
+        case BK_HLL: return ST_HLL;
         default: return -1;
     }
 }
 int storage_bytes(int st) {
-    switch (st) { case ST_I32: case ST_U32: case ST_F32: return 4; case ST_U8: return 1; case ST_BLOB16: return 16; default: return 8; }
+    switch (st) { case ST_I32: case ST_U32: case ST_F32: return 4; case ST_U8: return 1; case ST_BLOB16: return 16; case ST_HLL: return HLL_RAW_BYTES; default: return 8; }
 }
 static uint64_t dbits(double d) { uint64_t u; memcpy(&u, &d, 8); return u; }
 static double bitsd(uint64_t u) { double d; memcpy(&d, &u, 8); return d; }
@@ -389,6 +391,14 @@ static bool infer_expr(Infer& in, HExpr& e) {
             } else if (e.name == "min" || e.name == "max") {
                 if (e.ch.empty()) return in.fail(BKGPU_EINVAL, "%s() without an argument", e.name.c_str());
                 e.col_type = ct;
+            } else if (e.name == "hll_add_agg") {   // agg_fn_call.cpp:124-130
+                if (e.ch.empty()) return in.fail(BKGPU_EINVAL, "hll_add_agg() without an argument");
+                if (ct == BK_STRING)
+                    return in.fail(BKGPU_EUNSUPPORTED, "hll_add_agg over a STRING argument is outside the GPU path: a dictionary code would be hashed, not the text");
+                if (ct != BK_NULL_TYPE && !hll_key_bytes(ct)) return in.fail(BKGPU_EUNSUPPORTED, "hll_add_agg over an argument of type %d is outside the GPU path", ct);
+                e.col_type = BK_HLL;
+            } else if (e.name == "hll_merge_agg") {
+                return in.fail(BKGPU_EUNSUPPORTED, "hll_merge_agg over stored sketches is outside the GPU path: a DENSE or SPARSE sketch varies in length");
             } else return in.fail(BKGPU_EUNSUPPORTED, "aggregate '%s' is outside the GPU path", e.name.c_str());
             if (e.name != "count_star" && e.name != "count" && !e.ch.empty() && ct == BK_STRING)
                 return in.fail(BKGPU_EUNSUPPORTED, "%s over a STRING argument is outside the GPU path", e.name.c_str());
@@ -903,7 +913,7 @@ static bool lower_agg(Infer& in, Compiled& out, const HNode& agg, const std::vec
             if (st == BK_INVALID_TYPE) return in.fail(BKGPU_EINVAL, "MERGE_AGG: slot %d_%d is not declared", f.tuple_id, f.inter_slot);
             const int ci = lw.intern_col(f.tuple_id, f.inter_slot, st);
             if (ci >= MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d columns referenced", MAX_COLS);
-            if (!lw.emit(OP_LOAD_COL, (uint8_t)ci, st == BK_STRING ? 1 : 0, 0)) return false;
+            if (!lw.emit(OP_LOAD_COL, (uint8_t)ci, st == BK_STRING ? 1 : st == BK_HLL ? 4 : 0, 0)) return false;
             if (f.name == "count" || f.name == "count_star") {
                 const int z = lw.add_const(0, false); if (z < 0) return false;
                 if (!lw.emit(OP_CONST, (uint8_t)z) || !lw.emit(OP_CMP, (uint8_t)BK_FT_NE, (uint8_t)host_prim_class(st))) return false;
@@ -956,6 +966,22 @@ static bool lower_agg(Infer& in, Compiled& out, const HNode& agg, const std::vec
         const HExpr& f = agg.agg_fns[(size_t)k];
         AggSpec& a = ap.agg[k]; memset(&a, 0, sizeof a);
         a.arg_out = 0xFF; a.out_prim = (uint8_t)f.col_type;
+        if (out.is_merge && !f.distinct && f.name == "hll_add_agg") {
+            // MERGE_AGG_NODE over the stores' RAW sketches (AggFnCall::merge -> hll_merge_agg, hll_common.cpp:630-703): register-wise max
+            const int st = in.slot_type(f.tuple_id, f.inter_slot);
+            if (st != BK_HLL) return in.fail(BKGPU_EUNSUPPORTED, "MERGE_AGG: hll_add_agg over an intermediate slot of type %d (a RAW HLL sketch is merged)", st);
+            const int ci = lw.intern_col(f.tuple_id, f.inter_slot, BK_HLL);
+            if (ci >= MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d columns referenced", MAX_COLS);
+            out.arg_cols_mask[(size_t)k] = 1 << ci;
+            if (!lw.emit(OP_LOAD_COL, (uint8_t)ci, 4, 0)) return false;   // (the row: the merge reads the value's 16400 bytes itself)
+            a.arg_out = (uint8_t)reg; a.nullable = 1;
+            if (!lw.out_reg(reg++)) return false;
+            a.kind = AG_HLL; a.arg_prim = BK_HLL; a.hll_col = (uint8_t)ci;
+            const int l = new_lane(LN_HLL); if (l < 0) return false;
+            a.acc_lane = (uint8_t)l;
+            ap.n_hll++;
+            continue;
+        }
         if (out.is_merge && !f.distinct) {
             // MERGE_AGG_NODE: the input rows carry the stores' intermediate slots; AggFnCall::merge (agg_fn_call.cpp:719-822)
             // adds counts and sums, folds MIN/MAX, and adds both halves of an AVG blob.  NULL intermediates are skipped.
@@ -1007,6 +1033,29 @@ static bool lower_agg(Infer& in, Compiled& out, const HNode& agg, const std::vec
         const HExpr& arg = f.ch[0];
         // COUNT(non-null literal) is COUNT(*) (agg_fn_call.cpp:246-250)
         if (f.name == "count" && is_literal_node(arg.node_type) && !arg.lit_null) { a.kind = AG_COUNT_STAR; continue; }
+        if (f.name == "hll_add_agg") {
+            // the value lane references the group's sketch (AG_HLL); no counter, no lane shared with another aggregate
+            a.kind = AG_HLL; a.arg_prim = (uint8_t)arg.col_type; a.nullable = 1;
+            const int st = arg.node_type == BK_SLOT_REF ? in.slot_type(arg.tuple_id, arg.slot_id) : BK_INVALID_TYPE;
+            const bool raw_f32 = arg.node_type == BK_SLOT_REF && arg.col_type == BK_FLOAT && (st == BK_FLOAT || st == BK_INVALID_TYPE);
+            const std::string hkey = expr_key(arg) + (raw_f32 ? "#f32" : "");
+            if (!arg_reg_of.count(hkey)) {
+                if (raw_f32) {   // the column's own 4 bytes (OP_LOAD_COL b = 3), which the reference hashes
+                    const int ci = lw.intern_col(arg.tuple_id, arg.slot_id, BK_FLOAT);
+                    if (ci >= MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d columns referenced", MAX_COLS);
+                    if (!lw.emit(OP_LOAD_COL, (uint8_t)ci, 3, (uint8_t)out.col_side[(size_t)ci])) return false;
+                } else { depth = 0; if (!lw.expr(arg, depth)) return false; }
+                arg_reg_of[hkey] = reg;
+                if (!lw.out_reg(reg++)) return false;
+            }
+            a.arg_out = (uint8_t)arg_reg_of[hkey];
+            a.arg_vclass = (uint8_t)(raw_f32 ? VC_U64 : host_prim_class(arg.col_type));
+            int m = 0; expr_cols(arg, out, m); out.arg_cols_mask[(size_t)k] = m; out.arg_can_null[(size_t)k] = expr_makes_null(arg);
+            const int l = new_lane(LN_HLL); if (l < 0) return false;
+            a.acc_lane = (uint8_t)l;
+            ap.n_hll++;
+            continue;
+        }
         std::string key = expr_key(arg);
         if (!arg_reg_of.count(key)) {
             depth = 0;
@@ -1047,7 +1096,8 @@ static bool lower_agg(Infer& in, Compiled& out, const HNode& agg, const std::vec
         const HExpr& f = agg.agg_fns[(size_t)k];
         int ft = in.slot_type(f.tuple_id, f.final_slot);
         if (ft == BK_INVALID_TYPE || ft == BK_STRING) ft = f.col_type;
-        out.out_cols.push_back({f.tuple_id, f.final_slot, ft, 0});
+        if (ap.agg[k].kind == AG_HLL) ft = BK_HLL;
+        out.out_cols.push_back({f.tuple_id, f.final_slot, ft, ap.agg[k].kind == AG_HLL ? 2 : 0});
         ap.agg[k].out_prim = (uint8_t)ft;
         if (ap.agg[k].kind == AG_AVG) out.out_cols.push_back({f.tuple_id, f.inter_slot != f.final_slot ? f.inter_slot : -1, BK_STRING, 1});
     }
@@ -1056,7 +1106,7 @@ static bool lower_agg(Infer& in, Compiled& out, const HNode& agg, const std::vec
     DirectPlan& d = out.direct; memset(&d, 0, sizeof d); memset(d.agg_val, 0xFF, sizeof d.agg_val);
     do {
         std::vector<int> order;  // cols indices in [terms][key][values] order
-        if (!allow_direct || out.is_merge) break;
+        if (!allow_direct || out.is_merge || ap.n_hll) break;
         if (!conjuncts.empty()) {
             if (conjuncts.size() > 2) break;
             bool ok = true;
@@ -1156,6 +1206,12 @@ static void explain(Compiled& c) {
             const AggSpec& a = ap.agg[k];
             snprintf(buf, sizeof buf, "  agg[%d] kind=%d class=%d arg_class=%d acc_lane=%d cnt_lane=%d arg_out=%d out_prim=%d\n", k, a.kind, a.vclass,
                      a.arg_vclass, a.acc_lane, a.cnt_lane, a.arg_out, a.out_prim); s += buf;
+            if (a.kind == AG_HLL && a.arg_prim == BK_HLL) {
+                snprintf(buf, sizeof buf, "    hll_add_agg under MERGE_AGG: register-wise max of the RAW sketches of col[%d] (16400 bytes each)\n", a.hll_col); s += buf;
+            } else if (a.kind == AG_HLL) {
+                snprintf(buf, sizeof buf, "    hll_add_agg: arg_prim=%d hashes %d bytes%s (MurmurHash3_x64_128, seed 0x110) -> 16384 registers, RAW sketch of %d bytes\n",
+                         a.arg_prim, hll_key_bytes(a.arg_prim), a.arg_vclass == VC_U64 && a.arg_prim == BK_FLOAT ? " of the FLOAT column" : "", HLL_RAW_BYTES); s += buf;
+            }
         }
         if (c.has_direct) {
             for (int t = 0; t < c.direct.n_terms; t++) {
@@ -1305,7 +1361,7 @@ static bool intern_tuple(Infer& in, Compiled& out, Lower& lw, int tuple_id, cons
     for (auto& x : out.tuples) if (x.tuple_id == tuple_id) t = &x;
     if (!t || t->slots.empty()) return in.fail(BKGPU_EINVAL, "%s %d has no descriptor", tuple_name, tuple_id);
     for (auto& sl : t->slots) {
-        if (prim_storage(sl.second) < 0 || sl.second == BK_STRING)
+        if (prim_storage(sl.second) < 0 || sl.second == BK_STRING || sl.second == BK_HLL)
             return in.fail(BKGPU_EUNSUPPORTED, "column %d_%d has type %d: outside the GPU path", tuple_id, sl.first, sl.second);
         if (lw.intern_col(tuple_id, sl.first, sl.second) >= MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d columns in %s", MAX_COLS, row_name);
         out.out_cols.push_back({tuple_id, sl.first, sl.second, 0});
@@ -2031,6 +2087,15 @@ int compile_plan(const uint8_t* desc, size_t len, Compiled& out, std::string& er
         // LimitNode straight over the aggregate: the result extraction (agg_result) skips `offset` groups and then keeps `limit` of them,
         // so the limit is stored as it is — not as the first limit + offset rows that a sort or a filter keeps before skipping
         if (ok && limit_node && !post_sort && !post_having) { out.limit = limit_node->limit; out.offset = limit_node->offset; }
+        bool hll_out = false, hll_merge = false;
+        for (const OutCol& oc : out.out_cols) hll_out = hll_out || oc.kind == 2;
+        for (int k = 0; ok && k < out.ap.n_agg; k++) hll_merge = hll_merge || (out.ap.agg[k].kind == AG_HLL && out.ap.agg[k].arg_prim == BK_HLL);   // (ap is set once lowering succeeded)
+        if (ok && hll_merge && out.kind != PK_AGG) {   // (a join would have to gather 16400-byte values to the probe rows)
+            err = "MERGE_AGG of HLL sketches over a join is outside the GPU path (MERGE_AGG over a scan is lowered)"; return BKGPU_EUNSUPPORTED;
+        }
+        if (ok && (post_sort || post_having) && hll_out) {
+            err = "a SORT / HAVING / LIMIT above an aggregate that returns an HLL sketch is outside the GPU path"; return BKGPU_EUNSUPPORTED;
+        }
         if (ok && (post_sort || post_having))
             ok = lower_sink(in, out, {post_sort, post_having, post_having ? post_having->limit : -1, true, "aggregate output columns under a SORT / HAVING",
                                       "SORT / HAVING above an aggregate references a column the aggregate does not output"}, limit_node);

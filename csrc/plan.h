@@ -59,7 +59,8 @@ struct ColRef { int tuple_id, slot_id, prim; };
 
 struct OutCol {
     int tuple_id, slot_id, prim;
-    int kind;       // 0 = plain value column, 1 = AVG intermediate blob (two device images: sum, count)
+    int kind;       // 0 = plain value column, 1 = AVG intermediate blob (two device images: sum, count), 2 = HLL sketch (RAW, 16400 bytes;
+                    //   one device image: the sketch reference, whose registers the host copies from the arena)
 };
 
 enum PlanKind { PK_AGG = 1, PK_FILTER = 2, PK_SORT = 3, PK_JOIN_AGG = 4, PK_JOIN = 5, PK_STAR_AGG = 6, PK_WINDOW = 7 };

@@ -159,14 +159,17 @@ struct RuntimeState {
 
 // ---------------------------------------------------------------- rows <-> columns (f1: the MemRow / RowBatch bridge)
 // What `MemRow::get_value(tuple, slot)` hands an operator: a typed value or NULL (include/mem_row/mem_row.h:28-215,
-// ExprValue in include/common/expr_value.h).  64-bit payload in the slot's value class.
+// ExprValue in include/common/expr_value.h).  64-bit payload in the slot's value class; an HLL sketch (BK_HLL: hll_add_agg's RAW sketch
+// of 16400 bytes) is held as bytes, the way ExprValue holds it in str_val.
 struct Value {
     bool is_null = true;
     union { int64_t i64; uint64_t u64; double f64; };
+    std::string bytes;   // BK_HLL only
     Value() : i64(0) {}
     static Value of_int(int64_t v) { Value x; x.is_null = false; x.i64 = v; return x; }
     static Value of_uint(uint64_t v) { Value x; x.is_null = false; x.u64 = v; return x; }
     static Value of_double(double v) { Value x; x.is_null = false; x.f64 = v; return x; }
+    static Value of_bytes(std::string v) { Value x; x.is_null = false; x.bytes = std::move(v); return x; }
 };
 using MemRowValues = std::vector<Value>;   // one Value per slot of the chunk's schema, in schema order
 
@@ -181,11 +184,14 @@ public:
             case BK_BOOL: return 1;
             case BK_INT8: case BK_INT16: case BK_INT32: case BK_TIME: case BK_UINT8: case BK_UINT16: case BK_UINT32: case BK_TIMESTAMP: case BK_DATE: case BK_FLOAT: return 4;
             case BK_INT64: case BK_UINT64: case BK_DATETIME: case BK_DOUBLE: return 8;
+            case BK_HLL: return 16400;   // a RAW sketch (bkgpu.h)
             default: return -1;
         }
     }
     int add_row(const MemRowValues& row) {   // Chunk::add_row / decode_row (chunk.cpp:335-384)
         if (row.size() != _schema.size()) return -1;
+        for (size_t c = 0; c < _schema.size(); c++)   // (a sketch of another length would shift every later row)
+            if (_schema[c].prim_type == BK_HLL && !row[c].is_null && row[c].bytes.size() != (size_t)_batch.columns[c].elem_size) return -1;
         for (size_t c = 0; c < _schema.size(); c++) {
             Column& col = _batch.columns[c];
             const Value& v = row[c];
@@ -203,6 +209,7 @@ public:
                     case BK_FLOAT: { float f = (float)v.f64; memcpy(dst, &f, 4); } break;
                     case BK_DOUBLE: memcpy(dst, &v.f64, 8); break;
                     case BK_BOOL: dst[0] = v.i64 ? 1 : 0; break;
+                    case BK_HLL: memcpy(dst, v.bytes.data(), (size_t)eb); break;
                     default: memcpy(dst, &v.i64, (size_t)eb); break;   // little-endian narrowing of the integer payload
                 }
             }
@@ -232,6 +239,7 @@ public:
                     case BK_INT8: case BK_INT16: case BK_INT32: case BK_TIME: { int32_t x; memcpy(&x, src, 4); v.i64 = x; } break;
                     case BK_UINT8: case BK_UINT16: case BK_UINT32: case BK_TIMESTAMP: case BK_DATE: { uint32_t x; memcpy(&x, src, 4); v.u64 = x; } break;
                     case BK_STRING: memcpy(&v.f64, src, 8); break;   // AVG intermediate: the sum half (count: src + 8)
+                    case BK_HLL: v.bytes.assign((const char*)src, (size_t)col.elem_size); break;
                     default: memcpy(&v.i64, src, 8); break;
                 }
             }

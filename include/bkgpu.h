@@ -105,7 +105,9 @@ int   bkgpu_init(bkgpu_plan** out, const uint8_t* plan_desc, size_t len,
  *   "smem_capacity_log2"   slots of the per-CTA shared table (-1 = chosen per batch, 0 = none)
  *   "batch_capacity"       rows per bkgpu_get_next batch (RuntimeState::row_batch_capacity)
  *   "chunk_rows"           rows per host->device staging chunk of a host push
- *   "partial_capacity"     groups per rank in the exported partial state
+ *   "partial_capacity"     groups per rank in the exported partial state (a plan with hll_add_agg ships 16 KB of registers per group and sketch)
+ *   "hll_group_capacity"   sketches the hll_add_agg register arena holds: one per group and hll_add_agg aggregate that receives a non-NULL
+ *                          value, 16 KB of device memory each (default 4096 = 64 MB, at most 2^20); more -> BKGPU_ETOOBIG naming this option
  *   "region_base"          arrival index of this plan's first row: ORDER BY ties across GPUs break by (region, row)
  *   "peer_merge"           with a communicator: partial states are written straight into the peers' buffers over NVLink (CUDA IPC)
  *                          instead of gathered by NCCL (opt-in)
@@ -170,6 +172,16 @@ int   bkgpu_parse_datetime(const char* text, size_t length, int prim_type, uint6
  * conversion plan compilation applies to literals (DATE <-> DATETIME <-> TIMESTAMP in the reference's fixed UTC+8 zone included).
  * BKGPU_EUNSUPPORTED for a TIME source with another date/time target (relative to the current date in the reference). */
 int   bkgpu_cast_image(uint64_t image, int from_prim, int to_prim, uint64_t* out);
+
+/* ---- HyperLogLog sketches ----
+ * hll_add_agg returns a column of prim_type BK_HLL and elem_size 16400: the reference's RAW sketch (hll_row_init, src/common/
+ * hll_common.cpp:834-842): "HYLL", encoding byte 255, three zero bytes, 8 bytes of cached cardinality (bit 7 of the last one set = not
+ * cached), then 16384 one-byte registers.  bkgpu_hll_estimate is hll_estimate (hll_common.cpp:523-600) over such a sketch: the cached
+ * value when it is valid, else the histogram estimator; the sketch itself is not modified.  BKGPU_EINVAL for anything but a RAW sketch
+ * of 16400 bytes.  Needs no GPU.
+ * MERGE_AGG of hll_add_agg takes the stores' sketches as input columns of the same type and size (RAW only: any other value fails the push
+ * with BKGPU_EINVAL, or bkgpu_finish when the column is in device memory). */
+int   bkgpu_hll_estimate(const uint8_t* sketch, size_t len, uint64_t* estimate);
 
 /* ---- resident regions (the column store / parquet cache analogue, include/column/file_manager.h:252-272) ----
  * A region's columns are copied to HBM once (host or device source) and stay there across queries, keyed by
