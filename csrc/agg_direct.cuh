@@ -655,6 +655,10 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) k_agg_group_lean(const __grid
         fx_ext = smem_addr(smem_raw) + a.fx_ext_off;
         if (threadIdx.x < 4) fx_emax[threadIdx.x] = 0u;
         for (uint32_t i = threadIdx.x; i < (uint32_t)NA * tcap; i += LEAN_THREADS) sts32(fx_ext + i * 4u, 0u);
+        for (uint32_t i = threadIdx.x; i < tcap; i += LEAN_THREADS) {   // the limbs start from integer 0, not from the lane's -0.0
+#pragma unroll
+            for (int s = 0; s < NA; s++) if (acc_f64[s]) sts64(acc_addr[s] + i * 16u, 0ull);
+        }
         __syncthreads();
         const int64_t srow = (int64_t)((uint64_t)(blockIdx.x + (uint64_t)threadIdx.x * gridDim.x) * (uint64_t)a.nrows / ((uint64_t)gridDim.x * LEAN_THREADS));
 #pragma unroll
@@ -825,7 +829,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) k_agg_group_lean(const __grid
             if (NULLS) {
                 nb = lds8(qnull + e);
 #pragma unroll
-                for (int s = 0; s < NA; s++) if ((nb >> s) & 1u) v[s] = 0ull;   // +0 / +0.0 leaves the sum unchanged
+                for (int s = 0; s < NA; s++) if ((nb >> s) & 1u) v[s] = acc_f64[s] ? 0x8000000000000000ull : 0ull;   // 0 / -0.0 leaves the sum unchanged
             }
             const uint32_t h = ((uint32_t)k0 ^ (uint32_t)(k0 >> 32)) * 0x9E3779B1u;
             int slot = -1;

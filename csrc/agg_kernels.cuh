@@ -214,15 +214,15 @@ __device__ __forceinline__ void extract_group(const GroupTable& gt, const AggPla
             case AG_COUNT_STAR: v = nrows; break;
             case AG_COUNT: v = cnt; break;
             case AG_COUNT_MERGE: case AG_HLL: v = acc; break;   // (AG_HLL: the sketch reference; the host copies its registers)
-            case AG_AVG:
-                if (cnt == 0) isnull = 1; else v = f64_bits(__ddiv_rn(bits_f64(acc), (double)(int64_t)cnt));
+            case AG_AVG:   // (AVG's sum starts from +0.0 in the reference, agg_initialize: + 0.0 turns the lane's -0.0 into +0.0)
+                if (cnt == 0) isnull = 1; else v = f64_bits(__ddiv_rn(__dadd_rn(bits_f64(acc), 0.0), (double)(int64_t)cnt));
                 break;
             default: if (cnt == 0) isnull = 1; else v = acc; break;  // SUM / MIN / MAX: NULL without input
         }
         outv[(size_t)c * stride + pos] = v; outn[(size_t)c * stride + pos] = isnull; c++;
         if (a.kind == AG_AVG) {  // intermediate blob {double sum; int64 count}
             // the blank row of an empty scalar aggregate initialises only its counts (agg_node.cpp:489-503): blob stays NULL
-            outv[(size_t)c * stride + pos] = acc; outn[(size_t)c * stride + pos] = (ap.n_keyw == 0 && nrows == 0) ? 1 : 0; c++;
+            outv[(size_t)c * stride + pos] = f64_bits(__dadd_rn(bits_f64(acc), 0.0)); outn[(size_t)c * stride + pos] = (ap.n_keyw == 0 && nrows == 0) ? 1 : 0; c++;
             outv[(size_t)c * stride + pos] = cnt; outn[(size_t)c * stride + pos] = 0; c++;
         }
     }

@@ -269,6 +269,9 @@ __device__ __forceinline__ uint64_t lane_identity(int op) {
         case LN_MAX_U64: return 0ull;
         case LN_MIN_F64: return 0x7FF0000000000000ull;  // +inf
         case LN_MAX_F64: return 0xFFF0000000000000ull;  // -inf
+        // -0.0: the only double x with -0.0 + x == x for every x.  The reference's SUM takes its first value and adds the rest, so a SUM
+        // over only -0.0 is -0.0; a +0.0 start would make it +0.0 (AVG starts from +0.0: extract_group normalises its sum)
+        case LN_ADD_F64: return 0x8000000000000000ull;
         default: return 0ull;
     }
 }
