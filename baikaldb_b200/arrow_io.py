@@ -26,7 +26,7 @@ def arrow_type(prim_type: int) -> pa.DataType:
     pt = T(prim_type)
     if pt == T.BOOL:
         return pa.bool_()
-    if pt in (T.STRING, T.HLL):   # (HLL: hll_add_agg's 16400-byte RAW sketches, as binary values)
+    if pt in (T.STRING, T.HLL, T.BITMAP):   # (HLL: hll_add_agg's 16400-byte RAW sketches; BITMAP: rb_build_agg's serialized bitmaps)
         return pa.large_binary()
     return _ARROW_OF_STORAGE[np.dtype(storage_dtype(pt)).name]
 
@@ -43,7 +43,7 @@ def record_batch_from_columns(cols: Sequence[Column]) -> pa.RecordBatch:
     for c in cols:
         at = arrow_type(c.prim_type)
         mask = None if c.valid is None else ~np.asarray(c.valid, dtype=bool)
-        if c.prim_type in (T.STRING, T.HLL):
+        if c.prim_type in (T.STRING, T.HLL, T.BITMAP):
             vals = [bytes(v) for v in c.values]
             if mask is not None:
                 vals = [None if m else v for v, m in zip(vals, mask)]

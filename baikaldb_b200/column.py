@@ -16,7 +16,8 @@ class Column:
     tuple_id: int
     slot_id: int
     prim_type: int
-    values: np.ndarray                     # storage dtype (see plan.storage_dtype); (n,16) u1 for AVG blobs, (n,16400) u1 for HLL sketches
+    values: np.ndarray                     # storage dtype (see plan.storage_dtype); (n,16) u1 for AVG blobs, (n,16400) u1 for HLL sketches,
+                                           # an object array of bytes for BITMAP (rb_build_agg's serialized Roaring bitmaps)
     valid: Optional[np.ndarray] = None     # bool[n]; None = no NULLs
 
     @property
@@ -34,7 +35,7 @@ class Column:
 
     def to_list(self) -> list:
         v = self.values
-        if self.prim_type in (PrimitiveType.STRING, PrimitiveType.HLL):
+        if self.prim_type in (PrimitiveType.STRING, PrimitiveType.HLL, PrimitiveType.BITMAP):
             out = [bytes(x) for x in v]
         else:
             out = v.tolist()

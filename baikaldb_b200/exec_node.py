@@ -217,7 +217,12 @@ class GpuExecNode:
         n = nrows.value
         for i in range(ncols.value):
             oc = out[i]
-            if oc.prim_type in (PrimitiveType.STRING, PrimitiveType.HLL):   # byte blobs: AVG's {sum, count}, hll_add_agg's RAW sketch
+            if oc.prim_type == PrimitiveType.BITMAP:   # rb_build_agg: n + 1 int64 offsets, then the bytes (bkgpu.h)
+                offs = np.frombuffer((ctypes.c_int64 * (n + 1)).from_address(oc.values), dtype=np.int64)
+                raw = ctypes.string_at(oc.values + 8 * (n + 1), int(offs[n]))
+                vals = np.empty(n, dtype=object)
+                vals[:] = [raw[offs[r]:offs[r + 1]] for r in range(n)]
+            elif oc.prim_type in (PrimitiveType.STRING, PrimitiveType.HLL):   # byte blobs: AVG's {sum, count}, hll_add_agg's RAW sketch
                 w = oc.elem_size
                 raw = (ctypes.c_uint8 * (max(n, 1) * w)).from_address(oc.values)
                 vals = np.frombuffer(raw, dtype=np.uint8, count=n * w).reshape(n, w).copy()

@@ -79,6 +79,7 @@ class PrimitiveType(IntEnum):  # proto/common.proto:46-72
     DATE = 16
     HLL = 17
     TIME = 18
+    BITMAP = 21
 
 
 class FuncType(IntEnum):  # include/sqlparser/expr.h:48-89
@@ -587,7 +588,7 @@ class Plan:
 def agg_tuple_slots(agg_fns: Sequence[Expr], arg_types: Sequence[int]) -> List[Tuple[int, int]]:
     """Slot types of the aggregate tuple, as AggFnCall::type_inferer(tuple_desc) assigns them
     (src/expr/agg_fn_call.cpp:87-122,176-200): COUNT -> INT64, SUM -> INT64/UINT64/DOUBLE by argument,
-    AVG -> final DOUBLE + intermediate STRING blob, MIN/MAX -> argument type, hll_add_agg -> HLL."""
+    AVG -> final DOUBLE + intermediate STRING blob, MIN/MAX -> argument type, hll_add_agg -> HLL, rb_build_agg -> BITMAP."""
     slots: Dict[int, int] = {}
     for f, at in zip(agg_fns, arg_types):
         name = f.name
@@ -604,6 +605,8 @@ def agg_tuple_slots(agg_fns: Sequence[Expr], arg_types: Sequence[int]) -> List[T
             ft = T.DOUBLE
         elif name == "hll_add_agg":
             ft = T.HLL
+        elif name == "rb_build_agg":
+            ft = T.BITMAP
         else:
             ft = at
         slots[f.final_slot_id] = int(ft)

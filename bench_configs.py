@@ -3,7 +3,7 @@
 device-resident synthetic columns (SURVEY.md §8d), CUDA events around reset+push+finish+get_next, one JSON line per
 config with rows/s and achieved GB/s on the config's algorithmic bytes.  The headline line is bench.py's;
 this script measures the side configs on their own (C6, the star join, also its kernels, a parity flag and the Acero time).
-usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [c9] [c10] [c11] [c12] [c13] [--scale 0.1] [--steps 10]"""
+usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [c9] [c10] [c11] [c12] [c13] [c14] [--scale 0.1] [--steps 10]"""
 import argparse
 import ctypes
 import json
@@ -661,6 +661,73 @@ def c13(a):
     del g, x
 
 
+def c14(a):
+    """C14, exact value sets: rb_build_agg(x) over 100M device-resident rows, scalar and GROUP BY g (1000 groups), x INT64 uniform over
+    [0, 10M).  Each line carries the step time, the device time of each phase from a separate torch.profiler run (collect: the aggregate
+    kernel appending pair keys; sort: radix passes and deduplication; build: containers, offsets and bytes; scan: the prefix sums both
+    use), parity (every group's bytes parsed back by tests/roaring_oracle.py against torch.unique of (g, x & 0xFFFFFFFF), and a sample
+    of groups byte for byte), hll_add_agg on the same rows, and the card's clocks and throttle reasons around the timed region."""
+    from baikaldb_b200.exec_node import DeviceColumn, execute
+    from tests import hll_cases as HC, rb_cases as RC, roaring_oracle as R
+    import subprocess
+    from torch.profiler import ProfilerActivity, profile
+    n = int(100_000_000 * a.scale)
+    specs = [(0, 1, T.INT32, 0, 1, 0, 1000, 1.0), (0, 2, T.INT64, 0, 2, 0, 10_000_000, 1.0)]
+    g, x = gen(n, specs[0], 14), gen(n, specs[1], 14)
+    arr = cols_array(specs, [g, x])
+    dev = [DeviceColumn(0, 1, int(T.INT32), g.data_ptr(), n, keepalive=g), DeviceColumn(0, 2, int(T.INT64), x.data_ptr(), n, keepalive=x)]
+    q = "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm,clocks_throttle_reasons.active"
+
+    def smi():
+        try:
+            return subprocess.check_output(["nvidia-smi", q, "--format=csv,noheader"], text=True).split("\n")[0].strip()
+        except Exception:
+            return None
+    pk = torch.unique((g.to(torch.int64) << 32) | (x & 0xFFFFFFFF))
+    for grouped in (False, True):
+        plan = RC.scan_plan(T.INT64, grouped=grouped)
+        plan.tuples[0] = [(1, T.INT32), (2, T.INT64)]
+        name = f"C14 rb_build_agg(x){' GROUP BY g (1000 groups)' if grouped else ' scalar'}"
+        before = smi()
+        line = run(name, plan, [(arr, 2, n)], n, 12 * n, a.steps, a.warmup, emit=False)
+        line["smi_before"], line["smi_after"] = before, smi()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            got, _ = execute(plan, dev)
+            torch.cuda.synchronize()
+        phase = {"collect": 0.0, "sort": 0.0, "build": 0.0, "scan": 0.0}
+        for ev in prof.key_averages():
+            nm = ev.key
+            dt = getattr(ev, "device_time_total", getattr(ev, "cuda_time_total", 0.0)) / 1000.0
+            if "k_agg_interp" in nm: phase["collect"] += dt
+            elif "k_rs_" in nm or "k_uniq" in nm: phase["sort"] += dt
+            elif "k_scan" in nm: phase["scan"] += dt
+            elif any(k in nm for k in ("k_seg_", "k_containers", "k_bitmap_", "k_headers", "k_payloads", "k_bitsets")): phase["build"] += dt
+        line["phase_ms"] = {k: round(v, 3) for k, v in phase.items()}
+        cols = {c.name: c.to_list() for c in got}
+        bms = cols[f"{RC.AGG_TUPLE}_1"]
+        keys = cols["0_1"] if grouped else [0]
+        if grouped:
+            gk, vals = pk >> 32, pk & 0xFFFFFFFF
+        else:
+            vals = torch.unique(x & 0xFFFFFFFF)
+            gk = torch.zeros_like(vals)
+        bounds = torch.searchsorted(gk.contiguous(), torch.arange(1001 if grouped else 2, device=gk.device)).cpu().numpy()
+        v = vals.cpu().numpy().astype(np.uint32)
+        ok = len(bms) == (1000 if grouped else 1)
+        for i, (k, b) in enumerate(zip(keys, bms)):
+            want = v[bounds[k]:bounds[k + 1]]
+            ok = ok and np.array_equal(R.parse(b), want)
+            if i < 8:
+                ok = ok and b == R.serialize(want)
+        line["parity_vs_torch_unique"] = bool(ok)
+        line["bitmap_bytes"] = int(sum(len(b) for b in bms))
+        hplan = HC.scan_plan(T.INT64, grouped=grouped)
+        hplan.tuples[0] = [(1, T.INT32), (2, T.INT64)]
+        line["hll_add_agg_same_rows"] = run(name.replace("rb_build_agg", "hll_add_agg"), hplan, [(arr, 2, n)], n, 12 * n, a.steps, a.warmup, emit=False)["ms_per_step"]
+        print(json.dumps(line), flush=True)
+    del g, x
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("configs", nargs="*", default=["c1", "c3", "c5"])
@@ -728,6 +795,8 @@ def main():
         c12(a)
     if "c13" in a.configs:
         c13(a)
+    if "c14" in a.configs:
+        c14(a)
     if "c3" in a.configs:
         nf, nd = int(100_000_000 * a.scale), int(10_000_000 * a.scale)
         fs = [(0, 1, T.INT32, 0, 1, 0, nd, 1.0), (0, 2, T.DOUBLE, 1, 2, 0, 0, 1.0)]

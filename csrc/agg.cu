@@ -32,12 +32,32 @@ static __device__ __noinline__ void hll_row(const AggArgs& a, const uint64_t* ou
         else hll_add_value(a.gt, s, a.gt.lanes, a.gt.cap_mask + 1, slot, out[s.arg_out]);
     }
 }
+// the AG_RB aggregates of one row that reached group `slot`: each non-NULL argument appends its pair key (AggArgs::rb_keys) with one
+// atomic per warp.  rb_build_agg adds get_numberic<uint32_t>(value): the low 32 bits of the integer image (agg_fn_call.cpp:642-651)
+static __device__ __noinline__ void rb_row(const AggArgs& a, const uint64_t* out, uint32_t out_null, int slot) {
+    const AggPlan& ap = a.plan;
+    const int lane = threadIdx.x & 31;
+    for (int i = 0; i < ap.n_agg; i++) {
+        const AggSpec s = ap.agg[i];
+        if (s.kind != AG_RB) continue;
+        const bool has = !((out_null >> s.arg_out) & 1u);
+        const unsigned m = __ballot_sync(__activemask(), has);
+        if (!has) continue;
+        const int leader = __ffs(m) - 1;
+        unsigned long long base = 0;
+        if (lane == leader) base = atomicAdd(a.rb_ctr, (unsigned long long)__popc(m));
+        base = __shfl_sync(m, base, leader);
+        const unsigned long long pos = base + (unsigned long long)__popc(m & ((1u << lane) - 1u));
+        if (pos < a.rb_cap) a.rb_keys[pos] = ((uint64_t)slot << 34) | ((uint64_t)s.rb_idx << 32) | (uint32_t)out[s.arg_out];
+    }
+}
 // one (possibly joined) row through the program into the tables
 struct InterpCtx { SmemTable st; bool grouped, use_smem; uint32_t gcap; };
 // how: 0 = filter, then aggregate the row; 1 = filter only (SEMI / ANTI probe: does the joined row satisfy the conditions?);
 //      2 = aggregate without the filter (the NULL-extended / preserved rows of the join's tail)
-// HLL: the plan has AG_HLL aggregates (the instantiation without them keeps the interpreter's registers as they were)
-template <bool HLL = false>
+// MODE: IM_HLL = the plan has AG_HLL aggregates, IM_RB = AG_RB aggregates (IM_PLAIN keeps the interpreter's registers as they were)
+enum InterpMode { IM_PLAIN = 0, IM_HLL = 1, IM_RB = 2 };
+template <int MODE = IM_PLAIN>
 __device__ __forceinline__ uint32_t interp_row(const AggArgs& a, const InterpCtx& cx, int64_t row, int64_t brow, int how = 0) {
     const AggPlan& ap = a.plan;
     const GroupTable& gt = a.gt;
@@ -51,11 +71,11 @@ __device__ __forceinline__ uint32_t interp_row(const AggArgs& a, const InterpCtx
         if (r == 0xFF) { v = 0; isnull = true; return; }
         v = out[r]; isnull = (out_null >> r) & 1u;
     };
-    // hll_add_agg (a plan with AG_HLL never uses the shared table: a sketch lives in the global table's arena)
-    auto hll = [&](int slot) { if (HLL) hll_row(a, out, out_null, slot); };
+    // hll_add_agg / rb_build_agg (such a plan never uses the shared table: a sketch lives in the global table's arena, a pair in its buffer)
+    auto sketch = [&](int slot) { if (MODE == IM_HLL) hll_row(a, out, out_null, slot); else if (MODE == IM_RB) rb_row(a, out, out_null, slot); };
     if (!cx.grouped) {  // single group: slot 0 of the global table
         accumulate_row<false>(a, gt.lanes, cx.gcap, 0, arg);
-        hll(0);
+        sketch(0);
         return 1;
     }
     uint64_t key[MAX_KEYW];
@@ -75,12 +95,12 @@ __device__ __forceinline__ uint32_t interp_row(const AggArgs& a, const InterpCtx
     else {
         slot = table_upsert<false, 0>(gt.state, gt.keys, gt.cap_mask, key, ap.n_keyw, h, (int)cx.gcap, gt.n_groups);
         if (slot < 0) atomicExch(gt.overflow, 1u);
-        else { accumulate_row<false>(a, gt.lanes, cx.gcap, slot, arg); hll(slot); }
+        else { accumulate_row<false>(a, gt.lanes, cx.gcap, slot, arg); sketch(slot); }
     }
     return 1;
 }
 
-template <bool HLL>
+template <int MODE>
 __global__ void __launch_bounds__(256) k_agg_interp(const __grid_constant__ AggArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const AggPlan& ap = a.plan;
@@ -95,11 +115,11 @@ __global__ void __launch_bounds__(256) k_agg_interp(const __grid_constant__ AggA
         const int jt = a.join.join_type;
         for (int64_t br = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; br < a.join.n_build; br += (int64_t)gridDim.x * blockDim.x) {
             const uint8_t m = a.join.matched[br];   // (2: removed by the build side's own filter, never emitted)
-            if (jt == 4 /*SEMI*/ ? m == 1 : m == 0) passed += interp_row<HLL>(a, cx, -1, br, 2);
+            if (jt == 4 /*SEMI*/ ? m == 1 : m == 0) passed += interp_row<MODE>(a, cx, -1, br, 2);
         }
     } else
     for (int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; row < a.nrows; row += (int64_t)gridDim.x * blockDim.x) {
-        if (!a.join.enabled) { passed += interp_row<HLL>(a, cx, row, -1); continue; }
+        if (!a.join.enabled) { passed += interp_row<MODE>(a, cx, row, -1); continue; }
         // K4 probe: every build row whose cast key equals this row's (Joiner::encode_hash_key + FlatMap seek,
         // src/exec/joiner.cpp:608-622, join_node.cpp:1290-1292); a NULL key never matches (SQL / Acero hashjoin)
         const DevCol& pc = a.cols[a.join.probe_col];
@@ -110,8 +130,8 @@ __global__ void __launch_bounds__(256) k_agg_interp(const __grid_constant__ AggA
             const uint32_t br = a.join.rows[slot];
             if (br == 0xFFFFFFFFu) break;
             if (a.join.keys[slot] == img) {
-                if (a.join.join_type == 3 /*INNER*/ || !a.join.matched) passed += interp_row<HLL>(a, cx, row, (int64_t)br);
-                else if (a.join.join_type == 1 /*LEFT*/) { if (interp_row<HLL>(a, cx, row, (int64_t)br)) { passed++; a.join.matched[br] = 1; } }
+                if (a.join.join_type == 3 /*INNER*/ || !a.join.matched) passed += interp_row<MODE>(a, cx, row, (int64_t)br);
+                else if (a.join.join_type == 1 /*LEFT*/) { if (interp_row<MODE>(a, cx, row, (int64_t)br)) { passed++; a.join.matched[br] = 1; } }
                 else if (interp_row(a, cx, row, (int64_t)br, 1)) a.join.matched[br] = 1;   // SEMI / ANTI_SEMI: only whether a partner exists
             }
             slot = (slot + 1) & a.join.cap_mask;
@@ -491,7 +511,7 @@ cudaError_t launch_agg(const AggArgs& a, AggKernel k, size_t smem, int sm_count,
     if (a.nrows <= 0) return cudaSuccess;
     switch (k) {
         case INTERP: {
-            auto kern = a.gt.hll_regs ? k_agg_interp<true> : k_agg_interp<false>;
+            auto kern = a.gt.hll_regs ? k_agg_interp<IM_HLL> : a.rb_keys ? k_agg_interp<IM_RB> : k_agg_interp<IM_PLAIN>;
             if (smem > 48 * 1024) {
                 cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
                 if (e != cudaSuccess) return e;

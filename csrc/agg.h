@@ -66,6 +66,11 @@ struct AggArgs {
     // [32-byte counter block][values n_img x n][null bytes n_img x n], n = the groups in the table.  nullptr = no fused extraction
     uint8_t* fused_out;
     uint32_t fused_cap;      // rows the buffer holds: a table with more groups leaves only the counter block there (the host runs k_extract)
+    // rb_build_agg: the pair buffer, one key per (row, AG_RB aggregate) with a non-NULL value: slot << 34 | rb_idx << 32 | low 32 bits of the
+    // value.  *rb_ctr = keys appended (past rb_cap: keys were lost, the request fails with ETOOBIG).  nullptr without AG_RB
+    uint64_t* rb_keys;
+    unsigned long long* rb_ctr;
+    uint64_t rb_cap;
 };
 
 // typed columns built from the aggregate's extracted images (input of the post fragment)

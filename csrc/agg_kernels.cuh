@@ -214,6 +214,7 @@ __device__ __forceinline__ void extract_group(const GroupTable& gt, const AggPla
             case AG_COUNT_STAR: v = nrows; break;
             case AG_COUNT: v = cnt; break;
             case AG_COUNT_MERGE: case AG_HLL: v = acc; break;   // (AG_HLL: the sketch reference; the host copies its registers)
+            case AG_RB: v = i; break;   // the group's slot: the host finds its bitmaps by (slot, rb_idx)
             case AG_AVG:   // (AVG's sum starts from +0.0 in the reference, agg_initialize: + 0.0 turns the lane's -0.0 into +0.0)
                 if (cnt == 0) isnull = 1; else v = f64_bits(__ddiv_rn(__dadd_rn(bits_f64(acc), 0.0), (double)(int64_t)cnt));
                 break;

@@ -98,7 +98,7 @@ int select_agg_launch(const Compiled& c, const DevCol* cols, int64_t nrows, bool
     out = AggSelection{};
     memset(&a, 0, sizeof a);
     a.plan = c.ap; a.prog = c.prog; a.direct = c.direct;
-    const bool direct = c.has_direct && vec_ok && !env.force_generic && c.kind == PK_AGG && !c.ap.n_hll;   // (the join's fast-path plan is lowered as PK_AGG)
+    const bool direct = c.has_direct && vec_ok && !env.force_generic && c.kind == PK_AGG && !c.ap.n_hll && !c.n_rb;   // (the join's fast-path plan is lowered as PK_AGG)
     const int ncols = (int)c.cols.size();
     if (direct) { for (size_t i = 0; i < c.direct_cols.size(); i++) a.cols[i] = cols[c.direct_cols[i]]; a.n_cols = (int)c.direct_cols.size(); }
     else { for (int i = 0; i < ncols; i++) a.cols[i] = cols[i]; a.n_cols = ncols; }
@@ -107,7 +107,7 @@ int select_agg_launch(const Compiled& c, const DevCol* cols, int64_t nrows, bool
     a.smem_lane[0] = 0; a.n_smem_lanes = 1; a.alias_mask = 0;
     for (int k = 0; k < a.plan.n_agg; k++) {
         AggSpec& s = a.plan.agg[k];
-        if (s.kind == AG_COUNT_STAR) continue;
+        if (s.kind == AG_COUNT_STAR || s.kind == AG_RB) continue;   // (AG_RB: no lane; its keys go to the pair buffer)
         bool nullable = c.arg_can_null[(size_t)k] || env.tail_launch;   // (the tail's probe-side columns are NULL on every row)
         for (int i = 0; i < ncols; i++) if ((c.arg_cols_mask[(size_t)k] >> i) & 1) nullable = nullable || cols[i].validity != nullptr;
         s.nullable = nullable ? 1 : 0;
@@ -118,7 +118,7 @@ int select_agg_launch(const Compiled& c, const DevCol* cols, int64_t nrows, bool
         if (s.kind != AG_COUNT && a.smem_lane[s.acc_lane] == 0xFF) a.smem_lane[s.acc_lane] = (uint8_t)a.n_smem_lanes++;
     }
     for (int l = 1; l < a.plan.n_lanes; l++) if (a.smem_lane[l] != 0xFF) a.alias_mask &= ~(1u << l);
-    a.smem_cap_log2 = c.ap.n_hll ? 0 : pick_smem_log2(env, a.plan.n_keyw, a.n_smem_lanes, direct, c.direct.n_vals);   // (a sketch lives in the global table's arena)
+    a.smem_cap_log2 = c.ap.n_hll || c.n_rb ? 0 : pick_smem_log2(env, a.plan.n_keyw, a.n_smem_lanes, direct, c.direct.n_vals);   // (a sketch lives in the global table's arena, a pair in its buffer: both need the global slot)
     a.smem_sentinel = direct && a.plan.n_keyw == 1 ? 1 : 0;
     a.smem_keyw = a.plan.n_keyw;
 

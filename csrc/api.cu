@@ -193,6 +193,7 @@ extern "C" int bkgpu_set_option(bkgpu_plan* p, const char* key, int64_t v) {
     else if (k == "smem_capacity_log2") { if (v < -1 || v > 13) return p->fail(BKGPU_EINVAL, "smem_capacity_log2 out of range"); p->smem_cap_log2 = (int)v; }
     else if (k == "batch_capacity") { if (v < 1) return p->fail(BKGPU_EINVAL, "batch_capacity must be positive"); p->batch_capacity = v; }
     else if (k == "chunk_rows") { if (v < 1024) return p->fail(BKGPU_EINVAL, "chunk_rows too small"); p->chunk_rows = (v + 7) & ~7ll; }
+    else if (k == "rb_pair_capacity") { if (v < 1024 || v > ((int64_t)1 << 31)) return p->fail(BKGPU_EINVAL, "rb_pair_capacity out of range (1024 .. 2^31)"); p->rb_cap = v; }
     else if (k == "hll_group_capacity") { if (v < 1 || v > (1 << 20)) return p->fail(BKGPU_EINVAL, "hll_group_capacity out of range (1 .. 2^20)"); p->hll_cap = v; }
     else if (k == "partial_capacity") { if (v < 1) return p->fail(BKGPU_EINVAL, "partial_capacity must be positive"); p->partial_cap = v; }
     else if (k == "force_generic") p->force_generic = v != 0;
@@ -231,6 +232,14 @@ static int alloc_group_table(bkgpu_plan* p) {
         if ((rc = dev_alloc(p, (void**)&gt.hll_ctr, 16))) return rc;
         gt.hll_cap = (uint32_t)p->hll_cap;
         CK(p, cudaMemsetAsync(gt.hll_ctr, 0, 16, p->stream));
+    }
+    if (p->c.n_rb) {   // rb_build_agg: the pair buffer and the sort's second buffer (one word more each: the build's scan closes on it)
+        if ((rc = dev_alloc(p, (void**)&p->rb.keys, ((size_t)p->rb_cap + 1) * 8))) return rc;
+        if ((rc = dev_alloc(p, (void**)&p->rb.alt, ((size_t)p->rb_cap + 1) * 8))) return rc;
+        if ((rc = dev_alloc(p, (void**)&p->rb.ctr, 8))) return rc;
+        p->rb.cap = (uint64_t)p->rb_cap;
+        CK(p, cudaMemsetAsync(p->rb.ctr, 0, 8, p->stream));
+        p->rb.hi = 0;
     }
     p->d_cursor = gt.n_groups + 2;                       // [2] result cursor [3] merge info
     p->d_rows_passed = (uint64_t*)(gt.n_groups + 4);     // [4..5] rows that passed the filter
@@ -278,6 +287,8 @@ extern "C" int bkgpu_open(bkgpu_plan* p) {
     if (p->c.ap.n_hll && (p->repartition || p->peer_merge))
         return p->fail(BKGPU_EUNSUPPORTED, "hll_add_agg with the %s merge is outside the GPU path: its sketches travel only with the all-gather of group rows",
                        p->repartition ? "repartition" : "peer_merge");
+    if (p->c.n_rb && p->nccl_comm)
+        return p->fail(BKGPU_EUNSUPPORTED, "rb_build_agg with a communicator is outside the GPU path: bitmaps do not travel with the fixed-width partial rows");
     int rc = upload_in_sets(p);   // (before sort_open: it copies the programs)
     if (rc) return rc;
     if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) rc = alloc_group_table(p);
@@ -324,6 +335,26 @@ static bool ensure_fused(bkgpu_plan* p) {
     return true;
 }
 
+// rb_build_agg: a launch appends at most one key per row and rb_build_agg aggregate, except where a probe row meets several build rows (such
+// a launch can still overflow the pair buffer, and the request then fails at bkgpu_finish).  When the keys could outgrow the buffer, it is
+// sorted and deduplicated first (a set does not depend on order), and the launch shrinks to the rows that fit
+static int rb_room(bkgpu_plan* p, const Compiled& c, int64_t* rows) {
+    const uint64_t per = (uint64_t)c.n_rb, cap = p->rb.cap;
+    if (p->rb.hi + (uint64_t)*rows * per > cap) {
+        uint64_t n = 0;
+        const int rc = rb_compact(p, &n);
+        if (rc) return rc;
+        p->rb.hi = n;
+        const int64_t fit = (int64_t)((cap - n) / per) & ~7ll;   // (a multiple of 8 rows: the next launch's validity bitmaps stay byte-aligned)
+        if (fit < 8)
+            return p->fail(BKGPU_ETOOBIG, "rb_build_agg: the pair buffer holds %llu distinct (group, value) pairs and is full: raise rb_pair_capacity",
+                           (unsigned long long)n);
+        if (*rows > fit && !p->join.tail_launch) *rows = fit;   // (the join's tail walks every build row in one launch)
+    }
+    p->rb.hi += (uint64_t)*rows * per;
+    return BKGPU_OK;
+}
+
 int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp) {
     AggEnv env;
     env.force_generic = p->force_generic; env.no_lean = p->no_lean; env.no_lean_nulls = p->no_lean_nulls; env.no_lean_mm = p->no_lean_mm;
@@ -343,9 +374,16 @@ int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64
     const int64_t kMax = (int64_t)1 << 30;  // rows per launch (32-bit counters inside a CTA)
     int64_t algo_bytes_per_row = 0;
     for (int i = 0; i < a.n_cols; i++) algo_bytes_per_row += storage_bytes(a.cols[i].stype);
-    for (int64_t off = 0; off < nrows; off += kMax) {
+    int64_t b_rows = 0;
+    for (int64_t off = 0; off < nrows; off += b_rows) {
         AggArgs b = a;
         b.nrows = std::min(kMax, nrows - off);
+        if (c.n_rb) {   // (a compaction swaps the pair buffer with the sort's second buffer)
+            const int rrc = rb_room(p, c, &b.nrows);
+            if (rrc) return rrc;
+            b.rb_keys = p->rb.keys; b.rb_ctr = p->rb.ctr; b.rb_cap = p->rb.cap;
+        }
+        b_rows = b.nrows;
         for (int i = 0; i < b.n_cols; i++) b.cols[i] = col_at(a.cols[i], off);
         EventPair* ep = timer_begin(p, p->timed, b.nrows * algo_bytes_per_row, false);
         cudaError_t e = launch_agg(b, sel.kernel, sel.smem, p->sm_count, p->stream, ep ? ep->a : nullptr);
@@ -840,6 +878,32 @@ static int agg_take_counters(bkgpu_plan* p, const uint32_t* ctr) {
     return BKGPU_OK;
 }
 
+// a BITMAP column (bkgpu.h): one bitmap per row, each the device's bytes for (slot, rb_idx), or the 8-byte empty bitmap
+// ("3a300000 00000000": the reference's initialize gives every group an empty bitmap, so a group whose values were all NULL returns it)
+static void rb_column(bkgpu_plan* p, HostCol& hc, const uint64_t* slot, int64_t rows, int rb_idx) {
+    static const uint8_t empty[8] = {0x3a, 0x30, 0, 0, 0, 0, 0, 0};
+    std::vector<int64_t> b((size_t)rows);   // each row's bitmap in the directory, -1 = none
+    int64_t total = 0;
+    for (int64_t r = 0; r < rows; r++) {
+        const uint32_t id = (uint32_t)(slot[r] << 2) | (uint32_t)rb_idx;
+        const auto it = std::lower_bound(p->rb.bid.begin(), p->rb.bid.end(), id);
+        b[r] = it != p->rb.bid.end() && *it == id ? (int64_t)(it - p->rb.bid.begin()) : -1;
+        total += b[r] < 0 ? 8 : (int64_t)(p->rb.off[b[r] + 1] - p->rb.off[b[r]]);
+    }
+    std::vector<uint8_t>& col = p->rb.col[rb_idx];
+    col.resize(((size_t)rows + 1) * 8 + (size_t)total);
+    int64_t* offs = (int64_t*)col.data();
+    uint8_t* d = col.data() + ((size_t)rows + 1) * 8;
+    offs[0] = 0;
+    for (int64_t r = 0; r < rows; r++) {
+        const size_t len = b[r] < 0 ? 8 : (size_t)(p->rb.off[b[r] + 1] - p->rb.off[b[r]]);
+        memcpy(d + offs[r], b[r] < 0 ? empty : p->rb.bytes + p->rb.off[b[r]], len);
+        offs[r + 1] = offs[r] + (int64_t)len;
+    }
+    hc.elem = -1;
+    hc.varlen = &col;
+}
+
 // typed host columns from `n_out` extracted rows (images + null bytes, column-major with stride `stride`), after OFFSET / LIMIT
 static void agg_result(bkgpu_plan* p, const uint64_t* hv, const uint8_t* hn, size_t stride, uint32_t n_out) {
     const int64_t rows = n_out;
@@ -849,13 +913,19 @@ static void agg_result(bkgpu_plan* p, const uint64_t* hv, const uint8_t* hn, siz
     int64_t keep = rows - skip;
     if (lim >= 0 && keep > lim) keep = lim;
     p->result.clear();
-    int img = 0;
+    int img = 0, rb_idx = 0;
     for (const OutCol& oc : p->c.out_cols) {
         HostCol hc; hc.desc = oc;
-        hc.elem = oc.kind == 1 ? 16 : oc.kind == 2 ? HLL_RAW_BYTES : storage_bytes(prim_storage(oc.prim));
-        hc.values.assign((size_t)std::max<int64_t>(keep, 1) * (size_t)hc.elem, 0);
         const uint64_t* v = hv + (size_t)img * stride + skip;
         const uint8_t* nb = hn + (size_t)img * stride + skip;
+        if (oc.kind == 3) {   // rb_build_agg: the group's slot, whose bitmap the device build serialized (a group without a value: the empty one)
+            rb_column(p, hc, v, keep, rb_idx++);
+            img++;
+            p->result.push_back(std::move(hc));
+            continue;
+        }
+        hc.elem = oc.kind == 1 ? 16 : oc.kind == 2 ? HLL_RAW_BYTES : storage_bytes(prim_storage(oc.prim));
+        hc.values.assign((size_t)std::max<int64_t>(keep, 1) * (size_t)hc.elem, 0);
         // (a NULL's image is 0, which is also what a NULL row's value bytes hold)
         uint8_t* d = hc.values.data();
         if (oc.kind == 1) {
@@ -992,6 +1062,7 @@ static int agg_finish(bkgpu_plan* p) {
     uint32_t n_out = finish_n_out, out_cap = finish_out_cap;
     if (n_out > out_cap) n_out = out_cap;
     if ((rc = hll_fetch(p))) return rc;
+    if (p->c.n_rb && (rc = rb_build(p))) return rc;
     if (p->c.post) return agg_post(p, n_out, out_cap);
     agg_result(p, finish_hv, finish_hn, out_cap, n_out);
     return BKGPU_OK;
@@ -1072,6 +1143,19 @@ extern "C" int bkgpu_get_next(bkgpu_plan* p, bkgpu_column* out_cols, int* ncols,
         HostCol& hc = p->result[(size_t)i];
         bkgpu_column& o = out_cols[i];
         o.tuple_id = hc.desc.tuple_id; o.slot_id = hc.desc.slot_id; o.prim_type = hc.desc.prim; o.elem_size = hc.elem;
+        if (hc.elem < 0) {   // variable-length values: this batch's n + 1 offsets (from 0), then its bytes
+            const int64_t* all = (const int64_t*)hc.varlen->data();
+            const uint8_t* bytes = hc.varlen->data() + ((size_t)p->result_rows + 1) * 8;
+            if (p->result_pos == 0 && n == p->result_rows) o.values = hc.varlen->data();   // (the whole column in one batch: as it is)
+            else {
+                const int64_t b0 = all[p->result_pos], b1 = all[p->result_pos + n];
+                hc.batch.resize(((size_t)n + 1) * 8 + (size_t)(b1 - b0));
+                int64_t* offs = (int64_t*)hc.batch.data();
+                for (int64_t r = 0; r <= n; r++) offs[r] = all[p->result_pos + r] - b0;
+                if (b1 > b0) memcpy(hc.batch.data() + ((size_t)n + 1) * 8, bytes + b0, (size_t)(b1 - b0));
+                o.values = hc.batch.data();
+            }
+        } else
         o.values = hc.values.data() + (size_t)p->result_pos * (size_t)hc.elem;
         o.length = n;
         o.validity = nullptr;
@@ -1110,6 +1194,7 @@ static int bkgpu_reset_impl(bkgpu_plan* p) {
         else CK(p, launch_table_init(p->gt, p->c.ap, p->stream));
         p->finish_groups = -1;
         p->fused_last = false;
+        if (p->rb.ctr) { CK(p, cudaMemsetAsync(p->rb.ctr, 0, 8, p->stream)); p->rb.hi = 0; }   // (rb_build_agg: the pair buffer is empty again)
         p->stats.kernel_launches++;
     }
     join_reset(p);
@@ -1144,6 +1229,7 @@ extern "C" void bkgpu_close(bkgpu_plan* p) {
     if (p->wait_event) cudaEventDestroy(p->wait_event);
     if (p->h_pinned) cudaFreeHost(p->h_pinned);
     if (p->h_outv) cudaFreeHost(p->h_outv);
+    if (p->rb.bytes) cudaFreeHost(p->rb.bytes);
     if (p->h_fused && !mapped_cache().put(p->fused_bytes, p->h_fused)) cudaFreeHost(p->h_fused);   // (the stream was drained above)
     if (p->copy_stream) cudaStreamDestroy(p->copy_stream);
     if (p->own_stream && p->stream) cudaStreamDestroy(p->stream);
@@ -1232,6 +1318,7 @@ extern "C" int bkgpu_push_region(bkgpu_plan* p, int64_t region_id) {
 // ------------------------------------------------------------------ partial state
 extern "C" int bkgpu_partial_capacity(bkgpu_plan* p, size_t* bytes) {
     if (!p || !bytes) return thread_fail(BKGPU_EINVAL, "bkgpu_partial_capacity: NULL argument");
+    if (p->c.n_rb) return p->fail(BKGPU_EUNSUPPORTED, "rb_build_agg has no partial state: bitmaps do not fit the fixed-width partial rows");
     if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) {   // (a sketch's registers ride along: HLL_ROW_WORDS per hll_add_agg)
         *bytes = 8 * (1 + (size_t)(p->c.ap.n_keyw + p->c.ap.n_lanes + p->c.ap.n_hll * HLL_ROW_WORDS) * (size_t)eff_pcap(p));
         return BKGPU_OK;

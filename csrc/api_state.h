@@ -13,6 +13,7 @@
 #include "plan.h"
 #include "sort.h"
 #include "window.h"
+#include "rb.h"
 
 using namespace bk;
 
@@ -25,6 +26,8 @@ struct HostCol {  // one materialised result column (host memory owned by the pl
     int elem = 0;
     std::vector<uint8_t> values;
     std::vector<uint8_t> validity;  // LSB bitmap; empty = all valid
+    const std::vector<uint8_t>* varlen = nullptr;   // elem < 0 (BITMAP): the whole column, rows + 1 int64 offsets then the bytes
+    std::vector<uint8_t> batch;     // elem < 0: a later bkgpu_get_next batch, re-based (n + 1 offsets from 0, then its bytes)
     void* dev_values = nullptr;     // output_on_device
 };
 
@@ -96,6 +99,8 @@ struct bkgpu_plan {
     int64_t partial_cap = 1 << 16;
     int64_t hll_cap = 4096;       // option hll_group_capacity: sketches the register arena holds (16 KB each: 64 MB by default)
     std::vector<uint8_t> hll_host;   // the arena's claimed blocks, copied back by a finished request (agg_result reads the sketches there)
+    int64_t rb_cap = (int64_t)1 << 27;   // option rb_pair_capacity: keys the rb_build_agg pair buffer holds (8 bytes each, twice: the sort's buffers)
+    RbState rb;                   // rb_build_agg's pair buffer and build (rb.h)
     int force_generic = 0;
     int no_lean = 0;
     int output_on_device = 0;

@@ -95,7 +95,8 @@ struct Program {
 // so several aggregates share one counter).
 enum AggKind : uint8_t { AG_COUNT_STAR = 0, AG_COUNT = 1, AG_SUM = 2, AG_AVG = 3, AG_MIN = 4, AG_MAX = 5,
                          AG_COUNT_MERGE = 6,     // MERGE_AGG_NODE: counts shipped by the stores are summed (AggFnCall::merge, agg_fn_call.cpp:779-790)
-                         AG_HLL = 7 };           // hll_add_agg: the value lane holds the group's sketch (index + 1 into GroupTable::hll_regs, 0 = none yet)
+                         AG_HLL = 7,             // hll_add_agg: the value lane holds the group's sketch (index + 1 into GroupTable::hll_regs, 0 = none yet)
+                         AG_RB = 8 };            // rb_build_agg: no lane; each non-NULL value appends a key to AggArgs::rb_keys (rb.cu builds the bitmaps)
 enum LaneOp : uint8_t { LN_ADD_I64 = 0, LN_ADD_F64 = 1, LN_MIN_I64, LN_MAX_I64, LN_MIN_U64, LN_MAX_U64, LN_MIN_F64, LN_MAX_F64,
                         LN_HLL };                // a sketch reference: never combined as a number (its registers are, by the export / merge kernels)
 
@@ -115,7 +116,10 @@ struct AggSpec {
     uint8_t arg_prim;    // AG_HLL: the argument's type after inference, which sets the bytes hashed (hll_key_bytes); with arg_vclass VC_U64
                          // a FLOAT argument arrives as the column's own 4 bytes (OP_LOAD_COL b = 3), else as its widened double.
                          // BK_HLL: MERGE_AGG over RAW sketches: the argument is the row (OP_LOAD_COL b = 4) of column `hll_col`
-    uint8_t hll_col;
+    union {
+        uint8_t hll_col;
+        uint8_t rb_idx;  // AG_RB: which of the plan's rb_build_agg aggregates (0 .. MAX_RB - 1), bits 32-33 of its pair keys
+    };
 };
 
 struct AggPlan {
@@ -181,6 +185,7 @@ struct GroupTable {
     uint32_t* hll_ctr;
     uint32_t hll_cap;    // blocks the arena holds
 };
+constexpr int MAX_RB = 4;             // rb_build_agg aggregates per plan: two key bits name the bitmap's aggregate
 constexpr int HLL_ROW_WORDS = 2048;   // one sketch's 16384 registers as 64-bit words of an exported group row
 constexpr uint64_t HLL_LANE_BUSY = ~0ull;          // a sketch lane while its block is being claimed and zeroed
 constexpr uint64_t HLL_LANE_FULL = ~0ull - 1;      // a sketch lane whose claim found the arena full (the request fails with ETOOBIG)

@@ -397,6 +397,16 @@ static bool infer_expr(Infer& in, HExpr& e) {
                     return in.fail(BKGPU_EUNSUPPORTED, "hll_add_agg over a STRING argument is outside the GPU path: a dictionary code would be hashed, not the text");
                 if (ct != BK_NULL_TYPE && !hll_key_bytes(ct)) return in.fail(BKGPU_EUNSUPPORTED, "hll_add_agg over an argument of type %d is outside the GPU path", ct);
                 e.col_type = BK_HLL;
+            } else if (e.name == "rb_build_agg") {   // agg_fn_call.cpp:132-141: BITMAP; update adds get_numberic<uint32_t>(value) (:642-651)
+                if (e.ch.empty()) return in.fail(BKGPU_EINVAL, "rb_build_agg() without an argument");
+                if (is_double_t(ct))
+                    return in.fail(BKGPU_EUNSUPPORTED, "rb_build_agg over a FLOAT / DOUBLE argument is outside the GPU path: only integer and BOOL values are lowered");
+                if (ct == BK_STRING)
+                    return in.fail(BKGPU_EUNSUPPORTED, "rb_build_agg over a STRING argument is outside the GPU path: a dictionary code would be added, not the value");
+                if (ct == BK_DATETIME || ct == BK_TIMESTAMP || ct == BK_DATE || ct == BK_TIME)
+                    return in.fail(BKGPU_EUNSUPPORTED, "rb_build_agg over a date / time argument (type %d) is outside the GPU path", ct);
+                if (ct != BK_NULL_TYPE && ct != BK_BOOL && !is_int_t(ct)) return in.fail(BKGPU_EUNSUPPORTED, "rb_build_agg over an argument of type %d is outside the GPU path", ct);
+                e.col_type = BK_BITMAP;
             } else if (e.name == "hll_merge_agg") {
                 return in.fail(BKGPU_EUNSUPPORTED, "hll_merge_agg over stored sketches is outside the GPU path: a DENSE or SPARSE sketch varies in length");
             } else return in.fail(BKGPU_EUNSUPPORTED, "aggregate '%s' is outside the GPU path", e.name.c_str());
@@ -896,7 +906,7 @@ static bool lower_agg(Infer& in, Compiled& out, const HNode& agg, const std::vec
     if (agg.group_exprs.size() > MAX_GROUP) return in.fail(BKGPU_EUNSUPPORTED, "more than %d GROUP BY expressions", MAX_GROUP);
     if (agg.agg_fns.size() > MAX_AGG) return in.fail(BKGPU_EUNSUPPORTED, "more than %d aggregate functions", MAX_AGG);
     Program& p = out.prog; memset(&p, 0, sizeof p);
-    AggPlan& ap = out.ap; memset(&ap, 0, sizeof ap);
+    AggPlan& ap = out.ap; memset(&ap, 0, sizeof ap); out.n_rb = 0;
     Lower lw{&out, &in, &p};
     int reg = 0, depth = 0;
     // ---- predicate: all conjuncts non-NULL true (filter_node.cpp:726-734) ----
@@ -982,6 +992,8 @@ static bool lower_agg(Infer& in, Compiled& out, const HNode& agg, const std::vec
             ap.n_hll++;
             continue;
         }
+        if (out.is_merge && f.name == "rb_build_agg")
+            return in.fail(BKGPU_EUNSUPPORTED, "MERGE_AGG of rb_build_agg is outside the GPU path: its input would be the stores' variable-length bitmaps");
         if (out.is_merge && !f.distinct) {
             // MERGE_AGG_NODE: the input rows carry the stores' intermediate slots; AggFnCall::merge (agg_fn_call.cpp:719-822)
             // adds counts and sums, folds MIN/MAX, and adds both halves of an AVG blob.  NULL intermediates are skipped.
@@ -1056,6 +1068,23 @@ static bool lower_agg(Infer& in, Compiled& out, const HNode& agg, const std::vec
             ap.n_hll++;
             continue;
         }
+        if (f.name == "rb_build_agg") {
+            // no lane: each non-NULL value appends a (slot, rb_idx, low 32 bits) key to the pair buffer, which rb.cu turns into the bitmaps
+            if (out.n_rb >= MAX_RB) return in.fail(BKGPU_EUNSUPPORTED, "more than %d rb_build_agg in one aggregate is outside the GPU path", MAX_RB);
+            a.kind = AG_RB; a.arg_prim = (uint8_t)arg.col_type; a.nullable = 1; a.rb_idx = (uint8_t)out.n_rb++;
+            a.acc_lane = a.cnt_lane = 0xFF;
+            const std::string rkey = expr_key(arg);
+            if (!arg_reg_of.count(rkey)) {
+                depth = 0;
+                if (!lw.expr(arg, depth)) return false;
+                arg_reg_of[rkey] = reg;
+                if (!lw.out_reg(reg++)) return false;
+            }
+            a.arg_out = (uint8_t)arg_reg_of[rkey];
+            a.arg_vclass = (uint8_t)host_prim_class(arg.col_type);
+            int m = 0; expr_cols(arg, out, m); out.arg_cols_mask[(size_t)k] = m; out.arg_can_null[(size_t)k] = expr_makes_null(arg);
+            continue;
+        }
         std::string key = expr_key(arg);
         if (!arg_reg_of.count(key)) {
             depth = 0;
@@ -1097,7 +1126,8 @@ static bool lower_agg(Infer& in, Compiled& out, const HNode& agg, const std::vec
         int ft = in.slot_type(f.tuple_id, f.final_slot);
         if (ft == BK_INVALID_TYPE || ft == BK_STRING) ft = f.col_type;
         if (ap.agg[k].kind == AG_HLL) ft = BK_HLL;
-        out.out_cols.push_back({f.tuple_id, f.final_slot, ft, ap.agg[k].kind == AG_HLL ? 2 : 0});
+        if (ap.agg[k].kind == AG_RB) ft = BK_BITMAP;
+        out.out_cols.push_back({f.tuple_id, f.final_slot, ft, ap.agg[k].kind == AG_HLL ? 2 : ap.agg[k].kind == AG_RB ? 3 : 0});
         ap.agg[k].out_prim = (uint8_t)ft;
         if (ap.agg[k].kind == AG_AVG) out.out_cols.push_back({f.tuple_id, f.inter_slot != f.final_slot ? f.inter_slot : -1, BK_STRING, 1});
     }
@@ -1106,7 +1136,7 @@ static bool lower_agg(Infer& in, Compiled& out, const HNode& agg, const std::vec
     DirectPlan& d = out.direct; memset(&d, 0, sizeof d); memset(d.agg_val, 0xFF, sizeof d.agg_val);
     do {
         std::vector<int> order;  // cols indices in [terms][key][values] order
-        if (!allow_direct || out.is_merge || ap.n_hll) break;
+        if (!allow_direct || out.is_merge || ap.n_hll || out.n_rb) break;
         if (!conjuncts.empty()) {
             if (conjuncts.size() > 2) break;
             bool ok = true;
@@ -1211,6 +1241,9 @@ static void explain(Compiled& c) {
             } else if (a.kind == AG_HLL) {
                 snprintf(buf, sizeof buf, "    hll_add_agg: arg_prim=%d hashes %d bytes%s (MurmurHash3_x64_128, seed 0x110) -> 16384 registers, RAW sketch of %d bytes\n",
                          a.arg_prim, hll_key_bytes(a.arg_prim), a.arg_vclass == VC_U64 && a.arg_prim == BK_FLOAT ? " of the FLOAT column" : "", HLL_RAW_BYTES); s += buf;
+            } else if (a.kind == AG_RB) {
+                snprintf(buf, sizeof buf, "    rb_build_agg: rb=%d arg_prim=%d adds the low 32 bits of the value -> pair key (slot << 34 | %d << 32 | value), "
+                         "Roaring bitmap (runOptimize, portable serialization)\n", a.rb_idx, a.arg_prim, a.rb_idx); s += buf;
             }
         }
         if (c.has_direct) {
@@ -2087,11 +2120,17 @@ int compile_plan(const uint8_t* desc, size_t len, Compiled& out, std::string& er
         // LimitNode straight over the aggregate: the result extraction (agg_result) skips `offset` groups and then keeps `limit` of them,
         // so the limit is stored as it is — not as the first limit + offset rows that a sort or a filter keeps before skipping
         if (ok && limit_node && !post_sort && !post_having) { out.limit = limit_node->limit; out.offset = limit_node->offset; }
-        bool hll_out = false, hll_merge = false;
-        for (const OutCol& oc : out.out_cols) hll_out = hll_out || oc.kind == 2;
+        bool hll_out = false, hll_merge = false, rb_out = false;
+        for (const OutCol& oc : out.out_cols) { hll_out = hll_out || oc.kind == 2; rb_out = rb_out || oc.kind == 3; }
         for (int k = 0; ok && k < out.ap.n_agg; k++) hll_merge = hll_merge || (out.ap.agg[k].kind == AG_HLL && out.ap.agg[k].arg_prim == BK_HLL);   // (ap is set once lowering succeeded)
         if (ok && hll_merge && out.kind != PK_AGG) {   // (a join would have to gather 16400-byte values to the probe rows)
             err = "MERGE_AGG of HLL sketches over a join is outside the GPU path (MERGE_AGG over a scan is lowered)"; return BKGPU_EUNSUPPORTED;
+        }
+        if (ok && rb_out && out.ap.n_hll) {
+            err = "rb_build_agg beside hll_add_agg in one aggregate is outside the GPU path"; return BKGPU_EUNSUPPORTED;
+        }
+        if (ok && (post_sort || post_having) && rb_out) {
+            err = "a SORT / HAVING / LIMIT above an aggregate that returns a BITMAP is outside the GPU path"; return BKGPU_EUNSUPPORTED;
         }
         if (ok && (post_sort || post_having) && hll_out) {
             err = "a SORT / HAVING / LIMIT above an aggregate that returns an HLL sketch is outside the GPU path"; return BKGPU_EUNSUPPORTED;

@@ -60,7 +60,8 @@ struct ColRef { int tuple_id, slot_id, prim; };
 struct OutCol {
     int tuple_id, slot_id, prim;
     int kind;       // 0 = plain value column, 1 = AVG intermediate blob (two device images: sum, count), 2 = HLL sketch (RAW, 16400 bytes;
-                    //   one device image: the sketch reference, whose registers the host copies from the arena)
+                    //   one device image: the sketch reference, whose registers the host copies from the arena), 3 = rb_build_agg's BITMAP
+                    //   (one device image: the group's slot; the bytes come from the device build, rb.cu)
 };
 
 enum PlanKind { PK_AGG = 1, PK_FILTER = 2, PK_SORT = 3, PK_JOIN_AGG = 4, PK_JOIN = 5, PK_STAR_AGG = 6, PK_WINDOW = 7 };
@@ -131,6 +132,7 @@ struct Compiled {
     // aggregate
     AggPlan ap;
     bool is_merge = false, emit_default = false;
+    int n_rb = 0;                      // AG_RB aggregates in ap (at most MAX_RB): their keys go to the pair buffer (AggArgs::rb_keys)
     bool has_direct = false;
     DirectPlan direct;
     std::vector<int> direct_cols;      // indices into `cols`, in [terms][key][values] order

@@ -70,6 +70,7 @@ inline arrow::Result<std::shared_ptr<arrow::RecordBatch>> record_batch_from_colu
     std::vector<std::shared_ptr<arrow::Field>> fields; std::vector<std::shared_ptr<arrow::Array>> arrays;
     for (int i = 0; i < ncols; i++) {
         const bkgpu_column& c = cols[i];
+        if (c.prim_type == BK_BITMAP) return arrow::Status::NotImplemented("rb_build_agg's BITMAP column is not carried by the Arrow bridge");
         auto type = arrow_type_of(c.prim_type);
         if (!type) return arrow::Status::Invalid("column type outside the path");
         const std::string name = std::to_string(c.tuple_id) + "_" + std::to_string(c.slot_id);

@@ -299,12 +299,27 @@ private:
     Chunk _chunk; std::vector<MemRowValues> _rows; size_t _pos = 0; int64_t _capacity;
 };
 
+// why this mirror cannot run a serialized plan ("" = it can): its Column holds fixed-width values, so a plan that returns rb_build_agg's
+// variable-length BITMAP column is refused when the node is initialised (the C API and the Python binding return it)
+inline std::string host_refusal(const std::vector<uint8_t>& plan) {
+    std::string text(1 << 16, '\0');
+    if (bkgpu_plan_explain(plan.data(), plan.size(), &text[0], text.size()) < 0) return "";   // (bkgpu_init reports a plan that does not lower)
+    if (text.find("rb_build_agg: rb=") == std::string::npos) return "";
+    return "rb_build_agg returns a BITMAP column, which the C++ host mirror does not carry: run the plan through the C API or the Python binding";
+}
+
 // the fused AGG -> [FILTER] -> SCAN / SORT / AGG -> JOIN / FILTER subtree on the GPU
 class GpuExecNode : public ExecNode {
 public:
     ~GpuExecNode() override { if (_h) bkgpu_close(_h); }
-    int init(const Plan& plan) override { _plan = plan.serialize(); return 0; }
+    int init(const Plan& plan) override { return init_serialized(plan.serialize()); }
+    int init_serialized(std::vector<uint8_t> plan) {   // BKGPU_EUNSUPPORTED for a plan this mirror cannot carry; open() reports why
+        _plan = std::move(plan);
+        _refusal = host_refusal(_plan);
+        return _refusal.empty() ? 0 : BKGPU_EUNSUPPORTED;
+    }
     int open(RuntimeState* state) override {
+        if (!_refusal.empty()) { state->error_code = BKGPU_EUNSUPPORTED; state->error_msg = _refusal; return -1; }
         int rc = bkgpu_init(&_h, _plan.data(), _plan.size(), state->device, state->nccl_comm);
         if (rc != 0) return fail(state, rc, nullptr);
         if ((rc = bkgpu_set_option(_h, "batch_capacity", state->row_batch_capacity)) != 0 || (rc = bkgpu_open(_h)) != 0) return fail(state, rc, _h);
@@ -348,6 +363,7 @@ public:
 private:
     int fail(RuntimeState* state, int rc, bkgpu_plan* h) { state->error_code = rc; state->error_msg = bkgpu_last_error(h); return -1; }   // negative return + message
     std::vector<uint8_t> _plan;
+    std::string _refusal;
     bkgpu_plan* _h = nullptr;
 };
 

@@ -106,6 +106,9 @@ int   bkgpu_init(bkgpu_plan** out, const uint8_t* plan_desc, size_t len,
  *   "batch_capacity"       rows per bkgpu_get_next batch (RuntimeState::row_batch_capacity)
  *   "chunk_rows"           rows per host->device staging chunk of a host push
  *   "partial_capacity"     groups per rank in the exported partial state (a plan with hll_add_agg ships 16 KB of registers per group and sketch)
+ *   "rb_pair_capacity"     keys the rb_build_agg pair buffer holds: one per row and rb_build_agg with a non-NULL value until it is sorted
+ *                          and deduplicated, which happens whenever it could overflow (default 2^27; 16 bytes of device memory each, the sort
+ *                          needs a second buffer; 1024 .. 2^31); more distinct (group, value) pairs -> BKGPU_ETOOBIG naming this option
  *   "hll_group_capacity"   sketches the hll_add_agg register arena holds: one per group and hll_add_agg aggregate that receives a non-NULL
  *                          value, 16 KB of device memory each (default 4096 = 64 MB, at most 2^20); more -> BKGPU_ETOOBIG naming this option
  *   "region_base"          arrival index of this plan's first row: ORDER BY ties across GPUs break by (region, row)
@@ -182,6 +185,13 @@ int   bkgpu_cast_image(uint64_t image, int from_prim, int to_prim, uint64_t* out
  * MERGE_AGG of hll_add_agg takes the stores' sketches as input columns of the same type and size (RAW only: any other value fails the push
  * with BKGPU_EINVAL, or bkgpu_finish when the column is in device memory). */
 int   bkgpu_hll_estimate(const uint8_t* sketch, size_t len, uint64_t* estimate);
+
+/* ---- Roaring bitmaps ----
+ * rb_build_agg returns a column of prim_type BK_BITMAP (21) with elem_size -1 and no validity bitmap (a group whose values were all NULL
+ * holds the empty bitmap, 3a300000 00000000).  Its values are variable-length, in Arrow's large_binary layout in one buffer: `length + 1`
+ * int64 offsets (the first 0), followed directly by the bytes; value r is bytes [offsets[r], offsets[r + 1]).  Each value is the
+ * reference's bitmap of the group's values' low 32 bits after runOptimize(), in CRoaring's portable serialization (v0.2.66).
+ * The buffer stays valid until the next bkgpu_get_next, bkgpu_reset or bkgpu_close. */
 
 /* ---- resident regions (the column store / parquet cache analogue, include/column/file_manager.h:252-272) ----
  * A region's columns are copied to HBM once (host or device source) and stay there across queries, keyed by

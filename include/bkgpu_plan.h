@@ -82,7 +82,7 @@ enum bkgpu_primitive_type {
     BK_INVALID_TYPE = 0, BK_NULL_TYPE = 1, BK_BOOL = 2, BK_INT8 = 3, BK_INT16 = 4,
     BK_INT32 = 5, BK_INT64 = 6, BK_UINT8 = 7, BK_UINT16 = 8, BK_UINT32 = 9,
     BK_UINT64 = 10, BK_FLOAT = 11, BK_DOUBLE = 12, BK_STRING = 13, BK_DATETIME = 14,
-    BK_TIMESTAMP = 15, BK_DATE = 16, BK_HLL = 17, BK_TIME = 18
+    BK_TIMESTAMP = 15, BK_DATE = 16, BK_HLL = 17, BK_TIME = 18, BK_BITMAP = 21
 };
 
 /* parser::FuncType carried in pb::Function.fn_op — include/sqlparser/expr.h:48-89 */
