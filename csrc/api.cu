@@ -13,6 +13,7 @@
 #include "api_state.h"
 #include "hll.cuh"
 #include "nccl_dl.h"
+#include "prims.cuh"
 #include "build_id.h"
 
 thread_local std::string g_thread_error;
@@ -193,7 +194,7 @@ extern "C" int bkgpu_set_option(bkgpu_plan* p, const char* key, int64_t v) {
     else if (k == "smem_capacity_log2") { if (v < -1 || v > 13) return p->fail(BKGPU_EINVAL, "smem_capacity_log2 out of range"); p->smem_cap_log2 = (int)v; }
     else if (k == "batch_capacity") { if (v < 1) return p->fail(BKGPU_EINVAL, "batch_capacity must be positive"); p->batch_capacity = v; }
     else if (k == "chunk_rows") { if (v < 1024) return p->fail(BKGPU_EINVAL, "chunk_rows too small"); p->chunk_rows = (v + 7) & ~7ll; }
-    else if (k == "rb_pair_capacity") { if (v < 1024 || v > ((int64_t)1 << 31)) return p->fail(BKGPU_EINVAL, "rb_pair_capacity out of range (1024 .. 2^31)"); p->rb_cap = v; }
+    else if (k == "rb_pair_capacity") { if (v < 1024 || v > RADIX_MAX_KEYS) return p->fail(BKGPU_EINVAL, "rb_pair_capacity out of range (1024 .. 2^30 - 1)"); p->rb_cap = v; }
     else if (k == "hll_group_capacity") { if (v < 1 || v > (1 << 20)) return p->fail(BKGPU_EINVAL, "hll_group_capacity out of range (1 .. 2^20)"); p->hll_cap = v; }
     else if (k == "partial_capacity") { if (v < 1) return p->fail(BKGPU_EINVAL, "partial_capacity must be positive"); p->partial_cap = v; }
     else if (k == "force_generic") p->force_generic = v != 0;

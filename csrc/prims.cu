@@ -1,0 +1,272 @@
+// prims.cu — device primitives shared by ORDER BY and the window stage (sort.cu, window.cu) and rb_build_agg (rb.cu), for sm_90a.
+#include "prims.cuh"
+#include <algorithm>
+
+namespace bk {
+
+int grid_for(int64_t n, int sm, int per_sm) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sm * per_sm)); }
+
+int cuda_fail(std::string& err, cudaError_t e, const char* what) { err = std::string(what) + ": " + cudaGetErrorString(e); return e == cudaErrorMemoryAllocation ? BKGPU_ENOMEM : BKGPU_ENODEV; }
+
+__global__ void k_iota(uint32_t* ids, int64_t n) { for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) ids[i] = (uint32_t)i; }
+
+__global__ void k_pack_null_bytes(const uint8_t* nb, int64_t n, uint8_t* bitmap, uint32_t* any_null) {
+    const int64_t nbytes = (n + 7) / 8;
+    bool seen = false;
+    for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < nbytes; b += (int64_t)gridDim.x * blockDim.x) {
+        uint32_t v = 0;
+        for (int j = 0; j < 8; j++) { const int64_t r = b * 8 + j; if (r < n) { if (!nb[r]) v |= 1u << j; else seen = true; } }
+        bitmap[b] = (uint8_t)v;
+    }
+    if (seen && any_null) *any_null = 1u;   // (lets the sort skip the NULL-rank pass of a key column without NULLs)
+}
+
+namespace {
+
+// ---- exclusive prefix sum, in place, over any length (tiles of 2048, the tile sums scanned recursively) ----
+constexpr int SCAN_T = 256, SCAN_I = 8, SCAN_TILE = SCAN_T * SCAN_I;
+
+template <typename T>
+__global__ void __launch_bounds__(SCAN_T) k_scan_tile(T* d, T* sums, int64_t n) {
+    __shared__ T wsum[SCAN_T / 32];
+    const int64_t base = (int64_t)blockIdx.x * SCAN_TILE + (int64_t)threadIdx.x * SCAN_I;
+    T v[SCAN_I], acc = 0;
+#pragma unroll
+    for (int i = 0; i < SCAN_I; i++) { v[i] = base + i < n ? d[base + i] : T(0); acc += v[i]; }
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    T x = acc;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const T y = __shfl_up_sync(~0u, x, o); if (lane >= o) x += y; }
+    if (lane == 31) wsum[w] = x;
+    __syncthreads();
+    if (w == 0) {
+        T s = lane < SCAN_T / 32 ? wsum[lane] : T(0);
+#pragma unroll
+        for (int o = 1; o < SCAN_T / 32; o <<= 1) { const T y = __shfl_up_sync(~0u, s, o); if (lane >= o) s += y; }
+        if (lane < SCAN_T / 32) wsum[lane] = s;
+    }
+    __syncthreads();
+    T run = x - acc + (w ? wsum[w - 1] : T(0));
+#pragma unroll
+    for (int i = 0; i < SCAN_I; i++) { if (base + i < n) d[base + i] = run; run += v[i]; }
+    if (threadIdx.x == SCAN_T - 1) sums[blockIdx.x] = run;
+}
+
+template <typename T>
+__global__ void k_scan_add(T* d, const T* sums, int64_t n) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x + SCAN_TILE; i < n; i += (int64_t)gridDim.x * blockDim.x) d[i] += sums[i / SCAN_TILE];
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Stable LSD radix sort of 64-bit keys (optionally with a uint32_t id each), 8 bits per pass, one read and one write of the keys per pass
+// ("Onesweep": chained scan with decoupled look-back):
+//   k_rs_hist : ONE pass over the keys gives the histograms of all eight digits; a digit whose histogram has a single non-empty bin is
+//               skipped (small-range keys, the NULL-rank image, descending flags, the pair keys' group and aggregate bits ...)
+//   k_rs_pass : a CTA takes the next 3072-key tile (atomic ticket: tiles start in order, so the look-back never waits for a tile that has
+//               not started), ranks its keys per digit (ballot-built peer masks + per-warp counters: stable), publishes the tile's digit
+//               counts, looks back over the preceding tiles' published counts for its scatter bases, reorders the tile through shared
+//               memory and writes digit-contiguous (coalesced) runs
+// ------------------------------------------------------------------------------------------------------------
+constexpr int RS_THREADS = 256;
+constexpr int RS_ITEMS = 12;
+constexpr int RS_TILE = RS_THREADS * RS_ITEMS;   // 3072 keys per CTA tile (36 KB of shared memory for the reorder with ids): four CTAs per SM
+constexpr uint32_t RS_FLAG_AGG = 1u << 30, RS_FLAG_PREFIX = 2u << 30, RS_VAL_MASK = (uint32_t)RADIX_MAX_KEYS;
+constexpr size_t RS_HIST_BYTES = (8 * 256 * 2 + 8 + 8) * 4;   // histograms, bases, active flags, tickets
+
+__global__ void __launch_bounds__(256) k_rs_hist(const uint64_t* key, uint32_t n, uint32_t* hist /* [8][256] */) {
+    __shared__ uint32_t h[8][256];
+    for (int i = threadIdx.x; i < 8 * 256; i += blockDim.x) (&h[0][0])[i] = 0;
+    __syncthreads();
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const uint64_t k = key[i];
+#pragma unroll
+        for (int d = 0; d < 8; d++) atomicAdd(&h[d][(k >> (8 * d)) & 0xFF], 1u);
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < 8 * 256; i += blockDim.x) { const uint32_t v = (&h[0][0])[i]; if (v) atomicAdd(hist + i, v); }
+}
+// per digit: exclusive scan of its histogram -> global scatter bases; active[d] = more than one non-empty bin
+__global__ void k_rs_bases(const uint32_t* hist, uint32_t* bases, uint32_t* active) {
+    const int d = blockIdx.x;
+    __shared__ uint32_t s[256];
+    const uint32_t v = hist[d * 256 + threadIdx.x];
+    s[threadIdx.x] = v;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t run = 0, nz = 0;
+        for (int i = 0; i < 256; i++) { const uint32_t c = s[i]; s[i] = run; run += c; nz += c != 0; }
+        active[d] = nz > 1;
+    }
+    __syncthreads();
+    bases[d * 256 + threadIdx.x] = s[threadIdx.x];
+}
+
+// IDS == false: id_in / id_out are not touched, and the tile's ids take no shared memory
+template <bool IDS>
+__global__ void __launch_bounds__(RS_THREADS, 4) k_rs_pass(const uint64_t* key_in, const uint32_t* id_in, uint64_t* key_out, uint32_t* id_out, uint32_t n, int shift,
+                                                        const uint32_t* global_base /* [256] of this digit */, uint32_t* status /* [ntiles][256], zeroed */,
+                                                        uint32_t* ticket) {
+    extern __shared__ __align__(16) unsigned char rs_smem[];
+    uint64_t* s_key = (uint64_t*)rs_smem;                        // [RS_TILE]
+    uint32_t* s_id = (uint32_t*)(s_key + RS_TILE);               // [RS_TILE] (IDS)
+    uint32_t* wcnt = s_id + (IDS ? RS_TILE : 0);                 // [8][256] per-warp digit counts -> running offsets inside the digit's run
+    uint32_t* dstart = wcnt + 8 * 256;                           // [256] start of the digit inside the reordered tile
+    uint32_t* tbase = dstart + 256;                              // [256] global address of the tile's first key of the digit
+    __shared__ uint32_t s_tile;
+    __shared__ uint32_t wsum[8];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    if (threadIdx.x == 0) s_tile = atomicAdd(ticket, 1u);
+    for (int i = threadIdx.x; i < 8 * 256; i += RS_THREADS) wcnt[i] = 0;
+    __syncthreads();
+    const uint32_t tile = s_tile;
+    const uint32_t t0 = tile * RS_TILE;
+    const uint32_t tile_n = min((uint32_t)RS_TILE, n - t0);
+    // ---- load: warp w owns the contiguous chunk [t0 + w * 32 * RS_ITEMS, + 32 * RS_ITEMS), RS_ITEMS rounds of 32 consecutive keys ----
+    uint64_t k[RS_ITEMS]; uint32_t id[RS_ITEMS];
+    const uint32_t c0 = w * (RS_ITEMS * 32);
+#pragma unroll
+    for (int r = 0; r < RS_ITEMS; r++) {
+        const uint32_t li = c0 + r * 32 + lane;
+        if (li < tile_n) { k[r] = key_in[t0 + li]; if (IDS) id[r] = id_in[t0 + li]; } else { k[r] = ~0ull; id[r] = 0; }
+    }
+    // ---- early counts: the warp's digit histogram (order-free atomics), so the tile's counts are published BEFORE the ranking and the
+    //      following tiles' look-back finds them sooner ----
+    uint32_t* wc = wcnt + w * 256;
+#pragma unroll
+    for (int r = 0; r < RS_ITEMS; r++)
+        if (c0 + r * 32 + lane < tile_n) atomicAdd(wc + (uint32_t)((k[r] >> shift) & 0xFF), 1u);
+    __syncthreads();
+    // ---- thread d: the digit's count per warp -> per-warp offsets, tile count; publish; where the digit starts in the reordered tile ----
+    const int d_own = threadIdx.x;
+    uint32_t cnt;
+    volatile uint32_t* st = status + (size_t)tile * 256 + d_own;
+    {
+        uint32_t run = 0;
+#pragma unroll
+        for (int ww = 0; ww < 8; ww++) { const uint32_t c = wcnt[ww * 256 + d_own]; wcnt[ww * 256 + d_own] = run; run += c; }
+        cnt = run;
+        *st = (tile == 0 ? RS_FLAG_PREFIX : RS_FLAG_AGG) | cnt;   // (flag and count travel in ONE word: no fence around the publication)
+        uint32_t x = cnt;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o); if (lane >= o) x += y; }
+        if (lane == 31) wsum[w] = x;
+        __syncthreads();
+        uint32_t wpre = 0;
+        for (int ww = 0; ww < w; ww++) wpre += wsum[ww];
+        dstart[d_own] = wpre + x - cnt;
+    }
+    __syncthreads();
+    // ---- rank in element order (stable) and place: peers of the digit in this round + the digit's running offset.  The peer mask
+    //      comes from eight ballots, one per digit bit: MATCH.ANY would keep the XU pipe busy ----
+    const uint32_t lt_mask = (1u << lane) - 1u;
+#pragma unroll
+    for (int r = 0; r < RS_ITEMS; r++) {
+        const bool live = c0 + r * 32 + lane < tile_n;
+        const uint32_t d = (uint32_t)((k[r] >> shift) & 0xFF);
+        uint32_t peers = __ballot_sync(0xFFFFFFFFu, live);
+#pragma unroll
+        for (int b = 0; b < 8; b++) {
+            const uint32_t bit = (d >> b) & 1u;
+            peers &= ~(__ballot_sync(0xFFFFFFFFu, bit != 0) ^ (0u - bit));
+        }
+        uint32_t before = 0;
+        if (live) before = wc[d];
+        __syncwarp();
+        const uint32_t mine = __popc(peers & lt_mask);
+        if (live) {
+            if ((peers >> lane) == 1u) wc[d] = before + mine + 1u;   // the highest peer lane advances the offset by the group's size
+            const uint32_t pos = dstart[d] + before + mine;
+            s_key[pos] = k[r]; if (IDS) s_id[pos] = id[r];
+        }
+        __syncwarp();
+    }
+    // ---- chained scan with decoupled look-back over the preceding tiles (they all started before this one: ticket order) ----
+    {
+        uint32_t excl = 0;
+        if (tile != 0) {
+            // four predecessors per round trip: the loads are independent, the walk consumes them nearest first
+            for (int64_t p = (int64_t)tile - 1;;) {
+                uint32_t v[4];
+#pragma unroll
+                for (int j = 0; j < 4; j++) v[j] = p - j >= 0 ? *(volatile const uint32_t*)(status + (size_t)(p - j) * 256 + d_own) : RS_FLAG_PREFIX;
+                int j = 0; bool done = false;
+#pragma unroll
+                for (; j < 4; j++) {
+                    if ((v[j] & ~RS_VAL_MASK) == 0) break;            // not published yet: poll again from this tile
+                    excl += v[j] & RS_VAL_MASK;
+                    if (v[j] & RS_FLAG_PREFIX) { done = true; break; }
+                }
+                if (done) break;
+                p -= j;
+            }
+            *st = RS_FLAG_PREFIX | (excl + cnt);
+        }
+        tbase[d_own] = global_base[d_own] + excl;
+    }
+    __syncthreads();
+    // ---- write the digit-contiguous runs ----
+    for (uint32_t i = threadIdx.x; i < tile_n; i += RS_THREADS) {
+        const uint64_t kk = s_key[i];
+        const uint32_t d = (uint32_t)((kk >> shift) & 0xFF);
+        const uint32_t dst = tbase[d] + (i - dstart[d]);
+        key_out[dst] = kk; if (IDS) id_out[dst] = s_id[i];
+    }
+}
+
+}  // namespace
+
+int64_t scan_scratch(int64_t n) { int64_t t = 0; while (n > 1) { n = (n + SCAN_TILE - 1) / SCAN_TILE; t += n; } return t + 1; }
+
+template <typename T>
+cudaError_t scan_excl(T* d, int64_t n, T* sums, int sm, cudaStream_t s) {
+    const int64_t nb = (n + SCAN_TILE - 1) / SCAN_TILE;
+    k_scan_tile<T><<<(unsigned)nb, SCAN_T, 0, s>>>(d, sums, n);
+    if (nb > 1) {
+        cudaError_t e = scan_excl(sums, nb, sums + nb, sm, s);
+        if (e != cudaSuccess) return e;
+        k_scan_add<T><<<grid_for(n, sm, 16), 256, 0, s>>>(d, sums, n);
+    }
+    return cudaGetLastError();
+}
+template cudaError_t scan_excl<uint32_t>(uint32_t*, int64_t, uint32_t*, int, cudaStream_t);
+template cudaError_t scan_excl<uint64_t>(uint64_t*, int64_t, uint64_t*, int, cudaStream_t);
+
+int radix_sort(uint64_t* const keys[2], uint32_t* const ids[2], int cur, int64_t n, int sm, const RadixScratch& scratch, cudaStream_t st,
+               bkgpu_stats* stats, int64_t* bytes, std::string& err) {
+    if (n > RADIX_MAX_KEYS) { err = "the radix sort takes at most 2^30 - 1 keys"; return BKGPU_EUNSUPPORTED; }
+    if (n < 2) return cur;
+    const uint32_t un = (uint32_t)n, ntiles = (un + RS_TILE - 1) / RS_TILE;
+    uint32_t *hist, *status;
+    int rc;
+    if ((rc = scratch(0, RS_HIST_BYTES, (void**)&hist))) return rc;
+    uint32_t* bases = hist + 8 * 256; uint32_t* active = bases + 8 * 256; uint32_t* tickets = active + 8;
+    SCK(cudaMemsetAsync(hist, 0, RS_HIST_BYTES, st));
+    k_rs_hist<<<std::min(sm * 4, (int)((un + 1023) / 1024)), 256, 0, st>>>(keys[cur], un, hist);
+    k_rs_bases<<<8, 256, 0, st>>>(hist, bases, active);
+    uint32_t h_active[8];
+    SCK(cudaMemcpyAsync(h_active, active, 32, cudaMemcpyDeviceToHost, st));
+    SCK(cudaStreamSynchronize(st));
+    stats->kernel_launches += 2;
+    if (bytes) *bytes += n * 8;
+    int n_active = 0;
+    for (int d = 0; d < 8; d++) n_active += h_active[d] != 0;
+    if (!n_active) return cur;
+    const size_t status_bytes = (size_t)ntiles * 256 * 4 * (size_t)n_active;   // one look-back array per pass
+    if ((rc = scratch(1, status_bytes, (void**)&status))) return rc;
+    SCK(cudaMemsetAsync(status, 0, status_bytes, st));
+    const auto pass = ids ? k_rs_pass<true> : k_rs_pass<false>;
+    const size_t smem = (size_t)RS_TILE * (ids ? 12 : 8) + (8 * 256 + 256 + 256) * 4;   // under 48 KB: no opt-in needed
+    int slot = 0;
+    for (int d = 0; d < 8; d++) {
+        if (!h_active[d]) continue;
+        pass<<<ntiles, RS_THREADS, smem, st>>>(keys[cur], ids ? ids[cur] : nullptr, keys[cur ^ 1], ids ? ids[cur ^ 1] : nullptr, un, 8 * d,
+                                               bases + 256 * d, status + (size_t)slot * ntiles * 256, tickets + d);
+        cur ^= 1; slot++;
+        stats->kernel_launches++;
+        if (bytes) *bytes += n * (ids ? 24 : 16);
+    }
+    SCK(cudaGetLastError());
+    return cur;
+}
+
+}  // namespace bk

@@ -12,129 +12,12 @@
 #include <string.h>
 #include <algorithm>
 #include "api_state.h"
+#include "prims.cuh"
 #include "rb.h"
 
 namespace bk {
 
 namespace {
-
-// ---- exclusive prefix sum, in place, over any length (tiles of 2048, the tile sums scanned recursively) ----
-constexpr int SCAN_T = 256, SCAN_I = 8, SCAN_TILE = SCAN_T * SCAN_I;
-
-template <typename T>
-__global__ void __launch_bounds__(SCAN_T) k_scan_tile(T* d, T* sums, int64_t n) {
-    __shared__ T wsum[SCAN_T / 32];
-    const int64_t base = (int64_t)blockIdx.x * SCAN_TILE + (int64_t)threadIdx.x * SCAN_I;
-    T v[SCAN_I], acc = 0;
-#pragma unroll
-    for (int i = 0; i < SCAN_I; i++) { v[i] = base + i < n ? d[base + i] : T(0); acc += v[i]; }
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    T x = acc;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const T y = __shfl_up_sync(~0u, x, o); if (lane >= o) x += y; }
-    if (lane == 31) wsum[w] = x;
-    __syncthreads();
-    if (w == 0) {
-        T s = lane < SCAN_T / 32 ? wsum[lane] : T(0);
-#pragma unroll
-        for (int o = 1; o < SCAN_T / 32; o <<= 1) { const T y = __shfl_up_sync(~0u, s, o); if (lane >= o) s += y; }
-        if (lane < SCAN_T / 32) wsum[lane] = s;
-    }
-    __syncthreads();
-    T run = x - acc + (w ? wsum[w - 1] : T(0));
-#pragma unroll
-    for (int i = 0; i < SCAN_I; i++) { if (base + i < n) d[base + i] = run; run += v[i]; }
-    if (threadIdx.x == SCAN_T - 1) sums[blockIdx.x] = run;
-}
-
-template <typename T>
-__global__ void k_scan_add(T* d, const T* sums, int64_t n) {
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x + SCAN_TILE; i < n; i += (int64_t)gridDim.x * blockDim.x) d[i] += sums[i / SCAN_TILE];
-}
-
-int64_t scan_scratch(int64_t n) { int64_t t = 0; while (n > 1) { n = (n + SCAN_TILE - 1) / SCAN_TILE; t += n; } return t + 1; }
-
-int grid_of(int64_t n, int sm) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sm * 16)); }
-
-template <typename T>
-cudaError_t scan_excl(T* d, int64_t n, T* sums, int sm, cudaStream_t s) {
-    const int64_t nb = (n + SCAN_TILE - 1) / SCAN_TILE;
-    k_scan_tile<T><<<(unsigned)nb, SCAN_T, 0, s>>>(d, sums, n);
-    if (nb > 1) {
-        cudaError_t e = scan_excl(sums, nb, sums + nb, sm, s);
-        if (e != cudaSuccess) return e;
-        k_scan_add<T><<<grid_of(n, sm), 256, 0, s>>>(d, sums, n);
-    }
-    return cudaGetLastError();
-}
-
-// ---- LSD radix sort of 64-bit keys, 8 bits per pass ----
-constexpr int RS_T = 256, RS_I = 16, RS_TILE = RS_T * RS_I;   // a tile: 8 warps x 16 rounds x 32 keys, each warp a contiguous 512
-
-// OR and AND of every key: a digit where they agree is the same in every key, and its pass is skipped
-__global__ void k_rs_span(const uint64_t* k, int64_t n, unsigned long long* oa) {
-    unsigned long long o = 0, a = ~0ull;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) { o |= k[i]; a &= k[i]; }
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) { o |= __shfl_xor_sync(~0u, o, d); a &= __shfl_xor_sync(~0u, a, d); }
-    if ((threadIdx.x & 31) == 0) { atomicOr(oa, o); atomicAnd(oa + 1, a); }
-}
-
-// per tile, how many of its keys have each digit value: counts[digit * ntiles + tile] (digit-major, so one scan gives every
-// (digit, tile)'s first output position)
-__global__ void __launch_bounds__(RS_T) k_rs_hist(const uint64_t* k, int64_t n, int shift, uint32_t* counts, uint32_t ntiles) {
-    __shared__ uint32_t h[256];
-    h[threadIdx.x] = 0;
-    __syncthreads();
-    const int64_t base = (int64_t)blockIdx.x * RS_TILE;
-    const unsigned lt = (1u << (threadIdx.x & 31)) - 1u;
-#pragma unroll 4
-    for (int i = 0; i < RS_I; i++) {
-        const int64_t j = base + i * RS_T + threadIdx.x;
-        const uint32_t d = j < n ? (uint32_t)(k[j] >> shift) & 255u : 256u;
-        const unsigned peers = __match_any_sync(~0u, d);
-        if (d < 256 && (peers & lt) == 0) atomicAdd(&h[d], (uint32_t)__popc(peers));
-    }
-    __syncthreads();
-    counts[(size_t)threadIdx.x * ntiles + blockIdx.x] = h[threadIdx.x];
-}
-
-// stable scatter of one pass: a key's position is its (digit, tile) offset + the keys of the same digit before it in the tile
-__global__ void __launch_bounds__(RS_T) k_rs_scatter(const uint64_t* in, uint64_t* out, int64_t n, int shift, const uint32_t* offs, uint32_t ntiles) {
-    __shared__ uint32_t wc[RS_T / 32][256];
-    __shared__ uint32_t tile_off[256];
-    for (int t = threadIdx.x; t < (RS_T / 32) * 256; t += RS_T) (&wc[0][0])[t] = 0;
-    tile_off[threadIdx.x] = offs[(size_t)threadIdx.x * ntiles + blockIdx.x];
-    __syncthreads();
-    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const unsigned lt = (1u << lane) - 1u;
-    const int64_t base = (int64_t)blockIdx.x * RS_TILE + (int64_t)w * (RS_I * 32);
-    uint64_t key[RS_I];
-    uint32_t rank[RS_I];
-#pragma unroll
-    for (int i = 0; i < RS_I; i++) {
-        const int64_t j = base + i * 32 + lane;
-        key[i] = j < n ? in[j] : 0;
-        const uint32_t d = j < n ? (uint32_t)(key[i] >> shift) & 255u : 256u;
-        const unsigned peers = __match_any_sync(~0u, d);
-        const uint32_t before = d < 256 ? wc[w][d] : 0u;
-        __syncwarp();
-        if (d < 256 && (peers & lt) == 0) wc[w][d] = before + (uint32_t)__popc(peers);
-        __syncwarp();
-        rank[i] = before + (uint32_t)__popc(peers & lt);
-    }
-    __syncthreads();
-    {   // per digit: the keys of the warps before (warp-major is array order)
-        uint32_t run = 0;
-        for (int x = 0; x < RS_T / 32; x++) { const uint32_t t = wc[x][threadIdx.x]; wc[x][threadIdx.x] = run; run += t; }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int i = 0; i < RS_I; i++) {
-        const int64_t j = base + i * 32 + lane;
-        if (j < n) { const uint32_t d = (uint32_t)(key[i] >> shift) & 255u; out[tile_off[d] + wc[w][d] + rank[i]] = key[i]; }
-    }
-}
 
 // ---- duplicates ----
 __global__ void k_uniq_flags(const uint64_t* k, int64_t n, uint32_t* f) {
@@ -278,35 +161,14 @@ template <typename T> static T d2h(bkgpu_plan* p, const T* src, int* rc) {
     return v;
 }
 
-// sort keys [0, n) of the pair buffer (p->rb.keys; the sort's second buffer is p->rb.alt, and the two swap with every pass)
+// sort keys [0, n) of the pair buffer: p->rb.keys then points at the sorted keys (the sort's second buffer is p->rb.alt)
 static int rb_sort(bkgpu_plan* p, int64_t n) {
-    if (n < 2) return BKGPU_OK;
-    const cudaStream_t s = p->stream;
-    int rc;
-    unsigned long long* oa;
-    if ((rc = rb_buf(p, 0, 16, (void**)&oa))) return rc;
-    CK(p, cudaMemsetAsync(oa, 0, 8, s));
-    CK(p, cudaMemsetAsync(oa + 1, 0xFF, 8, s));
-    k_rs_span<<<grid_of(n, p->sm_count), 256, 0, s>>>(p->rb.keys, n, oa);
-    CK(p, cudaGetLastError());
-    unsigned long long span[2];
-    CK(p, cudaMemcpyAsync(span, oa, 16, cudaMemcpyDeviceToHost, s));
-    CK(p, cudaStreamSynchronize(s));
-    const uint64_t differ = span[0] ^ span[1];
-    const uint32_t ntiles = (uint32_t)((n + RS_TILE - 1) / RS_TILE);
-    const int64_t nc = (int64_t)ntiles * 256;
-    uint32_t *counts, *sums;
-    if ((rc = rb_buf(p, 1, (size_t)nc * 4, (void**)&counts)) || (rc = rb_buf(p, 2, (size_t)scan_scratch(nc) * 4, (void**)&sums))) return rc;
-    for (int d = 0; d < 8; d++) {
-        if (!((differ >> (8 * d)) & 0xFFu)) continue;
-        k_rs_hist<<<ntiles, RS_T, 0, s>>>(p->rb.keys, n, 8 * d, counts, ntiles);
-        CK(p, cudaGetLastError());
-        CK(p, scan_excl(counts, nc, sums, p->sm_count, s));
-        k_rs_scatter<<<ntiles, RS_T, 0, s>>>(p->rb.keys, p->rb.alt, n, 8 * d, counts, ntiles);
-        CK(p, cudaGetLastError());
-        std::swap(p->rb.keys, p->rb.alt);
-        p->stats.kernel_launches += 4;
-    }
+    uint64_t* keys[2] = {p->rb.keys, p->rb.alt};
+    std::string err;
+    const int r = radix_sort(keys, nullptr, 0, n, p->sm_count, [p](int slot, size_t bytes, void** out) { return rb_buf(p, slot, bytes, out); },
+                             p->stream, &p->stats, nullptr, err);
+    if (r < 0) return err.empty() ? r : p->fail(r, "rb_build_agg: %s", err.c_str());
+    if (r) std::swap(p->rb.keys, p->rb.alt);
     return BKGPU_OK;
 }
 
@@ -319,7 +181,7 @@ int rb_compact(bkgpu_plan* p, uint64_t* n_out) {
     if ((rc = rb_sort(p, (int64_t)n))) return rc;
     uint32_t *flags, *sums;
     if ((rc = rb_buf(p, 1, (n + 1) * 4, (void**)&flags)) || (rc = rb_buf(p, 2, (size_t)scan_scratch((int64_t)n + 1) * 4, (void**)&sums))) return rc;
-    const int g = grid_of((int64_t)n + 1, p->sm_count);
+    const int g = grid_for((int64_t)n + 1, p->sm_count, 16);
     k_uniq_flags<<<g, 256, 0, p->stream>>>(p->rb.keys, (int64_t)n, flags);
     CK(p, cudaGetLastError());
     CK(p, scan_excl(flags, (int64_t)n + 1, sums, p->sm_count, p->stream));
@@ -344,7 +206,7 @@ int rb_build(bkgpu_plan* p) {
     uint64_t* e = p->rb.alt;   // (cap + 1 words: room for the scan's closing entry)
     uint64_t* sums64;
     if ((rc = rb_buf(p, 2, (size_t)scan_scratch(m + 1) * 8, (void**)&sums64))) return rc;
-    k_seg_flags<<<grid_of(m + 1, sm), 256, 0, s>>>(u, m, e);
+    k_seg_flags<<<grid_for(m + 1, sm, 16), 256, 0, s>>>(u, m, e);
     CK(p, cudaGetLastError());
     CK(p, scan_excl(e, m + 1, sums64, sm, s));
     const uint64_t tot = d2h(p, e + m, &rc);
@@ -361,14 +223,14 @@ int rb_build(bkgpu_plan* p) {
         (rc = rb_buf(p, 13, (size_t)(nc + 1) * 8, (void**)&bo)) || (rc = rb_buf(p, 14, (size_t)(nc + 1) * 4, (void**)&bid)) ||
         (rc = rb_buf(p, 2, (size_t)scan_scratch(std::max(m, nc) + 1) * 8, (void**)&sums64)))
         return rc;
-    k_seg_mark<<<grid_of(m + 1, sm), 256, 0, s>>>(u, m, e, cst, crun, rst);
-    k_containers<<<grid_of(nc + 1, sm), 256, 0, s>>>(u, nc, cst, crun, ctype, psz, bi);
+    k_seg_mark<<<grid_for(m + 1, sm, 16), 256, 0, s>>>(u, m, e, cst, crun, rst);
+    k_containers<<<grid_for(nc + 1, sm, 16), 256, 0, s>>>(u, nc, cst, crun, ctype, psz, bi);
     CK(p, cudaGetLastError());
     CK(p, scan_excl(psz, nc + 1, sums64, sm, s));
     CK(p, scan_excl(bi, nc + 1, (uint32_t*)sums64, sm, s));
     CK(p, cudaMemsetAsync(bhas, 0, (size_t)(nc + 1), s));
-    k_bitmap_start<<<grid_of(nc + 1, sm), 256, 0, s>>>(nc, bi, ctype, bst, bhas);
-    k_bitmap_size<<<grid_of(nc + 1, sm), 256, 0, s>>>(u, nc, bi, bst, bhas, psz, cst, bhdr, bo, bid);
+    k_bitmap_start<<<grid_for(nc + 1, sm, 16), 256, 0, s>>>(nc, bi, ctype, bst, bhas);
+    k_bitmap_size<<<grid_for(nc + 1, sm, 16), 256, 0, s>>>(u, nc, bi, bst, bhas, psz, cst, bhdr, bo, bid);
     CK(p, cudaGetLastError());
     CK(p, scan_excl(bo, nc + 1, sums64, sm, s));
     uint32_t nb = 0; uint64_t total = 0;
@@ -376,8 +238,8 @@ int rb_build(bkgpu_plan* p) {
     CK(p, cudaMemcpyAsync(&total, bo + nc, 8, cudaMemcpyDeviceToHost, s));
     CK(p, cudaStreamSynchronize(s));
     if ((rc = rb_buf(p, 15, (size_t)total, (void**)&out))) return rc;
-    k_headers<<<grid_of(nc, sm), 256, 0, s>>>(u, nc, bi, bst, bhas, bhdr, bo, psz, cst, crun, ctype, out, coff);
-    k_payloads<<<grid_of(m, sm), 256, 0, s>>>(u, m, e, ctype, coff, cst, crun, rst, out);
+    k_headers<<<grid_for(nc, sm, 16), 256, 0, s>>>(u, nc, bi, bst, bhas, bhdr, bo, psz, cst, crun, ctype, out, coff);
+    k_payloads<<<grid_for(m, sm, 16), 256, 0, s>>>(u, m, e, ctype, coff, cst, crun, rst, out);
     k_bitsets<<<(unsigned)std::max<int64_t>(1, std::min<int64_t>(nc, (int64_t)sm * 8)), 256, 0, s>>>(u, nc, cst, ctype, coff, out);
     CK(p, cudaGetLastError());
     p->stats.kernel_launches += 16;

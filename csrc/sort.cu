@@ -23,6 +23,7 @@
 #include "dev_common.cuh"
 #include "interp.cuh"
 #include "nccl_dl.h"
+#include "prims.cuh"
 #include "sort_key.h"   // key_image: the order-preserving 64-bit image (ascending); DESC complements it
 
 namespace bk {
@@ -374,35 +375,6 @@ __global__ void __launch_bounds__(256) k_filter_count(RowArgs a, uint32_t* block
     __syncthreads();
     if (threadIdx.x == 0) { uint32_t t = 0; for (int i = 0; i < 8; i++) t += s[i]; block_counts[blockIdx.x] = t; }
 }
-__global__ void k_scan_counts(uint32_t* counts, uint32_t n, uint64_t* total) {  // single CTA exclusive scan (n <= a few thousand blocks)
-    __shared__ uint64_t carry;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (uint32_t base = 0; base < n; base += blockDim.x) {
-        const uint32_t i = base + threadIdx.x;
-        uint32_t v = i < n ? counts[i] : 0;
-        // inclusive warp scan
-        uint32_t x = v;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, d); if ((threadIdx.x & 31) >= d) x += y; }
-        __shared__ uint32_t ws[32];
-        if ((threadIdx.x & 31) == 31) ws[threadIdx.x >> 5] = x;
-        __syncthreads();
-        if (threadIdx.x < 32) {
-            uint32_t w = threadIdx.x < (blockDim.x >> 5) ? ws[threadIdx.x] : 0, xw = w;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) { uint32_t y = __shfl_up_sync(0xFFFFFFFFu, xw, d); if (threadIdx.x >= d) xw += y; }
-            ws[threadIdx.x] = xw - w;
-        }
-        __syncthreads();
-        const uint64_t excl = carry + ws[threadIdx.x >> 5] + (x - v);
-        if (i < n) counts[i] = (uint32_t)excl;  // offsets fit 32 bits per launch (<= 2^31 rows)
-        __syncthreads();
-        if (threadIdx.x == blockDim.x - 1) carry = excl + v;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *total = carry;
-}
 __global__ void __launch_bounds__(256) k_filter_write(RowArgs a, const uint32_t* block_offsets, int64_t rows_per_block, uint32_t* sel, uint64_t out_base, uint64_t cap) {
     const int64_t r0 = (int64_t)blockIdx.x * rows_per_block, r1 = min(r0 + rows_per_block, a.nrows);
     __shared__ uint32_t warp_cnt[8];
@@ -454,181 +426,16 @@ __global__ void k_sort_images(RowArgs a, int key_reg, int vclass, int desc, int 
         if (rid) rid[row] = (uint32_t)row;
     }
 }
-// ------------------------------------------------------------------------------------------------------------
-// Full ORDER BY (Sorter::sort, src/runtime/sorter.cpp:54-114): stable LSD radix sort of (key image, row id) PAIRS, 8 bits per
-// pass, one read and one write of the pairs per pass ("Onesweep": chained scan with decoupled look-back):
-//   k_rs_hist : ONE pass over the images gives the histograms of all eight digits; a digit whose histogram has a single
-//               non-empty bin is skipped (small-range keys, the NULL-rank image, descending flags ...)
-//   k_rs_pass : a CTA takes the next 4096-pair tile (atomic ticket: tiles start in order, so the look-back never waits for a
-//               tile that has not started), ranks its pairs per digit (warp match + per-warp counters: stable), publishes the
-//               tile's digit counts, looks back over the preceding tiles' published counts for its scatter bases, reorders the
-//               tile through shared memory and writes digit-contiguous (coalesced) runs
-// The previous version gathered key[perm[i]] (a random 8-byte read per element and pass) and scattered 32 elements at a time.
-// ------------------------------------------------------------------------------------------------------------
-constexpr int RS_THREADS = 256;
-constexpr int RS_ITEMS = 12;
-constexpr int RS_TILE = RS_THREADS * RS_ITEMS;   // 3072 pairs per CTA tile (36 KB of shared memory for the reorder): four CTAs per SM
-constexpr uint32_t RS_FLAG_AGG = 1u << 30, RS_FLAG_PREFIX = 2u << 30, RS_VAL_MASK = (1u << 30) - 1u;
-
-__global__ void __launch_bounds__(256) k_rs_hist(const uint64_t* key, uint32_t n, uint32_t* hist /* [8][256] */) {
-    __shared__ uint32_t h[8][256];
-    for (int i = threadIdx.x; i < 8 * 256; i += blockDim.x) (&h[0][0])[i] = 0;
-    __syncthreads();
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const uint64_t k = key[i];
-#pragma unroll
-        for (int d = 0; d < 8; d++) atomicAdd(&h[d][(k >> (8 * d)) & 0xFF], 1u);
-    }
-    __syncthreads();
-    for (int i = threadIdx.x; i < 8 * 256; i += blockDim.x) { const uint32_t v = (&h[0][0])[i]; if (v) atomicAdd(hist + i, v); }
-}
-// per digit: exclusive scan of its histogram -> global scatter bases; active[d] = more than one non-empty bin
-__global__ void k_rs_bases(const uint32_t* hist, uint32_t* bases, uint32_t* active) {
-    const int d = blockIdx.x;
-    __shared__ uint32_t s[256];
-    const uint32_t v = hist[d * 256 + threadIdx.x];
-    s[threadIdx.x] = v;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        uint32_t run = 0, nz = 0;
-        for (int i = 0; i < 256; i++) { const uint32_t c = s[i]; s[i] = run; run += c; nz += c != 0; }
-        active[d] = nz > 1;
-    }
-    __syncthreads();
-    bases[d * 256 + threadIdx.x] = s[threadIdx.x];
-}
-// null BYTES (1 = NULL) of a retained column -> Arrow validity bitmap (bit set = valid)
-__global__ void k_pack_null_bytes(const uint8_t* nb, int64_t n, uint8_t* bitmap, uint32_t* any_null) {
-    const int64_t nbytes = (n + 7) / 8;
-    bool seen = false;
-    for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < nbytes; b += (int64_t)gridDim.x * blockDim.x) {
-        uint32_t v = 0;
-        for (int j = 0; j < 8; j++) { const int64_t r = b * 8 + j; if (r < n) { if (!nb[r]) v |= 1u << j; else seen = true; } }
-        bitmap[b] = (uint8_t)v;
-    }
-    if (seen) *any_null = 1u;   // (lets the sort skip the NULL-rank pass of a key column without NULLs)
-}
 // key image of a plain column key, without the expression interpreter
 __global__ void k_sort_images_direct(DevCol c, int64_t n, int vclass, int desc, uint64_t* img) {
     for (int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; row < n; row += (int64_t)gridDim.x * blockDim.x)
         img[row] = elem_is_null(c, row) ? 0ull : key_image(load_elem(c, row), vclass, desc);
 }
-__global__ void k_rs_iota(uint32_t* ids, uint32_t n) { for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) ids[i] = i; }
 __global__ void k_rs_gather_u64(const uint64_t* src, const uint32_t* ids, uint64_t* dst, uint32_t n) {
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) dst[i] = src[ids[i]];
 }
 __global__ void k_rs_gather_bytes(const uint8_t* src, const uint32_t* ids, uint8_t* dst, uint64_t n) {
     for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) dst[i] = src[ids[i]];
-}
-
-__global__ void __launch_bounds__(RS_THREADS, 4) k_rs_pass(const uint64_t* key_in, const uint32_t* id_in, uint64_t* key_out, uint32_t* id_out, uint32_t n, int shift,
-                                                        const uint32_t* global_base /* [256] of this digit */, uint32_t* status /* [ntiles][256], zeroed */,
-                                                        uint32_t* ticket) {
-    extern __shared__ __align__(16) unsigned char rs_smem[];
-    uint64_t* s_key = (uint64_t*)rs_smem;                        // [RS_TILE]
-    uint32_t* s_id = (uint32_t*)(s_key + RS_TILE);               // [RS_TILE]
-    uint32_t* wcnt = s_id + RS_TILE;                             // [8][256] per-warp digit counts -> running offsets inside the digit's run
-    uint32_t* dstart = wcnt + 8 * 256;                           // [256] start of the digit inside the reordered tile
-    uint32_t* tbase = dstart + 256;                              // [256] global address of the tile's first pair of the digit
-    __shared__ uint32_t s_tile;
-    __shared__ uint32_t wsum[8];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    if (threadIdx.x == 0) s_tile = atomicAdd(ticket, 1u);
-    for (int i = threadIdx.x; i < 8 * 256; i += RS_THREADS) wcnt[i] = 0;
-    __syncthreads();
-    const uint32_t tile = s_tile;
-    const uint32_t t0 = tile * RS_TILE;
-    const uint32_t tile_n = min((uint32_t)RS_TILE, n - t0);
-    // ---- load: warp w owns the contiguous chunk [t0 + w * 32 * RS_ITEMS, + 32 * RS_ITEMS), RS_ITEMS rounds of 32 consecutive pairs ----
-    uint64_t k[RS_ITEMS]; uint32_t id[RS_ITEMS];
-    const uint32_t c0 = w * (RS_ITEMS * 32);
-#pragma unroll
-    for (int r = 0; r < RS_ITEMS; r++) {
-        const uint32_t li = c0 + r * 32 + lane;
-        if (li < tile_n) { k[r] = key_in[t0 + li]; id[r] = id_in[t0 + li]; } else { k[r] = ~0ull; id[r] = 0; }
-    }
-    // ---- early counts: the warp's digit histogram (order-free atomics), so the tile's counts are published BEFORE the ranking and the
-    //      following tiles' look-back finds them sooner ----
-    uint32_t* wc = wcnt + w * 256;
-#pragma unroll
-    for (int r = 0; r < RS_ITEMS; r++)
-        if (c0 + r * 32 + lane < tile_n) atomicAdd(wc + (uint32_t)((k[r] >> shift) & 0xFF), 1u);
-    __syncthreads();
-    // ---- thread d: the digit's count per warp -> per-warp offsets, tile count; publish; where the digit starts in the reordered tile ----
-    const int d_own = threadIdx.x;
-    uint32_t cnt;
-    volatile uint32_t* st = status + (size_t)tile * 256 + d_own;
-    {
-        uint32_t run = 0;
-#pragma unroll
-        for (int ww = 0; ww < 8; ww++) { const uint32_t c = wcnt[ww * 256 + d_own]; wcnt[ww * 256 + d_own] = run; run += c; }
-        cnt = run;
-        *st = (tile == 0 ? RS_FLAG_PREFIX : RS_FLAG_AGG) | cnt;   // (flag and count travel in ONE word: no fence around the publication)
-        uint32_t x = cnt;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o); if (lane >= o) x += y; }
-        if (lane == 31) wsum[w] = x;
-        __syncthreads();
-        uint32_t wpre = 0;
-        for (int ww = 0; ww < w; ww++) wpre += wsum[ww];
-        dstart[d_own] = wpre + x - cnt;
-    }
-    __syncthreads();
-    // ---- rank in element order (stable) and place: peers of the digit in this round + the digit's running offset.  The peer mask
-    //      comes from eight ballots, one per digit bit: MATCH.ANY would keep the XU pipe busy ----
-    const uint32_t lt_mask = (1u << lane) - 1u;
-#pragma unroll
-    for (int r = 0; r < RS_ITEMS; r++) {
-        const bool live = c0 + r * 32 + lane < tile_n;
-        const uint32_t d = (uint32_t)((k[r] >> shift) & 0xFF);
-        uint32_t peers = __ballot_sync(0xFFFFFFFFu, live);
-#pragma unroll
-        for (int b = 0; b < 8; b++) {
-            const uint32_t bit = (d >> b) & 1u;
-            peers &= ~(__ballot_sync(0xFFFFFFFFu, bit != 0) ^ (0u - bit));
-        }
-        uint32_t before = 0;
-        if (live) before = wc[d];
-        __syncwarp();
-        const uint32_t mine = __popc(peers & lt_mask);
-        if (live) {
-            if ((peers >> lane) == 1u) wc[d] = before + mine + 1u;   // the highest peer lane advances the offset by the group's size
-            const uint32_t pos = dstart[d] + before + mine;
-            s_key[pos] = k[r]; s_id[pos] = id[r];
-        }
-        __syncwarp();
-    }
-    // ---- chained scan with decoupled look-back over the preceding tiles (they all started before this one: ticket order) ----
-    {
-        uint32_t excl = 0;
-        if (tile != 0) {
-            // four predecessors per round trip: the loads are independent, the walk consumes them nearest first
-            for (int64_t p = (int64_t)tile - 1;;) {
-                uint32_t v[4];
-#pragma unroll
-                for (int j = 0; j < 4; j++) v[j] = p - j >= 0 ? *(volatile const uint32_t*)(status + (size_t)(p - j) * 256 + d_own) : RS_FLAG_PREFIX;
-                int j = 0; bool done = false;
-#pragma unroll
-                for (; j < 4; j++) {
-                    if ((v[j] & ~RS_VAL_MASK) == 0) break;            // not published yet: poll again from this tile
-                    excl += v[j] & RS_VAL_MASK;
-                    if (v[j] & RS_FLAG_PREFIX) { done = true; break; }
-                }
-                if (done) break;
-                p -= j;
-            }
-            *st = RS_FLAG_PREFIX | (excl + cnt);
-        }
-        tbase[d_own] = global_base[d_own] + excl;
-    }
-    __syncthreads();
-    // ---- write the digit-contiguous runs ----
-    for (uint32_t i = threadIdx.x; i < tile_n; i += RS_THREADS) {
-        const uint64_t kk = s_key[i];
-        const uint32_t d = (uint32_t)((kk >> shift) & 0xFF);
-        const uint32_t dst = tbase[d] + (i - dstart[d]);
-        key_out[dst] = kk; id_out[dst] = s_id[i];
-    }
 }
 
 }  // namespace
@@ -668,8 +475,6 @@ struct SortState {
 namespace {
 
 int fail(std::string& err, int code, const char* msg) { err = msg; return code; }
-int cuda_fail(std::string& err, cudaError_t e, const char* what) { err = std::string(what) + ": " + cudaGetErrorString(e); return e == cudaErrorMemoryAllocation ? BKGPU_ENOMEM : BKGPU_ENODEV; }
-#define SCK(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return cuda_fail(err, e__, #call); } while (0)
 
 template <class T> int dalloc(SortState* s, T** p, size_t bytes, std::string& err) {
     cudaError_t e = cudaMalloc((void**)p, bytes ? bytes : 8);
@@ -696,8 +501,6 @@ void fill_row_args(const SortState* s, const DevCol* cols, int64_t nrows, RowArg
         a.key.direct = s->c.has_direct ? 1 : 0; a.key.col = s->c.has_direct ? s->c.direct_cols[0] : 0;
     }
 }
-
-int grid_for(int64_t n, int per_block, int sm) { int64_t g = (n + per_block - 1) / per_block; int64_t cap = (int64_t)sm * 8; return (int)std::max<int64_t>(1, std::min(g, cap)); }
 
 // ---- selection of the k smallest composite keys of one class out of the batch; result merged into the pool ----
 int select_topk_class(SortState* s, const RowArgs& ra, int cls, cudaStream_t st, bkgpu_stats* stats, std::string& err) {
@@ -744,7 +547,7 @@ int select_topk_class(SortState* s, const RowArgs& ra, int cls, cudaStream_t st,
             if (kc.stype == ST_I32 || kc.stype == ST_U32) k_collect_rows_vec<4><<<g, 256, 0, st>>>(ra, thr, s->cand_key[0], s->cand_idx[0], cnt + 1, s->cand_cap, cnt + 3);
             else k_collect_rows_vec<8><<<g, 256, 0, st>>>(ra, thr, s->cand_key[0], s->cand_idx[0], cnt + 1, s->cand_cap, cnt + 3);
         } else
-        k_collect_rows<<<grid_for(ra.nrows, 256, s->sm_count), 256, 0, st>>>(ra, cls, thr, s->cand_key[0], s->cand_idx[0], cnt + 1, s->cand_cap, cnt + 3);
+        k_collect_rows<<<grid_for(ra.nrows, s->sm_count, 8), 256, 0, st>>>(ra, cls, thr, s->cand_key[0], s->cand_idx[0], cnt + 1, s->cand_cap, cnt + 3);
         // level 2: cand[0] (cnt[1]) -> cand[1] (cnt[2]);  level 3: cand[1] (cnt[2]) -> cand[0] (cnt[5])
         const int src_cnt[2] = {1, 2}, dst_cnt[2] = {2, 5};
         for (int lvl = 0; lvl < 2; lvl++) {
@@ -754,7 +557,7 @@ int select_topk_class(SortState* s, const RowArgs& ra, int cls, cudaStream_t st,
                                                                    0x9e3779b9ull + attempt * 104729 + lvl);
             // (levels keep trimming until about two k-fulls are left: the one-CTA sort below costs 35 us for <= 2048 keys, 150 us for 8192)
             k_select_rank<<<1, 1024, 0, st>>>(s->samp_key, s->samp_idx, cnt, SAMPLE_N, 0, thr + 3 * (lvl + 1), cnt + src_cnt[lvl], k, widen, trim, nullptr);
-            k_collect_pairs<<<grid_for(lvl == 0 ? (int64_t)s->cand_cap / 4 : 65536, 256, s->sm_count), 256, 0, st>>>(
+            k_collect_pairs<<<grid_for(lvl == 0 ? (int64_t)s->cand_cap / 4 : 65536, s->sm_count, 8), 256, 0, st>>>(
                 s->cand_key[from], s->cand_idx[from], cnt + src_cnt[lvl], thr + 3 * (lvl + 1), s->cand_key[to], s->cand_idx[to], cnt + dst_cnt[lvl], s->cand_cap);
             stats->kernel_launches += 3;
         }
@@ -818,13 +621,15 @@ int retain_batch(SortState* s, const RowArgs& ra, cudaStream_t st, bkgpu_stats* 
     if (limit_left == 0) return 0;   // FilterNode stops after `limit` passing rows (filter_node.cpp:786-791)
     const int64_t rows_per_block = 4096;
     const uint32_t nblocks = (uint32_t)((ra.nrows + rows_per_block - 1) / rows_per_block);
-    uint32_t* counts = nullptr; uint64_t* d_total = nullptr; uint32_t* sel = nullptr; int rc;
-    if ((rc = dalloc(s, &counts, (size_t)nblocks * 4, err))) return rc;
-    if ((rc = dalloc(s, &d_total, 8, err))) return rc;
+    // counts[b]: the passing rows of block b, scanned into its first output position; counts[nblocks] closes the scan with the total
+    uint32_t *counts = nullptr, *sums = nullptr, *sel = nullptr; int rc;
+    if ((rc = dalloc(s, &counts, ((size_t)nblocks + 1) * 4, err))) return rc;
+    if ((rc = dalloc(s, &sums, (size_t)scan_scratch((int64_t)nblocks + 1) * 4, err))) return rc;
+    SCK(cudaMemsetAsync(counts + nblocks, 0, 4, st));
     k_filter_count<<<nblocks, 256, 0, st>>>(ra, counts, rows_per_block);
-    k_scan_counts<<<1, 1024, 0, st>>>(counts, nblocks, d_total);
-    uint64_t total = 0;
-    SCK(cudaMemcpyAsync(&total, d_total, 8, cudaMemcpyDeviceToHost, st));
+    SCK(scan_excl(counts, (int64_t)nblocks + 1, sums, s->sm_count, st));
+    uint32_t total = 0;
+    SCK(cudaMemcpyAsync(&total, counts + nblocks, 4, cudaMemcpyDeviceToHost, st));
     SCK(cudaStreamSynchronize(st));
     const uint64_t take = std::min<uint64_t>(total, (uint64_t)limit_left);
     if (take > 0) {
@@ -834,14 +639,14 @@ int retain_batch(SortState* s, const RowArgs& ra, cudaStream_t st, bkgpu_stats* 
         GatherArgs g; memset(&g, 0, sizeof g);
         for (int i = 0; i < s->ncols; i++) { g.cols[i] = ra.cols[i]; g.dst_vals[i] = s->ret_vals[(size_t)i]; g.dst_null[i] = s->ret_null[(size_t)i]; }
         g.n_cols = s->ncols;
-        k_gather_sel<<<grid_for((int64_t)take, 256, s->sm_count), 256, 0, st>>>(g, sel, take, (uint64_t)s->ret_rows);
+        k_gather_sel<<<grid_for((int64_t)take, s->sm_count, 8), 256, 0, st>>>(g, sel, take, (uint64_t)s->ret_rows);
         SCK(cudaStreamSynchronize(st));
         s->ret_rows += (int64_t)take;
         stats->kernel_launches += 2;
     }
-    stats->kernel_launches += 2;
+    stats->kernel_launches += 2;   // the count and the scan: one launch up to 2048 blocks (8M rows), three beyond
     stats->rows_filtered += ra.nrows - (int64_t)total;
-    dfree(s, counts); dfree(s, d_total); dfree(s, sel);
+    dfree(s, counts); dfree(s, sums); dfree(s, sel);
     return 0;
 }
 
@@ -860,12 +665,7 @@ int copy_cols_out(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, con
             int rc;
             if ((rc = dalloc(s, &tv, (size_t)n * oc.elem, err))) return rc;
             if ((rc = dalloc(s, &tn, (size_t)n, err))) return rc;
-            GatherArgs g; memset(&g, 0, sizeof g);
-            g.cols[0].values = sv; g.cols[0].validity = nullptr; g.cols[0].stype = prim_storage(cr.prim); g.cols[0].prim = cr.prim;
-            g.n_cols = 1; g.dst_vals[0] = tv; g.dst_null[0] = tn;
-            k_gather_sel<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(g, perm_dev + skip, (uint64_t)n, 0);
-            // null bytes travel separately (k_gather_sel reads validity bitmaps, retained columns hold null BYTES)
-            k_rs_gather_bytes<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(sn, perm_dev + skip, tn, (uint64_t)n);
+            if ((rc = sort_gather_rows(s, sv, sn, cr.prim, perm_dev + skip, n, tv, tn, st))) return fail(err, rc, "gathering the sorted rows failed");
             SCK(cudaMemcpyAsync(oc.values.data(), tv, (size_t)n * oc.elem, cudaMemcpyDeviceToHost, st));
             SCK(cudaMemcpyAsync(nb.data(), tn, (size_t)n, cudaMemcpyDeviceToHost, st));
             SCK(cudaStreamSynchronize(st));
@@ -892,26 +692,22 @@ int copy_out(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, const ui
 
 // scratch of one radix sort of n (key image, row id) pairs
 struct RadixBufs {
-    uint64_t *img_row = nullptr, *img[2] = {nullptr, nullptr}; uint32_t *ids[2] = {nullptr, nullptr}, *hist = nullptr, *status = nullptr;
-    uint32_t n = 0, ntiles = 0; size_t rs_smem = 0;
+    uint64_t *img_row = nullptr, *img[2] = {nullptr, nullptr}; uint32_t* ids[2] = {nullptr, nullptr};
+    void* scratch[2] = {nullptr, nullptr}; size_t scratch_cap[2] = {0, 0};   // radix_sort's, grown as its sorts need
+    uint32_t n = 0;
 };
 int radix_alloc(SortState* s, int64_t n, RadixBufs& b, std::string& err) {
     b.n = (uint32_t)n;
-    b.ntiles = (b.n + RS_TILE - 1) / RS_TILE;
     int rc;
     if ((rc = dalloc(s, &b.img_row, (size_t)n * 8, err))) return rc;
     if ((rc = dalloc(s, &b.img[0], (size_t)n * 8, err))) return rc;
     if ((rc = dalloc(s, &b.img[1], (size_t)n * 8, err))) return rc;
     if ((rc = dalloc(s, &b.ids[0], (size_t)n * 4, err))) return rc;
     if ((rc = dalloc(s, &b.ids[1], (size_t)n * 4, err))) return rc;
-    if ((rc = dalloc(s, &b.hist, (size_t)(8 * 256 * 2 + 8 + 8) * 4, err))) return rc;       // histograms, bases, active flags, tickets
-    if ((rc = dalloc(s, &b.status, (size_t)b.ntiles * 256 * 8 * 4, err))) return rc;       // one look-back array per pass
-    b.rs_smem = (size_t)RS_TILE * 12 + (8 * 256 + 256 + 256) * 4;
-    SCK(cudaFuncSetAttribute(k_rs_pass, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b.rs_smem));
     return 0;
 }
 void radix_free(SortState* s, RadixBufs& b) {
-    dfree(s, b.img_row); dfree(s, b.img[0]); dfree(s, b.img[1]); dfree(s, b.ids[0]); dfree(s, b.ids[1]); dfree(s, b.hist); dfree(s, b.status);
+    dfree(s, b.img_row); dfree(s, b.img[0]); dfree(s, b.img[1]); dfree(s, b.ids[0]); dfree(s, b.ids[1]); dfree(s, b.scratch[0]); dfree(s, b.scratch[1]);
     b = RadixBufs();
 }
 
@@ -926,7 +722,7 @@ int retained_bitmaps(SortState* s, cudaStream_t st, RowArgs& ra, std::vector<uin
     SCK(cudaMemsetAsync(null_flags, 0, sizeof(uint32_t) * MAX_COLS, st));
     for (int c = 0; c < s->ncols; c++) {
         if ((rc = dalloc(s, &bitmaps[(size_t)c], (size_t)(n + 7) / 8 + 64, err))) return rc;
-        k_pack_null_bytes<<<grid_for((n + 7) / 8, 256, s->sm_count), 256, 0, st>>>(s->ret_null[(size_t)c], n, bitmaps[(size_t)c], null_flags + c);
+        k_pack_null_bytes<<<grid_for((n + 7) / 8, s->sm_count, 8), 256, 0, st>>>(s->ret_null[(size_t)c], n, bitmaps[(size_t)c], null_flags + c);
         ra.cols[c].validity = bitmaps[(size_t)c];
     }
     SCK(cudaMemcpyAsync(h_null_flags, null_flags, sizeof(uint32_t) * (size_t)s->ncols, cudaMemcpyDeviceToHost, st));
@@ -942,46 +738,32 @@ int retained_bitmaps(SortState* s, cudaStream_t st, RowArgs& ra, std::vector<uin
 int radix_sort_keys(SortState* s, RowArgs& ra, const std::vector<SortKey>& keys, const std::vector<const Program*>& progs, int direct_col,
                     bool direct_has_nulls, RadixBufs& b, int& cur, bool identity_start, cudaStream_t st, bkgpu_stats* stats, int64_t& pass_bytes, std::string& err) {
     const int64_t n = b.n;
-    const uint32_t un = b.n, ntiles = b.ntiles;
-    uint32_t* hist = b.hist; uint32_t* bases = hist + 8 * 256; uint32_t* active = bases + 8 * 256; uint32_t* tickets = active + 8;
-    uint64_t** img = b.img; uint32_t** ids = b.ids; uint64_t* img_row = b.img_row; uint32_t* status = b.status;
+    uint64_t** img = b.img; uint32_t** ids = b.ids; uint64_t* img_row = b.img_row;
     bool first = identity_start;
-    // sorts the pairs (img[cur], ids[cur]) by the 64-bit image: one histogram pass, then one Onesweep pass per digit that varies
-    auto sort_pairs = [&]() -> int {
-        SCK(cudaMemsetAsync(hist, 0, (size_t)(8 * 256 * 2 + 8 + 8) * 4, st));
-        k_rs_hist<<<std::min(s->sm_count * 4, (int)((un + 1023) / 1024)), 256, 0, st>>>(img[cur], un, hist);
-        k_rs_bases<<<8, 256, 0, st>>>(hist, bases, active);
-        uint32_t h_active[8];
-        SCK(cudaMemcpyAsync(h_active, active, 32, cudaMemcpyDeviceToHost, st));
-        SCK(cudaStreamSynchronize(st));
-        int n_active = 0;
-        for (int d = 0; d < 8; d++) n_active += h_active[d] != 0;
-        if (n_active) SCK(cudaMemsetAsync(status, 0, (size_t)ntiles * 256 * 4 * (size_t)n_active, st));
-        stats->kernel_launches += 2; pass_bytes += (int64_t)n * 8;
-        int slot = 0;
-        for (int d = 0; d < 8; d++) {
-            if (!h_active[d]) continue;
-            k_rs_pass<<<ntiles, RS_THREADS, b.rs_smem, st>>>(img[cur], ids[cur], img[cur ^ 1], ids[cur ^ 1], un, 8 * d, bases + 256 * d,
-                                                          status + (size_t)slot * ntiles * 256, tickets + d);
-            cur ^= 1; slot++;
-            stats->kernel_launches++; pass_bytes += (int64_t)n * 24;
+    const RadixScratch scratch = [&](int slot, size_t bytes, void** out) -> int {
+        if (b.scratch_cap[slot] < bytes) {
+            dfree(s, b.scratch[slot]); b.scratch[slot] = nullptr; b.scratch_cap[slot] = 0;
+            if (int rc = dalloc(s, &b.scratch[slot], bytes, err)) return rc;
+            b.scratch_cap[slot] = bytes;
         }
+        *out = b.scratch[slot];
         return 0;
     };
-    int rc;
     for (int ki = (int)keys.size() - 1; ki >= 0; ki--) {
         const SortKey& sk = keys[(size_t)ki];
         ra.prog = *progs[(size_t)ki];
         for (int mode = 0; mode < 2; mode++) {   // the key's value image first, then its NULL rank (stable: NULLs end up strictly first / last)
             if (mode == 1 && direct_col >= 0 && !direct_has_nulls) continue;
             uint64_t* dst = first ? img[cur] : img_row;
-            if (mode == 0 && direct_col >= 0) k_sort_images_direct<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(ra.cols[direct_col], n, host_prim_class(sk.prim), sk.asc ? 0 : 1, dst);
+            if (mode == 0 && direct_col >= 0) k_sort_images_direct<<<grid_for(n, s->sm_count, 8), 256, 0, st>>>(ra.cols[direct_col], n, host_prim_class(sk.prim), sk.asc ? 0 : 1, dst);
             else
-            k_sort_images<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(ra, sk.out_reg, host_prim_class(sk.prim), sk.asc ? 0 : 1, sk.null_first ? 1 : 0, mode, dst, nullptr);
-            if (!first) k_rs_gather_u64<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(img_row, ids[cur], img[cur], un);   // images in the current order
+            k_sort_images<<<grid_for(n, s->sm_count, 8), 256, 0, st>>>(ra, sk.out_reg, host_prim_class(sk.prim), sk.asc ? 0 : 1, sk.null_first ? 1 : 0, mode, dst, nullptr);
+            if (!first) k_rs_gather_u64<<<grid_for(n, s->sm_count, 8), 256, 0, st>>>(img_row, ids[cur], img[cur], b.n);   // images in the current order
             first = false;
             stats->kernel_launches += 2;
-            if ((rc = sort_pairs())) return rc;
+            const int r = radix_sort(img, ids, cur, n, s->sm_count, scratch, st, stats, &pass_bytes, err);
+            if (r < 0) return r;
+            cur = r;
         }
     }
     return 0;
@@ -1235,7 +1017,7 @@ int sort_finish(SortState* s, void* nccl_comm, int nranks, cudaStream_t st, bkgp
     }
     // ---- full ORDER BY: stable LSD radix sort of (key image, row id) pairs, least significant ORDER BY key first ----
     const int64_t n = s->ret_rows;
-    if (n >= (int64_t)RS_VAL_MASK) return fail(err, BKGPU_EUNSUPPORTED, "full sort is limited to 2^30 rows per GPU");
+    if (n > RADIX_MAX_KEYS) return fail(err, BKGPU_EUNSUPPORTED, "full sort is limited to 2^30 - 1 rows per GPU");
     if (n == 0) { *nrows = 0; return copy_out(s, s->ret_vals.data(), s->ret_null.data(), nullptr, 0, 0, st, out, err); }
     RadixBufs b; int rc;
     if ((rc = radix_alloc(s, n, b, err))) return rc;
@@ -1244,7 +1026,7 @@ int sort_finish(SortState* s, void* nccl_comm, int nranks, cudaStream_t st, bkgp
     std::vector<uint8_t*> bitmaps; uint32_t h_null_flags[MAX_COLS] = {0};
     if ((rc = retained_bitmaps(s, st, ra, bitmaps, h_null_flags, err))) return rc;
     ra.prog = s->c.prog; ra.key.pred_out = -1;
-    k_rs_iota<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(b.ids[0], (uint32_t)n);
+    k_iota<<<grid_for(n, s->sm_count, 8), 256, 0, st>>>(b.ids[0], n);
     int cur = 0;
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
     cudaEventRecord(e0, st);
@@ -1289,7 +1071,6 @@ void sort_free_scratch(SortState* s, std::vector<void*>& scratch) { for (void* p
 
 int sort_stable_ids(SortState* s, const DevCol* cols, int64_t n, const std::vector<SortKey>& keys, const std::vector<const Program*>& progs,
                     uint32_t* ids, cudaStream_t st, bkgpu_stats* stats, std::string& err) {
-    if (n >= (int64_t)RS_VAL_MASK) return fail(err, BKGPU_EUNSUPPORTED, "a window sort is limited to 2^30 rows per GPU");
     if (n == 0 || keys.empty()) return 0;
     RadixBufs b; int rc;
     if ((rc = radix_alloc(s, n, b, err))) return rc;
@@ -1316,8 +1097,9 @@ int sort_gather_rows(SortState* s, const uint8_t* src_vals, const uint8_t* src_n
     GatherArgs g; memset(&g, 0, sizeof g);
     g.cols[0].values = src_vals; g.cols[0].validity = nullptr; g.cols[0].stype = prim_storage(prim); g.cols[0].prim = prim;
     g.n_cols = 1; g.dst_vals[0] = dst_vals; g.dst_null[0] = dst_null;
-    k_gather_sel<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(g, perm_dev, (uint64_t)n, 0);
-    k_rs_gather_bytes<<<grid_for(n, 256, s->sm_count), 256, 0, st>>>(src_null, perm_dev, dst_null, (uint64_t)n);
+    k_gather_sel<<<grid_for(n, s->sm_count, 8), 256, 0, st>>>(g, perm_dev, (uint64_t)n, 0);
+    // null bytes travel separately (k_gather_sel reads validity bitmaps, retained columns hold null BYTES)
+    k_rs_gather_bytes<<<grid_for(n, s->sm_count, 8), 256, 0, st>>>(src_null, perm_dev, dst_null, (uint64_t)n);
     return cudaGetLastError() == cudaSuccess ? 0 : BKGPU_ENODEV;
 }
 

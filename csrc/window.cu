@@ -18,6 +18,7 @@
 #include <string.h>
 #include "dev_common.cuh"
 #include "interp.cuh"
+#include "prims.cuh"
 
 namespace bk {
 
@@ -286,18 +287,6 @@ __global__ void k_win_fn(FnArgs a) {
     }
 }
 
-__global__ void k_win_iota(uint32_t* p, int64_t n) { for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) p[i] = (uint32_t)i; }
-// null bytes (1 = NULL) -> Arrow validity bitmap (bit set = valid)
-__global__ void k_win_pack(const uint8_t* nb, int64_t n, uint8_t* bitmap) {
-    for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < (n + 7) / 8; b += (int64_t)gridDim.x * blockDim.x) {
-        uint32_t v = 0;
-        for (int j = 0; j < 8; j++) { const int64_t r = b * 8 + j; if (r < n && !nb[r]) v |= 1u << j; }
-        bitmap[b] = (uint8_t)v;
-    }
-}
-
-int cuda_fail(std::string& err, cudaError_t e, const char* what) { err = std::string(what) + ": " + cudaGetErrorString(e); return e == cudaErrorMemoryAllocation ? BKGPU_ENOMEM : BKGPU_ENODEV; }
-#define WCK(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return cuda_fail(err, e__, #call); } while (0)
 
 // the stage timer's two events, destroyed on every way out of window_finish
 struct EventPair {
@@ -317,8 +306,6 @@ struct Arena {
     }
     void drop(void* x) { auto it = std::find(p.begin(), p.end(), x); if (it != p.end()) { cudaFree(x); p.erase(it); } }
 };
-
-int grid_of(int64_t n, int sm) { const int64_t g = (n + 255) / 256; return (int)std::max<int64_t>(1, std::min<int64_t>(g, (int64_t)sm * 8)); }
 
 struct ScanBufs { Acc* agg = nullptr; Acc* carry = nullptr; uint32_t ntiles = 0; };
 
@@ -347,18 +334,18 @@ int window_finish(const Compiled& c, SortState* rows, SortState* post, cudaStrea
     std::vector<DevCol> cols; std::vector<void*> bitmaps; int64_t n = 0; int rc;
     if ((rc = sort_retained_cols(rows, st, cols, bitmaps, &n, err))) return rc;
     struct Release { SortState* s; std::vector<void*>& b; ~Release() { sort_free_scratch(s, b); } } release{rows, bitmaps};
-    if (n >= (int64_t)1 << 30) { err = "a window fragment is limited to 2^30 rows per GPU"; return BKGPU_EUNSUPPORTED; }
+    if (n > RADIX_MAX_KEYS) { err = "a window fragment is limited to 2^30 - 1 rows per GPU"; return BKGPU_EUNSUPPORTED; }
     const int ncols = (int)cols.size();
     uint32_t* perm = nullptr;
-    WCK(ar.get(&perm, (size_t)n * 4));
-    if (n) k_win_iota<<<grid_of(n, sm), 256, 0, st>>>(perm, n);
+    SCK(ar.get(&perm, (size_t)n * 4));
+    if (n) k_iota<<<grid_for(n, sm, 8), 256, 0, st>>>(perm, n);
     // window outputs, in row space
     std::vector<uint8_t*> wvals, wnull;
     for (const WinStage& w : c.win)
         for (const WinFn& f : w.fns) {
             uint8_t *v = nullptr, *nb = nullptr;
-            WCK(ar.get(&v, (size_t)std::max<int64_t>(n, 1) * storage_bytes(prim_storage(f.out_prim))));
-            WCK(ar.get(&nb, (size_t)std::max<int64_t>(n, 1)));
+            SCK(ar.get(&v, (size_t)std::max<int64_t>(n, 1) * storage_bytes(prim_storage(f.out_prim))));
+            SCK(ar.get(&nb, (size_t)std::max<int64_t>(n, 1)));
             wvals.push_back(v); wnull.push_back(nb);
         }
     EventPair ev_pair;
@@ -367,8 +354,8 @@ int window_finish(const Compiled& c, SortState* rows, SortState* post, cudaStrea
     size_t fn_index = 0;
     const uint32_t ntiles = (uint32_t)((n + SC_TILE - 1) / SC_TILE);
     ScanBufs sb; sb.ntiles = ntiles;
-    WCK(ar.get(&sb.agg, (size_t)std::max<uint32_t>(ntiles, 1) * sizeof(Acc)));
-    WCK(ar.get(&sb.carry, (size_t)std::max<uint32_t>(ntiles, 1) * sizeof(Acc)));
+    SCK(ar.get(&sb.agg, (size_t)std::max<uint32_t>(ntiles, 1) * sizeof(Acc)));
+    SCK(ar.get(&sb.carry, (size_t)std::max<uint32_t>(ntiles, 1) * sizeof(Acc)));
     for (const WinStage& w : c.win) {
         if (w.new_sort && n > 0) {   // stable radix sort of the current order by the stage's keys (each key: output 0 of its own program)
             std::vector<SortKey> keys; std::vector<const Program*> progs;
@@ -383,25 +370,25 @@ int window_finish(const Compiled& c, SortState* rows, SortState* post, cudaStrea
         for (int k = 0; k < ncols; k++) ea.cols[k] = cols[(size_t)k];
         ea.n_cols = ncols; ea.nrows = n;
         for (size_t e = 0; e < w.exprs.size(); e++) {
-            WCK(ar.get(&ev[e], (size_t)n * 8)); WCK(ar.get(&en[e], (size_t)n));
+            SCK(ar.get(&ev[e], (size_t)n * 8)); SCK(ar.get(&en[e], (size_t)n));
             ea.prog = w.exprs[e];
-            k_win_eval<<<grid_of(n, sm), 256, 0, st>>>(ea, perm, ev[e], en[e]);
+            k_win_eval<<<grid_for(n, sm, 8), 256, 0, st>>>(ea, perm, ev[e], en[e]);
             win_launches++; win_bytes += n * (4 + 9);
         }
         // 2. partition / peer starts
         uint8_t *part = nullptr, *peer = nullptr;
-        WCK(ar.get(&part, (size_t)n + 1)); WCK(ar.get(&peer, (size_t)n + 1));
+        SCK(ar.get(&part, (size_t)n + 1)); SCK(ar.get(&peer, (size_t)n + 1));
         KeyCmp kc; memset(&kc, 0, sizeof kc);
         kc.n_part = w.n_part; kc.n_keys = (int)w.sort_keys.size();
         for (int k = 0; k < kc.n_keys; k++) {
             const SortKey& sk = w.sort_keys[(size_t)k];
             kc.val[k] = ev[(size_t)sk.out_reg]; kc.nul[k] = en[(size_t)sk.out_reg]; kc.is_f64[k] = host_prim_class(sk.prim) == VC_F64;
         }
-        k_win_flags<<<grid_of(n, sm), 256, 0, st>>>(kc, n, part, peer);
+        k_win_flags<<<grid_for(n, sm, 8), 256, 0, st>>>(kc, n, part, peer);
         win_launches++; win_bytes += n * (9 * 2 * kc.n_keys + 2);
         // 3. partition and peer-group bounds: the first index of the segment, forward and backward
         uint64_t *ps = nullptr, *pl = nullptr, *qs = nullptr, *ql = nullptr;
-        WCK(ar.get(&ps, (size_t)n * 8)); WCK(ar.get(&pl, (size_t)n * 8)); WCK(ar.get(&qs, (size_t)n * 8)); WCK(ar.get(&ql, (size_t)n * 8));
+        SCK(ar.get(&ps, (size_t)n * 8)); SCK(ar.get(&pl, (size_t)n * 8)); SCK(ar.get(&qs, (size_t)n * 8)); SCK(ar.get(&ql, (size_t)n * 8));
         auto index_scan = [&](const uint8_t* seg, int rev, uint64_t* dst) {
             ScanIn in; memset(&in, 0, sizeof in);
             in.seg = seg; in.n = (uint32_t)n; in.rev = rev; in.mode = SM_INDEX;
@@ -423,7 +410,7 @@ int window_finish(const Compiled& c, SortState* rows, SortState* post, cudaStrea
             fa.perm = perm; fa.out_vals = wvals[fn_index]; fa.out_null = wnull[fn_index]; fa.out_stype = prim_storage(f.out_prim);
             const bool scanned = (f.kind <= WF_MAX && (f.method == WM_FWD || f.method == WM_BWD || f.method == WM_PEER)) || (f.kind == WF_DENSE_RANK && fa.has_order);
             if (scanned) {
-                if (!sv) { WCK(ar.get(&sv, (size_t)n * 8)); WCK(ar.get(&sc, (size_t)n * 8)); }
+                if (!sv) { SCK(ar.get(&sv, (size_t)n * 8)); SCK(ar.get(&sc, (size_t)n * 8)); }
                 ScanIn in; memset(&in, 0, sizeof in);
                 in.n = (uint32_t)n; in.vclass = fa.arg_vclass;
                 int op;
@@ -437,18 +424,18 @@ int window_finish(const Compiled& c, SortState* rows, SortState* post, cudaStrea
                 fa.sv = sv; fa.sc = sc;
                 win_launches += 3; win_bytes += n * (2 * (9 + 1) + 16);
             }
-            k_win_fn<<<grid_of(n, sm), 256, 0, st>>>(fa);
+            k_win_fn<<<grid_for(n, sm, 8), 256, 0, st>>>(fa);
             win_launches++; win_bytes += n * (4 * 8 + 4 + 9 + storage_bytes(fa.out_stype) + 1 + (scanned ? 16 : 0));
             fn_index++;
         }
         cudaEventRecord(e1, st);
-        WCK(cudaEventSynchronize(e1));
+        SCK(cudaEventSynchronize(e1));
         float ms = 0; cudaEventElapsedTime(&ms, e0, e1); win_ms += ms;
         for (size_t e = 0; e < ev.size(); e++) { ar.drop(ev[e]); ar.drop(en[e]); }
         ar.drop(part); ar.drop(peer); ar.drop(ps); ar.drop(pl); ar.drop(qs); ar.drop(ql);
         if (sv) { ar.drop(sv); ar.drop(sc); }
     }
-    WCK(cudaGetLastError());
+    SCK(cudaGetLastError());
     stats->main_kernel_ms += win_ms; stats->main_kernel_launches += 1; stats->main_kernel_bytes += win_bytes;
     stats->kernel_launches += win_launches;
     snprintf(stats->main_kernel_name, sizeof stats->main_kernel_name, "%s", "window_stage(k_win_fn)");
@@ -474,12 +461,12 @@ int window_finish(const Compiled& c, SortState* rows, SortState* post, cudaStrea
         for (size_t k = 0; k < desc.size(); k++) {
             const int eb = storage_bytes(prim_storage(desc[k].prim));
             uint8_t *v = nullptr, *nb = nullptr, *bm = nullptr;
-            WCK(ar.get(&v, (size_t)n * eb)); WCK(ar.get(&nb, (size_t)n)); WCK(ar.get(&bm, (size_t)(n + 7) / 8 + 64));
+            SCK(ar.get(&v, (size_t)n * eb)); SCK(ar.get(&nb, (size_t)n)); SCK(ar.get(&bm, (size_t)(n + 7) / 8 + 64));
             if ((rc = sort_gather_rows(rows, all_v[k], all_n[k], desc[k].prim, perm, n, v, nb, st))) { err = "window output gather failed"; return rc; }
-            k_win_pack<<<grid_of((n + 7) / 8, sm), 256, 0, st>>>(nb, n, bm);
+            k_pack_null_bytes<<<grid_for((n + 7) / 8, sm, 8), 256, 0, st>>>(nb, n, bm, nullptr);
             dc[k].values = v; dc[k].validity = bm; dc[k].stype = prim_storage(desc[k].prim); dc[k].prim = desc[k].prim;
         }
-        WCK(cudaGetLastError());
+        SCK(cudaGetLastError());
         bkgpu_stats scratch{};   // (the post fragment's kernels are not the request's main kernel)
         if ((rc = sort_push(post, dc.data(), n, st, &scratch, err))) return rc;
         stats->kernel_launches += scratch.kernel_launches;

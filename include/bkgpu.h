@@ -108,7 +108,8 @@ int   bkgpu_init(bkgpu_plan** out, const uint8_t* plan_desc, size_t len,
  *   "partial_capacity"     groups per rank in the exported partial state (a plan with hll_add_agg ships 16 KB of registers per group and sketch)
  *   "rb_pair_capacity"     keys the rb_build_agg pair buffer holds: one per row and rb_build_agg with a non-NULL value until it is sorted
  *                          and deduplicated, which happens whenever it could overflow (default 2^27; 16 bytes of device memory each, the sort
- *                          needs a second buffer; 1024 .. 2^31); more distinct (group, value) pairs -> BKGPU_ETOOBIG naming this option
+ *                          needs a second buffer, and its look-back scratch takes 1 KB per 3072 keys and active 8-bit digit; 1024 .. 2^30 - 1);
+ *                          more distinct (group, value) pairs -> BKGPU_ETOOBIG naming this option
  *   "hll_group_capacity"   sketches the hll_add_agg register arena holds: one per group and hll_add_agg aggregate that receives a non-NULL
  *                          value, 16 KB of device memory each (default 4096 = 64 MB, at most 2^20); more -> BKGPU_ETOOBIG naming this option
  *   "region_base"          arrival index of this plan's first row: ORDER BY ties across GPUs break by (region, row)

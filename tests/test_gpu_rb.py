@@ -1,7 +1,8 @@
 """GPU parity of rb_build_agg: every returned bitmap is byte-identical to tests/roaring_oracle.py's (the reference's add(), runOptimize()
 and portable serialization), across argument types with negative values wrapping, NULLs, scalar and empty input, filters, 1 to 100k
 groups, dense and sparse values, two bitmaps beside COUNT and SUM, host and device batches, reuse after bkgpu_reset, a pair buffer small
-enough to be compacted mid-request and one too small, the join, APPLY and star join fragments, and 100M device-generated rows."""
+enough to be compacted mid-request, one too small and one beyond the radix sort's limit, the join, APPLY and star join fragments, and
+100M device-generated rows."""
 import ctypes
 
 import numpy as np
@@ -217,6 +218,21 @@ def test_compaction_in_a_small_pair_buffer_and_too_small_a_buffer():
     with pytest.raises(BkgpuError) as e:
         execute(C.scan_plan(T.INT64), cols, options={"rb_pair_capacity": 1024})
     assert e.value.code == _lib.ETOOBIG and "rb_pair_capacity" in e.value.message
+
+
+def test_pair_capacity_below_the_radix_sort_limit():
+    """the radix sort takes at most 2^30 - 1 keys: rb_pair_capacity 2^30 is refused, 2^30 - 1 accepted (the plan is not opened, so
+    nothing is allocated)"""
+    L = _lib.lib()
+    plan = C.scan_plan(T.INT64).serialize()
+    h = ctypes.c_void_p()
+    _lib.check(L.bkgpu_init(ctypes.byref(h), plan, len(plan), 0, None))
+    try:
+        assert L.bkgpu_set_option(h, b"rb_pair_capacity", 2**30) == _lib.EINVAL
+        assert "rb_pair_capacity" in L.bkgpu_last_error(h).decode()
+        assert L.bkgpu_set_option(h, b"rb_pair_capacity", 2**30 - 1) == _lib.OK
+    finally:
+        L.bkgpu_close(h)
 
 
 def test_partial_state_and_communicator_refused():
