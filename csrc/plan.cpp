@@ -2025,6 +2025,8 @@ static bool lower_window(Infer& in, Compiled& out, const HNode& wtop, const HNod
             }
             if (wf.kind == WF_NTILE && (f.ch.empty() || !int_literal(f.ch[0], wf.n) || wf.n <= 0)) return in.fail(BKGPU_EUNSUPPORTED, "NTILE needs an integer literal > 0");
             if (wf.kind == WF_NTH_VALUE && (f.ch.size() < 2 || !int_literal(f.ch[1], wf.n) || wf.n <= 0)) return in.fail(BKGPU_EUNSUPPORTED, "NTH_VALUE needs an integer literal > 0");
+            if (wf.kind == WF_NTH_VALUE && wf.n > INT32_MAX)   // (the reference reads row start + n - 1 through an int: no meaning past it)
+                return in.fail(BKGPU_EUNSUPPORTED, "NTH_VALUE with n > 2147483647 is outside the GPU path (the reference truncates the row index to int)");
             if (wf.kind == WF_LEAD || wf.kind == WF_LAG) {
                 wf.n = 1;
                 if (f.ch.size() > 1 && (!int_literal(f.ch[1], wf.n) || wf.n < 0)) return in.fail(BKGPU_EUNSUPPORTED, "the LEAD / LAG offset must be an integer literal >= 0");

@@ -57,7 +57,9 @@ __global__ void k_win_flags(KeyCmp k, int64_t n, uint8_t* part, uint8_t* peer) {
 }
 
 // ---- segmented scan ----
-enum ScanOp { SC_FIRST = 0, SC_SUM_I64, SC_SUM_F64, SC_MIN, SC_MAX };
+// MIN / MAX of a FLOAT / DOUBLE argument keep the earlier row of -0.0 and +0.0 in frame order, as the reference's strict
+// ExprValue::compare does: the _F64 ops tie the two zeros; in a backward scan (_BWD) the left operand is the later row
+enum ScanOp { SC_FIRST = 0, SC_SUM_I64, SC_SUM_F64, SC_MIN, SC_MAX, SC_MIN_F64, SC_MAX_F64, SC_MIN_F64_BWD, SC_MAX_F64_BWD };
 enum ScanMode { SM_VALUE = 0, SM_INDEX = 1, SM_FLAG = 2 };
 struct Acc { uint64_t v, c; uint32_t f; };
 struct ScanIn {
@@ -68,7 +70,13 @@ struct ScanIn {
 };
 constexpr int SC_THREADS = 256, SC_ITEMS = 8, SC_TILE = SC_THREADS * SC_ITEMS;
 
-template <int OP> __device__ __forceinline__ uint64_t sc_ident() { return OP == SC_MIN ? ~0ull : 0ull; }
+constexpr bool sc_is_min(int op) { return op == SC_MIN || op == SC_MIN_F64 || op == SC_MIN_F64_BWD; }
+constexpr uint64_t IMG_NEG_ZERO = 0x7FFFFFFFFFFFFFFFull, IMG_POS_ZERO = 0x8000000000000000ull;   // ord_image of -0.0 / +0.0
+// the key MIN / MAX compare: the order-preserving image, with -0.0 equal to +0.0 for FLOAT / DOUBLE
+__device__ __forceinline__ uint64_t mm_key(uint64_t t, bool f64) { return f64 && t == IMG_NEG_ZERO ? IMG_POS_ZERO : t; }
+// SUM's identity is -0.0, the one double x with -0.0 + x == x for every x: a frame of only -0.0 (and NULLs) sums to -0.0, as the
+// reference's SUM (the first value, then the rest added) does
+template <int OP> __device__ __forceinline__ uint64_t sc_ident() { return sc_is_min(OP) ? ~0ull : OP == SC_SUM_F64 ? 0x8000000000000000ull : 0ull; }
 template <int OP> __device__ __forceinline__ Acc sc_identity() { Acc a; a.v = sc_ident<OP>(); a.c = 0; a.f = 0; return a; }
 template <int OP> __device__ __forceinline__ Acc sc_comb(const Acc& a, const Acc& b) {
     if (b.f) return b;
@@ -76,8 +84,13 @@ template <int OP> __device__ __forceinline__ Acc sc_comb(const Acc& a, const Acc
     if (OP == SC_FIRST) r.v = a.v;
     else if (OP == SC_SUM_I64) r.v = a.v + b.v;                                                     // two's-complement wrap
     else if (OP == SC_SUM_F64) r.v = __double_as_longlong(__longlong_as_double(a.v) + __longlong_as_double(b.v));
-    else if (OP == SC_MIN) r.v = a.v < b.v ? a.v : b.v;                                               // order-preserving images
-    else r.v = a.v > b.v ? a.v : b.v;
+    else {                                                                                           // order-preserving images
+        constexpr bool f64 = OP >= SC_MIN_F64, bwd = OP >= SC_MIN_F64_BWD;
+        const uint64_t ka = mm_key(a.v, f64), kb = mm_key(b.v, f64);
+        // b replaces a when strictly lower / higher; on a tie the backward scan takes b, the earlier row
+        const bool take_b = sc_is_min(OP) ? (bwd ? kb <= ka : kb < ka) : (bwd ? kb >= ka : kb > ka);
+        r.v = take_b ? b.v : a.v;
+    }
     return r;
 }
 // order-preserving image of a value of class vclass (MIN / MAX compare these), and back
@@ -101,7 +114,7 @@ template <int OP> __device__ __forceinline__ Acc sc_load(const ScanIn& in, uint3
     else if (in.mode == SM_FLAG) a.v = in.vflag[p];
     else if (!in.v) a.v = sc_ident<OP>();
     else if (in.nul[p]) { a.v = sc_ident<OP>(); a.c = 0; }
-    else a.v = (OP == SC_MIN || OP == SC_MAX) ? ord_image(in.v[p], in.vclass) : in.v[p];
+    else a.v = OP >= SC_MIN ? ord_image(in.v[p], in.vclass) : in.v[p];
     return a;
 }
 template <int OP> __device__ __forceinline__ Acc sc_shfl_up(const Acc& a, int d) {
@@ -241,30 +254,36 @@ __global__ void k_win_fn(FnArgs a) {
                 const int64_t q = size / a.param, rem = size % a.param, big = rem * (q + 1);
                 v = (uint64_t)(r < big ? r / (q + 1) + 1 : rem + (r - big) / q + 1);
             } break;
-            case WF_LEAD: case WF_LAG: {
-                const int64_t j = a.kind == WF_LEAD ? i + a.param : i - a.param;
-                if (j >= ps && j < pe) { v = a.arg[j]; isnull = a.arg_nul[j]; }
+            case WF_LEAD: case WF_LAG: {   // (offsets up to INT64_MAX: compared with the distance to the partition's edge, never added)
+                const bool inside = a.kind == WF_LEAD ? a.param < pe - i : a.param <= i - ps;
+                if (inside) { const int64_t j = a.kind == WF_LEAD ? i + a.param : i - a.param; v = a.arg[j]; isnull = a.arg_nul[j]; }
                 else if (a.def) { v = a.def[i]; isnull = a.def_nul[i]; }
                 else isnull = true;
             } break;
             case WF_FIRST_VALUE: case WF_LAST_VALUE: case WF_NTH_VALUE: {
-                const int64_t j = a.kind == WF_FIRST_VALUE ? fs : (a.kind == WF_LAST_VALUE ? fe - 1 : fs + a.param - 1);
-                if (empty || j >= fe) isnull = true;
-                else { v = a.arg[j]; isnull = a.arg_nul[j]; }
+                // (NTH_VALUE: n is compared with the frame's width, so fs + n - 1 is only formed when it lies inside the frame)
+                if (empty || (a.kind == WF_NTH_VALUE && a.param > fe - fs)) isnull = true;
+                else {
+                    const int64_t j = a.kind == WF_FIRST_VALUE ? fs : (a.kind == WF_LAST_VALUE ? fe - 1 : fs + a.param - 1);
+                    v = a.arg[j]; isnull = a.arg_nul[j];
+                }
             } break;
             default: {   // COUNT(*) COUNT SUM AVG MIN MAX over the frame
                 uint64_t acc = 0, cnt = 0;
                 if (!empty) {
                     if (a.method == WM_DIRECT) {
-                        const bool is_min = a.kind == WF_MIN, is_max = a.kind == WF_MAX;
+                        const bool is_min = a.kind == WF_MIN, is_max = a.kind == WF_MAX, f64 = a.arg_vclass == VC_F64;
                         acc = is_min ? ~0ull : 0ull;
-                        double dacc = 0.0; bool dsum = false;
+                        double dacc = -0.0; bool dsum = false;   // (SUM's identity, as in the scans)
                         for (int64_t j = fs; j < fe; j++) {
                             if (a.kind == WF_COUNT_STAR) { cnt++; continue; }
                             if (a.arg_nul[j]) continue;
                             const uint64_t x = a.arg[j];
                             cnt++;
-                            if (is_min || is_max) { const uint64_t t = ord_image(x, a.arg_vclass); acc = is_min ? (t < acc ? t : acc) : (t > acc ? t : acc); }
+                            if (is_min || is_max) {   // the first value, then strictly lower / higher ones (the earlier of equal zeros stays)
+                                const uint64_t t = ord_image(x, a.arg_vclass), kt = mm_key(t, f64), ka = mm_key(acc, f64);
+                                if (cnt == 1 || (is_min ? kt < ka : kt > ka)) acc = t;
+                            }
                             else if (a.kind == WF_AVG || (a.kind == WF_SUM && a.arg_vclass == VC_F64)) { dacc += __longlong_as_double(x); dsum = true; }
                             else acc += x;
                         }
@@ -276,7 +295,7 @@ __global__ void k_win_fn(FnArgs a) {
                 }
                 if (a.kind == WF_COUNT_STAR || a.kind == WF_COUNT) v = cnt;
                 else if (cnt == 0) isnull = true;
-                else if (a.kind == WF_AVG) v = (uint64_t)__double_as_longlong(__longlong_as_double(acc) / (double)cnt);
+                else if (a.kind == WF_AVG) v = (uint64_t)__double_as_longlong((__longlong_as_double(acc) + 0.0) / (double)cnt);   // (the reference's AVG sum starts at +0.0)
                 else if (a.kind == WF_MIN || a.kind == WF_MAX) v = ord_value(acc, a.arg_vclass);
                 else v = acc;
             }
@@ -320,7 +339,11 @@ void run_scan(int op, const ScanIn& in, const ScanBufs& b, uint64_t* out_v, uint
         case SC_SUM_I64: launch_scan<SC_SUM_I64>(in, b, out_v, out_c, st); break;
         case SC_SUM_F64: launch_scan<SC_SUM_F64>(in, b, out_v, out_c, st); break;
         case SC_MIN: launch_scan<SC_MIN>(in, b, out_v, out_c, st); break;
-        default: launch_scan<SC_MAX>(in, b, out_v, out_c, st); break;
+        case SC_MAX: launch_scan<SC_MAX>(in, b, out_v, out_c, st); break;
+        case SC_MIN_F64: launch_scan<SC_MIN_F64>(in, b, out_v, out_c, st); break;
+        case SC_MAX_F64: launch_scan<SC_MAX_F64>(in, b, out_v, out_c, st); break;
+        case SC_MIN_F64_BWD: launch_scan<SC_MIN_F64_BWD>(in, b, out_v, out_c, st); break;
+        default: launch_scan<SC_MAX_F64_BWD>(in, b, out_v, out_c, st); break;
     }
 }
 
@@ -419,6 +442,8 @@ int window_finish(const Compiled& c, SortState* rows, SortState* post, cudaStrea
                     in.mode = SM_VALUE; in.v = fa.arg; in.nul = fa.arg_nul;
                     in.seg = f.method == WM_PEER ? peer : part; in.rev = f.method == WM_BWD;
                     op = f.kind == WF_MIN ? SC_MIN : f.kind == WF_MAX ? SC_MAX : (f.kind == WF_AVG || (f.kind == WF_SUM && fa.arg_vclass == VC_F64)) ? SC_SUM_F64 : SC_SUM_I64;
+                    if (op == SC_MIN && fa.arg_vclass == VC_F64) op = in.rev ? SC_MIN_F64_BWD : SC_MIN_F64;
+                    if (op == SC_MAX && fa.arg_vclass == VC_F64) op = in.rev ? SC_MAX_F64_BWD : SC_MAX_F64;
                 }
                 run_scan(op, in, sb, sv, sc, st);
                 fa.sv = sv; fa.sc = sc;

@@ -9,6 +9,16 @@ frame)), and RANK / DENSE_RANK / PERCENT_RANK / CUME_DIST / NTILE / LEAD / LAG s
 get_result does.  The sort is stable (rows with equal keys keep their arrival order), with the device's total order: NULLs
 first / last per is_null_first, -0.0 and +0.0 equal keys (as in MemRowCompare), NaN by its IEEE bits.
 
+MIN / MAX replace their value only when ExprValue::compare is strictly lower / higher (window_fn_call.cpp, case MIN / MAX).  For
+FLOAT / DOUBLE that compare is `>` / `<`, so -0.0 and +0.0 are equal and the first zero in frame order is kept.  NaN is the one
+documented divergence (DESIGN §4): the reference's compare calls a NaN equal to everything, the device orders NaN by its IEEE bits,
+and so does this oracle.  SUM takes the first value and adds the rest (a SUM of only -0.0 is -0.0); AVG adds to a sum that starts
+at +0.0.
+
+assert_matches compares bit for bit.  The one declared exception is a DOUBLE SUM / AVG the device reads from a segmented scan
+(frames with an unbounded side, RANGE CURRENT ROW frames, the whole partition): the scan adds in tree order, so it is compared with
+the exact sum of its frame within the error bound of any summation order, and its class (NaN, +-inf, a zero's sign) must match.
+
 Expressions: slot references, INT / DOUBLE / NULL literals, + - *, comparisons and AND — enough for the tests' arguments,
 filters and keys.
 """
@@ -16,6 +26,7 @@ from __future__ import annotations
 
 import math
 import struct
+from fractions import Fraction
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -24,7 +35,12 @@ from baikaldb_b200.plan import BoundType, ExprNodeType, FrameType, FuncType, Pla
 
 M64 = (1 << 64) - 1
 FLOATS = (T.FLOAT, T.DOUBLE)
-UINTS = (T.UINT8, T.UINT16, T.UINT32, T.UINT64, T.TIMESTAMP, T.DATE)
+UINTS = (T.UINT8, T.UINT16, T.UINT32, T.UINT64, T.TIMESTAMP, T.DATE, T.DATETIME)
+# integer targets of cast_to: (bits, signed)
+_INT_WIDTH = {T.INT8: (8, True), T.INT16: (16, True), T.INT32: (32, True), T.TIME: (32, True), T.INT64: (64, True),
+              T.UINT8: (8, False), T.UINT16: (16, False), T.UINT32: (32, False), T.TIMESTAMP: (32, False), T.DATE: (32, False),
+              T.UINT64: (64, False), T.DATETIME: (64, False)}
+U = 2.0 ** -53   # unit roundoff of a DOUBLE
 
 
 def _wrap64(v: int) -> int:
@@ -98,15 +114,40 @@ def _eval(e, row: Dict[Tuple[int, int], object], types):
     raise NotImplementedError(f"expression node {nt}")
 
 
+def _wrapn(v: int, bits: int, signed: bool) -> int:
+    v &= (1 << bits) - 1
+    return v - (1 << bits) if signed and v >> (bits - 1) else v
+
+
+def _f64_to_i64_x86(d: float) -> int:
+    """cvttsd2si: truncation, and INT64_MIN for NaN and out-of-range values"""
+    return int(d) if -2.0 ** 63 <= d < 2.0 ** 63 else -(1 << 63)
+
+
 def _cast(v, to: int):
-    """ExprValue::cast_to for the window functions' argument casts"""
+    """ExprValue::cast_to of a numeric value (a Python int, or a float for FLOAT / DOUBLE), with the x86-64 conversions the
+    reference binary's static_casts compile to (csrc/dev_common.cuh cast_prim): FLOAT rounds through float32, BOOL is != 0, integers
+    wrap to their width (UINT64 -> INT64 reinterprets the bits), a double converts by truncation — to UINT64 / DATETIME the way gcc
+    does (values >= 2^63 through the signed path minus 2^63), to UINT32 / DATE / TIMESTAMP through int64, to the narrower types
+    through int32 (INT32_MIN when out of range) — and DATE / TIMESTAMP take a numeric value as uint32."""
     if v is None:
         return None
     if to in FLOATS:
-        return float(v)
-    if to == T.INT64:
-        return _wrap64(int(v))
-    return v
+        d = float(v)
+        return float(np.float32(d)) if to == T.FLOAT else d
+    if to == T.BOOL:
+        return 1 if v != 0 else 0
+    bits, signed = _INT_WIDTH[to]
+    if isinstance(v, float):
+        if to in (T.UINT64, T.DATETIME):
+            i = _f64_to_i64_x86(v - 2.0 ** 63) ^ (1 << 63) if v >= 2.0 ** 63 else _f64_to_i64_x86(v)
+        elif bits == 64 or to in (T.UINT32, T.DATE, T.TIMESTAMP):
+            i = _f64_to_i64_x86(v)
+        else:
+            i = int(v) if -2.0 ** 31 <= v < 2.0 ** 31 else -(1 << 31)
+    else:
+        i = int(v)
+    return _wrapn(i, bits, signed)
 
 
 def _same(a, b) -> bool:
@@ -169,7 +210,6 @@ class _Fn:
 
     def partition_reset(self):
         self.cnt, self.sum, self.avg_sum, self.min_max, self.value = 0, None, 0.0, None, None
-        self.abs_sum = 0.0   # Σ|x| over the frame: the scale of a DOUBLE sum's rounding error
         self.row_number = 0
         self.cur_idx, self.last_rank, self.batch = 0, 0, None
         self.cur_group_idx, self.quotient, self.remainder = 1, 0, 0
@@ -177,7 +217,6 @@ class _Fn:
     def frame_reset(self):
         if self.name in ("count_star", "count", "sum", "avg", "min", "max", "first_value", "last_value", "nth_value"):
             self.cnt, self.sum, self.avg_sum, self.min_max, self.value = 0, None, 0.0, None, None
-            self.abs_sum = 0.0
 
     def call(self, batch, start, end):
         nm = self.name
@@ -189,13 +228,11 @@ class _Fn:
             for i in range(start, end):
                 v = self._x(batch[i])
                 if v is not None:
-                    self.abs_sum += abs(float(v))
                     self.sum = v if self.sum is None else (self.sum + v if self.col_type == T.DOUBLE else _wrap64(self.sum + v))
         elif nm == "avg":
             for i in range(start, end):
                 v = self._x(batch[i])
                 if v is not None:
-                    self.abs_sum += abs(float(v))
                     self.avg_sum += float(v)
                     self.cnt += 1
         elif nm in ("min", "max"):
@@ -206,8 +243,8 @@ class _Fn:
                     continue
                 if self.min_max is None:
                     self.min_max = v
-                else:
-                    iv, im = _image(v, at, True, zeros_equal=False), _image(self.min_max, at, True, zeros_equal=False)
+                else:   # a strict compare: of -0.0 and +0.0 the first stays
+                    iv, im = _image(v, at, True), _image(self.min_max, at, True)
                     if (nm == "min" and im > iv) or (nm == "max" and im < iv):
                         self.min_max = v
         elif nm in ("rank", "dense_rank", "percent_rank", "cume_dist", "lead", "lag"):
@@ -223,13 +260,12 @@ class _Fn:
             if start <= idx < end:
                 self.value = self._x(batch[idx])
 
-    def error_scale(self) -> float:
-        """the bound on a result's rounding error over its frame: Σ|x| for SUM, Σ|x| / count for AVG, 0 (exact) otherwise"""
-        if self.name == "sum" and self.col_type == T.DOUBLE:
-            return self.abs_sum
-        if self.name == "avg" and self.cnt:
-            return self.abs_sum / self.cnt
-        return 0.0
+    def scanned_sum(self, fr) -> bool:
+        """a DOUBLE SUM / AVG the device reads from a segmented scan: every frame but a bounded ROWS frame (WM_DIRECT, which adds
+        row by row in frame order)"""
+        if not (self.name == "avg" or (self.name == "sum" and self.col_type == T.DOUBLE)):
+            return False
+        return fr is None or fr.start.is_unbounded or fr.end.is_unbounded or fr.frame_type == FrameType.RANGE
 
     def get_result(self):
         nm = self.name
@@ -325,32 +361,66 @@ def split_into_partitions(rows: List[dict], partition_exprs, types) -> List[Tupl
     return out
 
 
+class _Frames:
+    """one partition's argument values for the scanned DOUBLE sums: assert_matches bounds a result by its frame [s, t)"""
+
+    def __init__(self, fn, batch):
+        self.fn, self.batch, self._pre = fn, batch, None
+
+    def stats(self, s: int, t: int):
+        """(non-NULL count, exact sum of the finite values, Σ|x| of them, NaNs, +infs, -infs, -0.0s) over [s, t)"""
+        if self._pre is None:   # prefix sums, built on first use
+            acc = [0, Fraction(0), Fraction(0), 0, 0, 0, 0]
+            pre = [tuple(acc)]
+            for r in self.batch:
+                x = self.fn._x(r)
+                if x is not None:
+                    x = float(x)
+                    acc[0] += 1
+                    if math.isnan(x):
+                        acc[3] += 1
+                    elif math.isinf(x):
+                        acc[4 if x > 0 else 5] += 1
+                    else:
+                        acc[1] += Fraction(x)
+                        acc[2] += Fraction(abs(x))
+                        acc[6] += _dbits(x) == 1 << 63
+                pre.append(tuple(acc))
+            self._pre = pre
+        a, b = self._pre[s], self._pre[t]
+        return tuple(y - x for x, y in zip(a, b))
+
+
 def _window(rows, W, types):
     order_keys = W.order_exprs
     fns = [_Fn(e, types, order_keys) for e in W.window_fns]
     fr = W.frame
     non_frame = fr is None or (fr.start.is_unbounded and fr.end.is_unbounded)
+    scanned = [f.scanned_sum(fr) for f in fns]
     cmp = lambda a, b: all(_same(_eval(e, a, types), _eval(e, b, types)) for e in order_keys)   # noqa: E731
     for b, e in split_into_partitions(rows, W.partition_exprs, types):
         batch = rows[b:e]
+        frames = [_Frames(f, batch) if sc else None for f, sc in zip(fns, scanned)]
         for f in fns:
             f.partition_reset()
         if non_frame:
             for f in fns:
                 f.call(batch, 0, len(batch))
             for r in batch:
-                for f in fns:
+                for f, fm in zip(fns, frames):
                     r[f.slot] = f.get_result()
-                    r[("scale",) + f.slot] = f.error_scale()
+                    if fm is not None:
+                        r[("frame",) + f.slot] = (fm, 0, len(batch))
         else:
             for i, r in enumerate(batch):
-                for f in fns:
+                for f, fm in zip(fns, frames):
                     f.frame_reset()
                     s, t = _rows_start_end(fr, i, len(batch), batch, cmp)
                     if s < t:
                         f.call(batch, s, t)
                     r[f.slot] = f.get_result()
-                    r[("scale",) + f.slot] = f.error_scale()
+                    if fm is not None:
+                        r[("frame",) + f.slot] = (fm, s, t)
     return [(f.slot, f.col_type) for f in fns]
 
 
@@ -410,9 +480,45 @@ def execute(plan: Plan, cols: Sequence) -> Tuple[List[Tuple[int, int, int]], Lis
     return out_cols, rows
 
 
+def gamma(k: int) -> Fraction:
+    """γ_k = k·u / (1 - k·u): |computed - exact| <= γ_{m-1}·Σ|x| for a sum of m doubles added in any order"""
+    return Fraction(k) * Fraction(U) / (1 - Fraction(k) * Fraction(U))
+
+
+def check_scanned_sum(got: float, stats, avg: bool) -> Optional[str]:
+    """None when `got` can be a scan's SUM (or AVG) of a frame with these stats (_Frames.stats), else why not"""
+    m, exact, abs_sum, nans, pinf, ninf, negz = stats
+    if nans or (pinf and ninf):
+        return None if math.isnan(got) else "want NaN"
+    if pinf or ninf:
+        return None if got == (math.inf if pinf else -math.inf) else "want %sinf" % ("+" if pinf else "-")
+    if not math.isfinite(got):
+        return "want a finite value"
+    if got == 0:   # a sum is -0.0 in every order exactly when all its values are -0.0; AVG's sum starts at +0.0
+        want_neg = negz == m and not avg
+        if (_dbits(got) >> 63) != want_neg:
+            return "want %s0.0" % ("-" if want_neg else "+")
+    if avg:
+        err, bound = abs(Fraction(got) - exact / m), gamma(m) * abs_sum / m
+    else:
+        err, bound = abs(Fraction(got) - exact), gamma(m - 1) * abs_sum
+    return None if err <= bound else "error %g above the bound %g" % (float(err), float(bound))
+
+
+def _same_bits(a: float, b: float, ct: int) -> bool:
+    """FLOAT / DOUBLE equal by their bits (a zero's sign included); any NaN matches any NaN: the payload is the hardware's"""
+    if math.isnan(a) or math.isnan(b):
+        return math.isnan(a) and math.isnan(b)
+    if ct == T.FLOAT:
+        x, y = np.array([a, b], dtype=np.float32).view(np.uint32).tolist()
+        return x == y
+    return _dbits(float(a)) == _dbits(float(b))
+
+
 def assert_matches(got_cols, plan: Plan, cols: Sequence, rel: float = 1e-9) -> int:
-    """every row of the GPU result equals the oracle's, in the same order.  A DOUBLE SUM / AVG may differ by rel x Σ|x| over its
-    frame (divided by the count for AVG): the device adds in another order.  Every other value is exact."""
+    """every row of the GPU result equals the oracle's, in the same order, bit for bit.  A DOUBLE SUM / AVG read from a scan is
+    checked against the exact sum of its frame instead (check_scanned_sum).  `rel` is kept for callers of the tolerance this
+    comparison used to take; no result is compared within a relative tolerance any more."""
     out_cols, rows = execute(plan, cols)
     g = {(c.tuple_id, c.slot_id): c for c in got_cols}
     assert len(got_cols) == len(out_cols), (len(got_cols), len(out_cols))
@@ -424,9 +530,12 @@ def assert_matches(got_cols, plan: Plan, cols: Sequence, rel: float = 1e-9) -> i
             b = r[(tid, sid)]
             if a is None or b is None:
                 assert a is None and b is None, ((tid, sid), i, a, b)
+            elif ("frame", tid, sid) in r:
+                fm, s, t = r[("frame", tid, sid)]
+                why = check_scanned_sum(float(a), fm.stats(s, t), fm.fn.name == "avg")
+                assert why is None, ((tid, sid), i, a, b, why)
             elif ct in FLOATS:
-                tol = rel * r.get(("scale", tid, sid), 0.0)
-                assert (math.isnan(a) and math.isnan(b)) or abs(float(a) - float(b)) <= tol, ((tid, sid), i, a, b, tol)
+                assert _same_bits(float(a), float(b), ct), ((tid, sid), i, a, b, hex(_dbits(float(a))), hex(_dbits(float(b))))
             else:
                 assert int(a) == int(b), ((tid, sid), i, a, b)
     return len(rows)
