@@ -341,11 +341,16 @@ __device__ __forceinline__ void hll_merge_row(const AggPlan& ap, const GroupTabl
 }
 // K3 on the gathered rows: every rank folds the OTHER ranks' groups into its own table (its own groups are already there), so
 // nothing is re-initialised.  When some rank held more groups than `bound` nothing is merged anywhere (every rank reads the same
-// headers) and *max_count tells the host to repeat the exchange with a larger bound.
+// headers) and *max_count tells the host to repeat the exchange with a larger bound.  A merge of exported buffers (self < 0,
+// bkgpu_partial_merge) has no second exchange: a segment that holds more groups than its rows carry came from an export that failed
+// with ETOOBIG, and the merge fails with it (the overflow flag) instead of returning the other segments' groups alone.
 __global__ void k_partial_merge_rows(GroupTable gt, AggPlan ap, const uint64_t* src, size_t words_per_rank, uint32_t bound, int nranks, int self, uint32_t* max_count) {
     uint32_t mx = 0;
     for (int r = 0; r < nranks; r++) { const uint32_t c = (uint32_t)src[(size_t)r * words_per_rank]; mx = c > mx ? c : mx; }
-    if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) *max_count = mx;
+    if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {
+        *max_count = mx;
+        if (mx > bound && self < 0) atomicExch(gt.overflow, 1u);
+    }
     if (mx > bound) return;
     const int r = blockIdx.y;
     if (r == self) return;

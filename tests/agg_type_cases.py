@@ -19,6 +19,7 @@ from fractions import Fraction
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
+import pytest
 
 from baikaldb_b200 import plan as P
 from baikaldb_b200.column import Column, make_column
@@ -34,6 +35,9 @@ UNSIGNED = (T.UINT8, T.UINT16, T.UINT32, T.UINT64)
 LEAN_KEYS = (T.INT32, T.UINT32, T.INT64, T.UINT64, T.DATETIME)
 # value types the lean kernel takes: 8-byte columns
 LEAN_VALUES = (T.INT64, T.UINT64, T.DOUBLE, T.DATETIME)
+# the aggregate kernels (bkgpu_stats.main_kernel_name) and the options that pin each of them
+INTERP, DIRECT, LEAN, FX, SCALAR = "k_agg_interp", "k_agg_group_direct", "k_agg_group_lean", "k_agg_group_lean_fx", "k_agg_scalar_direct"
+OPTIONS = {INTERP: {"force_generic": 1}, DIRECT: {"no_lean": 1}, LEAN: {"lean_fx": 0}, FX: {"lean_fx": 1}, SCALAR: {}}
 RANGES = {**RANGE, T.TIME: RANGE[T.INT32], T.TIMESTAMP: RANGE[T.UINT32], T.DATE: RANGE[T.UINT32], T.DATETIME: RANGE[T.UINT64]}
 
 F64_MAX, F32_MAX = 1.7976931348623157e308, float(np.finfo(np.float32).max)
@@ -229,6 +233,30 @@ def value_table(rng, vt: int, n: int, groups=48, null_share=0.1, grouped=True) -
     return Table(T.INT32, vt, keys, None, rng.integers(0, 100, n).astype(np.int32), v, np.array(valid), w, grouped)
 
 
+# SUM over signed zeros: the value of the j-th row of a group, and whether it is present
+SIGNED_ZERO = {"minus_zero": lambda j: (-0.0, True), "minus_zero_nulls": lambda j: (-0.0, j % 3 != 1), "mixed": lambda j: (-0.0 if j % 5 else 0.0, True),
+               "cancel": lambda j: ([1.5, -1.5][j % 2] if j < 4 else -0.0, True)}
+
+
+def zero_table(rng, vt, what, n, grouped=True, nulls=True) -> Table:
+    """every group holds the values of one SIGNED_ZERO class (with `nulls`, -0.0 with NULLs and all-NULL groups too)"""
+    keys = [int(x) for x in rng.integers(0, 40, n)] if grouped else [0] * n
+    seen, v, ok = {}, [], []
+    for k in keys:
+        j = seen.get(k, 0)
+        seen[k] = j + 1
+        x, valid = SIGNED_ZERO[what](j)
+        v.append(x)
+        ok.append(valid if nulls else True)
+    return Table(T.INT32, vt, keys, None, rng.integers(0, 100, n).astype(np.int32), v, np.array(ok) if nulls else None, v, grouped)
+
+
+# FX keeps a slot's double sum as integer limbs, which have no -0.0: a SUM whose every value is -0.0 comes out +0.0 there.  Telling the
+# two apart needs a per-slot count of -0.0 rows; the version of that which was tried slowed C2's FX loop (1.00-1.02 ms per step against
+# 0.86 ms on an H100 SXM at 700 W), so the gap stays open and the cases that meet it record it.
+FX_OPEN = pytest.mark.xfail(strict=True, reason="FX's fixed-point limbs turn a SUM of only -0.0 into +0.0")
+
+
 # ---------------------------------------------------------------- plans
 FNS = ("count_star", "count", "sum", "min", "max", "avg")
 AVG_FNS = ("count_star", "count", "avg")
@@ -240,9 +268,9 @@ def main_fns(vt: int) -> Tuple[str, ...]:
     return FNS if vt in FLOATS else FNS[:5]
 
 
-def agg_plan(t: Table, fns: Sequence[str] = FNS, predicate=None, grouped=None, extra_slots=(), merge=False) -> P.Plan:
-    """[WHERE predicate (default: 0_2 < 50)] [GROUP BY 0_1] with `fns` over v (MIN / MAX over w for FLOAT / DOUBLE).  `merge`: the
-    MERGE_AGG of the same aggregates over partial rows (the key and the aggregate tuple's intermediate slots)"""
+def agg_plan(t: Table, fns: Sequence[str] = FNS, predicate=None, grouped=None, extra_slots=(), merge=False, extra_keys=()) -> P.Plan:
+    """[WHERE predicate (default: 0_2 < 50)] [GROUP BY 0_1 [, extra_keys]] with `fns` over v (MIN / MAX over w for FLOAT / DOUBLE).
+    `merge`: the MERGE_AGG of the same aggregates over partial rows (the key and the aggregate tuple's intermediate slots)"""
     grouped = t.grouped if grouped is None else grouped
     vt = t.vt
     v, w = P.slot_ref(0, 3, vt), P.slot_ref(0, 4 if vt in FLOATS else 3, vt)
@@ -259,7 +287,7 @@ def agg_plan(t: Table, fns: Sequence[str] = FNS, predicate=None, grouped=None, e
     slots = [(2, T.INT32), (3, vt)] + ([(1, t.kt)] if grouped else []) + ([(4, vt)] if vt in FLOATS else []) + list(extra_slots)
     pred = P.lt(P.slot_ref(0, 2, T.INT32), P.int_lit(50)) if predicate is None else predicate
     child = P.where(P.scan(0), pred) if not merge else P.scan(0)
-    a = P.agg(child, AT, [P.slot_ref(0, 1, t.kt)] if grouped else [], aggs, merge=merge)
+    a = P.agg(child, AT, [P.slot_ref(0, 1, t.kt)] + list(extra_keys) if grouped else [], aggs, merge=merge)
     return P.Plan(a if grouped else P.packet(a), {0: slots, AT: P.agg_tuple_slots(aggs, types)})
 
 

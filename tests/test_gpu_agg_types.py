@@ -16,13 +16,11 @@ from baikaldb_b200.exec_node import execute
 from baikaldb_b200.column import make_column
 from baikaldb_b200.plan import PlanNodeType, PrimitiveType as T
 from oracle import oracle
-from tests.agg_type_cases import (AT, AVG_FNS, FLOATS, FNS, main_fns, LEAN_KEYS, LEAN_VALUES, TYPES, UNSIGNED, Table, agg_plan, assert_matches, column_array,
-                                  date_img, datetime_img, edges, f32, key_image, key_table, out_names, reference, small_values, tname,
-                                  value_table)
+from tests.agg_type_cases import (AT, AVG_FNS, DIRECT, FLOATS, FNS, FX, FX_OPEN, INTERP, LEAN, LEAN_KEYS, LEAN_VALUES, OPTIONS, SCALAR, SIGNED_ZERO,
+                                  TYPES, UNSIGNED, Table, agg_plan, assert_matches, column_array, date_img, datetime_img, edges, f32, key_image,
+                                  key_table, main_fns, out_names, reference, small_values, tname, value_table, zero_table)
 
 N = 20_003
-INTERP, DIRECT, LEAN, FX, SCALAR = "k_agg_interp", "k_agg_group_direct", "k_agg_group_lean", "k_agg_group_lean_fx", "k_agg_scalar_direct"
-OPTIONS = {INTERP: {"force_generic": 1}, DIRECT: {"no_lean": 1}, LEAN: {"lean_fx": 0}, FX: {"lean_fx": 1}, SCALAR: {}}
 SUMS = ("count_star", "sum", "avg")   # the lean kernel's CAS / FX / NULLS shape: every value column feeds one SUM lane
 gpu = pytest.mark.gpu
 
@@ -85,29 +83,6 @@ def test_argument_types(vt, kernel):
     run(agg_plan(t, AVG_FNS), t, DIRECT if kernel == LEAN and vt != T.DOUBLE else kernel, AVG_FNS, OPTIONS[kernel])
 
 
-SIGNED_ZERO = {"minus_zero": lambda j: (-0.0, True), "minus_zero_nulls": lambda j: (-0.0, j % 3 != 1), "mixed": lambda j: (-0.0 if j % 5 else 0.0, True),
-               "cancel": lambda j: ([1.5, -1.5][j % 2] if j < 4 else -0.0, True)}
-
-
-def zero_table(rng, vt, what, grouped=True, nulls=True):
-    """every group holds the values of one SIGNED_ZERO class (with `nulls`, -0.0 with NULLs and all-NULL groups too)"""
-    keys = [int(x) for x in rng.integers(0, 40, N)] if grouped else [0] * N
-    seen, v, ok = {}, [], []
-    for k in keys:
-        j = seen.get(k, 0)
-        seen[k] = j + 1
-        x, valid = SIGNED_ZERO[what](j)
-        v.append(x)
-        ok.append(valid if nulls else True)
-    return Table(T.INT32, vt, keys, None, rng.integers(0, 100, N).astype(np.int32), v, np.array(ok) if nulls else None, v, grouped)
-
-
-# FX keeps a slot's double sum as integer limbs, which have no -0.0: a SUM whose every value is -0.0 comes out +0.0 there.  Telling the
-# two apart needs a per-slot count of -0.0 rows; the version of that which was tried slowed C2's FX loop (1.00-1.02 ms per step against
-# 0.86 ms on an H100 SXM at 700 W), so the gap stays open and this case records it.
-FX_OPEN = pytest.mark.xfail(strict=True, reason="FX's fixed-point limbs turn a SUM of only -0.0 into +0.0")
-
-
 @gpu
 @pytest.mark.parametrize("kernel", [INTERP, DIRECT, LEAN, pytest.param(FX, id=FX), SCALAR, "lean_nulls", "lean_mm"])
 @pytest.mark.parametrize("what", list(SIGNED_ZERO))
@@ -121,7 +96,7 @@ def test_sum_of_signed_zeros(what, kernel, request):
     if kernel == FX and what == "minus_zero":
         request.applymarker(FX_OPEN)
     rng = np.random.default_rng(4000 + list(SIGNED_ZERO).index(what))
-    t = zero_table(rng, vt, what, grouped=kernel != SCALAR, nulls=nulls)
+    t = zero_table(rng, vt, what, N, grouped=kernel != SCALAR, nulls=nulls)
     fns = FNS if kernel in (INTERP, DIRECT, SCALAR, "lean_mm") else SUMS
     name = {"lean_nulls": LEAN, "lean_mm": LEAN}.get(kernel, kernel)
     run(agg_plan(t, fns), t, name, fns, OPTIONS[name])

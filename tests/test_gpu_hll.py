@@ -10,9 +10,10 @@ import torch
 from baikaldb_b200 import _lib, datagen, plan as P
 from baikaldb_b200._lib import BkgpuError
 from baikaldb_b200.column import make_column
-from baikaldb_b200.exec_node import ColumnSource, DeviceColumn, GpuExecNode, RowBatch, RuntimeState, execute
+from baikaldb_b200.exec_node import DeviceColumn, execute
 from baikaldb_b200.plan import JoinType, PrimitiveType as T
 from tests import hll_cases as C, hll_oracle as H
+from tests.util import fetch, open_node
 
 pytestmark = pytest.mark.gpu
 SK = f"{C.AGG_TUPLE}_1"
@@ -190,24 +191,6 @@ def test_join_star_and_apply():
         assert sorted(by) == sorted(set(tk[hit].tolist())) and all(by[k] == want[k] for k in by)
 
 
-def _open(plan, cols, options=None):
-    st = RuntimeState(device=0, options=dict(options or {}))
-    node = GpuExecNode()
-    node.init(plan)
-    node.add_child(ColumnSource([cols]))
-    assert node.open(st) == 0, st.error_msg
-    return node, st
-
-
-def _fetch(node, st):
-    out, rb, eos = [], RowBatch(), False
-    while not eos:
-        rc, eos = node.get_next(st, rb)
-        assert rc == 0, st.error_msg
-        out = out or list(rb.columns)
-    return out
-
-
 @pytest.mark.parametrize("ranks,grouped", [(2, True), (3, True), (3, False)])
 def test_regions_partial_export_and_merge(ranks, grouped):
     """several regions on one GPU: each exports its partial state (registers with the group rows), one plan folds them all"""
@@ -220,7 +203,7 @@ def test_regions_partial_export_and_merge(ranks, grouped):
     valid[keys == 7] = False
     part = np.array_split(np.arange(n), ranks)
     opts = {"partial_capacity": 512}
-    nodes = [_open(C.scan_plan(T.INT64, grouped=grouped), [make_column(0, 1, T.INT32, keys[ix]), make_column(0, 2, T.INT64, vals[ix], valid[ix]),
+    nodes = [open_node(C.scan_plan(T.INT64, grouped=grouped), [make_column(0, 1, T.INT32, keys[ix]), make_column(0, 2, T.INT64, vals[ix], valid[ix]),
                                                             make_column(0, 3, T.DOUBLE, np.zeros(len(ix)))], opts) for ix in part]
     try:
         nbytes = ctypes.c_size_t(0)
@@ -231,7 +214,7 @@ def test_regions_partial_export_and_merge(ranks, grouped):
             _lib.check(L.bkgpu_partial_export(node.handle(), ctypes.c_void_p(bufs.data_ptr() + r * nbytes.value), nbytes.value), node.handle())
         node, st = nodes[0]
         _lib.check(L.bkgpu_partial_merge(node.handle(), ctypes.c_void_p(bufs.data_ptr()), nbytes.value, ranks), node.handle())
-        got = _fetch(node, st)
+        got = fetch(node, st)
     finally:
         for node, st in nodes:
             node.close(st)
@@ -271,7 +254,7 @@ def test_reset_reuse():
         keys = rng.integers(0, g, n).astype(np.int32)
         vals = rng.normal(size=n)
         runs.append((keys, vals, [make_column(0, 1, T.INT32, keys), make_column(0, 2, T.DOUBLE, vals), make_column(0, 3, T.DOUBLE, vals)]))
-    node, st = _open(C.scan_plan(T.DOUBLE), runs[0][2])
+    node, st = open_node(C.scan_plan(T.DOUBLE), runs[0][2])
     try:
         for i, (keys, vals, cols) in enumerate(runs):
             if i:
@@ -279,7 +262,7 @@ def test_reset_reuse():
                 node.push(cols)
                 node.finish()
             want = H.sketches(vals, T.DOUBLE, keys, g)
-            by = _by_key(_fetch(node, st))
+            by = _by_key(fetch(node, st))
             assert len(by) == g and all(by[k] == want[k] for k in range(g))
     finally:
         node.close(st)
@@ -412,7 +395,7 @@ def test_two_sketches_per_group_and_a_limit_above():
     for i, k in enumerate(c["0_1"]):
         assert c[SK][i] == wa[k] and c[f"{C.AGG_TUPLE}_3"][i] == wb[k] and c[f"{C.AGG_TUPLE}_2"][i] == int((keys == k).sum())
     # the two sketches travel through a partial export / merge in aggregate order
-    nodes = [_open(pl, [make_column(x.tuple_id, x.slot_id, x.prim_type, x.values[ix], None if x.valid is None else x.valid[ix]) for x in cols],
+    nodes = [open_node(pl, [make_column(x.tuple_id, x.slot_id, x.prim_type, x.values[ix], None if x.valid is None else x.valid[ix]) for x in cols],
                    {"partial_capacity": 512}) for ix in np.array_split(np.arange(n), 2)]
     try:
         L = _lib.lib()
@@ -423,7 +406,7 @@ def test_two_sketches_per_group_and_a_limit_above():
         for r, (node, _) in enumerate(nodes):
             _lib.check(L.bkgpu_partial_export(node.handle(), ctypes.c_void_p(buf.data_ptr() + r * nbytes.value), nbytes.value), node.handle())
         _lib.check(L.bkgpu_partial_merge(nodes[0][0].handle(), ctypes.c_void_p(buf.data_ptr()), nbytes.value, 2), nodes[0][0].handle())
-        c = {x.name: x.to_list() for x in _fetch(*nodes[0])}
+        c = {x.name: x.to_list() for x in fetch(*nodes[0])}
     finally:
         for node, st in nodes:
             node.close(st)

@@ -1,11 +1,14 @@
-"""Helpers shared by the parity tests: run a fragment on the GPU path and on the oracle and compare."""
+"""Helpers shared by the parity tests: run a fragment on the GPU path and on the oracle and compare; open plan handles and fold the
+partial states of several of them into one."""
+import ctypes
 import math
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
+from baikaldb_b200 import _lib
 from baikaldb_b200.column import Column, rows_as_set
-from baikaldb_b200.exec_node import execute
+from baikaldb_b200.exec_node import ColumnSource, DeviceColumn, GpuExecNode, RowBatch, RuntimeState, execute
 from oracle import oracle
 
 # names bkgpu_stats.main_kernel_name reports for the lean GROUP BY path (_fx: double sums as fixed-point limbs)
@@ -63,3 +66,63 @@ def run_both(plan, cols, keys, options: Optional[Dict[str, int]] = None, rel=REL
     if check_scanned:  # (a LIMIT lets the pull-based row engine stop scanning early; a pushed batch is always scanned whole)
         assert stats.rows_scanned == want.rows_scanned, (stats.rows_scanned, want.rows_scanned)
     return got, stats, want
+
+
+def open_node(plan, batches, options=None):
+    """one GpuExecNode on cuda:0, opened over `batches` (one batch or a list of batches): its rows are pushed and bkgpu_finish has run"""
+    if batches and isinstance(batches[0], (Column, DeviceColumn)):
+        batches = [batches]
+    st = RuntimeState(device=0, options=dict(options or {}))
+    node = GpuExecNode()
+    node.init(plan)
+    node.add_child(ColumnSource(batches))
+    assert node.open(st) == 0, st.error_msg
+    return node, st
+
+
+def fetch(node, st) -> List[Column]:
+    out, rb, eos = [], RowBatch(), False
+    while not eos:
+        rc, eos = node.get_next(st, rb)
+        assert rc == 0, st.error_msg
+        out = out or list(rb.columns)
+    return out
+
+
+def partial_capacity(node) -> int:
+    nbytes = ctypes.c_size_t(0)
+    _lib.check(_lib.lib().bkgpu_partial_capacity(node.handle(), ctypes.byref(nbytes)), node.handle())
+    return nbytes.value
+
+
+def export_and_merge(nodes, merger=0, headers=None) -> List[Column]:
+    """every node's partial state exported into slice r of one device buffer, all of them folded by node `merger`, its result fetched.
+    `headers`: a list that receives the first word of each slice (the groups an aggregate's export holds, the rows of a top-k's)"""
+    import torch
+    L = _lib.lib()
+    nbytes = partial_capacity(nodes[merger][0])
+    buf = torch.zeros(max(len(nodes) * nbytes, 8), dtype=torch.uint8, device="cuda")
+    torch.cuda.synchronize()
+    for r, (node, _) in enumerate(nodes):
+        _lib.check(L.bkgpu_partial_export(node.handle(), ctypes.c_void_p(buf.data_ptr() + r * nbytes), nbytes), node.handle())
+    if headers is not None:
+        headers.extend(int(x) for x in buf.view(torch.int64)[0:len(nodes) * nbytes // 8:nbytes // 8].tolist())
+    node, st = nodes[merger]
+    _lib.check(L.bkgpu_partial_merge(node.handle(), ctypes.c_void_p(buf.data_ptr()), nbytes, len(nodes)), node.handle())
+    return fetch(node, st)
+
+
+def merge_regions(plan, regions, options_per_region, merger=0, stats=None, headers=None) -> List[Column]:
+    """`plan` over each region (its batches) on its own handle on cuda:0, with that region's options; the regions' partial states
+    exported and merged by region `merger`.  `stats`: a list that receives each region's bkgpu_stats after its finish; `headers`: see
+    export_and_merge"""
+    nodes = []
+    try:
+        for batches, opts in zip(regions, options_per_region):
+            nodes.append(open_node(plan, batches, opts))
+            if stats is not None:
+                stats.append(nodes[-1][0].stats())
+        return export_and_merge(nodes, merger, headers)
+    finally:
+        for node, st in nodes:
+            node.close(st)
