@@ -294,8 +294,8 @@ extern "C" int bkgpu_open(bkgpu_plan* p) {
     if (rc) return rc;
     if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) rc = alloc_group_table(p);
     if (!rc && (p->c.kind == PK_SORT || p->c.kind == PK_FILTER || p->c.kind == PK_WINDOW))   // (a window retains its rows like a full sort)
-        rc = sort_check(p, sort_open(p->c, p->device, p->stream, p->region_base, &p->sort, p->last_error));
-    if (!rc && p->c.post) rc = sort_check(p, sort_open(*p->c.post, p->device, p->stream, 0, &p->post_sort, p->last_error));
+        rc = sort_open(p, p->c, p->region_base, &p->sort);
+    if (!rc && p->c.post) rc = sort_open(p, *p->c.post, 0, &p->post_sort);
     if (rc) return rc;
     p->state = S_OPEN;
     return BKGPU_OK;
@@ -619,14 +619,7 @@ int feed(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* col
 }
 
 static int agg_batch(bkgpu_plan* p, const DevCol* cols, int64_t nrows, int64_t, bool vec_ok) { return launch_agg_batch(p, p->c, cols, nrows, vec_ok); }
-static int sort_batch(bkgpu_plan* p, const DevCol* cols, int64_t nrows, int64_t, bool) {
-    return sort_check(p, sort_push(p->sort, cols, nrows, p->stream, &p->stats, p->last_error));
-}
-
-int sort_check(bkgpu_plan* p, int rc) {
-    if (rc) g_thread_error = p->last_error;
-    return rc;
-}
+static int sort_batch(bkgpu_plan* p, const DevCol* cols, int64_t nrows, int64_t, bool) { return sort_push(p->sort, cols, nrows, &p->stats); }
 
 void set_result(bkgpu_plan* p, std::vector<SortOutCol>& cols, int64_t rows, const OutCol* desc) {
     p->result.clear();
@@ -740,16 +733,6 @@ static uint32_t eff_pcap(const bkgpu_plan* p) {
     return (uint32_t)std::min<int64_t>(p->partial_cap, table);
 }
 
-// grow-only device buffers of the multi-GPU exchange
-static int ensure_words(bkgpu_plan* p, uint64_t** buf, size_t* have, size_t want) {
-    if (*have >= want) return BKGPU_OK;
-    dev_free(p, *buf); *buf = nullptr; *have = 0;
-    int rc = dev_alloc(p, (void**)buf, want * 8);
-    if (rc) return rc;
-    *have = want;
-    return BKGPU_OK;
-}
-
 // the collective step of bkgpu_finish: regions -> one set per GPU, the per-GPU partial tables meet once and are folded by K3.
 // Default: compact rows, one ncclAllGather of 1 + bound x (key + lane words) per rank — `bound` = the largest group count any rank
 // held in earlier runs of this plan (2048 on the first run); the merge reports the true maximum and the exchange is repeated once
@@ -770,8 +753,8 @@ static int agg_collective(bkgpu_plan* p, bool* rows_mode) {
         bound = std::min<uint32_t>(bound, pcap);
         const size_t rw = (size_t)(ap.n_keyw + ap.n_lanes + ap.n_hll * HLL_ROW_WORDS);
         const size_t words = 1 + rw * bound;
-        if ((rc = ensure_words(p, &p->d_partial, &p->d_partial_words, words))) return rc;
-        if ((rc = ensure_words(p, &p->d_gather, &p->d_gather_words, words * (size_t)p->nranks))) return rc;
+        if ((rc = ensure_buf(p, (void**)&p->d_partial, &p->d_partial_cap, words * 8))) return rc;
+        if ((rc = ensure_buf(p, (void**)&p->d_gather, &p->d_gather_cap, words * 8 * (size_t)p->nranks))) return rc;
         CK(p, launch_partial_export_rows(gt, ap, p->d_partial, bound, p->stream));
         if (nccl_all_gather(p->nccl_comm, p->d_partial, p->d_gather, words, p->stream) != 0) return p->fail(BKGPU_ENCCL, "ncclAllGather: %s", nccl_last_error());
         CK(p, launch_partial_merge_rows(gt, ap, p->d_gather, words, bound, p->nranks, p->peer_rank, p->d_cursor + 1, p->stream));
@@ -781,8 +764,8 @@ static int agg_collective(bkgpu_plan* p, bool* rows_mode) {
         return BKGPU_OK;
     }
     const size_t words = 1 + (size_t)(ap.n_keyw + ap.n_lanes) * pcap;
-    if ((rc = ensure_words(p, &p->d_partial, &p->d_partial_words, words * (repart ? (size_t)p->nranks : 1)))) return rc;
-    if ((rc = ensure_words(p, &p->d_gather, &p->d_gather_words, words * (size_t)p->nranks))) return rc;
+    if ((rc = ensure_buf(p, (void**)&p->d_partial, &p->d_partial_cap, words * 8 * (repart ? (size_t)p->nranks : 1)))) return rc;
+    if ((rc = ensure_buf(p, (void**)&p->d_gather, &p->d_gather_cap, words * 8 * (size_t)p->nranks))) return rc;
     if (p->peer_merge && !repart && (rc = peer_setup(p, words))) return rc;
     if (p->peer_merge && !repart) {
         const uint64_t seq = ++p->peer_seq;
@@ -842,11 +825,11 @@ static int agg_post(bkgpu_plan* p, uint32_t n_out, uint32_t out_cap) {
         dc[c].values = p->post_vals[c]; dc[c].validity = p->post_bitmap[c]; dc[c].stype = prim_storage(pc.cols[c].prim); dc[c].prim = pc.cols[c].prim;
     }
     p->stats.kernel_launches += 1 + (int64_t)nc;
-    if ((rc = sort_check(p, sort_reset(p->post_sort, p->stream, p->last_error)))) return rc;
+    sort_reset(p->post_sort);
     bkgpu_stats scratch{};   // (the post fragment's kernels are not the request's "main kernel")
-    if (n_out && (rc = sort_check(p, sort_push(p->post_sort, dc.data(), n_out, p->stream, &scratch, p->last_error)))) return rc;
+    if (n_out && (rc = sort_push(p->post_sort, dc.data(), n_out, &scratch))) return rc;
     std::vector<SortOutCol> cols; int64_t rows = 0;
-    if ((rc = sort_check(p, sort_finish(p->post_sort, nullptr, 1, p->stream, &scratch, cols, &rows, p->last_error)))) return rc;
+    if ((rc = sort_finish(p->post_sort, nullptr, 1, &scratch, cols, &rows))) return rc;
     p->stats.kernel_launches += scratch.kernel_launches;
     set_result(p, cols, rows, p->c.out_cols.data());
     return BKGPU_OK;
@@ -1107,19 +1090,19 @@ static int bkgpu_finish_impl(bkgpu_plan* p) {
         } break;
         case PK_JOIN: {   // the outer join's preserved rows, then the sink fragment's result
             std::vector<SortOutCol> cols; int64_t rows = 0;
-            if ((rc = join_tail(p)) || (rc = sort_check(p, sort_finish(p->post_sort, nullptr, 1, p->stream, &p->stats, cols, &rows, p->last_error)))) break;
+            if ((rc = join_tail(p)) || (rc = sort_finish(p->post_sort, nullptr, 1, &p->stats, cols, &rows))) break;
             set_result(p, cols, rows, p->c.out_cols.data());
             p->stats.rows_filtered = 0;
         } break;
         case PK_SORT: case PK_FILTER: {
             std::vector<SortOutCol> cols; int64_t rows = 0;
-            if ((rc = sort_check(p, sort_finish(p->sort, p->nccl_comm, p->nranks, p->stream, &p->stats, cols, &rows, p->last_error)))) break;
+            if ((rc = sort_finish(p->sort, p->nccl_comm, p->nranks, &p->stats, cols, &rows))) break;
             set_result(p, cols, rows, nullptr);
         } break;
         case PK_WINDOW: {   // the retained rows through the window stages (window.cu), then the query's ORDER BY when there is one
             if (p->nccl_comm && p->nranks > 1) { rc = p->fail(BKGPU_EUNSUPPORTED, "a window fragment runs on one GPU: multi-GPU merge is implemented for ORDER BY ... LIMIT (top-k) and aggregates"); break; }
             std::vector<SortOutCol> cols; int64_t rows = 0;
-            if ((rc = sort_check(p, window_finish(p->c, p->sort, p->post_sort, p->stream, &p->stats, cols, &rows, p->last_error)))) break;
+            if ((rc = window_finish(p, cols, &rows))) break;
             set_result(p, cols, rows, nullptr);
         } break;
         default: rc = p->fail(BKGPU_EUNSUPPORTED, "plan kind %d cannot finish", p->c.kind);
@@ -1199,8 +1182,8 @@ static int bkgpu_reset_impl(bkgpu_plan* p) {
         p->stats.kernel_launches++;
     }
     join_reset(p);
-    if (p->sort) { int rc = sort_check(p, sort_reset(p->sort, p->stream, p->last_error)); if (rc) return rc; }
-    if (p->c.kind == PK_JOIN && p->post_sort) { int rc = sort_check(p, sort_reset(p->post_sort, p->stream, p->last_error)); if (rc) return rc; }
+    if (p->sort) sort_reset(p->sort);
+    if (p->c.kind == PK_JOIN && p->post_sort) sort_reset(p->post_sort);
     p->result.clear(); p->result_rows = 0; p->result_pos = 0;
     bkgpu_stats z{}; z.kernel_launches = p->stats.kernel_launches; p->stats = z;
     p->state = S_OPEN;
@@ -1334,7 +1317,7 @@ extern "C" int bkgpu_partial_export(bkgpu_plan* p, void* dev_dst, size_t bytes) 
     if (rc) return rc;
     if (bytes < need) return p->fail(BKGPU_EINVAL, "partial buffer too small: %zu < %zu", bytes, need);
     CK(p, cudaSetDevice(p->device));
-    if (p->c.kind == PK_SORT) return sort_check(p, sort_partial_export(p->sort, dev_dst, p->stream, p->last_error));
+    if (p->c.kind == PK_SORT) return sort_partial_export(p->sort, dev_dst);
     // compact rows (the layout the in-library all-gather ships): [u64 groups][groups x (key words + lane words)]
     CK(p, launch_partial_export_rows(p->gt, p->c.ap, (uint64_t*)dev_dst, eff_pcap(p), p->stream));
     p->stats.kernel_launches += 1;
@@ -1358,7 +1341,7 @@ extern "C" int bkgpu_partial_merge(bkgpu_plan* p, const void* dev_src, size_t by
     CK(p, cudaSetDevice(p->device));
     if (p->c.kind == PK_SORT) {
         std::vector<SortOutCol> cols; int64_t rows = 0;
-        if ((rc = sort_check(p, sort_partial_merge(p->sort, dev_src, nranks, p->stream, cols, &rows, p->last_error)))) return rc;
+        if ((rc = sort_partial_merge(p->sort, dev_src, nranks, cols, &rows))) return rc;
         set_result(p, cols, rows, nullptr);
         p->stats.rows_returned = rows; p->state = S_FINISHED;
         return BKGPU_OK;

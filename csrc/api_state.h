@@ -111,7 +111,7 @@ struct bkgpu_plan {
     uint32_t* d_cursor = nullptr;
     uint64_t* d_partial = nullptr;  // export buffer (this rank)
     uint64_t* d_gather = nullptr;   // nranks export buffers
-    size_t d_partial_words = 0, d_gather_words = 0;
+    size_t d_partial_cap = 0, d_gather_cap = 0;
     HostClock hclk; bool trace = getenv("BKGPU_TRACE") != nullptr;
     std::vector<uint8_t*> bounce[2]; size_t bounce_rows = 0; cudaEvent_t bounce_done[2] = {nullptr, nullptr}; bool bounce_busy[2] = {false, false};
     int scalar_tma = 1;           // COUNT(*) WHERE int32 <cmp> c runs the TMA-staged kernel (scalar_tma.cu); 0 = the LDG kernel
@@ -172,6 +172,23 @@ struct bkgpu_plan {
 int dev_alloc(bkgpu_plan* p, void** out, size_t bytes);
 void dev_free(bkgpu_plan* p, void* ptr);
 int ensure_buf(bkgpu_plan* p, void** ptr, size_t* cap, size_t bytes);
+// device buffers of one call: returned to the plan's allocator when the scope ends, on every way out of the call
+struct DevScope {
+    bkgpu_plan* p;
+    std::vector<void*> bufs;
+    explicit DevScope(bkgpu_plan* plan) : p(plan) {}
+    DevScope(const DevScope&) = delete;
+    DevScope& operator=(const DevScope&) = delete;
+    ~DevScope() { for (void* b : bufs) dev_free(p, b); }
+    template <class T> int alloc(T** out, size_t bytes) {
+        const int rc = dev_alloc(p, (void**)out, bytes);
+        if (rc == BKGPU_OK) bufs.push_back(*out);
+        return rc;
+    }
+    void release(void* b) {   // before the scope ends
+        for (auto it = bufs.begin(); it != bufs.end(); ++it) if (*it == b) { bufs.erase(it); dev_free(p, b); return; }
+    }
+};
 // the plan's columns `want` resolved against one pushed batch
 int bind_columns(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* cols, int ncols, int64_t nrows, std::vector<const bkgpu_column*>& bound);
 // a batch as device columns (host columns chunk by chunk through the staging buffers), handed to `fn`
@@ -181,8 +198,6 @@ int feed(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* col
 int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp = nullptr);
 // the post fragment's input columns, reallocated with room for `cap` rows when they hold fewer than `need`
 int ensure_post(bkgpu_plan* p, size_t need, size_t cap);
-// the result of a sort_* call: a failure's message becomes the thread's error too
-int sort_check(bkgpu_plan* p, int rc);
 // the plan's result from a sort fragment's columns; `desc`: their output column descriptions (nullptr = the sort's own)
 void set_result(bkgpu_plan* p, std::vector<SortOutCol>& cols, int64_t rows, const OutCol* desc);
 

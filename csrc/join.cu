@@ -413,7 +413,7 @@ static int join_rows_emit(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t
     }
     p->stats.kernel_launches += 2 * (int64_t)nc;
     p->rows_passed_host += found;
-    if ((rc = sort_check(p, sort_push(p->post_sort, dc.data(), (int64_t)found, p->stream, &p->stats, p->last_error)))) return rc;
+    if ((rc = sort_push(p->post_sort, dc.data(), (int64_t)found, &p->stats))) return rc;
     CK(p, cudaStreamSynchronize(p->stream));   // the gather buffers are reused by the next batch
     return BKGPU_OK;
 }

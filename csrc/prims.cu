@@ -1,12 +1,11 @@
 // prims.cu — device primitives shared by ORDER BY and the window stage (sort.cu, window.cu) and rb_build_agg (rb.cu), for sm_90a.
 #include "prims.cuh"
 #include <algorithm>
+#include "api_state.h"
 
 namespace bk {
 
 int grid_for(int64_t n, int sm, int per_sm) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sm * per_sm)); }
-
-int cuda_fail(std::string& err, cudaError_t e, const char* what) { err = std::string(what) + ": " + cudaGetErrorString(e); return e == cudaErrorMemoryAllocation ? BKGPU_ENOMEM : BKGPU_ENODEV; }
 
 __global__ void k_iota(uint32_t* ids, int64_t n) { for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) ids[i] = (uint32_t)i; }
 
@@ -231,29 +230,32 @@ cudaError_t scan_excl(T* d, int64_t n, T* sums, int sm, cudaStream_t s) {
 template cudaError_t scan_excl<uint32_t>(uint32_t*, int64_t, uint32_t*, int, cudaStream_t);
 template cudaError_t scan_excl<uint64_t>(uint64_t*, int64_t, uint64_t*, int, cudaStream_t);
 
-int radix_sort(uint64_t* const keys[2], uint32_t* const ids[2], int cur, int64_t n, int sm, const RadixScratch& scratch, cudaStream_t st,
-               bkgpu_stats* stats, int64_t* bytes, std::string& err) {
-    if (n > RADIX_MAX_KEYS) { err = "the radix sort takes at most 2^30 - 1 keys"; return BKGPU_EUNSUPPORTED; }
+int radix_sort(bkgpu_plan* p, uint64_t* const keys[2], uint32_t* const ids[2], int cur, int64_t n, RadixScratch& scratch, bkgpu_stats* stats,
+               int64_t* bytes) {
+    if (n > RADIX_MAX_KEYS) return p->fail(BKGPU_EUNSUPPORTED, "the radix sort takes at most 2^30 - 1 keys");
     if (n < 2) return cur;
+    const cudaStream_t st = p->stream;
+    const int sm = p->sm_count;
     const uint32_t un = (uint32_t)n, ntiles = (un + RS_TILE - 1) / RS_TILE;
-    uint32_t *hist, *status;
     int rc;
-    if ((rc = scratch(0, RS_HIST_BYTES, (void**)&hist))) return rc;
+    if ((rc = ensure_buf(p, &scratch.hist, &scratch.hist_cap, RS_HIST_BYTES))) return rc;
+    uint32_t* hist = (uint32_t*)scratch.hist;
     uint32_t* bases = hist + 8 * 256; uint32_t* active = bases + 8 * 256; uint32_t* tickets = active + 8;
-    SCK(cudaMemsetAsync(hist, 0, RS_HIST_BYTES, st));
+    CK(p, cudaMemsetAsync(hist, 0, RS_HIST_BYTES, st));
     k_rs_hist<<<std::min(sm * 4, (int)((un + 1023) / 1024)), 256, 0, st>>>(keys[cur], un, hist);
     k_rs_bases<<<8, 256, 0, st>>>(hist, bases, active);
     uint32_t h_active[8];
-    SCK(cudaMemcpyAsync(h_active, active, 32, cudaMemcpyDeviceToHost, st));
-    SCK(cudaStreamSynchronize(st));
+    CK(p, cudaMemcpyAsync(h_active, active, 32, cudaMemcpyDeviceToHost, st));
+    CK(p, cudaStreamSynchronize(st));
     stats->kernel_launches += 2;
     if (bytes) *bytes += n * 8;
     int n_active = 0;
     for (int d = 0; d < 8; d++) n_active += h_active[d] != 0;
     if (!n_active) return cur;
     const size_t status_bytes = (size_t)ntiles * 256 * 4 * (size_t)n_active;   // one look-back array per pass
-    if ((rc = scratch(1, status_bytes, (void**)&status))) return rc;
-    SCK(cudaMemsetAsync(status, 0, status_bytes, st));
+    if ((rc = ensure_buf(p, &scratch.status, &scratch.status_cap, status_bytes))) return rc;
+    uint32_t* status = (uint32_t*)scratch.status;
+    CK(p, cudaMemsetAsync(status, 0, status_bytes, st));
     const auto pass = ids ? k_rs_pass<true> : k_rs_pass<false>;
     const size_t smem = (size_t)RS_TILE * (ids ? 12 : 8) + (8 * 256 + 256 + 256) * 4;   // under 48 KB: no opt-in needed
     int slot = 0;
@@ -265,7 +267,7 @@ int radix_sort(uint64_t* const keys[2], uint32_t* const ids[2], int cur, int64_t
         stats->kernel_launches++;
         if (bytes) *bytes += n * (ids ? 24 : 16);
     }
-    SCK(cudaGetLastError());
+    CK(p, cudaGetLastError());
     return cur;
 }
 

@@ -1,18 +1,14 @@
 // prims.cuh — device primitives of ORDER BY, the window stage and rb_build_agg (prims.cu): radix sort, prefix sum, row ids, null bitmaps
 #pragma once
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
-#include <functional>
-#include <string>
 #include "../include/bkgpu.h"
 
 namespace bk {
 
 // CTAs of 256 threads for a grid-stride loop over n items: at least one, at most `per_sm` per SM
 int grid_for(int64_t n, int sm, int per_sm);
-// err = "what: <CUDA's message>"; BKGPU_ENOMEM when the device ran out of memory, else BKGPU_ENODEV
-int cuda_fail(std::string& err, cudaError_t e, const char* what);
-#define SCK(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return cuda_fail(err, e__, #call); } while (0)
 
 __global__ void k_iota(uint32_t* ids, int64_t n);   // ids[i] = i
 // null BYTES (1 = NULL) -> Arrow validity bitmap (bit set = valid); *any_null = 1 when one is NULL (any_null may be nullptr)
@@ -24,13 +20,15 @@ int64_t scan_scratch(int64_t n);
 
 // the radix sort keeps a tile's prefix count in a 30-bit field
 constexpr int64_t RADIX_MAX_KEYS = ((int64_t)1 << 30) - 1;
-// device memory the radix sort asks for (slot 0: histograms, slot 1: look-back status), valid until it returns; a BKGPU code on failure,
-// whose message the callback records
-using RadixScratch = std::function<int(int slot, size_t bytes, void** out)>;
+// the radix sort's device scratch (the plan's buffers, grown as its sorts need): histograms and the look-back status
+struct RadixScratch {
+    void* hist = nullptr; size_t hist_cap = 0;
+    void* status = nullptr; size_t status_cap = 0;
+};
 // Stable LSD radix sort of n <= RADIX_MAX_KEYS 64-bit keys in keys[cur], 8 bits per pass, keys[cur ^ 1] the second buffer; with ids
-// (nullptr: keys alone), ids[cur] travel with their keys.  Returns the buffer that holds the result, or a BKGPU code < 0 (`err` set unless
-// the scratch failed).  Counts its launches in stats->kernel_launches and, with `bytes`, the bytes its passes move in *bytes.
-int radix_sort(uint64_t* const keys[2], uint32_t* const ids[2], int cur, int64_t n, int sm, const RadixScratch& scratch, cudaStream_t st,
-               bkgpu_stats* stats, int64_t* bytes, std::string& err);
+// (nullptr: keys alone), ids[cur] travel with their keys.  Runs on p->stream.  Returns the buffer that holds the result, or a BKGPU
+// code < 0 (set by p->fail).  Counts its launches in stats->kernel_launches and, with `bytes`, the bytes its passes move in *bytes.
+int radix_sort(bkgpu_plan* p, uint64_t* const keys[2], uint32_t* const ids[2], int cur, int64_t n, RadixScratch& scratch, bkgpu_stats* stats,
+               int64_t* bytes);
 
 }  // namespace bk

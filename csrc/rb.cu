@@ -164,10 +164,8 @@ template <typename T> static T d2h(bkgpu_plan* p, const T* src, int* rc) {
 // sort keys [0, n) of the pair buffer: p->rb.keys then points at the sorted keys (the sort's second buffer is p->rb.alt)
 static int rb_sort(bkgpu_plan* p, int64_t n) {
     uint64_t* keys[2] = {p->rb.keys, p->rb.alt};
-    std::string err;
-    const int r = radix_sort(keys, nullptr, 0, n, p->sm_count, [p](int slot, size_t bytes, void** out) { return rb_buf(p, slot, bytes, out); },
-                             p->stream, &p->stats, nullptr, err);
-    if (r < 0) return err.empty() ? r : p->fail(r, "rb_build_agg: %s", err.c_str());
+    const int r = radix_sort(p, keys, nullptr, 0, n, p->rb.sort, &p->stats, nullptr);
+    if (r < 0) return r;
     if (r) std::swap(p->rb.keys, p->rb.alt);
     return BKGPU_OK;
 }
@@ -180,7 +178,10 @@ int rb_compact(bkgpu_plan* p, uint64_t* n_out) {
         return p->fail(BKGPU_ETOOBIG, "rb_build_agg: more than %llu (group, value) pairs in one batch: raise rb_pair_capacity", (unsigned long long)p->rb.cap);
     if ((rc = rb_sort(p, (int64_t)n))) return rc;
     uint32_t *flags, *sums;
-    if ((rc = rb_buf(p, 1, (n + 1) * 4, (void**)&flags)) || (rc = rb_buf(p, 2, (size_t)scan_scratch((int64_t)n + 1) * 4, (void**)&sums))) return rc;
+    // (the flags reuse the sort's look-back status buffer: the sort is done with it)
+    if ((rc = ensure_buf(p, &p->rb.sort.status, &p->rb.sort.status_cap, (n + 1) * 4))) return rc;
+    flags = (uint32_t*)p->rb.sort.status;
+    if ((rc = rb_buf(p, 0, (size_t)scan_scratch((int64_t)n + 1) * 4, (void**)&sums))) return rc;
     const int g = grid_for((int64_t)n + 1, p->sm_count, 16);
     k_uniq_flags<<<g, 256, 0, p->stream>>>(p->rb.keys, (int64_t)n, flags);
     CK(p, cudaGetLastError());
@@ -205,7 +206,7 @@ int rb_build(bkgpu_plan* p) {
     const uint64_t* u = p->rb.keys;
     uint64_t* e = p->rb.alt;   // (cap + 1 words: room for the scan's closing entry)
     uint64_t* sums64;
-    if ((rc = rb_buf(p, 2, (size_t)scan_scratch(m + 1) * 8, (void**)&sums64))) return rc;
+    if ((rc = rb_buf(p, 0, (size_t)scan_scratch(m + 1) * 8, (void**)&sums64))) return rc;
     k_seg_flags<<<grid_for(m + 1, sm, 16), 256, 0, s>>>(u, m, e);
     CK(p, cudaGetLastError());
     CK(p, scan_excl(e, m + 1, sums64, sm, s));
@@ -215,13 +216,13 @@ int rb_build(bkgpu_plan* p) {
     uint32_t *cst, *crun, *rst, *bi, *bst, *bhdr, *bid;
     uint8_t *ctype, *bhas, *out;
     uint64_t *psz, *coff, *bo;
-    if ((rc = rb_buf(p, 3, (size_t)(nc + 1) * 4, (void**)&cst)) || (rc = rb_buf(p, 4, (size_t)(nc + 1) * 4, (void**)&crun)) ||
-        (rc = rb_buf(p, 5, (size_t)(nr + 1) * 4, (void**)&rst)) || (rc = rb_buf(p, 6, (size_t)nc, (void**)&ctype)) ||
-        (rc = rb_buf(p, 7, (size_t)(nc + 1) * 8, (void**)&psz)) || (rc = rb_buf(p, 8, (size_t)(nc + 1) * 4, (void**)&bi)) ||
-        (rc = rb_buf(p, 9, (size_t)nc * 8, (void**)&coff)) || (rc = rb_buf(p, 10, (size_t)(nc + 1) * 4, (void**)&bst)) ||
-        (rc = rb_buf(p, 11, (size_t)(nc + 1), (void**)&bhas)) || (rc = rb_buf(p, 12, (size_t)(nc + 1) * 4, (void**)&bhdr)) ||
-        (rc = rb_buf(p, 13, (size_t)(nc + 1) * 8, (void**)&bo)) || (rc = rb_buf(p, 14, (size_t)(nc + 1) * 4, (void**)&bid)) ||
-        (rc = rb_buf(p, 2, (size_t)scan_scratch(std::max(m, nc) + 1) * 8, (void**)&sums64)))
+    if ((rc = rb_buf(p, 1, (size_t)(nc + 1) * 4, (void**)&cst)) || (rc = rb_buf(p, 2, (size_t)(nc + 1) * 4, (void**)&crun)) ||
+        (rc = rb_buf(p, 3, (size_t)(nr + 1) * 4, (void**)&rst)) || (rc = rb_buf(p, 4, (size_t)nc, (void**)&ctype)) ||
+        (rc = rb_buf(p, 5, (size_t)(nc + 1) * 8, (void**)&psz)) || (rc = rb_buf(p, 6, (size_t)(nc + 1) * 4, (void**)&bi)) ||
+        (rc = rb_buf(p, 7, (size_t)nc * 8, (void**)&coff)) || (rc = rb_buf(p, 8, (size_t)(nc + 1) * 4, (void**)&bst)) ||
+        (rc = rb_buf(p, 9, (size_t)(nc + 1), (void**)&bhas)) || (rc = rb_buf(p, 10, (size_t)(nc + 1) * 4, (void**)&bhdr)) ||
+        (rc = rb_buf(p, 11, (size_t)(nc + 1) * 8, (void**)&bo)) || (rc = rb_buf(p, 12, (size_t)(nc + 1) * 4, (void**)&bid)) ||
+        (rc = rb_buf(p, 0, (size_t)scan_scratch(std::max(m, nc) + 1) * 8, (void**)&sums64)))
         return rc;
     k_seg_mark<<<grid_for(m + 1, sm, 16), 256, 0, s>>>(u, m, e, cst, crun, rst);
     k_containers<<<grid_for(nc + 1, sm, 16), 256, 0, s>>>(u, nc, cst, crun, ctype, psz, bi);
@@ -237,7 +238,7 @@ int rb_build(bkgpu_plan* p) {
     CK(p, cudaMemcpyAsync(&nb, bi + nc, 4, cudaMemcpyDeviceToHost, s));
     CK(p, cudaMemcpyAsync(&total, bo + nc, 8, cudaMemcpyDeviceToHost, s));
     CK(p, cudaStreamSynchronize(s));
-    if ((rc = rb_buf(p, 15, (size_t)total, (void**)&out))) return rc;
+    if ((rc = rb_buf(p, 13, (size_t)total, (void**)&out))) return rc;
     k_headers<<<grid_for(nc, sm, 16), 256, 0, s>>>(u, nc, bi, bst, bhas, bhdr, bo, psz, cst, crun, ctype, out, coff);
     k_payloads<<<grid_for(m, sm, 16), 256, 0, s>>>(u, m, e, ctype, coff, cst, crun, rst, out);
     k_bitsets<<<(unsigned)std::max<int64_t>(1, std::min<int64_t>(nc, (int64_t)sm * 8)), 256, 0, s>>>(u, nc, cst, ctype, coff, out);

@@ -3,6 +3,7 @@
 #include <stdint.h>
 #include <vector>
 #include "dev_types.h"
+#include "prims.cuh"
 
 struct bkgpu_plan;
 
@@ -14,7 +15,8 @@ struct RbState {
     uint64_t cap = 0;
     uint64_t hi = 0;                                   // upper bound of the keys it holds (exact after a compaction)
     uint64_t* alt = nullptr;                           // the radix sort's second buffer, as large as the pair buffer
-    void* scratch[16] = {}; size_t scratch_cap[16] = {};   // grow-only device scratch of the sort and the build
+    RadixScratch sort;                                 // the radix sort's scratch, grow-only
+    void* scratch[14] = {}; size_t scratch_cap[14] = {};   // grow-only device scratch of the build
     // the finished bitmaps of a request: ids (slot << 2 | rb_idx, ascending), offsets into `bytes` (one more than ids)
     std::vector<uint32_t> bid;
     std::vector<uint64_t> off;

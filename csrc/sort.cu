@@ -20,6 +20,7 @@
 #include "sort.h"
 #include <algorithm>
 #include <string.h>
+#include "api_state.h"
 #include "dev_common.cuh"
 #include "interp.cuh"
 #include "nccl_dl.h"
@@ -448,8 +449,8 @@ struct Pool {               // the k best rows seen so far of one class (keys pr
 };
 
 struct SortState {
+    bkgpu_plan* p = nullptr;        // the owning plan: its allocator, stream and SM count
     Compiled c;
-    int device = 0, sm_count = 132;
     int ncols = 0;
     int64_t k = -1;                 // rows to keep; -1 = all
     uint64_t row_base = 0, region_base = 0;
@@ -467,27 +468,12 @@ struct SortState {
     std::vector<uint8_t*> ret_vals, ret_null; int64_t ret_rows = 0, ret_cap = 0;
     std::vector<uint8_t*> key_img;  // per ORDER BY key: retained images (full sort)
     uint8_t* ret_keep = nullptr;
-    std::vector<void*> allocs;
     int64_t total_seen = 0;
     std::vector<SortOutCol> pending_out; int64_t pending_rows = 0;
 };
 
 namespace {
 
-int fail(std::string& err, int code, const char* msg) { err = msg; return code; }
-
-template <class T> int dalloc(SortState* s, T** p, size_t bytes, std::string& err) {
-    cudaError_t e = cudaMalloc((void**)p, bytes ? bytes : 8);
-    if (e != cudaSuccess) return cuda_fail(err, e, "cudaMalloc");
-    s->allocs.push_back(*p);
-    return 0;
-}
-void dfree(SortState* s, void* p) {
-    if (!p) return;
-    auto it = std::find(s->allocs.begin(), s->allocs.end(), p);
-    if (it != s->allocs.end()) s->allocs.erase(it);
-    cudaFree(p);
-}
 int elem_bytes_of(int prim) { return storage_bytes(prim_storage(prim)); }
 
 void fill_row_args(const SortState* s, const DevCol* cols, int64_t nrows, RowArgs& a) {
@@ -503,7 +489,10 @@ void fill_row_args(const SortState* s, const DevCol* cols, int64_t nrows, RowArg
 }
 
 // ---- selection of the k smallest composite keys of one class out of the batch; result merged into the pool ----
-int select_topk_class(SortState* s, const RowArgs& ra, int cls, cudaStream_t st, bkgpu_stats* stats, std::string& err) {
+int select_topk_class(SortState* s, const RowArgs& ra, int cls, bkgpu_stats* stats) {
+    bkgpu_plan* p = s->p;
+    const cudaStream_t st = p->stream;
+    const int sm_count = p->sm_count;
     Pool& P = s->pool[cls - 1];
     const uint32_t k = (uint32_t)s->k;
     uint32_t* cnt = s->d_counts;     // [0] sample count  [1] level-1 candidates  [2] level-2  [3] rows of this class  [4] kept rows  [5] level-3  [6] two_step: best of the batch
@@ -517,8 +506,8 @@ int select_topk_class(SortState* s, const RowArgs& ra, int cls, cudaStream_t st,
     const int nxt = P.cur ^ 1;
     const uint64_t* pool_thr = nullptr;
     if (P.n >= k) {   // later rows must beat the k-th composite key kept so far
-        SCK(cudaMemcpyAsync(thr + 12, P.key[P.cur] + (k - 1), 8, cudaMemcpyDeviceToDevice, st));
-        SCK(cudaMemcpyAsync(thr + 13, P.idx[P.cur] + (k - 1), 8, cudaMemcpyDeviceToDevice, st));
+        CK(p, cudaMemcpyAsync(thr + 12, P.key[P.cur] + (k - 1), 8, cudaMemcpyDeviceToDevice, st));
+        CK(p, cudaMemcpyAsync(thr + 13, P.idx[P.cur] + (k - 1), 8, cudaMemcpyDeviceToDevice, st));
         pool_thr = thr + 12;
     }
     uint32_t h[8];
@@ -527,7 +516,7 @@ int select_topk_class(SortState* s, const RowArgs& ra, int cls, cudaStream_t st,
     // threshold (too tight / too loose) repeats the chain with wider ranks.
     for (int attempt = 0; attempt < 6; attempt++) {
         const uint32_t widen = 1u << attempt;
-        SCK(cudaMemsetAsync(cnt, 0, 32, st));
+        CK(p, cudaMemsetAsync(cnt, 0, 32, st));
         const bool big = ra.nrows > (int64_t)s->cand_cap / 2;
         if (big) {
             k_sample_rows<<<(SAMPLE_N + 255) / 256, 256, 0, st>>>(ra, cls, s->samp_key, s->samp_idx, cnt, 0x5bd1e995ull + attempt * 7919);
@@ -536,28 +525,28 @@ int select_topk_class(SortState* s, const RowArgs& ra, int cls, cudaStream_t st,
             k_select_rank<<<1, 1024, 0, st>>>(s->samp_key, s->samp_idx, cnt, SAMPLE_N, rank, thr, nullptr, 0, 0, 0, pool_thr);
             stats->kernel_launches += 2;
         } else if (pool_thr) {
-            SCK(cudaMemcpyAsync(thr, pool_thr, 16, cudaMemcpyDeviceToDevice, st));
-        } else SCK(cudaMemsetAsync(thr, 0xFF, 16, st));
+            CK(p, cudaMemcpyAsync(thr, pool_thr, 16, cudaMemcpyDeviceToDevice, st));
+        } else CK(p, cudaMemsetAsync(thr, 0xFF, 16, st));
         const DevCol& kc = ra.cols[ra.key.col];
         const bool vec = cls == 1 && ra.key.direct && !kc.validity && (((uintptr_t)kc.values & 31) == 0) && kc.prim != BK_INT8 && kc.prim != BK_INT16 &&
                          kc.prim != BK_UINT8 && kc.prim != BK_UINT16 && (kc.stype == ST_I64 || kc.stype == ST_U64 || kc.stype == ST_F64 || kc.stype == ST_I32 || kc.stype == ST_U32);
         s->used_vec = vec;
         if (vec) {
-            const int g = std::max(1, std::min(s->sm_count * 8, (int)((ra.nrows / 4 + 511) / 512)));
+            const int g = std::max(1, std::min(sm_count * 8, (int)((ra.nrows / 4 + 511) / 512)));
             if (kc.stype == ST_I32 || kc.stype == ST_U32) k_collect_rows_vec<4><<<g, 256, 0, st>>>(ra, thr, s->cand_key[0], s->cand_idx[0], cnt + 1, s->cand_cap, cnt + 3);
             else k_collect_rows_vec<8><<<g, 256, 0, st>>>(ra, thr, s->cand_key[0], s->cand_idx[0], cnt + 1, s->cand_cap, cnt + 3);
         } else
-        k_collect_rows<<<grid_for(ra.nrows, s->sm_count, 8), 256, 0, st>>>(ra, cls, thr, s->cand_key[0], s->cand_idx[0], cnt + 1, s->cand_cap, cnt + 3);
+        k_collect_rows<<<grid_for(ra.nrows, sm_count, 8), 256, 0, st>>>(ra, cls, thr, s->cand_key[0], s->cand_idx[0], cnt + 1, s->cand_cap, cnt + 3);
         // level 2: cand[0] (cnt[1]) -> cand[1] (cnt[2]);  level 3: cand[1] (cnt[2]) -> cand[0] (cnt[5])
         const int src_cnt[2] = {1, 2}, dst_cnt[2] = {2, 5};
         for (int lvl = 0; lvl < 2; lvl++) {
             const int from = lvl, to = lvl ^ 1;
-            SCK(cudaMemsetAsync(cnt, 0, 4, st));
+            CK(p, cudaMemsetAsync(cnt, 0, 4, st));
             k_sample_pairs<<<(SAMPLE_N + 255) / 256, 256, 0, st>>>(s->cand_key[from], s->cand_idx[from], cnt + src_cnt[lvl], s->cand_cap, s->samp_key, s->samp_idx, cnt,
                                                                    0x9e3779b9ull + attempt * 104729 + lvl);
             // (levels keep trimming until about two k-fulls are left: the one-CTA sort below costs 35 us for <= 2048 keys, 150 us for 8192)
             k_select_rank<<<1, 1024, 0, st>>>(s->samp_key, s->samp_idx, cnt, SAMPLE_N, 0, thr + 3 * (lvl + 1), cnt + src_cnt[lvl], k, widen, trim, nullptr);
-            k_collect_pairs<<<grid_for(lvl == 0 ? (int64_t)s->cand_cap / 4 : 65536, s->sm_count, 8), 256, 0, st>>>(
+            k_collect_pairs<<<grid_for(lvl == 0 ? (int64_t)s->cand_cap / 4 : 65536, sm_count, 8), 256, 0, st>>>(
                 s->cand_key[from], s->cand_idx[from], cnt + src_cnt[lvl], thr + 3 * (lvl + 1), s->cand_key[to], s->cand_idx[to], cnt + dst_cnt[lvl], s->cand_cap);
             stats->kernel_launches += 3;
         }
@@ -576,10 +565,10 @@ int select_topk_class(SortState* s, const RowArgs& ra, int cls, cudaStream_t st,
         g.n_cols = s->ncols; g.row_base = ra.row_base; g.nrows = ra.nrows; g.old_idx = P.idx[P.cur]; g.old_n = old_n;
         k_gather_topk<<<std::max(1, (int)((k + 127) / 128)), 128, 0, st>>>(g, P.idx[nxt], cnt + 4);
         stats->kernel_launches += 3;
-        if (!s->h_counts) SCK(cudaHostAlloc((void**)&s->h_counts, 64, cudaHostAllocDefault));
-        SCK(cudaMemcpyAsync(s->h_counts, cnt, 32, cudaMemcpyDeviceToHost, st));
-        if (big && pool_thr) SCK(cudaMemcpyAsync(s->h_counts + 8, thr + 2, 8, cudaMemcpyDeviceToHost, st));
-        SCK(cudaStreamSynchronize(st));
+        if (!s->h_counts) CK(p, cudaHostAlloc((void**)&s->h_counts, 64, cudaHostAllocDefault));
+        CK(p, cudaMemcpyAsync(s->h_counts, cnt, 32, cudaMemcpyDeviceToHost, st));
+        if (big && pool_thr) CK(p, cudaMemcpyAsync(s->h_counts + 8, thr + 2, 8, cudaMemcpyDeviceToHost, st));
+        CK(p, cudaStreamSynchronize(st));
         memcpy(h, s->h_counts, 32);
         const uint32_t c1 = h[1], c2 = h[2], cls_rows = h[3], c3 = h[5];
         // fewer than k candidates are complete only when the threshold in force was the pool's k-th key (every row at or below it
@@ -592,23 +581,25 @@ int select_topk_class(SortState* s, const RowArgs& ra, int cls, cudaStream_t st,
         const bool ok3 = c3 <= room && (c3 >= std::min(k, c2));
         if (ok1 && ok2 && ok3) { P.cur = nxt; P.n = h[4]; return 0; }
     }
-    return fail(err, BKGPU_ETOOBIG, "top-k selection did not converge (candidate buffers too small for this key distribution)");
+    return p->fail(BKGPU_ETOOBIG, "top-k selection did not converge (candidate buffers too small for this key distribution)");
 }
 
-int ensure_retained(SortState* s, int64_t need, cudaStream_t st, std::string& err) {
+int ensure_retained(SortState* s, int64_t need) {
     if (need <= s->ret_cap) return 0;
+    bkgpu_plan* p = s->p;
+    const cudaStream_t st = p->stream;
     int64_t cap = std::max<int64_t>(need, std::max<int64_t>(s->ret_cap * 2, 1 << 16));
     for (int c = 0; c < s->ncols; c++) {
         const int eb = elem_bytes_of(s->c.cols[(size_t)c].prim);
         uint8_t *nv = nullptr, *nn = nullptr; int rc;
-        if ((rc = dalloc(s, &nv, (size_t)cap * eb, err))) return rc;
-        if ((rc = dalloc(s, &nn, (size_t)cap, err))) return rc;
+        if ((rc = dev_alloc(p, (void**)&nv, (size_t)cap * eb))) return rc;
+        if ((rc = dev_alloc(p, (void**)&nn, (size_t)cap))) return rc;
         if (s->ret_rows) {
-            SCK(cudaMemcpyAsync(nv, s->ret_vals[(size_t)c], (size_t)s->ret_rows * eb, cudaMemcpyDeviceToDevice, st));
-            SCK(cudaMemcpyAsync(nn, s->ret_null[(size_t)c], (size_t)s->ret_rows, cudaMemcpyDeviceToDevice, st));
+            CK(p, cudaMemcpyAsync(nv, s->ret_vals[(size_t)c], (size_t)s->ret_rows * eb, cudaMemcpyDeviceToDevice, st));
+            CK(p, cudaMemcpyAsync(nn, s->ret_null[(size_t)c], (size_t)s->ret_rows, cudaMemcpyDeviceToDevice, st));
         }
-        SCK(cudaStreamSynchronize(st));
-        dfree(s, s->ret_vals[(size_t)c]); dfree(s, s->ret_null[(size_t)c]);
+        CK(p, cudaStreamSynchronize(st));
+        dev_free(p, s->ret_vals[(size_t)c]); dev_free(p, s->ret_null[(size_t)c]);
         s->ret_vals[(size_t)c] = nv; s->ret_null[(size_t)c] = nn;
     }
     s->ret_cap = cap;
@@ -616,43 +607,47 @@ int ensure_retained(SortState* s, int64_t need, cudaStream_t st, std::string& er
 }
 
 // rows that pass the predicate are appended, in input order, to the retained columns (filter-only and full sort)
-int retain_batch(SortState* s, const RowArgs& ra, cudaStream_t st, bkgpu_stats* stats, std::string& err) {
+int retain_batch(SortState* s, const RowArgs& ra, bkgpu_stats* stats) {
     const int64_t limit_left = (s->c.kind == PK_FILTER && s->c.limit >= 0) ? std::max<int64_t>(s->c.limit - s->ret_rows, 0) : INT64_MAX;
     if (limit_left == 0) return 0;   // FilterNode stops after `limit` passing rows (filter_node.cpp:786-791)
+    bkgpu_plan* p = s->p;
+    const cudaStream_t st = p->stream;
     const int64_t rows_per_block = 4096;
     const uint32_t nblocks = (uint32_t)((ra.nrows + rows_per_block - 1) / rows_per_block);
     // counts[b]: the passing rows of block b, scanned into its first output position; counts[nblocks] closes the scan with the total
+    DevScope scope(p);
     uint32_t *counts = nullptr, *sums = nullptr, *sel = nullptr; int rc;
-    if ((rc = dalloc(s, &counts, ((size_t)nblocks + 1) * 4, err))) return rc;
-    if ((rc = dalloc(s, &sums, (size_t)scan_scratch((int64_t)nblocks + 1) * 4, err))) return rc;
-    SCK(cudaMemsetAsync(counts + nblocks, 0, 4, st));
+    if ((rc = scope.alloc(&counts, ((size_t)nblocks + 1) * 4))) return rc;
+    if ((rc = scope.alloc(&sums, (size_t)scan_scratch((int64_t)nblocks + 1) * 4))) return rc;
+    CK(p, cudaMemsetAsync(counts + nblocks, 0, 4, st));
     k_filter_count<<<nblocks, 256, 0, st>>>(ra, counts, rows_per_block);
-    SCK(scan_excl(counts, (int64_t)nblocks + 1, sums, s->sm_count, st));
+    CK(p, scan_excl(counts, (int64_t)nblocks + 1, sums, p->sm_count, st));
     uint32_t total = 0;
-    SCK(cudaMemcpyAsync(&total, counts + nblocks, 4, cudaMemcpyDeviceToHost, st));
-    SCK(cudaStreamSynchronize(st));
+    CK(p, cudaMemcpyAsync(&total, counts + nblocks, 4, cudaMemcpyDeviceToHost, st));
+    CK(p, cudaStreamSynchronize(st));
     const uint64_t take = std::min<uint64_t>(total, (uint64_t)limit_left);
     if (take > 0) {
-        if ((rc = dalloc(s, &sel, (size_t)take * 4, err))) return rc;
+        if ((rc = scope.alloc(&sel, (size_t)take * 4))) return rc;
         k_filter_write<<<nblocks, 256, 0, st>>>(ra, counts, rows_per_block, sel, 0, take);
-        if ((rc = ensure_retained(s, s->ret_rows + (int64_t)take, st, err))) return rc;
+        if ((rc = ensure_retained(s, s->ret_rows + (int64_t)take))) return rc;
         GatherArgs g; memset(&g, 0, sizeof g);
         for (int i = 0; i < s->ncols; i++) { g.cols[i] = ra.cols[i]; g.dst_vals[i] = s->ret_vals[(size_t)i]; g.dst_null[i] = s->ret_null[(size_t)i]; }
         g.n_cols = s->ncols;
-        k_gather_sel<<<grid_for((int64_t)take, s->sm_count, 8), 256, 0, st>>>(g, sel, take, (uint64_t)s->ret_rows);
-        SCK(cudaStreamSynchronize(st));
+        k_gather_sel<<<grid_for((int64_t)take, p->sm_count, 8), 256, 0, st>>>(g, sel, take, (uint64_t)s->ret_rows);
+        CK(p, cudaStreamSynchronize(st));
         s->ret_rows += (int64_t)take;
         stats->kernel_launches += 2;
     }
     stats->kernel_launches += 2;   // the count and the scan: one launch up to 2048 blocks (8M rows), three beyond
     stats->rows_filtered += ra.nrows - (int64_t)total;
-    dfree(s, counts); dfree(s, sums); dfree(s, sel);
     return 0;
 }
 
 int copy_cols_out(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, const std::vector<ColRef>& desc, const uint32_t* perm_dev, int64_t n, int64_t skip,
-                  cudaStream_t st, std::vector<SortOutCol>& out, std::string& err) {
+                  std::vector<SortOutCol>& out) {
     // perm_dev == nullptr: rows [skip, skip+n) in place; else gather through a device permutation first
+    bkgpu_plan* p = s->p;
+    const cudaStream_t st = p->stream;
     out.clear();
     for (size_t c = 0; c < desc.size(); c++) {
         const ColRef& cr = desc[c];
@@ -660,20 +655,19 @@ int copy_cols_out(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, con
         oc.values.assign((size_t)std::max<int64_t>(n, 1) * oc.elem, 0);
         std::vector<uint8_t> nb((size_t)std::max<int64_t>(n, 1));
         const uint8_t* sv = vals[c]; const uint8_t* sn = nulls[c];
-        uint8_t *tv = nullptr, *tn = nullptr;
         if (perm_dev && n > 0) {
-            int rc;
-            if ((rc = dalloc(s, &tv, (size_t)n * oc.elem, err))) return rc;
-            if ((rc = dalloc(s, &tn, (size_t)n, err))) return rc;
-            if ((rc = sort_gather_rows(s, sv, sn, cr.prim, perm_dev + skip, n, tv, tn, st))) return fail(err, rc, "gathering the sorted rows failed");
-            SCK(cudaMemcpyAsync(oc.values.data(), tv, (size_t)n * oc.elem, cudaMemcpyDeviceToHost, st));
-            SCK(cudaMemcpyAsync(nb.data(), tn, (size_t)n, cudaMemcpyDeviceToHost, st));
-            SCK(cudaStreamSynchronize(st));
-            dfree(s, tv); dfree(s, tn);
+            DevScope scope(p);   // the column's gather buffers
+            uint8_t *tv = nullptr, *tn = nullptr; int rc;
+            if ((rc = scope.alloc(&tv, (size_t)n * oc.elem))) return rc;
+            if ((rc = scope.alloc(&tn, (size_t)n))) return rc;
+            if ((rc = sort_gather_rows(s, sv, sn, cr.prim, perm_dev + skip, n, tv, tn))) return p->fail(rc, "gathering the sorted rows failed");
+            CK(p, cudaMemcpyAsync(oc.values.data(), tv, (size_t)n * oc.elem, cudaMemcpyDeviceToHost, st));
+            CK(p, cudaMemcpyAsync(nb.data(), tn, (size_t)n, cudaMemcpyDeviceToHost, st));
+            CK(p, cudaStreamSynchronize(st));
         } else if (n > 0) {
-            SCK(cudaMemcpyAsync(oc.values.data(), sv + (size_t)skip * oc.elem, (size_t)n * oc.elem, cudaMemcpyDeviceToHost, st));
-            SCK(cudaMemcpyAsync(nb.data(), sn + skip, (size_t)n, cudaMemcpyDeviceToHost, st));
-            SCK(cudaStreamSynchronize(st));
+            CK(p, cudaMemcpyAsync(oc.values.data(), sv + (size_t)skip * oc.elem, (size_t)n * oc.elem, cudaMemcpyDeviceToHost, st));
+            CK(p, cudaMemcpyAsync(nb.data(), sn + skip, (size_t)n, cudaMemcpyDeviceToHost, st));
+            CK(p, cudaStreamSynchronize(st));
         }
         bool any = false;
         for (int64_t i = 0; i < n; i++) any |= nb[(size_t)i] != 0;
@@ -685,49 +679,48 @@ int copy_cols_out(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, con
     }
     return 0;
 }
-int copy_out(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, const uint32_t* perm_dev, int64_t n, int64_t skip, cudaStream_t st,
-             std::vector<SortOutCol>& out, std::string& err) {
-    return copy_cols_out(s, vals, nulls, s->c.cols, perm_dev, n, skip, st, out, err);
+int copy_out(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, const uint32_t* perm_dev, int64_t n, int64_t skip, std::vector<SortOutCol>& out) {
+    return copy_cols_out(s, vals, nulls, s->c.cols, perm_dev, n, skip, out);
 }
 
-// scratch of one radix sort of n (key image, row id) pairs
+// the buffers of one radix sort of n (key image, row id) pairs, returned to the plan's allocator when it leaves scope
 struct RadixBufs {
+    DevScope scope;
     uint64_t *img_row = nullptr, *img[2] = {nullptr, nullptr}; uint32_t* ids[2] = {nullptr, nullptr};
-    void* scratch[2] = {nullptr, nullptr}; size_t scratch_cap[2] = {0, 0};   // radix_sort's, grown as its sorts need
+    RadixScratch scratch;   // radix_sort's, grown as its sorts need
     uint32_t n = 0;
+    explicit RadixBufs(bkgpu_plan* p) : scope(p) {}
+    ~RadixBufs() { dev_free(scope.p, scratch.hist); dev_free(scope.p, scratch.status); }
+    int alloc(int64_t rows) {
+        n = (uint32_t)rows;
+        int rc;
+        if ((rc = scope.alloc(&img_row, (size_t)n * 8)) || (rc = scope.alloc(&img[0], (size_t)n * 8)) || (rc = scope.alloc(&img[1], (size_t)n * 8)) ||
+            (rc = scope.alloc(&ids[0], (size_t)n * 4)) || (rc = scope.alloc(&ids[1], (size_t)n * 4)))
+            return rc;
+        return 0;
+    }
 };
-int radix_alloc(SortState* s, int64_t n, RadixBufs& b, std::string& err) {
-    b.n = (uint32_t)n;
-    int rc;
-    if ((rc = dalloc(s, &b.img_row, (size_t)n * 8, err))) return rc;
-    if ((rc = dalloc(s, &b.img[0], (size_t)n * 8, err))) return rc;
-    if ((rc = dalloc(s, &b.img[1], (size_t)n * 8, err))) return rc;
-    if ((rc = dalloc(s, &b.ids[0], (size_t)n * 4, err))) return rc;
-    if ((rc = dalloc(s, &b.ids[1], (size_t)n * 4, err))) return rc;
-    return 0;
-}
-void radix_free(SortState* s, RadixBufs& b) {
-    dfree(s, b.img_row); dfree(s, b.img[0]); dfree(s, b.img[1]); dfree(s, b.ids[0]); dfree(s, b.ids[1]); dfree(s, b.scratch[0]); dfree(s, b.scratch[1]);
-    b = RadixBufs();
-}
 
-// retained columns as DevCols of `ra` (values + validity bitmaps packed from the null bytes); h_null_flags[c]: column c holds a NULL
-int retained_bitmaps(SortState* s, cudaStream_t st, RowArgs& ra, std::vector<uint8_t*>& bitmaps, uint32_t* h_null_flags, std::string& err) {
+// retained columns as DevCols of `ra` (values + validity bitmaps packed from the null bytes, owned by `scope`); h_null_flags[c]: column c
+// holds a NULL
+int retained_bitmaps(SortState* s, DevScope& scope, RowArgs& ra, uint32_t* h_null_flags) {
+    bkgpu_plan* p = s->p;
+    const cudaStream_t st = p->stream;
     const int64_t n = s->ret_rows;
     int rc;
     for (int c = 0; c < s->ncols; c++) { ra.cols[c].values = s->ret_vals[(size_t)c]; ra.cols[c].validity = nullptr; ra.cols[c].stype = prim_storage(s->c.cols[(size_t)c].prim); ra.cols[c].prim = s->c.cols[(size_t)c].prim; }
-    bitmaps.assign((size_t)s->ncols, nullptr);
+    DevScope flags_scope(p);
     uint32_t* null_flags = nullptr;
-    if ((rc = dalloc(s, &null_flags, sizeof(uint32_t) * MAX_COLS, err))) return rc;
-    SCK(cudaMemsetAsync(null_flags, 0, sizeof(uint32_t) * MAX_COLS, st));
+    if ((rc = flags_scope.alloc(&null_flags, sizeof(uint32_t) * MAX_COLS))) return rc;
+    CK(p, cudaMemsetAsync(null_flags, 0, sizeof(uint32_t) * MAX_COLS, st));
     for (int c = 0; c < s->ncols; c++) {
-        if ((rc = dalloc(s, &bitmaps[(size_t)c], (size_t)(n + 7) / 8 + 64, err))) return rc;
-        k_pack_null_bytes<<<grid_for((n + 7) / 8, s->sm_count, 8), 256, 0, st>>>(s->ret_null[(size_t)c], n, bitmaps[(size_t)c], null_flags + c);
-        ra.cols[c].validity = bitmaps[(size_t)c];
+        uint8_t* bitmap = nullptr;
+        if ((rc = scope.alloc(&bitmap, (size_t)(n + 7) / 8 + 64))) return rc;
+        k_pack_null_bytes<<<grid_for((n + 7) / 8, p->sm_count, 8), 256, 0, st>>>(s->ret_null[(size_t)c], n, bitmap, null_flags + c);
+        ra.cols[c].validity = bitmap;
     }
-    SCK(cudaMemcpyAsync(h_null_flags, null_flags, sizeof(uint32_t) * (size_t)s->ncols, cudaMemcpyDeviceToHost, st));
-    SCK(cudaStreamSynchronize(st));
-    dfree(s, null_flags);
+    CK(p, cudaMemcpyAsync(h_null_flags, null_flags, sizeof(uint32_t) * (size_t)s->ncols, cudaMemcpyDeviceToHost, st));
+    CK(p, cudaStreamSynchronize(st));
     ra.n_cols = s->ncols; ra.nrows = n;
     return 0;
 }
@@ -736,32 +729,26 @@ int retained_bitmaps(SortState* s, cudaStream_t st, RowArgs& ra, std::vector<uin
 // output register keys[k].out_reg), or straight from column `direct_col` when that is >= 0 (one key).  identity_start: b.ids[cur] holds
 // 0..n-1, so the first key's images need no gather into the current order.
 int radix_sort_keys(SortState* s, RowArgs& ra, const std::vector<SortKey>& keys, const std::vector<const Program*>& progs, int direct_col,
-                    bool direct_has_nulls, RadixBufs& b, int& cur, bool identity_start, cudaStream_t st, bkgpu_stats* stats, int64_t& pass_bytes, std::string& err) {
+                    bool direct_has_nulls, RadixBufs& b, int& cur, bool identity_start, bkgpu_stats* stats, int64_t& pass_bytes) {
+    bkgpu_plan* p = s->p;
+    const cudaStream_t st = p->stream;
+    const int sm = p->sm_count;
     const int64_t n = b.n;
     uint64_t** img = b.img; uint32_t** ids = b.ids; uint64_t* img_row = b.img_row;
     bool first = identity_start;
-    const RadixScratch scratch = [&](int slot, size_t bytes, void** out) -> int {
-        if (b.scratch_cap[slot] < bytes) {
-            dfree(s, b.scratch[slot]); b.scratch[slot] = nullptr; b.scratch_cap[slot] = 0;
-            if (int rc = dalloc(s, &b.scratch[slot], bytes, err)) return rc;
-            b.scratch_cap[slot] = bytes;
-        }
-        *out = b.scratch[slot];
-        return 0;
-    };
     for (int ki = (int)keys.size() - 1; ki >= 0; ki--) {
         const SortKey& sk = keys[(size_t)ki];
         ra.prog = *progs[(size_t)ki];
         for (int mode = 0; mode < 2; mode++) {   // the key's value image first, then its NULL rank (stable: NULLs end up strictly first / last)
             if (mode == 1 && direct_col >= 0 && !direct_has_nulls) continue;
             uint64_t* dst = first ? img[cur] : img_row;
-            if (mode == 0 && direct_col >= 0) k_sort_images_direct<<<grid_for(n, s->sm_count, 8), 256, 0, st>>>(ra.cols[direct_col], n, host_prim_class(sk.prim), sk.asc ? 0 : 1, dst);
+            if (mode == 0 && direct_col >= 0) k_sort_images_direct<<<grid_for(n, sm, 8), 256, 0, st>>>(ra.cols[direct_col], n, host_prim_class(sk.prim), sk.asc ? 0 : 1, dst);
             else
-            k_sort_images<<<grid_for(n, s->sm_count, 8), 256, 0, st>>>(ra, sk.out_reg, host_prim_class(sk.prim), sk.asc ? 0 : 1, sk.null_first ? 1 : 0, mode, dst, nullptr);
-            if (!first) k_rs_gather_u64<<<grid_for(n, s->sm_count, 8), 256, 0, st>>>(img_row, ids[cur], img[cur], b.n);   // images in the current order
+            k_sort_images<<<grid_for(n, sm, 8), 256, 0, st>>>(ra, sk.out_reg, host_prim_class(sk.prim), sk.asc ? 0 : 1, sk.null_first ? 1 : 0, mode, dst, nullptr);
+            if (!first) k_rs_gather_u64<<<grid_for(n, sm, 8), 256, 0, st>>>(img_row, ids[cur], img[cur], b.n);   // images in the current order
             first = false;
             stats->kernel_launches += 2;
-            const int r = radix_sort(img, ids, cur, n, s->sm_count, scratch, st, stats, &pass_bytes, err);
+            const int r = radix_sort(p, img, ids, cur, n, b.scratch, stats, &pass_bytes);
             if (r < 0) return r;
             cur = r;
         }
@@ -771,12 +758,10 @@ int radix_sort_keys(SortState* s, RowArgs& ra, const std::vector<SortKey>& keys,
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------------------
-int sort_open(const Compiled& c, int device, cudaStream_t stream, int64_t region_base, SortState** out, std::string& err) {
-    (void)stream;
+int sort_open(bkgpu_plan* p, const Compiled& c, int64_t region_base, SortState** out) {
     SortState* s = new SortState();
-    s->c = c; s->device = device; s->ncols = (int)c.cols.size();
+    s->p = p; s->c = c; s->ncols = (int)c.cols.size();
     s->row_base = s->region_base = (uint64_t)region_base;
-    { int n = 0; if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device) == cudaSuccess && n > 0) s->sm_count = n; }
     s->k = c.kind == PK_SORT ? c.limit : -1;
     s->topk = c.kind == PK_SORT && c.sort_keys.size() == 1 && s->k >= 0 && s->k <= 4096;
     s->ret_vals.assign((size_t)s->ncols, nullptr); s->ret_null.assign((size_t)s->ncols, nullptr);
@@ -785,53 +770,53 @@ int sort_open(const Compiled& c, int device, cudaStream_t stream, int64_t region
         s->cand_cap = 1u << 22;   // 4M candidate pairs (64 MB per array pair)
         const size_t kk = (size_t)std::max<int64_t>(s->k, 1);
         for (int b = 0; b < 2 && !rc; b++) {
-            if ((rc = dalloc(s, &s->cand_key[b], (size_t)s->cand_cap * 8, err))) break;
-            if ((rc = dalloc(s, &s->cand_idx[b], (size_t)s->cand_cap * 8, err))) break;
+            if ((rc = dev_alloc(p, (void**)&s->cand_key[b], (size_t)s->cand_cap * 8))) break;
+            if ((rc = dev_alloc(p, (void**)&s->cand_idx[b], (size_t)s->cand_cap * 8))) break;
         }
-        if (!rc) rc = dalloc(s, &s->samp_key, SAMPLE_N * 8, err);
-        if (!rc) rc = dalloc(s, &s->samp_idx, SAMPLE_N * 8, err);
-        if (!rc) rc = dalloc(s, &s->d_counts, 64, err);
-        if (!rc) rc = dalloc(s, &s->d_rank, 128, err);
-        for (int p = 0; p < 2 && !rc; p++) for (int b = 0; b < 2 && !rc; b++) {
-            if ((rc = dalloc(s, &s->pool[p].key[b], kk * 8, err))) break;
-            if ((rc = dalloc(s, &s->pool[p].idx[b], kk * 8, err))) break;
+        if (!rc) rc = dev_alloc(p, (void**)&s->samp_key, SAMPLE_N * 8);
+        if (!rc) rc = dev_alloc(p, (void**)&s->samp_idx, SAMPLE_N * 8);
+        if (!rc) rc = dev_alloc(p, (void**)&s->d_counts, 64);
+        if (!rc) rc = dev_alloc(p, (void**)&s->d_rank, 128);
+        for (int q = 0; q < 2 && !rc; q++) for (int b = 0; b < 2 && !rc; b++) {
+            if ((rc = dev_alloc(p, (void**)&s->pool[q].key[b], kk * 8))) break;
+            if ((rc = dev_alloc(p, (void**)&s->pool[q].idx[b], kk * 8))) break;
             for (int ci = 0; ci < s->ncols && !rc; ci++) {
-                if ((rc = dalloc(s, &s->pool[p].vals[b][ci], kk * (size_t)elem_bytes_of(c.cols[(size_t)ci].prim), err))) break;
-                rc = dalloc(s, &s->pool[p].nulls[b][ci], kk, err);
+                if ((rc = dev_alloc(p, (void**)&s->pool[q].vals[b][ci], kk * (size_t)elem_bytes_of(c.cols[(size_t)ci].prim)))) break;
+                rc = dev_alloc(p, (void**)&s->pool[q].nulls[b][ci], kk);
             }
         }
-        if (!rc) { cudaError_t e = cudaFuncSetAttribute(k_sort_small, cudaFuncAttributeMaxDynamicSharedMemorySize, SMALL_N * 16); if (e != cudaSuccess) rc = cuda_fail(err, e, "cudaFuncSetAttribute"); }
+        if (!rc) { cudaError_t e = cudaFuncSetAttribute(k_sort_small, cudaFuncAttributeMaxDynamicSharedMemorySize, SMALL_N * 16); if (e != cudaSuccess) rc = p->cuda_fail(e, "cudaFuncSetAttribute"); }
     }
     if (rc) { sort_close(s); return rc; }
     *out = s;
     return 0;
 }
 
-int sort_reset(SortState* s, cudaStream_t, std::string&) {
-    for (auto& p : s->pool) { p.n = 0; p.cur = 0; }
+void sort_reset(SortState* s) {
+    for (auto& P : s->pool) { P.n = 0; P.cur = 0; }
     s->ret_rows = 0; s->total_seen = 0;
     s->row_base = s->region_base;
-    return 0;
 }
 
-int sort_push(SortState* s, const DevCol* cols, int64_t nrows, cudaStream_t stream, bkgpu_stats* stats, std::string& err) {
-    if (nrows > 0x7FFFFFFFll) return fail(err, BKGPU_EUNSUPPORTED, "a single pushed batch of a SORT/FILTER plan is limited to 2^31-1 rows");
+int sort_push(SortState* s, const DevCol* cols, int64_t nrows, bkgpu_stats* stats) {
+    if (nrows > 0x7FFFFFFFll) return s->p->fail(BKGPU_EUNSUPPORTED, "a single pushed batch of a SORT/FILTER plan is limited to 2^31-1 rows");
+    const cudaStream_t stream = s->p->stream;
     RowArgs ra; fill_row_args(s, cols, nrows, ra);
     int rc = 0;
     if (s->topk) {
         if (s->k == 0) { s->row_base += (uint64_t)nrows; return 0; }
         cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
         cudaEventRecord(e0, stream);
-        rc = select_topk_class(s, ra, 1, stream, stats, err);
+        rc = select_topk_class(s, ra, 1, stats);
         const bool need_nulls = ra.key.direct ? cols[ra.key.col].validity != nullptr : true;
-        if (!rc && need_nulls) rc = select_topk_class(s, ra, 2, stream, stats, err);
+        if (!rc && need_nulls) rc = select_topk_class(s, ra, 2, stats);
         cudaEventRecord(e1, stream); cudaEventSynchronize(e1);
         float ms = 0; cudaEventElapsedTime(&ms, e0, e1); cudaEventDestroy(e0); cudaEventDestroy(e1);
         stats->main_kernel_ms += ms; stats->main_kernel_launches += 1;
         stats->main_kernel_bytes += nrows * (ra.key.direct ? storage_bytes(cols[ra.key.col].stype) : 8);
         snprintf(stats->main_kernel_name, sizeof stats->main_kernel_name, "%s", s->used_vec ? "topk_select(k_collect_rows_vec)" : "topk_select(k_collect_rows)");
     } else {
-        rc = retain_batch(s, ra, stream, stats, err);
+        rc = retain_batch(s, ra, stats);
         snprintf(stats->main_kernel_name, sizeof stats->main_kernel_name, "%s", s->c.kind == PK_FILTER ? "k_filter_write" : "radix_sort(k_rs_pass)");
     }
     s->row_base += (uint64_t)nrows; s->total_seen += nrows;
@@ -853,7 +838,9 @@ struct HostRows {
 
 // the k surviving rows of both pools (keys present / NULL keys) land in ONE pinned staging block: every copy is truly
 // asynchronous and the whole result costs a single synchronisation
-static int topk_host_rows(SortState* s, HostRows& h, cudaStream_t st, std::string& err) {
+static int topk_host_rows(SortState* s, HostRows& h) {
+    bkgpu_plan* p = s->p;
+    const cudaStream_t st = p->stream;
     h.vals.assign((size_t)s->ncols, {}); h.nulls.assign((size_t)s->ncols, {});
     size_t row_bytes = 16;
     for (int c = 0; c < s->ncols; c++) row_bytes += (size_t)elem_bytes_of(s->c.cols[(size_t)c].prim) + 1;
@@ -862,35 +849,35 @@ static int topk_host_rows(SortState* s, HostRows& h, cudaStream_t st, std::strin
     if (s->h_stage_cap < need) {
         if (s->h_stage) cudaFreeHost(s->h_stage);
         s->h_stage = nullptr; s->h_stage_cap = 0;
-        SCK(cudaHostAlloc((void**)&s->h_stage, need * 2, cudaHostAllocDefault));
+        CK(p, cudaHostAlloc((void**)&s->h_stage, need * 2, cudaHostAllocDefault));
         s->h_stage_cap = need * 2;
     }
     struct Seg { size_t key, idx; std::vector<size_t> val, nul; } seg[2];
     size_t off = 0;
     auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 63) & ~(size_t)63; return o; };
-    for (int p = 0; p < 2; p++) {
-        Pool& P = s->pool[p];
+    for (int q = 0; q < 2; q++) {
+        Pool& P = s->pool[q];
         const size_t n = P.n;
         if (!n) continue;
-        seg[p].key = take(n * 8); seg[p].idx = take(n * 8);
-        SCK(cudaMemcpyAsync(s->h_stage + seg[p].key, P.key[P.cur], n * 8, cudaMemcpyDeviceToHost, st));
-        SCK(cudaMemcpyAsync(s->h_stage + seg[p].idx, P.idx[P.cur], n * 8, cudaMemcpyDeviceToHost, st));
+        seg[q].key = take(n * 8); seg[q].idx = take(n * 8);
+        CK(p, cudaMemcpyAsync(s->h_stage + seg[q].key, P.key[P.cur], n * 8, cudaMemcpyDeviceToHost, st));
+        CK(p, cudaMemcpyAsync(s->h_stage + seg[q].idx, P.idx[P.cur], n * 8, cudaMemcpyDeviceToHost, st));
         for (int c = 0; c < s->ncols; c++) {
             const size_t eb = (size_t)elem_bytes_of(s->c.cols[(size_t)c].prim);
-            seg[p].val.push_back(take(n * eb)); seg[p].nul.push_back(take(n));
-            SCK(cudaMemcpyAsync(s->h_stage + seg[p].val.back(), P.vals[P.cur][c], n * eb, cudaMemcpyDeviceToHost, st));
-            SCK(cudaMemcpyAsync(s->h_stage + seg[p].nul.back(), P.nulls[P.cur][c], n, cudaMemcpyDeviceToHost, st));
+            seg[q].val.push_back(take(n * eb)); seg[q].nul.push_back(take(n));
+            CK(p, cudaMemcpyAsync(s->h_stage + seg[q].val.back(), P.vals[P.cur][c], n * eb, cudaMemcpyDeviceToHost, st));
+            CK(p, cudaMemcpyAsync(s->h_stage + seg[q].nul.back(), P.nulls[P.cur][c], n, cudaMemcpyDeviceToHost, st));
         }
     }
-    SCK(cudaStreamSynchronize(st));
-    for (int p = 0; p < 2; p++) {
-        const size_t n = s->pool[p].n;
+    CK(p, cudaStreamSynchronize(st));
+    for (int q = 0; q < 2; q++) {
+        const size_t n = s->pool[q].n;
         if (!n) continue;
-        const uint64_t* key = (const uint64_t*)(s->h_stage + seg[p].key); const uint64_t* idx = (const uint64_t*)(s->h_stage + seg[p].idx);
-        for (size_t i = 0; i < n; i++) { h.cls.push_back((uint8_t)(p + 1)); h.key.push_back(key[i]); h.idx.push_back(idx[i]); }
+        const uint64_t* key = (const uint64_t*)(s->h_stage + seg[q].key); const uint64_t* idx = (const uint64_t*)(s->h_stage + seg[q].idx);
+        for (size_t i = 0; i < n; i++) { h.cls.push_back((uint8_t)(q + 1)); h.key.push_back(key[i]); h.idx.push_back(idx[i]); }
         for (int c = 0; c < s->ncols; c++) {
             const size_t eb = (size_t)elem_bytes_of(s->c.cols[(size_t)c].prim);
-            const uint8_t* v = s->h_stage + seg[p].val[(size_t)c]; const uint8_t* nb = s->h_stage + seg[p].nul[(size_t)c];
+            const uint8_t* v = s->h_stage + seg[q].val[(size_t)c]; const uint8_t* nb = s->h_stage + seg[q].nul[(size_t)c];
             h.vals[(size_t)c].insert(h.vals[(size_t)c].end(), v, v + n * eb);
             h.nulls[(size_t)c].insert(h.nulls[(size_t)c].end(), nb, nb + n);
         }
@@ -963,70 +950,74 @@ static void unpack_rows(SortState* s, const uint64_t* buf, HostRows& h) {
     }
 }
 
-int sort_partial_export(SortState* s, void* dev_dst, cudaStream_t st, std::string& err) {
-    if (!s->topk) return fail(err, BKGPU_EUNSUPPORTED, "only ORDER BY ... LIMIT plans have a partial state");
-    HostRows h; int rc = topk_host_rows(s, h, st, err);
+int sort_partial_export(SortState* s, void* dev_dst) {
+    bkgpu_plan* p = s->p;
+    if (!s->topk) return p->fail(BKGPU_EUNSUPPORTED, "only ORDER BY ... LIMIT plans have a partial state");
+    HostRows h; int rc = topk_host_rows(s, h);
     if (rc) return rc;
     std::vector<uint64_t> buf; pack_rows(s, h, buf);
-    SCK(cudaMemcpyAsync(dev_dst, buf.data(), buf.size() * 8, cudaMemcpyHostToDevice, st));
-    SCK(cudaStreamSynchronize(st));
+    CK(p, cudaMemcpyAsync(dev_dst, buf.data(), buf.size() * 8, cudaMemcpyHostToDevice, p->stream));
+    CK(p, cudaStreamSynchronize(p->stream));
     return 0;
 }
 
-int sort_partial_merge(SortState* s, const void* dev_src, int nranks, cudaStream_t st, std::vector<SortOutCol>& out, int64_t* nrows, std::string& err) {
-    if (!s->topk) return fail(err, BKGPU_EUNSUPPORTED, "only ORDER BY ... LIMIT plans have a partial state");
+int sort_partial_merge(SortState* s, const void* dev_src, int nranks, std::vector<SortOutCol>& out, int64_t* nrows) {
+    bkgpu_plan* p = s->p;
+    if (!s->topk) return p->fail(BKGPU_EUNSUPPORTED, "only ORDER BY ... LIMIT plans have a partial state");
     const size_t words = sort_partial_bytes(s) / 8;
     std::vector<uint64_t> all(words * (size_t)nranks);
-    SCK(cudaMemcpyAsync(all.data(), dev_src, all.size() * 8, cudaMemcpyDeviceToHost, st));
-    SCK(cudaStreamSynchronize(st));
+    CK(p, cudaMemcpyAsync(all.data(), dev_src, all.size() * 8, cudaMemcpyDeviceToHost, p->stream));
+    CK(p, cudaStreamSynchronize(p->stream));
     HostRows h;
     for (int r = 0; r < nranks; r++) unpack_rows(s, all.data() + (size_t)r * words, h);
     finish_host_rows(s, h, out, nrows);   // SelectManagerNode's merge of per-region sorted runs (select_manager_node.cpp:50-51)
     return 0;
 }
 
-int sort_finish(SortState* s, void* nccl_comm, int nranks, cudaStream_t st, bkgpu_stats* stats, std::vector<SortOutCol>& out, int64_t* nrows, std::string& err) {
+int sort_finish(SortState* s, void* nccl_comm, int nranks, bkgpu_stats* stats, std::vector<SortOutCol>& out, int64_t* nrows) {
+    bkgpu_plan* p = s->p;
+    const cudaStream_t st = p->stream;
     if (s->topk) {
-        HostRows h; int rc = topk_host_rows(s, h, st, err);
+        HostRows h; int rc = topk_host_rows(s, h);
         if (rc) return rc;
         if (nccl_comm && nranks > 1) {   // per-GPU top-k rows meet in one all-gather; every rank finishes the merge
             std::vector<uint64_t> buf; pack_rows(s, h, buf);
+            DevScope scope(p);
             uint64_t *d_send = nullptr, *d_recv = nullptr;
-            if ((rc = dalloc(s, &d_send, buf.size() * 8, err))) return rc;
-            if ((rc = dalloc(s, &d_recv, buf.size() * 8 * (size_t)nranks, err))) return rc;
+            if ((rc = scope.alloc(&d_send, buf.size() * 8))) return rc;
+            if ((rc = scope.alloc(&d_recv, buf.size() * 8 * (size_t)nranks))) return rc;
             cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-            SCK(cudaMemcpyAsync(d_send, buf.data(), buf.size() * 8, cudaMemcpyHostToDevice, st));
+            CK(p, cudaMemcpyAsync(d_send, buf.data(), buf.size() * 8, cudaMemcpyHostToDevice, st));
             cudaEventRecord(e0, st);
-            if (nccl_all_gather(nccl_comm, d_send, d_recv, buf.size(), st) != 0) { err = std::string("ncclAllGather: ") + nccl_last_error(); return BKGPU_ENCCL; }
+            if (nccl_all_gather(nccl_comm, d_send, d_recv, buf.size(), st) != 0) return p->fail(BKGPU_ENCCL, "ncclAllGather: %s", nccl_last_error());
             cudaEventRecord(e1, st);
-            rc = sort_partial_merge(s, d_recv, nranks, st, out, nrows, err);
+            rc = sort_partial_merge(s, d_recv, nranks, out, nrows);
             float ms = 0; cudaEventElapsedTime(&ms, e0, e1); stats->collective_ms += ms; cudaEventDestroy(e0); cudaEventDestroy(e1);
-            dfree(s, d_send); dfree(s, d_recv);
             return rc;
         }
         finish_host_rows(s, h, out, nrows);
         return 0;
     }
-    if (nccl_comm && nranks > 1) return fail(err, BKGPU_EUNSUPPORTED, "multi-GPU merge is implemented for ORDER BY ... LIMIT (top-k) and aggregates");
+    if (nccl_comm && nranks > 1) return p->fail(BKGPU_EUNSUPPORTED, "multi-GPU merge is implemented for ORDER BY ... LIMIT (top-k) and aggregates");
     if (s->c.kind == PK_FILTER) {
         int64_t n = s->ret_rows;
         int64_t skip = std::min<int64_t>(s->c.offset, n);
         n -= skip;
         *nrows = n;
-        return copy_out(s, s->ret_vals.data(), s->ret_null.data(), nullptr, n, skip, st, out, err);
+        return copy_out(s, s->ret_vals.data(), s->ret_null.data(), nullptr, n, skip, out);
     }
     // ---- full ORDER BY: stable LSD radix sort of (key image, row id) pairs, least significant ORDER BY key first ----
     const int64_t n = s->ret_rows;
-    if (n > RADIX_MAX_KEYS) return fail(err, BKGPU_EUNSUPPORTED, "full sort is limited to 2^30 - 1 rows per GPU");
-    if (n == 0) { *nrows = 0; return copy_out(s, s->ret_vals.data(), s->ret_null.data(), nullptr, 0, 0, st, out, err); }
-    RadixBufs b; int rc;
-    if ((rc = radix_alloc(s, n, b, err))) return rc;
+    if (n > RADIX_MAX_KEYS) return p->fail(BKGPU_EUNSUPPORTED, "full sort is limited to 2^30 - 1 rows per GPU");
+    if (n == 0) { *nrows = 0; return copy_out(s, s->ret_vals.data(), s->ret_null.data(), nullptr, 0, 0, out); }
+    RadixBufs b(p); int rc;
+    if ((rc = b.alloc(n))) return rc;
     RowArgs ra; memset(&ra, 0, sizeof ra);
     // retained columns carry null BYTES: pack them into bitmaps on the device so the key program sees NULLs
-    std::vector<uint8_t*> bitmaps; uint32_t h_null_flags[MAX_COLS] = {0};
-    if ((rc = retained_bitmaps(s, st, ra, bitmaps, h_null_flags, err))) return rc;
+    DevScope bitmaps(p); uint32_t h_null_flags[MAX_COLS] = {0};
+    if ((rc = retained_bitmaps(s, bitmaps, ra, h_null_flags))) return rc;
     ra.prog = s->c.prog; ra.key.pred_out = -1;
-    k_iota<<<grid_for(n, s->sm_count, 8), 256, 0, st>>>(b.ids[0], n);
+    k_iota<<<grid_for(n, p->sm_count, 8), 256, 0, st>>>(b.ids[0], n);
     int cur = 0;
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
     cudaEventRecord(e0, st);
@@ -1035,77 +1026,70 @@ int sort_finish(SortState* s, void* nccl_comm, int nranks, cudaStream_t st, bkgp
     const bool direct_key = s->c.has_direct && s->c.sort_keys.size() == 1 && !s->c.direct_cols.empty();
     const int dcol = direct_key ? s->c.direct_cols[0] : -1;
     std::vector<const Program*> progs(s->c.sort_keys.size(), &s->c.prog);
-    if ((rc = radix_sort_keys(s, ra, s->c.sort_keys, progs, dcol, dcol >= 0 && h_null_flags[dcol], b, cur, true, st, stats, pass_bytes, err))) return rc;
+    if ((rc = radix_sort_keys(s, ra, s->c.sort_keys, progs, dcol, dcol >= 0 && h_null_flags[dcol], b, cur, true, stats, pass_bytes))) return rc;
     cudaEventRecord(e1, st);
-    SCK(cudaStreamSynchronize(st));
+    CK(p, cudaStreamSynchronize(st));
     { float ms = 0; cudaEventElapsedTime(&ms, e0, e1); stats->main_kernel_ms += ms; stats->main_kernel_launches += 1; stats->main_kernel_bytes += pass_bytes; }
     cudaEventDestroy(e0); cudaEventDestroy(e1);
     snprintf(stats->main_kernel_name, sizeof stats->main_kernel_name, "%s", "radix_sort(k_rs_pass)");
     int64_t keep = n; if (s->k >= 0 && keep > s->k) keep = s->k;
     int64_t skip = std::min<int64_t>(s->c.offset, keep); keep -= skip;
     *nrows = keep;
-    rc = copy_out(s, s->ret_vals.data(), s->ret_null.data(), b.ids[cur], keep, skip, st, out, err);
-    radix_free(s, b);
-    for (auto bm : bitmaps) dfree(s, bm);
-    return rc;
+    return copy_out(s, s->ret_vals.data(), s->ret_null.data(), b.ids[cur], keep, skip, out);
 }
 
 // ---- the window stage's access to the retained rows and the radix sort (window.cu) ----
-int sort_retained_cols(SortState* s, cudaStream_t st, std::vector<DevCol>& cols, std::vector<void*>& scratch, int64_t* nrows, std::string& err) {
+int sort_retained_cols(SortState* s, DevScope& scope, std::vector<DevCol>& cols, int64_t* nrows) {
     RowArgs ra; memset(&ra, 0, sizeof ra);
-    std::vector<uint8_t*> bitmaps; uint32_t h_null_flags[MAX_COLS] = {0};
-    int rc = retained_bitmaps(s, st, ra, bitmaps, h_null_flags, err);
+    uint32_t h_null_flags[MAX_COLS] = {0};
+    int rc = retained_bitmaps(s, scope, ra, h_null_flags);
     if (rc) return rc;
     cols.assign(ra.cols, ra.cols + s->ncols);
-    for (auto bm : bitmaps) scratch.push_back(bm);
     *nrows = s->ret_rows;
     return 0;
 }
 
-int sort_retained_raw(SortState* s, std::vector<uint8_t*>& vals, std::vector<uint8_t*>& nulls) {
-    vals = s->ret_vals; nulls = s->ret_null;
-    return 0;
-}
-
-void sort_free_scratch(SortState* s, std::vector<void*>& scratch) { for (void* p : scratch) dfree(s, p); scratch.clear(); }
+void sort_retained_raw(SortState* s, std::vector<uint8_t*>& vals, std::vector<uint8_t*>& nulls) { vals = s->ret_vals; nulls = s->ret_null; }
 
 int sort_stable_ids(SortState* s, const DevCol* cols, int64_t n, const std::vector<SortKey>& keys, const std::vector<const Program*>& progs,
-                    uint32_t* ids, cudaStream_t st, bkgpu_stats* stats, std::string& err) {
+                    uint32_t* ids, bkgpu_stats* stats) {
     if (n == 0 || keys.empty()) return 0;
-    RadixBufs b; int rc;
-    if ((rc = radix_alloc(s, n, b, err))) return rc;
+    bkgpu_plan* p = s->p;
+    RadixBufs b(p); int rc;
+    if ((rc = b.alloc(n))) return rc;
     RowArgs ra; memset(&ra, 0, sizeof ra);
     for (int c = 0; c < s->ncols; c++) ra.cols[c] = cols[c];
     ra.n_cols = s->ncols; ra.nrows = n; ra.key.pred_out = -1;
-    SCK(cudaMemcpyAsync(b.ids[0], ids, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
+    CK(p, cudaMemcpyAsync(b.ids[0], ids, (size_t)n * 4, cudaMemcpyDeviceToDevice, p->stream));
     int cur = 0; int64_t pass_bytes = 0;
-    if ((rc = radix_sort_keys(s, ra, keys, progs, -1, true, b, cur, false, st, stats, pass_bytes, err))) return rc;
-    SCK(cudaMemcpyAsync(ids, b.ids[cur], (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
-    SCK(cudaStreamSynchronize(st));
-    radix_free(s, b);
+    if ((rc = radix_sort_keys(s, ra, keys, progs, -1, true, b, cur, false, stats, pass_bytes))) return rc;
+    CK(p, cudaMemcpyAsync(ids, b.ids[cur], (size_t)n * 4, cudaMemcpyDeviceToDevice, p->stream));
+    CK(p, cudaStreamSynchronize(p->stream));
     return 0;
 }
 
 int sort_copy_rows(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, const std::vector<ColRef>& desc, const uint32_t* perm_dev, int64_t n, int64_t skip,
-                   cudaStream_t st, std::vector<SortOutCol>& out, std::string& err) {
-    return copy_cols_out(s, vals, nulls, desc, perm_dev, n, skip, st, out, err);
+                   std::vector<SortOutCol>& out) {
+    return copy_cols_out(s, vals, nulls, desc, perm_dev, n, skip, out);
 }
 
 int sort_gather_rows(SortState* s, const uint8_t* src_vals, const uint8_t* src_null, int prim, const uint32_t* perm_dev, int64_t n,
-                     uint8_t* dst_vals, uint8_t* dst_null, cudaStream_t st) {
+                     uint8_t* dst_vals, uint8_t* dst_null) {
     if (n <= 0) return 0;
+    const cudaStream_t st = s->p->stream;
+    const int sm = s->p->sm_count;
     GatherArgs g; memset(&g, 0, sizeof g);
     g.cols[0].values = src_vals; g.cols[0].validity = nullptr; g.cols[0].stype = prim_storage(prim); g.cols[0].prim = prim;
     g.n_cols = 1; g.dst_vals[0] = dst_vals; g.dst_null[0] = dst_null;
-    k_gather_sel<<<grid_for(n, s->sm_count, 8), 256, 0, st>>>(g, perm_dev, (uint64_t)n, 0);
+    k_gather_sel<<<grid_for(n, sm, 8), 256, 0, st>>>(g, perm_dev, (uint64_t)n, 0);
     // null bytes travel separately (k_gather_sel reads validity bitmaps, retained columns hold null BYTES)
-    k_rs_gather_bytes<<<grid_for(n, s->sm_count, 8), 256, 0, st>>>(src_null, perm_dev, dst_null, (uint64_t)n);
+    k_rs_gather_bytes<<<grid_for(n, sm, 8), 256, 0, st>>>(src_null, perm_dev, dst_null, (uint64_t)n);
     return cudaGetLastError() == cudaSuccess ? 0 : BKGPU_ENODEV;
 }
 
+// (the device buffers belong to the plan: bkgpu_close returns them)
 void sort_close(SortState* s) {
     if (!s) return;
-    for (void* p : s->allocs) cudaFree(p);
     if (s->h_stage) cudaFreeHost(s->h_stage);
     if (s->h_counts) cudaFreeHost(s->h_counts);
     delete s;

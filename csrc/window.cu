@@ -16,6 +16,7 @@
 #include "window.h"
 #include <algorithm>
 #include <string.h>
+#include "api_state.h"
 #include "dev_common.cuh"
 #include "interp.cuh"
 #include "prims.cuh"
@@ -308,22 +309,10 @@ __global__ void k_win_fn(FnArgs a) {
 
 
 // the stage timer's two events, destroyed on every way out of window_finish
-struct EventPair {
+struct StageTimer {
     cudaEvent_t a = nullptr, b = nullptr;
-    EventPair() { cudaEventCreate(&a); cudaEventCreate(&b); }
-    ~EventPair() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); }
-};
-
-// device allocations of one window_finish call, released together when it returns (also on an error path)
-struct Arena {
-    std::vector<void*> p;
-    ~Arena() { for (void* x : p) cudaFree(x); }
-    template <class T> cudaError_t get(T** out, size_t bytes) {
-        cudaError_t e = cudaMalloc((void**)out, bytes ? bytes : 8);
-        if (e == cudaSuccess) p.push_back(*out);
-        return e;
-    }
-    void drop(void* x) { auto it = std::find(p.begin(), p.end(), x); if (it != p.end()) { cudaFree(x); p.erase(it); } }
+    StageTimer() { cudaEventCreate(&a); cudaEventCreate(&b); }
+    ~StageTimer() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); }
 };
 
 struct ScanBufs { Acc* agg = nullptr; Acc* carry = nullptr; uint32_t ntiles = 0; };
@@ -349,41 +338,42 @@ void run_scan(int op, const ScanIn& in, const ScanBufs& b, uint64_t* out_v, uint
 
 }  // namespace
 
-int window_finish(const Compiled& c, SortState* rows, SortState* post, cudaStream_t st, bkgpu_stats* stats,
-                  std::vector<SortOutCol>& out, int64_t* nrows, std::string& err) {
-    int sm = 132;
-    { int dev = 0, v = 0; if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) sm = v; }
-    Arena ar;
-    std::vector<DevCol> cols; std::vector<void*> bitmaps; int64_t n = 0; int rc;
-    if ((rc = sort_retained_cols(rows, st, cols, bitmaps, &n, err))) return rc;
-    struct Release { SortState* s; std::vector<void*>& b; ~Release() { sort_free_scratch(s, b); } } release{rows, bitmaps};
-    if (n > RADIX_MAX_KEYS) { err = "a window fragment is limited to 2^30 - 1 rows per GPU"; return BKGPU_EUNSUPPORTED; }
+int window_finish(bkgpu_plan* p, std::vector<SortOutCol>& out, int64_t* nrows) {
+    const Compiled& c = p->c;
+    SortState* rows = p->sort;
+    const cudaStream_t st = p->stream;
+    const int sm = p->sm_count;
+    bkgpu_stats* stats = &p->stats;
+    DevScope ar(p);   // every device buffer of the call
+    std::vector<DevCol> cols; int64_t n = 0; int rc;
+    if ((rc = sort_retained_cols(rows, ar, cols, &n))) return rc;
+    if (n > RADIX_MAX_KEYS) return p->fail(BKGPU_EUNSUPPORTED, "a window fragment is limited to 2^30 - 1 rows per GPU");
     const int ncols = (int)cols.size();
     uint32_t* perm = nullptr;
-    SCK(ar.get(&perm, (size_t)n * 4));
+    if ((rc = ar.alloc(&perm, (size_t)n * 4))) return rc;
     if (n) k_iota<<<grid_for(n, sm, 8), 256, 0, st>>>(perm, n);
     // window outputs, in row space
     std::vector<uint8_t*> wvals, wnull;
     for (const WinStage& w : c.win)
         for (const WinFn& f : w.fns) {
             uint8_t *v = nullptr, *nb = nullptr;
-            SCK(ar.get(&v, (size_t)std::max<int64_t>(n, 1) * storage_bytes(prim_storage(f.out_prim))));
-            SCK(ar.get(&nb, (size_t)std::max<int64_t>(n, 1)));
+            if ((rc = ar.alloc(&v, (size_t)std::max<int64_t>(n, 1) * storage_bytes(prim_storage(f.out_prim)))) || (rc = ar.alloc(&nb, (size_t)std::max<int64_t>(n, 1))))
+                return rc;
             wvals.push_back(v); wnull.push_back(nb);
         }
-    EventPair ev_pair;
-    cudaEvent_t e0 = ev_pair.a, e1 = ev_pair.b;
+    StageTimer timer;
+    cudaEvent_t e0 = timer.a, e1 = timer.b;
     float win_ms = 0; int64_t win_bytes = 0, win_launches = 0;
     size_t fn_index = 0;
     const uint32_t ntiles = (uint32_t)((n + SC_TILE - 1) / SC_TILE);
     ScanBufs sb; sb.ntiles = ntiles;
-    SCK(ar.get(&sb.agg, (size_t)std::max<uint32_t>(ntiles, 1) * sizeof(Acc)));
-    SCK(ar.get(&sb.carry, (size_t)std::max<uint32_t>(ntiles, 1) * sizeof(Acc)));
+    if ((rc = ar.alloc(&sb.agg, (size_t)std::max<uint32_t>(ntiles, 1) * sizeof(Acc))) || (rc = ar.alloc(&sb.carry, (size_t)std::max<uint32_t>(ntiles, 1) * sizeof(Acc))))
+        return rc;
     for (const WinStage& w : c.win) {
         if (w.new_sort && n > 0) {   // stable radix sort of the current order by the stage's keys (each key: output 0 of its own program)
             std::vector<SortKey> keys; std::vector<const Program*> progs;
             for (const SortKey& k : w.sort_keys) { keys.push_back({0, k.prim, k.asc, k.null_first}); progs.push_back(&w.exprs[(size_t)k.out_reg]); }
-            if ((rc = sort_stable_ids(rows, cols.data(), n, keys, progs, perm, st, stats, err))) return rc;
+            if ((rc = sort_stable_ids(rows, cols.data(), n, keys, progs, perm, stats))) return rc;
         }
         if (n == 0) { fn_index += w.fns.size(); continue; }
         cudaEventRecord(e0, st);
@@ -393,14 +383,14 @@ int window_finish(const Compiled& c, SortState* rows, SortState* post, cudaStrea
         for (int k = 0; k < ncols; k++) ea.cols[k] = cols[(size_t)k];
         ea.n_cols = ncols; ea.nrows = n;
         for (size_t e = 0; e < w.exprs.size(); e++) {
-            SCK(ar.get(&ev[e], (size_t)n * 8)); SCK(ar.get(&en[e], (size_t)n));
+            if ((rc = ar.alloc(&ev[e], (size_t)n * 8)) || (rc = ar.alloc(&en[e], (size_t)n))) return rc;
             ea.prog = w.exprs[e];
             k_win_eval<<<grid_for(n, sm, 8), 256, 0, st>>>(ea, perm, ev[e], en[e]);
             win_launches++; win_bytes += n * (4 + 9);
         }
         // 2. partition / peer starts
         uint8_t *part = nullptr, *peer = nullptr;
-        SCK(ar.get(&part, (size_t)n + 1)); SCK(ar.get(&peer, (size_t)n + 1));
+        if ((rc = ar.alloc(&part, (size_t)n + 1)) || (rc = ar.alloc(&peer, (size_t)n + 1))) return rc;
         KeyCmp kc; memset(&kc, 0, sizeof kc);
         kc.n_part = w.n_part; kc.n_keys = (int)w.sort_keys.size();
         for (int k = 0; k < kc.n_keys; k++) {
@@ -411,7 +401,8 @@ int window_finish(const Compiled& c, SortState* rows, SortState* post, cudaStrea
         win_launches++; win_bytes += n * (9 * 2 * kc.n_keys + 2);
         // 3. partition and peer-group bounds: the first index of the segment, forward and backward
         uint64_t *ps = nullptr, *pl = nullptr, *qs = nullptr, *ql = nullptr;
-        SCK(ar.get(&ps, (size_t)n * 8)); SCK(ar.get(&pl, (size_t)n * 8)); SCK(ar.get(&qs, (size_t)n * 8)); SCK(ar.get(&ql, (size_t)n * 8));
+        if ((rc = ar.alloc(&ps, (size_t)n * 8)) || (rc = ar.alloc(&pl, (size_t)n * 8)) || (rc = ar.alloc(&qs, (size_t)n * 8)) || (rc = ar.alloc(&ql, (size_t)n * 8)))
+            return rc;
         auto index_scan = [&](const uint8_t* seg, int rev, uint64_t* dst) {
             ScanIn in; memset(&in, 0, sizeof in);
             in.seg = seg; in.n = (uint32_t)n; in.rev = rev; in.mode = SM_INDEX;
@@ -433,7 +424,7 @@ int window_finish(const Compiled& c, SortState* rows, SortState* post, cudaStrea
             fa.perm = perm; fa.out_vals = wvals[fn_index]; fa.out_null = wnull[fn_index]; fa.out_stype = prim_storage(f.out_prim);
             const bool scanned = (f.kind <= WF_MAX && (f.method == WM_FWD || f.method == WM_BWD || f.method == WM_PEER)) || (f.kind == WF_DENSE_RANK && fa.has_order);
             if (scanned) {
-                if (!sv) { SCK(ar.get(&sv, (size_t)n * 8)); SCK(ar.get(&sc, (size_t)n * 8)); }
+                if (!sv && ((rc = ar.alloc(&sv, (size_t)n * 8)) || (rc = ar.alloc(&sc, (size_t)n * 8)))) return rc;
                 ScanIn in; memset(&in, 0, sizeof in);
                 in.n = (uint32_t)n; in.vclass = fa.arg_vclass;
                 int op;
@@ -454,13 +445,12 @@ int window_finish(const Compiled& c, SortState* rows, SortState* post, cudaStrea
             fn_index++;
         }
         cudaEventRecord(e1, st);
-        SCK(cudaEventSynchronize(e1));
+        CK(p, cudaEventSynchronize(e1));
         float ms = 0; cudaEventElapsedTime(&ms, e0, e1); win_ms += ms;
-        for (size_t e = 0; e < ev.size(); e++) { ar.drop(ev[e]); ar.drop(en[e]); }
-        ar.drop(part); ar.drop(peer); ar.drop(ps); ar.drop(pl); ar.drop(qs); ar.drop(ql);
-        if (sv) { ar.drop(sv); ar.drop(sc); }
+        for (size_t e = 0; e < ev.size(); e++) { ar.release(ev[e]); ar.release(en[e]); }
+        for (void* b : {(void*)part, (void*)peer, (void*)ps, (void*)pl, (void*)qs, (void*)ql, (void*)sv, (void*)sc}) ar.release(b);
     }
-    SCK(cudaGetLastError());
+    CK(p, cudaGetLastError());
     stats->main_kernel_ms += win_ms; stats->main_kernel_launches += 1; stats->main_kernel_bytes += win_bytes;
     stats->kernel_launches += win_launches;
     snprintf(stats->main_kernel_name, sizeof stats->main_kernel_name, "%s", "window_stage(k_win_fn)");
@@ -471,33 +461,34 @@ int window_finish(const Compiled& c, SortState* rows, SortState* post, cudaStrea
     all_v.insert(all_v.end(), wvals.begin(), wvals.end()); all_n.insert(all_n.end(), wnull.begin(), wnull.end());
     std::vector<ColRef> desc;
     for (const OutCol& oc : c.out_cols) desc.push_back({oc.tuple_id, oc.slot_id, oc.prim});
+    SortState* post = p->post_sort;
     if (!post) {
         int64_t keep = n;
         if (c.limit >= 0 && keep > c.limit) keep = c.limit;
         const int64_t skip = std::min<int64_t>(c.offset, keep);
         keep -= skip;
         *nrows = keep;
-        return sort_copy_rows(rows, all_v.data(), all_n.data(), desc, perm, keep, skip, st, out, err);
+        return sort_copy_rows(rows, all_v.data(), all_n.data(), desc, perm, keep, skip, out);
     }
     // the query's ORDER BY: the window rows in their order, as device columns, through the post fragment's sort
-    if ((rc = sort_reset(post, st, err))) return rc;
+    sort_reset(post);
     if (n > 0) {
         std::vector<DevCol> dc(desc.size());
         for (size_t k = 0; k < desc.size(); k++) {
             const int eb = storage_bytes(prim_storage(desc[k].prim));
             uint8_t *v = nullptr, *nb = nullptr, *bm = nullptr;
-            SCK(ar.get(&v, (size_t)n * eb)); SCK(ar.get(&nb, (size_t)n)); SCK(ar.get(&bm, (size_t)(n + 7) / 8 + 64));
-            if ((rc = sort_gather_rows(rows, all_v[k], all_n[k], desc[k].prim, perm, n, v, nb, st))) { err = "window output gather failed"; return rc; }
+            if ((rc = ar.alloc(&v, (size_t)n * eb)) || (rc = ar.alloc(&nb, (size_t)n)) || (rc = ar.alloc(&bm, (size_t)(n + 7) / 8 + 64))) return rc;
+            if ((rc = sort_gather_rows(rows, all_v[k], all_n[k], desc[k].prim, perm, n, v, nb))) return p->fail(rc, "window output gather failed");
             k_pack_null_bytes<<<grid_for((n + 7) / 8, sm, 8), 256, 0, st>>>(nb, n, bm, nullptr);
             dc[k].values = v; dc[k].validity = bm; dc[k].stype = prim_storage(desc[k].prim); dc[k].prim = desc[k].prim;
         }
-        SCK(cudaGetLastError());
+        CK(p, cudaGetLastError());
         bkgpu_stats scratch{};   // (the post fragment's kernels are not the request's main kernel)
-        if ((rc = sort_push(post, dc.data(), n, st, &scratch, err))) return rc;
+        if ((rc = sort_push(post, dc.data(), n, &scratch))) return rc;
         stats->kernel_launches += scratch.kernel_launches;
     }
     bkgpu_stats scratch{};
-    rc = sort_finish(post, nullptr, 1, st, &scratch, out, nrows, err);
+    rc = sort_finish(post, nullptr, 1, &scratch, out, nrows);
     stats->kernel_launches += scratch.kernel_launches;
     return rc;
 }

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""ab.py — A/B of two builds of libbkgpu.so over the aggregate and hash-join plans: each build runs the same seeded plans in its own
+"""ab.py — A/B of two builds of libbkgpu.so over the aggregate, hash-join, ORDER BY / filter, window and rb_build_agg plans: each build runs the same seeded plans in its own
 process (BKGPU_LIB is read when the library is loaded), and the two dumps are compared.
 
     BKGPU_LIB=/path/a/libbkgpu.so python profiles/ab.py run a.json
@@ -7,7 +7,7 @@ process (BKGPU_LIB is read when the library is loaded), and the two dumps are co
     python profiles/ab.py compare a.json b.json
 
 Per run the dump keeps the counters kernel_launches, main_kernel_name, h2d_bytes and d2h_bytes, and the result columns.  The comparison
-wants the same counters, the same group keys and integers, bit-identical doubles for the tables of tests/join_key_cases.py (their sums
+wants the same counters, the same group keys, integers and bitmap bytes, bit-identical doubles for the tables of tests/join_key_cases.py (their sums
 are integer-valued) and 1e-9 relative for other double sums (adds through global atomics are not ordered).  That includes the lean
 kernel's FX variant: its fixed-point limbs are exact within a CTA, but the CTAs flush their sums into the global table as double atomics,
 so two runs of the same build differ in the last bits."""
@@ -262,6 +262,65 @@ def scalar_sum():
     return scalar_sum_plan(), [[datagen.c2_table(0, 4_000_000)]] * 2, {}
 
 
+# ---- ORDER BY / top-k / filter-only, the window stage, rb_build_agg: sort.cu, window.cu, rb.cu ----
+def chunks(cols, cuts):
+    return [[make_column(c.tuple_id, c.slot_id, c.prim_type, c.values[a:b], None if c.valid is None else c.valid[a:b]) for c in cols]
+            for a, b in zip(cuts, cuts[1:])]
+
+
+@case(None, ordered=True)
+def filter_limit_offset_host_chunks():
+    rng = np.random.default_rng(19)
+    n = 600_000
+    cols = [make_column(0, 1, T.INT64, rng.integers(0, 100, n)), make_column(0, 2, T.INT32, np.arange(n, dtype=np.int32), rng.random(n) > 0.2)]
+    conj = P.and_(P.gt(P.slot_ref(0, 1, T.INT64), P.int_lit(90)), P.not_(P.is_null(P.slot_ref(0, 2, T.INT32))))
+    pl = P.Plan(P.limit(P.where(P.scan(0), conj), 30_000, 17), {0: [(1, T.INT64), (2, T.INT32)]})
+    batches = chunks(cols, [0, 250_000, 250_001, 600_000])
+    return pl, [batches, batches], {"chunk_rows": 40_000}   # host columns cross the staging buffers in 40k-row chunks
+
+
+@case(None, ordered=True)
+def full_sort_two_keys_nulls():
+    rng = np.random.default_rng(17)
+    n = 700_000
+    cols = [make_column(0, 1, T.INT64, rng.integers(0, 50, n), rng.random(n) > 0.05), make_column(0, 2, T.INT32, rng.integers(-5, 5, n), rng.random(n) > 0.1),
+            make_column(0, 3, T.DOUBLE, rng.normal(size=n))]
+    pl = P.Plan(P.sort(P.scan(0), [P.slot_ref(0, 1, T.INT64), P.slot_ref(0, 2, T.INT32)], [True, False], [False, True], tuple_id=0),
+                {0: [(1, T.INT64), (2, T.INT32), (3, T.DOUBLE)]})
+    return pl, [chunks(cols, [0, 300_000, n])] * 2, {}
+
+
+@case(None, ordered=True)
+def topk_null_keys():
+    rng = np.random.default_rng(5)
+    n = 2_000_000
+    cols = [make_column(0, 1, T.INT64, rng.integers(-1000, 1000, n), rng.random(n) > 0.01), make_column(0, 2, T.INT32, np.arange(n, dtype=np.int32))]
+    pl = P.Plan(P.sort(P.scan(0), [P.slot_ref(0, 1, T.INT64)], [True], [True], limit=700, tuple_id=0), {0: [(1, T.INT64), (2, T.INT32)]})
+    return pl, [[cols], chunks(cols, [0, 1_000_000, n])], {}
+
+
+@case(None, ordered=True)
+def window_stack_then_order_by():
+    from tests.test_gpu_window import FRAMES, SCAN, K, V, X, U, table
+    cols = table(19, 300_000, n_keys=250)
+    s0 = P.window_stage(P.scan(0), [P.window_expr("row_number", 1, 1), P.window_expr("lag", 1, 2, X)], [K], [V])
+    s1 = P.window_stage(s0, [P.window_expr("rank", 1, 3)], [U], [X], [False])
+    s2 = P.window_stage(s1, [P.window_expr("sum", 1, 4, X), P.window_expr("count", 1, 5, X)], [U], [X], [False], window_frame=FRAMES["rows_bounded"])
+    out = [(1, T.INT64), (2, T.DOUBLE), (3, T.INT64), (4, T.DOUBLE), (5, T.INT64)]
+    pl = P.Plan(P.limit(P.sort(s2, [P.slot_ref(1, 1, T.INT64), P.slot_ref(1, 4, T.DOUBLE)], [False, True], tuple_id=2), 50_000, 100), {0: SCAN, 1: out})
+    return pl, [[cols], [cols]], {}
+
+
+@case(["0_1"])
+def rb_compaction():
+    from tests import rb_cases
+    rng = np.random.default_rng(12)
+    n, g = 300_000, 10
+    cols = [make_column(0, 1, T.INT32, rng.integers(0, g, n).astype(np.int32)), make_column(0, 2, T.INT64, rng.integers(0, 150, n)),
+            make_column(0, 3, T.DOUBLE, rng.integers(0, 1000, n).astype(np.float64))]
+    return rb_cases.scan_plan(T.INT64, extra=True), [chunks(cols, list(range(0, n, 70_000)) + [n])] * 2, {"rb_pair_capacity": 4096}
+
+
 # ---- run ----
 def execute_runs(pl, runs, options):
     from baikaldb_b200._lib import BkgpuError
@@ -284,8 +343,9 @@ def execute_runs(pl, runs, options):
                 rc, eos = node.get_next(st, rb)
                 if rc < 0:
                     raise BkgpuError(rc, st.error_msg)
-                for c in rb.columns:   # (an AVG intermediate {double sum; int64 count} arrives as 16 bytes)
-                    cols.setdefault(c.name, []).extend([list(struct.unpack("<dq", v)) if isinstance(v, bytes) else v for v in c.to_list()])
+                for c in rb.columns:   # (a BITMAP arrives as its serialized bytes, an AVG intermediate {double sum; int64 count} as 16 bytes)
+                    unpack = (lambda v: v.hex()) if c.prim_type == T.BITMAP else (lambda v: list(struct.unpack("<dq", v)))
+                    cols.setdefault(c.name, []).extend([unpack(v) if isinstance(v, bytes) else v for v in c.to_list()])
             s = node.stats()
             out.append({"kernel_launches": s.kernel_launches, "main_kernel_name": s.main_kernel_name.decode(), "h2d_bytes": s.h2d_bytes,
                         "d2h_bytes": s.d2h_bytes, "columns": cols})
