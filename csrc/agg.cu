@@ -278,21 +278,6 @@ __global__ void k_table_clear(GroupTable gt, AggPlan ap, uint32_t n) {
     if (blockIdx.x == 0 && threadIdx.x < 3 && gt.hll_ctr) gt.hll_ctr[threadIdx.x] = 0;
 }
 
-// Partial state layout (fixed capacity `pcap` groups): [u64 n_groups][keys n_keyw x pcap][lanes n_lanes x pcap]
-__global__ void k_partial_export(GroupTable gt, AggPlan ap, uint64_t* dst, uint32_t pcap, uint32_t* cursor) {
-    const uint32_t cap = gt.cap_mask + 1;
-    uint64_t* dkeys = dst + 1;
-    uint64_t* dlanes = dkeys + (size_t)ap.n_keyw * pcap;
-    BK_FOR_EACH_GROUP(gt, ap, i) {
-        if (ap.n_keyw == 0 && gt.lanes[i] == 0) continue;  // no row reached the single group
-        const uint32_t pos = atomicAdd(cursor, 1u);
-        if (pos >= pcap) { atomicExch(gt.overflow, 1u); continue; }
-        for (int w = 0; w < ap.n_keyw; w++) dkeys[(size_t)w * pcap + pos] = gt.keys[(size_t)w * cap + i];
-        for (int l = 0; l < ap.n_lanes; l++) dlanes[(size_t)l * pcap + pos] = gt.lanes[(size_t)l * cap + i];
-    }
-}
-__global__ void k_partial_count(uint64_t* dst, const uint32_t* cursor, uint32_t pcap) { dst[0] = *cursor < pcap ? *cursor : pcap; }
-
 // Compact partial state for the all-gather (the default multi-GPU merge): dst[0] = the number of groups this rank holds (its low
 // half doubles as the export cursor, so it may exceed `bound`), followed by min(groups, bound) rows of n_keyw + n_lanes words.
 // Only `1 + bound * row words` cross NVLink; `bound` follows the group counts seen in earlier runs (api.cu).
@@ -371,62 +356,9 @@ __global__ void k_partial_merge_rows(GroupTable gt, AggPlan ap, const uint64_t* 
     }
 }
 
-// ---- merge over NVLink peer memory (option "peer_merge"): export, exchange and merge without a collective library call ----
-// Every rank owns one buffer [2 parities][nranks segments of the partial-state layout] + [2][nranks] sequence flags, mapped into
-// all peers through CUDA IPC.  k_peer_export writes this rank's groups straight into segment `rank` of EVERY peer's buffer,
-// k_peer_publish releases them (count, system-scope fence, sequence flag), k_peer_wait acquires the peers' flags, then the
-// ordinary K3 merge runs on the local buffer.  Parity = step & 1: a peer one step ahead writes the other half.
-__device__ __forceinline__ void st_release_sys(uint64_t* p, uint64_t v) { asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory"); }
-__device__ __forceinline__ uint64_t ld_acquire_sys(const uint64_t* p) { uint64_t v; asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory"); return v; }
-__global__ void k_peer_export(GroupTable gt, AggPlan ap, uint64_t* const* peers, int nranks, int rank, size_t seg_words, size_t parity_off, uint32_t pcap, uint32_t* cursor) {
-    const uint32_t cap = gt.cap_mask + 1;
-    BK_FOR_EACH_GROUP(gt, ap, i) {
-        if (ap.n_keyw == 0 && gt.lanes[i] == 0) continue;
-        const uint32_t pos = atomicAdd(cursor, 1u);
-        if (pos >= pcap) { atomicExch(gt.overflow, 1u); continue; }
-        for (int r = 0; r < nranks; r++) {
-            uint64_t* dkeys = peers[r] + parity_off + (size_t)rank * seg_words + 1;
-            uint64_t* dlanes = dkeys + (size_t)ap.n_keyw * pcap;
-            for (int w = 0; w < ap.n_keyw; w++) dkeys[(size_t)w * pcap + pos] = gt.keys[(size_t)w * cap + i];
-            for (int l = 0; l < ap.n_lanes; l++) dlanes[(size_t)l * pcap + pos] = gt.lanes[(size_t)l * cap + i];
-        }
-    }
-}
-__global__ void k_peer_publish(uint64_t* const* peers, int nranks, int rank, size_t seg_words, size_t parity_off, size_t flag_off, const uint32_t* cursor, uint32_t pcap, uint64_t seq) {
-    const int r = threadIdx.x;
-    if (r >= nranks) return;
-    const uint32_t n = *cursor < pcap ? *cursor : pcap;
-    peers[r][parity_off + (size_t)rank * seg_words] = n;     // (the entries themselves were written by the kernel before this one)
-    __threadfence_system();
-    st_release_sys(peers[r] + flag_off + rank, seq);
-}
-__global__ void k_peer_wait(const uint64_t* flags, int nranks, uint64_t seq, long long limit_cycles, uint32_t* timed_out) {
-    const int r = threadIdx.x;
-    if (r >= nranks) return;
-    const long long t0 = clock64();
-    while (ld_acquire_sys(flags + r) < seq) {
-        if (clock64() - t0 > limit_cycles) { atomicExch(timed_out, 1u); break; }   // a peer died: report instead of spinning forever
-        __nanosleep(200);
-    }
-    __threadfence_system();
-}
-cudaError_t launch_peer_exchange(const GroupTable& gt, const AggPlan& ap, uint64_t* const* d_peers, uint64_t* local, int nranks, int rank, size_t seg_words,
-                                 uint32_t pcap, uint64_t seq, uint32_t* cursor, uint32_t* timed_out, cudaStream_t s) {
-    if (nranks > 1024) return cudaErrorInvalidValue;
-    const size_t parity_off = (size_t)(seq & 1) * (size_t)nranks * seg_words;
-    const size_t flag_off = 2 * (size_t)nranks * seg_words + (size_t)(seq & 1) * (size_t)nranks;
-    const uint32_t cap = gt.cap_mask + 1;
-    int grid = (int)((cap + 255) / 256); if (grid > 1056) grid = 1056;
-    cudaError_t e = cudaMemsetAsync(cursor, 0, sizeof(uint32_t), s);
-    if (e != cudaSuccess) return e;
-    k_peer_export<<<grid, 256, 0, s>>>(gt, ap, d_peers, nranks, rank, seg_words, parity_off, pcap, cursor);
-    k_peer_publish<<<1, 1024, 0, s>>>(d_peers, nranks, rank, seg_words, parity_off, flag_off, cursor, pcap, seq);
-    k_peer_wait<<<1, 1024, 0, s>>>(local + flag_off, nranks, seq, 4000000000ll, timed_out);   // ~2 s at 1.9 GHz
-    return cudaGetLastError();
-}
-
 // hash repartition (the reference's exchange between fragments, src/exec/exchange_sender_node.cpp:867-957): every group of this
-// rank's table goes to the segment of the rank that OWNS its key; segment layout = the partial state layout above
+// rank's table goes to the segment of the rank that OWNS its key.  Segment layout (fixed capacity `pcap` groups):
+// [u64 n_groups][keys n_keyw x pcap][lanes n_lanes x pcap]
 __device__ __forceinline__ uint32_t owner_of(const uint64_t* key, int kw, int nranks) {
     uint64_t h = 0xC2B2AE3D27D4EB4Full;
     for (int i = 0; i < kw; i++) { h ^= key[i]; h *= 0x9FB21C651E98DF25ull; h ^= h >> 29; }
@@ -879,15 +811,6 @@ cudaError_t launch_partial_merge_rows(const GroupTable& gt, const AggPlan& ap, c
                                       uint32_t* max_count, cudaStream_t s) {
     int gx = (int)((bound + 255) / 256); if (gx > 64) gx = 64; if (gx < 1) gx = 1;
     k_partial_merge_rows<<<dim3((unsigned)gx, (unsigned)nranks), 256, 0, s>>>(gt, ap, src, words_per_rank, bound, nranks, self, max_count);
-    return cudaGetLastError();
-}
-cudaError_t launch_partial_export(const GroupTable& gt, const AggPlan& ap, uint64_t* dst, uint32_t pcap, uint32_t* cursor, cudaStream_t s) {
-    const uint32_t cap = gt.cap_mask + 1;
-    int grid = (int)((cap + 255) / 256); if (grid > 1056) grid = 1056;
-    cudaError_t e = cudaMemsetAsync(cursor, 0, sizeof(uint32_t), s);
-    if (e != cudaSuccess) return e;
-    k_partial_export<<<grid, 256, 0, s>>>(gt, ap, dst, pcap, cursor);
-    k_partial_count<<<1, 1, 0, s>>>(dst, cursor, pcap);
     return cudaGetLastError();
 }
 cudaError_t launch_partial_export_parts(const GroupTable& gt, const AggPlan& ap, uint64_t* dst, size_t words_per_seg, uint32_t pcap, uint32_t* cursors, int nranks, cudaStream_t s) {

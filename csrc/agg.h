@@ -121,9 +121,6 @@ cudaError_t launch_table_clear(const GroupTable& gt, const AggPlan& ap, uint32_t
 cudaError_t launch_partial_export_rows(const GroupTable& gt, const AggPlan& ap, uint64_t* dst, uint32_t bound, cudaStream_t s);
 cudaError_t launch_partial_merge_rows(const GroupTable& gt, const AggPlan& ap, const uint64_t* src, size_t words_per_rank, uint32_t bound, int nranks, int self,
                                       uint32_t* max_count, cudaStream_t s);
-cudaError_t launch_partial_export(const GroupTable& gt, const AggPlan& ap, uint64_t* dst, uint32_t pcap, uint32_t* cursor, cudaStream_t s);
-cudaError_t launch_peer_exchange(const GroupTable& gt, const AggPlan& ap, uint64_t* const* d_peers, uint64_t* local, int nranks, int rank, size_t seg_words,
-                                 uint32_t pcap, uint64_t seq, uint32_t* cursor, uint32_t* timed_out, cudaStream_t s);
 cudaError_t launch_partial_export_parts(const GroupTable& gt, const AggPlan& ap, uint64_t* dst, size_t words_per_seg, uint32_t pcap, uint32_t* cursors, int nranks, cudaStream_t s);
 cudaError_t launch_partial_merge(const GroupTable& gt, const AggPlan& ap, const uint64_t* src, size_t words_per_rank, uint32_t pcap, int nranks, cudaStream_t s);
 cudaError_t launch_extract(const GroupTable& gt, const AggPlan& ap, uint64_t* outv, uint8_t* outn, uint32_t out_cap, uint32_t* cursor, int emit_default, cudaStream_t s);

@@ -198,19 +198,15 @@ extern "C" int bkgpu_set_option(bkgpu_plan* p, const char* key, int64_t v) {
     else if (k == "hll_group_capacity") { if (v < 1 || v > (1 << 20)) return p->fail(BKGPU_EINVAL, "hll_group_capacity out of range (1 .. 2^20)"); p->hll_cap = v; }
     else if (k == "partial_capacity") { if (v < 1) return p->fail(BKGPU_EINVAL, "partial_capacity must be positive"); p->partial_cap = v; }
     else if (k == "force_generic") p->force_generic = v != 0;
-    else if (k == "no_stream_copy") p->no_stream_copy = v != 0;
     else if (k == "lean_fx") p->lean_fx = v != 0;
     else if (k == "blocking_sync") p->blocking_sync = (int)v;
     else if (k == "star_expand_capacity") { if (v < 0 || v > 0x7FFFFFFF) return p->fail(BKGPU_EINVAL, "star_expand_capacity out of range"); p->join.star_expand_cap = (int)v; }
     else if (k == "no_lean") p->no_lean = v != 0;
     else if (k == "no_fused_probe") p->join.no_fused_probe = v != 0;
     else if (k == "repartition") p->repartition = v != 0;
-    else if (k == "peer_merge") p->peer_merge = v != 0;
     else if (k == "no_lean_nulls") p->no_lean_nulls = v != 0;
     else if (k == "no_lean_mm") p->no_lean_mm = v != 0;
-    else if (k == "no_bounce") p->no_bounce = v != 0;
     else if (k == "scalar_tma") p->scalar_tma = v != 0;
-    else if (k == "output_on_device") p->output_on_device = v != 0;
     else if (k == "region_base") p->region_base = v;
     else return p->fail(BKGPU_EINVAL, "unknown option '%s'", key);
     return BKGPU_OK;
@@ -285,9 +281,8 @@ extern "C" int bkgpu_open(bkgpu_plan* p) {
         CK(p, cudaEventCreateWithFlags(&p->stage_ready[i], cudaEventDisableTiming));
     }
     p->blocking_wait = p->blocking_sync >= 0 ? p->blocking_sync != 0 : (p->nranks > 1 && cpu_budget() < 4 * p->nranks);
-    if (p->c.ap.n_hll && (p->repartition || p->peer_merge))
-        return p->fail(BKGPU_EUNSUPPORTED, "hll_add_agg with the %s merge is outside the GPU path: its sketches travel only with the all-gather of group rows",
-                       p->repartition ? "repartition" : "peer_merge");
+    if (p->c.ap.n_hll && p->repartition)
+        return p->fail(BKGPU_EUNSUPPORTED, "hll_add_agg with the repartition merge is outside the GPU path: its sketches travel only with the all-gather of group rows");
     if (p->c.n_rb && p->nccl_comm)
         return p->fail(BKGPU_EUNSUPPORTED, "rb_build_agg with a communicator is outside the GPU path: bitmaps do not travel with the fixed-width partial rows");
     int rc = upload_in_sets(p);   // (before sort_open: it copies the programs)
@@ -453,22 +448,18 @@ namespace bk { void stream_copy(void* dst, const void* src, size_t bytes); }   /
 namespace {
 class CopyPool {
   public:
-    explicit CopyPool(int n, double poll_ms) : poll_ms_(poll_ms) { for (int i = 0; i < n; i++) th_.emplace_back([this] { run(); }); }
-    ~CopyPool() { { std::lock_guard<std::mutex> g(mu_); stop_ = true; stop_pub_.store(true, std::memory_order_release); } cv_.notify_all(); for (auto& t : th_) t.join(); }
+    explicit CopyPool(int n) { for (int i = 0; i < n; i++) th_.emplace_back([this] { run(); }); }
+    ~CopyPool() { { std::lock_guard<std::mutex> g(mu_); stop_ = true; } cv_.notify_all(); for (auto& t : th_) t.join(); }
     int size() const { return (int)th_.size(); }
     // runs fn(0) .. fn(n - 1) on the workers and the caller; returns when all are done
     void parallel(int n, const std::function<void(int)>& fn) {
         if (n <= 0) return;
         {
             std::lock_guard<std::mutex> g(mu_);
-            fn_ = &fn; next_ = 0; total_ = n; done_ = 0; done_pub_.store(0, std::memory_order_release); gen_++;
-            gen_pub_.store(gen_, std::memory_order_release);
+            fn_ = &fn; next_ = 0; total_ = n; done_ = 0; gen_++;
         }
         cv_.notify_all();
         work();
-        if (poll_ms_ > 0)
-            for (const double t_end = HostClock::now() + 5.0; done_pub_.load(std::memory_order_acquire) < n && HostClock::now() < t_end;)   // (the last slices finish within microseconds)
-                for (int i = 0; i < 32; i++) __builtin_ia32_pause();
         std::unique_lock<std::mutex> g(mu_);
         done_cv_.wait(g, [this] { return done_ == total_; });
         fn_ = nullptr;
@@ -480,23 +471,15 @@ class CopyPool {
             const std::function<void(int)>* f;
             { std::lock_guard<std::mutex> g(mu_); if (!fn_ || next_ >= total_) return; i = next_++; f = fn_; }
             (*f)(i);
-            { std::lock_guard<std::mutex> g(mu_); ++done_; done_pub_.store(done_, std::memory_order_release); if (done_ == total_) done_cv_.notify_all(); }
+            { std::lock_guard<std::mutex> g(mu_); ++done_; if (done_ == total_) done_cv_.notify_all(); }
         }
     }
     void run() {
         uint64_t seen = 0;
         for (;;) {
-            // a push hands over one chunk per millisecond: a worker that went to sleep on the condition variable after each chunk paid a futex
-            // wake-up (tens of microseconds, staggered over the threads) on a ~0.3 ms copy — it polls for the next chunk for a short while first
-            const double t_end = HostClock::now() + poll_ms_;
-            bool got = false;
-            while (poll_ms_ > 0 && HostClock::now() < t_end) {
-                if (gen_pub_.load(std::memory_order_acquire) != seen || stop_pub_.load(std::memory_order_acquire)) { got = true; break; }
-                for (int i = 0; i < 64; i++) __builtin_ia32_pause();
-            }
             {
                 std::unique_lock<std::mutex> g(mu_);
-                if (!got) cv_.wait(g, [&] { return stop_ || gen_ != seen; });
+                cv_.wait(g, [&] { return stop_ || gen_ != seen; });
                 if (stop_) return;
                 seen = gen_;
             }
@@ -507,8 +490,6 @@ class CopyPool {
     std::mutex mu_; std::condition_variable cv_, done_cv_;
     const std::function<void(int)>* fn_ = nullptr;
     int next_ = 0, total_ = 0, done_ = 0; uint64_t gen_ = 0; bool stop_ = false;
-    const double poll_ms_;   // > 0: a worker polls this long for the next chunk before it sleeps on the condition variable (BKGPU_COPY_POLL_US)
-    std::atomic<uint64_t> gen_pub_{0}; std::atomic<bool> stop_pub_{false}; std::atomic<int> done_pub_{0};   // what the pollers read without the mutex
 };
 // CPUs this process may actually use: online CPUs, its affinity mask and its cgroup CPU quota (a container with a 16-CPU quota on a 128-CPU box
 // gets throttled for the rest of the scheduling period once its threads have burnt the quota — spinning or oversized pools make the copy SLOWER there)
@@ -534,7 +515,7 @@ CopyPool& copy_pool() {
         if (const char* e = getenv("BKGPU_COPY_THREADS")) { const int v = atoi(e); if (v > 0) return std::min(v, 64) - 1; }
         return std::max(1, std::min(23, cpu_budget() * 3 / 4 - 1));   // workers + the pushing thread = 3/4 of the CPU budget
                                                                        // (12 threads 0.895 of the pinned rate; 8: 0.82, 16: 0.85, 24: 0.81), 24 threads on an unconstrained host
-    }(), [] { const char* e = getenv("BKGPU_COPY_POLL_US"); return e ? atof(e) / 1000.0 : 0.0; }());
+    }());
     return pool;
 }
 bool is_pageable(const void* p) {
@@ -561,7 +542,7 @@ int feed(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* col
         return fn(p, dc.data(), nrows, 0, vec_ok);
     }
     bool pageable = false;
-    for (size_t i = 0; i < want.size() && !p->no_bounce; i++) pageable = pageable || is_pageable(bound[i]->values);
+    for (size_t i = 0; i < want.size(); i++) pageable = pageable || is_pageable(bound[i]->values);
     // (pageable input adds a CPU copy stage of about the link's speed in front of the H2D copy: smaller chunks keep the fill / drain
     //  of that three-stage pipeline at ~2 % of the batch instead of ~8 %)
     int64_t chunk_cap = pageable ? std::min<int64_t>(p->chunk_rows, (int64_t)2 << 20) : p->chunk_rows;
@@ -586,10 +567,9 @@ int feed(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* col
                 const uint8_t* src = (const uint8_t*)bound[i]->values + (size_t)off * eb;
                 for (size_t o = 0; o < bytes; o += slice) pieces.push_back({p->bounce[buf][i] + o, src + o, std::min(slice, bytes - o)});
             }
-            const bool nt = !p->no_stream_copy;
             copy_pool().parallel((int)pieces.size(), [&](int k) {
                 const Piece& pc = pieces[(size_t)k];
-                if (nt) stream_copy(pc.dst, pc.src, pc.bytes); else memcpy(pc.dst, pc.src, pc.bytes);
+                stream_copy(pc.dst, pc.src, pc.bytes);
             });
         }
         for (size_t i = 0; i < want.size(); i++) {
@@ -687,45 +667,6 @@ static int bkgpu_push_impl(bkgpu_plan* p, const bkgpu_column* cols, int ncols, i
 }
 
 
-// One-time setup of the peer-memory merge: allocate this rank's buffer, trade CUDA IPC handles through the communicator, map the peers'.
-static int peer_setup(bkgpu_plan* p, size_t seg_words) {
-    if (p->peer_ready) return p->peer_seg_words == seg_words ? BKGPU_OK : p->fail(BKGPU_ESTATE, "peer merge: the partial-state size changed after setup");
-    const int n = p->nranks;
-    if (nccl_comm_rank(p->nccl_comm, &p->peer_rank) != 0) return p->fail(BKGPU_ENCCL, "ncclCommUserRank: %s", nccl_last_error());
-    const size_t words = 2 * (size_t)n * seg_words + 2 * (size_t)n;
-    int rc;
-    if ((rc = dev_alloc(p, (void**)&p->peer_local, words * 8))) return rc;
-    CK(p, cudaMemsetAsync(p->peer_local, 0, words * 8, p->stream));
-    cudaIpcMemHandle_t mine;
-    CK(p, cudaIpcGetMemHandle(&mine, p->peer_local));
-    static_assert(sizeof(cudaIpcMemHandle_t) == 64, "CUDA IPC handles are 64 bytes");
-    uint64_t *d_mine = nullptr, *d_all = nullptr;
-    if ((rc = dev_alloc(p, (void**)&d_mine, 64))) return rc;
-    if ((rc = dev_alloc(p, (void**)&d_all, 64 * (size_t)n))) return rc;
-    CK(p, cudaMemcpyAsync(d_mine, &mine, 64, cudaMemcpyHostToDevice, p->stream));
-    if (nccl_all_gather(p->nccl_comm, d_mine, d_all, 8, p->stream) != 0) return p->fail(BKGPU_ENCCL, "ncclAllGather (IPC handles): %s", nccl_last_error());
-    std::vector<cudaIpcMemHandle_t> all((size_t)n);
-    CK(p, cudaMemcpyAsync(all.data(), d_all, 64 * (size_t)n, cudaMemcpyDeviceToHost, p->stream));
-    CK(p, cudaStreamSynchronize(p->stream));
-    p->peer_ptr.assign((size_t)n, nullptr);
-    for (int r = 0; r < n; r++) {
-        if (r == p->peer_rank) { p->peer_ptr[(size_t)r] = p->peer_local; continue; }
-        void* q = nullptr;
-        CK(p, cudaIpcOpenMemHandle(&q, all[(size_t)r], cudaIpcMemLazyEnablePeerAccess));
-        p->peer_ptr[(size_t)r] = (uint64_t*)q;
-    }
-    if ((rc = dev_alloc(p, (void**)&p->d_peer_ptrs, 8 * (size_t)n))) return rc;
-    if ((rc = dev_alloc(p, (void**)&p->d_peer_timeout, 8))) return rc;
-    CK(p, cudaMemcpyAsync(p->d_peer_ptrs, p->peer_ptr.data(), 8 * (size_t)n, cudaMemcpyHostToDevice, p->stream));
-    CK(p, cudaMemsetAsync(p->d_peer_timeout, 0, 8, p->stream));
-    // nobody may write into a buffer before its owner has zeroed it: one more trip through the communicator is the barrier
-    if (nccl_all_gather(p->nccl_comm, d_mine, d_all, 8, p->stream) != 0) return p->fail(BKGPU_ENCCL, "ncclAllGather (barrier): %s", nccl_last_error());
-    CK(p, cudaStreamSynchronize(p->stream));
-    dev_free(p, d_mine); dev_free(p, d_all);
-    p->peer_seg_words = seg_words; p->peer_ready = true;
-    return BKGPU_OK;
-}
-
 // groups per rank in the exchanged partial state: never more than the group table can hold (every rank runs the same plan with
 // the same options, so all ranks agree on it) — a 2^14-slot table ships 0.8 MB per rank instead of the 3 MB of the default cap
 static uint32_t eff_pcap(const bkgpu_plan* p) {
@@ -736,7 +677,7 @@ static uint32_t eff_pcap(const bkgpu_plan* p) {
 // the collective step of bkgpu_finish: regions -> one set per GPU, the per-GPU partial tables meet once and are folded by K3.
 // Default: compact rows, one ncclAllGather of 1 + bound x (key + lane words) per rank — `bound` = the largest group count any rank
 // held in earlier runs of this plan (2048 on the first run); the merge reports the true maximum and the exchange is repeated once
-// with a larger bound when it did not fit.  Options: peer_merge (NVLink peer memory), repartition (all-to-all by key owner).
+// with a larger bound when it did not fit.  Option repartition: all-to-all by key owner.
 static int agg_collective(bkgpu_plan* p, bool* rows_mode) {
     const AggPlan& ap = p->c.ap;
     GroupTable& gt = p->gt;
@@ -745,9 +686,9 @@ static int agg_collective(bkgpu_plan* p, bool* rows_mode) {
     int rc;
     const bool repart = p->repartition && ap.n_keyw > 0;   // (a scalar aggregate has one group: nothing to partition)
     EventPair* ep = timer_begin(p, p->timed_coll, 0);
-    if (!(p->peer_merge && !repart) && !repart) {
+    if (!repart) {
         *rows_mode = true;
-        if (p->peer_rank < 0 && nccl_comm_rank(p->nccl_comm, &p->peer_rank) != 0) return p->fail(BKGPU_ENCCL, "ncclCommUserRank: %s", nccl_last_error());
+        if (p->rank < 0 && nccl_comm_rank(p->nccl_comm, &p->rank) != 0) return p->fail(BKGPU_ENCCL, "ncclCommUserRank: %s", nccl_last_error());
         uint32_t bound = p->merge_bound ? p->merge_bound : 2048u;
         if (ap.n_keyw == 0) bound = 1;
         bound = std::min<uint32_t>(bound, pcap);
@@ -757,28 +698,17 @@ static int agg_collective(bkgpu_plan* p, bool* rows_mode) {
         if ((rc = ensure_buf(p, (void**)&p->d_gather, &p->d_gather_cap, words * 8 * (size_t)p->nranks))) return rc;
         CK(p, launch_partial_export_rows(gt, ap, p->d_partial, bound, p->stream));
         if (nccl_all_gather(p->nccl_comm, p->d_partial, p->d_gather, words, p->stream) != 0) return p->fail(BKGPU_ENCCL, "ncclAllGather: %s", nccl_last_error());
-        CK(p, launch_partial_merge_rows(gt, ap, p->d_gather, words, bound, p->nranks, p->peer_rank, p->d_cursor + 1, p->stream));
+        CK(p, launch_partial_merge_rows(gt, ap, p->d_gather, words, bound, p->nranks, p->rank, p->d_cursor + 1, p->stream));
         p->merge_bound_used = bound;
         p->stats.kernel_launches += 2;
         timer_end(p, ep);
         return BKGPU_OK;
     }
-    const size_t words = 1 + (size_t)(ap.n_keyw + ap.n_lanes) * pcap;
-    if ((rc = ensure_buf(p, (void**)&p->d_partial, &p->d_partial_cap, words * 8 * (repart ? (size_t)p->nranks : 1)))) return rc;
-    if ((rc = ensure_buf(p, (void**)&p->d_gather, &p->d_gather_cap, words * 8 * (size_t)p->nranks))) return rc;
-    if (p->peer_merge && !repart && (rc = peer_setup(p, words))) return rc;
-    if (p->peer_merge && !repart) {
-        const uint64_t seq = ++p->peer_seq;
-        CK(p, launch_peer_exchange(gt, ap, p->d_peer_ptrs, p->peer_local, p->nranks, p->peer_rank, words, pcap, seq, p->d_cursor, p->d_peer_timeout, p->stream));
-        CK(p, launch_table_init(gt, ap, p->stream, 1));
-        CK(p, launch_partial_merge(gt, ap, p->peer_local + (size_t)(seq & 1) * (size_t)p->nranks * words, words, pcap, p->nranks, p->stream));
-        timer_end(p, ep);
-        p->stats.kernel_launches += 5;
-        if (p->h_pinned) CK(p, cudaMemcpyAsync(p->h_pinned + 6, p->d_peer_timeout, 4, cudaMemcpyDeviceToHost, p->stream));   // checked after the result's synchronisation
-        return BKGPU_OK;
-    }
     // hash repartition: every rank keeps only the groups it owns — an all-to-all of per-owner segments instead of the
     // all-gather; the merged table (and the result) of a rank is its partition, the union over ranks is the answer
+    const size_t words = 1 + (size_t)(ap.n_keyw + ap.n_lanes) * pcap;
+    if ((rc = ensure_buf(p, (void**)&p->d_partial, &p->d_partial_cap, words * 8 * (size_t)p->nranks))) return rc;
+    if ((rc = ensure_buf(p, (void**)&p->d_gather, &p->d_gather_cap, words * 8 * (size_t)p->nranks))) return rc;
     if (!p->d_part_cursors && (rc = dev_alloc(p, (void**)&p->d_part_cursors, 4 * (size_t)p->nranks))) return rc;
     CK(p, launch_partial_export_parts(gt, ap, p->d_partial, words, pcap, p->d_part_cursors, p->nranks, p->stream));
     if (nccl_all_to_all(p->nccl_comm, p->d_partial, p->d_gather, words, p->nranks, p->stream) != 0) return p->fail(BKGPU_ENCCL, "all-to-all: %s", nccl_last_error());
@@ -1024,7 +954,6 @@ static int agg_finish(bkgpu_plan* p) {
         }
         if ((rc = agg_wait(p))) return rc;
         host_counts[0] = hc3[0]; host_counts[1] = hc3[1]; n_out = hc3[2]; merge_max = hc3[3];
-        if (p->peer_ready && p->h_pinned && p->h_pinned[6]) return p->fail(BKGPU_ENCCL, "peer merge: a rank did not publish its partial state within the time limit");
         if (rows_mode) {
             const uint32_t mx = merge_max;
             if (mx > p->merge_bound_used) {   // nothing was merged (k_partial_merge_rows): exchange again, sized for what the ranks really hold
@@ -1205,7 +1134,6 @@ extern "C" void bkgpu_close(bkgpu_plan* p) {
     resolve_timers(p);
     if (p->sort) sort_close(p->sort);
     if (p->post_sort) sort_close(p->post_sort);
-    for (size_t r = 0; r < p->peer_ptr.size(); r++) if ((int)r != p->peer_rank && p->peer_ptr[r]) cudaIpcCloseMemHandle(p->peer_ptr[r]);
     for (cudaEvent_t e : p->event_pool) cudaEventDestroy(e);
     for (auto& q : p->dev_allocs) if (!dev_cache().put(p->device, q.second, q.first)) cudaFree(q.first);   // (both streams were drained above)
     for (int i = 0; i < 2; i++) { if (p->stage_free[i]) cudaEventDestroy(p->stage_free[i]); if (p->stage_ready[i]) cudaEventDestroy(p->stage_ready[i]); }

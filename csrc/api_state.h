@@ -28,7 +28,6 @@ struct HostCol {  // one materialised result column (host memory owned by the pl
     std::vector<uint8_t> validity;  // LSB bitmap; empty = all valid
     const std::vector<uint8_t>* varlen = nullptr;   // elem < 0 (BITMAP): the whole column, rows + 1 int64 offsets then the bytes
     std::vector<uint8_t> batch;     // elem < 0: a later bkgpu_get_next batch, re-based (n + 1 offsets from 0, then its bytes)
-    void* dev_values = nullptr;     // output_on_device
 };
 
 struct EventPair { cudaEvent_t a, b; int64_t bytes; };
@@ -103,7 +102,6 @@ struct bkgpu_plan {
     RbState rb;                   // rb_build_agg's pair buffer and build (rb.h)
     int force_generic = 0;
     int no_lean = 0;
-    int output_on_device = 0;
     int64_t region_base = 0;      // arrival index of this plan's first row (ties across GPUs break by (region, row))
     // aggregate state
     GroupTable gt{};
@@ -115,18 +113,13 @@ struct bkgpu_plan {
     HostClock hclk; bool trace = getenv("BKGPU_TRACE") != nullptr;
     std::vector<uint8_t*> bounce[2]; size_t bounce_rows = 0; cudaEvent_t bounce_done[2] = {nullptr, nullptr}; bool bounce_busy[2] = {false, false};
     int scalar_tma = 1;           // COUNT(*) WHERE int32 <cmp> c runs the TMA-staged kernel (scalar_tma.cu); 0 = the LDG kernel
-    int no_bounce = 0;            // 1 = pageable host input goes straight to cudaMemcpyAsync (A/B of the bounce path)
-    int no_stream_copy = 0;       // 1 = the bounce copy uses memcpy instead of non-temporal stores (A/B, hostcopy.cpp)
     SortState* post_sort = nullptr;                         // the post fragment above the aggregate (Compiled::post)
     std::vector<uint8_t*> post_vals, post_nullb, post_bitmap; size_t post_cap = 0;
     uint64_t rows_passed_host = 0;
     int64_t finish_groups = -1;   // groups in the table when the last finish read the result back (-1 = unknown: full re-initialisation)
     uint32_t merge_bound = 0, merge_bound_used = 0;   // groups per rank the all-gather is sized for (learned from earlier runs)
     uint32_t* d_part_cursors = nullptr; int repartition = 0;   // hash repartition of the groups across ranks (option "repartition")
-    // merge over NVLink peer memory (option "peer_merge"): this rank's buffer, the peers' mappings of theirs, step counter
-    int peer_merge = 0, peer_rank = -1; bool peer_ready = false;
-    uint64_t* peer_local = nullptr; std::vector<uint64_t*> peer_ptr; uint64_t** d_peer_ptrs = nullptr; uint64_t peer_seq = 0; size_t peer_seg_words = 0;
-    uint32_t* d_peer_timeout = nullptr;
+    int rank = -1;                // this rank in the communicator (-1 = not asked yet; the all-gather merge skips its own rows)
     uint64_t* d_outv = nullptr; uint8_t* d_outn = nullptr; size_t out_cap_alloc = 0;  // extraction buffers (kept across resets)
     std::vector<cudaEvent_t> event_pool;
     uint64_t* h_outv = nullptr; uint8_t* h_outn = nullptr; size_t h_out_cap = 0;   // pinned landing area of the extracted rows

@@ -113,14 +113,10 @@ int   bkgpu_init(bkgpu_plan** out, const uint8_t* plan_desc, size_t len,
  *   "hll_group_capacity"   sketches the hll_add_agg register arena holds: one per group and hll_add_agg aggregate that receives a non-NULL
  *                          value, 16 KB of device memory each (default 4096 = 64 MB, at most 2^20); more -> BKGPU_ETOOBIG naming this option
  *   "region_base"          arrival index of this plan's first row: ORDER BY ties across GPUs break by (region, row)
- *   "peer_merge"           with a communicator: partial states are written straight into the peers' buffers over NVLink (CUDA IPC)
- *                          instead of gathered by NCCL (opt-in)
  *   "repartition"          with a communicator: groups are hash-partitioned across the ranks by one all-to-all (ncclSend/ncclRecv)
  *                          instead of gathered everywhere; each rank then returns only the groups it owns (high-cardinality GROUP BY)
  *   "force_generic" / "no_lean" / "no_lean_nulls" / "no_lean_mm" / "no_fused_probe"   pin the kernel variant (tests, A/B measurements)
  *   "scalar_tma"           0 = COUNT(*) WHERE int32 <cmp> c takes the LDG kernel instead of the TMA-staged one (csrc/scalar_tma.cu; default 1)
- *   "no_bounce"            pageable host input goes straight to cudaMemcpyAsync instead of the threaded pinned bounce buffers (A/B)
- *   "no_stream_copy"       the bounce copy uses memcpy instead of non-temporal stores (A/B)
  *   "star_expand_capacity" (tests) first capacity, in row-id tuples, of a star join's expansion pass over a dimension with duplicate keys
  *                          (0 = twice the pass's input); a pass that outgrows it is counted, grown to the exact count and run again
  *   "blocking_sync"        the wait for a request's result: 0 spins (cudaStreamSynchronize), 1 sleeps on a blocking-sync event, -1 (default) sleeps only

@@ -72,10 +72,6 @@ def main():
     node_big = GpuExecNode(); node_big.init(queries.c2_filter_groupby()); node_big.add_child(ColumnSource([mid]))
     assert node_big.open(st_big) == _lib.ETOOBIG, (st_big.error_code, st_big.error_msg)
     node_big.close(st_big)
-    # ---- the same merge over NVLink peer memory (CUDA IPC buffers, no collective call on the data path) ----
-    got_p, stats_p = run_plan(queries.c2_filter_groupby(), region, comm, dev, {"peer_merge": 1})
-    assert stats_p.collective_ms > 0
-    assert_same_rows(got_p, want.columns, ["0_1"])
     # ---- f3: hash repartition (all-to-all): every rank returns only the groups it owns; their union is the answer ----
     hi = datagen.c2_table(rank * n_region, n_region, n_groups=40_000)            # more groups than one 65536-slot partial would
     part, stats = run_plan(queries.c2_filter_groupby(), hi, comm, dev, {"repartition": 1, "group_capacity_log2": 18})   # comfortably merge N times

@@ -247,6 +247,23 @@ def test_group_table_overflow_is_an_error():
     assert ei.value.code == ETOOBIG
 
 
+def test_removed_options_are_unknown():
+    """the peer-memory merge, the pageable-copy switches and output_on_device are gone: setting one is an unknown option, not a no-op"""
+    import ctypes
+    from baikaldb_b200 import _lib
+    L = _lib.lib()
+    plan = queries.c2_filter_groupby().serialize()
+    h = ctypes.c_void_p()
+    _lib.check(L.bkgpu_init(ctypes.byref(h), plan, len(plan), 0, None))
+    try:
+        for key in ("peer_merge", "no_bounce", "no_stream_copy", "output_on_device"):
+            assert L.bkgpu_set_option(h, key.encode(), 1) == _lib.EINVAL, key
+            assert "unknown option" in L.bkgpu_last_error(h).decode() and key in L.bkgpu_last_error(h).decode()
+        assert L.bkgpu_set_option(h, b"repartition", 1) == _lib.OK
+    finally:
+        L.bkgpu_close(h)
+
+
 @pytest.mark.parametrize("n", [1, 4095, 4096, 4097, 70_001, 1_000_003])
 @pytest.mark.parametrize("op,c", [("lt", 1 << 19), ("le", 0), ("gt", (1 << 31) - 1), ("ge", -(1 << 31)), ("eq", 77), ("ne", 77)])
 def test_count_where_tma_staged_kernel(n, op, c):

@@ -238,12 +238,11 @@ def test_arena_overflow_is_an_error():
     assert len(got[0]) == 100
 
 
-def test_multi_gpu_merge_options_refused():
+def test_repartition_merge_refused():
     cols = [make_column(0, 1, T.INT32, np.zeros(4, np.int32)), make_column(0, 2, T.INT64, np.zeros(4, np.int64)), make_column(0, 3, T.DOUBLE, np.zeros(4))]
-    for opt in ("repartition", "peer_merge"):
-        with pytest.raises(BkgpuError) as e:
-            execute(C.scan_plan(T.INT64), cols, options={opt: 1})
-        assert e.value.code == _lib.EUNSUPPORTED and opt in e.value.message
+    with pytest.raises(BkgpuError) as e:
+        execute(C.scan_plan(T.INT64), cols, options={"repartition": 1})
+    assert e.value.code == _lib.EUNSUPPORTED and "repartition" in e.value.message
 
 
 def test_reset_reuse():
