@@ -161,7 +161,7 @@ def c6(a):
     kt = {}
     for e in prof.key_averages():
         name = e.key.split("(")[0].replace("bk::", "")
-        if name.startswith(("k_star_", "k_agg", "k_join_", "k_pack_validity")):
+        if name.startswith(("k_star_", "k_agg", "k_join_", "k_pack_null_bytes")):
             kt[name] = getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) / 1e3 / a.steps
     line["kernel_ms_per_step"] = kt
     # Acero: the same query over the same tables on the host (copied outside the timed region)
@@ -424,7 +424,7 @@ def c10(a):
     dev = lambda e: getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) / 1e3 / (steps + 1)   # (the profiled run: 1 warm-up + steps)
     ka = prof.key_averages()
     line["k_join_pairs_full_ms_per_step"] = sum(dev(e) for e in ka if "k_join_pairs_full" in e.key)
-    line["gather_ms_per_step (k_join_rows_gather + k_pack_validity)"] = sum(dev(e) for e in ka if "k_join_rows_gather" in e.key or "k_pack_validity" in e.key)
+    line["gather_ms_per_step (k_join_rows_gather + k_pack_null_bytes)"] = sum(dev(e) for e in ka if "k_join_rows_gather" in e.key or "k_pack_null_bytes" in e.key)
     line["aggregate_kernel_ms_per_step"] = sum(dev(e) for e in ka if line["main_kernel"] in e.key)
     for name, jt in (("left", P.JoinType.LEFT_JOIN), ("inner", P.JoinType.INNER_JOIN)):
         o = run(f"the same query as {name.upper()}, general path", plan(jt), pushes, nf, 12 * nf + 8 * nd, steps, 1,

@@ -742,30 +742,6 @@ cudaError_t launch_join_gather(const DevCol& probe_key, int from_prim, int cast_
     return cudaGetLastError();
 }
 
-__global__ void k_unpack_validity(const uint8_t* bitmap, int64_t n, uint8_t* null_bytes) {
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-        null_bytes[i] = bitmap ? (((bitmap[i >> 3] >> (i & 7)) & 1) ? 0 : 1) : 0;
-}
-__global__ void k_pack_validity(const uint8_t* null_bytes, int64_t n, uint8_t* bitmap) {
-    const int64_t nbytes = (n + 7) >> 3;
-    for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < nbytes; b += (int64_t)gridDim.x * blockDim.x) {
-        uint8_t v = 0;
-        for (int j = 0; j < 8; j++) { const int64_t i = b * 8 + j; if (i >= n || !null_bytes[i]) v |= (uint8_t)(1u << j); }
-        bitmap[b] = v;
-    }
-}
-cudaError_t launch_unpack_validity(const uint8_t* bitmap, int64_t n, uint8_t* null_bytes, cudaStream_t s) {
-    if (n == 0) return cudaSuccess;
-    int grid = (int)((n + 255) / 256); if (grid > 132 * 16) grid = 132 * 16;
-    k_unpack_validity<<<grid, 256, 0, s>>>(bitmap, n, null_bytes);
-    return cudaGetLastError();
-}
-cudaError_t launch_pack_validity(const uint8_t* null_bytes, int64_t n, uint8_t* bitmap, cudaStream_t s) {
-    if (n == 0) return cudaSuccess;
-    int grid = (int)(((n + 7) / 8 + 255) / 256); if (grid > 132 * 16) grid = 132 * 16;
-    k_pack_validity<<<grid, 256, 0, s>>>(null_bytes, n, bitmap);
-    return cudaGetLastError();
-}
 cudaError_t launch_join_pairs(const AggArgs& a, uint32_t* pairs, uint32_t cap, uint32_t* cursor, int sm_count, cudaStream_t s) {
     const int64_t n = a.join.tail ? a.join.n_build : a.nrows;
     if (n == 0) return cudaSuccess;

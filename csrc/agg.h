@@ -98,8 +98,6 @@ cudaError_t launch_join_minmax(const DevCol& key, int from_prim, int cast_prim, 
 cudaError_t launch_join_build_fast(const DevCol& key, int from_prim, int cast_prim, int64_t nrows, const JoinFast& jf, uint32_t* dense_w, uint64_t* packed_w, uint32_t* dup_flag, cudaStream_t s);
 cudaError_t launch_join_gather(const DevCol& probe_key, int from_prim, int cast_prim, int64_t nrows, const JoinFast& jf, const GatherCols& gc, uint32_t* miss_flag, cudaStream_t s);
 cudaError_t launch_join_compose(const JoinFast& jf, const uint32_t* attr_by_row, uint32_t* attr_of_key, uint64_t* packed_attr, uint32_t* bad_flag, cudaStream_t s);
-cudaError_t launch_unpack_validity(const uint8_t* bitmap, int64_t n, uint8_t* null_bytes, cudaStream_t s);
-cudaError_t launch_pack_validity(const uint8_t* null_bytes, int64_t n, uint8_t* bitmap, cudaStream_t s);
 // a JOIN that returns rows: (probe row, build row) pairs of the joined rows that pass the conditions, then one gather per output column
 // (FULL, not the tail: k_join_pairs_full, which also emits the probe rows without a partner)
 cudaError_t launch_join_pairs(const AggArgs& a, uint32_t* pairs, uint32_t cap, uint32_t* cursor, int sm_count, cudaStream_t s);

@@ -290,7 +290,7 @@ extern "C" int bkgpu_open(bkgpu_plan* p) {
     if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) rc = alloc_group_table(p);
     if (!rc && (p->c.kind == PK_SORT || p->c.kind == PK_FILTER || p->c.kind == PK_WINDOW))   // (a window retains its rows like a full sort)
         rc = sort_open(p, p->c, p->region_base, &p->sort);
-    if (!rc && p->c.post) rc = sort_open(p, *p->c.post, 0, &p->post_sort);
+    if (!rc && p->c.post) { rc = sort_open(p, *p->c.post, 0, &p->post_sort); store_init(p->post, p->c.post->cols); }
     if (rc) return rc;
     p->state = S_OPEN;
     return BKGPU_OK;
@@ -719,41 +719,25 @@ static int agg_collective(bkgpu_plan* p, bool* rows_mode) {
     return BKGPU_OK;
 }
 
-int ensure_post(bkgpu_plan* p, size_t need, size_t cap) {
-    const Compiled& pc = *p->c.post;
-    const size_t nc = pc.cols.size();
-    if (p->post_cap >= need && p->post_vals.size() == nc) return BKGPU_OK;
-    for (auto& v : {&p->post_vals, &p->post_nullb, &p->post_bitmap}) { for (uint8_t* q : *v) dev_free(p, q); v->assign(nc, nullptr); }
-    int rc;
-    for (size_t k = 0; k < nc; k++) {
-        if ((rc = dev_alloc(p, (void**)&p->post_vals[k], cap * (size_t)storage_bytes(prim_storage(pc.cols[k].prim)) + 64))) return rc;
-        if ((rc = dev_alloc(p, (void**)&p->post_nullb[k], cap + 64))) return rc;
-        if ((rc = dev_alloc(p, (void**)&p->post_bitmap[k], cap / 8 + 64))) return rc;
-    }
-    p->post_cap = cap;
-    return BKGPU_OK;
-}
-
 // [LIMIT ->] [SORT ->] [HAVING ->] above the aggregate: the extracted rows (still on the device) become typed columns and run through
 // the post fragment's sort / filter kernels; only the final rows travel to the host
 static int agg_post(bkgpu_plan* p, uint32_t n_out, uint32_t out_cap) {
     const Compiled& pc = *p->c.post;
     const size_t nc = pc.cols.size();
     int rc;
-    if ((rc = ensure_post(p, std::max<size_t>(n_out, 1), std::max<size_t>(n_out, 2048)))) return rc;
+    for (size_t c = 0; c < nc; c++)
+        if ((rc = store_reserve(p, p->post, c, std::max<int64_t>(n_out, 1), std::max<int64_t>(n_out, 2048), true))) return rc;
     PostCols pcs; memset(&pcs, 0, sizeof pcs);
     pcs.n = (int)nc;
     int img = 0;
     for (size_t c = 0; c < nc; c++) {   // (post columns = the aggregate's output columns, in order: plan.cpp::lower_post)
-        pcs.img[c] = img; pcs.stype[c] = prim_storage(pc.cols[c].prim); pcs.values[c] = p->post_vals[c]; pcs.null_bytes[c] = p->post_nullb[c];
+        pcs.img[c] = img; pcs.stype[c] = prim_storage(pc.cols[c].prim); pcs.values[c] = p->post.cols[c].vals; pcs.null_bytes[c] = p->post.cols[c].nulls;
         img += p->c.out_cols[c].kind == 1 ? 2 : 1;
     }
     CK(p, launch_images_to_columns(p->d_outv, p->d_outn, out_cap, n_out, pcs, p->stream));
     std::vector<DevCol> dc(std::max<size_t>(nc, 1));
-    for (size_t c = 0; c < nc; c++) {
-        if (n_out) CK(p, launch_pack_validity(p->post_nullb[c], n_out, p->post_bitmap[c], p->stream));
-        dc[c].values = p->post_vals[c]; dc[c].validity = p->post_bitmap[c]; dc[c].stype = prim_storage(pc.cols[c].prim); dc[c].prim = pc.cols[c].prim;
-    }
+    for (size_t c = 0; c < nc; c++)
+        if ((rc = store_pack(p, p->post, c, n_out, 16, nullptr, &dc[c]))) return rc;
     p->stats.kernel_launches += 1 + (int64_t)nc;
     sort_reset(p->post_sort);
     bkgpu_stats scratch{};   // (the post fragment's kernels are not the request's "main kernel")

@@ -34,19 +34,11 @@ struct EventPair { cudaEvent_t a, b; int64_t bytes; };
 
 // one retained build side of a hash join (K4) and its key indexes
 struct JoinSide {
-    std::vector<uint8_t*> vals, nullbytes, bitmap;   // per plan column (this side's columns only)
-    std::vector<bool> has_null;
-    int64_t rows = 0, cap = 0;
+    RowStore store;   // the table's rows, by plan column (this side's columns only)
     uint8_t* keybits = nullptr; size_t keybits_cap = 0;   // validity of the build key AND the dimension's (star) / build child's (two-table) own filter
     uint64_t* jt_keys = nullptr; uint32_t* jt_rows = nullptr; uint32_t jt_mask = 0; bool jt_generic = false;   // multimap (duplicate keys)
     JoinFast jf{}; uint32_t* jf_dense = nullptr; uint64_t* jf_packed = nullptr; size_t jf_dense_cap = 0, jf_packed_cap = 0;   // unique-key index
     bool learned = false; uint64_t learn_min = 0, learn_max = 0;   // key range of the side's previous build (skips the min/max pass + round trip)
-};
-
-// one plan column of a join's gathered chunk: values, and for a star join's columns with NULLs their null bytes and bitmap
-struct ChunkCol {
-    uint8_t *vals = nullptr, *nullb = nullptr, *bits = nullptr;
-    size_t vals_cap = 0, nullb_cap = 0, bits_cap = 0;
 };
 
 // the hash join (K4) of a plan (join.cu): retained build sides, their indexes, the probe's buffers.  Buffers and indexes are kept
@@ -63,7 +55,7 @@ struct JoinState {
     uint8_t* probe_bits = nullptr; size_t probe_bits_cap = 0;   // the probe key's validity AND the probe child's own filter, for one probe batch
     uint32_t* pairs = nullptr; size_t pairs_cap = 0; uint32_t* cursor = nullptr; size_t cursor_cap = 0;   // PK_JOIN: (probe row, build row) pairs of one batch
     uint32_t* tuples[2] = {nullptr, nullptr}; size_t tuples_cap[2] = {0, 0};   // star join: row-id tuples of one chunk (probe / expansion ping-pong)
-    std::vector<ChunkCol> chunk;   // the gathered chunk (two-table gather path, star join), per plan column
+    RowStore chunk;   // the gathered chunk (two-table gather path, FULL join under an aggregate, star join), by plan column
     // options
     int no_fused_probe = 0;
     int star_expand_cap = 0;     // test option "star_expand_capacity": first capacity (tuples) of a star join's expansion pass (0 = twice its input)
@@ -114,7 +106,7 @@ struct bkgpu_plan {
     std::vector<uint8_t*> bounce[2]; size_t bounce_rows = 0; cudaEvent_t bounce_done[2] = {nullptr, nullptr}; bool bounce_busy[2] = {false, false};
     int scalar_tma = 1;           // COUNT(*) WHERE int32 <cmp> c runs the TMA-staged kernel (scalar_tma.cu); 0 = the LDG kernel
     SortState* post_sort = nullptr;                         // the post fragment above the aggregate (Compiled::post)
-    std::vector<uint8_t*> post_vals, post_nullb, post_bitmap; size_t post_cap = 0;
+    RowStore post;                // the post fragment's input (Compiled::post's columns)
     uint64_t rows_passed_host = 0;
     int64_t finish_groups = -1;   // groups in the table when the last finish read the result back (-1 = unknown: full re-initialisation)
     uint32_t merge_bound = 0, merge_bound_used = 0;   // groups per rank the all-gather is sized for (learned from earlier runs)
@@ -189,8 +181,6 @@ typedef int (*BatchFn)(bkgpu_plan*, const DevCol*, int64_t nrows, int64_t row_ba
 int feed(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device, BatchFn fn);
 // the aggregate of `c` over one batch; `jp`: fused FK -> PK probe (lean kernel only), +1 without launching when the batch does not fit it
 int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp = nullptr);
-// the post fragment's input columns, reallocated with room for `cap` rows when they hold fewer than `need`
-int ensure_post(bkgpu_plan* p, size_t need, size_t cap);
 // the plan's result from a sort fragment's columns; `desc`: their output column descriptions (nullptr = the sort's own)
 void set_result(bkgpu_plan* p, std::vector<SortOutCol>& cols, int64_t rows, const OutCol* desc);
 

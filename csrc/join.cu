@@ -5,16 +5,6 @@
 #include <vector>
 #include "api_state.h"
 
-static void side_init(bkgpu_plan* p, JoinSide& s) {
-    const size_t nc = p->c.cols.size();
-    if (s.vals.empty()) { s.vals.assign(nc, nullptr); s.nullbytes.assign(nc, nullptr); s.bitmap.assign(nc, nullptr); s.has_null.assign(nc, false); }
-}
-// plan column i as retained by side s
-static DevCol side_col(const Compiled& c, const JoinSide& s, size_t i) {
-    DevCol d{};
-    d.values = s.vals[i]; d.validity = s.bitmap[i]; d.stype = prim_storage(c.cols[i].prim); d.prim = c.cols[i].prim;
-    return d;
-}
 // every plan column of the joined row: the build sides' retained columns and the probe batch's (nullptr: the outer-join tail, whose
 // probe-side columns are never read — row = -1 is NULL)
 static std::vector<DevCol> join_cols(const bkgpu_plan* p, const DevCol* probe_cols) {
@@ -22,7 +12,7 @@ static std::vector<DevCol> join_cols(const bkgpu_plan* p, const DevCol* probe_co
     std::vector<DevCol> all(c.cols.size());
     for (size_t i = 0; i < c.cols.size(); i++) {
         all[i].stype = prim_storage(c.cols[i].prim); all[i].prim = c.cols[i].prim;
-        if (c.col_side[i] > 0) all[i] = side_col(c, p->join.side[c.col_side[i] - 1], i);
+        if (c.col_side[i] > 0) all[i] = store_col(p->join.side[c.col_side[i] - 1].store, i);
     }
     if (probe_cols) for (size_t w = 0; w < p->join.probe_map.size(); w++) all[(size_t)p->join.probe_map[w]] = probe_cols[w];
     return all;
@@ -47,24 +37,13 @@ static int run_counted(bkgpu_plan* p, uint64_t cap, const uint32_t* cursor, uint
     return BKGPU_OK;
 }
 
-// the gathered chunk's buffers of plan column m for `rows` rows: values, and null bytes + bitmap when `nulls`
-static int chunk_col(bkgpu_plan* p, size_t m, size_t rows, bool nulls) {
-    std::vector<ChunkCol>& chunk = p->join.chunk;
-    if (chunk.empty()) chunk.assign(p->c.cols.size(), ChunkCol{});
-    ChunkCol& g = chunk[m];
-    int rc;
-    if ((rc = ensure_buf(p, (void**)&g.vals, &g.vals_cap, rows * (size_t)storage_bytes(prim_storage(p->c.cols[m].prim))))) return rc;
-    if (nulls && ((rc = ensure_buf(p, (void**)&g.nullb, &g.nullb_cap, rows)) || (rc = ensure_buf(p, (void**)&g.bits, &g.bits_cap, rows / 8 + 8)))) return rc;
-    return BKGPU_OK;
-}
-
 JoinArgs join_args(const bkgpu_plan* p, bool tail) {
     const Compiled& c = p->c;
     const JoinSide& s = p->join.side[0];
     JoinArgs a; memset(&a, 0, sizeof a);
     a.enabled = 1; a.keys = s.jt_keys; a.rows = s.jt_rows; a.cap_mask = s.jt_mask;
     a.probe_col = c.probe_key_col; a.probe_prim = c.cols[(size_t)c.probe_key_col].prim; a.cast_prim = c.join_key_prim;
-    a.join_type = c.join_type; a.matched = c.join_type == BK_INNER_JOIN ? nullptr : p->join.matched; a.n_build = s.rows;
+    a.join_type = c.join_type; a.matched = c.join_type == BK_INNER_JOIN ? nullptr : p->join.matched; a.n_build = s.store.rows;
     a.tail = tail ? 1 : 0;
     return a;
 }
@@ -76,50 +55,18 @@ static int join_retain_build(bkgpu_plan* p, int side, const bkgpu_column* cols, 
     JoinSide& s = p->join.side[side - 1];
     if (p->join.built) return p->fail(BKGPU_ESTATE, "build-side rows arrived after probing started (the reference fetches the whole driver table first, join_node.cpp:920-1022)");
     const size_t nc = c.cols.size();
-    side_init(p, s);
     std::vector<ColRef> want; std::vector<int> idx;
     for (size_t i = 0; i < nc; i++) if (c.col_side[i] == side) { want.push_back(c.cols[i]); idx.push_back((int)i); }
     std::vector<const bkgpu_column*> bound;
     int rc = bind_columns(p, want, cols, ncols, nrows, bound);
     if (rc) return rc;
-    if (s.rows + nrows > 0xFFFFFFF0ll) return p->fail(BKGPU_EUNSUPPORTED, "build side larger than 2^32 rows");
-    if (s.rows + nrows > s.cap) {
-        const int64_t cap = std::max<int64_t>(s.rows + nrows, std::max<int64_t>(s.cap * 2, 1 << 16));
-        for (int i : idx) {
-            const size_t eb = (size_t)storage_bytes(prim_storage(c.cols[(size_t)i].prim));
-            uint8_t *nv = nullptr, *nn = nullptr;
-            if ((rc = dev_alloc(p, (void**)&nv, (size_t)cap * eb))) return rc;
-            if ((rc = dev_alloc(p, (void**)&nn, (size_t)cap))) return rc;
-            if (s.rows) {
-                CK(p, cudaMemcpyAsync(nv, s.vals[(size_t)i], (size_t)s.rows * eb, cudaMemcpyDeviceToDevice, p->stream));
-                CK(p, cudaMemcpyAsync(nn, s.nullbytes[(size_t)i], (size_t)s.rows, cudaMemcpyDeviceToDevice, p->stream));
-                CK(p, cudaStreamSynchronize(p->stream));
-            }
-            dev_free(p, s.vals[(size_t)i]); dev_free(p, s.nullbytes[(size_t)i]);
-            s.vals[(size_t)i] = nv; s.nullbytes[(size_t)i] = nn;
-        }
-        s.cap = cap;
-    }
+    if (s.store.rows + nrows > 0xFFFFFFF0ll) return p->fail(BKGPU_EUNSUPPORTED, "build side larger than 2^32 rows");
+    if ((rc = store_retain(p, s.store, s.store.rows + nrows))) return rc;
     for (size_t w = 0; w < want.size(); w++) {
-        const int i = idx[w];
-        const size_t eb = (size_t)storage_bytes(prim_storage(c.cols[(size_t)i].prim));
-        uint8_t* dv = s.vals[(size_t)i] + (size_t)s.rows * eb;
-        uint8_t* dn = s.nullbytes[(size_t)i] + s.rows;
-        if (on_device) {
-            CK(p, cudaMemcpyAsync(dv, bound[w]->values, (size_t)nrows * eb, cudaMemcpyDeviceToDevice, p->stream));
-            CK(p, launch_unpack_validity(bound[w]->validity, nrows, dn, p->stream));
-            p->stats.kernel_launches++;
-        } else {
-            CK(p, cudaMemcpyAsync(dv, bound[w]->values, (size_t)nrows * eb, cudaMemcpyHostToDevice, p->stream));
-            std::vector<uint8_t> nb((size_t)nrows, 0);
-            if (bound[w]->validity) for (int64_t r = 0; r < nrows; r++) nb[(size_t)r] = ((bound[w]->validity[r >> 3] >> (r & 7)) & 1) ? 0 : 1;
-            CK(p, cudaMemcpyAsync(dn, nb.data(), (size_t)nrows, cudaMemcpyHostToDevice, p->stream));
-            CK(p, cudaStreamSynchronize(p->stream));
-            p->stats.h2d_bytes += (int64_t)((size_t)nrows * (eb + 1));
-        }
-        if (bound[w]->validity) s.has_null[(size_t)i] = true;
+        if ((rc = store_append(p, s.store, (size_t)idx[w], *bound[w], nrows, on_device))) return rc;
+        if (on_device) p->stats.kernel_launches++;   // (the unpack kernel)
     }
-    s.rows += nrows;
+    s.store.rows += nrows;
     return BKGPU_OK;
 }
 
@@ -153,29 +100,24 @@ static int join_compose_probe(bkgpu_plan* p, uint32_t* flag) {
     if (jp.mode == 1) {
         if ((rc = ensure_buf(p, (void**)&j.jp_attr, &j.jp_attr_cap, (size_t)jp.dense_size * 4))) return rc;
         jp.attr = j.jp_attr;
-        jp.present = (uint64_t)s.rows == jp.dense_size ? nullptr : s.jf.dense;   // unique, NULL-free keys filling the range: every key exists
+        jp.present = (uint64_t)s.store.rows == jp.dense_size ? nullptr : s.jf.dense;   // unique, NULL-free keys filling the range: every key exists
     } else {
         if ((rc = ensure_buf(p, (void**)&j.jp_packed, &j.jp_packed_cap, ((size_t)jp.packed_mask + 1) * 8))) return rc;
         jp.packed = j.jp_packed;
     }
-    CK(p, launch_join_compose(s.jf, (const uint32_t*)s.vals[(size_t)attr_main], j.jp_attr, j.jp_packed, flag, p->stream));
+    CK(p, launch_join_compose(s.jf, (const uint32_t*)s.store.cols[(size_t)attr_main].vals, j.jp_attr, j.jp_packed, flag, p->stream));
     p->stats.kernel_launches++;
     j.jp = jp; j.jp_key_pos = (int)kpos;   // (the caller drops it again when `flag` comes back set)
     return BKGPU_OK;
 }
 
-// validity bitmaps of the side's retained columns that hold NULLs
-static int join_pack_validity(bkgpu_plan* p, JoinSide& s, int side) {
-    const Compiled& c = p->c;
-    side_init(p, s);
+// validity bitmaps of the side's retained columns that some batch delivered NULLs for (store_col reads no bitmap of the others)
+static int join_pack_validity(bkgpu_plan* p, JoinSide& s) {
     int rc;
-    for (size_t i = 0; i < c.cols.size(); i++) {
-        if (c.col_side[i] != side) continue;
-        // (a bitmap kept from an earlier run of the plan must not mask this run's rows: a column without NULLs has none)
-        dev_free(p, s.bitmap[i]); s.bitmap[i] = nullptr;
-        if (!s.has_null[i]) continue;
-        if ((rc = dev_alloc(p, (void**)&s.bitmap[i], (size_t)(s.rows + 7) / 8 + 8))) return rc;
-        CK(p, launch_pack_validity(s.nullbytes[i], s.rows, s.bitmap[i], p->stream));
+    DevCol d;
+    for (size_t i = 0; i < s.store.cols.size(); i++) {
+        if (!s.store.cols[i].nullable) continue;
+        if ((rc = store_pack(p, s.store, i, s.store.rows, 16, nullptr, &d))) return rc;
         p->stats.kernel_launches++;
     }
     return BKGPU_OK;
@@ -188,7 +130,7 @@ static int join_build_index(bkgpu_plan* p, JoinSide& s, const DevCol& key, int c
     JoinState& j = p->join;
     int rc;
     s.jf = JoinFast{};
-    if (s.rows <= 0) return BKGPU_OK;
+    if (s.store.rows <= 0) return BKGPU_OK;
     bool retry_measured = false;
 again:
     const int cls = host_prim_class(cast_prim);
@@ -201,7 +143,7 @@ again:
     bool guessed = s.learned && !retry_measured;
     if (guessed) { h_mm[0] = s.learn_min; h_mm[1] = s.learn_max; }
     else {
-        CK(p, launch_join_minmax(key, key.prim, cast_prim, s.rows, bias, mm, p->stream));
+        CK(p, launch_join_minmax(key, key.prim, cast_prim, s.store.rows, bias, mm, p->stream));
         CK(p, cudaMemcpyAsync(h_mm, mm, 16, cudaMemcpyDeviceToHost, p->stream));
         CK(p, cudaStreamSynchronize(p->stream));
         p->stats.kernel_launches++;
@@ -209,18 +151,18 @@ again:
     JoinFast jf{}; jf.bias = bias;
     const uint64_t range = h_mm[1] >= h_mm[0] ? h_mm[1] - h_mm[0] + 1 : 0;
     const int kb = storage_bytes(prim_storage(cast_prim));
-    if (range > 0 && range <= (uint64_t)4 * (uint64_t)s.rows + 1024 && range <= (1ull << 30)) {
+    if (range > 0 && range <= (uint64_t)4 * (uint64_t)s.store.rows + 1024 && range <= (1ull << 30)) {
         jf.mode = 1; jf.dense_min = h_mm[0]; jf.dense_size = range;
         if ((rc = ensure_buf(p, (void**)&s.jf_dense, &s.jf_dense_cap, (size_t)range * 4))) return rc;
         jf.dense = s.jf_dense;
     } else if (kb <= 4) {
-        uint32_t pc = 1024; while ((int64_t)pc < 2 * s.rows) pc <<= 1;
+        uint32_t pc = 1024; while ((int64_t)pc < 2 * s.store.rows) pc <<= 1;
         jf.mode = 2; jf.packed_mask = pc - 1;
         if ((rc = ensure_buf(p, (void**)&s.jf_packed, &s.jf_packed_cap, (size_t)pc * 8))) return rc;
         jf.packed = s.jf_packed;
     }
     if (jf.mode) {
-        CK(p, launch_join_build_fast(key, key.prim, cast_prim, s.rows, jf, s.jf_dense, s.jf_packed, dup, p->stream));
+        CK(p, launch_join_build_fast(key, key.prim, cast_prim, s.store.rows, jf, s.jf_dense, s.jf_packed, dup, p->stream));
         p->stats.kernel_launches += 1;
         s.jf = jf;
         if (compose && (rc = join_compose_probe(p, dup + 1))) return rc;   // enqueued behind the build: all flags come back in one round trip
@@ -240,26 +182,26 @@ static int join_build_table(bkgpu_plan* p) {
     JoinState& j = p->join;
     JoinSide& s = j.side[0];
     int rc;
-    if ((rc = join_pack_validity(p, s, 1))) return rc;
+    if ((rc = join_pack_validity(p, s))) return rc;
     j.built = true; s.jt_generic = false;   // the multimap of the general probe is built on first use (join_generic_table)
     // ---- FK -> PK fast path: are the build keys unique, and is their range dense or their type <= 32 bits? ----
     s.jf = JoinFast{}; j.jp = JoinProbe{};
     bool build_nulls = false;
-    for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] == 1 && s.has_null[i]) build_nulls = true;   // gathered columns must be NULL-free
+    for (const RowStore::Col& col : s.store.cols) if (col.nullable) build_nulls = true;   // gathered columns must be NULL-free
     if (!c.jfast || c.join_type == BK_FULL_JOIN || build_nulls) return BKGPU_OK;
-    return join_build_index(p, s, side_col(c, s, (size_t)c.build_key_col), c.join_key_prim, true);
+    return join_build_index(p, s, store_col(s.store, (size_t)c.build_key_col), c.join_key_prim, true);
 }
 
 // the multimap of side `s` (duplicate build keys, the general probe): open addressing from the cast key image to the build row
 static int join_build_multimap(bkgpu_plan* p, JoinSide& s, const DevCol& key, int cast_prim) {
     int rc;
     uint32_t cap = 1024;
-    while ((int64_t)cap < 2 * s.rows) cap <<= 1;
+    while ((int64_t)cap < 2 * s.store.rows) cap <<= 1;
     dev_free(p, s.jt_keys); dev_free(p, s.jt_rows); s.jt_keys = nullptr; s.jt_rows = nullptr;
     if ((rc = dev_alloc(p, (void**)&s.jt_keys, (size_t)cap * 8))) return rc;
     if ((rc = dev_alloc(p, (void**)&s.jt_rows, (size_t)cap * 4))) return rc;
     s.jt_mask = cap - 1;
-    CK(p, launch_join_build(key, key.prim, cast_prim, s.rows, s.jt_keys, s.jt_rows, s.jt_mask, p->stream));
+    CK(p, launch_join_build(key, key.prim, cast_prim, s.store.rows, s.jt_keys, s.jt_rows, s.jt_mask, p->stream));
     p->stats.kernel_launches++;
     s.jt_generic = true;
     return BKGPU_OK;
@@ -286,13 +228,13 @@ static int join_generic_table(bkgpu_plan* p) {
     JoinSide& s = j.side[0];
     if (s.jt_generic) return BKGPU_OK;
     int rc;
-    DevCol key = side_col(c, s, (size_t)c.build_key_col);
+    DevCol key = store_col(s.store, (size_t)c.build_key_col);
     if (c.join_type != BK_INNER_JOIN) {   // one "found a partner" byte per build row
-        if ((rc = ensure_buf(p, (void**)&j.matched, &j.matched_cap, (size_t)std::max<int64_t>(s.rows, 1)))) return rc;
-        CK(p, cudaMemsetAsync(j.matched, 0, (size_t)std::max<int64_t>(s.rows, 1), p->stream));
+        if ((rc = ensure_buf(p, (void**)&j.matched, &j.matched_cap, (size_t)std::max<int64_t>(s.store.rows, 1)))) return rc;
+        CK(p, cudaMemsetAsync(j.matched, 0, (size_t)std::max<int64_t>(s.store.rows, 1), p->stream));
         if (c.n_build_filter > 0) {   // (SEMI / ANTI) a row that fails its own filter is neither in the multimap nor in the tail
             const std::vector<DevCol> all = join_cols(p, nullptr);
-            if ((rc = join_child_filter(p, c.build_filter, c.build_key_col, all.data(), s.rows, &s.keybits, &s.keybits_cap, j.matched))) return rc;
+            if ((rc = join_child_filter(p, c.build_filter, c.build_key_col, all.data(), s.store.rows, &s.keybits, &s.keybits_cap, j.matched))) return rc;
             key.validity = s.keybits;
         }
     }
@@ -340,9 +282,9 @@ static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nro
             for (size_t i = 0; i < f.cols.size(); i++) {
                 const size_t m = (size_t)c.jfast_of_main[i];
                 if (c.col_side[m] != 1) { fc[i] = col_at(all[m], off); continue; }
-                if ((rc = chunk_col(p, m, (size_t)chunk, false))) return rc;
-                uint8_t* dst = j.chunk[m].vals;
-                gc.src[gc.n] = s.vals[m]; gc.dst[gc.n] = dst; gc.elem[gc.n] = storage_bytes(all[m].stype); gc.n++;
+                if ((rc = store_reserve(p, j.chunk, m, chunk, chunk, false))) return rc;
+                uint8_t* dst = j.chunk.cols[m].vals;
+                gc.src[gc.n] = s.store.cols[m].vals; gc.dst[gc.n] = dst; gc.elem[gc.n] = storage_bytes(all[m].stype); gc.n++;
                 fc[i] = all[m]; fc[i].values = dst; fc[i].validity = nullptr;
             }
             CK(p, cudaMemsetAsync(p->d_cursor + 1, 0, 4, p->stream));
@@ -381,7 +323,7 @@ static int join_pairs(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t n_p
     a.join = join_args(p, tail);
     if ((rc = ensure_buf(p, (void**)&j.cursor, &j.cursor_cap, 64))) return rc;
     *found = 0;
-    return run_counted(p, (uint64_t)std::max<int64_t>(tail ? j.side[0].rows : n_probe, 1 << 12), j.cursor, found, [&](uint64_t want) -> int {
+    return run_counted(p, (uint64_t)std::max<int64_t>(tail ? j.side[0].store.rows : n_probe, 1 << 12), j.cursor, found, [&](uint64_t want) -> int {
         if (want > 0x7FFFFFF0ull) return p->fail(BKGPU_ETOOBIG, "a probe batch joins to more than 2^31 rows: push smaller batches");
         int r;
         if ((r = ensure_buf(p, (void**)&j.pairs, &j.pairs_cap, (size_t)want * 8))) return r;
@@ -403,13 +345,12 @@ static int join_rows_emit(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t
     if (rc || !found) return rc;
     const Compiled& pc = *c.post;
     const size_t nc = pc.cols.size();
-    if ((rc = ensure_post(p, found, std::max<size_t>((size_t)found + found / 4, 1 << 16)))) return rc;
     std::vector<DevCol> dc(std::max<size_t>(nc, 1));
     for (size_t k = 0; k < nc; k++) {   // sink column k = output column k = device column k of the join (plan.cpp::lower_join_rows)
-        const int st = prim_storage(pc.cols[k].prim);
-        CK(p, launch_join_rows_gather(all[k], j.pairs, 2, c.col_side[k] == 1 ? 1 : 0, found, storage_bytes(st), p->post_vals[k], p->post_nullb[k], p->stream));
-        CK(p, launch_pack_validity(p->post_nullb[k], found, p->post_bitmap[k], p->stream));
-        dc[k].values = p->post_vals[k]; dc[k].validity = p->post_bitmap[k]; dc[k].stype = st; dc[k].prim = pc.cols[k].prim;
+        const RowStore::Col& d = p->post.cols[k];
+        if ((rc = store_reserve(p, p->post, k, found, std::max<int64_t>((int64_t)found + found / 4, 1 << 16), true))) return rc;
+        CK(p, launch_join_rows_gather(all[k], j.pairs, 2, c.col_side[k] == 1 ? 1 : 0, found, storage_bytes(prim_storage(d.prim)), d.vals, d.nulls, p->stream));
+        if ((rc = store_pack(p, p->post, k, found, 16, nullptr, &dc[k]))) return rc;
     }
     p->stats.kernel_launches += 2 * (int64_t)nc;
     p->rows_passed_host += found;
@@ -437,12 +378,13 @@ static int full_join_agg(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t 
     std::vector<DevCol> fc(f.cols.size());
     for (size_t i = 0; i < f.cols.size(); i++) {
         const size_t m = (size_t)c.jfast_of_main[i];
-        if ((rc = chunk_col(p, m, found, true))) return rc;
-        const ChunkCol& g = j.chunk[m];
-        CK(p, launch_join_rows_gather(all[m], j.pairs, 2, c.col_side[m] == 1 ? 1 : 0, found, storage_bytes(all[m].stype), g.vals, g.nullb, p->stream));
-        CK(p, launch_pack_validity(g.nullb, found, g.bits, p->stream));
+        if ((rc = store_reserve(p, j.chunk, m, found, found, true))) return rc;
+        const RowStore::Col& g = j.chunk.cols[m];
+        CK(p, launch_join_rows_gather(all[m], j.pairs, 2, c.col_side[m] == 1 ? 1 : 0, found, storage_bytes(all[m].stype), g.vals, g.nulls, p->stream));
+        DevCol packed;
+        if ((rc = store_pack(p, j.chunk, m, found, 16, nullptr, &packed))) return rc;
         p->stats.kernel_launches += 2;
-        fc[i] = all[m]; fc[i].values = g.vals; fc[i].validity = g.bits;
+        fc[i] = all[m]; fc[i].values = g.vals; fc[i].validity = packed.validity;
     }
     return launch_agg_batch(p, f, fc.data(), found, true);
 }
@@ -466,7 +408,7 @@ static int full_join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_
 int join_tail(bkgpu_plan* p) {
     const Compiled& c = p->c;
     JoinState& j = p->join;
-    if (c.join_type == BK_INNER_JOIN || j.side[0].rows == 0) return BKGPU_OK;
+    if (c.join_type == BK_INNER_JOIN || j.side[0].store.rows == 0) return BKGPU_OK;
     int rc;
     if (!j.built && (rc = join_build_table(p))) return rc;
     if ((rc = join_generic_table(p))) return rc;
@@ -474,7 +416,7 @@ int join_tail(bkgpu_plan* p) {
     if (c.kind == PK_JOIN) return join_rows_emit(p, all, 0, true);
     if (c.join_type == BK_FULL_JOIN) return full_join_agg(p, all, 0, true);
     j.tail_launch = true;
-    rc = launch_agg_batch(p, c, all.data(), j.side[0].rows, false);
+    rc = launch_agg_batch(p, c, all.data(), j.side[0].store.rows, false);
     j.tail_launch = false;
     return rc;
 }
@@ -487,15 +429,15 @@ static int star_build(bkgpu_plan* p) {
     for (size_t d = 0; d < c.dims.size(); d++) {
         JoinSide& s = p->join.side[d];
         const StarDim& sd = c.dims[d];
-        if ((rc = join_pack_validity(p, s, 1 + (int)d))) return rc;
+        if ((rc = join_pack_validity(p, s))) return rc;
         s.jt_generic = false; s.jf = JoinFast{};
-        if (s.rows == 0) continue;
-        DevCol key = side_col(c, s, (size_t)sd.key_col);
+        if (s.store.rows == 0) continue;
+        DevCol key = store_col(s.store, (size_t)sd.key_col);
         if (sd.n_filter > 0) {   // the build key's validity: the key is not NULL and the dimension's own conjuncts are TRUE
-            if ((rc = ensure_buf(p, (void**)&s.keybits, &s.keybits_cap, ((size_t)s.rows + 31) / 32 * 4))) return rc;
+            if ((rc = ensure_buf(p, (void**)&s.keybits, &s.keybits_cap, ((size_t)s.store.rows + 31) / 32 * 4))) return rc;
             StarFilter f; memset(&f, 0, sizeof f);
-            for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] == 1 + (int)d) f.cols[i] = side_col(c, s, i);
-            f.prog = sd.filter; f.key_col = sd.key_col; f.nrows = s.rows;
+            for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] == 1 + (int)d) f.cols[i] = store_col(s.store, i);
+            f.prog = sd.filter; f.key_col = sd.key_col; f.nrows = s.store.rows;
             CK(p, launch_star_dim_filter(f, (uint32_t*)s.keybits, nullptr, p->stream));
             p->stats.kernel_launches++;
             key.validity = s.keybits;
@@ -521,7 +463,7 @@ static int star_probe_batch(bkgpu_plan* p, const DevCol* fact_cols, int64_t nrow
     const Compiled& f = *c.jfast;
     JoinState& j = p->join;
     const int D = (int)c.dims.size(), W = 1 + D;
-    for (int d = 0; d < D; d++) if (j.side[d].rows == 0) return BKGPU_OK;   // an empty dimension: no row joins
+    for (int d = 0; d < D; d++) if (j.side[d].store.rows == 0) return BKGPU_OK;   // an empty dimension: no row joins
     const std::vector<DevCol> all = join_cols(p, fact_cols);
     int rc;
     const int64_t chunk = 16 << 20;
@@ -566,15 +508,16 @@ static int star_probe_batch(bkgpu_plan* p, const DevCol* fact_cols, int64_t nrow
             const size_t m = (size_t)c.jfast_of_main[i];
             const int side = c.col_side[m];
             const DevCol src = side == 0 ? col_at(all[m], off) : all[m];
-            if ((rc = chunk_col(p, m, found, src.validity != nullptr))) return rc;   // NULLs travel along: null bytes, then a bitmap
-            const ChunkCol& g = j.chunk[m];
+            if ((rc = store_reserve(p, j.chunk, m, found, found, src.validity != nullptr))) return rc;   // NULLs travel along: null bytes, then a bitmap
+            const RowStore::Col& g = j.chunk.cols[m];
             fc[i] = src; fc[i].values = g.vals; fc[i].validity = nullptr;
-            CK(p, launch_join_rows_gather(src, j.tuples[cur], W, side, found, storage_bytes(src.stype), g.vals, src.validity ? g.nullb : nullptr, p->stream));
+            CK(p, launch_join_rows_gather(src, j.tuples[cur], W, side, found, storage_bytes(src.stype), g.vals, src.validity ? g.nulls : nullptr, p->stream));
             p->stats.kernel_launches++;
             if (src.validity) {
-                CK(p, launch_pack_validity(g.nullb, found, g.bits, p->stream));
+                DevCol packed;
+                if ((rc = store_pack(p, j.chunk, m, found, 16, nullptr, &packed))) return rc;
                 p->stats.kernel_launches++;
-                fc[i].validity = g.bits;
+                fc[i].validity = packed.validity;
             }
         }
         if ((rc = launch_agg_batch(p, f, fc.data(), found, true))) return rc;
@@ -587,6 +530,13 @@ int join_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows,
     const Compiled& c = p->c;
     JoinState& j = p->join;
     const bool star = c.kind == PK_STAR_AGG;
+    if (j.chunk.cols.empty()) {   // the stores' columns, by plan column: a build side holds its own table's
+        store_init(j.chunk, c.cols);
+        for (int d = 0; d < 4; d++) {
+            store_init(j.side[d].store, c.cols);
+            for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] != 1 + d) j.side[d].store.cols[i].prim = -1;
+        }
+    }
     int side = 0;   // (the Compiled::col_side value of the build table's columns)
     if (!star) { for (int k = 0; k < ncols; k++) if (cols[k].tuple_id == c.build_tuple) side = 1; }
     else for (size_t d = 0; d < c.dims.size() && !side; d++) for (int k = 0; k < ncols; k++) if (cols[k].tuple_id == c.dims[d].tuple_id) side = 1 + (int)d;
@@ -600,7 +550,7 @@ int join_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows,
 void join_reset(bkgpu_plan* p) {
     p->join.built = false;
     for (JoinSide& s : p->join.side) {
-        s.rows = 0; s.jt_generic = false; std::fill(s.has_null.begin(), s.has_null.end(), false);
-        for (size_t i = 0; i < s.bitmap.size(); i++) { dev_free(p, s.bitmap[i]); s.bitmap[i] = nullptr; }   // build-side validity of the previous run
+        s.store.rows = 0; s.jt_generic = false;
+        for (RowStore::Col& col : s.store.cols) col.nullable = false;   // (the previous run's bitmaps are not read again)
     }
 }

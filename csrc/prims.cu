@@ -1,7 +1,10 @@
-// prims.cu — device primitives shared by ORDER BY and the window stage (sort.cu, window.cu) and rb_build_agg (rb.cu), for sm_90a.
+// prims.cu — device primitives shared by ORDER BY and the window stage (sort.cu, window.cu), the hash join (join.cu) and rb_build_agg
+// (rb.cu), for sm_90a.
 #include "prims.cuh"
+#include <string.h>
 #include <algorithm>
 #include "api_state.h"
+#include "dev_common.cuh"
 
 namespace bk {
 
@@ -18,6 +21,167 @@ __global__ void k_pack_null_bytes(const uint8_t* nb, int64_t n, uint8_t* bitmap,
         bitmap[b] = (uint8_t)v;
     }
     if (seen && any_null) *any_null = 1u;   // (lets the sort skip the NULL-rank pass of a key column without NULLs)
+}
+
+// Arrow validity bitmap (nullptr: every row valid) -> null BYTES
+__global__ void k_unpack_validity(const uint8_t* bitmap, int64_t n, uint8_t* null_bytes) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        null_bytes[i] = bitmap ? (((bitmap[i >> 3] >> (i & 7)) & 1) ? 0 : 1) : 0;
+}
+
+__global__ void k_gather_sel(GatherArgs g, const uint32_t* sel, uint64_t n, uint64_t dst_off) {
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        const int64_t src = sel[i];
+        for (int c = 0; c < g.n_cols; c++) {
+            const int eb = g.cols[c].stype == ST_U8 ? 1 : (g.cols[c].stype == ST_BLOB16 ? 16 : ((g.cols[c].stype == ST_I32 || g.cols[c].stype == ST_U32 || g.cols[c].stype == ST_F32) ? 4 : 8));
+            const uint8_t* sv = (const uint8_t*)g.cols[c].values + (size_t)src * eb;
+            uint8_t* dv = g.dst_vals[c] + (size_t)(dst_off + i) * eb;
+            if (eb == 8) *(uint64_t*)dv = *(const uint64_t*)sv; else if (eb == 4) *(uint32_t*)dv = *(const uint32_t*)sv;
+            else if (eb == 16) { ((uint64_t*)dv)[0] = ((const uint64_t*)sv)[0]; ((uint64_t*)dv)[1] = ((const uint64_t*)sv)[1]; }   // AVG intermediate blob (payload only)
+            else *dv = *sv;
+            g.dst_null[c][dst_off + i] = elem_is_null(g.cols[c], src) ? 1 : 0;
+        }
+    }
+}
+
+namespace {
+
+__global__ void k_rs_gather_bytes(const uint8_t* src, const uint32_t* ids, uint8_t* dst, uint64_t n) {
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) dst[i] = src[ids[i]];
+}
+
+int elem_bytes_of(int prim) { return storage_bytes(prim_storage(prim)); }
+
+// *buf reallocated with `bytes`, its first `keep` bytes copied over
+int regrow(bkgpu_plan* p, uint8_t** buf, size_t bytes, size_t keep) {
+    uint8_t* nb = nullptr;
+    int rc;
+    if ((rc = dev_alloc(p, (void**)&nb, bytes))) return rc;
+    if (keep) {
+        CK(p, cudaMemcpyAsync(nb, *buf, keep, cudaMemcpyDeviceToDevice, p->stream));
+        CK(p, cudaStreamSynchronize(p->stream));
+    }
+    dev_free(p, *buf);
+    *buf = nb;
+    return BKGPU_OK;
+}
+
+}  // namespace
+
+// ------------------------------------------------------------------------------------------------------------
+void store_init(RowStore& s, const std::vector<ColRef>& cols) {
+    s.cols.assign(cols.size(), RowStore::Col{});
+    for (size_t i = 0; i < cols.size(); i++) s.cols[i].prim = cols[i].prim;
+}
+
+int store_reserve(bkgpu_plan* p, RowStore& s, size_t i, int64_t need, int64_t cap, bool nulls) {
+    RowStore::Col& c = s.cols[i];
+    const size_t eb = (size_t)elem_bytes_of(c.prim);
+    int rc;
+    if (c.cap < need) {
+        if ((rc = regrow(p, &c.vals, (size_t)cap * eb + 64, (size_t)s.rows * eb))) return rc;
+        c.cap = cap;
+    }
+    if (nulls && c.null_cap < need) {
+        if ((rc = regrow(p, &c.nulls, (size_t)cap + 64, (size_t)s.rows)) || (rc = regrow(p, &c.bitmap, (size_t)(cap + 7) / 8 + 64, 0))) return rc;
+        c.null_cap = cap;
+    }
+    return BKGPU_OK;
+}
+
+int store_retain(bkgpu_plan* p, RowStore& s, int64_t need) {
+    if (need <= s.cap) return BKGPU_OK;
+    const int64_t cap = std::max<int64_t>(need, std::max<int64_t>(s.cap * 2, 1 << 16));
+    int rc;
+    for (size_t i = 0; i < s.cols.size(); i++)
+        if (s.cols[i].prim >= 0 && (rc = store_reserve(p, s, i, need, cap, true))) return rc;
+    s.cap = cap;
+    return BKGPU_OK;
+}
+
+int store_append(bkgpu_plan* p, RowStore& s, size_t i, const bkgpu_column& in, int64_t n, bool on_device) {
+    RowStore::Col& c = s.cols[i];
+    const size_t eb = (size_t)elem_bytes_of(c.prim);
+    uint8_t* dv = c.vals + (size_t)s.rows * eb;
+    uint8_t* dn = c.nulls + s.rows;
+    if (on_device) {
+        CK(p, cudaMemcpyAsync(dv, in.values, (size_t)n * eb, cudaMemcpyDeviceToDevice, p->stream));
+        if (n > 0) k_unpack_validity<<<grid_for(n, p->sm_count, 16), 256, 0, p->stream>>>(in.validity, n, dn);
+        CK(p, cudaGetLastError());
+    } else {
+        CK(p, cudaMemcpyAsync(dv, in.values, (size_t)n * eb, cudaMemcpyHostToDevice, p->stream));
+        std::vector<uint8_t> nb((size_t)n, 0);
+        if (in.validity) for (int64_t r = 0; r < n; r++) nb[(size_t)r] = ((in.validity[r >> 3] >> (r & 7)) & 1) ? 0 : 1;
+        CK(p, cudaMemcpyAsync(dn, nb.data(), (size_t)n, cudaMemcpyHostToDevice, p->stream));
+        CK(p, cudaStreamSynchronize(p->stream));
+        p->stats.h2d_bytes += (int64_t)((size_t)n * (eb + 1));
+    }
+    if (in.validity) c.nullable = true;
+    return BKGPU_OK;
+}
+
+int store_pack(bkgpu_plan* p, const RowStore& s, size_t i, int64_t n, int per_sm, uint32_t* any_null, DevCol* out) {
+    const RowStore::Col& c = s.cols[i];
+    if (n > 0) k_pack_null_bytes<<<grid_for((n + 7) / 8, p->sm_count, per_sm), 256, 0, p->stream>>>(c.nulls, n, c.bitmap, any_null);
+    CK(p, cudaGetLastError());
+    *out = store_col(s, i);
+    out->validity = c.bitmap;
+    return BKGPU_OK;
+}
+
+DevCol store_col(const RowStore& s, size_t i) {
+    const RowStore::Col& c = s.cols[i];
+    DevCol d{};
+    d.values = c.vals; d.validity = c.nullable ? c.bitmap : nullptr; d.stype = prim_storage(c.prim); d.prim = c.prim;
+    return d;
+}
+
+int store_gather(bkgpu_plan* p, const RowStore::Col& src, const uint32_t* perm, int64_t n, uint8_t* dst_vals, uint8_t* dst_nulls) {
+    if (n <= 0) return BKGPU_OK;
+    const cudaStream_t st = p->stream;
+    GatherArgs g; memset(&g, 0, sizeof g);
+    g.cols[0].values = src.vals; g.cols[0].validity = nullptr; g.cols[0].stype = prim_storage(src.prim); g.cols[0].prim = src.prim;
+    g.n_cols = 1; g.dst_vals[0] = dst_vals; g.dst_null[0] = dst_nulls;
+    k_gather_sel<<<grid_for(n, p->sm_count, 8), 256, 0, st>>>(g, perm, (uint64_t)n, 0);
+    // null bytes travel separately (k_gather_sel reads validity bitmaps)
+    k_rs_gather_bytes<<<grid_for(n, p->sm_count, 8), 256, 0, st>>>(src.nulls, perm, dst_nulls, (uint64_t)n);
+    CK(p, cudaGetLastError());
+    return BKGPU_OK;
+}
+
+int store_copy_out(bkgpu_plan* p, const RowStore& s, const std::vector<ColRef>& desc, const uint32_t* perm, int64_t n, int64_t skip,
+                   std::vector<SortOutCol>& out) {
+    const cudaStream_t st = p->stream;
+    out.clear();
+    for (size_t c = 0; c < desc.size(); c++) {
+        const ColRef& cr = desc[c];
+        SortOutCol oc; oc.tuple_id = cr.tuple_id; oc.slot_id = cr.slot_id; oc.prim = cr.prim; oc.elem = elem_bytes_of(cr.prim);
+        oc.values.assign((size_t)std::max<int64_t>(n, 1) * oc.elem, 0);
+        std::vector<uint8_t> nb((size_t)std::max<int64_t>(n, 1));
+        const RowStore::Col& sc = s.cols[c];
+        if (perm && n > 0) {
+            DevScope scope(p);   // the column's gather buffers
+            uint8_t *tv = nullptr, *tn = nullptr; int rc;
+            if ((rc = scope.alloc(&tv, (size_t)n * oc.elem))) return rc;
+            if ((rc = scope.alloc(&tn, (size_t)n))) return rc;
+            if ((rc = store_gather(p, sc, perm + skip, n, tv, tn))) return rc;
+            CK(p, cudaMemcpyAsync(oc.values.data(), tv, (size_t)n * oc.elem, cudaMemcpyDeviceToHost, st));
+            CK(p, cudaMemcpyAsync(nb.data(), tn, (size_t)n, cudaMemcpyDeviceToHost, st));
+            CK(p, cudaStreamSynchronize(st));
+        } else if (n > 0) {
+            CK(p, cudaMemcpyAsync(oc.values.data(), sc.vals + (size_t)skip * oc.elem, (size_t)n * oc.elem, cudaMemcpyDeviceToHost, st));
+            CK(p, cudaMemcpyAsync(nb.data(), sc.nulls + skip, (size_t)n, cudaMemcpyDeviceToHost, st));
+            CK(p, cudaStreamSynchronize(st));
+        }
+        bool any = false;
+        for (int64_t i = 0; i < n; i++) any |= nb[(size_t)i] != 0;
+        if (any) {
+            oc.validity.assign((size_t)(n + 7) / 8 + 1, 0xFF);
+            for (int64_t i = 0; i < n; i++) if (nb[(size_t)i]) oc.validity[(size_t)i >> 3] &= (uint8_t)~(1u << (i & 7));
+        }
+        out.push_back(std::move(oc));
+    }
+    return BKGPU_OK;
 }
 
 namespace {

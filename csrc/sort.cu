@@ -333,12 +333,6 @@ __global__ void __launch_bounds__(1024) k_select_rank(const uint64_t* key, const
 }
 
 // ---- payload: gather rows of the current batch / move rows kept from earlier batches ----
-struct GatherArgs {
-    DevCol cols[MAX_COLS]; int32_t n_cols; uint64_t row_base; int64_t nrows;
-    uint8_t* dst_vals[MAX_COLS]; uint8_t* dst_null[MAX_COLS];
-    const uint8_t* old_vals[MAX_COLS]; const uint8_t* old_null[MAX_COLS];
-    const uint64_t* old_idx; uint32_t old_n;
-};
 __global__ void k_gather_topk(GatherArgs g, const uint64_t* idx, const uint32_t* np) {
     const uint32_t n = *np;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -399,21 +393,6 @@ __global__ void __launch_bounds__(256) k_filter_write(RowArgs a, const uint32_t*
         __syncthreads();
     }
 }
-__global__ void k_gather_sel(GatherArgs g, const uint32_t* sel, uint64_t n, uint64_t dst_off) {
-    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-        const int64_t src = sel[i];
-        for (int c = 0; c < g.n_cols; c++) {
-            const int eb = g.cols[c].stype == ST_U8 ? 1 : (g.cols[c].stype == ST_BLOB16 ? 16 : ((g.cols[c].stype == ST_I32 || g.cols[c].stype == ST_U32 || g.cols[c].stype == ST_F32) ? 4 : 8));
-            const uint8_t* sv = (const uint8_t*)g.cols[c].values + (size_t)src * eb;
-            uint8_t* dv = g.dst_vals[c] + (size_t)(dst_off + i) * eb;
-            if (eb == 8) *(uint64_t*)dv = *(const uint64_t*)sv; else if (eb == 4) *(uint32_t*)dv = *(const uint32_t*)sv;
-            else if (eb == 16) { ((uint64_t*)dv)[0] = ((const uint64_t*)sv)[0]; ((uint64_t*)dv)[1] = ((const uint64_t*)sv)[1]; }   // AVG intermediate blob (payload only)
-            else *dv = *sv;
-            g.dst_null[c][dst_off + i] = elem_is_null(g.cols[c], src) ? 1 : 0;
-        }
-    }
-}
-
 // ---- full sort: materialise (image, row id), LSD radix sort, gather ----
 // mode 0: order-preserving image of the key (NULL -> 0); mode 1: the NULL rank (0 sorts first) — sorted by one
 // extra radix pass AFTER the eight value passes so NULL keys come strictly first / last (is_null_first)
@@ -434,9 +413,6 @@ __global__ void k_sort_images_direct(DevCol c, int64_t n, int vclass, int desc, 
 }
 __global__ void k_rs_gather_u64(const uint64_t* src, const uint32_t* ids, uint64_t* dst, uint32_t n) {
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) dst[i] = src[ids[i]];
-}
-__global__ void k_rs_gather_bytes(const uint8_t* src, const uint32_t* ids, uint8_t* dst, uint64_t n) {
-    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) dst[i] = src[ids[i]];
 }
 
 }  // namespace
@@ -465,7 +441,7 @@ struct SortState {
     uint8_t* h_stage = nullptr; size_t h_stage_cap = 0;   // pinned landing area of the top-k rows
     uint32_t* h_counts = nullptr;                         // pinned copy of d_counts
     // full sort / filter-only: retained rows
-    std::vector<uint8_t*> ret_vals, ret_null; int64_t ret_rows = 0, ret_cap = 0;
+    RowStore ret;
     std::vector<uint8_t*> key_img;  // per ORDER BY key: retained images (full sort)
     uint8_t* ret_keep = nullptr;
     int64_t total_seen = 0;
@@ -584,31 +560,9 @@ int select_topk_class(SortState* s, const RowArgs& ra, int cls, bkgpu_stats* sta
     return p->fail(BKGPU_ETOOBIG, "top-k selection did not converge (candidate buffers too small for this key distribution)");
 }
 
-int ensure_retained(SortState* s, int64_t need) {
-    if (need <= s->ret_cap) return 0;
-    bkgpu_plan* p = s->p;
-    const cudaStream_t st = p->stream;
-    int64_t cap = std::max<int64_t>(need, std::max<int64_t>(s->ret_cap * 2, 1 << 16));
-    for (int c = 0; c < s->ncols; c++) {
-        const int eb = elem_bytes_of(s->c.cols[(size_t)c].prim);
-        uint8_t *nv = nullptr, *nn = nullptr; int rc;
-        if ((rc = dev_alloc(p, (void**)&nv, (size_t)cap * eb))) return rc;
-        if ((rc = dev_alloc(p, (void**)&nn, (size_t)cap))) return rc;
-        if (s->ret_rows) {
-            CK(p, cudaMemcpyAsync(nv, s->ret_vals[(size_t)c], (size_t)s->ret_rows * eb, cudaMemcpyDeviceToDevice, st));
-            CK(p, cudaMemcpyAsync(nn, s->ret_null[(size_t)c], (size_t)s->ret_rows, cudaMemcpyDeviceToDevice, st));
-        }
-        CK(p, cudaStreamSynchronize(st));
-        dev_free(p, s->ret_vals[(size_t)c]); dev_free(p, s->ret_null[(size_t)c]);
-        s->ret_vals[(size_t)c] = nv; s->ret_null[(size_t)c] = nn;
-    }
-    s->ret_cap = cap;
-    return 0;
-}
-
 // rows that pass the predicate are appended, in input order, to the retained columns (filter-only and full sort)
 int retain_batch(SortState* s, const RowArgs& ra, bkgpu_stats* stats) {
-    const int64_t limit_left = (s->c.kind == PK_FILTER && s->c.limit >= 0) ? std::max<int64_t>(s->c.limit - s->ret_rows, 0) : INT64_MAX;
+    const int64_t limit_left = (s->c.kind == PK_FILTER && s->c.limit >= 0) ? std::max<int64_t>(s->c.limit - s->ret.rows, 0) : INT64_MAX;
     if (limit_left == 0) return 0;   // FilterNode stops after `limit` passing rows (filter_node.cpp:786-791)
     bkgpu_plan* p = s->p;
     const cudaStream_t st = p->stream;
@@ -629,58 +583,18 @@ int retain_batch(SortState* s, const RowArgs& ra, bkgpu_stats* stats) {
     if (take > 0) {
         if ((rc = scope.alloc(&sel, (size_t)take * 4))) return rc;
         k_filter_write<<<nblocks, 256, 0, st>>>(ra, counts, rows_per_block, sel, 0, take);
-        if ((rc = ensure_retained(s, s->ret_rows + (int64_t)take))) return rc;
+        if ((rc = store_retain(p, s->ret, s->ret.rows + (int64_t)take))) return rc;
         GatherArgs g; memset(&g, 0, sizeof g);
-        for (int i = 0; i < s->ncols; i++) { g.cols[i] = ra.cols[i]; g.dst_vals[i] = s->ret_vals[(size_t)i]; g.dst_null[i] = s->ret_null[(size_t)i]; }
+        for (int i = 0; i < s->ncols; i++) { g.cols[i] = ra.cols[i]; g.dst_vals[i] = s->ret.cols[(size_t)i].vals; g.dst_null[i] = s->ret.cols[(size_t)i].nulls; }
         g.n_cols = s->ncols;
-        k_gather_sel<<<grid_for((int64_t)take, p->sm_count, 8), 256, 0, st>>>(g, sel, take, (uint64_t)s->ret_rows);
+        k_gather_sel<<<grid_for((int64_t)take, p->sm_count, 8), 256, 0, st>>>(g, sel, take, (uint64_t)s->ret.rows);
         CK(p, cudaStreamSynchronize(st));
-        s->ret_rows += (int64_t)take;
+        s->ret.rows += (int64_t)take;
         stats->kernel_launches += 2;
     }
     stats->kernel_launches += 2;   // the count and the scan: one launch up to 2048 blocks (8M rows), three beyond
     stats->rows_filtered += ra.nrows - (int64_t)total;
     return 0;
-}
-
-int copy_cols_out(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, const std::vector<ColRef>& desc, const uint32_t* perm_dev, int64_t n, int64_t skip,
-                  std::vector<SortOutCol>& out) {
-    // perm_dev == nullptr: rows [skip, skip+n) in place; else gather through a device permutation first
-    bkgpu_plan* p = s->p;
-    const cudaStream_t st = p->stream;
-    out.clear();
-    for (size_t c = 0; c < desc.size(); c++) {
-        const ColRef& cr = desc[c];
-        SortOutCol oc; oc.tuple_id = cr.tuple_id; oc.slot_id = cr.slot_id; oc.prim = cr.prim; oc.elem = elem_bytes_of(cr.prim);
-        oc.values.assign((size_t)std::max<int64_t>(n, 1) * oc.elem, 0);
-        std::vector<uint8_t> nb((size_t)std::max<int64_t>(n, 1));
-        const uint8_t* sv = vals[c]; const uint8_t* sn = nulls[c];
-        if (perm_dev && n > 0) {
-            DevScope scope(p);   // the column's gather buffers
-            uint8_t *tv = nullptr, *tn = nullptr; int rc;
-            if ((rc = scope.alloc(&tv, (size_t)n * oc.elem))) return rc;
-            if ((rc = scope.alloc(&tn, (size_t)n))) return rc;
-            if ((rc = sort_gather_rows(s, sv, sn, cr.prim, perm_dev + skip, n, tv, tn))) return p->fail(rc, "gathering the sorted rows failed");
-            CK(p, cudaMemcpyAsync(oc.values.data(), tv, (size_t)n * oc.elem, cudaMemcpyDeviceToHost, st));
-            CK(p, cudaMemcpyAsync(nb.data(), tn, (size_t)n, cudaMemcpyDeviceToHost, st));
-            CK(p, cudaStreamSynchronize(st));
-        } else if (n > 0) {
-            CK(p, cudaMemcpyAsync(oc.values.data(), sv + (size_t)skip * oc.elem, (size_t)n * oc.elem, cudaMemcpyDeviceToHost, st));
-            CK(p, cudaMemcpyAsync(nb.data(), sn + skip, (size_t)n, cudaMemcpyDeviceToHost, st));
-            CK(p, cudaStreamSynchronize(st));
-        }
-        bool any = false;
-        for (int64_t i = 0; i < n; i++) any |= nb[(size_t)i] != 0;
-        if (any) {
-            oc.validity.assign((size_t)(n + 7) / 8 + 1, 0xFF);
-            for (int64_t i = 0; i < n; i++) if (nb[(size_t)i]) oc.validity[(size_t)i >> 3] &= (uint8_t)~(1u << (i & 7));
-        }
-        out.push_back(std::move(oc));
-    }
-    return 0;
-}
-int copy_out(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, const uint32_t* perm_dev, int64_t n, int64_t skip, std::vector<SortOutCol>& out) {
-    return copy_cols_out(s, vals, nulls, s->c.cols, perm_dev, n, skip, out);
 }
 
 // the buffers of one radix sort of n (key image, row id) pairs, returned to the plan's allocator when it leaves scope
@@ -700,30 +614,6 @@ struct RadixBufs {
         return 0;
     }
 };
-
-// retained columns as DevCols of `ra` (values + validity bitmaps packed from the null bytes, owned by `scope`); h_null_flags[c]: column c
-// holds a NULL
-int retained_bitmaps(SortState* s, DevScope& scope, RowArgs& ra, uint32_t* h_null_flags) {
-    bkgpu_plan* p = s->p;
-    const cudaStream_t st = p->stream;
-    const int64_t n = s->ret_rows;
-    int rc;
-    for (int c = 0; c < s->ncols; c++) { ra.cols[c].values = s->ret_vals[(size_t)c]; ra.cols[c].validity = nullptr; ra.cols[c].stype = prim_storage(s->c.cols[(size_t)c].prim); ra.cols[c].prim = s->c.cols[(size_t)c].prim; }
-    DevScope flags_scope(p);
-    uint32_t* null_flags = nullptr;
-    if ((rc = flags_scope.alloc(&null_flags, sizeof(uint32_t) * MAX_COLS))) return rc;
-    CK(p, cudaMemsetAsync(null_flags, 0, sizeof(uint32_t) * MAX_COLS, st));
-    for (int c = 0; c < s->ncols; c++) {
-        uint8_t* bitmap = nullptr;
-        if ((rc = scope.alloc(&bitmap, (size_t)(n + 7) / 8 + 64))) return rc;
-        k_pack_null_bytes<<<grid_for((n + 7) / 8, p->sm_count, 8), 256, 0, st>>>(s->ret_null[(size_t)c], n, bitmap, null_flags + c);
-        ra.cols[c].validity = bitmap;
-    }
-    CK(p, cudaMemcpyAsync(h_null_flags, null_flags, sizeof(uint32_t) * (size_t)s->ncols, cudaMemcpyDeviceToHost, st));
-    CK(p, cudaStreamSynchronize(st));
-    ra.n_cols = s->ncols; ra.nrows = n;
-    return 0;
-}
 
 // stable LSD radix sort of the row ids b.ids[cur] by `keys` (least significant first).  Key k's image comes from program progs[k] (its
 // output register keys[k].out_reg), or straight from column `direct_col` when that is >= 0 (one key).  identity_start: b.ids[cur] holds
@@ -764,7 +654,7 @@ int sort_open(bkgpu_plan* p, const Compiled& c, int64_t region_base, SortState**
     s->row_base = s->region_base = (uint64_t)region_base;
     s->k = c.kind == PK_SORT ? c.limit : -1;
     s->topk = c.kind == PK_SORT && c.sort_keys.size() == 1 && s->k >= 0 && s->k <= 4096;
-    s->ret_vals.assign((size_t)s->ncols, nullptr); s->ret_null.assign((size_t)s->ncols, nullptr);
+    store_init(s->ret, c.cols);
     int rc = 0;
     if (s->topk) {
         s->cand_cap = 1u << 22;   // 4M candidate pairs (64 MB per array pair)
@@ -794,7 +684,7 @@ int sort_open(bkgpu_plan* p, const Compiled& c, int64_t region_base, SortState**
 
 void sort_reset(SortState* s) {
     for (auto& P : s->pool) { P.n = 0; P.cur = 0; }
-    s->ret_rows = 0; s->total_seen = 0;
+    s->ret.rows = 0; s->total_seen = 0;
     s->row_base = s->region_base;
 }
 
@@ -1000,23 +890,33 @@ int sort_finish(SortState* s, void* nccl_comm, int nranks, bkgpu_stats* stats, s
     }
     if (nccl_comm && nranks > 1) return p->fail(BKGPU_EUNSUPPORTED, "multi-GPU merge is implemented for ORDER BY ... LIMIT (top-k) and aggregates");
     if (s->c.kind == PK_FILTER) {
-        int64_t n = s->ret_rows;
+        int64_t n = s->ret.rows;
         int64_t skip = std::min<int64_t>(s->c.offset, n);
         n -= skip;
         *nrows = n;
-        return copy_out(s, s->ret_vals.data(), s->ret_null.data(), nullptr, n, skip, out);
+        return store_copy_out(p, s->ret, s->c.cols, nullptr, n, skip, out);
     }
     // ---- full ORDER BY: stable LSD radix sort of (key image, row id) pairs, least significant ORDER BY key first ----
-    const int64_t n = s->ret_rows;
+    const int64_t n = s->ret.rows;
     if (n > RADIX_MAX_KEYS) return p->fail(BKGPU_EUNSUPPORTED, "full sort is limited to 2^30 - 1 rows per GPU");
-    if (n == 0) { *nrows = 0; return copy_out(s, s->ret_vals.data(), s->ret_null.data(), nullptr, 0, 0, out); }
+    if (n == 0) { *nrows = 0; return store_copy_out(p, s->ret, s->c.cols, nullptr, 0, 0, out); }
     RadixBufs b(p); int rc;
     if ((rc = b.alloc(n))) return rc;
     RowArgs ra; memset(&ra, 0, sizeof ra);
-    // retained columns carry null BYTES: pack them into bitmaps on the device so the key program sees NULLs
-    DevScope bitmaps(p); uint32_t h_null_flags[MAX_COLS] = {0};
-    if ((rc = retained_bitmaps(s, bitmaps, ra, h_null_flags))) return rc;
-    ra.prog = s->c.prog; ra.key.pred_out = -1;
+    // retained columns carry null BYTES: pack them into bitmaps on the device so the key program sees NULLs; h_null_flags[c]: column c
+    // holds a NULL
+    uint32_t h_null_flags[MAX_COLS] = {0};
+    {
+        DevScope flags_scope(p);
+        uint32_t* null_flags = nullptr;
+        if ((rc = flags_scope.alloc(&null_flags, sizeof(uint32_t) * MAX_COLS))) return rc;
+        CK(p, cudaMemsetAsync(null_flags, 0, sizeof(uint32_t) * MAX_COLS, st));
+        for (int c = 0; c < s->ncols; c++)
+            if ((rc = store_pack(p, s->ret, (size_t)c, n, 8, null_flags + c, &ra.cols[c]))) return rc;
+        CK(p, cudaMemcpyAsync(h_null_flags, null_flags, sizeof(uint32_t) * (size_t)s->ncols, cudaMemcpyDeviceToHost, st));
+        CK(p, cudaStreamSynchronize(st));
+    }
+    ra.n_cols = s->ncols; ra.nrows = n; ra.prog = s->c.prog; ra.key.pred_out = -1;
     k_iota<<<grid_for(n, p->sm_count, 8), 256, 0, st>>>(b.ids[0], n);
     int cur = 0;
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
@@ -1035,21 +935,11 @@ int sort_finish(SortState* s, void* nccl_comm, int nranks, bkgpu_stats* stats, s
     int64_t keep = n; if (s->k >= 0 && keep > s->k) keep = s->k;
     int64_t skip = std::min<int64_t>(s->c.offset, keep); keep -= skip;
     *nrows = keep;
-    return copy_out(s, s->ret_vals.data(), s->ret_null.data(), b.ids[cur], keep, skip, out);
+    return store_copy_out(p, s->ret, s->c.cols, b.ids[cur], keep, skip, out);
 }
 
 // ---- the window stage's access to the retained rows and the radix sort (window.cu) ----
-int sort_retained_cols(SortState* s, DevScope& scope, std::vector<DevCol>& cols, int64_t* nrows) {
-    RowArgs ra; memset(&ra, 0, sizeof ra);
-    uint32_t h_null_flags[MAX_COLS] = {0};
-    int rc = retained_bitmaps(s, scope, ra, h_null_flags);
-    if (rc) return rc;
-    cols.assign(ra.cols, ra.cols + s->ncols);
-    *nrows = s->ret_rows;
-    return 0;
-}
-
-void sort_retained_raw(SortState* s, std::vector<uint8_t*>& vals, std::vector<uint8_t*>& nulls) { vals = s->ret_vals; nulls = s->ret_null; }
+RowStore& sort_retained(SortState* s) { return s->ret; }
 
 int sort_stable_ids(SortState* s, const DevCol* cols, int64_t n, const std::vector<SortKey>& keys, const std::vector<const Program*>& progs,
                     uint32_t* ids, bkgpu_stats* stats) {
@@ -1066,25 +956,6 @@ int sort_stable_ids(SortState* s, const DevCol* cols, int64_t n, const std::vect
     CK(p, cudaMemcpyAsync(ids, b.ids[cur], (size_t)n * 4, cudaMemcpyDeviceToDevice, p->stream));
     CK(p, cudaStreamSynchronize(p->stream));
     return 0;
-}
-
-int sort_copy_rows(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, const std::vector<ColRef>& desc, const uint32_t* perm_dev, int64_t n, int64_t skip,
-                   std::vector<SortOutCol>& out) {
-    return copy_cols_out(s, vals, nulls, desc, perm_dev, n, skip, out);
-}
-
-int sort_gather_rows(SortState* s, const uint8_t* src_vals, const uint8_t* src_null, int prim, const uint32_t* perm_dev, int64_t n,
-                     uint8_t* dst_vals, uint8_t* dst_null) {
-    if (n <= 0) return 0;
-    const cudaStream_t st = s->p->stream;
-    const int sm = s->p->sm_count;
-    GatherArgs g; memset(&g, 0, sizeof g);
-    g.cols[0].values = src_vals; g.cols[0].validity = nullptr; g.cols[0].stype = prim_storage(prim); g.cols[0].prim = prim;
-    g.n_cols = 1; g.dst_vals[0] = dst_vals; g.dst_null[0] = dst_null;
-    k_gather_sel<<<grid_for(n, sm, 8), 256, 0, st>>>(g, perm_dev, (uint64_t)n, 0);
-    // null bytes travel separately (k_gather_sel reads validity bitmaps, retained columns hold null BYTES)
-    k_rs_gather_bytes<<<grid_for(n, sm, 8), 256, 0, st>>>(src_null, perm_dev, dst_null, (uint64_t)n);
-    return cudaGetLastError() == cudaSuccess ? 0 : BKGPU_ENODEV;
 }
 
 // (the device buffers belong to the plan: bkgpu_close returns them)

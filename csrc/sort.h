@@ -7,8 +7,7 @@
 #include <vector>
 #include "../include/bkgpu.h"
 #include "plan.h"
-
-struct DevScope;
+#include "prims.cuh"
 
 namespace bk {
 
@@ -29,20 +28,11 @@ int  sort_partial_merge(SortState* s, const void* dev_src, int nranks, std::vect
 void sort_reset(SortState* s);
 
 // ---- the window stage (window.cu) over a SortState's retained rows (a PK_WINDOW plan retains its filtered rows like a full sort) ----
-// the retained rows as device columns with validity bitmaps; the bitmaps belong to `scope`
-int  sort_retained_cols(SortState* s, DevScope& scope, std::vector<DevCol>& cols, int64_t* nrows);
-// the retained columns' value buffers and null BYTES (1 = NULL), in arrival order
-void sort_retained_raw(SortState* s, std::vector<uint8_t*>& vals, std::vector<uint8_t*>& nulls);
+RowStore& sort_retained(SortState* s);
 // stable LSD radix sort of the row ids `ids` (device, n entries, the current order) by `keys`; key k's image is output keys[k].out_reg
 // of program progs[k] over `cols`
 int  sort_stable_ids(SortState* s, const DevCol* cols, int64_t n, const std::vector<SortKey>& keys, const std::vector<const Program*>& progs,
                      uint32_t* ids, bkgpu_stats* stats);
-// rows perm[skip .. skip+n) of value / null-byte columns described by `desc`, to the host
-int  sort_copy_rows(SortState* s, uint8_t* const* vals, uint8_t* const* nulls, const std::vector<ColRef>& desc, const uint32_t* perm_dev, int64_t n,
-                    int64_t skip, std::vector<SortOutCol>& out);
-// dst[i] = src[perm[i]] for one value / null-byte column of type `prim` (device)
-int  sort_gather_rows(SortState* s, const uint8_t* src_vals, const uint8_t* src_null, int prim, const uint32_t* perm_dev, int64_t n,
-                      uint8_t* dst_vals, uint8_t* dst_null);
 void sort_close(SortState* s);
 
 }  // namespace bk

@@ -345,21 +345,26 @@ int window_finish(bkgpu_plan* p, std::vector<SortOutCol>& out, int64_t* nrows) {
     const int sm = p->sm_count;
     bkgpu_stats* stats = &p->stats;
     DevScope ar(p);   // every device buffer of the call
-    std::vector<DevCol> cols; int64_t n = 0; int rc;
-    if ((rc = sort_retained_cols(rows, ar, cols, &n))) return rc;
+    const RowStore& ret = sort_retained(rows);
+    const int64_t n = ret.rows;
     if (n > RADIX_MAX_KEYS) return p->fail(BKGPU_EUNSUPPORTED, "a window fragment is limited to 2^30 - 1 rows per GPU");
-    const int ncols = (int)cols.size();
+    const int ncols = (int)ret.cols.size();
+    int rc;
+    // the retained rows as device columns: every bitmap packed from the null bytes
+    std::vector<DevCol> cols(ret.cols.size());
+    for (int k = 0; k < ncols; k++)
+        if ((rc = store_pack(p, ret, (size_t)k, n, 8, nullptr, &cols[(size_t)k]))) return rc;
     uint32_t* perm = nullptr;
     if ((rc = ar.alloc(&perm, (size_t)n * 4))) return rc;
     if (n) k_iota<<<grid_for(n, sm, 8), 256, 0, st>>>(perm, n);
-    // window outputs, in row space
-    std::vector<uint8_t*> wvals, wnull;
+    // the output rows: the retained scan columns, then the window outputs (buffers of this call), in row space
+    RowStore all = ret;
     for (const WinStage& w : c.win)
         for (const WinFn& f : w.fns) {
-            uint8_t *v = nullptr, *nb = nullptr;
-            if ((rc = ar.alloc(&v, (size_t)std::max<int64_t>(n, 1) * storage_bytes(prim_storage(f.out_prim)))) || (rc = ar.alloc(&nb, (size_t)std::max<int64_t>(n, 1))))
+            RowStore::Col o; o.prim = f.out_prim;
+            if ((rc = ar.alloc(&o.vals, (size_t)std::max<int64_t>(n, 1) * storage_bytes(prim_storage(f.out_prim)))) || (rc = ar.alloc(&o.nulls, (size_t)std::max<int64_t>(n, 1))))
                 return rc;
-            wvals.push_back(v); wnull.push_back(nb);
+            all.cols.push_back(o);
         }
     StageTimer timer;
     cudaEvent_t e0 = timer.a, e1 = timer.b;
@@ -421,7 +426,8 @@ int window_finish(bkgpu_plan* p, std::vector<SortOutCol>& out, int64_t* nrows) {
             fa.has_frame = w.has_frame; fa.ftype = w.frame_type;
             fa.s_type = w.start.type; fa.s_unb = w.start.unbounded; fa.s_num = w.start.num;
             fa.e_type = w.end.type; fa.e_unb = w.end.unbounded; fa.e_num = w.end.num;
-            fa.perm = perm; fa.out_vals = wvals[fn_index]; fa.out_null = wnull[fn_index]; fa.out_stype = prim_storage(f.out_prim);
+            const RowStore::Col& o = all.cols[(size_t)ncols + fn_index];
+            fa.perm = perm; fa.out_vals = o.vals; fa.out_null = o.nulls; fa.out_stype = prim_storage(f.out_prim);
             const bool scanned = (f.kind <= WF_MAX && (f.method == WM_FWD || f.method == WM_BWD || f.method == WM_PEER)) || (f.kind == WF_DENSE_RANK && fa.has_order);
             if (scanned) {
                 if (!sv && ((rc = ar.alloc(&sv, (size_t)n * 8)) || (rc = ar.alloc(&sc, (size_t)n * 8)))) return rc;
@@ -454,11 +460,6 @@ int window_finish(bkgpu_plan* p, std::vector<SortOutCol>& out, int64_t* nrows) {
     stats->main_kernel_ms += win_ms; stats->main_kernel_launches += 1; stats->main_kernel_bytes += win_bytes;
     stats->kernel_launches += win_launches;
     snprintf(stats->main_kernel_name, sizeof stats->main_kernel_name, "%s", "window_stage(k_win_fn)");
-    // output rows: the retained scan columns, then the window columns
-    std::vector<uint8_t*> rvals, rnull;
-    sort_retained_raw(rows, rvals, rnull);
-    std::vector<uint8_t*> all_v(rvals.begin(), rvals.begin() + ncols), all_n(rnull.begin(), rnull.begin() + ncols);
-    all_v.insert(all_v.end(), wvals.begin(), wvals.end()); all_n.insert(all_n.end(), wnull.begin(), wnull.end());
     std::vector<ColRef> desc;
     for (const OutCol& oc : c.out_cols) desc.push_back({oc.tuple_id, oc.slot_id, oc.prim});
     SortState* post = p->post_sort;
@@ -468,21 +469,18 @@ int window_finish(bkgpu_plan* p, std::vector<SortOutCol>& out, int64_t* nrows) {
         const int64_t skip = std::min<int64_t>(c.offset, keep);
         keep -= skip;
         *nrows = keep;
-        return sort_copy_rows(rows, all_v.data(), all_n.data(), desc, perm, keep, skip, out);
+        return store_copy_out(p, all, desc, perm, keep, skip, out);
     }
-    // the query's ORDER BY: the window rows in their order, as device columns, through the post fragment's sort
+    // the query's ORDER BY: the window rows in their order, as the post fragment's input, through its sort
     sort_reset(post);
     if (n > 0) {
         std::vector<DevCol> dc(desc.size());
         for (size_t k = 0; k < desc.size(); k++) {
-            const int eb = storage_bytes(prim_storage(desc[k].prim));
-            uint8_t *v = nullptr, *nb = nullptr, *bm = nullptr;
-            if ((rc = ar.alloc(&v, (size_t)n * eb)) || (rc = ar.alloc(&nb, (size_t)n)) || (rc = ar.alloc(&bm, (size_t)(n + 7) / 8 + 64))) return rc;
-            if ((rc = sort_gather_rows(rows, all_v[k], all_n[k], desc[k].prim, perm, n, v, nb))) return p->fail(rc, "window output gather failed");
-            k_pack_null_bytes<<<grid_for((n + 7) / 8, sm, 8), 256, 0, st>>>(nb, n, bm, nullptr);
-            dc[k].values = v; dc[k].validity = bm; dc[k].stype = prim_storage(desc[k].prim); dc[k].prim = desc[k].prim;
+            RowStore::Col& d = p->post.cols[k];
+            if ((rc = store_reserve(p, p->post, k, n, n, true)) || (rc = store_gather(p, all.cols[k], perm, n, d.vals, d.nulls)) ||
+                (rc = store_pack(p, p->post, k, n, 8, nullptr, &dc[k])))
+                return rc;
         }
-        CK(p, cudaGetLastError());
         bkgpu_stats scratch{};   // (the post fragment's kernels are not the request's main kernel)
         if ((rc = sort_push(post, dc.data(), n, &scratch))) return rc;
         stats->kernel_launches += scratch.kernel_launches;

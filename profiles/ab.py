@@ -83,6 +83,39 @@ def left_join_residual():
     return P.Plan(P.agg(j, 2, [P.slot_ref(1, 2, T.INT32)], aggs), tup), [[dim, fact], [dim, fact]], {}
 
 
+@case(["1_2"])
+def full_join_agg_nulls_both_sides():   # rows of both sides without a partner: every gathered column of the chunk holds NULLs
+    dim, fact, tup = outer_tables(11, nd=200_000, nf=1_500_000)
+    aggs = [P.agg_expr("count_star", 2, 1), P.agg_expr("count", 2, 2, None, P.slot_ref(0, 3, T.INT32)), P.agg_expr("sum", 2, 3, None, P.slot_ref(0, 2, T.DOUBLE)),
+            P.agg_expr("sum", 2, 4, None, P.slot_ref(1, 3, T.DOUBLE))]
+    tup[2] = P.agg_tuple_slots(aggs, [T.INT64, T.INT64, T.DOUBLE, T.DOUBLE])
+    j = P.join(P.scan(1), P.scan(0), left_conds()[:1], join_type=P.JoinType.FULL_JOIN)
+    return P.Plan(P.agg(j, 2, [P.slot_ref(1, 2, T.INT32)], aggs), tup), [[dim, fact], [dim, fact]], {}
+
+
+def device_columns(cols):
+    """CUDA tensors of the columns (values, and the validity bitmap with 8 bytes of slack)"""
+    import torch
+    from baikaldb_b200.exec_node import DeviceColumn
+    out = []
+    for c in cols:
+        t = torch.from_numpy(np.ascontiguousarray(c.values).copy()).cuda()
+        bm = c.validity_bitmap()
+        b = torch.from_numpy(np.concatenate([bm, np.zeros(8, np.uint8)])).cuda() if bm is not None else None
+        out.append(DeviceColumn(c.tuple_id, c.slot_id, c.prim_type, t.data_ptr(), len(c), b.data_ptr() if b is not None else 0, (t, b)))
+    return out
+
+
+@case(["1_2"])
+def join_device_build_side_in_two_batches():   # the retained build side grows past its first 65,536 rows while keeping them
+    dim, fact, tup = outer_tables(13, nd=150_000, nf=1_000_000)
+    aggs = [P.agg_expr("count_star", 2, 1), P.agg_expr("sum", 2, 2, None, P.slot_ref(0, 2, T.DOUBLE)), P.agg_expr("sum", 2, 3, None, P.slot_ref(1, 3, T.DOUBLE))]
+    tup[2] = P.agg_tuple_slots(aggs, [T.INT64, T.DOUBLE, T.DOUBLE])
+    j = P.join(P.scan(1), P.scan(0), left_conds()[:1])
+    halves = chunks(dim, [0, 50_000, 150_000])
+    return P.Plan(P.agg(j, 2, [P.slot_ref(1, 2, T.INT32)], aggs), tup), [[device_columns(h) for h in halves] + [fact]] * 2, {}
+
+
 @case(None)
 def left_join_rows():
     dim, fact, tup = outer_tables(31, nd=1_500, nf=20_000)
