@@ -12,9 +12,20 @@
 // double sums); each CTA merges its table once into the global group table (RED.ADD.F64 / RED.ADD.64).
 // Rows whose group does not fit the shared table go straight to the global table, so any
 // cardinality is handled; the global table is also the per-GPU partial state that NCCL ships.
+//
+// This file holds the generic (interpreted) kernel, the join probe loops that run the interpreter, the group table's maintenance,
+// exchange and extraction kernels, and the aggregate's host path: the group table's allocation, the launch of each batch, the
+// exchange between ranks and the result (agg_open / agg_push / agg_finish / agg_reset / agg_partial_*, declared in api_state.h).
+// The lean and direct kernels are agg_direct.cuh's.
+#include <string.h>
+#include <algorithm>
+#include <vector>
 #include "agg_kernels.cuh"
 #include "interp.cuh"
 #include "agg_select.h"
+#include "api_state.h"
+#include "nccl_dl.h"
+#include "prims.cuh"
 
 namespace bk {
 
@@ -145,7 +156,6 @@ __global__ void __launch_bounds__(256) k_agg_interp(const __grid_constant__ AggA
 
 // ---- a JOIN that returns rows (JoinNode::get_next_for_hash_inner_join / _other_join, join_node.cpp:1200-1326): the probe emits (probe row,
 // build row) pairs, a gather per output column follows.  LEFT: matched[] is set here, the tail emits (NONE, build row) for the rest.
-constexpr uint32_t JOIN_NO_ROW = 0xFFFFFFFFu;
 __global__ void __launch_bounds__(256) k_join_pairs(const __grid_constant__ AggArgs a, uint32_t* pairs, uint32_t cap, uint32_t* cursor) {
     InterpCtx cx; cx.grouped = false; cx.use_smem = false; cx.gcap = 0; cx.st = SmemTable{};
     auto emit = [&](uint32_t prow, uint32_t brow) {
@@ -211,38 +221,6 @@ __global__ void __launch_bounds__(256) k_join_pairs_full(const __grid_constant__
         }
     }
 }
-// one output column of the joined rows: element `which` of each row-id tuple (`width` row ids: (probe, build) pairs of a two-table join,
-// [fact, dim x D] of a star join) addresses `src`; JOIN_NO_ROW (the NULL-extended side) gives NULL.  dst_null may be nullptr when no
-// element can be NULL
-__global__ void k_join_rows_gather(DevCol src, const uint32_t* tuples, int width, int which, uint32_t n, int eb, uint8_t* dst, uint8_t* dst_null) {
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const uint32_t r = tuples[(size_t)width * i + which];
-        const bool isnull = r == JOIN_NO_ROW || elem_is_null(src, r);
-        if (dst_null) dst_null[i] = isnull ? 1 : 0;
-        const uint8_t* s = (const uint8_t*)src.values + (size_t)r * eb;
-        uint8_t* d = dst + (size_t)i * eb;
-        if (isnull) { for (int b = 0; b < eb; b++) d[b] = 0; continue; }
-        switch (eb) {
-            case 1: *d = *s; break;
-            case 4: *(uint32_t*)d = *(const uint32_t*)s; break;
-            case 8: *(uint64_t*)d = *(const uint64_t*)s; break;
-            default: for (int b = 0; b < eb; b++) d[b] = s[b]; break;
-        }
-    }
-}
-
-// K4 build: insert (cast key image, row) of every non-NULL build row (Joiner::construct_hash_map, joiner.cpp:624-631)
-__global__ void k_join_build(DevCol key, int from_prim, int cast_to, int64_t nrows, uint64_t* keys, uint32_t* rows, uint32_t cap_mask) {
-    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < nrows; r += (int64_t)gridDim.x * blockDim.x) {
-        if (elem_is_null(key, r)) continue;
-        const uint64_t img = cast_prim(load_elem(key, r), from_prim, cast_to);
-        uint32_t slot = hash_key1(img) & cap_mask;
-        for (;;) {
-            if (atomicCAS(rows + slot, 0xFFFFFFFFu, (uint32_t)r) == 0xFFFFFFFFu) { keys[slot] = img; break; }
-            slot = (slot + 1) & cap_mask;
-        }
-    }
-}
 
 // ------------------------------------------------------------------------------------------
 // table maintenance: init, partial export / import (K3), result extraction + finalize
@@ -280,7 +258,7 @@ __global__ void k_table_clear(GroupTable gt, AggPlan ap, uint32_t n) {
 
 // Compact partial state for the all-gather (the default multi-GPU merge): dst[0] = the number of groups this rank holds (its low
 // half doubles as the export cursor, so it may exceed `bound`), followed by min(groups, bound) rows of n_keyw + n_lanes words.
-// Only `1 + bound * row words` cross NVLink; `bound` follows the group counts seen in earlier runs (api.cu).
+// Only `1 + bound * row words` cross NVLink; `bound` follows the group counts seen in earlier runs (agg_collective).
 __global__ void k_partial_export_rows(GroupTable gt, AggPlan ap, uint64_t* dst, uint32_t bound) {
     const uint32_t cap = gt.cap_mask + 1;
     const int rw = ap.n_keyw + ap.n_lanes + ap.n_hll * HLL_ROW_WORDS;
@@ -410,6 +388,7 @@ __global__ void k_extract(GroupTable gt, AggPlan ap, uint64_t* outv, uint8_t* ou
 
 // The aggregate's extracted rows (canonical 64-bit images + null bytes, column-major with stride out_cap) as typed Arrow-layout
 // columns on the device: the input of the post fragment ([LIMIT ->] [SORT ->] [HAVING ->] above the aggregate).
+struct PostCols { int32_t n; int32_t img[MAX_COLS]; int32_t stype[MAX_COLS]; uint8_t* values[MAX_COLS]; uint8_t* null_bytes[MAX_COLS]; };
 __global__ void k_images_to_columns(const uint64_t* outv, const uint8_t* outn, uint32_t out_cap, uint32_t n, PostCols pc) {
     for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n; r += gridDim.x * blockDim.x) {
         for (int c = 0; c < pc.n; c++) {
@@ -427,12 +406,6 @@ __global__ void k_images_to_columns(const uint64_t* outv, const uint8_t* outn, u
         }
     }
 }
-cudaError_t launch_images_to_columns(const uint64_t* outv, const uint8_t* outn, uint32_t out_cap, uint32_t n, const PostCols& pc, cudaStream_t s) {
-    if (!n) return cudaSuccess;
-    int grid = (int)((n + 255) / 256); if (grid > 1056) grid = 1056;
-    k_images_to_columns<<<grid, 256, 0, s>>>(outv, outn, out_cap, n, pc);
-    return cudaGetLastError();
-}
 
 // ------------------------------------------------------------------------------------------
 // host-side launchers
@@ -444,7 +417,9 @@ static int occupancy_grid(K kernel, size_t smem, int sm_count) {
     return per_sm * sm_count;  // persistent grid: a whole number of CTAs per SM (132 SMs on H100 SXM)
 }
 
-cudaError_t launch_agg(const AggArgs& a, AggKernel k, size_t smem, int sm_count, cudaStream_t s, cudaEvent_t start) {
+// the aggregate kernel `k` over one batch; `smem`: its dynamic shared memory (AggSelection::smem).  `start` (optional) is recorded on `s`
+// right before the kernel launch, after the launch setup
+static cudaError_t launch_agg(const AggArgs& a, AggKernel k, size_t smem, int sm_count, cudaStream_t s, cudaEvent_t start) {
     if (a.nrows <= 0) return cudaSuccess;
     switch (k) {
         case INTERP: {
@@ -470,278 +445,6 @@ cudaError_t launch_agg(const AggArgs& a, AggKernel k, size_t smem, int sm_count,
     }
 }
 
-// ---- FK -> PK fast path (see JoinFast in agg.h) ----
-__global__ void k_join_minmax(DevCol key, int from_prim, int cast_to, int64_t nrows, uint64_t bias, uint64_t* mm) {
-    uint64_t lo = ~0ull, hi = 0;
-    const int64_t T = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t r0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r0 < nrows; r0 += 4 * T) {   // four independent loads in flight per thread
-        uint64_t v[4]; bool ok[4];
-#pragma unroll
-        for (int u = 0; u < 4; u++) {
-            const int64_t r = r0 + u * T;
-            ok[u] = r < nrows && !elem_is_null(key, r);
-            v[u] = ok[u] ? load_elem(key, r) : 0;
-        }
-#pragma unroll
-        for (int u = 0; u < 4; u++) {
-            if (!ok[u]) continue;
-            const uint64_t x = cast_prim(v[u], from_prim, cast_to) ^ bias;
-            lo = x < lo ? x : lo; hi = x > hi ? x : hi;
-        }
-    }
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) {
-        const uint64_t l2 = __shfl_xor_sync(0xFFFFFFFFu, lo, d), h2 = __shfl_xor_sync(0xFFFFFFFFu, hi, d);
-        lo = l2 < lo ? l2 : lo; hi = h2 > hi ? h2 : hi;
-    }
-    if ((threadIdx.x & 31) == 0) { atomicMin((unsigned long long*)mm, (unsigned long long)lo); atomicMax((unsigned long long*)(mm + 1), (unsigned long long)hi); }
-}
-__global__ void k_join_build_fast(DevCol key, int from_prim, int cast_to, int64_t nrows, JoinFast jf, uint32_t* dense_w, uint64_t* packed_w, uint32_t* dup_flag) {
-    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < nrows; r += (int64_t)gridDim.x * blockDim.x) {
-        if (elem_is_null(key, r)) continue;   // a NULL key never matches
-        const uint64_t img = cast_prim(load_elem(key, r), from_prim, cast_to);
-        if (jf.mode == 1) {
-            const uint64_t off = (img ^ jf.bias) - jf.dense_min;
-            if (off >= jf.dense_size) { atomicExch(dup_flag + 2, 1u); continue; }   // outside the range learned from an earlier run of the plan: the host rebuilds
-            if (atomicExch(dense_w + off, (uint32_t)r) != 0xFFFFFFFFu) atomicExch(dup_flag, 1u);
-        } else {
-            const uint32_t k32 = (uint32_t)img;
-            const uint64_t v = ((uint64_t)k32 << 32) | (uint32_t)r;
-            uint32_t slot = (k32 * 0x9E3779B1u) & jf.packed_mask;
-            for (;;) {
-                const uint64_t old = atomicCAS((unsigned long long*)(packed_w + slot), ~0ull, (unsigned long long)v);
-                if (old == ~0ull) break;
-                if ((uint32_t)(old >> 32) == k32) { atomicExch(dup_flag, 1u); break; }   // duplicate key: not a PK
-                slot = (slot + 1) & jf.packed_mask;
-            }
-        }
-    }
-}
-__device__ __forceinline__ uint32_t join_lookup(const JoinFast& jf, uint64_t img) {
-    if (jf.mode == 1) {
-        const uint64_t off = (img ^ jf.bias) - jf.dense_min;
-        return off < jf.dense_size ? __ldg(jf.dense + off) : 0xFFFFFFFFu;
-    }
-    const uint32_t k32 = (uint32_t)img;
-    uint32_t slot = (k32 * 0x9E3779B1u) & jf.packed_mask;
-    for (;;) {
-        const uint64_t v = __ldg((const unsigned long long*)(jf.packed + slot));
-        if (v == ~0ull) return 0xFFFFFFFFu;
-        if ((uint32_t)(v >> 32) == k32) return (uint32_t)v;
-        slot = (slot + 1) & jf.packed_mask;
-    }
-}
-// gather the build-side columns to probe-row alignment; four independent rows per thread keep the random
-// lookups and gathers in flight together
-__global__ void __launch_bounds__(256) k_join_gather(DevCol pk, int from_prim, int cast_to, int64_t nrows, JoinFast jf, GatherCols gc, uint32_t* miss_flag) {
-    const int64_t T = (int64_t)gridDim.x * blockDim.x;
-    bool miss = false;
-    for (int64_t base = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; base < nrows; base += 4 * T) {
-        uint32_t br[4];
-#pragma unroll
-        for (int u = 0; u < 4; u++) {
-            const int64_t r = base + u * T;
-            br[u] = 0xFFFFFFFEu;   // beyond the batch
-            if (r < nrows) br[u] = elem_is_null(pk, r) ? 0xFFFFFFFFu : join_lookup(jf, cast_prim(load_elem(pk, r), from_prim, cast_to));
-        }
-#pragma unroll
-        for (int u = 0; u < 4; u++) {
-            const int64_t r = base + u * T;
-            if (br[u] == 0xFFFFFFFEu) continue;
-            if (br[u] == 0xFFFFFFFFu) { miss = true; continue; }
-            for (int c = 0; c < gc.n; c++) {
-                if (gc.elem[c] == 8) ((uint64_t*)gc.dst[c])[r] = __ldg((const unsigned long long*)gc.src[c] + br[u]);
-                else if (gc.elem[c] == 4) ((uint32_t*)gc.dst[c])[r] = __ldg((const uint32_t*)gc.src[c] + br[u]);
-                else gc.dst[c][r] = __ldg(gc.src[c] + br[u]);
-            }
-        }
-    }
-    if (__any_sync(0xFFFFFFFFu, miss) && (threadIdx.x & 31) == 0) atomicExch(miss_flag, 1u);
-}
-// K4 fused probe (JoinProbe): compose the grouped-by build attribute onto the key index built by k_join_build_fast
-__global__ void k_join_compose(JoinFast jf, const uint32_t* attr_by_row, uint32_t* attr_of_key, uint64_t* packed_attr, uint32_t* bad_flag) {
-    const uint64_t n = jf.mode == 1 ? jf.dense_size : (uint64_t)jf.packed_mask + 1;
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-        if (jf.mode == 1) {
-            const uint32_t r = jf.dense[i];
-            attr_of_key[i] = r == 0xFFFFFFFFu ? 0u : __ldg(attr_by_row + r);
-        } else {
-            const uint64_t e = jf.packed[i];
-            uint64_t o = ~0ull;
-            if (e != ~0ull) {
-                o = (e & 0xFFFFFFFF00000000ull) | __ldg(attr_by_row + (uint32_t)e);
-                if (o == ~0ull) atomicExch(bad_flag, 1u);   // (key, attribute) = (0xFFFFFFFF, 0xFFFFFFFF) would read as a free slot
-            }
-            packed_attr[i] = o;
-        }
-    }
-}
-
-// ---- K4 star join (PK_STAR_AGG): one fact table INNER-joined to up to four dimensions ----
-// Build time: the conjuncts over one dimension alone, once per dimension row.  A row's build key is valid when the key is not NULL and the
-// conjunction is TRUE: this bitmap (beside the column's own) is the key's validity for k_join_build_fast / k_join_build, which skip NULL keys.
-// The two-table join runs it over a child's own filter: the build side's (with `dropped`: a row whose conjunction is not TRUE, whatever its
-// key, is marked 2 in matched[]) and each probe batch's.  The program reads the row both as the probe row and as the build row.
-__global__ void __launch_bounds__(256) k_star_dim_filter(const __grid_constant__ StarFilter a, uint32_t* keybits, uint8_t* dropped) {
-    const int lane = threadIdx.x & 31;
-    const int64_t T = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t w0 = (int64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31); w0 < a.nrows; w0 += T) {   // (warp-uniform: one bitmap word per warp and pass)
-        const int64_t r = w0 + lane;
-        bool ok = r < a.nrows && !elem_is_null(a.cols[a.key_col], r);
-        if ((ok || (dropped && r < a.nrows)) && a.prog.n_instr > 0) {
-            uint64_t out[1]; uint32_t out_null;
-            run_program(a.prog, a.cols, r, out, out_null, r);
-            const bool pass = !(out_null & 1u) && out[0] != 0;
-            ok = ok && pass;
-            if (dropped && !pass) dropped[r] = 2;
-        }
-        const uint32_t m = __ballot_sync(0xFFFFFFFFu, ok);
-        if (lane == 0) keybits[w0 >> 5] = m;
-    }
-}
-// four consecutive foreign keys [r0, r0 + 4) as canonical images: one 128-bit load (4-byte keys) or two (8-byte keys) when the chunk is 32-byte
-// aligned and the four rows exist
-__device__ __forceinline__ void load_quad(const DevCol& c, int64_t r0, int64_t nrows, bool vec, uint64_t (&v)[4]) {
-    if (vec && r0 + 4 <= nrows && (c.stype == ST_I32 || c.stype == ST_U32)) {
-        const uint4 q = __ldg((const uint4*)((const uint32_t*)c.values + r0));
-        const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-        for (int u = 0; u < 4; u++) v[u] = narrow_prim(c.stype == ST_I32 ? (uint64_t)(int64_t)(int32_t)w[u] : (uint64_t)w[u], c.prim);
-        return;
-    }
-    if (vec && r0 + 4 <= nrows && (c.stype == ST_I64 || c.stype == ST_U64)) {
-        const ulonglong2 a = __ldg((const ulonglong2*)((const unsigned long long*)c.values + r0));
-        const ulonglong2 b = __ldg((const ulonglong2*)((const unsigned long long*)c.values + r0 + 2));
-        v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
-        return;
-    }
-#pragma unroll
-    for (int u = 0; u < 4; u++) v[u] = r0 + u < nrows ? load_elem(c, r0 + u) : 0;
-}
-// Probe: one pass over a chunk's fact rows.  A row survives when every dimension with unique keys has a partner (a NULL foreign key has none:
-// one L2-resident index read per dimension).  Survivors leave as row-id tuples [fact row, dim row x D] in any order, compacted with warp
-// ballots and one cursor atomic per warp; the slots of dimensions with duplicate keys are filled by k_star_expand.
-__global__ void __launch_bounds__(256) k_star_probe(const __grid_constant__ StarProbe a, uint32_t* out, uint32_t* cursor) {
-    const int lane = threadIdx.x & 31;
-    const int64_t T = (int64_t)gridDim.x * blockDim.x;
-    const int64_t nq = (a.nrows + 3) / 4;
-    for (int64_t q0 = (int64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31); q0 < nq; q0 += T) {   // (warp-uniform trip count: the ballots below)
-        const int64_t r0 = (q0 + lane) * 4;
-        uint32_t br[4][4];
-        // every lookup is issued before any result is tested: up to 16 independent index reads in flight per thread
-#pragma unroll
-        for (int d = 0; d < 4; d++) {
-            if (d >= a.n) break;
-            const StarLookup& L = a.d[d];
-            uint64_t v[4];
-            load_quad(L.fk, r0, a.nrows, a.vec != 0, v);
-#pragma unroll
-            for (int u = 0; u < 4; u++)
-                br[u][d] = r0 + u < a.nrows && !elem_is_null(L.fk, r0 + u) ? join_lookup(L.jf, cast_prim(v[u], L.from_prim, L.cast_prim)) : JOIN_NO_ROW;
-        }
-        uint32_t live = 0;
-#pragma unroll
-        for (int u = 0; u < 4; u++) {
-            bool ok = r0 + u < a.nrows;
-#pragma unroll
-            for (int d = 0; d < 4; d++) if (d < a.n) ok = ok && br[u][d] != JOIN_NO_ROW;
-            if (ok) live |= 1u << u;
-        }
-        uint32_t b[4]; uint32_t total = 0;
-#pragma unroll
-        for (int u = 0; u < 4; u++) { b[u] = __ballot_sync(0xFFFFFFFFu, (live >> u) & 1u); total += (uint32_t)__popc(b[u]); }
-        if (total == 0) continue;
-        uint32_t base = 0;
-        if (lane == 0) base = atomicAdd(cursor, total);
-        base = __shfl_sync(0xFFFFFFFFu, base, 0);
-        const uint32_t lt = (1u << lane) - 1u;
-#pragma unroll
-        for (int u = 0; u < 4; u++) {
-            if ((live >> u) & 1u) {
-                uint32_t* t = out + (size_t)a.width * (base + (uint32_t)__popc(b[u] & lt));
-                t[0] = (uint32_t)(r0 + u);
-#pragma unroll
-                for (int d = 0; d < 4; d++) if (d < a.n) t[a.d[d].slot] = br[u][d];
-            }
-            base += (uint32_t)__popc(b[u]);
-        }
-    }
-}
-// A dimension with duplicate keys: every tuple becomes one tuple per matching row of the dimension's multimap (k_join_build), or none.
-// Past `cap` only the count goes on: the host grows the buffer to the count and runs the pass again.
-__global__ void __launch_bounds__(256) k_star_expand(DevCol fk, int from_prim, int cast_to, const uint64_t* keys, const uint32_t* rows, uint32_t cap_mask,
-                                                     const uint32_t* in, uint32_t n_in, int width, int slot, uint32_t* out, uint32_t cap, uint32_t* cursor) {
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_in; i += gridDim.x * blockDim.x) {
-        const uint32_t* t = in + (size_t)width * i;
-        const uint32_t f = t[0];
-        if (elem_is_null(fk, f)) continue;
-        const uint64_t img = cast_prim(load_elem(fk, f), from_prim, cast_to);
-        for (uint32_t h = hash_key1(img) & cap_mask;; h = (h + 1) & cap_mask) {
-            const uint32_t br = rows[h];
-            if (br == 0xFFFFFFFFu) break;
-            if (keys[h] != img) continue;
-            const uint32_t pos = atomicAdd(cursor, 1u);
-            if (pos >= cap) continue;
-            uint32_t* o = out + (size_t)width * pos;
-            for (int k = 0; k < width; k++) o[k] = t[k];
-            o[slot] = br;
-        }
-    }
-}
-cudaError_t launch_star_dim_filter(const StarFilter& f, uint32_t* keybits, uint8_t* dropped, cudaStream_t s) {
-    if (f.nrows == 0) return cudaSuccess;
-    int grid = (int)((f.nrows + 255) / 256); if (grid > 132 * 16) grid = 132 * 16;
-    k_star_dim_filter<<<grid, 256, 0, s>>>(f, keybits, dropped);
-    return cudaGetLastError();
-}
-cudaError_t launch_star_probe(const StarProbe& sp, uint32_t* out, uint32_t* cursor, int sm_count, cudaStream_t s) {
-    cudaError_t e = cudaMemsetAsync(cursor, 0, 4, s);
-    if (e != cudaSuccess || sp.nrows == 0) return e;
-    int64_t g = (sp.nrows + 1023) / 1024; if (g > (int64_t)sm_count * 8) g = (int64_t)sm_count * 8;
-    k_star_probe<<<(int)(g < 1 ? 1 : g), 256, 0, s>>>(sp, out, cursor);
-    return cudaGetLastError();
-}
-cudaError_t launch_star_expand(const DevCol& fk, int from_prim, int cast_prim_, const uint64_t* keys, const uint32_t* rows, uint32_t cap_mask, const uint32_t* in, uint32_t n_in,
-                               int width, int slot, uint32_t* out, uint32_t cap, uint32_t* cursor, cudaStream_t s) {
-    cudaError_t e = cudaMemsetAsync(cursor, 0, 4, s);
-    if (e != cudaSuccess || n_in == 0) return e;
-    int grid = (int)((n_in + 255) / 256); if (grid > 132 * 16) grid = 132 * 16;
-    k_star_expand<<<grid, 256, 0, s>>>(fk, from_prim, cast_prim_, keys, rows, cap_mask, in, n_in, width, slot, out, cap, cursor);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_join_compose(const JoinFast& jf, const uint32_t* attr_by_row, uint32_t* attr_of_key, uint64_t* packed_attr, uint32_t* bad_flag, cudaStream_t s) {
-    cudaError_t e = cudaMemsetAsync(bad_flag, 0, 4, s);
-    if (e != cudaSuccess) return e;
-    const uint64_t n = jf.mode == 1 ? jf.dense_size : (uint64_t)jf.packed_mask + 1;
-    int grid = (int)((n + 255) / 256); if (grid > 132 * 16) grid = 132 * 16; if (grid < 1) grid = 1;
-    k_join_compose<<<grid, 256, 0, s>>>(jf, attr_by_row, attr_of_key, packed_attr, bad_flag);
-    return cudaGetLastError();
-}
-cudaError_t launch_join_minmax(const DevCol& key, int from_prim, int cast_prim_, int64_t nrows, uint64_t bias, uint64_t* mm, cudaStream_t s) {
-    const uint64_t init[2] = {~0ull, 0ull};
-    cudaError_t e = cudaMemcpyAsync(mm, init, 16, cudaMemcpyHostToDevice, s);
-    if (e != cudaSuccess || nrows == 0) return e;
-    int grid = (int)((nrows + 255) / 256); if (grid > 132 * 8) grid = 132 * 8;
-    k_join_minmax<<<grid, 256, 0, s>>>(key, from_prim, cast_prim_, nrows, bias, mm);
-    return cudaGetLastError();
-}
-cudaError_t launch_join_build_fast(const DevCol& key, int from_prim, int cast_prim_, int64_t nrows, const JoinFast& jf, uint32_t* dense_w, uint64_t* packed_w, uint32_t* dup_flag, cudaStream_t s) {
-    cudaError_t e = cudaMemsetAsync(dup_flag, 0, 12, s);   // [0] duplicate key, [1] fused probe unusable (set by the compose step), [2] key outside the guessed range
-    if (e != cudaSuccess) return e;
-    if (jf.mode == 1) e = cudaMemsetAsync(dense_w, 0xFF, jf.dense_size * 4, s); else e = cudaMemsetAsync(packed_w, 0xFF, ((size_t)jf.packed_mask + 1) * 8, s);
-    if (e != cudaSuccess || nrows == 0) return e;
-    int grid = (int)((nrows + 255) / 256); if (grid > 132 * 16) grid = 132 * 16;
-    k_join_build_fast<<<grid, 256, 0, s>>>(key, from_prim, cast_prim_, nrows, jf, dense_w, packed_w, dup_flag);
-    return cudaGetLastError();
-}
-cudaError_t launch_join_gather(const DevCol& probe_key, int from_prim, int cast_prim_, int64_t nrows, const JoinFast& jf, const GatherCols& gc, uint32_t* miss_flag, cudaStream_t s) {
-    if (nrows == 0) return cudaSuccess;
-    int grid = (int)((nrows + 1023) / 1024); if (grid > 132 * 8) grid = 132 * 8; if (grid < 1) grid = 1;
-    k_join_gather<<<grid, 256, 0, s>>>(probe_key, from_prim, cast_prim_, nrows, jf, gc, miss_flag);
-    return cudaGetLastError();
-}
-
 cudaError_t launch_join_pairs(const AggArgs& a, uint32_t* pairs, uint32_t cap, uint32_t* cursor, int sm_count, cudaStream_t s) {
     const int64_t n = a.join.tail ? a.join.n_build : a.nrows;
     if (n == 0) return cudaSuccess;
@@ -751,66 +454,555 @@ cudaError_t launch_join_pairs(const AggArgs& a, uint32_t* pairs, uint32_t cap, u
     else k_join_pairs<<<grid, 256, 0, s>>>(a, pairs, cap, cursor);
     return cudaGetLastError();
 }
-cudaError_t launch_join_rows_gather(const DevCol& src, const uint32_t* tuples, int width, int which, uint32_t n, int eb, uint8_t* dst, uint8_t* dst_null, cudaStream_t s) {
-    if (n == 0) return cudaSuccess;
-    int grid = (int)((n + 255) / 256); if (grid > 132 * 16) grid = 132 * 16;
-    k_join_rows_gather<<<grid, 256, 0, s>>>(src, tuples, width, which, n, eb, dst, dst_null);
-    return cudaGetLastError();
-}
-cudaError_t launch_join_build(const DevCol& key, int from_prim, int cast_prim_, int64_t nrows, uint64_t* keys, uint32_t* rows, uint32_t cap_mask, cudaStream_t s) {
-    cudaError_t e = cudaMemsetAsync(rows, 0xFF, (size_t)(cap_mask + 1) * 4, s);
-    if (e != cudaSuccess || nrows == 0) return e;
-    int grid = (int)((nrows + 255) / 256); if (grid > 132 * 16) grid = 132 * 16;
-    k_join_build<<<grid, 256, 0, s>>>(key, from_prim, cast_prim_, nrows, keys, rows, cap_mask);
-    return cudaGetLastError();
-}
-cudaError_t launch_table_init(const GroupTable& gt, const AggPlan& ap, cudaStream_t s, int keep_overflow) {
-    const uint32_t cap = gt.cap_mask + 1;
-    int grid = (int)((cap + 255) / 256); if (grid > 1056) grid = 1056;
-    k_table_init<<<grid, 256, 0, s>>>(gt, ap, keep_overflow);
-    return cudaGetLastError();
-}
-cudaError_t launch_table_clear(const GroupTable& gt, const AggPlan& ap, uint32_t n_occupied, cudaStream_t s) {
-    int grid = (int)((n_occupied + 255) / 256); if (grid > 1056) grid = 1056; if (grid < 1) grid = 1;
-    k_table_clear<<<grid, 256, 0, s>>>(gt, ap, n_occupied);
-    return cudaGetLastError();
-}
-cudaError_t launch_partial_export_rows(const GroupTable& gt, const AggPlan& ap, uint64_t* dst, uint32_t bound, cudaStream_t s) {
-    const uint32_t cap = gt.cap_mask + 1;
-    int grid = (int)((cap + 255) / 256); if (grid > 132) grid = 132;   // (the kernel walks the occupied list, grid-stride)
-    cudaError_t e = cudaMemsetAsync(dst, 0, 8, s);
-    if (e != cudaSuccess) return e;
-    k_partial_export_rows<<<grid, 256, 0, s>>>(gt, ap, dst, bound);
-    return cudaGetLastError();
-}
-cudaError_t launch_partial_merge_rows(const GroupTable& gt, const AggPlan& ap, const uint64_t* src, size_t words_per_rank, uint32_t bound, int nranks, int self,
-                                      uint32_t* max_count, cudaStream_t s) {
-    int gx = (int)((bound + 255) / 256); if (gx > 64) gx = 64; if (gx < 1) gx = 1;
-    k_partial_merge_rows<<<dim3((unsigned)gx, (unsigned)nranks), 256, 0, s>>>(gt, ap, src, words_per_rank, bound, nranks, self, max_count);
-    return cudaGetLastError();
-}
-cudaError_t launch_partial_export_parts(const GroupTable& gt, const AggPlan& ap, uint64_t* dst, size_t words_per_seg, uint32_t pcap, uint32_t* cursors, int nranks, cudaStream_t s) {
-    if (nranks > 1024) return cudaErrorInvalidValue;
-    const uint32_t cap = gt.cap_mask + 1;
-    int grid = (int)((cap + 255) / 256); if (grid > 1056) grid = 1056;
-    cudaError_t e = cudaMemsetAsync(cursors, 0, sizeof(uint32_t) * (size_t)nranks, s);
-    if (e != cudaSuccess) return e;
-    k_partial_export_parts<<<grid, 256, 0, s>>>(gt, ap, dst, words_per_seg, pcap, cursors, nranks);
-    k_partial_counts<<<1, 1024, 0, s>>>(dst, words_per_seg, cursors, pcap, nranks);
-    return cudaGetLastError();
-}
-cudaError_t launch_partial_merge(const GroupTable& gt, const AggPlan& ap, const uint64_t* src, size_t words_per_rank, uint32_t pcap, int nranks, cudaStream_t s) {
-    int grid = (int)((pcap + 255) / 256); if (grid > 1056) grid = 1056; if (grid < 1) grid = 1;
-    k_partial_merge<<<grid, 256, 0, s>>>(gt, ap, src, words_per_rank, pcap, nranks);
-    return cudaGetLastError();
-}
-cudaError_t launch_extract(const GroupTable& gt, const AggPlan& ap, uint64_t* outv, uint8_t* outn, uint32_t out_cap, uint32_t* cursor, int emit_default, cudaStream_t s) {
-    const uint32_t cap = gt.cap_mask + 1;
-    int grid = (int)((cap + 255) / 256); if (grid > 132) grid = 132;   // (the kernel walks the occupied list, grid-stride)
-    cudaError_t e = cudaMemsetAsync(cursor, 0, sizeof(uint32_t), s);
-    if (e != cudaSuccess) return e;
-    k_extract<<<grid, 256, 0, s>>>(gt, ap, outv, outn, out_cap, cursor, emit_default);
-    return cudaGetLastError();
-}
 
 }  // namespace bk
+
+// ------------------------------------------------------------------------------------------
+// host path of the aggregate (PK_AGG, PK_JOIN_AGG, PK_STAR_AGG): the group table, its launches, the exchange between ranks and
+// the result
+// ------------------------------------------------------------------------------------------
+// record = false: the caller records ep->a itself (right before its launch)
+static EventPair* timer_begin(bkgpu_plan* p, std::vector<EventPair>& v, int64_t bytes, bool record = true) {
+    EventPair ep{};
+    for (cudaEvent_t* e : {&ep.a, &ep.b}) {   // events are recycled: a re-armed plan launches the same kernels again and again
+        if (!p->event_pool.empty()) { *e = p->event_pool.back(); p->event_pool.pop_back(); }
+        else if (cudaEventCreate(e) != cudaSuccess) return nullptr;
+    }
+    ep.bytes = bytes;
+    if (record) cudaEventRecord(ep.a, p->stream);
+    v.push_back(ep);
+    return &v.back();
+}
+static void timer_end(bkgpu_plan* p, EventPair* ep) { if (ep) cudaEventRecord(ep->b, p->stream); }
+
+int agg_open(bkgpu_plan* p) {
+    const AggPlan& ap = p->c.ap;
+    GroupTable& gt = p->gt;
+    int log2 = ap.n_keyw == 0 ? 0 : p->group_cap_log2;
+    size_t cap = (size_t)1 << log2;
+    gt.cap_mask = (uint32_t)(cap - 1); gt.cap_log2 = (uint32_t)log2;
+    int rc;
+    if ((rc = dev_alloc(p, (void**)&gt.state, cap * 4))) return rc;
+    if ((rc = dev_alloc(p, (void**)&gt.keys, cap * 8 * (size_t)std::max(ap.n_keyw, 1)))) return rc;
+    if ((rc = dev_alloc(p, (void**)&gt.lanes, cap * 8 * (size_t)ap.n_lanes))) return rc;
+    if ((rc = dev_alloc(p, (void**)&gt.n_groups, 4 * ((size_t)GT_OCC_OFF + cap)))) return rc;   // counter, overflow flag, occupied list
+    gt.overflow = gt.n_groups + 1;
+    if (ap.n_hll) {   // hll_add_agg: the register arena, one block per (group, sketch) that receives a value
+        if ((rc = dev_alloc(p, (void**)&gt.hll_regs, (size_t)p->hll_cap * HLL_REGISTERS))) return rc;
+        if ((rc = dev_alloc(p, (void**)&gt.hll_ctr, 16))) return rc;
+        gt.hll_cap = (uint32_t)p->hll_cap;
+        CK(p, cudaMemsetAsync(gt.hll_ctr, 0, 16, p->stream));
+    }
+    if (p->c.n_rb) {   // rb_build_agg: the pair buffer and the sort's second buffer (one word more each: the build's scan closes on it)
+        if ((rc = dev_alloc(p, (void**)&p->rb.keys, ((size_t)p->rb_cap + 1) * 8))) return rc;
+        if ((rc = dev_alloc(p, (void**)&p->rb.alt, ((size_t)p->rb_cap + 1) * 8))) return rc;
+        if ((rc = dev_alloc(p, (void**)&p->rb.ctr, 8))) return rc;
+        p->rb.cap = (uint64_t)p->rb_cap;
+        CK(p, cudaMemsetAsync(p->rb.ctr, 0, 8, p->stream));
+        p->rb.hi = 0;
+    }
+    p->d_cursor = gt.n_groups + 2;                       // [2] result cursor [3] merge info
+    p->d_rows_passed = (uint64_t*)(gt.n_groups + 4);     // [4..5] rows that passed the filter
+    CK(p, cudaMemsetAsync(gt.n_groups, 0, 4 * GT_OCC_OFF, p->stream));
+    k_table_init<<<grid_for((int64_t)cap, p->sm_count, 8), 256, 0, p->stream>>>(gt, ap, 0);
+    CK(p, cudaGetLastError());
+    p->stats.kernel_launches++;
+    return BKGPU_OK;
+}
+
+// the group count an earlier launch left in pinned memory: the 4-byte copy after a launch, or the counter block of a fused extraction
+// (read without a synchronisation: a stale value only costs speed)
+static void learn_groups(bkgpu_plan* p) {
+    if (p->h_pinned && p->h_pinned[0] > p->known_groups) p->known_groups = p->h_pinned[0];
+    if (p->h_fused) { const uint32_t g = *(const volatile uint32_t*)p->h_fused; if (g > p->known_groups) p->known_groups = g; }
+}
+
+// device images of an extracted row: one per group expression, per aggregate its final value (+2 for an AVG blob)
+static int agg_n_img(const AggPlan& ap) {
+    int n = ap.n_group;
+    for (int k = 0; k < ap.n_agg; k++) if (!ap.agg[k].hidden) n += ap.agg[k].kind == AG_AVG ? 3 : 1;
+    return n;
+}
+
+// the mapped host buffer of the fused extraction, sized for the groups seen so far (at least 2048 rows); false = too many groups
+// to extract this way (the table is then read back by k_extract)
+static bool ensure_fused(bkgpu_plan* p) {
+    uint32_t want = 2048;
+    while (want < p->known_groups && want < (1u << 16)) want *= 2;
+    if (want < p->known_groups) return false;
+    if (p->h_fused && p->fused_cap >= want) return true;
+    if (p->h_fused) {   // (a launch still running may write into it)
+        cudaStreamSynchronize(p->stream);
+        if (!mapped_put(p->fused_bytes, p->h_fused)) cudaFreeHost(p->h_fused);
+        p->h_fused = p->d_fused = nullptr; p->fused_cap = 0;
+    }
+    const size_t bytes = 32 + (size_t)want * (size_t)agg_n_img(p->c.ap) * 9;
+    uint8_t* h = mapped_take(bytes);
+    if (!h && cudaHostAlloc((void**)&h, bytes, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) { cudaGetLastError(); return false; }
+    if (cudaHostGetDevicePointer((void**)&p->d_fused, h, 0) != cudaSuccess) { cudaGetLastError(); cudaFreeHost(h); return false; }
+    memset(h, 0, 32);
+    p->h_fused = h; p->fused_bytes = bytes; p->fused_cap = want;
+    return true;
+}
+
+// rb_build_agg: a launch appends at most one key per row and rb_build_agg aggregate, except where a probe row meets several build rows (such
+// a launch can still overflow the pair buffer, and the request then fails at bkgpu_finish).  When the keys could outgrow the buffer, it is
+// sorted and deduplicated first (a set does not depend on order), and the launch shrinks to the rows that fit
+static int rb_room(bkgpu_plan* p, const Compiled& c, int64_t* rows) {
+    const uint64_t per = (uint64_t)c.n_rb, cap = p->rb.cap;
+    if (p->rb.hi + (uint64_t)*rows * per > cap) {
+        uint64_t n = 0;
+        const int rc = rb_compact(p, &n);
+        if (rc) return rc;
+        p->rb.hi = n;
+        const int64_t fit = (int64_t)((cap - n) / per) & ~7ll;   // (a multiple of 8 rows: the next launch's validity bitmaps stay byte-aligned)
+        if (fit < 8)
+            return p->fail(BKGPU_ETOOBIG, "rb_build_agg: the pair buffer holds %llu distinct (group, value) pairs and is full: raise rb_pair_capacity",
+                           (unsigned long long)n);
+        if (*rows > fit && !p->join.tail_launch) *rows = fit;   // (the join's tail walks every build row in one launch)
+    }
+    p->rb.hi += (uint64_t)*rows * per;
+    return BKGPU_OK;
+}
+
+int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp) {
+    AggEnv env;
+    env.force_generic = p->force_generic; env.no_lean = p->no_lean; env.no_lean_nulls = p->no_lean_nulls; env.no_lean_mm = p->no_lean_mm;
+    env.lean_fx = p->lean_fx; env.fx_off = p->fx_off;
+    env.scalar_tma = p->scalar_tma; env.smem_cap_log2 = p->smem_cap_log2;
+    env.tail_launch = p->join.tail_launch;
+    env.multi_rank = p->nccl_comm && p->nranks > 1; env.has_post = p->c.post != nullptr;
+    if (c.ap.n_keyw > 0 && p->smem_cap_log2 < 0) learn_groups(p);   // (the shared table is sized from it)
+    env.known_groups = p->known_groups;
+    AggArgs a; AggSelection sel;
+    const int rc = select_agg_launch(c, cols, nrows, vec_ok, jp, env, a, sel);
+    if (rc == BKGPU_ENOMEM) return p->fail(rc, "lean kernel: shared table does not fit");
+    if (rc) return rc;
+    a.gt = p->gt; a.rows_passed = p->d_rows_passed;
+    if (c.kind == PK_JOIN_AGG) a.join = join_args(p, p->join.tail_launch);
+    if (sel.fused_ok && ensure_fused(p)) { a.fused_out = p->d_fused; a.fused_cap = p->fused_cap; }
+    const int64_t kMax = (int64_t)1 << 30;  // rows per launch (32-bit counters inside a CTA)
+    int64_t algo_bytes_per_row = 0;
+    for (int i = 0; i < a.n_cols; i++) algo_bytes_per_row += storage_bytes(a.cols[i].stype);
+    int64_t b_rows = 0;
+    for (int64_t off = 0; off < nrows; off += b_rows) {
+        AggArgs b = a;
+        b.nrows = std::min(kMax, nrows - off);
+        if (c.n_rb) {   // (a compaction swaps the pair buffer with the sort's second buffer)
+            const int rrc = rb_room(p, c, &b.nrows);
+            if (rrc) return rrc;
+            b.rb_keys = p->rb.keys; b.rb_ctr = p->rb.ctr; b.rb_cap = p->rb.cap;
+        }
+        b_rows = b.nrows;
+        for (int i = 0; i < b.n_cols; i++) b.cols[i] = col_at(a.cols[i], off);
+        EventPair* ep = timer_begin(p, p->timed, b.nrows * algo_bytes_per_row, false);
+        cudaError_t e = launch_agg(b, sel.kernel, sel.smem, p->sm_count, p->stream, ep ? ep->a : nullptr);
+        timer_end(p, ep);
+        p->fused_last = b.fused_out != nullptr;
+        if (e != cudaSuccess) return p->cuda_fail(e, "launch_agg");
+        snprintf(p->stats.main_kernel_name, sizeof p->stats.main_kernel_name, "%s", agg_kernel_name(sel.kernel));
+        p->stats.kernel_launches++;
+    }
+    return BKGPU_OK;
+}
+
+static int agg_batch(bkgpu_plan* p, const DevCol* cols, int64_t nrows, int64_t, bool vec_ok) { return launch_agg_batch(p, p->c, cols, nrows, vec_ok); }
+
+// MERGE_AGG of hll_add_agg over host memory: every non-NULL input value must be a RAW sketch, or the push fails (device-resident input is
+// checked by the merge kernel itself, and the request then fails at bkgpu_finish)
+static int hll_check_host_sketches(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows) {
+    const AggPlan& ap = p->c.ap;
+    for (int k = 0; k < ap.n_agg; k++) {
+        if (ap.agg[k].kind != AG_HLL || ap.agg[k].arg_prim != BK_HLL) continue;
+        const ColRef& w = p->c.cols[ap.agg[k].hll_col];
+        for (int i = 0; i < ncols; i++) {
+            if (cols[i].tuple_id != w.tuple_id || cols[i].slot_id != w.slot_id || !cols[i].values || cols[i].length != nrows) continue;   // (bind_columns reports those)
+            for (int64_t r = 0; r < nrows; r++) {
+                if (cols[i].validity && !((cols[i].validity[r >> 3] >> (r & 7)) & 1)) continue;
+                const uint8_t* v = (const uint8_t*)cols[i].values + (size_t)r * HLL_RAW_BYTES;
+                if (memcmp(v, "HYLL", 4) != 0 || v[4] != HLL_ENC_RAW)
+                    return p->fail(BKGPU_EINVAL, "column %d_%d row %lld is not a RAW HLL sketch (\"HYLL\", encoding 255, 16400 bytes): MERGE_AGG of hll_add_agg "
+                                   "merges RAW sketches only", w.tuple_id, w.slot_id, (long long)r);
+            }
+        }
+    }
+    return BKGPU_OK;
+}
+
+// a PK_AGG batch
+int agg_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device) {
+    int rc = on_device ? BKGPU_OK : hll_check_host_sketches(p, cols, ncols, nrows);
+    if (rc) return rc;
+    rc = feed(p, p->c.cols, cols, ncols, nrows, on_device, agg_batch);
+    if (rc) return rc;
+    // learn the cardinality for later batches' table size (no sync: a stale value only costs speed); a launch that extracted its
+    // result has already left the count in h_fused
+    if (p->c.ap.n_keyw > 0 && p->smem_cap_log2 < 0 && p->h_pinned && !p->fused_last)
+        CK(p, cudaMemcpyAsync(p->h_pinned, p->gt.n_groups, 4, cudaMemcpyDeviceToHost, p->stream));
+    return BKGPU_OK;
+}
+
+// groups per rank in the exchanged partial state: never more than the group table can hold (every rank runs the same plan with
+// the same options, so all ranks agree on it) — a 2^14-slot table ships 0.8 MB per rank instead of the 3 MB of the default cap
+static uint32_t eff_pcap(const bkgpu_plan* p) {
+    const int64_t table = p->c.ap.n_keyw == 0 ? 1 : (int64_t)1 << p->group_cap_log2;
+    return (uint32_t)std::min<int64_t>(p->partial_cap, table);
+}
+
+// the collective step of bkgpu_finish: regions -> one set per GPU, the per-GPU partial tables meet once and are folded by K3.
+// Default: compact rows, one ncclAllGather of 1 + bound x (key + lane words) per rank — `bound` = the largest group count any rank
+// held in earlier runs of this plan (2048 on the first run); the merge reports the true maximum and the exchange is repeated once
+// with a larger bound when it did not fit.  Option repartition: all-to-all by key owner.
+static int agg_collective(bkgpu_plan* p, bool* rows_mode) {
+    const AggPlan& ap = p->c.ap;
+    GroupTable& gt = p->gt;
+    *rows_mode = false;
+    const uint32_t pcap = eff_pcap(p);
+    int rc;
+    const bool repart = p->repartition && ap.n_keyw > 0;   // (a scalar aggregate has one group: nothing to partition)
+    EventPair* ep = timer_begin(p, p->timed_coll, 0);
+    if (!repart) {
+        *rows_mode = true;
+        if (p->rank < 0 && nccl_comm_rank(p->nccl_comm, &p->rank) != 0) return p->fail(BKGPU_ENCCL, "ncclCommUserRank: %s", nccl_last_error());
+        uint32_t bound = p->merge_bound ? p->merge_bound : 2048u;
+        if (ap.n_keyw == 0) bound = 1;
+        bound = std::min<uint32_t>(bound, pcap);
+        const size_t rw = (size_t)(ap.n_keyw + ap.n_lanes + ap.n_hll * HLL_ROW_WORDS);
+        const size_t words = 1 + rw * bound;
+        if ((rc = ensure_buf(p, (void**)&p->d_partial, &p->d_partial_cap, words * 8))) return rc;
+        if ((rc = ensure_buf(p, (void**)&p->d_gather, &p->d_gather_cap, words * 8 * (size_t)p->nranks))) return rc;
+        CK(p, cudaMemsetAsync(p->d_partial, 0, 8, p->stream));
+        k_partial_export_rows<<<grid_for((int64_t)gt.cap_mask + 1, p->sm_count, 1), 256, 0, p->stream>>>(gt, ap, p->d_partial, bound);
+        CK(p, cudaGetLastError());
+        if (nccl_all_gather(p->nccl_comm, p->d_partial, p->d_gather, words, p->stream) != 0) return p->fail(BKGPU_ENCCL, "ncclAllGather: %s", nccl_last_error());
+        const int gx = (int)std::min<uint32_t>(std::max<uint32_t>((bound + 255) / 256, 1), 64);
+        k_partial_merge_rows<<<dim3((unsigned)gx, (unsigned)p->nranks), 256, 0, p->stream>>>(gt, ap, p->d_gather, words, bound, p->nranks, p->rank, p->d_cursor + 1);
+        CK(p, cudaGetLastError());
+        p->merge_bound_used = bound;
+        p->stats.kernel_launches += 2;
+        timer_end(p, ep);
+        return BKGPU_OK;
+    }
+    // hash repartition: every rank keeps only the groups it owns — an all-to-all of per-owner segments instead of the
+    // all-gather; the merged table (and the result) of a rank is its partition, the union over ranks is the answer
+    const size_t words = 1 + (size_t)(ap.n_keyw + ap.n_lanes) * pcap;
+    if ((rc = ensure_buf(p, (void**)&p->d_partial, &p->d_partial_cap, words * 8 * (size_t)p->nranks))) return rc;
+    if ((rc = ensure_buf(p, (void**)&p->d_gather, &p->d_gather_cap, words * 8 * (size_t)p->nranks))) return rc;
+    if (!p->d_part_cursors && (rc = dev_alloc(p, (void**)&p->d_part_cursors, 4 * (size_t)p->nranks))) return rc;
+    if (p->nranks > 1024) return p->cuda_fail(cudaErrorInvalidValue, "k_partial_counts: more than 1024 ranks");
+    CK(p, cudaMemsetAsync(p->d_part_cursors, 0, sizeof(uint32_t) * (size_t)p->nranks, p->stream));
+    k_partial_export_parts<<<grid_for((int64_t)gt.cap_mask + 1, p->sm_count, 8), 256, 0, p->stream>>>(gt, ap, p->d_partial, words, pcap, p->d_part_cursors, p->nranks);
+    k_partial_counts<<<1, 1024, 0, p->stream>>>(p->d_partial, words, p->d_part_cursors, pcap, p->nranks);
+    CK(p, cudaGetLastError());
+    if (nccl_all_to_all(p->nccl_comm, p->d_partial, p->d_gather, words, p->nranks, p->stream) != 0) return p->fail(BKGPU_ENCCL, "all-to-all: %s", nccl_last_error());
+    k_table_init<<<grid_for((int64_t)gt.cap_mask + 1, p->sm_count, 8), 256, 0, p->stream>>>(gt, ap, 1);   // (keeps the overflow flag an export beyond partial_capacity raised)
+    CK(p, cudaGetLastError());
+    k_partial_merge<<<grid_for(pcap, p->sm_count, 8), 256, 0, p->stream>>>(gt, ap, p->d_gather, words, pcap, p->nranks);
+    CK(p, cudaGetLastError());
+    timer_end(p, ep);
+    p->stats.kernel_launches += 4;
+    return BKGPU_OK;
+}
+
+// [LIMIT ->] [SORT ->] [HAVING ->] above the aggregate: the extracted rows (still on the device) become typed columns and run through
+// the post fragment's sort / filter kernels; only the final rows travel to the host
+static int agg_post(bkgpu_plan* p, uint32_t n_out, uint32_t out_cap) {
+    const Compiled& pc = *p->c.post;
+    const size_t nc = pc.cols.size();
+    int rc;
+    for (size_t c = 0; c < nc; c++)
+        if ((rc = store_reserve(p, p->post, c, std::max<int64_t>(n_out, 1), std::max<int64_t>(n_out, 2048), true))) return rc;
+    PostCols pcs; memset(&pcs, 0, sizeof pcs);
+    pcs.n = (int)nc;
+    int img = 0;
+    for (size_t c = 0; c < nc; c++) {   // (post columns = the aggregate's output columns, in order: plan.cpp::lower_post)
+        pcs.img[c] = img; pcs.stype[c] = prim_storage(pc.cols[c].prim); pcs.values[c] = p->post.cols[c].vals; pcs.null_bytes[c] = p->post.cols[c].nulls;
+        img += p->c.out_cols[c].kind == 1 ? 2 : 1;
+    }
+    if (n_out) {
+        k_images_to_columns<<<grid_for(n_out, p->sm_count, 8), 256, 0, p->stream>>>(p->d_outv, p->d_outn, out_cap, n_out, pcs);
+        CK(p, cudaGetLastError());
+    }
+    std::vector<DevCol> dc(std::max<size_t>(nc, 1));
+    for (size_t c = 0; c < nc; c++)
+        if ((rc = store_pack(p, p->post, c, n_out, 16, nullptr, &dc[c]))) return rc;
+    p->stats.kernel_launches += 1 + (int64_t)nc;
+    sort_reset(p->post_sort);
+    bkgpu_stats scratch{};   // (the post fragment's kernels are not the request's "main kernel")
+    if (n_out && (rc = sort_push(p->post_sort, dc.data(), n_out, &scratch))) return rc;
+    std::vector<SortOutCol> cols; int64_t rows = 0;
+    if ((rc = sort_finish(p->post_sort, nullptr, 1, &scratch, cols, &rows))) return rc;
+    p->stats.kernel_launches += scratch.kernel_launches;
+    set_result(p, cols, rows, p->c.out_cols.data());
+    return BKGPU_OK;
+}
+
+// the one wait of a request.  With several ranks on a host whose CPU budget is small (8 ranks under a 16-CPU cgroup quota: two CPUs per
+// rank for the python thread, NCCL's proxy thread and this wait) a spinning wait burns the quota the other ranks' launches need:
+// there the thread sleeps on a blocking-sync event instead (option blocking_sync: -1 auto, 0 spin, 1 sleep)
+static int agg_wait(bkgpu_plan* p) {
+    const double t0 = HostClock::now();
+    if (p->blocking_wait) {
+        if (!p->wait_event) CK(p, cudaEventCreateWithFlags(&p->wait_event, cudaEventBlockingSync | cudaEventDisableTiming));
+        CK(p, cudaEventRecord(p->wait_event, p->stream));
+        CK(p, cudaEventSynchronize(p->wait_event));
+    } else CK(p, cudaStreamSynchronize(p->stream));
+    p->hclk.extract_wait += HostClock::now() - t0;
+    return BKGPU_OK;
+}
+
+// what the counter block of a finished request tells the plan: rows that passed, FX's exact-path count, the groups it holds
+static int agg_take_counters(bkgpu_plan* p, const uint32_t* ctr) {
+    memcpy(&p->rows_passed_host, ctr + 4, 8);
+    // FX: values beyond the sampled scale are added exactly, one global atomic each; a plan whose double columns keep producing many of them
+    // (a column spanning dozens of binades, outliers dominating the sample) goes back to the CAS kernel for its later launches
+    if (ctr[GT_FX_EXACT] > 4096 && (uint64_t)ctr[GT_FX_EXACT] * 64 > (uint64_t)std::max<int64_t>(p->rows_passed_host, 1)) p->fx_off = 1;
+    if (ctr[1]) return p->fail(BKGPU_ETOOBIG, "group table overflow (capacity 2^%d slots / partial_capacity %lld): raise group_capacity_log2",
+                               (int)p->gt.cap_log2, (long long)p->partial_cap);
+    if (ctr[0] > p->known_groups) p->known_groups = ctr[0];
+    p->finish_groups = ctr[0];
+    return BKGPU_OK;
+}
+
+// a BITMAP column (bkgpu.h): one bitmap per row, each the device's bytes for (slot, rb_idx), or the 8-byte empty bitmap
+// ("3a300000 00000000": the reference's initialize gives every group an empty bitmap, so a group whose values were all NULL returns it)
+static void rb_column(bkgpu_plan* p, HostCol& hc, const uint64_t* slot, int64_t rows, int rb_idx) {
+    static const uint8_t empty[8] = {0x3a, 0x30, 0, 0, 0, 0, 0, 0};
+    std::vector<int64_t> b((size_t)rows);   // each row's bitmap in the directory, -1 = none
+    int64_t total = 0;
+    for (int64_t r = 0; r < rows; r++) {
+        const uint32_t id = (uint32_t)(slot[r] << 2) | (uint32_t)rb_idx;
+        const auto it = std::lower_bound(p->rb.bid.begin(), p->rb.bid.end(), id);
+        b[r] = it != p->rb.bid.end() && *it == id ? (int64_t)(it - p->rb.bid.begin()) : -1;
+        total += b[r] < 0 ? 8 : (int64_t)(p->rb.off[b[r] + 1] - p->rb.off[b[r]]);
+    }
+    std::vector<uint8_t>& col = p->rb.col[rb_idx];
+    col.resize(((size_t)rows + 1) * 8 + (size_t)total);
+    int64_t* offs = (int64_t*)col.data();
+    uint8_t* d = col.data() + ((size_t)rows + 1) * 8;
+    offs[0] = 0;
+    for (int64_t r = 0; r < rows; r++) {
+        const size_t len = b[r] < 0 ? 8 : (size_t)(p->rb.off[b[r] + 1] - p->rb.off[b[r]]);
+        memcpy(d + offs[r], b[r] < 0 ? empty : p->rb.bytes + p->rb.off[b[r]], len);
+        offs[r + 1] = offs[r] + (int64_t)len;
+    }
+    hc.elem = -1;
+    hc.varlen = &col;
+}
+
+// typed host columns from `n_out` extracted rows (images + null bytes, column-major with stride `stride`), after OFFSET / LIMIT
+static void agg_result(bkgpu_plan* p, const uint64_t* hv, const uint8_t* hn, size_t stride, uint32_t n_out) {
+    const int64_t rows = n_out;
+    const int64_t skip = p->c.offset > 0 ? std::min<int64_t>(p->c.offset, rows) : 0;
+    int64_t lim = p->c.agg_limit;   // AggNode::get_next stops at its limit (agg_node.cpp:555)
+    if (p->c.limit >= 0 && (lim < 0 || p->c.limit < lim)) lim = p->c.limit;
+    int64_t keep = rows - skip;
+    if (lim >= 0 && keep > lim) keep = lim;
+    p->result.clear();
+    int img = 0, rb_idx = 0;
+    for (const OutCol& oc : p->c.out_cols) {
+        HostCol hc; hc.desc = oc;
+        const uint64_t* v = hv + (size_t)img * stride + skip;
+        const uint8_t* nb = hn + (size_t)img * stride + skip;
+        if (oc.kind == 3) {   // rb_build_agg: the group's slot, whose bitmap the device build serialized (a group without a value: the empty one)
+            rb_column(p, hc, v, keep, rb_idx++);
+            img++;
+            p->result.push_back(std::move(hc));
+            continue;
+        }
+        hc.elem = oc.kind == 1 ? 16 : oc.kind == 2 ? HLL_RAW_BYTES : storage_bytes(prim_storage(oc.prim));
+        hc.values.assign((size_t)std::max<int64_t>(keep, 1) * (size_t)hc.elem, 0);
+        // (a NULL's image is 0, which is also what a NULL row's value bytes hold)
+        uint8_t* d = hc.values.data();
+        if (oc.kind == 1) {
+            const uint64_t* v2 = hv + (size_t)(img + 1) * stride + skip;
+            for (int64_t r = 0; r < keep; r++) { memcpy(d + (size_t)r * 16, v + r, 8); memcpy(d + (size_t)r * 16 + 8, v2 + r, 8); }
+        } else if (oc.kind == 2) {
+            // hll_row_init's RAW sketch (hll_common.cpp:834-842): "HYLL", encoding HLL_RAW, then the registers.  hll_row_add invalidates the
+            // cached cardinality (bit 7 of header byte 15) whenever a register grows, which the first value always does: a group that
+            // received a value has the bit set, a group without one (every argument NULL) is the empty sketch with the byte 0
+            for (int64_t r = 0; r < keep; r++) {
+                uint8_t* o = d + (size_t)r * HLL_RAW_BYTES;
+                memcpy(o, "HYLL", 4); o[4] = HLL_ENC_RAW;
+                if (v[r]) { o[15] = 0x80; memcpy(o + HLL_HDR_BYTES, p->hll_host.data() + (size_t)(v[r] - 1) * HLL_REGISTERS, HLL_REGISTERS); }
+            }
+        } else switch (prim_storage(oc.prim)) {
+            case ST_I32: for (int64_t r = 0; r < keep; r++) { const int32_t x = (int32_t)(int64_t)v[r]; memcpy(d + (size_t)r * 4, &x, 4); } break;
+            case ST_U32: for (int64_t r = 0; r < keep; r++) { const uint32_t x = (uint32_t)v[r]; memcpy(d + (size_t)r * 4, &x, 4); } break;
+            case ST_F32: for (int64_t r = 0; r < keep; r++) { double x; memcpy(&x, v + r, 8); const float f = (float)x; memcpy(d + (size_t)r * 4, &f, 4); } break;
+            case ST_U8: for (int64_t r = 0; r < keep; r++) d[r] = v[r] ? 1 : 0; break;
+            default:
+                if (hc.elem == 8) { if (keep > 0) memcpy(d, v, (size_t)keep * 8); }
+                else for (int64_t r = 0; r < keep; r++) memcpy(d + (size_t)r * hc.elem, v + r, 8);
+                break;
+        }
+        if (keep > 0 && memchr(nb, 1, (size_t)keep)) {
+            hc.validity.assign((size_t)(keep + 7) / 8 + 1, 0xFF);
+            for (int64_t r = 0; r < keep; r++) if (nb[r]) { hc.validity[(size_t)r >> 3] &= (uint8_t)~(1u << (r & 7)); if (oc.kind == 0) memset(d + (size_t)r * hc.elem, 0, (size_t)hc.elem); }
+        }
+        img += oc.kind == 1 ? 2 : 1;
+        p->result.push_back(std::move(hc));
+    }
+    p->result_rows = keep; p->result_pos = 0;
+}
+
+// hll_add_agg: the arena's claimed blocks to the host (the extracted rows reference them), after the request's last kernel.  A claim
+// that found the arena full fails the request: a sketch that lost values would be wrong, not approximate
+static int hll_fetch(bkgpu_plan* p) {
+    if (!p->c.ap.n_hll) return BKGPU_OK;
+    uint32_t ctr[3] = {0, 0, 0};
+    CK(p, cudaMemcpyAsync(ctr, p->gt.hll_ctr, 12, cudaMemcpyDeviceToHost, p->stream));
+    CK(p, cudaStreamSynchronize(p->stream));
+    if (ctr[2]) return p->fail(BKGPU_EINVAL, "MERGE_AGG of hll_add_agg: an input value is not a RAW HLL sketch (\"HYLL\", encoding 255, 16400 bytes)");
+    if (ctr[1] || ctr[0] > p->gt.hll_cap)
+        return p->fail(BKGPU_ETOOBIG, "hll_add_agg: more than %u sketches (groups x hll_add_agg aggregates with a value): raise hll_group_capacity",
+                       p->gt.hll_cap);
+    p->hll_host.resize((size_t)ctr[0] * HLL_REGISTERS);
+    if (ctr[0]) CK(p, cudaMemcpy(p->hll_host.data(), p->gt.hll_regs, (size_t)ctr[0] * HLL_REGISTERS, cudaMemcpyDeviceToHost));
+    p->stats.d2h_bytes += (int64_t)p->hll_host.size() + 8;
+    return BKGPU_OK;
+}
+
+int agg_finish(bkgpu_plan* p) {
+    const AggPlan& ap = p->c.ap;
+    GroupTable& gt = p->gt;
+    uint32_t host_counts[2] = {0, 0};
+    uint64_t* finish_hv = nullptr; uint8_t* finish_hn = nullptr; uint32_t finish_n_out = 0, finish_out_cap = 0;
+    const bool multi = p->nccl_comm && p->nranks > 1;
+    bool rows_mode = false;
+    const int n_img = agg_n_img(ap);
+    int rc;
+    // the request ended with a launch that extracted its own result into mapped host memory: one wait, nothing else on the device
+    if (p->fused_last && !multi && !p->c.post) {
+        if ((rc = agg_wait(p))) return rc;
+        const uint32_t* ctr = (const uint32_t*)p->h_fused;
+        if ((rc = agg_take_counters(p, ctr))) return rc;
+        const uint32_t n = ctr[0];
+        if (n <= p->fused_cap) {
+            p->stats.d2h_bytes += (int64_t)(32 + (size_t)n * (size_t)n_img * 9);
+            const uint64_t* hv = (const uint64_t*)(p->h_fused + 32);
+            agg_result(p, hv, (const uint8_t*)(hv + (size_t)n * (size_t)n_img), n, n);
+            return BKGPU_OK;
+        }
+        // more groups than the buffer holds: the table is read back below (the next launch's buffer is sized for them)
+    }
+  for (int mtry = 0; mtry < 3; mtry++) {   // (a second trip only when some rank held more groups than the exchange was sized for)
+    { const double t0 = HostClock::now(); if (multi && (rc = agg_collective(p, &rows_mode))) return rc; p->hclk.collective += HostClock::now() - t0; }
+    uint32_t n_out = 0, out_cap = 0, merge_max = 0;
+    uint64_t* hv = nullptr; uint8_t* hn = nullptr;
+    bool redo_merge = false;
+    for (int attempt = 0; attempt < 2; attempt++) {
+        // speculative extraction into the buffers kept from earlier runs: counts, cursor and rows come back
+        // in ONE synchronisation; only a result larger than the buffers costs a second round
+        uint32_t want = std::max<uint32_t>(std::max<uint32_t>(p->known_groups, 1), attempt ? std::max<uint32_t>(host_counts[0], 1) : 1);
+        if (ap.n_keyw == 0) want = 1;
+        if (p->out_cap_alloc < want) {
+            dev_free(p, p->d_outv); p->d_outv = nullptr; p->d_outn = nullptr;
+            size_t cap = std::max<size_t>(want, 2048);
+            if ((rc = dev_alloc(p, (void**)&p->d_outv, cap * 9 * (size_t)n_img + 64))) return rc;   // values, then the null bytes: ONE copy brings both back
+            p->d_outn = (uint8_t*)(p->d_outv + cap * (size_t)n_img);
+            p->out_cap_alloc = cap;
+        }
+        out_cap = (uint32_t)p->out_cap_alloc;
+        CK(p, cudaMemsetAsync(p->d_cursor, 0, sizeof(uint32_t), p->stream));
+        k_extract<<<grid_for((int64_t)gt.cap_mask + 1, p->sm_count, 1), 256, 0, p->stream>>>(gt, ap, p->d_outv, p->d_outn, out_cap, p->d_cursor, p->c.emit_default ? 1 : 0);
+        CK(p, cudaGetLastError());
+        p->stats.kernel_launches++;
+        const size_t n_words = (size_t)out_cap * (size_t)n_img;
+        if (p->h_out_cap < n_words) {   // pinned: the four copies below are truly asynchronous and land in one synchronisation
+            if (p->h_outv) cudaFreeHost(p->h_outv);
+            p->h_outv = nullptr; p->h_outn = nullptr; p->h_out_cap = 0;
+            CK(p, cudaHostAlloc((void**)&p->h_outv, n_words * 9 + 64, cudaHostAllocDefault));
+            p->h_out_cap = n_words;
+        }
+        hv = p->h_outv; hn = p->h_outn = (uint8_t*)(p->h_outv + n_words);
+        // two copies, one synchronisation: the 32-byte counter block (groups, overflow, rows extracted, merge info, rows passed) and
+        // the extracted rows (values + null bytes, contiguous on both sides)
+        uint32_t local_ctr[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        uint32_t* hc3 = p->h_pinned ? p->h_pinned + 8 : local_ctr;   // [8] groups [9] overflow [10] rows extracted [11] merge info [12..13] rows passed
+        CK(p, cudaMemcpyAsync(hc3, gt.n_groups, 32, cudaMemcpyDeviceToHost, p->stream));
+        if ((const uint8_t*)p->d_outn == (const uint8_t*)(p->d_outv + n_words)) CK(p, cudaMemcpyAsync(hv, p->d_outv, n_words * 9, cudaMemcpyDeviceToHost, p->stream));
+        else {
+            CK(p, cudaMemcpyAsync(hv, p->d_outv, n_words * 8, cudaMemcpyDeviceToHost, p->stream));
+            CK(p, cudaMemcpyAsync(hn, p->d_outn, n_words, cudaMemcpyDeviceToHost, p->stream));
+        }
+        if ((rc = agg_wait(p))) return rc;
+        host_counts[0] = hc3[0]; host_counts[1] = hc3[1]; n_out = hc3[2]; merge_max = hc3[3];
+        if (rows_mode) {
+            const uint32_t mx = merge_max;
+            if (mx > p->merge_bound_used) {   // nothing was merged (k_partial_merge_rows): exchange again, sized for what the ranks really hold
+                if (mx > eff_pcap(p)) return p->fail(BKGPU_ETOOBIG, "a rank holds %u groups, more than partial_capacity %lld: raise partial_capacity", mx, (long long)p->partial_cap);
+                p->merge_bound = (mx + 63u) & ~63u;
+                redo_merge = true;
+                break;
+            }
+            const uint32_t learned = (std::max<uint32_t>(mx, 1u) + 63u) & ~63u;
+            if (learned > p->merge_bound) p->merge_bound = learned;
+        }
+        p->stats.d2h_bytes += (int64_t)(n_words * 9 + 12);
+        if ((rc = agg_take_counters(p, hc3))) return rc;
+        if (n_out <= out_cap) break;   // everything fitted
+    }
+    if (!redo_merge) { finish_hv = hv; finish_hn = hn; finish_n_out = n_out; finish_out_cap = out_cap; break; }
+    if (mtry == 2) return p->fail(BKGPU_ENCCL, "partial-state exchange did not converge");
+  }
+    uint32_t n_out = finish_n_out, out_cap = finish_out_cap;
+    if (n_out > out_cap) n_out = out_cap;
+    if ((rc = hll_fetch(p))) return rc;
+    if (p->c.n_rb && (rc = rb_build(p))) return rc;
+    if (p->c.post) return agg_post(p, n_out, out_cap);
+    agg_result(p, finish_hv, finish_hn, out_cap, n_out);
+    return BKGPU_OK;
+}
+
+// Re-arm the table for the next request.  A finished run knows how many groups its table holds (the count came back with the result):
+// clear those slots through the occupied list instead of re-initialising the whole capacity (2^20 slots = 44 MB by default)
+int agg_reset(bkgpu_plan* p) {
+    if (p->state == S_FINISHED && p->finish_groups >= 0 && p->c.ap.n_keyw > 0)
+        k_table_clear<<<grid_for(p->finish_groups, p->sm_count, 8), 256, 0, p->stream>>>(p->gt, p->c.ap, (uint32_t)p->finish_groups);
+    else k_table_init<<<grid_for((int64_t)p->gt.cap_mask + 1, p->sm_count, 8), 256, 0, p->stream>>>(p->gt, p->c.ap, 0);
+    CK(p, cudaGetLastError());
+    p->finish_groups = -1;
+    p->fused_last = false;
+    if (p->rb.ctr) { CK(p, cudaMemsetAsync(p->rb.ctr, 0, 8, p->stream)); p->rb.hi = 0; }   // (rb_build_agg: the pair buffer is empty again)
+    p->stats.kernel_launches++;
+    return BKGPU_OK;
+}
+
+// ---- partial state (bkgpu_partial_*): compact rows, the layout the in-library all-gather ships: [u64 groups][groups x (key words +
+// lane words + HLL_ROW_WORDS per hll_add_agg)] ----
+size_t agg_partial_bytes(const bkgpu_plan* p) {
+    return 8 * (1 + (size_t)(p->c.ap.n_keyw + p->c.ap.n_lanes + p->c.ap.n_hll * HLL_ROW_WORDS) * (size_t)eff_pcap(p));
+}
+int agg_partial_export(bkgpu_plan* p, void* dev_dst) {
+    CK(p, cudaMemsetAsync(dev_dst, 0, 8, p->stream));
+    k_partial_export_rows<<<grid_for((int64_t)p->gt.cap_mask + 1, p->sm_count, 1), 256, 0, p->stream>>>(p->gt, p->c.ap, (uint64_t*)dev_dst, eff_pcap(p));
+    CK(p, cudaGetLastError());
+    p->stats.kernel_launches += 1;
+    uint64_t held = 0; uint32_t ov = 0, hll_ctr[3] = {0, 0, 0};
+    CK(p, cudaMemcpyAsync(&held, dev_dst, 8, cudaMemcpyDeviceToHost, p->stream));
+    CK(p, cudaMemcpyAsync(&ov, p->gt.overflow, 4, cudaMemcpyDeviceToHost, p->stream));
+    if (p->gt.hll_ctr) CK(p, cudaMemcpyAsync(hll_ctr, p->gt.hll_ctr, 12, cudaMemcpyDeviceToHost, p->stream));
+    CK(p, cudaStreamSynchronize(p->stream));
+    if (hll_ctr[2]) return p->fail(BKGPU_EINVAL, "MERGE_AGG of hll_add_agg: an input value is not a RAW HLL sketch (\"HYLL\", encoding 255, 16400 bytes)");
+    if (hll_ctr[1]) return p->fail(BKGPU_ETOOBIG, "hll_add_agg: more than %u sketches: raise hll_group_capacity", p->gt.hll_cap);
+    if (ov) return p->fail(BKGPU_ETOOBIG, "group table overflow (capacity 2^%d slots): raise group_capacity_log2", (int)p->gt.cap_log2);
+    if (held > eff_pcap(p)) return p->fail(BKGPU_ETOOBIG, "this rank holds %llu groups, more than partial_capacity=%lld", (unsigned long long)held, (long long)p->partial_cap);
+    return BKGPU_OK;
+}
+// fold `nranks` exported partial states into the table, then finish the request on this plan alone
+int agg_partial_merge(bkgpu_plan* p, const void* dev_src, int nranks) {
+    const uint32_t pcap = eff_pcap(p);
+    k_table_init<<<grid_for((int64_t)p->gt.cap_mask + 1, p->sm_count, 8), 256, 0, p->stream>>>(p->gt, p->c.ap, 1);
+    CK(p, cudaGetLastError());
+    const int gx = (int)std::min<uint32_t>(std::max<uint32_t>((pcap + 255) / 256, 1), 64);
+    k_partial_merge_rows<<<dim3((unsigned)gx, (unsigned)nranks), 256, 0, p->stream>>>(p->gt, p->c.ap, (const uint64_t*)dev_src, agg_partial_bytes(p) / 8, pcap, nranks,
+                                                                                   -1 /* fold every segment */, p->d_cursor + 1);
+    CK(p, cudaGetLastError());
+    p->fused_last = false;   // (the merged table is read back by k_extract)
+    p->stats.kernel_launches += 2;
+    void* comm = p->nccl_comm; int nr = p->nranks; p->nccl_comm = nullptr; p->nranks = 1;  // already merged: finalize locally
+    const int rc = agg_finish(p);
+    p->nccl_comm = comm; p->nranks = nr;
+    return rc;
+}

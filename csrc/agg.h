@@ -1,4 +1,5 @@
-// agg.h — kernel argument block and host launchers of the filter+aggregate kernels (agg.cu).
+// agg.h — the argument blocks of the filter+aggregate kernels and the launchers that cross translation units: the direct kernels
+// (agg_direct*.cu), the TMA-staged COUNT(*) WHERE (scalar_tma.cu) and the join that returns rows (agg.cu, called by join.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include "dev_types.h"
@@ -73,54 +74,16 @@ struct AggArgs {
     uint64_t rb_cap;
 };
 
-// typed columns built from the aggregate's extracted images (input of the post fragment)
-struct PostCols { int32_t n; int32_t img[MAX_COLS]; int32_t stype[MAX_COLS]; uint8_t* values[MAX_COLS]; uint8_t* null_bytes[MAX_COLS]; };
-cudaError_t launch_images_to_columns(const uint64_t* outv, const uint8_t* outn, uint32_t out_cap, uint32_t n, const PostCols& pc, cudaStream_t s);
+// a row id that is no row: the NULL-extended side of an outer join's pair, a dimension without a partner in a star join's tuple
+constexpr uint32_t JOIN_NO_ROW = 0xFFFFFFFFu;
 enum AggKernel : int;   // agg_select.h: the kernel select_agg_launch chose for a batch
 // scalar_tma.cu: TMA-staged COUNT(*) WHERE int32 <cmp> c (the batch has the kernel's shape)
 cudaError_t launch_count_where_tma(const AggArgs& a, int sm_count, cudaStream_t s, cudaEvent_t start);
-// the aggregate kernel `k` over one batch; `smem`: its dynamic shared memory (AggSelection::smem).  `start` (optional) is recorded on `s`
-// right before the kernel launch, after the launch setup
-cudaError_t launch_agg(const AggArgs& a, AggKernel k, size_t smem, int sm_count, cudaStream_t s, cudaEvent_t start);
 cudaError_t launch_direct_np0(const AggArgs& a, AggKernel k, int sm_count, size_t smem, cudaStream_t s, cudaEvent_t start);
 cudaError_t launch_direct_np1(const AggArgs& a, AggKernel k, int sm_count, size_t smem, cudaStream_t s, cudaEvent_t start);
 cudaError_t launch_direct_np2(const AggArgs& a, AggKernel k, int sm_count, size_t smem, cudaStream_t s, cudaEvent_t start);
-cudaError_t launch_join_build(const DevCol& key, int from_prim, int cast_prim, int64_t nrows, uint64_t* keys, uint32_t* rows, uint32_t cap_mask, cudaStream_t s);
-// FK -> PK join fast path: unique build keys, looked up through a dense array (small key range) or a packed
-// (key32 << 32 | row) table; build-side columns are gathered to probe-row alignment
-struct JoinFast {
-    int32_t mode;               // 0 = none, 1 = dense array, 2 = packed 32-bit-key table
-    const uint32_t* dense; uint64_t dense_min; uint64_t dense_size; uint64_t bias;
-    const uint64_t* packed; uint32_t packed_mask;
-};
-struct GatherCols { int32_t n; const uint8_t* src[MAX_COLS]; uint8_t* dst[MAX_COLS]; int32_t elem[MAX_COLS]; };
-cudaError_t launch_join_minmax(const DevCol& key, int from_prim, int cast_prim, int64_t nrows, uint64_t bias, uint64_t* mm, cudaStream_t s);
-cudaError_t launch_join_build_fast(const DevCol& key, int from_prim, int cast_prim, int64_t nrows, const JoinFast& jf, uint32_t* dense_w, uint64_t* packed_w, uint32_t* dup_flag, cudaStream_t s);
-cudaError_t launch_join_gather(const DevCol& probe_key, int from_prim, int cast_prim, int64_t nrows, const JoinFast& jf, const GatherCols& gc, uint32_t* miss_flag, cudaStream_t s);
-cudaError_t launch_join_compose(const JoinFast& jf, const uint32_t* attr_by_row, uint32_t* attr_of_key, uint64_t* packed_attr, uint32_t* bad_flag, cudaStream_t s);
 // a JOIN that returns rows: (probe row, build row) pairs of the joined rows that pass the conditions, then one gather per output column
 // (FULL, not the tail: k_join_pairs_full, which also emits the probe rows without a partner)
 cudaError_t launch_join_pairs(const AggArgs& a, uint32_t* pairs, uint32_t cap, uint32_t* cursor, int sm_count, cudaStream_t s);
-// element `which` of each `width`-word row-id tuple addresses `src` (pairs: width 2); dst_null may be nullptr when no element can be NULL
-cudaError_t launch_join_rows_gather(const DevCol& src, const uint32_t* tuples, int width, int which, uint32_t n, int elem_bytes, uint8_t* dst, uint8_t* dst_null, cudaStream_t s);
-// star join (PK_STAR_AGG): per dimension with unique keys, the fact foreign key, its slot in the row-id tuple and the dimension's key index
-struct StarLookup { DevCol fk; int32_t from_prim, cast_prim, slot; JoinFast jf; };
-struct StarProbe { StarLookup d[4]; int32_t n; int32_t width; int64_t nrows; int32_t vec; };
-// the build-time filter of one dimension: program over the plan's columns (this dimension's retained rows), validity of its join key.
-// Also a two-table join child's own filter (its retained build rows, or one probe batch).
-struct StarFilter { DevCol cols[MAX_COLS]; Program prog; int32_t key_col; int64_t nrows; };
-// `dropped` (optional): dropped[row] = 2 where the conjunction is not TRUE (the join's matched[] of a filtered build side)
-cudaError_t launch_star_dim_filter(const StarFilter& f, uint32_t* keybits, uint8_t* dropped, cudaStream_t s);
-cudaError_t launch_star_probe(const StarProbe& sp, uint32_t* out, uint32_t* cursor, int sm_count, cudaStream_t s);
-cudaError_t launch_star_expand(const DevCol& fk, int from_prim, int cast_prim, const uint64_t* keys, const uint32_t* rows, uint32_t cap_mask, const uint32_t* in, uint32_t n_in,
-                               int width, int slot, uint32_t* out, uint32_t cap, uint32_t* cursor, cudaStream_t s);
-cudaError_t launch_table_init(const GroupTable& gt, const AggPlan& ap, cudaStream_t s, int keep_overflow = 0);
-cudaError_t launch_table_clear(const GroupTable& gt, const AggPlan& ap, uint32_t n_occupied, cudaStream_t s);
-cudaError_t launch_partial_export_rows(const GroupTable& gt, const AggPlan& ap, uint64_t* dst, uint32_t bound, cudaStream_t s);
-cudaError_t launch_partial_merge_rows(const GroupTable& gt, const AggPlan& ap, const uint64_t* src, size_t words_per_rank, uint32_t bound, int nranks, int self,
-                                      uint32_t* max_count, cudaStream_t s);
-cudaError_t launch_partial_export_parts(const GroupTable& gt, const AggPlan& ap, uint64_t* dst, size_t words_per_seg, uint32_t pcap, uint32_t* cursors, int nranks, cudaStream_t s);
-cudaError_t launch_partial_merge(const GroupTable& gt, const AggPlan& ap, const uint64_t* src, size_t words_per_rank, uint32_t pcap, int nranks, cudaStream_t s);
-cudaError_t launch_extract(const GroupTable& gt, const AggPlan& ap, uint64_t* outv, uint8_t* outn, uint32_t out_cap, uint32_t* cursor, int emit_default, cudaStream_t s);
 
 }  // namespace bk

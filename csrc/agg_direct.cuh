@@ -555,7 +555,7 @@ static __device__ __noinline__ void global_add_f64(const AggArgs& a, uint64_t k0
     const int slot = table_upsert<false, 0>(gt.state, gt.keys, gt.cap_mask, key, ap.n_keyw, ap.n_keyw == 1 ? hash_key1(key[0]) : hash_key(key, ap.n_keyw), (int)gcap, gt.n_groups);
     if (slot < 0) { atomicExch(gt.overflow, 1u); return; }
     lane_atomic<false>(LN_ADD_F64, gt.lanes + (size_t)glob_lane * gcap + slot, f64_bits(x));
-    atomicAdd(gt.n_groups + GT_FX_EXACT, 1u);   // values that took this path: when they are many the host stops choosing FX for this plan (api.cu)
+    atomicAdd(gt.n_groups + GT_FX_EXACT, 1u);   // values that took this path: when they are many the host stops choosing FX for this plan (agg.cu)
 }
 __device__ __forceinline__ void reds_add32(uint32_t a, uint32_t v) { asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
 // one value into the fixed-point limbs of `slot`: word = shared address of the slot's {mid, hi} pair, ext = of its low-extension limb

@@ -1,6 +1,7 @@
 // api.cu — the C ABI of include/bkgpu.h: plan lifecycle (ExecNode::init/open/get_next/close
-// inverted into init/open/push/finish/get_next/close), batch staging, the aggregate's launch, exchange and result materialisation.
-// The hash join's host path is join.cu; the plan object (bkgpu_plan) is api_state.h.
+// inverted into init/open/push/finish/get_next/close), the device buffer cache, batch staging, resident regions and the partial-state entry
+// points.  Each plan kind's work is its stage's: the aggregate agg.cu, the hash join join.cu, ORDER BY / filter sort.cu, the window stage
+// window.cu; the plan object (bkgpu_plan) is api_state.h.
 #include <dlfcn.h>
 #include <sched.h>
 #include <string.h>
@@ -110,6 +111,8 @@ size_t size_class(size_t b) {   // eight classes per power of two: at most 12.5 
 }
 }  // namespace
 extern "C" void bkgpu_release_cache(void) { dev_cache().release_all(); mapped_cache().release_all(); }
+uint8_t* mapped_take(size_t bytes) { return mapped_cache().take(bytes); }
+bool mapped_put(size_t bytes, uint8_t* buf) { return mapped_cache().put(bytes, buf); }
 
 int dev_alloc(bkgpu_plan* p, void** out, size_t bytes) {
     const size_t sc = size_class(bytes ? bytes : 8);
@@ -143,20 +146,6 @@ int ensure_buf(bkgpu_plan* p, void** ptr, size_t* cap, size_t bytes) {
     if (rc == BKGPU_OK) *cap = bytes;
     return rc;
 }
-// record = false: the caller records ep->a itself (right before its launch)
-static EventPair* timer_begin(bkgpu_plan* p, std::vector<EventPair>& v, int64_t bytes, bool record = true) {
-    EventPair ep{};
-    for (cudaEvent_t* e : {&ep.a, &ep.b}) {   // events are recycled: a re-armed plan launches the same kernels again and again
-        if (!p->event_pool.empty()) { *e = p->event_pool.back(); p->event_pool.pop_back(); }
-        else if (cudaEventCreate(e) != cudaSuccess) return nullptr;
-    }
-    ep.bytes = bytes;
-    if (record) cudaEventRecord(ep.a, p->stream);
-    v.push_back(ep);
-    return &v.back();
-}
-static void timer_end(bkgpu_plan* p, EventPair* ep) { if (ep) cudaEventRecord(ep->b, p->stream); }
-
 // ------------------------------------------------------------------ lifecycle
 extern "C" int bkgpu_init(bkgpu_plan** out, const uint8_t* desc, size_t len, int device, void* nccl_comm) {
     if (!out) return thread_fail(BKGPU_EINVAL, "bkgpu_init: out is NULL");
@@ -212,40 +201,6 @@ extern "C" int bkgpu_set_option(bkgpu_plan* p, const char* key, int64_t v) {
     return BKGPU_OK;
 }
 
-static int alloc_group_table(bkgpu_plan* p) {
-    const AggPlan& ap = p->c.ap;
-    GroupTable& gt = p->gt;
-    int log2 = ap.n_keyw == 0 ? 0 : p->group_cap_log2;
-    size_t cap = (size_t)1 << log2;
-    gt.cap_mask = (uint32_t)(cap - 1); gt.cap_log2 = (uint32_t)log2;
-    int rc;
-    if ((rc = dev_alloc(p, (void**)&gt.state, cap * 4))) return rc;
-    if ((rc = dev_alloc(p, (void**)&gt.keys, cap * 8 * (size_t)std::max(ap.n_keyw, 1)))) return rc;
-    if ((rc = dev_alloc(p, (void**)&gt.lanes, cap * 8 * (size_t)ap.n_lanes))) return rc;
-    if ((rc = dev_alloc(p, (void**)&gt.n_groups, 4 * ((size_t)GT_OCC_OFF + cap)))) return rc;   // counter, overflow flag, occupied list
-    gt.overflow = gt.n_groups + 1;
-    if (ap.n_hll) {   // hll_add_agg: the register arena, one block per (group, sketch) that receives a value
-        if ((rc = dev_alloc(p, (void**)&gt.hll_regs, (size_t)p->hll_cap * HLL_REGISTERS))) return rc;
-        if ((rc = dev_alloc(p, (void**)&gt.hll_ctr, 16))) return rc;
-        gt.hll_cap = (uint32_t)p->hll_cap;
-        CK(p, cudaMemsetAsync(gt.hll_ctr, 0, 16, p->stream));
-    }
-    if (p->c.n_rb) {   // rb_build_agg: the pair buffer and the sort's second buffer (one word more each: the build's scan closes on it)
-        if ((rc = dev_alloc(p, (void**)&p->rb.keys, ((size_t)p->rb_cap + 1) * 8))) return rc;
-        if ((rc = dev_alloc(p, (void**)&p->rb.alt, ((size_t)p->rb_cap + 1) * 8))) return rc;
-        if ((rc = dev_alloc(p, (void**)&p->rb.ctr, 8))) return rc;
-        p->rb.cap = (uint64_t)p->rb_cap;
-        CK(p, cudaMemsetAsync(p->rb.ctr, 0, 8, p->stream));
-        p->rb.hi = 0;
-    }
-    p->d_cursor = gt.n_groups + 2;                       // [2] result cursor [3] merge info
-    p->d_rows_passed = (uint64_t*)(gt.n_groups + 4);     // [4..5] rows that passed the filter
-    CK(p, cudaMemsetAsync(gt.n_groups, 0, 4 * GT_OCC_OFF, p->stream));
-    CK(p, launch_table_init(gt, ap, p->stream));
-    p->stats.kernel_launches++;
-    return BKGPU_OK;
-}
-
 namespace { int cpu_budget(); }   // CPUs this process may use (affinity, cgroup quota): defined with the copy pool
 
 // the plan's IN sets (OP_IN_SET) in one device allocation, kept until bkgpu_close (bkgpu_reset keeps them), and their addresses
@@ -287,108 +242,12 @@ extern "C" int bkgpu_open(bkgpu_plan* p) {
         return p->fail(BKGPU_EUNSUPPORTED, "rb_build_agg with a communicator is outside the GPU path: bitmaps do not travel with the fixed-width partial rows");
     int rc = upload_in_sets(p);   // (before sort_open: it copies the programs)
     if (rc) return rc;
-    if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) rc = alloc_group_table(p);
+    if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) rc = agg_open(p);
     if (!rc && (p->c.kind == PK_SORT || p->c.kind == PK_FILTER || p->c.kind == PK_WINDOW))   // (a window retains its rows like a full sort)
         rc = sort_open(p, p->c, p->region_base, &p->sort);
     if (!rc && p->c.post) { rc = sort_open(p, *p->c.post, 0, &p->post_sort); store_init(p->post, p->c.post->cols); }
     if (rc) return rc;
     p->state = S_OPEN;
-    return BKGPU_OK;
-}
-
-// the group count an earlier launch left in pinned memory: the 4-byte copy after a launch, or the counter block of a fused extraction
-// (read without a synchronisation: a stale value only costs speed)
-static void learn_groups(bkgpu_plan* p) {
-    if (p->h_pinned && p->h_pinned[0] > p->known_groups) p->known_groups = p->h_pinned[0];
-    if (p->h_fused) { const uint32_t g = *(const volatile uint32_t*)p->h_fused; if (g > p->known_groups) p->known_groups = g; }
-}
-
-// device images of an extracted row: one per group expression, per aggregate its final value (+2 for an AVG blob)
-static int agg_n_img(const AggPlan& ap) {
-    int n = ap.n_group;
-    for (int k = 0; k < ap.n_agg; k++) if (!ap.agg[k].hidden) n += ap.agg[k].kind == AG_AVG ? 3 : 1;
-    return n;
-}
-
-// the mapped host buffer of the fused extraction, sized for the groups seen so far (at least 2048 rows); false = too many groups
-// to extract this way (the table is then read back by k_extract)
-static bool ensure_fused(bkgpu_plan* p) {
-    uint32_t want = 2048;
-    while (want < p->known_groups && want < (1u << 16)) want *= 2;
-    if (want < p->known_groups) return false;
-    if (p->h_fused && p->fused_cap >= want) return true;
-    if (p->h_fused) {   // (a launch still running may write into it)
-        cudaStreamSynchronize(p->stream);
-        if (!mapped_cache().put(p->fused_bytes, p->h_fused)) cudaFreeHost(p->h_fused);
-        p->h_fused = p->d_fused = nullptr; p->fused_cap = 0;
-    }
-    const size_t bytes = 32 + (size_t)want * (size_t)agg_n_img(p->c.ap) * 9;
-    uint8_t* h = mapped_cache().take(bytes);
-    if (!h && cudaHostAlloc((void**)&h, bytes, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) { cudaGetLastError(); return false; }
-    if (cudaHostGetDevicePointer((void**)&p->d_fused, h, 0) != cudaSuccess) { cudaGetLastError(); cudaFreeHost(h); return false; }
-    memset(h, 0, 32);
-    p->h_fused = h; p->fused_bytes = bytes; p->fused_cap = want;
-    return true;
-}
-
-// rb_build_agg: a launch appends at most one key per row and rb_build_agg aggregate, except where a probe row meets several build rows (such
-// a launch can still overflow the pair buffer, and the request then fails at bkgpu_finish).  When the keys could outgrow the buffer, it is
-// sorted and deduplicated first (a set does not depend on order), and the launch shrinks to the rows that fit
-static int rb_room(bkgpu_plan* p, const Compiled& c, int64_t* rows) {
-    const uint64_t per = (uint64_t)c.n_rb, cap = p->rb.cap;
-    if (p->rb.hi + (uint64_t)*rows * per > cap) {
-        uint64_t n = 0;
-        const int rc = rb_compact(p, &n);
-        if (rc) return rc;
-        p->rb.hi = n;
-        const int64_t fit = (int64_t)((cap - n) / per) & ~7ll;   // (a multiple of 8 rows: the next launch's validity bitmaps stay byte-aligned)
-        if (fit < 8)
-            return p->fail(BKGPU_ETOOBIG, "rb_build_agg: the pair buffer holds %llu distinct (group, value) pairs and is full: raise rb_pair_capacity",
-                           (unsigned long long)n);
-        if (*rows > fit && !p->join.tail_launch) *rows = fit;   // (the join's tail walks every build row in one launch)
-    }
-    p->rb.hi += (uint64_t)*rows * per;
-    return BKGPU_OK;
-}
-
-int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp) {
-    AggEnv env;
-    env.force_generic = p->force_generic; env.no_lean = p->no_lean; env.no_lean_nulls = p->no_lean_nulls; env.no_lean_mm = p->no_lean_mm;
-    env.lean_fx = p->lean_fx; env.fx_off = p->fx_off;
-    env.scalar_tma = p->scalar_tma; env.smem_cap_log2 = p->smem_cap_log2;
-    env.tail_launch = p->join.tail_launch;
-    env.multi_rank = p->nccl_comm && p->nranks > 1; env.has_post = p->c.post != nullptr;
-    if (c.ap.n_keyw > 0 && p->smem_cap_log2 < 0) learn_groups(p);   // (the shared table is sized from it)
-    env.known_groups = p->known_groups;
-    AggArgs a; AggSelection sel;
-    const int rc = select_agg_launch(c, cols, nrows, vec_ok, jp, env, a, sel);
-    if (rc == BKGPU_ENOMEM) return p->fail(rc, "lean kernel: shared table does not fit");
-    if (rc) return rc;
-    a.gt = p->gt; a.rows_passed = p->d_rows_passed;
-    if (c.kind == PK_JOIN_AGG) a.join = join_args(p, p->join.tail_launch);
-    if (sel.fused_ok && ensure_fused(p)) { a.fused_out = p->d_fused; a.fused_cap = p->fused_cap; }
-    const int64_t kMax = (int64_t)1 << 30;  // rows per launch (32-bit counters inside a CTA)
-    int64_t algo_bytes_per_row = 0;
-    for (int i = 0; i < a.n_cols; i++) algo_bytes_per_row += storage_bytes(a.cols[i].stype);
-    int64_t b_rows = 0;
-    for (int64_t off = 0; off < nrows; off += b_rows) {
-        AggArgs b = a;
-        b.nrows = std::min(kMax, nrows - off);
-        if (c.n_rb) {   // (a compaction swaps the pair buffer with the sort's second buffer)
-            const int rrc = rb_room(p, c, &b.nrows);
-            if (rrc) return rrc;
-            b.rb_keys = p->rb.keys; b.rb_ctr = p->rb.ctr; b.rb_cap = p->rb.cap;
-        }
-        b_rows = b.nrows;
-        for (int i = 0; i < b.n_cols; i++) b.cols[i] = col_at(a.cols[i], off);
-        EventPair* ep = timer_begin(p, p->timed, b.nrows * algo_bytes_per_row, false);
-        cudaError_t e = launch_agg(b, sel.kernel, sel.smem, p->sm_count, p->stream, ep ? ep->a : nullptr);
-        timer_end(p, ep);
-        p->fused_last = b.fused_out != nullptr;
-        if (e != cudaSuccess) return p->cuda_fail(e, "launch_agg");
-        snprintf(p->stats.main_kernel_name, sizeof p->stats.main_kernel_name, "%s", agg_kernel_name(sel.kernel));
-        p->stats.kernel_launches++;
-    }
     return BKGPU_OK;
 }
 
@@ -598,7 +457,6 @@ int feed(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* col
     return BKGPU_OK;
 }
 
-static int agg_batch(bkgpu_plan* p, const DevCol* cols, int64_t nrows, int64_t, bool vec_ok) { return launch_agg_batch(p, p->c, cols, nrows, vec_ok); }
 static int sort_batch(bkgpu_plan* p, const DevCol* cols, int64_t nrows, int64_t, bool) { return sort_push(p->sort, cols, nrows, &p->stats); }
 
 void set_result(bkgpu_plan* p, std::vector<SortOutCol>& cols, int64_t rows, const OutCol* desc) {
@@ -610,27 +468,6 @@ void set_result(bkgpu_plan* p, std::vector<SortOutCol>& cols, int64_t rows, cons
         p->result.push_back(std::move(hc));
     }
     p->result_rows = rows; p->result_pos = 0;
-}
-
-// MERGE_AGG of hll_add_agg over host memory: every non-NULL input value must be a RAW sketch, or the push fails (device-resident input is
-// checked by the merge kernel itself, and the request then fails at bkgpu_finish)
-static int hll_check_host_sketches(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows) {
-    const AggPlan& ap = p->c.ap;
-    for (int k = 0; k < ap.n_agg; k++) {
-        if (ap.agg[k].kind != AG_HLL || ap.agg[k].arg_prim != BK_HLL) continue;
-        const ColRef& w = p->c.cols[ap.agg[k].hll_col];
-        for (int i = 0; i < ncols; i++) {
-            if (cols[i].tuple_id != w.tuple_id || cols[i].slot_id != w.slot_id || !cols[i].values || cols[i].length != nrows) continue;   // (bind_columns reports those)
-            for (int64_t r = 0; r < nrows; r++) {
-                if (cols[i].validity && !((cols[i].validity[r >> 3] >> (r & 7)) & 1)) continue;
-                const uint8_t* v = (const uint8_t*)cols[i].values + (size_t)r * HLL_RAW_BYTES;
-                if (memcmp(v, "HYLL", 4) != 0 || v[4] != HLL_ENC_RAW)
-                    return p->fail(BKGPU_EINVAL, "column %d_%d row %lld is not a RAW HLL sketch (\"HYLL\", encoding 255, 16400 bytes): MERGE_AGG of hll_add_agg "
-                                   "merges RAW sketches only", w.tuple_id, w.slot_id, (long long)r);
-            }
-        }
-    }
-    return BKGPU_OK;
 }
 
 static int bkgpu_push_impl(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device);
@@ -649,320 +486,11 @@ static int bkgpu_push_impl(bkgpu_plan* p, const bkgpu_column* cols, int ncols, i
     p->stats.rows_scanned += nrows;
     if (nrows == 0) return BKGPU_OK;
     switch (p->c.kind) {
-        case PK_AGG: {
-            int rc = on_device ? BKGPU_OK : hll_check_host_sketches(p, cols, ncols, nrows);
-            if (rc) return rc;
-            rc = feed(p, p->c.cols, cols, ncols, nrows, on_device, agg_batch);
-            if (rc) return rc;
-            // learn the cardinality for later batches' table size (no sync: a stale value only costs speed); a launch that extracted its
-            // result has already left the count in h_fused
-            if (p->c.ap.n_keyw > 0 && p->smem_cap_log2 < 0 && p->h_pinned && !p->fused_last)
-                CK(p, cudaMemcpyAsync(p->h_pinned, p->gt.n_groups, 4, cudaMemcpyDeviceToHost, p->stream));
-            return BKGPU_OK;
-        }
+        case PK_AGG: return agg_push(p, cols, ncols, nrows, on_device);
         case PK_JOIN_AGG: case PK_JOIN: case PK_STAR_AGG: return join_push(p, cols, ncols, nrows, on_device);
         case PK_SORT: case PK_FILTER: case PK_WINDOW: return feed(p, p->c.cols, cols, ncols, nrows, on_device, sort_batch);
         default: return p->fail(BKGPU_EUNSUPPORTED, "plan kind %d has no push path yet", p->c.kind);
     }
-}
-
-
-// groups per rank in the exchanged partial state: never more than the group table can hold (every rank runs the same plan with
-// the same options, so all ranks agree on it) — a 2^14-slot table ships 0.8 MB per rank instead of the 3 MB of the default cap
-static uint32_t eff_pcap(const bkgpu_plan* p) {
-    const int64_t table = p->c.ap.n_keyw == 0 ? 1 : (int64_t)1 << p->group_cap_log2;
-    return (uint32_t)std::min<int64_t>(p->partial_cap, table);
-}
-
-// the collective step of bkgpu_finish: regions -> one set per GPU, the per-GPU partial tables meet once and are folded by K3.
-// Default: compact rows, one ncclAllGather of 1 + bound x (key + lane words) per rank — `bound` = the largest group count any rank
-// held in earlier runs of this plan (2048 on the first run); the merge reports the true maximum and the exchange is repeated once
-// with a larger bound when it did not fit.  Option repartition: all-to-all by key owner.
-static int agg_collective(bkgpu_plan* p, bool* rows_mode) {
-    const AggPlan& ap = p->c.ap;
-    GroupTable& gt = p->gt;
-    *rows_mode = false;
-    const uint32_t pcap = eff_pcap(p);
-    int rc;
-    const bool repart = p->repartition && ap.n_keyw > 0;   // (a scalar aggregate has one group: nothing to partition)
-    EventPair* ep = timer_begin(p, p->timed_coll, 0);
-    if (!repart) {
-        *rows_mode = true;
-        if (p->rank < 0 && nccl_comm_rank(p->nccl_comm, &p->rank) != 0) return p->fail(BKGPU_ENCCL, "ncclCommUserRank: %s", nccl_last_error());
-        uint32_t bound = p->merge_bound ? p->merge_bound : 2048u;
-        if (ap.n_keyw == 0) bound = 1;
-        bound = std::min<uint32_t>(bound, pcap);
-        const size_t rw = (size_t)(ap.n_keyw + ap.n_lanes + ap.n_hll * HLL_ROW_WORDS);
-        const size_t words = 1 + rw * bound;
-        if ((rc = ensure_buf(p, (void**)&p->d_partial, &p->d_partial_cap, words * 8))) return rc;
-        if ((rc = ensure_buf(p, (void**)&p->d_gather, &p->d_gather_cap, words * 8 * (size_t)p->nranks))) return rc;
-        CK(p, launch_partial_export_rows(gt, ap, p->d_partial, bound, p->stream));
-        if (nccl_all_gather(p->nccl_comm, p->d_partial, p->d_gather, words, p->stream) != 0) return p->fail(BKGPU_ENCCL, "ncclAllGather: %s", nccl_last_error());
-        CK(p, launch_partial_merge_rows(gt, ap, p->d_gather, words, bound, p->nranks, p->rank, p->d_cursor + 1, p->stream));
-        p->merge_bound_used = bound;
-        p->stats.kernel_launches += 2;
-        timer_end(p, ep);
-        return BKGPU_OK;
-    }
-    // hash repartition: every rank keeps only the groups it owns — an all-to-all of per-owner segments instead of the
-    // all-gather; the merged table (and the result) of a rank is its partition, the union over ranks is the answer
-    const size_t words = 1 + (size_t)(ap.n_keyw + ap.n_lanes) * pcap;
-    if ((rc = ensure_buf(p, (void**)&p->d_partial, &p->d_partial_cap, words * 8 * (size_t)p->nranks))) return rc;
-    if ((rc = ensure_buf(p, (void**)&p->d_gather, &p->d_gather_cap, words * 8 * (size_t)p->nranks))) return rc;
-    if (!p->d_part_cursors && (rc = dev_alloc(p, (void**)&p->d_part_cursors, 4 * (size_t)p->nranks))) return rc;
-    CK(p, launch_partial_export_parts(gt, ap, p->d_partial, words, pcap, p->d_part_cursors, p->nranks, p->stream));
-    if (nccl_all_to_all(p->nccl_comm, p->d_partial, p->d_gather, words, p->nranks, p->stream) != 0) return p->fail(BKGPU_ENCCL, "all-to-all: %s", nccl_last_error());
-    CK(p, launch_table_init(gt, ap, p->stream, 1));   // (keeps the overflow flag an export beyond partial_capacity raised)
-    CK(p, launch_partial_merge(gt, ap, p->d_gather, words, pcap, p->nranks, p->stream));
-    timer_end(p, ep);
-    p->stats.kernel_launches += 4;
-    return BKGPU_OK;
-}
-
-// [LIMIT ->] [SORT ->] [HAVING ->] above the aggregate: the extracted rows (still on the device) become typed columns and run through
-// the post fragment's sort / filter kernels; only the final rows travel to the host
-static int agg_post(bkgpu_plan* p, uint32_t n_out, uint32_t out_cap) {
-    const Compiled& pc = *p->c.post;
-    const size_t nc = pc.cols.size();
-    int rc;
-    for (size_t c = 0; c < nc; c++)
-        if ((rc = store_reserve(p, p->post, c, std::max<int64_t>(n_out, 1), std::max<int64_t>(n_out, 2048), true))) return rc;
-    PostCols pcs; memset(&pcs, 0, sizeof pcs);
-    pcs.n = (int)nc;
-    int img = 0;
-    for (size_t c = 0; c < nc; c++) {   // (post columns = the aggregate's output columns, in order: plan.cpp::lower_post)
-        pcs.img[c] = img; pcs.stype[c] = prim_storage(pc.cols[c].prim); pcs.values[c] = p->post.cols[c].vals; pcs.null_bytes[c] = p->post.cols[c].nulls;
-        img += p->c.out_cols[c].kind == 1 ? 2 : 1;
-    }
-    CK(p, launch_images_to_columns(p->d_outv, p->d_outn, out_cap, n_out, pcs, p->stream));
-    std::vector<DevCol> dc(std::max<size_t>(nc, 1));
-    for (size_t c = 0; c < nc; c++)
-        if ((rc = store_pack(p, p->post, c, n_out, 16, nullptr, &dc[c]))) return rc;
-    p->stats.kernel_launches += 1 + (int64_t)nc;
-    sort_reset(p->post_sort);
-    bkgpu_stats scratch{};   // (the post fragment's kernels are not the request's "main kernel")
-    if (n_out && (rc = sort_push(p->post_sort, dc.data(), n_out, &scratch))) return rc;
-    std::vector<SortOutCol> cols; int64_t rows = 0;
-    if ((rc = sort_finish(p->post_sort, nullptr, 1, &scratch, cols, &rows))) return rc;
-    p->stats.kernel_launches += scratch.kernel_launches;
-    set_result(p, cols, rows, p->c.out_cols.data());
-    return BKGPU_OK;
-}
-
-// the one wait of a request.  With several ranks on a host whose CPU budget is small (8 ranks under a 16-CPU cgroup quota: two CPUs per
-// rank for the python thread, NCCL's proxy thread and this wait) a spinning wait burns the quota the other ranks' launches need:
-// there the thread sleeps on a blocking-sync event instead (option blocking_sync: -1 auto, 0 spin, 1 sleep)
-static int agg_wait(bkgpu_plan* p) {
-    const double t0 = HostClock::now();
-    if (p->blocking_wait) {
-        if (!p->wait_event) CK(p, cudaEventCreateWithFlags(&p->wait_event, cudaEventBlockingSync | cudaEventDisableTiming));
-        CK(p, cudaEventRecord(p->wait_event, p->stream));
-        CK(p, cudaEventSynchronize(p->wait_event));
-    } else CK(p, cudaStreamSynchronize(p->stream));
-    p->hclk.extract_wait += HostClock::now() - t0;
-    return BKGPU_OK;
-}
-
-// what the counter block of a finished request tells the plan: rows that passed, FX's exact-path count, the groups it holds
-static int agg_take_counters(bkgpu_plan* p, const uint32_t* ctr) {
-    memcpy(&p->rows_passed_host, ctr + 4, 8);
-    // FX: values beyond the sampled scale are added exactly, one global atomic each; a plan whose double columns keep producing many of them
-    // (a column spanning dozens of binades, outliers dominating the sample) goes back to the CAS kernel for its later launches
-    if (ctr[GT_FX_EXACT] > 4096 && (uint64_t)ctr[GT_FX_EXACT] * 64 > (uint64_t)std::max<int64_t>(p->rows_passed_host, 1)) p->fx_off = 1;
-    if (ctr[1]) return p->fail(BKGPU_ETOOBIG, "group table overflow (capacity 2^%d slots / partial_capacity %lld): raise group_capacity_log2",
-                               (int)p->gt.cap_log2, (long long)p->partial_cap);
-    if (ctr[0] > p->known_groups) p->known_groups = ctr[0];
-    p->finish_groups = ctr[0];
-    return BKGPU_OK;
-}
-
-// a BITMAP column (bkgpu.h): one bitmap per row, each the device's bytes for (slot, rb_idx), or the 8-byte empty bitmap
-// ("3a300000 00000000": the reference's initialize gives every group an empty bitmap, so a group whose values were all NULL returns it)
-static void rb_column(bkgpu_plan* p, HostCol& hc, const uint64_t* slot, int64_t rows, int rb_idx) {
-    static const uint8_t empty[8] = {0x3a, 0x30, 0, 0, 0, 0, 0, 0};
-    std::vector<int64_t> b((size_t)rows);   // each row's bitmap in the directory, -1 = none
-    int64_t total = 0;
-    for (int64_t r = 0; r < rows; r++) {
-        const uint32_t id = (uint32_t)(slot[r] << 2) | (uint32_t)rb_idx;
-        const auto it = std::lower_bound(p->rb.bid.begin(), p->rb.bid.end(), id);
-        b[r] = it != p->rb.bid.end() && *it == id ? (int64_t)(it - p->rb.bid.begin()) : -1;
-        total += b[r] < 0 ? 8 : (int64_t)(p->rb.off[b[r] + 1] - p->rb.off[b[r]]);
-    }
-    std::vector<uint8_t>& col = p->rb.col[rb_idx];
-    col.resize(((size_t)rows + 1) * 8 + (size_t)total);
-    int64_t* offs = (int64_t*)col.data();
-    uint8_t* d = col.data() + ((size_t)rows + 1) * 8;
-    offs[0] = 0;
-    for (int64_t r = 0; r < rows; r++) {
-        const size_t len = b[r] < 0 ? 8 : (size_t)(p->rb.off[b[r] + 1] - p->rb.off[b[r]]);
-        memcpy(d + offs[r], b[r] < 0 ? empty : p->rb.bytes + p->rb.off[b[r]], len);
-        offs[r + 1] = offs[r] + (int64_t)len;
-    }
-    hc.elem = -1;
-    hc.varlen = &col;
-}
-
-// typed host columns from `n_out` extracted rows (images + null bytes, column-major with stride `stride`), after OFFSET / LIMIT
-static void agg_result(bkgpu_plan* p, const uint64_t* hv, const uint8_t* hn, size_t stride, uint32_t n_out) {
-    const int64_t rows = n_out;
-    const int64_t skip = p->c.offset > 0 ? std::min<int64_t>(p->c.offset, rows) : 0;
-    int64_t lim = p->c.agg_limit;   // AggNode::get_next stops at its limit (agg_node.cpp:555)
-    if (p->c.limit >= 0 && (lim < 0 || p->c.limit < lim)) lim = p->c.limit;
-    int64_t keep = rows - skip;
-    if (lim >= 0 && keep > lim) keep = lim;
-    p->result.clear();
-    int img = 0, rb_idx = 0;
-    for (const OutCol& oc : p->c.out_cols) {
-        HostCol hc; hc.desc = oc;
-        const uint64_t* v = hv + (size_t)img * stride + skip;
-        const uint8_t* nb = hn + (size_t)img * stride + skip;
-        if (oc.kind == 3) {   // rb_build_agg: the group's slot, whose bitmap the device build serialized (a group without a value: the empty one)
-            rb_column(p, hc, v, keep, rb_idx++);
-            img++;
-            p->result.push_back(std::move(hc));
-            continue;
-        }
-        hc.elem = oc.kind == 1 ? 16 : oc.kind == 2 ? HLL_RAW_BYTES : storage_bytes(prim_storage(oc.prim));
-        hc.values.assign((size_t)std::max<int64_t>(keep, 1) * (size_t)hc.elem, 0);
-        // (a NULL's image is 0, which is also what a NULL row's value bytes hold)
-        uint8_t* d = hc.values.data();
-        if (oc.kind == 1) {
-            const uint64_t* v2 = hv + (size_t)(img + 1) * stride + skip;
-            for (int64_t r = 0; r < keep; r++) { memcpy(d + (size_t)r * 16, v + r, 8); memcpy(d + (size_t)r * 16 + 8, v2 + r, 8); }
-        } else if (oc.kind == 2) {
-            // hll_row_init's RAW sketch (hll_common.cpp:834-842): "HYLL", encoding HLL_RAW, then the registers.  hll_row_add invalidates the
-            // cached cardinality (bit 7 of header byte 15) whenever a register grows, which the first value always does: a group that
-            // received a value has the bit set, a group without one (every argument NULL) is the empty sketch with the byte 0
-            for (int64_t r = 0; r < keep; r++) {
-                uint8_t* o = d + (size_t)r * HLL_RAW_BYTES;
-                memcpy(o, "HYLL", 4); o[4] = HLL_ENC_RAW;
-                if (v[r]) { o[15] = 0x80; memcpy(o + HLL_HDR_BYTES, p->hll_host.data() + (size_t)(v[r] - 1) * HLL_REGISTERS, HLL_REGISTERS); }
-            }
-        } else switch (prim_storage(oc.prim)) {
-            case ST_I32: for (int64_t r = 0; r < keep; r++) { const int32_t x = (int32_t)(int64_t)v[r]; memcpy(d + (size_t)r * 4, &x, 4); } break;
-            case ST_U32: for (int64_t r = 0; r < keep; r++) { const uint32_t x = (uint32_t)v[r]; memcpy(d + (size_t)r * 4, &x, 4); } break;
-            case ST_F32: for (int64_t r = 0; r < keep; r++) { double x; memcpy(&x, v + r, 8); const float f = (float)x; memcpy(d + (size_t)r * 4, &f, 4); } break;
-            case ST_U8: for (int64_t r = 0; r < keep; r++) d[r] = v[r] ? 1 : 0; break;
-            default:
-                if (hc.elem == 8) { if (keep > 0) memcpy(d, v, (size_t)keep * 8); }
-                else for (int64_t r = 0; r < keep; r++) memcpy(d + (size_t)r * hc.elem, v + r, 8);
-                break;
-        }
-        if (keep > 0 && memchr(nb, 1, (size_t)keep)) {
-            hc.validity.assign((size_t)(keep + 7) / 8 + 1, 0xFF);
-            for (int64_t r = 0; r < keep; r++) if (nb[r]) { hc.validity[(size_t)r >> 3] &= (uint8_t)~(1u << (r & 7)); if (oc.kind == 0) memset(d + (size_t)r * hc.elem, 0, (size_t)hc.elem); }
-        }
-        img += oc.kind == 1 ? 2 : 1;
-        p->result.push_back(std::move(hc));
-    }
-    p->result_rows = keep; p->result_pos = 0;
-}
-
-// hll_add_agg: the arena's claimed blocks to the host (the extracted rows reference them), after the request's last kernel.  A claim
-// that found the arena full fails the request: a sketch that lost values would be wrong, not approximate
-static int hll_fetch(bkgpu_plan* p) {
-    if (!p->c.ap.n_hll) return BKGPU_OK;
-    uint32_t ctr[3] = {0, 0, 0};
-    CK(p, cudaMemcpyAsync(ctr, p->gt.hll_ctr, 12, cudaMemcpyDeviceToHost, p->stream));
-    CK(p, cudaStreamSynchronize(p->stream));
-    if (ctr[2]) return p->fail(BKGPU_EINVAL, "MERGE_AGG of hll_add_agg: an input value is not a RAW HLL sketch (\"HYLL\", encoding 255, 16400 bytes)");
-    if (ctr[1] || ctr[0] > p->gt.hll_cap)
-        return p->fail(BKGPU_ETOOBIG, "hll_add_agg: more than %u sketches (groups x hll_add_agg aggregates with a value): raise hll_group_capacity",
-                       p->gt.hll_cap);
-    p->hll_host.resize((size_t)ctr[0] * HLL_REGISTERS);
-    if (ctr[0]) CK(p, cudaMemcpy(p->hll_host.data(), p->gt.hll_regs, (size_t)ctr[0] * HLL_REGISTERS, cudaMemcpyDeviceToHost));
-    p->stats.d2h_bytes += (int64_t)p->hll_host.size() + 8;
-    return BKGPU_OK;
-}
-
-static int agg_finish(bkgpu_plan* p) {
-    const AggPlan& ap = p->c.ap;
-    GroupTable& gt = p->gt;
-    uint32_t host_counts[2] = {0, 0};
-    uint64_t* finish_hv = nullptr; uint8_t* finish_hn = nullptr; uint32_t finish_n_out = 0, finish_out_cap = 0;
-    const bool multi = p->nccl_comm && p->nranks > 1;
-    bool rows_mode = false;
-    const int n_img = agg_n_img(ap);
-    int rc;
-    // the request ended with a launch that extracted its own result into mapped host memory: one wait, nothing else on the device
-    if (p->fused_last && !multi && !p->c.post) {
-        if ((rc = agg_wait(p))) return rc;
-        const uint32_t* ctr = (const uint32_t*)p->h_fused;
-        if ((rc = agg_take_counters(p, ctr))) return rc;
-        const uint32_t n = ctr[0];
-        if (n <= p->fused_cap) {
-            p->stats.d2h_bytes += (int64_t)(32 + (size_t)n * (size_t)n_img * 9);
-            const uint64_t* hv = (const uint64_t*)(p->h_fused + 32);
-            agg_result(p, hv, (const uint8_t*)(hv + (size_t)n * (size_t)n_img), n, n);
-            return BKGPU_OK;
-        }
-        // more groups than the buffer holds: the table is read back below (the next launch's buffer is sized for them)
-    }
-  for (int mtry = 0; mtry < 3; mtry++) {   // (a second trip only when some rank held more groups than the exchange was sized for)
-    { const double t0 = HostClock::now(); if (multi && (rc = agg_collective(p, &rows_mode))) return rc; p->hclk.collective += HostClock::now() - t0; }
-    uint32_t n_out = 0, out_cap = 0, merge_max = 0;
-    uint64_t* hv = nullptr; uint8_t* hn = nullptr;
-    bool redo_merge = false;
-    for (int attempt = 0; attempt < 2; attempt++) {
-        // speculative extraction into the buffers kept from earlier runs: counts, cursor and rows come back
-        // in ONE synchronisation; only a result larger than the buffers costs a second round
-        uint32_t want = std::max<uint32_t>(std::max<uint32_t>(p->known_groups, 1), attempt ? std::max<uint32_t>(host_counts[0], 1) : 1);
-        if (ap.n_keyw == 0) want = 1;
-        if (p->out_cap_alloc < want) {
-            dev_free(p, p->d_outv); p->d_outv = nullptr; p->d_outn = nullptr;
-            size_t cap = std::max<size_t>(want, 2048);
-            if ((rc = dev_alloc(p, (void**)&p->d_outv, cap * 9 * (size_t)n_img + 64))) return rc;   // values, then the null bytes: ONE copy brings both back
-            p->d_outn = (uint8_t*)(p->d_outv + cap * (size_t)n_img);
-            p->out_cap_alloc = cap;
-        }
-        out_cap = (uint32_t)p->out_cap_alloc;
-        CK(p, launch_extract(gt, ap, p->d_outv, p->d_outn, out_cap, p->d_cursor, p->c.emit_default ? 1 : 0, p->stream));
-        p->stats.kernel_launches++;
-        const size_t n_words = (size_t)out_cap * (size_t)n_img;
-        if (p->h_out_cap < n_words) {   // pinned: the four copies below are truly asynchronous and land in one synchronisation
-            if (p->h_outv) cudaFreeHost(p->h_outv);
-            p->h_outv = nullptr; p->h_outn = nullptr; p->h_out_cap = 0;
-            CK(p, cudaHostAlloc((void**)&p->h_outv, n_words * 9 + 64, cudaHostAllocDefault));
-            p->h_out_cap = n_words;
-        }
-        hv = p->h_outv; hn = p->h_outn = (uint8_t*)(p->h_outv + n_words);
-        // two copies, one synchronisation: the 32-byte counter block (groups, overflow, rows extracted, merge info, rows passed) and
-        // the extracted rows (values + null bytes, contiguous on both sides)
-        uint32_t local_ctr[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-        uint32_t* hc3 = p->h_pinned ? p->h_pinned + 8 : local_ctr;   // [8] groups [9] overflow [10] rows extracted [11] merge info [12..13] rows passed
-        CK(p, cudaMemcpyAsync(hc3, gt.n_groups, 32, cudaMemcpyDeviceToHost, p->stream));
-        if ((const uint8_t*)p->d_outn == (const uint8_t*)(p->d_outv + n_words)) CK(p, cudaMemcpyAsync(hv, p->d_outv, n_words * 9, cudaMemcpyDeviceToHost, p->stream));
-        else {
-            CK(p, cudaMemcpyAsync(hv, p->d_outv, n_words * 8, cudaMemcpyDeviceToHost, p->stream));
-            CK(p, cudaMemcpyAsync(hn, p->d_outn, n_words, cudaMemcpyDeviceToHost, p->stream));
-        }
-        if ((rc = agg_wait(p))) return rc;
-        host_counts[0] = hc3[0]; host_counts[1] = hc3[1]; n_out = hc3[2]; merge_max = hc3[3];
-        if (rows_mode) {
-            const uint32_t mx = merge_max;
-            if (mx > p->merge_bound_used) {   // nothing was merged (k_partial_merge_rows): exchange again, sized for what the ranks really hold
-                if (mx > eff_pcap(p)) return p->fail(BKGPU_ETOOBIG, "a rank holds %u groups, more than partial_capacity %lld: raise partial_capacity", mx, (long long)p->partial_cap);
-                p->merge_bound = (mx + 63u) & ~63u;
-                redo_merge = true;
-                break;
-            }
-            const uint32_t learned = (std::max<uint32_t>(mx, 1u) + 63u) & ~63u;
-            if (learned > p->merge_bound) p->merge_bound = learned;
-        }
-        p->stats.d2h_bytes += (int64_t)(n_words * 9 + 12);
-        if ((rc = agg_take_counters(p, hc3))) return rc;
-        if (n_out <= out_cap) break;   // everything fitted
-    }
-    if (!redo_merge) { finish_hv = hv; finish_hn = hn; finish_n_out = n_out; finish_out_cap = out_cap; break; }
-    if (mtry == 2) return p->fail(BKGPU_ENCCL, "partial-state exchange did not converge");
-  }
-    uint32_t n_out = finish_n_out, out_cap = finish_out_cap;
-    if (n_out > out_cap) n_out = out_cap;
-    if ((rc = hll_fetch(p))) return rc;
-    if (p->c.n_rb && (rc = rb_build(p))) return rc;
-    if (p->c.post) return agg_post(p, n_out, out_cap);
-    agg_result(p, finish_hv, finish_hn, out_cap, n_out);
-    return BKGPU_OK;
 }
 
 static void resolve_timers(bkgpu_plan* p) {
@@ -1085,14 +613,8 @@ static int bkgpu_reset_impl(bkgpu_plan* p) {
     CK(p, cudaSetDevice(p->device));
     p->cancelled.store(0);
     if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) {
-        // a finished run knows how many groups its table holds (the count came back with the result): clear those slots through the
-        // occupied list instead of re-initialising the whole capacity (2^20 slots = 44 MB by default)
-        if (p->state == S_FINISHED && p->finish_groups >= 0 && p->c.ap.n_keyw > 0) CK(p, launch_table_clear(p->gt, p->c.ap, (uint32_t)p->finish_groups, p->stream));
-        else CK(p, launch_table_init(p->gt, p->c.ap, p->stream));
-        p->finish_groups = -1;
-        p->fused_last = false;
-        if (p->rb.ctr) { CK(p, cudaMemsetAsync(p->rb.ctr, 0, 8, p->stream)); p->rb.hi = 0; }   // (rb_build_agg: the pair buffer is empty again)
-        p->stats.kernel_launches++;
+        const int rc = agg_reset(p);
+        if (rc) return rc;
     }
     join_reset(p);
     if (p->sort) sort_reset(p->sort);
@@ -1126,7 +648,7 @@ extern "C" void bkgpu_close(bkgpu_plan* p) {
     if (p->h_pinned) cudaFreeHost(p->h_pinned);
     if (p->h_outv) cudaFreeHost(p->h_outv);
     if (p->rb.bytes) cudaFreeHost(p->rb.bytes);
-    if (p->h_fused && !mapped_cache().put(p->fused_bytes, p->h_fused)) cudaFreeHost(p->h_fused);   // (the stream was drained above)
+    if (p->h_fused && !mapped_put(p->fused_bytes, p->h_fused)) cudaFreeHost(p->h_fused);   // (the stream was drained above)
     if (p->copy_stream) cudaStreamDestroy(p->copy_stream);
     if (p->own_stream && p->stream) cudaStreamDestroy(p->stream);
     delete p;
@@ -1215,10 +737,7 @@ extern "C" int bkgpu_push_region(bkgpu_plan* p, int64_t region_id) {
 extern "C" int bkgpu_partial_capacity(bkgpu_plan* p, size_t* bytes) {
     if (!p || !bytes) return thread_fail(BKGPU_EINVAL, "bkgpu_partial_capacity: NULL argument");
     if (p->c.n_rb) return p->fail(BKGPU_EUNSUPPORTED, "rb_build_agg has no partial state: bitmaps do not fit the fixed-width partial rows");
-    if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) {   // (a sketch's registers ride along: HLL_ROW_WORDS per hll_add_agg)
-        *bytes = 8 * (1 + (size_t)(p->c.ap.n_keyw + p->c.ap.n_lanes + p->c.ap.n_hll * HLL_ROW_WORDS) * (size_t)eff_pcap(p));
-        return BKGPU_OK;
-    }
+    if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) { *bytes = agg_partial_bytes(p); return BKGPU_OK; }
     if (p->c.kind == PK_SORT && p->sort) { *bytes = sort_partial_bytes(p->sort); return BKGPU_OK; }
     return p->fail(BKGPU_EUNSUPPORTED, "plan kind %d has no partial state", p->c.kind);
 }
@@ -1230,19 +749,7 @@ extern "C" int bkgpu_partial_export(bkgpu_plan* p, void* dev_dst, size_t bytes) 
     if (bytes < need) return p->fail(BKGPU_EINVAL, "partial buffer too small: %zu < %zu", bytes, need);
     CK(p, cudaSetDevice(p->device));
     if (p->c.kind == PK_SORT) return sort_partial_export(p->sort, dev_dst);
-    // compact rows (the layout the in-library all-gather ships): [u64 groups][groups x (key words + lane words)]
-    CK(p, launch_partial_export_rows(p->gt, p->c.ap, (uint64_t*)dev_dst, eff_pcap(p), p->stream));
-    p->stats.kernel_launches += 1;
-    uint64_t held = 0; uint32_t ov = 0, hll_ctr[3] = {0, 0, 0};
-    CK(p, cudaMemcpyAsync(&held, dev_dst, 8, cudaMemcpyDeviceToHost, p->stream));
-    CK(p, cudaMemcpyAsync(&ov, p->gt.overflow, 4, cudaMemcpyDeviceToHost, p->stream));
-    if (p->gt.hll_ctr) CK(p, cudaMemcpyAsync(hll_ctr, p->gt.hll_ctr, 12, cudaMemcpyDeviceToHost, p->stream));
-    CK(p, cudaStreamSynchronize(p->stream));
-    if (hll_ctr[2]) return p->fail(BKGPU_EINVAL, "MERGE_AGG of hll_add_agg: an input value is not a RAW HLL sketch (\"HYLL\", encoding 255, 16400 bytes)");
-    if (hll_ctr[1]) return p->fail(BKGPU_ETOOBIG, "hll_add_agg: more than %u sketches: raise hll_group_capacity", p->gt.hll_cap);
-    if (ov) return p->fail(BKGPU_ETOOBIG, "group table overflow (capacity 2^%d slots): raise group_capacity_log2", (int)p->gt.cap_log2);
-    if (held > eff_pcap(p)) return p->fail(BKGPU_ETOOBIG, "this rank holds %llu groups, more than partial_capacity=%lld", (unsigned long long)held, (long long)p->partial_cap);
-    return BKGPU_OK;
+    return agg_partial_export(p, dev_dst);
 }
 extern "C" int bkgpu_partial_merge(bkgpu_plan* p, const void* dev_src, size_t bytes_per_rank, int nranks) {
     if (!p || !dev_src || nranks < 1) return thread_fail(BKGPU_EINVAL, "bkgpu_partial_merge: bad argument");
@@ -1258,14 +765,7 @@ extern "C" int bkgpu_partial_merge(bkgpu_plan* p, const void* dev_src, size_t by
         p->stats.rows_returned = rows; p->state = S_FINISHED;
         return BKGPU_OK;
     }
-    CK(p, launch_table_init(p->gt, p->c.ap, p->stream, 1));
-    CK(p, launch_partial_merge_rows(p->gt, p->c.ap, (const uint64_t*)dev_src, need / 8, eff_pcap(p), nranks, -1 /* fold every segment */, p->d_cursor + 1, p->stream));
-    p->fused_last = false;   // (the merged table is read back by k_extract)
-    p->stats.kernel_launches += 2;
-    void* comm = p->nccl_comm; int nr = p->nranks; p->nccl_comm = nullptr; p->nranks = 1;  // already merged: finalize locally
-    rc = agg_finish(p);
-    p->nccl_comm = comm; p->nranks = nr;
-    if (rc) return rc;
+    if ((rc = agg_partial_merge(p, dev_src, nranks))) return rc;
     p->stats.rows_returned = p->result_rows; p->state = S_FINISHED;
     return BKGPU_OK;
 }

@@ -1,4 +1,4 @@
-// api_state.h — the plan object behind the C ABI (bkgpu_plan) and the host helpers api.cu and join.cu share.
+// api_state.h — the plan object behind the C ABI (bkgpu_plan) and the host helpers api.cu, agg.cu and join.cu share.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdarg.h>
@@ -31,6 +31,14 @@ struct HostCol {  // one materialised result column (host memory owned by the pl
 };
 
 struct EventPair { cudaEvent_t a, b; int64_t bytes; };
+
+// FK -> PK join fast path: unique build keys, looked up through a dense array (small key range) or a packed
+// (key32 << 32 | row) table; build-side columns are gathered to probe-row alignment
+struct JoinFast {
+    int32_t mode;               // 0 = none, 1 = dense array, 2 = packed 32-bit-key table
+    const uint32_t* dense; uint64_t dense_min; uint64_t dense_size; uint64_t bias;
+    const uint64_t* packed; uint32_t packed_mask;
+};
 
 // one retained build side of a hash join (K4) and its key indexes
 struct JoinSide {
@@ -157,6 +165,10 @@ struct bkgpu_plan {
 int dev_alloc(bkgpu_plan* p, void** out, size_t bytes);
 void dev_free(bkgpu_plan* p, void* ptr);
 int ensure_buf(bkgpu_plan* p, void** ptr, size_t* cap, size_t bytes);
+// mapped host buffers of the fused extraction, kept in a process-wide cache by size: take = nullptr when none is free, put = false when the
+// cache does not keep it (the caller frees it)
+uint8_t* mapped_take(size_t bytes);
+bool mapped_put(size_t bytes, uint8_t* buf);
 // device buffers of one call: returned to the plan's allocator when the scope ends, on every way out of the call
 struct DevScope {
     bkgpu_plan* p;
@@ -179,8 +191,6 @@ int bind_columns(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_col
 // a batch as device columns (host columns chunk by chunk through the staging buffers), handed to `fn`
 typedef int (*BatchFn)(bkgpu_plan*, const DevCol*, int64_t nrows, int64_t row_base, bool vec_ok);
 int feed(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device, BatchFn fn);
-// the aggregate of `c` over one batch; `jp`: fused FK -> PK probe (lean kernel only), +1 without launching when the batch does not fit it
-int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp = nullptr);
 // the plan's result from a sort fragment's columns; `desc`: their output column descriptions (nullptr = the sort's own)
 void set_result(bkgpu_plan* p, std::vector<SortOutCol>& cols, int64_t rows, const OutCol* desc);
 
@@ -191,6 +201,17 @@ inline DevCol col_at(const DevCol& c, int64_t off) {
     if (c.validity) x.validity = c.validity + off / 8;
     return x;
 }
+
+// ---- agg.cu: the aggregate (PK_AGG, PK_JOIN_AGG, PK_STAR_AGG)
+int agg_open(bkgpu_plan* p);     // bkgpu_open: the group table (and the HLL arena, the rb_build_agg pair buffer)
+int agg_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device);   // a PK_AGG batch
+// the aggregate of `c` over one batch; `jp`: fused FK -> PK probe (lean kernel only), +1 without launching when the batch does not fit it
+int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp = nullptr);
+int agg_finish(bkgpu_plan* p);   // the cross-rank merge (with a communicator), then the result
+int agg_reset(bkgpu_plan* p);    // bkgpu_reset: the table is empty again
+size_t agg_partial_bytes(const bkgpu_plan* p);
+int agg_partial_export(bkgpu_plan* p, void* dev_dst);
+int agg_partial_merge(bkgpu_plan* p, const void* dev_src, int nranks);   // and the result from the merged table
 
 // ---- join.cu
 int join_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device);   // PK_JOIN_AGG, PK_JOIN, PK_STAR_AGG

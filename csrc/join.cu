@@ -1,9 +1,278 @@
-// join.cu — host path of the hash join (K4): the retained build sides and their indexes, the two-table probe (fused into the lean
-// aggregate, gather, general), the outer-join tail, the join that returns rows, and the star join's build and probe.
+// join.cu — the hash join (K4): its kernels (multimap and unique-key index builds, gathers, the star join's filter, probe and expansion) and
+// its host path: the retained build sides and their indexes, the two-table probe (fused into the lean aggregate, gather, general), the
+// outer-join tail, the join that returns rows, and the star join's build and probe.  The probe loops that run the row interpreter over the
+// joined row (k_agg_interp, k_join_pairs) are agg.cu's.
 #include <string.h>
 #include <algorithm>
 #include <vector>
 #include "api_state.h"
+#include "dev_common.cuh"
+#include "interp.cuh"
+
+namespace bk {
+
+// build-side columns gathered to probe-row alignment (k_join_gather)
+struct GatherCols { int32_t n; const uint8_t* src[MAX_COLS]; uint8_t* dst[MAX_COLS]; int32_t elem[MAX_COLS]; };
+// star join (PK_STAR_AGG): per dimension with unique keys, the fact foreign key, its slot in the row-id tuple and the dimension's key index
+struct StarLookup { DevCol fk; int32_t from_prim, cast_prim, slot; JoinFast jf; };
+struct StarProbe { StarLookup d[4]; int32_t n; int32_t width; int64_t nrows; int32_t vec; };
+// the build-time filter of one dimension: program over the plan's columns (this dimension's retained rows), validity of its join key.
+// Also a two-table join child's own filter (its retained build rows, or one probe batch).
+struct StarFilter { DevCol cols[MAX_COLS]; Program prog; int32_t key_col; int64_t nrows; };
+
+// one output column of the joined rows: element `which` of each row-id tuple (`width` row ids: (probe, build) pairs of a two-table join,
+// [fact, dim x D] of a star join) addresses `src`; JOIN_NO_ROW (the NULL-extended side) gives NULL.  dst_null may be nullptr when no
+// element can be NULL
+__global__ void k_join_rows_gather(DevCol src, const uint32_t* tuples, int width, int which, uint32_t n, int eb, uint8_t* dst, uint8_t* dst_null) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const uint32_t r = tuples[(size_t)width * i + which];
+        const bool isnull = r == JOIN_NO_ROW || elem_is_null(src, r);
+        if (dst_null) dst_null[i] = isnull ? 1 : 0;
+        const uint8_t* s = (const uint8_t*)src.values + (size_t)r * eb;
+        uint8_t* d = dst + (size_t)i * eb;
+        if (isnull) { for (int b = 0; b < eb; b++) d[b] = 0; continue; }
+        switch (eb) {
+            case 1: *d = *s; break;
+            case 4: *(uint32_t*)d = *(const uint32_t*)s; break;
+            case 8: *(uint64_t*)d = *(const uint64_t*)s; break;
+            default: for (int b = 0; b < eb; b++) d[b] = s[b]; break;
+        }
+    }
+}
+
+// K4 build: insert (cast key image, row) of every non-NULL build row (Joiner::construct_hash_map, joiner.cpp:624-631)
+__global__ void k_join_build(DevCol key, int from_prim, int cast_to, int64_t nrows, uint64_t* keys, uint32_t* rows, uint32_t cap_mask) {
+    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < nrows; r += (int64_t)gridDim.x * blockDim.x) {
+        if (elem_is_null(key, r)) continue;
+        const uint64_t img = cast_prim(load_elem(key, r), from_prim, cast_to);
+        uint32_t slot = hash_key1(img) & cap_mask;
+        for (;;) {
+            if (atomicCAS(rows + slot, 0xFFFFFFFFu, (uint32_t)r) == 0xFFFFFFFFu) { keys[slot] = img; break; }
+            slot = (slot + 1) & cap_mask;
+        }
+    }
+}
+
+// ---- FK -> PK fast path (see JoinFast in api_state.h) ----
+__global__ void k_join_minmax(DevCol key, int from_prim, int cast_to, int64_t nrows, uint64_t bias, uint64_t* mm) {
+    uint64_t lo = ~0ull, hi = 0;
+    const int64_t T = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t r0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r0 < nrows; r0 += 4 * T) {   // four independent loads in flight per thread
+        uint64_t v[4]; bool ok[4];
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+            const int64_t r = r0 + u * T;
+            ok[u] = r < nrows && !elem_is_null(key, r);
+            v[u] = ok[u] ? load_elem(key, r) : 0;
+        }
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+            if (!ok[u]) continue;
+            const uint64_t x = cast_prim(v[u], from_prim, cast_to) ^ bias;
+            lo = x < lo ? x : lo; hi = x > hi ? x : hi;
+        }
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        const uint64_t l2 = __shfl_xor_sync(0xFFFFFFFFu, lo, d), h2 = __shfl_xor_sync(0xFFFFFFFFu, hi, d);
+        lo = l2 < lo ? l2 : lo; hi = h2 > hi ? h2 : hi;
+    }
+    if ((threadIdx.x & 31) == 0) { atomicMin((unsigned long long*)mm, (unsigned long long)lo); atomicMax((unsigned long long*)(mm + 1), (unsigned long long)hi); }
+}
+__global__ void k_join_build_fast(DevCol key, int from_prim, int cast_to, int64_t nrows, JoinFast jf, uint32_t* dense_w, uint64_t* packed_w, uint32_t* dup_flag) {
+    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < nrows; r += (int64_t)gridDim.x * blockDim.x) {
+        if (elem_is_null(key, r)) continue;   // a NULL key never matches
+        const uint64_t img = cast_prim(load_elem(key, r), from_prim, cast_to);
+        if (jf.mode == 1) {
+            const uint64_t off = (img ^ jf.bias) - jf.dense_min;
+            if (off >= jf.dense_size) { atomicExch(dup_flag + 2, 1u); continue; }   // outside the range learned from an earlier run of the plan: the host rebuilds
+            if (atomicExch(dense_w + off, (uint32_t)r) != 0xFFFFFFFFu) atomicExch(dup_flag, 1u);
+        } else {
+            const uint32_t k32 = (uint32_t)img;
+            const uint64_t v = ((uint64_t)k32 << 32) | (uint32_t)r;
+            uint32_t slot = (k32 * 0x9E3779B1u) & jf.packed_mask;
+            for (;;) {
+                const uint64_t old = atomicCAS((unsigned long long*)(packed_w + slot), ~0ull, (unsigned long long)v);
+                if (old == ~0ull) break;
+                if ((uint32_t)(old >> 32) == k32) { atomicExch(dup_flag, 1u); break; }   // duplicate key: not a PK
+                slot = (slot + 1) & jf.packed_mask;
+            }
+        }
+    }
+}
+__device__ __forceinline__ uint32_t join_lookup(const JoinFast& jf, uint64_t img) {
+    if (jf.mode == 1) {
+        const uint64_t off = (img ^ jf.bias) - jf.dense_min;
+        return off < jf.dense_size ? __ldg(jf.dense + off) : 0xFFFFFFFFu;
+    }
+    const uint32_t k32 = (uint32_t)img;
+    uint32_t slot = (k32 * 0x9E3779B1u) & jf.packed_mask;
+    for (;;) {
+        const uint64_t v = __ldg((const unsigned long long*)(jf.packed + slot));
+        if (v == ~0ull) return 0xFFFFFFFFu;
+        if ((uint32_t)(v >> 32) == k32) return (uint32_t)v;
+        slot = (slot + 1) & jf.packed_mask;
+    }
+}
+// gather the build-side columns to probe-row alignment; four independent rows per thread keep the random
+// lookups and gathers in flight together
+__global__ void __launch_bounds__(256) k_join_gather(DevCol pk, int from_prim, int cast_to, int64_t nrows, JoinFast jf, GatherCols gc, uint32_t* miss_flag) {
+    const int64_t T = (int64_t)gridDim.x * blockDim.x;
+    bool miss = false;
+    for (int64_t base = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; base < nrows; base += 4 * T) {
+        uint32_t br[4];
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+            const int64_t r = base + u * T;
+            br[u] = 0xFFFFFFFEu;   // beyond the batch
+            if (r < nrows) br[u] = elem_is_null(pk, r) ? 0xFFFFFFFFu : join_lookup(jf, cast_prim(load_elem(pk, r), from_prim, cast_to));
+        }
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+            const int64_t r = base + u * T;
+            if (br[u] == 0xFFFFFFFEu) continue;
+            if (br[u] == 0xFFFFFFFFu) { miss = true; continue; }
+            for (int c = 0; c < gc.n; c++) {
+                if (gc.elem[c] == 8) ((uint64_t*)gc.dst[c])[r] = __ldg((const unsigned long long*)gc.src[c] + br[u]);
+                else if (gc.elem[c] == 4) ((uint32_t*)gc.dst[c])[r] = __ldg((const uint32_t*)gc.src[c] + br[u]);
+                else gc.dst[c][r] = __ldg(gc.src[c] + br[u]);
+            }
+        }
+    }
+    if (__any_sync(0xFFFFFFFFu, miss) && (threadIdx.x & 31) == 0) atomicExch(miss_flag, 1u);
+}
+// K4 fused probe (JoinProbe): compose the grouped-by build attribute onto the key index built by k_join_build_fast
+__global__ void k_join_compose(JoinFast jf, const uint32_t* attr_by_row, uint32_t* attr_of_key, uint64_t* packed_attr, uint32_t* bad_flag) {
+    const uint64_t n = jf.mode == 1 ? jf.dense_size : (uint64_t)jf.packed_mask + 1;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        if (jf.mode == 1) {
+            const uint32_t r = jf.dense[i];
+            attr_of_key[i] = r == 0xFFFFFFFFu ? 0u : __ldg(attr_by_row + r);
+        } else {
+            const uint64_t e = jf.packed[i];
+            uint64_t o = ~0ull;
+            if (e != ~0ull) {
+                o = (e & 0xFFFFFFFF00000000ull) | __ldg(attr_by_row + (uint32_t)e);
+                if (o == ~0ull) atomicExch(bad_flag, 1u);   // (key, attribute) = (0xFFFFFFFF, 0xFFFFFFFF) would read as a free slot
+            }
+            packed_attr[i] = o;
+        }
+    }
+}
+
+// ---- K4 star join (PK_STAR_AGG): one fact table INNER-joined to up to four dimensions ----
+// Build time: the conjuncts over one dimension alone, once per dimension row.  A row's build key is valid when the key is not NULL and the
+// conjunction is TRUE: this bitmap (beside the column's own) is the key's validity for k_join_build_fast / k_join_build, which skip NULL keys.
+// The two-table join runs it over a child's own filter: the build side's (with `dropped`: a row whose conjunction is not TRUE, whatever its
+// key, is marked 2 in matched[]) and each probe batch's.  The program reads the row both as the probe row and as the build row.
+__global__ void __launch_bounds__(256) k_star_dim_filter(const __grid_constant__ StarFilter a, uint32_t* keybits, uint8_t* dropped) {
+    const int lane = threadIdx.x & 31;
+    const int64_t T = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t w0 = (int64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31); w0 < a.nrows; w0 += T) {   // (warp-uniform: one bitmap word per warp and pass)
+        const int64_t r = w0 + lane;
+        bool ok = r < a.nrows && !elem_is_null(a.cols[a.key_col], r);
+        if ((ok || (dropped && r < a.nrows)) && a.prog.n_instr > 0) {
+            uint64_t out[1]; uint32_t out_null;
+            run_program(a.prog, a.cols, r, out, out_null, r);
+            const bool pass = !(out_null & 1u) && out[0] != 0;
+            ok = ok && pass;
+            if (dropped && !pass) dropped[r] = 2;
+        }
+        const uint32_t m = __ballot_sync(0xFFFFFFFFu, ok);
+        if (lane == 0) keybits[w0 >> 5] = m;
+    }
+}
+// four consecutive foreign keys [r0, r0 + 4) as canonical images: one 128-bit load (4-byte keys) or two (8-byte keys) when the chunk is 32-byte
+// aligned and the four rows exist
+__device__ __forceinline__ void load_quad(const DevCol& c, int64_t r0, int64_t nrows, bool vec, uint64_t (&v)[4]) {
+    if (vec && r0 + 4 <= nrows && (c.stype == ST_I32 || c.stype == ST_U32)) {
+        const uint4 q = __ldg((const uint4*)((const uint32_t*)c.values + r0));
+        const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+        for (int u = 0; u < 4; u++) v[u] = narrow_prim(c.stype == ST_I32 ? (uint64_t)(int64_t)(int32_t)w[u] : (uint64_t)w[u], c.prim);
+        return;
+    }
+    if (vec && r0 + 4 <= nrows && (c.stype == ST_I64 || c.stype == ST_U64)) {
+        const ulonglong2 a = __ldg((const ulonglong2*)((const unsigned long long*)c.values + r0));
+        const ulonglong2 b = __ldg((const ulonglong2*)((const unsigned long long*)c.values + r0 + 2));
+        v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
+        return;
+    }
+#pragma unroll
+    for (int u = 0; u < 4; u++) v[u] = r0 + u < nrows ? load_elem(c, r0 + u) : 0;
+}
+// Probe: one pass over a chunk's fact rows.  A row survives when every dimension with unique keys has a partner (a NULL foreign key has none:
+// one L2-resident index read per dimension).  Survivors leave as row-id tuples [fact row, dim row x D] in any order, compacted with warp
+// ballots and one cursor atomic per warp; the slots of dimensions with duplicate keys are filled by k_star_expand.
+__global__ void __launch_bounds__(256) k_star_probe(const __grid_constant__ StarProbe a, uint32_t* out, uint32_t* cursor) {
+    const int lane = threadIdx.x & 31;
+    const int64_t T = (int64_t)gridDim.x * blockDim.x;
+    const int64_t nq = (a.nrows + 3) / 4;
+    for (int64_t q0 = (int64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31); q0 < nq; q0 += T) {   // (warp-uniform trip count: the ballots below)
+        const int64_t r0 = (q0 + lane) * 4;
+        uint32_t br[4][4];
+        // every lookup is issued before any result is tested: up to 16 independent index reads in flight per thread
+#pragma unroll
+        for (int d = 0; d < 4; d++) {
+            if (d >= a.n) break;
+            const StarLookup& L = a.d[d];
+            uint64_t v[4];
+            load_quad(L.fk, r0, a.nrows, a.vec != 0, v);
+#pragma unroll
+            for (int u = 0; u < 4; u++)
+                br[u][d] = r0 + u < a.nrows && !elem_is_null(L.fk, r0 + u) ? join_lookup(L.jf, cast_prim(v[u], L.from_prim, L.cast_prim)) : JOIN_NO_ROW;
+        }
+        uint32_t live = 0;
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+            bool ok = r0 + u < a.nrows;
+#pragma unroll
+            for (int d = 0; d < 4; d++) if (d < a.n) ok = ok && br[u][d] != JOIN_NO_ROW;
+            if (ok) live |= 1u << u;
+        }
+        uint32_t b[4]; uint32_t total = 0;
+#pragma unroll
+        for (int u = 0; u < 4; u++) { b[u] = __ballot_sync(0xFFFFFFFFu, (live >> u) & 1u); total += (uint32_t)__popc(b[u]); }
+        if (total == 0) continue;
+        uint32_t base = 0;
+        if (lane == 0) base = atomicAdd(cursor, total);
+        base = __shfl_sync(0xFFFFFFFFu, base, 0);
+        const uint32_t lt = (1u << lane) - 1u;
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+            if ((live >> u) & 1u) {
+                uint32_t* t = out + (size_t)a.width * (base + (uint32_t)__popc(b[u] & lt));
+                t[0] = (uint32_t)(r0 + u);
+#pragma unroll
+                for (int d = 0; d < 4; d++) if (d < a.n) t[a.d[d].slot] = br[u][d];
+            }
+            base += (uint32_t)__popc(b[u]);
+        }
+    }
+}
+// A dimension with duplicate keys: every tuple becomes one tuple per matching row of the dimension's multimap (k_join_build), or none.
+// Past `cap` only the count goes on: the host grows the buffer to the count and runs the pass again.
+__global__ void __launch_bounds__(256) k_star_expand(DevCol fk, int from_prim, int cast_to, const uint64_t* keys, const uint32_t* rows, uint32_t cap_mask,
+                                                     const uint32_t* in, uint32_t n_in, int width, int slot, uint32_t* out, uint32_t cap, uint32_t* cursor) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_in; i += gridDim.x * blockDim.x) {
+        const uint32_t* t = in + (size_t)width * i;
+        const uint32_t f = t[0];
+        if (elem_is_null(fk, f)) continue;
+        const uint64_t img = cast_prim(load_elem(fk, f), from_prim, cast_to);
+        for (uint32_t h = hash_key1(img) & cap_mask;; h = (h + 1) & cap_mask) {
+            const uint32_t br = rows[h];
+            if (br == 0xFFFFFFFFu) break;
+            if (keys[h] != img) continue;
+            const uint32_t pos = atomicAdd(cursor, 1u);
+            if (pos >= cap) continue;
+            uint32_t* o = out + (size_t)width * pos;
+            for (int k = 0; k < width; k++) o[k] = t[k];
+            o[slot] = br;
+        }
+    }
+}
+
+}  // namespace bk
 
 // every plan column of the joined row: the build sides' retained columns and the probe batch's (nullptr: the outer-join tail, whose
 // probe-side columns are never read — row = -1 is NULL)
@@ -105,7 +374,10 @@ static int join_compose_probe(bkgpu_plan* p, uint32_t* flag) {
         if ((rc = ensure_buf(p, (void**)&j.jp_packed, &j.jp_packed_cap, ((size_t)jp.packed_mask + 1) * 8))) return rc;
         jp.packed = j.jp_packed;
     }
-    CK(p, launch_join_compose(s.jf, (const uint32_t*)s.store.cols[(size_t)attr_main].vals, j.jp_attr, j.jp_packed, flag, p->stream));
+    CK(p, cudaMemsetAsync(flag, 0, 4, p->stream));
+    const uint64_t n_idx = s.jf.mode == 1 ? s.jf.dense_size : (uint64_t)s.jf.packed_mask + 1;
+    k_join_compose<<<grid_for((int64_t)n_idx, p->sm_count, 16), 256, 0, p->stream>>>(s.jf, (const uint32_t*)s.store.cols[(size_t)attr_main].vals, j.jp_attr, j.jp_packed, flag);
+    CK(p, cudaGetLastError());
     p->stats.kernel_launches++;
     j.jp = jp; j.jp_key_pos = (int)kpos;   // (the caller drops it again when `flag` comes back set)
     return BKGPU_OK;
@@ -143,7 +415,10 @@ again:
     bool guessed = s.learned && !retry_measured;
     if (guessed) { h_mm[0] = s.learn_min; h_mm[1] = s.learn_max; }
     else {
-        CK(p, launch_join_minmax(key, key.prim, cast_prim, s.store.rows, bias, mm, p->stream));
+        const uint64_t init[2] = {~0ull, 0ull};
+        CK(p, cudaMemcpyAsync(mm, init, 16, cudaMemcpyHostToDevice, p->stream));
+        k_join_minmax<<<grid_for(s.store.rows, p->sm_count, 8), 256, 0, p->stream>>>(key, key.prim, cast_prim, s.store.rows, bias, mm);
+        CK(p, cudaGetLastError());
         CK(p, cudaMemcpyAsync(h_mm, mm, 16, cudaMemcpyDeviceToHost, p->stream));
         CK(p, cudaStreamSynchronize(p->stream));
         p->stats.kernel_launches++;
@@ -162,7 +437,11 @@ again:
         jf.packed = s.jf_packed;
     }
     if (jf.mode) {
-        CK(p, launch_join_build_fast(key, key.prim, cast_prim, s.store.rows, jf, s.jf_dense, s.jf_packed, dup, p->stream));
+        CK(p, cudaMemsetAsync(dup, 0, 12, p->stream));   // [0] duplicate key, [1] fused probe unusable (set by the compose step), [2] key outside the guessed range
+        if (jf.mode == 1) CK(p, cudaMemsetAsync(s.jf_dense, 0xFF, jf.dense_size * 4, p->stream));
+        else CK(p, cudaMemsetAsync(s.jf_packed, 0xFF, ((size_t)jf.packed_mask + 1) * 8, p->stream));
+        k_join_build_fast<<<grid_for(s.store.rows, p->sm_count, 16), 256, 0, p->stream>>>(key, key.prim, cast_prim, s.store.rows, jf, s.jf_dense, s.jf_packed, dup);
+        CK(p, cudaGetLastError());
         p->stats.kernel_launches += 1;
         s.jf = jf;
         if (compose && (rc = join_compose_probe(p, dup + 1))) return rc;   // enqueued behind the build: all flags come back in one round trip
@@ -201,7 +480,11 @@ static int join_build_multimap(bkgpu_plan* p, JoinSide& s, const DevCol& key, in
     if ((rc = dev_alloc(p, (void**)&s.jt_keys, (size_t)cap * 8))) return rc;
     if ((rc = dev_alloc(p, (void**)&s.jt_rows, (size_t)cap * 4))) return rc;
     s.jt_mask = cap - 1;
-    CK(p, launch_join_build(key, key.prim, cast_prim, s.store.rows, s.jt_keys, s.jt_rows, s.jt_mask, p->stream));
+    CK(p, cudaMemsetAsync(s.jt_rows, 0xFF, (size_t)cap * 4, p->stream));
+    if (s.store.rows > 0) {
+        k_join_build<<<grid_for(s.store.rows, p->sm_count, 16), 256, 0, p->stream>>>(key, key.prim, cast_prim, s.store.rows, s.jt_keys, s.jt_rows, s.jt_mask);
+        CK(p, cudaGetLastError());
+    }
     p->stats.kernel_launches++;
     s.jt_generic = true;
     return BKGPU_OK;
@@ -216,7 +499,10 @@ static int join_child_filter(bkgpu_plan* p, const Program& prog, int key_col, co
     StarFilter f; memset(&f, 0, sizeof f);
     for (size_t i = 0; i < c.cols.size(); i++) f.cols[i] = cols[i];
     f.prog = prog; f.key_col = key_col; f.nrows = nrows;
-    CK(p, launch_star_dim_filter(f, (uint32_t*)*bits, dropped, p->stream));
+    if (nrows > 0) {
+        k_star_dim_filter<<<grid_for(nrows, p->sm_count, 16), 256, 0, p->stream>>>(f, (uint32_t*)*bits, dropped);
+        CK(p, cudaGetLastError());
+    }
     p->stats.kernel_launches++;
     return BKGPU_OK;
 }
@@ -288,7 +574,9 @@ static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nro
                 fc[i] = all[m]; fc[i].values = dst; fc[i].validity = nullptr;
             }
             CK(p, cudaMemsetAsync(p->d_cursor + 1, 0, 4, p->stream));
-            CK(p, launch_join_gather(col_at(all[(size_t)c.probe_key_col], off), c.cols[(size_t)c.probe_key_col].prim, c.join_key_prim, n, s.jf, gc, p->d_cursor + 1, p->stream));
+            k_join_gather<<<grid_for((n + 3) / 4, p->sm_count, 8), 256, 0, p->stream>>>(col_at(all[(size_t)c.probe_key_col], off), c.cols[(size_t)c.probe_key_col].prim,
+                                                                                       c.join_key_prim, n, s.jf, gc, p->d_cursor + 1);
+            CK(p, cudaGetLastError());
             p->stats.kernel_launches++;
             uint32_t miss = 0;
             if ((rc = read_u32(p, p->d_cursor + 1, &miss))) return rc;
@@ -349,7 +637,9 @@ static int join_rows_emit(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t
     for (size_t k = 0; k < nc; k++) {   // sink column k = output column k = device column k of the join (plan.cpp::lower_join_rows)
         const RowStore::Col& d = p->post.cols[k];
         if ((rc = store_reserve(p, p->post, k, found, std::max<int64_t>((int64_t)found + found / 4, 1 << 16), true))) return rc;
-        CK(p, launch_join_rows_gather(all[k], j.pairs, 2, c.col_side[k] == 1 ? 1 : 0, found, storage_bytes(prim_storage(d.prim)), d.vals, d.nulls, p->stream));
+        k_join_rows_gather<<<grid_for(found, p->sm_count, 16), 256, 0, p->stream>>>(all[k], j.pairs, 2, c.col_side[k] == 1 ? 1 : 0, found, storage_bytes(prim_storage(d.prim)),
+                                                                                    d.vals, d.nulls);
+        CK(p, cudaGetLastError());
         if ((rc = store_pack(p, p->post, k, found, 16, nullptr, &dc[k]))) return rc;
     }
     p->stats.kernel_launches += 2 * (int64_t)nc;
@@ -380,7 +670,8 @@ static int full_join_agg(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t 
         const size_t m = (size_t)c.jfast_of_main[i];
         if ((rc = store_reserve(p, j.chunk, m, found, found, true))) return rc;
         const RowStore::Col& g = j.chunk.cols[m];
-        CK(p, launch_join_rows_gather(all[m], j.pairs, 2, c.col_side[m] == 1 ? 1 : 0, found, storage_bytes(all[m].stype), g.vals, g.nulls, p->stream));
+        k_join_rows_gather<<<grid_for(found, p->sm_count, 16), 256, 0, p->stream>>>(all[m], j.pairs, 2, c.col_side[m] == 1 ? 1 : 0, found, storage_bytes(all[m].stype), g.vals, g.nulls);
+        CK(p, cudaGetLastError());
         DevCol packed;
         if ((rc = store_pack(p, j.chunk, m, found, 16, nullptr, &packed))) return rc;
         p->stats.kernel_launches += 2;
@@ -438,7 +729,8 @@ static int star_build(bkgpu_plan* p) {
             StarFilter f; memset(&f, 0, sizeof f);
             for (size_t i = 0; i < c.cols.size(); i++) if (c.col_side[i] == 1 + (int)d) f.cols[i] = store_col(s.store, i);
             f.prog = sd.filter; f.key_col = sd.key_col; f.nrows = s.store.rows;
-            CK(p, launch_star_dim_filter(f, (uint32_t*)s.keybits, nullptr, p->stream));
+            k_star_dim_filter<<<grid_for(s.store.rows, p->sm_count, 16), 256, 0, p->stream>>>(f, (uint32_t*)s.keybits, nullptr);
+            CK(p, cudaGetLastError());
             p->stats.kernel_launches++;
             key.validity = s.keybits;
         }
@@ -478,7 +770,9 @@ static int star_probe_batch(bkgpu_plan* p, const DevCol* fact_cols, int64_t nrow
             L.fk = col_at(all[(size_t)sd.fk_col], off); L.from_prim = c.cols[(size_t)sd.fk_col].prim; L.cast_prim = sd.cast_prim; L.slot = 1 + d; L.jf = j.side[d].jf;
         }
         if ((rc = star_tuples(p, 0, (uint64_t)n, W))) return rc;
-        CK(p, launch_star_probe(sp, j.tuples[0], p->d_cursor + 1, p->sm_count, p->stream));
+        CK(p, cudaMemsetAsync(p->d_cursor + 1, 0, 4, p->stream));
+        k_star_probe<<<grid_for((n + 3) / 4, p->sm_count, 8), 256, 0, p->stream>>>(sp, j.tuples[0], p->d_cursor + 1);   // (four rows per thread)
+        CK(p, cudaGetLastError());
         p->stats.kernel_launches++;
         uint32_t found = 0;
         if ((rc = read_u32(p, p->d_cursor + 1, &found))) return rc;
@@ -493,8 +787,10 @@ static int star_probe_batch(bkgpu_plan* p, const DevCol* fact_cols, int64_t nrow
                              [&](uint64_t cap) -> int {
                 int r;
                 if ((r = star_tuples(p, 1 - cur, cap, W))) return r;
-                CK(p, launch_star_expand(fk, c.cols[(size_t)sd.fk_col].prim, sd.cast_prim, s.jt_keys, s.jt_rows, s.jt_mask, j.tuples[cur], found,
-                                         W, 1 + d, j.tuples[1 - cur], (uint32_t)cap, p->d_cursor + 1, p->stream));
+                CK(p, cudaMemsetAsync(p->d_cursor + 1, 0, 4, p->stream));
+                k_star_expand<<<grid_for(found, p->sm_count, 16), 256, 0, p->stream>>>(fk, c.cols[(size_t)sd.fk_col].prim, sd.cast_prim, s.jt_keys, s.jt_rows, s.jt_mask,
+                                                                                       j.tuples[cur], found, W, 1 + d, j.tuples[1 - cur], (uint32_t)cap, p->d_cursor + 1);
+                CK(p, cudaGetLastError());
                 p->stats.kernel_launches++;
                 return BKGPU_OK;
             });
@@ -511,7 +807,9 @@ static int star_probe_batch(bkgpu_plan* p, const DevCol* fact_cols, int64_t nrow
             if ((rc = store_reserve(p, j.chunk, m, found, found, src.validity != nullptr))) return rc;   // NULLs travel along: null bytes, then a bitmap
             const RowStore::Col& g = j.chunk.cols[m];
             fc[i] = src; fc[i].values = g.vals; fc[i].validity = nullptr;
-            CK(p, launch_join_rows_gather(src, j.tuples[cur], W, side, found, storage_bytes(src.stype), g.vals, src.validity ? g.nulls : nullptr, p->stream));
+            k_join_rows_gather<<<grid_for(found, p->sm_count, 16), 256, 0, p->stream>>>(src, j.tuples[cur], W, side, found, storage_bytes(src.stype), g.vals,
+                                                                                        src.validity ? g.nulls : nullptr);
+            CK(p, cudaGetLastError());
             p->stats.kernel_launches++;
             if (src.validity) {
                 DevCol packed;

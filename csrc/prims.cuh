@@ -32,7 +32,7 @@ __global__ void k_gather_sel(GatherArgs g, const uint32_t* sel, uint64_t n, uint
 
 // Rows on the device, in the one format the library keeps them in: per column its values and null BYTES (1 = NULL), and the Arrow
 // validity bitmap packed from those bytes for the kernels that read DevCols.  Holds ORDER BY's / the window stage's retained rows
-// (sort.cu), the hash join's build sides and gathered chunk (join.cu) and the post fragment's input (api.cu, join.cu, window.cu).
+// (sort.cu), the hash join's build sides and gathered chunk (join.cu) and the post fragment's input (agg.cu, join.cu, window.cu).
 // The buffers come from the plan's allocator, which returns them at bkgpu_close.
 struct RowStore {
     struct Col {
