@@ -11,7 +11,8 @@
 
 namespace bk {
 
-// build-side columns gathered to probe-row alignment (k_join_gather)
+// build-side columns gathered to probe-row alignment (k_join_gather): elements of 8, 4, 16 (a STRING slot: the AVG blob a MERGE_AGG over
+// the join reads) or 1 byte
 struct GatherCols { int32_t n; const uint8_t* src[MAX_COLS]; uint8_t* dst[MAX_COLS]; int32_t elem[MAX_COLS]; };
 // star join (PK_STAR_AGG): per dimension with unique keys, the fact foreign key, its slot in the row-id tuple and the dimension's key index
 struct StarLookup { DevCol fk; int32_t from_prim, cast_prim, slot; JoinFast jf; };
@@ -135,6 +136,7 @@ __global__ void __launch_bounds__(256) k_join_gather(DevCol pk, int from_prim, i
             for (int c = 0; c < gc.n; c++) {
                 if (gc.elem[c] == 8) ((uint64_t*)gc.dst[c])[r] = __ldg((const unsigned long long*)gc.src[c] + br[u]);
                 else if (gc.elem[c] == 4) ((uint32_t*)gc.dst[c])[r] = __ldg((const uint32_t*)gc.src[c] + br[u]);
+                else if (gc.elem[c] == 16) ((uint4*)gc.dst[c])[r] = __ldg((const uint4*)gc.src[c] + br[u]);   // a MERGE_AGG's AVG {sum, count} blob
                 else gc.dst[c][r] = __ldg(gc.src[c] + br[u]);
             }
         }

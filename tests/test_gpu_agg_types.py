@@ -212,10 +212,10 @@ def _ordered(want, keys_desc):
 
 
 @gpu
-@pytest.mark.parametrize("vt", [T.INT8, T.FLOAT, T.BOOL, T.UINT16], ids=tname)
+@pytest.mark.parametrize("vt", TYPES, ids=tname)
 def test_having_and_order_by_over_narrow_results(vt):
-    """HAVING COUNT(*) > 3 and ORDER BY MIN(v) DESC, key LIMIT 20 above the aggregate: the post fragment writes MIN / MAX back as
-    4-byte (INT8, UINT16), FLOAT and 1-byte (BOOL) columns (k_images_to_columns)"""
+    """HAVING COUNT(*) > 3 and ORDER BY MIN(v) DESC, key LIMIT 20 above the aggregate: the post fragment writes MIN / MAX of every
+    type back as 1-, 4- and 8-byte columns (k_images_to_columns) into its input store"""
     rng = np.random.default_rng(8000 + int(vt))
     t = key_table(rng, T.INT32, N, vt=vt, value_nulls=0.05, n_random=200)
     t.v = [x if isinstance(x, (int, np.integer)) or x == x else 0.0 for x in t.v]

@@ -11,21 +11,13 @@ from baikaldb_b200.exec_node import ColumnSource, DeviceColumn, GpuExecNode, Row
 from baikaldb_b200.plan import PrimitiveType as T
 from tests import apply_cases as C
 from tests import apply_oracle as A
+from tests.util import ragged, to_device
 
 pytestmark = pytest.mark.gpu
 
 GROUP = [P.slot_ref(1, 2, T.INT32)]
 AGGS = [P.agg_expr("count_star", 2, 1), P.agg_expr("count", 2, 2, None, P.slot_ref(1, 1, T.INT32)), P.agg_expr("sum", 2, 3, None, P.slot_ref(1, 4, T.INT64)),
         P.agg_expr("min", 2, 4, None, P.slot_ref(1, 4, T.INT64)), P.agg_expr("max", 2, 5, None, P.slot_ref(1, 4, T.INT64))]
-
-
-def ragged(cols, cuts):
-    """`cols` as batches cut at the given row counts, the rest last"""
-    out, lo = [], 0
-    for n in cuts + [len(cols[0]) - sum(cuts)]:
-        out.append([make_column(c.tuple_id, c.slot_id, c.prim_type, c.values[lo:lo + n], None if c.valid is None else c.valid[lo:lo + n]) for c in cols])
-        lo += n
-    return out
 
 
 def check(c: C.Case, outer, inner, batches=None, group=GROUP, aggs=AGGS):
@@ -72,21 +64,6 @@ def test_empty_inner_empty_outer_and_all_null_keys(name):
     nulls = lambda cols: [make_column(x.tuple_id, x.slot_id, x.prim_type, x.values, np.zeros(len(x.values), bool) if x.slot_id == 1 else x.valid) for x in cols]
     all_null = check(c, nulls(outer), nulls(inner))
     assert bool(all_null) == (c.jt == "ANTI_SEMI_JOIN")   # a NULL key matches nothing
-
-
-def to_device(cols):
-    import torch
-    out = []
-    for x in cols:
-        v = torch.from_numpy(np.ascontiguousarray(x.values)).cuda()
-        bits = 0
-        keep = [v]
-        if x.valid is not None:
-            b = torch.from_numpy(np.concatenate([np.packbits(x.valid, bitorder="little"), np.zeros(64, np.uint8)])).cuda()
-            keep.append(b)
-            bits = b.data_ptr()
-        out.append(DeviceColumn(x.tuple_id, x.slot_id, x.prim_type, v.data_ptr(), len(x.values), bits, keepalive=keep))
-    return out
 
 
 @pytest.mark.parametrize("name", ["exists", "q21_not_exists", "long_in_list"])

@@ -12,18 +12,9 @@ from tests import filtered_join_cases as C
 from tests import full_join_cases as F
 from tests.date_fn_cases import date_image
 from tests.full_join_cases import col
-from tests.util import assert_same_rows, run_both
+from tests.util import assert_same_rows, ragged, run_both
 
 pytestmark = pytest.mark.gpu
-
-
-def ragged(cols, cuts):
-    """`cols` pushed as batches cut at the given row counts, the rest last"""
-    out, lo = [], 0
-    for n in cuts + [len(cols[0]) - sum(cuts)]:
-        out.append([make_column(c.tuple_id, c.slot_id, c.prim_type, c.values[lo:lo + n], None if c.valid is None else c.valid[lo:lo + n]) for c in cols])
-        lo += n
-    return out
 
 
 def pairs(jt, build, probe, bf=(), pf=(), residual=(), batches=None):

@@ -7,7 +7,7 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 
 from baikaldb_b200 import _lib
-from baikaldb_b200.column import Column, rows_as_set
+from baikaldb_b200.column import Column, make_column, rows_as_set
 from baikaldb_b200.exec_node import ColumnSource, DeviceColumn, GpuExecNode, RowBatch, RuntimeState, execute
 from oracle import oracle
 
@@ -66,6 +66,31 @@ def run_both(plan, cols, keys, options: Optional[Dict[str, int]] = None, rel=REL
     if check_scanned:  # (a LIMIT lets the pull-based row engine stop scanning early; a pushed batch is always scanned whole)
         assert stats.rows_scanned == want.rows_scanned, (stats.rows_scanned, want.rows_scanned)
     return got, stats, want
+
+
+def ragged(cols, cuts):
+    """`cols` as batches cut at the given row counts, the rest last"""
+    out, lo = [], 0
+    for n in cuts + [len(cols[0]) - sum(cuts)]:
+        out.append([make_column(c.tuple_id, c.slot_id, c.prim_type, c.values[lo:lo + n], None if c.valid is None else c.valid[lo:lo + n]) for c in cols])
+        lo += n
+    return out
+
+
+def to_device(cols):
+    """host columns as DeviceColumns on cuda:0 (validity bitmaps padded by 64 bytes)"""
+    import torch
+    out = []
+    for x in cols:
+        v = torch.from_numpy(np.ascontiguousarray(x.values)).cuda()
+        bits = 0
+        keep = [v]
+        if x.valid is not None:
+            b = torch.from_numpy(np.concatenate([np.packbits(x.valid, bitorder="little"), np.zeros(64, np.uint8)])).cuda()
+            keep.append(b)
+            bits = b.data_ptr()
+        out.append(DeviceColumn(x.tuple_id, x.slot_id, x.prim_type, v.data_ptr(), len(x.values), bits, keepalive=keep))
+    return out
 
 
 def open_node(plan, batches, options=None):
