@@ -477,8 +477,11 @@ static void timer_end(bkgpu_plan* p, EventPair* ep) { if (ep) cudaEventRecord(ep
 
 int agg_open(bkgpu_plan* p) {
     const AggPlan& ap = p->c.ap;
-    GroupTable& gt = p->gt;
-    int log2 = ap.n_keyw == 0 ? 0 : p->group_cap_log2;
+    AggState& g = p->agg;
+    GroupTable& gt = g.gt;
+    if (cudaHostAlloc((void**)&g.h_pinned, 64, cudaHostAllocDefault) == cudaSuccess) memset(g.h_pinned, 0, 64); else g.h_pinned = nullptr;
+    g.blocking_wait = g.blocking_sync >= 0 ? g.blocking_sync != 0 : (p->nranks > 1 && cpu_budget() < 4 * p->nranks);   // (agg_wait)
+    int log2 = ap.n_keyw == 0 ? 0 : g.group_cap_log2;
     size_t cap = (size_t)1 << log2;
     gt.cap_mask = (uint32_t)(cap - 1); gt.cap_log2 = (uint32_t)log2;
     int rc;
@@ -488,21 +491,21 @@ int agg_open(bkgpu_plan* p) {
     if ((rc = dev_alloc(p, (void**)&gt.n_groups, 4 * ((size_t)GT_OCC_OFF + cap)))) return rc;   // counter, overflow flag, occupied list
     gt.overflow = gt.n_groups + 1;
     if (ap.n_hll) {   // hll_add_agg: the register arena, one block per (group, sketch) that receives a value
-        if ((rc = dev_alloc(p, (void**)&gt.hll_regs, (size_t)p->hll_cap * HLL_REGISTERS))) return rc;
+        if ((rc = dev_alloc(p, (void**)&gt.hll_regs, (size_t)g.hll_cap * HLL_REGISTERS))) return rc;
         if ((rc = dev_alloc(p, (void**)&gt.hll_ctr, 16))) return rc;
-        gt.hll_cap = (uint32_t)p->hll_cap;
+        gt.hll_cap = (uint32_t)g.hll_cap;
         CK(p, cudaMemsetAsync(gt.hll_ctr, 0, 16, p->stream));
     }
     if (p->c.n_rb) {   // rb_build_agg: the pair buffer and the sort's second buffer (one word more each: the build's scan closes on it)
-        if ((rc = dev_alloc(p, (void**)&p->rb.keys, ((size_t)p->rb_cap + 1) * 8))) return rc;
-        if ((rc = dev_alloc(p, (void**)&p->rb.alt, ((size_t)p->rb_cap + 1) * 8))) return rc;
-        if ((rc = dev_alloc(p, (void**)&p->rb.ctr, 8))) return rc;
-        p->rb.cap = (uint64_t)p->rb_cap;
-        CK(p, cudaMemsetAsync(p->rb.ctr, 0, 8, p->stream));
-        p->rb.hi = 0;
+        if ((rc = dev_alloc(p, (void**)&g.rb.keys, ((size_t)g.rb_cap + 1) * 8))) return rc;
+        if ((rc = dev_alloc(p, (void**)&g.rb.alt, ((size_t)g.rb_cap + 1) * 8))) return rc;
+        if ((rc = dev_alloc(p, (void**)&g.rb.ctr, 8))) return rc;
+        g.rb.cap = (uint64_t)g.rb_cap;
+        CK(p, cudaMemsetAsync(g.rb.ctr, 0, 8, p->stream));
+        g.rb.hi = 0;
     }
-    p->d_cursor = gt.n_groups + 2;                       // [2] result cursor [3] merge info
-    p->d_rows_passed = (uint64_t*)(gt.n_groups + 4);     // [4..5] rows that passed the filter
+    g.d_cursor = gt.n_groups + 2;                       // [2] result cursor [3] merge info
+    g.d_rows_passed = (uint64_t*)(gt.n_groups + 4);     // [4..5] rows that passed the filter
     CK(p, cudaMemsetAsync(gt.n_groups, 0, 4 * GT_OCC_OFF, p->stream));
     k_table_init<<<grid_for((int64_t)cap, p->sm_count, 8), 256, 0, p->stream>>>(gt, ap, 0);
     CK(p, cudaGetLastError());
@@ -510,11 +513,21 @@ int agg_open(bkgpu_plan* p) {
     return BKGPU_OK;
 }
 
+// (the plan's device buffers go back to the allocator with every other buffer of the plan)
+void agg_close(bkgpu_plan* p) {
+    AggState& g = p->agg;
+    if (g.wait_event) cudaEventDestroy(g.wait_event);
+    if (g.h_pinned) cudaFreeHost(g.h_pinned);
+    if (g.h_outv) cudaFreeHost(g.h_outv);
+    if (g.rb.bytes) cudaFreeHost(g.rb.bytes);
+    if (g.h_fused && !mapped_put(g.fused_bytes, g.h_fused)) cudaFreeHost(g.h_fused);
+}
+
 // the group count an earlier launch left in pinned memory: the 4-byte copy after a launch, or the counter block of a fused extraction
 // (read without a synchronisation: a stale value only costs speed)
-static void learn_groups(bkgpu_plan* p) {
-    if (p->h_pinned && p->h_pinned[0] > p->known_groups) p->known_groups = p->h_pinned[0];
-    if (p->h_fused) { const uint32_t g = *(const volatile uint32_t*)p->h_fused; if (g > p->known_groups) p->known_groups = g; }
+static void learn_groups(AggState& g) {
+    if (g.h_pinned && g.h_pinned[0] > g.known_groups) g.known_groups = g.h_pinned[0];
+    if (g.h_fused) { const uint32_t n = *(const volatile uint32_t*)g.h_fused; if (n > g.known_groups) g.known_groups = n; }
 }
 
 // device images of an extracted row: one per group expression, per aggregate its final value (+2 for an AVG blob)
@@ -527,21 +540,22 @@ static int agg_n_img(const AggPlan& ap) {
 // the mapped host buffer of the fused extraction, sized for the groups seen so far (at least 2048 rows); false = too many groups
 // to extract this way (the table is then read back by k_extract)
 static bool ensure_fused(bkgpu_plan* p) {
+    AggState& g = p->agg;
     uint32_t want = 2048;
-    while (want < p->known_groups && want < (1u << 16)) want *= 2;
-    if (want < p->known_groups) return false;
-    if (p->h_fused && p->fused_cap >= want) return true;
-    if (p->h_fused) {   // (a launch still running may write into it)
+    while (want < g.known_groups && want < (1u << 16)) want *= 2;
+    if (want < g.known_groups) return false;
+    if (g.h_fused && g.fused_cap >= want) return true;
+    if (g.h_fused) {   // (a launch still running may write into it)
         cudaStreamSynchronize(p->stream);
-        if (!mapped_put(p->fused_bytes, p->h_fused)) cudaFreeHost(p->h_fused);
-        p->h_fused = p->d_fused = nullptr; p->fused_cap = 0;
+        if (!mapped_put(g.fused_bytes, g.h_fused)) cudaFreeHost(g.h_fused);
+        g.h_fused = g.d_fused = nullptr; g.fused_cap = 0;
     }
     const size_t bytes = 32 + (size_t)want * (size_t)agg_n_img(p->c.ap) * 9;
     uint8_t* h = mapped_take(bytes);
     if (!h && cudaHostAlloc((void**)&h, bytes, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) { cudaGetLastError(); return false; }
-    if (cudaHostGetDevicePointer((void**)&p->d_fused, h, 0) != cudaSuccess) { cudaGetLastError(); cudaFreeHost(h); return false; }
+    if (cudaHostGetDevicePointer((void**)&g.d_fused, h, 0) != cudaSuccess) { cudaGetLastError(); cudaFreeHost(h); return false; }
     memset(h, 0, 32);
-    p->h_fused = h; p->fused_bytes = bytes; p->fused_cap = want;
+    g.h_fused = h; g.fused_bytes = bytes; g.fused_cap = want;
     return true;
 }
 
@@ -549,38 +563,38 @@ static bool ensure_fused(bkgpu_plan* p) {
 // a launch can still overflow the pair buffer, and the request then fails at bkgpu_finish).  When the keys could outgrow the buffer, it is
 // sorted and deduplicated first (a set does not depend on order), and the launch shrinks to the rows that fit
 static int rb_room(bkgpu_plan* p, const Compiled& c, int64_t* rows) {
-    const uint64_t per = (uint64_t)c.n_rb, cap = p->rb.cap;
-    if (p->rb.hi + (uint64_t)*rows * per > cap) {
+    RbState& rb = p->agg.rb;
+    const uint64_t per = (uint64_t)c.n_rb, cap = rb.cap;
+    if (rb.hi + (uint64_t)*rows * per > cap) {
         uint64_t n = 0;
         const int rc = rb_compact(p, &n);
         if (rc) return rc;
-        p->rb.hi = n;
+        rb.hi = n;
         const int64_t fit = (int64_t)((cap - n) / per) & ~7ll;   // (a multiple of 8 rows: the next launch's validity bitmaps stay byte-aligned)
         if (fit < 8)
             return p->fail(BKGPU_ETOOBIG, "rb_build_agg: the pair buffer holds %llu distinct (group, value) pairs and is full: raise rb_pair_capacity",
                            (unsigned long long)n);
         if (*rows > fit && !p->join.tail_launch) *rows = fit;   // (the join's tail walks every build row in one launch)
     }
-    p->rb.hi += (uint64_t)*rows * per;
+    rb.hi += (uint64_t)*rows * per;
     return BKGPU_OK;
 }
 
 int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp) {
-    AggEnv env;
-    env.force_generic = p->force_generic; env.no_lean = p->no_lean; env.no_lean_nulls = p->no_lean_nulls; env.no_lean_mm = p->no_lean_mm;
-    env.lean_fx = p->lean_fx; env.fx_off = p->fx_off;
-    env.scalar_tma = p->scalar_tma; env.smem_cap_log2 = p->smem_cap_log2;
+    AggState& g = p->agg;
+    AggEnv env = g.env;   // the options, and what this launch adds to them
+    env.fx_off = g.fx_off;
     env.tail_launch = p->join.tail_launch;
     env.multi_rank = p->nccl_comm && p->nranks > 1; env.has_post = p->c.post != nullptr;
-    if (c.ap.n_keyw > 0 && p->smem_cap_log2 < 0) learn_groups(p);   // (the shared table is sized from it)
-    env.known_groups = p->known_groups;
+    if (c.ap.n_keyw > 0 && env.smem_cap_log2 < 0) learn_groups(g);   // (the shared table is sized from it)
+    env.known_groups = g.known_groups;
     AggArgs a; AggSelection sel;
     const int rc = select_agg_launch(c, cols, nrows, vec_ok, jp, env, a, sel);
     if (rc == BKGPU_ENOMEM) return p->fail(rc, "lean kernel: shared table does not fit");
     if (rc) return rc;
-    a.gt = p->gt; a.rows_passed = p->d_rows_passed;
+    a.gt = g.gt; a.rows_passed = g.d_rows_passed;
     if (c.kind == PK_JOIN_AGG) a.join = join_args(p, p->join.tail_launch);
-    if (sel.fused_ok && ensure_fused(p)) { a.fused_out = p->d_fused; a.fused_cap = p->fused_cap; }
+    if (sel.fused_ok && ensure_fused(p)) { a.fused_out = g.d_fused; a.fused_cap = g.fused_cap; }
     const int64_t kMax = (int64_t)1 << 30;  // rows per launch (32-bit counters inside a CTA)
     int64_t algo_bytes_per_row = 0;
     for (int i = 0; i < a.n_cols; i++) algo_bytes_per_row += storage_bytes(a.cols[i].stype);
@@ -591,14 +605,14 @@ int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64
         if (c.n_rb) {   // (a compaction swaps the pair buffer with the sort's second buffer)
             const int rrc = rb_room(p, c, &b.nrows);
             if (rrc) return rrc;
-            b.rb_keys = p->rb.keys; b.rb_ctr = p->rb.ctr; b.rb_cap = p->rb.cap;
+            b.rb_keys = g.rb.keys; b.rb_ctr = g.rb.ctr; b.rb_cap = g.rb.cap;
         }
         b_rows = b.nrows;
         for (int i = 0; i < b.n_cols; i++) b.cols[i] = col_at(a.cols[i], off);
         EventPair* ep = timer_begin(p, p->timed, b.nrows * algo_bytes_per_row, false);
         cudaError_t e = launch_agg(b, sel.kernel, sel.smem, p->sm_count, p->stream, ep ? ep->a : nullptr);
         timer_end(p, ep);
-        p->fused_last = b.fused_out != nullptr;
+        g.fused_last = b.fused_out != nullptr;
         if (e != cudaSuccess) return p->cuda_fail(e, "launch_agg");
         snprintf(p->stats.main_kernel_name, sizeof p->stats.main_kernel_name, "%s", agg_kernel_name(sel.kernel));
         p->stats.kernel_launches++;
@@ -631,54 +645,56 @@ static int hll_check_host_sketches(bkgpu_plan* p, const bkgpu_column* cols, int 
 
 // a PK_AGG batch
 int agg_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device) {
+    AggState& g = p->agg;
     int rc = on_device ? BKGPU_OK : hll_check_host_sketches(p, cols, ncols, nrows);
     if (rc) return rc;
     rc = feed(p, p->c.cols, cols, ncols, nrows, on_device, agg_batch);
     if (rc) return rc;
     // learn the cardinality for later batches' table size (no sync: a stale value only costs speed); a launch that extracted its
     // result has already left the count in h_fused
-    if (p->c.ap.n_keyw > 0 && p->smem_cap_log2 < 0 && p->h_pinned && !p->fused_last)
-        CK(p, cudaMemcpyAsync(p->h_pinned, p->gt.n_groups, 4, cudaMemcpyDeviceToHost, p->stream));
+    if (p->c.ap.n_keyw > 0 && g.env.smem_cap_log2 < 0 && g.h_pinned && !g.fused_last)
+        CK(p, cudaMemcpyAsync(g.h_pinned, g.gt.n_groups, 4, cudaMemcpyDeviceToHost, p->stream));
     return BKGPU_OK;
 }
 
 // groups per rank in the exchanged partial state: never more than the group table can hold (every rank runs the same plan with
 // the same options, so all ranks agree on it) — a 2^14-slot table ships 0.8 MB per rank instead of the 3 MB of the default cap
 static uint32_t eff_pcap(const bkgpu_plan* p) {
-    const int64_t table = p->c.ap.n_keyw == 0 ? 1 : (int64_t)1 << p->group_cap_log2;
-    return (uint32_t)std::min<int64_t>(p->partial_cap, table);
+    const int64_t table = p->c.ap.n_keyw == 0 ? 1 : (int64_t)1 << p->agg.group_cap_log2;
+    return (uint32_t)std::min<int64_t>(p->agg.partial_cap, table);
 }
 
 // the collective step of bkgpu_finish: regions -> one set per GPU, the per-GPU partial tables meet once and are folded by K3.
 // Default: compact rows, one ncclAllGather of 1 + bound x (key + lane words) per rank — `bound` = the largest group count any rank
 // held in earlier runs of this plan (2048 on the first run); the merge reports the true maximum and the exchange is repeated once
-// with a larger bound when it did not fit.  Option repartition: all-to-all by key owner.
+// with a larger bound when it did not fit.  Option repartition: all-to-all by key owner.  Runs only with two or more ranks.
 static int agg_collective(bkgpu_plan* p, bool* rows_mode) {
     const AggPlan& ap = p->c.ap;
-    GroupTable& gt = p->gt;
+    AggState& g = p->agg;
+    GroupTable& gt = g.gt;
     *rows_mode = false;
     const uint32_t pcap = eff_pcap(p);
     int rc;
-    const bool repart = p->repartition && ap.n_keyw > 0;   // (a scalar aggregate has one group: nothing to partition)
+    const bool repart = g.repartition && ap.n_keyw > 0;   // (a scalar aggregate has one group: nothing to partition)
     EventPair* ep = timer_begin(p, p->timed_coll, 0);
     if (!repart) {
         *rows_mode = true;
-        if (p->rank < 0 && nccl_comm_rank(p->nccl_comm, &p->rank) != 0) return p->fail(BKGPU_ENCCL, "ncclCommUserRank: %s", nccl_last_error());
-        uint32_t bound = p->merge_bound ? p->merge_bound : 2048u;
+        if (g.rank < 0 && nccl_comm_rank(p->nccl_comm, &g.rank) != 0) return p->fail(BKGPU_ENCCL, "ncclCommUserRank: %s", nccl_last_error());
+        uint32_t bound = g.merge_bound ? g.merge_bound : 2048u;
         if (ap.n_keyw == 0) bound = 1;
         bound = std::min<uint32_t>(bound, pcap);
         const size_t rw = (size_t)(ap.n_keyw + ap.n_lanes + ap.n_hll * HLL_ROW_WORDS);
         const size_t words = 1 + rw * bound;
-        if ((rc = ensure_buf(p, (void**)&p->d_partial, &p->d_partial_cap, words * 8))) return rc;
-        if ((rc = ensure_buf(p, (void**)&p->d_gather, &p->d_gather_cap, words * 8 * (size_t)p->nranks))) return rc;
-        CK(p, cudaMemsetAsync(p->d_partial, 0, 8, p->stream));
-        k_partial_export_rows<<<grid_for((int64_t)gt.cap_mask + 1, p->sm_count, 1), 256, 0, p->stream>>>(gt, ap, p->d_partial, bound);
+        if ((rc = ensure_buf(p, (void**)&g.d_partial, &g.d_partial_cap, words * 8))) return rc;
+        if ((rc = ensure_buf(p, (void**)&g.d_gather, &g.d_gather_cap, words * 8 * (size_t)p->nranks))) return rc;
+        CK(p, cudaMemsetAsync(g.d_partial, 0, 8, p->stream));
+        k_partial_export_rows<<<grid_for((int64_t)gt.cap_mask + 1, p->sm_count, 1), 256, 0, p->stream>>>(gt, ap, g.d_partial, bound);
         CK(p, cudaGetLastError());
-        if (nccl_all_gather(p->nccl_comm, p->d_partial, p->d_gather, words, p->stream) != 0) return p->fail(BKGPU_ENCCL, "ncclAllGather: %s", nccl_last_error());
+        if (nccl_all_gather(p->nccl_comm, g.d_partial, g.d_gather, words, p->stream) != 0) return p->fail(BKGPU_ENCCL, "ncclAllGather: %s", nccl_last_error());
         const int gx = (int)std::min<uint32_t>(std::max<uint32_t>((bound + 255) / 256, 1), 64);
-        k_partial_merge_rows<<<dim3((unsigned)gx, (unsigned)p->nranks), 256, 0, p->stream>>>(gt, ap, p->d_gather, words, bound, p->nranks, p->rank, p->d_cursor + 1);
+        k_partial_merge_rows<<<dim3((unsigned)gx, (unsigned)p->nranks), 256, 0, p->stream>>>(gt, ap, g.d_gather, words, bound, p->nranks, g.rank, g.d_cursor + 1);
         CK(p, cudaGetLastError());
-        p->merge_bound_used = bound;
+        g.merge_bound_used = bound;
         p->stats.kernel_launches += 2;
         timer_end(p, ep);
         return BKGPU_OK;
@@ -686,18 +702,18 @@ static int agg_collective(bkgpu_plan* p, bool* rows_mode) {
     // hash repartition: every rank keeps only the groups it owns — an all-to-all of per-owner segments instead of the
     // all-gather; the merged table (and the result) of a rank is its partition, the union over ranks is the answer
     const size_t words = 1 + (size_t)(ap.n_keyw + ap.n_lanes) * pcap;
-    if ((rc = ensure_buf(p, (void**)&p->d_partial, &p->d_partial_cap, words * 8 * (size_t)p->nranks))) return rc;
-    if ((rc = ensure_buf(p, (void**)&p->d_gather, &p->d_gather_cap, words * 8 * (size_t)p->nranks))) return rc;
-    if (!p->d_part_cursors && (rc = dev_alloc(p, (void**)&p->d_part_cursors, 4 * (size_t)p->nranks))) return rc;
+    if ((rc = ensure_buf(p, (void**)&g.d_partial, &g.d_partial_cap, words * 8 * (size_t)p->nranks))) return rc;
+    if ((rc = ensure_buf(p, (void**)&g.d_gather, &g.d_gather_cap, words * 8 * (size_t)p->nranks))) return rc;
+    if (!g.d_part_cursors && (rc = dev_alloc(p, (void**)&g.d_part_cursors, 4 * (size_t)p->nranks))) return rc;
     if (p->nranks > 1024) return p->cuda_fail(cudaErrorInvalidValue, "k_partial_counts: more than 1024 ranks");
-    CK(p, cudaMemsetAsync(p->d_part_cursors, 0, sizeof(uint32_t) * (size_t)p->nranks, p->stream));
-    k_partial_export_parts<<<grid_for((int64_t)gt.cap_mask + 1, p->sm_count, 8), 256, 0, p->stream>>>(gt, ap, p->d_partial, words, pcap, p->d_part_cursors, p->nranks);
-    k_partial_counts<<<1, 1024, 0, p->stream>>>(p->d_partial, words, p->d_part_cursors, pcap, p->nranks);
+    CK(p, cudaMemsetAsync(g.d_part_cursors, 0, sizeof(uint32_t) * (size_t)p->nranks, p->stream));
+    k_partial_export_parts<<<grid_for((int64_t)gt.cap_mask + 1, p->sm_count, 8), 256, 0, p->stream>>>(gt, ap, g.d_partial, words, pcap, g.d_part_cursors, p->nranks);
+    k_partial_counts<<<1, 1024, 0, p->stream>>>(g.d_partial, words, g.d_part_cursors, pcap, p->nranks);
     CK(p, cudaGetLastError());
-    if (nccl_all_to_all(p->nccl_comm, p->d_partial, p->d_gather, words, p->nranks, p->stream) != 0) return p->fail(BKGPU_ENCCL, "all-to-all: %s", nccl_last_error());
+    if (nccl_all_to_all(p->nccl_comm, g.d_partial, g.d_gather, words, p->nranks, p->stream) != 0) return p->fail(BKGPU_ENCCL, "all-to-all: %s", nccl_last_error());
     k_table_init<<<grid_for((int64_t)gt.cap_mask + 1, p->sm_count, 8), 256, 0, p->stream>>>(gt, ap, 1);   // (keeps the overflow flag an export beyond partial_capacity raised)
     CK(p, cudaGetLastError());
-    k_partial_merge<<<grid_for(pcap, p->sm_count, 8), 256, 0, p->stream>>>(gt, ap, p->d_gather, words, pcap, p->nranks);
+    k_partial_merge<<<grid_for(pcap, p->sm_count, 8), 256, 0, p->stream>>>(gt, ap, g.d_gather, words, pcap, p->nranks);
     CK(p, cudaGetLastError());
     timer_end(p, ep);
     p->stats.kernel_launches += 4;
@@ -720,7 +736,7 @@ static int agg_post(bkgpu_plan* p, uint32_t n_out, uint32_t out_cap) {
         img += p->c.out_cols[c].kind == 1 ? 2 : 1;
     }
     if (n_out) {
-        k_images_to_columns<<<grid_for(n_out, p->sm_count, 8), 256, 0, p->stream>>>(p->d_outv, p->d_outn, out_cap, n_out, pcs);
+        k_images_to_columns<<<grid_for(n_out, p->sm_count, 8), 256, 0, p->stream>>>(p->agg.d_outv, p->agg.d_outn, out_cap, n_out, pcs);
         CK(p, cudaGetLastError());
     }
     std::vector<DevCol> dc(std::max<size_t>(nc, 1));
@@ -741,11 +757,12 @@ static int agg_post(bkgpu_plan* p, uint32_t n_out, uint32_t out_cap) {
 // rank for the python thread, NCCL's proxy thread and this wait) a spinning wait burns the quota the other ranks' launches need:
 // there the thread sleeps on a blocking-sync event instead (option blocking_sync: -1 auto, 0 spin, 1 sleep)
 static int agg_wait(bkgpu_plan* p) {
+    AggState& g = p->agg;
     const double t0 = HostClock::now();
-    if (p->blocking_wait) {
-        if (!p->wait_event) CK(p, cudaEventCreateWithFlags(&p->wait_event, cudaEventBlockingSync | cudaEventDisableTiming));
-        CK(p, cudaEventRecord(p->wait_event, p->stream));
-        CK(p, cudaEventSynchronize(p->wait_event));
+    if (g.blocking_wait) {
+        if (!g.wait_event) CK(p, cudaEventCreateWithFlags(&g.wait_event, cudaEventBlockingSync | cudaEventDisableTiming));
+        CK(p, cudaEventRecord(g.wait_event, p->stream));
+        CK(p, cudaEventSynchronize(g.wait_event));
     } else CK(p, cudaStreamSynchronize(p->stream));
     p->hclk.extract_wait += HostClock::now() - t0;
     return BKGPU_OK;
@@ -753,14 +770,15 @@ static int agg_wait(bkgpu_plan* p) {
 
 // what the counter block of a finished request tells the plan: rows that passed, FX's exact-path count, the groups it holds
 static int agg_take_counters(bkgpu_plan* p, const uint32_t* ctr) {
-    memcpy(&p->rows_passed_host, ctr + 4, 8);
+    AggState& g = p->agg;
+    memcpy(&g.rows_passed_host, ctr + 4, 8);
     // FX: values beyond the sampled scale are added exactly, one global atomic each; a plan whose double columns keep producing many of them
     // (a column spanning dozens of binades, outliers dominating the sample) goes back to the CAS kernel for its later launches
-    if (ctr[GT_FX_EXACT] > 4096 && (uint64_t)ctr[GT_FX_EXACT] * 64 > (uint64_t)std::max<int64_t>(p->rows_passed_host, 1)) p->fx_off = 1;
+    if (ctr[GT_FX_EXACT] > 4096 && (uint64_t)ctr[GT_FX_EXACT] * 64 > (uint64_t)std::max<int64_t>(g.rows_passed_host, 1)) g.fx_off = 1;
     if (ctr[1]) return p->fail(BKGPU_ETOOBIG, "group table overflow (capacity 2^%d slots / partial_capacity %lld): raise group_capacity_log2",
-                               (int)p->gt.cap_log2, (long long)p->partial_cap);
-    if (ctr[0] > p->known_groups) p->known_groups = ctr[0];
-    p->finish_groups = ctr[0];
+                               (int)g.gt.cap_log2, (long long)g.partial_cap);
+    if (ctr[0] > g.known_groups) g.known_groups = ctr[0];
+    g.finish_groups = ctr[0];
     return BKGPU_OK;
 }
 
@@ -768,22 +786,23 @@ static int agg_take_counters(bkgpu_plan* p, const uint32_t* ctr) {
 // ("3a300000 00000000": the reference's initialize gives every group an empty bitmap, so a group whose values were all NULL returns it)
 static void rb_column(bkgpu_plan* p, HostCol& hc, const uint64_t* slot, int64_t rows, int rb_idx) {
     static const uint8_t empty[8] = {0x3a, 0x30, 0, 0, 0, 0, 0, 0};
+    RbState& rb = p->agg.rb;
     std::vector<int64_t> b((size_t)rows);   // each row's bitmap in the directory, -1 = none
     int64_t total = 0;
     for (int64_t r = 0; r < rows; r++) {
         const uint32_t id = (uint32_t)(slot[r] << 2) | (uint32_t)rb_idx;
-        const auto it = std::lower_bound(p->rb.bid.begin(), p->rb.bid.end(), id);
-        b[r] = it != p->rb.bid.end() && *it == id ? (int64_t)(it - p->rb.bid.begin()) : -1;
-        total += b[r] < 0 ? 8 : (int64_t)(p->rb.off[b[r] + 1] - p->rb.off[b[r]]);
+        const auto it = std::lower_bound(rb.bid.begin(), rb.bid.end(), id);
+        b[r] = it != rb.bid.end() && *it == id ? (int64_t)(it - rb.bid.begin()) : -1;
+        total += b[r] < 0 ? 8 : (int64_t)(rb.off[b[r] + 1] - rb.off[b[r]]);
     }
-    std::vector<uint8_t>& col = p->rb.col[rb_idx];
+    std::vector<uint8_t>& col = rb.col[rb_idx];
     col.resize(((size_t)rows + 1) * 8 + (size_t)total);
     int64_t* offs = (int64_t*)col.data();
     uint8_t* d = col.data() + ((size_t)rows + 1) * 8;
     offs[0] = 0;
     for (int64_t r = 0; r < rows; r++) {
-        const size_t len = b[r] < 0 ? 8 : (size_t)(p->rb.off[b[r] + 1] - p->rb.off[b[r]]);
-        memcpy(d + offs[r], b[r] < 0 ? empty : p->rb.bytes + p->rb.off[b[r]], len);
+        const size_t len = b[r] < 0 ? 8 : (size_t)(rb.off[b[r] + 1] - rb.off[b[r]]);
+        memcpy(d + offs[r], b[r] < 0 ? empty : rb.bytes + rb.off[b[r]], len);
         offs[r + 1] = offs[r] + (int64_t)len;
     }
     hc.elem = -1;
@@ -824,7 +843,7 @@ static void agg_result(bkgpu_plan* p, const uint64_t* hv, const uint8_t* hn, siz
             for (int64_t r = 0; r < keep; r++) {
                 uint8_t* o = d + (size_t)r * HLL_RAW_BYTES;
                 memcpy(o, "HYLL", 4); o[4] = HLL_ENC_RAW;
-                if (v[r]) { o[15] = 0x80; memcpy(o + HLL_HDR_BYTES, p->hll_host.data() + (size_t)(v[r] - 1) * HLL_REGISTERS, HLL_REGISTERS); }
+                if (v[r]) { o[15] = 0x80; memcpy(o + HLL_HDR_BYTES, p->agg.hll_host.data() + (size_t)(v[r] - 1) * HLL_REGISTERS, HLL_REGISTERS); }
             }
         } else switch (prim_storage(oc.prim)) {
             case ST_I32: for (int64_t r = 0; r < keep; r++) { const int32_t x = (int32_t)(int64_t)v[r]; memcpy(d + (size_t)r * 4, &x, 4); } break;
@@ -846,125 +865,144 @@ static void agg_result(bkgpu_plan* p, const uint64_t* hv, const uint8_t* hn, siz
     p->result_rows = keep; p->result_pos = 0;
 }
 
-// hll_add_agg: the arena's claimed blocks to the host (the extracted rows reference them), after the request's last kernel.  A claim
-// that found the arena full fails the request: a sketch that lost values would be wrong, not approximate
-static int hll_fetch(bkgpu_plan* p) {
-    if (!p->c.ap.n_hll) return BKGPU_OK;
-    uint32_t ctr[3] = {0, 0, 0};
-    CK(p, cudaMemcpyAsync(ctr, p->gt.hll_ctr, 12, cudaMemcpyDeviceToHost, p->stream));
+// the HLL arena's counters ([0] blocks claimed, [1] a claim found the arena full, [2] a merged value was not a RAW sketch) to the host, then
+// the one synchronisation (copies the caller queued before come back with it).  A claim that found the arena full fails the request, with
+// the caller's message `full` (its %u: hll_group_capacity): a sketch that lost values would be wrong, not approximate
+static int hll_counters(bkgpu_plan* p, uint32_t ctr[3], const char* full) {
+    const GroupTable& gt = p->agg.gt;
+    ctr[0] = ctr[1] = ctr[2] = 0;
+    if (gt.hll_ctr) CK(p, cudaMemcpyAsync(ctr, gt.hll_ctr, 12, cudaMemcpyDeviceToHost, p->stream));
     CK(p, cudaStreamSynchronize(p->stream));
     if (ctr[2]) return p->fail(BKGPU_EINVAL, "MERGE_AGG of hll_add_agg: an input value is not a RAW HLL sketch (\"HYLL\", encoding 255, 16400 bytes)");
-    if (ctr[1] || ctr[0] > p->gt.hll_cap)
-        return p->fail(BKGPU_ETOOBIG, "hll_add_agg: more than %u sketches (groups x hll_add_agg aggregates with a value): raise hll_group_capacity",
-                       p->gt.hll_cap);
-    p->hll_host.resize((size_t)ctr[0] * HLL_REGISTERS);
-    if (ctr[0]) CK(p, cudaMemcpy(p->hll_host.data(), p->gt.hll_regs, (size_t)ctr[0] * HLL_REGISTERS, cudaMemcpyDeviceToHost));
-    p->stats.d2h_bytes += (int64_t)p->hll_host.size() + 8;
+    if (ctr[1] || ctr[0] > gt.hll_cap) return p->fail(BKGPU_ETOOBIG, full, gt.hll_cap);
     return BKGPU_OK;
 }
 
-int agg_finish(bkgpu_plan* p) {
+// hll_add_agg: the arena's claimed blocks to the host (the extracted rows reference them), after the request's last kernel
+static int hll_fetch(bkgpu_plan* p) {
+    if (!p->c.ap.n_hll) return BKGPU_OK;
+    AggState& g = p->agg;
+    uint32_t ctr[3];
+    int rc;
+    if ((rc = hll_counters(p, ctr, "hll_add_agg: more than %u sketches (groups x hll_add_agg aggregates with a value): raise hll_group_capacity"))) return rc;
+    g.hll_host.resize((size_t)ctr[0] * HLL_REGISTERS);
+    if (ctr[0]) CK(p, cudaMemcpy(g.hll_host.data(), g.gt.hll_regs, (size_t)ctr[0] * HLL_REGISTERS, cudaMemcpyDeviceToHost));
+    p->stats.d2h_bytes += (int64_t)g.hll_host.size() + 8;
+    return BKGPU_OK;
+}
+
+// The table's groups into the pinned landing area (g.h_outv / h_outn, rows of stride g.out_cap_alloc).  The extraction is speculative, into
+// the buffers kept from earlier runs: the counter block and the rows come back in ONE synchronisation; only a result larger than the buffers
+// costs a second one.  ctr: the counter block ([0] groups [1] overflow [2] rows extracted [3] merge info [4..5] rows passed).
+// `rows_mode`: an all-gather ran before (agg_collective); when some rank held more groups than it was sized for, nothing was merged and this
+// returns after the first synchronisation, for the caller to exchange again
+static int agg_extract(bkgpu_plan* p, bool rows_mode, uint32_t ctr[8]) {
     const AggPlan& ap = p->c.ap;
-    GroupTable& gt = p->gt;
-    uint32_t host_counts[2] = {0, 0};
-    uint64_t* finish_hv = nullptr; uint8_t* finish_hn = nullptr; uint32_t finish_n_out = 0, finish_out_cap = 0;
-    const bool multi = p->nccl_comm && p->nranks > 1;
-    bool rows_mode = false;
+    AggState& g = p->agg;
     const int n_img = agg_n_img(ap);
     int rc;
-    // the request ended with a launch that extracted its own result into mapped host memory: one wait, nothing else on the device
-    if (p->fused_last && !multi && !p->c.post) {
+    for (int attempt = 0; attempt < 2; attempt++) {
+        uint32_t want = std::max<uint32_t>(std::max<uint32_t>(g.known_groups, 1), attempt ? std::max<uint32_t>(ctr[0], 1) : 1);
+        if (ap.n_keyw == 0) want = 1;
+        if (g.out_cap_alloc < want) {
+            dev_free(p, g.d_outv); g.d_outv = nullptr; g.d_outn = nullptr;
+            size_t cap = std::max<size_t>(want, 2048);
+            if ((rc = dev_alloc(p, (void**)&g.d_outv, cap * 9 * (size_t)n_img + 64))) return rc;   // values, then the null bytes: ONE copy brings both back
+            g.d_outn = (uint8_t*)(g.d_outv + cap * (size_t)n_img);
+            g.out_cap_alloc = cap;
+        }
+        const uint32_t out_cap = (uint32_t)g.out_cap_alloc;
+        CK(p, cudaMemsetAsync(g.d_cursor, 0, sizeof(uint32_t), p->stream));
+        k_extract<<<grid_for((int64_t)g.gt.cap_mask + 1, p->sm_count, 1), 256, 0, p->stream>>>(g.gt, ap, g.d_outv, g.d_outn, out_cap, g.d_cursor, p->c.emit_default ? 1 : 0);
+        CK(p, cudaGetLastError());
+        p->stats.kernel_launches++;
+        const size_t n_words = (size_t)out_cap * (size_t)n_img;
+        if (g.h_out_cap < n_words) {   // pinned: the copies below are truly asynchronous and land in one synchronisation
+            if (g.h_outv) cudaFreeHost(g.h_outv);
+            g.h_outv = nullptr; g.h_outn = nullptr; g.h_out_cap = 0;
+            CK(p, cudaHostAlloc((void**)&g.h_outv, n_words * 9 + 64, cudaHostAllocDefault));
+            g.h_out_cap = n_words;
+        }
+        g.h_outn = (uint8_t*)(g.h_outv + n_words);
+        // two copies, one synchronisation: the 32-byte counter block and the extracted rows (values + null bytes, contiguous on both sides)
+        uint32_t local_ctr[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        uint32_t* hc = g.h_pinned ? g.h_pinned + 8 : local_ctr;
+        CK(p, cudaMemcpyAsync(hc, g.gt.n_groups, 32, cudaMemcpyDeviceToHost, p->stream));
+        if ((const uint8_t*)g.d_outn == (const uint8_t*)(g.d_outv + n_words)) CK(p, cudaMemcpyAsync(g.h_outv, g.d_outv, n_words * 9, cudaMemcpyDeviceToHost, p->stream));
+        else {
+            CK(p, cudaMemcpyAsync(g.h_outv, g.d_outv, n_words * 8, cudaMemcpyDeviceToHost, p->stream));
+            CK(p, cudaMemcpyAsync(g.h_outn, g.d_outn, n_words, cudaMemcpyDeviceToHost, p->stream));
+        }
         if ((rc = agg_wait(p))) return rc;
-        const uint32_t* ctr = (const uint32_t*)p->h_fused;
+        memcpy(ctr, hc, 32);
+        if (rows_mode) {
+            if (ctr[3] > g.merge_bound_used) return BKGPU_OK;   // nothing was merged (k_partial_merge_rows)
+            const uint32_t learned = (std::max<uint32_t>(ctr[3], 1u) + 63u) & ~63u;   // the bound of the next request's all-gather
+            if (learned > g.merge_bound) g.merge_bound = learned;
+        }
+        p->stats.d2h_bytes += (int64_t)(n_words * 9 + 12);
+        if ((rc = agg_take_counters(p, ctr))) return rc;
+        if (ctr[2] <= out_cap) break;   // everything fitted
+    }
+    return BKGPU_OK;
+}
+
+// the result of the request from the table: `exchange` = first merge it with the other ranks' tables (agg_collective)
+static int agg_finish_table(bkgpu_plan* p, bool exchange) {
+    AggState& g = p->agg;
+    int rc;
+    // 1. the request ended with a launch that extracted its own result into mapped host memory: one wait, nothing else on the device
+    if (g.fused_last && !exchange && !p->c.post) {
+        if ((rc = agg_wait(p))) return rc;
+        const uint32_t* ctr = (const uint32_t*)g.h_fused;
         if ((rc = agg_take_counters(p, ctr))) return rc;
         const uint32_t n = ctr[0];
-        if (n <= p->fused_cap) {
+        if (n <= g.fused_cap) {
+            const int n_img = agg_n_img(p->c.ap);
             p->stats.d2h_bytes += (int64_t)(32 + (size_t)n * (size_t)n_img * 9);
-            const uint64_t* hv = (const uint64_t*)(p->h_fused + 32);
+            const uint64_t* hv = (const uint64_t*)(g.h_fused + 32);
             agg_result(p, hv, (const uint8_t*)(hv + (size_t)n * (size_t)n_img), n, n);
             return BKGPU_OK;
         }
         // more groups than the buffer holds: the table is read back below (the next launch's buffer is sized for them)
     }
-  for (int mtry = 0; mtry < 3; mtry++) {   // (a second trip only when some rank held more groups than the exchange was sized for)
-    { const double t0 = HostClock::now(); if (multi && (rc = agg_collective(p, &rows_mode))) return rc; p->hclk.collective += HostClock::now() - t0; }
-    uint32_t n_out = 0, out_cap = 0, merge_max = 0;
-    uint64_t* hv = nullptr; uint8_t* hn = nullptr;
-    bool redo_merge = false;
-    for (int attempt = 0; attempt < 2; attempt++) {
-        // speculative extraction into the buffers kept from earlier runs: counts, cursor and rows come back
-        // in ONE synchronisation; only a result larger than the buffers costs a second round
-        uint32_t want = std::max<uint32_t>(std::max<uint32_t>(p->known_groups, 1), attempt ? std::max<uint32_t>(host_counts[0], 1) : 1);
-        if (ap.n_keyw == 0) want = 1;
-        if (p->out_cap_alloc < want) {
-            dev_free(p, p->d_outv); p->d_outv = nullptr; p->d_outn = nullptr;
-            size_t cap = std::max<size_t>(want, 2048);
-            if ((rc = dev_alloc(p, (void**)&p->d_outv, cap * 9 * (size_t)n_img + 64))) return rc;   // values, then the null bytes: ONE copy brings both back
-            p->d_outn = (uint8_t*)(p->d_outv + cap * (size_t)n_img);
-            p->out_cap_alloc = cap;
-        }
-        out_cap = (uint32_t)p->out_cap_alloc;
-        CK(p, cudaMemsetAsync(p->d_cursor, 0, sizeof(uint32_t), p->stream));
-        k_extract<<<grid_for((int64_t)gt.cap_mask + 1, p->sm_count, 1), 256, 0, p->stream>>>(gt, ap, p->d_outv, p->d_outn, out_cap, p->d_cursor, p->c.emit_default ? 1 : 0);
-        CK(p, cudaGetLastError());
-        p->stats.kernel_launches++;
-        const size_t n_words = (size_t)out_cap * (size_t)n_img;
-        if (p->h_out_cap < n_words) {   // pinned: the four copies below are truly asynchronous and land in one synchronisation
-            if (p->h_outv) cudaFreeHost(p->h_outv);
-            p->h_outv = nullptr; p->h_outn = nullptr; p->h_out_cap = 0;
-            CK(p, cudaHostAlloc((void**)&p->h_outv, n_words * 9 + 64, cudaHostAllocDefault));
-            p->h_out_cap = n_words;
-        }
-        hv = p->h_outv; hn = p->h_outn = (uint8_t*)(p->h_outv + n_words);
-        // two copies, one synchronisation: the 32-byte counter block (groups, overflow, rows extracted, merge info, rows passed) and
-        // the extracted rows (values + null bytes, contiguous on both sides)
-        uint32_t local_ctr[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-        uint32_t* hc3 = p->h_pinned ? p->h_pinned + 8 : local_ctr;   // [8] groups [9] overflow [10] rows extracted [11] merge info [12..13] rows passed
-        CK(p, cudaMemcpyAsync(hc3, gt.n_groups, 32, cudaMemcpyDeviceToHost, p->stream));
-        if ((const uint8_t*)p->d_outn == (const uint8_t*)(p->d_outv + n_words)) CK(p, cudaMemcpyAsync(hv, p->d_outv, n_words * 9, cudaMemcpyDeviceToHost, p->stream));
-        else {
-            CK(p, cudaMemcpyAsync(hv, p->d_outv, n_words * 8, cudaMemcpyDeviceToHost, p->stream));
-            CK(p, cudaMemcpyAsync(hn, p->d_outn, n_words, cudaMemcpyDeviceToHost, p->stream));
-        }
-        if ((rc = agg_wait(p))) return rc;
-        host_counts[0] = hc3[0]; host_counts[1] = hc3[1]; n_out = hc3[2]; merge_max = hc3[3];
-        if (rows_mode) {
-            const uint32_t mx = merge_max;
-            if (mx > p->merge_bound_used) {   // nothing was merged (k_partial_merge_rows): exchange again, sized for what the ranks really hold
-                if (mx > eff_pcap(p)) return p->fail(BKGPU_ETOOBIG, "a rank holds %u groups, more than partial_capacity %lld: raise partial_capacity", mx, (long long)p->partial_cap);
-                p->merge_bound = (mx + 63u) & ~63u;
-                redo_merge = true;
-                break;
-            }
-            const uint32_t learned = (std::max<uint32_t>(mx, 1u) + 63u) & ~63u;
-            if (learned > p->merge_bound) p->merge_bound = learned;
-        }
-        p->stats.d2h_bytes += (int64_t)(n_words * 9 + 12);
-        if ((rc = agg_take_counters(p, hc3))) return rc;
-        if (n_out <= out_cap) break;   // everything fitted
+    // 2. [the exchange ->] the extraction; a round is repeated only when some rank held more groups than the all-gather was sized for
+    uint32_t ctr[8];
+    for (int round = 0;; round++) {
+        bool rows_mode = false;
+        { const double t0 = HostClock::now(); if (exchange && (rc = agg_collective(p, &rows_mode))) return rc; p->hclk.collective += HostClock::now() - t0; }
+        if ((rc = agg_extract(p, rows_mode, ctr))) return rc;
+        if (!rows_mode || ctr[3] <= g.merge_bound_used) break;
+        if (ctr[3] > eff_pcap(p)) return p->fail(BKGPU_ETOOBIG, "a rank holds %u groups, more than partial_capacity %lld: raise partial_capacity", ctr[3], (long long)g.partial_cap);
+        g.merge_bound = (ctr[3] + 63u) & ~63u;
+        if (round == 2) return p->fail(BKGPU_ENCCL, "partial-state exchange did not converge");
     }
-    if (!redo_merge) { finish_hv = hv; finish_hn = hn; finish_n_out = n_out; finish_out_cap = out_cap; break; }
-    if (mtry == 2) return p->fail(BKGPU_ENCCL, "partial-state exchange did not converge");
-  }
-    uint32_t n_out = finish_n_out, out_cap = finish_out_cap;
-    if (n_out > out_cap) n_out = out_cap;
+    // 3. the sketches and bitmaps the rows reference, then the post fragment or the host columns
+    const uint32_t out_cap = (uint32_t)g.out_cap_alloc, n_out = std::min(ctr[2], out_cap);
     if ((rc = hll_fetch(p))) return rc;
     if (p->c.n_rb && (rc = rb_build(p))) return rc;
     if (p->c.post) return agg_post(p, n_out, out_cap);
-    agg_result(p, finish_hv, finish_hn, out_cap, n_out);
+    agg_result(p, g.h_outv, g.h_outn, out_cap, n_out);
     return BKGPU_OK;
+}
+
+int agg_finish(bkgpu_plan* p) {
+    const int rc = agg_finish_table(p, p->nccl_comm && p->nranks > 1);
+    if (!rc) p->stats.rows_filtered = p->stats.rows_scanned - (int64_t)p->agg.rows_passed_host;   // (came back with the counter block)
+    return rc;
 }
 
 // Re-arm the table for the next request.  A finished run knows how many groups its table holds (the count came back with the result):
 // clear those slots through the occupied list instead of re-initialising the whole capacity (2^20 slots = 44 MB by default)
 int agg_reset(bkgpu_plan* p) {
-    if (p->state == S_FINISHED && p->finish_groups >= 0 && p->c.ap.n_keyw > 0)
-        k_table_clear<<<grid_for(p->finish_groups, p->sm_count, 8), 256, 0, p->stream>>>(p->gt, p->c.ap, (uint32_t)p->finish_groups);
-    else k_table_init<<<grid_for((int64_t)p->gt.cap_mask + 1, p->sm_count, 8), 256, 0, p->stream>>>(p->gt, p->c.ap, 0);
+    AggState& g = p->agg;
+    if (p->state == S_FINISHED && g.finish_groups >= 0 && p->c.ap.n_keyw > 0)
+        k_table_clear<<<grid_for(g.finish_groups, p->sm_count, 8), 256, 0, p->stream>>>(g.gt, p->c.ap, (uint32_t)g.finish_groups);
+    else k_table_init<<<grid_for((int64_t)g.gt.cap_mask + 1, p->sm_count, 8), 256, 0, p->stream>>>(g.gt, p->c.ap, 0);
     CK(p, cudaGetLastError());
-    p->finish_groups = -1;
-    p->fused_last = false;
-    if (p->rb.ctr) { CK(p, cudaMemsetAsync(p->rb.ctr, 0, 8, p->stream)); p->rb.hi = 0; }   // (rb_build_agg: the pair buffer is empty again)
+    g.finish_groups = -1;
+    g.fused_last = false;
+    if (g.rb.ctr) { CK(p, cudaMemsetAsync(g.rb.ctr, 0, 8, p->stream)); g.rb.hi = 0; }   // (rb_build_agg: the pair buffer is empty again)
     p->stats.kernel_launches++;
     return BKGPU_OK;
 }
@@ -975,34 +1013,31 @@ size_t agg_partial_bytes(const bkgpu_plan* p) {
     return 8 * (1 + (size_t)(p->c.ap.n_keyw + p->c.ap.n_lanes + p->c.ap.n_hll * HLL_ROW_WORDS) * (size_t)eff_pcap(p));
 }
 int agg_partial_export(bkgpu_plan* p, void* dev_dst) {
+    const GroupTable& gt = p->agg.gt;
     CK(p, cudaMemsetAsync(dev_dst, 0, 8, p->stream));
-    k_partial_export_rows<<<grid_for((int64_t)p->gt.cap_mask + 1, p->sm_count, 1), 256, 0, p->stream>>>(p->gt, p->c.ap, (uint64_t*)dev_dst, eff_pcap(p));
+    k_partial_export_rows<<<grid_for((int64_t)gt.cap_mask + 1, p->sm_count, 1), 256, 0, p->stream>>>(gt, p->c.ap, (uint64_t*)dev_dst, eff_pcap(p));
     CK(p, cudaGetLastError());
     p->stats.kernel_launches += 1;
-    uint64_t held = 0; uint32_t ov = 0, hll_ctr[3] = {0, 0, 0};
+    uint64_t held = 0; uint32_t ov = 0, hll_ctr[3];
     CK(p, cudaMemcpyAsync(&held, dev_dst, 8, cudaMemcpyDeviceToHost, p->stream));
-    CK(p, cudaMemcpyAsync(&ov, p->gt.overflow, 4, cudaMemcpyDeviceToHost, p->stream));
-    if (p->gt.hll_ctr) CK(p, cudaMemcpyAsync(hll_ctr, p->gt.hll_ctr, 12, cudaMemcpyDeviceToHost, p->stream));
-    CK(p, cudaStreamSynchronize(p->stream));
-    if (hll_ctr[2]) return p->fail(BKGPU_EINVAL, "MERGE_AGG of hll_add_agg: an input value is not a RAW HLL sketch (\"HYLL\", encoding 255, 16400 bytes)");
-    if (hll_ctr[1]) return p->fail(BKGPU_ETOOBIG, "hll_add_agg: more than %u sketches: raise hll_group_capacity", p->gt.hll_cap);
-    if (ov) return p->fail(BKGPU_ETOOBIG, "group table overflow (capacity 2^%d slots): raise group_capacity_log2", (int)p->gt.cap_log2);
-    if (held > eff_pcap(p)) return p->fail(BKGPU_ETOOBIG, "this rank holds %llu groups, more than partial_capacity=%lld", (unsigned long long)held, (long long)p->partial_cap);
+    CK(p, cudaMemcpyAsync(&ov, gt.overflow, 4, cudaMemcpyDeviceToHost, p->stream));
+    int rc;
+    if ((rc = hll_counters(p, hll_ctr, "hll_add_agg: more than %u sketches: raise hll_group_capacity"))) return rc;
+    if (ov) return p->fail(BKGPU_ETOOBIG, "group table overflow (capacity 2^%d slots): raise group_capacity_log2", (int)gt.cap_log2);
+    if (held > eff_pcap(p)) return p->fail(BKGPU_ETOOBIG, "this rank holds %llu groups, more than partial_capacity=%lld", (unsigned long long)held, (long long)p->agg.partial_cap);
     return BKGPU_OK;
 }
 // fold `nranks` exported partial states into the table, then finish the request on this plan alone
 int agg_partial_merge(bkgpu_plan* p, const void* dev_src, int nranks) {
+    AggState& g = p->agg;
     const uint32_t pcap = eff_pcap(p);
-    k_table_init<<<grid_for((int64_t)p->gt.cap_mask + 1, p->sm_count, 8), 256, 0, p->stream>>>(p->gt, p->c.ap, 1);
+    k_table_init<<<grid_for((int64_t)g.gt.cap_mask + 1, p->sm_count, 8), 256, 0, p->stream>>>(g.gt, p->c.ap, 1);
     CK(p, cudaGetLastError());
     const int gx = (int)std::min<uint32_t>(std::max<uint32_t>((pcap + 255) / 256, 1), 64);
-    k_partial_merge_rows<<<dim3((unsigned)gx, (unsigned)nranks), 256, 0, p->stream>>>(p->gt, p->c.ap, (const uint64_t*)dev_src, agg_partial_bytes(p) / 8, pcap, nranks,
-                                                                                   -1 /* fold every segment */, p->d_cursor + 1);
+    k_partial_merge_rows<<<dim3((unsigned)gx, (unsigned)nranks), 256, 0, p->stream>>>(g.gt, p->c.ap, (const uint64_t*)dev_src, agg_partial_bytes(p) / 8, pcap, nranks,
+                                                                                   -1 /* fold every segment */, g.d_cursor + 1);
     CK(p, cudaGetLastError());
-    p->fused_last = false;   // (the merged table is read back by k_extract)
+    g.fused_last = false;   // (the merged table is read back by k_extract)
     p->stats.kernel_launches += 2;
-    void* comm = p->nccl_comm; int nr = p->nranks; p->nccl_comm = nullptr; p->nranks = 1;  // already merged: finalize locally
-    const int rc = agg_finish(p);
-    p->nccl_comm = comm; p->nranks = nr;
-    return rc;
+    return agg_finish_table(p, false);   // (already merged)
 }

@@ -78,7 +78,7 @@ struct DevCache {
     }
 };
 DevCache& dev_cache() { static DevCache c; return c; }
-// the mapped host buffers of the fused extraction (bkgpu_plan::h_fused) are kept the same way: pinning and unpinning one costs a
+// the mapped host buffers of the fused extraction (AggState::h_fused) are kept the same way: pinning and unpinning one costs a
 // plan's open and close about a tenth of a millisecond
 struct MappedCache {
     std::mutex mu;
@@ -179,29 +179,27 @@ extern "C" int bkgpu_set_option(bkgpu_plan* p, const char* key, int64_t v) {
     if (p->state != S_INIT) return p->fail(BKGPU_ESTATE, "options must be set before bkgpu_open");
     std::string k = key;
     if (k == "stream") { p->stream = (cudaStream_t)(uintptr_t)v; p->own_stream = false; }
-    else if (k == "group_capacity_log2") { if (v < 4 || v > 30) return p->fail(BKGPU_EINVAL, "group_capacity_log2 out of range"); p->group_cap_log2 = (int)v; }
-    else if (k == "smem_capacity_log2") { if (v < -1 || v > 13) return p->fail(BKGPU_EINVAL, "smem_capacity_log2 out of range"); p->smem_cap_log2 = (int)v; }
+    else if (k == "group_capacity_log2") { if (v < 4 || v > 30) return p->fail(BKGPU_EINVAL, "group_capacity_log2 out of range"); p->agg.group_cap_log2 = (int)v; }
+    else if (k == "smem_capacity_log2") { if (v < -1 || v > 13) return p->fail(BKGPU_EINVAL, "smem_capacity_log2 out of range"); p->agg.env.smem_cap_log2 = (int)v; }
     else if (k == "batch_capacity") { if (v < 1) return p->fail(BKGPU_EINVAL, "batch_capacity must be positive"); p->batch_capacity = v; }
     else if (k == "chunk_rows") { if (v < 1024) return p->fail(BKGPU_EINVAL, "chunk_rows too small"); p->chunk_rows = (v + 7) & ~7ll; }
-    else if (k == "rb_pair_capacity") { if (v < 1024 || v > RADIX_MAX_KEYS) return p->fail(BKGPU_EINVAL, "rb_pair_capacity out of range (1024 .. 2^30 - 1)"); p->rb_cap = v; }
-    else if (k == "hll_group_capacity") { if (v < 1 || v > (1 << 20)) return p->fail(BKGPU_EINVAL, "hll_group_capacity out of range (1 .. 2^20)"); p->hll_cap = v; }
-    else if (k == "partial_capacity") { if (v < 1) return p->fail(BKGPU_EINVAL, "partial_capacity must be positive"); p->partial_cap = v; }
-    else if (k == "force_generic") p->force_generic = v != 0;
-    else if (k == "lean_fx") p->lean_fx = v != 0;
-    else if (k == "blocking_sync") p->blocking_sync = (int)v;
+    else if (k == "rb_pair_capacity") { if (v < 1024 || v > RADIX_MAX_KEYS) return p->fail(BKGPU_EINVAL, "rb_pair_capacity out of range (1024 .. 2^30 - 1)"); p->agg.rb_cap = v; }
+    else if (k == "hll_group_capacity") { if (v < 1 || v > (1 << 20)) return p->fail(BKGPU_EINVAL, "hll_group_capacity out of range (1 .. 2^20)"); p->agg.hll_cap = v; }
+    else if (k == "partial_capacity") { if (v < 1) return p->fail(BKGPU_EINVAL, "partial_capacity must be positive"); p->agg.partial_cap = v; }
+    else if (k == "force_generic") p->agg.env.force_generic = v != 0;
+    else if (k == "lean_fx") p->agg.env.lean_fx = v != 0;
+    else if (k == "blocking_sync") p->agg.blocking_sync = (int)v;
     else if (k == "star_expand_capacity") { if (v < 0 || v > 0x7FFFFFFF) return p->fail(BKGPU_EINVAL, "star_expand_capacity out of range"); p->join.star_expand_cap = (int)v; }
-    else if (k == "no_lean") p->no_lean = v != 0;
+    else if (k == "no_lean") p->agg.env.no_lean = v != 0;
     else if (k == "no_fused_probe") p->join.no_fused_probe = v != 0;
-    else if (k == "repartition") p->repartition = v != 0;
-    else if (k == "no_lean_nulls") p->no_lean_nulls = v != 0;
-    else if (k == "no_lean_mm") p->no_lean_mm = v != 0;
-    else if (k == "scalar_tma") p->scalar_tma = v != 0;
+    else if (k == "repartition") p->agg.repartition = v != 0;
+    else if (k == "no_lean_nulls") p->agg.env.no_lean_nulls = v != 0;
+    else if (k == "no_lean_mm") p->agg.env.no_lean_mm = v != 0;
+    else if (k == "scalar_tma") p->agg.env.scalar_tma = v != 0;
     else if (k == "region_base") p->region_base = v;
     else return p->fail(BKGPU_EINVAL, "unknown option '%s'", key);
     return BKGPU_OK;
 }
-
-namespace { int cpu_budget(); }   // CPUs this process may use (affinity, cgroup quota): defined with the copy pool
 
 // the plan's IN sets (OP_IN_SET) in one device allocation, kept until bkgpu_close (bkgpu_reset keeps them), and their addresses
 // patched into every program that probes them.  Part of opening the plan, not of a request: not counted in h2d_bytes.
@@ -230,13 +228,12 @@ extern "C" int bkgpu_open(bkgpu_plan* p) {
     CK(p, cudaSetDevice(p->device));
     if (!p->stream) { CK(p, cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking)); p->own_stream = true; }
     CK(p, cudaStreamCreateWithFlags(&p->copy_stream, cudaStreamNonBlocking));
-    if (cudaHostAlloc((void**)&p->h_pinned, 64, cudaHostAllocDefault) == cudaSuccess) memset(p->h_pinned, 0, 64); else p->h_pinned = nullptr;
     for (int i = 0; i < 2; i++) {
         CK(p, cudaEventCreateWithFlags(&p->stage_free[i], cudaEventDisableTiming));
         CK(p, cudaEventCreateWithFlags(&p->stage_ready[i], cudaEventDisableTiming));
     }
-    p->blocking_wait = p->blocking_sync >= 0 ? p->blocking_sync != 0 : (p->nranks > 1 && cpu_budget() < 4 * p->nranks);
-    if (p->c.ap.n_hll && p->repartition)
+    // (refusals that need only the plan and its options: before anything is allocated)
+    if (p->c.ap.n_hll && p->agg.repartition)
         return p->fail(BKGPU_EUNSUPPORTED, "hll_add_agg with the repartition merge is outside the GPU path: its sketches travel only with the all-gather of group rows");
     if (p->c.n_rb && p->nccl_comm)
         return p->fail(BKGPU_EUNSUPPORTED, "rb_build_agg with a communicator is outside the GPU path: bitmaps do not travel with the fixed-width partial rows");
@@ -350,6 +347,7 @@ class CopyPool {
     const std::function<void(int)>* fn_ = nullptr;
     int next_ = 0, total_ = 0, done_ = 0; uint64_t gen_ = 0; bool stop_ = false;
 };
+}  // namespace
 // CPUs this process may actually use: online CPUs, its affinity mask and its cgroup CPU quota (a container with a 16-CPU quota on a 128-CPU box
 // gets throttled for the rest of the scheduling period once its threads have burnt the quota — spinning or oversized pools make the copy SLOWER there)
 int cpu_budget() {
@@ -369,6 +367,7 @@ int cpu_budget() {
     }
     return n > 0 ? n : 1;
 }
+namespace {
 CopyPool& copy_pool() {
     static CopyPool pool([] {
         if (const char* e = getenv("BKGPU_COPY_THREADS")) { const int v = atoi(e); if (v > 0) return std::min(v, 64) - 1; }
@@ -522,13 +521,10 @@ static int bkgpu_finish_impl(bkgpu_plan* p) {
     CK(p, cudaSetDevice(p->device));
     int rc = BKGPU_OK;
     switch (p->c.kind) {
-        case PK_AGG: case PK_JOIN_AGG: case PK_STAR_AGG: {
+        case PK_AGG: case PK_JOIN_AGG: case PK_STAR_AGG:
             if (p->c.kind == PK_JOIN_AGG && (rc = join_tail(p))) break;
             rc = agg_finish(p);
-            if (!rc) {
-                p->stats.rows_filtered = p->stats.rows_scanned - (int64_t)p->rows_passed_host;   // (came back with the counter block)
-            }
-        } break;
+            break;
         case PK_JOIN: {   // the outer join's preserved rows, then the sink fragment's result
             std::vector<SortOutCol> cols; int64_t rows = 0;
             if ((rc = join_tail(p)) || (rc = sort_finish(p->post_sort, nullptr, 1, &p->stats, cols, &rows))) break;
@@ -644,11 +640,7 @@ extern "C" void bkgpu_close(bkgpu_plan* p) {
     for (auto& q : p->dev_allocs) if (!dev_cache().put(p->device, q.second, q.first)) cudaFree(q.first);   // (both streams were drained above)
     for (int i = 0; i < 2; i++) { if (p->stage_free[i]) cudaEventDestroy(p->stage_free[i]); if (p->stage_ready[i]) cudaEventDestroy(p->stage_ready[i]); }
     for (int i = 0; i < 2; i++) { for (uint8_t* q : p->bounce[i]) if (q) cudaFreeHost(q); if (p->bounce_done[i]) cudaEventDestroy(p->bounce_done[i]); }
-    if (p->wait_event) cudaEventDestroy(p->wait_event);
-    if (p->h_pinned) cudaFreeHost(p->h_pinned);
-    if (p->h_outv) cudaFreeHost(p->h_outv);
-    if (p->rb.bytes) cudaFreeHost(p->rb.bytes);
-    if (p->h_fused && !mapped_put(p->fused_bytes, p->h_fused)) cudaFreeHost(p->h_fused);   // (the stream was drained above)
+    agg_close(p);
     if (p->copy_stream) cudaStreamDestroy(p->copy_stream);
     if (p->own_stream && p->stream) cudaStreamDestroy(p->stream);
     delete p;

@@ -1,4 +1,6 @@
-// api_state.h — the plan object behind the C ABI (bkgpu_plan) and the host helpers api.cu, agg.cu and join.cu share.
+// api_state.h — the plan object behind the C ABI (bkgpu_plan), the state of its hash join (JoinState, join.cu) and of its aggregate
+// (AggState, agg.cu), and the host helpers api.cu, agg.cu and join.cu share.  bkgpu_plan itself holds what more than one stage uses: the
+// compiled plan, the device, streams and lifecycle state, the staging buffers, the result, the stats and the allocator.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdarg.h>
@@ -61,12 +63,53 @@ struct JoinState {
     uint32_t* jp_attr = nullptr; uint64_t* jp_packed = nullptr; size_t jp_attr_cap = 0, jp_packed_cap = 0;
     uint8_t* matched = nullptr; size_t matched_cap = 0;   // LEFT / SEMI / ANTI: build rows that found a partner (1), or that the build child's filter removed (2)
     uint8_t* probe_bits = nullptr; size_t probe_bits_cap = 0;   // the probe key's validity AND the probe child's own filter, for one probe batch
-    uint32_t* pairs = nullptr; size_t pairs_cap = 0; uint32_t* cursor = nullptr; size_t cursor_cap = 0;   // PK_JOIN: (probe row, build row) pairs of one batch
+    uint32_t* pairs = nullptr; size_t pairs_cap = 0;   // PK_JOIN, FULL: (probe row, build row) pairs of one batch
+    uint32_t* cursor = nullptr; size_t cursor_cap = 0;   // the count of a pass: pairs, the FK -> PK gather's misses, the star probe's survivors
     uint32_t* tuples[2] = {nullptr, nullptr}; size_t tuples_cap[2] = {0, 0};   // star join: row-id tuples of one chunk (probe / expansion ping-pong)
     RowStore chunk;   // the gathered chunk (two-table gather path, FULL join under an aggregate, star join), by plan column
     // options
     int no_fused_probe = 0;
     int star_expand_cap = 0;     // test option "star_expand_capacity": first capacity (tuples) of a star join's expansion pass (0 = twice its input)
+};
+
+// the aggregate of a plan (agg.cu): its group table, the exchange between ranks, the extraction of the result, what earlier requests taught
+// it, and its options.  Buffers are kept across bkgpu_reset; agg_reset clears what belongs to one request.
+struct AggState {
+    GroupTable gt{};
+    uint64_t* d_rows_passed = nullptr;   // the table's counter block: [4..5] rows that passed the filter
+    uint32_t* d_cursor = nullptr;        // ... [2] result cursor, [3] merge info (the largest group count of any rank)
+    // the exchange between ranks
+    uint64_t* d_partial = nullptr;  // export buffer (this rank)
+    uint64_t* d_gather = nullptr;   // nranks export buffers
+    size_t d_partial_cap = 0, d_gather_cap = 0;
+    uint32_t merge_bound = 0, merge_bound_used = 0;   // groups per rank the all-gather is sized for (learned from earlier runs)
+    uint32_t* d_part_cursors = nullptr;               // hash repartition of the groups across ranks (option "repartition")
+    int rank = -1;                // this rank in the communicator (-1 = not asked yet; the all-gather merge skips its own rows)
+    // extraction: device buffers (kept across resets) and their pinned landing area
+    uint64_t* d_outv = nullptr; uint8_t* d_outn = nullptr; size_t out_cap_alloc = 0;
+    uint64_t* h_outv = nullptr; uint8_t* h_outn = nullptr; size_t h_out_cap = 0;
+    // mapped host buffer the lean kernel's last CTA extracts the result into (AggArgs::fused_out), and whether the request's last
+    // aggregate launch did so: then agg_finish only waits and reads it
+    uint8_t* h_fused = nullptr; uint8_t* d_fused = nullptr; size_t fused_bytes = 0; uint32_t fused_cap = 0; bool fused_last = false;
+    // learned
+    uint32_t* h_pinned = nullptr;   // [0] groups seen (async copy after every aggregate launch that does not extract its result), [8..15] counter block; pinned
+    uint32_t known_groups = 0;
+    int64_t finish_groups = -1;     // groups in the table when the last finish read the result back (-1 = unknown: full re-initialisation)
+    int fx_off = 0;                 // set when a finished request saw more than 1/64 of its surviving rows take FX's exact path (see agg_take_counters)
+    uint64_t rows_passed_host = 0;
+    bool blocking_wait = false; cudaEvent_t wait_event = nullptr;   // see agg_wait
+    std::vector<uint8_t> hll_host;   // the HLL arena's claimed blocks, copied back by a finished request (agg_result reads the sketches there)
+    RbState rb;                      // rb_build_agg's pair buffer and build (rb.h)
+    // options: what the kernel choice reads (bkgpu_set_option writes them; launch_agg_batch fills in the per-launch fields of a copy).  By
+    // default COUNT(*) WHERE int32 <cmp> c runs the TMA-staged kernel (scalar_tma.cu), and the lean kernel's double sums are fixed-point
+    // limbs (FX, agg_direct.cuh) unless the environment's BKGPU_LEAN_FX says otherwise
+    AggEnv env = [] { AggEnv e; e.scalar_tma = 1; const char* v = getenv("BKGPU_LEAN_FX"); e.lean_fx = v ? atoi(v) != 0 : BK_LEAN_FX_DEFAULT; return e; }();
+    int group_cap_log2 = 20;
+    int64_t partial_cap = 1 << 16;
+    int64_t hll_cap = 4096;          // option hll_group_capacity: sketches the register arena holds (16 KB each: 64 MB by default)
+    int64_t rb_cap = (int64_t)1 << 27;   // option rb_pair_capacity: keys the rb_build_agg pair buffer holds (8 bytes each, twice: the sort's buffers)
+    int repartition = 0;
+    int blocking_sync = -1;
 };
 
 // BKGPU_TRACE=1: wall-clock time the HOST spends in each phase of a request (summed per plan, printed by bkgpu_close)
@@ -91,55 +134,22 @@ struct bkgpu_plan {
     // options
     cudaStream_t stream = nullptr; bool own_stream = false;
     cudaStream_t copy_stream = nullptr;
-    int group_cap_log2 = 20;
-    int smem_cap_log2 = -1;       // -1 = choose per batch
     int64_t batch_capacity = 1 << 20;
     int64_t chunk_rows = 8 << 20;
-    int64_t partial_cap = 1 << 16;
-    int64_t hll_cap = 4096;       // option hll_group_capacity: sketches the register arena holds (16 KB each: 64 MB by default)
-    std::vector<uint8_t> hll_host;   // the arena's claimed blocks, copied back by a finished request (agg_result reads the sketches there)
-    int64_t rb_cap = (int64_t)1 << 27;   // option rb_pair_capacity: keys the rb_build_agg pair buffer holds (8 bytes each, twice: the sort's buffers)
-    RbState rb;                   // rb_build_agg's pair buffer and build (rb.h)
-    int force_generic = 0;
-    int no_lean = 0;
     int64_t region_base = 0;      // arrival index of this plan's first row (ties across GPUs break by (region, row))
-    // aggregate state
-    GroupTable gt{};
-    uint64_t* d_rows_passed = nullptr;
-    uint32_t* d_cursor = nullptr;
-    uint64_t* d_partial = nullptr;  // export buffer (this rank)
-    uint64_t* d_gather = nullptr;   // nranks export buffers
-    size_t d_partial_cap = 0, d_gather_cap = 0;
     HostClock hclk; bool trace = getenv("BKGPU_TRACE") != nullptr;
-    std::vector<uint8_t*> bounce[2]; size_t bounce_rows = 0; cudaEvent_t bounce_done[2] = {nullptr, nullptr}; bool bounce_busy[2] = {false, false};
-    int scalar_tma = 1;           // COUNT(*) WHERE int32 <cmp> c runs the TMA-staged kernel (scalar_tma.cu); 0 = the LDG kernel
-    SortState* post_sort = nullptr;                         // the post fragment above the aggregate (Compiled::post)
-    RowStore post;                // the post fragment's input (Compiled::post's columns)
-    uint64_t rows_passed_host = 0;
-    int64_t finish_groups = -1;   // groups in the table when the last finish read the result back (-1 = unknown: full re-initialisation)
-    uint32_t merge_bound = 0, merge_bound_used = 0;   // groups per rank the all-gather is sized for (learned from earlier runs)
-    uint32_t* d_part_cursors = nullptr; int repartition = 0;   // hash repartition of the groups across ranks (option "repartition")
-    int rank = -1;                // this rank in the communicator (-1 = not asked yet; the all-gather merge skips its own rows)
-    uint64_t* d_outv = nullptr; uint8_t* d_outn = nullptr; size_t out_cap_alloc = 0;  // extraction buffers (kept across resets)
-    std::vector<cudaEvent_t> event_pool;
-    uint64_t* h_outv = nullptr; uint8_t* h_outn = nullptr; size_t h_out_cap = 0;   // pinned landing area of the extracted rows
-    uint32_t known_groups = 0;
-    uint32_t* h_pinned = nullptr;   // [0] groups seen (async copy after every aggregate launch that does not extract its result), pinned
-    // mapped host buffer the lean kernel's last CTA extracts the result into (AggArgs::fused_out), and whether the request's last
-    // aggregate launch did so: then bkgpu_finish only waits and reads it
-    uint8_t* h_fused = nullptr; uint8_t* d_fused = nullptr; size_t fused_bytes = 0; uint32_t fused_cap = 0; bool fused_last = false;
-    JoinState join;               // hash join (K4): PK_JOIN_AGG, PK_JOIN, PK_STAR_AGG
-    int fx_off = 0;               // set when a finished request saw more than 1/64 of its surviving rows take FX's exact path (see agg_finish)
-    int lean_fx = [] { const char* e = getenv("BKGPU_LEAN_FX"); return e ? atoi(e) != 0 : BK_LEAN_FX_DEFAULT; }();   // double sums as fixed-point limbs with native shared atomics (agg_direct.cuh, FX); option lean_fx
-    int blocking_sync = -1; bool blocking_wait = false; cudaEvent_t wait_event = nullptr;   // see agg_finish
-    int no_lean_nulls = 0, no_lean_mm = 0;
-    // sort / filter state
-    SortState* sort = nullptr;
     // host staging for pageable / pinned pushes
     std::vector<void*> stage[2];
     std::vector<void*> stage_valid[2];
     size_t stage_rows = 0;
     cudaEvent_t stage_free[2] = {nullptr, nullptr}, stage_ready[2] = {nullptr, nullptr};
+    std::vector<uint8_t*> bounce[2]; size_t bounce_rows = 0; cudaEvent_t bounce_done[2] = {nullptr, nullptr}; bool bounce_busy[2] = {false, false};
+    // the stages
+    SortState* post_sort = nullptr;   // the post fragment above the aggregate (Compiled::post)
+    RowStore post;                    // the post fragment's input (Compiled::post's columns)
+    SortState* sort = nullptr;        // ORDER BY / filter / window retention (PK_SORT, PK_FILTER, PK_WINDOW)
+    JoinState join;                   // hash join (K4): PK_JOIN_AGG, PK_JOIN, PK_STAR_AGG
+    AggState agg;                     // the aggregate: PK_AGG, PK_JOIN_AGG, PK_STAR_AGG
     // results
     std::vector<HostCol> result;
     int64_t result_rows = 0, result_pos = 0;
@@ -147,6 +157,7 @@ struct bkgpu_plan {
     bkgpu_stats stats{};
     std::vector<EventPair> timed;
     std::vector<EventPair> timed_coll;
+    std::vector<cudaEvent_t> event_pool;
     std::vector<std::pair<void*, size_t>> dev_allocs;   // (buffer, size class) — returned to the process-wide cache on free / close
 
     int fail(int code, const char* fmt, ...) {
@@ -169,6 +180,7 @@ int ensure_buf(bkgpu_plan* p, void** ptr, size_t* cap, size_t bytes);
 // cache does not keep it (the caller frees it)
 uint8_t* mapped_take(size_t bytes);
 bool mapped_put(size_t bytes, uint8_t* buf);
+int cpu_budget();   // CPUs this process may use (affinity, cgroup quota)
 // device buffers of one call: returned to the plan's allocator when the scope ends, on every way out of the call
 struct DevScope {
     bkgpu_plan* p;
@@ -203,12 +215,13 @@ inline DevCol col_at(const DevCol& c, int64_t off) {
 }
 
 // ---- agg.cu: the aggregate (PK_AGG, PK_JOIN_AGG, PK_STAR_AGG)
-int agg_open(bkgpu_plan* p);     // bkgpu_open: the group table (and the HLL arena, the rb_build_agg pair buffer)
+int agg_open(bkgpu_plan* p);     // bkgpu_open: the group table and the pinned counter words (and the HLL arena, the rb_build_agg pair buffer)
 int agg_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device);   // a PK_AGG batch
 // the aggregate of `c` over one batch; `jp`: fused FK -> PK probe (lean kernel only), +1 without launching when the batch does not fit it
 int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp = nullptr);
-int agg_finish(bkgpu_plan* p);   // the cross-rank merge (with a communicator), then the result
+int agg_finish(bkgpu_plan* p);   // the cross-rank merge (with a communicator), then the result and stats.rows_filtered
 int agg_reset(bkgpu_plan* p);    // bkgpu_reset: the table is empty again
+void agg_close(bkgpu_plan* p);   // bkgpu_close, once the plan's streams have drained: the host memory the aggregate holds
 size_t agg_partial_bytes(const bkgpu_plan* p);
 int agg_partial_export(bkgpu_plan* p, void* dev_dst);
 int agg_partial_merge(bkgpu_plan* p, const void* dev_src, int nranks);   // and the result from the merged table

@@ -405,6 +405,7 @@ static int join_build_index(bkgpu_plan* p, JoinSide& s, const DevCol& key, int c
     int rc;
     s.jf = JoinFast{};
     if (s.store.rows <= 0) return BKGPU_OK;
+    if ((rc = ensure_buf(p, (void**)&j.cursor, &j.cursor_cap, 64))) return rc;   // (the gather's misses, the star probe's survivors)
     bool retry_measured = false;
 again:
     const int cls = host_prim_class(cast_prim);
@@ -547,7 +548,7 @@ static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nro
     const JoinSide& s = j.side[0];
     std::vector<DevCol> all = join_cols(p, probe_cols);
     // ---- FK -> PK fast path: gather the build columns next to the probe rows, then the ordinary (lean) aggregate ----
-    if (s.jf.mode != 0 && j.jp.mode != 0 && c.jfast && !p->force_generic && !j.no_fused_probe) {
+    if (s.jf.mode != 0 && j.jp.mode != 0 && c.jfast && !p->agg.env.force_generic && !j.no_fused_probe) {
         // ---- fused probe: the lean aggregate reads the foreign key and looks the group key up itself ----
         const Compiled& f = *c.jfast;
         std::vector<DevCol> fc(f.cols.size());
@@ -560,7 +561,7 @@ static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nro
         const int rc = launch_agg_batch(p, f, fc.data(), nrows, vec_ok, &j.jp);
         if (rc <= 0) return rc;   // launched (0) or failed (< 0); +1: this batch does not fit the lean kernel
     }
-    if (s.jf.mode != 0 && c.jfast && !p->force_generic) {
+    if (s.jf.mode != 0 && c.jfast && !p->agg.env.force_generic) {
         const Compiled& f = *c.jfast;
         const int64_t chunk = 16 << 20;   // the gathered chunk is re-read immediately: keep it L2-sized
         for (int64_t off = 0; off < nrows; off += chunk) {
@@ -575,13 +576,13 @@ static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nro
                 gc.src[gc.n] = s.store.cols[m].vals; gc.dst[gc.n] = dst; gc.elem[gc.n] = storage_bytes(all[m].stype); gc.n++;
                 fc[i] = all[m]; fc[i].values = dst; fc[i].validity = nullptr;
             }
-            CK(p, cudaMemsetAsync(p->d_cursor + 1, 0, 4, p->stream));
+            CK(p, cudaMemsetAsync(j.cursor, 0, 4, p->stream));
             k_join_gather<<<grid_for((n + 3) / 4, p->sm_count, 8), 256, 0, p->stream>>>(col_at(all[(size_t)c.probe_key_col], off), c.cols[(size_t)c.probe_key_col].prim,
-                                                                                       c.join_key_prim, n, s.jf, gc, p->d_cursor + 1);
+                                                                                       c.join_key_prim, n, s.jf, gc, j.cursor);
             CK(p, cudaGetLastError());
             p->stats.kernel_launches++;
             uint32_t miss = 0;
-            if ((rc = read_u32(p, p->d_cursor + 1, &miss))) return rc;
+            if ((rc = read_u32(p, j.cursor, &miss))) return rc;
             if (miss) {   // some probe row has no partner (or a NULL key): this chunk takes the general probe
                 std::vector<DevCol> sl(all);
                 for (size_t i = 0; i < sl.size(); i++) if (c.col_side[i] == 0) sl[i] = col_at(all[i], off);
@@ -645,7 +646,6 @@ static int join_rows_emit(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t
         if ((rc = store_pack(p, p->post, k, found, 16, nullptr, &dc[k]))) return rc;
     }
     p->stats.kernel_launches += 2 * (int64_t)nc;
-    p->rows_passed_host += found;
     if ((rc = sort_push(p->post_sort, dc.data(), (int64_t)found, &p->stats))) return rc;
     CK(p, cudaStreamSynchronize(p->stream));   // the gather buffers are reused by the next batch
     return BKGPU_OK;
@@ -772,12 +772,12 @@ static int star_probe_batch(bkgpu_plan* p, const DevCol* fact_cols, int64_t nrow
             L.fk = col_at(all[(size_t)sd.fk_col], off); L.from_prim = c.cols[(size_t)sd.fk_col].prim; L.cast_prim = sd.cast_prim; L.slot = 1 + d; L.jf = j.side[d].jf;
         }
         if ((rc = star_tuples(p, 0, (uint64_t)n, W))) return rc;
-        CK(p, cudaMemsetAsync(p->d_cursor + 1, 0, 4, p->stream));
-        k_star_probe<<<grid_for((n + 3) / 4, p->sm_count, 8), 256, 0, p->stream>>>(sp, j.tuples[0], p->d_cursor + 1);   // (four rows per thread)
+        CK(p, cudaMemsetAsync(j.cursor, 0, 4, p->stream));
+        k_star_probe<<<grid_for((n + 3) / 4, p->sm_count, 8), 256, 0, p->stream>>>(sp, j.tuples[0], j.cursor);   // (four rows per thread)
         CK(p, cudaGetLastError());
         p->stats.kernel_launches++;
         uint32_t found = 0;
-        if ((rc = read_u32(p, p->d_cursor + 1, &found))) return rc;
+        if ((rc = read_u32(p, j.cursor, &found))) return rc;
         int cur = 0;
         for (int d = 0; d < D && found; d++) {   // dimensions with duplicate keys: one expansion pass each
             const JoinSide& s = j.side[d];
@@ -785,13 +785,13 @@ static int star_probe_batch(bkgpu_plan* p, const DevCol* fact_cols, int64_t nrow
             const StarDim& sd = c.dims[(size_t)d];
             const DevCol fk = col_at(all[(size_t)sd.fk_col], off);
             uint32_t got = 0;
-            rc = run_counted(p, j.star_expand_cap > 0 ? (uint64_t)j.star_expand_cap : std::max<uint64_t>(2 * (uint64_t)found, 4096), p->d_cursor + 1, &got,
+            rc = run_counted(p, j.star_expand_cap > 0 ? (uint64_t)j.star_expand_cap : std::max<uint64_t>(2 * (uint64_t)found, 4096), j.cursor, &got,
                              [&](uint64_t cap) -> int {
                 int r;
                 if ((r = star_tuples(p, 1 - cur, cap, W))) return r;
-                CK(p, cudaMemsetAsync(p->d_cursor + 1, 0, 4, p->stream));
+                CK(p, cudaMemsetAsync(j.cursor, 0, 4, p->stream));
                 k_star_expand<<<grid_for(found, p->sm_count, 16), 256, 0, p->stream>>>(fk, c.cols[(size_t)sd.fk_col].prim, sd.cast_prim, s.jt_keys, s.jt_rows, s.jt_mask,
-                                                                                       j.tuples[cur], found, W, 1 + d, j.tuples[1 - cur], (uint32_t)cap, p->d_cursor + 1);
+                                                                                       j.tuples[cur], found, W, 1 + d, j.tuples[1 - cur], (uint32_t)cap, j.cursor);
                 CK(p, cudaGetLastError());
                 p->stats.kernel_launches++;
                 return BKGPU_OK;

@@ -149,8 +149,8 @@ __global__ void __launch_bounds__(256) k_bitsets(const uint64_t* u, int64_t nc, 
 
 // scratch buffer `slot` of the plan's rb state, at least `bytes` long
 static int rb_buf(bkgpu_plan* p, int slot, size_t bytes, void** out) {
-    int rc = ensure_buf(p, &p->rb.scratch[slot], &p->rb.scratch_cap[slot], std::max<size_t>(bytes, 8));
-    *out = p->rb.scratch[slot];
+    int rc = ensure_buf(p, &p->agg.rb.scratch[slot], &p->agg.rb.scratch_cap[slot], std::max<size_t>(bytes, 8));
+    *out = p->agg.rb.scratch[slot];
     return rc;
 }
 template <typename T> static T d2h(bkgpu_plan* p, const T* src, int* rc) {
@@ -161,36 +161,36 @@ template <typename T> static T d2h(bkgpu_plan* p, const T* src, int* rc) {
     return v;
 }
 
-// sort keys [0, n) of the pair buffer: p->rb.keys then points at the sorted keys (the sort's second buffer is p->rb.alt)
+// sort keys [0, n) of the pair buffer: p->agg.rb.keys then points at the sorted keys (the sort's second buffer is p->agg.rb.alt)
 static int rb_sort(bkgpu_plan* p, int64_t n) {
-    uint64_t* keys[2] = {p->rb.keys, p->rb.alt};
-    const int r = radix_sort(p, keys, nullptr, 0, n, p->rb.sort, &p->stats, nullptr);
+    uint64_t* keys[2] = {p->agg.rb.keys, p->agg.rb.alt};
+    const int r = radix_sort(p, keys, nullptr, 0, n, p->agg.rb.sort, &p->stats, nullptr);
     if (r < 0) return r;
-    if (r) std::swap(p->rb.keys, p->rb.alt);
+    if (r) std::swap(p->agg.rb.keys, p->agg.rb.alt);
     return BKGPU_OK;
 }
 
 int rb_compact(bkgpu_plan* p, uint64_t* n_out) {
     int rc = BKGPU_OK;
-    const uint64_t n = d2h(p, p->rb.ctr, &rc);
+    const uint64_t n = d2h(p, p->agg.rb.ctr, &rc);
     if (rc) return rc;
-    if (n > p->rb.cap)
-        return p->fail(BKGPU_ETOOBIG, "rb_build_agg: more than %llu (group, value) pairs in one batch: raise rb_pair_capacity", (unsigned long long)p->rb.cap);
+    if (n > p->agg.rb.cap)
+        return p->fail(BKGPU_ETOOBIG, "rb_build_agg: more than %llu (group, value) pairs in one batch: raise rb_pair_capacity", (unsigned long long)p->agg.rb.cap);
     if ((rc = rb_sort(p, (int64_t)n))) return rc;
     uint32_t *flags, *sums;
     // (the flags reuse the sort's look-back status buffer: the sort is done with it)
-    if ((rc = ensure_buf(p, &p->rb.sort.status, &p->rb.sort.status_cap, (n + 1) * 4))) return rc;
-    flags = (uint32_t*)p->rb.sort.status;
+    if ((rc = ensure_buf(p, &p->agg.rb.sort.status, &p->agg.rb.sort.status_cap, (n + 1) * 4))) return rc;
+    flags = (uint32_t*)p->agg.rb.sort.status;
     if ((rc = rb_buf(p, 0, (size_t)scan_scratch((int64_t)n + 1) * 4, (void**)&sums))) return rc;
     const int g = grid_for((int64_t)n + 1, p->sm_count, 16);
-    k_uniq_flags<<<g, 256, 0, p->stream>>>(p->rb.keys, (int64_t)n, flags);
+    k_uniq_flags<<<g, 256, 0, p->stream>>>(p->agg.rb.keys, (int64_t)n, flags);
     CK(p, cudaGetLastError());
     CK(p, scan_excl(flags, (int64_t)n + 1, sums, p->sm_count, p->stream));
-    k_uniq_write<<<g, 256, 0, p->stream>>>(p->rb.keys, (int64_t)n, flags, p->rb.alt, p->rb.ctr);
+    k_uniq_write<<<g, 256, 0, p->stream>>>(p->agg.rb.keys, (int64_t)n, flags, p->agg.rb.alt, p->agg.rb.ctr);
     CK(p, cudaGetLastError());
-    std::swap(p->rb.keys, p->rb.alt);
+    std::swap(p->agg.rb.keys, p->agg.rb.alt);
     p->stats.kernel_launches += 4;
-    *n_out = d2h(p, p->rb.ctr, &rc);
+    *n_out = d2h(p, p->agg.rb.ctr, &rc);
     return rc;
 }
 
@@ -201,10 +201,10 @@ int rb_build(bkgpu_plan* p) {
     const int64_t m = (int64_t)m64;
     const cudaStream_t s = p->stream;
     const int sm = p->sm_count;
-    p->rb.bid.clear(); p->rb.off.assign(1, 0);
+    p->agg.rb.bid.clear(); p->agg.rb.off.assign(1, 0);
     if (m == 0) return BKGPU_OK;
-    const uint64_t* u = p->rb.keys;
-    uint64_t* e = p->rb.alt;   // (cap + 1 words: room for the scan's closing entry)
+    const uint64_t* u = p->agg.rb.keys;
+    uint64_t* e = p->agg.rb.alt;   // (cap + 1 words: room for the scan's closing entry)
     uint64_t* sums64;
     if ((rc = rb_buf(p, 0, (size_t)scan_scratch(m + 1) * 8, (void**)&sums64))) return rc;
     k_seg_flags<<<grid_for(m + 1, sm, 16), 256, 0, s>>>(u, m, e);
@@ -245,16 +245,16 @@ int rb_build(bkgpu_plan* p) {
     CK(p, cudaGetLastError());
     p->stats.kernel_launches += 16;
     // the finished bytes and the directory back to the host: bitmap ids ascend (the keys were sorted), offsets close with the total
-    p->rb.bid.resize(nb); p->rb.off.resize((size_t)nb + 1);
-    if (p->rb.bytes_cap < total) {
-        if (p->rb.bytes) cudaFreeHost(p->rb.bytes);
-        p->rb.bytes = nullptr; p->rb.bytes_cap = 0;
-        CK(p, cudaHostAlloc((void**)&p->rb.bytes, total + total / 4, cudaHostAllocDefault));
-        p->rb.bytes_cap = total + total / 4;
+    p->agg.rb.bid.resize(nb); p->agg.rb.off.resize((size_t)nb + 1);
+    if (p->agg.rb.bytes_cap < total) {
+        if (p->agg.rb.bytes) cudaFreeHost(p->agg.rb.bytes);
+        p->agg.rb.bytes = nullptr; p->agg.rb.bytes_cap = 0;
+        CK(p, cudaHostAlloc((void**)&p->agg.rb.bytes, total + total / 4, cudaHostAllocDefault));
+        p->agg.rb.bytes_cap = total + total / 4;
     }
-    CK(p, cudaMemcpyAsync(p->rb.bid.data(), bid, (size_t)nb * 4, cudaMemcpyDeviceToHost, s));
-    CK(p, cudaMemcpyAsync(p->rb.off.data(), bo, ((size_t)nb + 1) * 8, cudaMemcpyDeviceToHost, s));
-    CK(p, cudaMemcpyAsync(p->rb.bytes, out, total, cudaMemcpyDeviceToHost, s));
+    CK(p, cudaMemcpyAsync(p->agg.rb.bid.data(), bid, (size_t)nb * 4, cudaMemcpyDeviceToHost, s));
+    CK(p, cudaMemcpyAsync(p->agg.rb.off.data(), bo, ((size_t)nb + 1) * 8, cudaMemcpyDeviceToHost, s));
+    CK(p, cudaMemcpyAsync(p->agg.rb.bytes, out, total, cudaMemcpyDeviceToHost, s));
     CK(p, cudaStreamSynchronize(s));
     p->stats.d2h_bytes += (int64_t)(total + (size_t)nb * 12 + 8);
     return BKGPU_OK;

@@ -30,7 +30,7 @@ struct RbState {
 // BKGPU_ETOOBIG (naming rb_pair_capacity) when keys were already lost to a full buffer
 int rb_compact(bkgpu_plan* p, uint64_t* n_out);
 // after the request's last launch: compacts, builds and serializes every (group, rb_build_agg) bitmap on the device and copies the
-// bytes and their directory into p->rb
+// bytes and their directory into p->agg.rb
 int rb_build(bkgpu_plan* p);
 
 }  // namespace bk

@@ -289,6 +289,21 @@ def c2_smem_log2_11():   # 1,000 groups through the shared-table capacities of t
     return c2({"smem_capacity_log2": 11})
 
 
+@case(["0_1"])
+def c2_groups_past_the_fused_buffer():   # 200,000 groups: more than the fused extraction holds, so k_extract reads them back (the first run regrows its buffers)
+    return c2({}, n_groups=200_000)
+
+
+@case(["0_1"])
+def hll_grouped():   # hll_add_agg per group: the arena's counters and blocks come back after the extraction
+    from tests import hll_cases
+    rng = np.random.default_rng(21)
+    n = 1_000_000
+    cols = [make_column(0, 1, T.INT32, rng.integers(0, 300, n).astype(np.int32)), make_column(0, 2, T.INT64, rng.integers(0, 50_000, n), rng.random(n) > 0.1),
+            make_column(0, 3, T.DOUBLE, rng.normal(size=n))]
+    return hll_cases.scan_plan(T.INT64, extra=True), [chunks(cols, [0, 400_000, n])] * 2, {}
+
+
 @case([])
 def scalar_sum():
     from tests.test_agg_select import scalar_sum_plan
@@ -376,8 +391,8 @@ def execute_runs(pl, runs, options):
                 rc, eos = node.get_next(st, rb)
                 if rc < 0:
                     raise BkgpuError(rc, st.error_msg)
-                for c in rb.columns:   # (a BITMAP arrives as its serialized bytes, an AVG intermediate {double sum; int64 count} as 16 bytes)
-                    unpack = (lambda v: v.hex()) if c.prim_type == T.BITMAP else (lambda v: list(struct.unpack("<dq", v)))
+                for c in rb.columns:   # (a BITMAP or an HLL sketch arrives as its serialized bytes, an AVG intermediate {double sum; int64 count} as 16 bytes)
+                    unpack = (lambda v: v.hex()) if c.prim_type in (T.BITMAP, T.HLL) else (lambda v: list(struct.unpack("<dq", v)))
                     cols.setdefault(c.name, []).extend([unpack(v) if isinstance(v, bytes) else v for v in c.to_list()])
             s = node.stats()
             out.append({"kernel_launches": s.kernel_launches, "main_kernel_name": s.main_kernel_name.decode(), "h2d_bytes": s.h2d_bytes,
