@@ -723,33 +723,24 @@ static int agg_collective(bkgpu_plan* p, bool* rows_mode) {
 // [LIMIT ->] [SORT ->] [HAVING ->] above the aggregate: the extracted rows (still on the device) become typed columns and run through
 // the post fragment's sort / filter kernels; only the final rows travel to the host
 static int agg_post(bkgpu_plan* p, uint32_t n_out, uint32_t out_cap) {
-    const Compiled& pc = *p->c.post;
-    const size_t nc = pc.cols.size();
-    int rc;
-    for (size_t c = 0; c < nc; c++)
-        if ((rc = store_reserve(p, p->post, c, std::max<int64_t>(n_out, 1), std::max<int64_t>(n_out, 2048), true))) return rc;
-    PostCols pcs; memset(&pcs, 0, sizeof pcs);
-    pcs.n = (int)nc;
-    int img = 0;
-    for (size_t c = 0; c < nc; c++) {   // (post columns = the aggregate's output columns, in order: plan.cpp::lower_post)
-        pcs.img[c] = img; pcs.stype[c] = prim_storage(pc.cols[c].prim); pcs.values[c] = p->post.cols[c].vals; pcs.null_bytes[c] = p->post.cols[c].nulls;
-        img += p->c.out_cols[c].kind == 1 ? 2 : 1;
-    }
-    if (n_out) {
+    const size_t nc = p->c.post->cols.size();
+    sort_reset(p->post);
+    bkgpu_stats scratch{};   // (the post fragment's kernels are not the request's "main kernel")
+    int rc = sort_feed(p->post, n_out, std::max<int64_t>(n_out, 2048), 16, &scratch, [&](RowStore& in) {
+        PostCols pcs; memset(&pcs, 0, sizeof pcs);
+        pcs.n = (int)nc;
+        int img = 0;
+        for (size_t c = 0; c < nc; c++) {   // (post columns = the aggregate's output columns, in order: plan.cpp::lower_post)
+            pcs.img[c] = img; pcs.stype[c] = prim_storage(in.cols[c].prim); pcs.values[c] = in.cols[c].vals; pcs.null_bytes[c] = in.cols[c].nulls;
+            img += p->c.out_cols[c].kind == 1 ? 2 : 1;
+        }
         k_images_to_columns<<<grid_for(n_out, p->sm_count, 8), 256, 0, p->stream>>>(p->agg.d_outv, p->agg.d_outn, out_cap, n_out, pcs);
         CK(p, cudaGetLastError());
-    }
-    std::vector<DevCol> dc(std::max<size_t>(nc, 1));
-    for (size_t c = 0; c < nc; c++)
-        if ((rc = store_pack(p, p->post, c, n_out, 16, nullptr, &dc[c]))) return rc;
-    p->stats.kernel_launches += 1 + (int64_t)nc;
-    sort_reset(p->post_sort);
-    bkgpu_stats scratch{};   // (the post fragment's kernels are not the request's "main kernel")
-    if (n_out && (rc = sort_push(p->post_sort, dc.data(), n_out, &scratch))) return rc;
-    std::vector<SortOutCol> cols; int64_t rows = 0;
-    if ((rc = sort_finish(p->post_sort, nullptr, 1, &scratch, cols, &rows))) return rc;
+        return BKGPU_OK;
+    });
+    p->stats.kernel_launches += 1 + (int64_t)nc;   // (the extraction into columns and the packs, counted with no rows too)
+    if (rc || (rc = sort_finish(p->post, nullptr, 1, &scratch, p->c.out_cols.data()))) return rc;
     p->stats.kernel_launches += scratch.kernel_launches;
-    set_result(p, cols, rows, p->c.out_cols.data());
     return BKGPU_OK;
 }
 

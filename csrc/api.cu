@@ -237,12 +237,12 @@ extern "C" int bkgpu_open(bkgpu_plan* p) {
         return p->fail(BKGPU_EUNSUPPORTED, "hll_add_agg with the repartition merge is outside the GPU path: its sketches travel only with the all-gather of group rows");
     if (p->c.n_rb && p->nccl_comm)
         return p->fail(BKGPU_EUNSUPPORTED, "rb_build_agg with a communicator is outside the GPU path: bitmaps do not travel with the fixed-width partial rows");
-    int rc = upload_in_sets(p);   // (before sort_open: it copies the programs)
+    int rc = upload_in_sets(p);
     if (rc) return rc;
     if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) rc = agg_open(p);
     if (!rc && (p->c.kind == PK_SORT || p->c.kind == PK_FILTER || p->c.kind == PK_WINDOW))   // (a window retains its rows like a full sort)
         rc = sort_open(p, p->c, p->region_base, &p->sort);
-    if (!rc && p->c.post) { rc = sort_open(p, *p->c.post, 0, &p->post_sort); store_init(p->post, p->c.post->cols); }
+    if (!rc && p->c.post) rc = sort_open(p, *p->c.post, 0, &p->post);
     if (rc) return rc;
     p->state = S_OPEN;
     return BKGPU_OK;
@@ -458,17 +458,6 @@ int feed(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* col
 
 static int sort_batch(bkgpu_plan* p, const DevCol* cols, int64_t nrows, int64_t, bool) { return sort_push(p->sort, cols, nrows, &p->stats); }
 
-void set_result(bkgpu_plan* p, std::vector<SortOutCol>& cols, int64_t rows, const OutCol* desc) {
-    p->result.clear();
-    for (size_t k = 0; k < cols.size(); k++) {
-        SortOutCol& sc = cols[k];
-        HostCol hc; hc.desc = desc ? desc[k] : OutCol{sc.tuple_id, sc.slot_id, sc.prim, 0}; hc.elem = sc.elem;
-        hc.values = std::move(sc.values); hc.validity = std::move(sc.validity);
-        p->result.push_back(std::move(hc));
-    }
-    p->result_rows = rows; p->result_pos = 0;
-}
-
 static int bkgpu_push_impl(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device);
 extern "C" int bkgpu_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device) {
     const double t0 = HostClock::now();
@@ -525,23 +514,15 @@ static int bkgpu_finish_impl(bkgpu_plan* p) {
             if (p->c.kind == PK_JOIN_AGG && (rc = join_tail(p))) break;
             rc = agg_finish(p);
             break;
-        case PK_JOIN: {   // the outer join's preserved rows, then the sink fragment's result
-            std::vector<SortOutCol> cols; int64_t rows = 0;
-            if ((rc = join_tail(p)) || (rc = sort_finish(p->post_sort, nullptr, 1, &p->stats, cols, &rows))) break;
-            set_result(p, cols, rows, p->c.out_cols.data());
+        case PK_JOIN:   // the outer join's preserved rows, then the sink fragment's result
+            if ((rc = join_tail(p)) || (rc = sort_finish(p->post, nullptr, 1, &p->stats, p->c.out_cols.data()))) break;
             p->stats.rows_filtered = 0;
-        } break;
-        case PK_SORT: case PK_FILTER: {
-            std::vector<SortOutCol> cols; int64_t rows = 0;
-            if ((rc = sort_finish(p->sort, p->nccl_comm, p->nranks, &p->stats, cols, &rows))) break;
-            set_result(p, cols, rows, nullptr);
-        } break;
-        case PK_WINDOW: {   // the retained rows through the window stages (window.cu), then the query's ORDER BY when there is one
+            break;
+        case PK_SORT: case PK_FILTER: rc = sort_finish(p->sort, p->nccl_comm, p->nranks, &p->stats, nullptr); break;
+        case PK_WINDOW:   // the retained rows through the window stages (window.cu), then the query's ORDER BY when there is one
             if (p->nccl_comm && p->nranks > 1) { rc = p->fail(BKGPU_EUNSUPPORTED, "a window fragment runs on one GPU: multi-GPU merge is implemented for ORDER BY ... LIMIT (top-k) and aggregates"); break; }
-            std::vector<SortOutCol> cols; int64_t rows = 0;
-            if ((rc = window_finish(p, cols, &rows))) break;
-            set_result(p, cols, rows, nullptr);
-        } break;
+            rc = window_finish(p);
+            break;
         default: rc = p->fail(BKGPU_EUNSUPPORTED, "plan kind %d cannot finish", p->c.kind);
     }
     // (a finished aggregate without a post fragment has already waited for everything it queued: agg_wait)
@@ -614,7 +595,7 @@ static int bkgpu_reset_impl(bkgpu_plan* p) {
     }
     join_reset(p);
     if (p->sort) sort_reset(p->sort);
-    if (p->c.kind == PK_JOIN && p->post_sort) sort_reset(p->post_sort);
+    if (p->c.kind == PK_JOIN && p->post) sort_reset(p->post);
     p->result.clear(); p->result_rows = 0; p->result_pos = 0;
     bkgpu_stats z{}; z.kernel_launches = p->stats.kernel_launches; p->stats = z;
     p->state = S_OPEN;
@@ -635,7 +616,7 @@ extern "C" void bkgpu_close(bkgpu_plan* p) {
     if (p->copy_stream) cudaStreamSynchronize(p->copy_stream);
     resolve_timers(p);
     if (p->sort) sort_close(p->sort);
-    if (p->post_sort) sort_close(p->post_sort);
+    if (p->post) sort_close(p->post);
     for (cudaEvent_t e : p->event_pool) cudaEventDestroy(e);
     for (auto& q : p->dev_allocs) if (!dev_cache().put(p->device, q.second, q.first)) cudaFree(q.first);   // (both streams were drained above)
     for (int i = 0; i < 2; i++) { if (p->stage_free[i]) cudaEventDestroy(p->stage_free[i]); if (p->stage_ready[i]) cudaEventDestroy(p->stage_ready[i]); }
@@ -750,14 +731,7 @@ extern "C" int bkgpu_partial_merge(bkgpu_plan* p, const void* dev_src, size_t by
     if (rc) return rc;
     if (bytes_per_rank != need) return p->fail(BKGPU_EINVAL, "bytes_per_rank %zu != partial capacity %zu", bytes_per_rank, need);
     CK(p, cudaSetDevice(p->device));
-    if (p->c.kind == PK_SORT) {
-        std::vector<SortOutCol> cols; int64_t rows = 0;
-        if ((rc = sort_partial_merge(p->sort, dev_src, nranks, cols, &rows))) return rc;
-        set_result(p, cols, rows, nullptr);
-        p->stats.rows_returned = rows; p->state = S_FINISHED;
-        return BKGPU_OK;
-    }
-    if ((rc = agg_partial_merge(p, dev_src, nranks))) return rc;
+    if ((rc = p->c.kind == PK_SORT ? sort_partial_merge(p->sort, dev_src, nranks) : agg_partial_merge(p, dev_src, nranks))) return rc;
     p->stats.rows_returned = p->result_rows; p->state = S_FINISHED;
     return BKGPU_OK;
 }

@@ -1,6 +1,7 @@
 // api_state.h — the plan object behind the C ABI (bkgpu_plan), the state of its hash join (JoinState, join.cu) and of its aggregate
-// (AggState, agg.cu), and the host helpers api.cu, agg.cu and join.cu share.  bkgpu_plan itself holds what more than one stage uses: the
-// compiled plan, the device, streams and lifecycle state, the staging buffers, the result, the stats and the allocator.
+// (AggState, agg.cu), and the host helpers the stages share.  ORDER BY / filter / window retention and the post fragment each keep a
+// SortState (sort.cu).  bkgpu_plan itself holds what more than one stage uses: the compiled plan, the device, streams and lifecycle
+// state, the staging buffers, the result, the stats and the allocator.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdarg.h>
@@ -145,9 +146,8 @@ struct bkgpu_plan {
     cudaEvent_t stage_free[2] = {nullptr, nullptr}, stage_ready[2] = {nullptr, nullptr};
     std::vector<uint8_t*> bounce[2]; size_t bounce_rows = 0; cudaEvent_t bounce_done[2] = {nullptr, nullptr}; bool bounce_busy[2] = {false, false};
     // the stages
-    SortState* post_sort = nullptr;   // the post fragment above the aggregate (Compiled::post)
-    RowStore post;                    // the post fragment's input (Compiled::post's columns)
     SortState* sort = nullptr;        // ORDER BY / filter / window retention (PK_SORT, PK_FILTER, PK_WINDOW)
+    SortState* post = nullptr;        // the post fragment (Compiled::post) above an aggregate, a window or a join that returns rows
     JoinState join;                   // hash join (K4): PK_JOIN_AGG, PK_JOIN, PK_STAR_AGG
     AggState agg;                     // the aggregate: PK_AGG, PK_JOIN_AGG, PK_STAR_AGG
     // results
@@ -198,13 +198,19 @@ struct DevScope {
         for (auto it = bufs.begin(); it != bufs.end(); ++it) if (*it == b) { bufs.erase(it); dev_free(p, b); return; }
     }
 };
+// a stage timer's two events, destroyed on every way out of the scope that holds them
+struct StageTimer {
+    cudaEvent_t a = nullptr, b = nullptr;
+    StageTimer() { cudaEventCreate(&a); cudaEventCreate(&b); }
+    StageTimer(const StageTimer&) = delete;
+    StageTimer& operator=(const StageTimer&) = delete;
+    ~StageTimer() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); }
+};
 // the plan's columns `want` resolved against one pushed batch
 int bind_columns(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* cols, int ncols, int64_t nrows, std::vector<const bkgpu_column*>& bound);
 // a batch as device columns (host columns chunk by chunk through the staging buffers), handed to `fn`
 typedef int (*BatchFn)(bkgpu_plan*, const DevCol*, int64_t nrows, int64_t row_base, bool vec_ok);
 int feed(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device, BatchFn fn);
-// the plan's result from a sort fragment's columns; `desc`: their output column descriptions (nullptr = the sort's own)
-void set_result(bkgpu_plan* p, std::vector<SortOutCol>& cols, int64_t rows, const OutCol* desc);
 
 // rows [off, ...) of a device column
 inline DevCol col_at(const DevCol& c, int64_t off) {

@@ -626,7 +626,7 @@ static int join_pairs(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t n_p
     });
 }
 
-// ---- a JOIN that returns rows (PK_JOIN): pairs -> gather -> the sink fragment (p->post_sort) ----
+// ---- a JOIN that returns rows (PK_JOIN): pairs -> gather -> the sink fragment (p->post) ----
 static int join_rows_emit(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t n_probe, bool tail) {
     const Compiled& c = p->c;
     JoinState& j = p->join;
@@ -634,19 +634,17 @@ static int join_rows_emit(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t
     uint32_t found = 0;
     rc = join_pairs(p, all, n_probe, tail, &found);
     if (rc || !found) return rc;
-    const Compiled& pc = *c.post;
-    const size_t nc = pc.cols.size();
-    std::vector<DevCol> dc(std::max<size_t>(nc, 1));
-    for (size_t k = 0; k < nc; k++) {   // sink column k = output column k = device column k of the join (plan.cpp::lower_join_rows)
-        const RowStore::Col& d = p->post.cols[k];
-        if ((rc = store_reserve(p, p->post, k, found, std::max<int64_t>((int64_t)found + found / 4, 1 << 16), true))) return rc;
-        k_join_rows_gather<<<grid_for(found, p->sm_count, 16), 256, 0, p->stream>>>(all[k], j.pairs, 2, c.col_side[k] == 1 ? 1 : 0, found, storage_bytes(prim_storage(d.prim)),
-                                                                                    d.vals, d.nulls);
-        CK(p, cudaGetLastError());
-        if ((rc = store_pack(p, p->post, k, found, 16, nullptr, &dc[k]))) return rc;
-    }
-    p->stats.kernel_launches += 2 * (int64_t)nc;
-    if ((rc = sort_push(p->post_sort, dc.data(), (int64_t)found, &p->stats))) return rc;
+    rc = sort_feed(p->post, found, std::max<int64_t>((int64_t)found + found / 4, 1 << 16), 16, &p->stats, [&](RowStore& in) {
+        for (size_t k = 0; k < in.cols.size(); k++) {   // sink column k = output column k = device column k of the join (plan.cpp::lower_join_rows)
+            const RowStore::Col& d = in.cols[k];
+            k_join_rows_gather<<<grid_for(found, p->sm_count, 16), 256, 0, p->stream>>>(all[k], j.pairs, 2, c.col_side[k] == 1 ? 1 : 0, found,
+                                                                                        storage_bytes(prim_storage(d.prim)), d.vals, d.nulls);
+            CK(p, cudaGetLastError());
+        }
+        return BKGPU_OK;
+    });
+    if (rc) return rc;
+    p->stats.kernel_launches += 2 * (int64_t)c.post->cols.size();
     CK(p, cudaStreamSynchronize(p->stream));   // the gather buffers are reused by the next batch
     return BKGPU_OK;
 }

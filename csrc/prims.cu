@@ -149,13 +149,12 @@ int store_gather(bkgpu_plan* p, const RowStore::Col& src, const uint32_t* perm, 
     return BKGPU_OK;
 }
 
-int store_copy_out(bkgpu_plan* p, const RowStore& s, const std::vector<ColRef>& desc, const uint32_t* perm, int64_t n, int64_t skip,
-                   std::vector<SortOutCol>& out) {
+int store_copy_out(bkgpu_plan* p, const RowStore& s, const std::vector<ColRef>& desc, const uint32_t* perm, int64_t n, int64_t skip) {
     const cudaStream_t st = p->stream;
-    out.clear();
+    p->result.clear();
     for (size_t c = 0; c < desc.size(); c++) {
         const ColRef& cr = desc[c];
-        SortOutCol oc; oc.tuple_id = cr.tuple_id; oc.slot_id = cr.slot_id; oc.prim = cr.prim; oc.elem = elem_bytes_of(cr.prim);
+        HostCol oc; oc.desc = OutCol{cr.tuple_id, cr.slot_id, cr.prim, 0}; oc.elem = elem_bytes_of(cr.prim);
         oc.values.assign((size_t)std::max<int64_t>(n, 1) * oc.elem, 0);
         std::vector<uint8_t> nb((size_t)std::max<int64_t>(n, 1));
         const RowStore::Col& sc = s.cols[c];
@@ -179,8 +178,9 @@ int store_copy_out(bkgpu_plan* p, const RowStore& s, const std::vector<ColRef>& 
             oc.validity.assign((size_t)(n + 7) / 8 + 1, 0xFF);
             for (int64_t i = 0; i < n; i++) if (nb[(size_t)i]) oc.validity[(size_t)i >> 3] &= (uint8_t)~(1u << (i & 7));
         }
-        out.push_back(std::move(oc));
+        p->result.push_back(std::move(oc));
     }
+    p->result_rows = n; p->result_pos = 0;
     return BKGPU_OK;
 }
 

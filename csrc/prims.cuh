@@ -10,8 +10,6 @@
 
 namespace bk {
 
-struct SortOutCol;
-
 // CTAs of 256 threads for a grid-stride loop over n items: at least one, at most `per_sm` per SM
 int grid_for(int64_t n, int sm, int per_sm);
 
@@ -62,10 +60,9 @@ int store_pack(bkgpu_plan* p, const RowStore& s, size_t i, int64_t n, int per_sm
 DevCol store_col(const RowStore& s, size_t i);
 // dst_vals / dst_nulls [0, n) = the values / null bytes of rows perm[0, n) of column `src`
 int store_gather(bkgpu_plan* p, const RowStore::Col& src, const uint32_t* perm, int64_t n, uint8_t* dst_vals, uint8_t* dst_nulls);
-// rows [skip, skip + n) of the columns of `s` (through the device permutation `perm` when not nullptr) to the host, column c described
-// by desc[c]
-int store_copy_out(bkgpu_plan* p, const RowStore& s, const std::vector<ColRef>& desc, const uint32_t* perm, int64_t n, int64_t skip,
-                   std::vector<SortOutCol>& out);
+// rows [skip, skip + n) of the columns of `s` (through the device permutation `perm` when not nullptr) to the host as the plan's result
+// (p->result, result_rows), column c described by desc[c] with kind 0
+int store_copy_out(bkgpu_plan* p, const RowStore& s, const std::vector<ColRef>& desc, const uint32_t* perm, int64_t n, int64_t skip);
 
 // exclusive prefix sum of d[0, n) in place, for uint32_t and uint64_t; `sums` holds scan_scratch(n) entries
 template <typename T> cudaError_t scan_excl(T* d, int64_t n, T* sums, int sm, cudaStream_t s);

@@ -426,7 +426,7 @@ struct Pool {               // the k best rows seen so far of one class (keys pr
 
 struct SortState {
     bkgpu_plan* p = nullptr;        // the owning plan: its allocator, stream and SM count
-    Compiled c;
+    const Compiled* c = nullptr;    // the fragment, owned by the plan
     int ncols = 0;
     int64_t k = -1;                 // rows to keep; -1 = all
     uint64_t row_base = 0, region_base = 0;
@@ -442,10 +442,7 @@ struct SortState {
     uint32_t* h_counts = nullptr;                         // pinned copy of d_counts
     // full sort / filter-only: retained rows
     RowStore ret;
-    std::vector<uint8_t*> key_img;  // per ORDER BY key: retained images (full sort)
-    uint8_t* ret_keep = nullptr;
-    int64_t total_seen = 0;
-    std::vector<SortOutCol> pending_out; int64_t pending_rows = 0;
+    RowStore in;                    // a post fragment's input, refilled by every sort_feed
 };
 
 namespace {
@@ -455,12 +452,12 @@ int elem_bytes_of(int prim) { return storage_bytes(prim_storage(prim)); }
 void fill_row_args(const SortState* s, const DevCol* cols, int64_t nrows, RowArgs& a) {
     memset(&a, 0, sizeof a);
     for (int i = 0; i < s->ncols; i++) a.cols[i] = cols[i];
-    a.n_cols = s->ncols; a.nrows = nrows; a.row_base = s->row_base; a.prog = s->c.prog;
-    a.key.pred_out = s->c.ap.pred_out;
-    if (!s->c.sort_keys.empty()) {
-        const SortKey& k = s->c.sort_keys[0];
+    a.n_cols = s->ncols; a.nrows = nrows; a.row_base = s->row_base; a.prog = s->c->prog;
+    a.key.pred_out = s->c->ap.pred_out;
+    if (!s->c->sort_keys.empty()) {
+        const SortKey& k = s->c->sort_keys[0];
         a.key.out_reg = k.out_reg; a.key.vclass = host_prim_class(k.prim); a.key.desc = k.asc ? 0 : 1;
-        a.key.direct = s->c.has_direct ? 1 : 0; a.key.col = s->c.has_direct ? s->c.direct_cols[0] : 0;
+        a.key.direct = s->c->has_direct ? 1 : 0; a.key.col = s->c->has_direct ? s->c->direct_cols[0] : 0;
     }
 }
 
@@ -562,7 +559,7 @@ int select_topk_class(SortState* s, const RowArgs& ra, int cls, bkgpu_stats* sta
 
 // rows that pass the predicate are appended, in input order, to the retained columns (filter-only and full sort)
 int retain_batch(SortState* s, const RowArgs& ra, bkgpu_stats* stats) {
-    const int64_t limit_left = (s->c.kind == PK_FILTER && s->c.limit >= 0) ? std::max<int64_t>(s->c.limit - s->ret.rows, 0) : INT64_MAX;
+    const int64_t limit_left = (s->c->kind == PK_FILTER && s->c->limit >= 0) ? std::max<int64_t>(s->c->limit - s->ret.rows, 0) : INT64_MAX;
     if (limit_left == 0) return 0;   // FilterNode stops after `limit` passing rows (filter_node.cpp:786-791)
     bkgpu_plan* p = s->p;
     const cudaStream_t st = p->stream;
@@ -650,11 +647,12 @@ int radix_sort_keys(SortState* s, RowArgs& ra, const std::vector<SortKey>& keys,
 // ------------------------------------------------------------------------------------------------------------
 int sort_open(bkgpu_plan* p, const Compiled& c, int64_t region_base, SortState** out) {
     SortState* s = new SortState();
-    s->p = p; s->c = c; s->ncols = (int)c.cols.size();
+    s->p = p; s->c = &c; s->ncols = (int)c.cols.size();
     s->row_base = s->region_base = (uint64_t)region_base;
     s->k = c.kind == PK_SORT ? c.limit : -1;
     s->topk = c.kind == PK_SORT && c.sort_keys.size() == 1 && s->k >= 0 && s->k <= 4096;
     store_init(s->ret, c.cols);
+    store_init(s->in, c.cols);
     int rc = 0;
     if (s->topk) {
         s->cand_cap = 1u << 22;   // 4M candidate pairs (64 MB per array pair)
@@ -684,7 +682,7 @@ int sort_open(bkgpu_plan* p, const Compiled& c, int64_t region_base, SortState**
 
 void sort_reset(SortState* s) {
     for (auto& P : s->pool) { P.n = 0; P.cur = 0; }
-    s->ret.rows = 0; s->total_seen = 0;
+    s->ret.rows = 0;
     s->row_base = s->region_base;
 }
 
@@ -695,22 +693,35 @@ int sort_push(SortState* s, const DevCol* cols, int64_t nrows, bkgpu_stats* stat
     int rc = 0;
     if (s->topk) {
         if (s->k == 0) { s->row_base += (uint64_t)nrows; return 0; }
-        cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-        cudaEventRecord(e0, stream);
+        StageTimer t;
+        cudaEventRecord(t.a, stream);
         rc = select_topk_class(s, ra, 1, stats);
         const bool need_nulls = ra.key.direct ? cols[ra.key.col].validity != nullptr : true;
         if (!rc && need_nulls) rc = select_topk_class(s, ra, 2, stats);
-        cudaEventRecord(e1, stream); cudaEventSynchronize(e1);
-        float ms = 0; cudaEventElapsedTime(&ms, e0, e1); cudaEventDestroy(e0); cudaEventDestroy(e1);
+        cudaEventRecord(t.b, stream); cudaEventSynchronize(t.b);
+        float ms = 0; cudaEventElapsedTime(&ms, t.a, t.b);
         stats->main_kernel_ms += ms; stats->main_kernel_launches += 1;
         stats->main_kernel_bytes += nrows * (ra.key.direct ? storage_bytes(cols[ra.key.col].stype) : 8);
         snprintf(stats->main_kernel_name, sizeof stats->main_kernel_name, "%s", s->used_vec ? "topk_select(k_collect_rows_vec)" : "topk_select(k_collect_rows)");
     } else {
         rc = retain_batch(s, ra, stats);
-        snprintf(stats->main_kernel_name, sizeof stats->main_kernel_name, "%s", s->c.kind == PK_FILTER ? "k_filter_write" : "radix_sort(k_rs_pass)");
+        snprintf(stats->main_kernel_name, sizeof stats->main_kernel_name, "%s", s->c->kind == PK_FILTER ? "k_filter_write" : "radix_sort(k_rs_pass)");
     }
-    s->row_base += (uint64_t)nrows; s->total_seen += nrows;
+    s->row_base += (uint64_t)nrows;
     return rc;
+}
+
+int sort_feed(SortState* s, int64_t n, int64_t cap, int per_sm, bkgpu_stats* stats, const std::function<int(RowStore& in)>& fill) {
+    if (n == 0) return BKGPU_OK;
+    bkgpu_plan* p = s->p;
+    int rc;
+    for (size_t k = 0; k < s->in.cols.size(); k++)
+        if ((rc = store_reserve(p, s->in, k, n, cap, true))) return rc;
+    if ((rc = fill(s->in))) return rc;
+    std::vector<DevCol> dc(std::max<size_t>(s->in.cols.size(), 1));
+    for (size_t k = 0; k < s->in.cols.size(); k++)
+        if ((rc = store_pack(p, s->in, k, n, per_sm, nullptr, &dc[k]))) return rc;
+    return sort_push(s, dc.data(), n, stats);
 }
 
 // layout of the exported partial (top-k): [u64 n][k keys][k idx][per column: k values (8-byte slots)][per column: k null bytes padded to 8]
@@ -733,7 +744,7 @@ static int topk_host_rows(SortState* s, HostRows& h) {
     const cudaStream_t st = p->stream;
     h.vals.assign((size_t)s->ncols, {}); h.nulls.assign((size_t)s->ncols, {});
     size_t row_bytes = 16;
-    for (int c = 0; c < s->ncols; c++) row_bytes += (size_t)elem_bytes_of(s->c.cols[(size_t)c].prim) + 1;
+    for (int c = 0; c < s->ncols; c++) row_bytes += (size_t)elem_bytes_of(s->c->cols[(size_t)c].prim) + 1;
     const size_t n_tot = (size_t)s->pool[0].n + (size_t)s->pool[1].n;
     const size_t need = n_tot * row_bytes + 64 * (size_t)(s->ncols + 2) * 2;
     if (s->h_stage_cap < need) {
@@ -753,7 +764,7 @@ static int topk_host_rows(SortState* s, HostRows& h) {
         CK(p, cudaMemcpyAsync(s->h_stage + seg[q].key, P.key[P.cur], n * 8, cudaMemcpyDeviceToHost, st));
         CK(p, cudaMemcpyAsync(s->h_stage + seg[q].idx, P.idx[P.cur], n * 8, cudaMemcpyDeviceToHost, st));
         for (int c = 0; c < s->ncols; c++) {
-            const size_t eb = (size_t)elem_bytes_of(s->c.cols[(size_t)c].prim);
+            const size_t eb = (size_t)elem_bytes_of(s->c->cols[(size_t)c].prim);
             seg[q].val.push_back(take(n * eb)); seg[q].nul.push_back(take(n));
             CK(p, cudaMemcpyAsync(s->h_stage + seg[q].val.back(), P.vals[P.cur][c], n * eb, cudaMemcpyDeviceToHost, st));
             CK(p, cudaMemcpyAsync(s->h_stage + seg[q].nul.back(), P.nulls[P.cur][c], n, cudaMemcpyDeviceToHost, st));
@@ -766,7 +777,7 @@ static int topk_host_rows(SortState* s, HostRows& h) {
         const uint64_t* key = (const uint64_t*)(s->h_stage + seg[q].key); const uint64_t* idx = (const uint64_t*)(s->h_stage + seg[q].idx);
         for (size_t i = 0; i < n; i++) { h.cls.push_back((uint8_t)(q + 1)); h.key.push_back(key[i]); h.idx.push_back(idx[i]); }
         for (int c = 0; c < s->ncols; c++) {
-            const size_t eb = (size_t)elem_bytes_of(s->c.cols[(size_t)c].prim);
+            const size_t eb = (size_t)elem_bytes_of(s->c->cols[(size_t)c].prim);
             const uint8_t* v = s->h_stage + seg[q].val[(size_t)c]; const uint8_t* nb = s->h_stage + seg[q].nul[(size_t)c];
             h.vals[(size_t)c].insert(h.vals[(size_t)c].end(), v, v + n * eb);
             h.nulls[(size_t)c].insert(h.nulls[(size_t)c].end(), nb, nb + n);
@@ -774,8 +785,9 @@ static int topk_host_rows(SortState* s, HostRows& h) {
     }
     return 0;
 }
-static void finish_host_rows(SortState* s, const HostRows& h, std::vector<SortOutCol>& out, int64_t* nrows) {
-    const bool null_first = s->c.sort_keys[0].null_first;
+// the first k rows of h in ORDER BY order, after OFFSET, into p->result
+static void finish_host_rows(SortState* s, const HostRows& h) {
+    const bool null_first = s->c->sort_keys[0].null_first;
     std::vector<uint32_t> order(h.key.size());
     for (size_t i = 0; i < order.size(); i++) order[i] = (uint32_t)i;
     std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
@@ -786,12 +798,13 @@ static void finish_host_rows(SortState* s, const HostRows& h, std::vector<SortOu
     });
     int64_t n = (int64_t)order.size();
     if (s->k >= 0 && n > s->k) n = s->k;
-    int64_t skip = std::min<int64_t>(s->c.offset, n);
+    int64_t skip = std::min<int64_t>(s->c->offset, n);
     n -= skip;
-    out.clear();
+    bkgpu_plan* p = s->p;
+    p->result.clear();
     for (int c = 0; c < s->ncols; c++) {
-        const ColRef& cr = s->c.cols[(size_t)c];
-        SortOutCol oc; oc.tuple_id = cr.tuple_id; oc.slot_id = cr.slot_id; oc.prim = cr.prim; oc.elem = elem_bytes_of(cr.prim);
+        const ColRef& cr = s->c->cols[(size_t)c];
+        HostCol oc; oc.desc = OutCol{cr.tuple_id, cr.slot_id, cr.prim, 0}; oc.elem = elem_bytes_of(cr.prim);
         oc.values.assign((size_t)std::max<int64_t>(n, 1) * oc.elem, 0);
         bool any = false;
         std::vector<uint8_t> valid((size_t)(n + 7) / 8 + 1, 0xFF);
@@ -801,9 +814,9 @@ static void finish_host_rows(SortState* s, const HostRows& h, std::vector<SortOu
             if (h.nulls[(size_t)c][src]) { any = true; valid[(size_t)i >> 3] &= (uint8_t)~(1u << (i & 7)); }
         }
         if (any) oc.validity = std::move(valid);
-        out.push_back(std::move(oc));
+        p->result.push_back(std::move(oc));
     }
-    *nrows = n;
+    p->result_rows = n; p->result_pos = 0;
 }
 
 static void pack_rows(SortState* s, const HostRows& h, std::vector<uint64_t>& buf) {
@@ -816,7 +829,7 @@ static void pack_rows(SortState* s, const HostRows& h, std::vector<uint64_t>& bu
     uint64_t* col0 = idx + kk;
     for (size_t i = 0; i < n; i++) { keys[i] = h.key[i]; idx[i] = h.idx[i] | ((uint64_t)(h.cls[i] == 2) << 63); }
     for (int c = 0; c < s->ncols; c++) {
-        const int eb = elem_bytes_of(s->c.cols[(size_t)c].prim);
+        const int eb = elem_bytes_of(s->c->cols[(size_t)c].prim);
         uint64_t* v = col0 + (size_t)c * 2 * (k + nullw);
         uint8_t* nb = (uint8_t*)(v + kk);
         for (size_t i = 0; i < n; i++) { memcpy(&v[i], h.vals[(size_t)c].data() + i * eb, (size_t)eb); nb[i] = h.nulls[(size_t)c][i]; }
@@ -829,7 +842,7 @@ static void unpack_rows(SortState* s, const uint64_t* buf, HostRows& h) {
     if (h.vals.empty()) { h.vals.assign((size_t)s->ncols, {}); h.nulls.assign((size_t)s->ncols, {}); }
     for (size_t i = 0; i < n; i++) { h.key.push_back(keys[i]); h.idx.push_back(idx[i] & ~(1ull << 63)); h.cls.push_back((idx[i] >> 63) ? 2 : 1); }
     for (int c = 0; c < s->ncols; c++) {
-        const int eb = elem_bytes_of(s->c.cols[(size_t)c].prim);
+        const int eb = elem_bytes_of(s->c->cols[(size_t)c].prim);
         const uint64_t* v = col0 + (size_t)c * 2 * (k + nullw);
         const uint8_t* nb = (const uint8_t*)(v + kk);
         for (size_t i = 0; i < n; i++) {
@@ -851,7 +864,7 @@ int sort_partial_export(SortState* s, void* dev_dst) {
     return 0;
 }
 
-int sort_partial_merge(SortState* s, const void* dev_src, int nranks, std::vector<SortOutCol>& out, int64_t* nrows) {
+int sort_partial_merge(SortState* s, const void* dev_src, int nranks) {
     bkgpu_plan* p = s->p;
     if (!s->topk) return p->fail(BKGPU_EUNSUPPORTED, "only ORDER BY ... LIMIT plans have a partial state");
     const size_t words = sort_partial_bytes(s) / 8;
@@ -860,11 +873,11 @@ int sort_partial_merge(SortState* s, const void* dev_src, int nranks, std::vecto
     CK(p, cudaStreamSynchronize(p->stream));
     HostRows h;
     for (int r = 0; r < nranks; r++) unpack_rows(s, all.data() + (size_t)r * words, h);
-    finish_host_rows(s, h, out, nrows);   // SelectManagerNode's merge of per-region sorted runs (select_manager_node.cpp:50-51)
+    finish_host_rows(s, h);   // SelectManagerNode's merge of per-region sorted runs (select_manager_node.cpp:50-51)
     return 0;
 }
 
-int sort_finish(SortState* s, void* nccl_comm, int nranks, bkgpu_stats* stats, std::vector<SortOutCol>& out, int64_t* nrows) {
+static int finish_rows(SortState* s, void* nccl_comm, int nranks, bkgpu_stats* stats) {
     bkgpu_plan* p = s->p;
     const cudaStream_t st = p->stream;
     if (s->topk) {
@@ -876,30 +889,29 @@ int sort_finish(SortState* s, void* nccl_comm, int nranks, bkgpu_stats* stats, s
             uint64_t *d_send = nullptr, *d_recv = nullptr;
             if ((rc = scope.alloc(&d_send, buf.size() * 8))) return rc;
             if ((rc = scope.alloc(&d_recv, buf.size() * 8 * (size_t)nranks))) return rc;
-            cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
+            StageTimer t;
             CK(p, cudaMemcpyAsync(d_send, buf.data(), buf.size() * 8, cudaMemcpyHostToDevice, st));
-            cudaEventRecord(e0, st);
+            cudaEventRecord(t.a, st);
             if (nccl_all_gather(nccl_comm, d_send, d_recv, buf.size(), st) != 0) return p->fail(BKGPU_ENCCL, "ncclAllGather: %s", nccl_last_error());
-            cudaEventRecord(e1, st);
-            rc = sort_partial_merge(s, d_recv, nranks, out, nrows);
-            float ms = 0; cudaEventElapsedTime(&ms, e0, e1); stats->collective_ms += ms; cudaEventDestroy(e0); cudaEventDestroy(e1);
+            cudaEventRecord(t.b, st);
+            rc = sort_partial_merge(s, d_recv, nranks);
+            float ms = 0; cudaEventElapsedTime(&ms, t.a, t.b); stats->collective_ms += ms;
             return rc;
         }
-        finish_host_rows(s, h, out, nrows);
+        finish_host_rows(s, h);
         return 0;
     }
     if (nccl_comm && nranks > 1) return p->fail(BKGPU_EUNSUPPORTED, "multi-GPU merge is implemented for ORDER BY ... LIMIT (top-k) and aggregates");
-    if (s->c.kind == PK_FILTER) {
+    if (s->c->kind == PK_FILTER) {
         int64_t n = s->ret.rows;
-        int64_t skip = std::min<int64_t>(s->c.offset, n);
+        int64_t skip = std::min<int64_t>(s->c->offset, n);
         n -= skip;
-        *nrows = n;
-        return store_copy_out(p, s->ret, s->c.cols, nullptr, n, skip, out);
+        return store_copy_out(p, s->ret, s->c->cols, nullptr, n, skip);
     }
     // ---- full ORDER BY: stable LSD radix sort of (key image, row id) pairs, least significant ORDER BY key first ----
     const int64_t n = s->ret.rows;
     if (n > RADIX_MAX_KEYS) return p->fail(BKGPU_EUNSUPPORTED, "full sort is limited to 2^30 - 1 rows per GPU");
-    if (n == 0) { *nrows = 0; return store_copy_out(p, s->ret, s->c.cols, nullptr, 0, 0, out); }
+    if (n == 0) return store_copy_out(p, s->ret, s->c->cols, nullptr, 0, 0);
     RadixBufs b(p); int rc;
     if ((rc = b.alloc(n))) return rc;
     RowArgs ra; memset(&ra, 0, sizeof ra);
@@ -916,26 +928,30 @@ int sort_finish(SortState* s, void* nccl_comm, int nranks, bkgpu_stats* stats, s
         CK(p, cudaMemcpyAsync(h_null_flags, null_flags, sizeof(uint32_t) * (size_t)s->ncols, cudaMemcpyDeviceToHost, st));
         CK(p, cudaStreamSynchronize(st));
     }
-    ra.n_cols = s->ncols; ra.nrows = n; ra.prog = s->c.prog; ra.key.pred_out = -1;
+    ra.n_cols = s->ncols; ra.nrows = n; ra.prog = s->c->prog; ra.key.pred_out = -1;
     k_iota<<<grid_for(n, p->sm_count, 8), 256, 0, st>>>(b.ids[0], n);
     int cur = 0;
-    cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-    cudaEventRecord(e0, st);
+    StageTimer t;
+    cudaEventRecord(t.a, st);
     int64_t pass_bytes = 0;
     // a plain column key (config C5's shape): its image comes straight from the column, and without NULLs in it the NULL-rank pass is void
-    const bool direct_key = s->c.has_direct && s->c.sort_keys.size() == 1 && !s->c.direct_cols.empty();
-    const int dcol = direct_key ? s->c.direct_cols[0] : -1;
-    std::vector<const Program*> progs(s->c.sort_keys.size(), &s->c.prog);
-    if ((rc = radix_sort_keys(s, ra, s->c.sort_keys, progs, dcol, dcol >= 0 && h_null_flags[dcol], b, cur, true, stats, pass_bytes))) return rc;
-    cudaEventRecord(e1, st);
+    const bool direct_key = s->c->has_direct && s->c->sort_keys.size() == 1 && !s->c->direct_cols.empty();
+    const int dcol = direct_key ? s->c->direct_cols[0] : -1;
+    std::vector<const Program*> progs(s->c->sort_keys.size(), &s->c->prog);
+    if ((rc = radix_sort_keys(s, ra, s->c->sort_keys, progs, dcol, dcol >= 0 && h_null_flags[dcol], b, cur, true, stats, pass_bytes))) return rc;
+    cudaEventRecord(t.b, st);
     CK(p, cudaStreamSynchronize(st));
-    { float ms = 0; cudaEventElapsedTime(&ms, e0, e1); stats->main_kernel_ms += ms; stats->main_kernel_launches += 1; stats->main_kernel_bytes += pass_bytes; }
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
+    { float ms = 0; cudaEventElapsedTime(&ms, t.a, t.b); stats->main_kernel_ms += ms; stats->main_kernel_launches += 1; stats->main_kernel_bytes += pass_bytes; }
     snprintf(stats->main_kernel_name, sizeof stats->main_kernel_name, "%s", "radix_sort(k_rs_pass)");
     int64_t keep = n; if (s->k >= 0 && keep > s->k) keep = s->k;
-    int64_t skip = std::min<int64_t>(s->c.offset, keep); keep -= skip;
-    *nrows = keep;
-    return store_copy_out(p, s->ret, s->c.cols, b.ids[cur], keep, skip, out);
+    int64_t skip = std::min<int64_t>(s->c->offset, keep); keep -= skip;
+    return store_copy_out(p, s->ret, s->c->cols, b.ids[cur], keep, skip);
+}
+
+int sort_finish(SortState* s, void* nccl_comm, int nranks, bkgpu_stats* stats, const OutCol* desc) {
+    const int rc = finish_rows(s, nccl_comm, nranks, stats);
+    if (!rc && desc) for (size_t k = 0; k < s->p->result.size(); k++) s->p->result[k].desc = desc[k];
+    return rc;
 }
 
 // ---- the window stage's access to the retained rows and the radix sort (window.cu) ----

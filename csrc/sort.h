@@ -1,9 +1,10 @@
-// sort.h — K5 (ORDER BY / top-k) and K1 (filter-only stream compaction): host entry points used by api.cu.
-// A SortState belongs to a plan: it allocates through the plan's allocator, runs on its stream and reports failures through
-// bkgpu_plan::fail.
+// sort.h — K5 (ORDER BY / top-k) and K1 (filter-only stream compaction): host entry points of the sort stage.
+// A SortState belongs to a plan: it allocates through the plan's allocator, runs on its stream, reports failures through
+// bkgpu_plan::fail and writes its rows into the plan's result.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <functional>
 #include <vector>
 #include "../include/bkgpu.h"
 #include "plan.h"
@@ -13,18 +14,17 @@ namespace bk {
 
 struct SortState;  // opaque (sort.cu)
 
-struct SortOutCol {
-    int tuple_id, slot_id, prim, elem;
-    std::vector<uint8_t> values;
-    std::vector<uint8_t> validity;  // LSB bitmap, empty = all valid
-};
-
+// `c` belongs to the plan and outlives the state
 int  sort_open(bkgpu_plan* p, const Compiled& c, int64_t region_base, SortState** out);
 int  sort_push(SortState* s, const DevCol* cols, int64_t nrows, bkgpu_stats* stats);
-int  sort_finish(SortState* s, void* nccl_comm, int nranks, bkgpu_stats* stats, std::vector<SortOutCol>& out, int64_t* nrows);
+// n rows produced on the device into a post fragment: its input columns get room for n rows (`cap` when they grow), `fill` writes their
+// values and null bytes, then they are packed (CTAs: grid_for(…, p->sm_count, per_sm)) and pushed, the push counting into `stats`
+int  sort_feed(SortState* s, int64_t n, int64_t cap, int per_sm, bkgpu_stats* stats, const std::function<int(RowStore& in)>& fill);
+// the fragment's rows into p->result; `desc`: their output column descriptions (nullptr = the fragment's own columns, kind 0)
+int  sort_finish(SortState* s, void* nccl_comm, int nranks, bkgpu_stats* stats, const OutCol* desc);
 size_t sort_partial_bytes(SortState* s);
 int  sort_partial_export(SortState* s, void* dev_dst);
-int  sort_partial_merge(SortState* s, const void* dev_src, int nranks, std::vector<SortOutCol>& out, int64_t* nrows);
+int  sort_partial_merge(SortState* s, const void* dev_src, int nranks);   // and the merged rows into p->result
 void sort_reset(SortState* s);
 
 // ---- the window stage (window.cu) over a SortState's retained rows (a PK_WINDOW plan retains its filtered rows like a full sort) ----

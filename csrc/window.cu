@@ -307,14 +307,6 @@ __global__ void k_win_fn(FnArgs a) {
     }
 }
 
-
-// the stage timer's two events, destroyed on every way out of window_finish
-struct StageTimer {
-    cudaEvent_t a = nullptr, b = nullptr;
-    StageTimer() { cudaEventCreate(&a); cudaEventCreate(&b); }
-    ~StageTimer() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); }
-};
-
 struct ScanBufs { Acc* agg = nullptr; Acc* carry = nullptr; uint32_t ntiles = 0; };
 
 template <int OP> void launch_scan(const ScanIn& in, const ScanBufs& b, uint64_t* out_v, uint64_t* out_c, cudaStream_t st) {
@@ -338,7 +330,7 @@ void run_scan(int op, const ScanIn& in, const ScanBufs& b, uint64_t* out_v, uint
 
 }  // namespace
 
-int window_finish(bkgpu_plan* p, std::vector<SortOutCol>& out, int64_t* nrows) {
+int window_finish(bkgpu_plan* p) {
     const Compiled& c = p->c;
     SortState* rows = p->sort;
     const cudaStream_t st = p->stream;
@@ -462,31 +454,22 @@ int window_finish(bkgpu_plan* p, std::vector<SortOutCol>& out, int64_t* nrows) {
     snprintf(stats->main_kernel_name, sizeof stats->main_kernel_name, "%s", "window_stage(k_win_fn)");
     std::vector<ColRef> desc;
     for (const OutCol& oc : c.out_cols) desc.push_back({oc.tuple_id, oc.slot_id, oc.prim});
-    SortState* post = p->post_sort;
-    if (!post) {
+    if (!p->post) {
         int64_t keep = n;
         if (c.limit >= 0 && keep > c.limit) keep = c.limit;
         const int64_t skip = std::min<int64_t>(c.offset, keep);
         keep -= skip;
-        *nrows = keep;
-        return store_copy_out(p, all, desc, perm, keep, skip, out);
+        return store_copy_out(p, all, desc, perm, keep, skip);
     }
     // the query's ORDER BY: the window rows in their order, as the post fragment's input, through its sort
-    sort_reset(post);
-    if (n > 0) {
-        std::vector<DevCol> dc(desc.size());
-        for (size_t k = 0; k < desc.size(); k++) {
-            RowStore::Col& d = p->post.cols[k];
-            if ((rc = store_reserve(p, p->post, k, n, n, true)) || (rc = store_gather(p, all.cols[k], perm, n, d.vals, d.nulls)) ||
-                (rc = store_pack(p, p->post, k, n, 8, nullptr, &dc[k])))
-                return rc;
-        }
-        bkgpu_stats scratch{};   // (the post fragment's kernels are not the request's main kernel)
-        if ((rc = sort_push(post, dc.data(), n, &scratch))) return rc;
-        stats->kernel_launches += scratch.kernel_launches;
-    }
-    bkgpu_stats scratch{};
-    rc = sort_finish(post, nullptr, 1, &scratch, out, nrows);
+    sort_reset(p->post);
+    bkgpu_stats scratch{};   // (the post fragment's kernels are not the request's main kernel)
+    rc = sort_feed(p->post, n, n, 8, &scratch, [&](RowStore& in) {
+        int r = BKGPU_OK;
+        for (size_t k = 0; k < in.cols.size() && !r; k++) r = store_gather(p, all.cols[k], perm, n, in.cols[k].vals, in.cols[k].nulls);
+        return r;
+    });
+    if (!rc) rc = sort_finish(p->post, nullptr, 1, &scratch, nullptr);
     stats->kernel_launches += scratch.kernel_launches;
     return rc;
 }

@@ -6,9 +6,9 @@ process (BKGPU_LIB is read when the library is loaded), and the two dumps are co
     BKGPU_LIB=/path/b/libbkgpu.so python profiles/ab.py run b.json
     python profiles/ab.py compare a.json b.json
 
-Per run the dump keeps the counters kernel_launches, main_kernel_name, h2d_bytes and d2h_bytes, and the result columns.  The comparison
-wants the same counters, the same group keys, integers and bitmap bytes, bit-identical doubles for the tables of tests/join_key_cases.py (their sums
-are integer-valued) and 1e-9 relative for other double sums (adds through global atomics are not ordered).  That includes the lean
+Per run the dump keeps the counters kernel_launches, main_kernel_name, main_kernel_launches, main_kernel_bytes, h2d_bytes and d2h_bytes, and
+the result columns.  The comparison wants the same counters, the same group keys, integers and bitmap bytes, bit-identical doubles for the
+tables of tests/join_key_cases.py (their sums are integer-valued) and 1e-9 relative for other double sums (adds through global atomics are not ordered).  That includes the lean
 kernel's FX variant: its fixed-point limbs are exact within a CTA, but the CTAs flush their sums into the global table as double atomics,
 so two runs of the same build differ in the last bits."""
 import json
@@ -359,6 +359,25 @@ def window_stack_then_order_by():
     return pl, [[cols], [cols]], {}
 
 
+@case(None, ordered=True)
+def window_limit_offset():   # no query ORDER BY: the window rows leave through the stage's permutation after LIMIT / OFFSET
+    from tests.test_gpu_window import SCAN, K, V, X, table
+    st = P.window_stage(P.scan(0), [P.window_expr("row_number", 1, 1), P.window_expr("sum", 1, 2, X)], [K], [V])
+    pl = P.Plan(P.limit(st, 40_000, 1_234), {0: SCAN, 1: [(1, T.INT64), (2, T.DOUBLE)]})
+    cols = table(29, 300_000, n_keys=250)
+    return pl, [[cols], [cols]], {}
+
+
+@case(None, ordered=True)
+def order_by_over_group_by():   # no LIMIT: the post fragment radix-sorts every group
+    aggs = [P.agg_expr("count_star", 1, 1), P.agg_expr("sum", 1, 2, None, P.slot_ref(0, 3, T.DOUBLE))]
+    tup = {0: [(1, T.INT32), (2, T.INT32), (3, T.DOUBLE), (4, T.DOUBLE)], 1: P.agg_tuple_slots(aggs, [T.INT64, T.DOUBLE])}
+    a = P.agg(P.scan(0), 1, [P.slot_ref(0, 1, T.INT32)], aggs)
+    pl = P.Plan(P.sort(a, [P.slot_ref(0, 1, T.INT32)], [False], tuple_id=1), tup)   # (the group key: unique, so the order is fixed)
+    cols = datagen.c2_table(0, 2_000_000, n_groups=50_000)
+    return pl, [[cols], [cols]], {}
+
+
 @case(["0_1"])
 def rb_compaction():
     from tests import rb_cases
@@ -395,8 +414,8 @@ def execute_runs(pl, runs, options):
                     unpack = (lambda v: v.hex()) if c.prim_type in (T.BITMAP, T.HLL) else (lambda v: list(struct.unpack("<dq", v)))
                     cols.setdefault(c.name, []).extend([unpack(v) if isinstance(v, bytes) else v for v in c.to_list()])
             s = node.stats()
-            out.append({"kernel_launches": s.kernel_launches, "main_kernel_name": s.main_kernel_name.decode(), "h2d_bytes": s.h2d_bytes,
-                        "d2h_bytes": s.d2h_bytes, "columns": cols})
+            out.append({"kernel_launches": s.kernel_launches, "main_kernel_name": s.main_kernel_name.decode(), "main_kernel_launches": s.main_kernel_launches,
+                        "main_kernel_bytes": s.main_kernel_bytes, "h2d_bytes": s.h2d_bytes, "d2h_bytes": s.d2h_bytes, "columns": cols})
     finally:
         node.close(st)
     return out
@@ -423,13 +442,16 @@ def same_value(a, b, exact):
     return math.isclose(a, b, rel_tol=1e-9, abs_tol=0.0)
 
 
+COUNTERS = ("kernel_launches", "main_kernel_name", "main_kernel_launches", "main_kernel_bytes", "h2d_bytes", "d2h_bytes")
+
+
 def compare(path_a, path_b):
     A, B = json.load(open(path_a)), json.load(open(path_b))
     print("A:", A["version"], "\nB:", B["version"], "\nGPU:", A["gpu"], "/", B["gpu"])
     bad = 0
     for name, (_, keys, exact, ordered) in CASES.items():
         for i, (ra, rb) in enumerate(zip(A["cases"][name], B["cases"][name])):
-            problems = [f"{k} {ra[k]} != {rb[k]}" for k in ("kernel_launches", "main_kernel_name", "h2d_bytes", "d2h_bytes") if ra[k] != rb[k]]
+            problems = [f"{k} {ra[k]} != {rb[k]}" for k in COUNTERS if ra[k] != rb[k]]
             ca, cb = ra["columns"], rb["columns"]
             names = sorted(ca)
             if names != sorted(cb):
