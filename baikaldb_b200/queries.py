@@ -63,6 +63,23 @@ def c6_star_groupby(category: int = 12, region: int = 1) -> P.Plan:
     return P.Plan(root, {**STAR_TUPLES, 4: P.agg_tuple_slots(aggs, [T.DOUBLE, T.INT64])})
 
 
+def c6_star_window(category: int = 12, region: int = 1) -> P.Plan:
+    """SELECT d_year, p_brand, SUM(lo_revenue), COUNT(*),
+              RANK() OVER (PARTITION BY d_year ORDER BY SUM(lo_revenue) DESC) AS rnk,
+              SUM(SUM(lo_revenue)) OVER (PARTITION BY d_year) AS year_revenue
+       FROM <C6's star join> GROUP BY d_year, p_brand ORDER BY d_year, rnk, p_brand
+    The top brands of every year and the year's total beside them (TPC-DS q47 / q89-like), as the planner emits it: one WINDOW -> SORT pair
+    per window spec, the first function on top (select_planner.cpp:705-760), above the db-side aggregate of the join.  The window outputs land
+    in tuple 5."""
+    base = c6_star_groupby(category, region)
+    year, brand = P.slot_ref(1, 2, T.INT32), P.slot_ref(2, 2, T.INT32)
+    revenue = P.slot_ref(4, 1, T.DOUBLE)
+    total = P.window_stage(base.root, [P.window_expr("sum", 5, 2, revenue)], [year])
+    ranked = P.window_stage(total, [P.window_expr("rank", 5, 1)], [year], [revenue], [False])
+    root = P.sort(ranked, [year, P.slot_ref(5, 1, T.INT64), brand], [True, True, True], tuple_id=6)
+    return P.Plan(root, {**base.tuples, 5: [(1, T.INT64), (2, T.DOUBLE)]})
+
+
 def c5_topk(k: int = 1000, asc: bool = True) -> P.Plan:
     """SELECT `0_1`, `0_2` FROM t ORDER BY `0_1` ASC LIMIT k          (config C5)"""
     root = P.sort(P.scan(0), [P.slot_ref(0, 1, T.INT64)], [asc], limit=k, tuple_id=0)

@@ -3,7 +3,7 @@
 device-resident synthetic columns (SURVEY.md §8d), CUDA events around reset+push+finish+get_next, one JSON line per
 config with rows/s and achieved GB/s on the config's algorithmic bytes.  The headline line is bench.py's;
 this script measures the side configs on their own (C6, the star join, also its kernels, a parity flag and the Acero time).
-usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [c9] [c10] [c11] [c12] [c13] [c14] [--scale 0.1] [--steps 10]"""
+usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [c9] [c10] [c11] [c12] [c13] [c14] [c15] [--scale 0.1] [--steps 10]"""
 import argparse
 import ctypes
 import json
@@ -104,19 +104,12 @@ def run(name, plan, pushes, rows, algo_bytes, steps, warmup, options=(), collect
     print(json.dumps(line), flush=True)
 
 
-def c6(a):
-    """C6, a star join: lineorder (100M rows) JOIN date (2,556) JOIN part (1M, sparse keys) JOIN supplier (100k), two dimensions filtered,
-    GROUP BY d_year, p_brand.  Device-resident, dimensions pushed first.  Besides the step: the time of k_star_probe and of the aggregate
-    kernel (torch.profiler, a run of its own), a parity flag against a torch computation over all rows, and the same query as an Acero plan
-    (hashjoin chain + aggregate) over the same tables on all host threads."""
-    import time
-    import pyarrow.acero as ac
-    import pyarrow.compute as pc
-    from oracle.acero_oracle import to_table
+def c6_tables(a):
+    """C6's tables (the columns of datagen.c6_tables), generated on the device -> (fact rows, dimension rows, dimension columns, fact columns,
+    fact specs, the pushes (dimensions first), algorithmic bytes)"""
     nf = int(100_000_000 * a.scale)
     nd = {"date": 2_556, "part": max(1000, int(1_000_000 * a.scale)), "supplier": max(1000, int(100_000 * a.scale))}
     seed = 6
-    # the columns of datagen.c6_tables, generated on the device
     date_k = gen(nd["date"], (1, 1, T.INT32, 4, 11, 0, nd["date"], 1.0), seed)
     part_k = gen(nd["part"], (2, 1, T.INT32, 4, 21, 0, nd["part"], 1.0), seed) * datagen.PART_KEY_STRIDE + datagen.PART_KEY_BASE
     dims = {"date": ([(1, 1, T.INT32), (1, 2, T.INT32)], [date_k, (1992 + date_k // 365).to(torch.int32)]),
@@ -129,8 +122,84 @@ def c6(a):
     ft[1] = (ft[1] * datagen.PART_KEY_STRIDE + datagen.PART_KEY_BASE).to(torch.int32)
     fspec = [(0, 1, T.INT32), (0, 2, T.INT32), (0, 3, T.INT32), (0, 4, T.DOUBLE)]
     pushes = [(cols_array(s, t), len(s), t[0].numel()) for s, t in dims.values()] + [(cols_array(fspec, ft), 4, nf)]
-    plan = queries.c6_star_groupby()
     algo = (3 * 4 + 8) * nf + 8 * nd["date"] + 12 * nd["part"] + 8 * nd["supplier"]   # fact keys + revenue, every dimension column read once
+    return nf, nd, dims, ft, fspec, pushes, algo
+
+
+def window_kernel_ms(name, plan, pushes, rows, algo, steps, options=()):
+    """device time per step of the window stage's kernels (k_win_*, the segmented scans) and of the radix sorts, from a torch.profiler run
+    of its own"""
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        run(name, plan, pushes, rows, algo, steps, 1, options=options, emit=False)
+        torch.cuda.synchronize()
+    win = sort = 0.0
+    for e in prof.key_averages():
+        t = getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0)) / 1e3 / steps
+        k = e.key.replace("bk::", "").replace("(anonymous namespace)::", "")
+        if k.startswith(("k_win_", "k_scan_reduce", "k_scan_tiles", "k_scan_down")):
+            win += t
+        elif k.startswith(("k_rs_", "k_sort_images")):
+            sort += t
+    return win, sort
+
+
+def c15(a):
+    """C15, windows above the db-side aggregate.  (1) C6's query, and the same with RANK() OVER (PARTITION BY d_year ORDER BY
+    SUM(revenue) DESC) and SUM(SUM(revenue)) OVER (PARTITION BY d_year), ORDER BY d_year, rnk, p_brand (queries.c6_star_window); (2) a
+    MERGE_AGG over 2M partial rows of 1M groups (1000 classes), without and with RANK() OVER (PARTITION BY class ORDER BY SUM(x) DESC) and
+    SUM(SUM(x)) OVER (PARTITION BY class).  The two plans of a pair run alternately, `--steps` steps at a time, three rounds; each line
+    carries the step times of every round, and the window stage's kernels (k_win_*, the segmented scans) and radix sorts per step from a
+    torch.profiler run of its own.  The request's main kernel stays the aggregate's."""
+    from baikaldb_b200 import plan as P
+    nf, nd, dims, ft, fspec, pushes, algo = c6_tables(a)
+    pairs = [("C15 C6 star join + GROUP BY d_year, p_brand", queries.c6_star_groupby(), "C15 the same with RANK() and SUM(SUM()) OVER (PARTITION BY d_year)",
+              queries.c6_star_window(), pushes, nf, algo)]
+    # (2) the stores' partial rows: every group twice (two regions), class = k % 1000
+    ng = int(1_000_000 * max(a.scale, 0.01))
+    k = torch.arange(ng, dtype=torch.int64, device="cuda").repeat(2)
+    k = k[torch.randperm(k.numel(), device="cuda", generator=torch.Generator(device="cuda").manual_seed(15))]
+    cls = (k % 1000).to(torch.int32)
+    cnt = torch.randint(1, 50, (k.numel(),), dtype=torch.int64, device="cuda", generator=torch.Generator(device="cuda").manual_seed(16))
+    x = torch.rand(k.numel(), dtype=torch.float64, device="cuda", generator=torch.Generator(device="cuda").manual_seed(17)) * cnt
+    spec = [(0, 1, T.INT32), (0, 2, T.INT64), (1, 1, T.INT64), (1, 2, T.DOUBLE)]
+    aggs = [P.agg_expr("count_star", 1, 1), P.agg_expr("sum", 1, 2, None, P.slot_ref(0, 3, T.DOUBLE))]
+    c_, key, total = P.slot_ref(0, 1, T.INT32), P.slot_ref(0, 2, T.INT64), P.slot_ref(1, 2, T.DOUBLE)
+    tup = {0: [(1, T.INT32), (2, T.INT64), (3, T.DOUBLE)], 1: P.agg_tuple_slots(aggs, [T.INT64, T.DOUBLE]), 2: [(1, T.INT64), (2, T.DOUBLE)]}
+    merge = P.agg(P.scan(0), 1, [c_, key], aggs, merge=True)
+    win = P.window_stage(P.window_stage(merge, [P.window_expr("sum", 2, 2, total)], [c_]), [P.window_expr("rank", 2, 1)], [c_], [total], [False])
+    mp = [(cols_array(spec, [cls, k, cnt, x]), 4, k.numel())]
+    opts = [(b"group_capacity_log2", 22)]
+    pairs.append(("C15 MERGE_AGG of 2M partial rows into 1M groups", P.Plan(merge, tup), "C15 the same with RANK() and SUM(SUM()) OVER (PARTITION BY class)",
+                  P.Plan(win, tup), mp, k.numel(), 28 * k.numel()))
+    for base_name, base, win_name, wplan, pu, rows, ab in pairs:
+        o = opts if pu is mp else ()
+        lines = {}
+        for _ in range(3):   # alternated: the plain aggregate, then the same with the windows
+            for nm, pl in ((base_name, base), (win_name, wplan)):
+                ln = run(nm, pl, pu, rows, ab, a.steps, a.warmup, options=o, emit=False)
+                lines.setdefault(nm, ln).setdefault("ms_per_step_rounds", []).append(ln["ms_per_step"])
+        for nm, pl in ((base_name, base), (win_name, wplan)):
+            ln = lines[nm]
+            ln["ms_per_step"] = sorted(ln["ms_per_step_rounds"])[1]   # the median round
+            if pl is wplan:
+                ln["window_kernels_ms_per_step"], ln["radix_sort_ms_per_step"] = window_kernel_ms(nm, pl, pu, rows, ab, a.steps, o)
+            ln["gpu"] = torch.cuda.get_device_name()
+            print(json.dumps(ln), flush=True)
+    del ft, dims, k, cls, cnt, x
+
+
+def c6(a):
+    """C6, a star join: lineorder (100M rows) JOIN date (2,556) JOIN part (1M, sparse keys) JOIN supplier (100k), two dimensions filtered,
+    GROUP BY d_year, p_brand.  Device-resident, dimensions pushed first.  Besides the step: the time of k_star_probe and of the aggregate
+    kernel (torch.profiler, a run of its own), a parity flag against a torch computation over all rows, and the same query as an Acero plan
+    (hashjoin chain + aggregate) over the same tables on all host threads."""
+    import time
+    import pyarrow.acero as ac
+    import pyarrow.compute as pc
+    from oracle.acero_oracle import to_table
+    nf, nd, dims, ft, fspec, pushes, algo = c6_tables(a)
+    plan = queries.c6_star_groupby()
     line, got = run("C6 star join: lineorder JOIN date, part, supplier; 2 dimension filters; GROUP BY d_year, p_brand", plan, pushes, nf, algo,
                     a.steps, a.warmup, collect=True, emit=False)
     # parity: the same aggregate in torch over all rows (dense lookups by key; part keys are stride-7)
@@ -797,6 +866,8 @@ def main():
         c13(a)
     if "c14" in a.configs:
         c14(a)
+    if "c15" in a.configs:
+        c15(a)
     if "c3" in a.configs:
         nf, nd = int(100_000_000 * a.scale), int(10_000_000 * a.scale)
         fs = [(0, 1, T.INT32, 0, 1, 0, nd, 1.0), (0, 2, T.DOUBLE, 1, 2, 0, 0, 1.0)]

@@ -721,7 +721,8 @@ static int agg_collective(bkgpu_plan* p, bool* rows_mode) {
 }
 
 // [LIMIT ->] [SORT ->] [HAVING ->] above the aggregate: the extracted rows (still on the device) become typed columns and run through
-// the post fragment's sort / filter kernels; only the final rows travel to the host
+// the post fragment's sort / filter kernels; only the final rows travel to the host.  Window stages above the aggregate (post kind
+// PK_WINDOW): the rows that pass HAVING are retained, then run through the stages (window.cu) and the query's ORDER BY above them.
 static int agg_post(bkgpu_plan* p, uint32_t n_out, uint32_t out_cap) {
     const size_t nc = p->c.post->cols.size();
     sort_reset(p->post);
@@ -739,7 +740,10 @@ static int agg_post(bkgpu_plan* p, uint32_t n_out, uint32_t out_cap) {
         return BKGPU_OK;
     });
     p->stats.kernel_launches += 1 + (int64_t)nc;   // (the extraction into columns and the packs, counted with no rows too)
-    if (rc || (rc = sort_finish(p->post, nullptr, 1, &scratch, p->c.out_cols.data()))) return rc;
+    if (rc) return rc;
+    if (p->c.post->kind == PK_WINDOW) rc = window_finish(p, *p->c.post, p->post, p->outer, &scratch);
+    else rc = sort_finish(p->post, nullptr, 1, &scratch, p->c.out_cols.data());
+    if (rc) return rc;
     p->stats.kernel_launches += scratch.kernel_launches;
     return BKGPU_OK;
 }

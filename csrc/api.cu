@@ -237,12 +237,16 @@ extern "C" int bkgpu_open(bkgpu_plan* p) {
         return p->fail(BKGPU_EUNSUPPORTED, "hll_add_agg with the repartition merge is outside the GPU path: its sketches travel only with the all-gather of group rows");
     if (p->c.n_rb && p->nccl_comm)
         return p->fail(BKGPU_EUNSUPPORTED, "rb_build_agg with a communicator is outside the GPU path: bitmaps do not travel with the fixed-width partial rows");
+    if (p->c.post && p->c.post->kind == PK_WINDOW && p->c.kind != PK_WINDOW && p->agg.repartition)
+        return p->fail(BKGPU_EUNSUPPORTED, "a window above an aggregate with the repartition merge is outside the GPU path: each rank would hold only its own groups, "
+                       "and a window needs all of them");
     int rc = upload_in_sets(p);
     if (rc) return rc;
     if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) rc = agg_open(p);
     if (!rc && (p->c.kind == PK_SORT || p->c.kind == PK_FILTER || p->c.kind == PK_WINDOW))   // (a window retains its rows like a full sort)
         rc = sort_open(p, p->c, p->region_base, &p->sort);
     if (!rc && p->c.post) rc = sort_open(p, *p->c.post, 0, &p->post);
+    if (!rc && p->c.post && p->c.post->post) rc = sort_open(p, *p->c.post->post, 0, &p->outer);   // (windows above an aggregate: the query's ORDER BY)
     if (rc) return rc;
     p->state = S_OPEN;
     return BKGPU_OK;
@@ -521,7 +525,7 @@ static int bkgpu_finish_impl(bkgpu_plan* p) {
         case PK_SORT: case PK_FILTER: rc = sort_finish(p->sort, p->nccl_comm, p->nranks, &p->stats, nullptr); break;
         case PK_WINDOW:   // the retained rows through the window stages (window.cu), then the query's ORDER BY when there is one
             if (p->nccl_comm && p->nranks > 1) { rc = p->fail(BKGPU_EUNSUPPORTED, "a window fragment runs on one GPU: multi-GPU merge is implemented for ORDER BY ... LIMIT (top-k) and aggregates"); break; }
-            rc = window_finish(p);
+            rc = window_finish(p, p->c, p->sort, p->post, &p->stats);
             break;
         default: rc = p->fail(BKGPU_EUNSUPPORTED, "plan kind %d cannot finish", p->c.kind);
     }
@@ -596,6 +600,10 @@ static int bkgpu_reset_impl(bkgpu_plan* p) {
     join_reset(p);
     if (p->sort) sort_reset(p->sort);
     if (p->c.kind == PK_JOIN && p->post) sort_reset(p->post);
+    if (p->c.kind != PK_WINDOW && p->c.post && p->c.post->kind == PK_WINDOW) {   // windows above an aggregate: their input rows, the query's ORDER BY
+        sort_reset(p->post);
+        if (p->outer) sort_reset(p->outer);
+    }
     p->result.clear(); p->result_rows = 0; p->result_pos = 0;
     bkgpu_stats z{}; z.kernel_launches = p->stats.kernel_launches; p->stats = z;
     p->state = S_OPEN;
@@ -617,6 +625,7 @@ extern "C" void bkgpu_close(bkgpu_plan* p) {
     resolve_timers(p);
     if (p->sort) sort_close(p->sort);
     if (p->post) sort_close(p->post);
+    if (p->outer) sort_close(p->outer);
     for (cudaEvent_t e : p->event_pool) cudaEventDestroy(e);
     for (auto& q : p->dev_allocs) if (!dev_cache().put(p->device, q.second, q.first)) cudaFree(q.first);   // (both streams were drained above)
     for (int i = 0; i < 2; i++) { if (p->stage_free[i]) cudaEventDestroy(p->stage_free[i]); if (p->stage_ready[i]) cudaEventDestroy(p->stage_ready[i]); }

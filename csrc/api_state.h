@@ -147,7 +147,9 @@ struct bkgpu_plan {
     std::vector<uint8_t*> bounce[2]; size_t bounce_rows = 0; cudaEvent_t bounce_done[2] = {nullptr, nullptr}; bool bounce_busy[2] = {false, false};
     // the stages
     SortState* sort = nullptr;        // ORDER BY / filter / window retention (PK_SORT, PK_FILTER, PK_WINDOW)
-    SortState* post = nullptr;        // the post fragment (Compiled::post) above an aggregate, a window or a join that returns rows
+    SortState* post = nullptr;        // the post fragment (Compiled::post) above an aggregate, a window or a join that returns rows: above an
+                                      // aggregate, its sort / HAVING, or the input rows of its window stages
+    SortState* outer = nullptr;       // windows above an aggregate: the query's ORDER BY over the window rows (Compiled::post->post)
     JoinState join;                   // hash join (K4): PK_JOIN_AGG, PK_JOIN, PK_STAR_AGG
     AggState agg;                     // the aggregate: PK_AGG, PK_JOIN_AGG, PK_STAR_AGG
     // results

@@ -1216,6 +1216,34 @@ static std::string in_set_text(const InSet& s) {
     snprintf(buf, sizeof buf, "distinct=%u capacity=%zu class=%d null=%d bytes=%zu", s.n_distinct, cap, s.vclass, (int)s.has_null, s.image.size() * 8);
     return buf;
 }
+// the window stages of a PK_WINDOW fragment (over a scan, or above an aggregate) and the query's ORDER BY above them
+static void explain_window(const Compiled& c, std::string& s) {
+    static const char* fn_names[] = {"count_star", "count", "sum", "avg", "min", "max", "row_number", "rank", "dense_rank", "percent_rank",
+                                     "cume_dist", "ntile", "lead", "lag", "first_value", "last_value", "nth_value"};
+    static const char* bound_names[] = {"PRECEDING", "FOLLOWING", "CURRENT ROW"};
+    char buf[256];
+    for (size_t k = 0; k < c.win.size(); k++) {
+        const WinStage& w = c.win[k];
+        snprintf(buf, sizeof buf, "window stage[%zu]: sort=%s keys=%zu partition=%d exprs=%zu fns=%zu", k, w.new_sort ? "new" : (w.sort_keys.empty() ? "none" : "shared"),
+                 w.sort_keys.size(), w.n_part, w.exprs.size(), w.fns.size()); s += buf;
+        if (w.has_frame) {
+            auto bound = [&](const WinBound& b) {
+                char t[48];
+                if (b.unbounded) snprintf(t, sizeof t, "UNBOUNDED %s", bound_names[b.type]);
+                else if (b.type == BK_BT_CURRENT_ROW) snprintf(t, sizeof t, "CURRENT ROW");
+                else snprintf(t, sizeof t, "%lld %s", (long long)b.num, bound_names[b.type]);
+                return std::string(t);
+            };
+            s += std::string(" frame=") + (w.frame_type == BK_FRAME_ROWS ? "ROWS " : "RANGE ") + bound(w.start) + " .. " + bound(w.end);
+        }
+        s += "\n";
+        for (auto& sk : w.sort_keys) { snprintf(buf, sizeof buf, "  %s key: expr=%d prim=%d asc=%d\n", (&sk - w.sort_keys.data()) < w.n_part ? "partition" : "order", sk.out_reg, sk.prim, (int)sk.asc); s += buf; }
+        for (auto& f : w.fns) { snprintf(buf, sizeof buf, "  fn %s -> %d_%d prim=%d arg=%d default=%d n=%lld method=%d\n", fn_names[f.kind], f.tuple_id, f.slot_id, f.out_prim, f.arg, f.def,
+                                         (long long)f.n, f.method); s += buf; }
+    }
+    if (c.post) { snprintf(buf, sizeof buf, "post fragment above the window: kind=%d keys=%zu limit=%lld offset=%lld\n", c.post->kind, c.post->sort_keys.size(),
+                           (long long)c.post->limit, (long long)c.post->offset); s += buf; }
+}
 static void explain(Compiled& c) {
     char buf[256];
     std::string& s = c.explain;
@@ -1258,31 +1286,13 @@ static void explain(Compiled& c) {
         for (auto& k : c.sort_keys) { snprintf(buf, sizeof buf, "  order key: out=%d prim=%d asc=%d null_first=%d\n", k.out_reg, k.prim, (int)k.asc, (int)k.null_first); s += buf; }
     }
     if (c.kind == PK_WINDOW) {
-        static const char* fn_names[] = {"count_star", "count", "sum", "avg", "min", "max", "row_number", "rank", "dense_rank", "percent_rank",
-                                         "cume_dist", "ntile", "lead", "lag", "first_value", "last_value", "nth_value"};
-        static const char* bound_names[] = {"PRECEDING", "FOLLOWING", "CURRENT ROW"};
         snprintf(buf, sizeof buf, "rows: pred_out=%d limit=%lld offset=%lld stages=%zu\n", c.ap.pred_out, (long long)c.limit, (long long)c.offset, c.win.size()); s += buf;
-        for (size_t k = 0; k < c.win.size(); k++) {
-            const WinStage& w = c.win[k];
-            snprintf(buf, sizeof buf, "window stage[%zu]: sort=%s keys=%zu partition=%d exprs=%zu fns=%zu", k, w.new_sort ? "new" : (w.sort_keys.empty() ? "none" : "shared"),
-                     w.sort_keys.size(), w.n_part, w.exprs.size(), w.fns.size()); s += buf;
-            if (w.has_frame) {
-                auto bound = [&](const WinBound& b) {
-                    char t[48];
-                    if (b.unbounded) snprintf(t, sizeof t, "UNBOUNDED %s", bound_names[b.type]);
-                    else if (b.type == BK_BT_CURRENT_ROW) snprintf(t, sizeof t, "CURRENT ROW");
-                    else snprintf(t, sizeof t, "%lld %s", (long long)b.num, bound_names[b.type]);
-                    return std::string(t);
-                };
-                s += std::string(" frame=") + (w.frame_type == BK_FRAME_ROWS ? "ROWS " : "RANGE ") + bound(w.start) + " .. " + bound(w.end);
-            }
-            s += "\n";
-            for (auto& sk : w.sort_keys) { snprintf(buf, sizeof buf, "  %s key: expr=%d prim=%d asc=%d\n", (&sk - w.sort_keys.data()) < w.n_part ? "partition" : "order", sk.out_reg, sk.prim, (int)sk.asc); s += buf; }
-            for (auto& f : w.fns) { snprintf(buf, sizeof buf, "  fn %s -> %d_%d prim=%d arg=%d default=%d n=%lld method=%d\n", fn_names[f.kind], f.tuple_id, f.slot_id, f.out_prim, f.arg, f.def,
-                                             (long long)f.n, f.method); s += buf; }
-        }
-        if (c.post) { snprintf(buf, sizeof buf, "post fragment above the window: kind=%d keys=%zu limit=%lld offset=%lld\n", c.post->kind, c.post->sort_keys.size(),
-                               (long long)c.post->limit, (long long)c.post->offset); s += buf; }
+        explain_window(c, s);
+    } else if (c.post && c.post->kind == PK_WINDOW) {
+        const Compiled& w = *c.post;
+        snprintf(buf, sizeof buf, "window stages above the aggregate: input columns=%zu having pred_out=%d limit=%lld offset=%lld stages=%zu\n", w.cols.size(),
+                 w.ap.pred_out, (long long)w.limit, (long long)w.offset, w.win.size()); s += buf;
+        explain_window(w, s);
     } else
     if (c.post) { snprintf(buf, sizeof buf, "post fragment above the aggregate: kind=%d keys=%zu pred_out=%d limit=%lld offset=%lld\n", c.post->kind, c.post->sort_keys.size(),
                            c.post->ap.pred_out, (long long)c.post->limit, (long long)c.post->offset); s += buf; }
@@ -1899,30 +1909,36 @@ std::string sort_key_text(const HNode& s) {
 }
 }  // namespace
 
-static bool lower_window(Infer& in, Compiled& out, const HNode& wtop, const HNode* outer_sort, const HNode* limit_node) {
-    out.kind = PK_WINDOW;
-    std::vector<std::pair<const HNode*, const HNode*>> pairs;   // (WINDOW, SORT), top-down
-    const HNode* t = &wtop;
-    while (t && t->node_type == BK_WINDOW_NODE) {
-        const HNode* s = t->ch.empty() ? nullptr : skip_passthrough(&t->ch[0], nullptr);
-        if (!s || s->node_type != BK_SORT_NODE || s->ch.empty()) return in.fail(BKGPU_EUNSUPPORTED, "a WINDOW node's child must be its SORT node");
-        pairs.push_back({t, s});
-        t = skip_passthrough(&s->ch[0], nullptr);
-    }
+// (MERGE_)AGG -> [FILTER ->] SCAN / JOIN / APPLY: the aggregate, lowered into `out` (the aggregate root of a fragment, or the aggregate below
+// window stages)
+static bool lower_agg_node(Infer& in, Compiled& out, const HNode& top, bool under_packet) {
+    if (top.ch.empty()) return in.fail(BKGPU_EINVAL, "AGG node without a child");
+    const HNode* c = skip_passthrough(&top.ch[0], nullptr);
     const HNode* filter = nullptr;
-    if (is_filter(t)) { filter = t; t = t->ch.empty() ? nullptr : skip_passthrough(&t->ch[0], nullptr); }
-    if (!t || t->node_type != BK_SCAN_NODE)
-        return in.fail(BKGPU_EUNSUPPORTED, "window stages must sit on [FILTER ->] SCAN: a window over an aggregate or a join is outside the GPU path");
-    if (filter && filter->limit != -1) return in.fail(BKGPU_EUNSUPPORTED, "LIMIT on a filter below a window is order dependent");
-    out.scan_tuple = t->tuple_id;
-    Program& p = out.prog; memset(&p, 0, sizeof p);
-    memset(&out.ap, 0, sizeof out.ap);
-    Lower lw{&out, &in, &p};
-    if (!intern_tuple(in, out, lw, t->tuple_id, "scan tuple", "the scan tuple")) return false;
+    if (is_filter(c)) { filter = c; c = c->ch.empty() ? nullptr : skip_passthrough(&c->ch[0], nullptr); }
+    if (!c || (c->node_type != BK_SCAN_NODE && c->node_type != BK_JOIN_NODE && c->node_type != BK_APPLY_NODE)) return in.fail(BKGPU_EUNSUPPORTED, "AGG child must be [FILTER ->] SCAN or JOIN");
+    if (filter && filter->limit != -1) return in.fail(BKGPU_EUNSUPPORTED, "LIMIT on a filter below an aggregate is order dependent: outside the GPU path");
+    bool ok;
+    if (c->node_type == BK_SCAN_NODE) ok = lower_agg(in, out, top, conjuncts_of(filter), c->tuple_id, under_packet, true);
+    else if (c->node_type == BK_APPLY_NODE) ok = lower_apply_agg(in, out, top, *c, under_packet, filter);
+    // AGG -> [FILTER ->] JOIN: the store-side chain of a filtered join (separate.cpp:241-260)
+    else ok = join_leaves(c) > 2 ? lower_star_agg(in, out, top, *c, under_packet, filter) : lower_join_agg(in, out, top, *c, under_packet, filter);
+    if (!ok) return false;
+    bool hll_out = false, hll_merge = false, rb_out = false;
+    for (const OutCol& oc : out.out_cols) { hll_out = hll_out || oc.kind == 2; rb_out = rb_out || oc.kind == 3; }
+    for (int k = 0; k < out.ap.n_agg; k++) hll_merge = hll_merge || (out.ap.agg[k].kind == AG_HLL && out.ap.agg[k].arg_prim == BK_HLL);
+    if (hll_merge && out.kind != PK_AGG)   // (a join would have to gather 16400-byte values to the probe rows)
+        return in.fail(BKGPU_EUNSUPPORTED, "MERGE_AGG of HLL sketches over a join is outside the GPU path (MERGE_AGG over a scan is lowered)");
+    if (rb_out && out.ap.n_hll) return in.fail(BKGPU_EUNSUPPORTED, "rb_build_agg beside hll_add_agg in one aggregate is outside the GPU path");
+    return true;
+}
+
+// The WINDOW -> SORT pairs of `w` (a PK_WINDOW fragment whose input columns are interned already), bottom-up, then the window output columns
+// and the query's ORDER BY [+ LIMIT / OFFSET] above them.  `outside`: the refusal of a window expression that reads a column the input
+// rows do not hold.
+using WinPairs = std::vector<std::pair<const HNode*, const HNode*>>;   // (WINDOW, SORT), top-down
+static bool lower_win_stages(Infer& in, Compiled& out, const WinPairs& pairs, const HNode* outer_sort, const HNode* limit_node, const std::string& outside) {
     const size_t n_scan_cols = out.cols.size();
-    int reg = 0;
-    if (!lower_predicate(lw, filter, out.ap, reg)) return false;
-    p.n_out = reg;
     // one device program per distinct (expression, result type) of a stage
     auto intern_expr = [&](WinStage& st, std::map<std::string, int>& seen, const HExpr& e, int to) -> int {
         const std::string key = expr_key(e) + ":" + std::to_string(to);
@@ -1930,7 +1946,7 @@ static bool lower_window(Infer& in, Compiled& out, const HNode& wtop, const HNod
         if (it != seen.end()) return it->second;
         Program q;
         if (!lower_own_program(in, out, q, [&](Lower& l) { int depth = 0; return l.expr(e, depth) && l.cast(e.col_type, to) && l.out_reg(0); })) return -1;
-        if (out.cols.size() != n_scan_cols) { in.fail(BKGPU_EUNSUPPORTED, "a window expression reads a column outside the scan tuple %d", out.scan_tuple); return -1; }
+        if (out.cols.size() != n_scan_cols) { in.fail(BKGPU_EUNSUPPORTED, "%s", outside.c_str()); return -1; }
         st.exprs.push_back(q); st.expr_prim.push_back(to);
         return seen[key] = (int)st.exprs.size() - 1;
     };
@@ -2055,6 +2071,84 @@ static bool lower_window(Infer& in, Compiled& out, const HNode& wtop, const HNod
     return true;
 }
 
+// [LIMIT ->] [SORT ->] (WINDOW -> SORT){1..8} [HAVING ->] (MERGE_)AGG (select_planner.cpp:147-171): the aggregate is lowered as it is without
+// the windows; the stages become its post fragment (kind PK_WINDOW) over the aggregate's output rows, HAVING that fragment's predicate.
+// The windows sit above the db-side aggregate only: a MERGE_AGG over the stores' partial rows (separate.cpp:241-259), or an aggregate over a
+// join / APPLY.  An AGG straight over a scan is the store-side aggregate, which the planner never puts under a window.
+static bool lower_window_over_agg(Infer& in, Compiled& out, const WinPairs& pairs, const HNode* having, const HNode& agg, const HNode* outer_sort,
+                                  const HNode* limit_node, bool under_packet) {
+    if (having && having->limit != -1) return in.fail(BKGPU_EUNSUPPORTED, "LIMIT on a HAVING filter below a window is order dependent");
+    if (!lower_agg_node(in, out, agg, under_packet)) return false;
+    for (const OutCol& oc : out.out_cols) {
+        if (oc.kind == 3) return in.fail(BKGPU_EUNSUPPORTED, "a window above an aggregate that returns a BITMAP is outside the GPU path");
+        if (oc.kind == 2) return in.fail(BKGPU_EUNSUPPORTED, "a window above an aggregate that returns an HLL sketch is outside the GPU path");
+    }
+    if (out.out_cols.size() > (size_t)MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d aggregate output columns under a window", MAX_COLS);
+    auto post = std::make_shared<Compiled>();
+    Compiled& w = *post;
+    w.kind = PK_WINDOW;
+    w.tuples = out.tuples; w.scan_tuple = -1; w.in_sets = out.in_sets;
+    Program& p = w.prog; memset(&p, 0, sizeof p);
+    memset(&w.ap, 0, sizeof w.ap);
+    Lower lw{&w, &in, &p};
+    // the input row: the aggregate's output columns in order (AVG's intermediate blob rides along as a 16-byte payload column)
+    for (const OutCol& oc : out.out_cols) {
+        if (lw.intern_col(oc.tuple_id, oc.slot_id, oc.prim) != (int)w.out_cols.size())
+            return in.fail(BKGPU_EUNSUPPORTED, "aggregate output columns %d_%d appear twice", oc.tuple_id, oc.slot_id);
+        w.out_cols.push_back(oc);
+    }
+    int reg = 0;
+    if (!lower_predicate(lw, having, w.ap, reg)) return false;
+    p.n_out = reg;
+    if (w.cols.size() != out.out_cols.size()) return in.fail(BKGPU_EUNSUPPORTED, "HAVING below a window references a column the aggregate does not output");
+    if (!lower_win_stages(in, w, pairs, outer_sort, limit_node, "a window expression reads a column the aggregate does not output")) return false;
+    out.post = post;
+    return true;
+}
+
+// [LIMIT ->] [SORT ->] (WINDOW -> SORT){1..8} [FILTER ->] SCAN (select_planner.cpp:705-760): the planner gives every window spec its own
+// SORT by the partition expressions followed by the order expressions (is_null_first = is_asc) and a WINDOW that keeps the order part.
+// Each pair becomes one stage over the retained scan rows; the operators above the top WINDOW are the query's ORDER BY / LIMIT.  Above an
+// aggregate: lower_window_over_agg.
+static bool lower_window(Infer& in, Compiled& out, const HNode& wtop, const HNode* outer_sort, const HNode* limit_node, bool under_packet) {
+    WinPairs pairs;
+    const HNode* t = &wtop;
+    while (t && t->node_type == BK_WINDOW_NODE) {
+        const HNode* s = t->ch.empty() ? nullptr : skip_passthrough(&t->ch[0], nullptr);
+        if (!s || s->node_type != BK_SORT_NODE || s->ch.empty()) return in.fail(BKGPU_EUNSUPPORTED, "a WINDOW node's child must be its SORT node");
+        pairs.push_back({t, s});
+        t = skip_passthrough(&s->ch[0], nullptr);
+    }
+    {   // [HAVING ->] (MERGE_)AGG over the stores' rows, a join or an APPLY
+        const HNode* having = nullptr;
+        const HNode* a = t;
+        if (a && (is_filter(a) || a->node_type == BK_HAVING_FILTER_NODE)) { having = a; a = a->ch.empty() ? nullptr : skip_passthrough(&a->ch[0], nullptr); }
+        if (a && (a->node_type == BK_AGG_NODE || a->node_type == BK_MERGE_AGG_NODE) && !a->ch.empty()) {
+            const HNode* src = skip_passthrough(&a->ch[0], nullptr);
+            if (is_filter(src)) src = src->ch.empty() ? nullptr : skip_passthrough(&src->ch[0], nullptr);
+            const bool over_scan = src && src->node_type == BK_SCAN_NODE;
+            const bool over_rows = src && (src->node_type == BK_JOIN_NODE || src->node_type == BK_APPLY_NODE);
+            if ((over_scan && a->node_type == BK_MERGE_AGG_NODE) || over_rows)
+                return lower_window_over_agg(in, out, pairs, having, *a, outer_sort, limit_node, under_packet);
+        }
+    }
+    out.kind = PK_WINDOW;
+    const HNode* filter = nullptr;
+    if (is_filter(t)) { filter = t; t = t->ch.empty() ? nullptr : skip_passthrough(&t->ch[0], nullptr); }
+    if (!t || t->node_type != BK_SCAN_NODE)
+        return in.fail(BKGPU_EUNSUPPORTED, "window stages must sit on [FILTER ->] SCAN: a window over an aggregate or a join is outside the GPU path");
+    if (filter && filter->limit != -1) return in.fail(BKGPU_EUNSUPPORTED, "LIMIT on a filter below a window is order dependent");
+    out.scan_tuple = t->tuple_id;
+    Program& p = out.prog; memset(&p, 0, sizeof p);
+    memset(&out.ap, 0, sizeof out.ap);
+    Lower lw{&out, &in, &p};
+    if (!intern_tuple(in, out, lw, t->tuple_id, "scan tuple", "the scan tuple")) return false;
+    int reg = 0;
+    if (!lower_predicate(lw, filter, out.ap, reg)) return false;
+    p.n_out = reg;
+    return lower_win_stages(in, out, pairs, outer_sort, limit_node, "a window expression reads a column outside the scan tuple " + std::to_string(out.scan_tuple));
+}
+
 // ---------------------------------------------------------------- entry
 // [SORT ->] [FILTER ->] JOIN / APPLY (`node_type`) at the top of the fragment -> that node, else nullptr
 static const HNode* rows_shape(const HNode* t, int node_type) {
@@ -2107,30 +2201,14 @@ int compile_plan(const uint8_t* desc, size_t len, Compiled& out, std::string& er
         if (c && c->node_type == BK_WINDOW_NODE) win_sort = top;
     }
     if (win_sort || top->node_type == BK_WINDOW_NODE) {
-        ok = lower_window(in, out, win_sort ? *skip_passthrough(&win_sort->ch[0], nullptr) : *top, win_sort, limit_node);
+        ok = lower_window(in, out, win_sort ? *skip_passthrough(&win_sort->ch[0], nullptr) : *top, win_sort, limit_node, under_packet);
     } else if (top->node_type == BK_AGG_NODE || top->node_type == BK_MERGE_AGG_NODE) {
-        if (top->ch.empty()) { err = "AGG node without a child"; return BKGPU_EINVAL; }
-        const HNode* c = skip_passthrough(&top->ch[0], nullptr);
-        const HNode* filter = nullptr;
-        if (is_filter(c)) { filter = c; c = c->ch.empty() ? nullptr : skip_passthrough(&c->ch[0], nullptr); }
-        if (!c || (c->node_type != BK_SCAN_NODE && c->node_type != BK_JOIN_NODE && c->node_type != BK_APPLY_NODE)) { err = "AGG child must be [FILTER ->] SCAN or JOIN"; return BKGPU_EUNSUPPORTED; }
-        if (filter && filter->limit != -1) { err = "LIMIT on a filter below an aggregate is order dependent: outside the GPU path"; return BKGPU_EUNSUPPORTED; }
-        if (c->node_type == BK_SCAN_NODE) ok = lower_agg(in, out, *top, conjuncts_of(filter), c->tuple_id, under_packet, true);
-        else if (c->node_type == BK_APPLY_NODE) ok = lower_apply_agg(in, out, *top, *c, under_packet, filter);
-        // AGG -> [FILTER ->] JOIN: the store-side chain of a filtered join (separate.cpp:241-260)
-        else ok = join_leaves(c) > 2 ? lower_star_agg(in, out, *top, *c, under_packet, filter) : lower_join_agg(in, out, *top, *c, under_packet, filter);
+        ok = lower_agg_node(in, out, *top, under_packet);
         // LimitNode straight over the aggregate: the result extraction (agg_result) skips `offset` groups and then keeps `limit` of them,
         // so the limit is stored as it is — not as the first limit + offset rows that a sort or a filter keeps before skipping
         if (ok && limit_node && !post_sort && !post_having) { out.limit = limit_node->limit; out.offset = limit_node->offset; }
-        bool hll_out = false, hll_merge = false, rb_out = false;
+        bool hll_out = false, rb_out = false;
         for (const OutCol& oc : out.out_cols) { hll_out = hll_out || oc.kind == 2; rb_out = rb_out || oc.kind == 3; }
-        for (int k = 0; ok && k < out.ap.n_agg; k++) hll_merge = hll_merge || (out.ap.agg[k].kind == AG_HLL && out.ap.agg[k].arg_prim == BK_HLL);   // (ap is set once lowering succeeded)
-        if (ok && hll_merge && out.kind != PK_AGG) {   // (a join would have to gather 16400-byte values to the probe rows)
-            err = "MERGE_AGG of HLL sketches over a join is outside the GPU path (MERGE_AGG over a scan is lowered)"; return BKGPU_EUNSUPPORTED;
-        }
-        if (ok && rb_out && out.ap.n_hll) {
-            err = "rb_build_agg beside hll_add_agg in one aggregate is outside the GPU path"; return BKGPU_EUNSUPPORTED;
-        }
         if (ok && (post_sort || post_having) && rb_out) {
             err = "a SORT / HAVING / LIMIT above an aggregate that returns a BITMAP is outside the GPU path"; return BKGPU_EUNSUPPORTED;
         }

@@ -330,12 +330,9 @@ void run_scan(int op, const ScanIn& in, const ScanBufs& b, uint64_t* out_v, uint
 
 }  // namespace
 
-int window_finish(bkgpu_plan* p) {
-    const Compiled& c = p->c;
-    SortState* rows = p->sort;
+int window_finish(bkgpu_plan* p, const Compiled& c, SortState* rows, SortState* outer, bkgpu_stats* stats) {
     const cudaStream_t st = p->stream;
     const int sm = p->sm_count;
-    bkgpu_stats* stats = &p->stats;
     DevScope ar(p);   // every device buffer of the call
     const RowStore& ret = sort_retained(rows);
     const int64_t n = ret.rows;
@@ -454,7 +451,7 @@ int window_finish(bkgpu_plan* p) {
     snprintf(stats->main_kernel_name, sizeof stats->main_kernel_name, "%s", "window_stage(k_win_fn)");
     std::vector<ColRef> desc;
     for (const OutCol& oc : c.out_cols) desc.push_back({oc.tuple_id, oc.slot_id, oc.prim});
-    if (!p->post) {
+    if (!outer) {
         int64_t keep = n;
         if (c.limit >= 0 && keep > c.limit) keep = c.limit;
         const int64_t skip = std::min<int64_t>(c.offset, keep);
@@ -462,14 +459,14 @@ int window_finish(bkgpu_plan* p) {
         return store_copy_out(p, all, desc, perm, keep, skip);
     }
     // the query's ORDER BY: the window rows in their order, as the post fragment's input, through its sort
-    sort_reset(p->post);
+    sort_reset(outer);
     bkgpu_stats scratch{};   // (the post fragment's kernels are not the request's main kernel)
-    rc = sort_feed(p->post, n, n, 8, &scratch, [&](RowStore& in) {
+    rc = sort_feed(outer, n, n, 8, &scratch, [&](RowStore& in) {
         int r = BKGPU_OK;
         for (size_t k = 0; k < in.cols.size() && !r; k++) r = store_gather(p, all.cols[k], perm, n, in.cols[k].vals, in.cols[k].nulls);
         return r;
     });
-    if (!rc) rc = sort_finish(p->post, nullptr, 1, &scratch, nullptr);
+    if (!rc) rc = sort_finish(outer, nullptr, 1, &scratch, nullptr);
     stats->kernel_launches += scratch.kernel_launches;
     return rc;
 }

@@ -7,10 +7,10 @@
 
 namespace bk {
 
-// Runs every stage of p->c.win over the rows p->sort retained (stable radix sort when a stage's keys change, then the window functions),
-// and writes the output rows (the scan tuple's slots, then one column per window function) into p->result in the top stage's order after
-// LIMIT / OFFSET, or — when p->post is set (the query's ORDER BY, c.post) — in the post fragment's order.  p->stats.main_kernel_* report
-// the window kernels (sorts excluded).
-int window_finish(bkgpu_plan* p);
+// Runs every stage of w.win (a PK_WINDOW fragment: the plan itself over a scan, or the post fragment above an aggregate) over the rows
+// `rows` retained (stable radix sort when a stage's keys change, then the window functions), and writes the output rows (w's input
+// columns, then one column per window function) into p->result in the top stage's order after LIMIT / OFFSET, or — when `outer` is set
+// (the query's ORDER BY, w.post) — in that fragment's order.  stats->main_kernel_* report the window kernels (sorts excluded).
+int window_finish(bkgpu_plan* p, const Compiled& w, SortState* rows, SortState* outer, bkgpu_stats* stats);
 
 }  // namespace bk
