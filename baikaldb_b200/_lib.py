@@ -22,6 +22,10 @@ class BkgpuColumn(Structure):
                 ("values", c_void_p), ("validity", c_void_p), ("length", c_int64)]
 
 
+class BkgpuBinaryColumn(Structure):
+    _fields_ = [("offsets", c_void_p), ("data", c_void_p), ("validity", c_void_p), ("validity_offset", c_int64), ("length", c_int64)]
+
+
 class BkgpuStats(Structure):
     _fields_ = [("rows_scanned", c_int64), ("rows_filtered", c_int64), ("rows_returned", c_int64),
                 ("kernel_launches", c_int64), ("h2d_bytes", c_int64), ("d2h_bytes", c_int64),
@@ -67,6 +71,11 @@ SYMBOLS = [
     ("bkgpu_memcpy_d2h", c_int, [c_int, c_void_p, c_void_p, c_size_t]),
     ("bkgpu_gen_column", c_int, [c_int, c_void_p, c_int32, c_int32, c_uint64, c_uint32, c_int64, c_int64, c_int64,
                                  c_int64, c_double]),
+    ("bkgpu_dict_build", c_int, [POINTER(c_void_p), c_int, c_void_p, POINTER(BkgpuBinaryColumn), c_int, c_int]),
+    ("bkgpu_dict_size", c_int, [c_void_p, POINTER(c_int64), POINTER(c_int64)]),
+    ("bkgpu_dict_copy", c_int, [c_void_p, c_void_p, c_void_p, c_int]),
+    ("bkgpu_dict_codes", c_int, [c_void_p, c_int, c_void_p, c_void_p, POINTER(c_int64)]),
+    ("bkgpu_dict_free", None, [c_void_p]),
 ]
 
 _lib = None
@@ -109,4 +118,4 @@ def explain(plan_bytes: bytes) -> str:
     return buf.value.decode()
 
 
-__all__ = ["lib", "check", "explain", "BkgpuColumn", "BkgpuStats", "BkgpuError", "SYMBOLS", "LIB_PATH", "byref"]
+__all__ = ["lib", "check", "explain", "BkgpuColumn", "BkgpuBinaryColumn", "BkgpuStats", "BkgpuError", "SYMBOLS", "LIB_PATH", "byref"]

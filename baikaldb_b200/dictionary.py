@@ -14,22 +14,30 @@ include/common/expr_value.h:892-943; ``MutTableKey`` keys are memcomparable).  L
 
 ``s LIKE 'pat'`` is matched against the DICTIONARY on the host with the reference's own matcher (``LikePredicate::like``) and becomes an OR of
 rank ranges (one range for a prefix pattern).  Everything else on a string (concat, length, SUM ...) is refused here exactly as the library refuses it (``Unsupported``): nothing is
-ever answered differently.  The kernels that run are the verified INT32 ones; this module is host code and is checked on the CPU against
+ever answered differently.  The kernels that run are the verified INT32 ones; the rewriting is host code and is checked on the CPU against
 pyarrow's own string kernels (tests/test_dictionary.py).
+
+Where the strings are decides where the dictionary is built.  A domain whose columns are all on the host is encoded by Arrow's CPU kernels
+(unique, sort, index_in).  A domain with a column in device memory (``DeviceStrings``) is encoded on the GPU by the library
+(``bkgpu_dict_*``, csrc/dict.cu; its host columns are uploaded first): only the sorted dictionary comes back to the host — the literal
+thresholds, IN, LIKE's rank ranges and ``decode`` need it — and the code columns stay on the device as ``exec_node.DeviceColumn``s.  Both
+give the same dictionary and codes, hence the same rewritten fragment (tests/test_gpu_dictionary_device.py).
 """
 from __future__ import annotations
 
 import bisect
 import copy
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import pyarrow as pa
 import pyarrow.compute as pc
 
+from . import _lib
 from . import plan as P
 from .column import Column, make_column
+from .exec_node import DeviceColumn
 from .plan import ExprNodeType as E, FuncType as F, PrimitiveType as T
 
 
@@ -38,10 +46,40 @@ class Unsupported(Exception):
 
 
 @dataclass
+class DeviceStrings:
+    """A column in Arrow's large_binary layout in device memory (torch tensors on one CUDA device): value r is
+    ``data[offsets[offset + r] : offsets[offset + r + 1]]``, NULL where bit ``offset + r`` of ``validity`` is clear (``validity`` None: no
+    NULLs).  ``offsets`` int64 and ``data`` / ``validity`` uint8, contiguous; ``length`` -1 = every row the offsets describe."""
+    offsets: object
+    data: object
+    validity: object = None
+    offset: int = 0
+    length: int = -1
+
+    @property
+    def rows(self) -> int:
+        return self.length if self.length >= 0 else int(self.offsets.numel()) - self.offset - 1
+
+    @classmethod
+    def from_arrow(cls, values, device=0) -> "DeviceStrings":
+        """a pyarrow binary / string array (or a list of bytes) uploaded buffer by buffer: a sliced array stays sliced"""
+        import torch
+        arr = values if isinstance(values, (pa.Array, pa.ChunkedArray)) else pa.array(values, pa.large_binary())
+        arr = (arr.combine_chunks() if isinstance(arr, pa.ChunkedArray) else arr).cast(pa.large_binary())
+        vbuf, obuf, dbuf = arr.buffers()
+        up = lambda buf, dt: torch.from_numpy(np.frombuffer(buf, dtype=dt, count=buf.size // np.dtype(dt).itemsize).copy()).to(device)
+        need = arr.offset + len(arr) + 1
+        offsets = up(obuf, np.int64)[:need] if obuf is not None and obuf.size >= 8 * need else torch.zeros(need, dtype=torch.int64, device=device)
+        data = up(dbuf, np.uint8) if dbuf is not None and dbuf.size else torch.zeros(1, dtype=torch.uint8, device=device)
+        validity = up(vbuf, np.uint8) if vbuf is not None and arr.null_count else None
+        return cls(offsets, data, validity, arr.offset, len(arr))
+
+
+@dataclass
 class StringColumn:
     tuple_id: int
     slot_id: int
-    values: object                     # list of bytes (None = NULL), or a pyarrow binary / string array
+    values: object                     # list of bytes (None = NULL), a pyarrow binary / string array, or DeviceStrings
 
     @property
     def name(self) -> str:
@@ -51,7 +89,7 @@ class StringColumn:
 @dataclass
 class Encoded:
     plan: P.Plan                                   # the rewritten fragment: INT32 where the strings were
-    columns: List[Column]                          # the code columns, in the order of the string columns given
+    columns: List[Union[Column, DeviceColumn]]     # the code columns, in the order of the string columns given (device ones for a domain encoded on the GPU)
     dictionaries: Dict[Tuple[int, int], List[bytes]] = field(default_factory=dict)     # scan slot -> its domain's sorted dictionary
     result_slots: Dict[Tuple[int, int], List[bytes]] = field(default_factory=dict)     # result slot (tuple, slot) -> dictionary to decode it with
 
@@ -157,7 +195,56 @@ def like_one(target: bytes, pattern: bytes, charset: str = "utf8") -> bool:
 MAX_LIKE_RANGES = 16   # a LIKE becomes an OR of at most this many code ranges
 
 
-def encode_strings(plan: P.Plan, string_cols: Sequence[StringColumn], charset: str = "utf8") -> Encoded:
+def _encode_on_device(cols: List[DeviceStrings], hash_bits: int = 0):
+    """one comparison domain on the GPU (bkgpu_dict_*): its sorted dictionary (host list of bytes) and per column (codes, validity or None),
+    device tensors.  Runs on torch's current stream of the columns' device."""
+    import torch
+    from ctypes import byref, c_int64, c_void_p
+    dev = cols[0].data.device
+    for c in cols:
+        if c.offsets.dtype != torch.int64 or c.data.dtype != torch.uint8 or (c.validity is not None and c.validity.dtype != torch.uint8):
+            raise ValueError("DeviceStrings: int64 offsets and uint8 data / validity")
+        if any(t is not None and (t.device != dev or not t.is_contiguous()) for t in (c.offsets, c.data, c.validity)):
+            raise ValueError("DeviceStrings: contiguous tensors on one device")
+    index = dev.index if dev.index is not None else torch.cuda.current_device()
+    L = _lib.lib()
+    descs = (_lib.BkgpuBinaryColumn * len(cols))()
+    for i, c in enumerate(cols):
+        descs[i].offsets = c.offsets.data_ptr() + 8 * c.offset
+        descs[i].data = c.data.data_ptr()
+        descs[i].validity = c.validity.data_ptr() if c.validity is not None else None
+        descs[i].validity_offset = c.offset if c.validity is not None else 0
+        descs[i].length = c.rows
+    h = c_void_p()
+    rc = L.bkgpu_dict_build(byref(h), index, torch.cuda.current_stream(index).cuda_stream, descs, len(cols), hash_bits)
+    if rc != _lib.OK:
+        msg = (L.bkgpu_last_error(None) or b"").decode(errors="replace")
+        if rc == _lib.EUNSUPPORTED:
+            raise Unsupported(msg)
+        raise _lib.BkgpuError(rc, msg)
+    try:
+        nv, nb = c_int64(), c_int64()
+        _lib.check(L.bkgpu_dict_size(h, byref(nv), byref(nb)))
+        offs = np.empty(nv.value + 1, np.int64)
+        raw = np.empty(max(nb.value, 1), np.uint8)
+        _lib.check(L.bkgpu_dict_copy(h, offs.ctypes.data, raw.ctypes.data, 0))
+        blob, bounds = raw.tobytes(), offs.tolist()          # (slices of one bytes object: Arrow's to_pylist builds a scalar per value)
+        d = [blob[bounds[i]:bounds[i + 1]] for i in range(nv.value)]
+        out = []
+        for i, c in enumerate(cols):
+            n = c.rows
+            codes = torch.empty(n, dtype=torch.int32, device=dev)
+            valid = torch.empty(max((n + 7) // 8, 1), dtype=torch.uint8, device=dev)
+            nulls = c_int64()
+            _lib.check(L.bkgpu_dict_codes(h, i, codes.data_ptr(), valid.data_ptr(), byref(nulls)))
+            out.append((codes, valid if nulls.value else None))
+        return d, out
+    finally:
+        L.bkgpu_dict_free(h)
+
+
+def encode_strings(plan: P.Plan, string_cols: Sequence[StringColumn], charset: str = "utf8", hash_bits: int = 0) -> Encoded:
+    """``hash_bits`` (tests only): the device encoder keeps only that many bits of its string hash, forcing collisions (0 = all 64)"""
     strings = {(c.tuple_id, c.slot_id): c for c in string_cols}
     is_str = lambda e: e.node_type == E.SLOT_REF and (e.tuple_id, e.slot_id) in strings
     as_bytes = lambda v: v if isinstance(v, bytes) else str(v).encode()
@@ -179,11 +266,23 @@ def encode_strings(plan: P.Plan, string_cols: Sequence[StringColumn], charset: s
     for k in strings:
         members.setdefault(find(k), []).append(k)
     # the columns as Arrow binary arrays: distinct values, byte-wise sort and the value -> rank lookup below are Arrow's vectorised kernels
-    arrays = {k: (c.values if isinstance(c.values, (pa.Array, pa.ChunkedArray)) else pa.array(c.values, pa.large_binary())) for k, c in strings.items()}
+    on_device = {k for k, c in strings.items() if isinstance(c.values, DeviceStrings)}
+    host = {k: c for k, c in strings.items() if k not in on_device}
+    arrays = {k: (c.values if isinstance(c.values, (pa.Array, pa.ChunkedArray)) else pa.array(c.values, pa.large_binary())) for k, c in host.items()}
     arrays = {k: (a.combine_chunks() if isinstance(a, pa.ChunkedArray) else a).cast(pa.large_binary()) for k, a in arrays.items()}
     dictionary: Dict[Tuple[int, int], List[bytes]] = {}
     dict_arrays: Dict[Tuple[int, int], pa.Array] = {}
+    device_codes = {}                                      # scan slot -> (codes, validity or None) on the device
     for root, ks in members.items():
+        dev = [k for k in ks if k in on_device]
+        if dev:                                            # a domain with a device column is encoded on the GPU, its host columns uploaded
+            device = strings[dev[0]].values.data.device
+            cols = [strings[k].values if k in on_device else DeviceStrings.from_arrow(arrays[k], device) for k in ks]
+            d, codes = _encode_on_device(cols, hash_bits)
+            for k, kc in zip(ks, codes):
+                dictionary[k] = d
+                device_codes[k] = kc
+            continue
         distinct = pc.unique(pa.concat_arrays([arrays[k] for k in ks])).drop_null()
         distinct = distinct.take(pc.sort_indices(distinct))      # binary arrays sort by unsigned bytes = the reference's string order
         if len(distinct) >= 1 << 31:
@@ -307,6 +406,11 @@ def encode_strings(plan: P.Plan, string_cols: Sequence[StringColumn], charset: s
     # ---- columns: string -> rank in its domain's dictionary ----
     for c in string_cols:
         k = (c.tuple_id, c.slot_id)
+        if k in device_codes:
+            codes, valid = device_codes[k]
+            enc.columns.append(DeviceColumn(c.tuple_id, c.slot_id, int(T.INT32), codes.data_ptr(), int(codes.numel()),
+                                            valid.data_ptr() if valid is not None else 0, keepalive=(codes, valid)))
+            continue
         ranks = pc.index_in(arrays[k], value_set=dict_arrays[k])           # int32, NULL where the string is NULL
         ok = np.asarray(ranks.is_valid())
         codes = np.asarray(ranks.fill_null(0)).astype(np.int32)

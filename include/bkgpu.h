@@ -231,6 +231,43 @@ int   bkgpu_gen_column(int device, void* dev_dst, int32_t prim_type, int32_t dis
                        uint64_t seed, uint32_t column_id, int64_t row0, int64_t nrows,
                        int64_t lo, int64_t hi, double scale);
 
+/* ---- order-preserving dictionary of STRING columns (csrc/dict.cu) ----
+ * The device counterpart of baikaldb_b200/dictionary.py's encoder: one comparison domain (the columns that are compared with each other,
+ * e.g. the two sides of a join condition) -> its sorted distinct values and, per column, the INT32 rank of every row's value in them.
+ * Order: unsigned bytes, a proper prefix first (std::string::compare; Arrow's sort of binary values).  A NULL gets code 0 and a clear
+ * validity bit.  Needs no plan.
+ *
+ * A column in Arrow's large_binary layout, every buffer in device memory on the handle's device: value r is bytes
+ * [offsets[r], offsets[r + 1]) of `data`; `offsets` has length + 1 entries and need not start at 0 (a sliced array: pass the buffer
+ * advanced by the slice offset).  `validity`: LSB-first bitmap, row r at bit validity_offset + r, or NULL when no value is NULL.
+ * NOT validated: the device buffers themselves.  Offsets are trusted to be non-decreasing and inside `data`, as device batches of
+ * bkgpu_push are trusted; `data` must be non-NULL even when every value is empty. */
+typedef struct bkgpu_binary_column {
+    const int64_t* offsets;
+    const uint8_t* data;
+    const uint8_t* validity;
+    int64_t        validity_offset;
+    int64_t        length;
+} bkgpu_binary_column;
+
+typedef struct bkgpu_dict bkgpu_dict;   /* opaque; owns the dictionary and the codes in device memory */
+
+/* Build the dictionary of `ncols` columns on `device`, on `stream_or_null` (a cudaStream_t; NULL: the handle's own stream).  The columns
+ * are read during the call only.  hash_bits: 0 for the full 64-bit hash; 1 .. 63 keep only that many bits (tests: forces hash collisions,
+ * which the byte comparison resolves).  BKGPU_EINVAL: out or cols NULL, ncols < 1, a negative length or validity offset, NULL offsets or
+ * data, a bad device index; BKGPU_ENODEV: no device; BKGPU_EUNSUPPORTED: more than 2^30 rows in all, or 2^31 distinct values (the host
+ * encoder's limit); BKGPU_ENOMEM.  The message of a failure: bkgpu_last_error(NULL). */
+int   bkgpu_dict_build(bkgpu_dict** out, int device, void* stream_or_null, const bkgpu_binary_column* cols, int ncols, int hash_bits);
+/* distinct values, and their bytes in all */
+int   bkgpu_dict_size(bkgpu_dict*, int64_t* n_values, int64_t* n_bytes);
+/* the sorted values in large_binary layout: n_values + 1 offsets from 0, and n_bytes bytes; host (on_device = 0) or device destinations.
+ * Returns when the copy is done. */
+int   bkgpu_dict_copy(bkgpu_dict*, int64_t* offsets, uint8_t* bytes, int on_device);
+/* column `column`'s codes (length int32, device) and validity bitmap from bit 0 ((length + 7) / 8 bytes, device; NULL: not written);
+ * *null_count (may be NULL) = its NULLs.  Returns when the codes are written. */
+int   bkgpu_dict_codes(bkgpu_dict*, int column, int32_t* codes, uint8_t* validity, int64_t* null_count);
+void  bkgpu_dict_free(bkgpu_dict*);
+
 #ifdef __cplusplus
 }
 #endif
