@@ -16,6 +16,7 @@
 #include "nccl_dl.h"
 #include "prims.cuh"
 #include "build_id.h"
+#include "hostcopy.h"
 
 thread_local std::string g_thread_error;
 
@@ -41,7 +42,7 @@ extern "C" const char* bkgpu_last_error(bkgpu_plan* p) { return p ? p->last_erro
 extern "C" int bkgpu_plan_explain(const uint8_t* desc, size_t len, char* text, size_t text_len) {
     Compiled c; std::string err;
     int rc = compile_plan(desc, len, c, err);
-    if (rc != BKGPU_OK) { if (text && text_len) snprintf(text, text_len, "%s", err.c_str()); return thread_fail(rc, err.c_str()); }
+    if (rc != BKGPU_OK) { if (text && text_len) snprintf(text, text_len, "%s", err.c_str()); return thread_fail(rc, "%s", err.c_str()); }
     if (text && text_len) snprintf(text, text_len, "%s", c.explain.c_str());
     return BKGPU_OK;
 }
@@ -303,55 +304,7 @@ static int ensure_bounce(bkgpu_plan* p, const std::vector<ColRef>& want, size_t 
 
 // ---- host-side copy workers: pageable input (what an Arrow RecordBatch of RocksdbVectorizedReader hands over) is copied into
 // pinned bounce buffers by several threads — cudaMemcpyAsync from pageable memory goes through the driver's single staging buffer
-// at a fraction of the link rate ----
-namespace bk { void stream_copy(void* dst, const void* src, size_t bytes); }   // hostcopy.cpp
-namespace {
-class CopyPool {
-  public:
-    explicit CopyPool(int n) { for (int i = 0; i < n; i++) th_.emplace_back([this] { run(); }); }
-    ~CopyPool() { { std::lock_guard<std::mutex> g(mu_); stop_ = true; } cv_.notify_all(); for (auto& t : th_) t.join(); }
-    int size() const { return (int)th_.size(); }
-    // runs fn(0) .. fn(n - 1) on the workers and the caller; returns when all are done
-    void parallel(int n, const std::function<void(int)>& fn) {
-        if (n <= 0) return;
-        {
-            std::lock_guard<std::mutex> g(mu_);
-            fn_ = &fn; next_ = 0; total_ = n; done_ = 0; gen_++;
-        }
-        cv_.notify_all();
-        work();
-        std::unique_lock<std::mutex> g(mu_);
-        done_cv_.wait(g, [this] { return done_ == total_; });
-        fn_ = nullptr;
-    }
-  private:
-    void work() {
-        for (;;) {
-            int i;
-            const std::function<void(int)>* f;
-            { std::lock_guard<std::mutex> g(mu_); if (!fn_ || next_ >= total_) return; i = next_++; f = fn_; }
-            (*f)(i);
-            { std::lock_guard<std::mutex> g(mu_); ++done_; if (done_ == total_) done_cv_.notify_all(); }
-        }
-    }
-    void run() {
-        uint64_t seen = 0;
-        for (;;) {
-            {
-                std::unique_lock<std::mutex> g(mu_);
-                cv_.wait(g, [&] { return stop_ || gen_ != seen; });
-                if (stop_) return;
-                seen = gen_;
-            }
-            work();
-        }
-    }
-    std::vector<std::thread> th_;
-    std::mutex mu_; std::condition_variable cv_, done_cv_;
-    const std::function<void(int)>* fn_ = nullptr;
-    int next_ = 0, total_ = 0, done_ = 0; uint64_t gen_ = 0; bool stop_ = false;
-};
-}  // namespace
+// at a fraction of the link rate.  The pool (CopyPool, hostcopy.h) is process-wide; plans pushing from several threads take turns on it ----
 // CPUs this process may actually use: online CPUs, its affinity mask and its cgroup CPU quota (a container with a 16-CPU quota on a 128-CPU box
 // gets throttled for the rest of the scheduling period once its threads have burnt the quota — spinning or oversized pools make the copy SLOWER there)
 int cpu_budget() {
@@ -415,47 +368,54 @@ int feed(bkgpu_plan* p, const std::vector<ColRef>& want, const bkgpu_column* col
     if (pageable && (rc = ensure_bounce(p, want, (size_t)chunk))) return rc;
     int buf = 0;
     cudaEvent_t last_ready = nullptr;
-    for (int64_t off = 0; off < nrows; off += chunk, buf ^= 1) {
-        if (p->cancelled.load()) return p->fail(BKGPU_ECANCELLED, "cancelled");
-        const int64_t n = std::min(chunk, nrows - off);
-        CK(p, cudaStreamWaitEvent(p->copy_stream, p->stage_free[buf], 0));
-        if (pageable) {   // bounce: worker threads fill this buffer set's pinned copy of the chunk, the link then runs at the pinned rate
-            if (p->bounce_busy[buf]) { CK(p, cudaEventSynchronize(p->bounce_done[buf])); p->bounce_busy[buf] = false; }
-            struct Piece { uint8_t* dst; const uint8_t* src; size_t bytes; };
-            std::vector<Piece> pieces;
-            const size_t slice = (size_t)1 << 20;
+    bool issued = false;   // a host-to-device copy of the caller's buffers is queued on copy_stream
+    rc = [&]() -> int {
+        for (int64_t off = 0; off < nrows; off += chunk, buf ^= 1) {
+            if (p->cancelled.load()) return p->fail(BKGPU_ECANCELLED, "cancelled");
+            const int64_t n = std::min(chunk, nrows - off);
+            CK(p, cudaStreamWaitEvent(p->copy_stream, p->stage_free[buf], 0));
+            if (pageable) {   // bounce: worker threads fill this buffer set's pinned copy of the chunk, the link then runs at the pinned rate
+                if (p->bounce_busy[buf]) { CK(p, cudaEventSynchronize(p->bounce_done[buf])); p->bounce_busy[buf] = false; }
+                struct Piece { uint8_t* dst; const uint8_t* src; size_t bytes; };
+                std::vector<Piece> pieces;
+                const size_t slice = (size_t)1 << 20;
+                for (size_t i = 0; i < want.size(); i++) {
+                    const size_t eb = (size_t)storage_bytes(prim_storage(want[i].prim)), bytes = (size_t)n * eb;
+                    const uint8_t* src = (const uint8_t*)bound[i]->values + (size_t)off * eb;
+                    for (size_t o = 0; o < bytes; o += slice) pieces.push_back({p->bounce[buf][i] + o, src + o, std::min(slice, bytes - o)});
+                }
+                copy_pool().parallel((int)pieces.size(), [&](int k) {
+                    const Piece& pc = pieces[(size_t)k];
+                    stream_copy(pc.dst, pc.src, pc.bytes);
+                });
+            }
+            issued = true;
             for (size_t i = 0; i < want.size(); i++) {
-                const size_t eb = (size_t)storage_bytes(prim_storage(want[i].prim)), bytes = (size_t)n * eb;
-                const uint8_t* src = (const uint8_t*)bound[i]->values + (size_t)off * eb;
-                for (size_t o = 0; o < bytes; o += slice) pieces.push_back({p->bounce[buf][i] + o, src + o, std::min(slice, bytes - o)});
+                const int st = prim_storage(want[i].prim);
+                const size_t eb = (size_t)storage_bytes(st);
+                const void* hsrc = pageable ? (const void*)p->bounce[buf][i] : (const void*)((const uint8_t*)bound[i]->values + (size_t)off * eb);
+                CK(p, cudaMemcpyAsync(p->stage[buf][i], hsrc, (size_t)n * eb, cudaMemcpyHostToDevice, p->copy_stream));
+                p->stats.h2d_bytes += (int64_t)((size_t)n * eb);
+                dc[i].values = p->stage[buf][i]; dc[i].stype = st; dc[i].prim = want[i].prim; dc[i].validity = nullptr;
+                if (bound[i]->validity) {
+                    CK(p, cudaMemcpyAsync(p->stage_valid[buf][i], bound[i]->validity + off / 8, (size_t)(n + 7) / 8, cudaMemcpyHostToDevice, p->copy_stream));
+                    p->stats.h2d_bytes += (n + 7) / 8;
+                    dc[i].validity = (const uint8_t*)p->stage_valid[buf][i];
+                }
             }
-            copy_pool().parallel((int)pieces.size(), [&](int k) {
-                const Piece& pc = pieces[(size_t)k];
-                stream_copy(pc.dst, pc.src, pc.bytes);
-            });
+            CK(p, cudaEventRecord(p->stage_ready[buf], p->copy_stream));
+            if (pageable) { CK(p, cudaEventRecord(p->bounce_done[buf], p->copy_stream)); p->bounce_busy[buf] = true; }
+            CK(p, cudaStreamWaitEvent(p->stream, p->stage_ready[buf], 0));
+            if ((rc = fn(p, dc.data(), n, off, true))) return rc;
+            CK(p, cudaEventRecord(p->stage_free[buf], p->stream));
+            last_ready = p->stage_ready[buf];
         }
-        for (size_t i = 0; i < want.size(); i++) {
-            const int st = prim_storage(want[i].prim);
-            const size_t eb = (size_t)storage_bytes(st);
-            const void* hsrc = pageable ? (const void*)p->bounce[buf][i] : (const void*)((const uint8_t*)bound[i]->values + (size_t)off * eb);
-            CK(p, cudaMemcpyAsync(p->stage[buf][i], hsrc, (size_t)n * eb, cudaMemcpyHostToDevice, p->copy_stream));
-            p->stats.h2d_bytes += (int64_t)((size_t)n * eb);
-            dc[i].values = p->stage[buf][i]; dc[i].stype = st; dc[i].prim = want[i].prim; dc[i].validity = nullptr;
-            if (bound[i]->validity) {
-                CK(p, cudaMemcpyAsync(p->stage_valid[buf][i], bound[i]->validity + off / 8, (size_t)(n + 7) / 8, cudaMemcpyHostToDevice, p->copy_stream));
-                p->stats.h2d_bytes += (n + 7) / 8;
-                dc[i].validity = (const uint8_t*)p->stage_valid[buf][i];
-            }
-        }
-        CK(p, cudaEventRecord(p->stage_ready[buf], p->copy_stream));
-        if (pageable) { CK(p, cudaEventRecord(p->bounce_done[buf], p->copy_stream)); p->bounce_busy[buf] = true; }
-        CK(p, cudaStreamWaitEvent(p->stream, p->stage_ready[buf], 0));
-        if ((rc = fn(p, dc.data(), n, off, true))) return rc;
-        CK(p, cudaEventRecord(p->stage_free[buf], p->stream));
-        last_ready = p->stage_ready[buf];
-    }
+        return BKGPU_OK;
+    }();
     // the caller's host buffers are borrowed for the duration of the call only (bkgpu.h): the last host-to-device copy must have
-    // read them before bkgpu_push returns (the kernels read the staging buffers, they may still be running)
+    // read them before bkgpu_push returns (the kernels read the staging buffers, they may still be running).  That holds on the
+    // early returns too — a cancel, a failing stage, a failing CUDA call — since a pinned batch is read in place by the DMA engine.
+    if (rc) { if (issued) cudaStreamSynchronize(p->copy_stream); return rc; }
     if (last_ready) CK(p, cudaEventSynchronize(last_ready));
     return BKGPU_OK;
 }
@@ -540,8 +500,9 @@ static int bkgpu_finish_impl(bkgpu_plan* p) {
 
 extern "C" int bkgpu_get_next(bkgpu_plan* p, bkgpu_column* out_cols, int* ncols, int64_t* nrows, int* eos) {
     if (!p || !ncols || !nrows || !eos) return thread_fail(BKGPU_EINVAL, "bkgpu_get_next: NULL argument");
+    // cancelled: eos, like the reference's operators — also when the cancel cut the request short before its bkgpu_finish
+    if (p->cancelled.load() && (p->state == S_OPEN || p->state == S_FINISHED)) { *eos = 1; *nrows = 0; *ncols = 0; return BKGPU_OK; }
     if (p->state != S_FINISHED) return p->fail(BKGPU_ESTATE, "bkgpu_get_next before bkgpu_finish");
-    if (p->cancelled.load()) { *eos = 1; *nrows = 0; *ncols = 0; return BKGPU_OK; }  // cancelled: eos, like the reference's operators
     const int have = (int)p->result.size();
     if (*ncols < have || (have > 0 && !out_cols)) return p->fail(BKGPU_EINVAL, "bkgpu_get_next: need room for %d columns", have);
     const int64_t n = std::min(p->batch_capacity, p->result_rows - p->result_pos);

@@ -1,10 +1,11 @@
-// hostcopy.cpp — the CPU stage of the pageable-input path: worker threads copy slices of the caller's pageable columns into pinned
-// bounce buffers (api.cu, feed()).  The destination is written once and next read by the DMA engine, never by this core, so the copy
+// hostcopy.cpp — the CPU stage of the pageable-input path: worker threads (CopyPool) copy slices of the caller's pageable columns into
+// pinned bounce buffers (api.cu, feed()).  The destination is written once and next read by the DMA engine, never by this core, so the copy
 // uses non-temporal stores: an ordinary store first reads the destination line into the cache (read-for-ownership), which makes the
 // stage move three bytes over the memory bus for every byte copied instead of two.
 #include <immintrin.h>
 #include <stdint.h>
 #include <string.h>
+#include "hostcopy.h"
 
 namespace bk {
 
@@ -27,6 +28,51 @@ void stream_copy(void* dst, const void* src, size_t bytes) {
     static const bool avx2 = __builtin_cpu_supports("avx2");
     if (avx2 && bytes >= 4096) stream_copy_avx2((uint8_t*)dst, (const uint8_t*)src, bytes);
     else memcpy(dst, src, bytes);
+}
+
+CopyPool::CopyPool(int n) { for (int i = 0; i < n; i++) th_.emplace_back([this] { run(); }); }
+
+CopyPool::~CopyPool() {
+    { std::lock_guard<std::mutex> g(mu_); stop_ = true; }
+    cv_.notify_all();
+    for (auto& t : th_) t.join();
+}
+
+void CopyPool::parallel(int n, const std::function<void(int)>& fn) {
+    if (n <= 0) return;
+    std::lock_guard<std::mutex> job(job_mu_);   // (the job lives in the members below: a second caller must not replace it mid-run)
+    {
+        std::lock_guard<std::mutex> g(mu_);
+        fn_ = &fn; next_ = 0; total_ = n; done_ = 0; gen_++;
+    }
+    cv_.notify_all();
+    work();
+    std::unique_lock<std::mutex> g(mu_);
+    done_cv_.wait(g, [this] { return done_ == total_; });
+    fn_ = nullptr;
+}
+
+void CopyPool::work() {
+    for (;;) {
+        int i;
+        const std::function<void(int)>* f;
+        { std::lock_guard<std::mutex> g(mu_); if (!fn_ || next_ >= total_) return; i = next_++; f = fn_; }
+        (*f)(i);
+        { std::lock_guard<std::mutex> g(mu_); ++done_; if (done_ == total_) done_cv_.notify_all(); }
+    }
+}
+
+void CopyPool::run() {
+    uint64_t seen = 0;
+    for (;;) {
+        {
+            std::unique_lock<std::mutex> g(mu_);
+            cv_.wait(g, [&] { return stop_ || gen_ != seen; });
+            if (stop_) return;
+            seen = gen_;
+        }
+        work();
+    }
 }
 
 }  // namespace bk

@@ -18,6 +18,14 @@
  *     calling thread when the plan pointer is NULL).
  *   - one plan = one host thread + one CUDA stream (the reference runs one
  *     bthread per plan fragment, src/exec/agg_node.cpp:447-485).
+ *   - threads: different plans, and different bkgpu_dict handles, may be driven
+ *     from different host threads at the same time — pageable pushes and plans on
+ *     different devices included (the copy workers, the device-buffer caches and
+ *     the resident regions are process-wide and shared safely; concurrent pageable
+ *     pushes take turns on the copy workers).  One plan takes one call at a time;
+ *     the exception is bkgpu_cancel, which may come from any thread.  Calls that
+ *     need no plan (explain, regions, memory helpers) may come from any thread;
+ *     bkgpu_last_error(NULL) is the calling thread's own last message.
  *   - there is NO CPU fallback: without a usable CUDA device every call that
  *     needs one fails with BKGPU_ENODEV.
  */
@@ -150,7 +158,9 @@ int   bkgpu_get_next(bkgpu_plan*, bkgpu_column* out_cols, int* ncols, int64_t* n
  * prepared statements; a maintainer may instead init/close per request): tables are cleared,
  * allocations and streams kept.  Valid after open or finish. */
 int   bkgpu_reset(bkgpu_plan*);
-/* state->cancel(); polled between launches like RuntimeState::is_cancelled. */
+/* state->cancel(); polled between launches like RuntimeState::is_cancelled.  May be called from any thread while another thread
+ * drives the plan.  After it, the plan's bkgpu_push / bkgpu_finish give BKGPU_ECANCELLED and bkgpu_get_next gives eos with no rows,
+ * until bkgpu_reset re-arms the plan. */
 void  bkgpu_cancel(bkgpu_plan*);
 /* ExecNode::close + destroy_tree. */
 void  bkgpu_close(bkgpu_plan*);
@@ -193,7 +203,12 @@ int   bkgpu_hll_estimate(const uint8_t* sketch, size_t len, uint64_t* estimate);
 /* ---- resident regions (the column store / parquet cache analogue, include/column/file_manager.h:252-272) ----
  * A region's columns are copied to HBM once (host or device source) and stay there across queries, keyed by
  * (device, region_id); bkgpu_push_region feeds them to a plan exactly like bkgpu_push(..., on_device = 1) — a query
- * over a resident region moves no input over PCIe.  Registering an id again replaces the region. */
+ * over a resident region moves no input over PCIe.  Registering an id again replaces the region.
+ * bkgpu_region_info gives its rows and the bytes of its values and validity bitmaps.  A malformed column, an unknown id (never
+ * registered, or evicted) give BKGPU_EINVAL.
+ * Lifetime: the kernels of a plan that pushed a region read its device buffers asynchronously until that plan's bkgpu_finish has
+ * returned, as with any device batch.  A region must not be evicted or registered again while such a plan has not returned from
+ * bkgpu_finish (or been closed); other region ids may be registered and evicted at any time, from any thread. */
 int   bkgpu_region_register(int device, int64_t region_id, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device);
 int   bkgpu_region_evict(int device, int64_t region_id);
 int   bkgpu_region_info(int device, int64_t region_id, int64_t* nrows, size_t* bytes);

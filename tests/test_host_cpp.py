@@ -139,6 +139,20 @@ def test_stream_copy_is_a_byte_exact_copy(tmp_path):
     assert r.returncode == 0 and "bad=0" in r.stdout, r.stdout + r.stderr
 
 
+@pytest.mark.parametrize("flags", [["-O2"], ["-O1", "-g", "-fsanitize=thread"]], ids=["O2", "tsan"])
+def test_copy_pool_runs_each_callers_pieces_exactly_once(tmp_path, flags):
+    """the process-wide copy pool of the pageable-input path (csrc/hostcopy.h, CopyPool) driven by 1 .. 8 client threads at once, with
+    0, 1, 3 and 8 workers: every call runs exactly its own pieces, each once, before it returns and never after (tests/cpp/copy_pool_check.cpp).
+    A deadlock ends the check through its watchdog (exit code 2), or else through the timeout here."""
+    exe = str(tmp_path / "copy_pool_check")
+    subprocess.check_call(["g++", *flags, "-std=c++17", "-pthread", os.path.join(ROOT, "tests", "cpp", "copy_pool_check.cpp"),
+                           os.path.join(ROOT, "csrc", "hostcopy.cpp"), "-o", exe])
+    r = subprocess.run([exe], capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0 and "bad=0" in r.stdout, r.stdout + r.stderr
+    assert "ThreadSanitizer" not in r.stderr, r.stderr
+    assert r.stdout.count("miscounted_calls=0 late_pieces=0 out_of_range=0") == 16, r.stdout
+
+
 def _gen_strings(seed, n, domain, null_every):
     out, x = [], seed
     for _ in range(n):
