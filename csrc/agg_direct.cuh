@@ -533,13 +533,15 @@ __global__ void __launch_bounds__(DIRECT_THREADS, 1) k_agg_group_direct(const __
 // so that the largest value seen has M - 3 significant bits above the quantum; M = 62 - ceil(log2(rows this CTA can add)) keeps the
 // 64-bit sum of one slot from overflowing whatever the key distribution.  A value x becomes y = x * 2^F (exact) and takes one of
 //   main  2^(M-15) <= |y| < 2^M : round(y) added to the slot's {mid, hi} limbs, ATOMS.ADD.32 with the carry folded into a RED.32;
-//                                 relative rounding error per value <= 2^-(M-14) (M = 42 at 100M rows: 3.7e-9, typically 1e-12),
+//                                 relative rounding error per value <= 2^-(M-14), i.e. M - 14 significant bits; M falls with the rows
+//                                 one CTA adds: on 132 SMs one batch of 100M rows has M = 42 (28 bits, 3.7e-9), of 300M rows M = 40
+//                                 (26 bits, 1.5e-8); typically 1e-12,
 //   fine  2^(M-47) <= |y| < 2^(M-15) : round(y * 2^32) added to {ext, mid, hi} (three limbs, same per-value precision),
 //   zero  nothing to add,
 //   else  (beyond the sampled range, denormal, Inf, NaN): an exact double add into the global table.
-// A CTA's partial sum of a group is therefore the exact sum of values rounded to at least M-15 = 27 significant bits each — it does not
-// depend on the order in which the atomics land — with an error <= 2^-28 relative to sum(|x|) in the worst case, against north_star's
-// 1e-6.  At flush time the limbs become one double per lane and the table is merged as before (the CTAs' partial sums meet as doubles
+// A CTA's partial sum of a group is therefore the exact sum of values rounded to at least M-14 significant bits each — it does not
+// depend on the order in which the atomics land — with an error <= 2^-(M-14) relative to sum(|x|) in the worst case (2^-28 at M = 42,
+// 2^-26 at M = 40), against north_star's 1e-6 (tests/sum_bounds.py states the whole bound, tests/test_gpu_double_sums.py measures it).  At flush time the limbs become one double per lane and the table is merged as before (the CTAs' partial sums meet as doubles
 // in the global table: RED.E.ADD.F64).
 // (AggFnCall::update's `add` is a sequential double add, agg_fn_call.cpp:496-555; any parallel order already differs from it in the
 // last bits.)

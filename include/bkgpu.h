@@ -130,8 +130,9 @@ int   bkgpu_init(bkgpu_plan** out, const uint8_t* plan_desc, size_t len,
  *   "blocking_sync"        the wait for a request's result: 0 spins (cudaStreamSynchronize), 1 sleeps on a blocking-sync event, -1 (default) sleeps only
  *                          when several ranks share a small CPU budget (ranks > 1 and budget < 4 CPUs per rank)
  *   "lean_fx"              (default 1; environment BKGPU_LEAN_FX) SUM / AVG over DOUBLE columns in the lean kernel accumulate as fixed-point
- *                          limbs with native 32-bit shared-memory atomics (csrc/fx.h: every value keeps >= 27 significant bits, typically
- *                          1e-13 of sum|x|; 0 = IEEE adds through 64/128-bit compare-and-swap loops); bkgpu_stats.main_kernel_name says
+ *                          limbs with native 32-bit shared-memory atomics (csrc/fx.h: every value keeps M - 14 significant bits, where
+ *                          M = 62 - ceil(log2(rows one CTA adds)): 28 bits for a 100M-row batch on 132 SMs, 26 bits from about 277M
+ *                          rows; typically 1e-13 of sum|x|; 0 = IEEE adds through 64/128-bit compare-and-swap loops); bkgpu_stats.main_kernel_name says
  *                          "k_agg_group_lean_fx" when a batch ran that way */
 int   bkgpu_set_option(bkgpu_plan*, const char* key, int64_t value);
 /* ExecNode::open(RuntimeState*) (exec_node.h:140): allocate tables. */

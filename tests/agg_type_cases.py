@@ -24,6 +24,7 @@ import pytest
 from baikaldb_b200 import plan as P
 from baikaldb_b200.column import Column, make_column
 from baikaldb_b200.plan import PrimitiveType as T, storage_dtype
+from tests import sum_bounds
 from tests.join_key_cases import RANGE, date_img, datetime_img
 
 AT = 1
@@ -325,10 +326,11 @@ class Want:
     tol: float = 0.0            # "approx": the absolute tolerance
 
 
-def _float_sum(xs: List[float], avg: bool) -> Want:
+def _float_sum(xs: List[float], avg: bool, fx: Optional[sum_bounds.FxLaunch] = None) -> Want:
     """SUM / AVG's sum over doubles, in the reference's semantics: SUM takes the first value and adds the rest, so SUM over only -0.0 is
     -0.0; AVG's sum starts from +0.0 (agg_initialize), so it is +0.0 there.  A NaN result's payload depends on the hardware (x86 keeps
-    the first NaN operand's payload, the GPU returns its canonical NaN), so any NaN matches a NaN"""
+    the first NaN operand's payload, the GPU returns its canonical NaN), so any NaN matches a NaN.  `fx`: the sum runs through FX's
+    fixed-point limbs (csrc/fx.h), whose inexact sums are held to sum_bounds.fx_bound rather than to recursive summation's bound"""
     if any(math.isnan(x) for x in xs) or (math.inf in xs and -math.inf in xs):
         return Want("nan")
     if math.inf in xs:
@@ -348,11 +350,16 @@ def _float_sum(xs: List[float], avg: bool) -> Want:
     mag = sum(abs(f) for f in fr)
     if mag <= 2**53 * q:
         return Want("f64", float(s))
+    if fx is not None:
+        xa = np.array([float(f) for f in fr])
+        tol = sum_bounds.fx_bound(len(fr), float(mag), float(sum_bounds.fx_value_errors(xa, fx).sum()), fx) + float(sum_bounds.half_ulp(float(s)))
+        return Want("approx", float(s), tol=tol, why="FX rounds each value to its grid (sum_bounds.fx_bound)")
     return Want("approx", float(s), tol=float(mag) * len(fr) * 2.0**-52, why="the sum of these doubles depends on the order of addition")
 
 
-def reference(t: Table, fns: Sequence[str] = FNS, passes=None, grouped=None) -> Dict[tuple, Dict[str, Want]]:
-    """every aggregate of `fns` per group, computed from the Python values.  `passes(i)`: the WHERE clause (default 0_2 < 50)"""
+def reference(t: Table, fns: Sequence[str] = FNS, passes=None, grouped=None, fx: Optional[sum_bounds.FxLaunch] = None) -> Dict[tuple, Dict[str, Want]]:
+    """every aggregate of `fns` per group, computed from the Python values.  `passes(i)`: the WHERE clause (default 0_2 < 50); `fx`: the
+    double sums run through FX (see _float_sum)"""
     grouped = t.grouped if grouped is None else grouped
     passes = passes or (lambda i: t.filt[i] < 50)
     groups: Dict[tuple, List[int]] = {}
@@ -381,7 +388,7 @@ def reference(t: Table, fns: Sequence[str] = FNS, passes=None, grouped=None) -> 
                     row[name] = Want("blob", Want("f64", 0.0), 0)
             elif fn == "sum":
                 if fl:
-                    row[name] = _float_sum(xs, avg=False)
+                    row[name] = _float_sum(xs, avg=False, fx=fx)
                 else:
                     s = sum(xs) % 2**64
                     row[name] = Want("int", s - 2**64 if sum_type(t.vt) == T.INT64 and s >= 2**63 else s)
@@ -395,10 +402,10 @@ def reference(t: Table, fns: Sequence[str] = FNS, passes=None, grouped=None) -> 
                 else:
                     row[name] = Want("int", m)
             elif fn == "avg":
-                s = _float_sum([float(x) for x in xs], avg=True)
+                s = _float_sum([float(x) for x in xs], avg=True, fx=fx)
                 row[name] = _div(s, len(live))
             elif fn == "avg_blob":
-                row[name] = Want("blob", _float_sum([float(x) for x in xs], avg=True), len(live))
+                row[name] = Want("blob", _float_sum([float(x) for x in xs], avg=True, fx=fx), len(live))
         out[k] = row
     return out
 

@@ -16,6 +16,7 @@ from baikaldb_b200.exec_node import execute
 from baikaldb_b200.column import make_column
 from baikaldb_b200.plan import PlanNodeType, PrimitiveType as T
 from oracle import oracle
+from tests import sum_bounds
 from tests.agg_type_cases import (AT, AVG_FNS, DIRECT, FLOATS, FNS, FX, FX_OPEN, INTERP, LEAN, LEAN_KEYS, LEAN_VALUES, OPTIONS, SCALAR, SIGNED_ZERO,
                                   TYPES, UNSIGNED, Table, agg_plan, assert_matches, column_array, date_img, datetime_img, edges, f32, key_image,
                                   key_table, main_fns, out_names, reference, small_values, tname, value_table, zero_table)
@@ -28,7 +29,8 @@ gpu = pytest.mark.gpu
 def run(plan, t: Table, kernel, fns=FNS, options=None, batches=None, cols=None, want=None, passes=None):
     """`plan` on the GPU and on the oracle; both against the reference, bit for bit.  Returns the GPU's columns"""
     cols = cols or t.columns()
-    want = want if want is not None else reference(t, fns, passes)
+    fx = sum_bounds.fx_launch(t.v_arr[np.isfinite(t.v_arr)], rows=t.n) if kernel == FX and t.vt == T.DOUBLE else None
+    want = want if want is not None else reference(t, fns, passes, fx=fx)
     kt = t.kt if t.grouped else None
     assert_matches(oracle.execute(plan.serialize(), cols).columns, want, kt, what="oracle")
     got, st = execute(plan, batches or cols, device=0, options=options if options is not None else OPTIONS[kernel])
