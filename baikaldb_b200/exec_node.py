@@ -131,6 +131,17 @@ def _marshal(cols: Sequence[AnyColumn]):
     return arr, n, nrows, bool(on_device), keep
 
 
+def subquery_first(plan_bytes: bytes) -> bool:
+    """does the plan hold a scalar subquery (an APPLY with max_one_row over an aggregate)?  Its subquery's batches must all come before the
+    first batch of its outer tuple, since every outer row is looked up in the subquery's aggregate over all of them (bkgpu.h); the child
+    order of an APPLY is the other way round (child 0 the outer query, child 1 the subquery).  A plan that does not lower is left to
+    bkgpu_init to report."""
+    try:
+        return "\nscalar subquery: " in _lib.explain(plan_bytes)
+    except BkgpuError:
+        return False
+
+
 class GpuExecNode:
     """``GpuExecNode : ExecNode`` — the node ``ExecNode::create_exec_node`` would instantiate for a
     fused AGG->FILTER->SCAN / SORT / JOIN subtree (src/exec/exec_node.cpp:396-490)."""
@@ -139,6 +150,7 @@ class GpuExecNode:
         self._plan_bytes: Optional[bytes] = None
         self._handle = ctypes.c_void_p()
         self._children: List[ColumnSource] = []
+        self._subquery_first = False
         self._opened = False
         self._eos = False
         self.num_rows_returned = 0
@@ -146,7 +158,16 @@ class GpuExecNode:
     # -- ExecNode::init(const pb::PlanNode&)
     def init(self, plan: Union[Plan, bytes]) -> int:
         self._plan_bytes = plan.serialize() if isinstance(plan, Plan) else bytes(plan)
+        self._subquery_first = subquery_first(self._plan_bytes)
         return 0
+
+    def pull_order(self) -> List[int]:
+        """the children, by index, in the order open() drains them: as added (the plan's order: a join's outer child first), except that
+        a scalar subquery's subquery child (child 1) comes before its outer child (child 0)"""
+        order = list(range(len(self._children)))
+        if self._subquery_first and len(order) == 2:
+            order.reverse()
+        return order
 
     def add_child(self, child: ColumnSource) -> None:
         self._children.append(child)
@@ -170,7 +191,8 @@ class GpuExecNode:
                 _lib.check(L.bkgpu_set_option(self._handle, k.encode(), int(v)), self._handle)
             _lib.check(L.bkgpu_open(self._handle), self._handle)
             self._opened = True
-            for child in self._children:
+            for ci in self.pull_order():
+                child = self._children[ci]
                 eos = False
                 while not eos:
                     if state.is_cancelled():

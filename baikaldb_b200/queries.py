@@ -41,6 +41,21 @@ def c3_join_groupby() -> P.Plan:
                          2: P.agg_tuple_slots(aggs, [T.INT64, T.DOUBLE])})
 
 
+def q17_scalar_subquery(factor: float = 0.2) -> P.Plan:
+    """SELECT COUNT(*), SUM(l.price) FROM lineitem l WHERE l.qty < (SELECT factor * AVG(l2.qty) FROM lineitem l2 WHERE l2.partkey = l.partkey)
+    (TPC-H Q17's core).  The planner makes the subquery an APPLY (SEMI, max_one_row) whose condition reads the subquery's aggregate as an
+    AGG_EXPR; tuple 1 is the outer scan, tuple 0 the subquery's (1 partkey INT32, 2 qty INT32, 3 price DOUBLE each).  Push every batch of
+    tuple 0 before the first batch of tuple 1."""
+    cols = [(1, T.INT32), (2, T.INT32), (3, T.DOUBLE)]
+    avg = P.agg_expr("avg", 4, 1, None, P.slot_ref(0, 2, T.INT32))
+    sub = P.agg(P.where(P.scan(0), P.eq(P.slot_ref(0, 1, T.INT32), P.slot_ref(1, 1, T.INT32))), 4, [], [avg])
+    cond = P.lt(P.slot_ref(1, 2, T.INT32), P.multiplies(P.double_lit(factor), P.agg_expr("avg", 4, 1, None, P.slot_ref(0, 2, T.INT32))))
+    aggs = [P.agg_expr("count_star", 2, 1), P.agg_expr("sum", 2, 2, None, P.slot_ref(1, 3, T.DOUBLE))]
+    root = P.agg(P.apply(P.scan(1), sub, [cond], P.JoinType.SEMI_JOIN, max_one_row=True), 2, [], aggs)
+    return P.Plan(P.packet(root), {0: cols, 1: list(cols), 2: P.agg_tuple_slots(aggs, [T.INT64, T.DOUBLE]),
+                                   4: P.agg_tuple_slots([avg], [T.INT32])})
+
+
 STAR_TUPLES = {0: [(1, T.INT32), (2, T.INT32), (3, T.INT32), (4, T.DOUBLE)],   # lineorder: lo_orderdate, lo_partkey, lo_suppkey, lo_revenue
                1: [(1, T.INT32), (2, T.INT32)],                                # date: d_datekey, d_year
                2: [(1, T.INT32), (2, T.INT32), (3, T.INT32)],                  # part: p_partkey, p_brand, p_category

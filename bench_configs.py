@@ -3,7 +3,7 @@
 device-resident synthetic columns (SURVEY.md §8d), CUDA events around reset+push+finish+get_next, one JSON line per
 config with rows/s and achieved GB/s on the config's algorithmic bytes.  The headline line is bench.py's;
 this script measures the side configs on their own (C6, the star join, also its kernels, a parity flag and the Acero time).
-usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [c9] [c10] [c11] [c12] [c13] [c14] [c15] [--scale 0.1] [--steps 10]"""
+usage: python bench_configs.py [c1] [c3] [c5] [c6] [c7] [c8] [c9] [c10] [c11] [c12] [c13] [c14] [c15] [c16] [--scale 0.1] [--steps 10]"""
 import argparse
 import ctypes
 import json
@@ -797,6 +797,92 @@ def c14(a):
     del g, x
 
 
+def c16(a):
+    """C16, TPC-H Q17's core as a correlated scalar subquery: `SELECT COUNT(*), SUM(l.price) FROM lineitem l WHERE l.qty < (SELECT 0.2 *
+    AVG(l2.qty) FROM lineitem l2 WHERE l2.partkey = l.partkey)` over ONE device-resident table of 100M rows (2M part keys, qty 1..50) pushed
+    under both tuple ids: first as the subquery's tuple 0, then as the outer tuple 1 (queries.q17_scalar_subquery).  Per step, CUDA events on
+    the plan's stream time the subquery's push (its grouped aggregate) and the outer push (k_apply_lookup, then the outer aggregate); one
+    profiled run splits the outer push into k_apply_lookup and the aggregate kernel.  Parity against torch on every run (per-key sums and
+    counts by scatter, the comparison, the sum), and Acero's aggregate -> hashjoin -> filter -> aggregate on the host CPUs."""
+    import subprocess
+    import time
+    from torch.profiler import ProfilerActivity, profile
+    n, keys = int(100_000_000 * a.scale), max(1_000, int(2_000_000 * a.scale))
+    g = torch.Generator(device="cuda").manual_seed(16)
+    pk = torch.randint(0, keys, (n,), device="cuda", generator=g, dtype=torch.int32)
+    qty = torch.randint(1, 51, (n,), device="cuda", generator=g, dtype=torch.int32)
+    price = torch.rand(n, device="cuda", generator=g, dtype=torch.float64) * 1000
+    specs = lambda t: [(t, 1, T.INT32), (t, 2, T.INT32), (t, 3, T.DOUBLE)]
+    sub_arr, outer_arr = cols_array(specs(0), [pk, qty, price]), cols_array(specs(1), [pk, qty, price])
+    s = torch.zeros(keys, dtype=torch.float64, device="cuda").scatter_add_(0, pk.long(), qty.double())
+    c = torch.zeros(keys, dtype=torch.float64, device="cuda").scatter_add_(0, pk.long(), torch.ones(n, dtype=torch.float64, device="cuda"))
+    keep = (c[pk.long()] > 0) & (qty.double() < 0.2 * (s / c.clamp(min=1))[pk.long()])
+    want_n, want_sum = int(keep.sum()), float(price[keep].sum())
+    torch.cuda.synchronize()   # (the plan's stream reads the columns torch wrote)
+    pb = queries.q17_scalar_subquery().serialize()
+    h = ctypes.c_void_p()
+    _lib.check(L.bkgpu_init(ctypes.byref(h), pb, len(pb), 0, None))
+    stream = torch.cuda.Stream()   # (a stream of its own, not the legacy default stream, whose handle 0 would leave the plan to create one)
+    _lib.check(L.bkgpu_set_option(h, b"stream", stream.cuda_stream), h)
+    _lib.check(L.bkgpu_set_option(h, b"group_capacity_log2", max(12, (2 * keys - 1).bit_length())), h)
+    _lib.check(L.bkgpu_open(h), h)
+    out = (BkgpuColumn * 16)()
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+    parity = []
+
+    def step():
+        _lib.check(L.bkgpu_reset(h), h)
+        ev[0].record(stream)
+        _lib.check(L.bkgpu_push(h, sub_arr, 3, n, 1), h)
+        ev[1].record(stream)
+        _lib.check(L.bkgpu_push(h, outer_arr, 3, n, 1), h)
+        ev[2].record(stream)
+        _lib.check(L.bkgpu_finish(h), h)
+        ev[3].record(stream)
+        ncols, nrows, eos = ctypes.c_int(16), ctypes.c_int64(0), ctypes.c_int(0)
+        _lib.check(L.bkgpu_get_next(h, out, ctypes.byref(ncols), ctypes.byref(nrows), ctypes.byref(eos)), h)
+        by = {out[i].slot_id: out[i] for i in range(ncols.value)}
+        got_n = ctypes.c_int64.from_address(by[1].values).value
+        got_sum = ctypes.c_double.from_address(by[2].values).value
+        parity.append(got_n == want_n and abs(got_sum - want_sum) <= 1e-9 * abs(want_sum))
+        torch.cuda.synchronize()
+        return ev[0].elapsed_time(ev[1]), ev[1].elapsed_time(ev[2]), ev[0].elapsed_time(ev[3])
+    for _ in range(a.warmup):
+        step()
+    times = [step() for _ in range(a.steps)]
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(a.steps):
+            step()
+        torch.cuda.synchronize()
+    L.bkgpu_close(h)
+    dev = lambda e: getattr(e, "device_time_total", getattr(e, "cuda_time_total", 0.0))
+    lookup_ms = sum(dev(e) for e in prof.key_averages() if "k_apply_lookup" in e.key) / 1e3 / a.steps
+    med = lambda i: float(np.median([t[i] for t in times]))
+    line = {"config": "C16 TPC-H Q17 core: qty < 0.2 * AVG(qty) of the same part (scalar subquery, %dM rows x 2 pushes, %d keys)" % (n // 1_000_000, keys),
+            "rows": 2 * n, "steps": a.steps, "ms_per_step_median": med(2),
+            "subquery_aggregate_ms (event, subquery push)": med(0), "outer_push_ms (event: k_apply_lookup + outer aggregate)": med(1),
+            "k_apply_lookup_ms (profiled)": lookup_ms, "outer_aggregate_ms (outer push - k_apply_lookup)": med(1) - lookup_ms,
+            "lookup_bytes_per_row_min": 8 + 4, "parity_vs_torch_every_run": all(parity), "rows_kept": want_n}
+    import pyarrow as pa, pyarrow.acero as ac, pyarrow.compute as pc
+    t = pa.table({"k": pa.array(pk.cpu().numpy()), "q": pa.array(qty.cpu().numpy()), "p": pa.array(price.cpu().numpy())})
+    src = lambda: ac.Declaration("table_source", ac.TableSourceNodeOptions(t))
+    sub = ac.Declaration("aggregate", ac.AggregateNodeOptions([("q", "hash_mean", None, "avg_q")], keys=["k"]), inputs=[src()])
+    sub = ac.Declaration("project", ac.ProjectNodeOptions([pc.field("k"), pc.field("avg_q")], ["k2", "avg_q"]), inputs=[sub])
+    hj = ac.Declaration("hashjoin", ac.HashJoinNodeOptions("left outer", ["k"], ["k2"]), inputs=[src(), sub])
+    fl = ac.Declaration("filter", ac.FilterNodeOptions(pc.field("q").cast(pa.float64()) < pc.field("avg_q") * 0.2), inputs=[hj])
+    agg = ac.Declaration("aggregate", ac.AggregateNodeOptions([([], "count_all", None, "n"), ("p", "sum", None, "s")]), inputs=[fl])
+    t0 = time.perf_counter(); at = agg.to_table(use_threads=True); line["acero_host_s"] = time.perf_counter() - t0
+    ad = at.to_pydict()
+    line["acero_matches_torch"] = bool(ad["n"][0] == want_n and abs(ad["s"][0] - want_sum) <= 1e-9 * abs(want_sum))
+    line["acero_host_cpus"] = os.cpu_count()
+    line["gpu"] = torch.cuda.get_device_name(0)
+    try:
+        line["power_limit"] = subprocess.check_output(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"], text=True).split("\n")[0].strip()
+    except Exception:
+        line["power_limit"] = None
+    print(json.dumps(line), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("configs", nargs="*", default=["c1", "c3", "c5"])
@@ -868,6 +954,8 @@ def main():
         c14(a)
     if "c15" in a.configs:
         c15(a)
+    if "c16" in a.configs:
+        c16(a)
     if "c3" in a.configs:
         nf, nd = int(100_000_000 * a.scale), int(10_000_000 * a.scale)
         fs = [(0, 1, T.INT32, 0, 1, 0, nd, 1.0), (0, 2, T.DOUBLE, 1, 2, 0, 0, 1.0)]

@@ -475,9 +475,8 @@ static EventPair* timer_begin(bkgpu_plan* p, std::vector<EventPair>& v, int64_t 
 }
 static void timer_end(bkgpu_plan* p, EventPair* ep) { if (ep) cudaEventRecord(ep->b, p->stream); }
 
-int agg_open(bkgpu_plan* p) {
-    const AggPlan& ap = p->c.ap;
-    AggState& g = p->agg;
+int agg_open(bkgpu_plan* p, AggState& g, const Compiled& c) {
+    const AggPlan& ap = c.ap;
     GroupTable& gt = g.gt;
     if (cudaHostAlloc((void**)&g.h_pinned, 64, cudaHostAllocDefault) == cudaSuccess) memset(g.h_pinned, 0, 64); else g.h_pinned = nullptr;
     g.blocking_wait = g.blocking_sync >= 0 ? g.blocking_sync != 0 : (p->nranks > 1 && cpu_budget() < 4 * p->nranks);   // (agg_wait)
@@ -496,7 +495,7 @@ int agg_open(bkgpu_plan* p) {
         gt.hll_cap = (uint32_t)g.hll_cap;
         CK(p, cudaMemsetAsync(gt.hll_ctr, 0, 16, p->stream));
     }
-    if (p->c.n_rb) {   // rb_build_agg: the pair buffer and the sort's second buffer (one word more each: the build's scan closes on it)
+    if (c.n_rb) {   // rb_build_agg: the pair buffer and the sort's second buffer (one word more each: the build's scan closes on it)
         if ((rc = dev_alloc(p, (void**)&g.rb.keys, ((size_t)g.rb_cap + 1) * 8))) return rc;
         if ((rc = dev_alloc(p, (void**)&g.rb.alt, ((size_t)g.rb_cap + 1) * 8))) return rc;
         if ((rc = dev_alloc(p, (void**)&g.rb.ctr, 8))) return rc;
@@ -514,8 +513,7 @@ int agg_open(bkgpu_plan* p) {
 }
 
 // (the plan's device buffers go back to the allocator with every other buffer of the plan)
-void agg_close(bkgpu_plan* p) {
-    AggState& g = p->agg;
+void agg_close(AggState& g) {
     if (g.wait_event) cudaEventDestroy(g.wait_event);
     if (g.h_pinned) cudaFreeHost(g.h_pinned);
     if (g.h_outv) cudaFreeHost(g.h_outv);
@@ -539,8 +537,7 @@ static int agg_n_img(const AggPlan& ap) {
 
 // the mapped host buffer of the fused extraction, sized for the groups seen so far (at least 2048 rows); false = too many groups
 // to extract this way (the table is then read back by k_extract)
-static bool ensure_fused(bkgpu_plan* p) {
-    AggState& g = p->agg;
+static bool ensure_fused(bkgpu_plan* p, AggState& g, const Compiled& c) {
     uint32_t want = 2048;
     while (want < g.known_groups && want < (1u << 16)) want *= 2;
     if (want < g.known_groups) return false;
@@ -550,7 +547,7 @@ static bool ensure_fused(bkgpu_plan* p) {
         if (!mapped_put(g.fused_bytes, g.h_fused)) cudaFreeHost(g.h_fused);
         g.h_fused = g.d_fused = nullptr; g.fused_cap = 0;
     }
-    const size_t bytes = 32 + (size_t)want * (size_t)agg_n_img(p->c.ap) * 9;
+    const size_t bytes = 32 + (size_t)want * (size_t)agg_n_img(c.ap) * 9;
     uint8_t* h = mapped_take(bytes);
     if (!h && cudaHostAlloc((void**)&h, bytes, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) { cudaGetLastError(); return false; }
     if (cudaHostGetDevicePointer((void**)&g.d_fused, h, 0) != cudaSuccess) { cudaGetLastError(); cudaFreeHost(h); return false; }
@@ -580,12 +577,12 @@ static int rb_room(bkgpu_plan* p, const Compiled& c, int64_t* rows) {
     return BKGPU_OK;
 }
 
-int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp) {
-    AggState& g = p->agg;
+int launch_agg_batch(bkgpu_plan* p, AggState& g, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp) {
     AggEnv env = g.env;   // the options, and what this launch adds to them
     env.fx_off = g.fx_off;
     env.tail_launch = p->join.tail_launch;
-    env.multi_rank = p->nccl_comm && p->nranks > 1; env.has_post = p->c.post != nullptr;
+    // (a table that only k_apply_lookup reads is never extracted: its launches do not extract it either)
+    env.multi_rank = p->nccl_comm && p->nranks > 1; env.has_post = p->c.post != nullptr || g.lookup_only;
     if (c.ap.n_keyw > 0 && env.smem_cap_log2 < 0) learn_groups(g);   // (the shared table is sized from it)
     env.known_groups = g.known_groups;
     AggArgs a; AggSelection sel;
@@ -594,7 +591,7 @@ int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64
     if (rc) return rc;
     a.gt = g.gt; a.rows_passed = g.d_rows_passed;
     if (c.kind == PK_JOIN_AGG) a.join = join_args(p, p->join.tail_launch);
-    if (sel.fused_ok && ensure_fused(p)) { a.fused_out = g.d_fused; a.fused_cap = g.fused_cap; }
+    if (sel.fused_ok && ensure_fused(p, g, c)) { a.fused_out = g.d_fused; a.fused_cap = g.fused_cap; }
     const int64_t kMax = (int64_t)1 << 30;  // rows per launch (32-bit counters inside a CTA)
     int64_t algo_bytes_per_row = 0;
     for (int i = 0; i < a.n_cols; i++) algo_bytes_per_row += storage_bytes(a.cols[i].stype);
@@ -620,7 +617,7 @@ int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64
     return BKGPU_OK;
 }
 
-static int agg_batch(bkgpu_plan* p, const DevCol* cols, int64_t nrows, int64_t, bool vec_ok) { return launch_agg_batch(p, p->c, cols, nrows, vec_ok); }
+static int agg_batch(bkgpu_plan* p, const DevCol* cols, int64_t nrows, int64_t, bool vec_ok) { return launch_agg_batch(p, p->agg, p->c, cols, nrows, vec_ok); }
 
 // MERGE_AGG of hll_add_agg over host memory: every non-NULL input value must be a RAW sketch, or the push fails (device-resident input is
 // checked by the merge kernel itself, and the request then fails at bkgpu_finish)
@@ -645,14 +642,18 @@ static int hll_check_host_sketches(bkgpu_plan* p, const bkgpu_column* cols, int 
 
 // a PK_AGG batch
 int agg_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device) {
-    AggState& g = p->agg;
+    if (p->c.sub) return apply_push(p, cols, ncols, nrows, on_device);   // (a scalar subquery: apply.cu)
     int rc = on_device ? BKGPU_OK : hll_check_host_sketches(p, cols, ncols, nrows);
     if (rc) return rc;
     rc = feed(p, p->c.cols, cols, ncols, nrows, on_device, agg_batch);
     if (rc) return rc;
-    // learn the cardinality for later batches' table size (no sync: a stale value only costs speed); a launch that extracted its
-    // result has already left the count in h_fused
-    if (p->c.ap.n_keyw > 0 && g.env.smem_cap_log2 < 0 && g.h_pinned && !g.fused_last)
+    return learn_groups_async(p, p->agg, p->c);
+}
+
+// learn the cardinality for later batches' table size (no sync: a stale value only costs speed); a launch that extracted its result has
+// already left the count in h_fused
+int learn_groups_async(bkgpu_plan* p, AggState& g, const Compiled& c) {
+    if (c.ap.n_keyw > 0 && g.env.smem_cap_log2 < 0 && g.h_pinned && !g.fused_last)
         CK(p, cudaMemcpyAsync(g.h_pinned, g.gt.n_groups, 4, cudaMemcpyDeviceToHost, p->stream));
     return BKGPU_OK;
 }
@@ -764,14 +765,13 @@ static int agg_wait(bkgpu_plan* p) {
 }
 
 // what the counter block of a finished request tells the plan: rows that passed, FX's exact-path count, the groups it holds
-static int agg_take_counters(bkgpu_plan* p, const uint32_t* ctr) {
-    AggState& g = p->agg;
+int agg_take_counters(bkgpu_plan* p, AggState& g, const uint32_t* ctr) {
     memcpy(&g.rows_passed_host, ctr + 4, 8);
     // FX: values beyond the sampled scale are added exactly, one global atomic each; a plan whose double columns keep producing many of them
     // (a column spanning dozens of binades, outliers dominating the sample) goes back to the CAS kernel for its later launches
     if (ctr[GT_FX_EXACT] > 4096 && (uint64_t)ctr[GT_FX_EXACT] * 64 > (uint64_t)std::max<int64_t>(g.rows_passed_host, 1)) g.fx_off = 1;
-    if (ctr[1]) return p->fail(BKGPU_ETOOBIG, "group table overflow (capacity 2^%d slots / partial_capacity %lld): raise group_capacity_log2",
-                               (int)g.gt.cap_log2, (long long)g.partial_cap);
+    if (ctr[1]) return p->fail(BKGPU_ETOOBIG, "%s overflow (capacity 2^%d slots / partial_capacity %lld): raise group_capacity_log2",
+                               g.table_name, (int)g.gt.cap_log2, (long long)g.partial_cap);
     if (ctr[0] > g.known_groups) g.known_groups = ctr[0];
     g.finish_groups = ctr[0];
     return BKGPU_OK;
@@ -936,7 +936,7 @@ static int agg_extract(bkgpu_plan* p, bool rows_mode, uint32_t ctr[8]) {
             if (learned > g.merge_bound) g.merge_bound = learned;
         }
         p->stats.d2h_bytes += (int64_t)(n_words * 9 + 12);
-        if ((rc = agg_take_counters(p, ctr))) return rc;
+        if ((rc = agg_take_counters(p, p->agg, ctr))) return rc;
         if (ctr[2] <= out_cap) break;   // everything fitted
     }
     return BKGPU_OK;
@@ -950,7 +950,7 @@ static int agg_finish_table(bkgpu_plan* p, bool exchange) {
     if (g.fused_last && !exchange && !p->c.post) {
         if ((rc = agg_wait(p))) return rc;
         const uint32_t* ctr = (const uint32_t*)g.h_fused;
-        if ((rc = agg_take_counters(p, ctr))) return rc;
+        if ((rc = agg_take_counters(p, p->agg, ctr))) return rc;
         const uint32_t n = ctr[0];
         if (n <= g.fused_cap) {
             const int n_img = agg_n_img(p->c.ap);
@@ -989,11 +989,10 @@ int agg_finish(bkgpu_plan* p) {
 
 // Re-arm the table for the next request.  A finished run knows how many groups its table holds (the count came back with the result):
 // clear those slots through the occupied list instead of re-initialising the whole capacity (2^20 slots = 44 MB by default)
-int agg_reset(bkgpu_plan* p) {
-    AggState& g = p->agg;
-    if (p->state == S_FINISHED && g.finish_groups >= 0 && p->c.ap.n_keyw > 0)
-        k_table_clear<<<grid_for(g.finish_groups, p->sm_count, 8), 256, 0, p->stream>>>(g.gt, p->c.ap, (uint32_t)g.finish_groups);
-    else k_table_init<<<grid_for((int64_t)g.gt.cap_mask + 1, p->sm_count, 8), 256, 0, p->stream>>>(g.gt, p->c.ap, 0);
+int agg_reset(bkgpu_plan* p, AggState& g, const Compiled& c) {
+    if (p->state == S_FINISHED && g.finish_groups >= 0 && c.ap.n_keyw > 0)
+        k_table_clear<<<grid_for(g.finish_groups, p->sm_count, 8), 256, 0, p->stream>>>(g.gt, c.ap, (uint32_t)g.finish_groups);
+    else k_table_init<<<grid_for((int64_t)g.gt.cap_mask + 1, p->sm_count, 8), 256, 0, p->stream>>>(g.gt, c.ap, 0);
     CK(p, cudaGetLastError());
     g.finish_groups = -1;
     g.fused_last = false;

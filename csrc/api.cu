@@ -241,9 +241,13 @@ extern "C" int bkgpu_open(bkgpu_plan* p) {
     if (p->c.post && p->c.post->kind == PK_WINDOW && p->c.kind != PK_WINDOW && p->agg.repartition)
         return p->fail(BKGPU_EUNSUPPORTED, "a window above an aggregate with the repartition merge is outside the GPU path: each rank would hold only its own groups, "
                        "and a window needs all of them");
+    if (p->c.sub && p->nccl_comm)
+        return p->fail(BKGPU_EUNSUPPORTED, "a scalar subquery with a communicator is outside the GPU path: the subquery's group table would have to be merged "
+                       "across ranks before the first outer row is looked up");
     int rc = upload_in_sets(p);
     if (rc) return rc;
-    if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) rc = agg_open(p);
+    if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) rc = agg_open(p, p->agg, p->c);
+    if (!rc && p->c.sub) rc = apply_open(p);
     if (!rc && (p->c.kind == PK_SORT || p->c.kind == PK_FILTER || p->c.kind == PK_WINDOW))   // (a window retains its rows like a full sort)
         rc = sort_open(p, p->c, p->region_base, &p->sort);
     if (!rc && p->c.post) rc = sort_open(p, *p->c.post, 0, &p->post);
@@ -477,6 +481,7 @@ static int bkgpu_finish_impl(bkgpu_plan* p) {
         case PK_AGG: case PK_JOIN_AGG: case PK_STAR_AGG:
             if (p->c.kind == PK_JOIN_AGG && (rc = join_tail(p))) break;
             rc = agg_finish(p);
+            if (!rc && p->c.sub) rc = apply_finish(p);
             break;
         case PK_JOIN:   // the outer join's preserved rows, then the sink fragment's result
             if ((rc = join_tail(p)) || (rc = sort_finish(p->post, nullptr, 1, &p->stats, p->c.out_cols.data()))) break;
@@ -555,7 +560,8 @@ static int bkgpu_reset_impl(bkgpu_plan* p) {
     CK(p, cudaSetDevice(p->device));
     p->cancelled.store(0);
     if (p->c.kind == PK_AGG || p->c.kind == PK_JOIN_AGG || p->c.kind == PK_STAR_AGG) {
-        const int rc = agg_reset(p);
+        int rc = agg_reset(p, p->agg, p->c);
+        if (!rc && p->c.sub) rc = apply_reset(p);
         if (rc) return rc;
     }
     join_reset(p);
@@ -591,7 +597,8 @@ extern "C" void bkgpu_close(bkgpu_plan* p) {
     for (auto& q : p->dev_allocs) if (!dev_cache().put(p->device, q.second, q.first)) cudaFree(q.first);   // (both streams were drained above)
     for (int i = 0; i < 2; i++) { if (p->stage_free[i]) cudaEventDestroy(p->stage_free[i]); if (p->stage_ready[i]) cudaEventDestroy(p->stage_ready[i]); }
     for (int i = 0; i < 2; i++) { for (uint8_t* q : p->bounce[i]) if (q) cudaFreeHost(q); if (p->bounce_done[i]) cudaEventDestroy(p->bounce_done[i]); }
-    agg_close(p);
+    agg_close(p->agg);
+    apply_close(p);
     if (p->copy_stream) cudaStreamDestroy(p->copy_stream);
     if (p->own_stream && p->stream) cudaStreamDestroy(p->stream);
     delete p;

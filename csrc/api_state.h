@@ -111,6 +111,18 @@ struct AggState {
     int64_t rb_cap = (int64_t)1 << 27;   // option rb_pair_capacity: keys the rb_build_agg pair buffer holds (8 bytes each, twice: the sort's buffers)
     int repartition = 0;
     int blocking_sync = -1;
+    // a scalar subquery's table (bkgpu_plan::sub_agg) is read by k_apply_lookup and never extracted; its name is the overflow error's
+    bool lookup_only = false;
+    const char* table_name = "group table";
+};
+
+// a scalar subquery (Compiled::sub, apply.cu): the subquery's group table, and the lookup's columns for one chunk of an outer batch
+struct ApplyState {
+    bool outer_started = false;   // an outer batch has been looked up: a later subquery batch is out of order
+    void* out_vals[MAX_AGG] = {}; size_t vals_cap[MAX_AGG] = {};      // the looked-up columns (bytes), one per referenced subquery aggregate
+    void* out_valid[MAX_AGG] = {}; size_t valid_cap[MAX_AGG] = {};    // ... and their validity bitmaps
+    std::vector<ColRef> outer_want;   // the outer tuple's columns of the plan, and their index in c.cols
+    std::vector<int> outer_map;
 };
 
 // BKGPU_TRACE=1: wall-clock time the HOST spends in each phase of a request (summed per plan, printed by bkgpu_close)
@@ -152,6 +164,8 @@ struct bkgpu_plan {
     SortState* outer = nullptr;       // windows above an aggregate: the query's ORDER BY over the window rows (Compiled::post->post)
     JoinState join;                   // hash join (K4): PK_JOIN_AGG, PK_JOIN, PK_STAR_AGG
     AggState agg;                     // the aggregate: PK_AGG, PK_JOIN_AGG, PK_STAR_AGG
+    AggState* sub_agg = nullptr;      // a scalar subquery's group table (Compiled::sub), beside `agg`
+    ApplyState apply;                 // ... and its lookup
     // results
     std::vector<HostCol> result;
     int64_t result_rows = 0, result_pos = 0;
@@ -223,16 +237,26 @@ inline DevCol col_at(const DevCol& c, int64_t off) {
 }
 
 // ---- agg.cu: the aggregate (PK_AGG, PK_JOIN_AGG, PK_STAR_AGG)
-int agg_open(bkgpu_plan* p);     // bkgpu_open: the group table and the pinned counter words (and the HLL arena, the rb_build_agg pair buffer)
+int agg_open(bkgpu_plan* p, AggState& g, const Compiled& c);   // bkgpu_open: the group table of `c` and the pinned counter words (and the HLL arena,
+                                                                // the rb_build_agg pair buffer)
 int agg_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device);   // a PK_AGG batch
 // the aggregate of `c` over one batch; `jp`: fused FK -> PK probe (lean kernel only), +1 without launching when the batch does not fit it
-int launch_agg_batch(bkgpu_plan* p, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp = nullptr);
+int launch_agg_batch(bkgpu_plan* p, AggState& g, const Compiled& c, const DevCol* cols, int64_t nrows, bool vec_ok, const JoinProbe* jp = nullptr);
+int learn_groups_async(bkgpu_plan* p, AggState& g, const Compiled& c);   // after a batch: the group count for the next batches' table size
+int agg_take_counters(bkgpu_plan* p, AggState& g, const uint32_t* ctr);  // a finished request's counter block: overflow (ETOOBIG), what it taught
 int agg_finish(bkgpu_plan* p);   // the cross-rank merge (with a communicator), then the result and stats.rows_filtered
-int agg_reset(bkgpu_plan* p);    // bkgpu_reset: the table is empty again
-void agg_close(bkgpu_plan* p);   // bkgpu_close, once the plan's streams have drained: the host memory the aggregate holds
+int agg_reset(bkgpu_plan* p, AggState& g, const Compiled& c);   // bkgpu_reset: the table is empty again
+void agg_close(AggState& g);     // bkgpu_close, once the plan's streams have drained: the host memory the aggregate holds
 size_t agg_partial_bytes(const bkgpu_plan* p);
 int agg_partial_export(bkgpu_plan* p, void* dev_dst);
 int agg_partial_merge(bkgpu_plan* p, const void* dev_src, int nranks);   // and the result from the merged table
+
+// ---- apply.cu: a scalar subquery (Compiled::sub)
+int apply_open(bkgpu_plan* p);    // bkgpu_open: the subquery's group table (refused with a communicator)
+int apply_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device);   // a batch of the subquery or of the outer tuple
+int apply_finish(bkgpu_plan* p);  // bkgpu_finish, after the aggregate: the subquery table's overflow flag
+int apply_reset(bkgpu_plan* p);   // bkgpu_reset: the subquery's table is empty again
+void apply_close(bkgpu_plan* p);
 
 // ---- join.cu
 int join_push(bkgpu_plan* p, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device);   // PK_JOIN_AGG, PK_JOIN, PK_STAR_AGG

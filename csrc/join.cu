@@ -558,7 +558,7 @@ static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nro
             fc[i] = (int)i == key_fcol ? all[(size_t)c.probe_key_col] : all[(size_t)c.jfast_of_main[i]];
             if (((uintptr_t)fc[i].values & 31) != 0) vec_ok = false;
         }
-        const int rc = launch_agg_batch(p, f, fc.data(), nrows, vec_ok, &j.jp);
+        const int rc = launch_agg_batch(p, p->agg, f, fc.data(), nrows, vec_ok, &j.jp);
         if (rc <= 0) return rc;   // launched (0) or failed (< 0); +1: this batch does not fit the lean kernel
     }
     if (s.jf.mode != 0 && c.jfast && !p->agg.env.force_generic) {
@@ -587,17 +587,17 @@ static int join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nro
                 std::vector<DevCol> sl(all);
                 for (size_t i = 0; i < sl.size(); i++) if (c.col_side[i] == 0) sl[i] = col_at(all[i], off);
                 if ((rc = join_generic_table(p))) return rc;
-                if ((rc = launch_agg_batch(p, c, sl.data(), n, false))) return rc;
+                if ((rc = launch_agg_batch(p, p->agg, c, sl.data(), n, false))) return rc;
             } else {
                 bool vec_ok = true;
                 for (auto& d : fc) if (((uintptr_t)d.values & 31) != 0) vec_ok = false;
-                if ((rc = launch_agg_batch(p, f, fc.data(), n, vec_ok))) return rc;
+                if ((rc = launch_agg_batch(p, p->agg, f, fc.data(), n, vec_ok))) return rc;
             }
         }
         return BKGPU_OK;
     }
     { int rc; if ((rc = join_generic_table(p)) || (rc = join_probe_filter(p, all, nrows))) return rc; }
-    return launch_agg_batch(p, c, all.data(), nrows, false);
+    return launch_agg_batch(p, p->agg, c, all.data(), nrows, false);
 }
 
 // the (probe row, build row) pairs of `n_probe` probe rows (`all`: every plan column, the probe side's at the rows' start), or of the
@@ -677,7 +677,7 @@ static int full_join_agg(bkgpu_plan* p, const std::vector<DevCol>& all, int64_t 
         p->stats.kernel_launches += 2;
         fc[i] = all[m]; fc[i].values = g.vals; fc[i].validity = packed.validity;
     }
-    return launch_agg_batch(p, f, fc.data(), found, true);
+    return launch_agg_batch(p, p->agg, f, fc.data(), found, true);
 }
 static int full_join_probe_batch(bkgpu_plan* p, const DevCol* probe_cols, int64_t nrows, int64_t, bool) {
     const Compiled& c = p->c;
@@ -707,7 +707,7 @@ int join_tail(bkgpu_plan* p) {
     if (c.kind == PK_JOIN) return join_rows_emit(p, all, 0, true);
     if (c.join_type == BK_FULL_JOIN) return full_join_agg(p, all, 0, true);
     j.tail_launch = true;
-    rc = launch_agg_batch(p, c, all.data(), j.side[0].store.rows, false);
+    rc = launch_agg_batch(p, p->agg, c, all.data(), j.side[0].store.rows, false);
     j.tail_launch = false;
     return rc;
 }
@@ -818,7 +818,7 @@ static int star_probe_batch(bkgpu_plan* p, const DevCol* fact_cols, int64_t nrow
                 fc[i].validity = packed.validity;
             }
         }
-        if ((rc = launch_agg_batch(p, f, fc.data(), found, true))) return rc;
+        if ((rc = launch_agg_batch(p, p->agg, f, fc.data(), found, true))) return rc;
     }
     return BKGPU_OK;
 }

@@ -15,6 +15,8 @@
 #include <stdio.h>
 #include <string.h>
 #include <algorithm>
+#include <functional>
+#include <iterator>
 #include <map>
 #include "../include/bkgpu.h"
 #include "datetime.h"
@@ -1309,6 +1311,20 @@ static void explain(Compiled& c) {
         snprintf(buf, sizeof buf, "apply: %s decorrelated into the join above; conjuncts moved from the subquery into the join conditions=%d, "
                  "folded from the filter above into the outer filter=%d\n", c.apply_join_type == BK_SEMI_JOIN ? "SEMI" : "ANTI_SEMI", c.apply_moved, c.apply_folded); s += buf;
     }
+    if (c.sub) {   // the scalar subquery: its grouped aggregate, then the lookup that joins it to the outer rows
+        if (c.sub->explain.empty()) explain(*c.sub);
+        s += "scalar subquery: the subquery's aggregate grouped by its correlation keys {\n" + c.sub->explain + "}\n";
+        for (size_t k = 0; k < c.sub_key_cols.size(); k++) {
+            const ColRef& oc = c.cols[(size_t)c.sub_key_cols[k]];
+            snprintf(buf, sizeof buf, "  lookup key[%zu]: outer col[%d] = %d_%d prim=%d cast=%d\n", k, c.sub_key_cols[k], oc.tuple_id, oc.slot_id, oc.prim,
+                     c.sub->ap.key_prim[k]); s += buf;
+        }
+        for (size_t k = 0; k < c.sub_out_cols.size(); k++) {
+            snprintf(buf, sizeof buf, "  lookup col[%d] <- subquery agg[%d] (no group: %s)\n", c.sub_out_cols[k], c.sub_out_agg[k],
+                     c.sub->ap.agg[c.sub_out_agg[k]].kind <= AG_COUNT ? "0" : "NULL"); s += buf;
+        }
+        s += "  k_apply_lookup per outer batch, then the aggregate below over the outer columns and the looked-up ones\n";
+    }
     snprintf(buf, sizeof buf, "program: %d instr, %d outputs\n", c.prog.n_instr, c.prog.n_out); s += buf;
     for (int i = 0; i < c.prog.n_instr; i++) {
         const Instr& in = c.prog.code[i];
@@ -1335,6 +1351,7 @@ void patch_in_sets(Compiled& c, const std::vector<uint64_t>& addr) {
     for (WinStage& w : c.win) for (Program& q : w.exprs) fix(q);
     if (c.post) patch_in_sets(*c.post, addr);
     if (c.jfast) patch_in_sets(*c.jfast, addr);
+    if (c.sub) patch_in_sets(*c.sub, addr);
 }
 
 // ---------------------------------------------------------------- steps shared by the fragments
@@ -1763,11 +1780,118 @@ static bool lower_star_agg(Infer& in, Compiled& out, const HNode& agg, const HNo
 // An APPLY whose own conditions hold an outer = inner column equality (a correlated IN) runs as hash_apply instead: the subquery is opened
 // once, with no outer row, so a correlated conjunct inside it reads the outer columns as NULL and no subquery row passes.  That is not the
 // per-row meaning, and such a plan is refused.
+//
+// A scalar subquery: `x op (SELECT agg ... WHERE inner.k = outer.k ...)` reaches the library as APPLY(SEMI, max_one_row) whose subquery is
+// AGG (no GROUP BY) -> [FILTER ->]* SCAN and whose conditions read the subquery's aggregates as AGG_EXPR nodes (construct_apply_node inlines the
+// subquery's projections).  The reference runs it as nested_loop_apply: per outer row it substitutes the outer values into the subquery and
+// runs it again.  A scalar AGG yields exactly one row even over no input — the default row of AggNode::get_next (agg_node.cpp:489-503), which
+// needs a PACKET ancestor: get_parent_node walks up through the APPLY to the query's PACKET, and separate_apply leaves the subquery below the
+// APPLY — so the row exists, with COUNT / COUNT(*) 0 and SUM / AVG / MIN / MAX NULL.  When every correlated conjunct is an outer = inner column
+// equality, that per-row value is the group of the subquery's aggregate GROUP BY the inner columns (its own conjuncts as WHERE) whose key equals
+// the outer values, or the empty-input row when there is none (a NULL outer key finds none; the NULL-key group is never found).  So the
+// subquery becomes a grouped aggregate of its own (Compiled::sub), and the plan's aggregate runs over the outer rows plus one looked-up column
+// per subquery aggregate its conditions read (k_apply_lookup); its predicate is the outer filter, the filter above the APPLY and the conditions.
+static bool lower_scalar_apply(Infer& in, Compiled& out, const HNode& agg, const HNode& apply, const HNode& sa, bool under_packet, const HNode* above) {
+    auto below = [](const HNode* n) { return n->ch.empty() ? nullptr : skip_passthrough(&n->ch[0], nullptr); };
+    const HNode* o = skip_passthrough(&apply.ch[0], nullptr);
+    const HNode* ofilt = nullptr;
+    if (is_filter(o)) { ofilt = o; o = below(o); }
+    if (o && o->node_type == BK_JOIN_NODE) return in.fail(BKGPU_EUNSUPPORTED, "an APPLY whose outer child is a join is outside the GPU path");
+    if (!o || o->node_type != BK_SCAN_NODE) return in.fail(BKGPU_EUNSUPPORTED, "the outer child of an APPLY must be [FILTER ->] SCAN");
+    if (ofilt && ofilt->limit != -1) return in.fail(BKGPU_EUNSUPPORTED, "LIMIT on a filter below an APPLY is order dependent: outside the GPU path");
+    const int ot = o->tuple_id, at = sa.agg_tuple_id;
+    if (!sa.group_exprs.empty())
+        return in.fail(BKGPU_EUNSUPPORTED, "a GROUP BY inside a scalar subquery is outside the GPU path (the reference fails at run time when it yields more than one row)");
+    if (sa.limit != -1) return in.fail(BKGPU_EUNSUPPORTED, "a LIMIT inside the subquery of an APPLY is outside the GPU path");
+    for (const HExpr& f : sa.agg_fns) {
+        static const char* const taken[] = {"count_star", "count", "sum", "avg", "min", "max"};
+        if (f.distinct || std::none_of(std::begin(taken), std::end(taken), [&](const char* n) { return f.name == n; }))
+            return in.fail(BKGPU_EUNSUPPORTED, "aggregate %s%s in a scalar subquery is outside the GPU path (COUNT(*), COUNT, SUM, AVG, MIN and MAX are lowered)",
+                           f.name.c_str(), f.distinct ? " DISTINCT" : "");
+    }
+    // the subquery's own conjuncts, and its correlated ones: each an outer = inner column equality
+    std::vector<const HExpr*> own, moved;
+    const HNode* i = below(&sa);
+    for (; is_filter(i) && i->limit == -1; i = below(i))
+        for (auto& e : i->conjuncts) {
+            std::vector<int> ts; expr_tuples(e, ts);
+            (std::find(ts.begin(), ts.end(), ot) != ts.end() ? moved : own).push_back(&e);
+        }
+    if (i && (i->node_type == BK_LIMIT_NODE || i->limit != -1)) return in.fail(BKGPU_EUNSUPPORTED, "a LIMIT inside the subquery of an APPLY is outside the GPU path");
+    if (i && i->node_type == BK_JOIN_NODE) return in.fail(BKGPU_EUNSUPPORTED, "a join inside the subquery of an APPLY is outside the GPU path");
+    if (!i || i->node_type != BK_SCAN_NODE) return in.fail(BKGPU_EUNSUPPORTED, "the subquery of a max_one_row APPLY must be AGG -> [FILTER ->]* SCAN");
+    const int it = i->tuple_id;
+    if (it == ot) return in.fail(BKGPU_EINVAL, "both children of an APPLY scan tuple %d", it);
+    if (at == ot || at == it) return in.fail(BKGPU_EINVAL, "the subquery's aggregate tuple %d is also a scanned tuple", at);
+    std::vector<const HExpr*> ikeys, okeys;
+    for (const HExpr* e : moved) {
+        const bool eq = slot_eq(*e) && ((e->ch[0].tuple_id == ot && e->ch[1].tuple_id == it) || (e->ch[0].tuple_id == it && e->ch[1].tuple_id == ot));
+        if (!eq) return in.fail(BKGPU_EUNSUPPORTED, "a correlated conjunct of a scalar subquery that is not an outer = inner column equality runs as the reference's "
+                                "nested loop: outside the GPU path");
+        const bool inner_first = e->ch[0].tuple_id == it;
+        ikeys.push_back(&e->ch[inner_first ? 0 : 1]); okeys.push_back(&e->ch[inner_first ? 1 : 0]);
+    }
+    if (ikeys.empty()) return in.fail(BKGPU_EUNSUPPORTED, "a scalar subquery without an outer = inner column equality is outside the GPU path");
+    // 1. the subquery's aggregate, grouped by its inner key columns, each cast to the type the equality compares in
+    HNode grouped = sa;
+    for (size_t k = 0; k < ikeys.size(); k++) {
+        int cast;
+        if (!join_key_cast(in, ikeys[k]->col_type, okeys[k]->col_type, cast)) return false;
+        HExpr g = *ikeys[k]; g.col_type = cast;
+        grouped.group_exprs.push_back(g);
+    }
+    auto sub = std::make_shared<Compiled>();
+    sub->tuples = out.tuples; sub->in_sets = out.in_sets;
+    if (!lower_agg(in, *sub, grouped, own, it, false, true)) return false;
+    if ((int)sub->cols.size() > MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d columns referenced", MAX_COLS);
+    // 2. the outer aggregate: its predicate reads the subquery's aggregates as columns of the aggregate tuple
+    std::vector<HExpr> rewritten;
+    std::function<bool(HExpr&)> resolve = [&](HExpr& e) -> bool {
+        if ((e.node_type == BK_AGG_EXPR || e.node_type == BK_SLOT_REF) && e.tuple_id == at) {
+            const int slot = e.node_type == BK_AGG_EXPR ? e.final_slot : e.slot_id;
+            int k = -1;
+            for (size_t x = 0; x < sa.agg_fns.size(); x++) if (sa.agg_fns[x].final_slot == slot) k = (int)x;
+            if (k < 0) return in.fail(BKGPU_EINVAL, "the conditions of a scalar subquery read slot %d_%d, which its aggregate does not compute", at, slot);
+            const int prim = sub->ap.agg[k].out_prim, st = in.slot_type(at, slot);
+            if (st != BK_INVALID_TYPE && st != prim) return in.fail(BKGPU_EINVAL, "slot %d_%d is declared as type %d, its aggregate yields %d", at, slot, st, prim);
+            HExpr r; r.node_type = BK_SLOT_REF; r.tuple_id = at; r.slot_id = slot; r.col_type = prim;
+            e = r;
+            return true;
+        }
+        if (e.node_type == BK_SLOT_REF && e.tuple_id != ot)
+            return in.fail(BKGPU_EINVAL, "a condition of a scalar subquery reads tuple %d: only the outer tuple %d and the subquery's aggregates reach it", e.tuple_id, ot);
+        if (e.node_type == BK_AGG_EXPR) return in.fail(BKGPU_EINVAL, "a condition of a scalar subquery reads an aggregate of tuple %d", e.tuple_id);
+        for (auto& c : e.ch) if (!resolve(c)) return false;
+        return true;
+    };
+    for (const HNode* n : {ofilt, above, &apply}) if (n) for (const HExpr& e : n->conjuncts) rewritten.push_back(e);
+    for (HExpr& e : rewritten) if (!resolve(e)) return false;
+    std::vector<const HExpr*> conj;
+    for (const HExpr& e : rewritten) conj.push_back(&e);
+    if (!lower_agg(in, out, agg, conj, ot, under_packet, true)) return false;
+    Program dummy; memset(&dummy, 0, sizeof dummy);
+    Lower lw{&out, &in, &dummy};
+    for (const HExpr* k : okeys) out.sub_key_cols.push_back(lw.intern_col(ot, k->slot_id, in.slot_type(ot, k->slot_id)));
+    if ((int)out.cols.size() > MAX_COLS) return in.fail(BKGPU_EUNSUPPORTED, "more than %d columns referenced", MAX_COLS);
+    for (size_t c = 0; c < out.cols.size(); c++) {
+        if (out.cols[c].tuple_id != at) continue;
+        for (size_t x = 0; x < sa.agg_fns.size(); x++)
+            if (sa.agg_fns[x].final_slot == out.cols[c].slot_id) { out.sub_out_cols.push_back((int)c); out.sub_out_agg.push_back((int)x); }
+    }
+    out.sub = sub;
+    return true;
+}
+
 static bool lower_apply_agg(Infer& in, Compiled& out, const HNode& agg, const HNode& apply, bool under_packet, const HNode* above) {
     const int jt = apply.join_type;
     if (jt == BK_LEFT_JOIN) return in.fail(BKGPU_EUNSUPPORTED, "a LEFT apply (a scalar subquery) is outside the GPU path");
     if (jt != BK_SEMI_JOIN && jt != BK_ANTI_SEMI_JOIN) return in.fail(BKGPU_EUNSUPPORTED, "an APPLY of join type %d is outside the GPU path (SEMI / ANTI_SEMI are lowered)", jt);
-    if (apply.max_one_row) return in.fail(BKGPU_EUNSUPPORTED, "an APPLY with max_one_row (a subquery that must return at most one row) is outside the GPU path");
+    if (apply.max_one_row) {
+        const HNode* s = apply.ch.size() == 2 ? skip_passthrough(&apply.ch[1], nullptr) : nullptr;
+        if (jt == BK_SEMI_JOIN && !apply.is_select_field && apply.compare_type == BK_CMP_NULL && s && s->node_type == BK_AGG_NODE)
+            return lower_scalar_apply(in, out, agg, apply, *s, under_packet, above);
+        return in.fail(BKGPU_EUNSUPPORTED, "an APPLY with max_one_row (a subquery that must return at most one row) is outside the GPU path");
+    }
     if (apply.is_select_field) return in.fail(BKGPU_EUNSUPPORTED, "an APPLY of a subquery in the select list is outside the GPU path");
     if (apply.compare_type != BK_CMP_NULL) return in.fail(BKGPU_EUNSUPPORTED, "an APPLY with an ANY / ALL / SOME comparison (compare_type %d) is outside the GPU path", apply.compare_type);
     if (apply.ch.size() != 2) return in.fail(BKGPU_EINVAL, "APPLY node needs two children");

@@ -156,6 +156,14 @@ struct Compiled {
     // an APPLY (correlated subquery) lowered as the SEMI / ANTI_SEMI join above: its join type (0 = no APPLY), the conjuncts moved from the
     // subquery's filters into the join conditions, the conjuncts of the filter above it folded into the outer child's filter (explain only)
     int apply_join_type = 0, apply_moved = 0, apply_folded = 0;
+    // a scalar subquery (APPLY SEMI with max_one_row over an aggregate, lower_scalar_apply): `sub` is the subquery's aggregate grouped by the
+    // inner columns of its correlated equalities (kind PK_AGG over sub->scan_tuple).  This fragment aggregates the outer rows; beside the outer
+    // tuple's columns it reads one column per referenced subquery aggregate (a slot of the subquery's aggregate tuple), which k_apply_lookup
+    // fills for every outer batch from the subquery's group table
+    std::shared_ptr<Compiled> sub;
+    std::vector<int> sub_key_cols;     // per subquery key: index into cols of the outer column compared with it (cast to sub->ap.key_prim)
+    std::vector<int> sub_out_cols;     // per lookup column: index into cols
+    std::vector<int> sub_out_agg;      // ... and the subquery aggregate whose finalized value it holds (index into sub->ap.agg)
     // FK -> PK fast path: the same aggregate lowered over the virtual joined tuple (build-side columns are gathered
     // to probe-row alignment first); usable while every probe row has exactly one match
     std::shared_ptr<Compiled> jfast;

@@ -308,6 +308,14 @@ inline std::string host_refusal(const std::vector<uint8_t>& plan) {
     return "rb_build_agg returns a BITMAP column, which the C++ host mirror does not carry: run the plan through the C API or the Python binding";
 }
 
+// does the plan hold a scalar subquery (an APPLY with max_one_row over an aggregate)?  Every batch of its subquery must come before the first
+// batch of its outer tuple (bkgpu.h), while the APPLY's children are the other way round (child 0 the outer query, child 1 the subquery)
+inline bool host_subquery_first(const std::vector<uint8_t>& plan) {
+    std::string text(1 << 16, '\0');
+    if (bkgpu_plan_explain(plan.data(), plan.size(), &text[0], text.size()) < 0) return false;   // (bkgpu_init reports a plan that does not lower)
+    return text.find("\nscalar subquery: ") != std::string::npos;
+}
+
 // the fused AGG -> [FILTER] -> SCAN / SORT / AGG -> JOIN / FILTER subtree on the GPU
 class GpuExecNode : public ExecNode {
 public:
@@ -316,6 +324,7 @@ public:
     int init_serialized(std::vector<uint8_t> plan) {   // BKGPU_EUNSUPPORTED for a plan this mirror cannot carry; open() reports why
         _plan = std::move(plan);
         _refusal = host_refusal(_plan);
+        _subquery_first = host_subquery_first(_plan);
         return _refusal.empty() ? 0 : BKGPU_EUNSUPPORTED;
     }
     int open(RuntimeState* state) override {
@@ -323,7 +332,11 @@ public:
         int rc = bkgpu_init(&_h, _plan.data(), _plan.size(), state->device, state->nccl_comm);
         if (rc != 0) return fail(state, rc, nullptr);
         if ((rc = bkgpu_set_option(_h, "batch_capacity", state->row_batch_capacity)) != 0 || (rc = bkgpu_open(_h)) != 0) return fail(state, rc, _h);
-        for (auto& child : _children) {   // children in driver-table-first order (the join's outer child is child 0)
+        std::vector<size_t> order(_children.size());
+        for (size_t i = 0; i < order.size(); i++) order[i] = i;
+        if (_subquery_first && order.size() == 2) std::swap(order[0], order[1]);   // a scalar subquery: its subquery child (child 1) first
+        for (size_t ci : order) {   // children in driver-table-first order (the join's outer child is child 0)
+            auto& child = _children[ci];
             if (child->open(state) < 0) return -1;
             bool eos = false;
             while (!eos) {                 // the child-pull loop of AggNode::open (agg_node.cpp:447-485)
@@ -364,6 +377,7 @@ private:
     int fail(RuntimeState* state, int rc, bkgpu_plan* h) { state->error_code = rc; state->error_msg = bkgpu_last_error(h); return -1; }   // negative return + message
     std::vector<uint8_t> _plan;
     std::string _refusal;
+    bool _subquery_first = false;
     bkgpu_plan* _h = nullptr;
 };
 

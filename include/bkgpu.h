@@ -146,7 +146,10 @@ int   bkgpu_open(bkgpu_plan*);
  * Joins: a batch belongs to the table whose tuple its columns name.  Every batch of the build side (a two-table join's
  * outer child; every dimension of a star join) is retained and must come before the first batch of the probe side (the
  * inner child; the star join's fact table): a build-side batch after that returns BKGPU_ESTATE.  A caller that pulls
- * its children in order puts the fact scan last. */
+ * its children in order puts the fact scan last.
+ * Scalar subqueries (an APPLY with max_one_row over an aggregate) follow the same rule: every batch of the subquery's tuple comes before the
+ * first batch of the outer tuple, and one after it returns BKGPU_ESTATE.  Each plan must receive the whole subquery table, since every outer
+ * row is looked up in the subquery's aggregate over all of it; with no outer batch the result is the aggregate over no rows. */
 int   bkgpu_push(bkgpu_plan*, const bkgpu_column* cols, int ncols, int64_t nrows, int on_device);
 /* End of input: drain, run the cross-GPU merge when a communicator was given,
  * finalize aggregates (AggFnCall::finalize, src/expr/agg_fn_call.cpp:927-990). */
